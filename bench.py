@@ -11,7 +11,7 @@ JSON line (rank 0).
             launching stream, 256 MiB L2 flush between steps (outside the events), max over ranks.
   e2e       the same metric through the public operator API with HOST (pinned) input and output buffers, host<->device
             copies inside the timed region.
-  modes     fp32 models are measured in BOTH arithmetic modes of the library: "tf32" (single tcgen05 kind::tf32 pass,
+  modes     fp32 models are measured in BOTH arithmetic modes of the library: "tf32" (single wgmma tf32 pass,
             an explicit opt-in) and "tf32x3" (the library default: error-compensated, meets the reference's own f32
             tolerance).  The top-level value / e2e / roofline are the tf32 block (north_star names the TF32 roofline);
             `modes.tf32x3` carries the same keys for the fp32-grade path.  Algorithmic flops are counted 1x in both.
@@ -52,7 +52,7 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_burst": d["bf16_tflops"], "bf16_sustained": d["bf16_tflops_sustained"], "src": "MEASURED_PEAKS.json"}
-    return {"hbm_gbs": 6650.0, "bf16_burst": 1590.0, "bf16_sustained": 1400.0, "src": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "bf16_burst": 989.0, "bf16_sustained": 989.0, "src": "H100 SXM data sheet (dense, 700 W)"}
 
 
 class ClockSampler:
@@ -302,6 +302,8 @@ def main():
     ap.add_argument("--no-extras", action="store_true", help="skip the secondary numbers (other configs, 8192^3 GEMM TFLOP/s)")
     ap.add_argument("--no-peaks", action="store_true", help="skip the on-box cuBLAS peak measurement (uses MEASURED_PEAKS.json ratios)")
     ap.add_argument("--modes", default=None, help="comma list restricting the f32 modes measured (tf32,tf32x3)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the timed path returned in its last step as DIR/<name>.npy (float32, at most 64 MB in all)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     model = args.model
@@ -311,6 +313,8 @@ def main():
     world = int(os.environ.get("WORLD_SIZE", "1"))
 
     if args.impl == "reference":
+        if args.dump_outputs:
+            raise SystemExit("--dump-outputs records the GPU path's outputs; the reference arm (--impl reference) has none to write")
         if rank == 0:
             print(json.dumps(run_reference_arm(args, model, batch)), flush=True)
         return
@@ -322,7 +326,7 @@ def main():
     from oracle import oracle  # inputs / weights RNG + the cpu_baseline leg only
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: rten_b200 has no CPU fallback")
+        raise SystemExit("bench.py needs an H100: rten_b200 has no CPU fallback")
     torch.cuda.set_device(local_rank)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
@@ -453,6 +457,7 @@ def main():
             return ms, launches, clocks
 
         ms, launches, clocks = timed(device_step, args.steps, args.warmup, sampler)
+        dump_output(f"{model}_{mode}", out_t)  # the last timed step's result (device_step copied it there)
         res.update(value=batch * world * args.steps / (ms / 1e3), ms_per_step=ms / args.steps, gpu_launches=int(launches), clocks=clocks,
                    cuda_graph=graph is not None, flops_per_step=flops)
         if flops:
@@ -587,6 +592,7 @@ def main():
         clocks = sampler.stop() if sampler else None
         ms = sum(s.elapsed_time(e) for s, e in evs)
         launches = ctx.launches - l0
+        dump_output(f"{model}_{res['mode']}_logits", run._g_logits.numpy())
         if world > 1:
             t = torch.tensor([ms], dtype=torch.float64, device="cuda")
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -614,6 +620,19 @@ def main():
         kv = 2 * len(spec.layers) * batch * spec.hidden * 4 * (GPT2_PREFILL + 1)
         res["algorithmic_bytes_per_step"] = float(wbytes + kv)
         return res
+
+    def dump_output(name, arr):
+        """--dump-outputs: one float32 array per timed path, so that two builds can be compared output for output.  An
+        output larger than its share of the 64 MB budget is replaced by a fixed, seeded sample of its elements."""
+        if not args.dump_outputs or rank != 0:
+            return
+        a = (arr.detach().cpu().numpy() if hasattr(arr, "detach") else np.asarray(arr)).astype(np.float32)
+        cap = (64 << 20) // 4 // max(1, len(modes))
+        if a.size > cap:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, cap, replace=False))
+            a = a.reshape(-1)[idx]
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, f"{name}.npy"), a)
 
     # ---- the measured modes
     results = {}
@@ -669,9 +688,8 @@ def main():
                 lw["frac"] = lw["floor_us"] / (step_ms * 1e3)
                 lw["how"] = ("sum over the conv layers of max(layer flops / tensor peak, layer HBM bytes / HBM peak) divided by the step time: "
                              "the fraction of the per-layer roofline this step reaches (flops counted 1x in both f32 modes)")
-            return {"bound": "tensor", "layerwise": lw, "kernel": f"rtb::umma_gemm_kernel<{1 if kind == 'int8' else 0}> (tcgen05 kind::{'i8' if kind == 'int8' else 'tf32'} implicit-GEMM conv / GEMM)",
+            return {"bound": "tensor", "layerwise": lw, "kernel": f"rtb::umma_gemm_kernel<{1 if kind == 'int8' else 0}> (wgmma {'s8' if kind == 'int8' else 'tf32'} implicit-GEMM conv / GEMM)",
                     "achieved": ach, "peak": burst, "unit": "TFLOP/s" if kind == "tf32" else "TOP/s", "frac": ach / burst, "frac_of_sustained_peak": ach / sust,
-                    "traffic": ncu_traffic(model),
                     "lower_bound": {"achieved": lb, "frac": lb / burst, "how": "algorithmic flops / whole step time (kernel time <= step time)"},
                     "kernel_time_us_per_step": busy_us, "sum_of_kernel_durations_us": kern_us, "launches_per_step": n_kern,
                     "share_of_step": (busy_us / 1e3 / step_ms) if busy_us else None,
@@ -783,18 +801,6 @@ def layerwise_floor_us(model, spec, batch, tensor_tflops, hbm_gbs):
     t = sum(max(fl / (tensor_tflops * 1e12), by / (hbm_gbs * 1e9)) for fl, by in rows) * 1e6
     return {"floor_us": t, "tensor_only_us": t_f, "hbm_only_us": t_b, "layers": len(rows),
             "hbm_bound_layers": sum(1 for fl, by in rows if by / (hbm_gbs * 1e9) > fl / (tensor_tflops * 1e12))}
-
-
-def ncu_traffic(model):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed `ncu --set full`
-    capture of this same command (profiles/r02_ncu_<model>.json, falling back to round 1's); None if absent."""
-    for name in (f"r02_ncu_{model}.json", "r01_ncu_resnet50.json" if model == "resnet50" else ""):
-        p = os.path.join(ROOT, "profiles", name)
-        try:
-            return json.load(open(p))["umma_avg_dram_bytes_per_launch"]
-        except Exception:
-            continue
-    return None
 
 
 def secondary_numbers(rt, graphs, oracle, stream, torch, flush, sampler, device):

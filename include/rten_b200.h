@@ -1,5 +1,5 @@
 /*
- * rten_b200.h -- C ABI of librten_b200.so: the B200 (sm_100a) operator execution backend for RTen.
+ * rten_b200.h -- C ABI of librten_b200.so: the H100 (sm_90a) operator execution backend for RTen.
  *
  * This is the drop-in boundary for ONE path of robertknight/rten: `Operator::run` /
  * `run_in_place` / `prepack` (src/operator.rs:486-613) of the dense operators of ResNet-50 /
@@ -24,7 +24,7 @@
  *    tensor is involved; asynchronous CUDA errors surface on the next call or rten_b200_sync().
  *  - Errors: status codes mirror `OpError` (src/operator.rs:116-144); rten_b200_last_error()
  *    returns the reference's static message string for that error.
- *  - No CPU fallback exists: without a B200 + driver every op fails with RTEN_ERR_CUDA.
+ *  - No CPU fallback exists: without an H100 + driver every op fails with RTEN_ERR_CUDA.
  */
 #ifndef RTEN_B200_H
 #define RTEN_B200_H
@@ -72,8 +72,8 @@ typedef struct rten_packed rten_packed;
 
 /* fp32 GEMM/Conv arithmetic mode (SURVEY.md hard part A). */
 typedef enum {
-    RTEN_F32_TF32 = 0,  /* single tcgen05 kind::tf32 pass: operands rounded to 10 mantissa bits.  EXPLICIT OPT-IN
-                           (rten_b200_set_f32_mode or env RTEN_B200_F32_MODE=tf32); tolerance in DESIGN.md */
+    RTEN_F32_TF32 = 0,  /* single wgmma tf32 pass: operands rounded to 10 mantissa bits.  EXPLICIT OPT-IN
+                           (rten_b200_set_f32_mode or env RTEN_B200_F32_MODE=tf32); tolerance |d| <= 2^-9 sum_k |a_k b_k| */
     RTEN_F32_TF32X3 = 1 /* DEFAULT: 3-pass error-compensated split (hi*hi + hi*lo + lo*hi, f32 accumulation): meets the
                            reference's own f32 tolerance (rten-tensor/src/test_util.rs:47-92) at 1/3 of the tensor rate */
 } rten_f32_mode;

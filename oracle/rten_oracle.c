@@ -6,7 +6,7 @@
  * (rten_b200/, librten_b200.so) never links or calls anything in oracle/.
  *
  * The reference is Rust (edition 2024); no cargo/rustc exists in the build image, so
- * oracle/_ref cannot be built (see oracle/Makefile, DESIGN.md).  Every function below
+ * oracle/_ref cannot be built (see oracle/Makefile).  Every function below
  * restates the reference algorithm and cites the file:line (relative to the rten tree,
  * commit c7f7bad) it follows.  Parity pin: the golden vectors the reference's own tests
  * hold for this path (tests/test_oracle_golden.py).
@@ -495,7 +495,7 @@ void rto_gemm_f32(size_t M, size_t N, size_t K, const float *a, ptrdiff_t a_rs, 
 }
 
 /* float64 "truth" GEMM used for error budgeting of the TF32 GPU path, and the
- * sum(|a||b|) bound the tolerance is stated against (DESIGN.md). */
+ * sum(|a||b|) bound the tolerance is stated against (2^-9 sum |a||b| in the single-pass TF32 mode). */
 void rto_gemm_f64(size_t M, size_t N, size_t K, const float *a, ptrdiff_t a_rs, ptrdiff_t a_cs,
                   const float *b, ptrdiff_t b_rs, ptrdiff_t b_cs, double *c, double *cabs) {
 #pragma omp parallel for schedule(static) if (M * N * K > 262144)

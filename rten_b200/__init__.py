@@ -1,4 +1,4 @@
-"""rten_b200 -- B200 (sm_100a) operator execution backend for the RTen hot path.
+"""rten_b200 -- sm_90a (H100) operator execution backend for the RTen hot path.
 
 The product is `librten_b200.so` (hand-written CUDA behind the C ABI in include/rten_b200.h);
 `rten_b200.ops` is the host-side mirror of RTen's operator interface used by the tests, the model

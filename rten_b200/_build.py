@@ -1,4 +1,4 @@
-"""Build librten_b200.so (sm_100a only) in-tree with nvcc.  No torch involved: the library is a plain
+"""Build librten_b200.so (sm_90a only) in-tree with nvcc.  No torch involved: the library is a plain
 CUDA runtime shared object behind the C ABI of include/rten_b200.h."""
 from __future__ import annotations
 
@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "librten_b200.so")
 SOURCES = ["umma_gemm.cu", "umma_halo.cu", "rowops.cu", "skinny.cu", "attn_fused.cu", "api_core.cu", "api_ops.cu", "api_conv.cu", "api_rows.cu", "api_fused.cu", "onnx_reader.cu", "model.cu", "comm.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--cudart", "static",
 ]
 

@@ -1,7 +1,7 @@
 """ctypes binding of librten_b200.so (the C ABI in include/rten_b200.h).
 
 The library is the product; this module only marshals descriptors.  It fails loudly when the
-shared object is missing or no B200 is present -- there is no CPU fallback."""
+shared object is missing or no H100 is present -- there is no CPU fallback."""
 from __future__ import annotations
 
 import ctypes as C

@@ -208,7 +208,7 @@ using namespace rtb;
 // =========================================================================================
 extern "C" {
 
-const char* rten_b200_version(void) { return "rten-b200 0.1 (sm_100a)"; }
+const char* rten_b200_version(void) { return "rten-b200 0.1 (sm_90a)"; }
 
 // Measured launch plans can be kept across processes: RTEN_B200_TUNE_FILE names a text file that is read when a
 // context is created and rewritten when a context that measured new plans is destroyed (one line per problem:
@@ -267,7 +267,7 @@ rten_status rten_b200_ctx_create(int device, void* cuda_stream_or_null, size_t w
     if (cudaSetDevice(device) != cudaSuccess) return RTEN_ERR_CUDA;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return RTEN_ERR_CUDA;
-    if (prop.major != 10) return RTEN_ERR_CUDA;  // sm_100a kernels only: no fallback path exists
+    if (prop.major != 9) return RTEN_ERR_CUDA;  // sm_90a kernels only: no fallback path exists
     rten_ctx* ctx = new rten_ctx();
     ctx->device = device;
     ctx->num_sms = prop.multiProcessorCount;

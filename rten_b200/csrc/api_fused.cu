@@ -254,7 +254,7 @@ rten_status rten_b200_attention(rten_ctx* ctx, const rten_tensor* query, const r
             return sc.finish(st);
         }
     }
-    // ---- encoder shapes (128 keys, head size 64, value tensor stored transposed): ONE tcgen05 kernel per layer
+    // ---- encoder shapes (128 keys, head size 64, value tensor stored transposed): one fused kernel per layer where available
     // (single-pass TF32 products: only when the context opted in to that mode)
     if (resident && ctx->f32_mode == RTEN_F32_TF32 && !new_key && !nonpad_kv_seqlen && !prm->is_causal && qh == kvh && dv == dh &&
         query->strides[3] == 1 && key->strides[3] == 1 && (value->strides[2] == 1 || value->strides[3] == 1) &&

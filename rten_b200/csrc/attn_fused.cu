@@ -1,12 +1,11 @@
-// Fused attention for encoder-sized sequences (BERT: 128 keys, head size 64) on tcgen05: one CTA per (batch, head,
+// Fused attention for encoder-sized sequences (BERT: 128 keys, head size 64) on wgmma: one CTA per (batch, head,
 // 128-query tile) computes  O = softmax(scale * Q K^T + mask) V  without the score matrix ever leaving the SM:
-//   TMA: Q, K tiles (K-major, 128B swizzle), V^T tiles           ->  shared memory
-//   tcgen05.mma kind::tf32:  S = Q K^T                            ->  TMEM columns [0, 128)
-//   4 warps, one query row per thread: tcgen05.ld S, scale, + mask, the reference's softmax (rten-vecmath/src/softmax.rs:
+//   warp 4, TMA: Q, K tiles (K-major, 128B swizzle), V^T tiles    ->  shared memory
+//   warps 0-3 (one warpgroup), wgmma tf32:  S = Q K^T in two 64-column halves -> accumulator tile in shared memory
+//   the same warps, one query row per thread: S row, scale, + mask, the reference's softmax (rten-vecmath/src/softmax.rs:
 //       60-101,176-228: ReducedRangeExp, 16 lane partial sums in index order) -> P written as the A operand (128B-swizzled
 //       K-major tiles) in shared memory
-//   tcgen05.mma kind::tf32:  O = P V                              ->  TMEM columns [128, 192)
-//   tcgen05.ld O -> global
+//   wgmma tf32:  O = P V -> accumulator tile -> rows staged in shared memory -> global
 // Replaces, for these shapes, FusedMatMul(QK^T) + AddSoftmax + MatMul(PV) (src/ops/attention.rs:30-165, :518-560): three
 // launches and two round trips of the [batch, heads, 128, 128] score tensor through HBM per layer.
 #include <cuda.h>
@@ -26,7 +25,7 @@ namespace rtb {
 
 namespace {
 
-constexpr int AF_THREADS = 192;  // warps 0-3: one query row per thread; warp 4: TMA + MMA issue; warp 5: TMEM allocation
+constexpr int AF_THREADS = 160;  // warps 0-3: wgmma warpgroup, one query row per thread; warp 4: TMA
 constexpr int SQ = 128, SK = 128, DH = 64;
 constexpr uint32_t TILE = 128 * 128;      // a [128 rows x 32 floats] K-major tile
 constexpr uint32_t VT_TILE = DH * 128;    // a [64 rows x 32 floats] tile of V^T
@@ -42,22 +41,19 @@ struct AttnFusedParams {
     long long o_b, o_h, o_s;
 };
 
-__global__ void __launch_bounds__(AF_THREADS, 2)
+__global__ void __launch_bounds__(AF_THREADS, 1)
 attn_fused_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant__ CUtensorMap tma_k,
                   const __grid_constant__ CUtensorMap tma_v, const __grid_constant__ AttnFusedParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bar_qk = reinterpret_cast<uint64_t*>(base);
     uint64_t* bar_v = bar_qk + 1;
-    uint64_t* bar_s = bar_qk + 2;
-    uint64_t* bar_p = bar_qk + 3;
-    uint64_t* bar_o = bar_qk + 4;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bar_qk + 6);
-    uint8_t* sq = base + 1024;              // 2 tiles
+    const uint32_t acc_smem = smem_u32(base + 1024);  // 128 x 128 accumulator tile (ptx.cuh): S, later O
+    uint8_t* sq = base + 1024 + ACC_SMEM_BYTES;  // 2 tiles
     uint8_t* sk = sq + 2 * TILE;            // 2 tiles
     uint8_t* sv = sk + 2 * TILE;            // 4 tiles of V^T
-    uint8_t* sp = sq;                       // 4 tiles of P: over Q and K, which are dead once S = Q K^T has completed (bar_s)
-                                            // -> 98 KB per CTA, two CTAs per SM: one CTA's softmax overlaps the other's TMA / MMA
+    uint8_t* sp = sq;                       // 4 tiles of P: over Q and K, which are dead once S = Q K^T has completed
+
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int u = blockIdx.x;
     const int qt = u % p.q_tiles, h = (u / p.q_tiles) % p.heads, b = u / (p.q_tiles * p.heads);
@@ -68,19 +64,9 @@ attn_fused_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_consta
         tma_prefetch_desc(&tma_v);
         mbar_init(bar_qk, 1);
         mbar_init(bar_v, p.v ? 4 : 1);
-        mbar_init(bar_s, 1);
-        mbar_init(bar_p, 4);
-        mbar_init(bar_o, 1);
         fence_mbar_init();
     }
-    if (warp == 5) {
-        tmem_alloc(tmem_ptr, 256);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_ptr;
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
@@ -96,42 +82,38 @@ attn_fused_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_consta
                 for (int kb = 0; kb < 4; kb++) tma_load_4d(sv + kb * VT_TILE, &tma_v, bar_v, kb * 32, 0, h, b);
             }
         }
-        __syncwarp();
-        // ---- S = Q K^T
-        mbar_wait(bar_qk, 0);
-        tc_fence_after();
-        if (elect_one()) {
-            const uint32_t idesc = make_idesc(1, 2, 2, 128, SK);
-            for (int kb = 0; kb < 2; kb++) {
-                const uint64_t ad = make_kmajor_sw128_desc(smem_u32(sq + kb * TILE)), bd = make_kmajor_sw128_desc(smem_u32(sk + kb * TILE));
-#pragma unroll
-                for (int k = 0; k < 4; k++) umma_tf32(tmem, ad + 2 * k, bd + 2 * k, idesc, (kb | k) ? 1u : 0u);
-            }
-            umma_commit(bar_s);
-        }
-        __syncwarp();
-        // ---- O = P V
-        mbar_wait(bar_p, 0);
-        mbar_wait(bar_v, 0);
-        tc_fence_after();
-        if (elect_one()) {
-            const uint32_t idesc = make_idesc(1, 2, 2, 128, DH);
-            for (int kb = 0; kb < 4; kb++) {
-                const uint64_t ad = make_kmajor_sw128_desc(smem_u32(sp + kb * TILE)), bd = make_kmajor_sw128_desc(smem_u32(sv + kb * VT_TILE));
-#pragma unroll
-                for (int k = 0; k < 4; k++) umma_tf32(tmem + 128, ad + 2 * k, bd + 2 * k, idesc, (kb | k) ? 1u : 0u);
-            }
-            umma_commit(bar_o);
-        }
-        __syncwarp();
-    } else if (warp < 4) {
+    } else {
         // ---- one query row per thread
         const int r = warp * 32 + lane;
-        const uint32_t t_row = tmem + ((uint32_t)(warp * 32) << 16);
+        const uint32_t t_row = (uint32_t)(warp * 32) << 16;  // this warp's rows of the accumulator tile
+        // S = Q K^T, one 64-column half at a time (keys [64 h, 64 h + 64) = rows of the K tiles)
+        mbar_wait(bar_qk, 0);
+#pragma unroll
+        for (int half = 0; half < 2; half++) {
+            float d0[32], d1[32];
+#pragma unroll
+            for (int i = 0; i < 32; i++) d0[i] = d1[i] = 0.0f;
+            wgmma_fence();
+#pragma unroll
+            for (int kb = 0; kb < 2; kb++) {
+                const uint64_t ad = make_kmajor_sw128_desc(smem_u32(sq + kb * TILE));
+                const uint64_t bd = make_kmajor_sw128_desc(smem_u32(sk + kb * TILE + half * 64 * 128));
+#pragma unroll
+                for (int k = 0; k < 4; k++) {
+                    wgmma_k<0, 0, 64>(d0, ad + 2 * k, bd + 2 * k);
+                    wgmma_k<0, 0, 64>(d1, ad + (64 * 128 >> 4) + 2 * k, bd + 2 * k);
+                }
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            acc_store_frag<64>(acc_smem, d0, 0, half * 64);
+            acc_store_frag<64>(acc_smem, d1, 64, half * 64);
+        }
+        asm volatile("bar.sync 1, 128;" ::: "memory");  // the whole S tile is in shared memory; Q and K are dead
         const float* mrow = p.mask ? p.mask + (long long)b * p.m_b : nullptr;
         if (p.v) {
             // natural V [s][d]: this thread's key row s = r goes into column r of the K-major, 128B-swizzled V^T tiles
-            // (tile r / 32, row d, 16-byte chunk ((r % 32) / 4) ^ (d & 7)) while the tensor core is busy with Q K^T
+            // (tile r / 32, row d, 16-byte chunk ((r % 32) / 4) ^ (d & 7)); read by the P V product below
             const float4* vrow = reinterpret_cast<const float4*>(p.v + (long long)b * p.v_b + (long long)h * p.v_h + (long long)r * p.v_s);
             float4 vv[DH / 4];
 #pragma unroll
@@ -152,15 +134,12 @@ attn_fused_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_consta
             if (lane == 0) mbar_arrive(bar_v);
         }
         float z[SK];
-        mbar_wait(bar_s, 0);
-        tc_fence_after();
         float mx = -FLT_MAX;
         const f32x2 sc2 = splat2(p.scale);
 #pragma unroll
         for (int c = 0; c < 4; c++) {
             uint32_t v[32];
-            tmem_ld_32x32(t_row + c * 32, v);
-            tmem_ld_wait();
+            acc_ld(acc_smem, t_row + c * 32, v);
 #pragma unroll
             for (int j = 0; j < 32; j += 4) {
                 // FusedMatMul's alpha, then AddSoftmax's z = qk + mask: two lanes per packed instruction (same roundings)
@@ -215,21 +194,38 @@ attn_fused_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_consta
             }
         }
         fence_proxy_async();  // the tensor core reads these bytes through the async proxy
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_p);
-        // ---- O rows -> shared memory (the P tiles are dead once P V has completed) -> global, two whole 256-byte rows per
-        // warp instruction (a thread writing its own row costs 32 half-used sectors per instruction: tools/store_probe.cu)
-        mbar_wait(bar_o, 0);
-        tc_fence_after();
+        asm volatile("bar.sync 1, 128;" ::: "memory");  // all of P written, every row of S read
+        // ---- O = P V
+        mbar_wait(bar_v, 0);
+        {
+            float d0[32], d1[32];
+#pragma unroll
+            for (int i = 0; i < 32; i++) d0[i] = d1[i] = 0.0f;
+            wgmma_fence();
+#pragma unroll
+            for (int kb = 0; kb < 4; kb++) {
+                const uint64_t ad = make_kmajor_sw128_desc(smem_u32(sp + kb * TILE)), bd = make_kmajor_sw128_desc(smem_u32(sv + kb * VT_TILE));
+#pragma unroll
+                for (int k = 0; k < 4; k++) {
+                    wgmma_k<0, 0, 64>(d0, ad + 2 * k, bd + 2 * k);
+                    wgmma_k<0, 0, 64>(d1, ad + (64 * 128 >> 4) + 2 * k, bd + 2 * k);
+                }
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            acc_store_frag<64>(acc_smem, d0, 0, 0);
+            acc_store_frag<64>(acc_smem, d1, 64, 0);
+        }
+        asm volatile("bar.sync 1, 128;" ::: "memory");  // O complete in shared memory; P is dead
+        // ---- O rows -> shared memory (over P) -> global, two whole 256-byte rows per warp instruction (a thread writing
+        // its own row would cost 32 half-used sectors per instruction)
         uint8_t* so = sp + warp * (32 * 256);  // this warp's 32 rows x 256 B
         {
             uint8_t* rowp = so + lane * 256;
 #pragma unroll
             for (int c = 0; c < 2; c++) {
                 uint32_t v[32];
-                tmem_ld_32x32(t_row + 128 + c * 32, v);
-                tmem_ld_wait();
+                acc_ld(acc_smem, t_row + c * 32, v);
 #pragma unroll
                 for (int j = 0; j < 8; j++)
                     *reinterpret_cast<uint4*>(rowp + c * 128 + ((j ^ (lane & 7)) << 4)) = make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
@@ -243,12 +239,6 @@ attn_fused_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_consta
             const uint4 d = *reinterpret_cast<const uint4*>(so + row * 256 + (jj >> 3) * 128 + (((jj & 7) ^ (row & 7)) << 4));
             *reinterpret_cast<uint4*>(obase + (long long)row * p.o_s + jj * 4) = d;
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 5) {
-        tc_fence_after();
-        tmem_dealloc(tmem, 256);
     }
 }
 
@@ -290,7 +280,7 @@ rten_status launch_attn_fused(rten_ctx* ctx, const AttnFusedLaunch& L) {
     if (!encode_map(ctx, &mq, L.q, 4, true, qbox, ones) || !encode_map(ctx, &mk, L.k, 4, true, kbox, ones)) return RTEN_ERR_UNSUPPORTED_VALUE;
     mv = mq;  // (unused when the kernel transposes a natural V itself)
     if (!L.v && !encode_map(ctx, &mv, L.vt, 4, true, vbox, ones)) return RTEN_ERR_UNSUPPORTED_VALUE;
-    const size_t smem = 1024 + 1024 + 4 * (size_t)TILE + 4 * (size_t)VT_TILE;
+    const size_t smem = 1024 + 1024 + ACC_SMEM_BYTES + 4 * (size_t)TILE + 4 * (size_t)VT_TILE;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(L.B * L.heads * p.q_tiles);

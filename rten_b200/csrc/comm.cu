@@ -8,7 +8,7 @@
 // into its slot of every peer's mailbox, spins until every slot of its own mailbox carries the current epoch, and
 // reduces.  No fences are needed (each word is self-validating), slots are double-buffered by epoch parity (a rank
 // can be at most one exchange ahead of a peer), and the epoch lives in device memory so that CUDA-graph replays advance
-// it.  Measured against two ncclAllReduce calls of one int each (the fallback, RTEN_B200_NCCL_RANGES=1): DESIGN.md 5.
+// it.  The fallback is two ncclAllReduce calls of one int each (RTEN_B200_NCCL_RANGES=1).
 // NCCL is resolved at run time (dlopen of libnccl.so.2 -- the copy already loaded in the process if there is one), so
 // the library itself keeps no link-time dependency on it; it also carries the IPC handles at start-up.
 #include <dlfcn.h>

@@ -79,32 +79,19 @@ __device__ __forceinline__ float gelu_ref(float x) {
     return __fmul_rn(half_x, y);
 }
 
-// ---- two lanes at a time (packed f32x2 FMA / MUL / ADD: each half is the same IEEE operation as its scalar twin, so
-// gelu_ref_x2 is bit-identical to two gelu_ref calls with ~40 % fewer instructions -- the GEMM epilogue's Gelu)
+// ---- two lanes at a time: a pair type with the scalar IEEE operations applied to each half, so gelu_ref_x2 is
+// bit-identical to two gelu_ref calls (sm_90 has no packed f32x2 arithmetic; the pairs keep the code shared)
 struct f32x2 {
-    unsigned long long v;
+    float x, y;
 };
-__device__ __forceinline__ f32x2 pack2(float a, float b) {
-    f32x2 r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r.v) : "f"(a), "f"(b));
-    return r;
+__device__ __forceinline__ f32x2 pack2(float a, float b) { return {a, b}; }
+__device__ __forceinline__ void unpack2(f32x2 p, float& a, float& b) {
+    a = p.x;
+    b = p.y;
 }
-__device__ __forceinline__ void unpack2(f32x2 p, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(p.v)); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-    f32x2 r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r.v) : "l"(a.v), "l"(b.v), "l"(c.v));
-    return r;
-}
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-    f32x2 r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-    return r;
-}
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-    f32x2 r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-    return r;
-}
+__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return {__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)}; }
+__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return {__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)}; }
+__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return {__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)}; }
 __device__ __forceinline__ f32x2 splat2(float c) { return pack2(c, c); }
 
 // reduced_range_exp of two lanes (same roundings as the scalar recipe)

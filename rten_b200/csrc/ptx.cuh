@@ -1,9 +1,10 @@
-// Thin inline-PTX wrappers for the sm_100a features the GEMM/conv kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), fences.
-// Descriptor bit layouts follow the PTX ISA "tcgen05 matrix / instruction descriptor"
-// tables (also documented in CUTLASS cute/arch/mma_sm100_desc.hpp).
+// Thin inline-PTX wrappers for the sm_90a features the GEMM/conv kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma, fences.
+// The matrix descriptor layout follows the PTX ISA "wgmma matrix descriptor" table.
 #pragma once
 #include <cstdint>
+#include <cstring>
+#include <type_traits>
 #include <cuda.h>
 
 namespace rtb {
@@ -116,167 +117,175 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* s
                  : "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(ncols)
-                 : "memory");
+// ------------------------------------------------------------------ wgmma (sm_90a warpgroup MMA)
+// D (registers of the issuing warpgroup) += A[smem] * B[smem], both operands K-major.  One instruction covers 64 rows
+// of A and 32 bytes of K (tf32: k8, 8-bit integers: k32); the accumulator fragment of thread t of the warpgroup holds
+// rows 16 * (t / 32) + (t % 32) / 4 + {0, 8} and columns 8 * j + 2 * (t % 4) + {0, 1}.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Pins accumulator registers in place: the compiler may not move, copy or re-allocate them across this point.  Needed
+// around wgmma issue whenever a group can still be in flight, since the hardware writes those registers asynchronously.
+template <typename T, int M>
+__device__ __forceinline__ void wgmma_fence_operand(T (&d)[M]) {
+#pragma unroll
+    for (int i = 0; i < M; i++) {
+        if constexpr (sizeof(T) == 4 && std::is_floating_point<T>::value)
+            asm volatile("" : "+f"(d[i])::"memory");
+        else
+            asm volatile("" : "+r"(d[i])::"memory");
+    }
 }
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem];  accumulate == 0 overwrites D.
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    uint32_t z = 0;
+__device__ __forceinline__ void wgmma_tf32_n32(float (&d)[16], uint64_t adesc, uint64_t bdesc) {
     asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(z), "r"(z), "r"(z), "r"(z)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(adesc), "l"(bdesc));
 }
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                        uint32_t accumulate) {
-    uint32_t z = 0;
+__device__ __forceinline__ void wgmma_u8u8_n32(uint32_t (&d)[16], uint64_t adesc, uint64_t bdesc) {
     asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(z), "r"(z), "r"(z), "r"(z)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k32.s32.u8.u8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n\t}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+        : "l"(adesc), "l"(bdesc));
 }
+__device__ __forceinline__ void wgmma_u8s8_n32(uint32_t (&d)[16], uint64_t adesc, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k32.s32.u8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n\t}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+        : "l"(adesc), "l"(bdesc));
+}
+__device__ __forceinline__ void wgmma_s8u8_n32(uint32_t (&d)[16], uint64_t adesc, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.u8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n\t}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+        : "l"(adesc), "l"(bdesc));
+}
+__device__ __forceinline__ void wgmma_s8s8_n32(uint32_t (&d)[16], uint64_t adesc, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n\t}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+        : "l"(adesc), "l"(bdesc));
+}
+__device__ __forceinline__ void wgmma_tf32_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc));
+}
+__device__ __forceinline__ void wgmma_u8u8_n64(uint32_t (&d)[32], uint64_t adesc, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k32.s32.u8.u8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n\t}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+        : "l"(adesc), "l"(bdesc));
+}
+__device__ __forceinline__ void wgmma_u8s8_n64(uint32_t (&d)[32], uint64_t adesc, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k32.s32.u8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n\t}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+        : "l"(adesc), "l"(bdesc));
+}
+__device__ __forceinline__ void wgmma_s8u8_n64(uint32_t (&d)[32], uint64_t adesc, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.u8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n\t}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+        : "l"(adesc), "l"(bdesc));
+}
+__device__ __forceinline__ void wgmma_s8s8_n64(uint32_t (&d)[32], uint64_t adesc, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n\t}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+        : "l"(adesc), "l"(bdesc));
+}
+// KIND 0: tf32 -> f32; KIND 1: 8-bit integers -> s32 (SGN bit 0: A signed, bit 1: B signed).  The accumulators keep
+// their own register type (acc_t): a reinterpreting cast would let the compiler copy registers that an in-flight wgmma
+// still owns.
 template <int KIND>
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    if (KIND == 0)
-        umma_tf32(tmem_d, adesc, bdesc, idesc, accumulate);
-    else
-        umma_i8(tmem_d, adesc, bdesc, idesc, accumulate);
-}
-__device__ __forceinline__ void umma_commit_u32(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// Arrives on `bar` once all previously issued MMAs of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
+using acc_t = typename std::conditional<KIND == 0, float, uint32_t>::type;
+
+template <int KIND, int SGN, int N>
+__device__ __forceinline__ void wgmma_k(acc_t<KIND> (&d)[N / 2], uint64_t adesc, uint64_t bdesc) {
+    if constexpr (KIND == 0) {
+        if constexpr (N == 32) wgmma_tf32_n32(d, adesc, bdesc);
+        else wgmma_tf32_n64(d, adesc, bdesc);
+    } else if constexpr (N == 32) {
+        if constexpr (SGN == 0) wgmma_u8u8_n32(d, adesc, bdesc);
+        else if constexpr (SGN == 1) wgmma_s8u8_n32(d, adesc, bdesc);
+        else if constexpr (SGN == 2) wgmma_u8s8_n32(d, adesc, bdesc);
+        else wgmma_s8s8_n32(d, adesc, bdesc);
+    } else {
+        if constexpr (SGN == 0) wgmma_u8u8_n64(d, adesc, bdesc);
+        else if constexpr (SGN == 1) wgmma_s8u8_n64(d, adesc, bdesc);
+        else if constexpr (SGN == 2) wgmma_u8s8_n64(d, adesc, bdesc);
+        else wgmma_s8s8_n64(d, adesc, bdesc);
+    }
 }
 
-// ------------------------------------------------------------------ CTA pair (cta_group::2) variants
-// Two CTAs of a (2,1,1) cluster drive ONE 256-row MMA: each CTA stages its own 128 rows of A and HALF of the B tile,
-// the leader (cluster rank 0) issues the instruction, both tensor cores execute it.  Barriers that gate the leader's
-// MMA warp live in the leader's shared memory: clearing bit 24 of a shared::cluster address selects rank 0's copy.
-constexpr uint32_t PEER_BIT_MASK = 0xFEFFFFFFu;
+// ------------------------------------------------------------------ accumulator hand-off in shared memory
+// The MMA warpgroup of a kernel stores finished accumulator tiles into ACC_COLS columns x 128 rows of 32-bit words
+// (column-major, padded to ACC_LD rows so that both the fragment stores and the row-per-thread loads below are free of
+// bank conflicts); the epilogue warps read them back one row per thread.  An accumulator address packs
+// (row << 16) | column, the row being that of lane 0 of the reading warp.
+constexpr int ACC_LD = 132;
+constexpr int ACC_COLS = 128;
+constexpr int ACC_SMEM_BYTES = ACC_COLS * ACC_LD * 4;
+
+__device__ __forceinline__ uint32_t acc_word_addr(uint32_t acc_smem, uint32_t taddr) {
+    const uint32_t lane = threadIdx.x & 31;
+    return acc_smem + (((taddr & 0xFFFFu) * ACC_LD + (taddr >> 16) + lane) << 2);
+}
+template <int NC>
+__device__ __forceinline__ void acc_ld(uint32_t acc_smem, uint32_t taddr, uint32_t (&v)[NC]) {
+    const uint32_t a = acc_word_addr(acc_smem, taddr);
+#pragma unroll
+    for (int j = 0; j < NC; j++) asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v[j]) : "r"(a + j * ACC_LD * 4) : "memory");
+}
+
+// Store one warpgroup's accumulator fragment of rows [row0, row0 + 64) x columns [col0, col0 + N) (see wgmma above).
+template <int N, typename T>
+__device__ __forceinline__ void acc_store_frag(uint32_t acc_smem, const T (&d)[N / 2], int row0, int col0) {
+    const int t = threadIdx.x & 127;
+    const int row = row0 + 16 * (t >> 5) + ((t & 31) >> 2);
+    const int col = col0 + 2 * (t & 3);
+#pragma unroll
+    for (int i = 0; i < N / 2; i++) {
+        const uint32_t a = acc_smem + (((col + 8 * (i >> 2) + (i & 1)) * ACC_LD + row + 8 * ((i >> 1) & 1)) << 2);
+        uint32_t w;
+        memcpy(&w, &d[i], 4);
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(w) : "memory");
+    }
+}
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
     return r;
 }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// TMA load whose completion bytes are signalled on the LEADER's mbarrier (`bar` already masked with PEER_BIT_MASK)
-__device__ __forceinline__ void tma_load_4d_2sm(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2,
-                                                int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, "
-        "%5, %6}], [%2];" ::"r"(dst),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-template <int KIND>
-__device__ __forceinline__ void umma2(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    uint32_t z = 0;
-    if (KIND == 0)
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, {%5, %6, %7, %8, %5, %6, %7, %8}, p;\n\t"
-            "}\n" ::"r"(tmem_d),
-            "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(z), "r"(z), "r"(z), "r"(z)
-            : "memory");
-    else
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::2.kind::i8 [%0], %1, %2, %3, {%5, %6, %7, %8, %5, %6, %7, %8}, p;\n\t"
-            "}\n" ::"r"(tmem_d),
-            "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(z), "r"(z), "r"(z), "r"(z)
-            : "memory");
-}
-// completion of this thread's MMAs arrives on the barrier at the same offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_mc(uint32_t bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-                 "h"(mask)
-                 : "memory");
-}
-
-// 32 lanes x 32 columns of 32-bit accumulators: thread t of the warp receives TMEM lane
-// (lane_base + t), columns [col, col+32).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ------------------------------------------------------------------ descriptors
 // Shared-memory matrix descriptor for a K-major operand tile stored as rows of 128 bytes with the
 // 128B swizzle (what a TMA box {128 B, rows} with CU_TENSOR_MAP_SWIZZLE_128B writes):
 //   [0,14)  start address >> 4       [16,30) leading byte offset >> 4 (unused for swizzled K-major: 1)
 //   [32,46) stride byte offset >> 4  (8 rows * 128 B = 1024 -> 64)
-//   [46,48) version = 1 (Blackwell)  [49,52) base offset = 0 (tile base 1024-B aligned)
-//   [61,64) layout type: 2 = SWIZZLE_128B
+//   [49,52) base offset = 0 (tile base 1024-B aligned)
+//   [62,64) layout type: 1 = SWIZZLE_128B
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
     d |= static_cast<uint64_t>(1) << 16;
     d |= static_cast<uint64_t>(1024 >> 4) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
+    d |= static_cast<uint64_t>(1) << 62;
     return d;
 }
 

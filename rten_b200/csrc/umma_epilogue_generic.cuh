@@ -1,23 +1,23 @@
-// Specialised (FAST = 1 / 2) and generic (FAST = 0) epilogues of the tcgen05 GEMM / conv kernel: every zero-point, scale,
+// Specialised (FAST = 1 / 2) and generic (FAST = 0) epilogues of the wgmma GEMM / conv kernel: every zero-point, scale,
 // range, split-K and edge case of the operator family; the plain variants (umma_epilogue_plain.cuh) take the common cases.
 // Included by umma_kernel.cuh.
 #pragma once
 
 namespace rtb {
 
-template <int KIND, int FAST, int CTA2>
+template <int KIND, int FAST>
 __device__ __forceinline__ void epilogue_fast(const EpiCtx& c) {
     const KParams& p = c.p;
     const SmemLayout& L = c.L;
     uint8_t* const stg_base = c.stg_base;
     const int nbuf = c.nbuf;
-    uint64_t* const tmem_full = c.tmem_full;
-    uint64_t* const tmem_empty = c.tmem_empty;
+    uint64_t* const acc_full = c.acc_full;
+    uint64_t* const acc_empty = c.acc_empty;
     uint64_t* const res_bar = c.res_bar;
     int* const sk_flag = c.sk_flag;
     const CUtensorMap* const tma_d = c.tma_d;
     const CUtensorMap* const tma_r = c.tma_r;
-    const uint32_t tmem_base = c.tmem_base;
+    const uint32_t acc_smem = c.acc_smem;
     const int cta_rank = c.cta_rank, worker = c.worker, n_workers = c.n_workers;
     PipeState& st = c.st;
     const int warp = c.warp, lane = c.lane;
@@ -57,18 +57,17 @@ __device__ __forceinline__ void epilogue_fast(const EpiCtx& c) {
                 tma_load_4d(stg0 + b0 * STG_BYTES, tma_r, rb, tc0.n0 + grp * 32, tc0.m0, tc0.z0, tc0.z1);
         };
         if (p.res_tma && p.splitk == 1 && issuer && grp * 32 < p.bn) first_residual();
-        mbar_wait(&tmem_full[acc], acc_phase);
+        mbar_wait(&acc_full[acc], acc_phase);
         if (tr && st.it - it0 < 2048) p.trace[4096 + st.it - it0] = clock64();
-        tc_fence_after();
         bool owner = true;
         if (p.splitk > 1) {
-            owner = splitk_publish(p, CTA2 ? 2 * t + cta_rank : t, ks_u, grp, q, lane,
-                                   tmem_base + ((uint32_t)(q * 32) << 16) + acc * ACC_STRIDE, &sk_flag[grp]);
+            owner = splitk_publish(p, t, ks_u, grp, q, lane,
+                                   ((uint32_t)(q * 32) << 16) + acc * ACC_STRIDE, &sk_flag[grp], acc_smem);
             if (owner && p.res_tma && issuer && grp * 32 < p.bn) first_residual();
         }
         for (int sub = 0; owner && sub <= p.pair; sub++) {
             const TileCoord tc = decode_tile(p, t, sub, cta_rank);
-            const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + acc * ACC_STRIDE + sub * p.bn;
+            const uint32_t t_row = ((uint32_t)(q * 32) << 16) + acc * ACC_STRIDE + sub * p.bn;
             // integer zero-point terms of this thread's row:  C = acc - za*colsum[n] - zb[n]*(rowsum - K*za)
             unsigned za_v = 0, t_m = 0;
             bool row_ok = true;
@@ -94,9 +93,9 @@ __device__ __forceinline__ void epilogue_fast(const EpiCtx& c) {
             for (int c0 = grp * 32; c0 < p.bn; c0 += 64) {
                 uint32_t v[32];
                 if (p.splitk > 1)
-                    splitk_sum<KIND>(p, CTA2 ? 2 * t + cta_rank : t, sub, c0, r, v);
+                    splitk_sum<KIND>(p, t, sub, c0, r, v);
                 else
-                    tmem_ld_32x32(t_row + c0, v);
+                    acc_ld(acc_smem, t_row + c0, v);
                 const int nbase = tc.n0 + c0;
                 const int bcur = ci % nbuf;
                 uint8_t* stg = stg0 + bcur * STG_BYTES;
@@ -119,13 +118,11 @@ __device__ __forceinline__ void epilogue_fast(const EpiCtx& c) {
                             tma_load_4d(stg0 + bnext * STG_BYTES, tma_r, rb, tn.n0 + nc0, tn.m0, tn.z0, tn.z1);
                     }
                 }
-                tmem_ld_wait();
                 if (p.ksplit) {
 #pragma unroll
                     for (int h = 0; h < 2; h++) {
                         uint32_t w[16];
-                        tmem_ld_32x16(t_row + p.bn + c0 + h * 16, w);
-                        tmem_ld_wait();
+                        acc_ld(acc_smem, t_row + p.bn + c0 + h * 16, w);
 #pragma unroll
                         for (int j = 0; j < 16; j++) {
                             if (KIND == 0)
@@ -251,13 +248,9 @@ __device__ __forceinline__ void epilogue_fast(const EpiCtx& c) {
                 ci++;
             }
         }
-        tc_fence_before();
         __syncwarp();
         if (lane == 0) {
-            if (CTA2)
-                mbar_arrive_cluster(smem_u32(&tmem_empty[acc]) & PEER_BIT_MASK);  // the leader's MMA warp waits on it
-            else
-                mbar_arrive(&tmem_empty[acc]);
+            mbar_arrive(&acc_empty[acc]);
         }
         if (tr && st.it - it0 < 2048) p.trace[6144 + st.it - it0] = clock64();
     }
@@ -267,7 +260,7 @@ __device__ __forceinline__ void epilogue_fast(const EpiCtx& c) {
     if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
 
-template <int KIND, int CTA2>
+template <int KIND>
 __device__ __forceinline__ void epilogue_generic(const EpiCtx& c) {
     constexpr int FAST = 0;
     (void)FAST;
@@ -275,20 +268,20 @@ __device__ __forceinline__ void epilogue_generic(const EpiCtx& c) {
     const SmemLayout& L = c.L;
     uint8_t* const stg_base = c.stg_base;
     const int nbuf = c.nbuf;
-    uint64_t* const tmem_full = c.tmem_full;
-    uint64_t* const tmem_empty = c.tmem_empty;
+    uint64_t* const acc_full = c.acc_full;
+    uint64_t* const acc_empty = c.acc_empty;
     uint64_t* const res_bar = c.res_bar;
     int* const sk_flag = c.sk_flag;
     const CUtensorMap* const tma_d = c.tma_d;
     const CUtensorMap* const tma_r = c.tma_r;
-    const uint32_t tmem_base = c.tmem_base;
+    const uint32_t acc_smem = c.acc_smem;
     const int cta_rank = c.cta_rank, worker = c.worker, n_workers = c.n_workers;
     PipeState& st = c.st;
     const int warp = c.warp, lane = c.lane;
     (void)L; (void)sk_flag; (void)tma_r; (void)cta_rank; (void)res_bar;
     // ===================== epilogue (generic) =====================
     const EpilogueDesc& e = p.epi;
-    const int q = warp & 3;          // TMEM lane quadrant this warp may access
+    const int q = warp & 3;          // accumulator rows [32 q, 32 q + 32) are this warp's
     const int grp = (warp - 4) >> 2;  // epilogue group: chunks grp, grp+2, ...
     const int r = q * 32 + lane;
     uint8_t* stg0 = stg_base + grp * nbuf * STG_BYTES;
@@ -317,13 +310,12 @@ __device__ __forceinline__ void epilogue_generic(const EpiCtx& c) {
                 tma_load_4d(stg0 + b0 * STG_BYTES, tma_r, rb, tc0.n0 + grp * 32, tc0.m0, tc0.z0, tc0.z1);
         };
         if (p.res_tma && p.splitk == 1 && issuer && grp * 32 < p.bn) first_residual();
-        mbar_wait(&tmem_full[acc], acc_phase);
+        mbar_wait(&acc_full[acc], acc_phase);
         if (p.trace && blockIdx.x == 0 && warp == 4 && lane == 0 && it < 2048) p.trace[4096 + it] = clock64();
-        tc_fence_after();
         bool owner = true;
         if (p.splitk > 1) {
-            owner = splitk_publish(p, CTA2 ? 2 * t + cta_rank : t, ks_u, grp, q, lane,
-                                   tmem_base + ((uint32_t)(q * 32) << 16) + acc * ACC_STRIDE, &sk_flag[grp]);
+            owner = splitk_publish(p, t, ks_u, grp, q, lane,
+                                   ((uint32_t)(q * 32) << 16) + acc * ACC_STRIDE, &sk_flag[grp], acc_smem);
             if (owner && p.res_tma && issuer && grp * 32 < p.bn) first_residual();
         }
         for (int sub = 0; owner && sub <= p.pair; sub++) {
@@ -359,25 +351,24 @@ __device__ __forceinline__ void epilogue_generic(const EpiCtx& c) {
                 if (e.zb) rs_v = e.rowsum[m_idx];
             }
         }
-        const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + acc * ACC_STRIDE + sub * p.bn;
+        const uint32_t t_row = ((uint32_t)(q * 32) << 16) + acc * ACC_STRIDE + sub * p.bn;
         for (int c0 = grp * 32; c0 < p.bn; c0 += 64) {
             const bool tr = p.trace && blockIdx.x == 0 && warp == 4 && lane == 0;
             long long t0 = tr ? clock64() : 0;
             uint32_t v[32];
             const int ncols = (p.bn - c0) >= 32 ? 32 : 16;
             if (p.splitk > 1) {
-                splitk_sum<KIND>(p, CTA2 ? 2 * t + cta_rank : t, sub, c0, r, v);
+                splitk_sum<KIND>(p, t, sub, c0, r, v);
             } else if (ncols == 32) {
-                tmem_ld_32x32(t_row + c0, v);
+                acc_ld(acc_smem, t_row + c0, v);
             } else {
                 uint32_t w[16];
-                tmem_ld_32x16(t_row + c0, w);
+                acc_ld(acc_smem, t_row + c0, w);
 #pragma unroll
                 for (int j = 0; j < 16; j++) v[j] = w[j];
 #pragma unroll
                 for (int j = 16; j < 32; j++) v[j] = 0;
             }
-            tmem_ld_wait();
             if (tr) { const long long t1 = clock64(); p.trace[6144 + 1024 + 0] += t1 - t0; t0 = t1; }
             if (p.ksplit) {
                 // add the second partial accumulator (columns + bn), 16 columns at a time to bound registers
@@ -385,8 +376,7 @@ __device__ __forceinline__ void epilogue_generic(const EpiCtx& c) {
                 for (int h = 0; h < 2; h++) {
                     if (h * 16 < ncols) {
                         uint32_t w[16];
-                        tmem_ld_32x16(t_row + p.bn + c0 + h * 16, w);
-                        tmem_ld_wait();
+                        acc_ld(acc_smem, t_row + p.bn + c0 + h * 16, w);
 #pragma unroll
                         for (int j = 0; j < 16; j++) {
                             if (KIND == 0)
@@ -543,14 +533,10 @@ __device__ __forceinline__ void epilogue_generic(const EpiCtx& c) {
             __syncwarp();
         }
         }  // sub
-        tc_fence_before();
         __syncwarp();
         if (p.trace && blockIdx.x == 0 && warp == 4 && lane == 0 && it < 2048) p.trace[6144 + it] = clock64();
         if (lane == 0) {
-            if (CTA2)
-                mbar_arrive_cluster(smem_u32(&tmem_empty[acc]) & PEER_BIT_MASK);  // the leader's MMA warp waits on it
-            else
-                mbar_arrive(&tmem_empty[acc]);
+            mbar_arrive(&acc_empty[acc]);
         }
     }
     // smem must stay valid until the last bulk store has read it

@@ -1,6 +1,6 @@
-// Plain epilogues of the tcgen05 GEMM / conv kernel: the common f32 case (FAST = 3, + Gelu: 5) and the integer *ToFloat
+// Plain epilogues of the wgmma GEMM / conv kernel: the common f32 case (FAST = 3, + Gelu: 5) and the integer *ToFloat
 // case (FAST = 4, + Gelu: 6) as the shortest instruction streams their roundings allow -- column vectors of the unit in
-// shared memory, packed f32x2 arithmetic, output at the SM's store-port rate (DESIGN.md 4.1).  Included by umma_kernel.cuh.
+// shared memory, paired f32 arithmetic, output at the SM's store-port rate.  Included by umma_kernel.cuh.
 #pragma once
 
 namespace rtb {
@@ -12,16 +12,16 @@ struct EpiCtx {
     const SmemLayout& L;
     uint8_t* stg_base;  // staging buffers behind the operand ring
     int nbuf;
-    uint64_t *tmem_full, *tmem_empty, *res_bar;
+    uint64_t *acc_full, *acc_empty, *res_bar;
     int* sk_flag;
     const CUtensorMap *tma_d, *tma_r;
-    uint32_t tmem_base;
+    uint32_t acc_smem;  // shared-memory address of the accumulator tiles (ptx.cuh)
     int cta_rank, worker, n_workers;
     PipeState& st;
     int warp, lane;
 };
 
-template <int FAST, int CTA2>
+template <int FAST>
 __device__ __forceinline__ void epilogue_plain_f32(const EpiCtx& c) {
     constexpr int KIND = 0;
     (void)KIND;
@@ -29,13 +29,13 @@ __device__ __forceinline__ void epilogue_plain_f32(const EpiCtx& c) {
     const SmemLayout& L = c.L;
     uint8_t* const stg_base = c.stg_base;
     const int nbuf = c.nbuf;
-    uint64_t* const tmem_full = c.tmem_full;
-    uint64_t* const tmem_empty = c.tmem_empty;
+    uint64_t* const acc_full = c.acc_full;
+    uint64_t* const acc_empty = c.acc_empty;
     uint64_t* const res_bar = c.res_bar;
     int* const sk_flag = c.sk_flag;
     const CUtensorMap* const tma_d = c.tma_d;
     const CUtensorMap* const tma_r = c.tma_r;
-    const uint32_t tmem_base = c.tmem_base;
+    const uint32_t acc_smem = c.acc_smem;
     const int cta_rank = c.cta_rank, worker = c.worker, n_workers = c.n_workers;
     PipeState& st = c.st;
     const int warp = c.warp, lane = c.lane;
@@ -85,21 +85,20 @@ __device__ __forceinline__ void epilogue_plain_f32(const EpiCtx& c) {
             const int c = (r >> 5) * 64 + grp * 32 + (r & 31);
             if (c < p.bn && tc0.n0 + c < p.N) bv = __ldg(e.bias + tc0.n0 + c);
         }
-        mbar_wait(&tmem_full[acc], acc_phase);
+        mbar_wait(&acc_full[acc], acc_phase);
         if (tr && st.it - it0 < 2048) p.trace[4096 + st.it - it0] = clock64();
-        tc_fence_after();
         // (the previous unit's readers of bias_s are past their last chunk barrier: every thread arrives there after its math)
         bias_s[r] = bv;
         asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory");
         bool owner = true;
         if (p.splitk > 1) {  // raw partial accumulators to the workspace; the LAST CTA of the tile sums them in split order
-            owner = splitk_publish(p, CTA2 ? 2 * t + cta_rank : t, ks_u, grp, q, lane,
-                                   tmem_base + ((uint32_t)(q * 32) << 16) + acc * ACC_STRIDE, &sk_flag[grp]);
+            owner = splitk_publish(p, t, ks_u, grp, q, lane,
+                                   ((uint32_t)(q * 32) << 16) + acc * ACC_STRIDE, &sk_flag[grp], acc_smem);
             if (owner && p.res_tma && issuer && grp * 32 < p.bn) first_residual();
         }
         for (int sub = 0; owner && sub <= p.pair; sub++) {
             const TileCoord tc = decode_tile(p, t, sub, cta_rank);
-            const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + acc * ACC_STRIDE + sub * p.bn;
+            const uint32_t t_row = ((uint32_t)(q * 32) << 16) + acc * ACC_STRIDE + sub * p.bn;
             int k = 0;
             for (int c0 = grp * 32; c0 < p.bn; c0 += 64, k++) {
                 uint32_t v[32];
@@ -107,7 +106,7 @@ __device__ __forceinline__ void epilogue_plain_f32(const EpiCtx& c) {
                 long long tp0 = 0;
                 if (tr) tp0 = clock64();
 #endif
-#ifdef RTB_TRACE_PHASES  // per-phase clocks of the chunk loop (tools/layer_probe.py); off in production builds
+#ifdef RTB_TRACE_PHASES  // per-phase clocks of the chunk loop; off in production builds
 #define RTB_PLAIN_PHASE(i)                                \
 if (tr) {                                             \
     const long long tp1 = clock64();                  \
@@ -118,9 +117,9 @@ if (tr) {                                             \
 #define RTB_PLAIN_PHASE(i)
 #endif
                 if (p.splitk > 1)
-                    splitk_sum<0>(p, CTA2 ? 2 * t + cta_rank : t, sub, c0, r, v);
+                    splitk_sum<0>(p, t, sub, c0, r, v);
                 else
-                    tmem_ld_32x32(t_row + c0, v);
+                    acc_ld(acc_smem, t_row + c0, v);
                 const int nbase = tc.n0 + c0;
                 const int bcur = ci % nbuf;
                 uint8_t* stg = stg0 + bcur * STG_BYTES;
@@ -146,16 +145,13 @@ if (tr) {                                             \
                 RTB_PLAIN_PHASE(0)
                 if (p.ksplit) {  // even / odd K blocks accumulated separately (KParams::ksplit): add the second accumulator
                     uint32_t w0[16], w1[16];
-                    tmem_ld_32x16(t_row + p.bn + c0, w0);
-                    tmem_ld_wait();
-                    tmem_ld_32x16(t_row + p.bn + c0 + 16, w1);
+                    acc_ld(acc_smem, t_row + p.bn + c0, w0);
+                    acc_ld(acc_smem, t_row + p.bn + c0 + 16, w1);
 #pragma unroll
                     for (int j = 0; j < 16; j += 2) add_f32x2(v[j], v[j + 1], __uint_as_float(w0[j]), __uint_as_float(w0[j + 1]));
-                    tmem_ld_wait();
 #pragma unroll
                     for (int j = 0; j < 16; j += 2) add_f32x2(v[16 + j], v[17 + j], __uint_as_float(w1[j]), __uint_as_float(w1[j + 1]));
                 } else {
-                    tmem_ld_wait();
                 }
                 RTB_PLAIN_PHASE(1)
                 if (p.res_tma) {
@@ -218,20 +214,16 @@ if (tr) {                                             \
                 ci++;
             }
         }
-        tc_fence_before();
         __syncwarp();
         if (lane == 0) {
-            if (CTA2)
-                mbar_arrive_cluster(smem_u32(&tmem_empty[acc]) & PEER_BIT_MASK);  // the leader's MMA warp waits on it
-            else
-                mbar_arrive(&tmem_empty[acc]);
+            mbar_arrive(&acc_empty[acc]);
         }
         if (tr && st.it - it0 < 2048) p.trace[6144 + st.it - it0] = clock64();
     }
     if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
 
-template <int FAST, int CTA2>
+template <int FAST>
 __device__ __forceinline__ void epilogue_plain_i8(const EpiCtx& c) {
     constexpr int KIND = 1;
     (void)KIND;
@@ -239,13 +231,13 @@ __device__ __forceinline__ void epilogue_plain_i8(const EpiCtx& c) {
     const SmemLayout& L = c.L;
     uint8_t* const stg_base = c.stg_base;
     const int nbuf = c.nbuf;
-    uint64_t* const tmem_full = c.tmem_full;
-    uint64_t* const tmem_empty = c.tmem_empty;
+    uint64_t* const acc_full = c.acc_full;
+    uint64_t* const acc_empty = c.acc_empty;
     uint64_t* const res_bar = c.res_bar;
     int* const sk_flag = c.sk_flag;
     const CUtensorMap* const tma_d = c.tma_d;
     const CUtensorMap* const tma_r = c.tma_r;
-    const uint32_t tmem_base = c.tmem_base;
+    const uint32_t acc_smem = c.acc_smem;
     const int cta_rank = c.cta_rank, worker = c.worker, n_workers = c.n_workers;
     PipeState& st = c.st;
     const int warp = c.warp, lane = c.lane;
@@ -256,7 +248,7 @@ __device__ __forceinline__ void epilogue_plain_i8(const EpiCtx& c) {
     // with every operation rounded separately (bit-identical to the operator chain), plus the output's (min, max)
     // for the next DynamicQuantizeLinear.  The three column vectors of the unit are computed once into shared memory
     // while the main loop runs (the specialised epilogue fetched them with 24 dependent 128-bit global loads per
-    // chunk behind the accumulator wait), products / sums use packed f32x2 instructions.
+    // chunk behind the accumulator wait), products / sums are done two lanes at a time.
     const EpilogueDesc& e = p.epi;
     const int q = warp & 3;
     const int grp = (warp - 4) >> 2;
@@ -305,16 +297,15 @@ __device__ __forceinline__ void epilogue_plain_i8(const EpiCtx& c) {
                 if (has_bias) bv = __ldg(e.bias + n);
             }
         }
-        mbar_wait(&tmem_full[acc], acc_phase);
+        mbar_wait(&acc_full[acc], acc_phase);
         if (tr && st.it - it0 < 2048) p.trace[4096 + st.it - it0] = clock64();
-        tc_fence_after();
         zc_s[r] = zc;
         scl_s[r] = sc;
         bias_s[r] = bv;
         asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory");
         for (int sub = 0; sub <= p.pair; sub++) {
             const TileCoord tc = decode_tile(p, t, sub, cta_rank);
-            const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + acc * ACC_STRIDE + sub * p.bn;
+            const uint32_t t_row = ((uint32_t)(q * 32) << 16) + acc * ACC_STRIDE + sub * p.bn;
             bool row_ok = true;
             if (e.range) {  // rows of the tile beyond the tensor must not enter the range
                 if (p.conv) {
@@ -329,7 +320,7 @@ __device__ __forceinline__ void epilogue_plain_i8(const EpiCtx& c) {
             int k = 0;
             for (int c0 = grp * 32; c0 < p.bn; c0 += 64, k++) {
                 uint32_t v[32];
-                tmem_ld_32x32(t_row + c0, v);
+                acc_ld(acc_smem, t_row + c0, v);
                 const int nbase = tc.n0 + c0;
                 const int bcur = ci % nbuf;
                 uint8_t* stg = stg0 + bcur * STG_BYTES;
@@ -354,16 +345,13 @@ __device__ __forceinline__ void epilogue_plain_i8(const EpiCtx& c) {
                 }
                 if (p.ksplit) {  // even / odd K blocks accumulated separately: exact integer sum of the two accumulators
                     uint32_t w0[16], w1[16];
-                    tmem_ld_32x16(t_row + p.bn + c0, w0);
-                    tmem_ld_wait();
-                    tmem_ld_32x16(t_row + p.bn + c0 + 16, w1);
+                    acc_ld(acc_smem, t_row + p.bn + c0, w0);
+                    acc_ld(acc_smem, t_row + p.bn + c0 + 16, w1);
 #pragma unroll
                     for (int j = 0; j < 16; j++) v[j] += w0[j];
-                    tmem_ld_wait();
 #pragma unroll
                     for (int j = 0; j < 16; j++) v[16 + j] += w1[j];
                 } else {
-                    tmem_ld_wait();
                 }
                 if (p.res_tma) {
                     mbar_wait(&res_bar[grp * 4 + bcur], (rphase >> bcur) & 1);
@@ -441,13 +429,9 @@ __device__ __forceinline__ void epilogue_plain_i8(const EpiCtx& c) {
                 ci++;
             }
         }
-        tc_fence_before();
         __syncwarp();
         if (lane == 0) {
-            if (CTA2)
-                mbar_arrive_cluster(smem_u32(&tmem_empty[acc]) & PEER_BIT_MASK);  // the leader's MMA warp waits on it
-            else
-                mbar_arrive(&tmem_empty[acc]);
+            mbar_arrive(&acc_empty[acc]);
         }
         if (tr && st.it - it0 < 2048) p.trace[6144 + st.it - it0] = clock64();
     }

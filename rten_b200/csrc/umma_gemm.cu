@@ -1,25 +1,25 @@
-// tcgen05 GEMM / implicit-GEMM convolution for sm_100a.
+// wgmma GEMM / implicit-GEMM convolution for sm_90a.
 //
 // Replaces rten-gemm's packed BLIS-style GEMM (rten-gemm/src/lib.rs:794-1093, micro-kernels
 // rten-gemm/src/kernels/simd_generic.rs:285,576) and the im2col packing
 // (rten-gemm/src/im2col.rs:110-389) on the MatMul / MatMulInteger / Conv / ConvInteger path.
 //
-// Persistent, warp-specialised kernel, one CTA of 384 threads per SM (or one CTA per SM of a CTA pair):
-//   warp 0   : TMA producer   -- cp.async.bulk.tensor tiles of A (128 rows x 128 B, two of them in pair mode) and B
-//                                (bn rows x 128 B; half of them per CTA in CTA-pair mode) into a ring of 128B-swizzled
-//                                shared-memory stages; starts before the rest of the CTA has finished its set-up
-//   warp 1   : MMA issuer     -- one elected thread issues tcgen05.mma (kind::tf32 or kind::i8, cta_group::1 or ::2),
-//                                4 instructions per 128-byte K block, accumulating in TMEM
-//   warp 2   : TMEM allocator -- 512 columns = 2 accumulator stages of up to 256 columns (or one of 512)
+// Persistent, warp-specialised kernel, one CTA of 416 threads per SM:
+//   warp 12  : TMA producer   -- cp.async.bulk.tensor tiles of A (128 rows x 128 B) and B (bn rows x 128 B) into a
+//                                ring of 128B-swizzled shared-memory stages; starts before the rest of the CTA has
+//                                finished its set-up
+//   warps 0-3: MMA warpgroup  -- wgmma (tf32 -> f32 or 8-bit -> s32), 8 instructions per 128-byte K block (two 64-row
+//                                halves), accumulating in registers; a finished tile goes to one of two accumulator
+//                                stages of 64 columns in shared memory
 //   warps 4-11: epilogue      -- two groups of 4 warps, each taking every other 32-column chunk of the tile:
-//                                tcgen05.ld accumulator rows -> registers -> fused epilogue (alpha, residual /
+//                                accumulator rows -> registers -> fused epilogue (alpha, residual /
 //                                beta*C, bias, activation; or the integer zero-point correction, cast*scale, bias,
 //                                residual, activation; optionally the output's min / max) -> 128B-swizzled smem
 //                                staging -> cp.async.bulk.tensor store (full-line writes; TMA clips rows/columns
 //                                outside the output).  Outputs whose rows are not contiguous fall back to direct
 //                                register->global stores.  Runs concurrently with the next tile's main loop thanks
-//                                to the second TMEM stage.
-// Work decomposition (tile width, pair, split-K, CTA pair ...) is a launch `Plan` (see "Launch plans" below), ranked by
+//                                to the second accumulator stage.
+// Work decomposition (tile width, split-K, K blocks per stage) is a launch `Plan` (see "Launch plans" below), ranked by
 // a cost model and, optionally, measured on the device per problem.
 // For Conv the A tile is a TMA box over the NHWC activation tensor at (c0, ox0*sx - pad + kx*dx,
 // oy0*sy - pad + ky*dy, b0): padding comes from TMA out-of-bounds zero fill, the stride from the
@@ -150,62 +150,55 @@ struct Prepared {
 };
 
 constexpr int SK_CNT_INTS = 1 << 16;
-// 1 KB alignment slack, 1 KB barriers, column vectors of the plain epilogues (f32: 1 KB, integer kind: 3 KB)
-static int smem_budget_for(int n_stg, int kind) { return 227 * 1024 - (kind == 0 ? 3072 : 5120) - n_stg * STG_BYTES; }
+// 227 KB of shared memory per block; SMEM_FIXED_BYTES: alignment slack, barriers, column vectors, accumulators
+static int smem_budget_for(int n_stg, int /*kind*/) { return 227 * 1024 - SMEM_FIXED_BYTES - n_stg * STG_BYTES; }
 
 struct PlanShape {
     long long tiles_n, units_m, tiles, units;
     int kb_per, atom_bytes, stage_bytes, stages, n_stg;
 };
 
-// Derived sizes of a plan; false if the plan cannot run (TMEM columns, shared memory, counters).
+// Derived sizes of a plan; false if the plan cannot run (accumulator columns, shared memory, counters).  The kernel
+// computes one 128 x bn tile per unit, bn in {32, 64}: pair / ksplit / acc1 / cta2 are not available on sm_90.
 static bool plan_shape(const Prepared& q, const Plan& pl, PlanShape& ps) {
     const KParams& p = q.p;
-    if (pl.bn < 16 || pl.bn > 256 || pl.bn % q.step) return false;
-    if (pl.pair && p.tiles_m < 2) return false;
-    if (pl.cta2 && (p.tiles_m < 2 || pl.bn % 32)) return false;
-    if (pl.acc1 != ((pl.pair && pl.bn > 128) ? 1 : 0)) return false;
-    if (pl.ksplit && (pl.pair || pl.bn > 128 || pl.splitk > 1)) return false;
+    if (pl.bn < 16 || pl.bn > ACC_STRIDE || pl.bn % 32 || pl.bn % q.step) return false;
+    if (pl.pair || pl.ksplit || pl.acc1 || pl.cta2 || pl.katoms != 1) return false;  // one K block per stage: straight-line wgmma issue
     ps.tiles_n = (p.N + pl.bn - 1) / pl.bn;
-    const int mult = (pl.pair + 1) * (pl.cta2 + 1);
-    ps.units_m = (p.tiles_m + mult - 1) / mult;
+    ps.units_m = p.tiles_m;
     ps.tiles = ps.units_m * ps.tiles_n * q.batch;
     ps.units = ps.tiles * pl.splitk;
     if (ps.units > 0x7FFFFFFFll) return false;
     ps.kb_per = (p.k_blocks + pl.splitk - 1) / pl.splitk;
     if (pl.splitk > 1) {
         if (pl.bn % 32 || (long long)(pl.splitk - 1) * ps.kb_per >= p.k_blocks) return false;  // no empty split
-        if (ps.tiles * 2 * (pl.cta2 + 1) > SK_CNT_INTS) return false;
+        if (ps.tiles * 2 > SK_CNT_INTS) return false;
     }
     ps.n_stg = 2 * pl.nbuf;
-    ps.atom_bytes = (pl.pair ? 2 : 1) * A_STAGE_BYTES + (pl.bn >> pl.cta2) * KBYTES;  // pair mode: half of B per CTA
-    if (pl.katoms == 2 && ps.kb_per < 2) return false;
-    ps.stage_bytes = ps.atom_bytes * pl.katoms;
+    ps.atom_bytes = A_STAGE_BYTES + pl.bn * KBYTES;
+    ps.stage_bytes = ps.atom_bytes;
     ps.stages = std::min(MAX_STAGES, smem_budget_for(ps.n_stg, q.esize == 4 ? 0 : 1) / ps.stage_bytes);
     if (ps.stages < 2) return false;
     return true;
 }
 
-// Cost model in SM clocks.  Constants measured with the in-kernel trace (tools/trace_probe.py,
-// profiles/r01_trace_pipeline.txt) and from whole-layer timings:
-//   * the operand stream L2 -> shared memory is the first limit: ~7400 B/clk for the whole chip (all SMs loading),
-//     at most ~64 B/clk for one SM -> a K block of `atom_bytes` cannot take less than atom_bytes / bw;
-//   * the tensor pipe needs bn/2 clk per 128 x bn x 32-byte MMA, the elected thread ~42 clk to issue it;
-//   * every pipeline stage costs the issuing warp a fixed ~320 clk (barrier wait, fence, descriptors, commit);
-//   * a stage cannot complete faster than TMA latency (~2300 clk under load) / stages in flight;
-//   * the epilogue (~350 clk per 32-column chunk, two warp groups) overlaps the next main loop unless acc1.
+// Cost model in SM clocks.  Its constants are unmeasured estimates that only rank candidate plans:
+//   * the operand stream L2 -> shared memory (~7400 B/clk for the whole chip, at most ~64 B/clk for one SM) bounds a K block;
+//   * the tensor pipe needs bn/2 clk per 128 x bn x 32-byte step, issuing it ~42 clk;
+//   * every pipeline stage costs a fixed ~320 clk (barrier wait, fence, descriptors, commit);
+//   * a stage cannot complete faster than the TMA latency (~2300 clk under load) / stages in flight;
+//   * the epilogue (~350 clk per 32-column chunk, two warp groups) overlaps the next main loop.
 static double plan_cost(const Prepared& q, const Plan& pl, const PlanShape& ps, int num_sms) {
-    const int workers = pl.cta2 ? num_sms / 2 : num_sms;
-    const double active = (double)std::min<long long>(ps.units, workers) * (pl.cta2 + 1);
-    const double waves = std::ceil((double)ps.units / workers);
+    const double active = (double)std::min<long long>(ps.units, num_sms);
+    const double waves = std::ceil((double)ps.units / num_sms);
     const double bw = std::min(64.0, 7400.0 / active);
-    const double mmas = 4.0 * (pl.pair ? 2 : 1);
+    const double mmas = 4.0;
     const double t_kb = std::max(mmas * std::max(42.0, pl.bn / 2.0), ps.atom_bytes / bw);
-    double t_stage = std::max(pl.katoms * t_kb, 320.0 + pl.katoms * mmas * 42.0);
+    double t_stage = std::max(t_kb, 320.0 + mmas * 42.0);
     t_stage = std::max(t_stage, 2300.0 / ps.stages);
-    const double mainloop = std::ceil((double)ps.kb_per / pl.katoms) * t_stage;
-    const double epi = (pl.pair ? 2 : 1) * (pl.bn / 32.0) * 350.0 / 2.0 + 600.0;
-    double unit = pl.acc1 ? mainloop + epi + 1000.0 : std::max(mainloop, epi) + 1500.0;
+    const double mainloop = ps.kb_per * t_stage;
+    const double epi = (pl.bn / 32.0) * 350.0 / 2.0 + 600.0;
+    double unit = std::max(mainloop, epi) + 1500.0;
     double cost = waves * unit + 2500.0;
     if (pl.splitk > 1) cost += epi * (1.0 + 0.25 * pl.splitk) + 1500.0;  // publish + the owner's reduction
 
@@ -216,41 +209,31 @@ static void enumerate_plans(const Prepared& q, int num_sms, std::vector<std::pai
     const KParams& p = q.p;
     const int nmax = (p.N + q.step - 1) / q.step * q.step;
     static const int splits[] = {1, 2, 3, 4, 5, 6, 8, 10, 12, 16};
-    const bool allow_cta2 = !getenv("RTEN_B200_NO_CTA2");
-    for (int cta2 = 0; cta2 <= (allow_cta2 ? 1 : 0); cta2++)
-    for (int pair = 0; pair <= 1; pair++)
-        for (int bn = q.step; bn <= 256; bn += q.step) {
-            if (bn > nmax && bn != q.step) break;
-            for (int katoms = 1; katoms <= 2; katoms++)
-                for (int sk : splits) {
-                    Plan pl;
-                    pl.cta2 = cta2;
-                    pl.bn = bn;
-                    pl.pair = pair;
-                    pl.katoms = katoms;
-                    pl.splitk = sk;
-                    pl.acc1 = (pair && bn > 128) ? 1 : 0;
-                    if (sk > 1 && p.k_blocks / sk < 4) continue;
-                    pl.ksplit = (!pair && bn <= 128 && sk == 1 && !getenv("RTEN_B200_NO_KSPLIT")) ? 1 : 0;
-                    const int kb_per = (p.k_blocks + sk - 1) / sk;
-                    pl.nbuf = pl.acc1 ? 1 : ((q.res_tma || kb_per < 24) ? 2 : 1);
-                    PlanShape ps;
-                    if (pl.nbuf == 2 && !getenv("RTEN_B200_NO_NBUF3")) {
-                        // A third staging buffer per group takes the wait for the previous store's shared-memory read (a
-                        // 16 KB bulk store drains at the SM's ~32 B/clk write port: ~900 clk) and, with a residual, the
-                        // late request of the next residual tile off the chunk's critical path -- as long as the operand
-                        // ring keeps three stages (or loses none)
-                        PlanShape ps2;
-                        const bool ok2 = plan_shape(q, pl, ps2);
-                        pl.nbuf = 3;
-                        if (!plan_shape(q, pl, ps) || (ps.stages < 3 && !(ok2 && ps.stages == ps2.stages))) pl.nbuf = 2;
-                    }
-                    if (!plan_shape(q, pl, ps)) continue;
-                    if (sk > 1 && ps.tiles * (cta2 + 1) >= 2 * num_sms) continue;  // enough parallelism without splitting K
-                    if (ps.stages < 3 && !(katoms == 1 && ps.stages == 2)) continue;
-                    out.emplace_back(plan_cost(q, pl, ps, num_sms), pl);
-                }
+    for (int bn = 32; bn <= ACC_STRIDE; bn += 32) {
+        if (bn > nmax && bn != 32) break;
+        for (int sk : splits) {
+            Plan pl;
+            pl.bn = bn;
+            pl.splitk = sk;
+            if (sk > 1 && p.k_blocks / sk < 4) continue;
+            const int kb_per = (p.k_blocks + sk - 1) / sk;
+            pl.nbuf = (q.res_tma || kb_per < 24) ? 2 : 1;
+            PlanShape ps;
+            if (pl.nbuf == 2 && !getenv("RTEN_B200_NO_NBUF3")) {
+                // A third staging buffer per group takes the wait for the previous store's shared-memory read and, with a
+                // residual, the late request of the next residual tile off the chunk's critical path -- as long as the
+                // operand ring keeps three stages (or loses none)
+                PlanShape ps2;
+                const bool ok2 = plan_shape(q, pl, ps2);
+                pl.nbuf = 3;
+                if (!plan_shape(q, pl, ps) || (ps.stages < 3 && !(ok2 && ps.stages == ps2.stages))) pl.nbuf = 2;
+            }
+            if (!plan_shape(q, pl, ps)) continue;
+            if (sk > 1 && ps.tiles >= 2 * num_sms) continue;  // enough parallelism without splitting K
+            if (ps.stages < 2) continue;
+            out.emplace_back(plan_cost(q, pl, ps, num_sms), pl);
         }
+    }
     std::sort(out.begin(), out.end(), [](const std::pair<double, Plan>& x, const std::pair<double, Plan>& y) {
         return x.first < y.first;
     });
@@ -428,7 +411,7 @@ static void fill_launch_attrs(cudaLaunchConfig_t& cfg, cudaLaunchAttribute* attr
 // cls = kind * 3 + epilogue variant
 static rten_status launch_single(rten_ctx* ctx, int cls, const PendingLaunch& pl) {
     const KParams& p = pl.p;
-    const int grid = p.cta2 ? 2 * std::min(p.units_total, ctx->num_sms / 2) : std::min(p.units_total, ctx->num_sms);
+    const int grid = std::min(p.units_total, ctx->num_sms);
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(grid);
@@ -436,7 +419,7 @@ static rten_status launch_single(rten_ctx* ctx, int cls, const PendingLaunch& pl
     cfg.dynamicSmemBytes = pl.smem_bytes;
     cfg.stream = ctx->stream;
     cudaLaunchAttribute attr[2];
-    fill_launch_attrs(cfg, attr, p.cta2 != 0);
+    fill_launch_attrs(cfg, attr, false);
     auto launch = [&](auto kern) -> cudaError_t {
         cudaError_t e2 = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         if (e2 != cudaSuccess) return e2;
@@ -444,27 +427,21 @@ static rten_status launch_single(rten_ctx* ctx, int cls, const PendingLaunch& pl
     };
     cudaError_t e;
     if (pl.plain && cls == 1) {
-        e = p.cta2 ? launch(umma_gemm_kernel<0, 3, 1>) : launch(umma_gemm_kernel<0, 3, 0>);
+        e = launch(umma_gemm_kernel<0, 3>);
     } else if (pl.plain && cls == 2) {
-        e = p.cta2 ? launch(umma_gemm_kernel<0, 5, 1>) : launch(umma_gemm_kernel<0, 5, 0>);
+        e = launch(umma_gemm_kernel<0, 5>);
     } else if (pl.plain && cls == 5) {
-        e = p.cta2 ? launch(umma_gemm_kernel<1, 6, 1>) : launch(umma_gemm_kernel<1, 6, 0>);
+        e = launch(umma_gemm_kernel<1, 6>);
     } else if (pl.plain && cls == 4) {
-        e = p.cta2 ? launch(umma_gemm_kernel<1, 4, 1>) : launch(umma_gemm_kernel<1, 4, 0>);
+        e = launch(umma_gemm_kernel<1, 4>);
     } else
-    switch (cls * 2 + (p.cta2 ? 1 : 0)) {
-        case 0: e = launch(umma_gemm_kernel<0, 0, 0>); break;
-        case 1: e = launch(umma_gemm_kernel<0, 0, 1>); break;
-        case 2: e = launch(umma_gemm_kernel<0, 1, 0>); break;
-        case 3: e = launch(umma_gemm_kernel<0, 1, 1>); break;
-        case 4: e = launch(umma_gemm_kernel<0, 2, 0>); break;
-        case 5: e = launch(umma_gemm_kernel<0, 2, 1>); break;
-        case 6: e = launch(umma_gemm_kernel<1, 0, 0>); break;
-        case 7: e = launch(umma_gemm_kernel<1, 0, 1>); break;
-        case 8: e = launch(umma_gemm_kernel<1, 1, 0>); break;
-        case 9: e = launch(umma_gemm_kernel<1, 1, 1>); break;
-        case 10: e = launch(umma_gemm_kernel<1, 2, 0>); break;
-        default: e = launch(umma_gemm_kernel<1, 2, 1>); break;
+    switch (cls) {
+        case 0: e = launch(umma_gemm_kernel<0, 0>); break;
+        case 1: e = launch(umma_gemm_kernel<0, 1>); break;
+        case 2: e = launch(umma_gemm_kernel<0, 2>); break;
+        case 3: e = launch(umma_gemm_kernel<1, 0>); break;
+        case 4: e = launch(umma_gemm_kernel<1, 1>); break;
+        default: e = launch(umma_gemm_kernel<1, 2>); break;
     }
     if (e != cudaSuccess) return fail_cuda(ctx, e, "umma_gemm launch");
     e = cudaGetLastError();
@@ -564,9 +541,9 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
     p.stages = std::min(MAX_STAGES, smem_budget_for(n_stg, L.kind) / (int)p.stage_bytes);
     if (p.stages < 2) return RTEN_ERR_UNSUPPORTED_VALUE;
     if (L.kind == 0)
-        p.idesc = make_idesc(1 /*F32*/, 2 /*TF32*/, 2, BM << p.cta2, p.bn);
+        p.idesc = make_idesc(1 /*F32*/, 2 /*TF32*/, 2, BM, p.bn);
     else
-        p.idesc = make_idesc(2 /*S32*/, L.a_signed ? 1 : 0, L.b_signed ? 1 : 0, BM << p.cta2, p.bn);
+        p.idesc = make_idesc(2 /*S32*/, L.a_signed ? 1 : 0, L.b_signed ? 1 : 0, BM, p.bn);
     if (p.splitk > 1) {
         RTB_TRY(ensure_splitk_counters(ctx));
         if (!ws) RTB_TRY(temp_alloc(ctx, splitk_ws_bytes(ps, pl), &ws));
@@ -595,7 +572,7 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
         fprintf(stderr, "[umma_gemm] kind=%d conv=%d M=%d N=%d K=%d kb=%d tiles_m=%d bn=%d pair=%d ksplit=%d katoms=%d splitk=%d acc1=%d cta2=%d units=%d stages=%d tma_store=%d res_tma=%d nbuf=%d box=%dx%dx%d\n",
                 L.kind, L.conv, L.M, L.N, L.K, p.k_blocks, p.tiles_m, p.bn, p.pair, p.ksplit, p.katoms, p.splitk, p.acc1, p.cta2,
                 p.units_total, p.stages, p.tma_store, p.res_tma, p.nbuf, p.tw, p.th, p.tb);
-    const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + n_stg * STG_BYTES + 1024 /*align*/ + 1024 /*barriers*/ + (L.kind == 0 ? 1024 : 3072) /*column vectors*/;
+    const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + n_stg * STG_BYTES + SMEM_FIXED_BYTES;
     // specialised epilogue when every chunk qualifies for the register fast path
     const EpilogueDesc& ee = L.epi;
     bool fastk = p.tma_store && (L.N % 32) == 0 && (!ctx->trace || getenv("RTEN_B200_TRACE_FAST")) && !getenv("RTEN_B200_NO_FAST");
@@ -627,9 +604,8 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
     // kernel class = data kind x epilogue variant (0 generic, 1 specialised, 2 specialised + out-of-line Gelu)
     const int cls = L.kind * 3 + (fastk ? (ee.act > 1 ? 2 : 1) : 0);
     // Opt-in (RTEN_B200_SEQ=1): inside graph capture consecutive launches are collected and run as ONE sequence kernel
-    // (umma_seq_kernel).  Measured on B200 (tools/boundary_probe.py): a layer boundary inside the sequence kernel costs
-    // ~2.3 us MORE than a programmatic-dependent-launch kernel boundary (drain + grid barrier + cold operand pipe are not
-    // cheaper than what PDL already overlaps), so separate launches stay the default.
+    // (umma_seq_kernel).  A layer boundary inside the sequence kernel (drain + grid barrier + cold operand pipe) is not
+    // cheaper than what programmatic dependent launch already overlaps, so separate launches stay the default.
     const char* seq_env = getenv("RTEN_B200_SEQ");
     const bool seq_on = seq_env && atoi(seq_env) != 0;
     if (seq_on && ctx->capturing && !p.cta2 && !p.x3_cb && !ctx->trace && !no_defer && cls % 3 != 2) {
@@ -767,8 +743,7 @@ rten_status launch_umma_gemm(rten_ctx* ctx, const GemmLaunch& L) {
     Prepared q;
     RTB_TRY(prepare_launch(ctx, L, q));
     const bool verbose = getenv("RTEN_B200_VERBOSE") != nullptr;
-    const bool forced = getenv("RTEN_B200_FORCE_BN") || getenv("RTEN_B200_FORCE_PAIR") || getenv("RTEN_B200_FORCE_KATOMS") ||
-                        getenv("RTEN_B200_FORCE_SPLITK") || getenv("RTEN_B200_FORCE_CTA2");
+    const bool forced = getenv("RTEN_B200_FORCE_BN") || getenv("RTEN_B200_FORCE_SPLITK");
     if (!forced && !ctx->tune_cache.empty()) {  // measured plan on record: no need to enumerate and rank candidates
         auto hit = ctx->tune_cache.find(tune_key(L, q));
         if (hit != ctx->tune_cache.end()) {
@@ -791,18 +766,12 @@ rten_status launch_umma_gemm(rten_ctx* ctx, const GemmLaunch& L) {
     if (forced) {
         // debugging / sweeps: the best-ranked candidate that matches every forced field
         const char* fb = getenv("RTEN_B200_FORCE_BN");
-        const char* fp = getenv("RTEN_B200_FORCE_PAIR");
-        const char* fk = getenv("RTEN_B200_FORCE_KATOMS");
         const char* fs = getenv("RTEN_B200_FORCE_SPLITK");
-        const char* fc = getenv("RTEN_B200_FORCE_CTA2");
         bool found = false;
         for (const auto& c : cands) {
             const Plan& x = c.second;
             if (fb && x.bn != atoi(fb)) continue;
-            if (fp && x.pair != (atoi(fp) ? 1 : 0)) continue;
-            if (fk && x.katoms != atoi(fk)) continue;
             if (fs && x.splitk != atoi(fs)) continue;
-            if (fc && x.cta2 != (atoi(fc) ? 1 : 0)) continue;
             plan = x;
             found = true;
             break;
@@ -895,9 +864,9 @@ rten_status launch_umma_gemm(rten_ctx* ctx, const GemmLaunch& L) {
                 // stride-1 windows: the halo-reuse kernel (umma_halo.cu) over a few unit shapes, same timing
                 int halo_bn = 0, halo_T = 0;
                 if (L.conv && L.kind == 0 && L.g.kh * L.g.kw > 1 && !L.x3_cb && !getenv("RTEN_B200_NO_HALO")) {
-                    for (int hbn : {64, 128, 256})
-                        for (int hT : {1, 2, 4}) {
-                            if (hbn > L.N || hT * hbn > 512) continue;
+                    for (int hbn : {32, 64})  // the halo kernel's unit shapes: one 128-slot tile, bn <= 64
+                        for (int hT : {1}) {
+                            if (hbn > L.N) continue;
                             auto time_halo = [&](int n) -> double {
                                 if (launch_umma_halo_conv(ctx, L, hbn, hT) != RTEN_OK) return -1.0;
                                 cudaEventRecord(e0, ctx->stream);

@@ -1,9 +1,9 @@
-// Launch interface of the tcgen05 GEMM / implicit-GEMM-conv kernel (umma_gemm.cu).
+// Launch interface of the wgmma GEMM / implicit-GEMM-conv kernel (umma_gemm.cu).
 //
 // Computes, per batch z:   D[m, n] = epilogue( sum_k A[m, k] * B[n, k] )
 // with BOTH operands K-major in global memory (k contiguous), fetched by TMA into 128B-swizzled
-// shared-memory tiles and multiplied by tcgen05.mma (kind::tf32 for f32 data, kind::i8 for
-// u8/i8 data) with the accumulator in TMEM.
+// shared-memory tiles and multiplied by wgmma (tf32 for f32 data, s8/u8 for
+// u8/i8 data) with the accumulator in registers.
 //
 // The A operand is either a plain (k, m, z0, z1) tensor or an NHWC activation tensor addressed
 // as an implicit im2col matrix: row = output pixel (b, oy, ox), k = (ky, kx, c).

@@ -1,16 +1,17 @@
-// Halo-reuse convolution on tcgen05: stride-1 convolutions with a kh x kw window (the 3x3 layers of ResNet-50).
+// Halo-reuse convolution on wgmma: stride-1 convolutions with a kh x kw window (the 3x3 layers of ResNet-50).
 //
 // The generic implicit-GEMM kernel (umma_gemm.cu) streams one activation box per filter tap from L2: a 3x3 layer moves
 // its input nine times into shared memory, and at 4 bytes per TF32 operand the L2 -> SM stream, not the tensor pipe, sets
-// its pace (profiles/r01_trace_pipeline_v2.txt).  Here a CTA loads ONE zero-padded activation patch per 32-channel block
+// its pace.  Here a CTA loads ONE zero-padded activation patch per 32-channel block
 //     patch[b][y][x][32 ch]   y in [oy0 - pt, oy0 + R + kh - 1 - pt),  x in [-pl, -pl + P),  P = OW + kw - 1
 // with a single TMA box (out-of-bounds -> 0 = the padding) and treats it as a LINEAR array of P-pitched pixel slots of
 // 128 bytes: output slot s = y P + x reads, for tap (ky, kx), input slot s + ky P + kx.  Every tap is therefore the same
 // patch seen through a shared-memory matrix descriptor whose start address is shifted by (ky P + kx) x 128 bytes -- the
 // 128B swizzle is a function of the absolute shared-memory address, so TMA's layout and the shifted descriptor agree
-// (measured: tools/desc_probe.cu, profiles/r02_desc_probe.txt).  Slots with x >= OW (and the rows past the strip) are
+// (base offset 0; checked against float64 by the halo parity test).  Slots with x >= OW (and the rows past the strip) are
 // computed and thrown away: 2 / P of the MMA rows for a 3x3 window.  The weights stream through a ring of
-// stages of `tps` taps x (bn x 32 channel) tiles (one barrier hand-off per stage).
+// stages of one tap x (bn x 32 channel) tile.  A unit is one 128-slot tile of bn <= 64 output channels, accumulated in
+// the registers of the MMA warpgroup (warps 0-3) and handed to the epilogue warps through shared memory.
 //
 // Replaces rten-gemm/src/im2col.rs:110-212 (the A-operand gather of the packed GEMM) for these layers.
 #include <cuda.h>
@@ -30,7 +31,8 @@ namespace rtb {
 
 namespace {
 
-constexpr int HALO_THREADS = 384;  // warp 0 TMA, warp 1 MMA, warp 2 TMEM, warps 4-11 epilogue
+constexpr int HALO_THREADS = 416;  // warps 0-3 MMA warpgroup, warps 4-11 epilogue, warp 12 TMA
+constexpr int HALO_PRODUCER = 12;
 constexpr int HB_MAX = 8;          // weight ring stages
 
 struct HaloParams {
@@ -46,24 +48,20 @@ struct HaloParams {
     int c_blocks;  // 32-channel blocks
     int taps;
     int strips, units_n, units_total;
-    int acc_stages;     // 1 or 2 TMEM accumulator stages of T * bn columns
+    int acc_stages;     // accumulator stages of bn columns in shared memory (2)
     int b_stages;       // weight ring depth
-    int tps;            // filter taps per weight-ring stage (one barrier hand-off per stage: taps, kw or 1)
+    int tps;            // filter taps per weight-ring stage (1)
     uint32_t patch_bytes, patch_tx, b_bytes;
-    uint32_t idesc;
     long long* trace;  // debug (rten_b200_debug_trace + RTEN_B200_TRACE_FAST): clock64 stamps of CTA 0, layout of the GEMM kernel's
-    uint32_t tap_off[32];  // (ky P + kx) * 8: descriptor offset (16-byte units) of filter tap ky * kw + kx inside the patch
+    uint32_t tap_off[32];  // (ky P + kx) * 128: byte offset of filter tap ky * kw + kx inside the patch
     uint32_t m_img, m_P;  // floor(2^32 / d) + 1 for d = nr * P and d = P: n / d == __umulhi(n, m) for the slot numbers of a unit
     EpilogueDesc epi;
 };
 
-// (a0, a1) += (b0, b1): one packed FADD2, each half rounded to nearest like a scalar add
+// (a0, a1) += (b0, b1) on f32 bit patterns, each half rounded to nearest like a scalar add
 __device__ __forceinline__ void add_pair(uint32_t& a0, uint32_t& a1, float b0, float b1) {
-    unsigned long long a, b, d;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(a) : "r"(a0), "r"(a1));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(b) : "f"(b0), "f"(b1));
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    asm("mov.b64 {%0, %1}, %2;" : "=r"(a0), "=r"(a1) : "l"(d));
+    a0 = __float_as_uint(__fadd_rn(__uint_as_float(a0), b0));
+    a1 = __float_as_uint(__fadd_rn(__uint_as_float(a1), b1));
 }
 
 __device__ __forceinline__ void halo_unit(const HaloParams& p, int u, int& n0, int& oy0, int& b0) {
@@ -75,6 +73,54 @@ __device__ __forceinline__ void halo_unit(const HaloParams& p, int u, int& n0, i
     b0 = (rest / p.strips) * p.tb;
 }
 
+// MMA warpgroup: one 128-slot x N tile per unit, every (channel block, tap) one stage of 8 wgmma (two 64-slot halves).
+template <int N>
+__device__ __forceinline__ void halo_mma(const HaloParams& p, uint64_t* patch_full, uint64_t* patch_empty, uint64_t* b_full,
+                                         uint64_t* b_empty, uint64_t* acc_full, uint64_t* acc_empty, uint8_t* patch0,
+                                         uint8_t* bring, uint32_t acc_smem) {
+    const int lane = threadIdx.x & 31;
+    uint32_t pphase = 0, bphase = 0, aphase = 0;
+    int ps = 0, bs = 0, it = 0;
+    for (int u = blockIdx.x; u < p.units_total; u += gridDim.x, it++) {
+        const int acc = it & 1;
+        float d0[N / 2], d1[N / 2];
+#pragma unroll
+        for (int i = 0; i < N / 2; i++) d0[i] = d1[i] = 0.0f;
+        // (channel block, tap) pairs as one flat loop: the wgmma issue stays in straight-line code
+        const int steps = p.c_blocks * p.taps;
+        for (int i = 0, tap = 0; i < steps; i++) {
+            if (tap == 0) mbar_wait(&patch_full[ps], (pphase >> ps) & 1);
+            mbar_wait(&b_full[bs], (bphase >> bs) & 1);
+            wgmma_fence();
+            // the tap is the SAME patch seen (ky P + kx) pixel slots of 128 bytes further on
+            const uint32_t sa = smem_u32(patch0 + (size_t)ps * p.patch_bytes) + p.tap_off[tap];
+            const uint64_t adesc0 = make_kmajor_sw128_desc(sa), adesc1 = make_kmajor_sw128_desc(sa + 64 * 128);
+            const uint64_t bdesc = make_kmajor_sw128_desc(smem_u32(bring + (size_t)bs * p.b_bytes));
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                wgmma_k<0, 0, N>(d0, adesc0 + 2 * k, bdesc + 2 * k);
+                wgmma_k<0, 0, N>(d1, adesc1 + 2 * k, bdesc + 2 * k);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();  // (one group at a time: the patch / weight releases below follow it directly)
+            if (lane == 0) mbar_arrive(&b_empty[bs]);
+            bphase ^= 1u << bs;
+            if (++bs == p.b_stages) bs = 0;
+            if (++tap == p.taps) {
+                tap = 0;
+                if (lane == 0) mbar_arrive(&patch_empty[ps]);
+                pphase ^= 1u << ps;
+                ps ^= 1;
+            }
+        }
+        mbar_wait(&acc_empty[acc], ((aphase >> acc) & 1) ^ 1);
+        aphase ^= 1u << acc;
+        acc_store_frag<N>(acc_smem, d0, 0, acc * 64);
+        acc_store_frag<N>(acc_smem, d1, 64, acc * 64);
+        mbar_arrive(&acc_full[acc]);
+    }
+}
+
 __global__ void __launch_bounds__(HALO_THREADS, 1)
 umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const __grid_constant__ HaloParams p) {
     extern __shared__ uint8_t smem_raw[];
@@ -83,11 +129,11 @@ umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
     uint64_t* patch_empty = patch_full + 2;
     uint64_t* b_full = patch_empty + 2;                         // [HB_MAX]
     uint64_t* b_empty = b_full + HB_MAX;
-    uint64_t* tmem_full = b_empty + HB_MAX;                     // [2]
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+    uint64_t* acc_full = b_empty + HB_MAX;                     // [2]
+    uint64_t* acc_empty = acc_full + 2;
     float* bias_s = reinterpret_cast<float*>(base + 1024);  // [2 groups][128]: column bias of the current unit
-    uint8_t* stage0 = base + 2048;                             // [2 groups] 128 slots x 128 B output staging (128B-swizzled)
+    const uint32_t acc_smem = smem_u32(base + 2048);          // two accumulator stages of 64 columns (ptx.cuh)
+    uint8_t* stage0 = base + 2048 + ACC_SMEM_BYTES;            // [2 groups] 128 slots x 128 B output staging (128B-swizzled)
     uint8_t* patch0 = stage0 + 2 * 16384;
     uint8_t* bring = patch0 + 2 * (size_t)p.patch_bytes;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -101,30 +147,23 @@ umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
     if (warp == 1) {
         if (lane < 2) {
             mbar_init(&patch_full[lane], 1);
-            mbar_init(&patch_empty[lane], 1);
-            mbar_init(&tmem_full[lane], 1);
-            mbar_init(&tmem_empty[lane], 8);  // one arrival per epilogue warp
+            mbar_init(&patch_empty[lane], 4);  // one arrival per MMA warp
+            mbar_init(&acc_full[lane], 128);  // every thread of the MMA warpgroup stores part of the tile
+            mbar_init(&acc_empty[lane], 8);   // one arrival per epilogue warp
         }
         if (lane < HB_MAX) {
             mbar_init(&b_full[lane], 1);
-            mbar_init(&b_empty[lane], 1);
+            mbar_init(&b_empty[lane], 4);
         }
         fence_mbar_init();
     }
-    if (warp == 2) {
-        tmem_alloc(tmem_ptr, 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
     if (tr0 && threadIdx.x == 0) p.trace[6144 + 1101] = clock64();
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     if (tr0 && threadIdx.x == 0) p.trace[6144 + 1102] = clock64();
 
-    if (warp == 0) {
+    if (warp == HALO_PRODUCER) {
         // ===================== TMA producer =====================
         uint32_t pphase = 0, bphase = 0;  // bit s = uses of stage s so far, mod 2
         int ps = 0, bs = 0, tr_p = 0;
@@ -153,83 +192,15 @@ umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        uint32_t pphase = 0, bphase = 0, aphase = 0;
-        int ps = 0, bs = 0, it = 0, tr_m = 0;
-        // debug trace: where the issuing warp's clocks go (registers; written once at the end)
-        long long c_acc = 0, c_patch = 0, c_b = 0, c_issue = 0, c_commit = 0, n_mma = 0, tq = 0;
-        if (tr0) tq = clock64();
-#define HALO_LAP(var)                    \
-    if (tr0) {                           \
-        const long long now = clock64(); \
-        var += now - tq;                 \
-        tq = now;                        \
-    }
-        for (int u = blockIdx.x; u < p.units_total; u += gridDim.x, it++) {
-            const int acc = p.acc_stages == 2 ? (it & 1) : 0;
-            mbar_wait(&tmem_empty[acc], ((aphase >> acc) & 1) ^ 1);
-            aphase ^= 1u << acc;
-            tc_fence_after();
-            HALO_LAP(c_acc)
-            const uint32_t d_tmem = tmem_base + acc * 256;
-            for (int cb = 0; cb < p.c_blocks; cb++) {
-                mbar_wait(&patch_full[ps], (pphase >> ps) & 1);
-                HALO_LAP(c_patch)
-                const uint64_t adesc0 = make_kmajor_sw128_desc(smem_u32(patch0 + (size_t)ps * p.patch_bytes));
-                for (int tap0 = 0; tap0 < p.taps; tap0 += p.tps) {
-                    mbar_wait(&b_full[bs], (bphase >> bs) & 1);
-                    tc_fence_after();
-                    HALO_LAP(c_b)
-                    if (elect_one()) {
-                        if (tr0 && tr_m < 2048) p.trace[2048 + tr_m++] = tq;
-                        const uint64_t bdesc0 = make_kmajor_sw128_desc(smem_u32(bring + (size_t)bs * p.b_bytes));
-                        for (int ti = 0; ti < p.tps; ti++) {
-                            // the tap is the SAME patch seen (ky P + kx) pixel slots of 128 bytes further on (descriptor
-                            // addresses count 16-byte units; offsets tabulated on the host -- an integer division per tap
-                            // costs the single issuing thread ~200 clk)
-                            const uint64_t adesc = adesc0 + (uint64_t)p.tap_off[tap0 + ti];
-                            const uint64_t bdesc = bdesc0 + (uint64_t)(ti * p.bn * 8);
-                            const uint32_t first = (cb | tap0 | ti) ? 1u : 0u;
-                            for (int t = 0; t < p.T; t++) {
-#pragma unroll
-                                for (int k = 0; k < 4; k++)
-                                    umma_tf32(d_tmem + t * p.bn, adesc + (uint64_t)(t * 1024 + 2 * k), bdesc + 2 * k, p.idesc, (first | (uint32_t)k) ? 1u : 0u);
-                            }
-                        }
-                    }
-                    __syncwarp();
-                    HALO_LAP(c_issue)
-                    n_mma += p.tps * p.T * 4;
-                    if (elect_one()) {
-                        umma_commit(&b_empty[bs]);
-                        if (tap0 + p.tps >= p.taps) {
-                            umma_commit(&patch_empty[ps]);
-                            if (cb == p.c_blocks - 1) umma_commit(&tmem_full[acc]);
-                        }
-                    }
-                    __syncwarp();
-                    bphase ^= 1u << bs;
-                    if (++bs == p.b_stages) bs = 0;
-                    HALO_LAP(c_commit)
-                }
-                pphase ^= 1u << ps;
-                ps ^= 1;
-            }
-        }
-#undef HALO_LAP
-        if (tr0 && lane == 0) {
-            p.trace[6144 + 1030] = c_issue;
-            p.trace[6144 + 1031] = n_mma;
-            p.trace[6144 + 1032] = c_acc;
-            p.trace[6144 + 1033] = c_patch;
-            p.trace[6144 + 1034] = c_b;
-            p.trace[6144 + 1035] = c_commit;
-        }
+    } else if (warp < 4) {
+        if (p.bn == 32)
+            halo_mma<32>(p, patch_full, patch_empty, b_full, b_empty, acc_full, acc_empty, patch0, bring, acc_smem);
+        else
+            halo_mma<64>(p, patch_full, patch_empty, b_full, b_empty, acc_full, acc_empty, patch0, bring, acc_smem);
     } else if (warp >= 4) {
-        // ===================== epilogue: TMEM -> registers -> (+ bias, Relu) -> shared memory -> coalesced global stores ====
-        // A thread owns one slot (TMEM lane) of the 32-column chunk; writing its 128 bytes to global memory directly costs
-        // 32 scattered 16-byte sectors per instruction (8-10 B/clk/SM measured, tools/store_probe.cu).  The chunk is staged
+        // ===================== epilogue: accumulator tile -> registers -> (+ bias, Relu) -> shared memory -> coalesced global stores ====
+        // A thread owns one slot (accumulator row) of the 32-column chunk; writing its 128 bytes to global memory directly
+        // costs 32 scattered 16-byte sectors per instruction.  The chunk is staged
         // in shared memory (128B-swizzled rows) instead, and every warp instruction then writes four WHOLE 128-byte slot
         // rows (~24 B/clk/SM, the SM's store port).  Slots that are padding (x >= OW, rows past the strip / image, tail
         // images) are skipped on the way out.
@@ -256,10 +227,9 @@ umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
                 const int c = (r >> 5) * 64 + grp * 32 + (r & 31);
                 if (c < p.bn && n0 + c < p.N) bv = __ldg(e.bias + n0 + c);
             }
-            mbar_wait(&tmem_full[acc], (aphase >> acc) & 1);
+            mbar_wait(&acc_full[acc], (aphase >> acc) & 1);
             if (tr0 && warp == 4 && lane == 0 && it < 1024) p.trace[4096 + it] = clock64();
             aphase ^= 1u << acc;
-            tc_fence_after();
             bias_g[r] = bv;  // (readers of the previous unit's values are past that unit's last barrier)
             for (int t = 0; t < p.T; t++) {
                 // the eight slots this thread writes out per chunk: slot = t * 128 + q * 32 + i * 4 + lane / 8
@@ -276,12 +246,11 @@ umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
                     if ((int)img < p.tb && b < p.B && (int)yy < p.R && oy < p.OH && (int)ox < p.OW) valid |= 1u << i;
                     off[i] = (long long)b * e.s_z0 + (long long)oy * e.s_row + (long long)ox * e.s_z1 + n0 + piece * 4;
                 }
-                const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + acc * 256 + t * p.bn;
+                const uint32_t t_row = ((uint32_t)(q * 32) << 16) + acc * 64 + t * p.bn;
                 int k = 0;
                 for (int c0 = grp * 32; c0 < p.bn; c0 += 64, k++) {
                     uint32_t v[32];
-                    tmem_ld_32x32(t_row + c0, v);
-                    tmem_ld_wait();
+                    acc_ld(acc_smem, t_row + c0, v);
                     // every warp of the group has read the previous chunk out of the staging buffer (and, for the first
                     // chunk of a unit, the bias values are in place)
                     asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory");
@@ -310,17 +279,10 @@ umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
                     }
                 }
             }
-            tc_fence_before();
             __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[acc]);
+            if (lane == 0) mbar_arrive(&acc_empty[acc]);
             if (tr0 && warp == 4 && lane == 0 && it < 1024) p.trace[6144 + it] = clock64();
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
     }
     if (tr0 && threadIdx.x == 0) p.trace[6144 + 1104] = clock64();
 }
@@ -329,8 +291,7 @@ umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
 
 // force_bn / force_T > 0: that unit shape or RTEN_ERR_UNSUPPORTED_VALUE (the autotuner times a few of them against the
 // generic kernel's plans and records the winner); 0: the cost model's choice, and only with RTEN_B200_HALO=1 -- without
-// measurements the generic kernel stays the default (profiles/r02_halo_sweep.txt: the two are within a few percent of each
-// other on ResNet-50's layers, which one wins depends on the layer).
+// measurements the generic kernel stays the default (which of the two is faster depends on the layer).
 rten_status launch_umma_halo_conv(rten_ctx* ctx, const GemmLaunch& L, int force_bn, int force_T) {
     if (getenv("RTEN_B200_NO_HALO")) return RTEN_ERR_UNSUPPORTED_VALUE;
     if (!force_bn) {
@@ -373,11 +334,10 @@ rten_status launch_umma_halo_conv(rten_ctx* ctx, const GemmLaunch& L, int force_
     const char* fbn = getenv("RTEN_B200_HALO_BN");
     const char* fT = getenv("RTEN_B200_HALO_T");
     const int want_bn = force_bn ? force_bn : (fbn ? atoi(fbn) : 0), want_T = force_T ? force_T : (fT ? atoi(fT) : 0);
-    for (int bn = 32; bn <= std::min(L.N, 256); bn += 32) {
+    for (int bn = 32; bn <= std::min(L.N, 64); bn += 32) {  // accumulator stages of 64 columns
         if (L.N % bn) continue;
         if (want_bn && bn != want_bn) continue;
-        for (int T = 1; T <= 4; T++) {
-            if (T * bn > 512) break;
+        for (int T = 1; T <= 1; T++) {  // one 128-slot tile per unit: its accumulators live in the MMA warpgroup's registers
             if (want_T && T != want_T) continue;
             // whole-image mode when tb >= 1 padded images fit T tiles, else strips of R rows
             const int img_slots = (g.OH + g.kh - 1) * p.P;
@@ -396,30 +356,28 @@ rten_status launch_umma_halo_conv(rten_ctx* ctx, const GemmLaunch& L, int force_
             const long long loaded_slots = (long long)tb * nr * p.P;
             const long long patch_bytes = (std::max(alloc_slots, loaded_slots) * 128 + 1023) / 1024 * 1024;
             // taps per weight stage: the whole window, one window row, or one tap -- the most that leaves >= 2 stages
-            const long long budget = 227 * 1024 - 3072 - 2 * 16384 - 2 * patch_bytes;  // alignment, barriers, bias, output staging
+            const long long budget = 227 * 1024 - 3072 - ACC_SMEM_BYTES - 2 * 16384 - 2 * patch_bytes;  // alignment, barriers, bias, accumulators, output staging
             // a stage must be requested ~1500 clk (TMA latency + its own transfer) before its MMAs start: four stages in
             // flight keep the tensor pipe fed, two leave it waiting for every other stage
             // (and every hand-off costs the issuing warp ~300 clk: the most taps per stage that still leaves three stages)
             int tps = 0;
-            for (int cand : {g.kh * g.kw, g.kw, 1}) {
+            for (int cand : {1}) {
                 if ((long long)cand * bn * 128 * 3 <= budget) {
                     tps = cand;
                     break;
                 }
             }
             if (!tps || tps > 256) continue;
-            const long long b_bytes = (long long)tps * bn * 128;
             const long long strips = (g.OH + R - 1) / R;
             const long long units = strips * ((g.B + tb - 1) / tb) * (L.N / bn);
             const double waves = std::ceil((double)units / num_sms);
-            // per unit: MMA clocks (T tiles x taps x c_blocks x 4 instructions of bn / 2 clocks, issue >= 40 clk each) vs the
-            // operand bytes entering the SM at ~55 B/clk; epilogue not overlapped when there is a single accumulator stage
-            // (~42 clk to issue an MMA, ~320 clk per barrier hand-off of a weight stage: profiles/r01_trace_pipeline_v2.txt)
+            // per unit: MMA clocks (T tiles x taps x c_blocks x 4 instructions of bn / 2 clocks) vs the operand bytes entering
+            // the SM.  The clock and bandwidth constants are unmeasured estimates that only rank the candidate shapes.
             const double mma = (double)p.c_blocks * ((double)T * p.taps * 4.0 * std::max(42.0, bn / 2.0) + 320.0 * (p.taps / tps));
             const double bytes = (double)p.c_blocks * (loaded_slots * 128.0 + (double)p.taps * bn * 128.0);
             const double ingest = bytes / 55.0;
             const double epi = (double)T * (bn / 32.0) * 350.0 / 2.0;
-            const int acc_stages = (2 * T * bn <= 512) ? 2 : 1;
+            const int acc_stages = 2;
             const double unit = std::max(mma, ingest) + (acc_stages == 2 ? 0.25 * epi : epi) + 800.0;
             const double cost = waves * unit + 4000.0;
             if (cost < best) {
@@ -438,7 +396,7 @@ rten_status launch_umma_halo_conv(rten_ctx* ctx, const GemmLaunch& L, int force_
     p.R = bR;
     p.tb = btb;
     p.nr = p.R + g.kh - 1;
-    p.acc_stages = (2 * p.T * p.bn <= 512) ? 2 : 1;
+    p.acc_stages = 2;
     p.strips = (g.OH + p.R - 1) / p.R;
     p.units_n = L.N / p.bn;
     p.units_total = p.strips * ((g.B + p.tb - 1) / p.tb) * p.units_n;
@@ -448,10 +406,9 @@ rten_status launch_umma_halo_conv(rten_ctx* ctx, const GemmLaunch& L, int force_
     p.patch_tx = (uint32_t)(loaded_slots * 128);
     p.tps = btps;
     p.b_bytes = (uint32_t)(p.tps * p.bn) * 128u;
-    p.b_stages = (int)std::min<long long>(HB_MAX, (227 * 1024 - 3072 - 2 * 16384 - 2LL * p.patch_bytes) / p.b_bytes);
-    p.idesc = make_idesc(1 /*F32*/, 2 /*TF32*/, 2, 128, p.bn);
+    p.b_stages = (int)std::min<long long>(HB_MAX, (227 * 1024 - 3072 - ACC_SMEM_BYTES - 2 * 16384 - 2LL * p.patch_bytes) / p.b_bytes);
     for (int ky = 0; ky < g.kh; ky++)
-        for (int kx = 0; kx < g.kw; kx++) p.tap_off[ky * g.kw + kx] = (uint32_t)((ky * p.P + kx) * 8);
+        for (int kx = 0; kx < g.kw; kx++) p.tap_off[ky * g.kw + kx] = (uint32_t)((ky * p.P + kx) * 128);
     p.m_img = (uint32_t)(0x100000000ull / (unsigned long long)(p.nr * p.P)) + 1u;
     p.m_P = (uint32_t)(0x100000000ull / (unsigned long long)p.P) + 1u;
 
@@ -463,7 +420,7 @@ rten_status launch_umma_halo_conv(rten_ctx* ctx, const GemmLaunch& L, int force_
     if (getenv("RTEN_B200_VERBOSE"))
         fprintf(stderr, "[umma_halo] B=%d %dx%d C=%d N=%d k=%dx%d: bn=%d T=%d R=%d tb=%d P=%d units=%d acc_stages=%d b_stages=%d tps=%d patch=%u B\n", g.B,
                 g.OH, g.OW, g.C, L.N, g.kh, g.kw, p.bn, p.T, p.R, p.tb, p.P, p.units_total, p.acc_stages, p.b_stages, p.tps, p.patch_bytes);
-    const size_t smem = 1024 /*align*/ + 2048 /*barriers, bias*/ + 2 * 16384 /*output staging*/ + 2 * (size_t)p.patch_bytes + (size_t)p.b_stages * p.b_bytes;
+    const size_t smem = 1024 /*align*/ + 2048 /*barriers, bias*/ + ACC_SMEM_BYTES + 2 * 16384 /*output staging*/ + 2 * (size_t)p.patch_bytes + (size_t)p.b_stages * p.b_bytes;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(std::min(p.units_total, num_sms));

@@ -1,5 +1,5 @@
-// Device side of the tcgen05 GEMM / implicit-GEMM convolution: tile decode, the warp-specialised persistent kernel
-// (TMA producer / MMA issuer / TMEM allocator / two epilogue groups) and the opt-in sequence kernel.  Included ONLY by
+// Device side of the wgmma GEMM / implicit-GEMM convolution: tile decode, the warp-specialised persistent kernel
+// (MMA warpgroup / two epilogue groups / TMA producer) and the opt-in sequence kernel.  Included ONLY by
 // umma_gemm.cu, which holds the host side (launch plans, cost model, autotuner, tensor maps).  See umma_gemm.cu's header
 // comment for the design.
 #pragma once
@@ -14,12 +14,12 @@
 
 namespace rtb {
 
-constexpr int BM = 128;            // UMMA M (cta_group::1)
+constexpr int BM = 128;            // rows per tile: two 64-row wgmma instructions
 constexpr int KBYTES = 128;        // bytes of K per stage row = one 128B swizzle atom
 constexpr int A_STAGE_BYTES = BM * KBYTES;
-constexpr int TMEM_COLS = 512;
-constexpr int ACC_STRIDE = 256;    // TMEM columns per accumulator stage
-constexpr int NUM_THREADS = 384;   // 4 control warps + 8 epilogue warps (two groups of 4)
+constexpr int ACC_STRIDE = 64;     // accumulator columns per stage (two stages, ptx.cuh ACC_COLS); also the widest tile
+constexpr int PRODUCER_WARP = 12;
+constexpr int NUM_THREADS = 416;   // MMA warpgroup (warps 0-3) + 8 epilogue warps (two groups of 4) + TMA producer warp
 constexpr int STG_BYTES = 128 * 128;  // one 128-row x 128-byte output staging buffer per epilogue group
 constexpr int MAX_STAGES = 8;
 
@@ -61,29 +61,25 @@ struct KParams {
     int sy, sx, dy, dx, pt, pl, kw, c_blocks;
     int a_bcast0, a_bcast1, b_bcast0, b_bcast1;
     long long* trace;  // debug: per-event clock64 timestamps of CTA 0 (4 rows x 2048), or null
-    int pair;       // 1: each CTA iteration computes TWO 128-row tiles sharing one B tile (interleaved MMAs on two
-                    //    accumulators hide the dependent-accumulate latency when bn <= 128)
+    int pair;       // always 0 on sm_90 (plan_shape): two 128-row tiles sharing one B tile
     int katoms;     // consecutive 128-byte K blocks loaded / multiplied per pipeline stage (1 or 2): amortises the fixed
                     // per-stage barrier round trip of the issuing threads when tiles are small
     uint32_t atom_bytes;
-    int ksplit;     // 1: (single-tile mode, bn <= 128) even / odd K blocks accumulate into two TMEM accumulators that the
-                    //    epilogue adds: consecutive MMAs never depend on each other (no dependent-accumulate stall)
+    int ksplit;     // always 0 on sm_90 (plan_shape): even / odd K blocks in two accumulators added by the epilogue
     int nbuf;       // staging buffers per epilogue group (ring): nbuf-1 (nbuf-2 with res_tma) bulk stores stay in flight
     int res_tma;    // 1: the residual tile is prefetched by TMA into the staging buffer (needs tma_store)
     uint32_t res_tx_bytes;
     int tma_store;  // 1: epilogue stages 128x32 chunks in smem and writes them with TMA (output rows contiguous)
-    int acc1;       // 1: ONE accumulator stage of 512 TMEM columns (pair mode with bn = 256: a 256 x 256 tile per CTA halves
-                    //    the L2 -> SM operand traffic per flop; the epilogue no longer overlaps the next main loop)
+    int acc1;       // always 0 on sm_90 (plan_shape): one accumulator stage
     int splitk;     // > 1: `splitk` CTAs share one output tile, each over `kb_per` K blocks; raw partial accumulators go
                     // to `sk_ws`, the LAST CTA to arrive (per tile and epilogue group, `sk_cnt`) sums them in split order
                     // (deterministic) and runs the epilogue
     int kb_per;
-    int cta2;       // 1: CTA pairs (cluster 2x1x1) execute 256-row tcgen05.mma.cta_group::2 tiles; each CTA loads its own
-                    //    128 rows of A and HALF of the B tile, so operand bytes entering an SM per flop drop by up to 2x
+    int cta2;       // always 0 on sm_90 (plan_shape): no two-CTA MMA
     int units_total;  // tiles_total * splitk
     int x3_cb;      // > 0: 3xTF32 over TWO planes of A -- the K (channel) range is three segments of x3_cb K blocks,
                     //      [lo | hi | hi]: segment 0 reads the low-part plane (tma_a2), segments 1 and 2 read the ORIGINAL f32
-                    //      tensor (kind::tf32 ignores the 13 low mantissa bits, so the raw values ARE the high parts)
+                    //      tensor (tf32 wgmma ignores the 13 low mantissa bits, so the raw values ARE the high parts)
     FastDiv d_tiles_n, d_units_m, d_z0, d_tiles_x, d_tiles_y, d_tiles_total, d_c_blocks, d_kw, d_tw, d_th;
     uint32_t* sk_ws;
     int* sk_cnt;
@@ -121,22 +117,16 @@ __device__ __forceinline__ TileCoord decode_tile(const KParams& p, int t, int su
     return c;
 }
 
-// (a0, a1) += (b0, b1): one packed FADD2, each half rounded to nearest like a scalar add
+// (a0, a1) += (b0, b1) on f32 bit patterns, each half rounded to nearest like a scalar add
 __device__ __forceinline__ void add_f32x2(uint32_t& a0, uint32_t& a1, float b0, float b1) {
-    unsigned long long a, b, d;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(a) : "r"(a0), "r"(a1));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(b) : "f"(b0), "f"(b1));
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    asm("mov.b64 {%0, %1}, %2;" : "=r"(a0), "=r"(a1) : "l"(d));
+    a0 = __float_as_uint(__fadd_rn(__uint_as_float(a0), b0));
+    a1 = __float_as_uint(__fadd_rn(__uint_as_float(a1), b1));
 }
 
-// (a0, a1) *= (b0, b1): one packed FMUL2, each half rounded to nearest like a scalar multiply
+// (a0, a1) *= (b0, b1) on f32 bit patterns, each half rounded to nearest like a scalar multiply
 __device__ __forceinline__ void mul_f32x2(uint32_t& a0, uint32_t& a1, float b0, float b1) {
-    unsigned long long a, b, d;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(a) : "r"(a0), "r"(a1));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(b) : "f"(b0), "f"(b1));
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    asm("mov.b64 {%0, %1}, %2;" : "=r"(a0), "=r"(a1) : "l"(d));
+    a0 = __float_as_uint(__fmul_rn(__uint_as_float(a0), b0));
+    a1 = __float_as_uint(__fmul_rn(__uint_as_float(a1), b1));
 }
 
 // cp.async.bulk.wait_group.read takes an immediate: leave at most `n` of this thread's bulk stores un-read
@@ -186,14 +176,13 @@ __device__ __noinline__ float4 act4(float4 x, int act) {
 // Returns true for the group of the CTA that arrived last: it owns the epilogue of (tile, group).
 // Workspace layout: [tile][sub][split][chunk][column j][row r] so that a warp's 32 rows are contiguous.
 __device__ __forceinline__ bool splitk_publish(const KParams& p, int t, int ks, int grp, int q, int lane, uint32_t t_acc,
-                                               int* flag) {  // t = tile slot (tile, or 2 * tile + cluster rank)
+                                               int* flag, uint32_t acc_smem) {  // t = tile slot (tile, or 2 * tile + cluster rank)
     const int r = q * 32 + lane;
     const int nchunks = p.bn >> 5;
     for (int sub = 0; sub <= p.pair; sub++) {
         for (int c0 = grp * 32; c0 < p.bn; c0 += 64) {
             uint32_t v[32];
-            tmem_ld_32x32(t_acc + sub * p.bn + c0, v);
-            tmem_ld_wait();
+            acc_ld(acc_smem, t_acc + sub * p.bn + c0, v);
             uint32_t* w = p.sk_ws + ((((size_t)(t * 2 + sub) * p.splitk + ks) * nchunks + (c0 >> 5)) << 12) + r;
 #pragma unroll
             for (int j = 0; j < 32; j++) __stcg(w + j * 128, v[j]);
@@ -245,9 +234,10 @@ struct PipeState {
 
 struct SmemLayout {
     uint8_t* smem;  // operand stages (1024-B aligned), staging buffers behind them
-    uint64_t *full_bar, *empty_bar, *tmem_full, *tmem_empty, *res_bar;
+    uint64_t *full_bar, *empty_bar, *acc_full, *acc_empty, *res_bar;
     int* sk_flag;
     float* bias;
+    uint32_t acc_smem;  // accumulator tiles (ptx.cuh), between the column vectors and the operand stages
 };
 
 }  // namespace rtb
@@ -257,21 +247,86 @@ struct SmemLayout {
 
 namespace rtb {
 
+// One 128 x N tile per work unit, accumulated by the warpgroup of warps 0-3 over the unit's K blocks: two 64-row
+// wgmma instructions per 32 bytes of K, one wgmma group per pipeline stage.  A stage goes back to the producer once the
+// group after it has been issued and it has retired (one arrival per warp); the finished tile is stored to accumulator
+// stage (tile count & 1) once the epilogue has released it (8 warp arrivals), then announced (128 arrivals).
+template <int KIND, int SGN, int N>
+__device__ __forceinline__ void mma_units(const KParams& p, const SmemLayout& L, int worker, int n_workers, PipeState& st) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t smem0 = smem_u32(L.smem);
+    int stage = 0;
+    for (int u = worker; u < p.units_total; u += n_workers, st.it++) {
+        const int kb0 = p.d_tiles_total.div(u) * p.kb_per, kb1 = min(p.k_blocks, kb0 + p.kb_per);
+        const int acc = st.it & 1;
+        acc_t<KIND> d0[N / 2], d1[N / 2];
+#pragma unroll
+        for (int i = 0; i < N / 2; i++) d0[i] = d1[i] = 0;
+        int prev = -1;
+        for (int kb = kb0; kb < kb1; kb++) {
+            mbar_wait(&L.full_bar[stage], (st.ring >> stage) & 1);
+            wgmma_fence_operand(d0);
+            wgmma_fence_operand(d1);
+            wgmma_fence();
+            const uint32_t sa = smem0 + stage * p.stage_bytes;
+            const uint64_t adesc = make_kmajor_sw128_desc(sa);
+            const uint64_t bdesc = make_kmajor_sw128_desc(sa + A_STAGE_BYTES);
+#pragma unroll
+            for (int k = 0; k < 4; k++) {  // +2 in the (addr >> 4) field = 32 B along K in the swizzle atom
+                wgmma_k<KIND, SGN, N>(d0, adesc + 2 * k, bdesc + 2 * k);
+                wgmma_k<KIND, SGN, N>(d1, adesc + (64 * KBYTES >> 4) + 2 * k, bdesc + 2 * k);  // rows 64-127
+            }
+            wgmma_commit();
+            wgmma_fence_operand(d0);
+            wgmma_fence_operand(d1);
+            // one group stays in flight across the loop back-edge; the stage before this one has retired and goes back
+            wgmma_wait<1>();
+            if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
+            prev = stage;
+            st.ring ^= 1u << stage;
+            if (++stage == p.stages) stage = 0;
+        }
+        wgmma_wait<0>();
+        wgmma_fence_operand(d0);
+        wgmma_fence_operand(d1);
+        if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
+        mbar_wait(&L.acc_empty[acc], ((st.acc >> acc) & 1) ^ 1);
+        st.acc ^= 1u << acc;
+        acc_store_frag<N>(L.acc_smem, d0, 0, acc * ACC_STRIDE);
+        acc_store_frag<N>(L.acc_smem, d1, 64, acc * ACC_STRIDE);
+        mbar_arrive(&L.acc_full[acc]);
+    }
+}
+
+template <int KIND, int N>
+__device__ __forceinline__ void mma_role(const KParams& p, const SmemLayout& L, int worker, int n_workers, PipeState& st) {
+    if (KIND == 0) {
+        mma_units<KIND, 0, N>(p, L, worker, n_workers, st);
+    } else {
+        // signedness of A / B from the operand-format fields of p.idesc (ptx.cuh make_idesc)
+        const int sgn = ((p.idesc >> 7) & 1) | (((p.idesc >> 10) & 1) << 1);
+        if (sgn == 0) mma_units<KIND, 0, N>(p, L, worker, n_workers, st);
+        else if (sgn == 1) mma_units<KIND, 1, N>(p, L, worker, n_workers, st);
+        else if (sgn == 2) mma_units<KIND, 2, N>(p, L, worker, n_workers, st);
+        else mma_units<KIND, 3, N>(p, L, worker, n_workers, st);
+    }
+}
+
 // One launch worth of work (all roles).  FAST = the launch satisfies, for EVERY chunk, the conditions of the register
 // fast path (TMA-store output, N % 32 == 0, f32 with act in {none, relu} and bias / residual absent or
 // vector-addressable [residual via TMA], or raw i32): the epilogue is then a short straight-line loop.  The generic
 // variant (FAST = 0) keeps every edge case.
-template <int KIND, int FAST, int CTA2>
+template <int KIND, int FAST>
 __device__ __forceinline__ void run_layer(const KParams& p, const CUtensorMap* tma_a, const CUtensorMap* tma_a2,
                                           const CUtensorMap* tma_b, const CUtensorMap* tma_d, const CUtensorMap* tma_r, const SmemLayout& L,
-                                          uint32_t tmem_base, int cta_rank, int worker, int n_workers, PipeState& st) {
+                                          int worker, int n_workers, PipeState& st) {
     uint8_t* smem = L.smem;
     uint8_t* stg_base = smem + (size_t)p.stages * p.stage_bytes;
     const int nbuf = p.nbuf;
     uint64_t* full_bar = L.full_bar;
     uint64_t* empty_bar = L.empty_bar;
-    uint64_t* tmem_full = L.tmem_full;
-    uint64_t* tmem_empty = L.tmem_empty;
+    uint64_t* acc_full = L.acc_full;
+    uint64_t* acc_empty = L.acc_empty;
     uint64_t* res_bar = L.res_bar;
     int* sk_flag = L.sk_flag;
     const int warp = threadIdx.x >> 5;
@@ -279,20 +334,19 @@ __device__ __forceinline__ void run_layer(const KParams& p, const CUtensorMap* t
     // Control warps run their loops WARP-UNIFORMLY (all 32 lanes wait on the barriers, one elected lane issues the
     // TMA / MMA instructions): addresses and descriptors then live in uniform registers instead of being moved
     // there (R2UR) for every instruction, which is what bounds a single issuing thread.
-    if (warp == 0) {
+    if (warp == PRODUCER_WARP) {
         // ===================== TMA producer =====================
         int stage = 0;
         int tr_p = 0;
         const uint32_t smem0 = smem_u32(smem);
         const uint32_t full0 = smem_u32(full_bar);
         const uint32_t a_bytes = (p.pair ? 2 : 1) * A_STAGE_BYTES;
-        const int b_row0 = CTA2 ? cta_rank * (p.bn >> 1) : 0;  // this CTA's half of the B tile
         for (int u = worker; u < p.units_total; u += n_workers) {
             int t, ks;
             p.d_tiles_total.divmod(u, ks, t);
             const int kb0 = ks * p.kb_per, kb1 = min(p.k_blocks, kb0 + p.kb_per);
-            const TileCoord tc = decode_tile(p, t, 0, cta_rank);
-            const TileCoord tc1 = p.pair ? decode_tile(p, t, 1, cta_rank) : tc;
+            const TileCoord tc = decode_tile(p, t, 0);
+            const TileCoord tc1 = p.pair ? decode_tile(p, t, 1) : tc;
             // conv: K block -> (filter tap, channel block), kept incrementally
             int tap, cb, ky, kx;
             p.d_c_blocks.divmod(kb0, tap, cb);
@@ -311,24 +365,17 @@ __device__ __forceinline__ void run_layer(const KParams& p, const CUtensorMap* t
                 const int natoms = min(p.katoms, kb1 - kb);
                 mbar_wait(&empty_bar[stage], ((st.ring >> stage) & 1) ^ 1);
                 const bool leader = elect_one();
-                // CTA pair: both CTAs' loads complete on the LEADER's barrier, which expects the bytes of both
-                const uint32_t fb = CTA2 ? ((full0 + stage * 8) & PEER_BIT_MASK) : (full0 + stage * 8);
+                const uint32_t fb = full0 + stage * 8;
                 if (leader) {
                     if (p.trace && blockIdx.x == 0 && tr_p < 2048) p.trace[tr_p++] = clock64();
-                    if (!CTA2)
-                        mbar_expect_tx_u32(fb, p.tx_bytes * natoms);
-                    else if (cta_rank == 0)
-                        mbar_expect_tx_u32(fb, 2 * p.tx_bytes * natoms);
+                    mbar_expect_tx_u32(fb, p.tx_bytes * natoms);
                 }
                 for (int a = 0; a < natoms; a++) {
                     if (leader) {
                         const uint32_t sa = smem0 + stage * p.stage_bytes + a * p.atom_bytes;
                         const uint32_t sb = sa + a_bytes;
                         auto load = [&](uint32_t dst, const CUtensorMap* m, int c0, int c1, int c2, int c3) {
-                            if (CTA2)
-                                tma_load_4d_2sm(dst, m, fb, c0, c1, c2, c3);
-                            else
-                                tma_load_4d_u32(dst, m, fb, c0, c1, c2, c3);
+                            tma_load_4d_u32(dst, m, fb, c0, c1, c2, c3);
                         };
                         const CUtensorMap* ma = (p.x3_cb && seg == 0) ? tma_a2 : tma_a;
                         if (p.conv) {
@@ -338,14 +385,14 @@ __device__ __forceinline__ void run_layer(const KParams& p, const CUtensorMap* t
                             if (p.pair)
                                 load(sa + A_STAGE_BYTES, ma, ca, tc1.ox0 * p.sx - p.pl + kx * p.dx,
                                      tc1.oy0 * p.sy - p.pt + ky * p.dy, tc1.b0);
-                            load(sb, tma_b, c0, tc.n0 + b_row0, tap, 0);
+                            load(sb, tma_b, c0, tc.n0, tap, 0);
                         } else {
                             const int k0 = (kb + a) * p.kelems;
                             const int ka = p.x3_cb ? sblk * p.kelems : k0;
                             const int az0 = p.a_bcast0 ? 0 : tc.z0, az1 = p.a_bcast1 ? 0 : tc.z1;
                             load(sa, ma, ka, tc.m0, az0, az1);
                             if (p.pair) load(sa + A_STAGE_BYTES, ma, ka, tc1.m0, az0, az1);
-                            load(sb, tma_b, k0, tc.n0 + b_row0, p.b_bcast0 ? 0 : tc.z0, p.b_bcast1 ? 0 : tc.z1);
+                            load(sb, tma_b, k0, tc.n0, p.b_bcast0 ? 0 : tc.z0, p.b_bcast1 ? 0 : tc.z1);
                         }
                     }
                     if (p.x3_cb && ++sblk == p.x3_cb) {
@@ -366,179 +413,87 @@ __device__ __forceinline__ void run_layer(const KParams& p, const CUtensorMap* t
                 if (++stage == p.stages) stage = 0;
             }
         }
-    } else if (warp == 1 && cta_rank == 0) {
-        // ===================== MMA issuer (pair mode: the leader CTA only) =====================
-        int stage = 0;
-        int tr_m = 0;
-        const uint32_t smem0 = smem_u32(smem);
-        const uint32_t empty0 = smem_u32(empty_bar);
-        const uint32_t b_off = (p.pair ? 2 : 1) * A_STAGE_BYTES;
-        const uint32_t d1_off = (p.pair || p.ksplit) ? p.bn : 0;
-        for (int u = worker; u < p.units_total; u += n_workers, st.it++) {
-            const int kb0 = p.d_tiles_total.div(u) * p.kb_per, kb1 = min(p.k_blocks, kb0 + p.kb_per);
-            const int acc = p.acc1 ? 0 : (st.it & 1);
-            mbar_wait(&tmem_empty[acc], ((st.acc >> acc) & 1) ^ 1);
-            st.acc ^= 1u << acc;
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + acc * ACC_STRIDE;
-            for (int kb = kb0; kb < kb1; kb += p.katoms) {
-                const int natoms = min(p.katoms, kb1 - kb);
-                mbar_wait(&full_bar[stage], (st.ring >> stage) & 1);
-                tc_fence_after();
-                if (elect_one()) {
-                    if (p.trace && blockIdx.x == 0 && tr_m < 2048) p.trace[2048 + tr_m++] = clock64();
-                    for (int a = 0; a < natoms; a++) {
-                        const uint32_t sa = smem0 + stage * p.stage_bytes + a * p.atom_bytes;
-                        const uint64_t adesc = make_kmajor_sw128_desc(sa);
-                        const uint64_t bdesc = make_kmajor_sw128_desc(sa + b_off);
-                        const uint32_t first = (kb + a) == kb0 ? 0u : 1u;
-                        auto mma = [&](uint32_t d, uint64_t ad, uint64_t bd, uint32_t accum) {
-                            if (CTA2)
-                                umma2<KIND>(d, ad, bd, p.idesc, accum);
-                            else
-                                umma<KIND>(d, ad, bd, p.idesc, accum);
-                        };
-                        if (p.pair) {
-                            const uint64_t adesc1 = make_kmajor_sw128_desc(sa + A_STAGE_BYTES);
-#pragma unroll
-                            for (int k = 0; k < 4; k++) {  // +2 in the (addr >> 4) field = 32 B along K in the swizzle atom
-                                mma(d_tmem, adesc + 2 * k, bdesc + 2 * k, k == 0 ? first : 1u);
-                                mma(d_tmem + d1_off, adesc1 + 2 * k, bdesc + 2 * k, k == 0 ? first : 1u);
-                            }
-                        } else if (p.ksplit) {
-#pragma unroll
-                            for (int k = 0; k < 4; k++)  // k even -> accumulator 0, k odd -> accumulator 1
-                                mma(d_tmem + (k & 1) * d1_off, adesc + 2 * k, bdesc + 2 * k, k < 2 ? first : 1u);
-                        } else {
-#pragma unroll
-                            for (int k = 0; k < 4; k++)
-                                mma(d_tmem, adesc + 2 * k, bdesc + 2 * k, k == 0 ? first : 1u);
-                        }
-                    }
-                    // smem slot reusable once these MMAs retire; accumulator complete -> epilogue (of both CTAs)
-                    if (CTA2) {
-                        umma_commit_mc(empty0 + stage * 8, 3);
-                        if (kb + natoms >= kb1) umma_commit_mc(smem_u32(&tmem_full[acc]), 3);
-                    } else {
-                        umma_commit_u32(empty0 + stage * 8);
-                        if (kb + natoms >= kb1) umma_commit(&tmem_full[acc]);
-                    }
-                }
-                __syncwarp();
-                st.ring ^= 1u << stage;
-                if (++stage == p.stages) stage = 0;
-            }
-        }
+    } else if (warp < 4) {
+        // ===================== MMA warpgroup: accumulators in registers, finished tiles to shared memory
+        if (p.bn == 32)
+            mma_role<KIND, 32>(p, L, worker, n_workers, st);
+        else
+            mma_role<KIND, 64>(p, L, worker, n_workers, st);
     } else if (warp >= 4) {
         // ===================== epilogue warps: one of four variants (umma_epilogue_plain.cuh / umma_epilogue_generic.cuh)
-        const EpiCtx c{p, L, stg_base, nbuf, tmem_full, tmem_empty, res_bar, sk_flag, tma_d, tma_r, tmem_base, cta_rank, worker, n_workers, st, warp, lane};
+        const EpiCtx c{p, L, stg_base, nbuf, acc_full, acc_empty, res_bar, sk_flag, tma_d, tma_r, L.acc_smem, 0, worker, n_workers, st, warp, lane};
         if (KIND == 0 && (FAST == 3 || FAST == 5))
-            epilogue_plain_f32<FAST, CTA2>(c);
+            epilogue_plain_f32<FAST>(c);
         else if (KIND == 1 && (FAST == 4 || FAST == 6))
-            epilogue_plain_i8<FAST, CTA2>(c);
+            epilogue_plain_i8<FAST>(c);
         else if (FAST)
-            epilogue_fast<KIND, FAST, CTA2>(c);
+            epilogue_fast<KIND, FAST>(c);
         else
-            epilogue_generic<KIND, CTA2>(c);
+            epilogue_generic<KIND>(c);
     }
 
 }
 
 // Shared-memory carve-up: a fixed 1 KB block of mbarriers first (so that it does not move when the stage geometry changes
-// from layer to layer of a sequence kernel), operand stages behind it.
-template <int KIND>
+// from layer to layer of a sequence kernel), the column vectors, the accumulator tiles, operand stages behind them.
+constexpr int SMEM_FIXED_BYTES = 1024 /*align*/ + 4096 /*barriers, column vectors*/ + ACC_SMEM_BYTES;
+static_assert(ACC_SMEM_BYTES % 1024 == 0, "operand stages must stay 1024-B aligned");
+static_assert(2 * ACC_STRIDE <= ACC_COLS, "two accumulator stages");
+
 __device__ __forceinline__ SmemLayout carve_smem(uint8_t* smem_raw) {
-    // 1024-B alignment required by the 128B swizzle atoms / UMMA descriptors (base_offset = 0).
+    // 1024-B alignment required by the 128B swizzle atoms / wgmma descriptors (base_offset = 0).
     uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     SmemLayout L;
     L.full_bar = reinterpret_cast<uint64_t*>(base);
     L.empty_bar = L.full_bar + MAX_STAGES;
-    L.tmem_full = L.empty_bar + MAX_STAGES;
-    L.tmem_empty = L.tmem_full + 2;
-    L.res_bar = L.tmem_empty + 2;  // [group][buffer], up to 4 buffers per group
-    L.sk_flag = reinterpret_cast<int*>(L.res_bar + 8) + 2;  // [group]; the two ints before it hold the TMEM base
+    L.acc_full = L.empty_bar + MAX_STAGES;
+    L.acc_empty = L.acc_full + 2;
+    L.res_bar = L.acc_empty + 2;  // [group][buffer], up to 4 buffers per group
+    L.sk_flag = reinterpret_cast<int*>(L.res_bar + 8) + 2;  // [group]
     // column vectors of the current unit for the plain epilogues: f32 [group][128] bias (1 KB); integer kind
     // [3][group][128]: za * colsum, scale product, bias (3 KB)
     L.bias = reinterpret_cast<float*>(base + 1024);
-    L.smem = base + (KIND == 0 ? 2048 : 4096);
+    L.acc_smem = smem_u32(base + 4096);
+    L.smem = base + 4096 + ACC_SMEM_BYTES;
     return L;
 }
 
-template <int CTA2>
-__device__ __forceinline__ uint32_t kernel_setup(const SmemLayout& L) {
+__device__ __forceinline__ void kernel_setup(const SmemLayout& L) {
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(L.res_bar + 8);
-    if (warp == 0 && !CTA2) {
-        // the producer initialises its own ring barriers and does NOT wait for the rest of the set-up (TMEM allocation,
-        // the CTA-wide barrier): it only arrives on a named barrier, so its first TMA is issued that much earlier
-        if (lane < 2 * MAX_STAGES) mbar_init(&L.full_bar[lane], 1);  // full_bar and empty_bar are contiguous
+    if (warp == PRODUCER_WARP) {
+        // the producer initialises its own ring barriers and does NOT wait for the rest of the set-up: it only arrives
+        // on a named barrier, so its first TMA is issued that much earlier
+        if (lane < MAX_STAGES) {
+            mbar_init(&L.full_bar[lane], 1);
+            mbar_init(&L.empty_bar[lane], 4);  // one arrival per MMA warp
+        }
         fence_mbar_init();
         __syncwarp();
         asm volatile("bar.arrive 15, %0;" ::"r"(NUM_THREADS) : "memory");
-        return 0;  // (the producer never touches TMEM)
+        return;
     }
     if (warp == 1) {
-        // one barrier per lane (a single thread initialising them serially sat on the start-up critical path):
-        // lanes 0-15 ring full / empty (pair mode only, else the producer's), 16-17 accumulator full, 18-19 accumulator
-        // empty, 20-27 residual
-        if (lane < 2 * MAX_STAGES) {
-            if (CTA2) mbar_init(&L.full_bar[lane], 1);
-        } else if (lane < 2 * MAX_STAGES + 2) {
-            mbar_init(&L.tmem_full[lane - 2 * MAX_STAGES], 1);
-        } else if (lane < 2 * MAX_STAGES + 4) {
-            mbar_init(&L.tmem_empty[lane - 2 * MAX_STAGES - 2], CTA2 ? 16 : 8);  // one arrival per epilogue warp (of both CTAs of a pair)
-        } else if (lane < 2 * MAX_STAGES + 12) {
-            mbar_init(&L.res_bar[lane - 2 * MAX_STAGES - 4], 1);
-        }
+        // one barrier per lane: 0-1 accumulator full, 2-3 accumulator empty, 4-11 residual
+        if (lane < 2)
+            mbar_init(&L.acc_full[lane], 128);  // every thread of the MMA warpgroup stores part of the tile
+        else if (lane < 4)
+            mbar_init(&L.acc_empty[lane - 2], 8);  // one arrival per epilogue warp
+        else if (lane < 12)
+            mbar_init(&L.res_bar[lane - 4], 1);
         fence_mbar_init();
     }
-    if (warp == 2) {
-        if (CTA2) {
-            tmem_alloc2(tmem_ptr, TMEM_COLS);
-            tmem_relinquish2();
-        } else {
-            tmem_alloc(tmem_ptr, TMEM_COLS);
-            tmem_relinquish();
-        }
-    }
-    tc_fence_before();
-    if (CTA2)
-        cluster_sync_all();  // the peer's barriers must be initialised before any remote arrive / multicast commit
-    else
-        asm volatile("bar.sync 15, %0;" ::"r"(NUM_THREADS) : "memory");  // 11 warps wait, the producer warp only arrives
-    tc_fence_after();
-    return *tmem_ptr;
+    asm volatile("bar.sync 15, %0;" ::"r"(NUM_THREADS) : "memory");  // 12 warps wait, the producer warp only arrives
 }
 
-template <int CTA2>
-__device__ __forceinline__ void kernel_teardown(uint32_t tmem_base) {
-    tc_fence_before();
-    if (CTA2)
-        cluster_sync_all();  // neither CTA may exit (or free TMEM) while the pair's MMAs / remote arrives are in flight
-    else
-        __syncthreads();
-    if ((threadIdx.x >> 5) == 2) {
-        tc_fence_after();
-        if (CTA2)
-            tmem_dealloc2(tmem_base, TMEM_COLS);
-        else
-            tmem_dealloc(tmem_base, TMEM_COLS);
-    }
-}
-
-template <int KIND, int FAST, int CTA2>
+template <int KIND, int FAST>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 umma_gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                  const __grid_constant__ CUtensorMap tma_d, const __grid_constant__ CUtensorMap tma_r,
                  const __grid_constant__ CUtensorMap tma_a2, const __grid_constant__ KParams p) {
     extern __shared__ uint8_t smem_raw[];
-    const SmemLayout L = carve_smem<KIND>(smem_raw);
+    const SmemLayout L = carve_smem(smem_raw);
     if (p.trace && blockIdx.x == 0 && threadIdx.x == 0) p.trace[6144 + 1100] = clock64();  // kernel entry
-    // CTA pair: cluster rank 0 is the leader (issues the MMAs); work is distributed over clusters
-    const int cta_rank = CTA2 ? (int)cluster_ctarank() : 0;
-    const int worker = CTA2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-    const int n_workers = CTA2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tma_a);
         tma_prefetch_desc(&tma_b);
@@ -546,25 +501,23 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
         if (p.res_tma) tma_prefetch_desc(&tma_r);
         if (p.x3_cb) tma_prefetch_desc(&tma_a2);
     }
-    const uint32_t tmem_base = kernel_setup<CTA2>(L);
-    // Programmatic dependent launch: everything above (barrier init, TMEM allocation, descriptor prefetch) overlaps
-    // the tail of the previous kernel in the stream; global memory is only touched after this point.
+    kernel_setup(L);
+    // Programmatic dependent launch: everything above (barrier init, descriptor prefetch) overlaps the tail of the
+    // previous kernel in the stream; global memory is only touched after this point.
     if (p.trace && blockIdx.x == 0 && threadIdx.x == 0) p.trace[6144 + 1101] = clock64();  // set-up done
-    if (threadIdx.x >= 32) asm volatile("griddepcontrol.wait;" ::: "memory");  // (the producer warp waits after its tile decode)
+    if (threadIdx.x >> 5 != PRODUCER_WARP) asm volatile("griddepcontrol.wait;" ::: "memory");  // (the producer waits after its tile decode)
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     if (p.trace && blockIdx.x == 0 && threadIdx.x == 0) p.trace[6144 + 1102] = clock64();  // predecessor complete
     PipeState st;
-    run_layer<KIND, FAST, CTA2>(p, &tma_a, &tma_a2, &tma_b, &tma_d, &tma_r, L, tmem_base, cta_rank, worker, n_workers, st);
+    run_layer<KIND, FAST>(p, &tma_a, &tma_a2, &tma_b, &tma_d, &tma_r, L, (int)blockIdx.x, (int)gridDim.x, st);
     if (p.trace && blockIdx.x == 0 && threadIdx.x == 0) p.trace[6144 + 1103] = clock64();  // control thread done
-    kernel_teardown<CTA2>(tmem_base);
-    if (p.trace && blockIdx.x == 0 && threadIdx.x == 0) p.trace[6144 + 1104] = clock64();  // exit
 }
 
 // ------------------------------------------------------------------------------------------
 // Sequence kernel: up to SEQ_MAX consecutive launches (layers of a captured op list) run inside ONE persistent
 // kernel.  Between two layers every CTA drains its output stores and meets the others at a grid-wide barrier (an
 // arrival counter in global memory): a layer boundary costs one barrier round trip plus one TMA latency instead of a
-// kernel launch, TMEM allocation, tensor-map fetch and a cold pipeline.  Layer parameters and tensor maps live in the
+// kernel launch, tensor-map fetch and a cold pipeline.  Layer parameters and tensor maps live in the
 // kernel parameter block (constant bank), indexed by the layer number.
 // ------------------------------------------------------------------------------------------
 constexpr int SEQ_MAX = 28;
@@ -586,28 +539,28 @@ __device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
 template <int KIND, int FAST>
 __global__ void __launch_bounds__(NUM_THREADS, 1) umma_seq_kernel(const __grid_constant__ SeqParams sp) {
     extern __shared__ uint8_t smem_raw[];
-    const SmemLayout L = carve_smem<KIND>(smem_raw);
+    const int warp = threadIdx.x >> 5;
+    const SmemLayout L = carve_smem(smem_raw);
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&sp.maps[0][0]);
         tma_prefetch_desc(&sp.maps[0][1]);
     }
-    const uint32_t tmem_base = kernel_setup<0>(L);
-    if (threadIdx.x >= 32) asm volatile("griddepcontrol.wait;" ::: "memory");
+    kernel_setup(L);
+    if (warp != PRODUCER_WARP) asm volatile("griddepcontrol.wait;" ::: "memory");
     PipeState st;
-    const int warp = threadIdx.x >> 5;
     for (int l = 0; l < sp.n; l++) {
         const KParams& p = sp.layer[l];
         if (l + 1 == sp.n) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        run_layer<KIND, FAST, 0>(p, &sp.maps[l][0], &sp.maps[l][0], &sp.maps[l][1], &sp.maps[l][2], &sp.maps[l][3], L, tmem_base, 0,
-                                 (int)blockIdx.x, (int)gridDim.x, st);
+        run_layer<KIND, FAST>(p, &sp.maps[l][0], &sp.maps[l][0], &sp.maps[l][1], &sp.maps[l][2], &sp.maps[l][3], L,
+                              (int)blockIdx.x, (int)gridDim.x, st);
         if (l + 1 < sp.n) {
             // ---- layer boundary: this CTA's outputs are complete and visible, then wait for every other CTA's
-            if (warp >= 4) {
+            if (warp >= 4 && warp < PRODUCER_WARP) {
                 asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // TMA stores performed (issuer threads)
                 asm volatile("fence.proxy.async;" ::: "memory");
                 __threadfence();
             }
-            if (threadIdx.x == 32) {  // idle until the barrier anyway: fetch the next layer's tensor maps
+            if (threadIdx.x == 32 * PRODUCER_WARP) {  // idle until the barrier anyway: fetch the next layer's tensor maps
                 tma_prefetch_desc(&sp.maps[l + 1][0]);
                 tma_prefetch_desc(&sp.maps[l + 1][1]);
                 tma_prefetch_desc(&sp.maps[l + 1][2]);
@@ -633,7 +586,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) umma_seq_kernel(const __grid_c
         const unsigned old = atomicAdd(sp.gbar, 1u);
         if (old == gridDim.x * (unsigned)sp.n - 1u) *reinterpret_cast<volatile unsigned*>(sp.gbar) = 0u;
     }
-    kernel_teardown<0>(tmem_base);
 }
 
 }  // namespace rtb

@@ -473,7 +473,7 @@ class BertRunner:
             if self.fuse:
                 # one GEMM for Q | K | V (the three MatMuls share their input), then the Attention operator
                 # (src/ops/attention.rs:645-905) on strided [B,nh,S,dh] views of its output: for 128 keys / head size 64
-                # in single-pass TF32 one tcgen05 kernel (scores and probabilities never leave the SM, V transposed
+                # in single-pass TF32 one fused kernel (scores and probabilities never leave the SM, V transposed
                 # in shared memory); other shapes / the 3xTF32 mode compose MatMul -> Softmax -> MatMul
                 qkv = self._linear(x, d["wqkv"], d["bqkv"])                   # [B*S, 3H]
                 part = lambda i: qkv.view((B, nh, S, dh), (S * 3 * H, dh, 3 * H, 1), i * H)

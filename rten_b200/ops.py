@@ -45,7 +45,7 @@ class Context:
         h = C.c_void_p()
         st = self.lib.rten_b200_ctx_create(device, C.c_void_p(stream) if stream else None, workspace_bytes, C.byref(h))
         if st != 0:
-            raise OpError(st, "rten_b200_ctx_create failed: a B200 (sm_100a) with a working driver is required")
+            raise OpError(st, "rten_b200_ctx_create failed: an H100 (sm_90a) with a working driver is required")
         self.handle = h
         self.device = device
 

@@ -1,11 +1,11 @@
-"""Parity checks of the CUDA path against the CPU oracle, shared by `pytest -m gpu` (tests/test_gpu_*.py)
-and tools/gpu_probe.py.  Every check calls the product through the C ABI (rten_b200.ops -> ctypes ->
+"""Parity checks of the CUDA path against the CPU oracle, run by `pytest -m gpu` (tests/test_gpu_*.py).
+Every check calls the product through the C ABI (rten_b200.ops -> ctypes ->
 librten_b200.so) and the oracle through oracle/oracle.py.
 
 Tolerances
   integer / index work, elementwise f32 math, Softmax, LayerNormalization: bit-exact.
-  f32 GEMM / Conv (tcgen05 kind::tf32, single pass): |got - exact| <= 2^-9 * sum_k |a_k b_k| + 1e-6
-  (both operands lose at most 2^-10 relative each to TF32 rounding; fp32 accumulation in TMEM).
+  f32 GEMM / Conv (wgmma tf32, single pass): |got - exact| <= 2^-9 * sum_k |a_k b_k| + 1e-6
+  (both operands lose at most 2^-10 relative each to TF32 rounding; fp32 accumulation).
 """
 import numpy as np
 
@@ -374,19 +374,14 @@ def check_matmul_integer(rt, oracle):
 
 # ------------------------------------------------------------------------------------------
 def check_plans(rt, oracle):
-    """Every launch-plan family (pair, two K atoms, split-K with the last-arriver reduction, the single 512-column
-    accumulator stage of 256 x 256 tiles) must give the same answers: forced through the debug environment knobs,
+    """Every launch-plan family (32- and 64-column tiles, split-K with the last-arriver reduction) must give the same answers: forced through the debug environment knobs,
     then chosen by the autotuner."""
     import os
     ctx = new_ctx(rt)
     r = oracle.XorShiftRng(99)
-    keys = ("RTEN_B200_FORCE_BN", "RTEN_B200_FORCE_PAIR", "RTEN_B200_FORCE_KATOMS", "RTEN_B200_FORCE_SPLITK", "RTEN_B200_FORCE_CTA2")
-    plans = [dict(), dict(BN=64, PAIR=1, CTA2=0), dict(BN=128, PAIR=0, KATOMS=2, CTA2=0), dict(BN=256, PAIR=1, CTA2=0),
-             dict(BN=128, PAIR=1, SPLITK=2, CTA2=0), dict(BN=64, PAIR=0, SPLITK=3, CTA2=0), dict(BN=256, PAIR=1, SPLITK=2, CTA2=0),
-             dict(BN=96, PAIR=0, SPLITK=4, KATOMS=1, CTA2=0),
-             # CTA pairs (tcgen05.mma.cta_group::2, 256-row tiles, half of B per CTA)
-             dict(BN=128, PAIR=0, CTA2=1), dict(BN=256, PAIR=0, CTA2=1), dict(BN=256, PAIR=1, CTA2=1), dict(BN=64, PAIR=1, CTA2=1, KATOMS=2),
-             dict(BN=128, PAIR=0, CTA2=1, SPLITK=2), dict(BN=256, PAIR=1, CTA2=1, SPLITK=2), dict(BN=96, PAIR=0, CTA2=1)]
+    keys = ("RTEN_B200_FORCE_BN", "RTEN_B200_FORCE_SPLITK")
+    plans = [dict(), dict(BN=32), dict(BN=64), dict(BN=32, SPLITK=2), dict(BN=64, SPLITK=2), dict(BN=64, SPLITK=3),
+             dict(BN=32, SPLITK=3), dict(BN=64, SPLITK=4)]
     a8 = r.u8((300, 2048))
     b8 = r.i8((2048, 512))
     az, bz = r.u8((300,)), r.i8((512,))
@@ -410,12 +405,12 @@ def check_plans(rt, oracle):
             worst = max(worst, _conv_case(rt, oracle, ctx, (4, 256, 14, 14), (256, 256, 3, 3), pads=(1, 1, 1, 1), cl=True, prepack=True, act=1))
             worst = max(worst, _conv_case(rt, oracle, ctx, (8, 512, 7, 7), (512, 512, 3, 3), pads=(1, 1, 1, 1), cl=True, residual=True, act=1))
             worst = max(worst, _conv_case(rt, oracle, ctx, (2, 64, 20, 20), (96, 64, 1, 1), cl=False))
-            worst = max(worst, _conv_case(rt, oracle, ctx, (4, 512, 14, 14), (256, 512, 1, 1), cl=True, residual=True, act=1))  # 16 K blocks: split-K / CTA-pair plans exist
+            worst = max(worst, _conv_case(rt, oracle, ctx, (4, 512, 14, 14), (256, 512, 1, 1), cl=True, residual=True, act=1))  # 16 K blocks: split-K plans exist
             hit, miss = ctx.forced_plan_counts()
-            # every split-K / CTA-pair family must actually have run somewhere in the sweep (a forced combination that no
+            # every split-K family must actually have run somewhere in the sweep (a forced combination that no
             # launch can satisfy would make this check vacuous); the remaining combinations are reported
             if pl and hit == hits_before:
-                assert "SPLITK" not in pl and not (pl.get("CTA2") == 1 and "KATOMS" not in pl), \
+                assert "SPLITK" not in pl, \
                     f"{tag}: no launch of this sweep ran the forced plan ({miss} fell back to the model's choice)"
                 never.append(str(pl))
             hits_before = hit
@@ -1274,7 +1269,7 @@ def check_attention_decode(rt, oracle):
 
 def check_attention_encoder(rt, oracle):
     """rten_b200_attention on encoder shapes (128 keys, head size 64, q_seq a multiple of 128) in the single-pass TF32 mode:
-    the one-kernel tcgen05 path (QK^T -> masked softmax -> PV inside the SM) against a float64 restatement of
+    the one-kernel wgmma path (QK^T -> masked softmax -> PV inside the SM) against a float64 restatement of
     src/ops/attention.rs:645-905, for every value layout the kernel takes -- contiguous [B,nh,S,dh], strided views of a
     merged Q|K|V projection ([B,S,3H] memory, the layout BertRunner feeds it), and a transposed value tensor --
     with and without an additive [B,1,1,S] mask, output written through a strided [B,S,H] view.  TF32 operands
@@ -1310,7 +1305,12 @@ def check_attention_encoder(rt, oracle):
             layouts["transposed value"] = (layouts["contiguous"][0], layouts["contiguous"][1], dvt.view((B, nh, kv, dh), (nh * dh * kv, dh * kv, 1, kv)))
             for name, (dq, dk, dv) in layouts.items():
                 att = ctx.empty((B, S, H))
-                rt.Attention(scale=0.125).run(ctx, dq, dk, dv, attn_mask=dm, out=att.view((B, nh, S, dh), (S * H, dh, H, 1)))
+                run = lambda: rt.Attention(scale=0.125).run(ctx, dq, dk, dv, attn_mask=dm, out=att.view((B, nh, S, dh), (S * H, dh, H, 1)))
+                if tf32:  # the single-pass TF32 mode takes the one-kernel path for these shapes
+                    _, names = _kernels_launched(lambda: (run(), ctx.sync()))
+                    assert any("attn_fused_kernel" in k for k in names), f"the fused attention kernel did not run ({name}; kernels: {sorted(names)})"
+                else:
+                    run()
                 got = att.numpy().reshape(B, S, nh, dh).transpose(0, 2, 1, 3)
                 err = float(np.abs(got - ref).max() / np.abs(ref).max())
                 tol = 4e-3 if tf32 else 1e-4
@@ -1322,14 +1322,14 @@ def check_attention_encoder(rt, oracle):
 
 
 def check_gelu_epilogue(rt, oracle):
-    """The GEMM epilogue's Gelu (two lanes per packed f32x2 instruction, math.cuh gelu_ref_x2) must be BIT-IDENTICAL to
+    """The GEMM epilogue's Gelu (two lanes at a time, math.cuh gelu_ref_x2) must be BIT-IDENTICAL to
     the Gelu operator (the reference's scalar recipe, bit-exact against the oracle in check_unary) applied to the same
     product: FusedMatMul(bias, Gelu) vs FusedMatMul(bias) -> Gelu with the launch plan pinned (same accumulation order),
     for erf-Gelu and the tanh form, values spanning the exp cut-off, zeros and large magnitudes."""
     import os
     ctx = new_ctx(rt, tf32=True)
     r = oracle.XorShiftRng(2718)
-    forced = {"RTEN_B200_FORCE_BN": "128", "RTEN_B200_FORCE_PAIR": "0", "RTEN_B200_FORCE_KATOMS": "1", "RTEN_B200_FORCE_SPLITK": "1", "RTEN_B200_FORCE_CTA2": "0"}
+    forced = {"RTEN_B200_FORCE_BN": "64", "RTEN_B200_FORCE_SPLITK": "1"}
     os.environ.update(forced)
     try:
         n = 0
@@ -1371,13 +1371,26 @@ def check_skinny_f32(rt, oracle):
     return f"{worst} cases inside 1e-8 + 1e-5*|ref| in both modes"
 
 
+def _kernels_launched(fn):
+    """Run `fn` under CUPTI (torch.profiler) and return the names of the CUDA kernels it launched: lets a check insist
+    that a specialised kernel ran instead of a fall-back path that would meet the same tolerances."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.init()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        out = fn()
+        torch.cuda.synchronize()
+    names = {e.name for e in prof.events()}
+    return out, names
+
+
 def check_halo_conv(rt, oracle):
     """Stride-1 windows on the halo-reuse kernel (one activation patch per channel block in shared memory, the filter taps
     as shifted matrix descriptors): ResNet-50's 3x3 layer shapes at several batch sizes (row strips, whole images, several
     images per unit, batch tails), 5x5 / 1x3 / 3x1 windows, asymmetric padding, both f32 modes; against float64 within the
     TF32 bound, and the generic implicit-GEMM kernel must agree within the same bound."""
     import os
-    os.environ["RTEN_B200_HALO"] = "1"  # the kernel is opt-in (DESIGN.md 4.2)
+    os.environ["RTEN_B200_HALO"] = "1"  # the kernel is opt-in (the generic kernel stays the default)
     try:
         return _check_halo_conv(rt, oracle)
     finally:
@@ -1410,10 +1423,12 @@ def _check_halo_conv(rt, oracle):
     x, w, b = r.uniform((4, 128, 28, 28)), r.uniform((128, 128, 3, 3)) / np.float32(34.0), r.uniform((128,))
     xd = ctx.to_device(x, channels_last=True)
     op = rt.Conv(1, (1, 1), (1, 1, 1, 1), (1, 1), activation=1)
-    halo = op.run(ctx, xd, w, b).numpy()
+    halo, names = _kernels_launched(lambda: op.run(ctx, xd, w, b).numpy())
+    assert any("umma_halo_kernel" in k for k in names), f"the halo kernel did not run (kernels: {sorted(names)})"
     os.environ["RTEN_B200_NO_HALO"] = "1"
     try:
-        generic = op.run(ctx, xd, w, b).numpy()
+        generic, names = _kernels_launched(lambda: op.run(ctx, xd, w, b).numpy())
+        assert not any("umma_halo_kernel" in k for k in names), "RTEN_B200_NO_HALO must select the generic kernel"
     finally:
         os.environ.pop("RTEN_B200_NO_HALO", None)
     exact, absum = _conv_exact(x, w, b, (1, 1, 1, 1), 1, (1, 1), (1, 1))

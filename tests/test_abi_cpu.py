@@ -1,5 +1,5 @@
 """CPU-only checks of the drop-in boundary: the C-ABI library loads and exports every symbol
-include/rten_b200.h declares, and fails loudly (no fallback) when no B200 is present."""
+include/rten_b200.h declares, and fails loudly (no fallback) when no H100 is present."""
 import ctypes
 import os
 import re
@@ -44,7 +44,7 @@ def test_version_and_no_cpu_fallback(lib_path):
     import torch
     from rten_b200 import _lib
     lib = _lib.load()
-    assert b"sm_100a" in lib.rten_b200_version()
+    assert b"sm_90a" in lib.rten_b200_version()
     if torch.cuda.is_available():
         pytest.skip("GPU present")
     import rten_b200 as rt

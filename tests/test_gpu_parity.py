@@ -1,4 +1,4 @@
-"""`pytest -m gpu`: parity of the CUDA path (through the C ABI) against the CPU oracle on a real B200."""
+"""`pytest -m gpu`: parity of the CUDA path (through the C ABI) against the CPU oracle on a real H100."""
 import pytest
 
 import gpu_checks

@@ -10,7 +10,7 @@ import pytest
 import onnx_writer as W
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF_MNIST = "/root/reference/rten-onnx/test-data/mnist.onnx"
+REF_MNIST = os.path.join(HERE, "golden", "mnist.onnx")  # the reference's rten-onnx/test-data/mnist.onnx, byte for byte
 
 
 @pytest.fixture(scope="module")
@@ -46,7 +46,6 @@ def test_decode_mnist_reencoded(summary):
     assert s["inputs"][0]["dims"] == [-1, 1, 28, 28]  # symbolic batch dimension -> -1
 
 
-@pytest.mark.skipif(not os.path.exists(REF_MNIST), reason="reference checkout not present (GPU box)")
 def test_decode_reference_mnist_file(summary):
     s = summary(open(REF_MNIST, "rb").read())
     _assert_mnist_structure(s)
