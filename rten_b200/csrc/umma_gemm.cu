@@ -19,6 +19,13 @@
 //                                outside the output).  Outputs whose rows are not contiguous fall back to direct
 //                                register->global stores.  Runs concurrently with the next tile's main loop thanks
 //                                to the second accumulator stage.
+// Launches that take the plain f32 epilogue (alpha = 1, optional column bias, TMA-staged residual, none / Relu / Gelu)
+// can also run on umma_wide_kernel (umma_kernel.cuh), which computes 128 x 128 or 128 x 256 tiles with 384 threads:
+//   warpgroup 0    : the same TMA producer (one warp issues, registers released with setmaxnreg)
+//   warpgroups 1, 2: 64 rows each, m64n128k8 / m64n256k8 wgmma into registers, then the epilogue from those registers
+//                    through 128-row staging buffers and TMA stores; not overlapped with the next main loop.
+// A wide tile reads each A tile from shared memory once for up to 256 columns and amortises the fixed cost of a
+// pipeline stage over 2-4x the tensor work; the plans of both kernels compete in the cost model and the autotuner.
 // Work decomposition (tile width, split-K, K blocks per stage) is a launch `Plan` (see "Launch plans" below), ranked by
 // a cost model and, optionally, measured on the device per problem.
 // For Conv the A tile is a TMA box over the NHWC activation tensor at (c0, ox0*sx - pad + kx*dx,
@@ -145,6 +152,7 @@ struct Prepared {
     OperandDesc od, ord;
     uint32_t dbox[4];
     int tma_store, res_tma;  // eligibility
+    int wide;                // the wide-tile kernel may run this launch (plain f32 epilogue, see plain_f32_ok)
     int step;
     int esize, kelems;
 };
@@ -152,17 +160,37 @@ struct Prepared {
 constexpr int SK_CNT_INTS = 1 << 16;
 // 227 KB of shared memory per block; SMEM_FIXED_BYTES: alignment slack, barriers, column vectors, accumulators
 static int smem_budget_for(int n_stg, int /*kind*/) { return 227 * 1024 - SMEM_FIXED_BYTES - n_stg * STG_BYTES; }
+// operand stages of the wide-tile kernel: 6 at bn = 128, 4 at bn = 256
+static int wide_stages(int stage_bytes) { return std::min(MAX_STAGES, (227 * 1024 - WIDE_SMEM_FIXED_BYTES) / stage_bytes); }
+static bool is_wide(int bn) { return bn > ACC_STRIDE; }
+
+// The f32 launches whose every chunk takes the plain epilogue (kernel variants 3 and 5): TMA store, N % 32 == 0,
+// alpha = 1, optional aligned column bias, optional TMA-staged residual with r_scale = 1, act in {none, Relu, Gelu,
+// ApproxGelu}, no range output.
+static bool plain_f32_ok(const rten_ctx* ctx, const GemmLaunch& L, int tma_store, int res_tma) {
+    const EpilogueDesc& e = L.epi;
+    return L.kind == 0 && tma_store && (L.N % 32) == 0 && (!ctx->trace || getenv("RTEN_B200_TRACE_FAST")) &&
+           !getenv("RTEN_B200_NO_FAST") && !getenv("RTEN_B200_NO_PLAIN") && e.bias_kind != 2 &&
+           (e.bias_kind != 1 || (reinterpret_cast<uintptr_t>(e.bias) & 15) == 0) && e.alpha == 1.0f && e.act <= 3 &&
+           !e.range && (e.r == nullptr || (res_tma && e.r_scale == 1.0f));
+}
 
 struct PlanShape {
     long long tiles_n, units_m, tiles, units;
     int kb_per, atom_bytes, stage_bytes, stages, n_stg;
 };
 
-// Derived sizes of a plan; false if the plan cannot run (accumulator columns, shared memory, counters).  The kernel
-// computes one 128 x bn tile per unit, bn in {32, 64}: pair / ksplit / acc1 / cta2 are not available on sm_90.
+// Derived sizes of a plan; false if the plan cannot run (accumulator columns, shared memory, counters).  The kernels
+// compute one 128 x bn tile per unit: bn in {32, 64} (umma_gemm_kernel), or bn in {128, 256} without split-K for the
+// launches that take the plain f32 epilogue (umma_wide_kernel).  pair / ksplit / acc1 / cta2 are not available on sm_90.
 static bool plan_shape(const Prepared& q, const Plan& pl, PlanShape& ps) {
     const KParams& p = q.p;
-    if (pl.bn < 16 || pl.bn > ACC_STRIDE || pl.bn % 32 || pl.bn % q.step) return false;
+    if (is_wide(pl.bn)) {
+        if ((pl.bn != 128 && pl.bn != 256) || !q.wide || pl.splitk != 1) return false;
+        if (pl.bn == 256 && q.p.epi.act > 1) return false;  // Gelu: 128-column tiles only (umma_wide_kernel)
+    } else if (pl.bn < 16 || pl.bn % 32 || pl.bn % q.step) {
+        return false;
+    }
     if (pl.pair || pl.ksplit || pl.acc1 || pl.cta2 || pl.katoms != 1) return false;  // one K block per stage: straight-line wgmma issue
     ps.tiles_n = (p.N + pl.bn - 1) / pl.bn;
     ps.units_m = p.tiles_m;
@@ -177,28 +205,31 @@ static bool plan_shape(const Prepared& q, const Plan& pl, PlanShape& ps) {
     ps.n_stg = 2 * pl.nbuf;
     ps.atom_bytes = A_STAGE_BYTES + pl.bn * KBYTES;
     ps.stage_bytes = ps.atom_bytes;
-    ps.stages = std::min(MAX_STAGES, smem_budget_for(ps.n_stg, q.esize == 4 ? 0 : 1) / ps.stage_bytes);
+    ps.stages = is_wide(pl.bn) ? wide_stages(ps.stage_bytes)
+                               : std::min(MAX_STAGES, smem_budget_for(ps.n_stg, q.esize == 4 ? 0 : 1) / ps.stage_bytes);
     if (ps.stages < 2) return false;
     return true;
 }
 
 // Cost model in SM clocks.  Its constants are unmeasured estimates that only rank candidate plans:
 //   * the operand stream L2 -> shared memory (~7400 B/clk for the whole chip, at most ~64 B/clk for one SM) bounds a K block;
-//   * the tensor pipe needs bn/2 clk per 128 x bn x 32-byte step, issuing it ~42 clk;
+//   * the tensor pipe needs bn clk per 128 x bn x 32-byte step at the data-sheet TF32 rate (~1024 MAC / clk / SM),
+//     issuing it ~42 clk;
 //   * every pipeline stage costs a fixed ~320 clk (barrier wait, fence, descriptors, commit);
 //   * a stage cannot complete faster than the TMA latency (~2300 clk under load) / stages in flight;
-//   * the epilogue (~350 clk per 32-column chunk, two warp groups) overlaps the next main loop.
+//   * the narrow kernel's epilogue (~350 clk per 32-column chunk, two warp groups) overlaps the next main loop; the
+//     wide kernel's (~400 clk per chunk, both warpgroups on every chunk) follows its main loop.
 static double plan_cost(const Prepared& q, const Plan& pl, const PlanShape& ps, int num_sms) {
     const double active = (double)std::min<long long>(ps.units, num_sms);
     const double waves = std::ceil((double)ps.units / num_sms);
     const double bw = std::min(64.0, 7400.0 / active);
     const double mmas = 4.0;
-    const double t_kb = std::max(mmas * std::max(42.0, pl.bn / 2.0), ps.atom_bytes / bw);
+    const double t_kb = std::max(mmas * std::max(42.0, (double)pl.bn), ps.atom_bytes / bw);
     double t_stage = std::max(t_kb, 320.0 + mmas * 42.0);
     t_stage = std::max(t_stage, 2300.0 / ps.stages);
     const double mainloop = ps.kb_per * t_stage;
-    const double epi = (pl.bn / 32.0) * 350.0 / 2.0 + 600.0;
-    double unit = std::max(mainloop, epi) + 1500.0;
+    const double epi = is_wide(pl.bn) ? (pl.bn / 32.0) * 400.0 + 600.0 : (pl.bn / 32.0) * 350.0 / 2.0 + 600.0;
+    double unit = (is_wide(pl.bn) ? mainloop + epi : std::max(mainloop, epi)) + 1500.0;
     double cost = waves * unit + 2500.0;
     if (pl.splitk > 1) cost += epi * (1.0 + 0.25 * pl.splitk) + 1500.0;  // publish + the owner's reduction
 
@@ -209,7 +240,7 @@ static void enumerate_plans(const Prepared& q, int num_sms, std::vector<std::pai
     const KParams& p = q.p;
     const int nmax = (p.N + q.step - 1) / q.step * q.step;
     static const int splits[] = {1, 2, 3, 4, 5, 6, 8, 10, 12, 16};
-    for (int bn = 32; bn <= ACC_STRIDE; bn += 32) {
+    for (int bn : {32, 64, 128, 256}) {
         if (bn > nmax && bn != 32) break;
         for (int sk : splits) {
             Plan pl;
@@ -219,7 +250,9 @@ static void enumerate_plans(const Prepared& q, int num_sms, std::vector<std::pai
             const int kb_per = (p.k_blocks + sk - 1) / sk;
             pl.nbuf = (q.res_tma || kb_per < 24) ? 2 : 1;
             PlanShape ps;
-            if (pl.nbuf == 2 && !getenv("RTEN_B200_NO_NBUF3")) {
+            if (is_wide(bn)) {
+                pl.nbuf = 2;  // (the wide kernel has two fixed staging buffers)
+            } else if (pl.nbuf == 2 && !getenv("RTEN_B200_NO_NBUF3")) {
                 // A third staging buffer per group takes the wait for the previous store's shared-memory read and, with a
                 // residual, the late request of the next residual tile off the chunk's critical path -- as long as the
                 // operand ring keeps three stages (or loses none)
@@ -354,6 +387,8 @@ static rten_status prepare_launch(rten_ctx* ctx, const GemmLaunch& L, Prepared& 
     if (getenv("RTEN_B200_NO_RES_TMA")) q.res_tma = 0;
     p.res_tx_bytes = q.a_rows * KBYTES;
     q.step = q.tma_store ? 32 : 16;
+    // RTEN_B200_NO_WIDE=1: no wide-tile plans (measures what they gain; recorded wide plans are re-planned)
+    q.wide = plain_f32_ok(ctx, L, q.tma_store, q.res_tma) && !getenv("RTEN_B200_NO_WIDE");
     return RTEN_OK;
 }
 
@@ -415,7 +450,7 @@ static rten_status launch_single(rten_ctx* ctx, int cls, const PendingLaunch& pl
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(NUM_THREADS);
+    cfg.blockDim = dim3(is_wide(p.bn) ? WIDE_THREADS : NUM_THREADS);
     cfg.dynamicSmemBytes = pl.smem_bytes;
     cfg.stream = ctx->stream;
     cudaLaunchAttribute attr[2];
@@ -426,7 +461,9 @@ static rten_status launch_single(rten_ctx* ctx, int cls, const PendingLaunch& pl
         return cudaLaunchKernelEx(&cfg, kern, pl.maps[0], pl.maps[1], pl.maps[2], pl.maps[3], pl.maps[4], p);
     };
     cudaError_t e;
-    if (pl.plain && cls == 1) {
+    if (is_wide(p.bn)) {  // (plain f32 epilogue only: launch_plan)
+        e = launch(cls == 2 ? umma_wide_kernel<5> : umma_wide_kernel<3>);
+    } else if (pl.plain && cls == 1) {
         e = launch(umma_gemm_kernel<0, 3>);
     } else if (pl.plain && cls == 2) {
         e = launch(umma_gemm_kernel<0, 5>);
@@ -538,7 +575,7 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
     p.atom_bytes = ps.atom_bytes;
     p.stage_bytes = ps.stage_bytes;
     p.tx_bytes = (p.pair ? 2 : 1) * q.a_rows * KBYTES + (p.bn >> p.cta2) * KBYTES;  // per 128-byte K block and CTA
-    p.stages = std::min(MAX_STAGES, smem_budget_for(n_stg, L.kind) / (int)p.stage_bytes);
+    p.stages = is_wide(p.bn) ? ps.stages : std::min(MAX_STAGES, smem_budget_for(n_stg, L.kind) / (int)p.stage_bytes);
     if (p.stages < 2) return RTEN_ERR_UNSUPPORTED_VALUE;
     if (L.kind == 0)
         p.idesc = make_idesc(1 /*F32*/, 2 /*TF32*/, 2, BM, p.bn);
@@ -572,7 +609,8 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
         fprintf(stderr, "[umma_gemm] kind=%d conv=%d M=%d N=%d K=%d kb=%d tiles_m=%d bn=%d pair=%d ksplit=%d katoms=%d splitk=%d acc1=%d cta2=%d units=%d stages=%d tma_store=%d res_tma=%d nbuf=%d box=%dx%dx%d\n",
                 L.kind, L.conv, L.M, L.N, L.K, p.k_blocks, p.tiles_m, p.bn, p.pair, p.ksplit, p.katoms, p.splitk, p.acc1, p.cta2,
                 p.units_total, p.stages, p.tma_store, p.res_tma, p.nbuf, p.tw, p.th, p.tb);
-    const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + n_stg * STG_BYTES + SMEM_FIXED_BYTES;
+    const size_t smem_bytes = (size_t)p.stages * p.stage_bytes +
+                              (is_wide(p.bn) ? WIDE_SMEM_FIXED_BYTES : n_stg * STG_BYTES + SMEM_FIXED_BYTES);
     // specialised epilogue when every chunk qualifies for the register fast path
     const EpilogueDesc& ee = L.epi;
     bool fastk = p.tma_store && (L.N % 32) == 0 && (!ctx->trace || getenv("RTEN_B200_TRACE_FAST")) && !getenv("RTEN_B200_NO_FAST");
@@ -589,11 +627,12 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
     if (!fastk && (L.kind == 1 || ee.act > 1)) p.res_tma = 0;
     PendingLaunch pend;
     if (L.kind == 0)
-        pend.plain = fastk && ee.alpha == 1.0f && ee.act <= 3 && !ee.range && (ee.r == nullptr || (p.res_tma && ee.r_scale == 1.0f));
+        pend.plain = fastk && plain_f32_ok(ctx, L, p.tma_store, p.res_tma);
     else  // integer kind: the *ToFloat operators with a scalar (or no) activation zero point and symmetric weights
         pend.plain = fastk && ee.scale && !ee.za && !ee.zb && (ee.scale_len == 1 || ee.scale_len == L.N) && ee.act <= 3 && p.splitk == 1 &&
                      (ee.r == nullptr || p.res_tma) && (!ee.za8 || ee.colsum);
     if (getenv("RTEN_B200_NO_PLAIN")) pend.plain = false;
+    if (is_wide(p.bn) && !pend.plain) return RTEN_ERR_UNSUPPORTED_VALUE;  // (an output / residual map failed to encode)
     pend.p = p;
     pend.maps[0] = map_a;
     pend.maps[1] = map_b;
@@ -608,7 +647,7 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
     // cheaper than what programmatic dependent launch already overlaps, so separate launches stay the default.
     const char* seq_env = getenv("RTEN_B200_SEQ");
     const bool seq_on = seq_env && atoi(seq_env) != 0;
-    if (seq_on && ctx->capturing && !p.cta2 && !p.x3_cb && !ctx->trace && !no_defer && cls % 3 != 2) {
+    if (seq_on && ctx->capturing && !p.cta2 && !p.x3_cb && !ctx->trace && !no_defer && cls % 3 != 2 && !is_wide(p.bn)) {
         auto* q2 = pending_of(ctx);
         if (!q2->empty() && ctx->seq_class != cls) RTB_TRY(seq_flush(ctx));
         ctx->seq_class = cls;

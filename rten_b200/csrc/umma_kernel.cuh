@@ -1,5 +1,6 @@
 // Device side of the wgmma GEMM / implicit-GEMM convolution: tile decode, the warp-specialised persistent kernel
-// (MMA warpgroup / two epilogue groups / TMA producer) and the opt-in sequence kernel.  Included ONLY by
+// (MMA warpgroup / two epilogue groups / TMA producer), the opt-in sequence kernel and the wide-tile kernel (producer
+// warpgroup / two MMA + epilogue warpgroups).  Included ONLY by
 // umma_gemm.cu, which holds the host side (launch plans, cost model, autotuner, tensor maps).  See umma_gemm.cu's header
 // comment for the design.
 #pragma once
@@ -17,7 +18,7 @@ namespace rtb {
 constexpr int BM = 128;            // rows per tile: two 64-row wgmma instructions
 constexpr int KBYTES = 128;        // bytes of K per stage row = one 128B swizzle atom
 constexpr int A_STAGE_BYTES = BM * KBYTES;
-constexpr int ACC_STRIDE = 64;     // accumulator columns per stage (two stages, ptx.cuh ACC_COLS); also the widest tile
+constexpr int ACC_STRIDE = 64;     // accumulator columns per stage (two stages, ptx.cuh ACC_COLS); also the widest tile of umma_gemm_kernel
 constexpr int PRODUCER_WARP = 12;
 constexpr int NUM_THREADS = 416;   // MMA warpgroup (warps 0-3) + 8 epilogue warps (two groups of 4) + TMA producer warp
 constexpr int STG_BYTES = 128 * 128;  // one 128-row x 128-byte output staging buffer per epilogue group
@@ -312,6 +313,94 @@ __device__ __forceinline__ void mma_role(const KParams& p, const SmemLayout& L, 
     }
 }
 
+// TMA producer of both GEMM kernels: one warp walks this CTA's work units and fills the operand ring -- A (128 rows, or
+// two 128-row tiles in pair mode) and B (bn rows) per 128-byte K block, the conv filter tap / channel walk, the two-plane
+// 3xTF32 segments and broadcast batch dims.  Runs warp-uniformly, one elected lane issues.
+__device__ __forceinline__ void producer_role(const KParams& p, const CUtensorMap* tma_a, const CUtensorMap* tma_a2,
+                                              const CUtensorMap* tma_b, const SmemLayout& L, int worker, int n_workers,
+                                              PipeState& st) {
+    uint8_t* smem = L.smem;
+    uint64_t* full_bar = L.full_bar;
+    uint64_t* empty_bar = L.empty_bar;
+    int stage = 0;
+    int tr_p = 0;
+    const uint32_t smem0 = smem_u32(smem);
+    const uint32_t full0 = smem_u32(full_bar);
+    const uint32_t a_bytes = (p.pair ? 2 : 1) * A_STAGE_BYTES;
+    for (int u = worker; u < p.units_total; u += n_workers) {
+        int t, ks;
+        p.d_tiles_total.divmod(u, ks, t);
+        const int kb0 = ks * p.kb_per, kb1 = min(p.k_blocks, kb0 + p.kb_per);
+        const TileCoord tc = decode_tile(p, t, 0);
+        const TileCoord tc1 = p.pair ? decode_tile(p, t, 1) : tc;
+        // conv: K block -> (filter tap, channel block), kept incrementally
+        int tap, cb, ky, kx;
+        p.d_c_blocks.divmod(kb0, tap, cb);
+        p.d_kw.divmod(tap, ky, kx);
+        // two-plane 3xTF32: segment of the K / channel range and block inside it (kept incrementally)
+        int seg = 0, sblk = p.conv ? cb : kb0;
+        if (p.x3_cb)
+            while (sblk >= p.x3_cb) {
+                sblk -= p.x3_cb;
+                seg++;
+            }
+        // programmatic dependent launch: the producer is the first to touch the predecessor's output; everything
+        // above (tile decode) ran while the predecessor grid was still draining
+        if (u == worker) asm volatile("griddepcontrol.wait;" ::: "memory");
+        for (int kb = kb0; kb < kb1; kb += p.katoms) {
+            const int natoms = min(p.katoms, kb1 - kb);
+            mbar_wait(&empty_bar[stage], ((st.ring >> stage) & 1) ^ 1);
+            const bool leader = elect_one();
+            const uint32_t fb = full0 + stage * 8;
+            if (leader) {
+                if (p.trace && blockIdx.x == 0 && tr_p < 2048) p.trace[tr_p++] = clock64();
+                mbar_expect_tx_u32(fb, p.tx_bytes * natoms);
+            }
+            for (int a = 0; a < natoms; a++) {
+                if (leader) {
+                    const uint32_t sa = smem0 + stage * p.stage_bytes + a * p.atom_bytes;
+                    const uint32_t sb = sa + a_bytes;
+                    auto load = [&](uint32_t dst, const CUtensorMap* m, int c0, int c1, int c2, int c3) {
+                        tma_load_4d_u32(dst, m, fb, c0, c1, c2, c3);
+                    };
+                    const CUtensorMap* ma = (p.x3_cb && seg == 0) ? tma_a2 : tma_a;
+                    if (p.conv) {
+                        const int c0 = cb * p.kelems;
+                        const int ca = p.x3_cb ? sblk * p.kelems : c0;
+                        load(sa, ma, ca, tc.ox0 * p.sx - p.pl + kx * p.dx, tc.oy0 * p.sy - p.pt + ky * p.dy, tc.b0);
+                        if (p.pair)
+                            load(sa + A_STAGE_BYTES, ma, ca, tc1.ox0 * p.sx - p.pl + kx * p.dx,
+                                 tc1.oy0 * p.sy - p.pt + ky * p.dy, tc1.b0);
+                        load(sb, tma_b, c0, tc.n0, tap, 0);
+                    } else {
+                        const int k0 = (kb + a) * p.kelems;
+                        const int ka = p.x3_cb ? sblk * p.kelems : k0;
+                        const int az0 = p.a_bcast0 ? 0 : tc.z0, az1 = p.a_bcast1 ? 0 : tc.z1;
+                        load(sa, ma, ka, tc.m0, az0, az1);
+                        if (p.pair) load(sa + A_STAGE_BYTES, ma, ka, tc1.m0, az0, az1);
+                        load(sb, tma_b, k0, tc.n0, p.b_bcast0 ? 0 : tc.z0, p.b_bcast1 ? 0 : tc.z1);
+                    }
+                }
+                if (p.x3_cb && ++sblk == p.x3_cb) {
+                    sblk = 0;
+                    seg = seg == 2 ? 0 : seg + 1;  // (conv: the next filter tap starts over at segment 0)
+                }
+                if (++cb == p.c_blocks) {
+                    cb = 0;
+                    tap++;
+                    if (++kx == p.kw) {
+                        kx = 0;
+                        ky++;
+                    }
+                }
+            }
+            __syncwarp();
+            st.ring ^= 1u << stage;
+            if (++stage == p.stages) stage = 0;
+        }
+    }
+}
+
 // One launch worth of work (all roles).  FAST = the launch satisfies, for EVERY chunk, the conditions of the register
 // fast path (TMA-store output, N % 32 == 0, f32 with act in {none, relu} and bias / residual absent or
 // vector-addressable [residual via TMA], or raw i32): the epilogue is then a short straight-line loop.  The generic
@@ -323,8 +412,6 @@ __device__ __forceinline__ void run_layer(const KParams& p, const CUtensorMap* t
     uint8_t* smem = L.smem;
     uint8_t* stg_base = smem + (size_t)p.stages * p.stage_bytes;
     const int nbuf = p.nbuf;
-    uint64_t* full_bar = L.full_bar;
-    uint64_t* empty_bar = L.empty_bar;
     uint64_t* acc_full = L.acc_full;
     uint64_t* acc_empty = L.acc_empty;
     uint64_t* res_bar = L.res_bar;
@@ -335,84 +422,7 @@ __device__ __forceinline__ void run_layer(const KParams& p, const CUtensorMap* t
     // TMA / MMA instructions): addresses and descriptors then live in uniform registers instead of being moved
     // there (R2UR) for every instruction, which is what bounds a single issuing thread.
     if (warp == PRODUCER_WARP) {
-        // ===================== TMA producer =====================
-        int stage = 0;
-        int tr_p = 0;
-        const uint32_t smem0 = smem_u32(smem);
-        const uint32_t full0 = smem_u32(full_bar);
-        const uint32_t a_bytes = (p.pair ? 2 : 1) * A_STAGE_BYTES;
-        for (int u = worker; u < p.units_total; u += n_workers) {
-            int t, ks;
-            p.d_tiles_total.divmod(u, ks, t);
-            const int kb0 = ks * p.kb_per, kb1 = min(p.k_blocks, kb0 + p.kb_per);
-            const TileCoord tc = decode_tile(p, t, 0);
-            const TileCoord tc1 = p.pair ? decode_tile(p, t, 1) : tc;
-            // conv: K block -> (filter tap, channel block), kept incrementally
-            int tap, cb, ky, kx;
-            p.d_c_blocks.divmod(kb0, tap, cb);
-            p.d_kw.divmod(tap, ky, kx);
-            // two-plane 3xTF32: segment of the K / channel range and block inside it (kept incrementally)
-            int seg = 0, sblk = p.conv ? cb : kb0;
-            if (p.x3_cb)
-                while (sblk >= p.x3_cb) {
-                    sblk -= p.x3_cb;
-                    seg++;
-                }
-            // programmatic dependent launch: the producer is the first to touch the predecessor's output; everything
-            // above (tile decode) ran while the predecessor grid was still draining
-            if (u == worker) asm volatile("griddepcontrol.wait;" ::: "memory");
-            for (int kb = kb0; kb < kb1; kb += p.katoms) {
-                const int natoms = min(p.katoms, kb1 - kb);
-                mbar_wait(&empty_bar[stage], ((st.ring >> stage) & 1) ^ 1);
-                const bool leader = elect_one();
-                const uint32_t fb = full0 + stage * 8;
-                if (leader) {
-                    if (p.trace && blockIdx.x == 0 && tr_p < 2048) p.trace[tr_p++] = clock64();
-                    mbar_expect_tx_u32(fb, p.tx_bytes * natoms);
-                }
-                for (int a = 0; a < natoms; a++) {
-                    if (leader) {
-                        const uint32_t sa = smem0 + stage * p.stage_bytes + a * p.atom_bytes;
-                        const uint32_t sb = sa + a_bytes;
-                        auto load = [&](uint32_t dst, const CUtensorMap* m, int c0, int c1, int c2, int c3) {
-                            tma_load_4d_u32(dst, m, fb, c0, c1, c2, c3);
-                        };
-                        const CUtensorMap* ma = (p.x3_cb && seg == 0) ? tma_a2 : tma_a;
-                        if (p.conv) {
-                            const int c0 = cb * p.kelems;
-                            const int ca = p.x3_cb ? sblk * p.kelems : c0;
-                            load(sa, ma, ca, tc.ox0 * p.sx - p.pl + kx * p.dx, tc.oy0 * p.sy - p.pt + ky * p.dy, tc.b0);
-                            if (p.pair)
-                                load(sa + A_STAGE_BYTES, ma, ca, tc1.ox0 * p.sx - p.pl + kx * p.dx,
-                                     tc1.oy0 * p.sy - p.pt + ky * p.dy, tc1.b0);
-                            load(sb, tma_b, c0, tc.n0, tap, 0);
-                        } else {
-                            const int k0 = (kb + a) * p.kelems;
-                            const int ka = p.x3_cb ? sblk * p.kelems : k0;
-                            const int az0 = p.a_bcast0 ? 0 : tc.z0, az1 = p.a_bcast1 ? 0 : tc.z1;
-                            load(sa, ma, ka, tc.m0, az0, az1);
-                            if (p.pair) load(sa + A_STAGE_BYTES, ma, ka, tc1.m0, az0, az1);
-                            load(sb, tma_b, k0, tc.n0, p.b_bcast0 ? 0 : tc.z0, p.b_bcast1 ? 0 : tc.z1);
-                        }
-                    }
-                    if (p.x3_cb && ++sblk == p.x3_cb) {
-                        sblk = 0;
-                        seg = seg == 2 ? 0 : seg + 1;  // (conv: the next filter tap starts over at segment 0)
-                    }
-                    if (++cb == p.c_blocks) {
-                        cb = 0;
-                        tap++;
-                        if (++kx == p.kw) {
-                            kx = 0;
-                            ky++;
-                        }
-                    }
-                }
-                __syncwarp();
-                st.ring ^= 1u << stage;
-                if (++stage == p.stages) stage = 0;
-            }
-        }
+        producer_role(p, tma_a, tma_a2, tma_b, L, worker, n_workers, st);
     } else if (warp < 4) {
         // ===================== MMA warpgroup: accumulators in registers, finished tiles to shared memory
         if (p.bn == 32)
@@ -585,6 +595,224 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) umma_seq_kernel(const __grid_c
     if (threadIdx.x == 0) {
         const unsigned old = atomicAdd(sp.gbar, 1u);
         if (old == gridDim.x * (unsigned)sp.n - 1u) *reinterpret_cast<volatile unsigned*>(sp.gbar) = 0u;
+    }
+}
+
+// ------------------------------------------------------------------------------------------
+// Wide tiles: one 128 x 128 or 128 x 256 tile per work unit, for the launches that take the plain f32 epilogue
+// (FAST = 3, + Gelu: 5) without split-K.  A 64-column tile cannot keep the tensor core busy: every m64nNk8 reads
+// 2 KB of A from shared memory for N/2 clocks of math, and the fixed cost of a pipeline stage is as large as its
+// tensor work.  A wide tile reads A once for up to 256 columns.  Its accumulator (up to 256 f32 registers per
+// thread of one warpgroup) does not fit the narrow kernel's role layout, so this kernel has its own:
+//   warpgroup 0    : TMA producer (warp 0; producer_role, shared with umma_gemm_kernel), registers released
+//   warpgroups 1, 2: rows 0-63 / 64-127 of the tile, m64n{bn}k8 wgmma into bn/2 registers per thread, then the
+//                    epilogue straight from those registers in 32-column chunks
+// The epilogue is not overlapped with the next main loop; the producer keeps filling the operand ring meanwhile.
+// A conv tile's 128 rows form one TMA box (tw x th x tb pixels) that does not split at row 64, so both warpgroups
+// write each chunk into one shared 128-row staging buffer (two of them, alternating) stored by one TMA instruction.
+// ------------------------------------------------------------------------------------------
+constexpr int WIDE_THREADS = 384;
+// alignment slack, two 128-row staging buffers, then mbarriers (256 B) and the unit's bias (up to 1 KB)
+constexpr int WIDE_SMEM_FIXED_BYTES = 1024 + 2 * STG_BYTES + 2048;
+
+template <int N>
+__device__ __forceinline__ void wgmma_wide(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc) {
+    if constexpr (N == 128) wgmma_tf32_n128(d, adesc, bdesc);
+    else wgmma_tf32_n256(d, adesc, bdesc);
+}
+
+// both consumer warpgroups (named barrier 1)
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// Operand stages first (1024-B aligned, like the staging buffers behind them), the small items last.
+__device__ __forceinline__ SmemLayout carve_wide_smem(uint8_t* smem_raw, const KParams& p) {
+    uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t* tail = base + (size_t)p.stages * p.stage_bytes + 2 * STG_BYTES;
+    SmemLayout L;
+    L.smem = base;
+    L.full_bar = reinterpret_cast<uint64_t*>(tail);
+    L.empty_bar = L.full_bar + MAX_STAGES;
+    L.res_bar = L.empty_bar + MAX_STAGES;  // [staging buffer]
+    L.acc_full = L.acc_empty = nullptr;
+    L.sk_flag = nullptr;
+    L.bias = reinterpret_cast<float*>(tail + 256);
+    L.acc_smem = 0;
+    return L;
+}
+
+// Main loop and epilogue of one consumer warpgroup (wg = 0: rows 0-63, 1: rows 64-127).  Each 128-byte K block is four
+// k8 wgmma, one commit group, one group in flight across stages as in mma_units; a stage goes back to the producer
+// once both warpgroups have retired it (8 warp arrivals).  Epilogue: x = act((acc + residual) + bias), each add
+// rounded to nearest, in the order of epilogue_plain_f32 -- the results equal the narrow kernel's.
+template <int FAST, int N>
+__device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout& L, const CUtensorMap* tma_d,
+                                              const CUtensorMap* tma_r, int worker, int n_workers) {
+    const int t = threadIdx.x - 128;  // 0-255 over both warpgroups
+    const int wg = t >> 7;
+    const int lane = threadIdx.x & 31;
+    const int row0 = 64 * wg + 16 * ((t & 127) >> 5) + (lane >> 2);  // this thread's fragment rows: row0, row0 + 8
+    const int sw = lane >> 2;                                          // row0 & 7: 128B swizzle of both rows
+    const int cq = lane & 3;                                           // columns 8j + 2cq + {0, 1} of every 8
+    const bool issuer = t == 0;
+    const EpilogueDesc& e = p.epi;
+    const uint32_t smem0 = smem_u32(L.smem);
+    uint8_t* const stg0 = L.smem + (size_t)p.stages * p.stage_bytes;
+    float* const bias_s = L.bias;
+    uint32_t ring = 0, rphase = 0;
+    uint32_t ci = 0;  // chunks of this CTA so far: chunk ci uses staging buffer ci & 1
+    int stage = 0;
+    auto load_residual = [&](const TileCoord& tc, int c0, int buf) {
+        uint64_t* rb = &L.res_bar[buf];
+        mbar_expect_tx(rb, p.res_tx_bytes);
+        if (p.conv)
+            tma_load_4d(stg0 + buf * STG_BYTES, tma_r, rb, tc.n0 + c0, tc.ox0, tc.oy0, tc.b0);
+        else
+            tma_load_4d(stg0 + buf * STG_BYTES, tma_r, rb, tc.n0 + c0, tc.m0, tc.z0, tc.z1);
+    };
+    for (int u = worker; u < p.units_total; u += n_workers) {
+        {  // (the tile is decoded again after the main loop: its coordinates would hold registers through it)
+            const TileCoord tc = decode_tile(p, u, 0);  // (no split-K: a unit is a tile)
+            // The unit's bias (zeros without one: x + 0 keeps the -0 -> +0 of the other epilogues).  Every reader of the
+            // previous unit's values has passed the last chunk barrier; the barrier after the main loop publishes these.
+            if (t < N) bias_s[t] = (e.bias_kind == 1 && tc.n0 + t < p.N) ? __ldg(e.bias + tc.n0 + t) : 0.0f;
+            if (issuer) {
+                bulk_wait_read(0);  // staging buffers free
+                if (p.res_tma) load_residual(tc, 0, ci & 1);
+            }
+        }
+        float d[N / 2];
+#pragma unroll
+        for (int i = 0; i < N / 2; i++) d[i] = 0.0f;
+        int prev = -1;
+        for (int kb = 0; kb < p.k_blocks; kb++) {
+            mbar_wait(&L.full_bar[stage], (ring >> stage) & 1);
+            wgmma_fence_operand(d);
+            wgmma_fence();
+            const uint32_t sa = smem0 + stage * p.stage_bytes;
+            const uint64_t adesc = make_kmajor_sw128_desc(sa + wg * (64 * KBYTES));
+            const uint64_t bdesc = make_kmajor_sw128_desc(sa + A_STAGE_BYTES);
+#pragma unroll
+            for (int k = 0; k < 4; k++) wgmma_wide<N>(d, adesc + 2 * k, bdesc + 2 * k);
+            wgmma_commit();
+            wgmma_fence_operand(d);
+            wgmma_wait<1>();
+            if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
+            prev = stage;
+            ring ^= 1u << stage;
+            if (++stage == p.stages) stage = 0;
+        }
+        wgmma_wait<0>();
+        wgmma_fence_operand(d);
+        if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
+        const TileCoord tc = decode_tile(p, u, 0);
+        consumers_sync();
+#pragma unroll
+        for (int k = 0; k < N / 32; k++, ci++) {
+            const int buf = ci & 1;
+            uint8_t* stg = stg0 + buf * STG_BYTES;
+            const int nbase = tc.n0 + 32 * k;
+            if (issuer) {
+                // the previous chunk's store has read the other buffer: it takes the next residual chunk, and the
+                // writes of the next chunk (after this chunk's barrier) may land in it
+                bulk_wait_read(0);
+                if (p.res_tma && k + 1 < N / 32) load_residual(tc, 32 * (k + 1), buf ^ 1);
+            }
+            if (p.res_tma) {
+                mbar_wait(&L.res_bar[buf], (rphase >> buf) & 1);
+                rphase ^= 1u << buf;
+            }
+#pragma unroll
+            for (int j = 0; j < 4; j++) {  // columns 32k + 8j + 2cq + {0, 1}, rows row0 + 8h
+                const int i0 = 16 * k + 4 * j;
+                float2* px[2];
+#pragma unroll
+                for (int h = 0; h < 2; h++)
+                    px[h] = reinterpret_cast<float2*>(stg + (row0 + 8 * h) * 128 + (((2 * j + (cq >> 1)) ^ sw) << 4) + 8 * (cq & 1));
+                if (nbase < p.N) {  // (a tile may overhang N by whole chunks: the TMA store clips them)
+                    const float2 bb = *reinterpret_cast<const float2*>(bias_s + 32 * k + 8 * j + 2 * cq);
+#pragma unroll
+                    for (int h = 0; h < 2; h++) {
+                        uint32_t v0 = __float_as_uint(d[i0 + 2 * h]), v1 = __float_as_uint(d[i0 + 2 * h + 1]);
+                        if (p.res_tma) {
+                            const float2 rr = *px[h];
+                            add_f32x2(v0, v1, rr.x, rr.y);
+                        }
+                        add_f32x2(v0, v1, bb.x, bb.y);
+                        if (e.act == 1) {
+                            v0 = __float_as_uint(fmaxf(__uint_as_float(v0), 0.0f));
+                            v1 = __float_as_uint(fmaxf(__uint_as_float(v1), 0.0f));
+                        }
+                        d[i0 + 2 * h] = __uint_as_float(v0);
+                        d[i0 + 2 * h + 1] = __uint_as_float(v1);
+                    }
+                    if (FAST == 5) {  // Gelu / ApproxGelu: the out-of-line polynomial, four values per call
+                        const float4 g = act4(make_float4(d[i0], d[i0 + 1], d[i0 + 2], d[i0 + 3]), e.act);
+                        d[i0] = g.x;
+                        d[i0 + 1] = g.y;
+                        d[i0 + 2] = g.z;
+                        d[i0 + 3] = g.w;
+                    }
+                }
+#pragma unroll
+                for (int h = 0; h < 2; h++) *px[h] = make_float2(d[i0 + 2 * h], d[i0 + 2 * h + 1]);
+            }
+            fence_proxy_async();
+            consumers_sync();
+            if (issuer) {
+                if (p.conv)
+                    tma_store_4d(tma_d, stg, nbase, tc.ox0, tc.oy0, tc.b0);
+                else
+                    tma_store_4d(tma_d, stg, nbase, tc.m0, tc.z0, tc.z1);
+                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+            }
+        }
+    }
+    if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+}
+
+template <int FAST>
+__global__ void __launch_bounds__(WIDE_THREADS, 1)
+umma_wide_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
+                 const __grid_constant__ CUtensorMap tma_d, const __grid_constant__ CUtensorMap tma_r,
+                 const __grid_constant__ CUtensorMap tma_a2, const __grid_constant__ KParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    const SmemLayout L = carve_wide_smem(smem_raw, p);
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&tma_a);
+        tma_prefetch_desc(&tma_b);
+        tma_prefetch_desc(&tma_d);
+        if (p.res_tma) tma_prefetch_desc(&tma_r);
+        if (p.x3_cb) tma_prefetch_desc(&tma_a2);
+    }
+    if (warp == 1) {
+        if (lane < MAX_STAGES) {
+            mbar_init(&L.full_bar[lane], 1);
+            mbar_init(&L.empty_bar[lane], 8);  // one arrival per consumer warp
+        } else if (lane < MAX_STAGES + 2) {
+            mbar_init(&L.res_bar[lane - MAX_STAGES], 1);
+        }
+        fence_mbar_init();
+    }
+    __syncthreads();
+    // Programmatic dependent launch: the set-up above overlaps the tail of the previous kernel in the stream; global
+    // memory is only touched after this point (the producer waits after its first tile decode).
+    if (warp >= 4) asm volatile("griddepcontrol.wait;" ::: "memory");
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    if (warp < 4) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
+        if (warp == 0) {
+            PipeState st;
+            producer_role(p, &tma_a, &tma_a2, &tma_b, L, (int)blockIdx.x, (int)gridDim.x, st);
+        }
+    } else {
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
+        // (Gelu: 128 columns only -- the out-of-line act4 calls would spill around 128 live accumulators per thread)
+        if (FAST == 5 || p.bn == 128)
+            wide_consumer<FAST, 128>(p, L, &tma_d, &tma_r, (int)blockIdx.x, (int)gridDim.x);
+        else
+            wide_consumer<FAST, 256>(p, L, &tma_d, &tma_r, (int)blockIdx.x, (int)gridDim.x);
     }
 }
 
