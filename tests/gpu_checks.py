@@ -7,9 +7,43 @@ Tolerances
   f32 GEMM / Conv (wgmma tf32, single pass): |got - exact| <= 2^-9 * sum_k |a_k b_k| + 1e-6
   (both operands lose at most 2^-10 relative each to TF32 rounding; fp32 accumulation).
 """
+import contextlib
+import os
+
 import numpy as np
 
 TF32_REL = 2.0 ** -9
+
+FORCE_KEYS = ("RTEN_B200_FORCE_BN", "RTEN_B200_FORCE_SPLITK", "RTEN_B200_FORCE_STRICT")
+
+
+@contextlib.contextmanager
+def forced(bn, strict=True):
+    """Launches inside take the best-ranked plan with `bn`-column tiles and no split-K; under `strict` a launch that no
+    such plan can run fails instead of falling back to the model's choice."""
+    for k in FORCE_KEYS:
+        os.environ.pop(k, None)
+    os.environ["RTEN_B200_FORCE_BN"] = str(bn)
+    os.environ["RTEN_B200_FORCE_SPLITK"] = "1"
+    if strict:
+        os.environ["RTEN_B200_FORCE_STRICT"] = "1"
+    try:
+        yield
+    finally:
+        for k in FORCE_KEYS:
+            os.environ.pop(k, None)
+
+
+@contextlib.contextmanager
+def bound(tf32):
+    """assert_tf32_close's relative bound for single-pass TF32 (2^-9) or 3xTF32 (2^-18) inside the block."""
+    global TF32_REL
+    saved = TF32_REL
+    TF32_REL = 2.0 ** -9 if tf32 else 2.0 ** -18
+    try:
+        yield
+    finally:
+        TF32_REL = saved
 
 
 def new_ctx(rt, tf32=True):
@@ -507,14 +541,17 @@ def _check_sequence(rt, oracle):
 
 
 # ------------------------------------------------------------------------------------------
-def _conv_exact(x, w, bias, pads, groups, strides, dil):
+def _conv_exact(x, w, bias, pads, groups, strides, dil, device="cpu"):
+    """float64 convolution and the same convolution of |x|, |w| (the TF32 bound's sum of |products|), as numpy arrays;
+    `device="cuda"` computes them on the GPU (large batches)."""
     import torch
     import torch.nn.functional as F
-    xt = F.pad(torch.from_numpy(x).double(), (pads[1], pads[3], pads[0], pads[2]))
-    wt = torch.from_numpy(w).double()
-    y = F.conv2d(xt, wt, None if bias is None else torch.from_numpy(bias).double(), stride=strides, dilation=dil, groups=groups)
+    xt = F.pad(torch.from_numpy(x).to(device, torch.float64), (pads[1], pads[3], pads[0], pads[2]))
+    wt = torch.from_numpy(w).to(device, torch.float64)
+    bt = None if bias is None else torch.from_numpy(bias).to(device, torch.float64)
+    y = F.conv2d(xt, wt, bt, stride=strides, dilation=dil, groups=groups)
     ya = F.conv2d(xt.abs(), wt.abs(), None, stride=strides, dilation=dil, groups=groups)
-    return y.numpy(), ya.numpy()
+    return y.cpu().numpy(), ya.cpu().numpy()
 
 
 def _conv_case(rt, oracle, ctx, xs, ws, pads=(0, 0, 0, 0), groups=1, strides=(1, 1), dil=(1, 1), bias=True, cl=False, prepack=False,
