@@ -106,14 +106,10 @@ rten_status rten_b200_copy(rten_ctx* ctx, const rten_tensor* src, rten_tensor* d
 /* Number of CUDA kernels this context has launched so far (bench.py `gpu_launches`). */
 uint64_t rten_b200_launch_count(rten_ctx* ctx);
 const char* rten_b200_version(void);
-/* Debug aid for plan sweeps (env RTEN_B200_FORCE_BN / _PAIR / _KATOMS / _SPLITK / _CTA2): how many tensor-core launches
+/* Debug aid for plan sweeps (env RTEN_B200_FORCE_BN / _SPLITK): how many tensor-core launches
  * found a valid plan matching every forced field, and how many fell back to the cost model's choice because none did.
  * With env RTEN_B200_FORCE_STRICT=1 such a launch fails with RTEN_ERR_INVALID_VALUE instead. */
 rten_status rten_b200_debug_forced_plans(rten_ctx* ctx, uint64_t* matched, uint64_t* unmatched);
-/* Debug aid: when enabled, CTA 0 of every GEMM/conv launch records clock64() at its pipeline hand-offs into a
- * 4 x 2048 int64 buffer (rows: producer slot acquired, MMA operands landed, epilogue start, epilogue end).
- * `host_out_8192_or_null` receives the current contents before the state change. */
-rten_status rten_b200_debug_trace(rten_ctx* ctx, int enable, int64_t* host_out_8192_or_null);
 /* Capture everything enqueued between begin/end into a CUDA graph; replay with graph_launch.
  * (launch-bound op lists: the `Graph::run_plan` loop, src/graph.rs:880-1286, as one graph) */
 typedef struct rten_graph rten_graph;

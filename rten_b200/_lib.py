@@ -69,7 +69,6 @@ _SIGNATURES = {
     "rten_b200_copy": (C.c_int, [_vp, _TP, _TP]),
     "rten_b200_launch_count": (C.c_uint64, [_vp]),
     "rten_b200_debug_forced_plans": (C.c_int, [_vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
-    "rten_b200_debug_trace": (C.c_int, [_vp, C.c_int, C.POINTER(C.c_int64)]),
     "rten_b200_graph_begin": (C.c_int, [_vp]),
     "rten_b200_graph_end": (C.c_int, [_vp, C.POINTER(_vp)]),
     "rten_b200_graph_launch": (C.c_int, [_vp, _vp]),

@@ -107,7 +107,7 @@ rten_status OpScope::in(const rten_tensor* t, rten_tensor* view) {
     const size_t bytes = (size_t)span * dtype_size(t->dtype);
     void* d = nullptr;
     RTB_TRY(temp_alloc(ctx, bytes ? bytes : 16, &d));
-    if (bytes) RTB_CUDA(ctx, cudaMemcpyAsync(d, t->data, bytes, cudaMemcpyHostToDevice, rtb::launch_stream(ctx)));
+    if (bytes) RTB_CUDA(ctx, cudaMemcpyAsync(d, t->data, bytes, cudaMemcpyHostToDevice, ctx->stream));
     view->data = d;
     view->device = ctx->device;
     return RTEN_OK;
@@ -182,7 +182,7 @@ rten_status OpScope::finish(rten_status st) {
     if (st == RTEN_OK) {
         for (auto& cb : copybacks) {
             if (cb.bytes) {
-                cudaError_t e = cudaMemcpyAsync(cb.host, cb.dev, cb.bytes, cudaMemcpyDeviceToHost, rtb::launch_stream(ctx));
+                cudaError_t e = cudaMemcpyAsync(cb.host, cb.dev, cb.bytes, cudaMemcpyDeviceToHost, ctx->stream);
                 if (e != cudaSuccess) st = fail_cuda(ctx, e, "cudaMemcpyAsync(D2H)");
             }
         }
@@ -212,14 +212,15 @@ const char* rten_b200_version(void) { return "rten-b200 0.1 (sm_90a)"; }
 
 // Measured launch plans can be kept across processes: RTEN_B200_TUNE_FILE names a text file that is read when a
 // context is created and rewritten when a context that measured new plans is destroyed (one line per problem:
-// key integers, '|', plan integers).
+// key integers, '|', the three plan integers `bn splitk nbuf`).  Lines with any other number of plan integers (files
+// written by older builds) are skipped: those problems are planned afresh.
 static void tune_cache_load(rten_ctx* ctx, const char* path) {
     FILE* f = fopen(path, "r");
     if (!f) return;
     char line[2048];
     while (fgets(line, sizeof(line), f)) {
         std::vector<long long> key;
-        std::array<int, 8> plan{};
+        std::array<int, 3> plan{};
         char* p = line;
         bool in_plan = false;
         int np = 0;
@@ -235,13 +236,14 @@ static void tune_cache_load(rten_ctx* ctx, const char* path) {
             const long long v = strtoll(p, &end, 10);
             if (end == p) break;
             if (in_plan) {
-                if (np < 8) plan[np++] = (int)v;
+                if (np < 3) plan[np] = (int)v;
+                np++;
             } else {
                 key.push_back(v);
             }
             p = end;
         }
-        if (np == 8 && !key.empty()) ctx->tune_cache[key] = plan;
+        if (np == 3 && !key.empty()) ctx->tune_cache[key] = plan;
     }
     fclose(f);
 }
@@ -314,7 +316,6 @@ void rten_b200_ctx_destroy(rten_ctx* ctx) {
         if (ctx->tune_cache.size() > ctx->tune_loaded) tune_cache_save(ctx, tf);
     if (ctx->sk_counters) cudaFree(ctx->sk_counters);
     if (ctx->attn_cnt) cudaFree(ctx->attn_cnt);
-    seq_free(ctx);
     if (ctx->own_stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
 }
@@ -394,7 +395,7 @@ rten_status rten_b200_copy(rten_ctx* ctx, const rten_tensor* src, rten_tensor* d
         if (!bytes) return RTEN_OK;
         cudaMemcpyKind kind = src->device < 0 ? (dst->device < 0 ? cudaMemcpyHostToHost : cudaMemcpyHostToDevice)
                                               : (dst->device < 0 ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice);
-        RTB_CUDA(ctx, cudaMemcpyAsync(dst->data, src->data, bytes, kind, rtb::launch_stream(ctx)));
+        RTB_CUDA(ctx, cudaMemcpyAsync(dst->data, src->data, bytes, kind, ctx->stream));
         if ((src->device < 0 || dst->device < 0) && !ctx->capturing) RTB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
         return RTEN_OK;
     }
@@ -421,25 +422,6 @@ rten_status rten_b200_copy(rten_ctx* ctx, const rten_tensor* src, rten_tensor* d
     return sc.finish(st);
 }
 
-// ---- debug: in-kernel pipeline trace of CTA 0 of the GEMM kernel (clock64 at stage hand-offs)
-rten_status rten_b200_debug_trace(rten_ctx* ctx, int enable, int64_t* host_out_8192_or_null) {
-    if (!ctx) return RTEN_ERR_INVALID_VALUE;
-    cudaSetDevice(ctx->device);
-    const size_t bytes = 4 * 2048 * sizeof(int64_t);
-    if (ctx->trace && host_out_8192_or_null) {
-        RTB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        RTB_CUDA(ctx, cudaMemcpy(host_out_8192_or_null, ctx->trace, bytes, cudaMemcpyDeviceToHost));
-    }
-    if (enable) {
-        if (!ctx->trace) RTB_CUDA(ctx, cudaMalloc(&ctx->trace, bytes));
-        RTB_CUDA(ctx, cudaMemsetAsync(ctx->trace, 0, bytes, rtb::launch_stream(ctx)));
-    } else if (ctx->trace) {
-        cudaFree(ctx->trace);
-        ctx->trace = nullptr;
-    }
-    return RTEN_OK;
-}
-
 // ---- CUDA graphs --------------------------------------------------------------------------
 rten_status rten_b200_graph_begin(rten_ctx* ctx) {
     if (!ctx) return RTEN_ERR_INVALID_VALUE;
@@ -453,7 +435,6 @@ rten_status rten_b200_graph_begin(rten_ctx* ctx) {
 rten_status rten_b200_graph_end(rten_ctx* ctx, rten_graph** out) {
     if (!ctx || !out) return RTEN_ERR_INVALID_VALUE;
     if (!ctx->capturing) return fail(ctx, RTEN_ERR_INVALID_VALUE, "no graph capture active");
-    rten_status fs = seq_flush(ctx);  // tensor-core launches still collected for a sequence kernel
     ctx->capturing = false;
     rten_graph* g = new rten_graph();
     cudaError_t e = cudaStreamEndCapture(ctx->stream, &g->graph);
@@ -463,13 +444,6 @@ rten_status rten_b200_graph_end(rten_ctx* ctx, rten_graph** out) {
         delete g;
         capture_settle(ctx, nullptr);
         return fail_cuda(ctx, e, "graph capture/instantiate");
-    }
-    if (fs != RTEN_OK) {
-        cudaGraphExecDestroy(g->exec);
-        cudaGraphDestroy(g->graph);
-        delete g;
-        capture_settle(ctx, nullptr);
-        return fs;
     }
     g->ctx = ctx;
     ctx->graphs.push_back(g);

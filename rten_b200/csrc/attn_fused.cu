@@ -286,7 +286,7 @@ rten_status launch_attn_fused(rten_ctx* ctx, const AttnFusedLaunch& L) {
     cfg.gridDim = dim3(L.B * L.heads * p.q_tiles);
     cfg.blockDim = dim3(AF_THREADS);
     cfg.dynamicSmemBytes = smem;
-    cfg.stream = launch_stream(ctx);
+    cfg.stream = ctx->stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;

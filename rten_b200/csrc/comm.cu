@@ -84,7 +84,7 @@ namespace rtb {
 // min / max on that encoding is the float min / max, and is exact and order independent.
 rten_status comm_allreduce_minmax(rten_ctx* ctx, rten_comm* comm, int* mm) {
     if (!comm || comm->world <= 1) return RTEN_OK;
-    cudaStream_t s = launch_stream(ctx);
+    cudaStream_t s = ctx->stream;
     if (comm->peer_ok) {
         cudaLaunchConfig_t cfg;
         memset(&cfg, 0, sizeof(cfg));

@@ -66,14 +66,11 @@ struct rten_ctx {
     DevicePool pool;
     // scratch released at the end of each op call
     std::vector<void*> temps;
-    void* trace = nullptr;         // device buffer of 4 x 2048 int64 timestamps (debug), or null
     void* encode_tiled = nullptr;  // cuTensorMapEncodeTiled (driver entry point)
     void* sk_counters = nullptr;   // split-K arrival counters (zero between launches)
     bool autotune = false;         // time candidate launch plans on first sight of a problem (umma_gemm.cu)
-    void* seq_pending = nullptr;   // umma_gemm launches collected during graph capture (std::vector<PendingLaunch>*)
-    int seq_class = -1;            // kernel class (data kind, epilogue variant) of the pending launches
-    void* seq_gbar = nullptr;      // grid-barrier arrival counter of the sequence kernel
-    std::map<std::vector<long long>, std::array<int, 8>> tune_cache;
+    // autotuned plans: problem signature -> {bn, splitk, nbuf}, or {-1, bn, T} for the halo-reuse kernel (umma_gemm.cu)
+    std::map<std::vector<long long>, std::array<int, 3>> tune_cache;
     size_t tune_loaded = 0;        // entries read from RTEN_B200_TUNE_FILE (the file is rewritten when more exist at destroy)
     std::vector<rten_graph*> graphs;  // graphs captured on this context that still exist
     void* attn_cnt = nullptr;      // arrival counters of the split single-query attention kernel (zero between launches)
@@ -148,14 +145,5 @@ inline void count_launch(rten_ctx* ctx, int n = 1) { ctx->launches += (uint64_t)
 rten_status comm_allreduce_minmax(rten_ctx* ctx, struct ::rten_comm* comm, int* mm);
 struct RangeExchange;
 bool comm_range_exchange(struct ::rten_comm* comm, RangeExchange* out);  // true: the quantise kernel exchanges the range itself
-
-// Deferred tensor-core launches (graph capture batches them into sequence kernels, umma_gemm.cu) must be issued
-// before anything else is enqueued on the context stream: every other launch site asks for the stream through this.
-rten_status seq_flush(rten_ctx* ctx);
-void seq_free(rten_ctx* ctx);
-inline cudaStream_t launch_stream(rten_ctx* ctx) {
-    if (ctx->seq_pending) seq_flush(ctx);
-    return ctx->stream;
-}
 
 }  // namespace rtb

@@ -282,12 +282,6 @@ __device__ __forceinline__ void acc_store_frag(uint32_t acc_smem, const T (&d)[N
     }
 }
 
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-
 // ------------------------------------------------------------------ descriptors
 // Shared-memory matrix descriptor for a K-major operand tile stored as rows of 128 bytes with the
 // 128B swizzle (what a TMA box {128 B, rows} with CU_TENSOR_MAP_SWIZZLE_128B writes):
@@ -302,15 +296,6 @@ __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
     d |= static_cast<uint64_t>(1024 >> 4) << 32;
     d |= static_cast<uint64_t>(1) << 62;
     return d;
-}
-
-// Instruction descriptor (upper 32 bits of the idesc operand):
-//   [4,6) D format (1 = F32, 2 = S32)   [7,10) A format   [10,13) B format
-//   (kind::tf32: 2 = TF32; kind::i8: 0 = unsigned 8 bit, 1 = signed 8 bit)
-//   [15] A major (0 = K)  [16] B major (0 = K)  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ __forceinline__ uint32_t make_idesc(uint32_t d_fmt, uint32_t a_fmt, uint32_t b_fmt, uint32_t m,
-                                                        uint32_t n) {
-    return (d_fmt << 4) | (a_fmt << 7) | (b_fmt << 10) | ((n >> 3) << 17) | ((m >> 4) << 24);
 }
 
 }  // namespace rtb

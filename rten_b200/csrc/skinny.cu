@@ -406,7 +406,7 @@ rten_status launch_qlinear(rten_ctx* ctx, const QLinearLaunch& L) {
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(256);
     cfg.dynamicSmemBytes = smem;
-    cfg.stream = launch_stream(ctx);
+    cfg.stream = ctx->stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
@@ -548,7 +548,7 @@ rten_status launch_skinny_f32(rten_ctx* ctx, const SkinnyF32Launch& L) {
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(256);
     cfg.dynamicSmemBytes = smem;
-    cfg.stream = launch_stream(ctx);
+    cfg.stream = ctx->stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
@@ -867,7 +867,7 @@ rten_status launch_attn_decode(rten_ctx* ctx, const AttnDecodeLaunch& L) {
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(bh * ns);
     cfg.blockDim = dim3(nw * 32);
-    cfg.stream = launch_stream(ctx);
+    cfg.stream = ctx->stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;

@@ -26,7 +26,7 @@
 //                    through 128-row staging buffers and TMA stores; not overlapped with the next main loop.
 // A wide tile reads each A tile from shared memory once for up to 256 columns and amortises the fixed cost of a
 // pipeline stage over 2-4x the tensor work; the plans of both kernels compete in the cost model and the autotuner.
-// Work decomposition (tile width, split-K, K blocks per stage) is a launch `Plan` (see "Launch plans" below), ranked by
+// Work decomposition (tile width, split-K, staging buffers) is a launch `Plan` (see "Launch plans" below), ranked by
 // a cost model and, optionally, measured on the device per problem.
 // For Conv the A tile is a TMA box over the NHWC activation tensor at (c0, ox0*sx - pad + kx*dx,
 // oy0*sy - pad + ky*dy, b0): padding comes from TMA out-of-bounds zero fill, the stride from the
@@ -37,7 +37,6 @@
 #include <algorithm>
 #include <array>
 #include <cmath>
-#include <memory>
 #include <vector>
 #include <cmath>
 #include <cstdint>
@@ -140,7 +139,7 @@ static void pick_conv_tile(const ConvGeom& g, int& tw, int& th, int& tb) {
 // (b) the per-context autotune cache: with rten_b200_set_autotune(ctx, 1) the first launch of every distinct problem
 // times the model's best candidates on the device (CUDA events on the context stream) and remembers the winner.
 struct Plan {
-    int bn = 32, pair = 0, katoms = 1, ksplit = 0, splitk = 1, nbuf = 1, acc1 = 0, cta2 = 0;
+    int bn = 32, splitk = 1, nbuf = 1;
 };
 
 // Everything about a launch that does not depend on the plan.
@@ -159,7 +158,7 @@ struct Prepared {
 
 constexpr int SK_CNT_INTS = 1 << 16;
 // 227 KB of shared memory per block; SMEM_FIXED_BYTES: alignment slack, barriers, column vectors, accumulators
-static int smem_budget_for(int n_stg, int /*kind*/) { return 227 * 1024 - SMEM_FIXED_BYTES - n_stg * STG_BYTES; }
+static int smem_budget_for(int n_stg) { return 227 * 1024 - SMEM_FIXED_BYTES - n_stg * STG_BYTES; }
 // operand stages of the wide-tile kernel: 6 at bn = 128, 4 at bn = 256
 static int wide_stages(int stage_bytes) { return std::min(MAX_STAGES, (227 * 1024 - WIDE_SMEM_FIXED_BYTES) / stage_bytes); }
 static bool is_wide(int bn) { return bn > ACC_STRIDE; }
@@ -169,20 +168,20 @@ static bool is_wide(int bn) { return bn > ACC_STRIDE; }
 // ApproxGelu}, no range output.
 static bool plain_f32_ok(const rten_ctx* ctx, const GemmLaunch& L, int tma_store, int res_tma) {
     const EpilogueDesc& e = L.epi;
-    return L.kind == 0 && tma_store && (L.N % 32) == 0 && (!ctx->trace || getenv("RTEN_B200_TRACE_FAST")) &&
-           !getenv("RTEN_B200_NO_FAST") && !getenv("RTEN_B200_NO_PLAIN") && e.bias_kind != 2 &&
+    return L.kind == 0 && tma_store && (L.N % 32) == 0 && !getenv("RTEN_B200_NO_FAST") && !getenv("RTEN_B200_NO_PLAIN") &&
+           e.bias_kind != 2 &&
            (e.bias_kind != 1 || (reinterpret_cast<uintptr_t>(e.bias) & 15) == 0) && e.alpha == 1.0f && e.act <= 3 &&
            !e.range && (e.r == nullptr || (res_tma && e.r_scale == 1.0f));
 }
 
 struct PlanShape {
     long long tiles_n, units_m, tiles, units;
-    int kb_per, atom_bytes, stage_bytes, stages, n_stg;
+    int kb_per, stage_bytes, stages, n_stg;
 };
 
 // Derived sizes of a plan; false if the plan cannot run (accumulator columns, shared memory, counters).  The kernels
 // compute one 128 x bn tile per unit: bn in {32, 64} (umma_gemm_kernel), or bn in {128, 256} without split-K for the
-// launches that take the plain f32 epilogue (umma_wide_kernel).  pair / ksplit / acc1 / cta2 are not available on sm_90.
+// launches that take the plain f32 epilogue (umma_wide_kernel).  One 128-byte K block per pipeline stage.
 static bool plan_shape(const Prepared& q, const Plan& pl, PlanShape& ps) {
     const KParams& p = q.p;
     if (is_wide(pl.bn)) {
@@ -191,7 +190,8 @@ static bool plan_shape(const Prepared& q, const Plan& pl, PlanShape& ps) {
     } else if (pl.bn < 16 || pl.bn % 32 || pl.bn % q.step) {
         return false;
     }
-    if (pl.pair || pl.ksplit || pl.acc1 || pl.cta2 || pl.katoms != 1) return false;  // one K block per stage: straight-line wgmma issue
+    if (pl.nbuf < (q.res_tma ? 2 : 1) || pl.nbuf > 4) return false;  // staging buffers per group: res_bar has 4; a
+                                                                     // TMA-staged residual needs two
     ps.tiles_n = (p.N + pl.bn - 1) / pl.bn;
     ps.units_m = p.tiles_m;
     ps.tiles = ps.units_m * ps.tiles_n * q.batch;
@@ -203,10 +203,8 @@ static bool plan_shape(const Prepared& q, const Plan& pl, PlanShape& ps) {
         if (ps.tiles * 2 > SK_CNT_INTS) return false;
     }
     ps.n_stg = 2 * pl.nbuf;
-    ps.atom_bytes = A_STAGE_BYTES + pl.bn * KBYTES;
-    ps.stage_bytes = ps.atom_bytes;
-    ps.stages = is_wide(pl.bn) ? wide_stages(ps.stage_bytes)
-                               : std::min(MAX_STAGES, smem_budget_for(ps.n_stg, q.esize == 4 ? 0 : 1) / ps.stage_bytes);
+    ps.stage_bytes = A_STAGE_BYTES + pl.bn * KBYTES;
+    ps.stages = is_wide(pl.bn) ? wide_stages(ps.stage_bytes) : std::min(MAX_STAGES, smem_budget_for(ps.n_stg) / ps.stage_bytes);
     if (ps.stages < 2) return false;
     return true;
 }
@@ -224,7 +222,7 @@ static double plan_cost(const Prepared& q, const Plan& pl, const PlanShape& ps, 
     const double waves = std::ceil((double)ps.units / num_sms);
     const double bw = std::min(64.0, 7400.0 / active);
     const double mmas = 4.0;
-    const double t_kb = std::max(mmas * std::max(42.0, (double)pl.bn), ps.atom_bytes / bw);
+    const double t_kb = std::max(mmas * std::max(42.0, (double)pl.bn), ps.stage_bytes / bw);
     double t_stage = std::max(t_kb, 320.0 + mmas * 42.0);
     t_stage = std::max(t_stage, 2300.0 / ps.stages);
     const double mainloop = ps.kb_per * t_stage;
@@ -289,7 +287,6 @@ static rten_status prepare_launch(rten_ctx* ctx, const GemmLaunch& L, Prepared& 
     p.kelems = kelems;
     p.conv = L.conv;
     p.epi = L.epi;
-    p.trace = reinterpret_cast<long long*>(ctx->trace);
     p.c_blocks = 1;
     p.kw = 1;
     for (int i = 0; i < 4; i++) q.aes[i] = 1;
@@ -393,7 +390,7 @@ static rten_status prepare_launch(rten_ctx* ctx, const GemmLaunch& L, Prepared& 
 }
 
 static size_t splitk_ws_bytes(const PlanShape& ps, const Plan& pl) {
-    return pl.splitk > 1 ? (size_t)ps.tiles * (pl.cta2 + 1) * 2 * pl.splitk * (pl.bn / 32) * 4096 * 4 : 0;
+    return pl.splitk > 1 ? (size_t)ps.tiles * pl.splitk * (pl.bn / 32) * 4096 * 4 : 0;
 }
 
 static rten_status ensure_splitk_counters(rten_ctx* ctx) {
@@ -406,163 +403,23 @@ static rten_status ensure_splitk_counters(rten_ctx* ctx) {
     return RTEN_OK;
 }
 
-struct PendingLaunch {
-    bool plain = false;  // f32 launch that qualifies for the plain epilogue (kernel variant 3; a subset of variant 1)
-    KParams p;
-    CUtensorMap maps[5];  // a, b, d, residual, a2 (two-plane 3xTF32: low parts of A)
-    size_t smem_bytes;
-};
-
-static std::vector<PendingLaunch>* pending_of(rten_ctx* ctx) {
-    if (!ctx->seq_pending) ctx->seq_pending = new std::vector<PendingLaunch>();
-    return reinterpret_cast<std::vector<PendingLaunch>*>(ctx->seq_pending);
-}
-
-void seq_free(rten_ctx* ctx) {
-    if (ctx->seq_pending) delete reinterpret_cast<std::vector<PendingLaunch>*>(ctx->seq_pending);
-    ctx->seq_pending = nullptr;
-    if (ctx->seq_gbar) cudaFree(ctx->seq_gbar);
-    ctx->seq_gbar = nullptr;
-}
-
-static void fill_launch_attrs(cudaLaunchConfig_t& cfg, cudaLaunchAttribute* attr, bool cluster2) {
-    int nattr = 0;
-    if (!getenv("RTEN_B200_NO_PDL")) {
-        attr[nattr].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[nattr].val.programmaticStreamSerializationAllowed = 1;
-        nattr++;
-    }
-    if (cluster2) {
-        attr[nattr].id = cudaLaunchAttributeClusterDimension;
-        attr[nattr].val.clusterDim.x = 2;
-        attr[nattr].val.clusterDim.y = 1;
-        attr[nattr].val.clusterDim.z = 1;
-        nattr++;
-    }
-    cfg.attrs = attr;
-    cfg.numAttrs = nattr;
-}
-
-// cls = kind * 3 + epilogue variant
-static rten_status launch_single(rten_ctx* ctx, int cls, const PendingLaunch& pl) {
-    const KParams& p = pl.p;
-    const int grid = std::min(p.units_total, ctx->num_sms);
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(is_wide(p.bn) ? WIDE_THREADS : NUM_THREADS);
-    cfg.dynamicSmemBytes = pl.smem_bytes;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[2];
-    fill_launch_attrs(cfg, attr, false);
-    auto launch = [&](auto kern) -> cudaError_t {
-        cudaError_t e2 = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e2 != cudaSuccess) return e2;
-        return cudaLaunchKernelEx(&cfg, kern, pl.maps[0], pl.maps[1], pl.maps[2], pl.maps[3], pl.maps[4], p);
-    };
-    cudaError_t e;
-    if (is_wide(p.bn)) {  // (plain f32 epilogue only: launch_plan)
-        e = launch(cls == 2 ? umma_wide_kernel<5> : umma_wide_kernel<3>);
-    } else if (pl.plain && cls == 1) {
-        e = launch(umma_gemm_kernel<0, 3>);
-    } else if (pl.plain && cls == 2) {
-        e = launch(umma_gemm_kernel<0, 5>);
-    } else if (pl.plain && cls == 5) {
-        e = launch(umma_gemm_kernel<1, 6>);
-    } else if (pl.plain && cls == 4) {
-        e = launch(umma_gemm_kernel<1, 4>);
-    } else
-    switch (cls) {
-        case 0: e = launch(umma_gemm_kernel<0, 0>); break;
-        case 1: e = launch(umma_gemm_kernel<0, 1>); break;
-        case 2: e = launch(umma_gemm_kernel<0, 2>); break;
-        case 3: e = launch(umma_gemm_kernel<1, 0>); break;
-        case 4: e = launch(umma_gemm_kernel<1, 1>); break;
-        default: e = launch(umma_gemm_kernel<1, 2>); break;
-    }
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "umma_gemm launch");
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "umma_gemm launch");
-    count_launch(ctx);
-    return RTEN_OK;
-}
-
-// Launch whatever umma_gemm launches are pending on this context (one: the plain kernel; several: the sequence kernel).
-rten_status seq_flush(rten_ctx* ctx) {
-    if (!ctx->seq_pending) return RTEN_OK;
-    auto* q = reinterpret_cast<std::vector<PendingLaunch>*>(ctx->seq_pending);
-    if (q->empty()) return RTEN_OK;
-    std::vector<PendingLaunch> items;
-    items.swap(*q);  // (re-entrancy: launch paths below call seq_flush through launch_stream)
-    const int cls = ctx->seq_class;
-    if (items.size() == 1) return launch_single(ctx, cls, items[0]);
-    if (!ctx->seq_gbar) {
-        cudaError_t ce = cudaMalloc(&ctx->seq_gbar, 256);
-        if (ce != cudaSuccess) return fail_cuda(ctx, ce, "sequence barrier");
-        ce = cudaMemset(ctx->seq_gbar, 0, 256);
-        if (ce != cudaSuccess) return fail_cuda(ctx, ce, "sequence barrier");
-    }
-    std::unique_ptr<SeqParams> sp(new SeqParams());
-    memset(sp.get(), 0, sizeof(SeqParams));
-    sp->n = (int)items.size();
-    sp->gbar = reinterpret_cast<unsigned*>(ctx->seq_gbar);
-    int grid = 1;
-    for (size_t i = 0; i < items.size(); i++) {
-        sp->layer[i] = items[i].p;
-        for (int m = 0; m < 4; m++) sp->maps[i][m] = items[i].maps[m];
-        grid = std::max(grid, std::min(items[i].p.units_total, ctx->num_sms));
-    }
-    if (getenv("RTEN_B200_VERBOSE")) fprintf(stderr, "[umma_seq] %d layers in one kernel, grid %d, class %d\n", sp->n, grid, cls);
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(NUM_THREADS);
-    cfg.dynamicSmemBytes = 227 * 1024;  // one CTA per SM by construction: every CTA of the grid is resident (grid barrier)
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[2];
-    fill_launch_attrs(cfg, attr, false);
-    auto launch = [&](auto kern) -> cudaError_t {
-        cudaError_t e2 = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e2 != cudaSuccess) return e2;
-        return cudaLaunchKernelEx(&cfg, kern, *sp);
-    };
-    cudaError_t e;
-    switch (cls) {
-        case 0: e = launch(umma_seq_kernel<0, 0>); break;
-        case 1: e = launch(umma_seq_kernel<0, 1>); break;
-        case 3: e = launch(umma_seq_kernel<1, 0>); break;
-        default: e = launch(umma_seq_kernel<1, 1>); break;
-    }
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "umma_seq launch");
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "umma_seq launch");
-    count_launch(ctx);
-    return RTEN_OK;
-}
-
 // `ws`: split-K workspace of at least splitk_ws_bytes() (null: taken from the op's temporaries)
 static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepared& q, const Plan& pl, bool verbose,
-                               void* ws = nullptr, bool no_defer = false) {
+                               void* ws = nullptr) {
     PlanShape ps;
     if (!plan_shape(q, pl, ps)) return RTEN_ERR_UNSUPPORTED_VALUE;
     KParams p = q.p;
     p.bn = pl.bn;
-    p.pair = pl.pair;
-    p.katoms = pl.katoms;
-    p.ksplit = pl.ksplit;
     p.splitk = pl.splitk;
-    p.acc1 = pl.acc1;
-    p.cta2 = pl.cta2;
     p.nbuf = pl.nbuf;
     p.tma_store = q.tma_store;
     p.res_tma = q.res_tma ? 1 : 0;
-    if (p.res_tma && p.nbuf < 2) p.nbuf = 2;
     p.kb_per = ps.kb_per;
     p.tiles_n = (int)ps.tiles_n;
     p.tiles_total = (int)ps.tiles;
     p.units_total = (int)ps.units;
     p.d_tiles_n.set(p.tiles_n);
-    p.d_units_m.set((int)ps.units_m);
+    p.d_tiles_m.set(p.tiles_m);
     p.d_z0.set(p.z0);
     p.d_tiles_x.set(p.conv ? p.tiles_x : 1);
     p.d_tiles_y.set(p.conv ? p.tiles_y : 1);
@@ -571,16 +428,10 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
     p.d_kw.set(p.kw);
     p.d_tw.set(p.conv ? p.tw : 1);
     p.d_th.set(p.conv ? p.th : 1);
-    const int n_stg = 2 * p.nbuf;
-    p.atom_bytes = ps.atom_bytes;
     p.stage_bytes = ps.stage_bytes;
-    p.tx_bytes = (p.pair ? 2 : 1) * q.a_rows * KBYTES + (p.bn >> p.cta2) * KBYTES;  // per 128-byte K block and CTA
-    p.stages = is_wide(p.bn) ? ps.stages : std::min(MAX_STAGES, smem_budget_for(n_stg, L.kind) / (int)p.stage_bytes);
-    if (p.stages < 2) return RTEN_ERR_UNSUPPORTED_VALUE;
-    if (L.kind == 0)
-        p.idesc = make_idesc(1 /*F32*/, 2 /*TF32*/, 2, BM, p.bn);
-    else
-        p.idesc = make_idesc(2 /*S32*/, L.a_signed ? 1 : 0, L.b_signed ? 1 : 0, BM, p.bn);
+    p.tx_bytes = q.a_rows * KBYTES + p.bn * KBYTES;  // per 128-byte K block
+    p.stages = ps.stages;
+    p.sgn = L.kind == 0 ? 0 : (L.a_signed ? 1 : 0) | (L.b_signed ? 2 : 0);
     if (p.splitk > 1) {
         RTB_TRY(ensure_splitk_counters(ctx));
         if (!ws) RTB_TRY(temp_alloc(ctx, splitk_ws_bytes(ps, pl), &ws));
@@ -588,7 +439,7 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
         p.sk_cnt = reinterpret_cast<int*>(ctx->sk_counters);
     }
 
-    uint32_t bbox[4] = {(uint32_t)q.kelems, (uint32_t)(p.bn >> p.cta2), 1, 1}, bes[4] = {1, 1, 1, 1}, des[4] = {1, 1, 1, 1};
+    uint32_t bbox[4] = {(uint32_t)q.kelems, (uint32_t)p.bn, 1, 1}, bes[4] = {1, 1, 1, 1}, des[4] = {1, 1, 1, 1};
     CUtensorMap map_a, map_b;
     if (!encode_map(ctx, &map_a, L.a, q.esize, L.kind == 0, q.abox, q.aes)) return RTEN_ERR_UNSUPPORTED_VALUE;
     if (!encode_map(ctx, &map_b, L.b, q.esize, L.kind == 0, bbox, bes)) return RTEN_ERR_UNSUPPORTED_VALUE;
@@ -606,14 +457,14 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
     }
 
     if (verbose)
-        fprintf(stderr, "[umma_gemm] kind=%d conv=%d M=%d N=%d K=%d kb=%d tiles_m=%d bn=%d pair=%d ksplit=%d katoms=%d splitk=%d acc1=%d cta2=%d units=%d stages=%d tma_store=%d res_tma=%d nbuf=%d box=%dx%dx%d\n",
-                L.kind, L.conv, L.M, L.N, L.K, p.k_blocks, p.tiles_m, p.bn, p.pair, p.ksplit, p.katoms, p.splitk, p.acc1, p.cta2,
-                p.units_total, p.stages, p.tma_store, p.res_tma, p.nbuf, p.tw, p.th, p.tb);
+        fprintf(stderr, "[umma_gemm] kind=%d conv=%d M=%d N=%d K=%d kb=%d tiles_m=%d bn=%d splitk=%d units=%d stages=%d tma_store=%d res_tma=%d nbuf=%d box=%dx%dx%d\n",
+                L.kind, L.conv, L.M, L.N, L.K, p.k_blocks, p.tiles_m, p.bn, p.splitk, p.units_total, p.stages, p.tma_store,
+                p.res_tma, p.nbuf, p.tw, p.th, p.tb);
     const size_t smem_bytes = (size_t)p.stages * p.stage_bytes +
-                              (is_wide(p.bn) ? WIDE_SMEM_FIXED_BYTES : n_stg * STG_BYTES + SMEM_FIXED_BYTES);
+                              (is_wide(p.bn) ? WIDE_SMEM_FIXED_BYTES : ps.n_stg * STG_BYTES + SMEM_FIXED_BYTES);
     // specialised epilogue when every chunk qualifies for the register fast path
     const EpilogueDesc& ee = L.epi;
-    bool fastk = p.tma_store && (L.N % 32) == 0 && (!ctx->trace || getenv("RTEN_B200_TRACE_FAST")) && !getenv("RTEN_B200_NO_FAST");
+    bool fastk = p.tma_store && (L.N % 32) == 0 && !getenv("RTEN_B200_NO_FAST");
     if (L.kind == 0)
         fastk = fastk && ee.bias_kind != 2 && (ee.r == nullptr || p.res_tma) &&
                 (ee.bias_kind != 1 || (reinterpret_cast<uintptr_t>(ee.bias) & 15) == 0);
@@ -625,38 +476,54 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
                 (!ee.scale || ee.scale_len == 1 || (ee.scale_len == L.N && (reinterpret_cast<uintptr_t>(ee.scale) & 15) == 0));
     // the generic epilogue takes a TMA-staged residual only on its register path (f32, act <= Relu)
     if (!fastk && (L.kind == 1 || ee.act > 1)) p.res_tma = 0;
-    PendingLaunch pend;
+    bool plain;
     if (L.kind == 0)
-        pend.plain = fastk && plain_f32_ok(ctx, L, p.tma_store, p.res_tma);
+        plain = fastk && plain_f32_ok(ctx, L, p.tma_store, p.res_tma);
     else  // integer kind: the *ToFloat operators with a scalar (or no) activation zero point and symmetric weights
-        pend.plain = fastk && ee.scale && !ee.za && !ee.zb && (ee.scale_len == 1 || ee.scale_len == L.N) && ee.act <= 3 && p.splitk == 1 &&
-                     (ee.r == nullptr || p.res_tma) && (!ee.za8 || ee.colsum);
-    if (getenv("RTEN_B200_NO_PLAIN")) pend.plain = false;
-    if (is_wide(p.bn) && !pend.plain) return RTEN_ERR_UNSUPPORTED_VALUE;  // (an output / residual map failed to encode)
-    pend.p = p;
-    pend.maps[0] = map_a;
-    pend.maps[1] = map_b;
-    pend.maps[2] = map_d;
-    pend.maps[3] = map_r;
-    pend.maps[4] = map_a2;
-    pend.smem_bytes = smem_bytes;
-    // kernel class = data kind x epilogue variant (0 generic, 1 specialised, 2 specialised + out-of-line Gelu)
-    const int cls = L.kind * 3 + (fastk ? (ee.act > 1 ? 2 : 1) : 0);
-    // Opt-in (RTEN_B200_SEQ=1): inside graph capture consecutive launches are collected and run as ONE sequence kernel
-    // (umma_seq_kernel).  A layer boundary inside the sequence kernel (drain + grid barrier + cold operand pipe) is not
-    // cheaper than what programmatic dependent launch already overlaps, so separate launches stay the default.
-    const char* seq_env = getenv("RTEN_B200_SEQ");
-    const bool seq_on = seq_env && atoi(seq_env) != 0;
-    if (seq_on && ctx->capturing && !p.cta2 && !p.x3_cb && !ctx->trace && !no_defer && cls % 3 != 2 && !is_wide(p.bn)) {
-        auto* q2 = pending_of(ctx);
-        if (!q2->empty() && ctx->seq_class != cls) RTB_TRY(seq_flush(ctx));
-        ctx->seq_class = cls;
-        q2->push_back(pend);
-        if ((int)q2->size() == SEQ_MAX) RTB_TRY(seq_flush(ctx));
-        return RTEN_OK;
+        plain = fastk && ee.scale && !ee.za && !ee.zb && (ee.scale_len == 1 || ee.scale_len == L.N) && ee.act <= 3 && p.splitk == 1 &&
+                (ee.r == nullptr || p.res_tma) && (!ee.za8 || ee.colsum) && !getenv("RTEN_B200_NO_PLAIN");
+    // epilogue variant (umma_gemm_kernel): 0 generic, 1 specialised, 2 specialised + out-of-line Gelu; plain: 3 / 5 (f32),
+    // 4 / 6 (integer)
+    const bool gelu = ee.act > 1;
+    const int fast = !fastk ? 0 : !plain ? (gelu ? 2 : 1) : L.kind == 0 ? (gelu ? 5 : 3) : (gelu ? 6 : 4);
+    using Kernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, KParams);
+    Kernel kern;
+    if (is_wide(p.bn)) {
+        if (fast != 3 && fast != 5) return RTEN_ERR_UNSUPPORTED_VALUE;  // (an output / residual map failed to encode)
+        kern = fast == 5 ? umma_wide_kernel<5> : umma_wide_kernel<3>;
+    } else {
+        switch (L.kind * 8 + fast) {
+            case 0: kern = umma_gemm_kernel<0, 0>; break;
+            case 1: kern = umma_gemm_kernel<0, 1>; break;
+            case 2: kern = umma_gemm_kernel<0, 2>; break;
+            case 3: kern = umma_gemm_kernel<0, 3>; break;
+            case 5: kern = umma_gemm_kernel<0, 5>; break;
+            case 8: kern = umma_gemm_kernel<1, 0>; break;
+            case 9: kern = umma_gemm_kernel<1, 1>; break;
+            case 10: kern = umma_gemm_kernel<1, 2>; break;
+            case 12: kern = umma_gemm_kernel<1, 4>; break;
+            default: kern = umma_gemm_kernel<1, 6>; break;
+        }
     }
-    RTB_TRY(seq_flush(ctx));
-    return launch_single(ctx, cls, pend);
+
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3(std::min(p.units_total, ctx->num_sms));
+    cfg.blockDim = dim3(is_wide(p.bn) ? WIDE_THREADS : NUM_THREADS);
+    cfg.dynamicSmemBytes = smem_bytes;
+    cfg.stream = ctx->stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = getenv("RTEN_B200_NO_PDL") ? 0 : 1;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e == cudaSuccess) e = cudaLaunchKernelEx(&cfg, kern, map_a, map_b, map_d, map_r, map_a2, p);
+    if (e != cudaSuccess) return fail_cuda(ctx, e, "umma_gemm launch");
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return fail_cuda(ctx, e, "umma_gemm launch");
+    count_launch(ctx);
+    return RTEN_OK;
 }
 
 // Problem signature for the autotune cache: everything that changes which plan is fastest.
@@ -672,16 +539,11 @@ static std::vector<long long> tune_key(const GemmLaunch& L, const Prepared& q) {
     return k;
 }
 
-static Plan plan_from_array(const std::array<int, 8>& a) {
+static Plan plan_from_array(const std::array<int, 3>& a) {
     Plan pl;
     pl.bn = a[0];
-    pl.pair = a[1];
-    pl.katoms = a[2];
-    pl.ksplit = a[3];
-    pl.splitk = a[4];
-    pl.nbuf = a[5];
-    pl.acc1 = a[6];
-    pl.cta2 = a[7];
+    pl.splitk = a[1];
+    pl.nbuf = a[2];
     return pl;
 }
 
@@ -775,7 +637,7 @@ rten_status launch_umma_gemm(rten_ctx* ctx, const GemmLaunch& L) {
     if (L.kind == 0 && ctx->f32_mode == RTEN_F32_TF32X3) return launch_tf32x3(ctx, L);
     // stride-1 windows (the 3x3 layers): the halo-reuse kernel moves the activations into shared memory once per channel
     // block instead of once per filter tap (umma_halo.cu); everything it does not cover falls through
-    if (L.conv && L.kind == 0 && L.g.kh * L.g.kw > 1 && (!ctx->trace || getenv("RTEN_B200_TRACE_FAST")) && !L.x3_cb) {
+    if (L.conv && L.kind == 0 && L.g.kh * L.g.kw > 1 && !L.x3_cb) {
         const rten_status hs = launch_umma_halo_conv(ctx, L);
         if (hs != RTEN_ERR_UNSUPPORTED_VALUE) return hs;
     }
@@ -840,7 +702,7 @@ rten_status launch_umma_gemm(rten_ctx* ctx, const GemmLaunch& L) {
             cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
             cudaStreamIsCapturing(ctx->stream, &cs);
             // re-running the launch must be idempotent: the output may not alias the residual
-            const bool safe = !ctx->capturing && cs == cudaStreamCaptureStatusNone && !ctx->trace &&
+            const bool safe = !ctx->capturing && cs == cudaStreamCaptureStatusNone &&
                               (L.epi.r == nullptr || (const void*)L.epi.r != (const void*)L.epi.d);
             if (safe) {
                 cudaEvent_t e0, e1;
@@ -879,8 +741,8 @@ rten_status launch_umma_gemm(rten_ctx* ctx, const GemmLaunch& L) {
                     if (ms < 0) continue;
                     timed.emplace_back(ms, i);
                     if (verbose)
-                        fprintf(stderr, "[autotune] bn=%d pair=%d katoms=%d splitk=%d cta2=%d model=%.0f -> %.2f us\n", x.bn, x.pair,
-                                x.katoms, x.splitk, x.cta2, cands[i].first, ms * 1e3);
+                        fprintf(stderr, "[autotune] bn=%d splitk=%d nbuf=%d model=%.0f -> %.2f us\n", x.bn, x.splitk, x.nbuf,
+                                cands[i].first, ms * 1e3);
                     if (ms < best_ms) {
                         best_ms = ms;
                         plan = x;
@@ -930,10 +792,10 @@ rten_status launch_umma_gemm(rten_ctx* ctx, const GemmLaunch& L) {
                 cudaEventDestroy(e0);
                 cudaEventDestroy(e1);
                 if (halo_bn) {
-                    ctx->tune_cache[key] = {-1, halo_bn, halo_T, 0, 0, 0, 0, 0};
+                    ctx->tune_cache[key] = {-1, halo_bn, halo_T};
                     return launch_umma_halo_conv(ctx, L, halo_bn, halo_T);
                 }
-                ctx->tune_cache[key] = {plan.bn, plan.pair, plan.katoms, plan.ksplit, plan.splitk, plan.nbuf, plan.acc1, plan.cta2};
+                ctx->tune_cache[key] = {plan.bn, plan.splitk, plan.nbuf};
             }
         }
     }

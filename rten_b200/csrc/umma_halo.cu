@@ -52,7 +52,6 @@ struct HaloParams {
     int b_stages;       // weight ring depth
     int tps;            // filter taps per weight-ring stage (1)
     uint32_t patch_bytes, patch_tx, b_bytes;
-    long long* trace;  // debug (rten_b200_debug_trace + RTEN_B200_TRACE_FAST): clock64 stamps of CTA 0, layout of the GEMM kernel's
     uint32_t tap_off[32];  // (ky P + kx) * 128: byte offset of filter tap ky * kw + kx inside the patch
     uint32_t m_img, m_P;  // floor(2^32 / d) + 1 for d = nr * P and d = P: n / d == __umulhi(n, m) for the slot numbers of a unit
     EpilogueDesc epi;
@@ -138,8 +137,6 @@ umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
     uint8_t* bring = patch0 + 2 * (size_t)p.patch_bytes;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-    const bool tr0 = p.trace && blockIdx.x == 0;
-    if (tr0 && threadIdx.x == 0) p.trace[6144 + 1100] = clock64();
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tma_a);
         tma_prefetch_desc(&tma_b);
@@ -158,15 +155,13 @@ umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
         fence_mbar_init();
     }
     __syncthreads();
-    if (tr0 && threadIdx.x == 0) p.trace[6144 + 1101] = clock64();
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    if (tr0 && threadIdx.x == 0) p.trace[6144 + 1102] = clock64();
 
     if (warp == HALO_PRODUCER) {
         // ===================== TMA producer =====================
         uint32_t pphase = 0, bphase = 0;  // bit s = uses of stage s so far, mod 2
-        int ps = 0, bs = 0, tr_p = 0;
+        int ps = 0, bs = 0;
         for (int u = blockIdx.x; u < p.units_total; u += gridDim.x) {
             int n0, oy0, b0;
             halo_unit(p, u, n0, oy0, b0);
@@ -182,7 +177,6 @@ umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
                 for (int tap = 0; tap < p.taps; tap += p.tps) {
                     mbar_wait(&b_empty[bs], ((bphase >> bs) & 1) ^ 1);
                     if (elect_one()) {
-                        if (tr0 && tr_p < 2048) p.trace[tr_p++] = clock64();
                         mbar_expect_tx(&b_full[bs], p.b_bytes);
                         tma_load_4d(bring + (size_t)bs * p.b_bytes, &tma_b, &b_full[bs], cb * 32, n0, tap, 0);  // box: tps taps
                     }
@@ -228,7 +222,6 @@ umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
                 if (c < p.bn && n0 + c < p.N) bv = __ldg(e.bias + n0 + c);
             }
             mbar_wait(&acc_full[acc], (aphase >> acc) & 1);
-            if (tr0 && warp == 4 && lane == 0 && it < 1024) p.trace[4096 + it] = clock64();
             aphase ^= 1u << acc;
             bias_g[r] = bv;  // (readers of the previous unit's values are past that unit's last barrier)
             for (int t = 0; t < p.T; t++) {
@@ -281,10 +274,8 @@ umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(&acc_empty[acc]);
-            if (tr0 && warp == 4 && lane == 0 && it < 1024) p.trace[6144 + it] = clock64();
         }
     }
-    if (tr0 && threadIdx.x == 0) p.trace[6144 + 1104] = clock64();
 }
 
 }  // namespace
@@ -323,7 +314,6 @@ rten_status launch_umma_halo_conv(rten_ctx* ctx, const GemmLaunch& L, int force_
     p.c_blocks = g.C / 32;
     p.taps = g.kh * g.kw;
     p.epi = e;
-    p.trace = reinterpret_cast<long long*>(ctx->trace);
     if (p.P > 256) return RTEN_ERR_UNSUPPORTED_VALUE;
     // ---- unit shape.  Candidates: output-channel tile bn, MMA tiles T per unit, whole images (tb >= 1 images of
     // OH + kh - 1 patch rows) or row strips (R rows of one image).  Ranked by waves x (MMA clocks of a unit), with the
@@ -426,7 +416,7 @@ rten_status launch_umma_halo_conv(rten_ctx* ctx, const GemmLaunch& L, int force_
     cfg.gridDim = dim3(std::min(p.units_total, num_sms));
     cfg.blockDim = dim3(HALO_THREADS);
     cfg.dynamicSmemBytes = smem;
-    cfg.stream = launch_stream(ctx);
+    cfg.stream = ctx->stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;

@@ -1,6 +1,6 @@
 // Device side of the wgmma GEMM / implicit-GEMM convolution: tile decode, the warp-specialised persistent kernel
-// (MMA warpgroup / two epilogue groups / TMA producer), the opt-in sequence kernel and the wide-tile kernel (producer
-// warpgroup / two MMA + epilogue warpgroups).  Included ONLY by
+// (MMA warpgroup / two epilogue groups / TMA producer) and the wide-tile kernel (producer warpgroup / two MMA + epilogue
+// warpgroups).  Included ONLY by
 // umma_gemm.cu, which holds the host side (launch plans, cost model, autotuner, tensor maps).  See umma_gemm.cu's header
 // comment for the design.
 #pragma once
@@ -54,34 +54,26 @@ struct KParams {
     int tiles_m, tiles_n, tiles_total;
     int k_blocks, kelems;
     int bn, stages;
-    uint32_t stage_bytes, tx_bytes;
-    uint32_t idesc;
+    uint32_t stage_bytes, tx_bytes;  // one 128-byte K block of A and B per pipeline stage
+    int sgn;        // integer kind: bit 0 = A signed, bit 1 = B signed
     int conv;
     int tw, th, tb, tiles_x, tiles_y;
     int OH, OW, Bn;
     int sy, sx, dy, dx, pt, pl, kw, c_blocks;
     int a_bcast0, a_bcast1, b_bcast0, b_bcast1;
-    long long* trace;  // debug: per-event clock64 timestamps of CTA 0 (4 rows x 2048), or null
-    int pair;       // always 0 on sm_90 (plan_shape): two 128-row tiles sharing one B tile
-    int katoms;     // consecutive 128-byte K blocks loaded / multiplied per pipeline stage (1 or 2): amortises the fixed
-                    // per-stage barrier round trip of the issuing threads when tiles are small
-    uint32_t atom_bytes;
-    int ksplit;     // always 0 on sm_90 (plan_shape): even / odd K blocks in two accumulators added by the epilogue
     int nbuf;       // staging buffers per epilogue group (ring): nbuf-1 (nbuf-2 with res_tma) bulk stores stay in flight
     int res_tma;    // 1: the residual tile is prefetched by TMA into the staging buffer (needs tma_store)
     uint32_t res_tx_bytes;
     int tma_store;  // 1: epilogue stages 128x32 chunks in smem and writes them with TMA (output rows contiguous)
-    int acc1;       // always 0 on sm_90 (plan_shape): one accumulator stage
     int splitk;     // > 1: `splitk` CTAs share one output tile, each over `kb_per` K blocks; raw partial accumulators go
                     // to `sk_ws`, the LAST CTA to arrive (per tile and epilogue group, `sk_cnt`) sums them in split order
                     // (deterministic) and runs the epilogue
     int kb_per;
-    int cta2;       // always 0 on sm_90 (plan_shape): no two-CTA MMA
     int units_total;  // tiles_total * splitk
     int x3_cb;      // > 0: 3xTF32 over TWO planes of A -- the K (channel) range is three segments of x3_cb K blocks,
                     //      [lo | hi | hi]: segment 0 reads the low-part plane (tma_a2), segments 1 and 2 read the ORIGINAL f32
                     //      tensor (tf32 wgmma ignores the 13 low mantissa bits, so the raw values ARE the high parts)
-    FastDiv d_tiles_n, d_units_m, d_z0, d_tiles_x, d_tiles_y, d_tiles_total, d_c_blocks, d_kw, d_tw, d_th;
+    FastDiv d_tiles_n, d_tiles_m, d_z0, d_tiles_x, d_tiles_y, d_tiles_total, d_c_blocks, d_kw, d_tw, d_th;
     uint32_t* sk_ws;
     int* sk_cnt;
     EpilogueDesc epi;
@@ -94,15 +86,12 @@ struct TileCoord {
     int ox0, oy0, b0;  // conv
 };
 
-// t indexes work units: (n tile, m tile or PAIR of m tiles, batch); `sub` selects the tile inside a pair.
-__device__ __forceinline__ TileCoord decode_tile(const KParams& p, int t, int sub, int rank = 0) {
+// t indexes output tiles: (n tile, m tile, batch).
+__device__ __forceinline__ TileCoord decode_tile(const KParams& p, int t) {
     TileCoord c;
     int n_blk, rest, m_blk, z;
     p.d_tiles_n.divmod(t, rest, n_blk);
-    // one unit = (pair + 1) MMA tiles of (cta2 + 1) x 128 rows: `mult` consecutive 128-row blocks
-    const int mult = (p.pair + 1) * (p.cta2 + 1);
-    p.d_units_m.divmod(rest, z, m_blk);
-    m_blk = m_blk * mult + sub * (p.cta2 + 1) + rank;  // may be >= tiles_m in the tail: every row is then out of range
+    p.d_tiles_m.divmod(rest, z, m_blk);
     c.n0 = n_blk * p.bn;
     c.m0 = m_blk * BM;
     p.d_z0.divmod(z, c.z1, c.z0);
@@ -110,7 +99,7 @@ __device__ __forceinline__ TileCoord decode_tile(const KParams& p, int t, int su
     if (p.conv) {
         int xt, r2, yt, bt;
         p.d_tiles_x.divmod(m_blk, r2, xt);
-        p.d_tiles_y.divmod(r2, bt, yt);  // bt >= number of batch tiles for the odd tail of a pair -> b0 >= B
+        p.d_tiles_y.divmod(r2, bt, yt);
         c.ox0 = xt * p.tw;
         c.oy0 = yt * p.th;
         c.b0 = bt * p.tb;
@@ -175,19 +164,17 @@ __device__ __noinline__ float4 act4(float4 x, int act) {
 
 // Split-K hand-off of one epilogue group (128 threads): store this CTA's raw accumulator chunks, then count arrivals.
 // Returns true for the group of the CTA that arrived last: it owns the epilogue of (tile, group).
-// Workspace layout: [tile][sub][split][chunk][column j][row r] so that a warp's 32 rows are contiguous.
+// Workspace layout: [tile][split][chunk][column j][row r] so that a warp's 32 rows are contiguous.
 __device__ __forceinline__ bool splitk_publish(const KParams& p, int t, int ks, int grp, int q, int lane, uint32_t t_acc,
-                                               int* flag, uint32_t acc_smem) {  // t = tile slot (tile, or 2 * tile + cluster rank)
+                                               int* flag, uint32_t acc_smem) {
     const int r = q * 32 + lane;
     const int nchunks = p.bn >> 5;
-    for (int sub = 0; sub <= p.pair; sub++) {
-        for (int c0 = grp * 32; c0 < p.bn; c0 += 64) {
-            uint32_t v[32];
-            acc_ld(acc_smem, t_acc + sub * p.bn + c0, v);
-            uint32_t* w = p.sk_ws + ((((size_t)(t * 2 + sub) * p.splitk + ks) * nchunks + (c0 >> 5)) << 12) + r;
+    for (int c0 = grp * 32; c0 < p.bn; c0 += 64) {
+        uint32_t v[32];
+        acc_ld(acc_smem, t_acc + c0, v);
+        uint32_t* w = p.sk_ws + ((((size_t)t * p.splitk + ks) * nchunks + (c0 >> 5)) << 12) + r;
 #pragma unroll
-            for (int j = 0; j < 32; j++) __stcg(w + j * 128, v[j]);
-        }
+        for (int j = 0; j < 32; j++) __stcg(w + j * 128, v[j]);
     }
     __threadfence();
     asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory");
@@ -205,9 +192,9 @@ __device__ __forceinline__ bool splitk_publish(const KParams& p, int t, int ks, 
 
 // Sum of the `splitk` partial chunks in split order (the same order whichever CTA arrived last).
 template <int KIND>
-__device__ __forceinline__ void splitk_sum(const KParams& p, int t, int sub, int c0, int r, uint32_t (&v)[32]) {
+__device__ __forceinline__ void splitk_sum(const KParams& p, int t, int c0, int r, uint32_t (&v)[32]) {
     const int nchunks = p.bn >> 5;
-    const uint32_t* w = p.sk_ws + ((((size_t)(t * 2 + sub) * p.splitk) * nchunks + (c0 >> 5)) << 12) + r;
+    const uint32_t* w = p.sk_ws + ((((size_t)t * p.splitk) * nchunks + (c0 >> 5)) << 12) + r;
     const size_t stride = (size_t)nchunks << 12;
 #pragma unroll
     for (int j = 0; j < 32; j++) v[j] = __ldcg(w + j * 128);
@@ -224,14 +211,6 @@ __device__ __forceinline__ void splitk_sum(const KParams& p, int t, int sub, int
         }
     }
 }
-
-// Per-thread pipeline state that survives from one layer of a sequence kernel to the next: parity bits of the operand
-// ring (bit s = uses of stage s so far, mod 2), of the two accumulator barriers, of the residual barriers, and the
-// running tile count that picks the accumulator stage.  Each role keeps its own copy.
-struct PipeState {
-    uint32_t ring = 0, acc = 0, rphase = 0;
-    int it = 0;
-};
 
 struct SmemLayout {
     uint8_t* smem;  // operand stages (1024-B aligned), staging buffers behind them
@@ -253,19 +232,20 @@ namespace rtb {
 // group after it has been issued and it has retired (one arrival per warp); the finished tile is stored to accumulator
 // stage (tile count & 1) once the epilogue has released it (8 warp arrivals), then announced (128 arrivals).
 template <int KIND, int SGN, int N>
-__device__ __forceinline__ void mma_units(const KParams& p, const SmemLayout& L, int worker, int n_workers, PipeState& st) {
+__device__ __forceinline__ void mma_units(const KParams& p, const SmemLayout& L, int worker, int n_workers) {
     const int lane = threadIdx.x & 31;
     const uint32_t smem0 = smem_u32(L.smem);
+    uint32_t ring = 0, aphase = 0;  // bit s = uses of operand stage s / accumulator stage s so far, mod 2
     int stage = 0;
-    for (int u = worker; u < p.units_total; u += n_workers, st.it++) {
+    for (int u = worker, it = 0; u < p.units_total; u += n_workers, it++) {
         const int kb0 = p.d_tiles_total.div(u) * p.kb_per, kb1 = min(p.k_blocks, kb0 + p.kb_per);
-        const int acc = st.it & 1;
+        const int acc = it & 1;
         acc_t<KIND> d0[N / 2], d1[N / 2];
 #pragma unroll
         for (int i = 0; i < N / 2; i++) d0[i] = d1[i] = 0;
         int prev = -1;
         for (int kb = kb0; kb < kb1; kb++) {
-            mbar_wait(&L.full_bar[stage], (st.ring >> stage) & 1);
+            mbar_wait(&L.full_bar[stage], (ring >> stage) & 1);
             wgmma_fence_operand(d0);
             wgmma_fence_operand(d1);
             wgmma_fence();
@@ -284,15 +264,15 @@ __device__ __forceinline__ void mma_units(const KParams& p, const SmemLayout& L,
             wgmma_wait<1>();
             if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
             prev = stage;
-            st.ring ^= 1u << stage;
+            ring ^= 1u << stage;
             if (++stage == p.stages) stage = 0;
         }
         wgmma_wait<0>();
         wgmma_fence_operand(d0);
         wgmma_fence_operand(d1);
         if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
-        mbar_wait(&L.acc_empty[acc], ((st.acc >> acc) & 1) ^ 1);
-        st.acc ^= 1u << acc;
+        mbar_wait(&L.acc_empty[acc], ((aphase >> acc) & 1) ^ 1);
+        aphase ^= 1u << acc;
         acc_store_frag<N>(L.acc_smem, d0, 0, acc * ACC_STRIDE);
         acc_store_frag<N>(L.acc_smem, d1, 64, acc * ACC_STRIDE);
         mbar_arrive(&L.acc_full[acc]);
@@ -300,39 +280,30 @@ __device__ __forceinline__ void mma_units(const KParams& p, const SmemLayout& L,
 }
 
 template <int KIND, int N>
-__device__ __forceinline__ void mma_role(const KParams& p, const SmemLayout& L, int worker, int n_workers, PipeState& st) {
-    if (KIND == 0) {
-        mma_units<KIND, 0, N>(p, L, worker, n_workers, st);
-    } else {
-        // signedness of A / B from the operand-format fields of p.idesc (ptx.cuh make_idesc)
-        const int sgn = ((p.idesc >> 7) & 1) | (((p.idesc >> 10) & 1) << 1);
-        if (sgn == 0) mma_units<KIND, 0, N>(p, L, worker, n_workers, st);
-        else if (sgn == 1) mma_units<KIND, 1, N>(p, L, worker, n_workers, st);
-        else if (sgn == 2) mma_units<KIND, 2, N>(p, L, worker, n_workers, st);
-        else mma_units<KIND, 3, N>(p, L, worker, n_workers, st);
-    }
+__device__ __forceinline__ void mma_role(const KParams& p, const SmemLayout& L, int worker, int n_workers) {
+    if (KIND == 0) mma_units<KIND, 0, N>(p, L, worker, n_workers);
+    else if (p.sgn == 0) mma_units<KIND, 0, N>(p, L, worker, n_workers);
+    else if (p.sgn == 1) mma_units<KIND, 1, N>(p, L, worker, n_workers);
+    else if (p.sgn == 2) mma_units<KIND, 2, N>(p, L, worker, n_workers);
+    else mma_units<KIND, 3, N>(p, L, worker, n_workers);
 }
 
-// TMA producer of both GEMM kernels: one warp walks this CTA's work units and fills the operand ring -- A (128 rows, or
-// two 128-row tiles in pair mode) and B (bn rows) per 128-byte K block, the conv filter tap / channel walk, the two-plane
-// 3xTF32 segments and broadcast batch dims.  Runs warp-uniformly, one elected lane issues.
+// TMA producer of both GEMM kernels: one warp walks this CTA's work units and fills the operand ring -- A (128 rows)
+// and B (bn rows) of one 128-byte K block per stage, the conv filter tap / channel walk, the two-plane 3xTF32 segments
+// and broadcast batch dims.  Runs warp-uniformly, one elected lane issues.
 __device__ __forceinline__ void producer_role(const KParams& p, const CUtensorMap* tma_a, const CUtensorMap* tma_a2,
-                                              const CUtensorMap* tma_b, const SmemLayout& L, int worker, int n_workers,
-                                              PipeState& st) {
+                                              const CUtensorMap* tma_b, const SmemLayout& L, int worker, int n_workers) {
     uint8_t* smem = L.smem;
-    uint64_t* full_bar = L.full_bar;
     uint64_t* empty_bar = L.empty_bar;
+    uint32_t ring = 0;  // bit s = uses of stage s so far, mod 2
     int stage = 0;
-    int tr_p = 0;
     const uint32_t smem0 = smem_u32(smem);
-    const uint32_t full0 = smem_u32(full_bar);
-    const uint32_t a_bytes = (p.pair ? 2 : 1) * A_STAGE_BYTES;
+    const uint32_t full0 = smem_u32(L.full_bar);
     for (int u = worker; u < p.units_total; u += n_workers) {
         int t, ks;
         p.d_tiles_total.divmod(u, ks, t);
         const int kb0 = ks * p.kb_per, kb1 = min(p.k_blocks, kb0 + p.kb_per);
-        const TileCoord tc = decode_tile(p, t, 0);
-        const TileCoord tc1 = p.pair ? decode_tile(p, t, 1) : tc;
+        const TileCoord tc = decode_tile(p, t);
         // conv: K block -> (filter tap, channel block), kept incrementally
         int tap, cb, ky, kx;
         p.d_c_blocks.divmod(kb0, tap, cb);
@@ -347,105 +318,47 @@ __device__ __forceinline__ void producer_role(const KParams& p, const CUtensorMa
         // programmatic dependent launch: the producer is the first to touch the predecessor's output; everything
         // above (tile decode) ran while the predecessor grid was still draining
         if (u == worker) asm volatile("griddepcontrol.wait;" ::: "memory");
-        for (int kb = kb0; kb < kb1; kb += p.katoms) {
-            const int natoms = min(p.katoms, kb1 - kb);
-            mbar_wait(&empty_bar[stage], ((st.ring >> stage) & 1) ^ 1);
-            const bool leader = elect_one();
-            const uint32_t fb = full0 + stage * 8;
-            if (leader) {
-                if (p.trace && blockIdx.x == 0 && tr_p < 2048) p.trace[tr_p++] = clock64();
-                mbar_expect_tx_u32(fb, p.tx_bytes * natoms);
+        for (int kb = kb0; kb < kb1; kb++) {
+            mbar_wait(&empty_bar[stage], ((ring >> stage) & 1) ^ 1);
+            if (elect_one()) {
+                const uint32_t fb = full0 + stage * 8;
+                mbar_expect_tx_u32(fb, p.tx_bytes);
+                const uint32_t sa = smem0 + stage * p.stage_bytes;
+                const uint32_t sb = sa + A_STAGE_BYTES;
+                const CUtensorMap* ma = (p.x3_cb && seg == 0) ? tma_a2 : tma_a;
+                if (p.conv) {
+                    const int c0 = cb * p.kelems;
+                    const int ca = p.x3_cb ? sblk * p.kelems : c0;
+                    tma_load_4d_u32(sa, ma, fb, ca, tc.ox0 * p.sx - p.pl + kx * p.dx, tc.oy0 * p.sy - p.pt + ky * p.dy, tc.b0);
+                    tma_load_4d_u32(sb, tma_b, fb, c0, tc.n0, tap, 0);
+                } else {
+                    const int k0 = kb * p.kelems;
+                    const int ka = p.x3_cb ? sblk * p.kelems : k0;
+                    tma_load_4d_u32(sa, ma, fb, ka, tc.m0, p.a_bcast0 ? 0 : tc.z0, p.a_bcast1 ? 0 : tc.z1);
+                    tma_load_4d_u32(sb, tma_b, fb, k0, tc.n0, p.b_bcast0 ? 0 : tc.z0, p.b_bcast1 ? 0 : tc.z1);
+                }
             }
-            for (int a = 0; a < natoms; a++) {
-                if (leader) {
-                    const uint32_t sa = smem0 + stage * p.stage_bytes + a * p.atom_bytes;
-                    const uint32_t sb = sa + a_bytes;
-                    auto load = [&](uint32_t dst, const CUtensorMap* m, int c0, int c1, int c2, int c3) {
-                        tma_load_4d_u32(dst, m, fb, c0, c1, c2, c3);
-                    };
-                    const CUtensorMap* ma = (p.x3_cb && seg == 0) ? tma_a2 : tma_a;
-                    if (p.conv) {
-                        const int c0 = cb * p.kelems;
-                        const int ca = p.x3_cb ? sblk * p.kelems : c0;
-                        load(sa, ma, ca, tc.ox0 * p.sx - p.pl + kx * p.dx, tc.oy0 * p.sy - p.pt + ky * p.dy, tc.b0);
-                        if (p.pair)
-                            load(sa + A_STAGE_BYTES, ma, ca, tc1.ox0 * p.sx - p.pl + kx * p.dx,
-                                 tc1.oy0 * p.sy - p.pt + ky * p.dy, tc1.b0);
-                        load(sb, tma_b, c0, tc.n0, tap, 0);
-                    } else {
-                        const int k0 = (kb + a) * p.kelems;
-                        const int ka = p.x3_cb ? sblk * p.kelems : k0;
-                        const int az0 = p.a_bcast0 ? 0 : tc.z0, az1 = p.a_bcast1 ? 0 : tc.z1;
-                        load(sa, ma, ka, tc.m0, az0, az1);
-                        if (p.pair) load(sa + A_STAGE_BYTES, ma, ka, tc1.m0, az0, az1);
-                        load(sb, tma_b, k0, tc.n0, p.b_bcast0 ? 0 : tc.z0, p.b_bcast1 ? 0 : tc.z1);
-                    }
-                }
-                if (p.x3_cb && ++sblk == p.x3_cb) {
-                    sblk = 0;
-                    seg = seg == 2 ? 0 : seg + 1;  // (conv: the next filter tap starts over at segment 0)
-                }
-                if (++cb == p.c_blocks) {
-                    cb = 0;
-                    tap++;
-                    if (++kx == p.kw) {
-                        kx = 0;
-                        ky++;
-                    }
+            if (p.x3_cb && ++sblk == p.x3_cb) {
+                sblk = 0;
+                seg = seg == 2 ? 0 : seg + 1;  // (conv: the next filter tap starts over at segment 0)
+            }
+            if (++cb == p.c_blocks) {
+                cb = 0;
+                tap++;
+                if (++kx == p.kw) {
+                    kx = 0;
+                    ky++;
                 }
             }
             __syncwarp();
-            st.ring ^= 1u << stage;
+            ring ^= 1u << stage;
             if (++stage == p.stages) stage = 0;
         }
     }
 }
 
-// One launch worth of work (all roles).  FAST = the launch satisfies, for EVERY chunk, the conditions of the register
-// fast path (TMA-store output, N % 32 == 0, f32 with act in {none, relu} and bias / residual absent or
-// vector-addressable [residual via TMA], or raw i32): the epilogue is then a short straight-line loop.  The generic
-// variant (FAST = 0) keeps every edge case.
-template <int KIND, int FAST>
-__device__ __forceinline__ void run_layer(const KParams& p, const CUtensorMap* tma_a, const CUtensorMap* tma_a2,
-                                          const CUtensorMap* tma_b, const CUtensorMap* tma_d, const CUtensorMap* tma_r, const SmemLayout& L,
-                                          int worker, int n_workers, PipeState& st) {
-    uint8_t* smem = L.smem;
-    uint8_t* stg_base = smem + (size_t)p.stages * p.stage_bytes;
-    const int nbuf = p.nbuf;
-    uint64_t* acc_full = L.acc_full;
-    uint64_t* acc_empty = L.acc_empty;
-    uint64_t* res_bar = L.res_bar;
-    int* sk_flag = L.sk_flag;
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    // Control warps run their loops WARP-UNIFORMLY (all 32 lanes wait on the barriers, one elected lane issues the
-    // TMA / MMA instructions): addresses and descriptors then live in uniform registers instead of being moved
-    // there (R2UR) for every instruction, which is what bounds a single issuing thread.
-    if (warp == PRODUCER_WARP) {
-        producer_role(p, tma_a, tma_a2, tma_b, L, worker, n_workers, st);
-    } else if (warp < 4) {
-        // ===================== MMA warpgroup: accumulators in registers, finished tiles to shared memory
-        if (p.bn == 32)
-            mma_role<KIND, 32>(p, L, worker, n_workers, st);
-        else
-            mma_role<KIND, 64>(p, L, worker, n_workers, st);
-    } else if (warp >= 4) {
-        // ===================== epilogue warps: one of four variants (umma_epilogue_plain.cuh / umma_epilogue_generic.cuh)
-        const EpiCtx c{p, L, stg_base, nbuf, acc_full, acc_empty, res_bar, sk_flag, tma_d, tma_r, L.acc_smem, 0, worker, n_workers, st, warp, lane};
-        if (KIND == 0 && (FAST == 3 || FAST == 5))
-            epilogue_plain_f32<FAST>(c);
-        else if (KIND == 1 && (FAST == 4 || FAST == 6))
-            epilogue_plain_i8<FAST>(c);
-        else if (FAST)
-            epilogue_fast<KIND, FAST>(c);
-        else
-            epilogue_generic<KIND>(c);
-    }
-
-}
-
-// Shared-memory carve-up: a fixed 1 KB block of mbarriers first (so that it does not move when the stage geometry changes
-// from layer to layer of a sequence kernel), the column vectors, the accumulator tiles, operand stages behind them.
+// Shared-memory carve-up: a fixed 1 KB block of mbarriers first, the column vectors, the accumulator tiles, operand
+// stages behind them.
 constexpr int SMEM_FIXED_BYTES = 1024 /*align*/ + 4096 /*barriers, column vectors*/ + ACC_SMEM_BYTES;
 static_assert(ACC_SMEM_BYTES % 1024 == 0, "operand stages must stay 1024-B aligned");
 static_assert(2 * ACC_STRIDE <= ACC_COLS, "two accumulator stages");
@@ -496,6 +409,10 @@ __device__ __forceinline__ void kernel_setup(const SmemLayout& L) {
     asm volatile("bar.sync 15, %0;" ::"r"(NUM_THREADS) : "memory");  // 12 warps wait, the producer warp only arrives
 }
 
+// One CTA per SM walks the work units blockIdx.x, blockIdx.x + gridDim.x, ... in every role.  FAST selects the epilogue
+// (umma_epilogue_plain.cuh / umma_epilogue_generic.cuh): 0 generic, every edge case; 1 specialised, every chunk takes the
+// register fast path (TMA-store output, N % 32 == 0, column vectors and residual vector-addressable); 2 = 1 with the
+// out-of-line Gelu; 3 / 5 plain f32 (+ Gelu); 4 / 6 plain integer *ToFloat (+ Gelu).
 template <int KIND, int FAST>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 umma_gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
@@ -503,7 +420,6 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
                  const __grid_constant__ CUtensorMap tma_a2, const __grid_constant__ KParams p) {
     extern __shared__ uint8_t smem_raw[];
     const SmemLayout L = carve_smem(smem_raw);
-    if (p.trace && blockIdx.x == 0 && threadIdx.x == 0) p.trace[6144 + 1100] = clock64();  // kernel entry
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tma_a);
         tma_prefetch_desc(&tma_b);
@@ -514,87 +430,35 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
     kernel_setup(L);
     // Programmatic dependent launch: everything above (barrier init, descriptor prefetch) overlaps the tail of the
     // previous kernel in the stream; global memory is only touched after this point.
-    if (p.trace && blockIdx.x == 0 && threadIdx.x == 0) p.trace[6144 + 1101] = clock64();  // set-up done
     if (threadIdx.x >> 5 != PRODUCER_WARP) asm volatile("griddepcontrol.wait;" ::: "memory");  // (the producer waits after its tile decode)
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    if (p.trace && blockIdx.x == 0 && threadIdx.x == 0) p.trace[6144 + 1102] = clock64();  // predecessor complete
-    PipeState st;
-    run_layer<KIND, FAST>(p, &tma_a, &tma_a2, &tma_b, &tma_d, &tma_r, L, (int)blockIdx.x, (int)gridDim.x, st);
-    if (p.trace && blockIdx.x == 0 && threadIdx.x == 0) p.trace[6144 + 1103] = clock64();  // control thread done
-}
-
-// ------------------------------------------------------------------------------------------
-// Sequence kernel: up to SEQ_MAX consecutive launches (layers of a captured op list) run inside ONE persistent
-// kernel.  Between two layers every CTA drains its output stores and meets the others at a grid-wide barrier (an
-// arrival counter in global memory): a layer boundary costs one barrier round trip plus one TMA latency instead of a
-// kernel launch, tensor-map fetch and a cold pipeline.  Layer parameters and tensor maps live in the
-// kernel parameter block (constant bank), indexed by the layer number.
-// ------------------------------------------------------------------------------------------
-constexpr int SEQ_MAX = 28;
-struct SeqParams {
-    int n;
-    int pad;
-    unsigned* gbar;  // arrival counter, zero between launches
-    CUtensorMap maps[SEQ_MAX][4];
-    KParams layer[SEQ_MAX];
-};
-static_assert(sizeof(SeqParams) <= 32764, "kernel parameter block too large");
-
-__device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
-    unsigned v;
-    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-
-template <int KIND, int FAST>
-__global__ void __launch_bounds__(NUM_THREADS, 1) umma_seq_kernel(const __grid_constant__ SeqParams sp) {
-    extern __shared__ uint8_t smem_raw[];
+    const int worker = (int)blockIdx.x, n_workers = (int)gridDim.x;
     const int warp = threadIdx.x >> 5;
-    const SmemLayout L = carve_smem(smem_raw);
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&sp.maps[0][0]);
-        tma_prefetch_desc(&sp.maps[0][1]);
-    }
-    kernel_setup(L);
-    if (warp != PRODUCER_WARP) asm volatile("griddepcontrol.wait;" ::: "memory");
-    PipeState st;
-    for (int l = 0; l < sp.n; l++) {
-        const KParams& p = sp.layer[l];
-        if (l + 1 == sp.n) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        run_layer<KIND, FAST>(p, &sp.maps[l][0], &sp.maps[l][0], &sp.maps[l][1], &sp.maps[l][2], &sp.maps[l][3], L,
-                              (int)blockIdx.x, (int)gridDim.x, st);
-        if (l + 1 < sp.n) {
-            // ---- layer boundary: this CTA's outputs are complete and visible, then wait for every other CTA's
-            if (warp >= 4 && warp < PRODUCER_WARP) {
-                asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // TMA stores performed (issuer threads)
-                asm volatile("fence.proxy.async;" ::: "memory");
-                __threadfence();
-            }
-            if (threadIdx.x == 32 * PRODUCER_WARP) {  // idle until the barrier anyway: fetch the next layer's tensor maps
-                tma_prefetch_desc(&sp.maps[l + 1][0]);
-                tma_prefetch_desc(&sp.maps[l + 1][1]);
-                tma_prefetch_desc(&sp.maps[l + 1][2]);
-            }
-            __syncthreads();
-            if (threadIdx.x == 0) {
-                __threadfence();
-                atomicAdd(sp.gbar, 1u);
-                const unsigned target = gridDim.x * (unsigned)(l + 1);
-                uint32_t spins = 0;
-                while (ld_acquire_gpu(sp.gbar) < target) {
-                    __nanosleep(32);
-                    if (++spins > (1u << 25)) __trap();  // > ~1 s: a CTA of the grid never arrived
-                }
-                __threadfence();
-            }
-            __syncthreads();
-            asm volatile("fence.proxy.async;" ::: "memory");
-        }
-    }
-    // re-arm the arrival counter: the last CTA to leave (everyone has passed every barrier by then) zeroes it
-    if (threadIdx.x == 0) {
-        const unsigned old = atomicAdd(sp.gbar, 1u);
-        if (old == gridDim.x * (unsigned)sp.n - 1u) *reinterpret_cast<volatile unsigned*>(sp.gbar) = 0u;
+    const int lane = threadIdx.x & 31;
+    // Control warps run their loops WARP-UNIFORMLY (all 32 lanes wait on the barriers, one elected lane issues the
+    // TMA / MMA instructions): addresses and descriptors then live in uniform registers instead of being moved
+    // there (R2UR) for every instruction, which is what bounds a single issuing thread.
+    if (warp == PRODUCER_WARP) {
+        producer_role(p, &tma_a, &tma_a2, &tma_b, L, worker, n_workers);
+    } else if (warp < 4) {
+        // ===================== MMA warpgroup: accumulators in registers, finished tiles to shared memory
+        if (p.bn == 32)
+            mma_role<KIND, 32>(p, L, worker, n_workers);
+        else
+            mma_role<KIND, 64>(p, L, worker, n_workers);
+    } else {
+        // ===================== epilogue warps
+        uint8_t* stg_base = L.smem + (size_t)p.stages * p.stage_bytes;
+        const EpiCtx c{p, L, stg_base, p.nbuf, L.acc_full, L.acc_empty, L.res_bar, L.sk_flag, &tma_d, &tma_r, L.acc_smem,
+                       worker, n_workers, warp, lane};
+        if (KIND == 0 && (FAST == 3 || FAST == 5))
+            epilogue_plain_f32<FAST>(c);
+        else if (KIND == 1 && (FAST == 4 || FAST == 6))
+            epilogue_plain_i8<FAST>(c);
+        else if (FAST)
+            epilogue_fast<KIND, FAST>(c);
+        else
+            epilogue_generic<KIND>(c);
     }
 }
 
@@ -671,7 +535,7 @@ __device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout
     };
     for (int u = worker; u < p.units_total; u += n_workers) {
         {  // (the tile is decoded again after the main loop: its coordinates would hold registers through it)
-            const TileCoord tc = decode_tile(p, u, 0);  // (no split-K: a unit is a tile)
+            const TileCoord tc = decode_tile(p, u);  // (no split-K: a unit is a tile)
             // The unit's bias (zeros without one: x + 0 keeps the -0 -> +0 of the other epilogues).  Every reader of the
             // previous unit's values has passed the last chunk barrier; the barrier after the main loop publishes these.
             if (t < N) bias_s[t] = (e.bias_kind == 1 && tc.n0 + t < p.N) ? __ldg(e.bias + tc.n0 + t) : 0.0f;
@@ -704,7 +568,7 @@ __device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout
         wgmma_wait<0>();
         wgmma_fence_operand(d);
         if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
-        const TileCoord tc = decode_tile(p, u, 0);
+        const TileCoord tc = decode_tile(p, u);
         consumers_sync();
 #pragma unroll
         for (int k = 0; k < N / 32; k++, ci++) {
@@ -802,10 +666,7 @@ umma_wide_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     if (warp < 4) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-        if (warp == 0) {
-            PipeState st;
-            producer_role(p, &tma_a, &tma_a2, &tma_b, L, (int)blockIdx.x, (int)gridDim.x, st);
-        }
+        if (warp == 0) producer_role(p, &tma_a, &tma_a2, &tma_b, L, (int)blockIdx.x, (int)gridDim.x);
     } else {
         asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
         // (Gelu: 128 columns only -- the out-of-line act4 calls would spill around 128 live accumulators per thread)

@@ -301,7 +301,7 @@ def check_matmul_shapes(rt, oracle):
     worst = max(worst, _matmul_case(rt, oracle, ctx, (2, 5, 12), (12, 7), bias=True, alpha=0.125))
     worst = max(worst, _matmul_case(rt, oracle, ctx, (200, 96), (96, 80), bias=True, prepack=True))
     worst = max(worst, _matmul_case(rt, oracle, ctx, (4, 3, 128, 64), (4, 3, 64, 128), alpha=0.125, b_kmajor=True))
-    # many row tiles with a narrow N (pair mode), odd tile counts, N / K tails
+    # many row tiles with a narrow N, odd tile counts, N / K tails
     worst = max(worst, _matmul_case(rt, oracle, ctx, (128 * 301 + 5, 72), (72, 64), bias=True, prepack=True))
     worst = max(worst, _matmul_case(rt, oracle, ctx, (40000, 40), (40, 100), b_kmajor=True))
     worst = max(worst, _matmul_case(rt, oracle, ctx, (3, 128 * 151, 33), (33, 36)))
@@ -463,20 +463,10 @@ def check_plans(rt, oracle):
 
 
 # ------------------------------------------------------------------------------------------
-def check_sequence(rt, oracle):
-    """Inside graph capture consecutive tensor-core launches are fused into persistent sequence kernels (grid barrier
-    between layers).  Replaying the graph must reproduce the eager results bit for bit (same plans, same arithmetic),
-    for chains shorter and longer than one kernel's layer capacity, with residual links, and more than once.
-    (The sequence kernel is opt-in through RTEN_B200_SEQ=1, set here for the duration of the check.)"""
-    import os
-    os.environ["RTEN_B200_SEQ"] = "1"
-    try:
-        return _check_sequence(rt, oracle)
-    finally:
-        os.environ.pop("RTEN_B200_SEQ", None)
-
-
-def _check_sequence(rt, oracle):
+def check_graph_chains(rt, oracle):
+    """Chains of consecutive tensor-core launches captured into one CUDA graph.  Replaying the graph must reproduce the
+    eager results bit for bit (same plans, same arithmetic), for a short and a 45-layer chain, with residual links, and
+    more than once."""
     ctx = new_ctx(rt)
     r = oracle.XorShiftRng(321)
 
@@ -489,7 +479,7 @@ def _check_sequence(rt, oracle):
     # a: bottleneck-like chain with residual links (index of the producing layer, -1 = the input)
     chain_a = [conv_layer(64, 128, 1), conv_layer(128, 128, 3), conv_layer(128, 128, 1, res=0), conv_layer(128, 64, 3),
                conv_layer(64, 256, 1), conv_layer(256, 64, 1), conv_layer(64, 64, 3, res=5), conv_layer(64, 512, 1, act=0)]
-    # b: longer than SEQ_MAX layers -> split over several sequence kernels
+    # b: 45 layers, a residual link every third layer
     chain_b = [conv_layer(64, 64, 1, res=(i - 2 if i >= 2 and i % 3 == 0 else None)) for i in range(45)]
     x = ctx.to_device(r.uniform((4, 64, 28, 28)), channels_last=True)
 
@@ -518,9 +508,9 @@ def _check_sequence(rt, oracle):
             g.launch()
             ctx.sync()
             for i, (t, w) in enumerate(zip(eager, want)):
-                assert_bit_exact(t.numpy(), w, f"sequence chain {name} layer {i} replay {rep}")
+                assert_bit_exact(t.numpy(), w, f"graph chain {name} layer {i} replay {rep}")
         worst_layers = max(worst_layers, len(chain))
-    # integer launches in one capture (independent problems, one sequence kernel)
+    # three independent integer launches in one capture
     a8 = [r.u8((200, 512)) for _ in range(3)]
     b8 = [r.i8((512, 160)) for _ in range(3)]
     az, bz = r.u8((200,)), r.i8((160,))
@@ -536,7 +526,7 @@ def _check_sequence(rt, oracle):
     g.launch()
     ctx.sync()
     for o, w in zip(outs, want):
-        assert_bit_exact(o.numpy(), w, "sequence MatMulInteger")
+        assert_bit_exact(o.numpy(), w, "graph MatMulInteger")
     return f"chains of up to {worst_layers} layers replayed bit-exactly"
 
 
@@ -622,7 +612,7 @@ def check_conv_more(rt, oracle):
     w = max(w, _conv_case(rt, oracle, ctx, (1, 4, 12, 12), (8, 4, 5, 5), pads=(2, 2, 2, 2), cl=True))
     w = max(w, _conv_case(rt, oracle, ctx, (3, 2, 9, 14), (5, 2, 3, 4), pads=(0, 2, 1, 0), strides=(1, 3), dil=(2, 1)))
     w = max(w, _conv_case(rt, oracle, ctx, (2, 1, 10, 10), (6, 1, 3, 8), pads=(1, 4, 1, 3), residual=True))
-    # pair mode / odd tile counts / N tails through the TMA-store epilogue
+    # odd tile counts / N tails through the TMA-store epilogue
     w = max(w, _conv_case(rt, oracle, ctx, (5, 32, 20, 20), (72, 32, 3, 3), pads=(1, 1, 1, 1), cl=True))
     w = max(w, _conv_case(rt, oracle, ctx, (3, 64, 28, 28), (100, 64, 1, 1), cl=True, residual=True, act=1))
     # 1-D conv (conv.rs:142-185)
@@ -996,7 +986,7 @@ def _replayed(ctx, fn):
 
 
 def check_resnet50_b32_baseline(rt, oracle):
-    """configs[1] exactly as benched: ResNet-50 fp32, batch 32, autotuned launch plans (split-K, CTA pairs ...), the step
+    """configs[1] exactly as benched: ResNet-50 fp32, batch 32, autotuned launch plans (split-K, wide tiles ...), the step
     replayed from a CUDA graph.  TF32 single pass: logits within 1e-2 * max |ref|; 3xTF32 (library default): within
     1e-4 * max |ref| and the same arg-max on every image."""
     from rten_b200 import graphs
@@ -1705,7 +1695,7 @@ ALL_CHECKS = [
     ("dql", check_dql), ("glue", check_glue), ("matmul_small", check_matmul_small), ("matmul_shapes", check_matmul_shapes),
     ("matmul_bert", check_matmul_bert), ("gemm_op", check_gemm_op), ("matmul_integer", check_matmul_integer),
     ("conv_basic", check_conv_basic), ("conv_stride", check_conv_stride), ("conv_more", check_conv_more),
-    ("conv_integer", check_conv_integer), ("plans", check_plans), ("tf32x3", check_tf32x3), ("sequence", check_sequence), ("conv_integer_fused", check_conv_integer_fused),
+    ("conv_integer", check_conv_integer), ("plans", check_plans), ("tf32x3", check_tf32x3), ("graph_chains", check_graph_chains), ("conv_integer_fused", check_conv_integer_fused),
     ("resnet50_int8_model", check_resnet50_int8_model), ("gpt2_int8_kvcache", check_gpt2_int8_kvcache), ("mnist_model", check_mnist_model), ("resnet50_model", check_resnet50_model), ("bert_model", check_bert_model),
     ("model_executor", check_model_executor), ("generator", check_generator), ("halo_conv", check_halo_conv), ("quantized_linear", check_quantized_linear), ("attention_decode", check_attention_decode), ("attention_encoder", check_attention_encoder), ("gelu_epilogue", check_gelu_epilogue), ("skinny_f32", check_skinny_f32),
     ("reference_rule_f32", check_reference_rule_f32), ("graph_pool_isolation", check_graph_pool_isolation),
