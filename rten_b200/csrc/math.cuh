@@ -94,6 +94,17 @@ __device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return {__fmul_rn(a.x,
 __device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return {__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)}; }
 __device__ __forceinline__ f32x2 splat2(float c) { return pack2(c, c); }
 
+// (a0, a1) += (b0, b1) on f32 bit patterns, each half rounded to nearest like a scalar add
+__device__ __forceinline__ void add_f32x2(uint32_t& a0, uint32_t& a1, float b0, float b1) {
+    a0 = __float_as_uint(__fadd_rn(__uint_as_float(a0), b0));
+    a1 = __float_as_uint(__fadd_rn(__uint_as_float(a1), b1));
+}
+// (a0, a1) *= (b0, b1) on f32 bit patterns, each half rounded to nearest like a scalar multiply
+__device__ __forceinline__ void mul_f32x2(uint32_t& a0, uint32_t& a1, float b0, float b1) {
+    a0 = __float_as_uint(__fmul_rn(__uint_as_float(a0), b0));
+    a1 = __float_as_uint(__fmul_rn(__uint_as_float(a1), b1));
+}
+
 // reduced_range_exp of two lanes (same roundings as the scalar recipe)
 __device__ __forceinline__ void reduced_range_exp_x2(float& x0, float& x1) {
     const f32x2 x = pack2(x0, x1);

@@ -151,7 +151,7 @@ struct Prepared {
     OperandDesc od, ord;
     uint32_t dbox[4];
     int tma_store, res_tma;  // eligibility
-    int wide;                // the wide-tile kernel may run this launch (plain f32 epilogue, see plain_f32_ok)
+    int wide;                // the wide-tile kernel may run this launch (plain f32 epilogue, see pick_epilogue)
     int step;
     int esize, kelems;
 };
@@ -163,16 +163,38 @@ static int smem_budget_for(int n_stg) { return 227 * 1024 - SMEM_FIXED_BYTES - n
 static int wide_stages(int stage_bytes) { return std::min(MAX_STAGES, (227 * 1024 - WIDE_SMEM_FIXED_BYTES) / stage_bytes); }
 static bool is_wide(int bn) { return bn > ACC_STRIDE; }
 
-// The f32 launches whose every chunk takes the plain epilogue (kernel variants 3 and 5): TMA store, N % 32 == 0,
-// alpha = 1, optional aligned column bias, optional TMA-staged residual with r_scale = 1, act in {none, Relu, Gelu,
-// ApproxGelu}, no range output.
-static bool plain_f32_ok(const rten_ctx* ctx, const GemmLaunch& L, int tma_store, int res_tma) {
+// The epilogue variant (umma_epilogue.cuh) of a launch with the given output path and split.  RTEN_B200_NO_FAST=1 sends every launch to Generic, RTEN_B200_NO_PLAIN=1 keeps launches off the plain variants
+// (comparisons between variants).
+static Epi pick_epilogue(const GemmLaunch& L, int tma_store, int res_tma, int splitk) {
     const EpilogueDesc& e = L.epi;
-    return L.kind == 0 && tma_store && (L.N % 32) == 0 && !getenv("RTEN_B200_NO_FAST") && !getenv("RTEN_B200_NO_PLAIN") &&
-           e.bias_kind != 2 &&
-           (e.bias_kind != 1 || (reinterpret_cast<uintptr_t>(e.bias) & 15) == 0) && e.alpha == 1.0f && e.act <= 3 &&
-           !e.range && (e.r == nullptr || (res_tma && e.r_scale == 1.0f));
+    auto aligned = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
+    // Fast: every chunk qualifies for the register path -- TMA store, whole 32-column chunks, column vectors 128-bit
+    // loadable (integer: zero-point / scale vectors per column or scalar), residual TMA-staged
+    bool fast = tma_store && (L.N % 32) == 0 && !getenv("RTEN_B200_NO_FAST") && e.bias_kind != 2 &&
+                (e.r == nullptr || res_tma) && (e.bias_kind != 1 || aligned(e.bias));
+    if (L.kind == 1)
+        fast = fast && (!(e.za || e.za8) || aligned(e.colsum)) && (!e.zb || e.zb_len == 1 || (e.zb_len == L.N && aligned(e.zb))) &&
+               (!e.scale || e.scale_len == 1 || (e.scale_len == L.N && aligned(e.scale)));
+    if (!fast) return Epi::Generic;
+    const bool gelu = e.act > 1;
+    if (!getenv("RTEN_B200_NO_PLAIN") && e.act <= 3) {
+        // f32: alpha = 1, optional column bias, residual with r_scale = 1, no range output
+        if (L.kind == 0 && e.alpha == 1.0f && !e.range && (e.r == nullptr || e.r_scale == 1.0f))
+            return gelu ? Epi::PlainF32Gelu : Epi::PlainF32;
+        // integer: the *ToFloat operators with a scalar (or no) activation zero point and symmetric weights
+        if (L.kind == 1 && e.scale && !e.za && !e.zb && (e.scale_len == 1 || e.scale_len == L.N) && splitk == 1 &&
+            (!e.za8 || e.colsum))
+            return gelu ? Epi::PlainI8Gelu : Epi::PlainI8;
+    }
+    return gelu ? Epi::FastGelu : Epi::Fast;
 }
+
+static const char* epi_name(Epi v) {
+    static const char* const names[] = {"Generic", "Fast", "FastGelu", "PlainF32", "PlainF32Gelu", "PlainI8", "PlainI8Gelu"};
+    return names[(int)v];
+}
+
+static bool is_plain_f32(Epi v) { return v == Epi::PlainF32 || v == Epi::PlainF32Gelu; }
 
 struct PlanShape {
     long long tiles_n, units_m, tiles, units;
@@ -385,7 +407,7 @@ static rten_status prepare_launch(rten_ctx* ctx, const GemmLaunch& L, Prepared& 
     p.res_tx_bytes = q.a_rows * KBYTES;
     q.step = q.tma_store ? 32 : 16;
     // RTEN_B200_NO_WIDE=1: no wide-tile plans (measures what they gain; recorded wide plans are re-planned)
-    q.wide = plain_f32_ok(ctx, L, q.tma_store, q.res_tma) && !getenv("RTEN_B200_NO_WIDE");
+    q.wide = is_plain_f32(pick_epilogue(L, q.tma_store, q.res_tma, 1)) && !getenv("RTEN_B200_NO_WIDE");
     return RTEN_OK;
 }
 
@@ -447,7 +469,7 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
     p.x3_cb = L.x3_cb;
     if (L.x3_cb && !encode_map(ctx, &map_a2, L.a_lo, q.esize, true, q.abox, q.aes)) return RTEN_ERR_UNSUPPORTED_VALUE;
     if (p.tma_store && !encode_map(ctx, &map_d, q.od, 4, true, q.dbox, des)) {
-        p.tma_store = 0;  // direct stores still work for any bn that is a multiple of 16
+        p.tma_store = 0;  // the generic epilogue stores directly
         p.res_tma = 0;
         map_d = map_a;
     }
@@ -455,56 +477,27 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
         p.res_tma = 0;
         map_r = map_a;
     }
+    const Epi epi = pick_epilogue(L, p.tma_store, p.res_tma, p.splitk);
+    // the generic epilogue takes a TMA-staged residual only on its register path (f32, act <= Relu)
+    if (epi == Epi::Generic && (L.kind == 1 || L.epi.act > 1)) p.res_tma = 0;
 
     if (verbose)
-        fprintf(stderr, "[umma_gemm] kind=%d conv=%d M=%d N=%d K=%d kb=%d tiles_m=%d bn=%d splitk=%d units=%d stages=%d tma_store=%d res_tma=%d nbuf=%d box=%dx%dx%d\n",
+        fprintf(stderr, "[umma_gemm] kind=%d conv=%d M=%d N=%d K=%d kb=%d tiles_m=%d bn=%d splitk=%d units=%d stages=%d tma_store=%d res_tma=%d nbuf=%d box=%dx%dx%d epi=%s\n",
                 L.kind, L.conv, L.M, L.N, L.K, p.k_blocks, p.tiles_m, p.bn, p.splitk, p.units_total, p.stages, p.tma_store,
-                p.res_tma, p.nbuf, p.tw, p.th, p.tb);
+                p.res_tma, p.nbuf, p.tw, p.th, p.tb, epi_name(epi));
+    if (is_wide(p.bn) && !is_plain_f32(epi)) return RTEN_ERR_UNSUPPORTED_VALUE;  // (an output / residual map failed to encode)
     const size_t smem_bytes = (size_t)p.stages * p.stage_bytes +
                               (is_wide(p.bn) ? WIDE_SMEM_FIXED_BYTES : ps.n_stg * STG_BYTES + SMEM_FIXED_BYTES);
-    // specialised epilogue when every chunk qualifies for the register fast path
-    const EpilogueDesc& ee = L.epi;
-    bool fastk = p.tma_store && (L.N % 32) == 0 && !getenv("RTEN_B200_NO_FAST");
-    if (L.kind == 0)
-        fastk = fastk && ee.bias_kind != 2 && (ee.r == nullptr || p.res_tma) &&
-                (ee.bias_kind != 1 || (reinterpret_cast<uintptr_t>(ee.bias) & 15) == 0);
-    else  // integer: column vectors must be 128-bit loadable, zero-point / scale vectors per column or scalar
-        fastk = fastk && ee.bias_kind != 2 && (ee.r == nullptr || p.res_tma) &&
-                (ee.bias_kind != 1 || (reinterpret_cast<uintptr_t>(ee.bias) & 15) == 0) &&
-                (!(ee.za || ee.za8) || (reinterpret_cast<uintptr_t>(ee.colsum) & 15) == 0) &&
-                (!ee.zb || ee.zb_len == 1 || (ee.zb_len == L.N && (reinterpret_cast<uintptr_t>(ee.zb) & 15) == 0)) &&
-                (!ee.scale || ee.scale_len == 1 || (ee.scale_len == L.N && (reinterpret_cast<uintptr_t>(ee.scale) & 15) == 0));
-    // the generic epilogue takes a TMA-staged residual only on its register path (f32, act <= Relu)
-    if (!fastk && (L.kind == 1 || ee.act > 1)) p.res_tma = 0;
-    bool plain;
-    if (L.kind == 0)
-        plain = fastk && plain_f32_ok(ctx, L, p.tma_store, p.res_tma);
-    else  // integer kind: the *ToFloat operators with a scalar (or no) activation zero point and symmetric weights
-        plain = fastk && ee.scale && !ee.za && !ee.zb && (ee.scale_len == 1 || ee.scale_len == L.N) && ee.act <= 3 && p.splitk == 1 &&
-                (ee.r == nullptr || p.res_tma) && (!ee.za8 || ee.colsum) && !getenv("RTEN_B200_NO_PLAIN");
-    // epilogue variant (umma_gemm_kernel): 0 generic, 1 specialised, 2 specialised + out-of-line Gelu; plain: 3 / 5 (f32),
-    // 4 / 6 (integer)
-    const bool gelu = ee.act > 1;
-    const int fast = !fastk ? 0 : !plain ? (gelu ? 2 : 1) : L.kind == 0 ? (gelu ? 5 : 3) : (gelu ? 6 : 4);
     using Kernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, KParams);
-    Kernel kern;
-    if (is_wide(p.bn)) {
-        if (fast != 3 && fast != 5) return RTEN_ERR_UNSUPPORTED_VALUE;  // (an output / residual map failed to encode)
-        kern = fast == 5 ? umma_wide_kernel<5> : umma_wide_kernel<3>;
-    } else {
-        switch (L.kind * 8 + fast) {
-            case 0: kern = umma_gemm_kernel<0, 0>; break;
-            case 1: kern = umma_gemm_kernel<0, 1>; break;
-            case 2: kern = umma_gemm_kernel<0, 2>; break;
-            case 3: kern = umma_gemm_kernel<0, 3>; break;
-            case 5: kern = umma_gemm_kernel<0, 5>; break;
-            case 8: kern = umma_gemm_kernel<1, 0>; break;
-            case 9: kern = umma_gemm_kernel<1, 1>; break;
-            case 10: kern = umma_gemm_kernel<1, 2>; break;
-            case 12: kern = umma_gemm_kernel<1, 4>; break;
-            default: kern = umma_gemm_kernel<1, 6>; break;
-        }
-    }
+    // [kind][variant]: the integer kind has no plain f32 kernels, the f32 kind no plain integer ones
+    static const Kernel narrow[2][7] = {
+        {umma_gemm_kernel<0, Epi::Generic>, umma_gemm_kernel<0, Epi::Fast>, umma_gemm_kernel<0, Epi::FastGelu>,
+         umma_gemm_kernel<0, Epi::PlainF32>, umma_gemm_kernel<0, Epi::PlainF32Gelu>, nullptr, nullptr},
+        {umma_gemm_kernel<1, Epi::Generic>, umma_gemm_kernel<1, Epi::Fast>, umma_gemm_kernel<1, Epi::FastGelu>, nullptr,
+         nullptr, umma_gemm_kernel<1, Epi::PlainI8>, umma_gemm_kernel<1, Epi::PlainI8Gelu>}};
+    const Kernel kern = !is_wide(p.bn)              ? narrow[L.kind][(int)epi]
+                        : epi == Epi::PlainF32Gelu ? umma_wide_kernel<Epi::PlainF32Gelu>
+                                                   : umma_wide_kernel<Epi::PlainF32>;
 
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));

@@ -57,12 +57,6 @@ struct HaloParams {
     EpilogueDesc epi;
 };
 
-// (a0, a1) += (b0, b1) on f32 bit patterns, each half rounded to nearest like a scalar add
-__device__ __forceinline__ void add_pair(uint32_t& a0, uint32_t& a1, float b0, float b1) {
-    a0 = __float_as_uint(__fadd_rn(__uint_as_float(a0), b0));
-    a1 = __float_as_uint(__fadd_rn(__uint_as_float(a1), b1));
-}
-
 __device__ __forceinline__ void halo_unit(const HaloParams& p, int u, int& n0, int& oy0, int& b0) {
     const int nt = u % p.units_n;
     const int rest = u / p.units_n;
@@ -251,8 +245,8 @@ umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
 #pragma unroll
                     for (int j = 0; j < 32; j += 4) {
                         const float4 bb = bq[j >> 2];
-                        add_pair(v[j], v[j + 1], bb.x, bb.y);
-                        add_pair(v[j + 2], v[j + 3], bb.z, bb.w);
+                        add_f32x2(v[j], v[j + 1], bb.x, bb.y);
+                        add_f32x2(v[j + 2], v[j + 3], bb.z, bb.w);
                         if (do_relu) {
 #pragma unroll
                             for (int w = 0; w < 4; w++) v[j + w] = __float_as_uint(fmaxf(__uint_as_float(v[j + w]), 0.0f));

@@ -49,6 +49,10 @@ struct FastDiv {
     }
 };
 
+// Epilogue variants of umma_gemm_kernel (umma_epilogue.cuh); the host picks one per launch (pick_epilogue).  The wide
+// kernel runs the plain f32 epilogue only.
+enum class Epi { Generic, Fast, FastGelu, PlainF32, PlainF32Gelu, PlainI8, PlainI8Gelu };
+
 struct KParams {
     int M, N, K, z0, z1;
     int tiles_m, tiles_n, tiles_total;
@@ -107,16 +111,20 @@ __device__ __forceinline__ TileCoord decode_tile(const KParams& p, int t) {
     return c;
 }
 
-// (a0, a1) += (b0, b1) on f32 bit patterns, each half rounded to nearest like a scalar add
-__device__ __forceinline__ void add_f32x2(uint32_t& a0, uint32_t& a1, float b0, float b1) {
-    a0 = __float_as_uint(__fadd_rn(__uint_as_float(a0), b0));
-    a1 = __float_as_uint(__fadd_rn(__uint_as_float(a1), b1));
+// The 4-D output / residual TMA coordinates of column `col` of a tile: (n, x, y, image) for conv, (n, m, z0, z1) else.
+__device__ __forceinline__ int4 out_coord(const KParams& p, const TileCoord& tc, int col) {
+    return p.conv ? make_int4(tc.n0 + col, tc.ox0, tc.oy0, tc.b0) : make_int4(tc.n0 + col, tc.m0, tc.z0, tc.z1);
 }
 
-// (a0, a1) *= (b0, b1) on f32 bit patterns, each half rounded to nearest like a scalar multiply
-__device__ __forceinline__ void mul_f32x2(uint32_t& a0, uint32_t& a1, float b0, float b1) {
-    a0 = __float_as_uint(__fmul_rn(__uint_as_float(a0), b0));
-    a1 = __float_as_uint(__fmul_rn(__uint_as_float(a1), b1));
+// Two columns of the plain f32 epilogue, shared by both kernels: x = (acc + residual) + bias, each add rounded to
+// nearest, then Relu (Gelu follows on four columns at a time, act4).
+__device__ __forceinline__ void plain_f32_pair(uint32_t& v0, uint32_t& v1, bool res, float2 rr, float2 bb, bool relu) {
+    if (res) add_f32x2(v0, v1, rr.x, rr.y);
+    add_f32x2(v0, v1, bb.x, bb.y);
+    if (relu) {
+        v0 = __float_as_uint(fmaxf(__uint_as_float(v0), 0.0f));
+        v1 = __float_as_uint(fmaxf(__uint_as_float(v1), 0.0f));
+    }
 }
 
 // cp.async.bulk.wait_group.read takes an immediate: leave at most `n` of this thread's bulk stores un-read
@@ -222,8 +230,7 @@ struct SmemLayout {
 
 }  // namespace rtb
 
-#include "umma_epilogue_plain.cuh"
-#include "umma_epilogue_generic.cuh"
+#include "umma_epilogue.cuh"
 
 namespace rtb {
 
@@ -409,11 +416,9 @@ __device__ __forceinline__ void kernel_setup(const SmemLayout& L) {
     asm volatile("bar.sync 15, %0;" ::"r"(NUM_THREADS) : "memory");  // 12 warps wait, the producer warp only arrives
 }
 
-// One CTA per SM walks the work units blockIdx.x, blockIdx.x + gridDim.x, ... in every role.  FAST selects the epilogue
-// (umma_epilogue_plain.cuh / umma_epilogue_generic.cuh): 0 generic, every edge case; 1 specialised, every chunk takes the
-// register fast path (TMA-store output, N % 32 == 0, column vectors and residual vector-addressable); 2 = 1 with the
-// out-of-line Gelu; 3 / 5 plain f32 (+ Gelu); 4 / 6 plain integer *ToFloat (+ Gelu).
-template <int KIND, int FAST>
+// One CTA per SM walks the work units blockIdx.x, blockIdx.x + gridDim.x, ... in every role.  E selects the epilogue
+// variant (umma_epilogue.cuh).
+template <int KIND, Epi E>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 umma_gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                  const __grid_constant__ CUtensorMap tma_d, const __grid_constant__ CUtensorMap tma_r,
@@ -434,7 +439,6 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     const int worker = (int)blockIdx.x, n_workers = (int)gridDim.x;
     const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
     // Control warps run their loops WARP-UNIFORMLY (all 32 lanes wait on the barriers, one elected lane issues the
     // TMA / MMA instructions): addresses and descriptors then live in uniform registers instead of being moved
     // there (R2UR) for every instruction, which is what bounds a single issuing thread.
@@ -447,24 +451,13 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
         else
             mma_role<KIND, 64>(p, L, worker, n_workers);
     } else {
-        // ===================== epilogue warps
-        uint8_t* stg_base = L.smem + (size_t)p.stages * p.stage_bytes;
-        const EpiCtx c{p, L, stg_base, p.nbuf, L.acc_full, L.acc_empty, L.res_bar, L.sk_flag, &tma_d, &tma_r, L.acc_smem,
-                       worker, n_workers, warp, lane};
-        if (KIND == 0 && (FAST == 3 || FAST == 5))
-            epilogue_plain_f32<FAST>(c);
-        else if (KIND == 1 && (FAST == 4 || FAST == 6))
-            epilogue_plain_i8<FAST>(c);
-        else if (FAST)
-            epilogue_fast<KIND, FAST>(c);
-        else
-            epilogue_generic<KIND>(c);
+        epilogue<KIND, E>(p, L, &tma_d, &tma_r, worker, n_workers);
     }
 }
 
 // ------------------------------------------------------------------------------------------
 // Wide tiles: one 128 x 128 or 128 x 256 tile per work unit, for the launches that take the plain f32 epilogue
-// (FAST = 3, + Gelu: 5) without split-K.  A 64-column tile cannot keep the tensor core busy: every m64nNk8 reads
+// (Epi::PlainF32, PlainF32Gelu) without split-K.  A 64-column tile cannot keep the tensor core busy: every m64nNk8 reads
 // 2 KB of A from shared memory for N/2 clocks of math, and the fixed cost of a pipeline stage is as large as its
 // tensor work.  A wide tile reads A once for up to 256 columns.  Its accumulator (up to 256 f32 registers per
 // thread of one warpgroup) does not fit the narrow kernel's role layout, so this kernel has its own:
@@ -506,9 +499,9 @@ __device__ __forceinline__ SmemLayout carve_wide_smem(uint8_t* smem_raw, const K
 
 // Main loop and epilogue of one consumer warpgroup (wg = 0: rows 0-63, 1: rows 64-127).  Each 128-byte K block is four
 // k8 wgmma, one commit group, one group in flight across stages as in mma_units; a stage goes back to the producer
-// once both warpgroups have retired it (8 warp arrivals).  Epilogue: x = act((acc + residual) + bias), each add
-// rounded to nearest, in the order of epilogue_plain_f32 -- the results equal the narrow kernel's.
-template <int FAST, int N>
+// once both warpgroups have retired it (8 warp arrivals).  Epilogue: plain_f32_pair, then act4 for Gelu, as in the
+// narrow kernel's PlainF32 variant -- the results equal the narrow kernel's.
+template <Epi E, int N>
 __device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout& L, const CUtensorMap* tma_d,
                                               const CUtensorMap* tma_r, int worker, int n_workers) {
     const int t = threadIdx.x - 128;  // 0-255 over both warpgroups
@@ -528,10 +521,8 @@ __device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout
     auto load_residual = [&](const TileCoord& tc, int c0, int buf) {
         uint64_t* rb = &L.res_bar[buf];
         mbar_expect_tx(rb, p.res_tx_bytes);
-        if (p.conv)
-            tma_load_4d(stg0 + buf * STG_BYTES, tma_r, rb, tc.n0 + c0, tc.ox0, tc.oy0, tc.b0);
-        else
-            tma_load_4d(stg0 + buf * STG_BYTES, tma_r, rb, tc.n0 + c0, tc.m0, tc.z0, tc.z1);
+        const int4 x = out_coord(p, tc, c0);
+        tma_load_4d(stg0 + buf * STG_BYTES, tma_r, rb, x.x, x.y, x.z, x.w);
     };
     for (int u = worker; u < p.units_total; u += n_workers) {
         {  // (the tile is decoded again after the main loop: its coordinates would hold registers through it)
@@ -597,19 +588,13 @@ __device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout
 #pragma unroll
                     for (int h = 0; h < 2; h++) {
                         uint32_t v0 = __float_as_uint(d[i0 + 2 * h]), v1 = __float_as_uint(d[i0 + 2 * h + 1]);
-                        if (p.res_tma) {
-                            const float2 rr = *px[h];
-                            add_f32x2(v0, v1, rr.x, rr.y);
-                        }
-                        add_f32x2(v0, v1, bb.x, bb.y);
-                        if (e.act == 1) {
-                            v0 = __float_as_uint(fmaxf(__uint_as_float(v0), 0.0f));
-                            v1 = __float_as_uint(fmaxf(__uint_as_float(v1), 0.0f));
-                        }
+                        float2 rr = make_float2(0.f, 0.f);
+                        if (p.res_tma) rr = *px[h];
+                        plain_f32_pair(v0, v1, p.res_tma, rr, bb, e.act == 1);
                         d[i0 + 2 * h] = __uint_as_float(v0);
                         d[i0 + 2 * h + 1] = __uint_as_float(v1);
                     }
-                    if (FAST == 5) {  // Gelu / ApproxGelu: the out-of-line polynomial, four values per call
+                    if (E == Epi::PlainF32Gelu) {  // Gelu / ApproxGelu: the out-of-line polynomial, four values per call
                         const float4 g = act4(make_float4(d[i0], d[i0 + 1], d[i0 + 2], d[i0 + 3]), e.act);
                         d[i0] = g.x;
                         d[i0 + 1] = g.y;
@@ -623,10 +608,8 @@ __device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout
             fence_proxy_async();
             consumers_sync();
             if (issuer) {
-                if (p.conv)
-                    tma_store_4d(tma_d, stg, nbase, tc.ox0, tc.oy0, tc.b0);
-                else
-                    tma_store_4d(tma_d, stg, nbase, tc.m0, tc.z0, tc.z1);
+                const int4 x = out_coord(p, tc, 32 * k);
+                tma_store_4d(tma_d, stg, x.x, x.y, x.z, x.w);
                 asm volatile("cp.async.bulk.commit_group;" ::: "memory");
             }
         }
@@ -634,7 +617,7 @@ __device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout
     if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
 
-template <int FAST>
+template <Epi E>
 __global__ void __launch_bounds__(WIDE_THREADS, 1)
 umma_wide_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                  const __grid_constant__ CUtensorMap tma_d, const __grid_constant__ CUtensorMap tma_r,
@@ -670,10 +653,10 @@ umma_wide_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
     } else {
         asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
         // (Gelu: 128 columns only -- the out-of-line act4 calls would spill around 128 live accumulators per thread)
-        if (FAST == 5 || p.bn == 128)
-            wide_consumer<FAST, 128>(p, L, &tma_d, &tma_r, (int)blockIdx.x, (int)gridDim.x);
+        if (E == Epi::PlainF32Gelu || p.bn == 128)
+            wide_consumer<E, 128>(p, L, &tma_d, &tma_r, (int)blockIdx.x, (int)gridDim.x);
         else
-            wide_consumer<FAST, 256>(p, L, &tma_d, &tma_r, (int)blockIdx.x, (int)gridDim.x);
+            wide_consumer<E, 256>(p, L, &tma_d, &tma_r, (int)blockIdx.x, (int)gridDim.x);
     }
 }
 
