@@ -218,7 +218,16 @@ rten_status rten_b200_quantized_linear(rten_ctx* ctx, const rten_tensor* x, cons
  * q_seq = 1 (decode) with head size 64 / 128 is ONE kernel: scores, softmax and the value product stream the cache once,
  * split over the sequence to fill the SMs.  `new_key` / `new_value` [batch, kv_heads, 1, head] (optional) are written
  * into the caches at position nonpad_kv_seqlen[b] - 1 by the same kernel first (the cache append of rten-generate,
- * rten-generate/src/generator.rs:858-886, without a separate launch).  Other shapes compose MatMul / Softmax / MatMul. */
+ * rten-generate/src/generator.rs:858-886, without a separate launch).
+ * q_seq > 1 with is_causal, nonpad_kv_seqlen or q_heads != kv_heads (prompt / chunked prefill): ONE streaming kernel
+ * with the scores kept on chip, for device-resident f32 tensors of head size 64 / 128 (value head size equal), the
+ * head dimension contiguous in query, key and out, value with either of its last two dimensions contiguous, and any
+ * attn_mask with a contiguous key dimension.  Query row s attends to keys 0 ..= s + offset when causal (offset =
+ * valid_b - q_seq with nonpad_kv_seqlen, 0 without) and to keys below valid_b otherwise, where valid_b =
+ * clamp(nonpad_kv_seqlen[b], 0, total_seq): read on the device, an out-of-range entry is clamped, not reported.  Both
+ * products follow the context's f32 mode: 3xTF32 (default) or one TF32 pass.  Query head h reads kv head
+ * h / (q_heads / kv_heads).  Other shapes compose MatMul / Softmax / MatMul; causal, padded or grouped-query calls with
+ * q_seq > 1 that the kernel cannot take fail with RTEN_ERR_UNSUPPORTED_VALUE. */
 typedef struct {
     int32_t is_causal;
     int32_t q_num_heads;  /* informative for 4-D inputs */

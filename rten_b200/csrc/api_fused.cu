@@ -12,6 +12,7 @@
 
 #include "api_util.h"
 #include "attn_fused.h"
+#include "attn_prefill.h"
 #include "rowops.h"
 #include "skinny.h"
 
@@ -28,6 +29,32 @@ rten_tensor empty_tensor() {
     rten_tensor t;
     memset(&t, 0, sizeof(t));
     return t;
+}
+
+// a 4-D [b, h, s, d] tensor as the (d, s, h, b) operand of a TMA map, or (s, d, h, b) when `transposed` (key dimension
+// contiguous: a value tensor stored transposed)
+OperandDesc attn_operand(const rten_tensor* t, bool transposed) {
+    OperandDesc d;
+    d.base = t->data;
+    d.dims[0] = transposed ? t->shape[2] : t->shape[3];
+    d.dims[1] = transposed ? t->shape[3] : t->shape[2];
+    d.dims[2] = t->shape[1];
+    d.dims[3] = t->shape[0];
+    d.strides[0] = 1;
+    d.strides[1] = transposed ? t->strides[3] : t->strides[2];
+    d.strides[2] = t->strides[1];
+    d.strides[3] = t->strides[0];
+    return d;
+}
+
+// An output a one-kernel attention branch allocated but cannot write (its layout does not fit the kernel): back to the
+// pool, so that the branches below start from the caller's `out` as it was.
+void give_back_output(rten_ctx* ctx, OpScope& sc, rten_tensor* out, const rten_tensor& ov) {
+    if (out->data == ov.data && sc.allocated.size()) {
+        pool_free(ctx, ov.data);
+        out->data = nullptr;
+        sc.allocated.clear();
+    }
 }
 
 }  // namespace
@@ -265,28 +292,15 @@ rten_status rten_b200_attention(rten_ctx* ctx, const rten_tensor* query, const r
         L.q_seq = (int)qs;
         L.kv_seq = (int)total;
         L.dh = (int)dh;
-        auto od = [&](const rten_tensor* t, bool transposed) {
-            OperandDesc d;
-            d.base = t->data;
-            d.dims[0] = transposed ? t->shape[2] : t->shape[3];
-            d.dims[1] = transposed ? t->shape[3] : t->shape[2];
-            d.dims[2] = t->shape[1];
-            d.dims[3] = t->shape[0];
-            d.strides[0] = 1;
-            d.strides[1] = transposed ? t->strides[3] : t->strides[2];
-            d.strides[2] = t->strides[1];
-            d.strides[3] = t->strides[0];
-            return d;
-        };
-        L.q = od(query, false);
-        L.k = od(key, false);
+        L.q = attn_operand(query, false);
+        L.k = attn_operand(key, false);
         if (value->strides[3] == 1 && value->strides[2] != 1) {  // natural layout: the kernel transposes the tile itself
             L.v = (const float*)value->data;
             L.v_b = value->strides[0];
             L.v_h = value->strides[1];
             L.v_s = value->strides[2];
         } else {
-            L.vt = od(value, true);
+            L.vt = attn_operand(value, true);
         }
         L.mask = attn_mask ? (const float*)attn_mask->data : nullptr;
         L.m_b = ms[0];
@@ -301,11 +315,46 @@ rten_status rten_b200_attention(rten_ctx* ctx, const rten_tensor* query, const r
             L.o_h = ov.strides[1];
             L.o_s = ov.strides[2];
             if (ov.strides[3] == 1 && attn_fused_supported(L)) return sc.finish(launch_attn_fused(ctx, L));
-            if (out->data == ov.data && sc.allocated.size()) {  // allocated here but not usable: give it back, compose below
-                pool_free(ctx, ov.data);
-                out->data = nullptr;
-                sc.allocated.clear();
-            }
+            give_back_output(ctx, sc, out, ov);  // compose below
+        }
+        st = sc.finish(st);
+        if (st != RTEN_OK) return st;
+    }
+    // ---- causal, right-padded (nonpad_kv_seqlen) or grouped-query calls with q_seq > 1: the streaming prefill kernel
+    // (head size 64 / 128, f32 products in the context's mode); other layouts keep the errors below
+    if (qs > 1 && resident && !new_key && (prm->is_causal || nonpad_kv_seqlen || qh != kvh) && dv == dh && (dh == 64 || dh == 128) &&
+        query->strides[3] == 1 && key->strides[3] == 1 && (value->strides[2] == 1 || value->strides[3] == 1) &&
+        (!attn_mask || ms[3] == 1 || total == 1) && (!nonpad_kv_seqlen || nonpad_kv_seqlen->strides[0] == 1 || B == 1)) {
+        AttnPrefillLaunch L;
+        L.B = (int)B;
+        L.q_heads = (int)qh;
+        L.kv_heads = (int)kvh;
+        L.q_seq = (int)qs;
+        L.kv_seq = (int)total;
+        L.dh = (int)dh;
+        L.q = attn_operand(query, false);
+        L.k = attn_operand(key, false);
+        L.v_natural = value->strides[3] == 1;
+        L.v = attn_operand(value, !L.v_natural);
+        L.len = nonpad_kv_seqlen ? (const int32_t*)nonpad_kv_seqlen->data : nullptr;
+        L.causal = prm->is_causal ? 1 : 0;
+        L.mask = attn_mask ? (const float*)attn_mask->data : nullptr;
+        L.m_b = ms[0];
+        L.m_h = ms[1];
+        L.m_s = ms[2];
+        L.scale = scale;
+        L.x3 = ctx->f32_mode == RTEN_F32_TF32 ? 0 : 1;
+        OpScope sc(ctx);
+        rten_tensor ov;
+        const int64_t oshape[4] = {B, qh, qs, dh};
+        rten_status st = sc.out(out, RTEN_F32, 4, oshape, &ov, nullptr);
+        if (st == RTEN_OK) {
+            L.out = (float*)ov.data;
+            L.o_b = ov.strides[0];
+            L.o_h = ov.strides[1];
+            L.o_s = ov.strides[2];
+            if (ov.strides[3] == 1 && attn_prefill_supported(L)) return sc.finish(launch_attn_prefill(ctx, L));
+            give_back_output(ctx, sc, out, ov);
         }
         st = sc.finish(st);
         if (st != RTEN_OK) return st;

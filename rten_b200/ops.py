@@ -404,7 +404,13 @@ class QuantizedLinear:
 
 
 class Attention:
-    """src/ops/attention.rs:645-905 (ONNX `Attention`) on 4-D inputs; attributes as the reference's."""
+    """src/ops/attention.rs:645-905 (ONNX `Attention`) on 4-D inputs; attributes as the reference's.
+
+    q_seq == 1 runs the decode kernel.  q_seq > 1 with `is_causal`, `nonpad_kv_seqlen` or q_heads != kv_heads runs the
+    streaming prefill kernel (device tensors, head size 64 or 128): causal row s attends to keys 0 ..= s + offset, with
+    offset = valid - q_seq when `nonpad_kv_seqlen` is given (valid = nonpad_kv_seqlen[b] clamped to [0, total_seq] on
+    the device) and 0 otherwise; query head h reads kv head h // (q_heads // kv_heads); fully masked rows are zeros.  Its
+    products follow the context's f32 mode (3xTF32 by default, one TF32 pass after `set_f32_mode(False)`)."""
 
     def __init__(self, is_causal=False, kv_num_heads=None, q_num_heads=None, scale: Optional[float] = None, softcap: float = 0.0):
         self.is_causal, self.kv_num_heads, self.q_num_heads, self.scale, self.softcap = is_causal, kv_num_heads, q_num_heads, scale, softcap
