@@ -160,6 +160,20 @@ rten_status rten_b200_matmul_integer_ex(rten_ctx* ctx, const rten_tensor* a, con
                                         const rten_tensor* bias, const rten_tensor* residual, int activation,
                                         rten_tensor* out_range_or_null, rten_tensor* out);
 
+/* MatMulNBits (src/ops/matmul/contrib.rs:21-195, ONNX Runtime's com.microsoft.MatMulNBits): a f32 [..., M, K] (at
+ * least 2 dims, the leading dims flatten into rows) times a 4-bit block-quantized B: b u8 [N, k_blocks, blob_bytes] with
+ * block = 2 * blob_bytes elements (a power of two >= 16), byte j of a block holding element 2j in its low nibble and
+ * 2j + 1 in its high nibble, zero point 8; scales f32 [N, k_blocks], or 1-D [N * k_blocks] with k_blocks =
+ * K / block_size.  out f32 [..., M, N] = a . w with w[k, n] = f32(nibble - 8) * scales[n, k / block] (one f32 rounding);
+ * K == 0 gives zeros.  Only bits = 4.  Errors as the reference's, plus RTEN_ERR_INCOMPATIBLE_SHAPES for 2-D scales that
+ * are not [N, k_blocks].  Rows = prod(leading dims) * M <= 32 (T): a streaming kernel reads every column's nibbles and
+ * scales from HBM once and computes in exact f32 FMA arithmetic; more rows: a wgmma kernel dequantizes the nibbles into
+ * its shared-memory B tiles and follows the context's f32 mode (3xTF32 default, one TF32 pass opt-in).  B is never
+ * expanded to f32 in HBM.  Device-resident a / b / scales with 16-byte aligned rows (K % 32 == 0 for b) take exactly one
+ * kernel launch and no host synchronisation (capturable in a CUDA graph); other layouts are first copied. */
+rten_status rten_b200_matmul_nbits(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, const rten_tensor* scales,
+                                   int bits, int block_size, rten_tensor* out);
+
 /* Conv (src/ops/conv.rs:124-419).  x NCHW (or NCW), w OIHW, bias [O].  pads = {top,left,bottom,right};
  * auto_pad_same != 0 => `Padding::Same` (pads ignored).  n_spatial = 1 or 2 gives the expected
  * number of stride/dilation values (error strings as the reference). */
@@ -308,7 +322,8 @@ rten_status rten_b200_scatter_rows(rten_ctx* ctx, rten_tensor* table, const rten
  * executor holds the last reference to their input (src/graph.rs:973-1049); Reshape / Flatten / Squeeze / Unsqueeze /
  * Transpose / Identity are views.  Operators: Conv, ConvInteger, Relu, MaxPool, GlobalAveragePool, ReduceMean (spatial
  * axes), Gemm, MatMul, MatMulInteger, Add, Mul, Softmax, LayerNormalization, Gelu, Erf, Gather (rows), Cast (i32 -> f32),
- * DynamicQuantizeLinear, Attention (4-D), Constant and the view operators; anything else fails the LOAD with
+ * DynamicQuantizeLinear, Attention (4-D), MatMulNBits (com.microsoft, bits 4; constant B / scales used in place),
+ * Constant and the view operators; anything else fails the LOAD with
  * RTEN_ERR_UNSUPPORTED_VALUE ("unsupported operator <name>"). */
 typedef struct rten_model rten_model;
 rten_status rten_b200_model_load(rten_ctx* ctx, const void* onnx_bytes, size_t len, rten_model** out);

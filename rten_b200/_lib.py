@@ -81,6 +81,7 @@ _SIGNATURES = {
     "rten_b200_matmul_ex": (C.c_int, [_vp, _TP, _TP, _vp, _TP, C.c_float, _TP, C.c_int, _TP]),
     "rten_b200_matmul_integer": (C.c_int, [_vp, _TP, _TP, _vp, _TP, _TP, _TP, _TP]),
     "rten_b200_matmul_integer_ex": (C.c_int, [_vp, _TP, _TP, _vp, _TP, _TP, _TP, _TP, _TP, _TP, C.c_int, _TP, _TP]),
+    "rten_b200_matmul_nbits": (C.c_int, [_vp, _TP, _TP, _TP, C.c_int, C.c_int, _TP]),
     "rten_b200_conv2d": (C.c_int, [_vp, _TP, _TP, _vp, _TP, C.POINTER(RtenConvParams), _TP]),
     "rten_b200_conv2d_ex": (C.c_int, [_vp, _TP, _TP, _vp, _TP, C.POINTER(RtenConvParams), _TP, C.c_int, _TP]),
     "rten_b200_conv_integer": (C.c_int, [_vp, _TP, _TP, _vp, _TP, _TP, _TP, C.POINTER(RtenConvParams), _TP]),

@@ -11,6 +11,7 @@
 
 #include "api_shared.h"
 #include "api_util.h"
+#include "nbits.h"
 #include "rowops.h"
 #include "skinny.h"
 #include "umma_gemm.h"
@@ -415,6 +416,141 @@ rten_status matmul_core(OpScope& sc, MatMulArgs& A, rten_tensor* out) {
     return RTEN_OK;
 }
 
+// The leading ndim - 1 dims of `t` as one row dimension of uniform stride (*rs; any value when there is one row).
+bool flat_rows(const rten_tensor& t, int64_t* rs) {
+    *rs = 0;
+    int64_t next = -1;  // stride the next outer dim must have
+    for (int i = t.ndim - 2; i >= 0; i--) {
+        if (t.shape[i] == 1) continue;
+        if (next >= 0 && t.strides[i] != next) return false;
+        if (next < 0) *rs = t.strides[i];
+        next = t.strides[i] * t.shape[i];
+    }
+    return true;
+}
+
+// src/ops/matmul/contrib.rs:21-186 (MatMulNBits): validation in the reference's order, then one kernel (nbits.cu)
+rten_status matmul_nbits(OpScope& sc, const rten_tensor* a, const rten_tensor* b, const rten_tensor* scales, int bits,
+                         int block_size, rten_tensor* out) {
+    rten_ctx* ctx = sc.ctx;
+    rten_tensor av, bv, sv;
+    RTB_TRY(sc.in(a, &av));
+    RTB_TRY(sc.in(b, &bv));
+    RTB_TRY(sc.in(scales, &sv));
+    const int64_t N = bv.shape[0];
+    // `scales` [N, k_blocks], or 1-D [N * k_blocks] with k_blocks = K / block_size (older models)
+    int64_t s_n, s_k, s_blocks;
+    if (sv.ndim == 2) {
+        s_n = sv.strides[0];
+        s_k = sv.strides[1];
+        s_blocks = sv.shape[1];
+        if (sv.shape[0] != N) s_blocks = -1;
+    } else if (sv.ndim == 1) {
+        const int64_t k = av.ndim >= 1 ? av.shape[av.ndim - 1] : 1;
+        s_blocks = block_size > 0 ? k / block_size : 0;
+        if (sv.shape[0] != N * s_blocks)
+            return fail(ctx, RTEN_ERR_INVALID_VALUE, "Expected 1D `scales` size to match columns * block_size");
+        s_k = sv.strides[0];
+        s_n = s_blocks * s_k;
+    } else {
+        return fail(ctx, RTEN_ERR_INVALID_VALUE, "Expected `scales` to have one or two dims");
+    }
+    if (av.ndim < 2) return fail(ctx, RTEN_ERR_INVALID_VALUE, "A input must have at least 2 dims");
+    if (bits != 4) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Unsupported bits-per-element");
+    const int64_t kb = bv.shape[1], blob = bv.shape[2], block = 2 * blob;
+    if (block < 16 || (block & (block - 1))) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Unsupported K block size");
+    const int64_t K = av.shape[av.ndim - 1];
+    int64_t oshape[RTEN_MAX_DIMS];
+    int64_t rows = 1;
+    for (int i = 0; i < av.ndim - 1; i++) {
+        oshape[i] = av.shape[i];
+        rows *= av.shape[i];
+    }
+    oshape[av.ndim - 1] = N;
+    if (K != kb * block)
+        return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Columns of first matrix does not match rows of second matrix");
+    // (the reference does not check this and would read past the scales)
+    if (s_blocks != kb) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "MatMulNBits: `scales` must have shape [N, k_blocks]");
+    if (rows > 0x7fffffffll || N > 0x7fffffffll || K > 0x7fffffffll)
+        return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MatMulNBits: dimension out of range");
+    rten_tensor ov;
+    RTB_TRY(sc.out(out, RTEN_F32, av.ndim, oshape, &ov, nullptr));
+    if (rows == 0 || N == 0) return RTEN_OK;
+
+    // output: [rows, N] with unit column stride, else a contiguous temporary copied back
+    int64_t o_rs;
+    rten_tensor dv = ov;
+    const bool direct = flat_rows(ov, &o_rs) && ov.strides[ov.ndim - 1] == 1;
+    if (!direct) {
+        set_contiguous(&dv);
+        void* t = nullptr;
+        RTB_TRY(temp_alloc(ctx, (size_t)(rows * N) * 4, &t));
+        dv.data = t;
+        o_rs = N;
+    }
+    if (K == 0) {  // block_quant.rs:80-84
+        RTB_CUDA(ctx, cudaMemsetAsync(dv.data, 0, (size_t)(rows * N) * 4, ctx->stream));
+    } else {
+        // A: [rows, K] with 16-byte aligned rows (K is a multiple of 16), else packed into a workspace
+        int64_t a_rs;
+        const float* ap = (const float*)av.data;
+        if (!flat_rows(av, &a_rs) || av.strides[av.ndim - 1] != 1 || (a_rs & 3) || (reinterpret_cast<uintptr_t>(ap) & 15)) {
+            float* t = nullptr;
+            RTB_TRY(temp_alloc(ctx, (size_t)(rows * K) * 4, (void**)&t));
+            long long shape[RTEN_MAX_DIMS], ss[RTEN_MAX_DIMS], ds[RTEN_MAX_DIMS];
+            rten_tensor c = av;
+            set_contiguous(&c);
+            for (int i = 0; i < av.ndim; i++) {
+                shape[i] = av.shape[i];
+                ss[i] = av.strides[i];
+                ds[i] = c.strides[i];
+            }
+            RTB_TRY(launch_nd_copy(ctx, 4, av.data, t, av.ndim, shape, ss, ds));
+            ap = t;
+            a_rs = K;
+        }
+        // B: rows of K / 2 contiguous bytes at a pitch of a multiple of 16 bytes (K % 32 == 0), else copied to one
+        const uint8_t* qp = (const uint8_t*)bv.data;
+        int64_t q_rs = N > 1 ? bv.strides[0] : K / 2;
+        const bool dense = bv.strides[2] == 1 && (kb == 1 || bv.strides[1] == blob);
+        if (!dense || (q_rs & 15) || (reinterpret_cast<uintptr_t>(qp) & 15)) {
+            const int64_t pitch = round_up(K / 2, 16);
+            void* t = nullptr;
+            RTB_TRY(temp_alloc(ctx, (size_t)(N * pitch), &t));
+            long long shape[3] = {N, kb, blob}, ss[3] = {bv.strides[0], bv.strides[1], bv.strides[2]}, ds[3] = {pitch, blob, 1};
+            RTB_TRY(launch_nd_copy(ctx, 1, bv.data, t, 3, shape, ss, ds));
+            qp = (const uint8_t*)t;
+            q_rs = pitch;
+        }
+        NbitsLaunch L;
+        L.a = ap;
+        L.as = a_rs;
+        L.q = qp;
+        L.qs = q_rs;
+        L.scales = (const float*)sv.data;
+        L.s_n = s_n;
+        L.s_k = s_k;
+        L.M = (int)rows;
+        L.N = (int)N;
+        L.K = (int)K;
+        L.block = (int)block;
+        L.x3 = ctx->f32_mode == RTEN_F32_TF32X3;
+        L.out = (float*)dv.data;
+        L.os = o_rs;
+        RTB_TRY(launch_nbits(ctx, L));
+    }
+    if (!direct) {
+        long long shape[RTEN_MAX_DIMS], ss[RTEN_MAX_DIMS], ds[RTEN_MAX_DIMS];
+        for (int i = 0; i < ov.ndim; i++) {
+            shape[i] = ov.shape[i];
+            ss[i] = dv.strides[i];
+            ds[i] = ov.strides[i];
+        }
+        RTB_TRY(launch_nd_copy(ctx, 4, dv.data, ov.data, ov.ndim, shape, ss, ds));
+    }
+    return RTEN_OK;
+}
+
 // src/ops/matmul.rs:513-533 zero_point_to_vec validation
 }  // namespace
 
@@ -580,6 +716,17 @@ rten_status rten_b200_matmul_ex(rten_ctx* ctx, const rten_tensor* a, const rten_
 rten_status rten_b200_matmul(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, const rten_packed* pb,
                              const rten_tensor* bias, float alpha, rten_tensor* out) {
     return rten_b200_matmul_ex(ctx, a, b, pb, bias, alpha, nullptr, 0, out);
+}
+
+// ---- MatMulNBits ----------------------------------------------------------------------------
+rten_status rten_b200_matmul_nbits(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, const rten_tensor* scales,
+                                   int bits, int block_size, rten_tensor* out) {
+    RTB_TRY(check_ctx(ctx));
+    if (!a || !b || !scales || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    if (a->dtype != RTEN_F32 || scales->dtype != RTEN_F32 || b->dtype != RTEN_U8 || b->ndim != 3)
+        return fail(ctx, RTEN_ERR_CAST_FAILED, "MatMulNBits: A and scales must be f32, B u8 [N, k_blocks, blob_bytes]");
+    OpScope sc(ctx);
+    return sc.finish(matmul_nbits(sc, a, b, scales, bits, block_size, out));
 }
 
 // ---- MatMulInteger / MatMulIntegerToFloat ------------------------------------------------------

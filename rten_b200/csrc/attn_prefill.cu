@@ -27,6 +27,7 @@
 #include "attn_prefill.h"
 #include "math.cuh"
 #include "ptx.cuh"
+#include "tf32_split.cuh"
 
 namespace rtb {
 
@@ -90,16 +91,6 @@ __device__ __forceinline__ void mma_block(float (&d)[N / 2], const uint8_t* a, c
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_operand(d);
-}
-
-__device__ __forceinline__ float tf32_lo(float x) { return __fsub_rn(x, __uint_as_float(__float_as_uint(x) & 0xffffe000u)); }
-
-// dst = lo(src) elementwise over `bytes` (same swizzled layout), by the 128 threads of the warpgroup
-__device__ __forceinline__ void split_lo(uint8_t* dst, const uint8_t* src, uint32_t bytes, int tid) {
-    for (uint32_t i = tid; i < bytes / 16; i += 128) {
-        const float4 x = reinterpret_cast<const float4*>(src)[i];
-        reinterpret_cast<float4*>(dst)[i] = make_float4(tf32_lo(x.x), tf32_lo(x.y), tf32_lo(x.z), tf32_lo(x.w));
-    }
 }
 
 // byte offset of element (row, col) in a stack of K-major 128B-swizzled sub-tiles of 32 columns and `rows` rows

@@ -150,7 +150,7 @@ const std::set<std::string>& supported_ops() {
     static const std::set<std::string> s = {
         "Conv", "Relu", "MaxPool", "GlobalAveragePool", "ReduceMean", "Reshape", "Flatten", "Squeeze", "Unsqueeze", "Transpose",
         "Identity", "Gemm", "MatMul", "Add", "Mul", "Softmax", "LayerNormalization", "Gelu", "Erf", "Gather",
-        "DynamicQuantizeLinear", "MatMulInteger", "ConvInteger", "Cast", "Attention", "Constant"};
+        "DynamicQuantizeLinear", "MatMulInteger", "ConvInteger", "Cast", "Attention", "MatMulNBits", "Constant"};
     return s;
 }
 
@@ -252,6 +252,10 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
             const int id = m->value_id(t.name);
             RTB_TRY(upload_constant(m.get(), t, &m->values[(size_t)id]));
             continue;
+        }
+        if (n.op_type == "MatMulNBits") {  // src/op_registry/onnx_registry.rs:1376-1402
+            if (n.attr_i("bits", 4) != 4) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MatMulNBits: only bits = 4 is supported");
+            if (!n.attr("block_size")) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MatMulNBits: missing attribute block_size");
         }
         OpNode on;
         on.n = n;
@@ -588,6 +592,11 @@ struct Runner {
             st = rten_b200_matmul(ctx, T(0), T(1), o.packed, bias, 1.0f, &y);
         } else if (op == "MatMulInteger") {
             st = rten_b200_matmul_integer(ctx, T(0), T(1), o.packed, T(2), T(3), nullptr, &y);
+        } else if (op == "MatMulNBits") {
+            // accuracy_level only sets a minimum: every level computes in f32 (src/ops/matmul/contrib.rs:104-109)
+            if (o.in.size() > 3) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "zero_points, g_idx and bias inputs are unsupported");
+            if (!T(1) || !T(2)) return mfail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+            st = rten_b200_matmul_nbits(ctx, T(0), T(1), T(2), 4, (int)o.n.attr_i("block_size", 0), &y);
         } else if (op == "Add") {
             if (!T(1)) return mfail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
             st = rten_b200_add(ctx, T(0), T(1), &y);

@@ -385,6 +385,24 @@ class MatMulIntegerToFloat(MatMul):
         return A.wrap(o, out)
 
 
+class MatMulNBits:
+    """src/ops/matmul/contrib.rs:119-195 (com.microsoft MatMulNBits): a [..., M, K] f32 times a 4-bit block-quantized
+    b u8 [N, k_blocks, block_size / 2] with f32 scales [N, k_blocks] (or 1-D [N * k_blocks]).  `accuracy_level` 0-4 is
+    accepted and, as the reference allows, every level computes in f32: the context's f32 mode for more than 32 rows,
+    exact f32 FMAs for up to 32."""
+
+    def __init__(self, bits: int = 4, block_size: int = 32, accuracy_level: int = 0):
+        if not 0 <= int(accuracy_level) <= 4:
+            raise OpError(5, "accuracy_level must be 0-4")
+        self.bits, self.block_size, self.accuracy_level = int(bits), int(block_size), int(accuracy_level)
+
+    def run(self, ctx, a, b, scales, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        ctx.check(ctx.lib.rten_b200_matmul_nbits(ctx.handle, A.t(a), A.t(b), A.t(scales), self.bits, self.block_size, C.byref(o)))
+        return A.wrap(o, out)
+
+
 class QuantizedLinear:
     """[LayerNormalization] -> DynamicQuantizeLinear -> Mul -> MatMulIntegerToFloat -> Add(bias) -> Add(residual) -> activation
     as one call (rten_b200_quantized_linear): the skinny-M decode kernel for <= 16 rows, the operator chain otherwise;
