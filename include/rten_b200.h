@@ -254,6 +254,65 @@ rten_status rten_b200_attention(rten_ctx* ctx, const rten_tensor* query, const r
                                 const rten_attention_params* params, const rten_tensor* new_key_or_null,
                                 const rten_tensor* new_value_or_null, rten_tensor* out);
 
+/* RotaryEmbedding (src/ops/embedding.rs:46-252, the ai.onnx operator): input f32 [batch, seq, hidden] (num_heads heads of
+ * hidden / num_heads) or [batch, heads, seq, head] with any strides; the first rotary_embedding_dim elements of every head
+ * (0: the whole head) are rotated, the rest copied.  cos / sin [batch|1, seq|1, dim / 2], or with position_ids i32
+ * [batch|1, seq|1] tables [max_pos, dim / 2] gathered by position.  Pairs (2i, 2i + 1) when interleaved, else
+ * (i, i + dim / 2); y1 = x1 cos - x2 sin, y2 = x1 sin + x2 cos with each product and sum rounded to f32 on its own (no
+ * fused multiply-add: bit-identical to a float32 restatement).  out has the input's shape and must not overlap it.
+ * Host-resident position_ids are checked (the reference's Gather error); device-resident ones are clamped to
+ * [0, max_pos - 1] on the device, nothing is reported.  One kernel launch. */
+rten_status rten_b200_rotary_embedding(rten_ctx* ctx, const rten_tensor* input, const rten_tensor* cos, const rten_tensor* sin,
+                                       const rten_tensor* position_ids_or_null, int interleaved, int num_heads,
+                                       int rotary_embedding_dim, rten_tensor* out);
+
+/* GroupQueryAttention (com.microsoft; src/ops/attention/contrib.rs:369-417, :438-810): the attention operator of ONNX
+ * Runtime's int4 LLM exports.  query [B, S, H * D], key / value [B, S, Hkv * D] (both NULL: query is packed QKV
+ * [B, S, (H + 2 Hkv) * D]); past_key / past_value [B, Hkv, P, D] (optional); seqlens_k i32 [B] or [B, 1] = total length
+ * - 1; total_sequence_length i32 scalar; cos / sin [max_pos, rotary_dim / 2] and position_ids i32 [B, S] for do_rotary;
+ * attention_bias [B|1, H|1, >= S, >= P + S] added to the scores.  Outputs: out [B, S, H * D] and the present caches
+ * present_key / present_value [B, Hkv, P + S, D].
+ * S == total_sequence_length is a first prompt (past_len(b) = 0); otherwise past_len(b) = seqlens_k[b] + 1 - S, and S > 1
+ * needs B == 1.  Q and the new K are rotated (rotary_dim = 2 cos.shape[1] <= D, interleaved pairs or halves, the
+ * RotaryEmbedding arithmetic above) at position position_ids[b, s], else past_len(b) + s.  The present cache holds
+ * past[b, :, :past_len(b)], then the S new tokens, then zeros.  Query row s attends to keys [start, past_len(b) + s + 1)
+ * with start = past_len(b) + s + 1 - local_window_size when local_window_size > 0 and that is positive, else 0; query
+ * head h reads kv head h / (H / Hkv); scale <= 0 means 1 / sqrt(D).
+ * In-place present cache (the reference's run_in_place): present_key / present_value whose data pointer and strides
+ * equal past_key's / past_value's (the past buffer, with room for S more positions) receive only the new tokens; the
+ * prefix is already there and positions past past_len(b) + S are left untouched.  Otherwise (data == NULL or another
+ * buffer) the present cache is built whole, zeros included.  A present cache that overlaps a past cache's memory without
+ * being that buffer (same data pointer and strides) fails with RTEN_ERR_UNSUPPORTED_OUTPUT.
+ * Host-resident seqlens_k / position_ids are checked with the reference's errors; device-resident ones are read only on
+ * the device (seqlens_k clamped to [S - 1, P + S - 1], positions to [0, max_pos - 1], nothing reported), so a step is a
+ * fixed launch list.  total_sequence_length decides the prompt kind and is read on the host: if it is device-resident
+ * that is one synchronous 4-byte copy, and such a call cannot be captured in a CUDA graph.
+ * Paths (head size 64 or 128, device-resident tensors with 16-byte aligned rows and contiguous heads):
+ *  - decode step (S == 1, not a first prompt), P + 1 <= 8192: ONE single-query kernel launch rotates q and the new key
+ *    itself, appends the new key / value to the present caches and streams them once -- plus one launch that copies the
+ *    past prefix when the present caches are not the past buffers and P > 0.
+ *  - prompts: the rotary / append kernel (rotated Q to a scratch, new K / V into the present caches) and the streaming
+ *    prefill attention kernel (causal, key tiles below every row's window skipped), products in the context's f32 mode
+ *    -- plus the past-prefix launch as above.
+ * Other head sizes, longer decode caches and softcap > 0 fail with RTEN_ERR_UNSUPPORTED_VALUE; there is no composed
+ * fallback.  (smooth_softmax and head_sink are not parameters: the reference rejects them.) */
+typedef struct {
+    int32_t num_heads;
+    int32_t kv_num_heads;
+    float scale;               /* <= 0: 1 / sqrt(head size) */
+    int32_t do_rotary;
+    int32_t rotary_interleaved;
+    int32_t local_window_size; /* <= 0: no sliding window */
+    float softcap;             /* > 0 unsupported */
+} rten_gqa_params;
+rten_status rten_b200_group_query_attention(rten_ctx* ctx, const rten_tensor* query, const rten_tensor* key_or_null,
+                                            const rten_tensor* value_or_null, const rten_tensor* past_key_or_null,
+                                            const rten_tensor* past_value_or_null, const rten_tensor* seqlens_k,
+                                            const rten_tensor* total_sequence_length, const rten_tensor* cos_or_null,
+                                            const rten_tensor* sin_or_null, const rten_tensor* position_ids_or_null,
+                                            const rten_tensor* attention_bias_or_null, const rten_gqa_params* params,
+                                            rten_tensor* out, rten_tensor* present_key, rten_tensor* present_value);
+
 /* Softmax (src/ops/norm.rs:825-899) and AddSoftmax (src/ops/attention.rs:30-165) when mask != NULL
  * (mask broadcast to x, added lane-wise before the softmax over `axis`; AddSoftmax uses axis -1).
  * `out` may alias `x` (= run_in_place). */
@@ -323,6 +382,8 @@ rten_status rten_b200_scatter_rows(rten_ctx* ctx, rten_tensor* table, const rten
  * Transpose / Identity are views.  Operators: Conv, ConvInteger, Relu, MaxPool, GlobalAveragePool, ReduceMean (spatial
  * axes), Gemm, MatMul, MatMulInteger, Add, Mul, Softmax, LayerNormalization, Gelu, Erf, Gather (rows), Cast (i32 -> f32),
  * DynamicQuantizeLinear, Attention (4-D), MatMulNBits (com.microsoft, bits 4; constant B / scales used in place),
+ * RotaryEmbedding, GroupQueryAttention (com.microsoft; output and present_key / present_value, inputs 12-15 rejected;
+ * the executor allocates new present caches, so each decode step also copies the past: two launches, not one),
  * Constant and the view operators; anything else fails the LOAD with
  * RTEN_ERR_UNSUPPORTED_VALUE ("unsupported operator <name>"). */
 typedef struct rten_model rten_model;

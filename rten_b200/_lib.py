@@ -49,6 +49,11 @@ class RtenAttentionParams(C.Structure):
                 ("softcap", C.c_float)]
 
 
+class RtenGqaParams(C.Structure):
+    _fields_ = [("num_heads", C.c_int32), ("kv_num_heads", C.c_int32), ("scale", C.c_float), ("do_rotary", C.c_int32),
+                ("rotary_interleaved", C.c_int32), ("local_window_size", C.c_int32), ("softcap", C.c_float)]
+
+
 _TP = C.POINTER(RtenTensor)
 _vp = C.c_void_p
 
@@ -87,6 +92,9 @@ _SIGNATURES = {
     "rten_b200_conv_integer": (C.c_int, [_vp, _TP, _TP, _vp, _TP, _TP, _TP, C.POINTER(RtenConvParams), _TP]),
     "rten_b200_quantized_linear": (C.c_int, [_vp, _TP, _TP, _TP, C.c_float, _TP, _vp, _TP, _TP, _TP, _TP, C.c_int, _TP]),
     "rten_b200_attention": (C.c_int, [_vp, _TP, _TP, _TP, _TP, _TP, C.POINTER(RtenAttentionParams), _TP, _TP, _TP]),
+    "rten_b200_rotary_embedding": (C.c_int, [_vp, _TP, _TP, _TP, _TP, C.c_int, C.c_int, C.c_int, _TP]),
+    "rten_b200_group_query_attention": (C.c_int, [_vp, _TP, _TP, _TP, _TP, _TP, _TP, _TP, _TP, _TP, _TP, _TP,
+                                                  C.POINTER(RtenGqaParams), _TP, _TP, _TP]),
     "rten_b200_softmax": (C.c_int, [_vp, _TP, _TP, C.c_int, C.c_int, _TP]),
     "rten_b200_layer_norm": (C.c_int, [_vp, _TP, _TP, _TP, C.c_int, C.c_float, _TP]),
     "rten_b200_erf": (C.c_int, [_vp, _TP, _TP]),

@@ -54,7 +54,7 @@ struct Cfg {
 
 struct AttnPrefillParams {
     int heads, group, q_seq, kv_seq, q_tiles;
-    int v_natural, causal;
+    int v_natural, causal, window;
     const int32_t* len;
     const float* mask;
     long long m_b, m_h, m_s;
@@ -147,15 +147,17 @@ attn_prefill_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_cons
     int kend = p.causal ? min(lim, min(q0 + BM, p.q_seq) + off) : lim;
     kend = max(kend, 0);
     const int ntiles = (kend + BN - 1) / BN;
+    // sliding window: row s sees no key below s + off + 1 - window; tiles wholly below the first row's window are skipped
+    const int jlo = p.window > 0 ? min(max(q0 + off + 1 - p.window, 0) / BN, ntiles) : 0;
 
     if (warp == 4) {
         if (elect_one()) {
             mbar_expect_tx(bar_q, C::QT);
 #pragma unroll
             for (int c = 0; c < DH / 32; c++) tma_load_4d(sq + c * BM * 128, &tma_q, bar_q, c * 32, q0, h, b);
-            for (int j = 0; j < ntiles; j++) {
-                const int s = j % NS;
-                if (j >= NS) mbar_wait(&empty[s], ((j / NS) - 1) & 1);
+            for (int j = jlo; j < ntiles; j++) {
+                const int it = j - jlo, s = it % NS;
+                if (it >= NS) mbar_wait(&empty[s], ((it / NS) - 1) & 1);
                 mbar_expect_tx(&full[s], C::KT + C::VT);
                 uint8_t* dk = sk + s * C::KT;
                 uint8_t* dv = sv + s * C::VT;
@@ -179,6 +181,7 @@ attn_prefill_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_cons
     const int row0 = q0 + rl0, row1 = row0 + 8;
     const int lim0 = p.causal ? min(lim, row0 + off + 1) : lim;
     const int lim1 = p.causal ? min(lim, row1 + off + 1) : lim;
+    const int lo0 = p.window > 0 ? row0 + off + 1 - p.window : 0, lo1 = p.window > 0 ? row1 + off + 1 - p.window : 0;
     const float* mrow0 = nullptr;
     const float* mrow1 = nullptr;
     if (p.mask) {
@@ -195,14 +198,14 @@ attn_prefill_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_cons
     mbar_wait(bar_q, 0);
     if constexpr (X3) split_lo(sq_lo, sq, C::QT, tid);
 
-    for (int j = 0; j < ntiles; j++) {
-        const int s = j % NS;
+    for (int j = jlo; j < ntiles; j++) {
+        const int s = (j - jlo) % NS;
         const uint8_t* tk = sk + s * C::KT;
         const uint8_t* tv = sv + s * C::VT;
-        mbar_wait(&full[s], (j / NS) & 1);
+        mbar_wait(&full[s], ((j - jlo) / NS) & 1);
         if (X3 || p.v_natural) {
             // every warp's products of the previous tile have completed before its operands are overwritten
-            if (j > 0) asm volatile("bar.sync 1, 128;" ::: "memory");
+            if (j > jlo) asm volatile("bar.sync 1, 128;" ::: "memory");
             if constexpr (X3) split_lo(sk_lo, tk, C::KT, tid);
             if (p.v_natural) {
                 // V tile (key row, d column) -> V^T tile (d row, key column); 32 lanes write 32 keys of one row of V^T
@@ -237,7 +240,7 @@ attn_prefill_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_cons
         for (int i = 0; i < BN / 2; i++) {
             const bool r1 = (i >> 1) & 1;
             const int key = key0 + 8 * (i >> 2) + (i & 1);
-            const bool ok = key < (r1 ? lim1 : lim0);
+            const bool ok = key < (r1 ? lim1 : lim0) && key >= (r1 ? lo1 : lo0);
             float z = __fmul_rn(sc[i], p.scale);
             if (mrow0 && ok) z = __fadd_rn(z, __ldg((r1 ? mrow1 : mrow0) + key));
             z = ok ? z : -INFINITY;
@@ -341,6 +344,7 @@ rten_status launch_cfg(rten_ctx* ctx, const AttnPrefillLaunch& L, const AttnPref
 
 bool attn_prefill_supported(const AttnPrefillLaunch& L) {
     if (L.dh != 64 && L.dh != 128) return false;
+    if (L.window < 0) return false;
     if (L.B < 1 || L.q_heads < 1 || L.kv_heads < 1 || L.q_heads % L.kv_heads || L.q_seq < 1 || L.kv_seq < 1) return false;
     if ((long long)L.B * L.q_heads * ((L.q_seq + BM - 1) / BM) > 0x7fffffffll) return false;
     auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
@@ -359,6 +363,7 @@ rten_status launch_attn_prefill(rten_ctx* ctx, const AttnPrefillLaunch& L) {
     p.q_tiles = (L.q_seq + BM - 1) / BM;
     p.v_natural = L.v_natural ? 1 : 0;
     p.causal = L.causal ? 1 : 0;
+    p.window = L.window;
     p.len = L.len;
     p.mask = L.mask;
     p.m_b = L.m_b;

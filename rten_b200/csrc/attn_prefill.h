@@ -19,6 +19,7 @@ struct AttnPrefillLaunch {
     bool v_natural = true;
     const int32_t* len = nullptr;  // nonpad_kv_seqlen [B] (read on the device) or null
     int causal = 0;
+    int window = 0;  // > 0: keys t < s + offset + 1 - window are masked too (sliding window; key tiles wholly below skipped)
     const float* mask = nullptr;  // additive, element strides m_b / m_h / m_s (0 = broadcast), key dimension contiguous
     long long m_b = 0, m_h = 0, m_s = 0;
     float scale = 1.0f;

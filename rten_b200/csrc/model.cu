@@ -8,6 +8,9 @@
 //          returned to the context pool after their last consumer (src/graph.rs:1100-1180); an operator that can run in
 //          place does so when the executor holds the last reference to its input (src/graph.rs:973-1049); shape-only
 //          operators (Reshape, Flatten, Squeeze, Unsqueeze, Transpose, Identity) are views -- no kernel, no copy.
+// Operators: Conv, ConvInteger, Relu, MaxPool, GlobalAveragePool, ReduceMean, Gemm, MatMul, MatMulInteger, MatMulNBits
+// (com.microsoft), Add, Mul, Softmax, LayerNormalization, Gelu, Erf, Gather, Cast, DynamicQuantizeLinear, Attention,
+// RotaryEmbedding, GroupQueryAttention (com.microsoft, three outputs), Constant and the view operators.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -150,7 +153,8 @@ const std::set<std::string>& supported_ops() {
     static const std::set<std::string> s = {
         "Conv", "Relu", "MaxPool", "GlobalAveragePool", "ReduceMean", "Reshape", "Flatten", "Squeeze", "Unsqueeze", "Transpose",
         "Identity", "Gemm", "MatMul", "Add", "Mul", "Softmax", "LayerNormalization", "Gelu", "Erf", "Gather",
-        "DynamicQuantizeLinear", "MatMulInteger", "ConvInteger", "Cast", "Attention", "MatMulNBits", "Constant"};
+        "DynamicQuantizeLinear", "MatMulInteger", "ConvInteger", "Cast", "Attention", "MatMulNBits", "GroupQueryAttention",
+        "RotaryEmbedding", "Constant"};
     return s;
 }
 
@@ -257,6 +261,15 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
             if (n.attr_i("bits", 4) != 4) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MatMulNBits: only bits = 4 is supported");
             if (!n.attr("block_size")) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MatMulNBits: missing attribute block_size");
         }
+        if (n.op_type == "GroupQueryAttention") {  // src/op_registry/onnx_registry.rs:1467-1492, contrib.rs:817-821
+            if (n.domain != "com.microsoft") return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "unsupported operator GroupQueryAttention");
+            if (!n.attr("num_heads") || !n.attr("kv_num_heads"))
+                return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "GroupQueryAttention: missing attribute num_heads or kv_num_heads");
+            if (n.inputs.size() > 12)
+                return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "GroupQueryAttention: quantization and Q/K norm inputs (12-15) are not supported");
+        }
+        if (n.op_type == "RotaryEmbedding" && n.domain == "com.microsoft")
+            return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "unsupported operator com.microsoft.RotaryEmbedding");
         OpNode on;
         on.n = n;
         for (const std::string& s : n.inputs) {
@@ -651,6 +664,31 @@ struct Runner {
             p.softcap = o.n.attr_f("softcap", 0.0f);
             if (T(4) || T(5)) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Attention: past_key / past_value inputs are not supported by the executor");
             st = rten_b200_attention(ctx, T(0), T(1), T(2), T(3), T(6), &p, nullptr, nullptr, &y);
+        } else if (op == "RotaryEmbedding") {
+            if (!T(1) || !T(2)) return mfail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+            st = rten_b200_rotary_embedding(ctx, T(0), T(1), T(2), T(3), (int)o.n.attr_i("interleaved", 0), (int)o.n.attr_i("num_heads", 0),
+                                            (int)o.n.attr_i("rotary_embedding_dim", 0), &y);
+        } else if (op == "GroupQueryAttention") {
+            if (T(11)) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "head_sink is not supported");
+            if (o.n.attr_i("smooth_softmax", 0)) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "smooth_softmax is not supported");
+            rten_gqa_params p;
+            memset(&p, 0, sizeof(p));
+            p.num_heads = (int32_t)o.n.attr_i("num_heads", 0);
+            p.kv_num_heads = (int32_t)o.n.attr_i("kv_num_heads", 0);
+            p.scale = o.n.attr_f("scale", 0.0f);
+            p.do_rotary = (int32_t)o.n.attr_i("do_rotary", 0);
+            p.rotary_interleaved = (int32_t)o.n.attr_i("rotary_interleaved", 0);
+            p.local_window_size = (int32_t)o.n.attr_i("local_window_size", -1);
+            p.softcap = o.n.attr_f("softcap", 0.0f);
+            if (!T(5) || !T(6)) return mfail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+            rten_tensor pk, pv;
+            memset(&pk, 0, sizeof(pk));
+            memset(&pv, 0, sizeof(pv));
+            st = rten_b200_group_query_attention(ctx, T(0), T(1), T(2), T(3), T(4), T(5), T(6), T(7), T(8), T(9), T(10), &p, &y, &pk, &pv);
+            if (st == RTEN_OK) {
+                if (o.out.size() > 1 && o.out[1] >= 0) set_owned(o.out[1], pk); else pool_free(ctx, pk.data);
+                if (o.out.size() > 2 && o.out[2] >= 0) set_owned(o.out[2], pv); else pool_free(ctx, pv.data);
+            }
         } else {
             return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "unsupported operator " + op);
         }

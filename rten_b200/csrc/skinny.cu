@@ -12,6 +12,7 @@
 #include <cstdlib>
 
 #include "math.cuh"
+#include "rotary.cuh"
 #include "rowmath.cuh"
 #include "skinny.h"
 
@@ -581,10 +582,11 @@ rten_status launch_skinny_f32(rten_ctx* ctx, const SkinnyF32Launch& L) {
 // requested in one burst and consumed afterwards.
 // =========================================================================================
 struct AttnDecodeParams {
-    AttnDecodeLaunch L;
+    AttnDecodeCore L;
     int nsplit;
     float* ws;  // [B * q_heads][nsplit][2 + dh]  partial (max, sum, unnormalised output)
     int* cnt;   // [B * q_heads] arrival counters (zero between launches)
+    AttnDecodeExt X;
 };
 
 constexpr int ATTN_CHUNK = 128;  // cached positions per CTA (eight warps; the six-warp variant covers 96)
@@ -593,7 +595,9 @@ constexpr int ATTN_CHUNK = 128;  // cached positions per CTA (eight warps; the s
 // (444 on the chip) and 192-thread CTAs four (592): the launcher takes the variant whose grid needs fewer waves -- GPT-2's
 // 96 (batch x head) pairs over a 576-position cache are 480 CTAs of 8 warps (two waves, the second nearly empty) or 576 of 6
 // (one wave).
-template <int DH, int NW>
+// EXT: the GroupQueryAttention features of AttnDecodeLaunch (len stride / offset / floor, sliding window, rotary
+// embedding); without them the kernel is the plain Attention decode kernel, compiled from the same code as before.
+template <int DH, int NW, bool EXT>
 __global__ void __launch_bounds__(NW * 32, DH == 64 ? (NW == 8 ? 3 : 4) : 1) attn_decode_kernel(const AttnDecodeParams p) {
     // Every warp owns 16 consecutive cached positions of the CTA's chunk and runs the whole attention on them by itself
     // (scores, local max, exponentials, local sum, value product): no block barrier until the warps' partial
@@ -602,7 +606,9 @@ __global__ void __launch_bounds__(NW * 32, DH == 64 ? (NW == 8 ? 3 : 4) : 1) att
     __shared__ float s_m[NW], s_s[NW];
     __shared__ float s_o[NW][DH];
     __shared__ int s_last;
-    const AttnDecodeLaunch& L = p.L;
+    __shared__ __align__(16) float s_rot[EXT ? 2 : 1][EXT ? DH : 4];  // rotated q and new key row (EXT)
+    const AttnDecodeCore& L = p.L;
+    const AttnDecodeExt& X = p.X;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int bh = blockIdx.x / p.nsplit, split = blockIdx.x - bh * p.nsplit;
     const int b = bh / L.q_heads, h = bh - b * L.q_heads;
@@ -610,22 +616,34 @@ __global__ void __launch_bounds__(NW * 32, DH == 64 ? (NW == 8 ? 3 : 4) : 1) att
     const int hk = h / group;
     pdl_wait();
     pdl_launch_dependents();
-    int len = L.len ? L.len[b] : L.kv_cap;
-    len = max(0, min(len, L.kv_cap));
-    const int per = ((len + p.nsplit - 1) / p.nsplit + 3) & ~3;  // multiple of 4: 16-byte aligned rows of a transposed V
-    const int l0 = min(len, split * per), l1 = min(len, l0 + per);
+    int len, lo = 0;
+    if constexpr (EXT) {
+        len = L.len ? L.len[(long long)b * X.len_s] : L.kv_cap;
+        len = max(X.len_min, min(len, L.kv_cap - X.len_add) + X.len_add);
+        lo = X.window > 0 ? max(0, len - X.window) : 0;
+    } else {
+        len = L.len ? L.len[b] : L.kv_cap;
+        len = max(0, min(len, L.kv_cap));
+    }
+    // the splits cover [base, len): base = the window's first position rounded down to 4, the `skip` < 4 positions of
+    // the first split below the window are loaded but masked (window: natural value layout only)
+    const int base = lo & ~3;
+    const int per = ((len - base + p.nsplit - 1) / p.nsplit + 3) & ~3;  // multiple of 4: 16-byte aligned rows of a transposed V
+    const int l0 = min(len, base + split * per), l1 = min(len, l0 + per);
     const int nl = l1 - l0;      // <= ATTN_CHUNK (the launcher picks nsplit accordingly)
+    const int skip = EXT ? max(0, lo - l0) : 0;
     const int w0 = warp * 16;    // first position of this warp inside the chunk
     float* kc = L.k + (long long)b * L.k_b + (long long)hk * L.k_h;
     float* vc = L.v + (long long)b * L.v_b + (long long)hk * L.v_h;
     const float* knew = L.k_new ? L.k_new + (long long)b * L.kn_b + (long long)hk * L.kn_h : nullptr;
     const float* vnew = L.v_new ? L.v_new + (long long)b * L.vn_b + (long long)hk * L.vn_h : nullptr;
+    const float* qrow = L.q + (long long)b * L.q_b + (long long)h * L.q_h;
     // ---- everything this warp will need is requested here: K rows (8 lanes per position, DH / 8 floats per lane) ...
     constexpr int PER_LANE = DH / 8;
     constexpr int NV4 = PER_LANE / 4;
     const int sub = lane >> 3, l8 = lane & 7;
     float4 kreg[4][NV4], qreg[NV4];
-    const float4* q4 = reinterpret_cast<const float4*>(L.q + (long long)b * L.q_b + (long long)h * L.q_h + l8 * PER_LANE);
+    const float4* q4 = reinterpret_cast<const float4*>(qrow + l8 * PER_LANE);
 #pragma unroll
     for (int j = 0; j < NV4; j++) qreg[j] = q4[j];
 #pragma unroll
@@ -661,6 +679,37 @@ __global__ void __launch_bounds__(NW * 32, DH == 64 ? (NW == 8 ? 3 : 4) : 1) att
             }
         }
     }
+    if constexpr (EXT) {
+        if (X.rot_cos) {
+            // rotary embedding, while the loads above are in flight: every CTA rotates its query row, and a CTA that
+            // reads position len - 1 the new key row (through shared memory: a row's pairs span lanes)
+            int pos = X.rot_pos ? X.rot_pos[(long long)b * X.rot_pos_b] : len - 1;
+            pos = min(max(pos, 0), X.rot_max_pos - 1);
+            const float* c = X.rot_cos + (long long)pos * X.rot_half;
+            const float* sn = X.rot_sin + (long long)pos * X.rot_half;
+            const bool own_new = knew && l1 == len && nl > 0;
+            if (tid < DH) {
+                s_rot[0][tid] = rotary_elem(qrow, 1, tid, c, sn, X.rot_half, X.rot_interleaved);
+                if (own_new) s_rot[1][tid] = rotary_elem(knew, 1, tid, c, sn, X.rot_half, X.rot_interleaved);
+            }
+            __syncthreads();
+            const float4* rq4 = reinterpret_cast<const float4*>(s_rot[0] + l8 * PER_LANE);
+#pragma unroll
+            for (int j = 0; j < NV4; j++) qreg[j] = rq4[j];
+            if (own_new) {
+                knew = s_rot[1];
+                const float4* rk4 = reinterpret_cast<const float4*>(knew + l8 * PER_LANE);
+#pragma unroll
+                for (int it = 0; it < 4; it++) {
+                    const int i = w0 + it * 4 + sub;
+                    if (i < nl && l0 + i == len - 1) {
+#pragma unroll
+                        for (int j = 0; j < NV4; j++) kreg[it][j] = rk4[j];
+                    }
+                }
+            }
+        }
+    }
     // fused cache append: the split that owns position len - 1 writes the new key / value there (one CTA per kv head:
     // the query heads of a group share the cache row; every reader of that position takes k_new / v_new instead)
     if (knew && len > 0 && l1 == len && nl > 0 && (h % group) == 0 && tid < DH) {
@@ -687,7 +736,7 @@ __global__ void __launch_bounds__(NW * 32, DH == 64 ? (NW == 8 ? 3 : 4) : 1) att
         s += __shfl_xor_sync(0xffffffffu, s, 4);
         s += __shfl_xor_sync(0xffffffffu, s, 2);
         s += __shfl_xor_sync(0xffffffffu, s, 1);
-        if (i < nl) {
+        if (i >= skip && i < nl) {
             s *= L.scale;
             if (mrow) s += mrow[(long long)(l0 + i) * L.m_l];
             mw = fmaxf(mw, s);
@@ -701,7 +750,7 @@ __global__ void __launch_bounds__(NW * 32, DH == 64 ? (NW == 8 ? 3 : 4) : 1) att
 #pragma unroll
     for (int it = 0; it < 4; it++) {
         const int i = w0 + it * 4 + sub;
-        const float e = i < nl ? reduced_range_exp(sc[it] - mw) : 0.0f;
+        const float e = (i >= skip && i < nl) ? reduced_range_exp(sc[it] - mw) : 0.0f;
         sw += e;
         if (l8 == 0) s_pw[warp][it * 4 + sub] = e;
     }
@@ -740,7 +789,7 @@ __global__ void __launch_bounds__(NW * 32, DH == 64 ? (NW == 8 ? 3 : 4) : 1) att
         for (int j = 0; j < CH; j++) a[j] = 0.0f;
 #pragma unroll
         for (int i = 0; i < 16; i++) {
-            if (w0 + i < nl) {
+            if (w0 + i >= skip && w0 + i < nl) {
                 const float pw = s_pw[warp][i];
 #pragma unroll
                 for (int j = 0; j < CH; j++) a[j] = fmaf(pw, vnat[i][j], a[j]);
@@ -819,6 +868,9 @@ bool attn_decode_supported(const AttnDecodeLaunch& L) {
     if (!al16(L.q) || (L.q_b & 3) || (L.q_h & 3)) return false;
     if (L.k_new && (!al16(L.k_new) || (L.kn_b & 3) || (L.kn_h & 3) || !L.v_new)) return false;
     if (L.v_l != 1 && L.v_d != 1) return false;
+    if (L.rot_cos && (!L.rot_sin || L.rot_half < 0 || 2 * L.rot_half > L.dh || L.rot_max_pos < 1)) return false;
+    if (L.window < 0 || L.len_min < 0 || L.len_add < 0 || L.len_min > L.kv_cap) return false;
+    if (L.window > 0 && L.v_l == 1) return false;  // the sliding window masks within the natural value layout only
     if (L.v_l == 1 && (!al16(L.v) || (L.v_b & 3) || (L.v_h & 3) || (L.v_d & 3))) return false;  // float4 along the positions
     return true;
 }
@@ -826,7 +878,9 @@ bool attn_decode_supported(const AttnDecodeLaunch& L) {
 rten_status launch_attn_decode(rten_ctx* ctx, const AttnDecodeLaunch& L) {
     AttnDecodeParams p;
     p.L = L;
+    p.X = L;
     const int bh = L.B * L.q_heads;
+    const bool ext = L.rot_cos || L.window > 0 || L.len_s != 1 || L.len_add || L.len_min;
     // a split covers at most `chunk` positions (rounded to 4); more splits when (batch x heads) alone leaves SMs idle
     auto splits_for = [&](int chunk) {
         int ns = (L.kv_cap + chunk - 1) / chunk;
@@ -873,8 +927,13 @@ rten_status launch_attn_decode(rten_ctx* ctx, const AttnDecodeLaunch& L) {
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = getenv("RTEN_B200_NO_PDL") ? 0 : 1;
-    cudaError_t e = L.dh == 64 ? (nw == 6 ? cudaLaunchKernelEx(&cfg, attn_decode_kernel<64, 6>, p) : cudaLaunchKernelEx(&cfg, attn_decode_kernel<64, 8>, p))
-                               : cudaLaunchKernelEx(&cfg, attn_decode_kernel<128, 8>, p);
+    cudaError_t e;
+    if (ext)
+        e = L.dh == 64 ? (nw == 6 ? cudaLaunchKernelEx(&cfg, attn_decode_kernel<64, 6, true>, p) : cudaLaunchKernelEx(&cfg, attn_decode_kernel<64, 8, true>, p))
+                       : cudaLaunchKernelEx(&cfg, attn_decode_kernel<128, 8, true>, p);
+    else
+        e = L.dh == 64 ? (nw == 6 ? cudaLaunchKernelEx(&cfg, attn_decode_kernel<64, 6, false>, p) : cudaLaunchKernelEx(&cfg, attn_decode_kernel<64, 8, false>, p))
+                       : cudaLaunchKernelEx(&cfg, attn_decode_kernel<128, 8, false>, p);
     if (e != cudaSuccess) return fail_cuda(ctx, e, "attention launch");
     e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(ctx, e, "attention launch");

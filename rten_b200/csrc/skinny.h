@@ -60,8 +60,9 @@ rten_status launch_skinny_f32(rten_ctx* ctx, const SkinnyF32Launch& L);
 
 // Single-query attention (q_seq = 1) over a cache of `kv_cap` positions of which len[b] are valid:
 //   out[b, h, :] = softmax(scale * q[b, h, :] . K[b, hk, l, :] (+ mask[b, h, l]))_{l < len[b]} . V[b, hk, l, :]
-// Optional fused cache append: k_new / v_new [B, kv_heads, dh] are written at position len[b] - 1 first.
-struct AttnDecodeLaunch {
+// Optional fused cache append: k_new / v_new [B, kv_heads, dh] are written at position len[b] - 1 first, k_new rotated
+// like q when a rotary table is given.
+struct AttnDecodeCore {
     int B = 0, q_heads = 0, kv_heads = 0, dh = 0, kv_cap = 0;
     const float* q = nullptr;  // element strides: q_b, q_h (dh contiguous)
     long long q_b = 0, q_h = 0;
@@ -80,6 +81,20 @@ struct AttnDecodeLaunch {
     float* out = nullptr;  // strides o_b, o_h (dh contiguous)
     long long o_b = 0, o_h = 0;
 };
+// GroupQueryAttention's additions; with their defaults the plain kernel runs, compiled from the same code as before
+struct AttnDecodeExt {
+    long long len_s = 1;           // element stride of len
+    int len_add = 0, len_min = 0;  // valid positions = clamp(len[b * len_s] + len_add, len_min, kv_cap)
+    int window = 0;                // > 0: positions below (valid positions) - window are masked (natural value layout only)
+    // rotary embedding of q and k_new at position rot_pos[b * rot_pos_b] (null: valid positions - 1), clamped to
+    // [0, rot_max_pos - 1]; rot_cos / rot_sin [rot_max_pos, rot_half] contiguous, null = no rotation
+    const float* rot_cos = nullptr;
+    const float* rot_sin = nullptr;
+    int rot_half = 0, rot_interleaved = 0, rot_max_pos = 0;
+    const int32_t* rot_pos = nullptr;
+    long long rot_pos_b = 0;
+};
+struct AttnDecodeLaunch : AttnDecodeCore, AttnDecodeExt {};
 bool attn_decode_supported(const AttnDecodeLaunch& L);
 rten_status launch_attn_decode(rten_ctx* ctx, const AttnDecodeLaunch& L);
 

@@ -18,7 +18,7 @@ from typing import Optional, Sequence
 import numpy as np
 
 from . import _lib
-from ._lib import RTEN_DEVICE_HOST, RTEN_F32, RTEN_I8, RTEN_I32, RTEN_U8, RtenAttentionParams, RtenConvParams, RtenTensor
+from ._lib import RTEN_DEVICE_HOST, RTEN_F32, RTEN_I8, RTEN_I32, RTEN_U8, RtenAttentionParams, RtenConvParams, RtenGqaParams, RtenTensor
 
 _NP2RT = {np.dtype(np.float32): RTEN_F32, np.dtype(np.int32): RTEN_I32, np.dtype(np.int8): RTEN_I8,
           np.dtype(np.uint8): RTEN_U8}
@@ -443,6 +443,53 @@ class Attention:
         ctx.check(ctx.lib.rten_b200_attention(ctx.handle, A.t(query), A.t(key), A.t(value), A.t(attn_mask), A.t(nonpad_kv_seqlen),
                                               C.byref(p), A.t(new_key), A.t(new_value), C.byref(o)))
         return A.wrap(o, out)
+
+
+class RotaryEmbedding:
+    """src/ops/embedding.rs:209-252 (ai.onnx RotaryEmbedding): input [batch, seq, hidden] (`num_heads` heads) or
+    [batch, heads, seq, head]; cos / sin [batch|1, seq|1, dim / 2], or [max_pos, dim / 2] tables gathered by
+    `position_ids`.  Rotated values equal a float32 restatement bit for bit (no fused multiply-add)."""
+
+    def __init__(self, interleaved: bool = False, num_heads: int = 0, rotary_embedding_dim: int = 0):
+        self.interleaved, self.num_heads, self.rotary_embedding_dim = bool(interleaved), int(num_heads), int(rotary_embedding_dim)
+
+    def run(self, ctx, input, cos, sin, position_ids=None, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        ctx.check(ctx.lib.rten_b200_rotary_embedding(ctx.handle, A.t(input), A.t(cos), A.t(sin), A.t(position_ids), int(self.interleaved),
+                                                     self.num_heads, self.rotary_embedding_dim, C.byref(o)))
+        return A.wrap(o, out)
+
+
+class GroupQueryAttention:
+    """src/ops/attention/contrib.rs:419-810 (com.microsoft GroupQueryAttention); attribute names and defaults as the
+    reference's.  Decode steps (one query, not a first prompt) run the single-query attention kernel with the rotary
+    embedding and the cache append fused in; prompts run the rotary / append kernel and the streaming prefill kernel."""
+
+    def __init__(self, num_heads: int, kv_num_heads: int, scale: Optional[float] = None, do_rotary: bool = False,
+                 rotary_interleaved: bool = False, local_window_size: int = -1, softcap: float = 0.0, smooth_softmax: bool = False):
+        self.num_heads, self.kv_num_heads, self.scale = int(num_heads), int(kv_num_heads), scale
+        self.do_rotary, self.rotary_interleaved = bool(do_rotary), bool(rotary_interleaved)
+        self.local_window_size, self.softcap, self.smooth_softmax = int(local_window_size), float(softcap), bool(smooth_softmax)
+
+    def run(self, ctx, query, key, value, seqlens_k, total_sequence_length, past_key=None, past_value=None, cos_cache=None,
+            sin_cache=None, position_ids=None, attention_bias=None, out=None, present_key=None, present_value=None):
+        """Returns (output, present_key, present_value).  `key` / `value` None: `query` is packed QKV.  `present_key` /
+        `present_value` may be views of the `past_key` / `past_value` buffers (same data pointer and strides, S more
+        positions): then only the new tokens are written into them."""
+        if self.smooth_softmax:
+            raise OpError(6, "smooth_softmax is not supported")
+        A = _Args(ctx)
+        o, pk, pv = A.out(out), A.out(present_key), A.out(present_value)
+        p = RtenGqaParams(self.num_heads, self.kv_num_heads, float(self.scale) if self.scale else 0.0, int(self.do_rotary),
+                          int(self.rotary_interleaved), self.local_window_size, self.softcap)
+        total = total_sequence_length
+        if not isinstance(total, (DeviceTensor, np.ndarray)):
+            total = np.asarray(total, np.int32)
+        ctx.check(ctx.lib.rten_b200_group_query_attention(
+            ctx.handle, A.t(query), A.t(key), A.t(value), A.t(past_key), A.t(past_value), A.t(seqlens_k), A.t(total), A.t(cos_cache),
+            A.t(sin_cache), A.t(position_ids), A.t(attention_bias), C.byref(p), C.byref(o), C.byref(pk), C.byref(pv)))
+        return A.wrap(o, out), A.wrap(pk, present_key), A.wrap(pv, present_value)
 
 
 def _conv_params(padding, groups, strides, dilations) -> RtenConvParams:
