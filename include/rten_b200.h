@@ -194,6 +194,17 @@ rten_status rten_b200_conv2d_ex(rten_ctx* ctx, const rten_tensor* x, const rten_
                                 const rten_packed* packed_w_or_null, const rten_tensor* bias_or_null,
                                 const rten_conv_params* p, const rten_tensor* residual_or_null, int activation,
                                 rten_tensor* out);
+/* Extension: act(Conv(x, w, bias, p) + Conv(x_proj, w_proj, bias_proj, p_proj)) -- the ONNX pattern Conv, Conv -> Add
+   (-> Relu) of a residual block with a projection shortcut.  Both outputs must have the same shape
+   (RTEN_ERR_INCOMPATIBLE_SHAPES); all tensors are f32 (RTEN_ERR_UNSUPPORTED_TYPE); otherwise the checks of conv2d_ex.
+   Two 1x1 convolutions (groups 1, no padding or dilation) over channels-last, 16-byte addressable inputs whose channel
+   counts are multiples of 32 run as one GEMM over both inputs, and the projection is never written; any other pair
+   runs as the two calls conv2d_ex(x_proj) and conv2d_ex(x, residual = that result). */
+rten_status rten_b200_conv2d_projected(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w,
+                                       const rten_packed* packed_w_or_null, const rten_tensor* bias_or_null,
+                                       const rten_conv_params* p, const rten_tensor* x_proj, const rten_tensor* w_proj,
+                                       const rten_packed* packed_w_proj_or_null, const rten_tensor* bias_proj_or_null,
+                                       const rten_conv_params* p_proj, int activation, rten_tensor* out);
 /* ConvInteger (src/ops/conv.rs:421-533); scale_or_null != NULL => ConvIntegerToFloat (:535-587). */
 rten_status rten_b200_conv_integer(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w,
                                    const rten_packed* packed_w_or_null, const rten_tensor* x_zero_point_or_null,

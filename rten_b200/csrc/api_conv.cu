@@ -45,16 +45,31 @@ rten_status pack_conv_weight(rten_ctx* ctx, const rten_tensor* w, int esize, voi
     return launch_nd_copy(ctx, esize, w->data, dst, 4, shape, ss, ds);
 }
 
-rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
+// Validated geometry of one convolution (2-D form: a 1-D convolution is a 2-D one over a height-1 image).
+struct ConvShape {
+    rten_tensor x, w, bias_v;
+    bool one_d = false;
+    int64_t strides[2], dil[2];
+    int64_t B, C, H, W, O, Cg, kh, kw, OH, OW, pt, pb, pl, pr, Og;
+    int groups;
+};
+
+rten_status conv_shape(OpScope& sc, const ConvArgs& A, ConvShape& S) {
     rten_ctx* ctx = sc.ctx;
     const rten_conv_params* cp = A.p;
-    rten_tensor x, w;
+    rten_tensor& x = S.x;
+    rten_tensor& w = S.w;
     RTB_TRY(sc.in(A.x, &x));
     RTB_TRY(sc.in(A.w, &w));
     // 1-D convolution via 2-D (conv.rs:142-185)
-    const bool one_d = x.ndim == 3;
+    const bool one_d = S.one_d = x.ndim == 3;
     int64_t pads_in[4] = {cp->pads[0], cp->pads[1], cp->pads[2], cp->pads[3]};
-    int64_t strides[2] = {cp->strides[0], cp->strides[1]}, dil[2] = {cp->dilations[0], cp->dilations[1]};
+    int64_t* strides = S.strides;
+    int64_t* dil = S.dil;
+    strides[0] = cp->strides[0];
+    strides[1] = cp->strides[1];
+    dil[0] = cp->dilations[0];
+    dil[1] = cp->dilations[1];
     if (one_d) {
         if (w.ndim != 3) return fail(ctx, RTEN_ERR_INVALID_VALUE, "input must have 3 dims (OCW)");
         if (cp->n_strides != 1) return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected 1 stride value");
@@ -81,24 +96,57 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
         if (cp->n_strides != 2) return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected 2 stride values");
         if (cp->n_dilations != 2) return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected 2 dilation values");
     }
-    const int64_t B = x.shape[0], C = x.shape[1], H = x.shape[2], W = x.shape[3];
-    const int64_t O = w.shape[0], Cg = w.shape[1], kh = w.shape[2], kw = w.shape[3];
-    rten_tensor bias_v;
+    const int64_t B = S.B = x.shape[0], C = S.C = x.shape[1], H = S.H = x.shape[2], W = S.W = x.shape[3];
+    const int64_t O = S.O = w.shape[0], Cg = S.Cg = w.shape[1], kh = S.kh = w.shape[2], kw = S.kw = w.shape[3];
+    (void)B;
     if (A.bias) {
-        RTB_TRY(sc.in(A.bias, &bias_v));
-        if (bias_v.ndim != 1 || bias_v.shape[0] != O)
+        RTB_TRY(sc.in(A.bias, &S.bias_v));
+        if (S.bias_v.ndim != 1 || S.bias_v.shape[0] != O)
             return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "bias.size(0) != out_channels");
     }
-    int64_t OH, OW, pt, pb, pl, pr;
-    RTB_TRY(axis_out(ctx, H, kh, strides[0], cp->auto_pad_same != 0, pads_in[0], pads_in[2], dil[0], &OH, &pt, &pb));
-    RTB_TRY(axis_out(ctx, W, kw, strides[1], cp->auto_pad_same != 0, pads_in[1], pads_in[3], dil[1], &OW, &pl, &pr));
-    const int groups = cp->groups;
+    RTB_TRY(axis_out(ctx, H, kh, strides[0], cp->auto_pad_same != 0, pads_in[0], pads_in[2], dil[0], &S.OH, &S.pt, &S.pb));
+    RTB_TRY(axis_out(ctx, W, kw, strides[1], cp->auto_pad_same != 0, pads_in[1], pads_in[3], dil[1], &S.OW, &S.pl, &S.pr));
+    const int groups = S.groups = cp->groups;
     if (groups == 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Group count must be > 0");
     if (groups < 0 || C % groups != 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Input channel count not divisible by groups");
     if (C / groups != Cg)
         return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Input channels (per group) does not match kernel input channels");
     if (O % groups != 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Output channel count not divisible by groups");
-    const int64_t Og = O / groups;
+    S.Og = O / groups;
+    return RTEN_OK;
+}
+
+// Weights as [O, kh, kw, C]: the prepacked handle, or packed per call (the reference prepacks per call too)
+rten_status conv_weight(rten_ctx* ctx, const ConvArgs& A, const ConvShape& S, int esize, const void** wp,
+                        const int32_t** colsum) {
+    *colsum = nullptr;
+    if (A.pw) {
+        if (A.pw->kind != 1 || A.pw->O != S.O || A.pw->Cg != S.Cg || A.pw->kh != S.kh || A.pw->kw != S.kw)
+            return fail(ctx, RTEN_ERR_INVALID_VALUE, "prepacked conv weight does not match the kernel shape");
+        *wp = A.pw->data;
+        *colsum = A.pw->colsum;
+        return RTEN_OK;
+    }
+    void* buf = nullptr;
+    RTB_TRY(temp_alloc(ctx, (size_t)(S.O * S.kh * S.kw * S.Cg) * esize, &buf));
+    RTB_TRY(pack_conv_weight(ctx, &S.w, esize, buf));
+    *wp = buf;
+    return RTEN_OK;
+}
+
+rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
+    rten_ctx* ctx = sc.ctx;
+    ConvShape S;
+    RTB_TRY(conv_shape(sc, A, S));
+    const rten_tensor& x = S.x;
+    const rten_tensor& w = S.w;
+    const rten_tensor& bias_v = S.bias_v;
+    const bool one_d = S.one_d;
+    const int64_t* strides = S.strides;
+    const int64_t* dil = S.dil;
+    const int64_t B = S.B, C = S.C, H = S.H, W = S.W, O = S.O, Cg = S.Cg, kh = S.kh, kw = S.kw;
+    const int64_t OH = S.OH, OW = S.OW, pt = S.pt, pb = S.pb, pl = S.pl, pr = S.pr, Og = S.Og;
+    const int groups = S.groups;
 
     // ---- output (layout follows the input: channels-last in -> channels-last out)
     const int out_dtype = (A.kind == 1 && !A.scale) ? RTEN_I32 : RTEN_F32;
@@ -134,20 +182,9 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
     const int esize = A.kind == 0 ? 4 : 1;
     const int kelems = 128 / esize;
 
-    // ---- weights: prepacked handle or pack per call (the reference prepacks per call too)
     const void* wp = nullptr;
     const int32_t* w_colsum = nullptr;
-    if (A.pw) {
-        if (A.pw->kind != 1 || A.pw->O != O || A.pw->Cg != Cg || A.pw->kh != kh || A.pw->kw != kw)
-            return fail(ctx, RTEN_ERR_INVALID_VALUE, "prepacked conv weight does not match the kernel shape");
-        wp = A.pw->data;
-        w_colsum = A.pw->colsum;
-    } else {
-        void* buf = nullptr;
-        RTB_TRY(temp_alloc(ctx, (size_t)(O * kh * kw * Cg) * esize, &buf));
-        RTB_TRY(pack_conv_weight(ctx, &w, esize, buf));
-        wp = buf;
-    }
+    RTB_TRY(conv_weight(ctx, A, S, esize, &wp, &w_colsum));
 
     // ---- integer zero points (x_zp scalar, w_zp per output channel)
     const int32_t* za = nullptr;   // x zero point (GEMM A operand = activations), as i32 ...
@@ -638,6 +675,124 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
     return RTEN_OK;
 }
 
+// act(Conv(x, w, bias) + Conv(x_proj, w_proj, bias_proj)) -- a residual block's last convolution and its projection
+// shortcut.  Two 1x1 convolutions over channels-last, TMA-addressable inputs with whole 128-byte channel blocks run as
+// ONE GEMM over both K ranges (GemmLaunch::proj): the shortcut tensor is never written.  Anything else computes the
+// projection into a temporary and adds it as the residual of the main convolution, exactly as two conv2d_ex calls do.
+rten_status conv_projected(OpScope& sc, ConvArgs& M, ConvArgs& P, rten_tensor* out) {
+    rten_ctx* ctx = sc.ctx;
+    ConvShape sm, sp;
+    RTB_TRY(conv_shape(sc, M, sm));
+    RTB_TRY(conv_shape(sc, P, sp));
+    if (sm.one_d != sp.one_d || sm.B != sp.B || sm.O != sp.O || sm.OH != sp.OH || sm.OW != sp.OW)
+        return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "projection output shape does not match the convolution's output shape");
+    const int64_t B = sm.B, O = sm.O, OH = sm.OH, OW = sm.OW;
+    auto pointwise = [](const ConvShape& s) {
+        return !s.one_d && s.kh == 1 && s.kw == 1 && s.groups == 1 && (s.pt | s.pb | s.pl | s.pr) == 0 && s.dil[0] == 1 &&
+               s.dil[1] == 1 && s.x.strides[1] == 1 && s.C % 32 == 0;
+    };
+    // NHWC view (c, x, y, b) of an input
+    auto nhwc = [](const ConvShape& s) {
+        OperandDesc d;
+        d.base = s.x.data;
+        d.dims[0] = s.C;
+        d.dims[1] = s.W;
+        d.dims[2] = s.H;
+        d.dims[3] = s.B;
+        d.strides[0] = 1;
+        d.strides[1] = s.x.strides[3];
+        d.strides[2] = s.x.strides[2];
+        d.strides[3] = s.x.strides[0];
+        return d;
+    };
+    const OperandDesc am = nhwc(sm), ap = nhwc(sp);
+    const bool fold = pointwise(sm) && pointwise(sp) && sp.strides[0] == sp.strides[1] && tma_compatible(am, 4, 4) &&
+                      tma_compatible(ap, 4, 4) && (!out->data || out->device >= 0) && B * O * OH * OW > 0;
+    if (fold) {
+        const int64_t oshape[4] = {B, O, OH, OW}, pref[4] = {OH * OW * O, 1, OW * O, O};
+        rten_tensor ov;
+        RTB_TRY(sc.out(out, RTEN_F32, 4, oshape, &ov, out->data ? nullptr : pref));
+        const void *wm = nullptr, *wpj = nullptr;
+        const int32_t* unused = nullptr;
+        RTB_TRY(conv_weight(ctx, M, sm, 4, &wm, &unused));
+        RTB_TRY(conv_weight(ctx, P, sp, 4, &wpj, &unused));
+        auto weights = [](const void* w, const ConvShape& s) {  // (c, o, 1, 1) of the packed [O, 1, 1, C]
+            OperandDesc d;
+            d.base = w;
+            d.dims[0] = s.C;
+            d.dims[1] = s.O;
+            d.strides[0] = 1;
+            d.strides[1] = s.C;
+            return d;
+        };
+        GemmLaunch L;
+        L.kind = 0;
+        L.conv = 1;
+        L.N = (int)O;
+        L.K = (int)sm.C;
+        L.M = (int)(B * OH * OW);
+        L.g.B = (int)B;
+        L.g.H = (int)sm.H;
+        L.g.W = (int)sm.W;
+        L.g.C = (int)sm.C;
+        L.g.OH = (int)OH;
+        L.g.OW = (int)OW;
+        L.g.sy = (int)sm.strides[0];
+        L.g.sx = (int)sm.strides[1];
+        L.a = am;
+        L.b = weights(wm, sm);
+        if (M.pw) L.b_x3_slot = &const_cast<rten_packed*>(M.pw)->x3;
+        L.proj.C = (int)sp.C;
+        L.proj.stride = (int)sp.strides[0];
+        L.proj.a = ap;
+        L.proj.b = weights(wpj, sp);
+        if (P.pw) L.proj.b_x3_slot = &const_cast<rten_packed*>(P.pw)->x3;
+        EpilogueDesc& e = L.epi;
+        e.d = ov.data;
+        e.s_z0 = ov.strides[0];
+        e.s_row = ov.strides[2];
+        e.s_z1 = ov.strides[3];
+        e.s_col = ov.strides[1];
+        e.act = M.act;
+        rten_tensor bm, bp;
+        if (M.bias) RTB_TRY(sc.contiguous(&sm.bias_v, &bm));
+        if (P.bias) RTB_TRY(sc.contiguous(&sp.bias_v, &bp));
+        if (M.bias || P.bias) {
+            e.bias_kind = 1;
+            e.bias = (const float*)(M.bias ? bm.data : bp.data);
+            if (M.bias && P.bias) e.bias2 = (const float*)bp.data;
+        }
+        const rten_status st = launch_umma_gemm(ctx, L);
+        if (st != RTEN_ERR_UNSUPPORTED_VALUE) return st;
+        // (no launch plan takes the plain f32 epilogue for this output: two convolutions)
+    }
+    // the projection in the layout rten_b200_conv2d_ex would give it, then the main convolution with it as the residual
+    rten_tensor tmp{};
+    tmp.dtype = RTEN_F32;
+    tmp.device = ctx->device;
+    const bool cl = sp.x.strides[1] == 1 && sp.C > 1;
+    const int64_t sc_ = cl ? 1 : OH * OW, sw = cl ? O : 1, sh = OW * sw;
+    if (sp.one_d) {
+        tmp.ndim = 3;
+        const int64_t shape[3] = {B, O, OW}, st[3] = {O * OH * OW, sc_, sw};
+        for (int i = 0; i < 3; i++) {
+            tmp.shape[i] = shape[i];
+            tmp.strides[i] = st[i];
+        }
+    } else {
+        tmp.ndim = 4;
+        const int64_t shape[4] = {B, O, OH, OW}, st[4] = {O * OH * OW, sc_, sh, sw};
+        for (int i = 0; i < 4; i++) {
+            tmp.shape[i] = shape[i];
+            tmp.strides[i] = st[i];
+        }
+    }
+    RTB_TRY(temp_alloc(ctx, (size_t)std::max<int64_t>(B * O * OH * OW, 1) * 4, &tmp.data));
+    RTB_TRY(conv_core(sc, P, &tmp));
+    M.residual = &tmp;
+    return conv_core(sc, M, out);
+}
+
 }  // namespace
 
 extern "C" {
@@ -699,6 +854,31 @@ rten_status rten_b200_conv2d_ex(rten_ctx* ctx, const rten_tensor* x, const rten_
     A.residual = residual;
     A.act = activation;
     return sc.finish(conv_core(sc, A, out));
+}
+
+rten_status rten_b200_conv2d_projected(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w, const rten_packed* pw,
+                                       const rten_tensor* bias, const rten_conv_params* p, const rten_tensor* x_proj,
+                                       const rten_tensor* w_proj, const rten_packed* pw_proj, const rten_tensor* bias_proj,
+                                       const rten_conv_params* p_proj, int activation, rten_tensor* out) {
+    RTB_TRY(check_ctx(ctx));
+    if (!x || !w || !p || !x_proj || !w_proj || !p_proj || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    for (const rten_tensor* t : {x, w, bias, x_proj, w_proj, bias_proj})
+        if (t && t->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    OpScope sc(ctx);
+    ConvArgs M{}, P{};
+    M.kind = P.kind = 0;
+    M.x = x;
+    M.w = w;
+    M.pw = pw;
+    M.bias = bias;
+    M.p = p;
+    M.act = activation;
+    P.x = x_proj;
+    P.w = w_proj;
+    P.pw = pw_proj;
+    P.bias = bias_proj;
+    P.p = p_proj;
+    return sc.finish(conv_projected(sc, M, P, out));
 }
 
 rten_status rten_b200_conv2d(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w, const rten_packed* pw,

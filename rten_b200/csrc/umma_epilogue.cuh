@@ -300,7 +300,7 @@ struct PlainF32Epi : EpiBase {
     __device__ __forceinline__ void unit(const KParams& p, int t) {
         const TileCoord tc = decode_tile(p, t);
         bv = 0.0f;
-        if (p.epi.bias_kind == 1 && col < p.bn && tc.n0 + col < p.N) bv = __ldg(p.epi.bias + tc.n0 + col);
+        if (p.epi.bias_kind == 1 && col < p.bn && tc.n0 + col < p.N) bv = column_bias(p.epi, tc.n0 + col);
     }
     // (the previous unit's readers of bias_s are past their last chunk barrier: every thread arrives there after its math)
     __device__ __forceinline__ void ready(int grp) {

@@ -146,6 +146,7 @@ struct Plan {
 struct Prepared {
     KParams p;  // geometry filled in; plan-dependent fields zero
     uint32_t abox[4], aes[4], bbox_k;
+    uint32_t pbox[4], pes[4];  // A box / element strides of the projection source
     uint32_t a_rows;
     long long batch;
     OperandDesc od, ord;
@@ -406,8 +407,28 @@ static rten_status prepare_launch(rten_ctx* ctx, const GemmLaunch& L, Prepared& 
     if (getenv("RTEN_B200_NO_RES_TMA")) q.res_tma = 0;
     p.res_tx_bytes = q.a_rows * KBYTES;
     q.step = q.tma_store ? 32 : 16;
+    const bool plain = is_plain_f32(pick_epilogue(L, q.tma_store, q.res_tma, 1));
     // RTEN_B200_NO_WIDE=1: no wide-tile plans (measures what they gain; recorded wide plans are re-planned)
-    q.wide = is_plain_f32(pick_epilogue(L, q.tma_store, q.res_tma, 1)) && !getenv("RTEN_B200_NO_WIDE");
+    q.wide = plain && !getenv("RTEN_B200_NO_WIDE");
+    // ---- projection source: whole 128-byte channel blocks after the main K range; its A box covers the same 128 output
+    //      pixels as the main one, read at `stride` (element strides), so a stage's byte count does not change
+    p.kb_main = p.k_blocks;
+    if (L.proj.C > 0) {
+        const GemmLaunch::Projection& pr = L.proj;
+        const int s = pr.stride;
+        if (!L.conv || L.kind != 0 || pr.C % kelems || s < 1 || s > 8 || p.tw * s > 256 || p.th * s > 256 || !plain ||
+            pr.a.dims[0] * (pr.x3_cb ? 3 : 1) != pr.C || pr.b.dims[0] != pr.C || !tma_compatible(pr.a, 4, 4) || !tma_compatible(pr.b, 4, 4))
+            return RTEN_ERR_UNSUPPORTED_VALUE;
+        p.kb_proj = pr.C / kelems;
+        p.s_proj = s;
+        p.k_blocks += p.kb_proj;
+        const uint32_t box[4] = {(uint32_t)kelems, (uint32_t)(p.tw * s), (uint32_t)(p.th * s), (uint32_t)p.tb};
+        const uint32_t es[4] = {1, (uint32_t)s, (uint32_t)s, 1};
+        for (int i = 0; i < 4; i++) {
+            q.pbox[i] = box[i];
+            q.pes[i] = es[i];
+        }
+    }
     return RTEN_OK;
 }
 
@@ -462,33 +483,41 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
     }
 
     uint32_t bbox[4] = {(uint32_t)q.kelems, (uint32_t)p.bn, 1, 1}, bes[4] = {1, 1, 1, 1}, des[4] = {1, 1, 1, 1};
-    CUtensorMap map_a, map_b;
-    if (!encode_map(ctx, &map_a, L.a, q.esize, L.kind == 0, q.abox, q.aes)) return RTEN_ERR_UNSUPPORTED_VALUE;
-    if (!encode_map(ctx, &map_b, L.b, q.esize, L.kind == 0, bbox, bes)) return RTEN_ERR_UNSUPPORTED_VALUE;
-    CUtensorMap map_d = map_a, map_r = map_a, map_a2 = map_a;
+    TmaMaps m;
+    if (!encode_map(ctx, &m.a, L.a, q.esize, L.kind == 0, q.abox, q.aes)) return RTEN_ERR_UNSUPPORTED_VALUE;
+    if (!encode_map(ctx, &m.b, L.b, q.esize, L.kind == 0, bbox, bes)) return RTEN_ERR_UNSUPPORTED_VALUE;
+    m.d = m.r = m.a2 = m.a_proj = m.b_proj = m.a2_proj = m.a;  // (maps the launch does not use)
     p.x3_cb = L.x3_cb;
-    if (L.x3_cb && !encode_map(ctx, &map_a2, L.a_lo, q.esize, true, q.abox, q.aes)) return RTEN_ERR_UNSUPPORTED_VALUE;
-    if (p.tma_store && !encode_map(ctx, &map_d, q.od, 4, true, q.dbox, des)) {
+    if (L.x3_cb && !encode_map(ctx, &m.a2, L.a_lo, q.esize, true, q.abox, q.aes)) return RTEN_ERR_UNSUPPORTED_VALUE;
+    if (p.kb_proj) {
+        p.x3_cb_proj = L.proj.x3_cb;
+        if (!encode_map(ctx, &m.a_proj, L.proj.a, 4, true, q.pbox, q.pes) ||
+            !encode_map(ctx, &m.b_proj, L.proj.b, 4, true, bbox, bes) ||
+            (L.proj.x3_cb && !encode_map(ctx, &m.a2_proj, L.proj.a_lo, 4, true, q.pbox, q.pes)))
+            return RTEN_ERR_UNSUPPORTED_VALUE;
+    }
+    if (p.tma_store && !encode_map(ctx, &m.d, q.od, 4, true, q.dbox, des)) {
         p.tma_store = 0;  // the generic epilogue stores directly
         p.res_tma = 0;
-        map_d = map_a;
+        m.d = m.a;
     }
-    if (p.res_tma && !encode_map(ctx, &map_r, q.ord, 4, true, q.dbox, des)) {
+    if (p.res_tma && !encode_map(ctx, &m.r, q.ord, 4, true, q.dbox, des)) {
         p.res_tma = 0;
-        map_r = map_a;
+        m.r = m.a;
     }
     const Epi epi = pick_epilogue(L, p.tma_store, p.res_tma, p.splitk);
     // the generic epilogue takes a TMA-staged residual only on its register path (f32, act <= Relu)
     if (epi == Epi::Generic && (L.kind == 1 || L.epi.act > 1)) p.res_tma = 0;
 
     if (verbose)
-        fprintf(stderr, "[umma_gemm] kind=%d conv=%d M=%d N=%d K=%d kb=%d tiles_m=%d bn=%d splitk=%d units=%d stages=%d tma_store=%d res_tma=%d nbuf=%d box=%dx%dx%d epi=%s\n",
-                L.kind, L.conv, L.M, L.N, L.K, p.k_blocks, p.tiles_m, p.bn, p.splitk, p.units_total, p.stages, p.tma_store,
-                p.res_tma, p.nbuf, p.tw, p.th, p.tb, epi_name(epi));
-    if (is_wide(p.bn) && !is_plain_f32(epi)) return RTEN_ERR_UNSUPPORTED_VALUE;  // (an output / residual map failed to encode)
+        fprintf(stderr, "[umma_gemm] kind=%d conv=%d M=%d N=%d K=%d kb=%d kb_proj=%d tiles_m=%d bn=%d splitk=%d units=%d stages=%d tma_store=%d res_tma=%d nbuf=%d box=%dx%dx%d epi=%s\n",
+                L.kind, L.conv, L.M, L.N, L.K, p.k_blocks, p.kb_proj, p.tiles_m, p.bn, p.splitk, p.units_total, p.stages,
+                p.tma_store, p.res_tma, p.nbuf, p.tw, p.th, p.tb, epi_name(epi));
+    // (an output / residual map failed to encode; a projection source and a second bias need the plain f32 epilogue)
+    if ((is_wide(p.bn) || p.kb_proj || L.epi.bias2) && !is_plain_f32(epi)) return RTEN_ERR_UNSUPPORTED_VALUE;
     const size_t smem_bytes = (size_t)p.stages * p.stage_bytes +
                               (is_wide(p.bn) ? WIDE_SMEM_FIXED_BYTES : ps.n_stg * STG_BYTES + SMEM_FIXED_BYTES);
-    using Kernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, KParams);
+    using Kernel = void (*)(TmaMaps, KParams);
     // [kind][variant]: the integer kind has no plain f32 kernels, the f32 kind no plain integer ones
     static const Kernel narrow[2][7] = {
         {umma_gemm_kernel<0, Epi::Generic>, umma_gemm_kernel<0, Epi::Fast>, umma_gemm_kernel<0, Epi::FastGelu>,
@@ -511,7 +540,7 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
     cfg.attrs = attr;
     cfg.numAttrs = getenv("RTEN_B200_NO_PDL") ? 0 : 1;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess) e = cudaLaunchKernelEx(&cfg, kern, map_a, map_b, map_d, map_r, map_a2, p);
+    if (e == cudaSuccess) e = cudaLaunchKernelEx(&cfg, kern, m, p);
     if (e != cudaSuccess) return fail_cuda(ctx, e, "umma_gemm launch");
     e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(ctx, e, "umma_gemm launch");
@@ -528,6 +557,12 @@ static std::vector<long long> tune_key(const GemmLaunch& L, const Prepared& q) {
     if (L.conv) {
         const ConvGeom& g = L.g;
         for (long long v : {g.B, g.H, g.W, g.C, g.OH, g.OW, g.kh, g.kw, g.sy, g.sx, g.dy, g.dx, g.pt, g.pl}) k.push_back(v);
+    }
+    if (L.proj.C > 0) {  // (absent from keys without one: recorded plans of unfolded launches stay valid)
+        const GemmLaunch::Projection& pr = L.proj;
+        for (int64_t v : {(int64_t)-1, (int64_t)pr.C, (int64_t)pr.stride, (int64_t)pr.x3_cb, pr.a.dims[1], pr.a.dims[2],
+                          pr.a.strides[1], pr.a.strides[2], pr.a.strides[3], pr.b.strides[1]})
+            k.push_back(v);
     }
     return k;
 }
@@ -548,8 +583,7 @@ static Plan plan_from_array(const std::array<int, 3>& a) {
 //    (KParams::x3_cb).  Needs K (C) % 32 == 0 and a TMA-addressable A; otherwise the three-segment copy is built.
 static rten_status launch_tf32x3(rten_ctx* ctx, const GemmLaunch& L0) {
     GemmLaunch L = L0;
-    const long long d0 = L0.a.dims[0];               // K, or channels per group
-    const long long d0p = (d0 + 3) / 4 * 4;          // thirds stay 16-byte aligned for TMA
+    long long d0 = 0, d0p = 0;  // K or channels per group of the source being split; thirds stay 16-byte aligned for TMA
     auto split = [&](const OperandDesc& src, OperandDesc& dst, int role, void* into) -> rten_status {
         const long long planes = role == 2 ? 1 : 3;
         long long dims[4], strides[4], n = planes * d0p;
@@ -572,53 +606,66 @@ static rten_status launch_tf32x3(rten_ctx* ctx, const GemmLaunch& L0) {
         }
         return RTEN_OK;
     };
-    if (L0.b.dims[0] != d0) return RTEN_ERR_UNSUPPORTED_VALUE;
-    // ---- B
-    if (L0.b_x3_slot && !getenv("RTEN_B200_X3_NO_CACHE")) {
-        if (!*L0.b_x3_slot && !ctx->capturing) {
-            long long n = 3 * d0p;
-            for (int i = 1; i < 4; i++) n *= (L0.b.strides[i] == 0 ? 1 : L0.b.dims[i]);
-            void* buf = nullptr;
-            if (cudaMalloc(&buf, (size_t)n * 4) != cudaSuccess) return fail(ctx, RTEN_ERR_CUDA, "cudaMalloc failed for the 3xTF32 copy of a prepacked operand");
-            OperandDesc tmp;
-            const rten_status st = split(L0.b, tmp, 1, buf);
-            if (st != RTEN_OK) {
-                cudaFree(buf);
-                return st;
+    // One (A, B) source -- the main one, or the projection source (GemmLaunch::proj) with its own B copy and A planes
+    auto split_source = [&](const OperandDesc& a0, const OperandDesc& b0, void** slot, const void* a_lo_base,
+                            OperandDesc& a, OperandDesc& b, OperandDesc& a_lo, int& x3_cb) -> rten_status {
+        d0 = a0.dims[0];
+        d0p = (d0 + 3) / 4 * 4;
+        if (b0.dims[0] != d0) return RTEN_ERR_UNSUPPORTED_VALUE;
+        // ---- B
+        if (slot && !getenv("RTEN_B200_X3_NO_CACHE")) {
+            if (!*slot && !ctx->capturing) {
+                long long n = 3 * d0p;
+                for (int i = 1; i < 4; i++) n *= (b0.strides[i] == 0 ? 1 : b0.dims[i]);
+                void* buf = nullptr;
+                if (cudaMalloc(&buf, (size_t)n * 4) != cudaSuccess) return fail(ctx, RTEN_ERR_CUDA, "cudaMalloc failed for the 3xTF32 copy of a prepacked operand");
+                OperandDesc tmp;
+                const rten_status st = split(b0, tmp, 1, buf);
+                if (st != RTEN_OK) {
+                    cudaFree(buf);
+                    return st;
+                }
+                *slot = buf;
             }
-            *L0.b_x3_slot = buf;
         }
-    }
-    if (L0.b_x3_slot && *L0.b_x3_slot && !getenv("RTEN_B200_X3_NO_CACHE")) {
-        L.b = L0.b;
-        L.b.base = *L0.b_x3_slot;
-        L.b.dims[0] = 3 * d0p;
-        long long st = 3 * d0p;
-        for (int i = 1; i < 4; i++) {
-            const long long di = L0.b.strides[i] == 0 ? 1 : L0.b.dims[i];
-            L.b.strides[i] = (L0.b.strides[i] == 0 && L0.b.dims[i] > 1) ? 0 : st;
-            st *= di;
+        if (slot && *slot && !getenv("RTEN_B200_X3_NO_CACHE")) {
+            b = b0;
+            b.base = *slot;
+            b.dims[0] = 3 * d0p;
+            long long st = 3 * d0p;
+            for (int i = 1; i < 4; i++) {
+                const long long di = b0.strides[i] == 0 ? 1 : b0.dims[i];
+                b.strides[i] = (b0.strides[i] == 0 && b0.dims[i] > 1) ? 0 : st;
+                st *= di;
+            }
+        } else {
+            RTB_TRY(split(b0, b, 1, nullptr));
         }
-    } else {
-        RTB_TRY(split(L0.b, L.b, 1, nullptr));
-    }
-    // ---- A
-    const bool two_plane = d0 % 32 == 0 && tma_compatible(L0.a, 4, 4) && !getenv("RTEN_B200_X3_THREE_PLANES");
-    if (two_plane && L0.a_lo_base) {
-        L.a_lo = L0.a;
-        L.a_lo.base = L0.a_lo_base;
-        L.x3_cb = (int)(d0 / 32);
-    } else if (two_plane) {
-        RTB_TRY(split(L0.a, L.a_lo, 2, nullptr));
-        L.x3_cb = (int)(d0 / 32);
-    } else {
-        RTB_TRY(split(L0.a, L.a, 0, nullptr));
-    }
+        // ---- A
+        const bool two_plane = d0 % 32 == 0 && tma_compatible(a0, 4, 4) && !getenv("RTEN_B200_X3_THREE_PLANES");
+        if (two_plane && a_lo_base) {
+            a_lo = a0;
+            a_lo.base = a_lo_base;
+            x3_cb = (int)(d0 / 32);
+        } else if (two_plane) {
+            RTB_TRY(split(a0, a_lo, 2, nullptr));
+            x3_cb = (int)(d0 / 32);
+        } else {
+            RTB_TRY(split(a0, a, 0, nullptr));
+        }
+        return RTEN_OK;
+    };
+    RTB_TRY(split_source(L0.a, L0.b, L0.b_x3_slot, L0.a_lo_base, L.a, L.b, L.a_lo, L.x3_cb));
     if (L.conv)
         L.g.C = (int)(3 * d0p);
     L.K = L.conv ? (int)(L0.K / d0 * 3 * d0p) : (int)(3 * d0p);
     L.b_x3_slot = nullptr;
     L.a_lo_base = nullptr;
+    if (L0.proj.C > 0) {
+        RTB_TRY(split_source(L0.proj.a, L0.proj.b, L0.proj.b_x3_slot, nullptr, L.proj.a, L.proj.b, L.proj.a_lo, L.proj.x3_cb));
+        L.proj.C = (int)(3 * d0p);
+        L.proj.b_x3_slot = nullptr;
+    }
     const int saved = ctx->f32_mode;
     ctx->f32_mode = RTEN_F32_TF32;
     const rten_status st = launch_umma_gemm(ctx, L);
@@ -630,7 +677,7 @@ rten_status launch_umma_gemm(rten_ctx* ctx, const GemmLaunch& L) {
     if (L.kind == 0 && ctx->f32_mode == RTEN_F32_TF32X3) return launch_tf32x3(ctx, L);
     // stride-1 windows (the 3x3 layers): the halo-reuse kernel moves the activations into shared memory once per channel
     // block instead of once per filter tap (umma_halo.cu); everything it does not cover falls through
-    if (L.conv && L.kind == 0 && L.g.kh * L.g.kw > 1 && !L.x3_cb) {
+    if (L.conv && L.kind == 0 && L.g.kh * L.g.kw > 1 && !L.x3_cb && !L.proj.C) {
         const rten_status hs = launch_umma_halo_conv(ctx, L);
         if (hs != RTEN_ERR_UNSUPPORTED_VALUE) return hs;
     }
@@ -757,7 +804,7 @@ rten_status launch_umma_gemm(rten_ctx* ctx, const GemmLaunch& L) {
                 }
                 // stride-1 windows: the halo-reuse kernel (umma_halo.cu) over a few unit shapes, same timing
                 int halo_bn = 0, halo_T = 0;
-                if (L.conv && L.kind == 0 && L.g.kh * L.g.kw > 1 && !L.x3_cb && !getenv("RTEN_B200_NO_HALO")) {
+                if (L.conv && L.kind == 0 && L.g.kh * L.g.kw > 1 && !L.x3_cb && !L.proj.C && !getenv("RTEN_B200_NO_HALO")) {
                     for (int hbn : {32, 64})  // the halo kernel's unit shapes: one 128-slot tile, bn <= 64
                         for (int hT : {1}) {
                             if (hbn > L.N) continue;

@@ -35,6 +35,7 @@ struct EpilogueDesc {
     int64_t r_z0 = 0, r_z1 = 0, r_row = 0, r_col = 0;
     const float* bias = nullptr;
     int bias_kind = 0;  // 1: per column n, 2: per row m
+    const float* bias2 = nullptr;  // bias_kind 1, plain f32 epilogue only: a second column bias, added to `bias` first
     float alpha = 1.0f;
     int act = 0;  // 0 none, 1 relu, 2 gelu(erf), 3 gelu(tanh)
     // integer path: C = acc - za[m % za_len]*colsum[n] - zb[n % zb_len]*rowsum[m] + K*za*zb
@@ -82,6 +83,18 @@ struct GemmLaunch {
     // internal (launch_tf32x3 -> kernel): two-plane A -- `a` is the original tensor (segments 1, 2), `a_lo` its low parts
     int x3_cb = 0;
     OperandDesc a_lo;
+    // optional projection source of a 1x1, unpadded conv launch (`proj.C` > 0): a second 1x1, unpadded convolution
+    // into the same output pixels, summed in the same accumulator -- D = act(A*B + A_proj*B_proj + bias + epi.bias2).
+    // Its K blocks follow the main ones.  Runs only with the plain f32 epilogue (else RTEN_ERR_UNSUPPORTED_VALUE).
+    struct Projection {
+        int C = 0;       // channels of a (a multiple of 32)
+        int stride = 1;  // pixel (ox, oy) reads a at (ox * stride, oy * stride)
+        OperandDesc a;   // (c, x, y, b) of the NHWC input
+        OperandDesc b;   // (c, o, 1, 1)
+        void** b_x3_slot = nullptr;  // as b_x3_slot above
+        int x3_cb = 0;               // internal, as x3_cb / a_lo above
+        OperandDesc a_lo;
+    } proj;
 };
 
 // Returns RTEN_OK and enqueues the kernel, or RTEN_ERR_UNSUPPORTED_VALUE (without touching ctx->err

@@ -77,6 +77,11 @@ struct KParams {
     int x3_cb;      // > 0: 3xTF32 over TWO planes of A -- the K (channel) range is three segments of x3_cb K blocks,
                     //      [lo | hi | hi]: segment 0 reads the low-part plane (tma_a2), segments 1 and 2 read the ORIGINAL f32
                     //      tensor (tf32 wgmma ignores the 13 low mantissa bits, so the raw values ARE the high parts)
+    // Projection source (conv only): K blocks [kb_main, k_blocks) are a second 1x1, unpadded convolution of another
+    // tensor into the same output pixels -- A from tma_a_proj at (c, ox0 * s_proj, oy0 * s_proj, b0), B from
+    // tma_b_proj at (c, n0, 0, 0); x3_cb_proj is its own two-plane 3xTF32 segment length (low parts: tma_a2_proj).
+    // Without one, kb_main = k_blocks.
+    int kb_main, kb_proj, s_proj, x3_cb_proj;
     FastDiv d_tiles_n, d_tiles_m, d_z0, d_tiles_x, d_tiles_y, d_tiles_total, d_c_blocks, d_kw, d_tw, d_th;
     uint32_t* sk_ws;
     int* sk_cnt;
@@ -125,6 +130,13 @@ __device__ __forceinline__ void plain_f32_pair(uint32_t& v0, uint32_t& v1, bool 
         v0 = __float_as_uint(fmaxf(__uint_as_float(v0), 0.0f));
         v1 = __float_as_uint(fmaxf(__uint_as_float(v1), 0.0f));
     }
+}
+
+// The bias of output column n in the plain f32 epilogues: bias[n], or bias[n] + bias2[n] rounded once (the two biases
+// of a launch with a projection source)
+__device__ __forceinline__ float column_bias(const EpilogueDesc& e, int n) {
+    const float b = __ldg(e.bias + n);
+    return e.bias2 ? __fadd_rn(b, __ldg(e.bias2 + n)) : b;
 }
 
 // cp.async.bulk.wait_group.read takes an immediate: leave at most `n` of this thread's bulk stores un-read
@@ -295,11 +307,30 @@ __device__ __forceinline__ void mma_role(const KParams& p, const SmemLayout& L, 
     else mma_units<KIND, 3, N>(p, L, worker, n_workers);
 }
 
+// The tensor maps of one launch: main operands, output, residual, the low-part plane of A (3xTF32) and the projection
+// source's A, B and low-part plane (KParams::kb_main).
+struct TmaMaps {
+    CUtensorMap a, b, d, r, a2, a_proj, b_proj, a2_proj;
+};
+
+__device__ __forceinline__ void prefetch_maps(const TmaMaps& m, const KParams& p) {
+    tma_prefetch_desc(&m.a);
+    tma_prefetch_desc(&m.b);
+    if (p.tma_store) tma_prefetch_desc(&m.d);
+    if (p.res_tma) tma_prefetch_desc(&m.r);
+    if (p.x3_cb) tma_prefetch_desc(&m.a2);
+    if (p.kb_proj) {
+        tma_prefetch_desc(&m.a_proj);
+        tma_prefetch_desc(&m.b_proj);
+        if (p.x3_cb_proj) tma_prefetch_desc(&m.a2_proj);
+    }
+}
+
 // TMA producer of both GEMM kernels: one warp walks this CTA's work units and fills the operand ring -- A (128 rows)
-// and B (bn rows) of one 128-byte K block per stage, the conv filter tap / channel walk, the two-plane 3xTF32 segments
-// and broadcast batch dims.  Runs warp-uniformly, one elected lane issues.
-__device__ __forceinline__ void producer_role(const KParams& p, const CUtensorMap* tma_a, const CUtensorMap* tma_a2,
-                                              const CUtensorMap* tma_b, const SmemLayout& L, int worker, int n_workers) {
+// and B (bn rows) of one 128-byte K block per stage, the conv filter tap / channel walk, the two-plane 3xTF32 segments,
+// the projection source and broadcast batch dims.  Runs warp-uniformly, one elected lane issues.
+__device__ __forceinline__ void producer_role(const KParams& p, const TmaMaps& m, const SmemLayout& L, int worker,
+                                              int n_workers) {
     uint8_t* smem = L.smem;
     uint64_t* empty_bar = L.empty_bar;
     uint32_t ring = 0;  // bit s = uses of stage s so far, mod 2
@@ -311,45 +342,58 @@ __device__ __forceinline__ void producer_role(const KParams& p, const CUtensorMa
         p.d_tiles_total.divmod(u, ks, t);
         const int kb0 = ks * p.kb_per, kb1 = min(p.k_blocks, kb0 + p.kb_per);
         const TileCoord tc = decode_tile(p, t);
+        // projection source: its blocks follow the main source's, one filter tap, its own channel and segment walk
+        bool proj = kb0 >= p.kb_main;
+        int x3 = proj ? p.x3_cb_proj : p.x3_cb;
         // conv: K block -> (filter tap, channel block), kept incrementally
-        int tap, cb, ky, kx;
-        p.d_c_blocks.divmod(kb0, tap, cb);
+        int tap = 0, cb = kb0 - p.kb_main, ky, kx;
+        if (!proj) p.d_c_blocks.divmod(kb0, tap, cb);
         p.d_kw.divmod(tap, ky, kx);
         // two-plane 3xTF32: segment of the K / channel range and block inside it (kept incrementally)
         int seg = 0, sblk = p.conv ? cb : kb0;
-        if (p.x3_cb)
-            while (sblk >= p.x3_cb) {
-                sblk -= p.x3_cb;
+        if (x3)
+            while (sblk >= x3) {
+                sblk -= x3;
                 seg++;
             }
         // programmatic dependent launch: the producer is the first to touch the predecessor's output; everything
         // above (tile decode) ran while the predecessor grid was still draining
         if (u == worker) asm volatile("griddepcontrol.wait;" ::: "memory");
         for (int kb = kb0; kb < kb1; kb++) {
+            if (kb == p.kb_main) {  // (never without a projection source: kb_main = k_blocks)
+                proj = true;
+                x3 = p.x3_cb_proj;
+                cb = sblk = seg = 0;
+            }
             mbar_wait(&empty_bar[stage], ((ring >> stage) & 1) ^ 1);
             if (elect_one()) {
                 const uint32_t fb = full0 + stage * 8;
                 mbar_expect_tx_u32(fb, p.tx_bytes);
                 const uint32_t sa = smem0 + stage * p.stage_bytes;
                 const uint32_t sb = sa + A_STAGE_BYTES;
-                const CUtensorMap* ma = (p.x3_cb && seg == 0) ? tma_a2 : tma_a;
-                if (p.conv) {
+                const bool lo = x3 && seg == 0;
+                if (proj) {
                     const int c0 = cb * p.kelems;
-                    const int ca = p.x3_cb ? sblk * p.kelems : c0;
-                    tma_load_4d_u32(sa, ma, fb, ca, tc.ox0 * p.sx - p.pl + kx * p.dx, tc.oy0 * p.sy - p.pt + ky * p.dy, tc.b0);
-                    tma_load_4d_u32(sb, tma_b, fb, c0, tc.n0, tap, 0);
+                    tma_load_4d_u32(sa, lo ? &m.a2_proj : &m.a_proj, fb, x3 ? sblk * p.kelems : c0, tc.ox0 * p.s_proj,
+                                    tc.oy0 * p.s_proj, tc.b0);
+                    tma_load_4d_u32(sb, &m.b_proj, fb, c0, tc.n0, 0, 0);
+                } else if (p.conv) {
+                    const int c0 = cb * p.kelems;
+                    const int ca = x3 ? sblk * p.kelems : c0;
+                    tma_load_4d_u32(sa, lo ? &m.a2 : &m.a, fb, ca, tc.ox0 * p.sx - p.pl + kx * p.dx, tc.oy0 * p.sy - p.pt + ky * p.dy, tc.b0);
+                    tma_load_4d_u32(sb, &m.b, fb, c0, tc.n0, tap, 0);
                 } else {
                     const int k0 = kb * p.kelems;
-                    const int ka = p.x3_cb ? sblk * p.kelems : k0;
-                    tma_load_4d_u32(sa, ma, fb, ka, tc.m0, p.a_bcast0 ? 0 : tc.z0, p.a_bcast1 ? 0 : tc.z1);
-                    tma_load_4d_u32(sb, tma_b, fb, k0, tc.n0, p.b_bcast0 ? 0 : tc.z0, p.b_bcast1 ? 0 : tc.z1);
+                    const int ka = x3 ? sblk * p.kelems : k0;
+                    tma_load_4d_u32(sa, lo ? &m.a2 : &m.a, fb, ka, tc.m0, p.a_bcast0 ? 0 : tc.z0, p.a_bcast1 ? 0 : tc.z1);
+                    tma_load_4d_u32(sb, &m.b, fb, k0, tc.n0, p.b_bcast0 ? 0 : tc.z0, p.b_bcast1 ? 0 : tc.z1);
                 }
             }
-            if (p.x3_cb && ++sblk == p.x3_cb) {
+            if (x3 && ++sblk == x3) {
                 sblk = 0;
                 seg = seg == 2 ? 0 : seg + 1;  // (conv: the next filter tap starts over at segment 0)
             }
-            if (++cb == p.c_blocks) {
+            if (++cb == p.c_blocks && !proj) {
                 cb = 0;
                 tap++;
                 if (++kx == p.kw) {
@@ -420,18 +464,10 @@ __device__ __forceinline__ void kernel_setup(const SmemLayout& L) {
 // variant (umma_epilogue.cuh).
 template <int KIND, Epi E>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-umma_gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
-                 const __grid_constant__ CUtensorMap tma_d, const __grid_constant__ CUtensorMap tma_r,
-                 const __grid_constant__ CUtensorMap tma_a2, const __grid_constant__ KParams p) {
+umma_gemm_kernel(const __grid_constant__ TmaMaps m, const __grid_constant__ KParams p) {
     extern __shared__ uint8_t smem_raw[];
     const SmemLayout L = carve_smem(smem_raw);
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tma_a);
-        tma_prefetch_desc(&tma_b);
-        if (p.tma_store) tma_prefetch_desc(&tma_d);
-        if (p.res_tma) tma_prefetch_desc(&tma_r);
-        if (p.x3_cb) tma_prefetch_desc(&tma_a2);
-    }
+    if (threadIdx.x == 0) prefetch_maps(m, p);
     kernel_setup(L);
     // Programmatic dependent launch: everything above (barrier init, descriptor prefetch) overlaps the tail of the
     // previous kernel in the stream; global memory is only touched after this point.
@@ -443,7 +479,7 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
     // TMA / MMA instructions): addresses and descriptors then live in uniform registers instead of being moved
     // there (R2UR) for every instruction, which is what bounds a single issuing thread.
     if (warp == PRODUCER_WARP) {
-        producer_role(p, &tma_a, &tma_a2, &tma_b, L, worker, n_workers);
+        producer_role(p, m, L, worker, n_workers);
     } else if (warp < 4) {
         // ===================== MMA warpgroup: accumulators in registers, finished tiles to shared memory
         if (p.bn == 32)
@@ -451,7 +487,7 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
         else
             mma_role<KIND, 64>(p, L, worker, n_workers);
     } else {
-        epilogue<KIND, E>(p, L, &tma_d, &tma_r, worker, n_workers);
+        epilogue<KIND, E>(p, L, &m.d, &m.r, worker, n_workers);
     }
 }
 
@@ -529,7 +565,7 @@ __device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout
             const TileCoord tc = decode_tile(p, u);  // (no split-K: a unit is a tile)
             // The unit's bias (zeros without one: x + 0 keeps the -0 -> +0 of the other epilogues).  Every reader of the
             // previous unit's values has passed the last chunk barrier; the barrier after the main loop publishes these.
-            if (t < N) bias_s[t] = (e.bias_kind == 1 && tc.n0 + t < p.N) ? __ldg(e.bias + tc.n0 + t) : 0.0f;
+            if (t < N) bias_s[t] = (e.bias_kind == 1 && tc.n0 + t < p.N) ? column_bias(e, tc.n0 + t) : 0.0f;
             if (issuer) {
                 bulk_wait_read(0);  // staging buffers free
                 if (p.res_tma) load_residual(tc, 0, ci & 1);
@@ -619,20 +655,12 @@ __device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout
 
 template <Epi E>
 __global__ void __launch_bounds__(WIDE_THREADS, 1)
-umma_wide_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
-                 const __grid_constant__ CUtensorMap tma_d, const __grid_constant__ CUtensorMap tma_r,
-                 const __grid_constant__ CUtensorMap tma_a2, const __grid_constant__ KParams p) {
+umma_wide_kernel(const __grid_constant__ TmaMaps m, const __grid_constant__ KParams p) {
     extern __shared__ uint8_t smem_raw[];
     const SmemLayout L = carve_wide_smem(smem_raw, p);
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tma_a);
-        tma_prefetch_desc(&tma_b);
-        tma_prefetch_desc(&tma_d);
-        if (p.res_tma) tma_prefetch_desc(&tma_r);
-        if (p.x3_cb) tma_prefetch_desc(&tma_a2);
-    }
+    if (threadIdx.x == 0) prefetch_maps(m, p);
     if (warp == 1) {
         if (lane < MAX_STAGES) {
             mbar_init(&L.full_bar[lane], 1);
@@ -649,14 +677,14 @@ umma_wide_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     if (warp < 4) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-        if (warp == 0) producer_role(p, &tma_a, &tma_a2, &tma_b, L, (int)blockIdx.x, (int)gridDim.x);
+        if (warp == 0) producer_role(p, m, L, (int)blockIdx.x, (int)gridDim.x);
     } else {
         asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
         // (Gelu: 128 columns only -- the out-of-line act4 calls would spill around 128 live accumulators per thread)
         if (E == Epi::PlainF32Gelu || p.bn == 128)
-            wide_consumer<E, 128>(p, L, &tma_d, &tma_r, (int)blockIdx.x, (int)gridDim.x);
+            wide_consumer<E, 128>(p, L, &m.d, &m.r, (int)blockIdx.x, (int)gridDim.x);
         else
-            wide_consumer<E, 256>(p, L, &tma_d, &tma_r, (int)blockIdx.x, (int)gridDim.x);
+            wide_consumer<E, 256>(p, L, &m.d, &m.r, (int)blockIdx.x, (int)gridDim.x);
     }
 }
 

@@ -101,7 +101,8 @@ def resnet50_flops(spec: ResNet50Spec, hw: int = 224) -> float:
 class ResNet50Runner:
     """Executes the op list on one GPU with activations resident in HBM (channels-last strides;
     logical shapes stay NCHW at the ABI).  `fuse=True` uses the epilogue fusions (bias + residual +
-    Relu inside the conv kernel); `fuse=False` issues the reference's separate Conv / Add / Relu ops."""
+    Relu inside the conv kernel) and runs a projection block's last conv and its downsample conv as one call, so the
+    shortcut tensor is never written; `fuse=False` issues the reference's separate Conv / Add / Relu ops."""
 
     def __init__(self, ctx: O.Context, spec: ResNet50Spec, fuse: bool = True):
         self.ctx, self.spec, self.fuse = ctx, spec, fuse
@@ -137,12 +138,24 @@ class ResNet50Runner:
             y = self.relu.run(self.ctx, y, in_place=True)
         return y
 
+    def _conv_projected(self, c: ConvSpec, t, down: ConvSpec, x):
+        """relu(c(t) + down(x)) in one call (Conv.run_projected)."""
+        op, w, b, pk = self._convs[id(c)]
+        dop, dw, db, dpk = self._convs[id(down)]
+        op.activation = O.ACT_RELU
+        return op.run_projected(self.ctx, t, w, b, packed_w=pk, proj=dop, x_proj=x, w_proj=dw, bias_proj=db, packed_w_proj=dpk)
+
     def run(self, x: O.DeviceTensor) -> O.DeviceTensor:
         """x: [B,3,224,224] f32 (any strides) -> logits [B,1000]."""
         s = self.spec
         y = self._conv(s.stem, x, True)
         y = self.maxpool.run(self.ctx, y)
         for b in s.blocks:
+            if self.fuse and b.down is not None:
+                t = self._conv(b.c1, y, True)
+                t = self._conv(b.c2, t, True)
+                y = self._conv_projected(b.c3, t, b.down, y)
+                continue
             ident = y if b.down is None else self._conv(b.down, y, False)
             t = self._conv(b.c1, y, True)
             t = self._conv(b.c2, t, True)

@@ -539,6 +539,19 @@ class Conv:
                                               A.t(residual), self.activation, C.byref(o)))
         return A.wrap(o, out)
 
+    def run_projected(self, ctx, x, w, bias=None, packed_w: Optional[Packed] = None, *, proj: "Conv", x_proj, w_proj,
+                      bias_proj=None, packed_w_proj: Optional[Packed] = None, out=None):
+        """act(self(x, w, bias) + proj(x_proj, w_proj, bias_proj)) with this op's activation: a residual block's last
+        convolution and its projection shortcut (rten_b200_conv2d_projected)."""
+        A = _Args(ctx)
+        o = A.out(out)
+        p = _conv_params(self.padding, self.groups, self.strides, self.dilations)
+        pp = _conv_params(proj.padding, proj.groups, proj.strides, proj.dilations)
+        ctx.check(ctx.lib.rten_b200_conv2d_projected(ctx.handle, A.t(x), A.t(w), _ph(packed_w), A.t(bias), C.byref(p),
+                                                     A.t(x_proj), A.t(w_proj), _ph(packed_w_proj), A.t(bias_proj),
+                                                     C.byref(pp), self.activation, C.byref(o)))
+        return A.wrap(o, out)
+
 
 class ConvInteger(Conv):
     """src/ops/conv.rs:477-533"""
