@@ -205,6 +205,24 @@ rten_status rten_b200_conv2d_projected(rten_ctx* ctx, const rten_tensor* x, cons
                                        const rten_conv_params* p, const rten_tensor* x_proj, const rten_tensor* w_proj,
                                        const rten_packed* packed_w_proj_or_null, const rten_tensor* bias_proj_or_null,
                                        const rten_conv_params* p_proj, int activation, rten_tensor* out);
+/* Extension: out = act(Conv(x, w, bias, p) [+ residual | + Conv(x_proj, w_proj, bias_proj, p_proj)]) and
+   out_next = activation_next(Conv(out, w_next, bias_next, p_next)) -- a residual block's last convolution and the next
+   block's first.  residual and x_proj are exclusive (RTEN_ERR_INVALID_VALUE); mismatched projection or residual shapes
+   return RTEN_ERR_INCOMPATIBLE_SHAPES; all tensors are f32 (RTEN_ERR_UNSUPPORTED_TYPE); otherwise the checks of
+   conv2d_ex / conv2d_projected.  In single-pass TF32, a 1x1 convolution (groups 1, no padding or dilation; a projection
+   as conv2d_projected folds it) over channels-last, 16-byte addressable inputs with up to 256 output channels, a
+   multiple of 32, followed by a 1x1, stride-1, unpadded convolution to 64 or 128 channels, runs as one launch that
+   computes out_next from out's tiles while they are stored, so out is not read back.  Any other pair runs as the calls
+   conv2d_ex (or conv2d_projected) then conv2d_ex(out, w_next), with the same results. */
+rten_status rten_b200_conv2d_chained(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w,
+                                     const rten_packed* packed_w_or_null, const rten_tensor* bias_or_null,
+                                     const rten_conv_params* p, const rten_tensor* residual_or_null,
+                                     const rten_tensor* x_proj_or_null, const rten_tensor* w_proj_or_null,
+                                     const rten_packed* packed_w_proj_or_null, const rten_tensor* bias_proj_or_null,
+                                     const rten_conv_params* p_proj_or_null, int activation, const rten_tensor* w_next,
+                                     const rten_packed* packed_w_next_or_null, const rten_tensor* bias_next_or_null,
+                                     const rten_conv_params* p_next, int activation_next, rten_tensor* out,
+                                     rten_tensor* out_next);
 /* ConvInteger (src/ops/conv.rs:421-533); scale_or_null != NULL => ConvIntegerToFloat (:535-587). */
 rten_status rten_b200_conv_integer(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w,
                                    const rten_packed* packed_w_or_null, const rten_tensor* x_zero_point_or_null,

@@ -91,6 +91,9 @@ _SIGNATURES = {
     "rten_b200_conv2d_ex": (C.c_int, [_vp, _TP, _TP, _vp, _TP, C.POINTER(RtenConvParams), _TP, C.c_int, _TP]),
     "rten_b200_conv2d_projected": (C.c_int, [_vp, _TP, _TP, _vp, _TP, C.POINTER(RtenConvParams), _TP, _TP, _vp, _TP,
                                              C.POINTER(RtenConvParams), C.c_int, _TP]),
+    "rten_b200_conv2d_chained": (C.c_int, [_vp, _TP, _TP, _vp, _TP, C.POINTER(RtenConvParams), _TP, _TP, _TP, _vp, _TP,
+                                           C.POINTER(RtenConvParams), C.c_int, _TP, _vp, _TP, C.POINTER(RtenConvParams),
+                                           C.c_int, _TP, _TP]),
     "rten_b200_conv_integer": (C.c_int, [_vp, _TP, _TP, _vp, _TP, _TP, _TP, C.POINTER(RtenConvParams), _TP]),
     "rten_b200_quantized_linear": (C.c_int, [_vp, _TP, _TP, _TP, C.c_float, _TP, _vp, _TP, _TP, _TP, _TP, C.c_int, _TP]),
     "rten_b200_attention": (C.c_int, [_vp, _TP, _TP, _TP, _TP, _TP, C.POINTER(RtenAttentionParams), _TP, _TP, _TP]),

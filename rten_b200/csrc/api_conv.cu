@@ -793,6 +793,147 @@ rten_status conv_projected(OpScope& sc, ConvArgs& M, ConvArgs& P, rten_tensor* o
     return conv_core(sc, M, out);
 }
 
+// y = act(Conv(x, w, bias) [+ residual | + Conv(x_proj, ...)]) and z = act_next(Conv1x1(y, w_next, bias_next)): a
+// residual block's last convolution and the next block's first.  In single-pass TF32, a 1x1 convolution over a
+// channels-last input (with a 1x1 projection, as conv_projected folds it) whose N <= 256 output channels are a multiple
+// of 32, followed by a 1x1, stride-1, unpadded convolution to 64 or 128 channels, runs as ONE launch
+// (GemmLaunch::chain): z is computed from y's tiles as they are stored, and y is not read back.  Anything else runs as
+// the calls it replaces, with the same results.
+rten_status conv_chained(OpScope& sc, ConvArgs& M, ConvArgs* P, ConvArgs& Nx, rten_tensor* out, rten_tensor* out_next) {
+    rten_ctx* ctx = sc.ctx;
+    ConvShape sm, sp, sn;
+    RTB_TRY(conv_shape(sc, M, sm));
+    if (P) {
+        RTB_TRY(conv_shape(sc, *P, sp));
+        if (sm.one_d != sp.one_d || sm.B != sp.B || sm.O != sp.O || sm.OH != sp.OH || sm.OW != sp.OW)
+            return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "projection output shape does not match the convolution's output shape");
+    }
+    const int64_t B = sm.B, O = sm.O, OH = sm.OH, OW = sm.OW;
+    const rten_conv_params* np = Nx.p;
+    const bool next_1x1 = Nx.w->ndim == 4 && Nx.w->shape[1] == O && Nx.w->shape[2] == 1 && Nx.w->shape[3] == 1 &&
+                          np->groups == 1 && np->n_strides == 2 && np->n_dilations == 2 && np->strides[0] == 1 &&
+                          np->strides[1] == 1 && np->dilations[0] == 1 && np->dilations[1] == 1 && !np->auto_pad_same &&
+                          (np->pads[0] | np->pads[1] | np->pads[2] | np->pads[3]) == 0;
+    const int64_t N2 = Nx.w->ndim == 4 ? Nx.w->shape[0] : 0;
+    auto pointwise = [](const ConvShape& s) {
+        return !s.one_d && s.kh == 1 && s.kw == 1 && s.groups == 1 && (s.pt | s.pb | s.pl | s.pr) == 0 && s.dil[0] == 1 &&
+               s.dil[1] == 1 && s.x.strides[1] == 1 && s.C % 32 == 0;
+    };
+    auto nhwc = [](const ConvShape& s) {
+        OperandDesc d;
+        d.base = s.x.data;
+        d.dims[0] = s.C;
+        d.dims[1] = s.W;
+        d.dims[2] = s.H;
+        d.dims[3] = s.B;
+        d.strides[1] = s.x.strides[3];
+        d.strides[2] = s.x.strides[2];
+        d.strides[3] = s.x.strides[0];
+        return d;
+    };
+    const OperandDesc am = nhwc(sm);
+    OperandDesc ap;
+    if (P) ap = nhwc(sp);
+    rten_tensor res_v;
+    if (M.residual) RTB_TRY(sc.in(M.residual, &res_v));
+    const bool chain = ctx->f32_mode == RTEN_F32_TF32 && next_1x1 && (N2 == 64 || N2 == 128) && O % 32 == 0 && O <= 256 &&
+                       pointwise(sm) && tma_compatible(am, 4, 4) &&
+                       (!P || (pointwise(sp) && sp.strides[0] == sp.strides[1] && tma_compatible(ap, 4, 4))) &&
+                       (!M.residual || (res_v.ndim == 4 && res_v.strides[1] == 1)) && (!out->data || out->device >= 0) &&
+                       (!out_next->data || out_next->device >= 0) && B * O * OH * OW > 0;
+    if (chain) {
+        const int64_t oshape[4] = {B, O, OH, OW}, pref[4] = {OH * OW * O, 1, OW * O, O};
+        const int64_t zshape[4] = {B, N2, OH, OW}, zpref[4] = {OH * OW * N2, 1, OW * N2, N2};
+        rten_tensor ov, zv;
+        RTB_TRY(sc.out(out, RTEN_F32, 4, oshape, &ov, out->data ? nullptr : pref));
+        RTB_TRY(sc.out(out_next, RTEN_F32, 4, zshape, &zv, out_next->data ? nullptr : zpref));
+        for (int i = 0; M.residual && i < 4; i++)
+            if (res_v.shape[i] != oshape[i]) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "residual shape does not match output");
+        RTB_TRY(conv_shape(sc, Nx, sn));  // (x = y: checks w_next and bias_next against it)
+        const void *wm = nullptr, *wpj = nullptr, *wn = nullptr;
+        const int32_t* unused = nullptr;
+        RTB_TRY(conv_weight(ctx, M, sm, 4, &wm, &unused));
+        if (P) RTB_TRY(conv_weight(ctx, *P, sp, 4, &wpj, &unused));
+        RTB_TRY(conv_weight(ctx, Nx, sn, 4, &wn, &unused));
+        auto weights = [](const void* w, int64_t C, int64_t O_) {  // (c, o, 1, 1) of the packed [O, 1, 1, C]
+            OperandDesc d;
+            d.base = w;
+            d.dims[0] = C;
+            d.dims[1] = O_;
+            d.strides[1] = C;
+            return d;
+        };
+        GemmLaunch L;
+        L.kind = 0;
+        L.conv = 1;
+        L.N = (int)O;
+        L.K = (int)sm.C;
+        L.M = (int)(B * OH * OW);
+        L.g.B = (int)B;
+        L.g.H = (int)sm.H;
+        L.g.W = (int)sm.W;
+        L.g.C = (int)sm.C;
+        L.g.OH = (int)OH;
+        L.g.OW = (int)OW;
+        L.g.sy = (int)sm.strides[0];
+        L.g.sx = (int)sm.strides[1];
+        L.a = am;
+        L.b = weights(wm, sm.C, O);
+        if (P) {
+            L.proj.C = (int)sp.C;
+            L.proj.stride = (int)sp.strides[0];
+            L.proj.a = ap;
+            L.proj.b = weights(wpj, sp.C, O);
+        }
+        EpilogueDesc& e = L.epi;
+        e.d = ov.data;
+        e.s_z0 = ov.strides[0];
+        e.s_row = ov.strides[2];
+        e.s_z1 = ov.strides[3];
+        e.s_col = ov.strides[1];
+        e.act = M.act;
+        rten_tensor bm, bp, bn;
+        if (M.bias) RTB_TRY(sc.contiguous(&sm.bias_v, &bm));
+        if (P && P->bias) RTB_TRY(sc.contiguous(&sp.bias_v, &bp));
+        if (M.bias || (P && P->bias)) {
+            e.bias_kind = 1;
+            e.bias = (const float*)(M.bias ? bm.data : bp.data);
+            if (M.bias && P && P->bias) e.bias2 = (const float*)bp.data;
+        }
+        if (M.residual) {
+            e.r = (const float*)res_v.data;
+            e.r_z0 = res_v.strides[0];
+            e.r_row = res_v.strides[2];
+            e.r_z1 = res_v.strides[3];
+            e.r_col = res_v.strides[1];
+        }
+        GemmLaunch::Chain& c = L.chain;
+        c.N2 = (int)N2;
+        c.w = weights(wn, O, N2);
+        if (Nx.bias) {
+            RTB_TRY(sc.contiguous(&sn.bias_v, &bn));
+            c.bias = (const float*)bn.data;
+        }
+        c.act = Nx.act;
+        c.z.base = zv.data;
+        c.z.dims[0] = N2;
+        c.z.dims[1] = OW;
+        c.z.dims[2] = OH;
+        c.z.dims[3] = B;
+        c.z.strides[1] = zv.strides[3];
+        c.z.strides[2] = zv.strides[2];
+        c.z.strides[3] = zv.strides[0];
+        if (zv.strides[1] == 1) {
+            const rten_status st = launch_umma_gemm(ctx, L);
+            if (st != RTEN_ERR_UNSUPPORTED_VALUE) return st;
+        }
+        // (no chained launch for these operands: the separate calls)
+    }
+    RTB_TRY(P ? conv_projected(sc, M, *P, out) : conv_core(sc, M, out));
+    Nx.x = out;
+    return conv_core(sc, Nx, out_next);
+}
+
 }  // namespace
 
 extern "C" {
@@ -879,6 +1020,43 @@ rten_status rten_b200_conv2d_projected(rten_ctx* ctx, const rten_tensor* x, cons
     P.bias = bias_proj;
     P.p = p_proj;
     return sc.finish(conv_projected(sc, M, P, out));
+}
+
+rten_status rten_b200_conv2d_chained(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w, const rten_packed* pw,
+                                     const rten_tensor* bias, const rten_conv_params* p, const rten_tensor* residual,
+                                     const rten_tensor* x_proj, const rten_tensor* w_proj, const rten_packed* pw_proj,
+                                     const rten_tensor* bias_proj, const rten_conv_params* p_proj, int activation,
+                                     const rten_tensor* w_next, const rten_packed* pw_next, const rten_tensor* bias_next,
+                                     const rten_conv_params* p_next, int activation_next, rten_tensor* out,
+                                     rten_tensor* out_next) {
+    RTB_TRY(check_ctx(ctx));
+    if (!x || !w || !p || !w_next || !p_next || !out || !out_next || (x_proj && (!w_proj || !p_proj)))
+        return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    if (residual && x_proj) return fail(ctx, RTEN_ERR_INVALID_VALUE, "a residual and a projection shortcut are exclusive");
+    for (const rten_tensor* t : {x, w, bias, residual, x_proj, w_proj, bias_proj, w_next, bias_next})
+        if (t && t->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    OpScope sc(ctx);
+    ConvArgs M{}, P{}, Nx{};
+    M.kind = P.kind = Nx.kind = 0;
+    M.x = x;
+    M.w = w;
+    M.pw = pw;
+    M.bias = bias;
+    M.p = p;
+    M.residual = residual;
+    M.act = activation;
+    P.x = x_proj;
+    P.w = w_proj;
+    P.pw = pw_proj;
+    P.bias = bias_proj;
+    P.p = p_proj;
+    Nx.x = out;
+    Nx.w = w_next;
+    Nx.pw = pw_next;
+    Nx.bias = bias_next;
+    Nx.p = p_next;
+    Nx.act = activation_next;
+    return sc.finish(conv_chained(sc, M, x_proj ? &P : nullptr, Nx, out, out_next));
 }
 
 rten_status rten_b200_conv2d(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w, const rten_packed* pw,

@@ -153,6 +153,7 @@ struct Prepared {
     uint32_t dbox[4];
     int tma_store, res_tma;  // eligibility
     int wide;                // the wide-tile kernel may run this launch (plain f32 epilogue, see pick_epilogue)
+    int chain_bytes;         // > 0: a chained launch (GemmLaunch::chain) and the bytes of its resident second weights
     int step;
     int esize, kelems;
 };
@@ -160,8 +161,11 @@ struct Prepared {
 constexpr int SK_CNT_INTS = 1 << 16;
 // 227 KB of shared memory per block; SMEM_FIXED_BYTES: alignment slack, barriers, column vectors, accumulators
 static int smem_budget_for(int n_stg) { return 227 * 1024 - SMEM_FIXED_BYTES - n_stg * STG_BYTES; }
-// operand stages of the wide-tile kernel: 6 at bn = 128, 4 at bn = 256
-static int wide_stages(int stage_bytes) { return std::min(MAX_STAGES, (227 * 1024 - WIDE_SMEM_FIXED_BYTES) / stage_bytes); }
+// operand stages of the wide-tile kernel: 6 at bn = 128, 4 at bn = 256; chained at bn = 128, 4 with 64 KB of second
+// weights (N2 = 64), 2 with 128 KB (N2 = 128)
+static int wide_stages(int stage_bytes, int chain_bytes) {
+    return std::min(MAX_STAGES, (227 * 1024 - WIDE_SMEM_FIXED_BYTES - chain_bytes) / stage_bytes);
+}
 static bool is_wide(int bn) { return bn > ACC_STRIDE; }
 
 // The epilogue variant (umma_epilogue.cuh) of a launch with the given output path and split.  RTEN_B200_NO_FAST=1 sends every launch to Generic, RTEN_B200_NO_PLAIN=1 keeps launches off the plain variants
@@ -215,7 +219,7 @@ static bool plan_shape(const Prepared& q, const Plan& pl, PlanShape& ps) {
     }
     if (pl.nbuf < (q.res_tma ? 2 : 1) || pl.nbuf > 4) return false;  // staging buffers per group: res_bar has 4; a
                                                                      // TMA-staged residual needs two
-    ps.tiles_n = (p.N + pl.bn - 1) / pl.bn;
+    ps.tiles_n = q.chain_bytes ? 1 : (p.N + pl.bn - 1) / pl.bn;  // (chained: all N columns in one unit, by passes)
     ps.units_m = p.tiles_m;
     ps.tiles = ps.units_m * ps.tiles_n * q.batch;
     ps.units = ps.tiles * pl.splitk;
@@ -227,7 +231,7 @@ static bool plan_shape(const Prepared& q, const Plan& pl, PlanShape& ps) {
     }
     ps.n_stg = 2 * pl.nbuf;
     ps.stage_bytes = A_STAGE_BYTES + pl.bn * KBYTES;
-    ps.stages = is_wide(pl.bn) ? wide_stages(ps.stage_bytes) : std::min(MAX_STAGES, smem_budget_for(ps.n_stg) / ps.stage_bytes);
+    ps.stages = is_wide(pl.bn) ? wide_stages(ps.stage_bytes, q.chain_bytes) : std::min(MAX_STAGES, smem_budget_for(ps.n_stg) / ps.stage_bytes);
     if (ps.stages < 2) return false;
     return true;
 }
@@ -429,6 +433,18 @@ static rten_status prepare_launch(rten_ctx* ctx, const GemmLaunch& L, Prepared& 
             q.pes[i] = es[i];
         }
     }
+    // ---- chained 1x1 convolution of the output: the wide kernel's plain f32 epilogue, whole 32-column chunks, a unit
+    //      holds all N columns
+    q.chain_bytes = 0;
+    if (L.chain.N2 > 0) {
+        const GemmLaunch::Chain& c = L.chain;
+        if (!L.conv || L.kind != 0 || ctx->f32_mode != RTEN_F32_TF32 || !q.wide || !q.tma_store || L.epi.act > 1 ||
+            L.N % 32 || L.N > 256 || (c.N2 != 64 && c.N2 != 128) || c.act < 0 || c.act > 1 || c.w.dims[0] != L.N ||
+            c.w.dims[1] != c.N2 || c.z.dims[0] != c.N2 || !tma_compatible(c.w, 4, 4) || !tma_compatible(c.z, 4, 4) ||
+            (L.epi.r && !q.res_tma))
+            return RTEN_ERR_UNSUPPORTED_VALUE;
+        q.chain_bytes = L.N / 32 * c.N2 * KBYTES;
+    }
     return RTEN_OK;
 }
 
@@ -486,7 +502,7 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
     TmaMaps m;
     if (!encode_map(ctx, &m.a, L.a, q.esize, L.kind == 0, q.abox, q.aes)) return RTEN_ERR_UNSUPPORTED_VALUE;
     if (!encode_map(ctx, &m.b, L.b, q.esize, L.kind == 0, bbox, bes)) return RTEN_ERR_UNSUPPORTED_VALUE;
-    m.d = m.r = m.a2 = m.a_proj = m.b_proj = m.a2_proj = m.a;  // (maps the launch does not use)
+    m.d = m.r = m.a2 = m.a_proj = m.b_proj = m.a2_proj = m.w2 = m.z = m.a;  // (maps the launch does not use)
     p.x3_cb = L.x3_cb;
     if (L.x3_cb && !encode_map(ctx, &m.a2, L.a_lo, q.esize, true, q.abox, q.aes)) return RTEN_ERR_UNSUPPORTED_VALUE;
     if (p.kb_proj) {
@@ -508,14 +524,26 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
     const Epi epi = pick_epilogue(L, p.tma_store, p.res_tma, p.splitk);
     // the generic epilogue takes a TMA-staged residual only on its register path (f32, act <= Relu)
     if (epi == Epi::Generic && (L.kind == 1 || L.epi.act > 1)) p.res_tma = 0;
+    if (q.chain_bytes) {
+        const GemmLaunch::Chain& c = L.chain;
+        const uint32_t wbox[4] = {32, (uint32_t)c.N2, 1, 1}, zbox[4] = {32, q.dbox[1], q.dbox[2], q.dbox[3]};
+        if (epi != Epi::PlainF32 || (L.epi.r && !p.res_tma) || !encode_map(ctx, &m.w2, c.w, 4, true, wbox, des) ||
+            !encode_map(ctx, &m.z, c.z, 4, true, zbox, des))
+            return RTEN_ERR_UNSUPPORTED_VALUE;
+        p.chain_n2 = c.N2;
+        p.chain_passes = (L.N + p.bn - 1) / p.bn;
+        p.chain_act = c.act;
+        p.chain_bias = c.bias;
+    }
 
     if (verbose)
-        fprintf(stderr, "[umma_gemm] kind=%d conv=%d M=%d N=%d K=%d kb=%d kb_proj=%d tiles_m=%d bn=%d splitk=%d units=%d stages=%d tma_store=%d res_tma=%d nbuf=%d box=%dx%dx%d epi=%s\n",
+        fprintf(stderr, "[umma_gemm] kind=%d conv=%d M=%d N=%d K=%d kb=%d kb_proj=%d tiles_m=%d bn=%d splitk=%d units=%d stages=%d tma_store=%d res_tma=%d nbuf=%d box=%dx%dx%d epi=%s%s\n",
                 L.kind, L.conv, L.M, L.N, L.K, p.k_blocks, p.kb_proj, p.tiles_m, p.bn, p.splitk, p.units_total, p.stages,
-                p.tma_store, p.res_tma, p.nbuf, p.tw, p.th, p.tb, epi_name(epi));
+                p.tma_store, p.res_tma, p.nbuf, p.tw, p.th, p.tb, epi_name(epi),
+                p.chain_n2 == 64 ? " chain=64" : p.chain_n2 == 128 ? " chain=128" : "");
     // (an output / residual map failed to encode; a projection source and a second bias need the plain f32 epilogue)
     if ((is_wide(p.bn) || p.kb_proj || L.epi.bias2) && !is_plain_f32(epi)) return RTEN_ERR_UNSUPPORTED_VALUE;
-    const size_t smem_bytes = (size_t)p.stages * p.stage_bytes +
+    const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + q.chain_bytes +
                               (is_wide(p.bn) ? WIDE_SMEM_FIXED_BYTES : ps.n_stg * STG_BYTES + SMEM_FIXED_BYTES);
     using Kernel = void (*)(TmaMaps, KParams);
     // [kind][variant]: the integer kind has no plain f32 kernels, the f32 kind no plain integer ones
@@ -525,6 +553,8 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
         {umma_gemm_kernel<1, Epi::Generic>, umma_gemm_kernel<1, Epi::Fast>, umma_gemm_kernel<1, Epi::FastGelu>, nullptr,
          nullptr, umma_gemm_kernel<1, Epi::PlainI8>, umma_gemm_kernel<1, Epi::PlainI8Gelu>}};
     const Kernel kern = !is_wide(p.bn)              ? narrow[L.kind][(int)epi]
+                        : p.chain_n2 == 64         ? umma_wide_kernel<Epi::PlainF32, 64>
+                        : p.chain_n2 == 128        ? umma_wide_kernel<Epi::PlainF32, 128>
                         : epi == Epi::PlainF32Gelu ? umma_wide_kernel<Epi::PlainF32Gelu>
                                                    : umma_wide_kernel<Epi::PlainF32>;
 
@@ -674,6 +704,18 @@ static rten_status launch_tf32x3(rten_ctx* ctx, const GemmLaunch& L0) {
 }
 
 rten_status launch_umma_gemm(rten_ctx* ctx, const GemmLaunch& L) {
+    if (L.chain.N2 > 0) {
+        // chained: a fixed plan (128-column passes of one pixel tile), not autotuned; single-pass TF32 only (a 3xTF32
+        // chain would not equal the separate launches)
+        if (L.kind != 0 || ctx->f32_mode != RTEN_F32_TF32 || L.x3_cb || getenv("RTEN_B200_NO_CHAIN"))
+            return RTEN_ERR_UNSUPPORTED_VALUE;
+        Prepared q;
+        RTB_TRY(prepare_launch(ctx, L, q));
+        Plan pl;
+        pl.bn = 128;
+        pl.nbuf = 2;
+        return launch_plan(ctx, L, q, pl, getenv("RTEN_B200_VERBOSE") != nullptr);
+    }
     if (L.kind == 0 && ctx->f32_mode == RTEN_F32_TF32X3) return launch_tf32x3(ctx, L);
     // stride-1 windows (the 3x3 layers): the halo-reuse kernel moves the activations into shared memory once per channel
     // block instead of once per filter tap (umma_halo.cu); everything it does not cover falls through

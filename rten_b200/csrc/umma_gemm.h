@@ -95,6 +95,17 @@ struct GemmLaunch {
         int x3_cb = 0;               // internal, as x3_cb / a_lo above
         OperandDesc a_lo;
     } proj;
+    // optional chained 1x1 convolution of the output (`chain.N2` > 0): z = act(D * W^T + bias) over N2 columns, computed
+    // from the output tile while it is staged for its store, so D is not read back.  Runs only for a conv launch in
+    // single-pass TF32 with the plain f32 epilogue (no Gelu), N % 32 == 0, N <= 256, N2 in {64, 128}, TMA-addressable
+    // w and z (else RTEN_ERR_UNSUPPORTED_VALUE).
+    struct Chain {
+        int N2 = 0;
+        OperandDesc w;  // (c, o, 1, 1): dims {N, N2}, K-major
+        const float* bias = nullptr;
+        int act = 0;    // 0 none, 1 relu
+        OperandDesc z;  // (n, x, y, b) of the NHWC output: dims {N2, OW, OH, B}
+    } chain;
 };
 
 // Returns RTEN_OK and enqueues the kernel, or RTEN_ERR_UNSUPPORTED_VALUE (without touching ctx->err

@@ -82,6 +82,10 @@ struct KParams {
     // tma_b_proj at (c, n0, 0, 0); x3_cb_proj is its own two-plane 3xTF32 segment length (low parts: tma_a2_proj).
     // Without one, kb_main = k_blocks.
     int kb_main, kb_proj, s_proj, x3_cb_proj;
+    // Chained 1x1 convolution (umma_wide_kernel with CHAIN_N2 > 0): a unit is one pixel tile x all N columns, computed
+    // in chain_passes passes of bn columns; z = act(y * W2 + chain_bias) over chain_n2 columns, from the staged y chunks
+    int chain_n2, chain_passes, chain_act;
+    const float* chain_bias;
     FastDiv d_tiles_n, d_tiles_m, d_z0, d_tiles_x, d_tiles_y, d_tiles_total, d_c_blocks, d_kw, d_tw, d_th;
     uint32_t* sk_ws;
     int* sk_cnt;
@@ -234,7 +238,7 @@ __device__ __forceinline__ void splitk_sum(const KParams& p, int t, int c0, int 
 
 struct SmemLayout {
     uint8_t* smem;  // operand stages (1024-B aligned), staging buffers behind them
-    uint64_t *full_bar, *empty_bar, *acc_full, *acc_empty, *res_bar;
+    uint64_t *full_bar, *empty_bar, *acc_full, *acc_empty, *res_bar, *w_bar;
     int* sk_flag;
     float* bias;
     uint32_t acc_smem;  // accumulator tiles (ptx.cuh), between the column vectors and the operand stages
@@ -308,9 +312,9 @@ __device__ __forceinline__ void mma_role(const KParams& p, const SmemLayout& L, 
 }
 
 // The tensor maps of one launch: main operands, output, residual, the low-part plane of A (3xTF32) and the projection
-// source's A, B and low-part plane (KParams::kb_main).
+// source's A, B and low-part plane (KParams::kb_main); a chained launch's second weights and output (KParams::chain_n2).
 struct TmaMaps {
-    CUtensorMap a, b, d, r, a2, a_proj, b_proj, a2_proj;
+    CUtensorMap a, b, d, r, a2, a_proj, b_proj, a2_proj, w2, z;
 };
 
 __device__ __forceinline__ void prefetch_maps(const TmaMaps& m, const KParams& p) {
@@ -329,6 +333,9 @@ __device__ __forceinline__ void prefetch_maps(const TmaMaps& m, const KParams& p
 // TMA producer of both GEMM kernels: one warp walks this CTA's work units and fills the operand ring -- A (128 rows)
 // and B (bn rows) of one 128-byte K block per stage, the conv filter tap / channel walk, the two-plane 3xTF32 segments,
 // the projection source and broadcast batch dims.  Runs warp-uniformly, one elected lane issues.
+// CHAIN: a unit is one pixel tile in p.chain_passes passes of bn columns, and the chained convolution's weights (N / 32
+// K blocks of chain_n2 rows) are loaded once, behind the operand stages, on L.w_bar.
+template <bool CHAIN = false>
 __device__ __forceinline__ void producer_role(const KParams& p, const TmaMaps& m, const SmemLayout& L, int worker,
                                               int n_workers) {
     uint8_t* smem = L.smem;
@@ -338,10 +345,12 @@ __device__ __forceinline__ void producer_role(const KParams& p, const TmaMaps& m
     const uint32_t smem0 = smem_u32(smem);
     const uint32_t full0 = smem_u32(L.full_bar);
     for (int u = worker; u < p.units_total; u += n_workers) {
+      for (int pass = 0; pass < (CHAIN ? p.chain_passes : 1); pass++) {
         int t, ks;
         p.d_tiles_total.divmod(u, ks, t);
         const int kb0 = ks * p.kb_per, kb1 = min(p.k_blocks, kb0 + p.kb_per);
-        const TileCoord tc = decode_tile(p, t);
+        TileCoord tc = decode_tile(p, t);
+        if (CHAIN) tc.n0 += pass * p.bn;
         // projection source: its blocks follow the main source's, one filter tap, its own channel and segment walk
         bool proj = kb0 >= p.kb_main;
         int x3 = proj ? p.x3_cb_proj : p.x3_cb;
@@ -358,7 +367,17 @@ __device__ __forceinline__ void producer_role(const KParams& p, const TmaMaps& m
             }
         // programmatic dependent launch: the producer is the first to touch the predecessor's output; everything
         // above (tile decode) ran while the predecessor grid was still draining
-        if (u == worker) asm volatile("griddepcontrol.wait;" ::: "memory");
+        if (u == worker && pass == 0) {
+            asm volatile("griddepcontrol.wait;" ::: "memory");
+            if (CHAIN && elect_one()) {
+                const int cb2 = p.N / 32;
+                const uint32_t wbytes = (uint32_t)(p.chain_n2 * KBYTES);
+                uint8_t* w2 = smem + (size_t)p.stages * p.stage_bytes;
+                mbar_expect_tx(L.w_bar, cb2 * wbytes);
+                for (int c = 0; c < cb2; c++) tma_load_4d(w2 + c * wbytes, &m.w2, L.w_bar, 32 * c, 0, 0, 0);
+            }
+            if (CHAIN) __syncwarp();
+        }
         for (int kb = kb0; kb < kb1; kb++) {
             if (kb == p.kb_main) {  // (never without a projection source: kb_main = k_blocks)
                 proj = true;
@@ -405,6 +424,7 @@ __device__ __forceinline__ void producer_role(const KParams& p, const TmaMaps& m
             ring ^= 1u << stage;
             if (++stage == p.stages) stage = 0;
         }
+      }
     }
 }
 
@@ -517,26 +537,100 @@ __device__ __forceinline__ void wgmma_wide(float (&d)[N / 2], uint64_t adesc, ui
 // both consumer warpgroups (named barrier 1)
 __device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-// Operand stages first (1024-B aligned, like the staging buffers behind them), the small items last.
+// Bytes of a chained launch's resident second weights: N / 32 K blocks of chain_n2 rows x 128 B.
+__device__ __forceinline__ int chain_w_bytes(const KParams& p) { return (p.N / 32) * p.chain_n2 * KBYTES; }
+
+// Operand stages first (1024-B aligned, like the staging buffers behind them), then a chained launch's second weights,
+// the staging buffers, the small items last.
+template <bool CHAIN>
 __device__ __forceinline__ SmemLayout carve_wide_smem(uint8_t* smem_raw, const KParams& p) {
     uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* tail = base + (size_t)p.stages * p.stage_bytes + 2 * STG_BYTES;
+    uint8_t* tail = base + (size_t)p.stages * p.stage_bytes + (CHAIN ? chain_w_bytes(p) : 0) + 2 * STG_BYTES;
     SmemLayout L;
     L.smem = base;
     L.full_bar = reinterpret_cast<uint64_t*>(tail);
     L.empty_bar = L.full_bar + MAX_STAGES;
     L.res_bar = L.empty_bar + MAX_STAGES;  // [staging buffer]
+    L.w_bar = L.res_bar + 2;
     L.acc_full = L.acc_empty = nullptr;
     L.sk_flag = nullptr;
-    L.bias = reinterpret_cast<float*>(tail + 256);
+    L.bias = reinterpret_cast<float*>(tail + 256);  // up to 1.5 KB: [0, 256) the unit's columns, [256, 384) chained
     L.acc_smem = 0;
     return L;
 }
 
-// Main loop and epilogue of one consumer warpgroup (wg = 0: rows 0-63, 1: rows 64-127).  Each 128-byte K block is four
-// k8 wgmma, one commit group, one group in flight across stages as in mma_units; a stage goes back to the producer
-// once both warpgroups have retired it (8 warp arrivals).  Epilogue: plain_f32_pair, then act4 for Gelu, as in the
-// narrow kernel's PlainF32 variant -- the results equal the narrow kernel's.
+// The K loop of one wide-tile consumer warpgroup into d (see wide_consumer): four k8 wgmma per 128-byte K block, one
+// commit group, one group in flight across stages; a stage goes back to the producer once both warpgroups have retired
+// it (8 warp arrivals).
+template <int N>
+__device__ __forceinline__ void wide_main_loop(const KParams& p, const SmemLayout& L, float (&d)[N / 2], int wg, int lane,
+                                               int& stage, uint32_t& ring) {
+    const uint32_t smem0 = smem_u32(L.smem);
+#pragma unroll
+    for (int i = 0; i < N / 2; i++) d[i] = 0.0f;
+    int prev = -1;
+    for (int kb = 0; kb < p.k_blocks; kb++) {
+        mbar_wait(&L.full_bar[stage], (ring >> stage) & 1);
+        wgmma_fence_operand(d);
+        wgmma_fence();
+        const uint32_t sa = smem0 + stage * p.stage_bytes;
+        const uint64_t adesc = make_kmajor_sw128_desc(sa + wg * (64 * KBYTES));
+        const uint64_t bdesc = make_kmajor_sw128_desc(sa + A_STAGE_BYTES);
+#pragma unroll
+        for (int k = 0; k < 4; k++) wgmma_wide<N>(d, adesc + 2 * k, bdesc + 2 * k);
+        wgmma_commit();
+        wgmma_fence_operand(d);
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
+        prev = stage;
+        ring ^= 1u << stage;
+        if (++stage == p.stages) stage = 0;
+    }
+    wgmma_wait<0>();
+    wgmma_fence_operand(d);
+    if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
+}
+
+// Columns 32k .. 32k + 31 of a wide accumulator (fragment rows row0, row0 + 8; columns 8j + 2cq + {0, 1}) through
+// plain_f32_pair -- residual from the staging buffer, bias from `bias` (the chunk's 32 values), Relu -- then act4 for
+// Gelu, into the 128-row, 128B-swizzled staging buffer `stg`.  `valid` = false (a chunk past N) stores d unchanged.
+template <Epi E, int NA>
+__device__ __forceinline__ void stage_chunk(float (&d)[NA], int k, uint8_t* stg, const float* bias, bool valid, bool res,
+                                            int act, int row0, int sw, int cq) {
+#pragma unroll
+    for (int j = 0; j < 4; j++) {  // columns 32k + 8j + 2cq + {0, 1}, rows row0 + 8h
+        const int i0 = 16 * k + 4 * j;
+        float2* px[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+            px[h] = reinterpret_cast<float2*>(stg + (row0 + 8 * h) * 128 + (((2 * j + (cq >> 1)) ^ sw) << 4) + 8 * (cq & 1));
+        if (valid) {
+            const float2 bb = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * cq);
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                uint32_t v0 = __float_as_uint(d[i0 + 2 * h]), v1 = __float_as_uint(d[i0 + 2 * h + 1]);
+                float2 rr = make_float2(0.f, 0.f);
+                if (res) rr = *px[h];
+                plain_f32_pair(v0, v1, res, rr, bb, act == 1);
+                d[i0 + 2 * h] = __uint_as_float(v0);
+                d[i0 + 2 * h + 1] = __uint_as_float(v1);
+            }
+            if (E == Epi::PlainF32Gelu) {  // Gelu / ApproxGelu: the out-of-line polynomial, four values per call
+                const float4 g = act4(make_float4(d[i0], d[i0 + 1], d[i0 + 2], d[i0 + 3]), act);
+                d[i0] = g.x;
+                d[i0 + 1] = g.y;
+                d[i0 + 2] = g.z;
+                d[i0 + 3] = g.w;
+            }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; h++) *px[h] = make_float2(d[i0 + 2 * h], d[i0 + 2 * h + 1]);
+    }
+}
+
+// Main loop (wide_main_loop) and epilogue of one consumer warpgroup (wg = 0: rows 0-63, 1: rows 64-127).  Epilogue:
+// plain_f32_pair, then act4 for Gelu, as in the narrow kernel's PlainF32 variant -- the results equal the narrow
+// kernel's.
 template <Epi E, int N>
 __device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout& L, const CUtensorMap* tma_d,
                                               const CUtensorMap* tma_r, int worker, int n_workers) {
@@ -548,7 +642,6 @@ __device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout
     const int cq = lane & 3;                                           // columns 8j + 2cq + {0, 1} of every 8
     const bool issuer = t == 0;
     const EpilogueDesc& e = p.epi;
-    const uint32_t smem0 = smem_u32(L.smem);
     uint8_t* const stg0 = L.smem + (size_t)p.stages * p.stage_bytes;
     float* const bias_s = L.bias;
     uint32_t ring = 0, rphase = 0;
@@ -572,29 +665,7 @@ __device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout
             }
         }
         float d[N / 2];
-#pragma unroll
-        for (int i = 0; i < N / 2; i++) d[i] = 0.0f;
-        int prev = -1;
-        for (int kb = 0; kb < p.k_blocks; kb++) {
-            mbar_wait(&L.full_bar[stage], (ring >> stage) & 1);
-            wgmma_fence_operand(d);
-            wgmma_fence();
-            const uint32_t sa = smem0 + stage * p.stage_bytes;
-            const uint64_t adesc = make_kmajor_sw128_desc(sa + wg * (64 * KBYTES));
-            const uint64_t bdesc = make_kmajor_sw128_desc(sa + A_STAGE_BYTES);
-#pragma unroll
-            for (int k = 0; k < 4; k++) wgmma_wide<N>(d, adesc + 2 * k, bdesc + 2 * k);
-            wgmma_commit();
-            wgmma_fence_operand(d);
-            wgmma_wait<1>();
-            if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
-            prev = stage;
-            ring ^= 1u << stage;
-            if (++stage == p.stages) stage = 0;
-        }
-        wgmma_wait<0>();
-        wgmma_fence_operand(d);
-        if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
+        wide_main_loop<N>(p, L, d, wg, lane, stage, ring);
         const TileCoord tc = decode_tile(p, u);
         consumers_sync();
 #pragma unroll
@@ -612,35 +683,8 @@ __device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout
                 mbar_wait(&L.res_bar[buf], (rphase >> buf) & 1);
                 rphase ^= 1u << buf;
             }
-#pragma unroll
-            for (int j = 0; j < 4; j++) {  // columns 32k + 8j + 2cq + {0, 1}, rows row0 + 8h
-                const int i0 = 16 * k + 4 * j;
-                float2* px[2];
-#pragma unroll
-                for (int h = 0; h < 2; h++)
-                    px[h] = reinterpret_cast<float2*>(stg + (row0 + 8 * h) * 128 + (((2 * j + (cq >> 1)) ^ sw) << 4) + 8 * (cq & 1));
-                if (nbase < p.N) {  // (a tile may overhang N by whole chunks: the TMA store clips them)
-                    const float2 bb = *reinterpret_cast<const float2*>(bias_s + 32 * k + 8 * j + 2 * cq);
-#pragma unroll
-                    for (int h = 0; h < 2; h++) {
-                        uint32_t v0 = __float_as_uint(d[i0 + 2 * h]), v1 = __float_as_uint(d[i0 + 2 * h + 1]);
-                        float2 rr = make_float2(0.f, 0.f);
-                        if (p.res_tma) rr = *px[h];
-                        plain_f32_pair(v0, v1, p.res_tma, rr, bb, e.act == 1);
-                        d[i0 + 2 * h] = __uint_as_float(v0);
-                        d[i0 + 2 * h + 1] = __uint_as_float(v1);
-                    }
-                    if (E == Epi::PlainF32Gelu) {  // Gelu / ApproxGelu: the out-of-line polynomial, four values per call
-                        const float4 g = act4(make_float4(d[i0], d[i0 + 1], d[i0 + 2], d[i0 + 3]), e.act);
-                        d[i0] = g.x;
-                        d[i0 + 1] = g.y;
-                        d[i0 + 2] = g.z;
-                        d[i0 + 3] = g.w;
-                    }
-                }
-#pragma unroll
-                for (int h = 0; h < 2; h++) *px[h] = make_float2(d[i0 + 2 * h], d[i0 + 2 * h + 1]);
-            }
+            // (a tile may overhang N by whole chunks: the TMA store clips them)
+            stage_chunk<E>(d, k, stg, bias_s + 32 * k, nbase < p.N, p.res_tma, e.act, row0, sw, cq);
             fence_proxy_async();
             consumers_sync();
             if (issuer) {
@@ -653,20 +697,132 @@ __device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout
     if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
 
-template <Epi E>
+// A chained unit (umma_wide_kernel with N2 > 0): one conv pixel tile x all N <= 256 columns of y = act(conv + residual
+// or projection + bias), computed in 128-column passes (rows of one warpgroup: d[64]), and z = act2(y * W2 + b2) over
+// N2 columns (acc2[N2 / 2]).  Each staged 32-column chunk of y is, as the 128B-swizzled 128-row buffer the TMA store
+// reads, also the K-major SW128 A operand of one 32-channel K block of z: once it is visible, each warpgroup issues four
+// m64nN2k8 wgmma from it (its own 64 rows) against the resident W2 block.  They run behind the next chunk's epilogue and
+// retire (wgmma_wait<0> before the chunk barrier) before the buffer they read is reused: the next residual TMA load
+// into it, issued after that barrier, and the writes of the chunk after next.  The issuer waits for the previous chunk's
+// TMA store before the barrier too, so no chunk writes into a buffer a store still reads.  K order and epilogue equal
+// those of the separate 1x1 convolution of y: z is bit-identical to it.
+template <int N2>
+__device__ __forceinline__ void wide_chain_consumer(const KParams& p, const SmemLayout& L, const TmaMaps& m, int worker,
+                                                    int n_workers) {
+    constexpr int N = 128;  // columns of a pass
+    const int t = threadIdx.x - 128;
+    const int wg = t >> 7;
+    const int lane = threadIdx.x & 31;
+    const int row0 = 64 * wg + 16 * ((t & 127) >> 5) + (lane >> 2);
+    const int sw = lane >> 2;
+    const int cq = lane & 3;
+    const bool issuer = t == 0;
+    const EpilogueDesc& e = p.epi;
+    const uint32_t w2 = smem_u32(L.smem) + p.stages * p.stage_bytes;
+    uint8_t* const stg0 = L.smem + (size_t)p.stages * p.stage_bytes + chain_w_bytes(p);
+    float* const bias_s = L.bias;
+    uint32_t ring = 0, rphase = 0;
+    uint32_t ci = 0;  // chunks of this CTA so far: chunk ci uses staging buffer ci & 1
+    int stage = 0;
+    auto load_residual = [&](const TileCoord& tc, int c0, int buf) {
+        uint64_t* rb = &L.res_bar[buf];
+        mbar_expect_tx(rb, p.res_tx_bytes);
+        const int4 x = out_coord(p, tc, c0);
+        tma_load_4d(stg0 + buf * STG_BYTES, &m.r, rb, x.x, x.y, x.z, x.w);
+    };
+    // closes chunk ci in buffer stg: the other buffer's wgmma have retired and its store has been read, then the barrier
+    auto chunk_barrier = [&](float (&acc2)[N2 / 2]) {
+        wgmma_wait<0>();
+        wgmma_fence_operand(acc2);
+        if (issuer) bulk_wait_read(0);
+        fence_proxy_async();
+        consumers_sync();
+    };
+    mbar_wait(L.w_bar, 0);
+    for (int u = worker; u < p.units_total; u += n_workers) {
+        {
+            const TileCoord tc = decode_tile(p, u);
+            if (t < p.N) bias_s[t] = e.bias_kind == 1 ? column_bias(e, t) : 0.0f;
+            if (t < N2) bias_s[256 + t] = p.chain_bias ? __ldg(p.chain_bias + t) : 0.0f;
+            if (issuer && p.res_tma) load_residual(tc, 0, ci & 1);
+        }
+        float acc2[N2 / 2];
+#pragma unroll
+        for (int i = 0; i < N2 / 2; i++) acc2[i] = 0.0f;
+        for (int pass = 0; pass < p.chain_passes; pass++) {
+            float d[N / 2];
+            wide_main_loop<N>(p, L, d, wg, lane, stage, ring);
+            const TileCoord tc = decode_tile(p, u);
+            consumers_sync();
+#pragma unroll
+            for (int k = 0; k < N / 32; k++) {
+                const int c0 = N * pass + 32 * k;
+                if (c0 >= p.N) break;  // (N % 32 == 0: whole chunks; uniform over the CTA)
+                const int buf = ci & 1;
+                uint8_t* stg = stg0 + buf * STG_BYTES;
+                if (p.res_tma) {
+                    mbar_wait(&L.res_bar[buf], (rphase >> buf) & 1);
+                    rphase ^= 1u << buf;
+                }
+                stage_chunk<Epi::PlainF32>(d, k, stg, bias_s + c0, true, p.res_tma, e.act, row0, sw, cq);
+                chunk_barrier(acc2);
+                if (issuer) {
+                    const int4 x = out_coord(p, tc, c0);
+                    tma_store_4d(&m.d, stg, x.x, x.y, x.z, x.w);
+                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+                    if (p.res_tma && c0 + 32 < p.N) load_residual(tc, c0 + 32, buf ^ 1);
+                }
+                wgmma_fence();
+                const uint64_t adesc = make_kmajor_sw128_desc(smem_u32(stg) + wg * (64 * KBYTES));
+                const uint64_t bdesc = make_kmajor_sw128_desc(w2 + (c0 / 32) * (N2 * KBYTES));
+#pragma unroll
+                for (int kk = 0; kk < 4; kk++) {
+                    if constexpr (N2 == 64) wgmma_tf32_n64(acc2, adesc + 2 * kk, bdesc + 2 * kk);
+                    else wgmma_tf32_n128(acc2, adesc + 2 * kk, bdesc + 2 * kk);
+                }
+                wgmma_commit();
+                wgmma_fence_operand(acc2);
+                ci++;
+            }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_operand(acc2);
+        const TileCoord tc = decode_tile(p, u);
+#pragma unroll
+        for (int k = 0; k < N2 / 32; k++, ci++) {
+            uint8_t* stg = stg0 + (ci & 1) * STG_BYTES;
+            stage_chunk<Epi::PlainF32>(acc2, k, stg, bias_s + 256 + 32 * k, true, false, p.chain_act, row0, sw, cq);
+            chunk_barrier(acc2);
+            if (issuer) {
+                tma_store_4d(&m.z, stg, 32 * k, tc.ox0, tc.oy0, tc.b0);
+                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+            }
+        }
+    }
+    if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+}
+
+// CHAIN_N2 > 0: the chained launches (wide_chain_consumer), plain f32 epilogue only
+template <Epi E, int CHAIN_N2 = 0>
 __global__ void __launch_bounds__(WIDE_THREADS, 1)
 umma_wide_kernel(const __grid_constant__ TmaMaps m, const __grid_constant__ KParams p) {
     extern __shared__ uint8_t smem_raw[];
-    const SmemLayout L = carve_wide_smem(smem_raw, p);
+    const SmemLayout L = carve_wide_smem<(CHAIN_N2 > 0)>(smem_raw, p);
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) prefetch_maps(m, p);
+    if (threadIdx.x == 0) {
+        prefetch_maps(m, p);
+        if constexpr (CHAIN_N2 > 0) {
+            tma_prefetch_desc(&m.w2);
+            tma_prefetch_desc(&m.z);
+        }
+    }
     if (warp == 1) {
         if (lane < MAX_STAGES) {
             mbar_init(&L.full_bar[lane], 1);
             mbar_init(&L.empty_bar[lane], 8);  // one arrival per consumer warp
-        } else if (lane < MAX_STAGES + 2) {
-            mbar_init(&L.res_bar[lane - MAX_STAGES], 1);
+        } else if (lane < MAX_STAGES + (CHAIN_N2 > 0 ? 3 : 2)) {
+            mbar_init(&L.res_bar[lane - MAX_STAGES], 1);  // (chained: + L.w_bar)
         }
         fence_mbar_init();
     }
@@ -677,14 +833,18 @@ umma_wide_kernel(const __grid_constant__ TmaMaps m, const __grid_constant__ KPar
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     if (warp < 4) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-        if (warp == 0) producer_role(p, m, L, (int)blockIdx.x, (int)gridDim.x);
+        if (warp == 0) producer_role<(CHAIN_N2 > 0)>(p, m, L, (int)blockIdx.x, (int)gridDim.x);
     } else {
         asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-        // (Gelu: 128 columns only -- the out-of-line act4 calls would spill around 128 live accumulators per thread)
-        if (E == Epi::PlainF32Gelu || p.bn == 128)
-            wide_consumer<E, 128>(p, L, &m.d, &m.r, (int)blockIdx.x, (int)gridDim.x);
-        else
-            wide_consumer<E, 256>(p, L, &m.d, &m.r, (int)blockIdx.x, (int)gridDim.x);
+        if constexpr (CHAIN_N2 > 0) {
+            wide_chain_consumer<CHAIN_N2>(p, L, m, (int)blockIdx.x, (int)gridDim.x);
+        } else {
+            // (Gelu: 128 columns only -- the out-of-line act4 calls would spill around 128 live accumulators per thread)
+            if (E == Epi::PlainF32Gelu || p.bn == 128)
+                wide_consumer<E, 128>(p, L, &m.d, &m.r, (int)blockIdx.x, (int)gridDim.x);
+            else
+                wide_consumer<E, 256>(p, L, &m.d, &m.r, (int)blockIdx.x, (int)gridDim.x);
+        }
     }
 }
 

@@ -102,10 +102,13 @@ class ResNet50Runner:
     """Executes the op list on one GPU with activations resident in HBM (channels-last strides;
     logical shapes stay NCHW at the ABI).  `fuse=True` uses the epilogue fusions (bias + residual +
     Relu inside the conv kernel) and runs a projection block's last conv and its downsample conv as one call, so the
-    shortcut tensor is never written; `fuse=False` issues the reference's separate Conv / Add / Relu ops."""
+    shortcut tensor is never written; `fuse=False` issues the reference's separate Conv / Add / Relu ops.  With `fuse`,
+    `chain=True` also runs each block's last conv together with the next block's first (Conv.run_chained): where the
+    pair qualifies (the layer-1 blocks in single-pass TF32) the block output is not read back for it, elsewhere the
+    call runs as the separate convolutions."""
 
-    def __init__(self, ctx: O.Context, spec: ResNet50Spec, fuse: bool = True):
-        self.ctx, self.spec, self.fuse = ctx, spec, fuse
+    def __init__(self, ctx: O.Context, spec: ResNet50Spec, fuse: bool = True, chain: bool = True):
+        self.ctx, self.spec, self.fuse, self.chain = ctx, spec, fuse, chain
         self._convs = {}
 
         def prep(c: ConvSpec):
@@ -145,19 +148,37 @@ class ResNet50Runner:
         op.activation = O.ACT_RELU
         return op.run_projected(self.ctx, t, w, b, packed_w=pk, proj=dop, x_proj=x, w_proj=dw, bias_proj=db, packed_w_proj=dpk)
 
+    def _conv_chained(self, b: Bottleneck, t, x, nxt: ConvSpec):
+        """(relu(b.c3(t) + shortcut(x)), relu(nxt(that))) in one call (Conv.run_chained)."""
+        op, w, bias, pk = self._convs[id(b.c3)]
+        nop, nw, nb, npk = self._convs[id(nxt)]
+        op.activation = nop.activation = O.ACT_RELU
+        kw = dict(nxt=nop, w_next=nw, bias_next=nb, packed_w_next=npk)
+        if b.down is None:
+            return op.run_chained(self.ctx, t, w, bias, packed_w=pk, residual=x, **kw)
+        dop, dw, db, dpk = self._convs[id(b.down)]
+        return op.run_chained(self.ctx, t, w, bias, packed_w=pk, proj=dop, x_proj=x, w_proj=dw, bias_proj=db,
+                              packed_w_proj=dpk, **kw)
+
     def run(self, x: O.DeviceTensor) -> O.DeviceTensor:
         """x: [B,3,224,224] f32 (any strides) -> logits [B,1000]."""
         s = self.spec
         y = self._conv(s.stem, x, True)
         y = self.maxpool.run(self.ctx, y)
-        for b in s.blocks:
+        t1 = None  # the block's first conv, when the previous block's call computed it
+        for i, b in enumerate(s.blocks):
+            if self.fuse and self.chain and i + 1 < len(s.blocks):
+                t = t1 if t1 is not None else self._conv(b.c1, y, True)
+                t = self._conv(b.c2, t, True)
+                y, t1 = self._conv_chained(b, t, y, s.blocks[i + 1].c1)
+                continue
             if self.fuse and b.down is not None:
                 t = self._conv(b.c1, y, True)
                 t = self._conv(b.c2, t, True)
                 y = self._conv_projected(b.c3, t, b.down, y)
                 continue
             ident = y if b.down is None else self._conv(b.down, y, False)
-            t = self._conv(b.c1, y, True)
+            t = t1 if t1 is not None else self._conv(b.c1, y, True)
             t = self._conv(b.c2, t, True)
             y = self._conv(b.c3, t, True, residual=ident)
         p = self.gap.run(self.ctx, y)

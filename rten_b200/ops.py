@@ -552,6 +552,24 @@ class Conv:
                                                      C.byref(pp), self.activation, C.byref(o)))
         return A.wrap(o, out)
 
+    def run_chained(self, ctx, x, w, bias=None, packed_w: Optional[Packed] = None, residual=None, *, nxt: "Conv", w_next,
+                    bias_next=None, packed_w_next: Optional[Packed] = None, proj: Optional["Conv"] = None, x_proj=None,
+                    w_proj=None, bias_proj=None, packed_w_proj: Optional[Packed] = None, out=None, out_next=None):
+        """(y, z): y = act(self(x, w, bias) [+ residual | + proj(x_proj, w_proj, bias_proj)]) with this op's activation,
+        z = nxt(y, w_next, bias_next) with nxt's -- a residual block's last convolution and the next block's first
+        (rten_b200_conv2d_chained)."""
+        A = _Args(ctx)
+        o, o2 = A.out(out), A.out(out_next)
+        p = _conv_params(self.padding, self.groups, self.strides, self.dilations)
+        pn = _conv_params(nxt.padding, nxt.groups, nxt.strides, nxt.dilations)
+        pp = _conv_params(proj.padding, proj.groups, proj.strides, proj.dilations) if proj is not None else None
+        ctx.check(ctx.lib.rten_b200_conv2d_chained(ctx.handle, A.t(x), A.t(w), _ph(packed_w), A.t(bias), C.byref(p),
+                                                   A.t(residual), A.t(x_proj), A.t(w_proj), _ph(packed_w_proj),
+                                                   A.t(bias_proj), C.byref(pp) if pp is not None else None,
+                                                   self.activation, A.t(w_next), _ph(packed_w_next), A.t(bias_next),
+                                                   C.byref(pn), nxt.activation, C.byref(o), C.byref(o2)))
+        return A.wrap(o, out), A.wrap(o2, out_next)
+
 
 class ConvInteger(Conv):
     """src/ops/conv.rs:477-533"""
