@@ -223,6 +223,36 @@ rten_status rten_b200_conv2d_chained(rten_ctx* ctx, const rten_tensor* x, const 
                                      const rten_packed* packed_w_next_or_null, const rten_tensor* bias_next_or_null,
                                      const rten_conv_params* p_next, int activation_next, rten_tensor* out,
                                      rten_tensor* out_next);
+/* ConvTranspose (src/ops/conv_transpose.rs:226-410), f32.  x NCHW (or NCW), w [C_in, C_out/groups, kh, kw] (or
+ * [C_in, C_out/groups, kw]), bias [C_out]; the output layout follows the input (channels-last in, channels-last out).
+ * pads = {top, left, bottom, right} (1-D: {start, end}); auto_pad_same != 0 => `Padding::Same` (output = input * stride,
+ * pads ignored).  The n_* counts give how many entries of each array are set: the reference checks them against the
+ * spatial rank (n_output_padding = 0: the attribute is absent, zeros).  Errors and messages as the reference
+ * (conv_transpose.rs:144-345); batch 0 gives an empty output.  Strides above 256 return RTEN_ERR_UNSUPPORTED_VALUE.
+ *
+ * Computed as stride-phase convolutions: output rows o = q + s*j of phase q = o mod s (per axis) receive the taps k
+ * with k*d = q + pad (mod s), so each phase with taps is an ordinary stride-1 convolution with a reversed sub-kernel,
+ * run on the implicit-GEMM conv kernel and stored through a strided view of the output; every phase without taps gets
+ * the bias (or 0) from one fill launch.  prepack builds the sub-kernels of every residue phase once (they depend only
+ * on the weight, groups, strides and dilations); a channels-last, single-pass TF32 call with prepacked weights and
+ * groups 1 is (phases with taps) + (1 if a phase has none) launches. */
+typedef struct {
+    int32_t pads[4];
+    int32_t auto_pad_same;
+    int32_t groups;
+    int32_t strides[2];
+    int32_t dilations[2];
+    int32_t output_padding[2];
+    int32_t n_pads;
+    int32_t n_strides;
+    int32_t n_dilations;
+    int32_t n_output_padding;
+} rten_conv_transpose_params;
+rten_status rten_b200_conv_transpose(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w,
+                                     const rten_packed* packed_w_or_null, const rten_tensor* bias_or_null,
+                                     const rten_conv_transpose_params* p, rten_tensor* out);
+rten_status rten_b200_prepack_conv_transpose_weight(rten_ctx* ctx, const rten_tensor* w, const rten_conv_transpose_params* p,
+                                                    rten_packed** out);
 /* ConvInteger (src/ops/conv.rs:421-533); scale_or_null != NULL => ConvIntegerToFloat (:535-587). */
 rten_status rten_b200_conv_integer(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w,
                                    const rten_packed* packed_w_or_null, const rten_tensor* x_zero_point_or_null,
@@ -408,8 +438,8 @@ rten_status rten_b200_scatter_rows(rten_ctx* ctx, rten_tensor* table, const rten
  * A run executes the nodes in topological order, one operator call of this library each; temporaries are reference
  * counted and return to the context pool after their last consumer; Relu / Gelu / Erf / Softmax run in place when the
  * executor holds the last reference to their input (src/graph.rs:973-1049); Reshape / Flatten / Squeeze / Unsqueeze /
- * Transpose / Identity are views.  Operators: Conv, ConvInteger, Relu, MaxPool, GlobalAveragePool, ReduceMean (spatial
- * axes), Gemm, MatMul, MatMulInteger, Add, Mul, Softmax, LayerNormalization, Gelu, Erf, Gather (rows), Cast (i32 -> f32),
+ * Transpose / Identity are views.  Operators: Conv, ConvInteger, ConvTranspose (constant weights prepacked at load; a
+ * node that sets output_shape fails the load), Relu, MaxPool, GlobalAveragePool, ReduceMean (spatial axes), Gemm, MatMul, MatMulInteger, Add, Mul, Softmax, LayerNormalization, Gelu, Erf, Gather (rows), Cast (i32 -> f32),
  * DynamicQuantizeLinear, Attention (4-D), MatMulNBits (com.microsoft, bits 4; constant B / scales used in place),
  * RotaryEmbedding, GroupQueryAttention (com.microsoft; output and present_key / present_value, inputs 12-15 rejected;
  * the executor allocates new present caches, so each decode step also copies the past: two launches, not one),

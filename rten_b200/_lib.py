@@ -44,6 +44,21 @@ class RtenConvParams(C.Structure):
     ]
 
 
+class RtenConvTransposeParams(C.Structure):
+    _fields_ = [
+        ("pads", C.c_int32 * 4),
+        ("auto_pad_same", C.c_int32),
+        ("groups", C.c_int32),
+        ("strides", C.c_int32 * 2),
+        ("dilations", C.c_int32 * 2),
+        ("output_padding", C.c_int32 * 2),
+        ("n_pads", C.c_int32),
+        ("n_strides", C.c_int32),
+        ("n_dilations", C.c_int32),
+        ("n_output_padding", C.c_int32),
+    ]
+
+
 class RtenAttentionParams(C.Structure):
     _fields_ = [("is_causal", C.c_int32), ("q_num_heads", C.c_int32), ("kv_num_heads", C.c_int32), ("scale", C.c_float),
                 ("softcap", C.c_float)]
@@ -94,6 +109,8 @@ _SIGNATURES = {
     "rten_b200_conv2d_chained": (C.c_int, [_vp, _TP, _TP, _vp, _TP, C.POINTER(RtenConvParams), _TP, _TP, _TP, _vp, _TP,
                                            C.POINTER(RtenConvParams), C.c_int, _TP, _vp, _TP, C.POINTER(RtenConvParams),
                                            C.c_int, _TP, _TP]),
+    "rten_b200_conv_transpose": (C.c_int, [_vp, _TP, _TP, _vp, _TP, C.POINTER(RtenConvTransposeParams), _TP]),
+    "rten_b200_prepack_conv_transpose_weight": (C.c_int, [_vp, _TP, C.POINTER(RtenConvTransposeParams), C.POINTER(_vp)]),
     "rten_b200_conv_integer": (C.c_int, [_vp, _TP, _TP, _vp, _TP, _TP, _TP, C.POINTER(RtenConvParams), _TP]),
     "rten_b200_quantized_linear": (C.c_int, [_vp, _TP, _TP, _TP, C.c_float, _TP, _vp, _TP, _TP, _TP, _TP, C.c_int, _TP]),
     "rten_b200_attention": (C.c_int, [_vp, _TP, _TP, _TP, _TP, _TP, C.POINTER(RtenAttentionParams), _TP, _TP, _TP]),

@@ -7,6 +7,7 @@
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
+#include <numeric>
 #include <vector>
 
 #include "api_shared.h"
@@ -34,6 +35,9 @@ struct ConvArgs {
     const rten_tensor* scale = nullptr;
     const rten_tensor* scale_b = nullptr;  // optional second scalar factor (x_scale of a DynamicQuantizeLinear)
     const rten_tensor* out_range = nullptr;  // optional i32[2] device tensor: (min, max) of the output, ordered-int encoded
+    // 3xTF32: low parts of x computed by the caller, laid out like x (same strides), used when x is read in place
+    const void* x_lo = nullptr;
+    bool cache_x3 = true;  // pw outlives the call: its 3xTF32 split may be cached with it
 };
 
 rten_status pack_conv_weight(rten_ctx* ctx, const rten_tensor* w, int esize, void* dst) {
@@ -548,7 +552,9 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
             L.b.strides[1] = kh * kw * Cg;
             L.b.strides[2] = Cg;
             L.b.strides[3] = 0;
-            if (A.pw && A.kind == 0 && groups == 1 && wg == A.pw->data) L.b_x3_slot = &const_cast<rten_packed*>(A.pw)->x3;
+            if (A.pw && A.kind == 0 && groups == 1 && wg == A.pw->data && A.cache_x3)
+                L.b_x3_slot = &const_cast<rten_packed*>(A.pw)->x3;
+            if (A.x_lo && xs.data == x.data) L.a_lo_base = (const float*)A.x_lo + g * Cg;
             if (zb) {
                 // per-pixel window sums of the image = N=1 GEMM against an all-ones kernel row
                 int32_t* rs = nullptr;
@@ -934,6 +940,360 @@ rten_status conv_chained(OpScope& sc, ConvArgs& M, ConvArgs* P, ConvArgs& Nx, rt
     return conv_core(sc, Nx, out_next);
 }
 
+// ---- ConvTranspose as stride-phase convolutions ----------------------------------------------------------------------
+// Per spatial axis (input length H, kernel k, stride s, dilation d, top pad pt), output row o receives x[i] * W[k]
+// wherever i*s + k*d = o + pt.  The rows o = q + s*j of phase q = o mod s receive exactly the taps k with
+// k*d = q + pt (mod s); they step by s / gcd(d, s).  With the taps in decreasing order k_0 > k_1 > ... and
+// e_0 = (q + pt - k_0*d) / s, out_q[j] = sum_t x[j + e_0 + t*d/gcd(d, s)] * W[k_t]: a stride-1 convolution with
+// dilation d/gcd(d, s), the reversed sub-kernel and top pad -e_0.  The sub-kernel depends only on the residue
+// r = (q + pt) mod s, so a prepacked weight holds one per residue.
+
+// Taps of residue r of one axis
+struct AxisTaps {
+    int64_t T = 0;     // count; 0: a phase with this residue receives only the bias
+    int64_t k0 = 0;    // largest tap
+    int64_t step = 1;  // s / gcd(d, s)
+};
+
+AxisTaps axis_taps(int64_t k, int64_t s, int64_t d, int64_t r) {
+    AxisTaps t;
+    t.step = s / std::gcd(d, s);
+    for (int64_t kk = k - 1; kk >= 0; kk--)
+        if ((kk * d) % s == r) {
+            if (t.T == 0) t.k0 = kk;
+            t.T++;
+        }
+    return t;
+}
+
+// Phase q of one axis as a convolution over rows [row0, row0 + rows) of the input
+struct AxisPhase {
+    bool live = false;  // has taps that reach the input
+    int64_t n = 0;      // output rows q, q + s, ...
+    int64_t r = 0;      // residue: which sub-kernel
+    AxisTaps taps;
+    int64_t dil = 1;
+    int64_t row0 = 0, rows = 0, pad0 = 0, pad1 = 0;
+};
+
+AxisPhase axis_phase(int64_t H, int64_t OH, int64_t k, int64_t s, int64_t d, int64_t pt, int64_t q) {
+    AxisPhase a;
+    a.n = q < OH ? (OH - q + s - 1) / s : 0;
+    a.r = (q + pt) % s;
+    a.taps = axis_taps(k, s, d, a.r);
+    a.dil = d / std::gcd(d, s);
+    if (a.n == 0 || a.taps.T == 0) return a;
+    const int64_t e0 = (q + pt - a.taps.k0 * d) / s;  // exact
+    const int64_t last = a.n - 1 + e0 + (a.taps.T - 1) * a.dil;  // last input row any output of the phase reads
+    const int64_t r0 = std::max<int64_t>(e0, 0), r1 = std::min<int64_t>(last, H - 1) + 1;
+    if (r0 >= r1) return a;  // every window lies in the padding
+    a.live = true;
+    a.row0 = r0;
+    a.rows = r1 - r0;
+    a.pad0 = r0 - e0;
+    a.pad1 = last - (r1 - 1);
+    return a;
+}
+
+// Validated geometry of a transposed convolution (2-D form: a 1-D one runs over a height-1 image)
+struct ConvTShape {
+    rten_tensor x, w;
+    bool one_d = false;
+    int64_t B, C, H, W, O, Og, Cg, kh, kw, OH, OW, sy, sx, dy, dx, pt, pl, pb, pr;
+    int groups;
+};
+
+void expand_1d(rten_tensor& t) {
+    t.ndim = 4;
+    t.shape[3] = t.shape[2];
+    t.strides[3] = t.strides[2];
+    t.shape[2] = 1;
+    t.strides[2] = 0;
+}
+
+// Argument checks in the reference's order (conv_transpose.rs:226-345, conv_transpose_output_size_and_padding
+// :144-220) on the kernel `w` (and input `x` when given)
+rten_status conv_transpose_shape(rten_ctx* ctx, const rten_tensor* xp, const rten_tensor& w0, const rten_tensor* bias,
+                                 const rten_conv_transpose_params* cp, ConvTShape& S) {
+    const bool one_d = S.one_d = xp ? xp->ndim == 3 : w0.ndim == 3;
+    if (xp) S.x = *xp;
+    S.w = w0;
+    int64_t pads[4] = {cp->pads[0], cp->pads[1], cp->pads[2], cp->pads[3]};
+    int64_t st[2] = {cp->strides[0], cp->strides[1]}, dl[2] = {cp->dilations[0], cp->dilations[1]};
+    int64_t op[2] = {0, 0};
+    const bool same = cp->auto_pad_same != 0;
+    if (one_d) {
+        if (S.w.ndim != 3) return fail(ctx, RTEN_ERR_INVALID_VALUE, "kernel must have 3 dims (OCW)");
+        if (!same && cp->n_pads != 2) return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected 2 pad values");
+        if (cp->n_strides != 1) return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected 1 stride value");
+        if (cp->n_dilations != 1) return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected 1 dilation value");
+        if (cp->n_output_padding != 0 && cp->n_output_padding != 1)
+            return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected 1 output_padding value");
+        if (xp) expand_1d(S.x);
+        expand_1d(S.w);
+        pads[0] = pads[2] = 0;
+        pads[1] = cp->pads[0];
+        pads[3] = cp->pads[1];
+        st[1] = st[0];
+        st[0] = 1;
+        dl[1] = dl[0];
+        dl[0] = 1;
+        op[1] = cp->n_output_padding ? cp->output_padding[0] : 0;
+    } else if (cp->n_output_padding == 2) {
+        op[0] = cp->output_padding[0];
+        op[1] = cp->output_padding[1];
+    }
+    const int groups = S.groups = cp->groups;
+    if (groups <= 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Group count must be > 0");
+    if (xp && S.x.ndim != 4) return fail(ctx, RTEN_ERR_INVALID_VALUE, "input must have 4 dims (NCHW)");
+    if (S.w.ndim != 4) return fail(ctx, RTEN_ERR_INVALID_VALUE, "kernel must have 4 dims (COHW)");
+    const int64_t Cin = S.w.shape[0];
+    S.Og = S.w.shape[1];
+    S.O = S.Og * groups;
+    S.kh = S.w.shape[2];
+    S.kw = S.w.shape[3];
+    if (bias && (bias->ndim != 1 || bias->shape[0] != S.O))
+        return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "bias.size(0) != out_channels");
+    if (xp && S.x.shape[1] != Cin)
+        return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Input channels does not match kernel input channels");
+    if (Cin % groups != 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Input channel count not divisible by groups");
+    S.Cg = Cin / groups;
+    if (!one_d) {
+        if (cp->n_strides != 2) return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected 2 stride values");
+        if (cp->n_dilations != 2) return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected 2 dilation values");
+        if (cp->n_output_padding != 0 && cp->n_output_padding != 2)
+            return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected 2 output_padding values");
+    }
+    S.sy = st[0];
+    S.sx = st[1];
+    S.dy = dl[0];
+    S.dx = dl[1];
+    if (S.sy <= 0 || S.sx <= 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Strides must be > 0");
+    if (S.dy <= 0 || S.dx <= 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Dilations must be > 0");
+    if (S.kh <= 0 || S.kw <= 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Kernel size must be > 0");
+    if (!xp) return RTEN_OK;  // (prepack: the weight's checks only)
+    S.B = S.x.shape[0];
+    S.C = S.x.shape[1];
+    S.H = S.x.shape[2];
+    S.W = S.x.shape[3];
+    if (S.H == 0 || S.W == 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Input width and height must be > 0");
+    if (!same && !one_d && cp->n_pads != 4) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Wrong number of pad values");
+    for (int i = 0; i < 4; i++)
+        if (!same && pads[i] < 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Pads must be >= 0");
+    if (op[0] < 0 || op[1] < 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Output padding must be >= 0");
+    const int64_t keh = (S.kh - 1) * S.dy + 1, kew = (S.kw - 1) * S.dx + 1;
+    const int64_t full_h = (S.H - 1) * S.sy + op[0] + keh, full_w = (S.W - 1) * S.sx + op[1] + kew;
+    if (same) {
+        S.OH = S.H * S.sy;
+        S.OW = S.W * S.sx;
+        const int64_t ph = full_h - S.OH, pw = full_w - S.OW;
+        if (ph < 0 || pw < 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Input is too small");
+        S.pt = ph / 2;
+        S.pb = ph - S.pt;
+        S.pl = pw / 2;
+        S.pr = pw - S.pl;
+    } else {
+        S.pt = pads[0];
+        S.pl = pads[1];
+        S.pb = pads[2];
+        S.pr = pads[3];
+        S.OH = full_h - S.pt - S.pb;
+        S.OW = full_w - S.pl - S.pr;
+        if (S.OH < 0 || S.OW < 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Input is too small");
+    }
+    return RTEN_OK;
+}
+
+// The sub-kernel of residue phase (ty, tx) of W (4-D view) as a conv weight [O, Th, Tw, Cg]
+rten_status pack_transpose_phase(rten_ctx* ctx, const ConvTShape& S, const AxisTaps& ty, const AxisTaps& tx, void* dst) {
+    ConvTransposePack p;
+    p.O = (int)S.O;
+    p.Og = (int)S.Og;
+    p.Cg = (int)S.Cg;
+    p.Th = (int)ty.T;
+    p.Tw = (int)tx.T;
+    p.ky0 = (int)ty.k0;
+    p.kx0 = (int)tx.k0;
+    p.step_y = (int)ty.step;
+    p.step_x = (int)tx.step;
+    p.ws_i = S.w.strides[0];
+    p.ws_o = S.w.strides[1];
+    p.ws_h = S.w.strides[2];
+    p.ws_w = S.w.strides[3];
+    return launch_conv_transpose_pack(ctx, (const float*)S.w.data, (float*)dst, p);
+}
+
+rten_status conv_transpose_core(OpScope& sc, const rten_tensor* x_in, const rten_tensor* w_in, const rten_packed* pw,
+                                const rten_tensor* bias_in, const rten_conv_transpose_params* cp, rten_tensor* out) {
+    rten_ctx* ctx = sc.ctx;
+    rten_tensor xd, wd, bd;
+    RTB_TRY(sc.in(x_in, &xd));
+    RTB_TRY(sc.in(w_in, &wd));
+    if (bias_in) RTB_TRY(sc.in(bias_in, &bd));
+    ConvTShape S;
+    RTB_TRY(conv_transpose_shape(ctx, &xd, wd, bias_in ? &bd : nullptr, cp, S));
+    const int64_t B = S.B, C = S.C, H = S.H, W = S.W, O = S.O, Cg = S.Cg, OH = S.OH, OW = S.OW;
+    const int groups = S.groups;
+
+    // ---- output (layout follows the input: channels-last in -> channels-last out)
+    rten_tensor x = S.x;
+    const bool x_cl = x.strides[1] == 1 && C > 1;
+    const int64_t oshape[4] = {B, O, OH, OW};
+    const int64_t pref[4] = {x_cl ? OH * OW * O : O * OH * OW, x_cl ? 1 : OH * OW, x_cl ? OW * O : OW, x_cl ? O : 1};
+    rten_tensor ov;
+    if (S.one_d) {
+        const int64_t os3[3] = {B, O, OW}, pf3[3] = {pref[0], pref[1], pref[3]};
+        RTB_TRY(sc.out(out, RTEN_F32, 3, os3, &ov, out->data ? nullptr : pf3));
+        expand_1d(ov);
+    } else {
+        RTB_TRY(sc.out(out, RTEN_F32, 4, oshape, &ov, out->data ? nullptr : pref));
+    }
+    if (B * O * OH * OW == 0) return RTEN_OK;
+    if (S.sy > 256 || S.sx > 256) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "ConvTranspose strides above 256 are not supported");
+    if (pw && (pw->kind != 2 || pw->O != O || pw->Cg != Cg || pw->kh != S.kh || pw->kw != S.kw || pw->groups != groups ||
+               pw->sy != S.sy || pw->sx != S.sx || pw->dy != S.dy || pw->dx != S.dx))
+        return fail(ctx, RTEN_ERR_INVALID_VALUE, "prepacked conv transpose weight does not match the kernel and parameters");
+
+    std::vector<AxisPhase> py, px;
+    for (int64_t q = 0; q < S.sy; q++) py.push_back(axis_phase(H, OH, S.kh, S.sy, S.dy, S.pt, q));
+    for (int64_t q = 0; q < S.sx; q++) px.push_back(axis_phase(W, OW, S.kw, S.sx, S.dx, S.pl, q));
+    bool any_live = false, any_empty = false;
+    for (int64_t qy = 0; qy < std::min(S.sy, OH); qy++)
+        for (int64_t qx = 0; qx < std::min(S.sx, OW); qx++) {
+            const bool live = py[qy].live && px[qx].live;
+            any_live |= live;
+            any_empty |= !live;
+        }
+    rten_tensor bias_c;
+    if (bias_in) RTB_TRY(sc.contiguous(&bd, &bias_c));
+
+    // ---- every phase without a convolution: the bias, in one launch
+    if (any_empty) {
+        ConvTransposeFill f;
+        memset(&f, 0, sizeof(f));
+        f.B = (int)B;
+        f.O = (int)O;
+        f.OH = (int)OH;
+        f.OW = (int)OW;
+        f.sy = (int)S.sy;
+        f.sx = (int)S.sx;
+        f.s_b = ov.strides[0];
+        f.s_o = ov.strides[1];
+        f.s_h = ov.strides[2];
+        f.s_w = ov.strides[3];
+        for (int64_t q = 0; q < S.sy; q++)
+            if (py[q].live) f.live_y[q >> 5] |= 1u << (q & 31);
+        for (int64_t q = 0; q < S.sx; q++)
+            if (px[q].live) f.live_x[q >> 5] |= 1u << (q & 31);
+        RTB_TRY(launch_conv_transpose_fill(ctx, (float*)ov.data, bias_in ? (const float*)bias_c.data : nullptr, f));
+    }
+    if (!any_live) return RTEN_OK;
+
+    // ---- the input, shared by every phase: channels-last and 16-byte addressable for the implicit-GEMM path (one
+    //      copy when it is not), and in 3xTF32 its low parts, split once
+    const bool implicit = (Cg * 4) % 16 == 0 && Cg * 4 >= 32;
+    if (implicit) {
+        const bool direct = x.strides[1] == 1 && (reinterpret_cast<uintptr_t>(x.data) % 16 == 0) && x.strides[3] % 4 == 0 &&
+                            x.strides[2] % 4 == 0 && x.strides[0] % 4 == 0;
+        if (!direct) {
+            void* buf = nullptr;
+            RTB_TRY(temp_alloc(ctx, (size_t)(B * H * W * C) * 4, &buf));
+            long long shape[4] = {B, H, W, C};
+            long long ss[4] = {x.strides[0], x.strides[2], x.strides[3], x.strides[1]};
+            long long ds[4] = {H * W * C, W * C, C, 1};
+            RTB_TRY(launch_nd_copy(ctx, 4, x.data, buf, 4, shape, ss, ds));
+            x.data = buf;
+            x.strides[0] = H * W * C;
+            x.strides[1] = 1;
+            x.strides[2] = W * C;
+            x.strides[3] = C;
+        }
+    }
+    const float* x_lo = nullptr;
+    const bool compact_nhwc = x.strides[1] == 1 && x.strides[3] == C && x.strides[2] == W * C && x.strides[0] == H * W * C;
+    if (implicit && ctx->f32_mode == RTEN_F32_TF32X3 && Cg % 32 == 0 && compact_nhwc && !getenv("RTEN_B200_X3_THREE_PLANES")) {
+        float* lo = nullptr;
+        RTB_TRY(temp_alloc(ctx, (size_t)(B * H * W * C) * 4, (void**)&lo));
+        const long long dims[4] = {C, W, H, B}, strides[4] = {1, C, W * C, H * W * C};
+        RTB_TRY(launch_tf32x3_split(ctx, (const float*)x.data, lo, dims, strides, C, 2));
+        x_lo = lo;
+    }
+
+    // ---- the sub-kernels: prepacked, or packed here for the residues this call uses
+    std::vector<rten_packed> call_packs;
+    std::vector<int> call_index((size_t)(S.sy * S.sx), -1);
+    if (!pw) {
+        for (int64_t qy = 0; qy < std::min(S.sy, OH); qy++)
+            for (int64_t qx = 0; qx < std::min(S.sx, OW); qx++) {
+                if (!py[qy].live || !px[qx].live) continue;
+                const size_t ri = (size_t)(py[qy].r * S.sx + px[qx].r);
+                if (call_index[ri] >= 0) continue;
+                rten_packed p;
+                p.kind = 1;
+                p.O = O;
+                p.Cg = Cg;
+                p.kh = py[qy].taps.T;
+                p.kw = px[qx].taps.T;
+                p.groups = groups;
+                RTB_TRY(temp_alloc(ctx, (size_t)(O * p.kh * p.kw * Cg) * 4, &p.data));
+                RTB_TRY(pack_transpose_phase(ctx, S, py[qy].taps, px[qx].taps, p.data));
+                call_index[ri] = (int)call_packs.size();
+                call_packs.push_back(p);
+            }
+    }
+
+    // ---- one stride-1 convolution per phase with taps, into a strided view of the output
+    for (int64_t qy = 0; qy < std::min(S.sy, OH); qy++)
+        for (int64_t qx = 0; qx < std::min(S.sx, OW); qx++) {
+            const AxisPhase &ay = py[qy], &ax = px[qx];
+            if (!ay.live || !ax.live) continue;
+            const size_t ri = (size_t)(ay.r * S.sx + ax.r);
+            const rten_packed* pp = pw ? pw->phases[ri] : &call_packs[(size_t)call_index[ri]];
+            const int64_t xoff = ay.row0 * x.strides[2] + ax.row0 * x.strides[3];
+            rten_tensor xv = x;
+            xv.data = (float*)x.data + xoff;
+            xv.shape[2] = ay.rows;
+            xv.shape[3] = ax.rows;
+            rten_tensor wv{};
+            wv.data = pp->data;
+            wv.dtype = RTEN_F32;
+            wv.device = ctx->device;
+            wv.ndim = 4;
+            const int64_t wshape[4] = {O, Cg, pp->kh, pp->kw}, wstr[4] = {pp->kh * pp->kw * Cg, 1, pp->kw * Cg, Cg};
+            for (int i = 0; i < 4; i++) {
+                wv.shape[i] = wshape[i];
+                wv.strides[i] = wstr[i];
+            }
+            rten_tensor oq = ov;
+            oq.data = (float*)ov.data + qy * ov.strides[2] + qx * ov.strides[3];
+            oq.shape[2] = ay.n;
+            oq.shape[3] = ax.n;
+            oq.strides[2] = ov.strides[2] * S.sy;
+            oq.strides[3] = ov.strides[3] * S.sx;
+            rten_conv_params p{};
+            p.pads[0] = (int32_t)ay.pad0;
+            p.pads[1] = (int32_t)ax.pad0;
+            p.pads[2] = (int32_t)ay.pad1;
+            p.pads[3] = (int32_t)ax.pad1;
+            p.groups = groups;
+            p.strides[0] = p.strides[1] = 1;
+            p.dilations[0] = (int32_t)ay.dil;
+            p.dilations[1] = (int32_t)ax.dil;
+            p.n_strides = p.n_dilations = 2;
+            ConvArgs A{};
+            A.kind = 0;
+            A.x = &xv;
+            A.w = &wv;
+            A.pw = pp;
+            A.bias = bias_in ? &bias_c : nullptr;
+            A.p = &p;
+            A.x_lo = x_lo ? x_lo + xoff : nullptr;
+            A.cache_x3 = pw != nullptr;
+            RTB_TRY(conv_core(sc, A, &oq));
+        }
+    return RTEN_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1057,6 +1417,69 @@ rten_status rten_b200_conv2d_chained(rten_ctx* ctx, const rten_tensor* x, const 
     Nx.p = p_next;
     Nx.act = activation_next;
     return sc.finish(conv_chained(sc, M, x_proj ? &P : nullptr, Nx, out, out_next));
+}
+
+// ---- ConvTranspose ------------------------------------------------------------------------------------------------
+rten_status rten_b200_prepack_conv_transpose_weight(rten_ctx* ctx, const rten_tensor* w, const rten_conv_transpose_params* params,
+                                                    rten_packed** out) {
+    RTB_TRY(check_ctx(ctx));
+    if (!w || !params || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    *out = nullptr;
+    if (w->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    OpScope sc(ctx);
+    rten_tensor wv;
+    ConvTShape S;
+    rten_status st = sc.in(w, &wv);
+    if (st == RTEN_OK) st = conv_transpose_shape(ctx, nullptr, wv, nullptr, params, S);
+    if (st == RTEN_OK && (S.sy > 256 || S.sx > 256))
+        st = fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "ConvTranspose strides above 256 are not supported");
+    rten_packed* p = nullptr;
+    if (st == RTEN_OK) {
+        p = new rten_packed();
+        p->kind = 2;
+        p->O = S.O;
+        p->Cg = S.Cg;
+        p->kh = S.kh;
+        p->kw = S.kw;
+        p->groups = S.groups;
+        p->sy = S.sy;
+        p->sx = S.sx;
+        p->dy = S.dy;
+        p->dx = S.dx;
+        p->phases.assign((size_t)(S.sy * S.sx), nullptr);
+        for (int64_t ry = 0; ry < S.sy && st == RTEN_OK; ry++)
+            for (int64_t rx = 0; rx < S.sx && st == RTEN_OK; rx++) {
+                const AxisTaps ty = axis_taps(S.kh, S.sy, S.dy, ry), tx = axis_taps(S.kw, S.sx, S.dx, rx);
+                if (ty.T == 0 || tx.T == 0) continue;
+                rten_packed* ph = new rten_packed();
+                p->phases[(size_t)(ry * S.sx + rx)] = ph;
+                ph->kind = 1;
+                ph->O = S.O;
+                ph->Cg = S.Cg;
+                ph->kh = ty.T;
+                ph->kw = tx.T;
+                ph->groups = S.groups;
+                st = pool_alloc(ctx, (size_t)std::max<int64_t>(S.O * ty.T * tx.T * S.Cg, 1) * 4, &ph->data);
+                if (st == RTEN_OK) st = pack_transpose_phase(ctx, S, ty, tx, ph->data);
+            }
+    }
+    st = sc.finish(st);
+    if (st != RTEN_OK) {
+        if (p) rten_b200_packed_free(ctx, p);
+        return st;
+    }
+    *out = p;
+    return RTEN_OK;
+}
+
+rten_status rten_b200_conv_transpose(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w, const rten_packed* pw,
+                                     const rten_tensor* bias, const rten_conv_transpose_params* p, rten_tensor* out) {
+    RTB_TRY(check_ctx(ctx));
+    if (!x || !w || !p || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    if (x->dtype != RTEN_F32 || w->dtype != RTEN_F32 || (bias && bias->dtype != RTEN_F32))
+        return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    OpScope sc(ctx);
+    return sc.finish(conv_transpose_core(sc, x, w, pw, bias, p, out));
 }
 
 rten_status rten_b200_conv2d(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w, const rten_packed* pw,

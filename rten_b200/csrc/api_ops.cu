@@ -596,6 +596,7 @@ rten_status rten_b200_prepack_b(rten_ctx* ctx, const rten_tensor* b, rten_packed
 
 void rten_b200_packed_free(rten_ctx* ctx, rten_packed* p) {
     if (!p) return;
+    for (rten_packed* ph : p->phases) rten_b200_packed_free(ctx, ph);
     if (ctx) {
         pool_free(ctx, p->data);
         pool_free(ctx, p->colsum);

@@ -16,6 +16,10 @@ struct rten_packed {
     void* data = nullptr;
     int32_t* colsum = nullptr;  // int8: sum over K per output column / channel
     void* x3 = nullptr;         // f32: [hi | lo | hi] copy for the 3xTF32 mode, built by the first launch that needs it (cudaMalloc)
+    // conv transpose (kind 2): W [C_in, C_out/groups, kh, kw] with O = C_out, Cg = C_in/groups, kh, kw, groups as above;
+    // one conv-weight pack (kind 1) per residue phase (ry, rx) of the strides, row-major, null where it has no taps
+    int64_t sy = 1, sx = 1, dy = 1, dx = 1;
+    std::vector<rten_packed*> phases;
 };
 
 namespace rtb {

@@ -8,7 +8,7 @@
 //          returned to the context pool after their last consumer (src/graph.rs:1100-1180); an operator that can run in
 //          place does so when the executor holds the last reference to its input (src/graph.rs:973-1049); shape-only
 //          operators (Reshape, Flatten, Squeeze, Unsqueeze, Transpose, Identity) are views -- no kernel, no copy.
-// Operators: Conv, ConvInteger, Relu, MaxPool, GlobalAveragePool, ReduceMean, Gemm, MatMul, MatMulInteger, MatMulNBits
+// Operators: Conv, ConvInteger, ConvTranspose (without output_shape), Relu, MaxPool, GlobalAveragePool, ReduceMean, Gemm, MatMul, MatMulInteger, MatMulNBits
 // (com.microsoft), Add, Mul, Softmax, LayerNormalization, Gelu, Erf, Gather, Cast, DynamicQuantizeLinear, Attention,
 // RotaryEmbedding, GroupQueryAttention (com.microsoft, three outputs), Constant and the view operators.
 #include <cuda_runtime.h>
@@ -151,7 +151,7 @@ rten_status upload_constant(rten_model* m, const onnx::Tensor& t, ValueSlot* v) 
 
 const std::set<std::string>& supported_ops() {
     static const std::set<std::string> s = {
-        "Conv", "Relu", "MaxPool", "GlobalAveragePool", "ReduceMean", "Reshape", "Flatten", "Squeeze", "Unsqueeze", "Transpose",
+        "Conv", "ConvTranspose", "Relu", "MaxPool", "GlobalAveragePool", "ReduceMean", "Reshape", "Flatten", "Squeeze", "Unsqueeze", "Transpose",
         "Identity", "Gemm", "MatMul", "Add", "Mul", "Softmax", "LayerNormalization", "Gelu", "Erf", "Gather",
         "DynamicQuantizeLinear", "MatMulInteger", "ConvInteger", "Cast", "Attention", "MatMulNBits", "GroupQueryAttention",
         "RotaryEmbedding", "Constant"};
@@ -184,6 +184,30 @@ rten_status fill_conv_params(rten_ctx* ctx, const onnx::Node& n, rten_conv_param
         p->strides[i] = i < (int)st.size() ? (int32_t)st[(size_t)i] : 1;
         p->dilations[i] = i < (int)dl.size() ? (int32_t)dl[(size_t)i] : 1;
     }
+    return RTEN_OK;
+}
+
+// ConvTranspose attributes as the reference reads them (src/op_registry/onnx_registry.rs:912-972, 1032-1052): strides,
+// dilations and pads default to as many values as kernel_shape has spatial axes (none without kernel_shape), auto_pad
+// SAME_UPPER / SAME_LOWER is `Padding::Same`, output_padding is absent unless set.
+rten_status fill_conv_transpose_params(rten_ctx* ctx, const onnx::Node& n, rten_conv_transpose_params* p) {
+    memset(p, 0, sizeof(*p));
+    const onnx::Attribute* ap = n.attr("auto_pad");
+    if (ap && !ap->s.empty() && ap->s != "NOTSET" && ap->s != "VALID" && ap->s != "SAME_UPPER" && ap->s != "SAME_LOWER")
+        return mfail(ctx, RTEN_ERR_INVALID_VALUE, "auto_pad: unsupported value");
+    p->auto_pad_same = ap && (ap->s == "SAME_UPPER" || ap->s == "SAME_LOWER");
+    const size_t nsp = n.attr_ints("kernel_shape").size();
+    // (a count that does not match the input's rank fails in the operator, with the reference's message)
+    auto read = [&](const char* name, size_t dflt_len, int32_t dflt, int32_t* dst, size_t cap, int32_t* count) {
+        const std::vector<int64_t> v = n.attr(name) ? n.attr_ints(name) : std::vector<int64_t>(dflt_len, dflt);
+        for (size_t i = 0; i < v.size() && i < cap; i++) dst[i] = (int32_t)v[i];
+        *count = (int32_t)v.size();
+    };
+    read("strides", nsp, 1, p->strides, 2, &p->n_strides);
+    read("dilations", nsp, 1, p->dilations, 2, &p->n_dilations);
+    read("pads", 2 * nsp, 0, p->pads, 4, &p->n_pads);
+    if (n.attr("output_padding")) read("output_padding", 0, 0, p->output_padding, 2, &p->n_output_padding);
+    p->groups = (int32_t)n.attr_i("group", 1);
     return RTEN_OK;
 }
 
@@ -268,6 +292,8 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
             if (n.inputs.size() > 12)
                 return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "GroupQueryAttention: quantization and Q/K norm inputs (12-15) are not supported");
         }
+        if (n.op_type == "ConvTranspose" && n.attr("output_shape"))  // (the reference does not read it)
+            return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "ConvTranspose: the output_shape attribute is not supported");
         if (n.op_type == "RotaryEmbedding" && n.domain == "com.microsoft")
             return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "unsupported operator com.microsoft.RotaryEmbedding");
         OpNode on;
@@ -333,6 +359,12 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
         if ((op == "Conv" || op == "ConvInteger") && o.in.size() >= 2 && m->values[(size_t)o.in[1]].kind == V_CONST &&
             m->values[(size_t)o.in[1]].t.ndim == 4) {
             RTB_TRY(rten_b200_prepack_conv_weight(ctx, &m->values[(size_t)o.in[1]].t, (int)o.n.attr_i("group", 1), &o.packed));
+        } else if (op == "ConvTranspose" && o.in.size() >= 2 && m->values[(size_t)o.in[1]].kind == V_CONST &&
+                   m->values[(size_t)o.in[1]].t.dtype == RTEN_F32) {
+            // (a weight whose attributes the operator would refuse is not prepacked: the run reports the error)
+            rten_conv_transpose_params p;
+            RTB_TRY(fill_conv_transpose_params(ctx, o.n, &p));
+            if (rten_b200_prepack_conv_transpose_weight(ctx, &m->values[(size_t)o.in[1]].t, &p, &o.packed) != RTEN_OK) o.packed = nullptr;
         } else if ((op == "MatMul" || op == "MatMulInteger") && o.in.size() >= 2 && m->values[(size_t)o.in[1]].kind == V_CONST &&
                    m->values[(size_t)o.in[1]].t.ndim == 2) {
             RTB_TRY(rten_b200_prepack_b(ctx, &m->values[(size_t)o.in[1]].t, &o.packed));
@@ -562,6 +594,10 @@ struct Runner {
                 st = rten_b200_conv2d_ex(ctx, T(0), T(1), o.packed, T(2), &p, nullptr, o.activation, &y);
             else
                 st = rten_b200_conv_integer(ctx, T(0), T(1), o.packed, T(2), T(3), nullptr, &p, &y);
+        } else if (op == "ConvTranspose") {
+            rten_conv_transpose_params p;
+            RTB_TRY(fill_conv_transpose_params(ctx, o.n, &p));
+            st = rten_b200_conv_transpose(ctx, T(0), T(1), o.packed, T(2), &p, &y);
         } else if (op == "Relu") {
             st = rten_b200_relu(ctx, T(0), &y);
         } else if (op == "Gelu") {

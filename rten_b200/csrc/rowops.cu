@@ -1608,4 +1608,78 @@ rten_status launch_tf32x3_split(rten_ctx* ctx, const float* x, float* y, const l
     return RTEN_OK;
 }
 
+// =========================================================================================
+// ConvTranspose as stride-phase convolutions (api_conv.cu)
+// =========================================================================================
+// dst[o, ty, tx, ci] = W[g*Cg + ci, o - g*Og, ky0 - ty*step_y, kx0 - tx*step_x] with g = o / Og: the OIHW sub-kernel of
+// one residue phase, taps in decreasing order, in the [O, kh, kw, C] K-major layout of a prepacked conv weight
+__global__ void __launch_bounds__(256) conv_transpose_pack_kernel(const float* __restrict__ w, float* __restrict__ dst,
+                                                                  ConvTransposePack p) {
+    const long long n = (long long)p.O * p.Th * p.Tw * p.Cg;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        long long r = i;
+        const int ci = (int)(r % p.Cg);
+        r /= p.Cg;
+        const int tx = (int)(r % p.Tw);
+        r /= p.Tw;
+        const int ty = (int)(r % p.Th);
+        const int o = (int)(r / p.Th);
+        const int g = o / p.Og, co = o - g * p.Og;
+        const long long ky = p.ky0 - (long long)ty * p.step_y, kx = p.kx0 - (long long)tx * p.step_x;
+        dst[i] = w[(long long)(g * p.Cg + ci) * p.ws_i + co * p.ws_o + ky * p.ws_h + kx * p.ws_w];
+    }
+}
+
+rten_status launch_conv_transpose_pack(rten_ctx* ctx, const float* w, float* dst, const ConvTransposePack& p) {
+    const long long n = (long long)p.O * p.Th * p.Tw * p.Cg;
+    if (n == 0) return RTEN_OK;
+    conv_transpose_pack_kernel<<<ew_grid(ctx, n), 256, 0, ctx->stream>>>(w, dst, p);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail_cuda(ctx, e, "conv_transpose_pack launch");
+    count_launch(ctx);
+    return RTEN_OK;
+}
+
+// out[b, o, y, x] = bias[o] (or 0) wherever phase (y mod sy, x mod sx) has no convolution; other elements untouched.
+// Elements are visited channel-fastest for a channels-last output, column-fastest otherwise (coalesced stores).
+__global__ void __launch_bounds__(256) conv_transpose_fill_kernel(float* __restrict__ out, const float* __restrict__ bias,
+                                                                  ConvTransposeFill p) {
+    const long long n = (long long)p.B * p.O * p.OH * p.OW;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    const bool cl = p.s_o == 1;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        long long r = i;
+        int o, y, x;
+        if (cl) {
+            o = (int)(r % p.O);
+            r /= p.O;
+            x = (int)(r % p.OW);
+            r /= p.OW;
+            y = (int)(r % p.OH);
+            r /= p.OH;
+        } else {
+            x = (int)(r % p.OW);
+            r /= p.OW;
+            y = (int)(r % p.OH);
+            r /= p.OH;
+            o = (int)(r % p.O);
+            r /= p.O;
+        }
+        const int qy = y % p.sy, qx = x % p.sx;
+        if (((p.live_y[qy >> 5] >> (qy & 31)) & 1u) && ((p.live_x[qx >> 5] >> (qx & 31)) & 1u)) continue;
+        out[r * p.s_b + (long long)o * p.s_o + (long long)y * p.s_h + (long long)x * p.s_w] = bias ? bias[o] : 0.0f;
+    }
+}
+
+rten_status launch_conv_transpose_fill(rten_ctx* ctx, float* out, const float* bias, const ConvTransposeFill& p) {
+    const long long n = (long long)p.B * p.O * p.OH * p.OW;
+    if (n == 0) return RTEN_OK;
+    conv_transpose_fill_kernel<<<ew_grid(ctx, n), 256, 0, ctx->stream>>>(out, bias, p);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail_cuda(ctx, e, "conv_transpose_fill launch");
+    count_launch(ctx);
+    return RTEN_OK;
+}
+
 }  // namespace rtb

@@ -78,6 +78,22 @@ rten_status launch_smallc8_pad(rten_ctx* ctx, const void* x, void* xp, int B, in
 rten_status launch_smallc8_pack_w(rten_ctx* ctx, const void* w, void* wp, int O, int C, int kh, int kw, long long ws_o,
                                   long long ws_c, long long ws_h, long long ws_w);
 
+// ConvTranspose as stride-phase convolutions (api_conv.cu).  Sub-kernel of one residue phase: taps ky0, ky0 - step_y, ...
+// (Th of them) and kx0, kx0 - step_x, ... (Tw) of W [C_in, Og, kh, kw], written as the [O = groups*Og, Th, Tw, Cg] pack
+struct ConvTransposePack {
+    int O, Og, Cg, Th, Tw, ky0, kx0, step_y, step_x;
+    long long ws_i, ws_o, ws_h, ws_w;  // W element strides
+};
+rten_status launch_conv_transpose_pack(rten_ctx* ctx, const float* w, float* dst, const ConvTransposePack& p);
+// bias[o] (or 0 without one) into every output element of a phase without a convolution: phase (qy, qx) has one iff
+// bit qy of live_y and bit qx of live_x are set (strides up to 256)
+struct ConvTransposeFill {
+    int B, O, OH, OW, sy, sx;
+    long long s_b, s_o, s_h, s_w;  // output element strides
+    uint32_t live_y[8], live_x[8];
+};
+rten_status launch_conv_transpose_fill(rten_ctx* ctx, float* out, const float* bias, const ConvTransposeFill& p);
+
 rten_status launch_dql_quantize_rows(rten_ctx* ctx, const float* x, uint8_t* y, long long rows, int row_len, int rows_inner,
                                      long long y_inner, long long y_outer, int* mm, float* scale_out, uint8_t* zp_out,
                                      const RangeExchange* xch = nullptr);

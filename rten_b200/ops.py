@@ -18,7 +18,8 @@ from typing import Optional, Sequence
 import numpy as np
 
 from . import _lib
-from ._lib import RTEN_DEVICE_HOST, RTEN_F32, RTEN_I8, RTEN_I32, RTEN_U8, RtenAttentionParams, RtenConvParams, RtenGqaParams, RtenTensor
+from ._lib import (RTEN_DEVICE_HOST, RTEN_F32, RTEN_I8, RTEN_I32, RTEN_U8, RtenAttentionParams, RtenConvParams,
+                   RtenConvTransposeParams, RtenGqaParams, RtenTensor)
 
 _NP2RT = {np.dtype(np.float32): RTEN_F32, np.dtype(np.int32): RTEN_I32, np.dtype(np.int8): RTEN_I8,
           np.dtype(np.uint8): RTEN_U8}
@@ -569,6 +570,57 @@ class Conv:
                                                    self.activation, A.t(w_next), _ph(packed_w_next), A.t(bias_next),
                                                    C.byref(pn), nxt.activation, C.byref(o), C.byref(o2)))
         return A.wrap(o, out), A.wrap(o2, out_next)
+
+
+def _conv_transpose_params(padding, groups, strides, dilations, output_padding) -> RtenConvTransposeParams:
+    p = RtenConvTransposeParams()
+    if isinstance(padding, str):
+        if padding.lower() != "same":
+            raise OpError(5, "unknown padding mode")
+        p.auto_pad_same = 1
+    else:
+        pads = list(padding)
+        p.n_pads = len(pads)
+        for i in range(min(4, len(pads))):
+            p.pads[i] = int(pads[i])
+    p.groups = int(groups)
+    for arr, vals, n in ((p.strides, strides, "n_strides"), (p.dilations, dilations, "n_dilations"),
+                         (p.output_padding, output_padding or (), "n_output_padding")):
+        setattr(p, n, len(vals))
+        for i in range(min(2, len(vals))):
+            arr[i] = int(vals[i])
+    return p
+
+
+class ConvTranspose:
+    """src/ops/conv_transpose.rs:412-440: attributes groups, dilations, padding ('same' or [t, l, b, r]; 1-D: [start,
+    end]), strides and output_padding (None: zeros).  Weights are [C_in, C_out / groups, kh, kw] (1-D: [C_in,
+    C_out / groups, kw])."""
+
+    def __init__(self, groups=1, dilations=(1, 1), padding=(0, 0, 0, 0), strides=(1, 1), output_padding=None):
+        self.groups, self.dilations, self.padding, self.strides = groups, tuple(dilations), padding, tuple(strides)
+        self.output_padding = None if output_padding is None else tuple(output_padding)
+
+    def _params(self):
+        return _conv_transpose_params(self.padding, self.groups, self.strides, self.dilations, self.output_padding)
+
+    def prepack(self, ctx, index, value):
+        """The per-phase sub-kernels of the weight (input 1), built once."""
+        if index != 1:
+            return None
+        A = _Args(ctx)
+        h = C.c_void_p()
+        p = self._params()
+        ctx.check(ctx.lib.rten_b200_prepack_conv_transpose_weight(ctx.handle, A.t(value), C.byref(p), C.byref(h)))
+        return Packed(ctx, h)
+
+    def run(self, ctx, x, w, bias=None, packed_w: Optional[Packed] = None, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        p = self._params()
+        ctx.check(ctx.lib.rten_b200_conv_transpose(ctx.handle, A.t(x), A.t(w), _ph(packed_w), A.t(bias), C.byref(p),
+                                                   C.byref(o)))
+        return A.wrap(o, out)
 
 
 class ConvInteger(Conv):
