@@ -49,6 +49,15 @@ rten_status pack_conv_weight(rten_ctx* ctx, const rten_tensor* w, int esize, voi
     return launch_nd_copy(ctx, esize, w->data, dst, 4, shape, ss, ds);
 }
 
+// t (3-D, the [B, C, W] of a 1-D convolution) as the 4-D [B, C, 1, W]
+void expand_1d(rten_tensor& t) {
+    t.ndim = 4;
+    t.shape[3] = t.shape[2];
+    t.strides[3] = t.strides[2];
+    t.shape[2] = 1;
+    t.strides[2] = 0;
+}
+
 // Validated geometry of one convolution (2-D form: a 1-D convolution is a 2-D one over a height-1 image).
 struct ConvShape {
     rten_tensor x, w, bias_v;
@@ -78,15 +87,8 @@ rten_status conv_shape(OpScope& sc, const ConvArgs& A, ConvShape& S) {
         if (w.ndim != 3) return fail(ctx, RTEN_ERR_INVALID_VALUE, "input must have 3 dims (OCW)");
         if (cp->n_strides != 1) return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected 1 stride value");
         if (cp->n_dilations != 1) return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected 1 dilation value");
-        auto expand = [](rten_tensor& t) {
-            t.ndim = 4;
-            t.shape[3] = t.shape[2];
-            t.strides[3] = t.strides[2];
-            t.shape[2] = 1;
-            t.strides[2] = 0;
-        };
-        expand(x);
-        expand(w);
+        expand_1d(x);
+        expand_1d(w);
         strides[1] = strides[0];
         strides[0] = 1;
         dil[1] = dil[0];
@@ -100,9 +102,9 @@ rten_status conv_shape(OpScope& sc, const ConvArgs& A, ConvShape& S) {
         if (cp->n_strides != 2) return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected 2 stride values");
         if (cp->n_dilations != 2) return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected 2 dilation values");
     }
-    const int64_t B = S.B = x.shape[0], C = S.C = x.shape[1], H = S.H = x.shape[2], W = S.W = x.shape[3];
+    S.B = x.shape[0];
+    const int64_t C = S.C = x.shape[1], H = S.H = x.shape[2], W = S.W = x.shape[3];
     const int64_t O = S.O = w.shape[0], Cg = S.Cg = w.shape[1], kh = S.kh = w.shape[2], kw = S.kw = w.shape[3];
-    (void)B;
     if (A.bias) {
         RTB_TRY(sc.in(A.bias, &S.bias_v));
         if (S.bias_v.ndim != 1 || S.bias_v.shape[0] != O)
@@ -138,13 +140,139 @@ rten_status conv_weight(rten_ctx* ctx, const ConvArgs& A, const ConvShape& S, in
     return RTEN_OK;
 }
 
+// An output [B, C, OH, OW] ([B, C, OW] when one_d) laid out like the input x: channels-last when x is (channel stride 1,
+// more than one channel), else NCHW
+struct OutLayout {
+    int ndim = 0;
+    int64_t shape[4], strides[4];
+};
+
+OutLayout layout_like(const rten_tensor& x, bool one_d, int64_t B, int64_t C, int64_t OH, int64_t OW) {
+    const bool cl = x.strides[1] == 1 && x.shape[1] > 1;
+    const int64_t shape[4] = {B, C, OH, OW};
+    const int64_t strides[4] = {C * OH * OW, cl ? 1 : OH * OW, cl ? OW * C : OW, cl ? C : 1};
+    OutLayout l;
+    for (int i = 0; i < 4; i++)
+        if (!one_d || i != 2) {
+            l.shape[l.ndim] = shape[i];
+            l.strides[l.ndim++] = strides[i];
+        }
+    return l;
+}
+
+// The output of an op on x, allocated here (when out->data is null) in x's layout; *ov is its 4-D view
+rten_status out_like(OpScope& sc, rten_tensor* out, int dtype, const rten_tensor& x, bool one_d, int64_t B, int64_t C,
+                     int64_t OH, int64_t OW, rten_tensor* ov) {
+    const OutLayout l = layout_like(x, one_d, B, C, OH, OW);
+    RTB_TRY(sc.out(out, dtype, l.ndim, l.shape, ov, out->data ? nullptr : l.strides));
+    if (one_d) expand_1d(*ov);
+    return RTEN_OK;
+}
+
+// x (4-D) as the implicit-GEMM kernel addresses it: channels-last with a 16-byte aligned base and pixel strides.  That is
+// x itself when it qualifies, else a channels-last copy in a temp.  A padded copy (pt, pl, pb, pr) is always made, its
+// border filled with `fill` (the reference's pad value of a u8 image).
+rten_status nhwc_input(rten_ctx* ctx, const rten_tensor& x, rten_tensor* xs, int64_t pt = 0, int64_t pl = 0, int64_t pb = 0,
+                       int64_t pr = 0, uint8_t fill = 0) {
+    const int es = dtype_size(x.dtype);
+    const bool padded = (pt | pl | pb | pr) != 0;
+    *xs = x;
+    if (!padded && x.strides[1] == 1 && reinterpret_cast<uintptr_t>(x.data) % 16 == 0 && (x.strides[3] * es) % 16 == 0 &&
+        (x.strides[2] * es) % 16 == 0 && (x.strides[0] * es) % 16 == 0)
+        return RTEN_OK;
+    const int64_t B = x.shape[0], C = x.shape[1], H = x.shape[2], W = x.shape[3], Hp = H + pt + pb, Wp = W + pl + pr;
+    void* buf = nullptr;
+    RTB_TRY(temp_alloc(ctx, (size_t)(B * Hp * Wp * C) * es, &buf));
+    if (padded) RTB_TRY(launch_fill8(ctx, buf, B * Hp * Wp * C, fill));
+    long long shape[4] = {B, H, W, C};
+    long long ss[4] = {x.strides[0], x.strides[2], x.strides[3], x.strides[1]};
+    long long ds[4] = {Hp * Wp * C, Wp * C, C, 1};
+    RTB_TRY(launch_nd_copy(ctx, es, x.data, (uint8_t*)buf + ((pt * Wp + pl) * C) * es, 4, shape, ss, ds));
+    xs->data = buf;
+    xs->shape[2] = Hp;
+    xs->shape[3] = Wp;
+    xs->strides[0] = Hp * Wp * C;
+    xs->strides[1] = 1;
+    xs->strides[2] = Wp * C;
+    xs->strides[3] = C;
+    return RTEN_OK;
+}
+
+// (c, x, y, b) of `channels` channels of a 4-D channels-last view, from element offset `off`: an implicit-GEMM A operand
+OperandDesc nhwc(const rten_tensor& v, int64_t channels, int64_t off = 0) {
+    OperandDesc d;
+    d.base = (const uint8_t*)v.data + off * dtype_size(v.dtype);
+    d.dims[0] = channels;
+    d.dims[1] = v.shape[3];
+    d.dims[2] = v.shape[2];
+    d.dims[3] = v.shape[0];
+    d.strides[1] = v.strides[3];
+    d.strides[2] = v.strides[2];
+    d.strides[3] = v.strides[0];
+    return d;
+}
+
+// (c, o, tap) of a packed conv weight [O, taps, C]: an implicit-GEMM B operand
+OperandDesc packed_weight(const void* w, int64_t C, int64_t O, int64_t taps) {
+    OperandDesc d;
+    d.base = w;
+    d.dims[0] = C;
+    d.dims[1] = O;
+    d.dims[2] = taps;
+    d.strides[1] = taps * C;
+    d.strides[2] = C;
+    return d;
+}
+
+// Conv-mode launch geometry of one group of S: M output pixels, N = Og, K = kh*kw*Cg
+void conv_geom(GemmLaunch& L, const ConvShape& S) {
+    L.conv = 1;
+    L.M = (int)(S.B * S.OH * S.OW);
+    L.N = (int)S.Og;
+    L.K = (int)(S.kh * S.kw * S.Cg);
+    ConvGeom& g = L.g;
+    g.B = (int)S.B;
+    g.H = (int)S.H;
+    g.W = (int)S.W;
+    g.C = (int)S.Cg;
+    g.OH = (int)S.OH;
+    g.OW = (int)S.OW;
+    g.kh = (int)S.kh;
+    g.kw = (int)S.kw;
+    g.sy = (int)S.strides[0];
+    g.sx = (int)S.strides[1];
+    g.dy = (int)S.dil[0];
+    g.dx = (int)S.dil[1];
+    g.pt = (int)S.pt;
+    g.pl = (int)S.pl;
+}
+
+// Points the epilogue at the 4-D output view v (f32 or i32) from channel c0 on
+void epi_out(EpilogueDesc& e, const rten_tensor& v, int64_t c0 = 0) {
+    e.d = (uint8_t*)v.data + (size_t)(c0 * v.strides[1]) * 4;
+    e.d_is_i32 = v.dtype == RTEN_I32;
+    e.s_z0 = v.strides[0];
+    e.s_row = v.strides[2];
+    e.s_z1 = v.strides[3];
+    e.s_col = v.strides[1];
+}
+
+// ... and its residual at the 4-D view r
+void epi_residual(EpilogueDesc& e, const rten_tensor& r, int64_t c0 = 0) {
+    e.r = (const float*)r.data + c0 * r.strides[1];
+    e.r_scale = 1.0f;
+    e.r_z0 = r.strides[0];
+    e.r_row = r.strides[2];
+    e.r_z1 = r.strides[3];
+    e.r_col = r.strides[1];
+}
+
 rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
     rten_ctx* ctx = sc.ctx;
     ConvShape S;
     RTB_TRY(conv_shape(sc, A, S));
     const rten_tensor& x = S.x;
     const rten_tensor& w = S.w;
-    const rten_tensor& bias_v = S.bias_v;
     const bool one_d = S.one_d;
     const int64_t* strides = S.strides;
     const int64_t* dil = S.dil;
@@ -154,45 +282,18 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
 
     // ---- output (layout follows the input: channels-last in -> channels-last out)
     const int out_dtype = (A.kind == 1 && !A.scale) ? RTEN_I32 : RTEN_F32;
-    int64_t oshape[4] = {B, O, OH, OW};
-    int64_t pref[4];
-    const bool x_cl = (x.strides[1] == 1 && C > 1);
-    if (x_cl) {
-        pref[1] = 1;
-        pref[3] = O;
-        pref[2] = OW * O;
-        pref[0] = OH * OW * O;
-    } else {
-        pref[3] = 1;
-        pref[2] = OW;
-        pref[1] = OH * OW;
-        pref[0] = O * OH * OW;
-    }
     rten_tensor ov;
-    if (one_d) {
-        int64_t os3[3] = {B, O, OW};
-        int64_t pf3[3] = {pref[0], pref[1], pref[3]};
-        RTB_TRY(sc.out(out, out_dtype, 3, os3, &ov, out->data ? nullptr : pf3));
-        ov.ndim = 4;
-        ov.shape[3] = ov.shape[2];
-        ov.strides[3] = ov.strides[2];
-        ov.shape[2] = 1;
-        ov.strides[2] = 0;
-    } else {
-        RTB_TRY(sc.out(out, out_dtype, 4, oshape, &ov, out->data ? nullptr : pref));
-    }
+    RTB_TRY(out_like(sc, out, out_dtype, x, one_d, B, O, OH, OW, &ov));
     if (B * O * OH * OW == 0) return RTEN_OK;
 
     const int esize = A.kind == 0 ? 4 : 1;
-    const int kelems = 128 / esize;
 
     const void* wp = nullptr;
     const int32_t* w_colsum = nullptr;
     RTB_TRY(conv_weight(ctx, A, S, esize, &wp, &w_colsum));
 
     // ---- integer zero points (x_zp scalar, w_zp per output channel)
-    const int32_t* za = nullptr;   // x zero point (GEMM A operand = activations), as i32 ...
-    const uint8_t* za8 = nullptr;  // ... or the 8-bit scalar as it is
+    const uint8_t* za8 = nullptr;  // x zero point (GEMM A operand = activations): the 8-bit scalar as it is
     const int32_t* zb = nullptr;   // w zero points per column
     int zb_len = 0;
     int pad_value = 0;
@@ -248,15 +349,9 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
     if (A.residual) {
         RTB_TRY(sc.in(A.residual, &res_v));
         if (res_v.ndim != (one_d ? 3 : 4)) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "residual shape does not match output");
-        if (one_d) {
-            res_v.ndim = 4;
-            res_v.shape[3] = res_v.shape[2];
-            res_v.strides[3] = res_v.strides[2];
-            res_v.shape[2] = 1;
-            res_v.strides[2] = 0;
-        }
+        if (one_d) expand_1d(res_v);
         for (int i = 0; i < 4; i++)
-            if (res_v.shape[i] != oshape[i]) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "residual shape does not match output");
+            if (res_v.shape[i] != ov.shape[i]) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "residual shape does not match output");
     }
 
     // ---- choose the addressing path
@@ -264,209 +359,95 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
     //  explicit: materialise the im2col matrix (odd channel counts such as the 3-channel stem)
     const bool need_pad_copy = (A.kind == 1 && !x_signed && (pt | pb | pl | pr) != 0);
     rten_tensor xs = x;  // source tensor for addressing (may be replaced by an NHWC / padded copy)
-    int64_t Hs = H, Ws = W, pt_s = pt, pl_s = pl;
     bool implicit_ok = (Cg * esize) % 16 == 0 && Cg * esize >= 32;
-    if (implicit_ok) {
-        const bool direct = x.strides[1] == 1 && !need_pad_copy && (reinterpret_cast<uintptr_t>(x.data) % 16 == 0) &&
-                            (x.strides[3] * esize) % 16 == 0 && (x.strides[2] * esize) % 16 == 0 &&
-                            (x.strides[0] * esize) % 16 == 0;
-        if (!direct) {
-            // copy to NHWC (with the reference's pad value baked in for u8 images)
-            const int64_t Hp = need_pad_copy ? H + pt + pb : H, Wp = need_pad_copy ? W + pl + pr : W;
-            void* buf = nullptr;
-            RTB_TRY(temp_alloc(ctx, (size_t)(B * Hp * Wp * C) * esize, &buf));
-            if (need_pad_copy) RTB_TRY(launch_fill8(ctx, buf, B * Hp * Wp * C, (uint8_t)pad_value));
-            long long shape[4] = {B, H, W, C};
-            long long ss[4] = {x.strides[0], x.strides[2], x.strides[3], x.strides[1]};
-            long long ds[4] = {Hp * Wp * C, Wp * C, C, 1};
-            uint8_t* dst = (uint8_t*)buf + (need_pad_copy ? ((pt * Wp + pl) * C) * esize : 0);
-            RTB_TRY(launch_nd_copy(ctx, esize, x.data, dst, 4, shape, ss, ds));
-            xs.data = buf;
-            xs.strides[0] = Hp * Wp * C;
-            xs.strides[1] = 1;
-            xs.strides[2] = Wp * C;
-            xs.strides[3] = C;
-            if (need_pad_copy) {
-                Hs = Hp;
-                Ws = Wp;
-                pt_s = 0;
-                pl_s = 0;
-            }
-        }
-    }
+    if (implicit_ok)  // (u8 images with padding: a copy with the reference's pad value baked in)
+        RTB_TRY(need_pad_copy ? nhwc_input(ctx, x, &xs, pt, pl, pb, pr, (uint8_t)pad_value) : nhwc_input(ctx, x, &xs));
 
-    // ---- small-channel path (C <= 4, e.g. the RGB stem): NHWC4 zero-padded copy, one 128-byte K block per filter
-    //      row holding kw pixels x 4 channels; vertical padding / stride stay in the TMA tile addressing.
-    const bool smallc_ok = !implicit_ok && A.kind == 0 && groups == 1 && Cg <= 4 && kw * 4 <= 32 && dil[1] == 1 &&
-                           (int64_t)B * OH * OW > 0 && !getenv("RTEN_B200_NO_SMALLC");
+    rten_tensor bias_c;
+    if (A.bias) RTB_TRY(sc.contiguous(&S.bias_v, &bias_c));
+    // the epilogue of output channels [c0, c0 + N)
+    auto epilogue = [&](EpilogueDesc& e, int64_t c0) {
+        epi_out(e, ov, c0);
+        e.act = A.act;
+        if (A.bias) {
+            e.bias = (const float*)bias_c.data + c0;
+            e.bias_kind = 1;
+        }
+        if (A.residual) epi_residual(e, res_v, c0);
+        if (A.kind == 1) {
+            e.za8 = za8;
+            e.za8_signed = x_signed;
+            e.scale2 = scale2_p;
+            e.range = range_p;
+            e.colsum = w_colsum ? w_colsum + c0 : nullptr;
+            e.zb = zb ? (zb_len == 1 ? zb : zb + c0) : nullptr;
+            e.zb_len = zb ? (zb_len == 1 ? 1 : (int)Og) : 0;
+            e.scale = scale_p;
+            e.scale_len = scale_p ? 1 : 0;
+        }
+    };
+
+    // ---- small-channel path (the RGB stem: C <= 4 in f32, C <= 16 in 8-bit): a zero-padded copy with `pitch` channels
+    //      per pixel, one 128-byte K block per filter row holding kw pixels x pitch channels.  The 8-bit copy also holds
+    //      the vertical padding (the reference's pad value); f32 leaves vertical padding / stride to the TMA tile addressing.
+    const bool smallc_ok = !implicit_ok && groups == 1 && dil[1] == 1 && (int64_t)B * OH * OW > 0 &&
+                           !getenv("RTEN_B200_NO_SMALLC") &&
+                           (A.kind == 0 ? Cg <= 4 && kw * 4 <= 32 : Cg <= 16 && kw <= 8 && !zb);
     if (smallc_ok) {
-        const int64_t Wp = (OW - 1) * strides[1] + 8;  // every window of 8 pixels stays inside the padded row
-        float* xp = nullptr;
-        RTB_TRY(temp_alloc(ctx, (size_t)(B * H * Wp * 4) * 4, (void**)&xp));
-        RTB_TRY(launch_smallc_pad(ctx, (const float*)x.data, xp, (int)B, (int)C, (int)H, (int)W, (int)Wp, (int)pl, x.strides[0],
-                                  x.strides[1], x.strides[2], x.strides[3]));
-        float* wsm = nullptr;
-        RTB_TRY(temp_alloc(ctx, (size_t)(O * kh * 32) * 4, (void**)&wsm));
-        RTB_TRY(launch_smallc_pack_w(ctx, (const float*)w.data, wsm, (int)O, (int)C, (int)kh, (int)kw, w.strides[0], w.strides[1],
-                                     w.strides[2], w.strides[3]));
+        const bool q8 = A.kind == 1;
+        const int64_t pitch = q8 ? 16 : 4, kb = 128 / esize;  // channels per pixel of the copy, elements per K block
+        const int64_t Hp = q8 ? H + pt + pb : H;
+        // every window of 8 pixels stays inside the padded row
+        const int64_t Wp = std::max<int64_t>(q8 ? W + pl + pr : 0, (OW - 1) * strides[1] + 8);
+        void *xp = nullptr, *wsm = nullptr;
+        RTB_TRY(temp_alloc(ctx, (size_t)(B * Hp * Wp * pitch) * esize, &xp));
+        if (q8) {
+            RTB_TRY(launch_smallc8_pad(ctx, x.data, xp, (int)B, (int)C, (int)H, (int)W, (int)Hp, (int)Wp, (int)pt, (int)pl,
+                                       x.strides[0], x.strides[1], x.strides[2], x.strides[3], pad_value));
+        } else {
+            RTB_TRY(launch_smallc_pad(ctx, (const float*)x.data, (float*)xp, (int)B, (int)C, (int)H, (int)W, (int)Wp, (int)pl,
+                                      x.strides[0], x.strides[1], x.strides[2], x.strides[3]));
+        }
+        RTB_TRY(temp_alloc(ctx, (size_t)(O * kh * 128), &wsm));
+        if (q8) {
+            RTB_TRY(launch_smallc8_pack_w(ctx, w.data, wsm, (int)O, (int)C, (int)kh, (int)kw, w.strides[0], w.strides[1],
+                                          w.strides[2], w.strides[3]));
+        } else {
+            RTB_TRY(launch_smallc_pack_w(ctx, (const float*)w.data, (float*)wsm, (int)O, (int)C, (int)kh, (int)kw, w.strides[0],
+                                         w.strides[1], w.strides[2], w.strides[3]));
+        }
         GemmLaunch L;
-        L.kind = 0;
-        L.conv = 1;
-        L.N = (int)O;
-        L.K = (int)(kh * 32);
-        L.M = (int)(B * OH * OW);
-        L.g.B = (int)B;
-        L.g.H = (int)H;
+        L.kind = A.kind;
+        L.a_signed = x_signed;
+        L.b_signed = w_signed;
+        conv_geom(L, S);
+        L.K = (int)(kh * kb);
+        L.g.H = (int)Hp;
         L.g.W = (int)OW;  // dim 1 of the A map indexes output columns directly
-        L.g.C = 32;
-        L.g.OH = (int)OH;
-        L.g.OW = (int)OW;
-        L.g.kh = (int)kh;
+        L.g.C = (int)kb;
         L.g.kw = 1;
-        L.g.sy = (int)strides[0];
         L.g.sx = 1;
-        L.g.dy = (int)dil[0];
-        L.g.dx = 1;
-        L.g.pt = (int)pt;
+        L.g.pt = q8 ? 0 : (int)pt;
         L.g.pl = 0;
         L.a.base = xp;
-        L.a.dims[0] = 32;
+        L.a.dims[0] = kb;
         L.a.dims[1] = OW;
-        L.a.dims[2] = H;
+        L.a.dims[2] = Hp;
         L.a.dims[3] = B;
-        L.a.strides[0] = 1;
-        L.a.strides[1] = strides[1] * 4;
-        L.a.strides[2] = Wp * 4;
-        L.a.strides[3] = H * Wp * 4;
-        if (ctx->f32_mode == RTEN_F32_TF32X3 && !getenv("RTEN_B200_X3_THREE_PLANES")) {
-            // 3xTF32: the low parts of the padded copy, once (the window view below overlaps itself 8 / stride times)
+        L.a.strides[1] = strides[1] * pitch;
+        L.a.strides[2] = Wp * pitch;
+        L.a.strides[3] = Hp * Wp * pitch;
+        if (!q8 && ctx->f32_mode == RTEN_F32_TF32X3 && !getenv("RTEN_B200_X3_THREE_PLANES")) {
+            // 3xTF32: the low parts of the padded copy, once (the window view above overlaps itself 8 / stride times)
             float* xlo = nullptr;
             const long long n = (long long)B * H * Wp * 4;
             RTB_TRY(temp_alloc(ctx, (size_t)n * 4, (void**)&xlo));
             const long long fd[4] = {n, 1, 1, 1}, fs[4] = {1, n, n, n};
-            RTB_TRY(launch_tf32x3_split(ctx, xp, xlo, fd, fs, n, 2));
+            RTB_TRY(launch_tf32x3_split(ctx, (const float*)xp, xlo, fd, fs, n, 2));
             L.a_lo_base = xlo;
         }
-        L.b.base = wsm;
-        L.b.dims[0] = 32;
-        L.b.dims[1] = O;
-        L.b.dims[2] = kh;
-        L.b.dims[3] = 1;
-        L.b.strides[0] = 1;
-        L.b.strides[1] = kh * 32;
-        L.b.strides[2] = 32;
-        L.b.strides[3] = 0;
-        EpilogueDesc& e = L.epi;
-        e.d = ov.data;
-        e.s_z0 = ov.strides[0];
-        e.s_row = ov.strides[2];
-        e.s_z1 = ov.strides[3];
-        e.s_col = ov.strides[1];
-        e.act = A.act;
-        if (A.bias) {
-            rten_tensor bc;
-            RTB_TRY(sc.contiguous(&bias_v, &bc));
-            e.bias = (const float*)bc.data;
-            e.bias_kind = 1;
-        }
-        if (A.residual) {
-            e.r = (const float*)res_v.data;
-            e.r_scale = 1.0f;
-            e.r_z0 = res_v.strides[0];
-            e.r_row = res_v.strides[2];
-            e.r_z1 = res_v.strides[3];
-            e.r_col = res_v.strides[1];
-        }
-        rten_status st = launch_umma_gemm(ctx, L);
-        if (st == RTEN_OK) return RTEN_OK;
-        if (st != RTEN_ERR_UNSUPPORTED_VALUE) return st;
-        // otherwise fall through to the generic explicit path
-    }
-
-    // ---- 8-bit small-channel path (the quantised RGB stem): padded [B,Hp,Wp,16] copy, one 128-byte K block per filter row
-    const bool smallc8_ok = !implicit_ok && A.kind == 1 && groups == 1 && Cg <= 16 && kw <= 8 && dil[1] == 1 && !zb &&
-                            (int64_t)B * OH * OW > 0 && !getenv("RTEN_B200_NO_SMALLC");
-    if (smallc8_ok) {
-        const int64_t Hp = H + pt + pb;
-        const int64_t Wp = std::max<int64_t>(W + pl + pr, (OW - 1) * strides[1] + 8);
-        void *xp = nullptr, *wsm = nullptr;
-        RTB_TRY(temp_alloc(ctx, (size_t)(B * Hp * Wp * 16), &xp));
-        RTB_TRY(launch_smallc8_pad(ctx, x.data, xp, (int)B, (int)C, (int)H, (int)W, (int)Hp, (int)Wp, (int)pt, (int)pl,
-                                   x.strides[0], x.strides[1], x.strides[2], x.strides[3], pad_value));
-        RTB_TRY(temp_alloc(ctx, (size_t)(O * kh * 128), &wsm));
-        RTB_TRY(launch_smallc8_pack_w(ctx, w.data, wsm, (int)O, (int)C, (int)kh, (int)kw, w.strides[0], w.strides[1],
-                                      w.strides[2], w.strides[3]));
-        GemmLaunch L;
-        L.kind = 1;
-        L.a_signed = x_signed;
-        L.b_signed = w_signed;
-        L.conv = 1;
-        L.N = (int)O;
-        L.K = (int)(kh * 128);
-        L.M = (int)(B * OH * OW);
-        L.g.B = (int)B;
-        L.g.H = (int)Hp;
-        L.g.W = (int)OW;  // dim 1 of the A map indexes output columns directly
-        L.g.C = 128;
-        L.g.OH = (int)OH;
-        L.g.OW = (int)OW;
-        L.g.kh = (int)kh;
-        L.g.kw = 1;
-        L.g.sy = (int)strides[0];
-        L.g.sx = 1;
-        L.g.dy = (int)dil[0];
-        L.g.dx = 1;
-        L.g.pt = 0;
-        L.g.pl = 0;
-        L.a.base = xp;
-        L.a.dims[0] = 128;
-        L.a.dims[1] = OW;
-        L.a.dims[2] = Hp;
-        L.a.dims[3] = B;
-        L.a.strides[0] = 1;
-        L.a.strides[1] = strides[1] * 16;
-        L.a.strides[2] = Wp * 16;
-        L.a.strides[3] = Hp * Wp * 16;
-        L.b.base = wsm;
-        L.b.dims[0] = 128;
-        L.b.dims[1] = O;
-        L.b.dims[2] = kh;
-        L.b.dims[3] = 1;
-        L.b.strides[0] = 1;
-        L.b.strides[1] = kh * 128;
-        L.b.strides[2] = 128;
-        L.b.strides[3] = 0;
-        EpilogueDesc& e = L.epi;
-        e.d = ov.data;
-        e.d_is_i32 = out_dtype == RTEN_I32;
-        e.s_z0 = ov.strides[0];
-        e.s_row = ov.strides[2];
-        e.s_z1 = ov.strides[3];
-        e.s_col = ov.strides[1];
-        e.act = A.act;
-        if (A.bias) {
-            rten_tensor bc;
-            RTB_TRY(sc.contiguous(&bias_v, &bc));
-            e.bias = (const float*)bc.data;
-            e.bias_kind = 1;
-        }
-        if (A.residual) {
-            e.r = (const float*)res_v.data;
-            e.r_scale = 1.0f;
-            e.r_z0 = res_v.strides[0];
-            e.r_row = res_v.strides[2];
-            e.r_z1 = res_v.strides[3];
-            e.r_col = res_v.strides[1];
-        }
-        e.za = za;
-        e.za_len = za ? 1 : 0;
-        e.za8 = za8;
-        e.za8_signed = x_signed;
-        e.colsum = w_colsum;
-        e.scale = scale_p;
-        e.scale_len = scale_p ? 1 : 0;
-        e.scale2 = scale2_p;
-        e.range = range_p;
+        L.b = packed_weight(wsm, kb, O, kh);
+        epilogue(L.epi, 0);
         rten_status st = launch_umma_gemm(ctx, L);
         if (st == RTEN_OK) return RTEN_OK;
         if (st != RTEN_ERR_UNSUPPORTED_VALUE) return st;
@@ -481,77 +462,16 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
         L.N = (int)Og;
         L.K = (int)(kh * kw * Cg);
         EpilogueDesc& e = L.epi;
-        e.d = (uint8_t*)ov.data + (size_t)(g * Og * ov.strides[1]) * 4;
-        e.d_is_i32 = out_dtype == RTEN_I32;
-        e.s_z0 = ov.strides[0];
-        e.s_row = ov.strides[2];
-        e.s_z1 = ov.strides[3];
-        e.s_col = ov.strides[1];
-        e.act = A.act;
-        if (A.bias) {
-            rten_tensor bc;
-            RTB_TRY(sc.contiguous(&bias_v, &bc));
-            e.bias = (const float*)bc.data + g * Og;
-            e.bias_kind = 1;
-        }
-        if (A.residual) {
-            e.r = (const float*)res_v.data + g * Og * res_v.strides[1];
-            e.r_scale = 1.0f;
-            e.r_z0 = res_v.strides[0];
-            e.r_row = res_v.strides[2];
-            e.r_z1 = res_v.strides[3];
-            e.r_col = res_v.strides[1];
-        }
-        if (A.kind == 1) {
-            e.za = za;
-            e.za_len = za ? 1 : 0;
-            e.za8 = za8;
-            e.za8_signed = x_signed;
-            e.scale2 = scale2_p;
-            e.range = range_p;
-            e.colsum = w_colsum ? w_colsum + g * Og : nullptr;
-            e.zb = zb ? (zb_len == 1 ? zb : zb + g * Og) : nullptr;
-            e.zb_len = zb ? (zb_len == 1 ? 1 : (int)Og) : 0;
-            e.scale = scale_p;
-            e.scale_len = scale_p ? 1 : 0;
-        }
+        epilogue(e, g * Og);
         const uint8_t* wg = (const uint8_t*)wp + (size_t)(g * Og * kh * kw * Cg) * esize;
 
         if (implicit_ok) {
-            L.conv = 1;
-            L.g.B = (int)B;
-            L.g.H = (int)Hs;
-            L.g.W = (int)Ws;
-            L.g.C = (int)Cg;
-            L.g.OH = (int)OH;
-            L.g.OW = (int)OW;
-            L.g.kh = (int)kh;
-            L.g.kw = (int)kw;
-            L.g.sy = (int)strides[0];
-            L.g.sx = (int)strides[1];
-            L.g.dy = (int)dil[0];
-            L.g.dx = (int)dil[1];
-            L.g.pt = (int)pt_s;
-            L.g.pl = (int)pl_s;
-            L.M = (int)(B * OH * OW);
-            L.a.base = (const uint8_t*)xs.data + (size_t)(g * Cg) * esize;
-            L.a.dims[0] = Cg;
-            L.a.dims[1] = Ws;
-            L.a.dims[2] = Hs;
-            L.a.dims[3] = B;
-            L.a.strides[0] = 1;
-            L.a.strides[1] = xs.strides[3];
-            L.a.strides[2] = xs.strides[2];
-            L.a.strides[3] = xs.strides[0];
-            L.b.base = wg;
-            L.b.dims[0] = Cg;
-            L.b.dims[1] = Og;
-            L.b.dims[2] = kh * kw;
-            L.b.dims[3] = 1;
-            L.b.strides[0] = 1;
-            L.b.strides[1] = kh * kw * Cg;
-            L.b.strides[2] = Cg;
-            L.b.strides[3] = 0;
+            conv_geom(L, S);
+            L.g.H = (int)xs.shape[2];
+            L.g.W = (int)xs.shape[3];
+            if (need_pad_copy) L.g.pt = L.g.pl = 0;  // (the copy holds the padding)
+            L.a = nhwc(xs, Cg, g * Cg);
+            L.b = packed_weight(wg, Cg, Og, kh * kw);
             if (A.pw && A.kind == 0 && groups == 1 && wg == A.pw->data && A.cache_x3)
                 L.b_x3_slot = &const_cast<rten_packed*>(A.pw)->x3;
             if (A.x_lo && xs.data == x.data) L.a_lo_base = (const float*)A.x_lo + g * Cg;
@@ -681,6 +601,46 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
     return RTEN_OK;
 }
 
+// A 1x1, unpadded convolution over a channels-last, TMA-addressable input whose channels fill whole 128-byte K blocks:
+// one side of a folded launch
+bool pointwise(const ConvShape& s) {
+    return !s.one_d && s.kh == 1 && s.kw == 1 && s.groups == 1 && (s.pt | s.pb | s.pl | s.pr) == 0 && s.dil[0] == 1 &&
+           s.dil[1] == 1 && s.x.strides[1] == 1 && s.C % 32 == 0 && tma_compatible(nhwc(s.x, s.C), 4, 4);
+}
+
+// The launch of act(Conv(x, w, bias) [+ Conv(x_proj, w_proj, bias_proj)]) into the 4-D view ov: with a projection, ONE
+// GEMM over both K ranges (GemmLaunch::proj)
+rten_status folded_launch(OpScope& sc, const ConvArgs& M, const ConvShape& sm, const ConvArgs* P, const ConvShape& sp,
+                          const rten_tensor& ov, GemmLaunch& L) {
+    const void *wm = nullptr, *wpj = nullptr;
+    const int32_t* unused = nullptr;
+    RTB_TRY(conv_weight(sc.ctx, M, sm, 4, &wm, &unused));
+    if (P) RTB_TRY(conv_weight(sc.ctx, *P, sp, 4, &wpj, &unused));
+    L.kind = 0;
+    conv_geom(L, sm);
+    L.a = nhwc(sm.x, sm.C);
+    L.b = packed_weight(wm, sm.C, sm.O, 1);
+    if (P) {
+        L.proj.C = (int)sp.C;
+        L.proj.stride = (int)sp.strides[0];
+        L.proj.a = nhwc(sp.x, sp.C);
+        L.proj.b = packed_weight(wpj, sp.C, sp.O, 1);
+    }
+    EpilogueDesc& e = L.epi;
+    epi_out(e, ov);
+    e.act = M.act;
+    const bool p_bias = P && P->bias;
+    rten_tensor bm, bp;
+    if (M.bias) RTB_TRY(sc.contiguous(&sm.bias_v, &bm));
+    if (p_bias) RTB_TRY(sc.contiguous(&sp.bias_v, &bp));
+    if (M.bias || p_bias) {
+        e.bias_kind = 1;
+        e.bias = (const float*)(M.bias ? bm.data : bp.data);
+        if (M.bias && p_bias) e.bias2 = (const float*)bp.data;
+    }
+    return RTEN_OK;
+}
+
 // act(Conv(x, w, bias) + Conv(x_proj, w_proj, bias_proj)) -- a residual block's last convolution and its projection
 // shortcut.  Two 1x1 convolutions over channels-last, TMA-addressable inputs with whole 128-byte channel blocks run as
 // ONE GEMM over both K ranges (GemmLaunch::proj): the shortcut tensor is never written.  Anything else computes the
@@ -693,106 +653,27 @@ rten_status conv_projected(OpScope& sc, ConvArgs& M, ConvArgs& P, rten_tensor* o
     if (sm.one_d != sp.one_d || sm.B != sp.B || sm.O != sp.O || sm.OH != sp.OH || sm.OW != sp.OW)
         return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "projection output shape does not match the convolution's output shape");
     const int64_t B = sm.B, O = sm.O, OH = sm.OH, OW = sm.OW;
-    auto pointwise = [](const ConvShape& s) {
-        return !s.one_d && s.kh == 1 && s.kw == 1 && s.groups == 1 && (s.pt | s.pb | s.pl | s.pr) == 0 && s.dil[0] == 1 &&
-               s.dil[1] == 1 && s.x.strides[1] == 1 && s.C % 32 == 0;
-    };
-    // NHWC view (c, x, y, b) of an input
-    auto nhwc = [](const ConvShape& s) {
-        OperandDesc d;
-        d.base = s.x.data;
-        d.dims[0] = s.C;
-        d.dims[1] = s.W;
-        d.dims[2] = s.H;
-        d.dims[3] = s.B;
-        d.strides[0] = 1;
-        d.strides[1] = s.x.strides[3];
-        d.strides[2] = s.x.strides[2];
-        d.strides[3] = s.x.strides[0];
-        return d;
-    };
-    const OperandDesc am = nhwc(sm), ap = nhwc(sp);
-    const bool fold = pointwise(sm) && pointwise(sp) && sp.strides[0] == sp.strides[1] && tma_compatible(am, 4, 4) &&
-                      tma_compatible(ap, 4, 4) && (!out->data || out->device >= 0) && B * O * OH * OW > 0;
+    const bool fold = pointwise(sm) && pointwise(sp) && sp.strides[0] == sp.strides[1] && (!out->data || out->device >= 0) &&
+                      B * O * OH * OW > 0;
     if (fold) {
-        const int64_t oshape[4] = {B, O, OH, OW}, pref[4] = {OH * OW * O, 1, OW * O, O};
         rten_tensor ov;
-        RTB_TRY(sc.out(out, RTEN_F32, 4, oshape, &ov, out->data ? nullptr : pref));
-        const void *wm = nullptr, *wpj = nullptr;
-        const int32_t* unused = nullptr;
-        RTB_TRY(conv_weight(ctx, M, sm, 4, &wm, &unused));
-        RTB_TRY(conv_weight(ctx, P, sp, 4, &wpj, &unused));
-        auto weights = [](const void* w, const ConvShape& s) {  // (c, o, 1, 1) of the packed [O, 1, 1, C]
-            OperandDesc d;
-            d.base = w;
-            d.dims[0] = s.C;
-            d.dims[1] = s.O;
-            d.strides[0] = 1;
-            d.strides[1] = s.C;
-            return d;
-        };
+        RTB_TRY(out_like(sc, out, RTEN_F32, sm.x, false, B, O, OH, OW, &ov));  // (x is channels-last: so is the output)
         GemmLaunch L;
-        L.kind = 0;
-        L.conv = 1;
-        L.N = (int)O;
-        L.K = (int)sm.C;
-        L.M = (int)(B * OH * OW);
-        L.g.B = (int)B;
-        L.g.H = (int)sm.H;
-        L.g.W = (int)sm.W;
-        L.g.C = (int)sm.C;
-        L.g.OH = (int)OH;
-        L.g.OW = (int)OW;
-        L.g.sy = (int)sm.strides[0];
-        L.g.sx = (int)sm.strides[1];
-        L.a = am;
-        L.b = weights(wm, sm);
+        RTB_TRY(folded_launch(sc, M, sm, &P, sp, ov, L));
         if (M.pw) L.b_x3_slot = &const_cast<rten_packed*>(M.pw)->x3;
-        L.proj.C = (int)sp.C;
-        L.proj.stride = (int)sp.strides[0];
-        L.proj.a = ap;
-        L.proj.b = weights(wpj, sp);
         if (P.pw) L.proj.b_x3_slot = &const_cast<rten_packed*>(P.pw)->x3;
-        EpilogueDesc& e = L.epi;
-        e.d = ov.data;
-        e.s_z0 = ov.strides[0];
-        e.s_row = ov.strides[2];
-        e.s_z1 = ov.strides[3];
-        e.s_col = ov.strides[1];
-        e.act = M.act;
-        rten_tensor bm, bp;
-        if (M.bias) RTB_TRY(sc.contiguous(&sm.bias_v, &bm));
-        if (P.bias) RTB_TRY(sc.contiguous(&sp.bias_v, &bp));
-        if (M.bias || P.bias) {
-            e.bias_kind = 1;
-            e.bias = (const float*)(M.bias ? bm.data : bp.data);
-            if (M.bias && P.bias) e.bias2 = (const float*)bp.data;
-        }
         const rten_status st = launch_umma_gemm(ctx, L);
         if (st != RTEN_ERR_UNSUPPORTED_VALUE) return st;
         // (no launch plan takes the plain f32 epilogue for this output: two convolutions)
     }
     // the projection in the layout rten_b200_conv2d_ex would give it, then the main convolution with it as the residual
+    const OutLayout l = layout_like(sp.x, sp.one_d, B, O, OH, OW);
     rten_tensor tmp{};
     tmp.dtype = RTEN_F32;
     tmp.device = ctx->device;
-    const bool cl = sp.x.strides[1] == 1 && sp.C > 1;
-    const int64_t sc_ = cl ? 1 : OH * OW, sw = cl ? O : 1, sh = OW * sw;
-    if (sp.one_d) {
-        tmp.ndim = 3;
-        const int64_t shape[3] = {B, O, OW}, st[3] = {O * OH * OW, sc_, sw};
-        for (int i = 0; i < 3; i++) {
-            tmp.shape[i] = shape[i];
-            tmp.strides[i] = st[i];
-        }
-    } else {
-        tmp.ndim = 4;
-        const int64_t shape[4] = {B, O, OH, OW}, st[4] = {O * OH * OW, sc_, sh, sw};
-        for (int i = 0; i < 4; i++) {
-            tmp.shape[i] = shape[i];
-            tmp.strides[i] = st[i];
-        }
-    }
+    tmp.ndim = l.ndim;
+    std::copy(l.shape, l.shape + l.ndim, tmp.shape);
+    std::copy(l.strides, l.strides + l.ndim, tmp.strides);
     RTB_TRY(temp_alloc(ctx, (size_t)std::max<int64_t>(B * O * OH * OW, 1) * 4, &tmp.data));
     RTB_TRY(conv_core(sc, P, &tmp));
     M.residual = &tmp;
@@ -821,114 +702,35 @@ rten_status conv_chained(OpScope& sc, ConvArgs& M, ConvArgs* P, ConvArgs& Nx, rt
                           np->strides[1] == 1 && np->dilations[0] == 1 && np->dilations[1] == 1 && !np->auto_pad_same &&
                           (np->pads[0] | np->pads[1] | np->pads[2] | np->pads[3]) == 0;
     const int64_t N2 = Nx.w->ndim == 4 ? Nx.w->shape[0] : 0;
-    auto pointwise = [](const ConvShape& s) {
-        return !s.one_d && s.kh == 1 && s.kw == 1 && s.groups == 1 && (s.pt | s.pb | s.pl | s.pr) == 0 && s.dil[0] == 1 &&
-               s.dil[1] == 1 && s.x.strides[1] == 1 && s.C % 32 == 0;
-    };
-    auto nhwc = [](const ConvShape& s) {
-        OperandDesc d;
-        d.base = s.x.data;
-        d.dims[0] = s.C;
-        d.dims[1] = s.W;
-        d.dims[2] = s.H;
-        d.dims[3] = s.B;
-        d.strides[1] = s.x.strides[3];
-        d.strides[2] = s.x.strides[2];
-        d.strides[3] = s.x.strides[0];
-        return d;
-    };
-    const OperandDesc am = nhwc(sm);
-    OperandDesc ap;
-    if (P) ap = nhwc(sp);
     rten_tensor res_v;
     if (M.residual) RTB_TRY(sc.in(M.residual, &res_v));
     const bool chain = ctx->f32_mode == RTEN_F32_TF32 && next_1x1 && (N2 == 64 || N2 == 128) && O % 32 == 0 && O <= 256 &&
-                       pointwise(sm) && tma_compatible(am, 4, 4) &&
-                       (!P || (pointwise(sp) && sp.strides[0] == sp.strides[1] && tma_compatible(ap, 4, 4))) &&
+                       pointwise(sm) && (!P || (pointwise(sp) && sp.strides[0] == sp.strides[1])) &&
                        (!M.residual || (res_v.ndim == 4 && res_v.strides[1] == 1)) && (!out->data || out->device >= 0) &&
                        (!out_next->data || out_next->device >= 0) && B * O * OH * OW > 0;
     if (chain) {
-        const int64_t oshape[4] = {B, O, OH, OW}, pref[4] = {OH * OW * O, 1, OW * O, O};
-        const int64_t zshape[4] = {B, N2, OH, OW}, zpref[4] = {OH * OW * N2, 1, OW * N2, N2};
-        rten_tensor ov, zv;
-        RTB_TRY(sc.out(out, RTEN_F32, 4, oshape, &ov, out->data ? nullptr : pref));
-        RTB_TRY(sc.out(out_next, RTEN_F32, 4, zshape, &zv, out_next->data ? nullptr : zpref));
+        rten_tensor ov, zv;  // (x is channels-last: so are y and z)
+        RTB_TRY(out_like(sc, out, RTEN_F32, sm.x, false, B, O, OH, OW, &ov));
+        RTB_TRY(out_like(sc, out_next, RTEN_F32, sm.x, false, B, N2, OH, OW, &zv));
         for (int i = 0; M.residual && i < 4; i++)
-            if (res_v.shape[i] != oshape[i]) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "residual shape does not match output");
+            if (res_v.shape[i] != ov.shape[i]) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "residual shape does not match output");
         RTB_TRY(conv_shape(sc, Nx, sn));  // (x = y: checks w_next and bias_next against it)
-        const void *wm = nullptr, *wpj = nullptr, *wn = nullptr;
-        const int32_t* unused = nullptr;
-        RTB_TRY(conv_weight(ctx, M, sm, 4, &wm, &unused));
-        if (P) RTB_TRY(conv_weight(ctx, *P, sp, 4, &wpj, &unused));
-        RTB_TRY(conv_weight(ctx, Nx, sn, 4, &wn, &unused));
-        auto weights = [](const void* w, int64_t C, int64_t O_) {  // (c, o, 1, 1) of the packed [O, 1, 1, C]
-            OperandDesc d;
-            d.base = w;
-            d.dims[0] = C;
-            d.dims[1] = O_;
-            d.strides[1] = C;
-            return d;
-        };
         GemmLaunch L;
-        L.kind = 0;
-        L.conv = 1;
-        L.N = (int)O;
-        L.K = (int)sm.C;
-        L.M = (int)(B * OH * OW);
-        L.g.B = (int)B;
-        L.g.H = (int)sm.H;
-        L.g.W = (int)sm.W;
-        L.g.C = (int)sm.C;
-        L.g.OH = (int)OH;
-        L.g.OW = (int)OW;
-        L.g.sy = (int)sm.strides[0];
-        L.g.sx = (int)sm.strides[1];
-        L.a = am;
-        L.b = weights(wm, sm.C, O);
-        if (P) {
-            L.proj.C = (int)sp.C;
-            L.proj.stride = (int)sp.strides[0];
-            L.proj.a = ap;
-            L.proj.b = weights(wpj, sp.C, O);
-        }
-        EpilogueDesc& e = L.epi;
-        e.d = ov.data;
-        e.s_z0 = ov.strides[0];
-        e.s_row = ov.strides[2];
-        e.s_z1 = ov.strides[3];
-        e.s_col = ov.strides[1];
-        e.act = M.act;
-        rten_tensor bm, bp, bn;
-        if (M.bias) RTB_TRY(sc.contiguous(&sm.bias_v, &bm));
-        if (P && P->bias) RTB_TRY(sc.contiguous(&sp.bias_v, &bp));
-        if (M.bias || (P && P->bias)) {
-            e.bias_kind = 1;
-            e.bias = (const float*)(M.bias ? bm.data : bp.data);
-            if (M.bias && P && P->bias) e.bias2 = (const float*)bp.data;
-        }
-        if (M.residual) {
-            e.r = (const float*)res_v.data;
-            e.r_z0 = res_v.strides[0];
-            e.r_row = res_v.strides[2];
-            e.r_z1 = res_v.strides[3];
-            e.r_col = res_v.strides[1];
-        }
+        RTB_TRY(folded_launch(sc, M, sm, P, sp, ov, L));
+        if (M.residual) epi_residual(L.epi, res_v);
+        const void* wn = nullptr;
+        const int32_t* unused = nullptr;
+        RTB_TRY(conv_weight(ctx, Nx, sn, 4, &wn, &unused));
         GemmLaunch::Chain& c = L.chain;
         c.N2 = (int)N2;
-        c.w = weights(wn, O, N2);
+        c.w = packed_weight(wn, O, N2, 1);
+        rten_tensor bn;
         if (Nx.bias) {
             RTB_TRY(sc.contiguous(&sn.bias_v, &bn));
             c.bias = (const float*)bn.data;
         }
         c.act = Nx.act;
-        c.z.base = zv.data;
-        c.z.dims[0] = N2;
-        c.z.dims[1] = OW;
-        c.z.dims[2] = OH;
-        c.z.dims[3] = B;
-        c.z.strides[1] = zv.strides[3];
-        c.z.strides[2] = zv.strides[2];
-        c.z.strides[3] = zv.strides[0];
+        c.z = nhwc(zv, N2);
         if (zv.strides[1] == 1) {
             const rten_status st = launch_umma_gemm(ctx, L);
             if (st != RTEN_ERR_UNSUPPORTED_VALUE) return st;
@@ -1002,14 +804,6 @@ struct ConvTShape {
     int64_t B, C, H, W, O, Og, Cg, kh, kw, OH, OW, sy, sx, dy, dx, pt, pl, pb, pr;
     int groups;
 };
-
-void expand_1d(rten_tensor& t) {
-    t.ndim = 4;
-    t.shape[3] = t.shape[2];
-    t.strides[3] = t.strides[2];
-    t.shape[2] = 1;
-    t.strides[2] = 0;
-}
 
 // Argument checks in the reference's order (conv_transpose.rs:226-345, conv_transpose_output_size_and_padding
 // :144-220) on the kernel `w` (and input `x` when given)
@@ -1136,18 +930,8 @@ rten_status conv_transpose_core(OpScope& sc, const rten_tensor* x_in, const rten
     const int groups = S.groups;
 
     // ---- output (layout follows the input: channels-last in -> channels-last out)
-    rten_tensor x = S.x;
-    const bool x_cl = x.strides[1] == 1 && C > 1;
-    const int64_t oshape[4] = {B, O, OH, OW};
-    const int64_t pref[4] = {x_cl ? OH * OW * O : O * OH * OW, x_cl ? 1 : OH * OW, x_cl ? OW * O : OW, x_cl ? O : 1};
     rten_tensor ov;
-    if (S.one_d) {
-        const int64_t os3[3] = {B, O, OW}, pf3[3] = {pref[0], pref[1], pref[3]};
-        RTB_TRY(sc.out(out, RTEN_F32, 3, os3, &ov, out->data ? nullptr : pf3));
-        expand_1d(ov);
-    } else {
-        RTB_TRY(sc.out(out, RTEN_F32, 4, oshape, &ov, out->data ? nullptr : pref));
-    }
+    RTB_TRY(out_like(sc, out, RTEN_F32, S.x, S.one_d, B, O, OH, OW, &ov));
     if (B * O * OH * OW == 0) return RTEN_OK;
     if (S.sy > 256 || S.sx > 256) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "ConvTranspose strides above 256 are not supported");
     if (pw && (pw->kind != 2 || pw->O != O || pw->Cg != Cg || pw->kh != S.kh || pw->kw != S.kw || pw->groups != groups ||
@@ -1192,23 +976,8 @@ rten_status conv_transpose_core(OpScope& sc, const rten_tensor* x_in, const rten
     // ---- the input, shared by every phase: channels-last and 16-byte addressable for the implicit-GEMM path (one
     //      copy when it is not), and in 3xTF32 its low parts, split once
     const bool implicit = (Cg * 4) % 16 == 0 && Cg * 4 >= 32;
-    if (implicit) {
-        const bool direct = x.strides[1] == 1 && (reinterpret_cast<uintptr_t>(x.data) % 16 == 0) && x.strides[3] % 4 == 0 &&
-                            x.strides[2] % 4 == 0 && x.strides[0] % 4 == 0;
-        if (!direct) {
-            void* buf = nullptr;
-            RTB_TRY(temp_alloc(ctx, (size_t)(B * H * W * C) * 4, &buf));
-            long long shape[4] = {B, H, W, C};
-            long long ss[4] = {x.strides[0], x.strides[2], x.strides[3], x.strides[1]};
-            long long ds[4] = {H * W * C, W * C, C, 1};
-            RTB_TRY(launch_nd_copy(ctx, 4, x.data, buf, 4, shape, ss, ds));
-            x.data = buf;
-            x.strides[0] = H * W * C;
-            x.strides[1] = 1;
-            x.strides[2] = W * C;
-            x.strides[3] = C;
-        }
-    }
+    rten_tensor x = S.x;
+    if (implicit) RTB_TRY(nhwc_input(ctx, S.x, &x));
     const float* x_lo = nullptr;
     const bool compact_nhwc = x.strides[1] == 1 && x.strides[3] == C && x.strides[2] == W * C && x.strides[0] == H * W * C;
     if (implicit && ctx->f32_mode == RTEN_F32_TF32X3 && Cg % 32 == 0 && compact_nhwc && !getenv("RTEN_B200_X3_THREE_PLANES")) {
@@ -1542,16 +1311,7 @@ rten_status rten_b200_max_pool(rten_ctx* ctx, const rten_tensor* x, const int32_
     if (st == RTEN_OK) st = axis_out(ctx, xv.shape[3], kernel[1], strides[1], false, pads[1], pads[3], 1, &OW, &p0, &p1);
     if (st == RTEN_OK) {
         const int64_t B = xv.shape[0], C = xv.shape[1];
-        int64_t oshape[4] = {B, C, OH, OW};
-        const bool cl = xv.strides[1] == 1 && C > 1;
-        int64_t pref[4] = {C * OH * OW, OH * OW, OW, 1};
-        if (cl) {
-            pref[0] = OH * OW * C;
-            pref[1] = 1;
-            pref[2] = OW * C;
-            pref[3] = C;
-        }
-        st = sc.out(out, RTEN_F32, 4, oshape, &ov, out->data ? nullptr : pref);
+        st = out_like(sc, out, RTEN_F32, xv, false, B, C, OH, OW, &ov);
         if (st == RTEN_OK) {
             PoolParams p;
             p.B = (int)B;
