@@ -189,7 +189,24 @@ typedef struct {
 rten_status rten_b200_conv2d(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w,
                              const rten_packed* packed_w_or_null, const rten_tensor* bias_or_null,
                              const rten_conv_params* p, rten_tensor* out);
-/* Extension: fused residual add (same shape as out) + activation (see matmul_ex). */
+/* Extension: fused residual add (same shape as out) + activation (see matmul_ex).
+ *
+ * Depthwise convolutions -- the reference's condition (src/ops/conv.rs:248-284): not the pointwise case (1x1, no
+ * padding, strides and dilations 1, groups 1), and in channels == out channels == groups, which includes 1-channel
+ * convolutions with groups 1 -- of conv2d, conv2d_ex, conv_integer and conv_integer_ex (and the separate calls of
+ * conv2d_projected / conv2d_chained and the stride phases of conv_transpose) run on a direct depthwise kernel in ONE
+ * launch over all batches and channels, for x in any strides (NCHW and channels-last without a copy) and w as given or
+ * its rten_b200_prepack_conv_weight(groups = C) handle; zero points are read in place on the device, so a
+ * device-resident call is exactly one launch and can be captured in a CUDA graph.  Its arithmetic is the reference's
+ * depthwise executor's (src/ops/conv/depthwise.rs), per output and in its order:
+ *   f32: bias[c] (or +0.0), then for ky, then kx, ascending, out = out + x * w with the product and the sum each rounded
+ *        (no fused multiply-add) over the taps inside the image only -- padded taps are skipped, not multiplied by 0 --
+ *        then the residual add and activation.  Bit-identical to the reference in both f32 modes (no tensor cores).
+ *   ConvInteger: wrapping i32 sums of (x - x_zero_point) * (w - w_zero_point[c]) over the taps inside the image only, so
+ *        padding acts as x_zero_point.  The GEMM path of other convolutions pads with the reference's literal 0 in the
+ *        shifted-i8 domain (128 for u8 images) instead: a padded depthwise ConvInteger whose x zero point is not 128
+ *        (u8) / 0 (i8) gives the reference's depthwise border values, which that path would not.  The f32 output of
+ *        conv_integer_ex is formed as its GEMM epilogue forms it. */
 rten_status rten_b200_conv2d_ex(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w,
                                 const rten_packed* packed_w_or_null, const rten_tensor* bias_or_null,
                                 const rten_conv_params* p, const rten_tensor* residual_or_null, int activation,
@@ -380,6 +397,12 @@ rten_status rten_b200_softmax(rten_ctx* ctx, const rten_tensor* x, const rten_te
 /* LayerNormalization (src/ops/norm.rs:437-569); epsilon < 0 => default 1e-5. */
 rten_status rten_b200_layer_norm(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* scale,
                                  const rten_tensor* bias_or_null, int axis, float epsilon, rten_tensor* out);
+/* Clip (src/ops/unary_elementwise.rs:249-333), f32 or i32: x.max(min).min(max) with `a > b ? a : b` comparisons, so
+ * NaN becomes min and -0.0 clipped at min = 0 becomes +0.0.  min / max are scalar tensors of x's type (NULL: the type's
+ * finite minimum / maximum), read on the device: no host synchronisation, capturable in a CUDA graph.  `out` may alias
+ * `x`.  One kernel launch for dense device-resident x. */
+rten_status rten_b200_clip(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* min_or_null, const rten_tensor* max_or_null,
+                           rten_tensor* out);
 /* Erf / Gelu (src/ops/unary_elementwise.rs:384-435); approximate != 0 => tanh form. */
 rten_status rten_b200_erf(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
 rten_status rten_b200_gelu(rten_ctx* ctx, const rten_tensor* x, int approximate, rten_tensor* out);

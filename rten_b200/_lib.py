@@ -128,6 +128,7 @@ _SIGNATURES = {
     "rten_b200_comm_uses_peer_memory": (C.c_int, [_vp]),
     "rten_b200_comm_timeouts": (C.c_int, [_vp]),
     "rten_b200_relu": (C.c_int, [_vp, _TP, _TP]),
+    "rten_b200_clip": (C.c_int, [_vp, _TP, _TP, _TP, _TP]),
     "rten_b200_add": (C.c_int, [_vp, _TP, _TP, _TP]),
     "rten_b200_mul": (C.c_int, [_vp, _TP, _TP, _TP]),
     "rten_b200_conv_integer_ex": (C.c_int, [_vp, _TP, _TP, _vp, _TP, _TP, _TP, _TP, C.POINTER(RtenConvParams), _TP, _TP, C.c_int, _TP, _TP]),

@@ -12,6 +12,7 @@
 
 #include "api_shared.h"
 #include "api_util.h"
+#include "depthwise.h"
 #include "rowops.h"
 #include "skinny.h"
 #include "umma_gemm.h"
@@ -122,13 +123,18 @@ rten_status conv_shape(OpScope& sc, const ConvArgs& A, ConvShape& S) {
     return RTEN_OK;
 }
 
+rten_status check_packed(rten_ctx* ctx, const ConvArgs& A, const ConvShape& S) {
+    if (A.pw && (A.pw->kind != 1 || A.pw->O != S.O || A.pw->Cg != S.Cg || A.pw->kh != S.kh || A.pw->kw != S.kw))
+        return fail(ctx, RTEN_ERR_INVALID_VALUE, "prepacked conv weight does not match the kernel shape");
+    return RTEN_OK;
+}
+
 // Weights as [O, kh, kw, C]: the prepacked handle, or packed per call (the reference prepacks per call too)
 rten_status conv_weight(rten_ctx* ctx, const ConvArgs& A, const ConvShape& S, int esize, const void** wp,
                         const int32_t** colsum) {
     *colsum = nullptr;
     if (A.pw) {
-        if (A.pw->kind != 1 || A.pw->O != S.O || A.pw->Cg != S.Cg || A.pw->kh != S.kh || A.pw->kw != S.kw)
-            return fail(ctx, RTEN_ERR_INVALID_VALUE, "prepacked conv weight does not match the kernel shape");
+        RTB_TRY(check_packed(ctx, A, S));
         *wp = A.pw->data;
         *colsum = A.pw->colsum;
         return RTEN_OK;
@@ -287,43 +293,20 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
     if (B * O * OH * OW == 0) return RTEN_OK;
 
     const int esize = A.kind == 0 ? 4 : 1;
+    RTB_TRY(check_packed(ctx, A, S));
 
-    const void* wp = nullptr;
-    const int32_t* w_colsum = nullptr;
-    RTB_TRY(conv_weight(ctx, A, S, esize, &wp, &w_colsum));
-
-    // ---- integer zero points (x_zp scalar, w_zp per output channel)
-    const uint8_t* za8 = nullptr;  // x zero point (GEMM A operand = activations): the 8-bit scalar as it is
-    const int32_t* zb = nullptr;   // w zero points per column
-    int zb_len = 0;
-    int pad_value = 0;
-    bool x_signed = x.dtype == RTEN_I8, w_signed = w.dtype == RTEN_I8;
+    // ---- integer zero points (x_zp scalar, w_zp per output channel), as given
+    const bool x_signed = x.dtype == RTEN_I8, w_signed = w.dtype == RTEN_I8;
+    rten_tensor xz_v{}, wz_v{};
     if (A.kind == 1) {
-        // padded taps: literal 0 in the reference's shifted-i8 domain (rten-gemm/src/im2col.rs:340-358)
-        // == 128 for u8 images, 0 for i8 images
-        pad_value = x_signed ? 0 : 128;
         if (A.x_zp) {
-            rten_tensor z;
-            RTB_TRY(sc.in(A.x_zp, &z));
-            if (numel(&z) != 1) return fail(ctx, RTEN_ERR_INVALID_VALUE, "input zero point must be a scalar");
-            if (z.dtype != x.dtype) return fail(ctx, RTEN_ERR_CAST_FAILED, "zero point type does not match its tensor");
-            za8 = (const uint8_t*)z.data;  // scalar: read in place by the epilogue
-            if (!w_colsum) {
-                int32_t* cs = nullptr;
-                RTB_TRY(temp_alloc(ctx, (size_t)O * 4, (void**)&cs));
-                RTB_TRY(launch_rowsum8(ctx, wp, w_signed, O, (int)(kh * kw * Cg), kh * kw * Cg, cs));
-                w_colsum = cs;
-            }
+            RTB_TRY(sc.in(A.x_zp, &xz_v));
+            if (numel(&xz_v) != 1) return fail(ctx, RTEN_ERR_INVALID_VALUE, "input zero point must be a scalar");
+            if (xz_v.dtype != x.dtype) return fail(ctx, RTEN_ERR_CAST_FAILED, "zero point type does not match its tensor");
         }
         if (A.w_zp) {
             RTB_TRY(check_zero_point(ctx, A.w_zp, O, w.dtype));
-            rten_tensor z;
-            RTB_TRY(sc.in(A.w_zp, &z));
-            zb_len = z.ndim == 0 ? 1 : (int)z.shape[0];
-            int32_t* p = nullptr;
-            RTB_TRY(temp_alloc(ctx, (size_t)zb_len * 4, (void**)&p));
-            RTB_TRY(launch_zp_to_i32(ctx, z.data, w_signed, zb_len, z.ndim == 0 ? 0 : z.strides[0], p));
-            zb = p;
+            RTB_TRY(sc.in(A.w_zp, &wz_v));
         }
     }
     const float *scale_p = nullptr, *scale2_p = nullptr;
@@ -352,6 +335,94 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
         if (one_d) expand_1d(res_v);
         for (int i = 0; i < 4; i++)
             if (res_v.shape[i] != ov.shape[i]) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "residual shape does not match output");
+    }
+
+    // ---- depthwise (the reference's condition, src/ops/conv.rs:248-284: not the pointwise case, then C == O and
+    //      groups == C): one direct launch on x, w (or its pack) and the zero points as they are
+    const bool pointwise_1x1 = kh == 1 && kw == 1 && (pt | pb | pl | pr) == 0 && groups == 1 && strides[0] == 1 &&
+                               strides[1] == 1 && dil[0] == 1 && dil[1] == 1;
+    if (C == O && groups == C && !pointwise_1x1) {
+        DepthwiseParams d;
+        d.x_dtype = x.dtype;
+        d.w_dtype = w.dtype;
+        d.B = (int)B;
+        d.C = (int)C;
+        d.H = (int)H;
+        d.W = (int)W;
+        d.OH = (int)OH;
+        d.OW = (int)OW;
+        d.kh = (int)kh;
+        d.kw = (int)kw;
+        d.sy = (int)strides[0];
+        d.sx = (int)strides[1];
+        d.dy = (int)dil[0];
+        d.dx = (int)dil[1];
+        d.pt = (int)pt;
+        d.pl = (int)pl;
+        d.x = x.data;
+        d.out = ov.data;
+        for (int i = 0; i < 4; i++) {
+            d.xs[i] = x.strides[i];
+            d.os[i] = ov.strides[i];
+        }
+        if (A.pw) {  // [C, kh, kw, 1]
+            d.w = A.pw->data;
+            d.ws_c = kh * kw;
+            d.ws_h = kw;
+            d.ws_w = 1;
+        } else {
+            d.w = w.data;
+            d.ws_c = w.strides[0];
+            d.ws_h = w.strides[2];
+            d.ws_w = w.strides[3];
+        }
+        if (A.bias) {
+            d.bias = (const float*)S.bias_v.data;
+            d.bias_stride = S.bias_v.strides[0];
+        }
+        if (A.residual) {
+            d.res = (const float*)res_v.data;
+            for (int i = 0; i < 4; i++) d.rs[i] = res_v.strides[i];
+        }
+        d.act = A.act;
+        if (A.kind == 1) {
+            d.x_zp = A.x_zp ? xz_v.data : nullptr;
+            d.w_zp = A.w_zp ? wz_v.data : nullptr;
+            d.w_zp_stride = (A.w_zp && wz_v.ndim == 1) ? wz_v.strides[0] : 0;
+            d.scale = scale_p;
+            d.scale_b = scale2_p;
+            d.range = range_p;
+        }
+        return launch_depthwise(ctx, d);
+    }
+
+    const void* wp = nullptr;
+    const int32_t* w_colsum = nullptr;
+    RTB_TRY(conv_weight(ctx, A, S, esize, &wp, &w_colsum));
+    const uint8_t* za8 = nullptr;  // x zero point (GEMM A operand = activations): the 8-bit scalar as it is
+    const int32_t* zb = nullptr;   // w zero points per column
+    int zb_len = 0;
+    int pad_value = 0;
+    if (A.kind == 1) {
+        // padded taps: literal 0 in the reference's shifted-i8 domain (rten-gemm/src/im2col.rs:340-358)
+        // == 128 for u8 images, 0 for i8 images
+        pad_value = x_signed ? 0 : 128;
+        if (A.x_zp) {
+            za8 = (const uint8_t*)xz_v.data;  // scalar: read in place by the epilogue
+            if (!w_colsum) {
+                int32_t* cs = nullptr;
+                RTB_TRY(temp_alloc(ctx, (size_t)O * 4, (void**)&cs));
+                RTB_TRY(launch_rowsum8(ctx, wp, w_signed, O, (int)(kh * kw * Cg), kh * kw * Cg, cs));
+                w_colsum = cs;
+            }
+        }
+        if (A.w_zp) {
+            zb_len = wz_v.ndim == 0 ? 1 : (int)wz_v.shape[0];
+            int32_t* p = nullptr;
+            RTB_TRY(temp_alloc(ctx, (size_t)zb_len * 4, (void**)&p));
+            RTB_TRY(launch_zp_to_i32(ctx, wz_v.data, w_signed, zb_len, wz_v.ndim == 0 ? 0 : wz_v.strides[0], p));
+            zb = p;
+        }
     }
 
     // ---- choose the addressing path

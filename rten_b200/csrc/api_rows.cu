@@ -217,32 +217,32 @@ rten_status rten_b200_layer_norm(rten_ctx* ctx, const rten_tensor* x, const rten
 }
 
 // ---- unary elementwise ----------------------------------------------------------------------------
-static rten_status unary_op(rten_ctx* ctx, int op, const rten_tensor* x, rten_tensor* out) {
-    RTB_TRY(check_ctx(ctx));
-    if (!x || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
-    if (x->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
-    OpScope sc(ctx);
+// out = f(x) elementwise for a 4-byte element type, `flat(in, out, n)` launching f over n contiguous elements.  Dense
+// (any dim order) tensors are processed in memory order: the output takes the input's strides.
+extern "C++" {
+template <class Flat>
+rten_status elementwise_op(OpScope& sc, const rten_tensor* x, rten_tensor* out, Flat flat) {
+    rten_ctx* ctx = sc.ctx;
     rten_tensor xv, ov;
     rten_status st = sc.in(x, &xv);
-    // dense (any dim order) tensors are processed in memory order: output takes the input's strides
     bool dense = false;
     if (st == RTEN_OK) dense = span_elems(&xv) == numel(&xv);
-    if (st == RTEN_OK) st = sc.out(out, RTEN_F32, xv.ndim, xv.shape, &ov, (out->data == nullptr && dense) ? xv.strides : nullptr);
+    if (st == RTEN_OK) st = sc.out(out, xv.dtype, xv.ndim, xv.shape, &ov, (out->data == nullptr && dense) ? xv.strides : nullptr);
     if (st == RTEN_OK && numel(&xv) > 0) {
         bool same_layout = dense;
         for (int i = 0; i < xv.ndim && same_layout; i++)
             if (xv.shape[i] != 1 && xv.strides[i] != ov.strides[i]) same_layout = false;
         if (same_layout) {
-            st = launch_unary(ctx, op, (const float*)xv.data, (float*)ov.data, numel(&xv));
+            st = flat(xv.data, ov.data, numel(&xv));
         } else {
             rten_tensor xc;
             st = sc.contiguous(&xv, &xc);
             if (st == RTEN_OK && is_contiguous(&ov)) {
-                st = launch_unary(ctx, op, (const float*)xc.data, (float*)ov.data, numel(&xv));
+                st = flat(xc.data, ov.data, numel(&xv));
             } else if (st == RTEN_OK) {
                 void* t = nullptr;
                 st = temp_alloc(ctx, (size_t)numel(&xv) * 4, &t);
-                if (st == RTEN_OK) st = launch_unary(ctx, op, (const float*)xc.data, (float*)t, numel(&xv));
+                if (st == RTEN_OK) st = flat(xc.data, t, numel(&xv));
                 if (st == RTEN_OK) {
                     long long shape[RTEN_MAX_DIMS], ss[RTEN_MAX_DIMS], ds[RTEN_MAX_DIMS];
                     for (int i = 0; i < xv.ndim; i++) {
@@ -255,6 +255,36 @@ static rten_status unary_op(rten_ctx* ctx, int op, const rten_tensor* x, rten_te
             }
         }
     }
+    return st;
+}
+}  // extern "C++"
+
+static rten_status unary_op(rten_ctx* ctx, int op, const rten_tensor* x, rten_tensor* out) {
+    RTB_TRY(check_ctx(ctx));
+    if (!x || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    if (x->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    OpScope sc(ctx);
+    return sc.finish(elementwise_op(sc, x, out, [&](const void* a, void* y, long long n) {
+        return launch_unary(ctx, op, (const float*)a, (float*)y, n);
+    }));
+}
+
+rten_status rten_b200_clip(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* min, const rten_tensor* max, rten_tensor* out) {
+    RTB_TRY(check_ctx(ctx));
+    if (!x || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    if (x->dtype != RTEN_F32 && x->dtype != RTEN_I32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    for (const rten_tensor* b : {min, max})
+        if (b && (b->dtype != x->dtype || numel(b) != 1))
+            return fail(ctx, RTEN_ERR_INVALID_VALUE, "min and max must be scalars of the input's type");
+    OpScope sc(ctx);
+    rten_tensor mn, mx;  // (read on the device by the kernel: no host synchronisation)
+    rten_status st = RTEN_OK;
+    if (min) st = sc.in(min, &mn);
+    if (st == RTEN_OK && max) st = sc.in(max, &mx);
+    if (st == RTEN_OK)
+        st = elementwise_op(sc, x, out, [&](const void* a, void* y, long long n) {
+            return launch_clip(ctx, x->dtype == RTEN_I32, a, y, n, min ? mn.data : nullptr, max ? mx.data : nullptr);
+        });
     return sc.finish(st);
 }
 

@@ -8,7 +8,7 @@
 //          returned to the context pool after their last consumer (src/graph.rs:1100-1180); an operator that can run in
 //          place does so when the executor holds the last reference to its input (src/graph.rs:973-1049); shape-only
 //          operators (Reshape, Flatten, Squeeze, Unsqueeze, Transpose, Identity) are views -- no kernel, no copy.
-// Operators: Conv, ConvInteger, ConvTranspose (without output_shape), Relu, MaxPool, GlobalAveragePool, ReduceMean, Gemm, MatMul, MatMulInteger, MatMulNBits
+// Operators: Conv, ConvInteger, ConvTranspose (without output_shape), Relu, Clip, MaxPool, GlobalAveragePool, ReduceMean, Gemm, MatMul, MatMulInteger, MatMulNBits
 // (com.microsoft), Add, Mul, Softmax, LayerNormalization, Gelu, Erf, Gather, Cast, DynamicQuantizeLinear, Attention,
 // RotaryEmbedding, GroupQueryAttention (com.microsoft, three outputs), Constant and the view operators.
 #include <cuda_runtime.h>
@@ -151,7 +151,7 @@ rten_status upload_constant(rten_model* m, const onnx::Tensor& t, ValueSlot* v) 
 
 const std::set<std::string>& supported_ops() {
     static const std::set<std::string> s = {
-        "Conv", "ConvTranspose", "Relu", "MaxPool", "GlobalAveragePool", "ReduceMean", "Reshape", "Flatten", "Squeeze", "Unsqueeze", "Transpose",
+        "Conv", "ConvTranspose", "Relu", "Clip", "MaxPool", "GlobalAveragePool", "ReduceMean", "Reshape", "Flatten", "Squeeze", "Unsqueeze", "Transpose",
         "Identity", "Gemm", "MatMul", "Add", "Mul", "Softmax", "LayerNormalization", "Gelu", "Erf", "Gather",
         "DynamicQuantizeLinear", "MatMulInteger", "ConvInteger", "Cast", "Attention", "MatMulNBits", "GroupQueryAttention",
         "RotaryEmbedding", "Constant"};
@@ -161,7 +161,9 @@ const std::set<std::string>& supported_ops() {
 bool is_view_op(const std::string& op) {
     return op == "Reshape" || op == "Flatten" || op == "Squeeze" || op == "Unsqueeze" || op == "Transpose" || op == "Identity";
 }
-bool is_in_place_op(const std::string& op) { return op == "Relu" || op == "Gelu" || op == "Erf" || op == "Softmax"; }
+bool is_in_place_op(const std::string& op) {
+    return op == "Relu" || op == "Clip" || op == "Gelu" || op == "Erf" || op == "Softmax";
+}
 
 rten_status fill_conv_params(rten_ctx* ctx, const onnx::Node& n, rten_conv_params* p) {
     memset(p, 0, sizeof(*p));
@@ -298,7 +300,26 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
             return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "unsupported operator com.microsoft.RotaryEmbedding");
         OpNode on;
         on.n = n;
-        for (const std::string& s : n.inputs) {
+        if (n.op_type == "Clip") {
+            // legacy (opset < 11) min / max attributes become constant inputs 1 / 2, as the reference's reader does
+            // (src/op_registry/onnx_registry.rs:887-898)
+            const char* names[2] = {"min", "max"};
+            for (int k = 0; k < 2; k++) {
+                const onnx::Attribute* a = n.attr(names[k]);
+                if (!a) continue;
+                onnx::Tensor t;
+                t.name = n.name + "/" + (n.outputs.empty() ? std::string() : n.outputs[0]) + "/clip_" + names[k];
+                t.data_type = onnx::DT_FLOAT;
+                const float v = a->f;
+                t.data.resize(4);
+                memcpy(t.data.data(), &v, 4);
+                const int id = m->value_id(t.name);
+                RTB_TRY(upload_constant(m.get(), t, &m->values[(size_t)id]));
+                if (on.n.inputs.size() < (size_t)k + 2) on.n.inputs.resize((size_t)k + 2);
+                on.n.inputs[(size_t)k + 1] = t.name;
+            }
+        }
+        for (const std::string& s : on.n.inputs) {
             const int id = m->value_id(s);
             if (id >= 0 && m->values[(size_t)id].kind == V_UNSET)
                 return mfail(ctx, RTEN_ERR_INVALID_VALUE, "node '" + n.name + "' (" + n.op_type + ") reads '" + s + "' before it is produced");
@@ -600,6 +621,8 @@ struct Runner {
             st = rten_b200_conv_transpose(ctx, T(0), T(1), o.packed, T(2), &p, &y);
         } else if (op == "Relu") {
             st = rten_b200_relu(ctx, T(0), &y);
+        } else if (op == "Clip") {
+            st = rten_b200_clip(ctx, T(0), T(1), T(2), &y);
         } else if (op == "Gelu") {
             const onnx::Attribute* a = o.n.attr("approximate");
             st = rten_b200_gelu(ctx, T(0), (a && a->s == "tanh") ? 1 : 0, &y);

@@ -9,6 +9,7 @@
 #include <cuda_runtime.h>
 
 #include <cfloat>
+#include <climits>
 #include <cstdint>
 #include <cstdlib>
 
@@ -1670,6 +1671,34 @@ __global__ void __launch_bounds__(256) conv_transpose_fill_kernel(float* __restr
         if (((p.live_y[qy >> 5] >> (qy & 31)) & 1u) && ((p.live_x[qx >> 5] >> (qx & 31)) & 1u)) continue;
         out[r * p.s_b + (long long)o * p.s_o + (long long)y * p.s_h + (long long)x * p.s_w] = bias ? bias[o] : 0.0f;
     }
+}
+
+// Clip (src/ops/unary_elementwise.rs:249-309): x.max(min).min(max) with the reference's `a > b ? a : b` / `a < b ? a :
+// b`, so NaN becomes min and -0.0 clipped at min = +0.0 becomes +0.0.  Bounds are device scalars (null: the type's
+// finite extreme), read by the kernel.
+template <typename T>
+__global__ void __launch_bounds__(256) clip_kernel(const T* x, T* y, long long n, const T* mn,
+                                                   const T* mx, T lo_default, T hi_default) {
+    const T lo = mn ? *mn : lo_default, hi = mx ? *mx : hi_default;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        T v = x[i];
+        v = v > lo ? v : lo;
+        y[i] = v < hi ? v : hi;
+    }
+}
+
+rten_status launch_clip(rten_ctx* ctx, int is_i32, const void* x, void* y, long long n, const void* mn, const void* mx) {
+    if (n == 0) return RTEN_OK;
+    if (is_i32)
+        clip_kernel<int><<<ew_grid(ctx, n), 256, 0, ctx->stream>>>((const int*)x, (int*)y, n, (const int*)mn, (const int*)mx,
+                                                                   INT_MIN, INT_MAX);
+    else
+        clip_kernel<float><<<ew_grid(ctx, n), 256, 0, ctx->stream>>>((const float*)x, (float*)y, n, (const float*)mn,
+                                                                     (const float*)mx, -FLT_MAX, FLT_MAX);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail_cuda(ctx, e, "clip launch");
+    count_launch(ctx);
+    return RTEN_OK;
 }
 
 rten_status launch_conv_transpose_fill(rten_ctx* ctx, float* out, const float* bias, const ConvTransposeFill& p) {

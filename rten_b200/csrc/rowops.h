@@ -24,6 +24,8 @@ rten_status launch_layer_norm(rten_ctx* ctx, const float* x, float* y, long long
 rten_status launch_row_mean(rten_ctx* ctx, const float* x, float* y, long long rows, int n, long long rows_inner,
                             long long s_outer, long long s_inner, long long kstride);
 rten_status launch_unary(rten_ctx* ctx, int op, const float* x, float* y, long long n);
+// Clip of n contiguous f32 (or i32) elements; y may be x; mn / mx: device scalars of the same type, or null
+rten_status launch_clip(rten_ctx* ctx, int is_i32, const void* x, void* y, long long n, const void* mn, const void* mx);
 rten_status launch_nd_copy(rten_ctx* ctx, int esize, const void* src, void* dst, int ndim, const long long* shape,
                            const long long* sstride, const long long* dstride);
 rten_status launch_nd_add(rten_ctx* ctx, const float* a, const float* b, float* d, int ndim, const long long* shape,

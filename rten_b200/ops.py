@@ -731,6 +731,18 @@ class Relu(_Unary):
         return ctx.lib.rten_b200_relu(ctx.handle, x, o)
 
 
+class Clip:
+    """src/ops/unary_elementwise.rs:249-333: x.max(min).min(max), f32 or i32; `min` / `max` are scalars of x's type (or
+    None: the type's finite extreme), read on the device.  `in_place` = run_in_place on input 0."""
+
+    def run(self, ctx, x, min=None, max=None, in_place=False, out=None):
+        A = _Args(ctx)
+        into = x if (in_place and isinstance(x, DeviceTensor)) else out
+        o = A.out(into)
+        ctx.check(ctx.lib.rten_b200_clip(ctx.handle, A.t(x), A.t(min), A.t(max), C.byref(o)))
+        return A.wrap(o, into)
+
+
 class DynamicQuantizeLinear:
     """src/ops/quantize.rs:436-468 -> (y u8, y_scale f32 scalar, y_zero_point u8 scalar)"""
 
