@@ -211,6 +211,7 @@ struct PlanShape {
 // launches that take the plain f32 epilogue (umma_wide_kernel).  One 128-byte K block per pipeline stage.
 static bool plan_shape(const Prepared& q, const Plan& pl, PlanShape& ps) {
     const KParams& p = q.p;
+    if (pl.splitk < 1) return false;  // (recorded plans are read from a text file: no division by zero, no negative units)
     if (is_wide(pl.bn)) {
         if ((pl.bn != 128 && pl.bn != 256) || !q.wide || pl.splitk != 1) return false;
         if (pl.bn == 256 && q.p.epi.act > 1) return false;  // Gelu: 128-column tiles only (umma_wide_kernel)

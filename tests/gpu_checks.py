@@ -1411,11 +1411,34 @@ def _kernels_launched(fn):
     return out, names
 
 
+def _launch_lines(fn):
+    """Run `fn` under RTEN_B200_VERBOSE with file descriptor 2 sent to a temporary file: (its result, the launch lines
+    the library printed)."""
+    import sys
+    import tempfile
+    sys.stderr.flush()
+    saved = os.dup(2)
+    with tempfile.TemporaryFile() as f:
+        os.dup2(f.fileno(), 2)
+        os.environ["RTEN_B200_VERBOSE"] = "1"
+        try:
+            out = fn()
+        finally:
+            os.environ.pop("RTEN_B200_VERBOSE", None)
+            os.dup2(saved, 2)
+            os.close(saved)
+        f.seek(0)
+        return out, f.read().decode(errors="replace")
+
+
 def check_halo_conv(rt, oracle):
     """Stride-1 windows on the halo-reuse kernel (one activation patch per channel block in shared memory, the filter taps
-    as shifted matrix descriptors): ResNet-50's 3x3 layer shapes at several batch sizes (row strips, whole images, several
-    images per unit, batch tails), 5x5 / 1x3 / 3x1 windows, asymmetric padding, both f32 modes; against float64 within the
-    TF32 bound, and the generic implicit-GEMM kernel must agree within the same bound."""
+    as shifted matrix descriptors): ResNet-50's 3x3 layer shapes at several batch sizes (row strips, whole images, batch
+    tails), 5x5 / 1x3 / 3x1 windows, asymmetric padding; against float64 within the TF32 bound, each case's launch line
+    showing the halo kernel ran, and the generic implicit-GEMM kernel must agree within the same bound.  (Every case here
+    comes out at one image per unit; tests/test_gpu_plan_space.py pins units of several.)  The same cases in 3xTF32 run
+    on the generic kernel, which is asserted too: the split operands carry a second A plane (x3_cb), which the halo
+    kernel does not take."""
     import os
     os.environ["RTEN_B200_HALO"] = "1"  # the kernel is opt-in (the generic kernel stays the default)
     try:
@@ -1440,7 +1463,12 @@ def _check_halo_conv(rt, oracle):
         try:
             for xs, ws, pads in cases:
                 for act in (0, 1):
-                    worst = max(worst, _conv_case(rt, oracle, ctx, xs, ws, pads=pads, cl=True, prepack=True, act=act))
+                    w, log = _launch_lines(lambda: _conv_case(rt, oracle, ctx, xs, ws, pads=pads, cl=True, prepack=True, act=act))
+                    kernel = "umma_halo" if tf32 else "umma_gemm"
+                    other = "umma_gemm" if tf32 else "umma_halo"
+                    assert f"[{kernel}]" in log and f"[{other}]" not in log, \
+                        f"Conv x{xs} w{ws} pads={pads} {'tf32' if tf32 else 'tf32x3'}: expected the {kernel} kernel, printed: {log.strip()}"
+                    worst = max(worst, w)
                     n += 1
         finally:
             TF32_REL = saved
@@ -1461,7 +1489,7 @@ def _check_halo_conv(rt, oracle):
     exact, absum = _conv_exact(x, w, b, (1, 1, 1, 1), 1, (1, 1), (1, 1))
     assert_tf32_close(halo, np.maximum(exact, 0), absum, "halo kernel")
     assert_tf32_close(generic, np.maximum(exact, 0), absum, "generic kernel")
-    return f"{n} cases, worst err/bound {worst:.3f}; halo vs generic max |d| {float(np.abs(halo - generic).max()):.2e}"
+    return f"{n} cases (tf32 on the halo kernel, tf32x3 on the generic one), worst err/bound {worst:.3f}; halo vs generic max |d| {float(np.abs(halo - generic).max()):.2e}"
 
 
 # ------------------------------------------------------------------------------------------
