@@ -389,6 +389,48 @@ rten_status rten_b200_group_query_attention(rten_ctx* ctx, const rten_tensor* qu
                                             const rten_tensor* attention_bias_or_null, const rten_gqa_params* params,
                                             rten_tensor* out, rten_tensor* present_key, rten_tensor* present_value);
 
+/* MultiHeadAttention (com.microsoft; src/ops/attention/contrib.rs:56-300): the attention of ONNX Runtime's optimized
+ * encoder and encoder-decoder exports.  query [B, S, H * D], or packed QKV [B, S, H, 3, D] (key, value and bias NULL);
+ * key [B, L, H * D] and value [B, L, H * Dv] (key NULL: key = value = query, a given value is ignored); bias
+ * [2 H D + H Dv], its three slices added to q, k and v (one rounded f32 add each) before the heads are split;
+ * key_padding_mask i32 [B, P + L]; attention_bias f32 broadcastable to [B, H, S, P + L] (any dimension may be 1,
+ * the key dimension included); past_key / past_value [B, H, P, D].  Outputs: out [B, S, H * Dv] and, when not NULL,
+ * present_key / present_value [B, H, P + L, D] = concat(past, new k / v).
+ * scores = scale q k^T (scale <= 0: 1 / sqrt(D)), then in this order: + attention_bias; with unidirectional, keys
+ * t > P + s REPLACED by mask_filter_value; keys with key_padding_mask[b, t] == 0 REPLACED by mask_filter_value;
+ * softmax with NaN flushed to 0; times v.  A finite mask_filter_value keeps masked keys in the softmax: a row whose
+ * keys are all masked is the mean of v over all keys.
+ * past_sequence_length and cache_indirection (inputs 8 and 9) fail with the reference's errors, as does every shape
+ * error it raises, with its messages.
+ * In-place present caches as for GroupQueryAttention: present_key / present_value whose data pointer and strides equal
+ * past_key's / past_value's (the past buffer with room for L more positions) receive only the new positions; positions
+ * beyond P + L stay untouched.  A present cache overlapping a past cache without being that buffer fails with
+ * RTEN_ERR_UNSUPPORTED_OUTPUT.  Host-resident tensors are staged; nothing is read back to the host, so a
+ * device-resident call can be captured in a CUDA graph.
+ * Paths (head size 64 or 128 with Dv == D; device-resident tensors with 16-byte aligned rows):
+ *  - prep, when there is a bias, a past cache or a present output: ONE launch of the rotary / append kernel adds the
+ *    bias to q (into a scratch buffer), writes k' and v' into the present caches (or scratch caches when a present
+ *    output is not requested) and copies the past prefix unless the caches are in place.
+ *  - S == 1: the single-query attention kernel (caches up to 8192 positions; longer ones take the prefill kernel).
+ *  - S >= 2: the streaming prefill attention kernel, products in the context's f32 mode.  q / k / v are read in place
+ *    through strided views when there is no prep, and out is written in place.  Key tiles above every row's causal
+ *    diagonal are skipped and added back as masked keys; their values are read only when their weight is not 0.
+ *  Launches: one without prep, two with it.
+ * Other head sizes and Dv != D fail with RTEN_ERR_UNSUPPORTED_VALUE; there is no composed fallback. */
+typedef struct {
+    int32_t num_heads;
+    float scale;             /* <= 0: 1 / sqrt(head size) */
+    float mask_filter_value; /* the score of a masked key (the reference's default: -10000) */
+    int32_t unidirectional;
+} rten_mha_params;
+rten_status rten_b200_multi_head_attention(rten_ctx* ctx, const rten_tensor* query, const rten_tensor* key_or_null,
+                                           const rten_tensor* value_or_null, const rten_tensor* bias_or_null,
+                                           const rten_tensor* key_padding_mask_or_null, const rten_tensor* attention_bias_or_null,
+                                           const rten_tensor* past_key_or_null, const rten_tensor* past_value_or_null,
+                                           const rten_tensor* past_sequence_length_or_null, const rten_tensor* cache_indirection_or_null,
+                                           const rten_mha_params* params, rten_tensor* out, rten_tensor* present_key_or_null,
+                                           rten_tensor* present_value_or_null);
+
 /* Softmax (src/ops/norm.rs:825-899) and AddSoftmax (src/ops/attention.rs:30-165) when mask != NULL
  * (mask broadcast to x, added lane-wise before the softmax over `axis`; AddSoftmax uses axis -1).
  * `out` may alias `x` (= run_in_place). */
@@ -466,7 +508,8 @@ rten_status rten_b200_scatter_rows(rten_ctx* ctx, rten_tensor* table, const rten
  * DynamicQuantizeLinear, Attention (4-D), MatMulNBits (com.microsoft, bits 4; constant B / scales used in place),
  * RotaryEmbedding, GroupQueryAttention (com.microsoft; output and present_key / present_value, inputs 12-15 rejected;
  * the executor allocates new present caches, so each decode step also copies the past: two launches, not one),
- * Constant and the view operators; anything else fails the LOAD with
+ * MultiHeadAttention (com.microsoft; outputs 0-2; a missing num_heads, an explicit scale <= 0, inputs 8 / 9 and the
+ * qk output 3 fail the load; the executor allocates new present caches), Constant and the view operators; anything else fails the LOAD with
  * RTEN_ERR_UNSUPPORTED_VALUE ("unsupported operator <name>"). */
 typedef struct rten_model rten_model;
 rten_status rten_b200_model_load(rten_ctx* ctx, const void* onnx_bytes, size_t len, rten_model** out);

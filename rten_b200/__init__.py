@@ -7,5 +7,5 @@ from . import _lib  # noqa: F401
 from .ops import (  # noqa: F401
     ACT_GELU, ACT_GELU_TANH, ACT_NONE, ACT_RELU, Add, AddSoftmax, Attention, Clip, Comm, Context, Conv, ConvInteger, ConvIntegerToFloat,
     ConvTranspose, DeviceTensor, DynamicQuantizeLinear, Erf, FusedMatMul, GatherRows, Gelu, Gemm, GlobalAveragePool, GroupQueryAttention,
-    LayerNormalization, MatMul, MatMulInteger, MatMulIntegerToFloat, MatMulNBits, MaxPool, Mul, OpError, Packed, QuantizedLinear, Relu, RotaryEmbedding, ScatterRows, Softmax, from_torch,
+    LayerNormalization, MatMul, MatMulInteger, MatMulIntegerToFloat, MatMulNBits, MaxPool, Mul, MultiHeadAttention, OpError, Packed, QuantizedLinear, Relu, RotaryEmbedding, ScatterRows, Softmax, from_torch,
 )

@@ -69,6 +69,10 @@ class RtenGqaParams(C.Structure):
                 ("rotary_interleaved", C.c_int32), ("local_window_size", C.c_int32), ("softcap", C.c_float)]
 
 
+class RtenMhaParams(C.Structure):
+    _fields_ = [("num_heads", C.c_int32), ("scale", C.c_float), ("mask_filter_value", C.c_float), ("unidirectional", C.c_int32)]
+
+
 _TP = C.POINTER(RtenTensor)
 _vp = C.c_void_p
 
@@ -117,6 +121,8 @@ _SIGNATURES = {
     "rten_b200_rotary_embedding": (C.c_int, [_vp, _TP, _TP, _TP, _TP, C.c_int, C.c_int, C.c_int, _TP]),
     "rten_b200_group_query_attention": (C.c_int, [_vp, _TP, _TP, _TP, _TP, _TP, _TP, _TP, _TP, _TP, _TP, _TP,
                                                   C.POINTER(RtenGqaParams), _TP, _TP, _TP]),
+    "rten_b200_multi_head_attention": (C.c_int, [_vp, _TP, _TP, _TP, _TP, _TP, _TP, _TP, _TP, _TP, _TP,
+                                                 C.POINTER(RtenMhaParams), _TP, _TP, _TP]),
     "rten_b200_softmax": (C.c_int, [_vp, _TP, _TP, C.c_int, C.c_int, _TP]),
     "rten_b200_layer_norm": (C.c_int, [_vp, _TP, _TP, _TP, C.c_int, C.c_float, _TP]),
     "rten_b200_erf": (C.c_int, [_vp, _TP, _TP]),

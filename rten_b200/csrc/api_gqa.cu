@@ -1,7 +1,9 @@
-// Entry points of the C ABI for rotary-embedded grouped-query attention (include/rten_b200.h):
+// Entry points of the C ABI for rotary-embedded grouped-query attention and multi-head attention (include/rten_b200.h):
 //   rten_b200_rotary_embedding        : ai.onnx RotaryEmbedding (src/ops/embedding.rs:46-252)
 //   rten_b200_group_query_attention   : com.microsoft GroupQueryAttention (src/ops/attention/contrib.rs:369-417,
 //                                       :438-810), the attention operator of quantized decoder-only LLM exports
+//   rten_b200_multi_head_attention    : com.microsoft MultiHeadAttention (src/ops/attention/contrib.rs:56-300), the
+//                                       attention of ONNX Runtime's optimized encoder and encoder-decoder exports
 // Validation restates the reference's checks and messages on everything the host can see.  The work runs on three
 // kernels: the rotary / cache-append kernel (rotary.cu), the single-query attention kernel for a decode step
 // (skinny.cu, with the rotary embedding, cache append and sliding window fused in) and the streaming prefill kernel
@@ -548,6 +550,327 @@ rten_status rten_b200_group_query_attention(rten_ctx* ctx, const rten_tensor* qu
         return sc.finish(fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "GroupQueryAttention: the present caches and the output need 16-byte aligned rows"));
     if (build) st = launch_rotary(ctx, Rb);
     if (st == RTEN_OK) st = launch_rotary(ctx, R);
+    if (st == RTEN_OK) st = launch_attn_prefill(ctx, A);
+    return sc.finish(st);
+}
+
+rten_status rten_b200_multi_head_attention(rten_ctx* ctx, const rten_tensor* query, const rten_tensor* key, const rten_tensor* value,
+                                           const rten_tensor* bias, const rten_tensor* key_padding_mask, const rten_tensor* attention_bias,
+                                           const rten_tensor* past_key, const rten_tensor* past_value, const rten_tensor* past_sequence_length,
+                                           const rten_tensor* cache_indirection, const rten_mha_params* prm, rten_tensor* out,
+                                           rten_tensor* present_key, rten_tensor* present_value) {
+    if (!ctx) return RTEN_ERR_INVALID_VALUE;
+    if (!query || !prm || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    for (const rten_tensor* t : {query, key, value, bias, attention_bias, past_key, past_value})
+        if (t && t->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    for (const rten_tensor* t : {key_padding_mask, past_sequence_length, cache_indirection})
+        if (t && t->dtype != RTEN_I32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    // inputs as the reference reads them: past caches (in `run`), query, then inputs 1-5, 8, 9 (in `run_impl`)
+    if (past_key && past_key->ndim != 4) return rank_fail(ctx, 6, 4, past_key->ndim);
+    if (past_value && past_value->ndim != 4) return rank_fail(ctx, 7, 4, past_value->ndim);
+    if (query->ndim != 3 && query->ndim != 5) return fail(ctx, RTEN_ERR_INVALID_VALUE, "query must have 3 or 5 dims");
+    {
+        const rten_tensor* ts[] = {key, value, bias, key_padding_mask, attention_bias};
+        const int rank[] = {3, 3, 1, 2, 4};
+        for (int i = 0; i < 5; i++)
+            if (ts[i] && ts[i]->ndim != rank[i]) return rank_fail(ctx, i + 1, rank[i], ts[i]->ndim);
+    }
+    if (past_sequence_length) {
+        if (past_sequence_length->ndim != 0) return rank_fail(ctx, 8, 0, past_sequence_length->ndim);
+        return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "past_seq_len is not supported");
+    }
+    if (cache_indirection) {
+        if (cache_indirection->ndim != 3) return rank_fail(ctx, 9, 3, cache_indirection->ndim);
+        return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "cache_indirection is not supported");
+    }
+    const int64_t H = prm->num_heads;
+    if (H <= 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "num_heads must be positive");
+    const bool packed = query->ndim == 5;
+    const int64_t B = query->shape[0], S = query->shape[1];
+    int64_t D, Dv, L, hidden = 0;
+    if (packed) {  // [B, S, H, 3, D]
+        if (key) return fail(ctx, RTEN_ERR_INVALID_VALUE, "key must be None when query is packed");
+        if (value) return fail(ctx, RTEN_ERR_INVALID_VALUE, "value must be None when query is packed");
+        if (bias) return fail(ctx, RTEN_ERR_INVALID_VALUE, "bias is not supported with packed QKV format");
+        if (query->shape[3] != 3) return fail(ctx, RTEN_ERR_INVALID_VALUE, "4th dimension of packed qkv input must be 3");
+        if (query->shape[2] != H)
+            return fail(ctx, RTEN_ERR_INVALID_VALUE, "2nd dimension of packed qkv input must be equal to number of attention heads");
+        D = Dv = query->shape[4];
+        L = S;
+    } else {
+        hidden = query->shape[2];
+        if (hidden % H) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Hidden size must be divisible by number of attention heads");
+        D = hidden / H;
+        if (key && !value) return fail(ctx, RTEN_ERR_INVALID_VALUE, "value input must be set if key input is present");
+        const rten_tensor* k = key ? key : query;  // (no key: key = value = query, a given value is ignored)
+        const rten_tensor* v = key ? value : query;
+        if (k->shape[0] != B || v->shape[0] != B || v->shape[1] != k->shape[1])
+            return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Key and value batch or sequence lengths do not match");
+        if (k->shape[2] != hidden) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Key hidden size does not match query hidden size");
+        if (v->shape[2] % H) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Value hidden size must be divisible by number of attention heads");
+        Dv = v->shape[2] / H;
+        L = k->shape[1];
+        if (bias && bias->shape[0] != 2 * hidden + v->shape[2])
+            return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Bias shape does not match QKV hidden sizes");
+    }
+    int64_t P = 0;
+    if (past_key && past_value) {
+        const int64_t* a = past_key->shape;
+        const int64_t* v = past_value->shape;
+        if (a[0] != B || v[0] != B || a[1] != H || v[1] != H || a[3] != D || v[3] != Dv || a[2] != v[2])
+            return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "past_key/past_value shape does not match key/value shape");
+        P = a[2];
+    } else if (past_key || past_value) {
+        return fail(ctx, RTEN_ERR_INVALID_VALUE, "past_key and past_value must either both be present or both be absent");
+    }
+    const int64_t T = P + L;
+    if (attention_bias) {
+        const int64_t target[4] = {B, H, S, T};
+        for (int i = 0; i < 4; i++)
+            if (attention_bias->shape[i] != target[i] && attention_bias->shape[i] != 1)
+                return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Cannot broadcast inputs");
+    }
+    if (key_padding_mask && (key_padding_mask->shape[0] != B || key_padding_mask->shape[1] != T))
+        return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "key_padding_mask shape does not match key sequence length");
+    if (D != 64 && D != 128) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MultiHeadAttention: the head size must be 64 or 128");
+    if (Dv != D) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MultiHeadAttention: the value head size must equal the head size");
+    if (T == 0 && B * S > 0) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MultiHeadAttention: there must be at least one key position");
+    const float scale = prm->scale > 0.0f ? prm->scale : 1.0f / std::sqrt((float)D);
+
+    // ---- present caches: the past buffer itself (in place), new memory, or refused when they overlap a past cache
+    auto aliased = [&](const rten_tensor* pres, const rten_tensor* past) {
+        if (!pres || !past || !pres->data || pres->data != past->data || pres->device < 0 || past->device < 0 || pres->ndim != 4) return false;
+        for (int i = 0; i < 4; i++)
+            if (pres->strides[i] != past->strides[i]) return false;
+        return true;
+    };
+    const bool alias_k = aliased(present_key, past_key), alias_v = aliased(present_value, past_value);
+    for (const rten_tensor* pres : {present_key, present_value})
+        for (const rten_tensor* past : {past_key, past_value}) {
+            if (!pres || !past || !pres->data || pres->device < 0 || past->device < 0 || aliased(pres, past)) continue;
+            uintptr_t a0, a1, b0, b1;
+            rten_tensor pshape = *pres;
+            pshape.ndim = 4;
+            pshape.shape[0] = B;
+            pshape.shape[1] = H;
+            pshape.shape[2] = T;
+            pshape.shape[3] = D;
+            byte_span(&pshape, &a0, &a1);
+            byte_span(past, &b0, &b1);
+            if (a0 < b1 && b0 < a1)
+                return fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT,
+                            "MultiHeadAttention: present_key / present_value overlap a past cache without being that buffer (same data and strides)");
+        }
+
+    // ---- device views (head dimension contiguous)
+    OpScope sc(ctx);
+    auto view = [&](const rten_tensor* t, rten_tensor* v) {
+        rten_status s = sc.in(t, v);
+        if (s == RTEN_OK && v->strides[v->ndim - 1] != 1 && v->shape[v->ndim - 1] > 1) {
+            rten_tensor c;
+            s = sc.contiguous(v, &c);
+            *v = c;
+        }
+        return s;
+    };
+    rten_tensor qv, kv, vv, bv, mv, abv, pkv, pvv;
+    rten_status st = view(query, &qv);
+    if (st == RTEN_OK && key) st = view(key, &kv);
+    if (st == RTEN_OK && key) st = view(value, &vv);
+    if (st == RTEN_OK && bias) st = view(bias, &bv);
+    if (st == RTEN_OK && key_padding_mask) st = view(key_padding_mask, &mv);
+    if (st == RTEN_OK && attention_bias) st = sc.in(attention_bias, &abv);
+    if (st == RTEN_OK && past_key) st = view(past_key, &pkv);
+    if (st == RTEN_OK && past_value) st = view(past_value, &pvv);
+    rten_tensor ov, pk, pv;
+    const int64_t oshape[3] = {B, S, H * D}, cshape[4] = {B, H, T, D};
+    if (st == RTEN_OK) st = sc.out(out, RTEN_F32, 3, oshape, &ov, nullptr);
+    if (st == RTEN_OK && present_key) st = sc.out(present_key, RTEN_F32, 4, cshape, &pk, nullptr);
+    if (st == RTEN_OK && present_value) st = sc.out(present_value, RTEN_F32, 4, cshape, &pv, nullptr);
+    if (st == RTEN_OK && (ov.strides[2] != 1 || (present_key && pk.strides[3] != 1) || (present_value && pv.strides[3] != 1)))
+        st = fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "MultiHeadAttention: the outputs need a contiguous last dimension");
+    if (st != RTEN_OK) return sc.finish(st);
+    if (B * S == 0) return sc.finish(RTEN_OK);
+
+    // head rows (b, s, h, i) of q and of the new k / v
+    RotaryRows qr, kr, vr;
+    if (packed) {
+        auto comp = [&](int c) {
+            RotaryRows r;
+            r.p = (float*)qv.data + c * qv.strides[3];
+            r.sb = qv.strides[0];
+            r.ss = qv.strides[1];
+            r.sh = qv.strides[2];
+            r.sd = qv.strides[4];
+            return r;
+        };
+        qr = comp(0);
+        kr = comp(1);
+        vr = comp(2);
+    } else {
+        qr = rows3(&qv, D, 0);
+        kr = key ? rows3(&kv, D, 0) : qr;
+        vr = key ? rows3(&vv, D, 0) : qr;
+    }
+    // prep (one rotary / append launch) when there is a bias to add or a cache to build; else q / k / v are read in place
+    const bool prep = bias || P > 0 || present_key || present_value;
+    RotaryRows qa = qr;    // what the attention kernel reads
+    RotaryRows kc, vc;     // [B, H, T, D] caches as rows (b, t, h) when prepped
+    RotaryLaunch R;
+    if (prep) {
+        auto scratch = [&](size_t n, void** p) { return temp_alloc(ctx, n * 4, p); };
+        void* qs = nullptr;
+        void* ks = nullptr;
+        void* vs = nullptr;
+        const size_t ncache = (size_t)(B * H * T * D);
+        if (bias) st = scratch((size_t)(B * S * H * D), &qs);
+        if (st == RTEN_OK && !present_key) st = scratch(ncache, &ks);
+        if (st == RTEN_OK && !present_value) st = scratch(ncache, &vs);
+        if (st != RTEN_OK) return sc.finish(st);
+        auto dense_cache = [&](void* p) {
+            RotaryRows r;
+            r.p = (float*)p;
+            r.sb = H * T * D;
+            r.ss = D;
+            r.sh = T * D;
+            r.sd = 1;
+            return r;
+        };
+        kc = present_key ? cache_rows(&pk) : dense_cache(ks);
+        vc = present_value ? cache_rows(&pv) : dense_cache(vs);
+        R.B = (int)B;
+        R.S = (int)S;
+        R.D = (int)D;
+        R.H = (int)H;
+        R.Hkv = (int)H;
+        R.T = (int)T;
+        if (bias) {
+            R.x = qr;
+            R.y.p = (float*)qs;
+            R.y.sb = S * H * D;
+            R.y.ss = H * D;
+            R.y.sh = D;
+            R.y.sd = 1;
+            qa = R.y;
+            const float* bb = (const float*)bv.data;
+            R.x_bias = bb;
+            R.k_bias = bb + hidden;
+            R.v_bias = bb + 2 * hidden;
+        }
+        R.k_new = kr;
+        R.v_new = vr;
+        R.k_cache = kc;
+        R.v_cache = vc;
+        R.build_k = P > 0 && !alias_k;
+        R.build_v = P > 0 && !alias_v;
+        if (P > 0) {
+            R.k_past = cache_rows(&pkv);
+            R.v_past = cache_rows(&pvv);
+        }
+        R.mha = 1;
+        R.S_kv = (int)L;
+        R.past = (int)P;
+    } else {
+        kc = kr;  // (b, t, h) rows of the inputs: T = L
+        vc = vr;
+    }
+    const int32_t* kpm_d = key_padding_mask ? (const int32_t*)mv.data : nullptr;
+    const long long kpm_b = key_padding_mask ? mv.strides[0] : 0;
+    const float fill = prm->mask_filter_value;
+
+    if (S == 1) {
+        AttnDecodeLaunch A;
+        A.B = (int)B;
+        A.q_heads = (int)H;
+        A.kv_heads = (int)H;
+        A.dh = (int)D;
+        A.kv_cap = (int)T;
+        A.q = qa.p;
+        A.q_b = qa.sb;
+        A.q_h = qa.sh;
+        A.k = kc.p;
+        A.k_b = kc.sb;
+        A.k_h = kc.sh;
+        A.k_l = kc.ss;
+        A.v = vc.p;
+        A.v_b = vc.sb;
+        A.v_h = vc.sh;
+        A.v_l = vc.ss;
+        A.v_d = 1;
+        if (attention_bias) {
+            A.mask = (const float*)abv.data;
+            A.m_b = bstride(&abv, 0);
+            A.m_h = bstride(&abv, 1);
+            A.m_l = bstride(&abv, 3);
+        }
+        A.scale = scale;
+        A.out = (float*)ov.data;
+        A.o_b = ov.strides[0];
+        A.o_h = D;
+        A.mha = 1;
+        A.vis_end = prm->unidirectional ? (int)P + 1 : (int)T;
+        A.fill = fill;
+        A.kpm = kpm_d;
+        A.kpm_b = kpm_b;
+        if (attn_decode_supported(A)) {
+            if (prep) st = launch_rotary(ctx, R);
+            if (st == RTEN_OK) st = launch_attn_decode(ctx, A);
+            return sc.finish(st);
+        }
+        // (a cache longer than the single-query kernel takes: the prefill kernel serves one query as well)
+    }
+    auto rows_desc = [](const RotaryRows& r, int64_t D_, int64_t n, int64_t heads, int64_t batch) {
+        OperandDesc d;
+        d.base = r.p;
+        d.dims[0] = D_;
+        d.dims[1] = n;
+        d.dims[2] = heads;
+        d.dims[3] = batch;
+        d.strides[0] = 1;
+        d.strides[1] = r.ss;
+        d.strides[2] = r.sh;
+        d.strides[3] = r.sb;
+        return d;
+    };
+    AttnPrefillMha M;
+    M.causal_offset = (int)P;
+    M.fill = fill;
+    M.kpm = kpm_d;
+    M.kpm_b = kpm_b;
+    M.v_rows = vc.p;
+    M.v_b = vc.sb;
+    M.v_h = vc.sh;
+    M.v_t = vc.ss;
+    AttnPrefillLaunch A;
+    A.B = (int)B;
+    A.q_heads = (int)H;
+    A.kv_heads = (int)H;
+    A.q_seq = (int)S;
+    A.kv_seq = (int)T;
+    A.dh = (int)D;
+    A.q = rows_desc(qa, D, S, H, B);
+    A.k = rows_desc(kc, D, T, H, B);
+    A.v = rows_desc(vc, D, T, H, B);
+    A.v_natural = true;
+    A.causal = prm->unidirectional ? 1 : 0;
+    if (attention_bias) {
+        A.mask = (const float*)abv.data;
+        A.m_b = bstride(&abv, 0);
+        A.m_h = bstride(&abv, 1);
+        A.m_s = bstride(&abv, 2);
+        M.m_t = bstride(&abv, 3);
+    }
+    A.scale = scale;
+    A.x3 = ctx->f32_mode == RTEN_F32_TF32 ? 0 : 1;
+    A.out = (float*)ov.data;
+    A.o_b = ov.strides[0];
+    A.o_h = D;
+    A.o_s = ov.strides[1];
+    A.mha = &M;
+    if (qa.sd != 1 || kc.sd != 1 || vc.sd != 1 || !attn_prefill_supported(A))
+        return sc.finish(fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE,
+                              "MultiHeadAttention: query, key, value, the caches and the output need 16-byte aligned rows"));
+    if (prep) st = launch_rotary(ctx, R);
     if (st == RTEN_OK) st = launch_attn_prefill(ctx, A);
     return sc.finish(st);
 }

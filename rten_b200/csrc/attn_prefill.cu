@@ -61,6 +61,13 @@ struct AttnPrefillParams {
     float scale;
     float* out;
     long long o_b, o_h, o_s;
+    // MultiHeadAttention (attn_prefill_mha_kernel only; see AttnPrefillMha)
+    int c_off;
+    float fill;
+    const int32_t* kpm;
+    long long kpm_b, m_t;
+    const float* v_rows;
+    long long v_b, v_h, v_t;
 };
 
 template <int N>
@@ -98,10 +105,14 @@ __device__ __forceinline__ uint32_t sw_off(int row, int col, int rows) {
     return (uint32_t)((col >> 5) * rows * 128 + row * 128 + ((((col & 31) >> 2) ^ (row & 7)) << 4) + ((col & 3) << 2));
 }
 
-template <int DH, bool X3>
-__global__ void __launch_bounds__(AP_THREADS, 1)
-attn_prefill_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant__ CUtensorMap tma_k,
-                    const __grid_constant__ CUtensorMap tma_v, const __grid_constant__ AttnPrefillParams p) {
+// MHA: the MultiHeadAttention scores (attn_prefill_mha_kernel).  Masked keys (causal, key_padding_mask) score p.fill
+// instead of -inf, the causal diagonal is offset by p.c_off, the mask's key stride is p.m_t, and the key tiles above
+// every row's diagonal, skipped as usual, are added back afterwards as n_tail keys of score fill (a row's weight of
+// them is e^(fill - m): only when that is non-zero somewhere in the CTA is their value sum read, with plain loads).
+// Without MHA this is the Attention / GroupQueryAttention kernel exactly as before.
+template <int DH, bool X3, bool MHA>
+__device__ __forceinline__ void attn_prefill_body(const CUtensorMap& tma_q, const CUtensorMap& tma_k, const CUtensorMap& tma_v,
+                                                  const AttnPrefillParams& p) {
     using C = Cfg<DH, X3>;
     constexpr int BN = C::BN;
     extern __shared__ uint8_t smem_raw[];
@@ -135,6 +146,7 @@ attn_prefill_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_cons
             mbar_init(&empty[s], 4);
         }
         mbar_init(bar_q, 1);
+        if constexpr (MHA) *reinterpret_cast<volatile int*>(bar_q + 1) = 0;  // the causal tail's flag
         fence_mbar_init();
     }
     __syncthreads();
@@ -143,7 +155,7 @@ attn_prefill_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_cons
 
     // keys [0, lim) exist for every row; a causal row s sees keys [0, s + off]
     const int lim = p.len ? min(max(__ldg(p.len + b), 0), p.kv_seq) : p.kv_seq;
-    const int off = p.len ? lim - p.q_seq : 0;
+    const int off = MHA ? p.c_off : (p.len ? lim - p.q_seq : 0);
     int kend = p.causal ? min(lim, min(q0 + BM, p.q_seq) + off) : lim;
     kend = max(kend, 0);
     const int ntiles = (kend + BN - 1) / BN;
@@ -189,6 +201,7 @@ attn_prefill_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_cons
         mrow0 = mh + (long long)min(row0, p.q_seq - 1) * p.m_s;
         mrow1 = mh + (long long)min(row1, p.q_seq - 1) * p.m_s;
     }
+    const int32_t* krow = MHA && p.kpm ? p.kpm + (long long)b * p.kpm_b : nullptr;
 
     float o[DH / 2];
 #pragma unroll
@@ -240,10 +253,18 @@ attn_prefill_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_cons
         for (int i = 0; i < BN / 2; i++) {
             const bool r1 = (i >> 1) & 1;
             const int key = key0 + 8 * (i >> 2) + (i & 1);
-            const bool ok = key < (r1 ? lim1 : lim0) && key >= (r1 ? lo1 : lo0);
             float z = __fmul_rn(sc[i], p.scale);
-            if (mrow0 && ok) z = __fadd_rn(z, __ldg((r1 ? mrow1 : mrow0) + key));
-            z = ok ? z : -INFINITY;
+            if constexpr (MHA) {
+                // absent (beyond the keys: tile padding) -> -inf; masked (causal, padding) -> fill, replacing the bias
+                const bool exists = key < lim;
+                const bool vis = key < (r1 ? lim1 : lim0) && (!krow || __ldg(krow + min(key, lim - 1)) != 0);
+                if (mrow0 && exists) z = __fadd_rn(z, __ldg((r1 ? mrow1 : mrow0) + (long long)key * p.m_t));
+                z = !exists ? -INFINITY : vis ? z : p.fill;
+            } else {
+                const bool ok = key < (r1 ? lim1 : lim0) && key >= (r1 ? lo1 : lo0);
+                if (mrow0 && ok) z = __fadd_rn(z, __ldg((r1 ? mrow1 : mrow0) + key));
+                z = ok ? z : -INFINITY;
+            }
             sc[i] = z;
             if (r1) mx1 = fmaxf(mx1, z);
             else mx0 = fmaxf(mx0, z);
@@ -296,6 +317,36 @@ attn_prefill_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_cons
     l0 = __fadd_rn(l0, __shfl_xor_sync(0xffffffffu, l0, 2));
     l1 = __fadd_rn(l1, __shfl_xor_sync(0xffffffffu, l1, 1));
     l1 = __fadd_rn(l1, __shfl_xor_sync(0xffffffffu, l1, 2));
+    if constexpr (MHA) {
+        // the causal tail [kt, kv_seq): keys of score fill for every row of the tile, never loaded
+        const int kt = min(ntiles * BN, lim), n_tail = lim - kt;
+        if (n_tail > 0) {  // (uniform over the CTA)
+            volatile int* flag = reinterpret_cast<volatile int*>(bar_q + 1);
+            const float mn0 = fmaxf(m0, p.fill), mn1 = fmaxf(m1, p.fill);
+            const float e0 = reduced_range_exp(__fsub_rn(p.fill, mn0)), e1 = reduced_range_exp(__fsub_rn(p.fill, mn1));
+            if (e0 != 0.0f || e1 != 0.0f) *flag = 1;
+            asm volatile("bar.sync 1, 128;" ::: "memory");  // every product done (P is free) and every row's flag set
+            if (*flag) {
+                float* vsum = reinterpret_cast<float*>(sp);
+                if (tid < DH) {
+                    const float* vr = p.v_rows + (long long)b * p.v_b + (long long)hk * p.v_h + tid;
+                    float acc = 0.0f;
+                    for (int key = kt; key < lim; key++) acc = __fadd_rn(acc, __ldg(vr + (long long)key * p.v_t));
+                    vsum[tid] = acc;
+                }
+                asm volatile("bar.sync 1, 128;" ::: "memory");
+                const float a0 = reduced_range_exp(__fsub_rn(m0, mn0)), a1 = reduced_range_exp(__fsub_rn(m1, mn1));
+                l0 = __fadd_rn(__fmul_rn(l0, a0), __fmul_rn((float)n_tail, e0));
+                l1 = __fadd_rn(__fmul_rn(l1, a1), __fmul_rn((float)n_tail, e1));
+#pragma unroll
+                for (int i = 0; i < DH / 2; i++) {
+                    const bool r1 = (i >> 1) & 1;
+                    const float vs = vsum[8 * (i >> 2) + 2 * t + (i & 1)];
+                    o[i] = __fadd_rn(__fmul_rn(o[i], r1 ? a1 : a0), __fmul_rn(r1 ? e1 : e0, vs));
+                }
+            }
+        }
+    }
     const float inv0 = __fdiv_rn(1.0f, l0), inv1 = __fdiv_rn(1.0f, l1);
     float* ob = p.out + (long long)b * p.o_b + (long long)h * p.o_h;
 #pragma unroll
@@ -308,6 +359,20 @@ attn_prefill_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_cons
         y1 = y1 != y1 ? 0.0f : y1;
         *reinterpret_cast<float2*>(ob + (long long)row * p.o_s + 8 * (i >> 2) + 2 * t) = make_float2(y0, y1);
     }
+}
+
+template <int DH, bool X3>
+__global__ void __launch_bounds__(AP_THREADS, 1)
+attn_prefill_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant__ CUtensorMap tma_k,
+                    const __grid_constant__ CUtensorMap tma_v, const __grid_constant__ AttnPrefillParams p) {
+    attn_prefill_body<DH, X3, false>(tma_q, tma_k, tma_v, p);
+}
+
+template <int DH, bool X3>
+__global__ void __launch_bounds__(AP_THREADS, 1)
+attn_prefill_mha_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant__ CUtensorMap tma_k,
+                        const __grid_constant__ CUtensorMap tma_v, const __grid_constant__ AttnPrefillParams p) {
+    attn_prefill_body<DH, X3, true>(tma_q, tma_k, tma_v, p);
 }
 
 template <int DH, bool X3>
@@ -331,8 +396,9 @@ rten_status launch_cfg(rten_ctx* ctx, const AttnPrefillLaunch& L, const AttnPref
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = getenv("RTEN_B200_NO_PDL") ? 0 : 1;
-    cudaError_t e = cudaFuncSetAttribute(attn_prefill_kernel<DH, X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
-    if (e == cudaSuccess) e = cudaLaunchKernelEx(&cfg, attn_prefill_kernel<DH, X3>, mq, mk, mv, p);
+    auto kernel = L.mha ? attn_prefill_mha_kernel<DH, X3> : attn_prefill_kernel<DH, X3>;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
+    if (e == cudaSuccess) e = cudaLaunchKernelEx(&cfg, kernel, mq, mk, mv, p);
     if (e != cudaSuccess) return fail_cuda(ctx, e, "prefill attention launch");
     e = cudaGetLastError();
     if (e != cudaSuccess) return fail_cuda(ctx, e, "prefill attention launch");
@@ -350,6 +416,7 @@ bool attn_prefill_supported(const AttnPrefillLaunch& L) {
     auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
     if (!al16(L.out) || (L.o_b & 3) || (L.o_h & 3) || (L.o_s & 3)) return false;
     if (L.mask && (reinterpret_cast<uintptr_t>(L.mask) & 3)) return false;
+    if (L.mha && (L.window || L.len || !L.v_natural || !L.mha->v_rows || L.mha->causal_offset < 0)) return false;
     return tma_compatible(L.q, 4, 4) && tma_compatible(L.k, 4, 4) && tma_compatible(L.v, 4, 4);
 }
 
@@ -374,6 +441,18 @@ rten_status launch_attn_prefill(rten_ctx* ctx, const AttnPrefillLaunch& L) {
     p.o_b = L.o_b;
     p.o_h = L.o_h;
     p.o_s = L.o_s;
+    if (L.mha) {
+        const AttnPrefillMha& M = *L.mha;
+        p.c_off = M.causal_offset;
+        p.fill = M.fill;
+        p.kpm = M.kpm;
+        p.kpm_b = M.kpm_b;
+        p.m_t = M.m_t;
+        p.v_rows = M.v_rows;
+        p.v_b = M.v_b;
+        p.v_h = M.v_h;
+        p.v_t = M.v_t;
+    }
     if (L.dh == 64) return L.x3 ? launch_cfg<64, true>(ctx, L, p) : launch_cfg<64, false>(ctx, L, p);
     return L.x3 ? launch_cfg<128, true>(ctx, L, p) : launch_cfg<128, false>(ctx, L, p);
 }

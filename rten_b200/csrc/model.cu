@@ -10,7 +10,8 @@
 //          operators (Reshape, Flatten, Squeeze, Unsqueeze, Transpose, Identity) are views -- no kernel, no copy.
 // Operators: Conv, ConvInteger, ConvTranspose (without output_shape), Relu, Clip, MaxPool, GlobalAveragePool, ReduceMean, Gemm, MatMul, MatMulInteger, MatMulNBits
 // (com.microsoft), Add, Mul, Softmax, LayerNormalization, Gelu, Erf, Gather, Cast, DynamicQuantizeLinear, Attention,
-// RotaryEmbedding, GroupQueryAttention (com.microsoft, three outputs), Constant and the view operators.
+// RotaryEmbedding, GroupQueryAttention and MultiHeadAttention (com.microsoft, three outputs), Constant and the view
+// operators.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -154,7 +155,7 @@ const std::set<std::string>& supported_ops() {
         "Conv", "ConvTranspose", "Relu", "Clip", "MaxPool", "GlobalAveragePool", "ReduceMean", "Reshape", "Flatten", "Squeeze", "Unsqueeze", "Transpose",
         "Identity", "Gemm", "MatMul", "Add", "Mul", "Softmax", "LayerNormalization", "Gelu", "Erf", "Gather",
         "DynamicQuantizeLinear", "MatMulInteger", "ConvInteger", "Cast", "Attention", "MatMulNBits", "GroupQueryAttention",
-        "RotaryEmbedding", "Constant"};
+        "MultiHeadAttention", "RotaryEmbedding", "Constant"};
     return s;
 }
 
@@ -293,6 +294,17 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
                 return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "GroupQueryAttention: missing attribute num_heads or kv_num_heads");
             if (n.inputs.size() > 12)
                 return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "GroupQueryAttention: quantization and Q/K norm inputs (12-15) are not supported");
+        }
+        if (n.op_type == "MultiHeadAttention") {  // src/op_registry/onnx_registry.rs:1495-1505, contrib.rs:302-315
+            if (n.domain != "com.microsoft") return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "unsupported operator MultiHeadAttention");
+            if (!n.attr("num_heads")) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MultiHeadAttention: missing attribute num_heads");
+            if (n.attr("scale") && !(n.attr_f("scale", 0.0f) > 0.0f))
+                return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MultiHeadAttention: an explicit scale must be positive");
+            for (size_t i = 8; i < n.inputs.size(); i++)
+                if (!n.inputs[i].empty())
+                    return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MultiHeadAttention: past_sequence_length and cache_indirection (inputs 8, 9) are not supported");
+            if (n.outputs.size() > 3 && !n.outputs[3].empty())
+                return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MultiHeadAttention: the qk output (3) is not supported");
         }
         if (n.op_type == "ConvTranspose" && n.attr("output_shape"))  // (the reference does not read it)
             return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "ConvTranspose: the output_shape attribute is not supported");
@@ -747,6 +759,23 @@ struct Runner {
             if (st == RTEN_OK) {
                 if (o.out.size() > 1 && o.out[1] >= 0) set_owned(o.out[1], pk); else pool_free(ctx, pk.data);
                 if (o.out.size() > 2 && o.out[2] >= 0) set_owned(o.out[2], pv); else pool_free(ctx, pv.data);
+            }
+        } else if (op == "MultiHeadAttention") {
+            rten_mha_params p;
+            memset(&p, 0, sizeof(p));
+            p.num_heads = (int32_t)o.n.attr_i("num_heads", 0);
+            p.scale = o.n.attr_f("scale", 0.0f);
+            p.mask_filter_value = o.n.attr_f("mask_filter_value", -10000.0f);
+            p.unidirectional = (int32_t)o.n.attr_i("unidirectional", 0);
+            const bool want_k = o.out.size() > 1 && o.out[1] >= 0, want_v = o.out.size() > 2 && o.out[2] >= 0;
+            rten_tensor pk, pv;
+            memset(&pk, 0, sizeof(pk));
+            memset(&pv, 0, sizeof(pv));
+            st = rten_b200_multi_head_attention(ctx, T(0), T(1), T(2), T(3), T(4), T(5), T(6), T(7), nullptr, nullptr, &p, &y,
+                                                want_k ? &pk : nullptr, want_v ? &pv : nullptr);
+            if (st == RTEN_OK) {
+                if (want_k) set_owned(o.out[1], pk);
+                if (want_v) set_owned(o.out[2], pv);
             }
         } else {
             return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "unsupported operator " + op);

@@ -38,7 +38,7 @@ struct RotaryTable {
 //                 past_len(b) + S on (the positions of the new tokens are left to the append)
 // and writes len_eff[b] = past_len(b) + S when len_eff is set.  past_len(b) = 0 for a first prompt (or without
 // seqlens), else clamp(seqlens[b], S - 1, T - 1) + 1 - S, read on the device.
-struct RotaryLaunch {
+struct RotaryCore {
     int B = 0, S = 0, D = 0, H = 0, Hkv = 0, T = 0;
     RotaryTable rot;
     RotaryRows x, y;
@@ -49,6 +49,18 @@ struct RotaryLaunch {
     int first = 0;
     int32_t* len_eff = nullptr;
 };
+// MultiHeadAttention's prep (mha = 1; no rotation, seqlens and len_eff unused): the new K / V streams have S_kv rows per
+// batch, past_len(b) = past for every batch (present caches of T = past + S_kv positions), and each stream may add a
+// bias vector -- element h * D + i to element i of a head-h row, one rounded f32 add (null: none)
+struct RotaryMha {
+    int mha = 0;
+    int S_kv = 0;
+    int past = 0;
+    const float* x_bias = nullptr;
+    const float* k_bias = nullptr;
+    const float* v_bias = nullptr;
+};
+struct RotaryLaunch : RotaryCore, RotaryMha {};
 rten_status launch_rotary(rten_ctx* ctx, const RotaryLaunch& L);
 
 }  // namespace rtb

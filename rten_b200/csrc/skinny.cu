@@ -597,8 +597,10 @@ constexpr int ATTN_CHUNK = 128;  // cached positions per CTA (eight warps; the s
 // (one wave).
 // EXT: the GroupQueryAttention features of AttnDecodeLaunch (len stride / offset / floor, sliding window, rotary
 // embedding); without them the kernel is the plain Attention decode kernel, compiled from the same code as before.
-template <int DH, int NW, bool EXT>
-__global__ void __launch_bounds__(NW * 32, DH == 64 ? (NW == 8 ? 3 : 4) : 1) attn_decode_kernel(const AttnDecodeParams p) {
+// MHA (attn_decode_mha_kernel, EXT off): MultiHeadAttention's masking -- a position at or beyond X.vis_end or with
+// key_padding_mask 0 scores X.fill (finite: it still counts in the softmax) instead of its biased score.
+template <int DH, int NW, bool EXT, bool MHA>
+__device__ __forceinline__ void attn_decode_body(const AttnDecodeParams& p) {
     // Every warp owns 16 consecutive cached positions of the CTA's chunk and runs the whole attention on them by itself
     // (scores, local max, exponentials, local sum, value product): no block barrier until the warps' partial
     // (max, sum, output) triples are merged -- the same merge that later combines the splits of a (batch, head).
@@ -739,6 +741,10 @@ __global__ void __launch_bounds__(NW * 32, DH == 64 ? (NW == 8 ? 3 : 4) : 1) att
         if (i >= skip && i < nl) {
             s *= L.scale;
             if (mrow) s += mrow[(long long)(l0 + i) * L.m_l];
+            if constexpr (MHA) {
+                const int l = l0 + i;
+                if (l >= X.vis_end || (X.kpm && X.kpm[(long long)b * X.kpm_b + l] == 0)) s = X.fill;
+            }
             mw = fmaxf(mw, s);
         }
         sc[it] = s;
@@ -858,6 +864,16 @@ __global__ void __launch_bounds__(NW * 32, DH == 64 ? (NW == 8 ? 3 : 4) : 1) att
     }
 }
 
+template <int DH, int NW, bool EXT>
+__global__ void __launch_bounds__(NW * 32, DH == 64 ? (NW == 8 ? 3 : 4) : 1) attn_decode_kernel(const AttnDecodeParams p) {
+    attn_decode_body<DH, NW, EXT, false>(p);
+}
+
+template <int DH, int NW>
+__global__ void __launch_bounds__(NW * 32, DH == 64 ? (NW == 8 ? 3 : 4) : 1) attn_decode_mha_kernel(const AttnDecodeParams p) {
+    attn_decode_body<DH, NW, false, true>(p);
+}
+
 bool attn_decode_supported(const AttnDecodeLaunch& L) {
     if (getenv("RTEN_B200_NO_SKINNY")) return false;
     if (L.dh != 64 && L.dh != 128) return false;
@@ -871,6 +887,8 @@ bool attn_decode_supported(const AttnDecodeLaunch& L) {
     if (L.rot_cos && (!L.rot_sin || L.rot_half < 0 || 2 * L.rot_half > L.dh || L.rot_max_pos < 1)) return false;
     if (L.window < 0 || L.len_min < 0 || L.len_add < 0 || L.len_min > L.kv_cap) return false;
     if (L.window > 0 && L.v_l == 1) return false;  // the sliding window masks within the natural value layout only
+    // MultiHeadAttention's masking replaces the GroupQueryAttention features (attn_decode_mha_kernel is built without them)
+    if (L.mha && (L.rot_cos || L.window > 0 || L.len_s != 1 || L.len_add || L.len_min || L.k_new)) return false;
     if (L.v_l == 1 && (!al16(L.v) || (L.v_b & 3) || (L.v_h & 3) || (L.v_d & 3))) return false;  // float4 along the positions
     return true;
 }
@@ -928,7 +946,10 @@ rten_status launch_attn_decode(rten_ctx* ctx, const AttnDecodeLaunch& L) {
     cfg.attrs = attr;
     cfg.numAttrs = getenv("RTEN_B200_NO_PDL") ? 0 : 1;
     cudaError_t e;
-    if (ext)
+    if (L.mha)
+        e = L.dh == 64 ? (nw == 6 ? cudaLaunchKernelEx(&cfg, attn_decode_mha_kernel<64, 6>, p) : cudaLaunchKernelEx(&cfg, attn_decode_mha_kernel<64, 8>, p))
+                       : cudaLaunchKernelEx(&cfg, attn_decode_mha_kernel<128, 8>, p);
+    else if (ext)
         e = L.dh == 64 ? (nw == 6 ? cudaLaunchKernelEx(&cfg, attn_decode_kernel<64, 6, true>, p) : cudaLaunchKernelEx(&cfg, attn_decode_kernel<64, 8, true>, p))
                        : cudaLaunchKernelEx(&cfg, attn_decode_kernel<128, 8, true>, p);
     else

@@ -93,6 +93,13 @@ struct AttnDecodeExt {
     int rot_half = 0, rot_interleaved = 0, rot_max_pos = 0;
     const int32_t* rot_pos = nullptr;
     long long rot_pos_b = 0;
+    // MultiHeadAttention (mha = 1, none of the fields above): positions l >= vis_end, and positions whose
+    // kpm[b * kpm_b + l] is 0, score `fill` in place of scale * q.k + mask
+    int mha = 0;
+    int vis_end = 0;
+    float fill = 0.0f;
+    const int32_t* kpm = nullptr;
+    long long kpm_b = 0;
 };
 struct AttnDecodeLaunch : AttnDecodeCore, AttnDecodeExt {};
 bool attn_decode_supported(const AttnDecodeLaunch& L);

@@ -19,7 +19,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import (RTEN_DEVICE_HOST, RTEN_F32, RTEN_I8, RTEN_I32, RTEN_U8, RtenAttentionParams, RtenConvParams,
-                   RtenConvTransposeParams, RtenGqaParams, RtenTensor)
+                   RtenConvTransposeParams, RtenGqaParams, RtenMhaParams, RtenTensor)
 
 _NP2RT = {np.dtype(np.float32): RTEN_F32, np.dtype(np.int32): RTEN_I32, np.dtype(np.int8): RTEN_I8,
           np.dtype(np.uint8): RTEN_U8}
@@ -491,6 +491,35 @@ class GroupQueryAttention:
             ctx.handle, A.t(query), A.t(key), A.t(value), A.t(past_key), A.t(past_value), A.t(seqlens_k), A.t(total), A.t(cos_cache),
             A.t(sin_cache), A.t(position_ids), A.t(attention_bias), C.byref(p), C.byref(o), C.byref(pk), C.byref(pv)))
         return A.wrap(o, out), A.wrap(pk, present_key), A.wrap(pv, present_value)
+
+
+class MultiHeadAttention:
+    """src/ops/attention/contrib.rs:43-300 (com.microsoft MultiHeadAttention); attribute names and defaults as the
+    reference's.  Masked keys (unidirectional, key_padding_mask) score `mask_filter_value` and stay in the softmax.  One
+    query runs the single-query attention kernel, more the streaming prefill kernel; a bias, a past cache or a present
+    output adds one launch of the rotary / append kernel before it."""
+
+    def __init__(self, num_heads: int, scale: Optional[float] = None, mask_filter_value: float = -10000.0, unidirectional: bool = False):
+        self.num_heads, self.scale = int(num_heads), scale
+        self.mask_filter_value, self.unidirectional = float(mask_filter_value), bool(unidirectional)
+
+    def run(self, ctx, query, key=None, value=None, bias=None, key_padding_mask=None, attention_bias=None, past_key=None,
+            past_value=None, past_sequence_length=None, cache_indirection=None, out=None, present_key=None, present_value=None,
+            want_present: bool = True):
+        """Returns (output, present_key, present_value); the present caches are None with `want_present=False`.
+        `present_key` / `present_value` may be views of the `past_key` / `past_value` buffers (same data pointer and
+        strides, L more positions): then only the new positions are written into them."""
+        A = _Args(ctx)
+        o = A.out(out)
+        pk = A.out(present_key) if want_present else None
+        pv = A.out(present_value) if want_present else None
+        p = RtenMhaParams(self.num_heads, float(self.scale) if self.scale else 0.0, self.mask_filter_value, int(self.unidirectional))
+        ctx.check(ctx.lib.rten_b200_multi_head_attention(
+            ctx.handle, A.t(query), A.t(key), A.t(value), A.t(bias), A.t(key_padding_mask), A.t(attention_bias), A.t(past_key),
+            A.t(past_value), A.t(past_sequence_length), A.t(cache_indirection), C.byref(p), C.byref(o),
+            C.byref(pk) if want_present else None, C.byref(pv) if want_present else None))
+        return (A.wrap(o, out), A.wrap(pk, present_key) if want_present else None,
+                A.wrap(pv, present_value) if want_present else None)
 
 
 def _conv_params(padding, groups, strides, dilations) -> RtenConvParams:
