@@ -431,6 +431,55 @@ rten_status rten_b200_multi_head_attention(rten_ctx* ctx, const rten_tensor* que
                                            const rten_mha_params* params, rten_tensor* out, rten_tensor* present_key_or_null,
                                            rten_tensor* present_value_or_null);
 
+/* GRU and LSTM (src/ops/rnn.rs gru / lstm), f32.  x [T, B, I]; w [dirs, G * H, I] and r [dirs, G * H, H] with G = 3
+ * (GRU gates z, r, h) or 4 (LSTM gates i, o, f, c), in that ONNX order; bias [dirs, 2 * G * H] (input biases, then
+ * recurrent biases); initial_h (and initial_c) [dirs, B, H].  Outputs y [T, dirs, B, H], y_h [dirs, B, H] and y_c
+ * [dirs, B, H]; every optional input and output may be NULL.  dirs = 2 for bidirectional; direction 1 of a
+ * bidirectional layer and a reverse layer run t = T - 1 .. 0, and y stays indexed by t.  H is read from w, as the
+ * reference does (params->hidden_size is informative).  sequence_lens (i32) is accepted and ignored, as the reference
+ * ignores it: every sequence runs all T steps.
+ * Arithmetic, in the reference's order with every operation rounded on its own:
+ *   GRU : gx = x W^T (+ Wb); s = h R^T (+ Rb); z, r = sigmoid(gx + s); h~ = tanh(gx_h + r s_h); h = (1 - z) h~ + z h
+ *   LSTM: g = ((x W^T (+ Wb)) + h R^T) (+ Rb); i, o, f = sigmoid(g); c~ = tanh(g_c); c = f c + i c~; h = o tanhf(c)
+ * sigmoid = 1 / (1 + exp(-x)) and tanh are rten-vecmath's recipes; the LSTM's last tanh is a correctly rounded tanhf
+ * (the reference's f32::tanh).  GRU requires linear_before_reset = 1 (0 fails with RTEN_ERR_UNSUPPORTED_VALUE, as in the
+ * reference); a non-NULL LSTM peephole input fails with RTEN_ERR_UNSUPPORTED_VALUE.  Every shape error the reference
+ * raises comes back with its message; mismatched dimensions it does not check fail with RTEN_ERR_INVALID_VALUE.
+ * Paths:
+ *  - input projection: ONE wgmma GEMM [T * B, I] x [dirs * G * H, I]^T for every step and direction, in the context's
+ *    f32 mode.  packed_w_or_null = rten_b200_prepack_b of w viewed as [I, dirs * G * H] (the transpose of w reshaped to
+ *    [dirs * G * H, I]); in 3xTF32 mode its split copy is cached with the handle.
+ *  - recurrence, cluster path: ONE launch of rnn_cluster_kernel.  A thread-block cluster per (direction, batch slice)
+ *    keeps its direction's R in shared memory for all T steps, split over its CTAs by hidden unit; each step every CTA
+ *    computes its gates' h R^T as exact f32 FMA chains (in both f32 modes), applies the gate arithmetic and pushes its
+ *    slice of h to every CTA of the cluster through distributed shared memory, then crosses one cluster barrier.  The
+ *    cluster size is the smallest of 1, 2, 4, 8, 16 CTAs whose shared memory holds R (16 needs the non-portable size
+ *    and is checked with cudaOccupancyMaxActiveClusters).  This covers H <= 256 for GRU and LSTM at any B and I: up to
+ *    H = 336 (LSTM) / 388 (GRU) with 8-CTA clusters, and H = 468 / 544 where 16-CTA clusters schedule; H need not be a
+ *    multiple of 4.
+ *  - recurrence, per-step path (larger H, or env RTEN_B200_NO_RNN_CLUSTER=1 for comparison): per step and direction
+ *    the recurrent product on the skinny f32 kernel (B <= 32: exact f32; R is copied once into zero-padded 16-byte
+ *    rows when its rows are not) or else on the wgmma GEMM in 3xTF32 in both f32 modes (R split once per call), then
+ *    one gate kernel for all directions.
+ * Launches of a device-resident call with contiguous x and packed w: cluster path 2 (plus the TF32 low-part split of
+ * x in 3xTF32 mode); per-step path 2 + T * (dirs + 1) with R in 16-byte rows and B <= 32 (plus one launch per step and
+ * direction for the 3xTF32 split of h on the wgmma GEMM).
+ * Nothing is read back to the host, so such a call can be captured in a CUDA graph. */
+typedef struct {
+    int32_t direction;           /* 0 forward, 1 reverse, 2 bidirectional */
+    int32_t hidden_size;         /* informative */
+    int32_t linear_before_reset; /* GRU: must be 1 */
+} rten_rnn_params;
+rten_status rten_b200_gru(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w, const rten_packed* packed_w_or_null,
+                          const rten_tensor* r, const rten_tensor* bias_or_null, const rten_tensor* sequence_lens_or_null,
+                          const rten_tensor* initial_h_or_null, const rten_rnn_params* params, rten_tensor* y_or_null,
+                          rten_tensor* y_h_or_null);
+rten_status rten_b200_lstm(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w, const rten_packed* packed_w_or_null,
+                           const rten_tensor* r, const rten_tensor* bias_or_null, const rten_tensor* sequence_lens_or_null,
+                           const rten_tensor* initial_h_or_null, const rten_tensor* initial_c_or_null,
+                           const rten_tensor* peephole_or_null, const rten_rnn_params* params, rten_tensor* y_or_null,
+                           rten_tensor* y_h_or_null, rten_tensor* y_c_or_null);
+
 /* Softmax (src/ops/norm.rs:825-899) and AddSoftmax (src/ops/attention.rs:30-165) when mask != NULL
  * (mask broadcast to x, added lane-wise before the softmax over `axis`; AddSoftmax uses axis -1).
  * `out` may alias `x` (= run_in_place). */
@@ -509,7 +558,9 @@ rten_status rten_b200_scatter_rows(rten_ctx* ctx, rten_tensor* table, const rten
  * RotaryEmbedding, GroupQueryAttention (com.microsoft; output and present_key / present_value, inputs 12-15 rejected;
  * the executor allocates new present caches, so each decode step also copies the past: two launches, not one),
  * MultiHeadAttention (com.microsoft; outputs 0-2; a missing num_heads, an explicit scale <= 0, inputs 8 / 9 and the
- * qk output 3 fail the load; the executor allocates new present caches), Constant and the view operators; anything else fails the LOAD with
+ * qk output 3 fail the load; the executor allocates new present caches), GRU / LSTM (outputs 0-2; constant W prepacked at
+ * load; activation_alpha / activation_beta, non-default activations, clip != 0, layout != 0, LSTM input_forget != 0, a
+ * missing hidden_size and a non-empty peephole input fail the load), Constant and the view operators; anything else fails the LOAD with
  * RTEN_ERR_UNSUPPORTED_VALUE ("unsupported operator <name>"). */
 typedef struct rten_model rten_model;
 rten_status rten_b200_model_load(rten_ctx* ctx, const void* onnx_bytes, size_t len, rten_model** out);

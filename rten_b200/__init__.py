@@ -6,6 +6,6 @@ runners and bench.py.  There is no CPU implementation in this package."""
 from . import _lib  # noqa: F401
 from .ops import (  # noqa: F401
     ACT_GELU, ACT_GELU_TANH, ACT_NONE, ACT_RELU, Add, AddSoftmax, Attention, Clip, Comm, Context, Conv, ConvInteger, ConvIntegerToFloat,
-    ConvTranspose, DeviceTensor, DynamicQuantizeLinear, Erf, FusedMatMul, GatherRows, Gelu, Gemm, GlobalAveragePool, GroupQueryAttention,
-    LayerNormalization, MatMul, MatMulInteger, MatMulIntegerToFloat, MatMulNBits, MaxPool, Mul, MultiHeadAttention, OpError, Packed, QuantizedLinear, Relu, RotaryEmbedding, ScatterRows, Softmax, from_torch,
+    ConvTranspose, DeviceTensor, DynamicQuantizeLinear, Erf, FusedMatMul, GatherRows, Gelu, Gemm, GlobalAveragePool, GroupQueryAttention, GRU,
+    LayerNormalization, LSTM, MatMul, MatMulInteger, MatMulIntegerToFloat, MatMulNBits, MaxPool, Mul, MultiHeadAttention, OpError, Packed, QuantizedLinear, Relu, RotaryEmbedding, ScatterRows, Softmax, from_torch,
 )

@@ -73,6 +73,10 @@ class RtenMhaParams(C.Structure):
     _fields_ = [("num_heads", C.c_int32), ("scale", C.c_float), ("mask_filter_value", C.c_float), ("unidirectional", C.c_int32)]
 
 
+class RtenRnnParams(C.Structure):
+    _fields_ = [("direction", C.c_int32), ("hidden_size", C.c_int32), ("linear_before_reset", C.c_int32)]
+
+
 _TP = C.POINTER(RtenTensor)
 _vp = C.c_void_p
 
@@ -123,6 +127,8 @@ _SIGNATURES = {
                                                   C.POINTER(RtenGqaParams), _TP, _TP, _TP]),
     "rten_b200_multi_head_attention": (C.c_int, [_vp, _TP, _TP, _TP, _TP, _TP, _TP, _TP, _TP, _TP, _TP,
                                                  C.POINTER(RtenMhaParams), _TP, _TP, _TP]),
+    "rten_b200_gru": (C.c_int, [_vp, _TP, _TP, _vp, _TP, _TP, _TP, _TP, C.POINTER(RtenRnnParams), _TP, _TP]),
+    "rten_b200_lstm": (C.c_int, [_vp, _TP, _TP, _vp, _TP, _TP, _TP, _TP, _TP, _TP, C.POINTER(RtenRnnParams), _TP, _TP, _TP]),
     "rten_b200_softmax": (C.c_int, [_vp, _TP, _TP, C.c_int, C.c_int, _TP]),
     "rten_b200_layer_norm": (C.c_int, [_vp, _TP, _TP, _TP, C.c_int, C.c_float, _TP]),
     "rten_b200_erf": (C.c_int, [_vp, _TP, _TP]),

@@ -19,19 +19,8 @@
 using namespace rtb;
 using namespace rtb::api;
 
-namespace {
-
-// ---------------------------------------------------------------------------------------
-// K-major 2-level operand: rows x K with element strides.  Packs into an aligned workspace when
-// TMA cannot address the original (k stride != 1, misaligned base / pitch).
-// ---------------------------------------------------------------------------------------
-struct Mat {
-    const void* base;
-    int64_t rows, K;
-    int64_t rs, ks;       // element strides
-    int64_t z0 = 1, z1 = 1;  // batch dims (z0 inner)
-    int64_t zs0 = 0, zs1 = 0;
-};
+namespace rtb {
+namespace api {
 
 rten_status to_kmajor(rten_ctx* ctx, int esize, const Mat& m, OperandDesc* od) {
     OperandDesc d;
@@ -70,6 +59,11 @@ rten_status to_kmajor(rten_ctx* ctx, int esize, const Mat& m, OperandDesc* od) {
     *od = d;
     return RTEN_OK;
 }
+
+}  // namespace api
+}  // namespace rtb
+
+namespace {
 
 // Collapse broadcast prefix dims of a matmul into at most 2 batch dims (z0 inner, z1 outer).  Dims are merged
 // only when A, B and the output all advance uniformly across them.

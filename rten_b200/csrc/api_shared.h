@@ -1,15 +1,30 @@
 // Helpers shared by the operator entry points (api_ops.cu: MatMul family, api_conv.cu: Conv family and pooling,
-// api_rows.cu: row / elementwise operators).
+// api_rows.cu: row / elementwise operators, api_rnn.cu: GRU / LSTM).
 #pragma once
 #include <algorithm>
 #include <cstdint>
 
 #include "api_util.h"
+#include "umma_gemm.h"
 
 namespace rtb {
 namespace api {
 
 inline int64_t round_up(int64_t v, int64_t m) { return (v + m - 1) / m * m; }
+
+// ---------------------------------------------------------------------------------------
+// K-major 2-level operand: rows x K with element strides.  Packs into an aligned workspace when
+// TMA cannot address the original (k stride != 1, misaligned base / pitch).
+// ---------------------------------------------------------------------------------------
+struct Mat {
+    const void* base;
+    int64_t rows, K;
+    int64_t rs, ks;       // element strides
+    int64_t z0 = 1, z1 = 1;  // batch dims (z0 inner)
+    int64_t zs0 = 0, zs1 = 0;
+};
+
+rten_status to_kmajor(rten_ctx* ctx, int esize, const Mat& m, OperandDesc* od);
 
 inline rten_status check_ctx(rten_ctx* ctx) { return ctx ? RTEN_OK : RTEN_ERR_INVALID_VALUE; }
 

@@ -10,8 +10,8 @@
 //          operators (Reshape, Flatten, Squeeze, Unsqueeze, Transpose, Identity) are views -- no kernel, no copy.
 // Operators: Conv, ConvInteger, ConvTranspose (without output_shape), Relu, Clip, MaxPool, GlobalAveragePool, ReduceMean, Gemm, MatMul, MatMulInteger, MatMulNBits
 // (com.microsoft), Add, Mul, Softmax, LayerNormalization, Gelu, Erf, Gather, Cast, DynamicQuantizeLinear, Attention,
-// RotaryEmbedding, GroupQueryAttention and MultiHeadAttention (com.microsoft, three outputs), Constant and the view
-// operators.
+// RotaryEmbedding, GroupQueryAttention and MultiHeadAttention (com.microsoft, three outputs), GRU and LSTM, Constant and
+// the view operators.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -155,8 +155,49 @@ const std::set<std::string>& supported_ops() {
         "Conv", "ConvTranspose", "Relu", "Clip", "MaxPool", "GlobalAveragePool", "ReduceMean", "Reshape", "Flatten", "Squeeze", "Unsqueeze", "Transpose",
         "Identity", "Gemm", "MatMul", "Add", "Mul", "Softmax", "LayerNormalization", "Gelu", "Erf", "Gather",
         "DynamicQuantizeLinear", "MatMulInteger", "ConvInteger", "Cast", "Attention", "MatMulNBits", "GroupQueryAttention",
-        "MultiHeadAttention", "RotaryEmbedding", "Constant"};
+        "MultiHeadAttention", "RotaryEmbedding", "GRU", "LSTM", "Constant"};
     return s;
+}
+
+// RNN direction attribute (src/op_registry/onnx_registry.rs get_common_rnn_attrs): 0 forward, 1 reverse, 2 bidirectional,
+// -1 for any other value
+int rnn_direction(const onnx::Node& n) {
+    const onnx::Attribute* a = n.attr("direction");
+    if (!a) return 0;
+    if (a->s == "forward") return 0;
+    if (a->s == "reverse") return 1;
+    if (a->s == "bidirectional") return 2;
+    return -1;
+}
+
+// The attributes get_common_rnn_attrs and the GRU / LSTM readers refuse, refused at load with the operator's name
+rten_status check_rnn_attrs(rten_ctx* ctx, const onnx::Node& n) {
+    const bool gru = n.op_type == "GRU";
+    const std::string& op = n.op_type;
+    if (!n.attr("hidden_size")) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, op + ": missing attribute hidden_size");
+    const int dir = rnn_direction(n);
+    if (dir < 0) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, op + ": unsupported direction");
+    for (const char* name : {"activation_alpha", "activation_beta"}) {
+        const onnx::Attribute* a = n.attr(name);
+        if (a && !a->floats.empty()) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, op + ": " + name + " is not supported");
+    }
+    if (const onnx::Attribute* a = n.attr("activations")) {
+        const std::vector<std::string> dflt = gru ? std::vector<std::string>{"Sigmoid", "Tanh"}
+                                                  : std::vector<std::string>{"Sigmoid", "Tanh", "Tanh"};
+        bool ok = a->strings.empty();
+        if (!ok && a->strings.size() == dflt.size() * (dir == 2 ? 2 : 1)) {
+            ok = true;
+            for (size_t i = 0; i < a->strings.size(); i++) ok = ok && a->strings[i] == dflt[i % dflt.size()];
+        }
+        if (!ok) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, op + ": only the default activations are supported");
+    }
+    if (n.attr_f("clip", 0.0f) != 0.0f) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, op + ": clip is not supported");
+    if (n.attr_i("layout", 0) != 0) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, op + ": layout = 1 is not supported");
+    if (!gru && n.attr_i("input_forget", 0) != 0)
+        return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, op + ": input_forget is not supported");
+    if (!gru && n.inputs.size() > 7 && !n.inputs[7].empty())
+        return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, op + ": peephole weights (input 7) are not supported");
+    return RTEN_OK;
 }
 
 bool is_view_op(const std::string& op) {
@@ -306,6 +347,7 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
             if (n.outputs.size() > 3 && !n.outputs[3].empty())
                 return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MultiHeadAttention: the qk output (3) is not supported");
         }
+        if (n.op_type == "GRU" || n.op_type == "LSTM") RTB_TRY(check_rnn_attrs(ctx, n));
         if (n.op_type == "ConvTranspose" && n.attr("output_shape"))  // (the reference does not read it)
             return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "ConvTranspose: the output_shape attribute is not supported");
         if (n.op_type == "RotaryEmbedding" && n.domain == "com.microsoft")
@@ -401,6 +443,17 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
         } else if ((op == "MatMul" || op == "MatMulInteger") && o.in.size() >= 2 && m->values[(size_t)o.in[1]].kind == V_CONST &&
                    m->values[(size_t)o.in[1]].t.ndim == 2) {
             RTB_TRY(rten_b200_prepack_b(ctx, &m->values[(size_t)o.in[1]].t, &o.packed));
+        } else if ((op == "GRU" || op == "LSTM") && o.in.size() >= 2 && o.in[1] >= 0 && m->values[(size_t)o.in[1]].kind == V_CONST &&
+                   m->values[(size_t)o.in[1]].t.dtype == RTEN_F32 && m->values[(size_t)o.in[1]].t.ndim == 3) {
+            // W [dirs, G * H, I] is the input projection's K-major B: prepack it as the [I, dirs * G * H] matrix
+            rten_tensor w = m->values[(size_t)o.in[1]].t;
+            const int64_t rows = w.shape[0] * w.shape[1], I = w.shape[2];
+            w.ndim = 2;
+            w.shape[0] = I;
+            w.shape[1] = rows;
+            w.strides[0] = 1;
+            w.strides[1] = I;
+            RTB_TRY(rten_b200_prepack_b(ctx, &w, &o.packed));
         }
     }
     RTB_TRY(rten_b200_sync(ctx));
@@ -777,6 +830,26 @@ struct Runner {
                 if (want_k) set_owned(o.out[1], pk);
                 if (want_v) set_owned(o.out[2], pv);
             }
+        } else if (op == "GRU" || op == "LSTM") {
+            const bool gru = op == "GRU";
+            rten_rnn_params p;
+            memset(&p, 0, sizeof(p));
+            p.direction = rnn_direction(o.n);
+            p.hidden_size = (int32_t)o.n.attr_i("hidden_size", 0);
+            p.linear_before_reset = (int32_t)o.n.attr_i("linear_before_reset", 0);
+            auto want = [&](size_t i) { return o.out.size() > i && o.out[i] >= 0; };
+            rten_tensor ys[3];
+            memset(ys, 0, sizeof(ys));
+            if (gru)
+                st = rten_b200_gru(ctx, T(0), T(1), o.packed, T(2), T(3), T(4), T(5), &p, want(0) ? &ys[0] : nullptr,
+                                   want(1) ? &ys[1] : nullptr);
+            else
+                st = rten_b200_lstm(ctx, T(0), T(1), o.packed, T(2), T(3), T(4), T(5), T(6), nullptr, &p,
+                                    want(0) ? &ys[0] : nullptr, want(1) ? &ys[1] : nullptr, want(2) ? &ys[2] : nullptr);
+            RTB_TRY(st);
+            for (size_t i = 0; i < 3; i++)
+                if (want(i) && (i < 2 || !gru)) set_owned(o.out[i], ys[i]);
+            return RTEN_OK;
         } else {
             return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "unsupported operator " + op);
         }

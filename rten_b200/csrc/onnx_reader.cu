@@ -189,6 +189,13 @@ bool decode_attribute(Reader r, Attribute* a, std::string* err) {
                 }
                 break;
             case 8: repeated<int64_t>(wt, v, sub, &a->ints, [](uint64_t x) { return (int64_t)x; }); break;
+            case 9:  // strings: one length-delimited entry per string
+                if (wt != 2) {
+                    *err = "malformed AttributeProto";
+                    return false;
+                }
+                a->strings.push_back(sub.str());
+                break;
             case 20: a->type = (int32_t)v; break;
             default: break;
         }
@@ -373,7 +380,22 @@ std::string summary_json(const Model& m) {
             if (k) o << ", ";
             json_str(o, n.attrs[k].name);
         }
-        o << "]}";
+        o << "]";
+        // the values of STRINGS attributes (e.g. an RNN's activations), by attribute name
+        bool any = false;
+        for (const Attribute& a : n.attrs) {
+            if (a.strings.empty()) continue;
+            o << (any ? ", " : ", \"strings\": {");
+            any = true;
+            json_str(o, a.name);
+            o << ": [";
+            for (size_t k = 0; k < a.strings.size(); k++) {
+                if (k) o << ", ";
+                json_str(o, a.strings[k]);
+            }
+            o << "]";
+        }
+        o << (any ? "}}" : "}");
     }
     o << "], \"initializers\": [";
     for (size_t i = 0; i < m.graph.initializers.size(); i++) {

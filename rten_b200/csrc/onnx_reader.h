@@ -30,12 +30,13 @@ struct Tensor {
 // AttributeProto (rten-onnx/src/onnx.rs:30-103)
 struct Attribute {
     std::string name;
-    int32_t type = 0;  // 1 FLOAT, 2 INT, 3 STRING, 4 TENSOR, 6 FLOATS, 7 INTS
+    int32_t type = 0;  // 1 FLOAT, 2 INT, 3 STRING, 4 TENSOR, 6 FLOATS, 7 INTS, 8 STRINGS
     float f = 0.0f;
     int64_t i = 0;
     std::string s;
     std::vector<float> floats;
     std::vector<int64_t> ints;
+    std::vector<std::string> strings;
     Tensor t;
     bool has_f = false, has_i = false, has_t = false;
 };

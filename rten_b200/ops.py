@@ -19,7 +19,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import (RTEN_DEVICE_HOST, RTEN_F32, RTEN_I8, RTEN_I32, RTEN_U8, RtenAttentionParams, RtenConvParams,
-                   RtenConvTransposeParams, RtenGqaParams, RtenMhaParams, RtenTensor)
+                   RtenConvTransposeParams, RtenGqaParams, RtenMhaParams, RtenTensor, RtenRnnParams)
 
 _NP2RT = {np.dtype(np.float32): RTEN_F32, np.dtype(np.int32): RTEN_I32, np.dtype(np.int8): RTEN_I8,
           np.dtype(np.uint8): RTEN_U8}
@@ -520,6 +520,64 @@ class MultiHeadAttention:
             C.byref(pk) if want_present else None, C.byref(pv) if want_present else None))
         return (A.wrap(o, out), A.wrap(pk, present_key) if want_present else None,
                 A.wrap(pv, present_value) if want_present else None)
+
+
+_RNN_DIRECTIONS = {"forward": 0, "reverse": 1, "bidirectional": 2}
+
+
+class _Rnn:
+    """Shared plumbing of GRU / LSTM (src/ops/rnn.rs).  `direction` is "forward", "reverse" or "bidirectional";
+    `hidden_size` is informative (H is read from the weights, as the reference does)."""
+
+    def __init__(self, direction: str = "forward", hidden_size: int = 0):
+        if direction not in _RNN_DIRECTIONS:
+            raise OpError(5, f"unsupported direction {direction!r}")
+        self.direction, self.hidden_size = direction, int(hidden_size)
+
+    def prepack(self, ctx, w) -> Packed:
+        """W [dirs, G * H, I] packed for the input projection (the [I, dirs * G * H] matrix the GEMM reads)."""
+        wa = np.ascontiguousarray(w.numpy() if isinstance(w, DeviceTensor) else np.asarray(w, np.float32))
+        A = _Args(ctx)
+        h = C.c_void_p()
+        ctx.check(ctx.lib.rten_b200_prepack_b(ctx.handle, A.t(wa.reshape(-1, wa.shape[-1]).T), C.byref(h)))
+        return Packed(ctx, h)
+
+
+class GRU(_Rnn):
+    """src/ops/rnn.rs gru: input projection on the wgmma GEMM, the recurrence in one cluster-resident kernel (or one
+    launch pair per step for large hidden sizes).  Only linear_before_reset = 1 is supported, as in the reference."""
+
+    def __init__(self, direction: str = "forward", hidden_size: int = 0, linear_before_reset: bool = True):
+        super().__init__(direction, hidden_size)
+        self.linear_before_reset = bool(linear_before_reset)
+
+    def run(self, ctx, x, w, r, b=None, sequence_lens=None, initial_h=None, packed_w: Optional[Packed] = None,
+            outputs=(0, 1)):
+        """Returns (Y, Y_h); an output whose index is not in `outputs` is not computed and comes back as None.
+        sequence_lens is accepted and ignored, as the reference ignores it."""
+        A = _Args(ctx)
+        y, yh = A.out(), A.out()
+        p = RtenRnnParams(_RNN_DIRECTIONS[self.direction], self.hidden_size, int(self.linear_before_reset))
+        ctx.check(ctx.lib.rten_b200_gru(ctx.handle, A.t(x), A.t(w), _ph(packed_w), A.t(r), A.t(b), A.t(sequence_lens),
+                                        A.t(initial_h), C.byref(p), C.byref(y) if 0 in outputs else None,
+                                        C.byref(yh) if 1 in outputs else None))
+        return tuple(A.wrap(o, None) if i in outputs else None for i, o in enumerate((y, yh)))
+
+
+class LSTM(_Rnn):
+    """src/ops/rnn.rs lstm, on the same kernels as GRU.  Peephole weights (input 7) are refused."""
+
+    def run(self, ctx, x, w, r, b=None, sequence_lens=None, initial_h=None, initial_c=None, peephole=None,
+            packed_w: Optional[Packed] = None, outputs=(0, 1, 2)):
+        """Returns (Y, Y_h, Y_c); outputs not in `outputs` are None.  sequence_lens is accepted and ignored."""
+        A = _Args(ctx)
+        y, yh, yc = A.out(), A.out(), A.out()
+        p = RtenRnnParams(_RNN_DIRECTIONS[self.direction], self.hidden_size, 1)
+        ctx.check(ctx.lib.rten_b200_lstm(ctx.handle, A.t(x), A.t(w), _ph(packed_w), A.t(r), A.t(b), A.t(sequence_lens),
+                                         A.t(initial_h), A.t(initial_c), A.t(peephole), C.byref(p),
+                                         C.byref(y) if 0 in outputs else None, C.byref(yh) if 1 in outputs else None,
+                                         C.byref(yc) if 2 in outputs else None))
+        return tuple(A.wrap(o, None) if i in outputs else None for i, o in enumerate((y, yh, yc)))
 
 
 def _conv_params(padding, groups, strides, dilations) -> RtenConvParams:
