@@ -47,4 +47,17 @@ struct OpScope {
     rten_status finish(rten_status st);
 };
 
+// a tensor with no data, shape or strides, for an entry point to allocate
+inline rten_tensor empty_tensor() {
+    rten_tensor t;
+    memset(&t, 0, sizeof(t));
+    return t;
+}
+
+// releases a temporary an entry point allocated
+inline void free_if(rten_ctx* ctx, rten_tensor& t) {
+    if (t.data) rten_b200_free(ctx, t.data);
+    t.data = nullptr;
+}
+
 }  // namespace rtb

@@ -590,6 +590,7 @@ struct AttnDecodeParams {
 };
 
 constexpr int ATTN_CHUNK = 128;  // cached positions per CTA (eight warps; the six-warp variant covers 96)
+static_assert(ATTN_DECODE_MAX_CACHE == 64 * ATTN_CHUNK, "a decode launch has at most 64 splits");
 
 // NW warps per CTA (8 or 6).  Registers cap the kernel at 80 per thread either way, so 256-thread CTAs run three to an SM
 // (444 on the chip) and 192-thread CTAs four (592): the launcher takes the variant whose grid needs fewer waves -- GPT-2's
@@ -878,7 +879,7 @@ bool attn_decode_supported(const AttnDecodeLaunch& L) {
     if (getenv("RTEN_B200_NO_SKINNY")) return false;
     if (L.dh != 64 && L.dh != 128) return false;
     if (L.B < 1 || L.q_heads < 1 || L.kv_heads < 1 || L.q_heads % L.kv_heads) return false;
-    if (L.kv_cap < 1 || L.kv_cap > 64 * ATTN_CHUNK) return false;
+    if (L.kv_cap < 1 || L.kv_cap > ATTN_DECODE_MAX_CACHE) return false;
     auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
     if (!al16(L.k) || (L.k_b & 3) || (L.k_h & 3) || (L.k_l & 3)) return false;
     if (!al16(L.q) || (L.q_b & 3) || (L.q_h & 3)) return false;

@@ -102,6 +102,7 @@ struct AttnDecodeExt {
     long long kpm_b = 0;
 };
 struct AttnDecodeLaunch : AttnDecodeCore, AttnDecodeExt {};
+constexpr int ATTN_DECODE_MAX_CACHE = 8192;  // kv_cap limit: 64 splits of the kernel's 128-position chunks
 bool attn_decode_supported(const AttnDecodeLaunch& L);
 rten_status launch_attn_decode(rten_ctx* ctx, const AttnDecodeLaunch& L);
 

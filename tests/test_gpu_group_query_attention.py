@@ -453,19 +453,22 @@ def test_group_query_attention_matches_the_restatement(rt, name, case):
 
 @pytest.mark.gpu
 def test_group_query_attention_rejects_a_present_cache_overlapping_the_past(rt):
-    """A present cache in the past buffer's memory but with other strides (a contiguous [B, Hkv, P + 1, D] view over a
-    contiguous [B, Hkv, P, D] past) is refused rather than read and written by one kernel at once."""
+    """A present cache in a past buffer's memory but with other strides is refused rather than read and written by one
+    kernel at once: a contiguous [B, Hkv, P + 1, D] present_key over a contiguous [B, Hkv, P, D] past, and an in-place
+    present_key (the past_key buffer itself) that overlaps past_value."""
     B, H, Hkv, D, P = 2, 4, 2, 64, 10
     ctx = _ctx(rt)
     buf = ctx.empty((B * Hkv * (P + 1) * D,))
-    past = buf.view((B, Hkv, P, D), (Hkv * P * D, P * D, D, 1))
+    dense = buf.view((B, Hkv, P, D), (Hkv * P * D, P * D, D, 1))
     pres = buf.view((B, Hkv, P + 1, D), (Hkv * (P + 1) * D, (P + 1) * D, D, 1))
+    in_place = buf.view((B, Hkv, P, D), (Hkv * (P + 1) * D, (P + 1) * D, D, 1))
     other = ctx.empty((B, Hkv, P + 1, D))
     q, k = ctx.empty((B, 1, H * D)), ctx.empty((B, 1, Hkv * D))
-    with pytest.raises(rt.OpError) as e:
-        rt.GroupQueryAttention(H, Hkv).run(ctx, q, k, k, np.array([P, P], np.int32), P + 1, past_key=past, past_value=past,
-                                            present_key=pres, present_value=other)
-    assert e.value.kind == "UnsupportedOutput" and "overlap a past cache" in e.value.msg
+    for past_key, past_value in ((dense, dense), (in_place, dense)):
+        with pytest.raises(rt.OpError) as e:
+            rt.GroupQueryAttention(H, Hkv).run(ctx, q, k, k, np.array([P, P], np.int32), P + 1, past_key=past_key,
+                                                past_value=past_value, present_key=pres, present_value=other)
+        assert e.value.kind == "UnsupportedOutput" and "overlap a past cache" in e.value.msg
 
 
 @pytest.mark.gpu
