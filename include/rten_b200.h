@@ -78,6 +78,25 @@ typedef enum {
                            reference's own f32 tolerance (rten-tensor/src/test_util.rs:47-92) at 1/3 of the tensor rate */
 } rten_f32_mode;
 
+/* Activation fused into an operator's epilogue (the node that follows it in the graph), applied after the bias and the
+ * residual add with the standalone operator's exact f32 roundings: the fused result is bit-identical to the operator
+ * chain.  Codes 0-3 are the `int activation` of the *_ex functions. */
+typedef enum {
+    RTEN_ACT_NONE = 0,
+    RTEN_ACT_RELU = 1,
+    RTEN_ACT_GELU = 2,         /* erf form */
+    RTEN_ACT_GELU_TANH = 3,    /* tanh approximation */
+    RTEN_ACT_SIGMOID = 4,      /* rten_b200_sigmoid */
+    RTEN_ACT_SILU = 5,         /* rten_b200_silu */
+    RTEN_ACT_HARD_SIGMOID = 6, /* rten_b200_hard_sigmoid with (alpha, beta) */
+    RTEN_ACT_HARD_SWISH = 7    /* rten_b200_hard_swish */
+} rten_activation_kind;
+typedef struct {
+    int32_t kind; /* rten_activation_kind */
+    float alpha;  /* RTEN_ACT_HARD_SIGMOID only (ONNX defaults 0.2, 0.5); ignored otherwise */
+    float beta;
+} rten_activation;
+
 /* ---- context, memory, diagnostics ----------------------------------------------------------- */
 rten_status rten_b200_ctx_create(int device, void* cuda_stream_or_null, size_t workspace_bytes, rten_ctx** out);
 void rten_b200_ctx_destroy(rten_ctx* ctx);
@@ -138,7 +157,7 @@ rten_status rten_b200_gemm(rten_ctx* ctx, const rten_tensor* a, const rten_tenso
 rten_status rten_b200_matmul(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b,
                              const rten_packed* packed_b_or_null, const rten_tensor* row_bias_or_null, float alpha,
                              rten_tensor* out);
-/* Extension used by whole-model runners: fused activation after bias (0 none, 1 relu, 2 gelu(erf),
+/* Extension used by whole-model runners: fused activation after bias (rten_activation_kind 0 none, 1 relu, 2 gelu(erf),
  * 3 gelu(tanh)) and optional residual add (same shape as out) before the activation. */
 rten_status rten_b200_matmul_ex(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b,
                                 const rten_packed* packed_b_or_null, const rten_tensor* row_bias_or_null, float alpha,
@@ -189,7 +208,8 @@ typedef struct {
 rten_status rten_b200_conv2d(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w,
                              const rten_packed* packed_w_or_null, const rten_tensor* bias_or_null,
                              const rten_conv_params* p, rten_tensor* out);
-/* Extension: fused residual add (same shape as out) + activation (see matmul_ex).
+/* Extension: fused residual add (same shape as out) + activation, codes 0-3 of rten_activation_kind (any other code:
+ * RTEN_ERR_INVALID_VALUE; conv2d_act takes the others).
  *
  * Depthwise convolutions -- the reference's condition (src/ops/conv.rs:248-284): not the pointwise case (1x1, no
  * padding, strides and dilations 1, groups 1), and in channels == out channels == groups, which includes 1-channel
@@ -211,6 +231,15 @@ rten_status rten_b200_conv2d_ex(rten_ctx* ctx, const rten_tensor* x, const rten_
                                 const rten_packed* packed_w_or_null, const rten_tensor* bias_or_null,
                                 const rten_conv_params* p, const rten_tensor* residual_or_null, int activation,
                                 rten_tensor* out);
+/* Extension: conv2d_ex with any rten_activation (NULL: none) -- Conv followed by Relu, Gelu, Sigmoid, Silu (the
+ * reference's fusion of Mul(x, Sigmoid(x))), HardSigmoid or HardSwish in the convolution's epilogue, on every path
+ * (implicit GEMM, small-channel stem, explicit im2col, NCHW outputs, depthwise), bit-identical to conv2d_ex followed by
+ * the standalone operator.  An unknown kind is RTEN_ERR_INVALID_VALUE.  Kinds above Relu after a residual need a
+ * pixel-contiguous output (else RTEN_ERR_UNSUPPORTED_VALUE), as Gelu always has. */
+rten_status rten_b200_conv2d_act(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w,
+                                 const rten_packed* packed_w_or_null, const rten_tensor* bias_or_null,
+                                 const rten_conv_params* p, const rten_tensor* residual_or_null,
+                                 const rten_activation* act_or_null, rten_tensor* out);
 /* Extension: act(Conv(x, w, bias, p) + Conv(x_proj, w_proj, bias_proj, p_proj)) -- the ONNX pattern Conv, Conv -> Add
    (-> Relu) of a residual block with a projection shortcut.  Both outputs must have the same shape
    (RTEN_ERR_INCOMPATIBLE_SHAPES); all tensors are f32 (RTEN_ERR_UNSUPPORTED_TYPE); otherwise the checks of conv2d_ex.
@@ -497,6 +526,20 @@ rten_status rten_b200_clip(rten_ctx* ctx, const rten_tensor* x, const rten_tenso
 /* Erf / Gelu (src/ops/unary_elementwise.rs:384-435); approximate != 0 => tanh form. */
 rten_status rten_b200_erf(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
 rten_status rten_b200_gelu(rten_ctx* ctx, const rten_tensor* x, int approximate, rten_tensor* out);
+/* Sigmoid, Silu, HardSigmoid and HardSwish, f32, bit-identical to the reference, every operation a separate exactly
+ * rounded one (no fused multiply-add):
+ *   Sigmoid     1 / (1 + exp(0 - x))                   rten-vecmath/src/exp.rs:201-212
+ *   Silu        x / (1 + exp(0 - x)): ONE division, not x * Sigmoid(x) (exp.rs:217-228; the reference's optimizer
+ *               rewrites Mul(x, Sigmoid(x)) into it)
+ *   HardSigmoid clamp(alpha * x + beta, 0, 1)          src/ops/unary_elementwise.rs:437-449 (ONNX defaults 0.2, 0.5)
+ *   HardSwish   x * clamp(x / 6 + 0.5, 0, 1)           :457-469, with 1/6 rounded to f32 and multiplied
+ * exp is rten-vecmath's Exp (inf from 104 on), so Silu(x <= -104) = -0.0 and Silu(-inf) = NaN.  clamp is f32::clamp
+ * (comparisons): NaN passes through and -0.0 stays -0.0, so HardSwish(-4) = -0.0.  x in any strides; `out` may alias
+ * `x` (run_in_place).  One kernel launch for dense device-resident x, capturable in a CUDA graph. */
+rten_status rten_b200_sigmoid(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
+rten_status rten_b200_silu(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
+rten_status rten_b200_hard_sigmoid(rten_ctx* ctx, const rten_tensor* x, float alpha, float beta, rten_tensor* out);
+rten_status rten_b200_hard_swish(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
 /* Communicator of a batch-sharded run (one process per GPU).  The reference has no counterpart (single process, rayon
  * threads); it exists so that DynamicQuantizeLinear can use the range of the WHOLE tensor when the batch is split over
  * ranks.  NCCL (libnccl.so.2) is resolved with dlopen at the first call; rank 0 creates the 128-byte id, the host
@@ -547,13 +590,17 @@ rten_status rten_b200_scatter_rows(rten_ctx* ctx, rten_tensor* table, const rten
 /* ---- model loading and graph execution (SURVEY.md 8f-3 / 8f-4) ------------------------------------------------- */
 /* `Model::load` + `Graph::run_plan` (src/model.rs, src/graph.rs:880-1286) for the hot-path operator set: the ONNX file is
  * decoded by a hand-written wire-format reader (rten-onnx/src/onnx.rs), int64 tensors become i32 as in rten's loader,
- * constants are uploaded to HBM once, Conv + Relu and MatMul + Add(bias) are fused at load (the subset of
- * src/optimize.rs these models need), constant weights are prepacked once (`Operator::prepack`, src/graph.rs:488-565).
+ * constants are uploaded to HBM once, Mul(x, Sigmoid(x)) becomes Silu (SiluFusion: either operand order, only when the
+ * Sigmoid has no other consumer), then Conv + {Relu, Sigmoid, Silu, HardSigmoid, HardSwish} and MatMul + Add(bias) are
+ * fused at load (the subset of src/optimize.rs these models need; Clip is not fused), constant weights are prepacked
+ * once (`Operator::prepack`, src/graph.rs:488-565).
  * A run executes the nodes in topological order, one operator call of this library each; temporaries are reference
- * counted and return to the context pool after their last consumer; Relu / Gelu / Erf / Softmax run in place when the
+ * counted and return to the context pool after their last consumer; Relu / Clip / Gelu / Erf / Sigmoid / HardSigmoid /
+ * HardSwish / Softmax run in place when the
  * executor holds the last reference to their input (src/graph.rs:973-1049); Reshape / Flatten / Squeeze / Unsqueeze /
  * Transpose / Identity are views.  Operators: Conv, ConvInteger, ConvTranspose (constant weights prepacked at load; a
- * node that sets output_shape fails the load), Relu, MaxPool, GlobalAveragePool, ReduceMean (spatial axes), Gemm, MatMul, MatMulInteger, Add, Mul, Softmax, LayerNormalization, Gelu, Erf, Gather (rows), Cast (i32 -> f32),
+ * node that sets output_shape fails the load), Relu, Clip, Sigmoid, HardSigmoid (alpha / beta, defaults 0.2 / 0.5),
+ * HardSwish, MaxPool, GlobalAveragePool, ReduceMean (spatial axes), Gemm, MatMul, MatMulInteger, Add, Mul, Softmax, LayerNormalization, Gelu, Erf, Gather (rows), Cast (i32 -> f32),
  * DynamicQuantizeLinear, Attention (4-D), MatMulNBits (com.microsoft, bits 4; constant B / scales used in place),
  * RotaryEmbedding, GroupQueryAttention (com.microsoft; output and present_key / present_value, inputs 12-15 rejected;
  * the executor allocates new present caches, so each decode step also copies the past: two launches, not one),

@@ -5,7 +5,7 @@ The product is `librten_b200.so` (hand-written CUDA behind the C ABI in include/
 runners and bench.py.  There is no CPU implementation in this package."""
 from . import _lib  # noqa: F401
 from .ops import (  # noqa: F401
-    ACT_GELU, ACT_GELU_TANH, ACT_NONE, ACT_RELU, Add, AddSoftmax, Attention, Clip, Comm, Context, Conv, ConvInteger, ConvIntegerToFloat,
-    ConvTranspose, DeviceTensor, DynamicQuantizeLinear, Erf, FusedMatMul, GatherRows, Gelu, Gemm, GlobalAveragePool, GroupQueryAttention, GRU,
-    LayerNormalization, LSTM, MatMul, MatMulInteger, MatMulIntegerToFloat, MatMulNBits, MaxPool, Mul, MultiHeadAttention, OpError, Packed, QuantizedLinear, Relu, RotaryEmbedding, ScatterRows, Softmax, from_torch,
+    ACT_GELU, ACT_GELU_TANH, ACT_HARD_SIGMOID, ACT_HARD_SWISH, ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_SILU, Add, AddSoftmax, Attention, Clip, Comm, Context, Conv, ConvInteger, ConvIntegerToFloat,
+    ConvTranspose, DeviceTensor, DynamicQuantizeLinear, Erf, FusedMatMul, GatherRows, Gelu, Gemm, GlobalAveragePool, GroupQueryAttention, GRU, HardSigmoid, HardSwish,
+    LayerNormalization, LSTM, MatMul, MatMulInteger, MatMulIntegerToFloat, MatMulNBits, MaxPool, Mul, MultiHeadAttention, OpError, Packed, QuantizedLinear, Relu, RotaryEmbedding, ScatterRows, Sigmoid, Silu, Softmax, from_torch,
 )

@@ -73,6 +73,10 @@ class RtenMhaParams(C.Structure):
     _fields_ = [("num_heads", C.c_int32), ("scale", C.c_float), ("mask_filter_value", C.c_float), ("unidirectional", C.c_int32)]
 
 
+class RtenActivation(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("alpha", C.c_float), ("beta", C.c_float)]
+
+
 class RtenRnnParams(C.Structure):
     _fields_ = [("direction", C.c_int32), ("hidden_size", C.c_int32), ("linear_before_reset", C.c_int32)]
 
@@ -112,6 +116,7 @@ _SIGNATURES = {
     "rten_b200_matmul_nbits": (C.c_int, [_vp, _TP, _TP, _TP, C.c_int, C.c_int, _TP]),
     "rten_b200_conv2d": (C.c_int, [_vp, _TP, _TP, _vp, _TP, C.POINTER(RtenConvParams), _TP]),
     "rten_b200_conv2d_ex": (C.c_int, [_vp, _TP, _TP, _vp, _TP, C.POINTER(RtenConvParams), _TP, C.c_int, _TP]),
+    "rten_b200_conv2d_act": (C.c_int, [_vp, _TP, _TP, _vp, _TP, C.POINTER(RtenConvParams), _TP, C.POINTER(RtenActivation), _TP]),
     "rten_b200_conv2d_projected": (C.c_int, [_vp, _TP, _TP, _vp, _TP, C.POINTER(RtenConvParams), _TP, _TP, _vp, _TP,
                                              C.POINTER(RtenConvParams), C.c_int, _TP]),
     "rten_b200_conv2d_chained": (C.c_int, [_vp, _TP, _TP, _vp, _TP, C.POINTER(RtenConvParams), _TP, _TP, _TP, _vp, _TP,
@@ -140,6 +145,10 @@ _SIGNATURES = {
     "rten_b200_comm_uses_peer_memory": (C.c_int, [_vp]),
     "rten_b200_comm_timeouts": (C.c_int, [_vp]),
     "rten_b200_relu": (C.c_int, [_vp, _TP, _TP]),
+    "rten_b200_sigmoid": (C.c_int, [_vp, _TP, _TP]),
+    "rten_b200_silu": (C.c_int, [_vp, _TP, _TP]),
+    "rten_b200_hard_sigmoid": (C.c_int, [_vp, _TP, C.c_float, C.c_float, _TP]),
+    "rten_b200_hard_swish": (C.c_int, [_vp, _TP, _TP]),
     "rten_b200_clip": (C.c_int, [_vp, _TP, _TP, _TP, _TP]),
     "rten_b200_add": (C.c_int, [_vp, _TP, _TP, _TP]),
     "rten_b200_mul": (C.c_int, [_vp, _TP, _TP, _TP]),

@@ -30,7 +30,8 @@ struct ConvArgs {
     const rten_tensor* bias = nullptr;
     const rten_conv_params* p;
     const rten_tensor* residual = nullptr;
-    int act = 0;
+    int act = 0;                              // apply_act code (math.cuh)
+    float act_alpha = 0.0f, act_beta = 0.0f;  // HardSigmoid's alpha / beta (act 6)
     const rten_tensor* x_zp = nullptr;
     const rten_tensor* w_zp = nullptr;
     const rten_tensor* scale = nullptr;
@@ -385,6 +386,8 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
             for (int i = 0; i < 4; i++) d.rs[i] = res_v.strides[i];
         }
         d.act = A.act;
+        d.act_alpha = A.act_alpha;
+        d.act_beta = A.act_beta;
         if (A.kind == 1) {
             d.x_zp = A.x_zp ? xz_v.data : nullptr;
             d.w_zp = A.w_zp ? wz_v.data : nullptr;
@@ -440,6 +443,8 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
     auto epilogue = [&](EpilogueDesc& e, int64_t c0) {
         epi_out(e, ov, c0);
         e.act = A.act;
+        e.act_alpha = A.act_alpha;
+        e.act_beta = A.act_beta;
         if (A.bias) {
             e.bias = (const float*)bias_c.data + c0;
             e.bias_kind = 1;
@@ -663,7 +668,8 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
             if (A.residual) {
                 long long rs4[4] = {res_v.strides[0], res_v.strides[2], res_v.strides[3], res_v.strides[1]};
                 RTB_TRY(launch_nd_add(ctx, (const float*)tmp, e.r, (float*)e.d, 4, shape, ss, rs4, ds, A.act == 1));
-                if (A.act > 1) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "gelu after residual needs a pixel-contiguous output");
+                if (A.act > 1)
+                    return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "an activation other than Relu after a residual needs a pixel-contiguous output");
             } else {
                 RTB_TRY(launch_nd_copy(ctx, 4, tmp, e.d, 4, shape, ss, ds));
             }
@@ -1177,13 +1183,15 @@ rten_status rten_b200_prepack_conv_weight(rten_ctx* ctx, const rten_tensor* w, i
 }
 
 // ---- Conv family ----------------------------------------------------------------------------
-rten_status rten_b200_conv2d_ex(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w, const rten_packed* pw,
-                                const rten_tensor* bias, const rten_conv_params* p, const rten_tensor* residual,
-                                int activation, rten_tensor* out) {
+rten_status rten_b200_conv2d_act(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w, const rten_packed* pw,
+                                 const rten_tensor* bias, const rten_conv_params* p, const rten_tensor* residual,
+                                 const rten_activation* act, rten_tensor* out) {
     RTB_TRY(check_ctx(ctx));
     if (!x || !w || !p || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
     if (x->dtype != RTEN_F32 || w->dtype != RTEN_F32 || (bias && bias->dtype != RTEN_F32))
         return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    if (act && (act->kind < RTEN_ACT_NONE || act->kind > RTEN_ACT_HARD_SWISH))
+        return fail(ctx, RTEN_ERR_INVALID_VALUE, "unknown activation");
     OpScope sc(ctx);
     ConvArgs A{};
     A.kind = 0;
@@ -1193,8 +1201,21 @@ rten_status rten_b200_conv2d_ex(rten_ctx* ctx, const rten_tensor* x, const rten_
     A.bias = bias;
     A.p = p;
     A.residual = residual;
-    A.act = activation;
+    if (act) {
+        A.act = act->kind;
+        A.act_alpha = act->alpha;
+        A.act_beta = act->beta;
+    }
     return sc.finish(conv_core(sc, A, out));
+}
+
+rten_status rten_b200_conv2d_ex(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w, const rten_packed* pw,
+                                const rten_tensor* bias, const rten_conv_params* p, const rten_tensor* residual,
+                                int activation, rten_tensor* out) {
+    RTB_TRY(check_ctx(ctx));
+    if (activation < RTEN_ACT_NONE || activation > RTEN_ACT_GELU_TANH) return fail(ctx, RTEN_ERR_INVALID_VALUE, "unknown activation");
+    const rten_activation a = {activation, 0.0f, 0.0f};
+    return rten_b200_conv2d_act(ctx, x, w, pw, bias, p, residual, &a, out);
 }
 
 rten_status rten_b200_conv2d_projected(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* w, const rten_packed* pw,
@@ -1205,6 +1226,7 @@ rten_status rten_b200_conv2d_projected(rten_ctx* ctx, const rten_tensor* x, cons
     if (!x || !w || !p || !x_proj || !w_proj || !p_proj || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
     for (const rten_tensor* t : {x, w, bias, x_proj, w_proj, bias_proj})
         if (t && t->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    if (activation < RTEN_ACT_NONE || activation > RTEN_ACT_GELU_TANH) return fail(ctx, RTEN_ERR_INVALID_VALUE, "unknown activation");
     OpScope sc(ctx);
     ConvArgs M{}, P{};
     M.kind = P.kind = 0;
@@ -1235,6 +1257,8 @@ rten_status rten_b200_conv2d_chained(rten_ctx* ctx, const rten_tensor* x, const 
     if (residual && x_proj) return fail(ctx, RTEN_ERR_INVALID_VALUE, "a residual and a projection shortcut are exclusive");
     for (const rten_tensor* t : {x, w, bias, residual, x_proj, w_proj, bias_proj, w_next, bias_next})
         if (t && t->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    for (int a : {activation, activation_next})
+        if (a < RTEN_ACT_NONE || a > RTEN_ACT_GELU_TANH) return fail(ctx, RTEN_ERR_INVALID_VALUE, "unknown activation");
     OpScope sc(ctx);
     ConvArgs M{}, P{}, Nx{};
     M.kind = P.kind = Nx.kind = 0;

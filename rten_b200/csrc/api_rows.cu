@@ -259,13 +259,14 @@ rten_status elementwise_op(OpScope& sc, const rten_tensor* x, rten_tensor* out, 
 }
 }  // extern "C++"
 
-static rten_status unary_op(rten_ctx* ctx, int op, const rten_tensor* x, rten_tensor* out) {
+static rten_status unary_op(rten_ctx* ctx, int op, const rten_tensor* x, rten_tensor* out, float alpha = 0.0f,
+                            float beta = 0.0f) {
     RTB_TRY(check_ctx(ctx));
     if (!x || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
     if (x->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
     OpScope sc(ctx);
     return sc.finish(elementwise_op(sc, x, out, [&](const void* a, void* y, long long n) {
-        return launch_unary(ctx, op, (const float*)a, (float*)y, n);
+        return launch_unary(ctx, op, (const float*)a, (float*)y, n, alpha, beta);
     }));
 }
 
@@ -293,6 +294,14 @@ rten_status rten_b200_gelu(rten_ctx* ctx, const rten_tensor* x, int approximate,
     return unary_op(ctx, approximate ? UNARY_APPROX_GELU : UNARY_GELU, x, out);
 }
 rten_status rten_b200_relu(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out) { return unary_op(ctx, UNARY_RELU, x, out); }
+rten_status rten_b200_sigmoid(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out) { return unary_op(ctx, UNARY_SIGMOID, x, out); }
+rten_status rten_b200_silu(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out) { return unary_op(ctx, UNARY_SILU, x, out); }
+rten_status rten_b200_hard_sigmoid(rten_ctx* ctx, const rten_tensor* x, float alpha, float beta, rten_tensor* out) {
+    return unary_op(ctx, UNARY_HARD_SIGMOID, x, out, alpha, beta);
+}
+rten_status rten_b200_hard_swish(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out) {
+    return unary_op(ctx, UNARY_HARD_SWISH, x, out);
+}
 
 // ---- Add ----------------------------------------------------------------------------------------------
 // Add / Mul with numpy broadcasting (src/ops/binary_elementwise.rs); flags: 0 = Add, 2 = Mul

@@ -31,10 +31,13 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kSmemMax = 48 * 1024;  // weights of a channel slice; larger kernels shrink the slice
 
-enum { OUT_F32 = 0, OUT_I32 = 1, OUT_QF32 = 2 };  // f32 conv; ConvInteger; ConvIntegerToFloat
+// f32 conv; ConvInteger; ConvIntegerToFloat; f32 conv followed by Sigmoid, Silu, HardSigmoid or HardSwish (apply_act
+// codes 4-7: a kernel of their own, since their exp and divisions in every output loop slow the codes 0-3 by ~2%)
+enum { OUT_F32 = 0, OUT_I32 = 1, OUT_QF32 = 2, OUT_F32_ACT = 3 };
+__host__ __device__ constexpr bool f32_out(int out) { return out == OUT_F32 || out == OUT_F32_ACT; }
 
 template <int OUT>
-using AccT = typename std::conditional<OUT == OUT_F32, float, unsigned>::type;
+using AccT = typename std::conditional<f32_out(OUT), float, unsigned>::type;
 
 __device__ __forceinline__ int ordered_f32(float f) {  // the encoding of EpilogueDesc::range
     const int i = __float_as_int(f);
@@ -69,7 +72,7 @@ __device__ __forceinline__ void mac(AccT<OUT> (&acc)[VEC], const XT (&xv)[VEC], 
                                     const int (&wz)[VEC]) {
 #pragma unroll
     for (int k = 0; k < VEC; k++) {
-        if constexpr (OUT == OUT_F32)
+        if constexpr (f32_out(OUT))
             acc[k] = __fadd_rn(acc[k], __fmul_rn(xv[k], wv[k]));
         else  // |x - xz|, |w - wz| <= 255: the product is exact, the sum wraps
             acc[k] += (unsigned)(((int)xv[k] - xz) * ((int)wv[k] - wz[k]));
@@ -80,7 +83,7 @@ template <int OUT, int VEC>
 __device__ __forceinline__ void init_acc(const DepthwiseParams& p, int c0, int n, AccT<OUT> (&acc)[VEC]) {
 #pragma unroll
     for (int k = 0; k < VEC; k++) {
-        if constexpr (OUT == OUT_F32)
+        if constexpr (f32_out(OUT))
             acc[k] = (p.bias && k < n) ? __ldg(p.bias + (long long)(c0 + k) * p.bias_stride) : 0.0f;
         else
             acc[k] = 0u;
@@ -92,7 +95,7 @@ __device__ __forceinline__ void zero_points(const DepthwiseParams& p, int c0, in
     xz = 0;
 #pragma unroll
     for (int k = 0; k < VEC; k++) wz[k] = 0;
-    if constexpr (OUT != OUT_F32) {
+    if constexpr (!f32_out(OUT)) {
         if (p.x_zp) xz = (int)__ldg(reinterpret_cast<const XT*>(p.x_zp));
         if (p.w_zp) {
 #pragma unroll
@@ -120,14 +123,17 @@ __device__ __forceinline__ void epilogue(const DepthwiseParams& p, AccT<OUT> (&a
             y[k] = acc[k];
         } else {
             float v;
-            if constexpr (OUT == OUT_F32) {
+            if constexpr (f32_out(OUT)) {
                 v = acc[k];
             } else {
                 v = __fmul_rn(__int2float_rn((int)acc[k]), sv);
                 if (p.bias && k < n) v = __fadd_rn(v, __ldg(p.bias + (long long)(c0 + k) * p.bias_stride));
             }
             if (p.res && k < n) v = __fadd_rn(v, __ldg(p.res + roff + k * p.rs[1]));
-            v = apply_act(v, p.act);
+            if constexpr (OUT == OUT_F32_ACT)
+                v = apply_act(v, p.act, p.act_alpha, p.act_beta);
+            else
+                v = apply_act(v, p.act);
             if constexpr (OUT == OUT_QF32) {
                 if (k < n) {
                     lo = fminf(lo, v);
@@ -326,7 +332,8 @@ rten_status launch_int_w(rten_ctx* ctx, const DepthwiseParams& p) {
 
 rten_status launch_depthwise(rten_ctx* ctx, const DepthwiseParams& p) {
     if ((long long)p.B * p.C * p.OH * p.OW == 0) return RTEN_OK;
-    if (p.x_dtype == RTEN_F32) return launch_typed<float, float, OUT_F32>(ctx, p);
+    if (p.x_dtype == RTEN_F32)
+        return p.act > 3 ? launch_typed<float, float, OUT_F32_ACT>(ctx, p) : launch_typed<float, float, OUT_F32>(ctx, p);
     return p.x_dtype == RTEN_I8 ? launch_int_w<int8_t>(ctx, p) : launch_int_w<uint8_t>(ctx, p);
 }
 

@@ -21,6 +21,7 @@ struct DepthwiseParams {
     const float* res = nullptr;  // residual laid out like out (its own strides)
     long long rs[4] = {0, 0, 0, 0};
     int act = 0;  // apply_act code (integer outputs: 0 or 1)
+    float act_alpha = 0.0f, act_beta = 0.0f;  // HardSigmoid's (act 6)
     // ConvInteger: zero points in their own 8-bit type, read on the device; w_zp one per channel (w_zp_stride apart) or a
     // scalar (stride 0)
     const void* x_zp = nullptr;

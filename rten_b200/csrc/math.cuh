@@ -208,12 +208,43 @@ __device__ __forceinline__ float approx_gelu_ref(float x) {
     return __fmul_rn(half_x, y);
 }
 
+// Sigmoid / Silu (rten-vecmath/src/exp.rs:201-228): 1 / (1 + exp(0 - x)) and x / (1 + exp(0 - x)) -- Silu is ONE
+// division, not x * Sigmoid(x).  exp_ref is inf from 104 on, so Silu(x <= -104) = -0 and Silu(-inf) = -inf / inf = NaN.
+__device__ __forceinline__ float sigmoid_ref(float x) {
+    return __fdiv_rn(1.0f, __fadd_rn(1.0f, exp_ref(__fsub_rn(0.0f, x))));
+}
+__device__ __forceinline__ float silu_ref(float x) { return __fdiv_rn(x, __fadd_rn(1.0f, exp_ref(__fsub_rn(0.0f, x)))); }
+
+// Rust's f32::clamp(0, 1): `<` / `>` comparisons, so NaN passes through and -0.0 stays -0.0 (fminf / fmaxf would not)
+__device__ __forceinline__ float clamp01_ref(float v) {
+    if (v < 0.0f) v = 0.0f;
+    if (v > 1.0f) v = 1.0f;
+    return v;
+}
+// HardSigmoid / HardSwish (src/ops/unary_elementwise.rs:437-469): product and sum each rounded (Rust does not contract)
+__device__ __forceinline__ float hard_sigmoid_ref(float x, float alpha, float beta) {
+    return clamp01_ref(__fadd_rn(__fmul_rn(alpha, x), beta));
+}
+__device__ __forceinline__ float hard_swish_ref(float x) { return __fmul_rn(x, hard_sigmoid_ref(x, 1.0f / 6.0f, 0.5f)); }
+
+// Activation codes of the fused epilogues: 0 none, 1 Relu, 2 Gelu, 3 Gelu (tanh), 4 Sigmoid, 5 Silu, 6 HardSigmoid
+// (alpha, beta), 7 HardSwish.  Codes 0-3 only: the decode GEMV kernels (skinny.cu), whose operators take no others.
 __device__ __forceinline__ float apply_act(float v, int act) {
     switch (act) {
         case 1: return v > 0.0f ? v : 0.0f;
         case 2: return gelu_ref(v);
         case 3: return approx_gelu_ref(v);
         default: return v;
+    }
+}
+// Every code; alpha / beta are read by code 6 only.
+__device__ __forceinline__ float apply_act(float v, int act, float alpha, float beta) {
+    switch (act) {
+        case 4: return sigmoid_ref(v);
+        case 5: return silu_ref(v);
+        case 6: return hard_sigmoid_ref(v, alpha, beta);
+        case 7: return hard_swish_ref(v);
+        default: return apply_act(v, act);
     }
 }
 

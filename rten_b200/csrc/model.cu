@@ -2,13 +2,15 @@
 // `Graph::run_plan` do around the operators of this library (src/model.rs, src/graph.rs:880-1286), restated for the
 // hot-path operator set:
 //   load : ONNX bytes -> nodes + initialisers (onnx_reader.cu; int64 tensors become i32 like rten's loader does) ->
-//          constants uploaded to HBM once -> load-time fusions (Conv + Relu, MatMul + Add(bias): the subset of
-//          src/optimize.rs the models need) -> weights prepacked once (`Operator::prepack`, src/graph.rs:488-565).
+//          constants uploaded to HBM once -> load-time fusions (Mul(x, Sigmoid(x)) -> Silu, then Conv + activation
+//          and MatMul + Add(bias): the subset of src/optimize.rs the models need) -> weights prepacked once
+//          (`Operator::prepack`, src/graph.rs:488-565).
 //   run  : the nodes in topological (file) order, one C-ABI operator call each; temporaries are reference counted and
 //          returned to the context pool after their last consumer (src/graph.rs:1100-1180); an operator that can run in
 //          place does so when the executor holds the last reference to its input (src/graph.rs:973-1049); shape-only
 //          operators (Reshape, Flatten, Squeeze, Unsqueeze, Transpose, Identity) are views -- no kernel, no copy.
-// Operators: Conv, ConvInteger, ConvTranspose (without output_shape), Relu, Clip, MaxPool, GlobalAveragePool, ReduceMean, Gemm, MatMul, MatMulInteger, MatMulNBits
+// Operators: Conv, ConvInteger, ConvTranspose (without output_shape), Relu, Clip, Sigmoid, HardSigmoid, HardSwish,
+// MaxPool, GlobalAveragePool, ReduceMean, Gemm, MatMul, MatMulInteger, MatMulNBits
 // (com.microsoft), Add, Mul, Softmax, LayerNormalization, Gelu, Erf, Gather, Cast, DynamicQuantizeLinear, Attention,
 // RotaryEmbedding, GroupQueryAttention and MultiHeadAttention (com.microsoft, three outputs), GRU and LSTM, Constant and
 // the view operators.
@@ -51,7 +53,7 @@ struct OpNode {
     onnx::Node n;
     std::vector<int> in, out;  // value ids (-1 = absent optional input)
     rten_packed* packed = nullptr;
-    int activation = 0;        // fused Relu
+    rten_activation activation = {RTEN_ACT_NONE, 0.0f, 0.0f};  // fused activation of a Conv
     int bias_value = -1;       // fused Add(bias) of a MatMul
 };
 
@@ -152,7 +154,7 @@ rten_status upload_constant(rten_model* m, const onnx::Tensor& t, ValueSlot* v) 
 
 const std::set<std::string>& supported_ops() {
     static const std::set<std::string> s = {
-        "Conv", "ConvTranspose", "Relu", "Clip", "MaxPool", "GlobalAveragePool", "ReduceMean", "Reshape", "Flatten", "Squeeze", "Unsqueeze", "Transpose",
+        "Conv", "ConvTranspose", "Relu", "Clip", "Sigmoid", "HardSigmoid", "HardSwish", "MaxPool", "GlobalAveragePool", "ReduceMean", "Reshape", "Flatten", "Squeeze", "Unsqueeze", "Transpose",
         "Identity", "Gemm", "MatMul", "Add", "Mul", "Softmax", "LayerNormalization", "Gelu", "Erf", "Gather",
         "DynamicQuantizeLinear", "MatMulInteger", "ConvInteger", "Cast", "Attention", "MatMulNBits", "GroupQueryAttention",
         "MultiHeadAttention", "RotaryEmbedding", "GRU", "LSTM", "Constant"};
@@ -204,7 +206,23 @@ bool is_view_op(const std::string& op) {
     return op == "Reshape" || op == "Flatten" || op == "Squeeze" || op == "Unsqueeze" || op == "Transpose" || op == "Identity";
 }
 bool is_in_place_op(const std::string& op) {
-    return op == "Relu" || op == "Clip" || op == "Gelu" || op == "Erf" || op == "Softmax";
+    return op == "Relu" || op == "Clip" || op == "Gelu" || op == "Erf" || op == "Softmax" || op == "Sigmoid" || op == "Silu" ||
+           op == "HardSigmoid" || op == "HardSwish";
+}
+
+// HardSigmoid's attributes with the reference's defaults (src/op_registry/onnx_registry.rs:1228-1232)
+float hard_sigmoid_alpha(const onnx::Node& n) { return n.attr_f("alpha", 0.2f); }
+float hard_sigmoid_beta(const onnx::Node& n) { return n.attr_f("beta", 0.5f); }
+
+// The activation node `n` as a fused Conv epilogue, or RTEN_ACT_NONE for any other node (Clip is not fused)
+rten_activation conv_activation(const onnx::Node& n) {
+    const std::string& op = n.op_type;
+    if (op == "Relu") return {RTEN_ACT_RELU, 0.0f, 0.0f};
+    if (op == "Sigmoid") return {RTEN_ACT_SIGMOID, 0.0f, 0.0f};
+    if (op == "Silu") return {RTEN_ACT_SILU, 0.0f, 0.0f};
+    if (op == "HardSigmoid") return {RTEN_ACT_HARD_SIGMOID, hard_sigmoid_alpha(n), hard_sigmoid_beta(n)};
+    if (op == "HardSwish") return {RTEN_ACT_HARD_SWISH, 0.0f, 0.0f};
+    return {RTEN_ACT_NONE, 0.0f, 0.0f};
 }
 
 rten_status fill_conv_params(rten_ctx* ctx, const onnx::Node& n, rten_conv_params* p) {
@@ -392,7 +410,7 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
             return mfail(ctx, RTEN_ERR_INVALID_VALUE, "graph output '" + vi.name + "' is never produced");
         m->outputs.push_back(it->second);
     }
-    // ---- load-time fusions (src/optimize.rs: the two patterns the hot-path models contain)
+    // ---- load-time fusions (src/optimize.rs: the patterns the hot-path models contain)
     auto consumers = [&](int vid) {
         int c = 0;
         for (const OpNode& o : m->nodes)
@@ -402,6 +420,26 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
             if (o == vid) c++;
         return c;
     };
+    // SiluFusion (src/optimize/fusions.rs:567-588): Mul(x, Sigmoid(x)), either operand order, becomes Silu(x) when the
+    // Sigmoid's output has no other consumer.  Silu rounds once where Mul(x, Sigmoid(x)) rounds twice, so the reference's
+    // Model::run computes Silu.  First, because the Sigmoid and the Mul are two consumers of a Conv's output.
+    for (size_t i = m->nodes.size(); i-- > 0;) {  // (backwards: erasing node i keeps the indices still to visit)
+        OpNode& s = m->nodes[i];
+        if (s.n.op_type != "Sigmoid" || s.in.size() != 1 || s.out.size() != 1 || consumers(s.out[0]) != 1) continue;
+        size_t j = i + 1;
+        for (; j < m->nodes.size(); j++)
+            if (std::find(m->nodes[j].in.begin(), m->nodes[j].in.end(), s.out[0]) != m->nodes[j].in.end()) break;
+        if (j == m->nodes.size()) continue;
+        OpNode& mul = m->nodes[j];
+        if (mul.n.op_type != "Mul" || mul.in.size() != 2 || mul.out.size() != 1) continue;
+        const int x = s.in[0];
+        if (!((mul.in[0] == s.out[0] && mul.in[1] == x) || (mul.in[1] == s.out[0] && mul.in[0] == x))) continue;
+        mul.n.op_type = "Silu";
+        mul.n.inputs = {s.n.inputs[0]};
+        mul.n.attrs.clear();
+        mul.in = {x};
+        m->nodes.erase(m->nodes.begin() + (long)i);
+    }
     for (size_t i = 0; i + 1 < m->nodes.size(); i++) {
         OpNode& a = m->nodes[i];
         if (a.out.size() != 1 || consumers(a.out[0]) != 1) continue;
@@ -411,8 +449,8 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
             if (std::find(m->nodes[j].in.begin(), m->nodes[j].in.end(), a.out[0]) != m->nodes[j].in.end()) break;
         if (j == m->nodes.size()) continue;
         OpNode& b = m->nodes[j];
-        if (a.n.op_type == "Conv" && b.n.op_type == "Relu" && a.activation == 0) {
-            a.activation = 1;  // Relu in the convolution epilogue
+        if (a.n.op_type == "Conv" && a.activation.kind == RTEN_ACT_NONE && conv_activation(b.n).kind != RTEN_ACT_NONE) {
+            a.activation = conv_activation(b.n);  // the activation in the convolution epilogue
             a.out = b.out;
             m->nodes.erase(m->nodes.begin() + (long)j);
         } else if (a.n.op_type == "MatMul" && b.n.op_type == "Add" && a.bias_value < 0 && b.in.size() == 2) {
@@ -677,7 +715,7 @@ struct Runner {
             rten_conv_params p;
             RTB_TRY(fill_conv_params(ctx, o.n, &p));
             if (op == "Conv")
-                st = rten_b200_conv2d_ex(ctx, T(0), T(1), o.packed, T(2), &p, nullptr, o.activation, &y);
+                st = rten_b200_conv2d_act(ctx, T(0), T(1), o.packed, T(2), &p, nullptr, &o.activation, &y);
             else
                 st = rten_b200_conv_integer(ctx, T(0), T(1), o.packed, T(2), T(3), nullptr, &p, &y);
         } else if (op == "ConvTranspose") {
@@ -688,6 +726,14 @@ struct Runner {
             st = rten_b200_relu(ctx, T(0), &y);
         } else if (op == "Clip") {
             st = rten_b200_clip(ctx, T(0), T(1), T(2), &y);
+        } else if (op == "Sigmoid") {
+            st = rten_b200_sigmoid(ctx, T(0), &y);
+        } else if (op == "Silu") {
+            st = rten_b200_silu(ctx, T(0), &y);
+        } else if (op == "HardSigmoid") {
+            st = rten_b200_hard_sigmoid(ctx, T(0), hard_sigmoid_alpha(o.n), hard_sigmoid_beta(o.n), &y);
+        } else if (op == "HardSwish") {
+            st = rten_b200_hard_swish(ctx, T(0), &y);
         } else if (op == "Gelu") {
             const onnx::Attribute* a = o.n.attr("approximate");
             st = rten_b200_gelu(ctx, T(0), (a && a->s == "tanh") ? 1 : 0, &y);

@@ -23,10 +23,6 @@ namespace {
 constexpr int RNN_THREADS = 256;
 constexpr int RNN_MAX_SMEM = 227 * 1024;  // sm_90 opt-in shared memory per block
 
-__device__ __forceinline__ float sigmoid_ref(float x) {
-    return __fdiv_rn(1.0f, __fadd_rn(1.0f, exp_ref(__fsub_rn(0.0f, x))));
-}
-
 // Inputs of one (direction, batch row, hidden unit) update.  xg: x . W^T of the G gates; rec: h . R^T of the G gates.
 template <bool GRU>
 __device__ __forceinline__ void gate_update(const RnnLaunch& L, int d, int j, const float* xg, const float* rec, float& h,

@@ -551,34 +551,39 @@ rten_status launch_row_mean(rten_ctx* ctx, const float* x, float* y, long long r
 }
 
 // =========================================================================================
-// Elementwise (contiguous): Erf, Gelu, ApproxGelu, Relu, and same-shape Add (+ optional Relu)
-// 128-bit loads/stores, grid sized to fill the SMs.
+// Elementwise (contiguous): Erf, Gelu, ApproxGelu, Relu, Sigmoid, Silu, HardSigmoid, HardSwish, and same-shape Add
+// (+ optional Relu).  128-bit loads/stores, grid sized to fill the SMs.
 // =========================================================================================
 template <int OP>
-__device__ __forceinline__ float unary_apply(float v) {
+__device__ __forceinline__ float unary_apply(float v, float alpha, float beta) {
     if (OP == UNARY_ERF) return erf_ref(v);
     if (OP == UNARY_GELU) return gelu_ref(v);
     if (OP == UNARY_APPROX_GELU) return approx_gelu_ref(v);
+    if (OP == UNARY_SIGMOID) return sigmoid_ref(v);
+    if (OP == UNARY_SILU) return silu_ref(v);
+    if (OP == UNARY_HARD_SIGMOID) return hard_sigmoid_ref(v, alpha, beta);
+    if (OP == UNARY_HARD_SWISH) return hard_swish_ref(v);
     return v > 0.0f ? v : 0.0f;  // UNARY_RELU
 }
 
+// (x and y may be the same buffer: every element is read once, by the thread that writes it, before it is written)
 template <int OP>
 __global__ void __launch_bounds__(256)
-unary_kernel(const float* __restrict__ x, float* __restrict__ y, long long n, int vec) {
+unary_kernel(const float* __restrict__ x, float* __restrict__ y, long long n, int vec, float alpha, float beta) {
     const long long n4 = vec ? (n >> 2) : 0;
     const long long stride = (long long)gridDim.x * blockDim.x;
     long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     for (; i < n4; i += stride) {
         float4 v = reinterpret_cast<const float4*>(x)[i];
-        v.x = unary_apply<OP>(v.x);
-        v.y = unary_apply<OP>(v.y);
-        v.z = unary_apply<OP>(v.z);
-        v.w = unary_apply<OP>(v.w);
+        v.x = unary_apply<OP>(v.x, alpha, beta);
+        v.y = unary_apply<OP>(v.y, alpha, beta);
+        v.z = unary_apply<OP>(v.z, alpha, beta);
+        v.w = unary_apply<OP>(v.w, alpha, beta);
         reinterpret_cast<float4*>(y)[i] = v;
     }
     // tail (everything when the buffers are not 16-B aligned)
     for (long long j = (n4 << 2) + (long long)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride)
-        y[j] = unary_apply<OP>(x[j]);
+        y[j] = unary_apply<OP>(x[j], alpha, beta);
 }
 
 static int ew_grid(rten_ctx* ctx, long long work_items) {
@@ -589,15 +594,20 @@ static int ew_grid(rten_ctx* ctx, long long work_items) {
     return (int)blocks;
 }
 
-rten_status launch_unary(rten_ctx* ctx, int op, const float* x, float* y, long long n) {
+rten_status launch_unary(rten_ctx* ctx, int op, const float* x, float* y, long long n, float alpha, float beta) {
     if (n == 0) return RTEN_OK;
     const int vec = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0 ? 1 : 0;
     const int grid = ew_grid(ctx, vec ? (n + 3) / 4 : n);
+    auto go = [&](auto kernel) { kernel<<<grid, 256, 0, ctx->stream>>>(x, y, n, vec, alpha, beta); };
     switch (op) {
-        case UNARY_ERF: unary_kernel<UNARY_ERF><<<grid, 256, 0, ctx->stream>>>(x, y, n, vec); break;
-        case UNARY_GELU: unary_kernel<UNARY_GELU><<<grid, 256, 0, ctx->stream>>>(x, y, n, vec); break;
-        case UNARY_APPROX_GELU: unary_kernel<UNARY_APPROX_GELU><<<grid, 256, 0, ctx->stream>>>(x, y, n, vec); break;
-        case UNARY_RELU: unary_kernel<UNARY_RELU><<<grid, 256, 0, ctx->stream>>>(x, y, n, vec); break;
+        case UNARY_ERF: go(unary_kernel<UNARY_ERF>); break;
+        case UNARY_GELU: go(unary_kernel<UNARY_GELU>); break;
+        case UNARY_APPROX_GELU: go(unary_kernel<UNARY_APPROX_GELU>); break;
+        case UNARY_RELU: go(unary_kernel<UNARY_RELU>); break;
+        case UNARY_SIGMOID: go(unary_kernel<UNARY_SIGMOID>); break;
+        case UNARY_SILU: go(unary_kernel<UNARY_SILU>); break;
+        case UNARY_HARD_SIGMOID: go(unary_kernel<UNARY_HARD_SIGMOID>); break;
+        case UNARY_HARD_SWISH: go(unary_kernel<UNARY_HARD_SWISH>); break;
         default: return fail(ctx, RTEN_ERR_INVALID_VALUE, "unknown unary op");
     }
     cudaError_t e = cudaGetLastError();

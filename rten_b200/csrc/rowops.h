@@ -7,7 +7,16 @@
 
 namespace rtb {
 
-enum { UNARY_ERF = 0, UNARY_GELU = 1, UNARY_APPROX_GELU = 2, UNARY_RELU = 3 };
+enum {
+    UNARY_ERF = 0,
+    UNARY_GELU = 1,
+    UNARY_APPROX_GELU = 2,
+    UNARY_RELU = 3,
+    UNARY_SIGMOID = 4,
+    UNARY_SILU = 5,
+    UNARY_HARD_SIGMOID = 6,  // alpha * x + beta, clamped
+    UNARY_HARD_SWISH = 7
+};
 
 // Softmax over the last (contiguous) axis of x viewed as [rows, n]; optional mask broadcast over
 // up to 4 leading dims: row index is decomposed over lead[0..nlead) (row-major), mask element =
@@ -23,7 +32,8 @@ rten_status launch_layer_norm(rten_ctx* ctx, const float* x, float* y, long long
 // x + (r / rows_inner) * s_outer + (r % rows_inner) * s_inner, elements kstride apart.
 rten_status launch_row_mean(rten_ctx* ctx, const float* x, float* y, long long rows, int n, long long rows_inner,
                             long long s_outer, long long s_inner, long long kstride);
-rten_status launch_unary(rten_ctx* ctx, int op, const float* x, float* y, long long n);
+// y may be x; alpha / beta are read by UNARY_HARD_SIGMOID only
+rten_status launch_unary(rten_ctx* ctx, int op, const float* x, float* y, long long n, float alpha = 0.0f, float beta = 0.0f);
 // Clip of n contiguous f32 (or i32) elements; y may be x; mn / mx: device scalars of the same type, or null
 rten_status launch_clip(rten_ctx* ctx, int is_i32, const void* x, void* y, long long n, const void* mn, const void* mx);
 rten_status launch_nd_copy(rten_ctx* ctx, int esize, const void* src, void* dst, int ndim, const long long* shape,

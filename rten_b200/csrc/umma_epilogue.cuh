@@ -46,9 +46,10 @@ __device__ __forceinline__ uint32_t* staged_word(uint8_t* rowp, int sw, int j) {
 // named barrier of one epilogue group (128 threads)
 __device__ __forceinline__ void group_sync(int grp) { asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory"); }
 
-// Gelu / ApproxGelu of four f32 bit patterns in place (the out-of-line act4)
-__device__ __forceinline__ void act4_bits(uint32_t& a, uint32_t& b, uint32_t& c, uint32_t& d, int act) {
-    const float4 g = act4(make_float4(__uint_as_float(a), __uint_as_float(b), __uint_as_float(c), __uint_as_float(d)), act);
+// The activation (any code above Relu) of four f32 bit patterns in place (the out-of-line act4)
+__device__ __forceinline__ void act4_bits(uint32_t& a, uint32_t& b, uint32_t& c, uint32_t& d, const EpilogueDesc& e) {
+    const float4 g = act4(make_float4(__uint_as_float(a), __uint_as_float(b), __uint_as_float(c), __uint_as_float(d)),
+                          e.act, e.act_alpha, e.act_beta);
     a = __float_as_uint(g.x);
     b = __float_as_uint(g.y);
     c = __float_as_uint(g.z);
@@ -155,7 +156,7 @@ struct GenericEpi : RangedEpi {
                     if (e.r) x = fmaf(e.r_scale, __ldcg(e.r + r_off + (long long)n * e.r_col), x);
                     if (e.bias_kind == 1) x += e.bias[n];
                     x += row_bias;
-                    *sp = __float_as_uint(apply_act(x, e.act));
+                    *sp = __float_as_uint(apply_act(x, e.act, e.act_alpha, e.act_beta));
                 } else {
                     // exact i32 arithmetic with wrap-around (unsigned ops)
                     unsigned c = *sp;
@@ -171,7 +172,7 @@ struct GenericEpi : RangedEpi {
                         float x = __fmul_rn(__int2float_rn((int)c), sv);
                         if (e.bias_kind == 1) x = __fadd_rn(x, e.bias[n]);
                         if (e.r) x = __fadd_rn(x, __ldcg(e.r + r_off + (long long)n * e.r_col));
-                        *sp = __float_as_uint(apply_act(x, e.act));
+                        *sp = __float_as_uint(apply_act(x, e.act, e.act_alpha, e.act_beta));
                     } else {
                         *sp = c;
                     }
@@ -227,7 +228,7 @@ struct FastEpi : RangedEpi {
                     x = x + b4[u];
                     v[j + u] = __float_as_uint(do_relu ? fmaxf(x, 0.0f) : x);
                 }
-                if (GELU && e.act > 1) act4_bits(v[j], v[j + 1], v[j + 2], v[j + 3], e.act);
+                if (GELU && e.act > 1) act4_bits(v[j], v[j + 1], v[j + 2], v[j + 3], e);
             }
         } else if (e.za || e.za8 || e.zb || e.scale) {
             // exact i32 arithmetic with wrap-around (unsigned ops), column vectors fetched 128 bits at a time
@@ -276,7 +277,7 @@ struct FastEpi : RangedEpi {
                         v[j + u] = c;
                     }
                 }
-                if (GELU && e.scale && e.act > 1) act4_bits(v[j], v[j + 1], v[j + 2], v[j + 3], e.act);
+                if (GELU && e.scale && e.act > 1) act4_bits(v[j], v[j + 1], v[j + 2], v[j + 3], e);
             }
         }
         if (e.range && row_ok) {
@@ -318,7 +319,7 @@ struct PlainF32Epi : EpiBase {
             const float4 bb = bq[j >> 2];  // (zeros without a bias: x + 0 keeps the generic path's -0 -> +0)
             plain_f32_pair(v[j], v[j + 1], p.res_tma, make_float2(rr.x, rr.y), make_float2(bb.x, bb.y), p.epi.act == 1);
             plain_f32_pair(v[j + 2], v[j + 3], p.res_tma, make_float2(rr.z, rr.w), make_float2(bb.z, bb.w), p.epi.act == 1);
-            if (GELU) act4_bits(v[j], v[j + 1], v[j + 2], v[j + 3], p.epi.act);
+            if (GELU) act4_bits(v[j], v[j + 1], v[j + 2], v[j + 3], p.epi);
         }
     }
 };
@@ -402,7 +403,7 @@ struct PlainI8Epi : RangedEpi {
                 f2 = __float_as_uint(fmaxf(__uint_as_float(f2), 0.0f));
                 f3 = __float_as_uint(fmaxf(__uint_as_float(f3), 0.0f));
             }
-            if (GELU) act4_bits(f0, f1, f2, f3, e.act);  // Gelu / ApproxGelu after the integer product
+            if (GELU) act4_bits(f0, f1, f2, f3, e);  // Gelu / ApproxGelu after the integer product
             v[j] = f0;
             v[j + 1] = f1;
             v[j + 2] = f2;

@@ -181,8 +181,8 @@ static Epi pick_epilogue(const GemmLaunch& L, int tma_store, int res_tma, int sp
         fast = fast && (!(e.za || e.za8) || aligned(e.colsum)) && (!e.zb || e.zb_len == 1 || (e.zb_len == L.N && aligned(e.zb))) &&
                (!e.scale || e.scale_len == 1 || (e.scale_len == L.N && aligned(e.scale)));
     if (!fast) return Epi::Generic;
-    const bool gelu = e.act > 1;
-    if (!getenv("RTEN_B200_NO_PLAIN") && e.act <= 3) {
+    const bool gelu = e.act > 1;  // every activation but Relu: the out-of-line act4 of the *Gelu variants
+    if (!getenv("RTEN_B200_NO_PLAIN") && e.act <= 7) {
         // f32: alpha = 1, optional column bias, residual with r_scale = 1, no range output
         if (L.kind == 0 && e.alpha == 1.0f && !e.range && (e.r == nullptr || e.r_scale == 1.0f))
             return gelu ? Epi::PlainF32Gelu : Epi::PlainF32;
@@ -214,7 +214,7 @@ static bool plan_shape(const Prepared& q, const Plan& pl, PlanShape& ps) {
     if (pl.splitk < 1) return false;  // (recorded plans are read from a text file: no division by zero, no negative units)
     if (is_wide(pl.bn)) {
         if ((pl.bn != 128 && pl.bn != 256) || !q.wide || pl.splitk != 1) return false;
-        if (pl.bn == 256 && q.p.epi.act > 1) return false;  // Gelu: 128-column tiles only (umma_wide_kernel)
+        if (pl.bn == 256 && q.p.epi.act > 1) return false;  // act4 (Gelu and up): 128-column tiles only (umma_wide_kernel)
     } else if (pl.bn < 16 || pl.bn % 32 || pl.bn % q.step) {
         return false;
     }

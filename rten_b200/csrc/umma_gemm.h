@@ -37,7 +37,8 @@ struct EpilogueDesc {
     int bias_kind = 0;  // 1: per column n, 2: per row m
     const float* bias2 = nullptr;  // bias_kind 1, plain f32 epilogue only: a second column bias, added to `bias` first
     float alpha = 1.0f;
-    int act = 0;  // 0 none, 1 relu, 2 gelu(erf), 3 gelu(tanh)
+    int act = 0;  // apply_act code (math.cuh): 0 none, 1 relu, 2 gelu(erf), 3 gelu(tanh), 4-7 sigmoid, silu, hard
+                  // sigmoid (act_alpha, act_beta), hard swish
     // integer path: C = acc - za[m % za_len]*colsum[n] - zb[n % zb_len]*rowsum[m] + K*za*zb
     const int32_t* za = nullptr;
     int za_len = 0;
@@ -55,6 +56,9 @@ struct EpilogueDesc {
     int* range = nullptr;
     const float* scale2 = nullptr;    // optional scalar factor: the effective scale is fmul(scale2[0], scale[n]) -- the
                                       // graph's Mul(x_scale, w_scale) node folded into the epilogue, same rounding
+    // HardSigmoid's alpha / beta (act 6).  Last in the struct, which is last in KParams: the kernel parameter offsets
+    // of every other field stay where they were.
+    float act_alpha = 0.0f, act_beta = 0.0f;
 };
 
 struct ConvGeom {

@@ -50,7 +50,8 @@ struct FastDiv {
 };
 
 // Epilogue variants of umma_gemm_kernel (umma_epilogue.cuh); the host picks one per launch (pick_epilogue).  The wide
-// kernel runs the plain f32 epilogue only.
+// kernel runs the plain f32 epilogue only.  A "Gelu" variant is the one with the out-of-line activation call (act4):
+// it runs every activation code above Relu, not only Gelu.
 enum class Epi { Generic, Fast, FastGelu, PlainF32, PlainF32Gelu, PlainI8, PlainI8Gelu };
 
 struct KParams {
@@ -170,19 +171,20 @@ __device__ __forceinline__ void range_commit(int* range, float lo, float hi) {
     }
 }
 
-// Gelu (erf / tanh form) of four values as an out-of-line call: the specialised epilogue stays short straight-line
-// code (an unrolled polynomial per element would multiply its size and thrash the instruction cache), yet Gelu no
-// longer forces a launch into the generic epilogue.
-__device__ __noinline__ float4 act4(float4 x, int act) {
+// Every activation but Relu (Gelu, its tanh form, Sigmoid, Silu, HardSigmoid, HardSwish) of four values as an
+// out-of-line call: the specialised epilogue stays short straight-line code (an unrolled polynomial per element would
+// multiply its size and thrash the instruction cache), yet these activations do not force a launch into the generic
+// epilogue.  The "Gelu" epilogue variants (Epi::*Gelu) are the ones that make this call.
+__device__ __noinline__ float4 act4(float4 x, int act, float alpha, float beta) {
     if (act == 2) {  // Gelu: two lanes per packed instruction (bit-identical to gelu_ref, math.cuh)
         gelu_ref_x2(x.x, x.y);
         gelu_ref_x2(x.z, x.w);
         return x;
     }
-    x.x = apply_act(x.x, act);
-    x.y = apply_act(x.y, act);
-    x.z = apply_act(x.z, act);
-    x.w = apply_act(x.w, act);
+    x.x = apply_act(x.x, act, alpha, beta);
+    x.y = apply_act(x.y, act, alpha, beta);
+    x.z = apply_act(x.z, act, alpha, beta);
+    x.w = apply_act(x.w, act, alpha, beta);
     return x;
 }
 
@@ -593,10 +595,11 @@ __device__ __forceinline__ void wide_main_loop(const KParams& p, const SmemLayou
 
 // Columns 32k .. 32k + 31 of a wide accumulator (fragment rows row0, row0 + 8; columns 8j + 2cq + {0, 1}) through
 // plain_f32_pair -- residual from the staging buffer, bias from `bias` (the chunk's 32 values), Relu -- then act4 for
-// Gelu, into the 128-row, 128B-swizzled staging buffer `stg`.  `valid` = false (a chunk past N) stores d unchanged.
+// the other activations, into the 128-row, 128B-swizzled staging buffer `stg`.  `valid` = false (a chunk past N)
+// stores d unchanged.
 template <Epi E, int NA>
 __device__ __forceinline__ void stage_chunk(float (&d)[NA], int k, uint8_t* stg, const float* bias, bool valid, bool res,
-                                            int act, int row0, int sw, int cq) {
+                                            int act, int row0, int sw, int cq, float alpha = 0.0f, float beta = 0.0f) {
 #pragma unroll
     for (int j = 0; j < 4; j++) {  // columns 32k + 8j + 2cq + {0, 1}, rows row0 + 8h
         const int i0 = 16 * k + 4 * j;
@@ -615,8 +618,8 @@ __device__ __forceinline__ void stage_chunk(float (&d)[NA], int k, uint8_t* stg,
                 d[i0 + 2 * h] = __uint_as_float(v0);
                 d[i0 + 2 * h + 1] = __uint_as_float(v1);
             }
-            if (E == Epi::PlainF32Gelu) {  // Gelu / ApproxGelu: the out-of-line polynomial, four values per call
-                const float4 g = act4(make_float4(d[i0], d[i0 + 1], d[i0 + 2], d[i0 + 3]), act);
+            if (E == Epi::PlainF32Gelu) {  // the out-of-line activation, four values per call
+                const float4 g = act4(make_float4(d[i0], d[i0 + 1], d[i0 + 2], d[i0 + 3]), act, alpha, beta);
                 d[i0] = g.x;
                 d[i0 + 1] = g.y;
                 d[i0 + 2] = g.z;
@@ -684,7 +687,7 @@ __device__ __forceinline__ void wide_consumer(const KParams& p, const SmemLayout
                 rphase ^= 1u << buf;
             }
             // (a tile may overhang N by whole chunks: the TMA store clips them)
-            stage_chunk<E>(d, k, stg, bias_s + 32 * k, nbase < p.N, p.res_tma, e.act, row0, sw, cq);
+            stage_chunk<E>(d, k, stg, bias_s + 32 * k, nbase < p.N, p.res_tma, e.act, row0, sw, cq, e.act_alpha, e.act_beta);
             fence_proxy_async();
             consumers_sync();
             if (issuer) {

@@ -18,7 +18,7 @@ from typing import Optional, Sequence
 import numpy as np
 
 from . import _lib
-from ._lib import (RTEN_DEVICE_HOST, RTEN_F32, RTEN_I8, RTEN_I32, RTEN_U8, RtenAttentionParams, RtenConvParams,
+from ._lib import (RTEN_DEVICE_HOST, RTEN_F32, RTEN_I8, RTEN_I32, RTEN_U8, RtenActivation, RtenAttentionParams, RtenConvParams,
                    RtenConvTransposeParams, RtenGqaParams, RtenMhaParams, RtenTensor, RtenRnnParams)
 
 _NP2RT = {np.dtype(np.float32): RTEN_F32, np.dtype(np.int32): RTEN_I32, np.dtype(np.int8): RTEN_I8,
@@ -26,6 +26,9 @@ _NP2RT = {np.dtype(np.float32): RTEN_F32, np.dtype(np.int32): RTEN_I32, np.dtype
 _RT2NP = {v: k for k, v in _NP2RT.items()}
 
 ACT_NONE, ACT_RELU, ACT_GELU, ACT_GELU_TANH = 0, 1, 2, 3
+# activations fused into a Conv epilogue through Conv(activation=...) only (rten_b200_conv2d_act); ACT_HARD_SIGMOID takes
+# (alpha, beta): pass (ACT_HARD_SIGMOID, alpha, beta), or the code alone for the ONNX defaults
+ACT_SIGMOID, ACT_SILU, ACT_HARD_SIGMOID, ACT_HARD_SWISH = 4, 5, 6, 7
 
 
 class OpError(Exception):
@@ -604,10 +607,19 @@ def _conv_params(padding, groups, strides, dilations) -> RtenConvParams:
     return p
 
 
-class Conv:
-    """src/ops/conv.rs:367-419: attributes groups, dilations, padding ('same' or [t,l,b,r]), strides."""
+def _activation(activation) -> RtenActivation:
+    """An ACT_* code, or (kind, alpha, beta), as the rten_activation struct.  A bare code takes HardSigmoid's ONNX
+    defaults (0.2, 0.5), which the other kinds ignore."""
+    kind, alpha, beta = tuple(activation) if isinstance(activation, (tuple, list)) else (activation, 0.2, 0.5)
+    return RtenActivation(int(kind), float(alpha), float(beta))
 
-    def __init__(self, groups=1, dilations=(1, 1), padding=(0, 0, 0, 0), strides=(1, 1), activation: int = ACT_NONE):
+
+class Conv:
+    """src/ops/conv.rs:367-419: attributes groups, dilations, padding ('same' or [t,l,b,r]), strides.  `activation`: an
+    ACT_* code or (kind, alpha, beta), applied in the convolution's epilogue (run / run_projected / run_chained take the
+    codes ACT_NONE .. ACT_GELU_TANH; run takes every kind)."""
+
+    def __init__(self, groups=1, dilations=(1, 1), padding=(0, 0, 0, 0), strides=(1, 1), activation=ACT_NONE):
         self.groups, self.dilations, self.padding, self.strides = groups, tuple(dilations), padding, tuple(strides)
         self.activation = activation
 
@@ -623,8 +635,9 @@ class Conv:
         A = _Args(ctx)
         o = A.out(out)
         p = _conv_params(self.padding, self.groups, self.strides, self.dilations)
-        ctx.check(ctx.lib.rten_b200_conv2d_ex(ctx.handle, A.t(x), A.t(w), _ph(packed_w), A.t(bias), C.byref(p),
-                                              A.t(residual), self.activation, C.byref(o)))
+        act = _activation(self.activation)
+        ctx.check(ctx.lib.rten_b200_conv2d_act(ctx.handle, A.t(x), A.t(w), _ph(packed_w), A.t(bias), C.byref(p),
+                                               A.t(residual), C.byref(act), C.byref(o)))
         return A.wrap(o, out)
 
     def run_projected(self, ctx, x, w, bias=None, packed_w: Optional[Packed] = None, *, proj: "Conv", x_proj, w_proj,
@@ -816,6 +829,37 @@ class Gelu(_Unary):
 class Relu(_Unary):
     def _call(self, ctx, x, o):
         return ctx.lib.rten_b200_relu(ctx.handle, x, o)
+
+
+class Sigmoid(_Unary):
+    """rten-vecmath/src/exp.rs:201-212: 1 / (1 + exp(0 - x))"""
+
+    def _call(self, ctx, x, o):
+        return ctx.lib.rten_b200_sigmoid(ctx.handle, x, o)
+
+
+class Silu(_Unary):
+    """exp.rs:217-228: x / (1 + exp(0 - x)), one division -- what the reference runs for Mul(x, Sigmoid(x))"""
+
+    def _call(self, ctx, x, o):
+        return ctx.lib.rten_b200_silu(ctx.handle, x, o)
+
+
+class HardSigmoid(_Unary):
+    """src/ops/unary_elementwise.rs:437-449: clamp(alpha * x + beta, 0, 1)"""
+
+    def __init__(self, alpha=0.2, beta=0.5):
+        self.alpha, self.beta = alpha, beta
+
+    def _call(self, ctx, x, o):
+        return ctx.lib.rten_b200_hard_sigmoid(ctx.handle, x, float(self.alpha), float(self.beta), o)
+
+
+class HardSwish(_Unary):
+    """src/ops/unary_elementwise.rs:457-469: x * clamp(x / 6 + 0.5, 0, 1)"""
+
+    def _call(self, ctx, x, o):
+        return ctx.lib.rten_b200_hard_swish(ctx.handle, x, o)
 
 
 class Clip:
