@@ -517,6 +517,23 @@ rten_status rten_b200_softmax(rten_ctx* ctx, const rten_tensor* x, const rten_te
 /* LayerNormalization (src/ops/norm.rs:437-569); epsilon < 0 => default 1e-5. */
 rten_status rten_b200_layer_norm(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* scale,
                                  const rten_tensor* bias_or_null, int axis, float epsilon, rten_tensor* out);
+/* RMSNormalization / SimplifiedLayerNormalization (src/ops/norm.rs rms_normalization): layer_normalization_impl with
+ * DynamicRootMeanSquare -- mean 0, rstd = scale / sqrt(SumSquare / n + epsilon), no bias.  `scale` broadcasts to the
+ * normalized axes [axis, ndim), or is a scalar when it has one element; epsilon < 0 => default 1e-5.  `out` must be
+ * contiguous (allocated when out->data == NULL).  Bit-identical to the reference. */
+rten_status rten_b200_rms_norm(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* scale, int axis, float epsilon,
+                               rten_tensor* out);
+/* com.microsoft SkipLayerNormalization (rms == 0) and SkipSimplifiedLayerNormalization (rms != 0), src/ops/norm/contrib.rs:
+ * s = (x + skip) + bias, two rounded adds; out = LayerNormalization (or RMSNormalization) of s over the last axis with
+ * gamma and, for SkipLayerNormalization only, beta (beta_or_null must be NULL when rms != 0).  x is [B, S, H] or [S, H];
+ * skip has the same trailing two dims and broadcasts over the batch ([B, S, H], [1, S, H] or [S, H]); gamma, beta and
+ * bias are 1-D.  sum_out_or_null receives s (the operator's output 3, input_skip_bias_sum).  The reference's error
+ * statuses and messages, with one deviation: a bias whose length is neither H nor 1 returns RTEN_ERR_INVALID_VALUE
+ * (the reference panics).  Outputs must be contiguous.  Bit-identical to the reference, one kernel launch for dense
+ * device-resident operands (capturable in a CUDA graph), no temporary beyond the outputs. */
+rten_status rten_b200_skip_layer_norm(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* skip, const rten_tensor* gamma,
+                                      const rten_tensor* beta_or_null, const rten_tensor* bias_or_null, float epsilon, int rms,
+                                      rten_tensor* out, rten_tensor* sum_out_or_null);
 /* Clip (src/ops/unary_elementwise.rs:249-333), f32 or i32: x.max(min).min(max) with `a > b ? a : b` comparisons, so
  * NaN becomes min and -0.0 clipped at min = 0 becomes +0.0.  min / max are scalar tensors of x's type (NULL: the type's
  * finite minimum / maximum), read on the device: no host synchronisation, capturable in a CUDA graph.  `out` may alias
@@ -600,7 +617,10 @@ rten_status rten_b200_scatter_rows(rten_ctx* ctx, rten_tensor* table, const rten
  * executor holds the last reference to their input (src/graph.rs:973-1049); Reshape / Flatten / Squeeze / Unsqueeze /
  * Transpose / Identity are views.  Operators: Conv, ConvInteger, ConvTranspose (constant weights prepacked at load; a
  * node that sets output_shape fails the load), Relu, Clip, Sigmoid, HardSigmoid (alpha / beta, defaults 0.2 / 0.5),
- * HardSwish, MaxPool, GlobalAveragePool, ReduceMean (spatial axes), Gemm, MatMul, MatMulInteger, Add, Mul, Softmax, LayerNormalization, Gelu, Erf, Gather (rows), Cast (i32 -> f32),
+ * HardSwish, MaxPool, GlobalAveragePool, ReduceMean (spatial axes), Gemm, MatMul, MatMulInteger, Add, Mul, Softmax, LayerNormalization,
+ * RMSNormalization and SimplifiedLayerNormalization (stash_type 1), SkipLayerNormalization and
+ * SkipSimplifiedLayerNormalization (com.microsoft; outputs 0 and 3: a missing epsilon or a named mean / inv_std_var output
+ * fails the load), Gelu, Erf, Gather (rows), Cast (i32 -> f32),
  * DynamicQuantizeLinear, Attention (4-D), MatMulNBits (com.microsoft, bits 4; constant B / scales used in place),
  * RotaryEmbedding, GroupQueryAttention (com.microsoft; output and present_key / present_value, inputs 12-15 rejected;
  * the executor allocates new present caches, so each decode step also copies the past: two launches, not one),

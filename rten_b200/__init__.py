@@ -7,5 +7,6 @@ from . import _lib  # noqa: F401
 from .ops import (  # noqa: F401
     ACT_GELU, ACT_GELU_TANH, ACT_HARD_SIGMOID, ACT_HARD_SWISH, ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_SILU, Add, AddSoftmax, Attention, Clip, Comm, Context, Conv, ConvInteger, ConvIntegerToFloat,
     ConvTranspose, DeviceTensor, DynamicQuantizeLinear, Erf, FusedMatMul, GatherRows, Gelu, Gemm, GlobalAveragePool, GroupQueryAttention, GRU, HardSigmoid, HardSwish,
-    LayerNormalization, LSTM, MatMul, MatMulInteger, MatMulIntegerToFloat, MatMulNBits, MaxPool, Mul, MultiHeadAttention, OpError, Packed, QuantizedLinear, Relu, RotaryEmbedding, ScatterRows, Sigmoid, Silu, Softmax, from_torch,
+    LayerNormalization, LSTM, MatMul, MatMulInteger, MatMulIntegerToFloat, MatMulNBits, MaxPool, Mul, MultiHeadAttention, OpError, Packed, QuantizedLinear, Relu, RMSNormalization, RotaryEmbedding, ScatterRows, Sigmoid,
+    SimplifiedLayerNormalization, Silu, SkipLayerNormalization, SkipSimplifiedLayerNormalization, Softmax, from_torch,
 )

@@ -126,6 +126,38 @@ rten_status rten_b200_softmax(rten_ctx* ctx, const rten_tensor* x, const rten_te
 }
 
 // ---- LayerNormalization -------------------------------------------------------------------------
+// A scale / bias of the normalization over x's dims [ax, ndim) (src/ops/norm.rs layer_normalization_impl): one element
+// stays a scalar (`item()`), read on the device later; anything else is broadcast to the normalized shape and
+// materialised contiguous, or fails with `err`.
+static rten_status norm_param(OpScope& sc, const rten_tensor& pv, const rten_tensor& xv, int ax, const char* err,
+                              const float** ptr, bool* is_scalar) {
+    if (numel(&pv) == 1) {
+        *is_scalar = true;
+        *ptr = (const float*)pv.data;
+        return RTEN_OK;
+    }
+    *is_scalar = false;
+    const int nn = xv.ndim - ax;  // normalized dims
+    if (pv.ndim > nn) return fail(sc.ctx, RTEN_ERR_INVALID_VALUE, err);
+    rten_tensor b = pv;
+    b.ndim = nn;
+    for (int i = 0; i < nn; i++) {
+        const int pi = i - (nn - pv.ndim);
+        const int64_t want = xv.shape[ax + i];
+        b.shape[i] = want;
+        if (pi < 0 || pv.shape[pi] == 1)
+            b.strides[i] = 0;
+        else if (pv.shape[pi] == want)
+            b.strides[i] = pv.strides[pi];
+        else
+            return fail(sc.ctx, RTEN_ERR_INVALID_VALUE, err);
+    }
+    rten_tensor c;
+    RTB_TRY(sc.contiguous(&b, &c));
+    *ptr = (const float*)c.data;
+    return RTEN_OK;
+}
+
 rten_status rten_b200_layer_norm(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* scale, const rten_tensor* bias,
                                  int axis, float epsilon, rten_tensor* out) {
     RTB_TRY(check_ctx(ctx));
@@ -141,41 +173,11 @@ rten_status rten_b200_layer_norm(rten_ctx* ctx, const rten_tensor* x, const rten
     rten_status st = sc.in(x, &xv);
     if (st == RTEN_OK) st = sc.in(scale, &sv);
     if (st == RTEN_OK && bias) st = sc.in(bias, &bv);
-    const int nn = nd - ax;  // normalized dims
-    // broadcast a parameter to the normalized shape, materialised contiguous; scalars stay scalar
-    auto param = [&](const rten_tensor& pv, const char* err, const float** ptr, float* scalar, bool* is_scalar) -> rten_status {
-        if (numel(&pv) == 1) {
-            // scale.item(): read on device later -> use a 1-element broadcast with stride 0
-            *is_scalar = true;
-            *ptr = (const float*)pv.data;
-            (void)scalar;
-            return RTEN_OK;
-        }
-        *is_scalar = false;
-        if (pv.ndim > nn) return fail(ctx, RTEN_ERR_INVALID_VALUE, err);
-        rten_tensor b = pv;
-        b.ndim = nn;
-        for (int i = 0; i < nn; i++) {
-            const int pi = i - (nn - pv.ndim);
-            const int64_t want = xv.shape[ax + i];
-            b.shape[i] = want;
-            if (pi < 0 || pv.shape[pi] == 1)
-                b.strides[i] = 0;
-            else if (pv.shape[pi] == want)
-                b.strides[i] = pv.strides[pi];
-            else
-                return fail(ctx, RTEN_ERR_INVALID_VALUE, err);
-        }
-        rten_tensor c;
-        RTB_TRY(sc.contiguous(&b, &c));
-        *ptr = (const float*)c.data;
-        return RTEN_OK;
-    };
     const float *gp = nullptr, *bp = nullptr;
     float gs = 1.0f, bs = 0.0f;
     bool g_scalar = false, b_scalar = false;
-    if (st == RTEN_OK) st = param(sv, "`scale` is not broadcastable to normalized axes of input", &gp, &gs, &g_scalar);
-    if (st == RTEN_OK && bias) st = param(bv, "`bias` is not broadcastable to normalized axes of input", &bp, &bs, &b_scalar);
+    if (st == RTEN_OK) st = norm_param(sc, sv, xv, ax, "`scale` is not broadcastable to normalized axes of input", &gp, &g_scalar);
+    if (st == RTEN_OK && bias) st = norm_param(sc, bv, xv, ax, "`bias` is not broadcastable to normalized axes of input", &bp, &b_scalar);
     if (st == RTEN_OK) st = sc.contiguous(&xv, &xc);
     if (st == RTEN_OK) st = sc.out(out, RTEN_F32, nd, xv.shape, &ov, nullptr);
     if (st == RTEN_OK && numel(&xv) > 0) {
@@ -212,6 +214,134 @@ rten_status rten_b200_layer_norm(rten_ctx* ctx, const rten_tensor* x, const rten
             }
             st = launch_nd_copy(ctx, 4, yc.data, ov.data, nd, shape, ss, ds);
         }
+    }
+    return sc.finish(st);
+}
+
+// ---- RMSNormalization and the skip layer norms ------------------------------------------------------
+// Row stride of x viewed as rows over its dims [ax, ndim), when those are packed (element stride 1) and the leading
+// dims step uniformly; false for any other layout.
+static bool row_stride(const rten_tensor& t, int ax, long long* rs) {
+    long long s = 1;
+    for (int i = t.ndim - 1; i >= ax; i--) {
+        if (t.shape[i] != 1 && t.strides[i] != s) return false;
+        s *= t.shape[i];
+    }
+    long long step = -1, span = 1;  // stride of the row index; rows spanned by the dims after i
+    for (int i = ax - 1; i >= 0; i--) {
+        if (t.shape[i] == 1) continue;
+        if (step < 0) {
+            step = t.strides[i];
+        } else if (t.strides[i] != step * span) {
+            return false;
+        }
+        span *= t.shape[i];
+    }
+    *rs = step < 0 ? s : step;
+    return true;
+}
+
+// x as rows for the kernels: a device view, a contiguous copy when the layout has no single row stride
+static rten_status norm_rows(OpScope& sc, const rten_tensor& xv, int ax, rten_tensor* xr, long long* rs) {
+    if (row_stride(xv, ax, rs)) {
+        *xr = xv;
+        return RTEN_OK;
+    }
+    RTB_TRY(sc.contiguous(&xv, xr));
+    return row_stride(*xr, ax, rs) ? RTEN_OK : fail(sc.ctx, RTEN_ERR_INVALID_VALUE, "row view");
+}
+
+static rten_status norm_out(OpScope& sc, rten_tensor* o, const rten_tensor& xv, rten_tensor* ov) {
+    RTB_TRY(sc.out(o, RTEN_F32, xv.ndim, xv.shape, ov, nullptr));
+    return is_contiguous(ov) ? RTEN_OK : fail(sc.ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "normalization outputs must be contiguous");
+}
+
+rten_status rten_b200_rms_norm(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* scale, int axis, float epsilon,
+                               rten_tensor* out) {
+    RTB_TRY(check_ctx(ctx));
+    if (!x || !scale || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    if (x->dtype != RTEN_F32 || scale->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    const int nd = x->ndim;
+    if (axis < -nd || axis >= std::max(nd, 1)) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Axis is invalid");
+    const int ax = axis < 0 ? axis + nd : axis;
+    OpScope sc(ctx);
+    rten_tensor xv, sv, xr, ov;
+    SkipNormParams p;
+    p.eps = epsilon < 0.0f ? 1e-5f : epsilon;
+    p.rms = 1;
+    bool g_scalar = false;
+    rten_status st = sc.in(x, &xv);
+    if (st == RTEN_OK) st = sc.in(scale, &sv);
+    if (st == RTEN_OK) st = norm_param(sc, sv, xv, ax, "`scale` is not broadcastable to normalized axes of input", &p.gamma, &g_scalar);
+    if (st == RTEN_OK) st = norm_out(sc, out, xv, &ov);
+    if (st == RTEN_OK && numel(&xv) > 0) {
+        st = norm_rows(sc, xv, ax, &xr, &p.xs);
+        if (g_scalar) std::swap(p.gamma, p.gamma_sp);
+        long long n = 1;
+        for (int i = ax; i < nd; i++) n *= xv.shape[i];
+        p.x = (const float*)xr.data;
+        p.y = (float*)ov.data;
+        p.n = (int)n;
+        p.rows = numel(&xv) / n;
+        if (st == RTEN_OK) st = launch_skip_norm(ctx, p);
+    }
+    return sc.finish(st);
+}
+
+rten_status rten_b200_skip_layer_norm(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* skip, const rten_tensor* gamma,
+                                      const rten_tensor* beta, const rten_tensor* bias, float epsilon, int rms,
+                                      rten_tensor* out, rten_tensor* sum_out) {
+    RTB_TRY(check_ctx(ctx));
+    if (!x || !skip || !gamma || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    for (const rten_tensor* t : {x, skip, gamma, beta, bias})
+        if (t && t->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    for (const rten_tensor* t : {gamma, beta, bias})
+        if (t && t->ndim != 1) return fail(ctx, RTEN_ERR_CAST_FAILED, "gamma, beta and bias must be 1-D tensors");
+    if (rms && beta) return fail(ctx, RTEN_ERR_INVALID_VALUE, "SkipSimplifiedLayerNormalization has no beta input");
+    // src/ops/norm/contrib.rs skip_layer_normalization
+    const int nd = x->ndim, sd = skip->ndim;
+    if (nd != 2 && nd != 3) return fail(ctx, RTEN_ERR_INVALID_VALUE, "input must be 2 or 3 dimensioned");
+    if (sd != 2 && sd != 3) return fail(ctx, RTEN_ERR_INVALID_VALUE, "skip must be 2 or 3 dimensioned");
+    bool bcast = skip->shape[sd - 1] == x->shape[nd - 1] && skip->shape[sd - 2] == x->shape[nd - 2] && sd <= nd;
+    if (bcast && sd == 3) bcast = skip->shape[0] == x->shape[0] || skip->shape[0] == 1;
+    if (!bcast) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "skip must broadcast to input over the batch dimension");
+    const int64_t H = x->shape[nd - 1];
+    // (the reference panics in add_in_place on any other length)
+    if (bias && bias->shape[0] != H && bias->shape[0] != 1)
+        return fail(ctx, RTEN_ERR_INVALID_VALUE, "bias length must equal the hidden size");
+    OpScope sc(ctx);
+    rten_tensor xv, kv, gv, bev, biv, xr, kr, ov, smv;
+    SkipNormParams p;
+    p.eps = epsilon;
+    p.rms = rms ? 1 : 0;
+    bool g_scalar = false, b_scalar = false;
+    rten_status st = sc.in(x, &xv);
+    if (st == RTEN_OK) st = sc.in(skip, &kv);
+    if (st == RTEN_OK) st = sc.in(gamma, &gv);
+    if (st == RTEN_OK && beta) st = sc.in(beta, &bev);
+    if (st == RTEN_OK && bias) st = sc.in(bias, &biv);
+    const int ax = nd - 1;
+    if (st == RTEN_OK) st = norm_param(sc, gv, xv, ax, "`scale` is not broadcastable to normalized axes of input", &p.gamma, &g_scalar);
+    if (st == RTEN_OK && beta) st = norm_param(sc, bev, xv, ax, "`bias` is not broadcastable to normalized axes of input", &p.beta, &b_scalar);
+    if (st == RTEN_OK) st = norm_out(sc, out, xv, &ov);
+    if (st == RTEN_OK && sum_out) st = norm_out(sc, sum_out, xv, &smv);
+    if (st == RTEN_OK && numel(&xv) > 0) {
+        st = norm_rows(sc, xv, ax, &xr, &p.xs);
+        if (st == RTEN_OK) st = norm_rows(sc, kv, sd - 1, &kr, &p.ss);
+        if (g_scalar) std::swap(p.gamma, p.gamma_sp);
+        if (b_scalar) std::swap(p.beta, p.beta_sp);
+        if (bias) {
+            p.bias = (const float*)biv.data;
+            p.bias_inc = biv.shape[0] == 1 ? 0 : (int)biv.strides[0];
+        }
+        p.x = (const float*)xr.data;
+        p.skip = (const float*)kr.data;
+        p.skip_rows = numel(&kv) / H;
+        p.y = (float*)ov.data;
+        p.sum = sum_out ? (float*)smv.data : nullptr;
+        p.n = (int)H;
+        p.rows = numel(&xv) / H;
+        if (st == RTEN_OK) st = launch_skip_norm(ctx, p);
     }
     return sc.finish(st);
 }

@@ -11,8 +11,9 @@
 //          operators (Reshape, Flatten, Squeeze, Unsqueeze, Transpose, Identity) are views -- no kernel, no copy.
 // Operators: Conv, ConvInteger, ConvTranspose (without output_shape), Relu, Clip, Sigmoid, HardSigmoid, HardSwish,
 // MaxPool, GlobalAveragePool, ReduceMean, Gemm, MatMul, MatMulInteger, MatMulNBits
-// (com.microsoft), Add, Mul, Softmax, LayerNormalization, Gelu, Erf, Gather, Cast, DynamicQuantizeLinear, Attention,
-// RotaryEmbedding, GroupQueryAttention and MultiHeadAttention (com.microsoft, three outputs), GRU and LSTM, Constant and
+// (com.microsoft), Add, Mul, Softmax, LayerNormalization, RMSNormalization, SimplifiedLayerNormalization,
+// SkipLayerNormalization and SkipSimplifiedLayerNormalization (com.microsoft, outputs 0 and 3), Gelu, Erf, Gather, Cast,
+// DynamicQuantizeLinear, Attention, RotaryEmbedding, GroupQueryAttention and MultiHeadAttention (com.microsoft, three outputs), GRU and LSTM, Constant and
 // the view operators.
 #include <cuda_runtime.h>
 
@@ -157,7 +158,8 @@ const std::set<std::string>& supported_ops() {
         "Conv", "ConvTranspose", "Relu", "Clip", "Sigmoid", "HardSigmoid", "HardSwish", "MaxPool", "GlobalAveragePool", "ReduceMean", "Reshape", "Flatten", "Squeeze", "Unsqueeze", "Transpose",
         "Identity", "Gemm", "MatMul", "Add", "Mul", "Softmax", "LayerNormalization", "Gelu", "Erf", "Gather",
         "DynamicQuantizeLinear", "MatMulInteger", "ConvInteger", "Cast", "Attention", "MatMulNBits", "GroupQueryAttention",
-        "MultiHeadAttention", "RotaryEmbedding", "GRU", "LSTM", "Constant"};
+        "MultiHeadAttention", "RotaryEmbedding", "GRU", "LSTM", "Constant", "RMSNormalization", "SimplifiedLayerNormalization",
+        "SkipLayerNormalization", "SkipSimplifiedLayerNormalization"};
     return s;
 }
 
@@ -364,6 +366,21 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
                     return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MultiHeadAttention: past_sequence_length and cache_indirection (inputs 8, 9) are not supported");
             if (n.outputs.size() > 3 && !n.outputs[3].empty())
                 return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MultiHeadAttention: the qk output (3) is not supported");
+        }
+        if (n.op_type == "RMSNormalization" || n.op_type == "SimplifiedLayerNormalization") {  // onnx_registry.rs:1584-1590, 1905-1911
+            if (n.domain == "com.microsoft") return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "unsupported operator com.microsoft." + n.op_type);
+            if (n.attr_i("stash_type", 1) != 1) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, n.op_type + ": stash_type must be 1");
+            for (size_t i = 1; i < n.outputs.size(); i++)
+                if (!n.outputs[i].empty())
+                    return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, n.op_type + ": only the normalized output (0) is supported");
+        }
+        if (n.op_type == "SkipLayerNormalization" || n.op_type == "SkipSimplifiedLayerNormalization") {  // onnx_registry.rs:1918-1932
+            if (n.domain != "com.microsoft") return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "unsupported operator " + n.op_type);
+            if (!n.attr("epsilon")) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, n.op_type + ": missing attribute epsilon");
+            // (the reference returns placeholder zeros for the training statistics, which no inference graph reads)
+            for (size_t i = 1; i < 3 && i < n.outputs.size(); i++)
+                if (!n.outputs[i].empty())
+                    return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, n.op_type + ": the mean and inv_std_var outputs (1, 2) are not supported");
         }
         if (n.op_type == "GRU" || n.op_type == "LSTM") RTB_TRY(check_rnn_attrs(ctx, n));
         if (n.op_type == "ConvTranspose" && n.attr("output_shape"))  // (the reference does not read it)
@@ -788,6 +805,18 @@ struct Runner {
             st = rten_b200_mul(ctx, T(0), T(1), &y);
         } else if (op == "LayerNormalization") {
             st = rten_b200_layer_norm(ctx, T(0), T(1), T(2), (int)o.n.attr_i("axis", -1), o.n.attr_f("epsilon", 1e-5f), &y);
+        } else if (op == "RMSNormalization" || op == "SimplifiedLayerNormalization") {
+            if (!T(1)) return mfail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+            st = rten_b200_rms_norm(ctx, T(0), T(1), (int)o.n.attr_i("axis", -1), o.n.attr_f("epsilon", 1e-5f), &y);
+        } else if (op == "SkipLayerNormalization" || op == "SkipSimplifiedLayerNormalization") {
+            // inputs: x, skip, gamma, beta, bias (SkipLayerNormalization); x, skip, gamma, bias (the simplified one)
+            const bool rms = op == "SkipSimplifiedLayerNormalization";
+            const bool want_sum = o.out.size() > 3 && o.out[3] >= 0;
+            rten_tensor s;
+            memset(&s, 0, sizeof(s));
+            st = rten_b200_skip_layer_norm(ctx, T(0), T(1), T(2), rms ? nullptr : T(3), rms ? T(3) : T(4), o.n.attr_f("epsilon", 0.0f),
+                                           rms ? 1 : 0, &y, want_sum ? &s : nullptr);
+            if (st == RTEN_OK && want_sum) set_owned(o.out[3], s);
         } else if (op == "Gather") {
             if (o.n.attr_i("axis", 0) != 0 || T(0)->ndim != 2)
                 return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Gather: only axis 0 of a 2-D table is supported");

@@ -94,4 +94,38 @@ __device__ __forceinline__ float ln_vec_fold(const float4 (&v)[FMAX], int F, flo
     return __shfl_sync(0xffffffffu, s, base + (S - 1) * 16 + 3);
 }
 
+// The same fold over a row staged in shared memory as F * 16 float4s (n = 64 F), by one whole warp: lane c = lane & 15
+// walks the float4s f = c + 16 k, k < F -- its four chains in ascending i -- and lanes 16..31 repeat lanes 0..15.
+// Every lane returns the total.
+template <bool SQSUB>
+__device__ __forceinline__ float ln_smem_fold(const float4* s4, int F, float off) {
+    const int c = threadIdx.x & 15;
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int k = 0; k < F; k++) {
+        const float4 v = s4[c + 16 * k];
+        acc.x = fold_step<SQSUB>(acc.x, v.x, off);
+        acc.y = fold_step<SQSUB>(acc.y, v.y, off);
+        acc.z = fold_step<SQSUB>(acc.z, v.z, off);
+        acc.w = fold_step<SQSUB>(acc.w, v.w, off);
+    }
+    float4 r = acc;  // acc[0][l] = ((acc[0][l] + acc[1][l]) + acc[2][l]) + acc[3][l], as in ln_vec_fold
+#pragma unroll
+    for (int u = 1; u < 4; u++) {
+        r.x = __fadd_rn(r.x, __shfl_down_sync(0xffffffffu, acc.x, 4 * u));
+        r.y = __fadd_rn(r.y, __shfl_down_sync(0xffffffffu, acc.y, 4 * u));
+        r.z = __fadd_rn(r.z, __shfl_down_sync(0xffffffffu, acc.z, 4 * u));
+        r.w = __fadd_rn(r.w, __shfl_down_sync(0xffffffffu, acc.w, 4 * u));
+    }
+    float s = 0.0f;
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+        const float in = __shfl_up_sync(0xffffffffu, s, 1);
+        if (c == q) {
+            if (q > 0) s = in;
+            s = __fadd_rn(__fadd_rn(__fadd_rn(__fadd_rn(s, r.x), r.y), r.z), r.w);
+        }
+    }
+    return __shfl_sync(0xffffffffu, s, 3);
+}
+
 }  // namespace rtb

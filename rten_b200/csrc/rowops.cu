@@ -466,6 +466,251 @@ rten_status launch_layer_norm(rten_ctx* ctx, const float* x, float* y, long long
     return RTEN_OK;
 }
 
+// =========================================================================================
+// RMSNormalization and the skip layer norms (src/ops/norm.rs layer_normalization_impl, src/ops/norm/contrib.rs).
+// s = (x + skip) + bias, two rounded adds as the reference's `add` then `add_in_place`; the statistics of s in the
+// LayerNormalization kernels' fold order (SumSquare = SumSquareSub at offset 0 for RMS, mean 0); the output through the
+// same three Normalize arms.  Three paths, each one launch and no temporary beyond the outputs:
+//   skip_norm_vec_kernel   n % 64 == 0, n <= 1024, or n % 128 == 0, n <= 2048: the row in the registers of 16 S lanes,
+//                          as layer_norm_vec_kernel
+//   skip_norm_wide_kernel  the other n % 64 == 0, n <= 8192: one CTA per row, s in registers and staged once in shared memory
+//                          for the one-warp fold, rstd broadcast through shared memory
+//   skip_norm_kernel       anything else: one warp per row, s staged in the output row
+// =========================================================================================
+enum { NORM_RMS = 1, NORM_SKIP = 2, NORM_BIAS = 4, NORM_SUM = 8 };
+
+__device__ __forceinline__ float4 add4(float4 a, float4 b) {
+    return make_float4(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z), __fadd_rn(a.w, b.w));
+}
+
+// Normalize's three arms (rten-vecmath/src/normalize.rs:101-169), as in layer_norm_kernel: 0 = scalar scale and bias,
+// 1 = per-element scale, no bias; 2 = the general one (g = 1 without a per-element scale, b = 0 without a per-element bias)
+__device__ __forceinline__ float norm_arm(int mode, float a, float mean, float rstd, float g, float b, float beta_scalar) {
+    if (mode == 0) return __fmaf_rn(__fsub_rn(a, mean), rstd, beta_scalar);
+    if (mode == 1) return __fmul_rn(__fsub_rn(a, mean), __fmul_rn(g, rstd));
+    return __fmaf_rn(__fsub_rn(a, mean), __fmul_rn(g, rstd), __fadd_rn(b, beta_scalar));
+}
+__device__ __forceinline__ float4 norm_arm4(int mode, float4 a, float mean, float rstd, float4 g, float4 b, float bs) {
+    return make_float4(norm_arm(mode, a.x, mean, rstd, g.x, b.x, bs), norm_arm(mode, a.y, mean, rstd, g.y, b.y, bs),
+                       norm_arm(mode, a.z, mean, rstd, g.z, b.z, bs), norm_arm(mode, a.w, mean, rstd, g.w, b.w, bs));
+}
+__device__ __forceinline__ int norm_mode(const SkipNormParams& p, float beta_scalar) {
+    return (!p.gamma && !p.beta) ? 0 : ((p.gamma && !p.beta && beta_scalar == 0.0f) ? 1 : 2);
+}
+
+// float4 f of s for the row: x (+ skip (+ bias))
+template <int FL>
+__device__ __forceinline__ float4 skip_sum4(const float4* x4, const float4* k4, const float4* b4, int f) {
+    float4 a = __ldg(x4 + f);
+    if (FL & NORM_SKIP) a = add4(a, __ldg(k4 + f));
+    if (FL & NORM_BIAS) a = add4(a, __ldg(b4 + f));
+    return a;
+}
+
+template <int FL>
+__device__ __forceinline__ void skip_row_ptrs(const SkipNormParams& p, long long r, const float4*& x4, const float4*& k4) {
+    x4 = reinterpret_cast<const float4*>(p.x + r * p.xs);
+    k4 = (FL & NORM_SKIP) ? reinterpret_cast<const float4*>(p.skip + (r % p.skip_rows) * p.ss) : nullptr;
+}
+
+template <int S, int FMAX, int FL>
+__global__ void __launch_bounds__(128) skip_norm_vec_kernel(const SkipNormParams p) {
+    constexpr int LPR = 16 * S;
+    constexpr int RPW = 32 / LPR;
+    const int lane = threadIdx.x & 31;
+    const int c = lane & 15, seg = (lane >> 4) & (S - 1), rw = lane / LPR;
+    const long long row = ((long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * RPW + rw;
+    const bool live = row < p.rows;
+    const int n = p.n;
+    const int F = n / (64 * S);
+    const long long rr = live ? row : 0;
+    const float4 *x4, *k4;
+    skip_row_ptrs<FL>(p, rr, x4, k4);
+    const float4* b4 = reinterpret_cast<const float4*>(p.bias);
+    float4* s4 = reinterpret_cast<float4*>(p.sum + rr * n);
+    float4 v[FMAX];
+#pragma unroll
+    for (int k = 0; k < FMAX; k++) {
+        if (k < F) {
+            const int f = c + 16 * (seg * F + k);
+            v[k] = skip_sum4<FL>(x4, k4, b4, f);
+            if ((FL & NORM_SUM) && live) s4[f] = v[k];
+        }
+    }
+    const float gamma_scalar = p.gamma_sp ? __ldg(p.gamma_sp) : 1.0f;
+    const float beta_scalar = p.beta_sp ? __ldg(p.beta_sp) : 0.0f;
+    const float mean = (FL & NORM_RMS) ? 0.0f : __fdiv_rn(ln_vec_fold<S, false, FMAX>(v, F, 0.0f, c, seg), (float)n);
+    const float var = __fdiv_rn(ln_vec_fold<S, true, FMAX>(v, F, mean, c, seg), (float)n);
+    const float rstd = __fdiv_rn(gamma_scalar, __fsqrt_rn(__fadd_rn(var, p.eps)));
+    if (!live) return;
+    float4* y4 = reinterpret_cast<float4*>(p.y + rr * n);
+    const float4* g4 = reinterpret_cast<const float4*>(p.gamma);
+    const float4* be4 = reinterpret_cast<const float4*>(p.beta);
+    const int mode = norm_mode(p, beta_scalar);
+#pragma unroll
+    for (int k = 0; k < FMAX; k++) {
+        if (k < F) {
+            const int f = c + 16 * (seg * F + k);
+            const float4 g = p.gamma ? __ldg(g4 + f) : make_float4(1.f, 1.f, 1.f, 1.f);
+            const float4 b = p.beta ? __ldg(be4 + f) : make_float4(0.f, 0.f, 0.f, 0.f);
+            y4[f] = norm_arm4(mode, v[k], mean, rstd, g, b, beta_scalar);
+        }
+    }
+}
+
+constexpr int WIDE_THREADS = 256;
+
+template <int VPT, int FL>
+__global__ void __launch_bounds__(WIDE_THREADS) skip_norm_wide_kernel(const SkipNormParams p) {
+    extern __shared__ float4 srow[];  // the row's s, n / 4 float4s
+    __shared__ float stat[2];
+    const long long row = blockIdx.x;
+    const int n = p.n, n4 = n >> 2, t = threadIdx.x;
+    const float4 *x4, *k4;
+    skip_row_ptrs<FL>(p, row, x4, k4);
+    const float4* b4 = reinterpret_cast<const float4*>(p.bias);
+    float4* s4 = reinterpret_cast<float4*>(p.sum + row * n);
+    float4 v[VPT];
+#pragma unroll
+    for (int k = 0; k < VPT; k++) {
+        const int f = t + WIDE_THREADS * k;
+        if (f < n4) {
+            v[k] = skip_sum4<FL>(x4, k4, b4, f);
+            srow[f] = v[k];
+            if (FL & NORM_SUM) s4[f] = v[k];
+        }
+    }
+    __syncthreads();
+    if (t < 32) {
+        const int F = n / 64;
+        const float mean = (FL & NORM_RMS) ? 0.0f : __fdiv_rn(ln_smem_fold<false>(srow, F, 0.0f), (float)n);
+        const float var = __fdiv_rn(ln_smem_fold<true>(srow, F, mean), (float)n);
+        if (t == 0) {
+            const float gamma_scalar = p.gamma_sp ? __ldg(p.gamma_sp) : 1.0f;
+            stat[0] = mean;
+            stat[1] = __fdiv_rn(gamma_scalar, __fsqrt_rn(__fadd_rn(var, p.eps)));
+        }
+    }
+    __syncthreads();
+    const float mean = stat[0], rstd = stat[1];
+    const float beta_scalar = p.beta_sp ? __ldg(p.beta_sp) : 0.0f;
+    float4* y4 = reinterpret_cast<float4*>(p.y + row * n);
+    const float4* g4 = reinterpret_cast<const float4*>(p.gamma);
+    const float4* be4 = reinterpret_cast<const float4*>(p.beta);
+    const int mode = norm_mode(p, beta_scalar);
+#pragma unroll
+    for (int k = 0; k < VPT; k++) {
+        const int f = t + WIDE_THREADS * k;
+        if (f < n4) {
+            const float4 g = p.gamma ? __ldg(g4 + f) : make_float4(1.f, 1.f, 1.f, 1.f);
+            const float4 b = p.beta ? __ldg(be4 + f) : make_float4(0.f, 0.f, 0.f, 0.f);
+            y4[f] = norm_arm4(mode, v[k], mean, rstd, g, b, beta_scalar);
+        }
+    }
+}
+
+// Odd widths, unaligned rows, a one-element bias: one warp per row; s goes to the output row first and is read back
+// from there by the fold (simd_fold_unroll4: full 64-element chunks, then 16-element chunks and the masked tail).
+__global__ void __launch_bounds__(256) skip_norm_kernel(const SkipNormParams p) {
+    const int lane = threadIdx.x & 31;
+    const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= p.rows) return;
+    const int n = p.n;
+    const float* x = p.x + row * p.xs;
+    const float* k = p.skip ? p.skip + (row % p.skip_rows) * p.ss : nullptr;
+    float* y = p.y + row * n;  // (never aliases x or skip: the operators take no in-place outputs)
+    float* sm = p.sum ? p.sum + row * n : nullptr;
+    for (int i = lane; i < n; i += 32) {
+        float s = x[i];
+        if (k) s = __fadd_rn(s, k[i]);
+        if (p.bias) s = __fadd_rn(s, p.bias[(long long)i * p.bias_inc]);
+        y[i] = s;
+        if (sm) sm[i] = s;
+    }
+    __syncwarp();
+    const float gamma_scalar = p.gamma_sp ? __ldg(p.gamma_sp) : 1.0f;
+    const float beta_scalar = p.beta_sp ? __ldg(p.beta_sp) : 0.0f;
+    const float mean = p.rms ? 0.0f : __fdiv_rn(simd_fold_unroll4<false>(y, n, 0.0f, lane), (float)n);
+    const float var = __fdiv_rn(simd_fold_unroll4<true>(y, n, mean, lane), (float)n);
+    const float rstd = __fdiv_rn(gamma_scalar, __fsqrt_rn(__fadd_rn(var, p.eps)));
+    __syncwarp();
+    const int mode = norm_mode(p, beta_scalar);
+    for (int i = lane; i < n; i += 32)
+        y[i] = norm_arm(mode, y[i], mean, rstd, p.gamma ? p.gamma[i] : 1.0f, p.beta ? p.beta[i] : 0.0f, beta_scalar);
+}
+
+template <int FL>
+static void launch_skip_norm_fl(const SkipNormParams& p, int S, int fm, int vpt, unsigned blocks, cudaStream_t st) {
+    if (vpt) {
+        const size_t smem = (size_t)p.n * 4;
+        switch (vpt) {
+            case 4: skip_norm_wide_kernel<4, FL><<<blocks, WIDE_THREADS, smem, st>>>(p); break;
+            default: skip_norm_wide_kernel<8, FL><<<blocks, WIDE_THREADS, smem, st>>>(p); break;
+        }
+        return;
+    }
+    switch (S * 100 + fm) {
+        case 104: skip_norm_vec_kernel<1, 4, FL><<<blocks, 128, 0, st>>>(p); break;
+        case 108: skip_norm_vec_kernel<1, 8, FL><<<blocks, 128, 0, st>>>(p); break;
+        case 116: skip_norm_vec_kernel<1, 16, FL><<<blocks, 128, 0, st>>>(p); break;
+        case 204: skip_norm_vec_kernel<2, 4, FL><<<blocks, 128, 0, st>>>(p); break;
+        case 208: skip_norm_vec_kernel<2, 8, FL><<<blocks, 128, 0, st>>>(p); break;
+        default: skip_norm_vec_kernel<2, 16, FL><<<blocks, 128, 0, st>>>(p); break;
+    }
+}
+
+rten_status launch_skip_norm(rten_ctx* ctx, const SkipNormParams& p) {
+    if (p.rows == 0 || p.n == 0) return RTEN_OK;
+    const int n = p.n;
+    auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+    const bool vec_ok = n % 64 == 0 && al16(p.x) && p.xs % 4 == 0 && (!p.skip || (al16(p.skip) && p.ss % 4 == 0)) &&
+                        (!p.bias || (al16(p.bias) && p.bias_inc == 1)) && al16(p.gamma) && al16(p.beta) && al16(p.y) &&
+                        al16(p.sum) && p.rows < 0x7fffffffLL;
+    const int fl = (p.rms ? NORM_RMS : 0) | (p.skip ? NORM_SKIP : 0) | (p.bias ? NORM_BIAS : 0) | (p.sum ? NORM_SUM : 0);
+    const bool flags_ok = p.skip || (!p.bias && !p.sum);  // (no bias or sum output without a skip input)
+    cudaStream_t st = ctx->stream;
+    if (vec_ok && flags_ok && n <= 8192) {
+        int S = 0, fm = 0, vpt = 0;
+        unsigned blocks;
+        // as launch_layer_norm: 16 S lanes per row, F = n / (64 S) <= 16 float4s per thread; two segments per row when
+        // that is possible and the rows alone would leave the SMs short of warps.  No S fits widths such as 1600
+        // (n / 64 > 16 and odd): those take the wide kernel.
+        for (int c = 1; c <= 2; c *= 2) {
+            if (n % (64 * c) != 0 || n / (64 * c) > 16) continue;
+            S = c;
+            if ((p.rows * 16 * c + 31) / 32 >= 32LL * ctx->num_sms) break;
+        }
+        if (S) {
+            const int F = n / (64 * S);
+            fm = F <= 4 ? 4 : (F <= 8 ? 8 : 16);
+            const long long warps = (p.rows + 2 / S - 1) / (2 / S);
+            blocks = (unsigned)((warps + 3) / 4);
+        } else {
+            vpt = n <= 4 * 4 * WIDE_THREADS ? 4 : 8;  // float4s per thread
+            blocks = (unsigned)p.rows;
+        }
+        switch (fl) {
+            case NORM_RMS: launch_skip_norm_fl<NORM_RMS>(p, S, fm, vpt, blocks, st); break;
+#define RTB_SKIP_NORM_CASE(F) \
+    case F: launch_skip_norm_fl<F>(p, S, fm, vpt, blocks, st); break; \
+    case F | NORM_RMS: launch_skip_norm_fl<F | NORM_RMS>(p, S, fm, vpt, blocks, st); break;
+            RTB_SKIP_NORM_CASE(NORM_SKIP)
+            RTB_SKIP_NORM_CASE(NORM_SKIP | NORM_BIAS)
+            RTB_SKIP_NORM_CASE(NORM_SKIP | NORM_SUM)
+            RTB_SKIP_NORM_CASE(NORM_SKIP | NORM_BIAS | NORM_SUM)
+#undef RTB_SKIP_NORM_CASE
+            default: return fail(ctx, RTEN_ERR_INVALID_VALUE, "skip_norm: no kernel for these flags");
+        }
+    } else {
+        const long long blocks = (p.rows + 7) / 8;
+        skip_norm_kernel<<<(unsigned)blocks, 256, 0, st>>>(p);
+    }
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail_cuda(ctx, e, "skip_norm launch");
+    count_launch(ctx);
+    return RTEN_OK;
+}
+
 // Row sums in the reference's Sum order (GlobalAveragePool = Sum / len, src/ops/pooling.rs:516-521).
 // Element k of row r lives at x[r_off(r) + k * kstride].
 __global__ void __launch_bounds__(256)

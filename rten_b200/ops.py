@@ -798,6 +798,54 @@ class LayerNormalization:
         return A.wrap(o, out)
 
 
+class RMSNormalization:
+    """src/ops/norm.rs rms_normalization: LayerNormalization without centring, rstd = scale / sqrt(mean(x^2) + epsilon)"""
+
+    def __init__(self, axis=-1, epsilon: Optional[float] = None):
+        self.axis, self.epsilon = axis, epsilon
+
+    def run(self, ctx, x, scale, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        ctx.check(ctx.lib.rten_b200_rms_norm(ctx.handle, A.t(x), A.t(scale), self.axis,
+                                             -1.0 if self.epsilon is None else float(self.epsilon), C.byref(o)))
+        return A.wrap(o, out)
+
+
+class SimplifiedLayerNormalization(RMSNormalization):
+    """src/ops/norm/contrib.rs: ONNX Runtime's name for RMSNormalization"""
+
+
+class SkipLayerNormalization:
+    """src/ops/norm/contrib.rs (com.microsoft): LayerNormalization of (x + skip) + bias over the last axis.
+    `run(..., want_sum=True)` also returns that sum (the operator's output 3, input_skip_bias_sum)."""
+
+    _rms = 0
+
+    def __init__(self, epsilon: float):
+        self.epsilon = float(epsilon)
+
+    def _run(self, ctx, x, skip, gamma, beta, bias, want_sum):
+        A = _Args(ctx)
+        o = A.out()
+        s = A.out() if want_sum else None
+        ctx.check(ctx.lib.rten_b200_skip_layer_norm(ctx.handle, A.t(x), A.t(skip), A.t(gamma), A.t(beta), A.t(bias),
+                                                    self.epsilon, self._rms, C.byref(o), C.byref(s) if want_sum else None))
+        return (A.wrap(o, None), A.wrap(s, None)) if want_sum else A.wrap(o, None)
+
+    def run(self, ctx, x, skip, gamma, beta=None, bias=None, want_sum=False):
+        return self._run(ctx, x, skip, gamma, beta, bias, want_sum)
+
+
+class SkipSimplifiedLayerNormalization(SkipLayerNormalization):
+    """src/ops/norm/contrib.rs (com.microsoft): RMSNormalization of (x + skip) + bias over the last axis (no beta)."""
+
+    _rms = 1
+
+    def run(self, ctx, x, skip, gamma, bias=None, want_sum=False):
+        return self._run(ctx, x, skip, gamma, None, bias, want_sum)
+
+
 class _Unary:
     fn = ""
 
