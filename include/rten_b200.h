@@ -596,6 +596,57 @@ rten_status rten_b200_mul(rten_ctx* ctx, const rten_tensor* a, const rten_tensor
 rten_status rten_b200_max_pool(rten_ctx* ctx, const rten_tensor* x, const int32_t kernel[2], const int32_t pads[4],
                                const int32_t strides[2], rten_tensor* out);
 rten_status rten_b200_global_average_pool(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
+/* AveragePool 2-D (src/ops/pooling.rs:263-333, 391-417), f32 NCHW in any strides; the output layout follows the input.
+ * Per output: the sum, from +0.0, of the taps inside the image in (ky, kx) order, each add rounded, then ONE division by
+ * kh * kw (count_include_pad != 0) or by the number of taps inside the image.  Bit-identical to the reference.  There
+ * is no ceil_mode parameter (rten_b200_max_pool has none either): the model executor rejects ceil_mode = 1. */
+rten_status rten_b200_average_pool(rten_ctx* ctx, const rten_tensor* x, const int32_t kernel[2], const int32_t pads[4],
+                                   const int32_t strides[2], int count_include_pad, rten_tensor* out);
+/* Resize (src/ops/resize.rs), f32: nearest or bilinear resampling of the last two axes.  The target is `scales`
+ * (output size floor(in as f32 * scale), output -> input scale 1 / scale) or, with use_sizes != 0, `sizes` (scale
+ * in as f32 / out as f32), `n` values each, one per input axis (resize.rs:273-308).  1-D to 4-D inputs of which at most
+ * the last two axes change, expanded to NCHW as the reference does (resize.rs:350-407: NCHW; NCW before NHW; HW; W); an
+ * output shape equal to the input's is a copy; an empty output comes back empty.  Errors as the
+ * reference: n != rank RTEN_ERR_INCOMPATIBLE_SHAPES "scales/sizes length should equal input rank", a negative size
+ * RTEN_ERR_INVALID_VALUE "scales/sizes must be positive", anything else RTEN_ERR_UNSUPPORTED_VALUE "Only 1D to 4D
+ * inputs are supported with up to two resized dimensions".
+ * Every coordinate, weight and blend is computed on the device in f32 with separately rounded operations in the
+ * reference's order (x direction first, then y): the result is bit-identical to it, including NaN for a bilinear
+ * align_corners output of one pixel along a resized axis (its coordinate is 0 / 0 there too).
+ * x in any strides.  A library-allocated output follows the input's layout (channels-last in, channels-last out); a
+ * caller's `out` is written through its strides.  One kernel launch: channels-last with C % 4 == 0 and 16-byte
+ * addressable pixels moves one float4 of channels per thread; other layouts produce runs of 4 output columns per
+ * thread, stored as a float4 when the output row is aligned. */
+typedef enum { RTEN_RESIZE_NEAREST = 0, RTEN_RESIZE_LINEAR = 1 } rten_resize_mode;
+typedef enum {
+    RTEN_RESIZE_HALF_PIXEL = 0,
+    RTEN_RESIZE_ASYMMETRIC = 1,
+    RTEN_RESIZE_ALIGN_CORNERS = 2,
+    RTEN_RESIZE_PYTORCH_HALF_PIXEL = 3
+} rten_resize_coord_mode;
+typedef enum {
+    RTEN_RESIZE_FLOOR = 0,
+    RTEN_RESIZE_CEIL = 1,
+    RTEN_RESIZE_ROUND_PREFER_FLOOR = 2,
+    RTEN_RESIZE_ROUND_PREFER_CEIL = 3
+} rten_resize_nearest_mode;
+typedef struct {
+    int32_t mode;         /* rten_resize_mode */
+    int32_t coord_mode;   /* rten_resize_coord_mode */
+    int32_t nearest_mode; /* rten_resize_nearest_mode (nearest only) */
+    int32_t n;            /* entries of scales / sizes that are set */
+    float scales[4];
+    int64_t sizes[4];
+    int32_t use_sizes;
+} rten_resize_params;
+rten_status rten_b200_resize(rten_ctx* ctx, const rten_tensor* x, const rten_resize_params* p, rten_tensor* out);
+/* Concat (src/ops/concat.rs): `n` >= 1 inputs of one type (f32, i32, i8 or u8) and rank, equal in every dimension but
+ * `axis` (negative counts from the end); errors as `concatenated_shape` (concat.rs:20-47).  Inputs and `out` in any
+ * strides; a library-allocated output follows the layout of input 0 (channels-last in, channels-last out).  ONE kernel
+ * launch per 16 inputs copies every slice, in 16-byte units when every slice is 16-byte addressable and the innermost
+ * dimension is contiguous on both sides.  An input that already is its slice of `out` (same address and strides) is
+ * skipped: a caller that had the producers write into `out` pays nothing for it. */
+rten_status rten_b200_concat(rten_ctx* ctx, const rten_tensor* const* inputs, int n, int axis, rten_tensor* out);
 /* Gather along axis 0 of a 2-D table with i32 indices (embedding lookups, src/ops/gather.rs). */
 rten_status rten_b200_gather_rows(rten_ctx* ctx, const rten_tensor* table, const rten_tensor* indices_i32,
                                   rten_tensor* out);
@@ -615,9 +666,18 @@ rten_status rten_b200_scatter_rows(rten_ctx* ctx, rten_tensor* table, const rten
  * counted and return to the context pool after their last consumer; Relu / Clip / Gelu / Erf / Sigmoid / HardSigmoid /
  * HardSwish / Softmax run in place when the
  * executor holds the last reference to their input (src/graph.rs:973-1049); Reshape / Flatten / Squeeze / Unsqueeze /
- * Transpose / Identity are views.  Operators: Conv, ConvInteger, ConvTranspose (constant weights prepacked at load; a
+ * Transpose / Identity are views.  A Concat over axis 1 whose input channel counts the file determines is written in
+ * place: each input produced by Conv (with its fused activation), ConvTranspose, MaxPool, AveragePool, Resize or
+ * Upsample -- unless it is a graph output, feeds the Concat twice, already feeds another such Concat, or its channel
+ * slice would not start 16-byte aligned -- gets a strided view of its slice of the Concat's buffer as `out`; the Concat
+ * node copies the remaining inputs in one launch, and launches nothing when there are none.  Results are bit-identical
+ * to the copying plan; env RTEN_B200_NO_CONCAT_ELISION=1 at load selects that plan for comparisons, and
+ * rten_b200_model_summary lists the plan under "concat_in_place".  Operators: Conv, ConvInteger, ConvTranspose (constant weights prepacked at load; a
  * node that sets output_shape fails the load), Relu, Clip, Sigmoid, HardSigmoid (alpha / beta, defaults 0.2 / 0.5),
- * HardSwish, MaxPool, GlobalAveragePool, ReduceMean (spatial axes), Gemm, MatMul, MatMulInteger, Add, Mul, Softmax, LayerNormalization,
+ * HardSwish, MaxPool, AveragePool (ceil_mode = 1 fails the load), Resize and Upsample (scales / sizes must be constants;
+ * the attribute checks and defaults of the reference's reader: antialias, exclude_outside, extrapolation_value,
+ * keep_aspect_ratio_policy and cubic_coeff_a at their defaults, cubic computed as linear), Concat (a missing axis fails
+ * the load), GlobalAveragePool, ReduceMean (spatial axes), Gemm, MatMul, MatMulInteger, Add, Mul, Softmax, LayerNormalization,
  * RMSNormalization and SimplifiedLayerNormalization (stash_type 1), SkipLayerNormalization and
  * SkipSimplifiedLayerNormalization (com.microsoft; outputs 0 and 3: a missing epsilon or a named mean / inv_std_var output
  * fails the load), Gelu, Erf, Gather (rows), Cast (i32 -> f32),
@@ -638,7 +698,7 @@ const char* rten_b200_model_input_name(const rten_model* model, int32_t index);
 const char* rten_b200_model_output_name(const rten_model* model, int32_t index);
 int32_t rten_b200_model_num_nodes(const rten_model* model); /* after the load-time fusions */
 const char* rten_b200_model_node_op(const rten_model* model, int32_t index);
-const char* rten_b200_model_summary(const rten_model* model); /* JSON: the decoded file (before fusion) */
+const char* rten_b200_model_summary(const rten_model* model); /* JSON: the decoded file (before fusion) + "concat_in_place" */
 /* Inputs by name (device tensors, or host tensors staged for the run; integer inputs are i32).  Outputs by name: any
  * value of the graph may be requested (`Model::run` with arbitrary output nodes); each comes back as a contiguous device
  * tensor the caller owns (rten_b200_free). */

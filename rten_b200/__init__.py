@@ -5,8 +5,8 @@ The product is `librten_b200.so` (hand-written CUDA behind the C ABI in include/
 runners and bench.py.  There is no CPU implementation in this package."""
 from . import _lib  # noqa: F401
 from .ops import (  # noqa: F401
-    ACT_GELU, ACT_GELU_TANH, ACT_HARD_SIGMOID, ACT_HARD_SWISH, ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_SILU, Add, AddSoftmax, Attention, Clip, Comm, Context, Conv, ConvInteger, ConvIntegerToFloat,
+    ACT_GELU, ACT_GELU_TANH, ACT_HARD_SIGMOID, ACT_HARD_SWISH, ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_SILU, Add, AddSoftmax, Attention, AveragePool, Clip, Concat, Comm, Context, Conv, ConvInteger, ConvIntegerToFloat,
     ConvTranspose, DeviceTensor, DynamicQuantizeLinear, Erf, FusedMatMul, GatherRows, Gelu, Gemm, GlobalAveragePool, GroupQueryAttention, GRU, HardSigmoid, HardSwish,
-    LayerNormalization, LSTM, MatMul, MatMulInteger, MatMulIntegerToFloat, MatMulNBits, MaxPool, Mul, MultiHeadAttention, OpError, Packed, QuantizedLinear, Relu, RMSNormalization, RotaryEmbedding, ScatterRows, Sigmoid,
-    SimplifiedLayerNormalization, Silu, SkipLayerNormalization, SkipSimplifiedLayerNormalization, Softmax, from_torch,
+    LayerNormalization, LSTM, MatMul, MatMulInteger, MatMulIntegerToFloat, MatMulNBits, MaxPool, Mul, MultiHeadAttention, OpError, Packed, QuantizedLinear, Relu, Resize, RMSNormalization, RotaryEmbedding, ScatterRows, Sigmoid,
+    SimplifiedLayerNormalization, Silu, SkipLayerNormalization, SkipSimplifiedLayerNormalization, Softmax, Upsample, from_torch,
 )

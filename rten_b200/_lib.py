@@ -77,6 +77,11 @@ class RtenActivation(C.Structure):
     _fields_ = [("kind", C.c_int32), ("alpha", C.c_float), ("beta", C.c_float)]
 
 
+class RtenResizeParams(C.Structure):
+    _fields_ = [("mode", C.c_int32), ("coord_mode", C.c_int32), ("nearest_mode", C.c_int32), ("n", C.c_int32),
+                ("scales", C.c_float * 4), ("sizes", C.c_int64 * 4), ("use_sizes", C.c_int32)]
+
+
 class RtenRnnParams(C.Structure):
     _fields_ = [("direction", C.c_int32), ("hidden_size", C.c_int32), ("linear_before_reset", C.c_int32)]
 
@@ -159,6 +164,9 @@ _SIGNATURES = {
     "rten_b200_dynamic_quantize_linear_ranged": (C.c_int, [_vp, _TP, _TP, _TP, _TP, _TP, _vp]),
     "rten_b200_max_pool": (C.c_int, [_vp, _TP, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _TP]),
     "rten_b200_global_average_pool": (C.c_int, [_vp, _TP, _TP]),
+    "rten_b200_average_pool": (C.c_int, [_vp, _TP, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int, _TP]),
+    "rten_b200_resize": (C.c_int, [_vp, _TP, C.POINTER(RtenResizeParams), _TP]),
+    "rten_b200_concat": (C.c_int, [_vp, C.POINTER(_TP), C.c_int, C.c_int, _TP]),
     "rten_b200_gather_rows": (C.c_int, [_vp, _TP, _TP, _TP]),
     "rten_b200_scatter_rows": (C.c_int, [_vp, _TP, _TP, _TP]),
     "rten_b200_model_load": (C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(_vp)]),

@@ -13,6 +13,7 @@
 #include "api_shared.h"
 #include "api_util.h"
 #include "depthwise.h"
+#include "resize.h"
 #include "rowops.h"
 #include "skinny.h"
 #include "umma_gemm.h"
@@ -1392,8 +1393,9 @@ rten_status rten_b200_conv_integer_ex(rten_ctx* ctx, const rten_tensor* x, const
 }
 
 // ---- pooling / gather ---------------------------------------------------------------------------------
-rten_status rten_b200_max_pool(rten_ctx* ctx, const rten_tensor* x, const int32_t kernel[2], const int32_t pads[4],
-                               const int32_t strides[2], rten_tensor* out) {
+// MaxPool (average = false) and AveragePool over an NCHW tensor in any strides; the output follows the input's layout
+static rten_status pool2d(rten_ctx* ctx, const rten_tensor* x, const int32_t kernel[2], const int32_t pads[4],
+                          const int32_t strides[2], bool average, int count_include_pad, rten_tensor* out) {
     RTB_TRY(check_ctx(ctx));
     if (!x || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
     if (x->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
@@ -1430,8 +1432,254 @@ rten_status rten_b200_max_pool(rten_ctx* ctx, const rten_tensor* x, const int32_
             p.ys_h = ov.strides[2];
             p.ys_w = ov.strides[3];
             p.channels_fastest = ov.strides[1] == 1;
-            st = launch_maxpool(ctx, (const float*)xv.data, (float*)ov.data, p);
+            st = average ? launch_avgpool(ctx, (const float*)xv.data, (float*)ov.data, p, count_include_pad)
+                         : launch_maxpool(ctx, (const float*)xv.data, (float*)ov.data, p);
         }
+    }
+    return sc.finish(st);
+}
+
+rten_status rten_b200_max_pool(rten_ctx* ctx, const rten_tensor* x, const int32_t kernel[2], const int32_t pads[4],
+                               const int32_t strides[2], rten_tensor* out) {
+    return pool2d(ctx, x, kernel, pads, strides, false, 0, out);
+}
+
+rten_status rten_b200_average_pool(rten_ctx* ctx, const rten_tensor* x, const int32_t kernel[2], const int32_t pads[4],
+                                   const int32_t strides[2], int count_include_pad, rten_tensor* out) {
+    return pool2d(ctx, x, kernel, pads, strides, true, count_include_pad, out);
+}
+
+// ---- Resize -------------------------------------------------------------------------------------------
+// `f32 as i32` (saturating, NaN -> 0)
+static int64_t f32_as_i32(float v) {
+    if (v != v) return 0;
+    if (v >= 2147483648.0f) return INT32_MAX;
+    if (v <= -2147483648.0f) return INT32_MIN;
+    return (int64_t)v;
+}
+
+rten_status rten_b200_resize(rten_ctx* ctx, const rten_tensor* x, const rten_resize_params* p, rten_tensor* out) {
+    RTB_TRY(check_ctx(ctx));
+    if (!x || !p || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    if (x->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    if (p->mode < RTEN_RESIZE_NEAREST || p->mode > RTEN_RESIZE_LINEAR || p->coord_mode < RTEN_RESIZE_HALF_PIXEL ||
+        p->coord_mode > RTEN_RESIZE_PYTORCH_HALF_PIXEL || p->nearest_mode < RTEN_RESIZE_FLOOR ||
+        p->nearest_mode > RTEN_RESIZE_ROUND_PREFER_CEIL)
+        return fail(ctx, RTEN_ERR_INVALID_VALUE, "unknown resize mode");
+    OpScope sc(ctx);
+    rten_tensor xv;
+    RTB_TRY(sc.in(x, &xv));
+    const int nd = xv.ndim;
+    // calc_output_size (src/ops/resize.rs:273-308).  Each value is ONE rounded f32 operation (a product, a quotient),
+    // which no host compiler can contract; everything that chains operations runs on the device.
+    if (p->n != nd) return sc.finish(fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "scales/sizes length should equal input rank"));
+    if (nd > 4) return sc.finish(fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Only 1D to 4D inputs are supported with up to two resized dimensions"));
+    int64_t osz[4] = {0, 0, 0, 0};
+    float inv[4] = {1.0f, 1.0f, 1.0f, 1.0f};
+    for (int i = 0; i < nd; i++) {
+        const volatile float in = (float)xv.shape[i];
+        if (p->use_sizes) {
+            const volatile float o = (float)p->sizes[i];
+            osz[i] = p->sizes[i];
+            inv[i] = in / o;
+        } else {
+            const volatile float s = p->scales[i];
+            const volatile float prod = in * s;
+            osz[i] = f32_as_i32(floorf(prod));
+            inv[i] = 1.0f / s;
+        }
+    }
+    for (int i = 0; i < nd; i++)
+        if (osz[i] < 0) return sc.finish(fail(ctx, RTEN_ERR_INVALID_VALUE, "scales/sizes must be positive"));
+    // resize_impl (resize.rs:350-407): which input axis plays (n, c, h, w); -1 = an added axis of size 1
+    bool same = true;
+    for (int i = 0; i < nd; i++) same = same && osz[i] == xv.shape[i];
+    auto eq = [&](int i) { return osz[i] == xv.shape[i]; };
+    int map[4] = {-1, -1, -1, -1};
+    if (same) {
+    } else if (nd == 4 && eq(0) && eq(1)) {
+        map[0] = 0, map[1] = 1, map[2] = 2, map[3] = 3;
+    } else if (nd == 3 && eq(0) && eq(1)) {  // NCW
+        map[0] = 0, map[1] = 1, map[3] = 2;
+    } else if (nd == 3 && eq(0)) {  // NHW
+        map[0] = 0, map[2] = 1, map[3] = 2;
+    } else if (nd == 2) {
+        map[2] = 0, map[3] = 1;
+    } else if (nd == 1) {
+        map[3] = 0;
+    } else {
+        return sc.finish(fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Only 1D to 4D inputs are supported with up to two resized dimensions"));
+    }
+    // output: a 4-D result follows the input's layout, like MaxPool and the convolutions
+    rten_tensor ov;
+    {
+        const rten_status st = nd == 4 ? out_like(sc, out, RTEN_F32, xv, false, osz[0], osz[1], osz[2], osz[3], &ov)
+                                       : sc.out(out, RTEN_F32, nd, osz, &ov, nullptr);
+        if (st != RTEN_OK) return sc.finish(st);
+    }
+    if (same) {
+        long long shape[RTEN_MAX_DIMS], ss[RTEN_MAX_DIMS], ds[RTEN_MAX_DIMS];
+        for (int i = 0; i < nd; i++) shape[i] = xv.shape[i], ss[i] = xv.strides[i], ds[i] = ov.strides[i];
+        return sc.finish(numel(&xv) ? launch_nd_copy(ctx, 4, xv.data, ov.data, nd, shape, ss, ds) : RTEN_OK);
+    }
+    ResizeParams r;
+    r.mode = p->mode;
+    r.coord_mode = p->coord_mode;
+    r.nearest_mode = p->nearest_mode;
+    int64_t in4[4], out4[4];
+    for (int i = 0; i < 4; i++) {
+        const int a = map[i];
+        in4[i] = a >= 0 ? xv.shape[a] : 1;
+        out4[i] = a >= 0 ? osz[a] : 1;
+        r.xs[i] = a >= 0 ? xv.strides[a] : 0;
+        r.os[i] = a >= 0 ? ov.strides[a] : 0;
+    }
+    if (out4[0] * out4[1] * out4[2] * out4[3] != 0 && in4[2] * in4[3] == 0)
+        return sc.finish(fail(ctx, RTEN_ERR_INVALID_VALUE, "cannot resize an empty input"));
+    for (int i = 0; i < 4; i++)
+        if (in4[i] > INT32_MAX || out4[i] > INT32_MAX) return sc.finish(fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "dimension too large"));
+    r.B = (int)out4[0];
+    r.C = (int)out4[1];
+    r.H = (int)in4[2];
+    r.W = (int)in4[3];
+    r.OH = (int)out4[2];
+    r.OW = (int)out4[3];
+    r.inv_y = map[2] >= 0 ? inv[map[2]] : 1.0f;
+    r.inv_x = inv[map[3]];
+    r.x = (const float*)xv.data;
+    r.out = (float*)ov.data;
+    return sc.finish(launch_resize(ctx, r));
+}
+
+// ---- Concat -------------------------------------------------------------------------------------------
+rten_status rten_b200_concat(rten_ctx* ctx, const rten_tensor* const* inputs, int n, int axis, rten_tensor* out) {
+    RTB_TRY(check_ctx(ctx));
+    if (!inputs || n < 1 || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    for (int i = 0; i < n; i++)
+        if (!inputs[i]) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    const rten_tensor& first = *inputs[0];
+    const int nd = first.ndim, dt = first.dtype;
+    if (dt != RTEN_F32 && dt != RTEN_I32 && dt != RTEN_I8 && dt != RTEN_U8) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    for (int i = 1; i < n; i++)
+        if (inputs[i]->dtype != dt) return fail(ctx, RTEN_ERR_CAST_FAILED, "inputs must have the same type");
+    if (nd < 1 || nd > RTEN_MAX_DIMS || axis < -nd || axis >= nd) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Axis is invalid");
+    if (axis < 0) axis += nd;
+    // concatenated_shape (src/ops/concat.rs:20-47)
+    int64_t oshape[RTEN_MAX_DIMS];
+    for (int d = 0; d < nd; d++) oshape[d] = first.shape[d];
+    for (int i = 1; i < n; i++) {
+        if (inputs[i]->ndim != nd) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Tensors must have the same number of dimensions");
+        for (int d = 0; d < nd; d++) {
+            if (d != axis && inputs[i]->shape[d] != first.shape[d])
+                return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Dimensions must be the same except for concat axis");
+            if (d == axis) oshape[d] += inputs[i]->shape[d];
+        }
+    }
+    OpScope sc(ctx);
+    std::vector<rten_tensor> iv((size_t)n);
+    for (int i = 0; i < n; i++) {
+        rten_status st = sc.in(inputs[i], &iv[(size_t)i]);
+        if (st != RTEN_OK) return sc.finish(st);
+    }
+    rten_tensor ov;
+    {
+        // an allocated 4-D output follows input 0's layout
+        OutLayout l;
+        if (nd == 4) l = layout_like(iv[0], false, oshape[0], oshape[1], oshape[2], oshape[3]);
+        rten_status st = sc.out(out, dt, nd, oshape, &ov, (nd == 4 && !out->data) ? l.strides : nullptr);
+        if (st != RTEN_OK) return sc.finish(st);
+    }
+    const int es = dtype_size(dt);
+    // dimensions of extent 1 dropped, the rest put in the output's memory order, then adjacent dimensions merged where the
+    // output and every copied input allow it (the concat axis merges with the dimensions inside it only)
+    struct Src {
+        const uint8_t* p;
+        long long ext, start;
+        long long st[RTEN_MAX_DIMS];
+    };
+    std::vector<Src> srcs;
+    long long shape[RTEN_MAX_DIMS], ost[RTEN_MAX_DIMS];
+    int dims[RTEN_MAX_DIMS], k = 0, ax = 0;
+    for (int d = 0; d < nd; d++)
+        if (d == axis || oshape[d] != 1) dims[k++] = d;
+    // in the output's memory order, outermost first: a channels-last output iterates (b, h, w, c)
+    std::stable_sort(dims, dims + k, [&](int a, int b) { return ov.strides[a] > ov.strides[b]; });
+    for (int j = 0; j < k; j++)
+        if (dims[j] == axis) ax = j;
+    for (int j = 0; j < k; j++) shape[j] = oshape[dims[j]], ost[j] = ov.strides[dims[j]];
+    long long start = 0;
+    for (int i = 0; i < n; i++) {
+        const rten_tensor& t = iv[(size_t)i];
+        Src s;
+        s.p = (const uint8_t*)t.data;
+        s.ext = t.shape[axis];
+        s.start = start;
+        start += s.ext;
+        for (int j = 0; j < k; j++) s.st[j] = t.strides[dims[j]];
+        if (numel(&t) == 0) continue;
+        // already its slice of the output: nothing to copy
+        bool in_place = s.p == (const uint8_t*)ov.data + s.start * ost[ax] * es;
+        for (int j = 0; j < k && in_place; j++) in_place = (j == ax ? s.ext : shape[j]) == 1 || s.st[j] == ost[j];
+        if (!in_place) srcs.push_back(s);
+    }
+    for (int j = k - 2; j >= 0; j--) {
+        if (j + 1 == ax) continue;
+        bool ok = ost[j] == ost[j + 1] * shape[j + 1];
+        for (const Src& s : srcs) ok = ok && s.st[j] == s.st[j + 1] * shape[j + 1];
+        if (!ok) continue;
+        const long long inner = shape[j + 1];
+        shape[j] *= inner;
+        ost[j] = ost[j + 1];
+        for (Src& s : srcs) {
+            s.st[j] = s.st[j + 1];
+            if (j == ax) s.ext *= inner, s.start *= inner;
+        }
+        for (int m = j + 1; m + 1 < k; m++) {
+            shape[m] = shape[m + 1];
+            ost[m] = ost[m + 1];
+            for (Src& s : srcs) s.st[m] = s.st[m + 1];
+        }
+        if (ax > j) ax--;
+        k--;
+    }
+    // 16-byte units when every slice is 16-byte addressable and the innermost dimension is contiguous on both sides
+    const long long v = 16 / es;
+    bool vec = ost[k - 1] == 1 && reinterpret_cast<uintptr_t>(ov.data) % 16 == 0 && (ax == k - 1 || shape[k - 1] % v == 0);
+    for (int j = 0; j + 1 < k && vec; j++) vec = ost[j] % v == 0;
+    for (const Src& s : srcs) {
+        vec = vec && s.st[k - 1] == 1 && reinterpret_cast<uintptr_t>(s.p) % 16 == 0;
+        if (ax == k - 1) vec = vec && s.ext % v == 0 && s.start % v == 0;
+        for (int j = 0; j + 1 < k && vec; j++) vec = s.st[j] % v == 0;
+    }
+    // strides and innermost extents in units of the copied element
+    auto stride_of = [&](int j, long long st) { return vec ? (j == k - 1 ? 1 : st / v) : st; };
+    const long long unit = vec ? v : 1;
+    ConcatParams cp;
+    memset(&cp, 0, sizeof(cp));
+    cp.esize = vec ? 16 : es;
+    cp.ndim = k;
+    cp.axis = ax;
+    cp.out = ov.data;
+    for (int j = 0; j < k; j++) {
+        cp.shape[j] = j == k - 1 ? shape[j] / unit : shape[j];
+        cp.out_strides[j] = stride_of(j, ost[j]);
+    }
+    rten_status st = RTEN_OK;
+    for (size_t base = 0; base < srcs.size() && st == RTEN_OK; base += kConcatMaxSources) {
+        cp.nsrc = (int)std::min<size_t>(kConcatMaxSources, srcs.size() - base);
+        for (int i = 0; i < cp.nsrc; i++) {
+            const Src& s = srcs[base + (size_t)i];
+            ConcatSource& c = cp.s[i];
+            c.src = s.p;
+            c.ext = ax == k - 1 ? s.ext / unit : s.ext;
+            c.dst_off = s.start * ost[ax] / unit;
+            c.n = 1;
+            for (int j = 0; j < k; j++) {
+                c.strides[j] = stride_of(j, s.st[j]);
+                c.n *= j == ax ? c.ext : cp.shape[j];
+            }
+        }
+        st = launch_concat(ctx, cp);
     }
     return sc.finish(st);
 }

@@ -9,8 +9,12 @@
 //          returned to the context pool after their last consumer (src/graph.rs:1100-1180); an operator that can run in
 //          place does so when the executor holds the last reference to its input (src/graph.rs:973-1049); shape-only
 //          operators (Reshape, Flatten, Squeeze, Unsqueeze, Transpose, Identity) are views -- no kernel, no copy.
+//          A Concat over the channels of NCHW tensors is written in place by its producers where the load found that
+//          possible (plan_concat_elision): the first such producer to run allocates the Concat's buffer and every one of
+//          them gets a strided view of its channel slice as `out`, so the Concat node copies only the other inputs --
+//          nothing when there are none.  RTEN_B200_NO_CONCAT_ELISION=1 (read at load) turns that off for comparisons.
 // Operators: Conv, ConvInteger, ConvTranspose (without output_shape), Relu, Clip, Sigmoid, HardSigmoid, HardSwish,
-// MaxPool, GlobalAveragePool, ReduceMean, Gemm, MatMul, MatMulInteger, MatMulNBits
+// MaxPool, AveragePool (ceil_mode 0), GlobalAveragePool, ReduceMean, Resize and Upsample (constant scales / sizes), Concat, Gemm, MatMul, MatMulInteger, MatMulNBits
 // (com.microsoft), Add, Mul, Softmax, LayerNormalization, RMSNormalization, SimplifiedLayerNormalization,
 // SkipLayerNormalization and SkipSimplifiedLayerNormalization (com.microsoft, outputs 0 and 3), Gelu, Erf, Gather, Cast,
 // DynamicQuantizeLinear, Attention, RotaryEmbedding, GroupQueryAttention and MultiHeadAttention (com.microsoft, three outputs), GRU and LSTM, Constant and
@@ -20,12 +24,14 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <memory>
 #include <set>
 #include <string>
 #include <vector>
 
+#include "api_shared.h"
 #include "api_util.h"
 #include "onnx_reader.h"
 #include "rowops.h"
@@ -42,6 +48,8 @@ struct ValueSlot {
     rten_tensor t{};
     bool has_host_ints = false;       // shape-like constant (int64 in the file): usable by Reshape / axes inputs
     std::vector<int64_t> host_ints;
+    bool has_host_floats = false;     // small f32 constant: usable as the scales of Resize / Upsample
+    std::vector<float> host_floats;
     // run state
     int root = -1;        // value that owns the allocation (self for owners)
     int pending = 0;      // consumers still to run
@@ -56,6 +64,11 @@ struct OpNode {
     rten_packed* packed = nullptr;
     rten_activation activation = {RTEN_ACT_NONE, 0.0f, 0.0f};  // fused activation of a Conv
     int bias_value = -1;       // fused Add(bias) of a MatMul
+    // Concat elision (plan_concat_elision).  On a Concat: the channel count of every input and whether its producer
+    // writes it in place.  On a producer: the Concat node and the input slot its output is written into.
+    std::vector<int64_t> cat_channels;
+    std::vector<char> cat_in_place;
+    int cat_node = -1, cat_slot = -1;
 };
 
 }  // namespace
@@ -128,6 +141,10 @@ rten_status upload_constant(rten_model* m, const onnx::Tensor& t, ValueSlot* v) 
             memcpy(conv.data() + 4 * i, &y, 4);
         }
         src = conv.data();
+    } else if (t.data_type == onnx::DT_FLOAT && n <= RTEN_MAX_DIMS) {
+        v->has_host_floats = true;
+        v->host_floats.resize((size_t)n);
+        if (n) memcpy(v->host_floats.data(), t.data.data(), (size_t)n * 4);
     } else if (t.data_type == onnx::DT_INT32) {
         v->has_host_ints = true;
         v->host_ints.resize((size_t)n);
@@ -155,7 +172,7 @@ rten_status upload_constant(rten_model* m, const onnx::Tensor& t, ValueSlot* v) 
 
 const std::set<std::string>& supported_ops() {
     static const std::set<std::string> s = {
-        "Conv", "ConvTranspose", "Relu", "Clip", "Sigmoid", "HardSigmoid", "HardSwish", "MaxPool", "GlobalAveragePool", "ReduceMean", "Reshape", "Flatten", "Squeeze", "Unsqueeze", "Transpose",
+        "Conv", "ConvTranspose", "Relu", "Clip", "Sigmoid", "HardSigmoid", "HardSwish", "MaxPool", "AveragePool", "Resize", "Upsample", "Concat", "GlobalAveragePool", "ReduceMean", "Reshape", "Flatten", "Squeeze", "Unsqueeze", "Transpose",
         "Identity", "Gemm", "MatMul", "Add", "Mul", "Softmax", "LayerNormalization", "Gelu", "Erf", "Gather",
         "DynamicQuantizeLinear", "MatMulInteger", "ConvInteger", "Cast", "Attention", "MatMulNBits", "GroupQueryAttention",
         "MultiHeadAttention", "RotaryEmbedding", "GRU", "LSTM", "Constant", "RMSNormalization", "SimplifiedLayerNormalization",
@@ -225,6 +242,70 @@ rten_activation conv_activation(const onnx::Node& n) {
     if (op == "HardSigmoid") return {RTEN_ACT_HARD_SIGMOID, hard_sigmoid_alpha(n), hard_sigmoid_beta(n)};
     if (op == "HardSwish") return {RTEN_ACT_HARD_SWISH, 0.0f, 0.0f};
     return {RTEN_ACT_NONE, 0.0f, 0.0f};
+}
+
+// Resize / Upsample attributes as the reference reads them (src/op_registry/onnx_registry.rs:1721-1778, 1789-1810):
+// antialias, exclude_outside, extrapolation_value, keep_aspect_ratio_policy and cubic_coeff_a must have their defaults;
+// `cubic` falls back to linear; defaults nearest, round_prefer_floor, half_pixel.  Upsample is always asymmetric + floor
+// (src/ops/resize.rs:629-642).
+rten_status fill_resize_params(rten_ctx* ctx, const onnx::Node& n, rten_resize_params* p) {
+    memset(p, 0, sizeof(*p));
+    const bool upsample = n.op_type == "Upsample";
+    auto str = [&](const char* name, const char* dflt) {
+        const onnx::Attribute* a = n.attr(name);
+        return a ? a->s : std::string(dflt);
+    };
+    const std::string mode = str("mode", "nearest");
+    if (mode == "nearest") p->mode = RTEN_RESIZE_NEAREST;
+    else if (mode == "linear" || (mode == "cubic" && !upsample)) p->mode = RTEN_RESIZE_LINEAR;
+    else return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, n.op_type + ": unsupported mode '" + mode + "'");
+    if (upsample) {
+        p->coord_mode = RTEN_RESIZE_ASYMMETRIC;
+        p->nearest_mode = RTEN_RESIZE_FLOOR;
+        return RTEN_OK;
+    }
+    if (n.attr_i("antialias", 0) != 0) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Resize: antialias must be 0");
+    if (n.attr_f("cubic_coeff_a", -0.75f) != -0.75f) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Resize: cubic_coeff_a must be -0.75");
+    if (n.attr_i("exclude_outside", 0) != 0) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Resize: exclude_outside must be 0");
+    if (n.attr_f("extrapolation_value", 0.0f) != 0.0f) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Resize: extrapolation_value must be 0");
+    if (str("keep_aspect_ratio_policy", "stretch") != "stretch")
+        return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Resize: keep_aspect_ratio_policy must be stretch");
+    const std::string nm = str("nearest_mode", "round_prefer_floor"), cm = str("coordinate_transformation_mode", "half_pixel");
+    if (nm == "floor") p->nearest_mode = RTEN_RESIZE_FLOOR;
+    else if (nm == "ceil") p->nearest_mode = RTEN_RESIZE_CEIL;
+    else if (nm == "round_prefer_floor") p->nearest_mode = RTEN_RESIZE_ROUND_PREFER_FLOOR;
+    else if (nm == "round_prefer_ceil") p->nearest_mode = RTEN_RESIZE_ROUND_PREFER_CEIL;
+    else return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Resize: unsupported nearest_mode '" + nm + "'");
+    if (cm == "half_pixel") p->coord_mode = RTEN_RESIZE_HALF_PIXEL;
+    else if (cm == "asymmetric") p->coord_mode = RTEN_RESIZE_ASYMMETRIC;
+    else if (cm == "align_corners") p->coord_mode = RTEN_RESIZE_ALIGN_CORNERS;
+    else if (cm == "pytorch_half_pixel") p->coord_mode = RTEN_RESIZE_PYTORCH_HALF_PIXEL;
+    else return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Resize: unsupported coordinate_transformation_mode '" + cm + "'");
+    return RTEN_OK;
+}
+
+// MaxPool / AveragePool attributes (kernel_shape, pads, strides)
+struct PoolAttrs {
+    int32_t kernel[2], pads[4] = {0, 0, 0, 0}, strides[2] = {1, 1};
+};
+rten_status fill_pool_attrs(rten_ctx* ctx, const onnx::Node& n, PoolAttrs* a) {
+    const std::vector<int64_t> k = n.attr_ints("kernel_shape"), pd = n.attr_ints("pads"), sd = n.attr_ints("strides");
+    if (k.size() != 2) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, n.op_type + ": only 2-D kernels are supported");
+    a->kernel[0] = (int32_t)k[0];
+    a->kernel[1] = (int32_t)k[1];
+    for (size_t i = 0; i < pd.size() && i < 4; i++) a->pads[i] = (int32_t)pd[i];
+    for (size_t i = 0; i < sd.size() && i < 2; i++) a->strides[i] = (int32_t)sd[i];
+    return RTEN_OK;
+}
+
+bool writes_concat_in_place(const std::string& op) {
+    // The operators whose entry points write a caller's strided `out` directly: every store path of the convolutions
+    // takes the output's pixel and channel strides (the TMA store map is built from them, the register epilogues and
+    // the depthwise and halo kernels index with them, the explicit-im2col path falls back to a strided copy), the
+    // stride phases of ConvTranspose are such views already, and the pooling and Resize kernels index with the output
+    // strides.  The elementwise activations are left out: they reach a strided `out` through a temporary and a copy,
+    // which costs what the Concat copy costs.  So is a nested Concat, whose buffer would have to exist before its own.
+    return op == "Conv" || op == "ConvTranspose" || op == "MaxPool" || op == "AveragePool" || op == "Resize" || op == "Upsample";
 }
 
 rten_status fill_conv_params(rten_ctx* ctx, const onnx::Node& n, rten_conv_params* p) {
@@ -382,6 +463,13 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
                 if (!n.outputs[i].empty())
                     return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, n.op_type + ": the mean and inv_std_var outputs (1, 2) are not supported");
         }
+        if (n.op_type == "Resize" || n.op_type == "Upsample") {
+            rten_resize_params rp;
+            RTB_TRY(fill_resize_params(ctx, n, &rp));
+        }
+        if (n.op_type == "AveragePool" && n.attr_i("ceil_mode", 0) != 0)
+            return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "AveragePool: ceil_mode = 1 is not supported");
+        if (n.op_type == "Concat" && !n.attr("axis")) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Concat: missing attribute axis");
         if (n.op_type == "GRU" || n.op_type == "LSTM") RTB_TRY(check_rnn_attrs(ctx, n));
         if (n.op_type == "ConvTranspose" && n.attr("output_shape"))  // (the reference does not read it)
             return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "ConvTranspose: the output_shape attribute is not supported");
@@ -407,6 +495,20 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
                 if (on.n.inputs.size() < (size_t)k + 2) on.n.inputs.resize((size_t)k + 2);
                 on.n.inputs[(size_t)k + 1] = t.name;
             }
+        }
+        if (n.op_type == "Upsample" && n.attr("scales")) {
+            // opset 7: the scales attribute becomes constant input 1, as the reference's reader does (onnx_registry.rs:1802-1807)
+            const onnx::Attribute* a = n.attr("scales");
+            onnx::Tensor t;
+            t.name = n.name + "/" + (n.outputs.empty() ? std::string() : n.outputs[0]) + "/upsample_scales";
+            t.data_type = onnx::DT_FLOAT;
+            t.dims = {(int64_t)a->floats.size()};
+            t.data.resize(a->floats.size() * 4);
+            if (!a->floats.empty()) memcpy(t.data.data(), a->floats.data(), t.data.size());
+            const int id = m->value_id(t.name);
+            RTB_TRY(upload_constant(m.get(), t, &m->values[(size_t)id]));
+            on.n.inputs.resize(2);
+            on.n.inputs[1] = t.name;
         }
         for (const std::string& s : on.n.inputs) {
             const int id = m->value_id(s);
@@ -483,6 +585,80 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
             }
         }
     }
+    // ---- Concat elision, decided once: which inputs of which channel Concat their producers write in place
+    if (!getenv("RTEN_B200_NO_CONCAT_ELISION")) {
+        std::map<std::string, std::vector<int64_t>> input_dims;
+        for (const onnx::ValueInfo& vi : om.graph.inputs) input_dims[vi.name] = vi.dims;
+        auto producer = [&](int vid) {
+            for (size_t i = 0; i < m->nodes.size(); i++)
+                for (int o : m->nodes[i].out)
+                    if (o == vid) return (int)i;
+            return -1;
+        };
+        // channels of a 4-D value as far as the file tells them, else -1
+        std::function<int64_t(int, int)> channels = [&](int vid, int depth) -> int64_t {
+            if (vid < 0 || depth > 64) return -1;
+            const ValueSlot& v = m->values[(size_t)vid];
+            if (v.kind == V_INPUT) {
+                const std::vector<int64_t>& d = input_dims[v.name];
+                return d.size() == 4 && d[1] > 0 ? d[1] : -1;
+            }
+            const int pi = producer(vid);
+            if (pi < 0) return -1;
+            const OpNode& p = m->nodes[(size_t)pi];
+            const std::string& op = p.n.op_type;
+            auto weight = [&]() -> const rten_tensor* {
+                if (p.in.size() < 2 || p.in[1] < 0 || m->values[(size_t)p.in[1]].kind != V_CONST) return nullptr;
+                const rten_tensor& w = m->values[(size_t)p.in[1]].t;
+                return w.ndim == 4 ? &w : nullptr;
+            };
+            if (op == "Conv") return weight() ? weight()->shape[0] : -1;
+            if (op == "ConvTranspose") return weight() ? weight()->shape[1] * p.n.attr_i("group", 1) : -1;
+            if (op == "MaxPool" || op == "AveragePool" || op == "Resize" || op == "Upsample" || is_in_place_op(op))
+                return channels(p.in[0], depth + 1);
+            if (op == "Concat" && p.n.attr_i("axis", 0) == 1) {
+                int64_t sum = 0;
+                for (int i : p.in) {
+                    const int64_t c = channels(i, depth + 1);
+                    if (c < 0) return -1;
+                    sum += c;
+                }
+                return sum;
+            }
+            return -1;
+        };
+        std::string report;
+        for (size_t k = 0; k < m->nodes.size(); k++) {
+            OpNode& c = m->nodes[k];
+            if (c.n.op_type != "Concat" || c.n.attr_i("axis", 0) != 1 || c.out.size() != 1 || consumers(c.out[0]) < 1) continue;
+            std::vector<int64_t> ch;
+            for (int i : c.in) ch.push_back(channels(i, 0));
+            if (std::find(ch.begin(), ch.end(), (int64_t)-1) != ch.end()) continue;
+            std::vector<char> mark(c.in.size(), 0);
+            std::string names;
+            for (size_t i = 0; i < c.in.size(); i++) {
+                const int vid = c.in[i];
+                if (m->values[(size_t)vid].kind != V_TEMP) continue;
+                if (std::count(c.in.begin(), c.in.end(), vid) != 1) continue;
+                if (std::find(m->outputs.begin(), m->outputs.end(), vid) != m->outputs.end()) continue;  // a graph output is copied
+                const int pi = producer(vid);
+                OpNode& p = m->nodes[(size_t)pi];
+                if (!writes_concat_in_place(p.n.op_type) || p.out.size() != 1 || p.cat_node >= 0) continue;
+                p.cat_node = (int)k;
+                p.cat_slot = (int)i;
+                mark[i] = 1;
+                names += (names.empty() ? "\"" : ",\"") + m->values[(size_t)vid].name + "\"";
+            }
+            if (names.empty()) continue;
+            c.cat_channels = ch;
+            c.cat_in_place = mark;
+            report += (report.empty() ? "" : ",") + std::string("{\"output\":\"") + m->values[(size_t)c.out[0]].name +
+                      "\",\"copied\":" + std::to_string(std::count(mark.begin(), mark.end(), 0)) + ",\"in_place\":[" + names + "]}";
+        }
+        // (the summary is the decoded file's JSON object: the plan is appended as one more member)
+        const size_t close = m->summary.rfind('}');
+        if (close != std::string::npos) m->summary.insert(close, ",\"concat_in_place\":[" + report + "]");
+    }
     // ---- prepack constant weights once (Operator::prepack at load, src/graph.rs:488-565)
     for (OpNode& o : m->nodes) {
         const std::string& op = o.n.op_type;
@@ -541,6 +717,14 @@ struct Runner {
     rten_model* m;
     rten_ctx* ctx;
     std::set<int> keep;  // requested outputs: never released, never overwritten in place
+    // A Concat written in place, this run: its buffer (owned by the Concat's output value from the moment the first
+    // producer runs) and which inputs are written into it (`on`: the planned ones whose slice starts 16-byte aligned)
+    struct CatState {
+        bool tried = false, active = false;
+        rten_tensor buf{};
+        std::vector<char> on;
+    };
+    std::map<int, CatState> cats;
 
     ValueSlot& V(int id) { return m->values[(size_t)id]; }
     int root_of(int id) { return V(id).root < 0 ? id : V(id).root; }
@@ -619,6 +803,142 @@ struct Runner {
         if (id < 0 || !V(id).has_host_ints) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "shape-like operator input must be a constant");
         *out = V(id).host_ints;
         return RTEN_OK;
+    }
+
+    rten_status floats_of(int id, std::vector<float>* out) {
+        if (id < 0 || !V(id).has_host_floats) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "the scales of Resize / Upsample must be a constant");
+        *out = V(id).host_floats;
+        return RTEN_OK;
+    }
+
+    // The target of a Resize (opset 11+: X, roi, scales, sizes; opset 10: X, scales) or Upsample (X, scales) node.  Empty
+    // tensors count as missing (src/ops/resize.rs:491-507); roi is ignored, as in the reference.
+    rten_status resize_target(const OpNode& o, rten_resize_params* p) {
+        RTB_TRY(fill_resize_params(ctx, o.n, p));
+        const bool old = o.n.op_type == "Upsample" || o.in.size() == 2;
+        const int scales = old ? (o.in.size() > 1 ? o.in[1] : -1) : (o.in.size() > 2 ? o.in[2] : -1);
+        const int sizes = (!old && o.in.size() > 3) ? o.in[3] : -1;
+        if (scales >= 0 && numel(&V(scales).t) > 0) {
+            std::vector<float> f;
+            RTB_TRY(floats_of(scales, &f));
+            if (V(scales).t.ndim != 1) return mfail(ctx, RTEN_ERR_INVALID_VALUE, "scales must have 1 dims");
+            p->n = (int32_t)f.size();
+            for (size_t i = 0; i < f.size() && i < 4; i++) p->scales[i] = f[i];
+        } else if (sizes >= 0 && numel(&V(sizes).t) > 0) {
+            std::vector<int64_t> v;
+            RTB_TRY(ints_of(sizes, &v));
+            if (V(sizes).t.ndim != 1) return mfail(ctx, RTEN_ERR_INVALID_VALUE, "sizes must have 1 dims");
+            p->n = (int32_t)v.size();
+            p->use_sizes = 1;
+            for (size_t i = 0; i < v.size() && i < 4; i++) p->sizes[i] = v[i];
+        } else {
+            return mfail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+        }
+        return RTEN_OK;
+    }
+
+    // Shape [B, C, H, W] a producer of an in-place Concat input will give its output, and whether that output would be
+    // channels-last (the operators follow their input's layout).  false: not known here -- the node then runs as usual.
+    // A wrong answer cannot corrupt anything: the operator checks the `out` it is given against the shape it computes.
+    bool producer_shape(const OpNode& o, int64_t shape[4], bool* channels_last) {
+        const rten_tensor& x = V(o.in[0]).t;
+        if (x.ndim != 4) return false;
+        *channels_last = x.strides[1] == 1 && x.shape[1] > 1;
+        const std::string& op = o.n.op_type;
+        shape[0] = x.shape[0];
+        shape[1] = x.shape[1];
+        int64_t p0, p1;
+        if (op == "Conv") {
+            const rten_tensor& w = V(o.in[1]).t;
+            rten_conv_params p;
+            if (w.ndim != 4 || fill_conv_params(ctx, o.n, &p) != RTEN_OK) return false;
+            shape[1] = w.shape[0];
+            for (int a = 0; a < 2; a++)
+                if (api::axis_out(ctx, x.shape[2 + a], w.shape[2 + a], p.strides[a], p.auto_pad_same != 0, p.pads[a], p.pads[2 + a],
+                                  p.dilations[a], &shape[2 + a], &p0, &p1) != RTEN_OK)
+                    return false;
+            return true;
+        }
+        if (op == "ConvTranspose") {  // src/ops/conv_transpose.rs:144-224
+            const rten_tensor& w = V(o.in[1]).t;
+            rten_conv_transpose_params p;
+            if (w.ndim != 4 || fill_conv_transpose_params(ctx, o.n, &p) != RTEN_OK || p.n_strides != 2 || p.n_dilations != 2) return false;
+            shape[1] = w.shape[1] * p.groups;
+            for (int a = 0; a < 2; a++) {
+                const int64_t full = (x.shape[2 + a] - 1) * p.strides[a] + (p.n_output_padding ? p.output_padding[a] : 0) +
+                                     (w.shape[2 + a] - 1) * p.dilations[a] + 1;
+                shape[2 + a] = p.auto_pad_same ? x.shape[2 + a] * p.strides[a] : full - p.pads[a] - p.pads[2 + a];
+            }
+            return p.auto_pad_same || p.n_pads == 4;
+        }
+        if (op == "MaxPool" || op == "AveragePool") {
+            PoolAttrs a;
+            if (fill_pool_attrs(ctx, o.n, &a) != RTEN_OK) return false;
+            for (int i = 0; i < 2; i++)
+                if (api::axis_out(ctx, x.shape[2 + i], a.kernel[i], a.strides[i], false, a.pads[i], a.pads[2 + i], 1, &shape[2 + i], &p0, &p1) != RTEN_OK)
+                    return false;
+            return true;
+        }
+        if (op == "Resize" || op == "Upsample") {  // calc_output_size (src/ops/resize.rs:287-298)
+            rten_resize_params p;
+            if (resize_target(o, &p) != RTEN_OK || p.n != 4) return false;
+            for (int i = 0; i < 4; i++) {
+                const volatile float prod = (float)x.shape[i] * p.scales[i];
+                const int64_t d = p.use_sizes ? p.sizes[i] : (int64_t)floorf(prod);
+                if (i < 2 && d != x.shape[i]) return false;
+                shape[i] = d;
+            }
+            return true;
+        }
+        return false;
+    }
+
+    // `out` for a node whose output is planned to be written into a Concat's buffer: the strided view of its channel
+    // slice, allocating the buffer when this is the first such producer to run.  false: the node allocates as usual.
+    bool concat_slice(const OpNode& o, rten_tensor* slice) {
+        OpNode& c = m->nodes[(size_t)o.cat_node];
+        CatState& cs = cats[o.cat_node];
+        int64_t shape[4];
+        bool cl = false;
+        if (!producer_shape(o, shape, &cl)) return false;
+        const size_t n = c.cat_channels.size();
+        if (!cs.tried) {
+            cs.tried = true;
+            int64_t total = 0;
+            for (int64_t ch : c.cat_channels) total += ch;
+            rten_tensor b{};
+            b.dtype = RTEN_F32;
+            b.ndim = 4;
+            b.device = ctx->device;
+            b.shape[0] = shape[0], b.shape[1] = total, b.shape[2] = shape[2], b.shape[3] = shape[3];
+            b.strides[0] = total * shape[2] * shape[3];
+            b.strides[1] = cl ? 1 : shape[2] * shape[3];
+            b.strides[2] = cl ? shape[3] * total : shape[3];
+            b.strides[3] = cl ? total : 1;
+            cs.on.assign(n, 0);
+            int64_t start = 0;
+            bool any = false;
+            for (size_t i = 0; i < n; i++) {
+                cs.on[i] = c.cat_in_place[i] && (start * b.strides[1]) % 4 == 0;  // the slice starts 16-byte aligned
+                any = any || cs.on[i];
+                start += c.cat_channels[i];
+            }
+            if (!any || numel(&b) == 0) return false;
+            if (pool_alloc(ctx, (size_t)numel(&b) * 4, &b.data) != RTEN_OK) return false;
+            cs.buf = b;
+            cs.active = true;
+            set_owned(c.out[0], b);
+        }
+        if (!cs.active || !cs.on[(size_t)o.cat_slot]) return false;
+        const rten_tensor& b = cs.buf;
+        if (shape[0] != b.shape[0] || shape[1] != c.cat_channels[(size_t)o.cat_slot] || shape[2] != b.shape[2] || shape[3] != b.shape[3])
+            return false;  // (the Concat node will report the mismatch)
+        int64_t start = 0;
+        for (int i = 0; i < o.cat_slot; i++) start += c.cat_channels[(size_t)i];
+        *slice = b;
+        slice->shape[1] = shape[1];
+        slice->data = (float*)b.data + start * b.strides[1];
+        return true;
     }
 
     rten_status run_view(OpNode& o) {
@@ -728,6 +1048,7 @@ struct Runner {
             in_place = x.kind == V_TEMP && x.owned && x.root < 0 && x.pending == 1 && x.views == 0 && !keep.count(o.in[0]) && contiguous(x.t);
             if (in_place) y = x.t;
         }
+        const bool into_concat = o.cat_node >= 0 && concat_slice(o, &y);
         if (op == "Conv" || op == "ConvInteger") {
             rten_conv_params p;
             RTB_TRY(fill_conv_params(ctx, o.n, &p));
@@ -758,13 +1079,28 @@ struct Runner {
             st = rten_b200_erf(ctx, T(0), &y);
         } else if (op == "Softmax") {
             st = rten_b200_softmax(ctx, T(0), nullptr, (int)o.n.attr_i("axis", -1), 0, &y);
-        } else if (op == "MaxPool") {
-            const std::vector<int64_t> k = o.n.attr_ints("kernel_shape"), pd = o.n.attr_ints("pads"), sd = o.n.attr_ints("strides");
-            if (k.size() != 2) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MaxPool: only 2-D kernels are supported");
-            int32_t kk[2] = {(int32_t)k[0], (int32_t)k[1]}, pp[4] = {0, 0, 0, 0}, ss[2] = {1, 1};
-            for (size_t i = 0; i < pd.size() && i < 4; i++) pp[i] = (int32_t)pd[i];
-            for (size_t i = 0; i < sd.size() && i < 2; i++) ss[i] = (int32_t)sd[i];
-            st = rten_b200_max_pool(ctx, T(0), kk, pp, ss, &y);
+        } else if (op == "MaxPool" || op == "AveragePool") {
+            PoolAttrs a;
+            RTB_TRY(fill_pool_attrs(ctx, o.n, &a));
+            if (op == "MaxPool")
+                st = rten_b200_max_pool(ctx, T(0), a.kernel, a.pads, a.strides, &y);
+            else
+                st = rten_b200_average_pool(ctx, T(0), a.kernel, a.pads, a.strides, (int)o.n.attr_i("count_include_pad", 0), &y);
+        } else if (op == "Resize" || op == "Upsample") {
+            rten_resize_params p;
+            RTB_TRY(resize_target(o, &p));
+            st = rten_b200_resize(ctx, T(0), &p, &y);
+        } else if (op == "Concat") {
+            std::vector<const rten_tensor*> ins;
+            for (size_t i = 0; i < o.in.size(); i++)
+                if (T(i)) ins.push_back(T(i));
+            auto cs = cats.find((int)(&o - m->nodes.data()));
+            if (cs != cats.end() && cs->second.active) {
+                // the buffer is the output value already; inputs that are their slice of it are skipped by the operator
+                rten_tensor b = cs->second.buf;
+                return rten_b200_concat(ctx, ins.data(), (int)ins.size(), (int)o.n.attr_i("axis", 0), &b);
+            }
+            st = rten_b200_concat(ctx, ins.data(), (int)ins.size(), (int)o.n.attr_i("axis", 0), &y);
         } else if (op == "GlobalAveragePool" || op == "ReduceMean") {
             const rten_tensor* x = T(0);
             bool keepdims = true;
@@ -935,7 +1271,10 @@ struct Runner {
             x.owned = false;
             x.live = false;
         }
-        set_owned(o.out[0], y);
+        if (into_concat)
+            set_view(o.out[0], y, m->nodes[(size_t)o.cat_node].out[0]);
+        else
+            set_owned(o.out[0], y);
         return RTEN_OK;
     }
 };
@@ -947,7 +1286,7 @@ extern "C" rten_status rten_b200_model_run(rten_model* m, int32_t n_inputs, cons
     if (!m || (n_inputs && (!input_names || !inputs)) || n_outputs < 1 || !output_names || !outputs) return RTEN_ERR_INVALID_VALUE;
     rten_ctx* ctx = m->ctx;
     cudaSetDevice(ctx->device);
-    Runner r{m, ctx, {}};
+    Runner r{m, ctx, {}, {}};
     // reset run state
     for (ValueSlot& v : m->values) {
         if (v.kind == V_TEMP || v.kind == V_INPUT) {

@@ -1593,6 +1593,101 @@ rten_status launch_maxpool(rten_ctx* ctx, const float* x, float* y, const PoolPa
     return RTEN_OK;
 }
 
+// AveragePool (src/ops/pooling.rs:263-333, 400-416): the sum, from +0.0, of the taps inside the image in (ky, kx) order,
+// then one division by kh * kw (count_include_pad) or by the number of those taps.  Same thread mappings as MaxPool.
+__global__ void __launch_bounds__(256) avgpool_cl4_kernel(const float* __restrict__ x, float* __restrict__ y, PoolParams p,
+                                                          int count_include_pad) {
+    const int C4 = p.C >> 2;
+    const long long total = (long long)p.B * p.OH * p.OW * C4;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+        long long rem = i;
+        const int c = (int)(rem % C4) << 2;
+        rem /= C4;
+        const int ox = (int)(rem % p.OW);
+        rem /= p.OW;
+        const int oy = (int)(rem % p.OH);
+        const int b = (int)(rem / p.OH);
+        float4 s = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        int taps = 0;
+        for (int ky = 0; ky < p.kh; ky++) {
+            const int iy = oy * p.sy - p.pt + ky;
+            if (iy < 0 || iy >= p.H) continue;
+            for (int kx = 0; kx < p.kw; kx++) {
+                const int ix = ox * p.sx - p.pl + kx;
+                if (ix < 0 || ix >= p.W) continue;
+                const float4 v = *reinterpret_cast<const float4*>(x + (long long)b * p.xs_b + (long long)iy * p.xs_h + (long long)ix * p.xs_w + c);
+                s.x = __fadd_rn(s.x, v.x);
+                s.y = __fadd_rn(s.y, v.y);
+                s.z = __fadd_rn(s.z, v.z);
+                s.w = __fadd_rn(s.w, v.w);
+                taps++;
+            }
+        }
+        const float div = (float)(count_include_pad ? p.kh * p.kw : taps);
+        s.x = __fdiv_rn(s.x, div);
+        s.y = __fdiv_rn(s.y, div);
+        s.z = __fdiv_rn(s.z, div);
+        s.w = __fdiv_rn(s.w, div);
+        *reinterpret_cast<float4*>(y + (long long)b * p.ys_b + (long long)oy * p.ys_h + (long long)ox * p.ys_w + c) = s;
+    }
+}
+
+__global__ void __launch_bounds__(256) avgpool_kernel(const float* __restrict__ x, float* __restrict__ y, PoolParams p,
+                                                      int count_include_pad) {
+    const long long total = (long long)p.B * p.C * p.OH * p.OW;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+        int b, c, oy, ox;
+        long long rem = i;
+        if (p.channels_fastest) {
+            c = (int)(rem % p.C);
+            rem /= p.C;
+            ox = (int)(rem % p.OW);
+            rem /= p.OW;
+            oy = (int)(rem % p.OH);
+            b = (int)(rem / p.OH);
+        } else {
+            ox = (int)(rem % p.OW);
+            rem /= p.OW;
+            oy = (int)(rem % p.OH);
+            rem /= p.OH;
+            c = (int)(rem % p.C);
+            b = (int)(rem / p.C);
+        }
+        float s = 0.0f;
+        int taps = 0;
+        for (int ky = 0; ky < p.kh; ky++) {
+            const int iy = oy * p.sy - p.pt + ky;
+            if (iy < 0 || iy >= p.H) continue;
+            for (int kx = 0; kx < p.kw; kx++) {
+                const int ix = ox * p.sx - p.pl + kx;
+                if (ix < 0 || ix >= p.W) continue;
+                s = __fadd_rn(s, x[(long long)b * p.xs_b + (long long)c * p.xs_c + (long long)iy * p.xs_h + (long long)ix * p.xs_w]);
+                taps++;
+            }
+        }
+        y[(long long)b * p.ys_b + (long long)c * p.ys_c + (long long)oy * p.ys_h + (long long)ox * p.ys_w] =
+            __fdiv_rn(s, (float)(count_include_pad ? p.kh * p.kw : taps));
+    }
+}
+
+rten_status launch_avgpool(rten_ctx* ctx, const float* x, float* y, const PoolParams& p, int count_include_pad) {
+    const long long total = (long long)p.B * p.C * p.OH * p.OW;
+    if (total == 0) return RTEN_OK;
+    const bool cl4 = p.xs_c == 1 && p.ys_c == 1 && (p.C % 4) == 0 && (p.xs_b % 4) == 0 && (p.xs_h % 4) == 0 &&
+                     (p.xs_w % 4) == 0 && (p.ys_b % 4) == 0 && (p.ys_h % 4) == 0 && (p.ys_w % 4) == 0 &&
+                     ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;
+    if (cl4)
+        avgpool_cl4_kernel<<<ew_grid(ctx, total / 4), 256, 0, ctx->stream>>>(x, y, p, count_include_pad);
+    else
+        avgpool_kernel<<<ew_grid(ctx, total), 256, 0, ctx->stream>>>(x, y, p, count_include_pad);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail_cuda(ctx, e, "avgpool launch");
+    count_launch(ctx);
+    return RTEN_OK;
+}
+
 __global__ void __launch_bounds__(256)
 gather_rows_kernel(const float* __restrict__ table, const int* __restrict__ idx, float* __restrict__ out, long long nidx,
                    int width, long long t_rs, long long t_cs, long long rows) {

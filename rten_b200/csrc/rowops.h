@@ -89,6 +89,7 @@ struct PoolParams {
     int channels_fastest;  // thread -> element mapping that keeps warps coalesced for NHWC memory
 };
 rten_status launch_maxpool(rten_ctx* ctx, const float* x, float* y, const PoolParams& p);
+rten_status launch_avgpool(rten_ctx* ctx, const float* x, float* y, const PoolParams& p, int count_include_pad);
 rten_status launch_gather_rows(rten_ctx* ctx, const float* table, const int* idx, float* out, long long nidx,
                                int width, long long t_rs, long long t_cs, long long rows);
 

@@ -19,7 +19,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import (RTEN_DEVICE_HOST, RTEN_F32, RTEN_I8, RTEN_I32, RTEN_U8, RtenActivation, RtenAttentionParams, RtenConvParams,
-                   RtenConvTransposeParams, RtenGqaParams, RtenMhaParams, RtenTensor, RtenRnnParams)
+                   RtenConvTransposeParams, RtenGqaParams, RtenMhaParams, RtenResizeParams, RtenTensor, RtenRnnParams)
 
 _NP2RT = {np.dtype(np.float32): RTEN_F32, np.dtype(np.int32): RTEN_I32, np.dtype(np.int8): RTEN_I8,
           np.dtype(np.uint8): RTEN_U8}
@@ -1007,6 +1007,81 @@ class MaxPool:
         p = (C.c_int32 * 4)(*self.padding)
         s = (C.c_int32 * 2)(*self.strides)
         ctx.check(ctx.lib.rten_b200_max_pool(ctx.handle, A.t(x), k, p, s, C.byref(o)))
+        return A.wrap(o, out)
+
+
+class AveragePool:
+    """src/ops/pooling.rs AveragePool: kernel_size, padding [t,l,b,r], strides, count_include_pad."""
+
+    def __init__(self, kernel_size, padding=(0, 0, 0, 0), strides=(1, 1), count_include_pad=False):
+        self.kernel_size, self.padding, self.strides = tuple(kernel_size), tuple(padding), tuple(strides)
+        self.count_include_pad = bool(count_include_pad)
+
+    def run(self, ctx, x, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        k = (C.c_int32 * 2)(*self.kernel_size)
+        p = (C.c_int32 * 4)(*self.padding)
+        s = (C.c_int32 * 2)(*self.strides)
+        ctx.check(ctx.lib.rten_b200_average_pool(ctx.handle, A.t(x), k, p, s, int(self.count_include_pad), C.byref(o)))
+        return A.wrap(o, out)
+
+
+RESIZE_MODES = {"nearest": 0, "linear": 1}
+RESIZE_COORD_MODES = {"half_pixel": 0, "asymmetric": 1, "align_corners": 2, "pytorch_half_pixel": 3}
+RESIZE_NEAREST_MODES = {"floor": 0, "ceil": 1, "round_prefer_floor": 2, "round_prefer_ceil": 3}
+
+
+class Resize:
+    """src/ops/resize.rs Resize: `scales` or `sizes`, one value per input axis (the ONNX defaults: nearest, half_pixel,
+    round_prefer_floor)."""
+
+    def __init__(self, mode="nearest", coord_mode="half_pixel", nearest_mode="round_prefer_floor"):
+        self.mode, self.coord_mode, self.nearest_mode = mode, coord_mode, nearest_mode
+
+    def run(self, ctx, x, scales=None, sizes=None, out=None):
+        if scales is None and sizes is None:
+            raise OpError(4, "missing inputs")
+        A = _Args(ctx)
+        o = A.out(out)
+        p = RtenResizeParams()
+        p.mode = RESIZE_MODES[self.mode]
+        p.coord_mode = RESIZE_COORD_MODES[self.coord_mode]
+        p.nearest_mode = RESIZE_NEAREST_MODES[self.nearest_mode]
+        target = list(scales if scales is not None else sizes)
+        p.n = len(target)
+        p.use_sizes = int(scales is None)
+        for i, v in enumerate(target[:4]):
+            if scales is not None:
+                p.scales[i] = float(v)
+            else:
+                p.sizes[i] = int(v)
+        ctx.check(ctx.lib.rten_b200_resize(ctx.handle, A.t(x), C.byref(p), C.byref(o)))
+        return A.wrap(o, out)
+
+
+class Upsample(Resize):
+    """src/ops/resize.rs:616-643 Upsample: Resize by scales with the asymmetric transform and floor rounding."""
+
+    def __init__(self, mode="nearest"):
+        super().__init__(mode, "asymmetric", "floor")
+
+    def run(self, ctx, x, scales, out=None):
+        return super().run(ctx, x, scales=scales, out=out)
+
+
+class Concat:
+    """src/ops/concat.rs Concat along `axis`."""
+
+    def __init__(self, axis):
+        self.axis = int(axis)
+
+    def run(self, ctx, inputs, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        refs = [A.t(t) for t in inputs]
+        arr = (C.POINTER(RtenTensor) * max(len(refs), 1))(*[C.cast(r, C.POINTER(RtenTensor)) for r in refs])
+        ctx.check(ctx.lib.rten_b200_concat(ctx.handle, arr, len(refs), self.axis, C.byref(o)))
         return A.wrap(o, out)
 
 
