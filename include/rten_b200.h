@@ -687,8 +687,11 @@ rten_status rten_b200_scatter_rows(rten_ctx* ctx, rten_tensor* table, const rten
  * MultiHeadAttention (com.microsoft; outputs 0-2; a missing num_heads, an explicit scale <= 0, inputs 8 / 9 and the
  * qk output 3 fail the load; the executor allocates new present caches), GRU / LSTM (outputs 0-2; constant W prepacked at
  * load; activation_alpha / activation_beta, non-default activations, clip != 0, layout != 0, LSTM input_forget != 0, a
- * missing hidden_size and a non-empty peephole input fail the load), Constant and the view operators; anything else fails the LOAD with
- * RTEN_ERR_UNSUPPORTED_VALUE ("unsupported operator <name>"). */
+ * missing hidden_size and a non-empty peephole input fail the load), Constant and the view operators.  MatMulNBits,
+ * GroupQueryAttention, MultiHeadAttention and the two Skip norms are com.microsoft operators, Gelu is both, every other
+ * one is of the default domain ("" or "ai.onnx"); any other (domain, operator) pair fails the LOAD with
+ * RTEN_ERR_UNSUPPORTED_VALUE ("unsupported operator <name>", "com.microsoft.<name>" in that domain), and any other
+ * domain with "unsupported operator domain '<domain>'". */
 typedef struct rten_model rten_model;
 rten_status rten_b200_model_load(rten_ctx* ctx, const void* onnx_bytes, size_t len, rten_model** out);
 void rten_b200_model_free(rten_model* model);

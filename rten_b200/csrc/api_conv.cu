@@ -875,18 +875,12 @@ AxisPhase axis_phase(int64_t H, int64_t OH, int64_t k, int64_t s, int64_t d, int
     return a;
 }
 
-// Validated geometry of a transposed convolution (2-D form: a 1-D one runs over a height-1 image)
-struct ConvTShape {
-    rten_tensor x, w;
-    bool one_d = false;
-    int64_t B, C, H, W, O, Og, Cg, kh, kw, OH, OW, sy, sx, dy, dx, pt, pl, pb, pr;
-    int groups;
-};
+}  // namespace
 
 // Argument checks in the reference's order (conv_transpose.rs:226-345, conv_transpose_output_size_and_padding
 // :144-220) on the kernel `w` (and input `x` when given)
-rten_status conv_transpose_shape(rten_ctx* ctx, const rten_tensor* xp, const rten_tensor& w0, const rten_tensor* bias,
-                                 const rten_conv_transpose_params* cp, ConvTShape& S) {
+rten_status api::conv_transpose_shape(rten_ctx* ctx, const rten_tensor* xp, const rten_tensor& w0, const rten_tensor* bias,
+                                      const rten_conv_transpose_params* cp, ConvTShape& S) {
     const bool one_d = S.one_d = xp ? xp->ndim == 3 : w0.ndim == 3;
     if (xp) S.x = *xp;
     S.w = w0;
@@ -975,6 +969,8 @@ rten_status conv_transpose_shape(rten_ctx* ctx, const rten_tensor* xp, const rte
     }
     return RTEN_OK;
 }
+
+namespace {
 
 // The sub-kernel of residue phase (ty, tx) of W (4-D view) as a conv weight [O, Th, Tw, Cg]
 rten_status pack_transpose_phase(rten_ctx* ctx, const ConvTShape& S, const AxisTaps& ty, const AxisTaps& tx, void* dst) {
@@ -1141,7 +1137,39 @@ rten_status conv_transpose_core(OpScope& sc, const rten_tensor* x_in, const rten
     return RTEN_OK;
 }
 
+// `f32 as i32` (saturating, NaN -> 0)
+int64_t f32_as_i32(float v) {
+    if (v != v) return 0;
+    if (v >= 2147483648.0f) return INT32_MAX;
+    if (v <= -2147483648.0f) return INT32_MIN;
+    return (int64_t)v;
+}
+
 }  // namespace
+
+// calc_output_size of Resize (src/ops/resize.rs:273-308).  Each value is ONE rounded f32 operation (a product, a
+// quotient), which no host compiler can contract; everything that chains operations runs on the device.
+rten_status api::resize_output_size(rten_ctx* ctx, const rten_tensor& x, const rten_resize_params* p, int64_t osz[4], float inv[4]) {
+    const int nd = x.ndim;
+    if (p->n != nd) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "scales/sizes length should equal input rank");
+    if (nd > 4) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Only 1D to 4D inputs are supported with up to two resized dimensions");
+    for (int i = 0; i < nd; i++) {
+        const volatile float in = (float)x.shape[i];
+        if (p->use_sizes) {
+            const volatile float o = (float)p->sizes[i];
+            osz[i] = p->sizes[i];
+            inv[i] = in / o;
+        } else {
+            const volatile float s = p->scales[i];
+            const volatile float prod = in * s;
+            osz[i] = f32_as_i32(floorf(prod));
+            inv[i] = 1.0f / s;
+        }
+    }
+    for (int i = 0; i < nd; i++)
+        if (osz[i] < 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "scales/sizes must be positive");
+    return RTEN_OK;
+}
 
 extern "C" {
 
@@ -1450,14 +1478,6 @@ rten_status rten_b200_average_pool(rten_ctx* ctx, const rten_tensor* x, const in
 }
 
 // ---- Resize -------------------------------------------------------------------------------------------
-// `f32 as i32` (saturating, NaN -> 0)
-static int64_t f32_as_i32(float v) {
-    if (v != v) return 0;
-    if (v >= 2147483648.0f) return INT32_MAX;
-    if (v <= -2147483648.0f) return INT32_MIN;
-    return (int64_t)v;
-}
-
 rten_status rten_b200_resize(rten_ctx* ctx, const rten_tensor* x, const rten_resize_params* p, rten_tensor* out) {
     RTB_TRY(check_ctx(ctx));
     if (!x || !p || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
@@ -1470,27 +1490,9 @@ rten_status rten_b200_resize(rten_ctx* ctx, const rten_tensor* x, const rten_res
     rten_tensor xv;
     RTB_TRY(sc.in(x, &xv));
     const int nd = xv.ndim;
-    // calc_output_size (src/ops/resize.rs:273-308).  Each value is ONE rounded f32 operation (a product, a quotient),
-    // which no host compiler can contract; everything that chains operations runs on the device.
-    if (p->n != nd) return sc.finish(fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "scales/sizes length should equal input rank"));
-    if (nd > 4) return sc.finish(fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Only 1D to 4D inputs are supported with up to two resized dimensions"));
     int64_t osz[4] = {0, 0, 0, 0};
     float inv[4] = {1.0f, 1.0f, 1.0f, 1.0f};
-    for (int i = 0; i < nd; i++) {
-        const volatile float in = (float)xv.shape[i];
-        if (p->use_sizes) {
-            const volatile float o = (float)p->sizes[i];
-            osz[i] = p->sizes[i];
-            inv[i] = in / o;
-        } else {
-            const volatile float s = p->scales[i];
-            const volatile float prod = in * s;
-            osz[i] = f32_as_i32(floorf(prod));
-            inv[i] = 1.0f / s;
-        }
-    }
-    for (int i = 0; i < nd; i++)
-        if (osz[i] < 0) return sc.finish(fail(ctx, RTEN_ERR_INVALID_VALUE, "scales/sizes must be positive"));
+    if (const rten_status st = resize_output_size(ctx, xv, p, osz, inv)) return sc.finish(st);
     // resize_impl (resize.rs:350-407): which input axis plays (n, c, h, w); -1 = an added axis of size 1
     bool same = true;
     for (int i = 0; i < nd; i++) same = same && osz[i] == xv.shape[i];

@@ -65,5 +65,19 @@ inline rten_status axis_out(rten_ctx* ctx, int64_t in, int64_t k, int64_t stride
     return RTEN_OK;
 }
 
+// Validated geometry of a transposed convolution (2-D form: a 1-D one runs over a height-1 image)
+struct ConvTShape {
+    rten_tensor x, w;
+    bool one_d = false;
+    int64_t B, C, H, W, O, Og, Cg, kh, kw, OH, OW, sy, sx, dy, dx, pt, pl, pb, pr;
+    int groups;
+};
+
+// ConvTranspose's argument checks on `w` (and `x` when given) and its output geometry (api_conv.cu)
+rten_status conv_transpose_shape(rten_ctx* ctx, const rten_tensor* xp, const rten_tensor& w0, const rten_tensor* bias,
+                                 const rten_conv_transpose_params* cp, ConvTShape& S);
+// Resize's output sizes `osz` on `x` and the input / output size ratio `inv` of each axis (api_conv.cu)
+rten_status resize_output_size(rten_ctx* ctx, const rten_tensor& x, const rten_resize_params* p, int64_t osz[4], float inv[4]);
+
 }  // namespace api
 }  // namespace rtb

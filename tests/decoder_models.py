@@ -158,4 +158,13 @@ def skip_and_output(B=2, C=16, H=16, W_=16, seed=6):
     return b.build((B, 8, H, W_), [b.conv(y, C, C, relu=False), other])
 
 
-MODELS = {"unet": unet, "fpn": fpn, "aspp": aspp, "sppf": sppf, "densenet": densenet, "skip_and_output": skip_and_output}
+def upsample_concat(B=2, C=16, H=16, W_=16, seed=7):
+    """A Resize by scales (nearest x2) and a skip convolution concatenated: both write their channel slice in place."""
+    b = _Builder(seed)
+    skip = b.conv("x", 8, C)
+    up = b.op("Resize", [b.conv(skip, C, C, stride=2), "", b.const(np.array([1, 1, 2, 2], np.float32), "s")], mode="nearest")
+    return b.build((B, 8, H, W_), [b.conv(b.op("Concat", [up, skip], axis=1), 2 * C, C, k=1, relu=False)])
+
+
+MODELS = {"unet": unet, "fpn": fpn, "aspp": aspp, "sppf": sppf, "densenet": densenet, "skip_and_output": skip_and_output,
+          "upsample_concat": upsample_concat}
