@@ -67,8 +67,8 @@ attn_fused_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_consta
         fence_mbar_init();
     }
     __syncthreads();
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    pdl_wait();
+    pdl_launch_dependents();
 
     if (warp == 4) {
         if (elect_one()) {
@@ -281,24 +281,8 @@ rten_status launch_attn_fused(rten_ctx* ctx, const AttnFusedLaunch& L) {
     mv = mq;  // (unused when the kernel transposes a natural V itself)
     if (!L.v && !encode_map(ctx, &mv, L.vt, 4, true, vbox, ones)) return RTEN_ERR_UNSUPPORTED_VALUE;
     const size_t smem = 1024 + 1024 + ACC_SMEM_BYTES + 4 * (size_t)TILE + 4 * (size_t)VT_TILE;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(L.B * L.heads * p.q_tiles);
-    cfg.blockDim = dim3(AF_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = getenv("RTEN_B200_NO_PDL") ? 0 : 1;
-    cudaError_t e = cudaFuncSetAttribute(attn_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) e = cudaLaunchKernelEx(&cfg, attn_fused_kernel, mq, mk, mv, p);
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "fused attention launch");
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "fused attention launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "fused attention launch", attn_fused_kernel, {L.B * L.heads * p.q_tiles, AF_THREADS, smem, (int)smem, true}, mq,
+                  mk, mv, p);
 }
 
 }  // namespace rtb

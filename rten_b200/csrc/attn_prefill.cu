@@ -150,8 +150,8 @@ __device__ __forceinline__ void attn_prefill_body(const CUtensorMap& tma_q, cons
         fence_mbar_init();
     }
     __syncthreads();
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    pdl_wait();
+    pdl_launch_dependents();
 
     // keys [0, lim) exist for every row; a causal row s sees keys [0, s + off]
     const int lim = p.len ? min(max(__ldg(p.len + b), 0), p.kv_seq) : p.kv_seq;
@@ -385,25 +385,9 @@ rten_status launch_cfg(rten_ctx* ctx, const AttnPrefillLaunch& L, const AttnPref
     if (!encode_map(ctx, &mq, L.q, 4, true, qbox, ones) || !encode_map(ctx, &mk, L.k, 4, true, kbox, ones) ||
         !encode_map(ctx, &mv, L.v, 4, true, vbox, ones))
         return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "prefill attention: the tensor maps of query, key or value could not be encoded");
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)((long long)L.B * L.q_heads * p.q_tiles));
-    cfg.blockDim = dim3(AP_THREADS);
-    cfg.dynamicSmemBytes = C::SMEM;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = getenv("RTEN_B200_NO_PDL") ? 0 : 1;
     auto kernel = L.mha ? attn_prefill_mha_kernel<DH, X3> : attn_prefill_kernel<DH, X3>;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
-    if (e == cudaSuccess) e = cudaLaunchKernelEx(&cfg, kernel, mq, mk, mv, p);
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "prefill attention launch");
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "prefill attention launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "prefill attention launch", kernel,
+                  {(unsigned)((long long)L.B * L.q_heads * p.q_tiles), AP_THREADS, C::SMEM, (int)C::SMEM, true}, mq, mk, mv, p);
 }
 
 }  // namespace

@@ -17,6 +17,7 @@
 
 #include "comm_device.cuh"
 #include "common.h"
+#include "ptx.cuh"
 
 struct Id128 {  // ncclUniqueId: 128 opaque bytes, passed BY VALUE to ncclCommInitRank
     char bytes[128];
@@ -64,7 +65,7 @@ constexpr int kNcclMin = 3;    // ncclMin
 
 // mm[0] / mm[1]: ordered-int encodings of the local min / max (integer order == float order)
 __global__ void __launch_bounds__(32) peer_minmax_kernel(int* mm, const PeerTable peers, int rank, int world) {
-    asm volatile("griddepcontrol.wait;" ::: "memory");
+    pdl_wait();
     peer_minmax_warp(mm, peers, rank, world);
 }
 
@@ -84,23 +85,11 @@ namespace rtb {
 // min / max on that encoding is the float min / max, and is exact and order independent.
 rten_status comm_allreduce_minmax(rten_ctx* ctx, rten_comm* comm, int* mm) {
     if (!comm || comm->world <= 1) return RTEN_OK;
+    if (comm->peer_ok)
+        return launch(ctx, "peer min/max exchange launch", peer_minmax_kernel, {1, 32, 0, 0, true}, mm, comm->peers, comm->rank,
+                      comm->world);
+    // NCCL launches its own kernels, so its two all-reduces are counted here
     cudaStream_t s = ctx->stream;
-    if (comm->peer_ok) {
-        cudaLaunchConfig_t cfg;
-        memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = dim3(1);
-        cfg.blockDim = dim3(32);
-        cfg.stream = s;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = getenv("RTEN_B200_NO_PDL") ? 0 : 1;
-        cudaError_t e = cudaLaunchKernelEx(&cfg, peer_minmax_kernel, mm, comm->peers, comm->rank, comm->world);
-        if (e != cudaSuccess) return fail_cuda(ctx, e, "peer min/max exchange launch");
-        count_launch(ctx);
-        return RTEN_OK;
-    }
     int r = g_nccl.AllReduce(mm, mm, 1, kNcclInt32, kNcclMin, comm->nccl, s);
     if (r == 0) r = g_nccl.AllReduce(mm + 1, mm + 1, 1, kNcclInt32, kNcclMax, comm->nccl, s);
     if (r != 0) {

@@ -7,6 +7,7 @@
 #include <array>
 #include <cstdint>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <map>
 #include <string>
@@ -140,6 +141,41 @@ inline int64_t span_elems(const rten_tensor* t) {
 }
 
 inline void count_launch(rten_ctx* ctx, int n = 1) { ctx->launches += (uint64_t)n; }
+
+// ---- kernel launch ------------------------------------------------------------------------
+struct LaunchShape {
+    dim3 grid, block;
+    size_t smem = 0;     // dynamic shared memory, bytes
+    int smem_optin = 0;  // > 0: the kernel's MaxDynamicSharedMemorySize is set to this before the launch
+    bool pdl = false;    // programmatic dependent launch: the kernel must pdl_wait() (ptx.cuh) before it reads its inputs
+};
+
+// Launches `kern` on the context stream and counts it.  A failed launch returns RTEN_ERR_CUDA with `what` in the
+// message, is not counted, and leaves no pending error behind for the next launch's check.
+// RTEN_B200_NO_PDL turns programmatic dependent launch off for every kernel.
+template <typename... P, typename... A>
+rten_status launch(rten_ctx* ctx, const char* what, void (*kern)(P...), const LaunchShape& s, A&&... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = s.grid;
+    cfg.blockDim = s.block;
+    cfg.dynamicSmemBytes = s.smem;
+    cfg.stream = ctx->stream;
+    cudaLaunchAttribute attr[1];
+    if (s.pdl && !getenv("RTEN_B200_NO_PDL")) {
+        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[0].val.programmaticStreamSerializationAllowed = 1;
+        cfg.attrs = attr;
+        cfg.numAttrs = 1;
+    }
+    cudaError_t e = cudaSuccess;
+    if (s.smem_optin > 0) e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, s.smem_optin);
+    if (e == cudaSuccess) e = cudaLaunchKernelEx(&cfg, kern, std::forward<A>(args)...);
+    const cudaError_t last = cudaGetLastError();
+    if (e == cudaSuccess) e = last;
+    if (e != cudaSuccess) return fail_cuda(ctx, e, what);
+    count_launch(ctx);
+    return RTEN_OK;
+}
 
 // cross-rank min / max of the DynamicQuantizeLinear range (comm.cu)
 rten_status comm_allreduce_minmax(rten_ctx* ctx, struct ::rten_comm* comm, int* mm);

@@ -302,20 +302,13 @@ rten_status launch_typed(rten_ctx* ctx, const DepthwiseParams& p) {
         if (gx > INT_MAX || gy > 65535) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "depthwise convolution is too large");
         const dim3 grid((unsigned)gx, (unsigned)gy);
         const size_t sb = use_smem ? (size_t)smem : 0;
-        if (vec)
-            depthwise_cl_kernel<XT, WT, OUT, 4><<<grid, kThreads, sb, ctx->stream>>>(p, nv, runs, use_smem, npix);
-        else
-            depthwise_cl_kernel<XT, WT, OUT, 1><<<grid, kThreads, sb, ctx->stream>>>(p, nv, runs, use_smem, npix);
-    } else {
-        const long long n = npix * p.C;
-        const long long g = (n + kThreads - 1) / kThreads;
-        if (g > INT_MAX) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "depthwise convolution is too large");
-        depthwise_planar_kernel<XT, WT, OUT><<<(unsigned)g, kThreads, 0, ctx->stream>>>(p, n);
+        auto kern = vec ? depthwise_cl_kernel<XT, WT, OUT, 4> : depthwise_cl_kernel<XT, WT, OUT, 1>;
+        return launch(ctx, "depthwise convolution launch", kern, {grid, kThreads, sb}, p, nv, runs, use_smem, npix);
     }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "depthwise convolution launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    const long long n = npix * p.C;
+    const long long g = (n + kThreads - 1) / kThreads;
+    if (g > INT_MAX) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "depthwise convolution is too large");
+    return launch(ctx, "depthwise convolution launch", depthwise_planar_kernel<XT, WT, OUT>, {(unsigned)g, kThreads}, p, n);
 }
 
 template <typename XT, typename WT>

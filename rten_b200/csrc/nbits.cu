@@ -57,8 +57,8 @@ __global__ void __launch_bounds__(SK_THREADS, MT <= 8 ? 2 : 1) nbits_skinny_kern
     const int K = L.K, M = L.M, N = L.N;
     const int lb = __ffs(L.block) - 1;
     constexpr int F = KC / 4;
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    pdl_wait();
+    pdl_launch_dependents();
     for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x) {
         const int n0 = tile * 8 * CPW + warp * CPW;
         float acc[MT * CPW];
@@ -144,40 +144,14 @@ __global__ void __launch_bounds__(SK_THREADS, MT <= 8 ? 2 : 1) nbits_skinny_kern
     }
 }
 
-template <int MT, int CPW>
-cudaError_t go_skinny(rten_ctx* ctx, const NbitsLaunch& L) {
+rten_status launch_skinny(rten_ctx* ctx, const NbitsLaunch& L) {
+    const int mt = L.M <= 8 ? 8 : (L.M <= 16 ? 16 : 32), cpw = mt == 32 ? 2 : 4;
     SkinnyParams p;
     p.L = L;
-    p.tiles = (L.N + 8 * CPW - 1) / (8 * CPW);
-    const size_t smem = (size_t)MT * KC * sizeof(float);
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)std::min(p.tiles, 2 * ctx->num_sms));
-    cfg.blockDim = dim3(SK_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = getenv("RTEN_B200_NO_PDL") ? 0 : 1;
-    cudaError_t e = cudaFuncSetAttribute(nbits_skinny_kernel<MT, CPW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) e = cudaLaunchKernelEx(&cfg, nbits_skinny_kernel<MT, CPW>, p);
-    return e;
-}
-
-rten_status launch_skinny(rten_ctx* ctx, const NbitsLaunch& L) {
-    cudaError_t e;
-    if (L.M <= 8)
-        e = go_skinny<8, 4>(ctx, L);
-    else if (L.M <= 16)
-        e = go_skinny<16, 4>(ctx, L);
-    else
-        e = go_skinny<32, 2>(ctx, L);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "MatMulNBits skinny launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    p.tiles = (L.N + 8 * cpw - 1) / (8 * cpw);
+    const size_t smem = (size_t)mt * KC * sizeof(float);
+    auto kern = mt == 8 ? nbits_skinny_kernel<8, 4> : (mt == 16 ? nbits_skinny_kernel<16, 4> : nbits_skinny_kernel<32, 2>);
+    return launch(ctx, "MatMulNBits skinny launch", kern, {std::min(p.tiles, 2 * ctx->num_sms), SK_THREADS, smem, (int)smem, true}, p);
 }
 
 // =====================================================================================================================
@@ -261,8 +235,8 @@ nbits_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
         fence_mbar_init();
     }
     __syncthreads();
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    pdl_wait();
+    pdl_launch_dependents();
 
     if (warp == 8) {
         if (elect_one()) {
@@ -399,23 +373,8 @@ rten_status launch_wgmma(rten_ctx* ctx, const NbitsLaunch& L) {
     p.out = L.out;
     p.os = L.os;
     if ((long long)p.mtiles * p.ntiles > 0x7fffffffll) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MatMulNBits: too many output tiles");
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)(p.mtiles * p.ntiles));
-    cfg.blockDim = dim3(WG_THREADS);
-    cfg.dynamicSmemBytes = WCfg<X3>::SMEM;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = getenv("RTEN_B200_NO_PDL") ? 0 : 1;
-    cudaError_t e = cudaFuncSetAttribute(nbits_wgmma_kernel<X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WCfg<X3>::SMEM);
-    if (e == cudaSuccess) e = cudaLaunchKernelEx(&cfg, nbits_wgmma_kernel<X3>, ma, mq, p);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "MatMulNBits wgmma launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "MatMulNBits wgmma launch", nbits_wgmma_kernel<X3>,
+                  {(unsigned)(p.mtiles * p.ntiles), WG_THREADS, WCfg<X3>::SMEM, (int)WCfg<X3>::SMEM, true}, ma, mq, p);
 }
 
 }  // namespace

@@ -25,6 +25,12 @@ __device__ __forceinline__ bool elect_one() {
     return pred != 0;
 }
 
+// ------------------------------------------------------------------ programmatic dependent launch
+// A kernel launched with LaunchShape::pdl may start while its predecessor is still running: it must pdl_wait() before
+// it reads the predecessor's output.  pdl_launch_dependents() lets the next kernel start its own set-up.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
 // ------------------------------------------------------------------ mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");

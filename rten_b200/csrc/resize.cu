@@ -218,30 +218,14 @@ rten_status launch_resize(rten_ctx* ctx, const ResizeParams& p) {
     const bool out16 = (reinterpret_cast<uintptr_t>(p.out) & 15) == 0;
     const bool cl4 = p.xs[1] == 1 && p.os[1] == 1 && p.C % 4 == 0 && aligned4(p.xs, 0, 2, 3) && aligned4(p.os, 0, 2, 3) &&
                      (reinterpret_cast<uintptr_t>(p.x) & 15) == 0 && out16;
-    if (cl4) {
-        const int grid = grid_for(ctx, total / 4);
-        if (linear)
-            resize_cl4_kernel<true><<<grid, 256, 0, ctx->stream>>>(p);
-        else
-            resize_cl4_kernel<false><<<grid, 256, 0, ctx->stream>>>(p);
-    } else if (p.os[1] == 1 && p.C > 1) {
-        const int grid = grid_for(ctx, total);
-        if (linear)
-            resize_kernel<true, false><<<grid, 256, 0, ctx->stream>>>(p, 0);
-        else
-            resize_kernel<false, false><<<grid, 256, 0, ctx->stream>>>(p, 0);
-    } else {
-        const int vec = p.os[3] == 1 && aligned4(p.os, 0, 1, 2) && out16;
-        const int grid = grid_for(ctx, (long long)p.B * p.C * p.OH * ((p.OW + 3) / 4));
-        if (linear)
-            resize_kernel<true, true><<<grid, 256, 0, ctx->stream>>>(p, vec);
-        else
-            resize_kernel<false, true><<<grid, 256, 0, ctx->stream>>>(p, vec);
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "resize launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    const char* what = "resize launch";
+    if (cl4)
+        return launch(ctx, what, linear ? resize_cl4_kernel<true> : resize_cl4_kernel<false>, {grid_for(ctx, total / 4), 256}, p);
+    if (p.os[1] == 1 && p.C > 1)
+        return launch(ctx, what, linear ? resize_kernel<true, false> : resize_kernel<false, false>, {grid_for(ctx, total), 256}, p, 0);
+    const int vec = p.os[3] == 1 && aligned4(p.os, 0, 1, 2) && out16;
+    const int grid = grid_for(ctx, (long long)p.B * p.C * p.OH * ((p.OW + 3) / 4));
+    return launch(ctx, what, linear ? resize_kernel<true, true> : resize_kernel<false, true>, {grid, 256}, p, vec);
 }
 
 rten_status launch_concat(rten_ctx* ctx, const ConcatParams& p) {
@@ -249,16 +233,8 @@ rten_status launch_concat(rten_ctx* ctx, const ConcatParams& p) {
     for (int i = 0; i < p.nsrc; i++) most = std::max(most, p.s[i].n);
     if (p.nsrc == 0 || most == 0) return RTEN_OK;
     const dim3 grid((unsigned)grid_for(ctx, most), (unsigned)p.nsrc);
-    if (p.esize == 16)
-        concat_kernel<uint4><<<grid, 256, 0, ctx->stream>>>(p);
-    else if (p.esize == 4)
-        concat_kernel<uint32_t><<<grid, 256, 0, ctx->stream>>>(p);
-    else
-        concat_kernel<uint8_t><<<grid, 256, 0, ctx->stream>>>(p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "concat launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    auto kern = p.esize == 16 ? concat_kernel<uint4> : (p.esize == 4 ? concat_kernel<uint32_t> : concat_kernel<uint8_t>);
+    return launch(ctx, "concat launch", kern, {grid, 256}, p);
 }
 
 }  // namespace rtb

@@ -255,6 +255,7 @@ rten_status launch_cluster_t(rten_ctx* ctx, const ClusterPlan& P, const ClusterP
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
+    // not launch(): the occupancy query must see this exact cluster config, and its failure means "use the per-step path"
     int active = 0;
     e = cudaOccupancyMaxActiveClusters(&active, kern, &cfg);
     if (e != cudaSuccess || active < 1) {
@@ -357,25 +358,15 @@ rten_status launch_rnn_state_init(rten_ctx* ctx, const RnnLaunch& L, float* h, f
     const long long n = (long long)L.dirs * L.B * L.H;
     if (n == 0) return RTEN_OK;
     const int grid = (int)std::min<long long>((n + 255) / 256, 4LL * ctx->num_sms);
-    rnn_state_init_kernel<<<grid, 256, 0, ctx->stream>>>(L, h, c, ld);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "rnn_state_init_kernel launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "rnn_state_init_kernel launch", rnn_state_init_kernel, {grid, 256}, L, h, c, ld);
 }
 
 rten_status launch_rnn_step_gates(rten_ctx* ctx, const RnnLaunch& L, int s, const float* rec, float* h, float* c, int ld) {
     const long long n = (long long)L.dirs * L.B * L.H;
     if (n == 0) return RTEN_OK;
     const long long grid = (n + 255) / 256;
-    if (L.gru)
-        rnn_step_gates_kernel<true><<<(unsigned)grid, 256, 0, ctx->stream>>>(L, s, rec, h, c, ld);
-    else
-        rnn_step_gates_kernel<false><<<(unsigned)grid, 256, 0, ctx->stream>>>(L, s, rec, h, c, ld);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "rnn_step_gates_kernel launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "rnn_step_gates_kernel launch", L.gru ? rnn_step_gates_kernel<true> : rnn_step_gates_kernel<false>,
+                  {(unsigned)grid, 256}, L, s, rec, h, c, ld);
 }
 
 }  // namespace rtb

@@ -135,14 +135,8 @@ rten_status launch_rotary(rten_ctx* ctx, const RotaryLaunch& L) {
     const long long rows = p.nq + p.nk + p.nv + p.nbuilt;
     const long long grid = std::max<long long>(1, (rows + RT_WARPS - 1) / RT_WARPS);
     if (grid > 0x7fffffffll) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "rotary embedding: too many rows for one launch");
-    if (L.mha)
-        rotary_mha_kernel<<<(unsigned)grid, RT_WARPS * 32, 0, ctx->stream>>>(p, L);
-    else
-        rotary_kernel<<<(unsigned)grid, RT_WARPS * 32, 0, ctx->stream>>>(p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "rotary launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    if (L.mha) return launch(ctx, "rotary launch", rotary_mha_kernel, {(unsigned)grid, RT_WARPS * 32}, p, L);
+    return launch(ctx, "rotary launch", rotary_kernel, {(unsigned)grid, RT_WARPS * 32}, p);
 }
 
 }  // namespace rtb

@@ -272,27 +272,17 @@ rten_status launch_softmax(rten_ctx* ctx, const float* x, float* y, long long ro
         const unsigned blocks = (unsigned)((warps + vwpb - 1) / vwpb);
         const int F = n / (16 * S);
         const int fm = F <= 2 ? 2 : (F <= 4 ? 4 : (F <= 8 ? 8 : 16));
-        cudaStream_t st = ctx->stream;
-#define RTB_SOFTMAX_CASE(SS, FF) \
-    case SS * 100 + FF: softmax_vec_kernel<SS, FF><<<blocks, vwpb * 32, 0, st>>>(p); break;
-        switch (S * 100 + fm) {
-            RTB_SOFTMAX_CASE(1, 2) RTB_SOFTMAX_CASE(1, 4) RTB_SOFTMAX_CASE(1, 8) RTB_SOFTMAX_CASE(1, 16)
-            RTB_SOFTMAX_CASE(2, 2) RTB_SOFTMAX_CASE(2, 4) RTB_SOFTMAX_CASE(2, 8) RTB_SOFTMAX_CASE(2, 16)
-            RTB_SOFTMAX_CASE(4, 2) RTB_SOFTMAX_CASE(4, 4) RTB_SOFTMAX_CASE(4, 8) RTB_SOFTMAX_CASE(4, 16)
-            RTB_SOFTMAX_CASE(8, 2) RTB_SOFTMAX_CASE(8, 4) RTB_SOFTMAX_CASE(8, 8) RTB_SOFTMAX_CASE(8, 16)
-        }
-#undef RTB_SOFTMAX_CASE
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return fail_cuda(ctx, e, "softmax launch");
-        count_launch(ctx);
-        return RTEN_OK;
+        using Kernel = void (*)(SoftmaxParams);
+        // [log2 S][log2 fm - 1]
+        static const Kernel vec[4][4] = {
+            {softmax_vec_kernel<1, 2>, softmax_vec_kernel<1, 4>, softmax_vec_kernel<1, 8>, softmax_vec_kernel<1, 16>},
+            {softmax_vec_kernel<2, 2>, softmax_vec_kernel<2, 4>, softmax_vec_kernel<2, 8>, softmax_vec_kernel<2, 16>},
+            {softmax_vec_kernel<4, 2>, softmax_vec_kernel<4, 4>, softmax_vec_kernel<4, 8>, softmax_vec_kernel<4, 16>},
+            {softmax_vec_kernel<8, 2>, softmax_vec_kernel<8, 4>, softmax_vec_kernel<8, 8>, softmax_vec_kernel<8, 16>}};
+        return launch(ctx, "softmax launch", vec[__builtin_ctz(S)][__builtin_ctz(fm) - 1], {blocks, vwpb * 32}, p);
     }
     const long long blocks = (rows + wpb - 1) / wpb;
-    softmax_kernel<<<(unsigned)blocks, wpb * 32, 0, ctx->stream>>>(p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "softmax launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "softmax launch", softmax_kernel, {(unsigned)blocks, wpb * 32}, p);
 }
 
 // =========================================================================================
@@ -448,22 +438,15 @@ rten_status launch_layer_norm(rten_ctx* ctx, const float* x, float* y, long long
         const unsigned blocks = (unsigned)((warps + vwpb - 1) / vwpb);
         const int F = n / (64 * S);
         const int fm = F <= 4 ? 4 : (F <= 8 ? 8 : (F <= 12 ? 12 : 16));
-        cudaStream_t st = ctx->stream;
-#define RTB_LN_CASE(SS, FF) \
-    case SS * 100 + FF: layer_norm_vec_kernel<SS, FF><<<blocks, vwpb * 32, 0, st>>>(p); break;
-        switch (S * 100 + fm) {
-            RTB_LN_CASE(1, 4) RTB_LN_CASE(1, 8) RTB_LN_CASE(1, 12) RTB_LN_CASE(1, 16)
-            RTB_LN_CASE(2, 4) RTB_LN_CASE(2, 8) RTB_LN_CASE(2, 12) RTB_LN_CASE(2, 16)
-        }
-#undef RTB_LN_CASE
-    } else {
-        const long long blocks = (rows + wpb - 1) / wpb;
-        layer_norm_kernel<<<(unsigned)blocks, wpb * 32, 0, ctx->stream>>>(p);
+        using Kernel = void (*)(LayerNormParams);
+        // [S - 1][fm / 4 - 1]
+        static const Kernel vec[2][4] = {
+            {layer_norm_vec_kernel<1, 4>, layer_norm_vec_kernel<1, 8>, layer_norm_vec_kernel<1, 12>, layer_norm_vec_kernel<1, 16>},
+            {layer_norm_vec_kernel<2, 4>, layer_norm_vec_kernel<2, 8>, layer_norm_vec_kernel<2, 12>, layer_norm_vec_kernel<2, 16>}};
+        return launch(ctx, "layer_norm launch", vec[S - 1][fm / 4 - 1], {blocks, vwpb * 32}, p);
     }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "layer_norm launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    const long long blocks = (rows + wpb - 1) / wpb;
+    return launch(ctx, "layer_norm launch", layer_norm_kernel, {(unsigned)blocks, wpb * 32}, p);
 }
 
 // =========================================================================================
@@ -639,23 +622,18 @@ __global__ void __launch_bounds__(256) skip_norm_kernel(const SkipNormParams p) 
         y[i] = norm_arm(mode, y[i], mean, rstd, p.gamma ? p.gamma[i] : 1.0f, p.beta ? p.beta[i] : 0.0f, beta_scalar);
 }
 
+using SkipNormKernel = void (*)(SkipNormParams);
+
 template <int FL>
-static void launch_skip_norm_fl(const SkipNormParams& p, int S, int fm, int vpt, unsigned blocks, cudaStream_t st) {
-    if (vpt) {
-        const size_t smem = (size_t)p.n * 4;
-        switch (vpt) {
-            case 4: skip_norm_wide_kernel<4, FL><<<blocks, WIDE_THREADS, smem, st>>>(p); break;
-            default: skip_norm_wide_kernel<8, FL><<<blocks, WIDE_THREADS, smem, st>>>(p); break;
-        }
-        return;
-    }
+static SkipNormKernel skip_norm_fl_kernel(int S, int fm, int vpt) {
+    if (vpt) return vpt == 4 ? skip_norm_wide_kernel<4, FL> : skip_norm_wide_kernel<8, FL>;
     switch (S * 100 + fm) {
-        case 104: skip_norm_vec_kernel<1, 4, FL><<<blocks, 128, 0, st>>>(p); break;
-        case 108: skip_norm_vec_kernel<1, 8, FL><<<blocks, 128, 0, st>>>(p); break;
-        case 116: skip_norm_vec_kernel<1, 16, FL><<<blocks, 128, 0, st>>>(p); break;
-        case 204: skip_norm_vec_kernel<2, 4, FL><<<blocks, 128, 0, st>>>(p); break;
-        case 208: skip_norm_vec_kernel<2, 8, FL><<<blocks, 128, 0, st>>>(p); break;
-        default: skip_norm_vec_kernel<2, 16, FL><<<blocks, 128, 0, st>>>(p); break;
+        case 104: return skip_norm_vec_kernel<1, 4, FL>;
+        case 108: return skip_norm_vec_kernel<1, 8, FL>;
+        case 116: return skip_norm_vec_kernel<1, 16, FL>;
+        case 204: return skip_norm_vec_kernel<2, 4, FL>;
+        case 208: return skip_norm_vec_kernel<2, 8, FL>;
+        default: return skip_norm_vec_kernel<2, 16, FL>;
     }
 }
 
@@ -668,7 +646,6 @@ rten_status launch_skip_norm(rten_ctx* ctx, const SkipNormParams& p) {
                         al16(p.sum) && p.rows < 0x7fffffffLL;
     const int fl = (p.rms ? NORM_RMS : 0) | (p.skip ? NORM_SKIP : 0) | (p.bias ? NORM_BIAS : 0) | (p.sum ? NORM_SUM : 0);
     const bool flags_ok = p.skip || (!p.bias && !p.sum);  // (no bias or sum output without a skip input)
-    cudaStream_t st = ctx->stream;
     if (vec_ok && flags_ok && n <= 8192) {
         int S = 0, fm = 0, vpt = 0;
         unsigned blocks;
@@ -689,11 +666,12 @@ rten_status launch_skip_norm(rten_ctx* ctx, const SkipNormParams& p) {
             vpt = n <= 4 * 4 * WIDE_THREADS ? 4 : 8;  // float4s per thread
             blocks = (unsigned)p.rows;
         }
+        SkipNormKernel kern;
         switch (fl) {
-            case NORM_RMS: launch_skip_norm_fl<NORM_RMS>(p, S, fm, vpt, blocks, st); break;
+            case NORM_RMS: kern = skip_norm_fl_kernel<NORM_RMS>(S, fm, vpt); break;
 #define RTB_SKIP_NORM_CASE(F) \
-    case F: launch_skip_norm_fl<F>(p, S, fm, vpt, blocks, st); break; \
-    case F | NORM_RMS: launch_skip_norm_fl<F | NORM_RMS>(p, S, fm, vpt, blocks, st); break;
+    case F: kern = skip_norm_fl_kernel<F>(S, fm, vpt); break; \
+    case F | NORM_RMS: kern = skip_norm_fl_kernel<F | NORM_RMS>(S, fm, vpt); break;
             RTB_SKIP_NORM_CASE(NORM_SKIP)
             RTB_SKIP_NORM_CASE(NORM_SKIP | NORM_BIAS)
             RTB_SKIP_NORM_CASE(NORM_SKIP | NORM_SUM)
@@ -701,14 +679,11 @@ rten_status launch_skip_norm(rten_ctx* ctx, const SkipNormParams& p) {
 #undef RTB_SKIP_NORM_CASE
             default: return fail(ctx, RTEN_ERR_INVALID_VALUE, "skip_norm: no kernel for these flags");
         }
-    } else {
-        const long long blocks = (p.rows + 7) / 8;
-        skip_norm_kernel<<<(unsigned)blocks, 256, 0, st>>>(p);
+        if (vpt) return launch(ctx, "skip_norm launch", kern, {blocks, WIDE_THREADS, (size_t)n * 4}, p);
+        return launch(ctx, "skip_norm launch", kern, {blocks, 128}, p);
     }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "skip_norm launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    const long long blocks = (p.rows + 7) / 8;
+    return launch(ctx, "skip_norm launch", skip_norm_kernel, {(unsigned)blocks, 256}, p);
 }
 
 // Row sums in the reference's Sum order (GlobalAveragePool = Sum / len, src/ops/pooling.rs:516-521).
@@ -778,21 +753,12 @@ row_mean_thread_kernel(const float* x, float* y, long long rows, int n, long lon
 rten_status launch_row_mean(rten_ctx* ctx, const float* x, float* y, long long rows, int n, long long rows_inner,
                             long long s_outer, long long s_inner, long long kstride) {
     if (rows == 0) return RTEN_OK;
-    if (s_inner == 1 && kstride != 1) {
-        row_mean_thread_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, ctx->stream>>>(x, y, rows, n, rows_inner, s_outer,
-                                                                                        s_inner, kstride);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return fail_cuda(ctx, e, "row_mean launch");
-        count_launch(ctx);
-        return RTEN_OK;
-    }
+    if (s_inner == 1 && kstride != 1)
+        return launch(ctx, "row_mean launch", row_mean_thread_kernel, {(unsigned)((rows + 127) / 128), 128}, x, y, rows, n,
+                      rows_inner, s_outer, s_inner, kstride);
     const int wpb = 8;
-    row_mean_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, ctx->stream>>>(x, y, rows, n, rows_inner,
-                                                                                       s_outer, s_inner, kstride);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "row_mean launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "row_mean launch", row_mean_kernel, {(unsigned)((rows + wpb - 1) / wpb), wpb * 32}, x, y, rows, n,
+                  rows_inner, s_outer, s_inner, kstride);
 }
 
 // =========================================================================================
@@ -843,22 +809,19 @@ rten_status launch_unary(rten_ctx* ctx, int op, const float* x, float* y, long l
     if (n == 0) return RTEN_OK;
     const int vec = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0 ? 1 : 0;
     const int grid = ew_grid(ctx, vec ? (n + 3) / 4 : n);
-    auto go = [&](auto kernel) { kernel<<<grid, 256, 0, ctx->stream>>>(x, y, n, vec, alpha, beta); };
+    void (*kern)(const float*, float*, long long, int, float, float);
     switch (op) {
-        case UNARY_ERF: go(unary_kernel<UNARY_ERF>); break;
-        case UNARY_GELU: go(unary_kernel<UNARY_GELU>); break;
-        case UNARY_APPROX_GELU: go(unary_kernel<UNARY_APPROX_GELU>); break;
-        case UNARY_RELU: go(unary_kernel<UNARY_RELU>); break;
-        case UNARY_SIGMOID: go(unary_kernel<UNARY_SIGMOID>); break;
-        case UNARY_SILU: go(unary_kernel<UNARY_SILU>); break;
-        case UNARY_HARD_SIGMOID: go(unary_kernel<UNARY_HARD_SIGMOID>); break;
-        case UNARY_HARD_SWISH: go(unary_kernel<UNARY_HARD_SWISH>); break;
+        case UNARY_ERF: kern = unary_kernel<UNARY_ERF>; break;
+        case UNARY_GELU: kern = unary_kernel<UNARY_GELU>; break;
+        case UNARY_APPROX_GELU: kern = unary_kernel<UNARY_APPROX_GELU>; break;
+        case UNARY_RELU: kern = unary_kernel<UNARY_RELU>; break;
+        case UNARY_SIGMOID: kern = unary_kernel<UNARY_SIGMOID>; break;
+        case UNARY_SILU: kern = unary_kernel<UNARY_SILU>; break;
+        case UNARY_HARD_SIGMOID: kern = unary_kernel<UNARY_HARD_SIGMOID>; break;
+        case UNARY_HARD_SWISH: kern = unary_kernel<UNARY_HARD_SWISH>; break;
         default: return fail(ctx, RTEN_ERR_INVALID_VALUE, "unknown unary op");
     }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "unary launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "unary launch", kern, {grid, 256}, x, y, n, vec, alpha, beta);
 }
 
 // General N-d strided kernels (up to 8 dims): copy / broadcast add.  Used for layout changes
@@ -985,17 +948,14 @@ rten_status launch_nd_copy(rten_ctx* ctx, int esize, const void* src, void* dst,
         }
     }
     const int grid = ew_grid(ctx, p.n);
+    const char* what = "nd_copy launch";
     switch (es) {
-        case 1: nd_copy_kernel<uint8_t><<<grid, 256, 0, ctx->stream>>>((const uint8_t*)src, (uint8_t*)dst, p); break;
-        case 2: nd_copy_kernel<uint16_t><<<grid, 256, 0, ctx->stream>>>((const uint16_t*)src, (uint16_t*)dst, p); break;
-        case 4: nd_copy_kernel<uint32_t><<<grid, 256, 0, ctx->stream>>>((const uint32_t*)src, (uint32_t*)dst, p); break;
-        case 8: nd_copy_kernel<uint2><<<grid, 256, 0, ctx->stream>>>((const uint2*)src, (uint2*)dst, p); break;
-        default: nd_copy_kernel<uint4><<<grid, 256, 0, ctx->stream>>>((const uint4*)src, (uint4*)dst, p); break;
+        case 1: return launch(ctx, what, nd_copy_kernel<uint8_t>, {grid, 256}, (const uint8_t*)src, (uint8_t*)dst, p);
+        case 2: return launch(ctx, what, nd_copy_kernel<uint16_t>, {grid, 256}, (const uint16_t*)src, (uint16_t*)dst, p);
+        case 4: return launch(ctx, what, nd_copy_kernel<uint32_t>, {grid, 256}, (const uint32_t*)src, (uint32_t*)dst, p);
+        case 8: return launch(ctx, what, nd_copy_kernel<uint2>, {grid, 256}, (const uint2*)src, (uint2*)dst, p);
+        default: return launch(ctx, what, nd_copy_kernel<uint4>, {grid, 256}, (const uint4*)src, (uint4*)dst, p);
     }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "nd_copy launch");
-    count_launch(ctx);
-    return RTEN_OK;
 }
 
 // a and d dense, b dense over the TRAILING dims and broadcast over the leading ones (bias rows, position embeddings):
@@ -1039,14 +999,10 @@ rten_status launch_nd_add(rten_ctx* ctx, const float* a, const float* b, float* 
             n *= shape[i];
         }
         if (ok && in_bcast && period > 0 && (period & 3) == 0 && n < 0x7fffffffLL && n > 0 &&
-            ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(d)) & 15) == 0) {
-            add_periodic_kernel<<<ew_grid(ctx, n / 4), 256, 0, ctx->stream>>>(reinterpret_cast<const float4*>(a), reinterpret_cast<const float4*>(b),
-                                                                               reinterpret_cast<float4*>(d), (unsigned)(n / 4), (unsigned)(period / 4), relu);
-            cudaError_t e = cudaGetLastError();
-            if (e != cudaSuccess) return fail_cuda(ctx, e, "nd_add launch");
-            count_launch(ctx);
-            return RTEN_OK;
-        }
+            ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(d)) & 15) == 0)
+            return launch(ctx, "nd_add launch", add_periodic_kernel, {ew_grid(ctx, n / 4), 256}, reinterpret_cast<const float4*>(a),
+                          reinterpret_cast<const float4*>(b), reinterpret_cast<float4*>(d), (unsigned)(n / 4), (unsigned)(period / 4),
+                          relu);
     }
     NdParams p;
     memset(&p, 0, sizeof(p));
@@ -1060,11 +1016,7 @@ rten_status launch_nd_add(rten_ctx* ctx, const float* a, const float* b, float* 
         p.n *= shape[i];
     }
     if (p.n == 0) return RTEN_OK;
-    nd_add_kernel<<<ew_grid(ctx, p.n), 256, 0, ctx->stream>>>(a, b, d, p, relu);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "nd_add launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "nd_add launch", nd_add_kernel, {ew_grid(ctx, p.n), 256}, a, b, d, p, relu);
 }
 
 rten_status launch_add_flat(rten_ctx* ctx, const float* a, const float* b, float* d, long long n, int relu) {
@@ -1075,11 +1027,7 @@ rten_status launch_add_flat(rten_ctx* ctx, const float* a, const float* b, float
         long long shape[1] = {n}, s1[1] = {1};
         return launch_nd_add(ctx, a, b, d, 1, shape, s1, s1, s1, relu);
     }
-    add_flat_kernel<<<ew_grid(ctx, (n + 3) / 4), 256, 0, ctx->stream>>>(a, b, d, n, relu);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "add launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "add launch", add_flat_kernel, {ew_grid(ctx, (n + 3) / 4), 256}, a, b, d, n, relu);
 }
 
 // =========================================================================================
@@ -1249,20 +1197,12 @@ rten_status launch_dql_quantize_rows(rten_ctx* ctx, const float* x, uint8_t* y, 
     if (total == 0) return RTEN_OK;
     RangeExchange none;
     memset(&none, 0, sizeof(none));
-    dql_quantize_rows_kernel<<<ew_grid(ctx, total), 256, 0, ctx->stream>>>(x, y, rows, row_len, rows_inner, y_inner, y_outer,
-                                                                          mm, scale_out, zp_out, xch ? *xch : none);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "dql launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "dql launch", dql_quantize_rows_kernel, {ew_grid(ctx, total), 256}, x, y, rows, row_len, rows_inner, y_inner,
+                  y_outer, mm, scale_out, zp_out, xch ? *xch : none);
 }
 
 rten_status launch_dql_small(rten_ctx* ctx, const float* x, uint8_t* y, int n, float* scale_out, uint8_t* zp_out) {
-    dql_small_kernel<<<1, 1024, 0, ctx->stream>>>(x, y, n, scale_out, zp_out);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "dql launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "dql launch", dql_small_kernel, {1, 1024}, x, y, n, scale_out, zp_out);
 }
 
 __global__ void range_reset_kernel(int* mm, int pairs) {
@@ -1275,34 +1215,21 @@ __global__ void range_reset_kernel(int* mm, int pairs) {
 
 rten_status launch_range_reset(rten_ctx* ctx, int* mm, int pairs) {
     if (pairs == 0) return RTEN_OK;
-    range_reset_kernel<<<(pairs + 127) / 128, 128, 0, ctx->stream>>>(mm, pairs);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "range reset launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "range reset launch", range_reset_kernel, {(pairs + 127) / 128, 128}, mm, pairs);
 }
 
 rten_status launch_minmax(rten_ctx* ctx, const float* x, long long n, int* mm) {
-    minmax_init_kernel<<<1, 1, 0, ctx->stream>>>(mm);
-    count_launch(ctx);
-    if (n > 0) {
-        minmax_kernel<<<ew_grid(ctx, (n + 3) / 4), 256, 0, ctx->stream>>>(x, n, mm);
-        count_launch(ctx);
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "minmax launch");
-    return RTEN_OK;
+    RTB_TRY(launch(ctx, "minmax launch", minmax_init_kernel, {1, 1}, mm));
+    if (n == 0) return RTEN_OK;
+    return launch(ctx, "minmax launch", minmax_kernel, {ew_grid(ctx, (n + 3) / 4), 256}, x, n, mm);
 }
 
 rten_status launch_dql_quantize(rten_ctx* ctx, const float* x, uint8_t* y, long long n, int* mm, float* scale_out,
                                 uint8_t* zp_out, const RangeExchange* xch) {
     RangeExchange none;
     memset(&none, 0, sizeof(none));
-    dql_quantize_kernel<<<ew_grid(ctx, (n + 15) / 16), 256, 0, ctx->stream>>>(x, y, n, mm, scale_out, zp_out, xch ? *xch : none);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "dql launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "dql launch", dql_quantize_kernel, {ew_grid(ctx, (n + 15) / 16), 256}, x, y, n, mm, scale_out, zp_out,
+                  xch ? *xch : none);
 }
 
 // =========================================================================================
@@ -1325,12 +1252,8 @@ rowsum8_kernel(const uint8_t* __restrict__ a, int is_signed, long long rows, int
 rten_status launch_rowsum8(rten_ctx* ctx, const void* a, int is_signed, long long rows, int K, long long ld, int* out) {
     if (rows == 0) return RTEN_OK;
     const int wpb = 8;
-    rowsum8_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, ctx->stream>>>((const uint8_t*)a, is_signed, rows,
-                                                                                      K, ld, out);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "rowsum launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "rowsum launch", rowsum8_kernel, {(unsigned)((rows + wpb - 1) / wpb), wpb * 32}, (const uint8_t*)a, is_signed,
+                  rows, K, ld, out);
 }
 
 // zero points (u8 or i8, element stride zs) -> i32
@@ -1341,11 +1264,7 @@ __global__ void zp_to_i32_kernel(const uint8_t* zp, int is_signed, int n, long l
 
 rten_status launch_zp_to_i32(rten_ctx* ctx, const void* zp, int is_signed, int n, long long zs, int* out) {
     if (n == 0) return RTEN_OK;
-    zp_to_i32_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>((const uint8_t*)zp, is_signed, n, zs, out);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "zp_to_i32 launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "zp_to_i32 launch", zp_to_i32_kernel, {(n + 127) / 128, 128}, (const uint8_t*)zp, is_signed, n, zs, out);
 }
 
 __global__ void fill8_kernel(uint8_t* p, long long n, uint8_t v) {
@@ -1354,11 +1273,7 @@ __global__ void fill8_kernel(uint8_t* p, long long n, uint8_t v) {
 }
 rten_status launch_fill8(rten_ctx* ctx, void* p, long long n, uint8_t v) {
     if (n == 0) return RTEN_OK;
-    fill8_kernel<<<ew_grid(ctx, n), 256, 0, ctx->stream>>>((uint8_t*)p, n, v);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "fill launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "fill launch", fill8_kernel, {ew_grid(ctx, n), 256}, (uint8_t*)p, n, v);
 }
 
 // cast_scale (src/ops/matmul.rs:734-773) for the unfused case
@@ -1372,11 +1287,7 @@ cast_scale_kernel(const int* __restrict__ in, float* __restrict__ out, long long
 rten_status launch_cast_scale(rten_ctx* ctx, const int* in, float* out, long long n, int cols, const float* scale,
                               int scale_len) {
     if (n == 0) return RTEN_OK;
-    cast_scale_kernel<<<ew_grid(ctx, n), 256, 0, ctx->stream>>>(in, out, n, cols, scale, scale_len);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "cast_scale launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "cast_scale launch", cast_scale_kernel, {ew_grid(ctx, n), 256}, in, out, n, cols, scale, scale_len);
 }
 
 // =========================================================================================
@@ -1433,17 +1344,10 @@ rten_status launch_im2col(rten_ctx* ctx, int esize, const void* x, void* out, co
         return fail(ctx, RTEN_ERR_INVALID_VALUE, "im2col rows must be multiples of 16 bytes");
     const long long total = (long long)p.B * p.OH * p.OW * (p.kpad * esize / 16);
     if (total == 0) return RTEN_OK;
-    if (esize == 4) {
-        float pv = 0.0f;
-        im2col_kernel<float><<<ew_grid(ctx, total), 256, 0, ctx->stream>>>((const float*)x, (float*)out, p, pv);
-    } else {
-        im2col_kernel<uint8_t><<<ew_grid(ctx, total), 256, 0, ctx->stream>>>((const uint8_t*)x, (uint8_t*)out, p,
-                                                                             (uint8_t)pad_value);
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "im2col launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    if (esize == 4)
+        return launch(ctx, "im2col launch", im2col_kernel<float>, {ew_grid(ctx, total), 256}, (const float*)x, (float*)out, p, 0.0f);
+    return launch(ctx, "im2col launch", im2col_kernel<uint8_t>, {ew_grid(ctx, total), 256}, (const uint8_t*)x, (uint8_t*)out, p,
+                  (uint8_t)pad_value);
 }
 
 // =========================================================================================
@@ -1488,22 +1392,16 @@ rten_status launch_smallc_pad(rten_ctx* ctx, const float* x, float* xp, int B, i
                               long long xs_b, long long xs_c, long long xs_h, long long xs_w) {
     const long long total = (long long)B * H * Wp;
     if (total == 0) return RTEN_OK;
-    smallc_pad_kernel<<<ew_grid(ctx, total), 256, 0, ctx->stream>>>(x, xp, B, C, H, W, Wp, pl, xs_b, xs_c, xs_h, xs_w);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "smallc_pad launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "smallc_pad launch", smallc_pad_kernel, {ew_grid(ctx, total), 256}, x, xp, B, C, H, W, Wp, pl, xs_b, xs_c,
+                  xs_h, xs_w);
 }
 
 rten_status launch_smallc_pack_w(rten_ctx* ctx, const float* w, float* wp, int O, int C, int kh, int kw, long long ws_o,
                                  long long ws_c, long long ws_h, long long ws_w) {
     const int total = O * kh * 32;
     if (total == 0) return RTEN_OK;
-    smallc_pack_w_kernel<<<(total + 255) / 256, 256, 0, ctx->stream>>>(w, wp, O, C, kh, kw, ws_o, ws_c, ws_h, ws_w);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "smallc_pack_w launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "smallc_pack_w launch", smallc_pack_w_kernel, {(total + 255) / 256, 256}, w, wp, O, C, kh, kw, ws_o, ws_c,
+                  ws_h, ws_w);
 }
 
 // =========================================================================================
@@ -1584,13 +1482,8 @@ rten_status launch_maxpool(rten_ctx* ctx, const float* x, float* y, const PoolPa
                      (p.xs_w % 4) == 0 && (p.ys_b % 4) == 0 && (p.ys_h % 4) == 0 && (p.ys_w % 4) == 0 &&
                      ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;
     if (cl4)
-        maxpool_cl4_kernel<<<ew_grid(ctx, total / 4), 256, 0, ctx->stream>>>(x, y, p);
-    else
-        maxpool_kernel<<<ew_grid(ctx, total), 256, 0, ctx->stream>>>(x, y, p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "maxpool launch");
-    count_launch(ctx);
-    return RTEN_OK;
+        return launch(ctx, "maxpool launch", maxpool_cl4_kernel, {ew_grid(ctx, total / 4), 256}, x, y, p);
+    return launch(ctx, "maxpool launch", maxpool_kernel, {ew_grid(ctx, total), 256}, x, y, p);
 }
 
 // AveragePool (src/ops/pooling.rs:263-333, 400-416): the sum, from +0.0, of the taps inside the image in (ky, kx) order,
@@ -1679,13 +1572,8 @@ rten_status launch_avgpool(rten_ctx* ctx, const float* x, float* y, const PoolPa
                      (p.xs_w % 4) == 0 && (p.ys_b % 4) == 0 && (p.ys_h % 4) == 0 && (p.ys_w % 4) == 0 &&
                      ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;
     if (cl4)
-        avgpool_cl4_kernel<<<ew_grid(ctx, total / 4), 256, 0, ctx->stream>>>(x, y, p, count_include_pad);
-    else
-        avgpool_kernel<<<ew_grid(ctx, total), 256, 0, ctx->stream>>>(x, y, p, count_include_pad);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "avgpool launch");
-    count_launch(ctx);
-    return RTEN_OK;
+        return launch(ctx, "avgpool launch", avgpool_cl4_kernel, {ew_grid(ctx, total / 4), 256}, x, y, p, count_include_pad);
+    return launch(ctx, "avgpool launch", avgpool_kernel, {ew_grid(ctx, total), 256}, x, y, p, count_include_pad);
 }
 
 __global__ void __launch_bounds__(256)
@@ -1720,19 +1608,11 @@ rten_status launch_gather_rows(rten_ctx* ctx, const float* table, const int* idx
     if (nidx * width == 0) return RTEN_OK;
     if (t_cs == 1 && (width & 3) == 0 && (t_rs & 3) == 0 && nidx * width < 0x7fffffffLL &&
         ((reinterpret_cast<uintptr_t>(table) | reinterpret_cast<uintptr_t>(out)) & 15) == 0) {
-        gather_rows_vec_kernel<<<ew_grid(ctx, nidx * width / 4), 256, 0, ctx->stream>>>(table, idx, reinterpret_cast<float4*>(out),
-                                                                                       (unsigned)(nidx * width / 4), (unsigned)(width / 4), t_rs, rows);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return fail_cuda(ctx, e, "gather launch");
-        count_launch(ctx);
-        return RTEN_OK;
+        return launch(ctx, "gather launch", gather_rows_vec_kernel, {ew_grid(ctx, nidx * width / 4), 256}, table, idx,
+                      reinterpret_cast<float4*>(out), (unsigned)(nidx * width / 4), (unsigned)(width / 4), t_rs, rows);
     }
-    gather_rows_kernel<<<ew_grid(ctx, nidx * width), 256, 0, ctx->stream>>>(table, idx, out, nidx, width, t_rs, t_cs,
-                                                                            rows);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "gather launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "gather launch", gather_rows_kernel, {ew_grid(ctx, nidx * width), 256}, table, idx, out, nidx, width, t_rs,
+                  t_cs, rows);
 }
 
 
@@ -1781,24 +1661,16 @@ rten_status launch_smallc8_pad(rten_ctx* ctx, const void* x, void* xp, int B, in
                                int pl, long long xs_b, long long xs_c, long long xs_h, long long xs_w, int pad_value) {
     const long long total = (long long)B * Hp * Wp;
     if (total == 0) return RTEN_OK;
-    smallc8_pad_kernel<<<ew_grid(ctx, total), 256, 0, ctx->stream>>>((const uint8_t*)x, (uint8_t*)xp, B, C, H, W, Hp, Wp,
-                                                                     pt, pl, xs_b, xs_c, xs_h, xs_w, pad_value);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "smallc8 pad launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "smallc8 pad launch", smallc8_pad_kernel, {ew_grid(ctx, total), 256}, (const uint8_t*)x, (uint8_t*)xp, B,
+                  C, H, W, Hp, Wp, pt, pl, xs_b, xs_c, xs_h, xs_w, pad_value);
 }
 
 rten_status launch_smallc8_pack_w(rten_ctx* ctx, const void* w, void* wp, int O, int C, int kh, int kw, long long ws_o,
                                   long long ws_c, long long ws_h, long long ws_w) {
     const int total = O * kh * 128;
     if (total == 0) return RTEN_OK;
-    smallc8_pack_w_kernel<<<(total + 255) / 256, 256, 0, ctx->stream>>>((const uint8_t*)w, (uint8_t*)wp, O, C, kh, kw,
-                                                                         ws_o, ws_c, ws_h, ws_w);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "smallc8 pack launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "smallc8 pack launch", smallc8_pack_w_kernel, {(total + 255) / 256, 256}, (const uint8_t*)w, (uint8_t*)wp,
+                  O, C, kh, kw, ws_o, ws_c, ws_h, ws_w);
 }
 
 // ScatterElements-style row update (the KV-cache append of rten-generate when the write position lives on the device):
@@ -1820,12 +1692,8 @@ scatter_rows_kernel(float* __restrict__ table, const int* __restrict__ idx, cons
 rten_status launch_scatter_rows(rten_ctx* ctx, float* table, const int* idx, const float* src, long long nidx, int width,
                                 long long t_rs, long long t_cs, long long s_rs, long long s_cs, long long rows) {
     if (nidx * width == 0) return RTEN_OK;
-    scatter_rows_kernel<<<ew_grid(ctx, nidx * width), 256, 0, ctx->stream>>>(table, idx, src, nidx, width, t_rs, t_cs,
-                                                                             s_rs, s_cs, rows);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "scatter launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "scatter launch", scatter_rows_kernel, {ew_grid(ctx, nidx * width), 256}, table, idx, src, nidx, width,
+                  t_rs, t_cs, s_rs, s_cs, rows);
 }
 
 // =========================================================================================
@@ -1941,22 +1809,14 @@ rten_status launch_tf32x3_split(rten_ctx* ctx, const float* x, float* y, const l
                        (p.d3 == 1 || p.s3 == p.d0 * p.d1 * p.d2) && (reinterpret_cast<uintptr_t>(x) & 15) == 0 &&
                        (reinterpret_cast<uintptr_t>(y) & 15) == 0;
     if (dense) {
-        tf32x3_lo_flat_kernel<<<ew_grid(ctx, p.n / 16), 256, 0, ctx->stream>>>(reinterpret_cast<const float4*>(x), reinterpret_cast<float4*>(y), p.n / 4);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return fail_cuda(ctx, e, "tf32x3 split launch");
-        count_launch(ctx);
-        return RTEN_OK;
+        return launch(ctx, "tf32x3 split launch", tf32x3_lo_flat_kernel, {ew_grid(ctx, p.n / 16), 256},
+                      reinterpret_cast<const float4*>(x), reinterpret_cast<float4*>(y), p.n / 4);
     }
     const bool vec = (p.d0 & 3) == 0 && (p.d0p & 3) == 0 && (p.s1 & 3) == 0 && (p.s2 & 3) == 0 && (p.s3 & 3) == 0 &&
                      (reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0 && p.n < 0x7fffffffLL;
     if (vec)
-        tf32x3_split_vec_kernel<<<ew_grid(ctx, p.n / 4), 256, 0, ctx->stream>>>(x, y, p);
-    else
-        tf32x3_split_kernel<<<ew_grid(ctx, p.n), 256, 0, ctx->stream>>>(x, y, p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "tf32x3 split launch");
-    count_launch(ctx);
-    return RTEN_OK;
+        return launch(ctx, "tf32x3 split launch", tf32x3_split_vec_kernel, {ew_grid(ctx, p.n / 4), 256}, x, y, p);
+    return launch(ctx, "tf32x3 split launch", tf32x3_split_kernel, {ew_grid(ctx, p.n), 256}, x, y, p);
 }
 
 // =========================================================================================
@@ -1985,11 +1845,7 @@ __global__ void __launch_bounds__(256) conv_transpose_pack_kernel(const float* _
 rten_status launch_conv_transpose_pack(rten_ctx* ctx, const float* w, float* dst, const ConvTransposePack& p) {
     const long long n = (long long)p.O * p.Th * p.Tw * p.Cg;
     if (n == 0) return RTEN_OK;
-    conv_transpose_pack_kernel<<<ew_grid(ctx, n), 256, 0, ctx->stream>>>(w, dst, p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "conv_transpose_pack launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "conv_transpose_pack launch", conv_transpose_pack_kernel, {ew_grid(ctx, n), 256}, w, dst, p);
 }
 
 // out[b, o, y, x] = bias[o] (or 0) wherever phase (y mod sy, x mod sx) has no convolution; other elements untouched.
@@ -2040,25 +1896,16 @@ __global__ void __launch_bounds__(256) clip_kernel(const T* x, T* y, long long n
 rten_status launch_clip(rten_ctx* ctx, int is_i32, const void* x, void* y, long long n, const void* mn, const void* mx) {
     if (n == 0) return RTEN_OK;
     if (is_i32)
-        clip_kernel<int><<<ew_grid(ctx, n), 256, 0, ctx->stream>>>((const int*)x, (int*)y, n, (const int*)mn, (const int*)mx,
-                                                                   INT_MIN, INT_MAX);
-    else
-        clip_kernel<float><<<ew_grid(ctx, n), 256, 0, ctx->stream>>>((const float*)x, (float*)y, n, (const float*)mn,
-                                                                     (const float*)mx, -FLT_MAX, FLT_MAX);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "clip launch");
-    count_launch(ctx);
-    return RTEN_OK;
+        return launch(ctx, "clip launch", clip_kernel<int>, {ew_grid(ctx, n), 256}, (const int*)x, (int*)y, n, (const int*)mn,
+                      (const int*)mx, INT_MIN, INT_MAX);
+    return launch(ctx, "clip launch", clip_kernel<float>, {ew_grid(ctx, n), 256}, (const float*)x, (float*)y, n, (const float*)mn,
+                  (const float*)mx, -FLT_MAX, FLT_MAX);
 }
 
 rten_status launch_conv_transpose_fill(rten_ctx* ctx, float* out, const float* bias, const ConvTransposeFill& p) {
     const long long n = (long long)p.B * p.O * p.OH * p.OW;
     if (n == 0) return RTEN_OK;
-    conv_transpose_fill_kernel<<<ew_grid(ctx, n), 256, 0, ctx->stream>>>(out, bias, p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "conv_transpose_fill launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "conv_transpose_fill launch", conv_transpose_fill_kernel, {ew_grid(ctx, n), 256}, out, bias, p);
 }
 
 }  // namespace rtb

@@ -12,6 +12,7 @@
 #include <cstdlib>
 
 #include "math.cuh"
+#include "ptx.cuh"
 #include "rotary.cuh"
 #include "rowmath.cuh"
 #include "skinny.h"
@@ -30,8 +31,6 @@ __device__ __forceinline__ int dp4a_uu(unsigned a, unsigned b, int c) {
     asm("dp4a.u32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"((unsigned)c));
     return (int)d;
 }
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
 // Sum of v[i] over the 32 lanes for NV values with ~NV shuffles instead of 5 NV: at every step a lane hands half of
@@ -174,7 +173,7 @@ struct QTile {
             zb[i] = (ok && L.zb) ? (unsigned)__ldg(L.zb + (L.zb_len == 1 ? 0 : n)) : 0u;
         }
     }
-    // the residual is written by the predecessor kernel: only after griddepcontrol.wait
+    // the residual is written by the predecessor kernel: only after pdl_wait()
     __device__ __forceinline__ void load_residual(const QLinearLaunch& L, int n0, int base) {
 #pragma unroll
         for (int i = 0; i < NOUT; i++) {
@@ -402,31 +401,13 @@ rten_status launch_qlinear(rten_ctx* ctx, const QLinearLaunch& L) {
     p.tiles = (L.N + nt - 1) / nt;
     const int grid = cpw == 4 ? std::min(p.tiles, 2 * ctx->num_sms) : p.tiles;  // (one tile per CTA unless double-buffered)
     const size_t smem = (size_t)mt * L.K + mt * sizeof(int) + 16 * sizeof(float) + 16;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(256);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = getenv("RTEN_B200_NO_PDL") ? 0 : 1;
-    auto go = [&](auto kern) -> cudaError_t {
-        if (smem > 48 * 1024) {
-            cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            if (e != cudaSuccess) return e;
-        }
-        return cudaLaunchKernelEx(&cfg, kern, p);
-    };
-    cudaError_t e = cudaSuccess;
+    void (*kern)(QLinearParams);
     const int fln = (L.has_ln && (L.K >> 7) > 6) ? 8 : 6;
     const int key = (mt == 16 ? 10000 : 0) + cpw * 1000 + ki * 100 + fln * 10 + (L.w_signed ? 1 : 0);
     switch (key) {
 #define RTB_QL_CASE(MT_, CPW_, KI_, FLN_)                                                                                          \
-    case (MT_ == 16 ? 10000 : 0) + CPW_ * 1000 + KI_ * 100 + FLN_ * 10 + 0: e = go(qlinear_kernel<MT_, CPW_, KI_, false, FLN_, (CPW_ == 4)>); break; \
-    case (MT_ == 16 ? 10000 : 0) + CPW_ * 1000 + KI_ * 100 + FLN_ * 10 + 1: e = go(qlinear_kernel<MT_, CPW_, KI_, true, FLN_, (CPW_ == 4)>); break;
+    case (MT_ == 16 ? 10000 : 0) + CPW_ * 1000 + KI_ * 100 + FLN_ * 10 + 0: kern = qlinear_kernel<MT_, CPW_, KI_, false, FLN_, (CPW_ == 4)>; break; \
+    case (MT_ == 16 ? 10000 : 0) + CPW_ * 1000 + KI_ * 100 + FLN_ * 10 + 1: kern = qlinear_kernel<MT_, CPW_, KI_, true, FLN_, (CPW_ == 4)>; break;
         RTB_QL_CASE(8, 1, 2, 6) RTB_QL_CASE(8, 2, 2, 6) RTB_QL_CASE(8, 4, 2, 6) RTB_QL_CASE(8, 1, 6, 6)
         RTB_QL_CASE(16, 1, 2, 6) RTB_QL_CASE(16, 2, 2, 6) RTB_QL_CASE(16, 4, 2, 6) RTB_QL_CASE(16, 1, 6, 6)
         RTB_QL_CASE(8, 1, 2, 8) RTB_QL_CASE(8, 2, 2, 8) RTB_QL_CASE(8, 4, 2, 8)
@@ -434,11 +415,7 @@ rten_status launch_qlinear(rten_ctx* ctx, const QLinearLaunch& L) {
 #undef RTB_QL_CASE
         default: return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "quantized linear: no kernel variant for this shape");
     }
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "qlinear launch");
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "qlinear launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "qlinear launch", kern, {grid, 256, smem, smem > 48 * 1024 ? (int)smem : 0, true}, p);
 }
 
 // =========================================================================================
@@ -544,34 +521,10 @@ rten_status launch_skinny_f32(rten_ctx* ctx, const SkinnyF32Launch& L) {
     p.kc = std::min((L.K + 3) / 4 * 4, 1024);
     const int grid = std::min(p.tiles, 2 * ctx->num_sms);
     const size_t smem = (size_t)mt * p.kc * sizeof(float);
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(256);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = getenv("RTEN_B200_NO_PDL") ? 0 : 1;
-    auto go = [&](auto kern) -> cudaError_t {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-        if (e != cudaSuccess) return e;
-        return cudaLaunchKernelEx(&cfg, kern, p);
-    };
-    cudaError_t e;
-    if (mt == 8)
-        e = cpw == 2 ? go(skinny_f32_kernel<8, 2>) : go(skinny_f32_kernel<8, 1>);
-    else if (mt == 16)
-        e = cpw == 2 ? go(skinny_f32_kernel<16, 2>) : go(skinny_f32_kernel<16, 1>);
-    else
-        e = go(skinny_f32_kernel<32, 1>);
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "skinny f32 launch");
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "skinny f32 launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    auto kern = mt == 8    ? (cpw == 2 ? skinny_f32_kernel<8, 2> : skinny_f32_kernel<8, 1>)
+                : mt == 16 ? (cpw == 2 ? skinny_f32_kernel<16, 2> : skinny_f32_kernel<16, 1>)
+                           : skinny_f32_kernel<32, 1>;
+    return launch(ctx, "skinny f32 launch", kern, {grid, 256, smem, 160 * 1024, true}, p);
 }
 
 // =========================================================================================
@@ -936,31 +889,14 @@ rten_status launch_attn_decode(rten_ctx* ctx, const AttnDecodeLaunch& L) {
         p.ws = reinterpret_cast<float*>(ws);
         p.cnt = reinterpret_cast<int*>(ctx->attn_cnt);
     }
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(bh * ns);
-    cfg.blockDim = dim3(nw * 32);
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = getenv("RTEN_B200_NO_PDL") ? 0 : 1;
-    cudaError_t e;
-    if (L.mha)
-        e = L.dh == 64 ? (nw == 6 ? cudaLaunchKernelEx(&cfg, attn_decode_mha_kernel<64, 6>, p) : cudaLaunchKernelEx(&cfg, attn_decode_mha_kernel<64, 8>, p))
-                       : cudaLaunchKernelEx(&cfg, attn_decode_mha_kernel<128, 8>, p);
-    else if (ext)
-        e = L.dh == 64 ? (nw == 6 ? cudaLaunchKernelEx(&cfg, attn_decode_kernel<64, 6, true>, p) : cudaLaunchKernelEx(&cfg, attn_decode_kernel<64, 8, true>, p))
-                       : cudaLaunchKernelEx(&cfg, attn_decode_kernel<128, 8, true>, p);
-    else
-        e = L.dh == 64 ? (nw == 6 ? cudaLaunchKernelEx(&cfg, attn_decode_kernel<64, 6, false>, p) : cudaLaunchKernelEx(&cfg, attn_decode_kernel<64, 8, false>, p))
-                       : cudaLaunchKernelEx(&cfg, attn_decode_kernel<128, 8, false>, p);
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "attention launch");
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "attention launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    using Kernel = void (*)(AttnDecodeParams);
+    // [MHA, GQA with extensions, plain GQA][dh 64 with six warps, dh 64 with eight, dh 128]
+    static const Kernel kernels[3][3] = {
+        {attn_decode_mha_kernel<64, 6>, attn_decode_mha_kernel<64, 8>, attn_decode_mha_kernel<128, 8>},
+        {attn_decode_kernel<64, 6, true>, attn_decode_kernel<64, 8, true>, attn_decode_kernel<128, 8, true>},
+        {attn_decode_kernel<64, 6, false>, attn_decode_kernel<64, 8, false>, attn_decode_kernel<128, 8, false>}};
+    const Kernel kern = kernels[L.mha ? 0 : ext ? 1 : 2][L.dh == 64 ? (nw == 6 ? 0 : 1) : 2];
+    return launch(ctx, "attention launch", kern, {bh * ns, nw * 32, 0, 0, true}, p);
 }
 
 }  // namespace rtb

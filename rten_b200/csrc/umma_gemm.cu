@@ -559,24 +559,8 @@ static rten_status launch_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepare
                         : epi == Epi::PlainF32Gelu ? umma_wide_kernel<Epi::PlainF32Gelu>
                                                    : umma_wide_kernel<Epi::PlainF32>;
 
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(std::min(p.units_total, ctx->num_sms));
-    cfg.blockDim = dim3(is_wide(p.bn) ? WIDE_THREADS : NUM_THREADS);
-    cfg.dynamicSmemBytes = smem_bytes;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = getenv("RTEN_B200_NO_PDL") ? 0 : 1;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess) e = cudaLaunchKernelEx(&cfg, kern, m, p);
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "umma_gemm launch");
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda(ctx, e, "umma_gemm launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    const int threads = is_wide(p.bn) ? WIDE_THREADS : NUM_THREADS;
+    return launch(ctx, "umma_gemm launch", kern, {std::min(p.units_total, ctx->num_sms), threads, smem_bytes, 227 * 1024, true}, m, p);
 }
 
 // Problem signature for the autotune cache: everything that changes which plan is fastest.

@@ -149,8 +149,8 @@ umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
         fence_mbar_init();
     }
     __syncthreads();
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    pdl_wait();
+    pdl_launch_dependents();
 
     if (warp == HALO_PRODUCER) {
         // ===================== TMA producer =====================
@@ -405,24 +405,8 @@ rten_status launch_umma_halo_conv(rten_ctx* ctx, const GemmLaunch& L, int force_
         fprintf(stderr, "[umma_halo] B=%d %dx%d C=%d N=%d k=%dx%d: bn=%d T=%d R=%d tb=%d P=%d units=%d acc_stages=%d b_stages=%d tps=%d patch=%u B\n", g.B,
                 g.OH, g.OW, g.C, L.N, g.kh, g.kw, p.bn, p.T, p.R, p.tb, p.P, p.units_total, p.acc_stages, p.b_stages, p.tps, p.patch_bytes);
     const size_t smem = 1024 /*align*/ + 2048 /*barriers, bias*/ + ACC_SMEM_BYTES + 2 * 16384 /*output staging*/ + 2 * (size_t)p.patch_bytes + (size_t)p.b_stages * p.b_bytes;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(std::min(p.units_total, num_sms));
-    cfg.blockDim = dim3(HALO_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = getenv("RTEN_B200_NO_PDL") ? 0 : 1;
-    cudaError_t ce = cudaFuncSetAttribute(umma_halo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (ce == cudaSuccess) ce = cudaLaunchKernelEx(&cfg, umma_halo_kernel, map_a, map_b, p);
-    if (ce != cudaSuccess) return fail_cuda(ctx, ce, "umma_halo launch");
-    ce = cudaGetLastError();
-    if (ce != cudaSuccess) return fail_cuda(ctx, ce, "umma_halo launch");
-    count_launch(ctx);
-    return RTEN_OK;
+    return launch(ctx, "umma_halo launch", umma_halo_kernel, {std::min(p.units_total, num_sms), HALO_THREADS, smem, 227 * 1024, true},
+                  map_a, map_b, p);
 }
 
 }  // namespace rtb

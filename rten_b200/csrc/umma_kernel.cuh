@@ -370,7 +370,7 @@ __device__ __forceinline__ void producer_role(const KParams& p, const TmaMaps& m
         // programmatic dependent launch: the producer is the first to touch the predecessor's output; everything
         // above (tile decode) ran while the predecessor grid was still draining
         if (u == worker && pass == 0) {
-            asm volatile("griddepcontrol.wait;" ::: "memory");
+            pdl_wait();
             if (CHAIN && elect_one()) {
                 const int cb2 = p.N / 32;
                 const uint32_t wbytes = (uint32_t)(p.chain_n2 * KBYTES);
@@ -493,8 +493,8 @@ umma_gemm_kernel(const __grid_constant__ TmaMaps m, const __grid_constant__ KPar
     kernel_setup(L);
     // Programmatic dependent launch: everything above (barrier init, descriptor prefetch) overlaps the tail of the
     // previous kernel in the stream; global memory is only touched after this point.
-    if (threadIdx.x >> 5 != PRODUCER_WARP) asm volatile("griddepcontrol.wait;" ::: "memory");  // (the producer waits after its tile decode)
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    if (threadIdx.x >> 5 != PRODUCER_WARP) pdl_wait();  // (the producer waits after its tile decode)
+    pdl_launch_dependents();
     const int worker = (int)blockIdx.x, n_workers = (int)gridDim.x;
     const int warp = threadIdx.x >> 5;
     // Control warps run their loops WARP-UNIFORMLY (all 32 lanes wait on the barriers, one elected lane issues the
@@ -832,8 +832,8 @@ umma_wide_kernel(const __grid_constant__ TmaMaps m, const __grid_constant__ KPar
     __syncthreads();
     // Programmatic dependent launch: the set-up above overlaps the tail of the previous kernel in the stream; global
     // memory is only touched after this point (the producer waits after its first tile decode).
-    if (warp >= 4) asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    if (warp >= 4) pdl_wait();
+    pdl_launch_dependents();
     if (warp < 4) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
         if (warp == 0) producer_role<(CHAIN_N2 > 0)>(p, m, L, (int)blockIdx.x, (int)gridDim.x);
