@@ -167,34 +167,25 @@ rten_status rten_b200_layer_norm(rten_ctx* ctx, const rten_tensor* x, const rten
     const int nd = x->ndim;
     if (axis < -nd || axis >= std::max(nd, 1)) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Axis is invalid");
     const int ax = axis < 0 ? axis + nd : axis;
-    const float eps = epsilon < 0.0f ? 1e-5f : epsilon;
     OpScope sc(ctx);
     rten_tensor xv, xc, sv, bv, ov;
+    NormParams p;
+    p.eps = epsilon < 0.0f ? 1e-5f : epsilon;
     rten_status st = sc.in(x, &xv);
     if (st == RTEN_OK) st = sc.in(scale, &sv);
     if (st == RTEN_OK && bias) st = sc.in(bias, &bv);
-    const float *gp = nullptr, *bp = nullptr;
-    float gs = 1.0f, bs = 0.0f;
     bool g_scalar = false, b_scalar = false;
-    if (st == RTEN_OK) st = norm_param(sc, sv, xv, ax, "`scale` is not broadcastable to normalized axes of input", &gp, &g_scalar);
-    if (st == RTEN_OK && bias) st = norm_param(sc, bv, xv, ax, "`bias` is not broadcastable to normalized axes of input", &bp, &b_scalar);
+    if (st == RTEN_OK) st = norm_param(sc, sv, xv, ax, "`scale` is not broadcastable to normalized axes of input", &p.gamma, &g_scalar);
+    if (st == RTEN_OK && bias) st = norm_param(sc, bv, xv, ax, "`bias` is not broadcastable to normalized axes of input", &p.beta, &b_scalar);
     if (st == RTEN_OK) st = sc.contiguous(&xv, &xc);
     if (st == RTEN_OK) st = sc.out(out, RTEN_F32, nd, xv.shape, &ov, nullptr);
     if (st == RTEN_OK && numel(&xv) > 0) {
         long long n = 1;
         for (int i = ax; i < nd; i++) n *= xv.shape[i];
-        const long long rows = numel(&xv) / n;
         // scalar gamma / beta stay on the device and are read by the kernel (the reference's scalar-scale arm computes
         // rstd = scale / sqrt(var + eps), src/ops/norm.rs:456-529): no host read, no synchronisation, capturable
-        const float *gsp = nullptr, *bsp = nullptr;
-        if (g_scalar) {
-            gsp = gp;
-            gp = nullptr;
-        }
-        if (bias && b_scalar) {
-            bsp = bp;
-            bp = nullptr;
-        }
+        if (g_scalar) std::swap(p.gamma, p.gamma_sp);
+        if (b_scalar) std::swap(p.beta, p.beta_sp);
         rten_tensor yc = ov;
         const bool direct = is_contiguous(&ov);
         if (!direct) {
@@ -203,8 +194,12 @@ rten_status rten_b200_layer_norm(rten_ctx* ctx, const rten_tensor* x, const rten
             st = temp_alloc(ctx, (size_t)numel(&xv) * 4, &t);
             yc.data = t;
         }
-        if (st == RTEN_OK)
-            st = launch_layer_norm(ctx, (const float*)xc.data, (float*)yc.data, rows, (int)n, gp, gs, bp, bs, eps, gsp, bsp);
+        p.x = (const float*)xc.data;
+        p.xs = n;
+        p.y = (float*)yc.data;
+        p.n = (int)n;
+        p.rows = numel(&xv) / n;
+        if (st == RTEN_OK) st = launch_norm(ctx, p);
         if (st == RTEN_OK && !direct) {
             long long shape[RTEN_MAX_DIMS], ss[RTEN_MAX_DIMS], ds[RTEN_MAX_DIMS];
             for (int i = 0; i < nd; i++) {
@@ -266,7 +261,7 @@ rten_status rten_b200_rms_norm(rten_ctx* ctx, const rten_tensor* x, const rten_t
     const int ax = axis < 0 ? axis + nd : axis;
     OpScope sc(ctx);
     rten_tensor xv, sv, xr, ov;
-    SkipNormParams p;
+    NormParams p;
     p.eps = epsilon < 0.0f ? 1e-5f : epsilon;
     p.rms = 1;
     bool g_scalar = false;
@@ -283,7 +278,7 @@ rten_status rten_b200_rms_norm(rten_ctx* ctx, const rten_tensor* x, const rten_t
         p.y = (float*)ov.data;
         p.n = (int)n;
         p.rows = numel(&xv) / n;
-        if (st == RTEN_OK) st = launch_skip_norm(ctx, p);
+        if (st == RTEN_OK) st = launch_norm(ctx, p);
     }
     return sc.finish(st);
 }
@@ -311,7 +306,7 @@ rten_status rten_b200_skip_layer_norm(rten_ctx* ctx, const rten_tensor* x, const
         return fail(ctx, RTEN_ERR_INVALID_VALUE, "bias length must equal the hidden size");
     OpScope sc(ctx);
     rten_tensor xv, kv, gv, bev, biv, xr, kr, ov, smv;
-    SkipNormParams p;
+    NormParams p;
     p.eps = epsilon;
     p.rms = rms ? 1 : 0;
     bool g_scalar = false, b_scalar = false;
@@ -341,7 +336,7 @@ rten_status rten_b200_skip_layer_norm(rten_ctx* ctx, const rten_tensor* x, const
         p.sum = sum_out ? (float*)smv.data : nullptr;
         p.n = (int)H;
         p.rows = numel(&xv) / H;
-        if (st == RTEN_OK) st = launch_skip_norm(ctx, p);
+        if (st == RTEN_OK) st = launch_norm(ctx, p);
     }
     return sc.finish(st);
 }

@@ -1,6 +1,6 @@
 // Device helpers shared by the row kernels (rowops.cu) and the fused skinny-M kernels (skinny.cu): the exact scalar
-// recipes of DynamicQuantizeLinear (src/ops/quantize.rs:352-434, rten-vecmath/src/quantize.rs:38-77) and the fold step
-// of Sum / SumSquareSub (rten-vecmath/src/sum.rs:22-35,111-130).
+// recipes of DynamicQuantizeLinear (src/ops/quantize.rs:352-434, rten-vecmath/src/quantize.rs:38-77), the fold step
+// of Sum / SumSquareSub (rten-vecmath/src/sum.rs:22-35,111-130) and Normalize's output arms.
 #pragma once
 #include <cstdint>
 
@@ -45,8 +45,24 @@ __device__ __forceinline__ float fold_step(float acc, float x, float off) {
     return __fadd_rn(acc, x);
 }
 
+__device__ __forceinline__ float4 add4(float4 a, float4 b) {
+    return make_float4(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z), __fadd_rn(a.w, b.w));
+}
+
+// Normalize's three arms (rten-vecmath/src/normalize.rs:101-169): 0 = scalar scale and bias, 1 = per-element scale, no
+// bias; 2 = the general one (g = 1 without a per-element scale, b = 0 without a per-element bias)
+__device__ __forceinline__ float norm_arm(int mode, float a, float mean, float rstd, float g, float b, float beta_scalar) {
+    if (mode == 0) return __fmaf_rn(__fsub_rn(a, mean), rstd, beta_scalar);
+    if (mode == 1) return __fmul_rn(__fsub_rn(a, mean), __fmul_rn(g, rstd));
+    return __fmaf_rn(__fsub_rn(a, mean), __fmul_rn(g, rstd), __fadd_rn(b, beta_scalar));
+}
+__device__ __forceinline__ float4 norm_arm4(int mode, float4 a, float mean, float rstd, float4 g, float4 b, float bs) {
+    return make_float4(norm_arm(mode, a.x, mean, rstd, g.x, b.x, bs), norm_arm(mode, a.y, mean, rstd, g.y, b.y, bs),
+                       norm_arm(mode, a.z, mean, rstd, g.z, b.z, bs), norm_arm(mode, a.w, mean, rstd, g.w, b.w, bs));
+}
+
 // Sum / SumSquareSub of one row held in registers as float4s, in the reference's fold_unroll<4> x 16-lane order (see
-// layer_norm_vec_kernel in rowops.cu for the thread <-> chain mapping): thread (c = lane & 15, segment seg) of a row
+// norm_vec_kernel in rowops.cu for the thread <-> chain mapping): thread (c = lane & 15, segment seg) of a row
 // that spans 16 S lanes holds the float4s f = c + 16 (seg F + k), k < F.  Every lane of the row returns the total.
 template <int S, bool SQSUB, int FMAX = 16>
 __device__ __forceinline__ float ln_vec_fold(const float4 (&v)[FMAX], int F, float off, int c, int seg) {

@@ -1,8 +1,9 @@
-// HBM-bound kernels of the hot path: Softmax / AddSoftmax, LayerNormalization, Erf / Gelu,
-// DynamicQuantizeLinear, plus the layout / glue kernels that keep whole models resident.
+// HBM-bound kernels of the hot path: Softmax / AddSoftmax, the row normalizations (LayerNormalization,
+// RMSNormalization and the skip layer norms, one kernel family), Erf / Gelu, DynamicQuantizeLinear, plus the
+// layout / glue kernels that keep whole models resident.
 //
 // Accumulation ORDER follows the reference's AVX-512 path (16 f32 lanes, fold_unroll<4>), so
-// Softmax and LayerNormalization results are bit-identical to it, not merely close:
+// Softmax and normalization results are bit-identical to it, not merely close:
 //   softmax lane sums  : rten-vecmath/src/softmax.rs:192-228 (per-SIMD-lane partial sums, lanes summed in order)
 //   Sum / SumSquareSub : rten-vecmath/src/sum.rs:22-35,111-130 + rten-simd/src/iter.rs:70-120
 //   Normalize          : rten-vecmath/src/normalize.rs:101-169
@@ -286,17 +287,27 @@ rten_status launch_softmax(rten_ctx* ctx, const float* x, float* y, long long ro
 }
 
 // =========================================================================================
-// LayerNormalization: one warp per row.
-// fold_unroll<4> with V=16: position p = i % 64 owns accumulator (u = p / 16, l = p % 16) for the
-// full 64-element chunks; thread t owns p = t and p = t + 32.
+// Row normalization, one kernel family for LayerNormalization, RMSNormalization / SimplifiedLayerNormalization and the
+// skip layer norms (src/ops/norm.rs layer_normalization_impl, src/ops/norm/contrib.rs).
+// s = (x + skip) + bias, two rounded adds as the reference's `add` then `add_in_place` (s = x without a skip); the
+// statistics of s in the reference's fold order (SumSquare = SumSquareSub at offset 0 for RMS, mean 0); the output
+// through Normalize's three arms.  Three paths, each one launch and no temporary beyond the outputs:
+//   norm_vec_kernel   n % 64 == 0, n <= 1024, or n % 128 == 0, n <= 2048: the row in the registers of 16 S lanes
+//   norm_wide_kernel  the other n % 64 == 0, n <= 8192: one CTA per row, s in registers and staged once in shared memory
+//                     for the one-warp fold, rstd broadcast through shared memory
+//   norm_kernel       anything else: one warp per row
 // =========================================================================================
+enum { NORM_RMS = 1, NORM_SKIP = 2, NORM_BIAS = 4, NORM_SUM = 8 };
+
+// fold_unroll<4> with V=16 over one row by one warp, element i at x[i * stride]: position p = i % 64 owns accumulator
+// (u = p / 16, l = p % 16) for the full 64-element chunks; thread t owns p = t and p = t + 32.
 template <bool SQSUB>
-__device__ __forceinline__ float simd_fold_unroll4(const float* x, int n, float off, int lane) {
+__device__ __forceinline__ float simd_fold_unroll4(const float* x, int n, long long stride, float off, int lane) {
     float a0 = 0.0f, a1 = 0.0f;
     const int nfull = n / 64;
     for (int c = 0; c < nfull; c++) {
-        a0 = fold_step<SQSUB>(a0, x[c * 64 + lane], off);
-        a1 = fold_step<SQSUB>(a1, x[c * 64 + 32 + lane], off);
+        a0 = fold_step<SQSUB>(a0, x[(long long)(c * 64 + lane) * stride], off);
+        a1 = fold_step<SQSUB>(a1, x[(long long)(c * 64 + 32 + lane) * stride], off);
     }
     // acc[0][l] = ((acc[0][l] + acc[1][l]) + acc[2][l]) + acc[3][l]
     const float b = __shfl_down_sync(0xffffffffu, a0, 16);
@@ -305,8 +316,8 @@ __device__ __forceinline__ float simd_fold_unroll4(const float* x, int n, float 
     // remaining full 16-chunks and the masked tail go into acc[0]
     int i = nfull * 64;
     if (lane < VL) {
-        for (; i + VL <= n; i += VL) acc = fold_step<SQSUB>(acc, x[i + lane], off);
-        if (i + lane < n) acc = fold_step<SQSUB>(acc, x[i + lane], off);
+        for (; i + VL <= n; i += VL) acc = fold_step<SQSUB>(acc, x[(long long)(i + lane) * stride], off);
+        if (i + lane < n) acc = fold_step<SQSUB>(acc, x[(long long)(i + lane) * stride], off);
     }
     float s = 0.0f;
 #pragma unroll
@@ -314,170 +325,7 @@ __device__ __forceinline__ float simd_fold_unroll4(const float* x, int n, float 
     return s;
 }
 
-struct LayerNormParams {
-    const float* x;
-    float* y;
-    long long rows;
-    int n;
-    const float* gamma;  // per element or null
-    float gamma_scalar;
-    const float* beta;  // per element or null
-    float beta_scalar;
-    float eps;
-    // scalar scale / bias that live on the device (read by the kernel: the call stays asynchronous and capturable)
-    const float* gamma_sp;
-    const float* beta_sp;
-};
-
-__global__ void __launch_bounds__(256) layer_norm_kernel(const LayerNormParams p) {
-    const int lane = threadIdx.x & 31;
-    const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (row >= p.rows) return;
-    const float* x = p.x + row * p.n;
-    float* y = p.y + row * p.n;
-    const int n = p.n;
-    const float gamma_scalar = p.gamma_sp ? __ldg(p.gamma_sp) : p.gamma_scalar;
-    const float beta_scalar = p.beta_sp ? __ldg(p.beta_sp) : p.beta_scalar;
-    const float mean = __fdiv_rn(simd_fold_unroll4<false>(x, n, 0.0f, lane), (float)n);
-    const float var = __fdiv_rn(simd_fold_unroll4<true>(x, n, mean, lane), (float)n);
-    const float rstd = __fdiv_rn(gamma_scalar, __fsqrt_rn(__fadd_rn(var, p.eps)));
-    if (!p.gamma && !p.beta) {
-        for (int i = lane; i < n; i += 32) y[i] = __fmaf_rn(__fsub_rn(x[i], mean), rstd, beta_scalar);
-    } else if (p.gamma && !p.beta && beta_scalar == 0.0f) {
-        for (int i = lane; i < n; i += 32) y[i] = __fmul_rn(__fsub_rn(x[i], mean), __fmul_rn(p.gamma[i], rstd));
-    } else {
-        for (int i = lane; i < n; i += 32) {
-            const float sv = __fmul_rn(p.gamma ? p.gamma[i] : 1.0f, rstd);
-            const float bv = __fadd_rn(p.beta ? p.beta[i] : 0.0f, beta_scalar);
-            y[i] = __fmaf_rn(__fsub_rn(x[i], mean), sv, bv);
-        }
-    }
-}
-
-// -----------------------------------------------------------------------------------------
-// Vectorised LayerNormalization: row in registers, one pass over global memory, 128-bit accesses.
-// fold_unroll<4> over 16 lanes = 64 independent chains, chain p owning the elements i = p (mod 64) in ascending i
-// (only full 64-element chunks exist here: n % 64 == 0).  The float4 at index f holds chains 4 (f mod 16) .. + 3:
-// thread (c = f mod 16, segment s) keeps f = c + 16 (s F + k), k < F, and so owns its four chains outright; segment
-// s continues from segment s - 1's sums.  Then acc[0][l] = ((acc[0][l] + acc[1][l]) + acc[2][l]) + acc[3][l] with
-// chain p = 16 u + l, and the 16 lanes are summed in order (rten-vecmath/src/sum.rs:22-35, rten-simd/src/iter.rs:70-120).
-// -----------------------------------------------------------------------------------------
-template <int S, int FMAX>
-__global__ void __launch_bounds__(128) layer_norm_vec_kernel(const LayerNormParams p) {
-    constexpr int LPR = 16 * S;
-    constexpr int RPW = 32 / LPR;
-    const int lane = threadIdx.x & 31;
-    const int c = lane & 15, seg = (lane >> 4) & (S - 1), rw = lane / LPR;
-    const long long warp_id = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    const long long row = warp_id * RPW + rw;
-    const bool live = row < p.rows;
-    const int n = p.n;
-    const int F = n / (64 * S);
-    const long long rr = live ? row : 0;
-    const float4* x4 = reinterpret_cast<const float4*>(p.x + rr * n);
-    float4 v[FMAX];
-#pragma unroll
-    for (int k = 0; k < FMAX; k++)
-        if (k < F) v[k] = __ldg(x4 + c + 16 * (seg * F + k));
-    const float gamma_scalar = p.gamma_sp ? __ldg(p.gamma_sp) : p.gamma_scalar;
-    const float beta_scalar = p.beta_sp ? __ldg(p.beta_sp) : p.beta_scalar;
-    const float mean = __fdiv_rn(ln_vec_fold<S, false, FMAX>(v, F, 0.0f, c, seg), (float)n);
-    const float var = __fdiv_rn(ln_vec_fold<S, true, FMAX>(v, F, mean, c, seg), (float)n);
-    const float rstd = __fdiv_rn(gamma_scalar, __fsqrt_rn(__fadd_rn(var, p.eps)));
-    if (!live) return;
-    float4* y4 = reinterpret_cast<float4*>(p.y + rr * n);
-    const float4* g4 = reinterpret_cast<const float4*>(p.gamma);
-    const float4* b4 = reinterpret_cast<const float4*>(p.beta);
-    const int mode = (!p.gamma && !p.beta) ? 0 : ((p.gamma && !p.beta && beta_scalar == 0.0f) ? 1 : 2);
-#pragma unroll
-    for (int k = 0; k < FMAX; k++) {
-        if (k < F) {
-            const int f = c + 16 * (seg * F + k);
-            const float4 a = v[k];
-            float4 o;
-            if (mode == 0) {
-                o = make_float4(__fmaf_rn(__fsub_rn(a.x, mean), rstd, beta_scalar), __fmaf_rn(__fsub_rn(a.y, mean), rstd, beta_scalar),
-                                __fmaf_rn(__fsub_rn(a.z, mean), rstd, beta_scalar), __fmaf_rn(__fsub_rn(a.w, mean), rstd, beta_scalar));
-            } else if (mode == 1) {
-                const float4 g = __ldg(g4 + f);
-                o = make_float4(__fmul_rn(__fsub_rn(a.x, mean), __fmul_rn(g.x, rstd)), __fmul_rn(__fsub_rn(a.y, mean), __fmul_rn(g.y, rstd)),
-                                __fmul_rn(__fsub_rn(a.z, mean), __fmul_rn(g.z, rstd)), __fmul_rn(__fsub_rn(a.w, mean), __fmul_rn(g.w, rstd)));
-            } else {
-                const float4 g = p.gamma ? __ldg(g4 + f) : make_float4(1.f, 1.f, 1.f, 1.f);
-                const float4 b = p.beta ? __ldg(b4 + f) : make_float4(0.f, 0.f, 0.f, 0.f);
-                o = make_float4(__fmaf_rn(__fsub_rn(a.x, mean), __fmul_rn(g.x, rstd), __fadd_rn(b.x, beta_scalar)),
-                                __fmaf_rn(__fsub_rn(a.y, mean), __fmul_rn(g.y, rstd), __fadd_rn(b.y, beta_scalar)),
-                                __fmaf_rn(__fsub_rn(a.z, mean), __fmul_rn(g.z, rstd), __fadd_rn(b.z, beta_scalar)),
-                                __fmaf_rn(__fsub_rn(a.w, mean), __fmul_rn(g.w, rstd), __fadd_rn(b.w, beta_scalar)));
-            }
-            y4[f] = o;
-        }
-    }
-}
-
-rten_status launch_layer_norm(rten_ctx* ctx, const float* x, float* y, long long rows, int n, const float* gamma,
-                              float gamma_scalar, const float* beta, float beta_scalar, float eps, const float* gamma_sp,
-                              const float* beta_sp) {
-    if (rows == 0 || n == 0) return RTEN_OK;
-    LayerNormParams p{x, y, rows, n, gamma, gamma_scalar, beta, beta_scalar, eps, gamma_sp, beta_sp};
-    const int wpb = 8;
-    // 16 S lanes per row, F = n / (64 S) <= 16 float4s per thread; two segments per row when that is possible and the
-    // rows alone would leave the SMs short of warps
-    int S = 0;
-    for (int c = 1; c <= 2; c *= 2) {
-        if (n % (64 * c) != 0 || n / (64 * c) > 16) continue;
-        S = c;
-        const long long warps = (rows * 16 * c + 31) / 32;
-        if (warps >= 32LL * ctx->num_sms) break;
-    }
-    auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-    if (S && al16(x) && al16(y) && al16(gamma) && al16(beta) && !getenv("RTEN_B200_NO_VEC_ROWS")) {
-        const int rpw = 2 / S;
-        const int vwpb = 4;
-        const long long warps = (rows + rpw - 1) / rpw;
-        const unsigned blocks = (unsigned)((warps + vwpb - 1) / vwpb);
-        const int F = n / (64 * S);
-        const int fm = F <= 4 ? 4 : (F <= 8 ? 8 : (F <= 12 ? 12 : 16));
-        using Kernel = void (*)(LayerNormParams);
-        // [S - 1][fm / 4 - 1]
-        static const Kernel vec[2][4] = {
-            {layer_norm_vec_kernel<1, 4>, layer_norm_vec_kernel<1, 8>, layer_norm_vec_kernel<1, 12>, layer_norm_vec_kernel<1, 16>},
-            {layer_norm_vec_kernel<2, 4>, layer_norm_vec_kernel<2, 8>, layer_norm_vec_kernel<2, 12>, layer_norm_vec_kernel<2, 16>}};
-        return launch(ctx, "layer_norm launch", vec[S - 1][fm / 4 - 1], {blocks, vwpb * 32}, p);
-    }
-    const long long blocks = (rows + wpb - 1) / wpb;
-    return launch(ctx, "layer_norm launch", layer_norm_kernel, {(unsigned)blocks, wpb * 32}, p);
-}
-
-// =========================================================================================
-// RMSNormalization and the skip layer norms (src/ops/norm.rs layer_normalization_impl, src/ops/norm/contrib.rs).
-// s = (x + skip) + bias, two rounded adds as the reference's `add` then `add_in_place`; the statistics of s in the
-// LayerNormalization kernels' fold order (SumSquare = SumSquareSub at offset 0 for RMS, mean 0); the output through the
-// same three Normalize arms.  Three paths, each one launch and no temporary beyond the outputs:
-//   skip_norm_vec_kernel   n % 64 == 0, n <= 1024, or n % 128 == 0, n <= 2048: the row in the registers of 16 S lanes,
-//                          as layer_norm_vec_kernel
-//   skip_norm_wide_kernel  the other n % 64 == 0, n <= 8192: one CTA per row, s in registers and staged once in shared memory
-//                          for the one-warp fold, rstd broadcast through shared memory
-//   skip_norm_kernel       anything else: one warp per row, s staged in the output row
-// =========================================================================================
-enum { NORM_RMS = 1, NORM_SKIP = 2, NORM_BIAS = 4, NORM_SUM = 8 };
-
-__device__ __forceinline__ float4 add4(float4 a, float4 b) {
-    return make_float4(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z), __fadd_rn(a.w, b.w));
-}
-
-// Normalize's three arms (rten-vecmath/src/normalize.rs:101-169), as in layer_norm_kernel: 0 = scalar scale and bias,
-// 1 = per-element scale, no bias; 2 = the general one (g = 1 without a per-element scale, b = 0 without a per-element bias)
-__device__ __forceinline__ float norm_arm(int mode, float a, float mean, float rstd, float g, float b, float beta_scalar) {
-    if (mode == 0) return __fmaf_rn(__fsub_rn(a, mean), rstd, beta_scalar);
-    if (mode == 1) return __fmul_rn(__fsub_rn(a, mean), __fmul_rn(g, rstd));
-    return __fmaf_rn(__fsub_rn(a, mean), __fmul_rn(g, rstd), __fadd_rn(b, beta_scalar));
-}
-__device__ __forceinline__ float4 norm_arm4(int mode, float4 a, float mean, float rstd, float4 g, float4 b, float bs) {
-    return make_float4(norm_arm(mode, a.x, mean, rstd, g.x, b.x, bs), norm_arm(mode, a.y, mean, rstd, g.y, b.y, bs),
-                       norm_arm(mode, a.z, mean, rstd, g.z, b.z, bs), norm_arm(mode, a.w, mean, rstd, g.w, b.w, bs));
-}
-__device__ __forceinline__ int norm_mode(const SkipNormParams& p, float beta_scalar) {
+__device__ __forceinline__ int norm_mode(const NormParams& p, float beta_scalar) {
     return (!p.gamma && !p.beta) ? 0 : ((p.gamma && !p.beta && beta_scalar == 0.0f) ? 1 : 2);
 }
 
@@ -491,13 +339,21 @@ __device__ __forceinline__ float4 skip_sum4(const float4* x4, const float4* k4, 
 }
 
 template <int FL>
-__device__ __forceinline__ void skip_row_ptrs(const SkipNormParams& p, long long r, const float4*& x4, const float4*& k4) {
+__device__ __forceinline__ void skip_row_ptrs(const NormParams& p, long long r, const float4*& x4, const float4*& k4) {
     x4 = reinterpret_cast<const float4*>(p.x + r * p.xs);
     k4 = (FL & NORM_SKIP) ? reinterpret_cast<const float4*>(p.skip + (r % p.skip_rows) * p.ss) : nullptr;
 }
 
+// -----------------------------------------------------------------------------------------
+// Row in registers, one pass over global memory, 128-bit accesses.
+// fold_unroll<4> over 16 lanes = 64 independent chains, chain p owning the elements i = p (mod 64) in ascending i
+// (only full 64-element chunks exist here: n % 64 == 0).  The float4 at index f holds chains 4 (f mod 16) .. + 3:
+// thread (c = f mod 16, segment s) keeps f = c + 16 (s F + k), k < F, and so owns its four chains outright; segment
+// s continues from segment s - 1's sums.  Then acc[0][l] = ((acc[0][l] + acc[1][l]) + acc[2][l]) + acc[3][l] with
+// chain p = 16 u + l, and the 16 lanes are summed in order (rten-vecmath/src/sum.rs:22-35, rten-simd/src/iter.rs:70-120).
+// -----------------------------------------------------------------------------------------
 template <int S, int FMAX, int FL>
-__global__ void __launch_bounds__(128) skip_norm_vec_kernel(const SkipNormParams p) {
+__global__ void __launch_bounds__(128) norm_vec_kernel(const NormParams p) {
     constexpr int LPR = 16 * S;
     constexpr int RPW = 32 / LPR;
     const int lane = threadIdx.x & 31;
@@ -544,7 +400,7 @@ __global__ void __launch_bounds__(128) skip_norm_vec_kernel(const SkipNormParams
 constexpr int WIDE_THREADS = 256;
 
 template <int VPT, int FL>
-__global__ void __launch_bounds__(WIDE_THREADS) skip_norm_wide_kernel(const SkipNormParams p) {
+__global__ void __launch_bounds__(WIDE_THREADS) norm_wide_kernel(const NormParams p) {
     extern __shared__ float4 srow[];  // the row's s, n / 4 float4s
     __shared__ float stat[2];
     const long long row = blockIdx.x;
@@ -592,52 +448,57 @@ __global__ void __launch_bounds__(WIDE_THREADS) skip_norm_wide_kernel(const Skip
     }
 }
 
-// Odd widths, unaligned rows, a one-element bias: one warp per row; s goes to the output row first and is read back
-// from there by the fold (simd_fold_unroll4: full 64-element chunks, then 16-element chunks and the masked tail).
-__global__ void __launch_bounds__(256) skip_norm_kernel(const SkipNormParams p) {
+// Odd widths, unaligned rows, a one-element bias: one warp per row, the fold in simd_fold_unroll4's order (full
+// 64-element chunks, then 16-element chunks and the masked tail).  With a skip, a bias or a sum output, s goes to the
+// output row first and the fold reads it back from there (y then never aliases x: those operators take no in-place
+// outputs); otherwise the fold reads x, which y may alias.
+__global__ void __launch_bounds__(256) norm_kernel(const NormParams p) {
     const int lane = threadIdx.x & 31;
     const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (row >= p.rows) return;
     const int n = p.n;
     const float* x = p.x + row * p.xs;
     const float* k = p.skip ? p.skip + (row % p.skip_rows) * p.ss : nullptr;
-    float* y = p.y + row * n;  // (never aliases x or skip: the operators take no in-place outputs)
+    float* y = p.y + row * n;
     float* sm = p.sum ? p.sum + row * n : nullptr;
-    for (int i = lane; i < n; i += 32) {
-        float s = x[i];
-        if (k) s = __fadd_rn(s, k[i]);
-        if (p.bias) s = __fadd_rn(s, p.bias[(long long)i * p.bias_inc]);
-        y[i] = s;
-        if (sm) sm[i] = s;
+    const float* s = x;
+    if (k || p.bias || sm) {
+#pragma unroll 1  // (unrolled, this loop takes the kernel from 32 to 40 registers)
+        for (int i = lane; i < n; i += 32) {
+            float v = x[i];
+            if (k) v = __fadd_rn(v, k[i]);
+            if (p.bias) v = __fadd_rn(v, p.bias[(long long)i * p.bias_inc]);
+            y[i] = v;
+            if (sm) sm[i] = v;
+        }
+        __syncwarp();
+        s = y;
     }
-    __syncwarp();
     const float gamma_scalar = p.gamma_sp ? __ldg(p.gamma_sp) : 1.0f;
     const float beta_scalar = p.beta_sp ? __ldg(p.beta_sp) : 0.0f;
-    const float mean = p.rms ? 0.0f : __fdiv_rn(simd_fold_unroll4<false>(y, n, 0.0f, lane), (float)n);
-    const float var = __fdiv_rn(simd_fold_unroll4<true>(y, n, mean, lane), (float)n);
+    const float mean = p.rms ? 0.0f : __fdiv_rn(simd_fold_unroll4<false>(s, n, 1, 0.0f, lane), (float)n);
+    const float var = __fdiv_rn(simd_fold_unroll4<true>(s, n, 1, mean, lane), (float)n);
     const float rstd = __fdiv_rn(gamma_scalar, __fsqrt_rn(__fadd_rn(var, p.eps)));
     __syncwarp();
     const int mode = norm_mode(p, beta_scalar);
     for (int i = lane; i < n; i += 32)
-        y[i] = norm_arm(mode, y[i], mean, rstd, p.gamma ? p.gamma[i] : 1.0f, p.beta ? p.beta[i] : 0.0f, beta_scalar);
+        y[i] = norm_arm(mode, s[i], mean, rstd, p.gamma ? p.gamma[i] : 1.0f, p.beta ? p.beta[i] : 0.0f, beta_scalar);
 }
 
-using SkipNormKernel = void (*)(SkipNormParams);
+using NormKernel = void (*)(NormParams);
+struct NormKernels {
+    NormKernel vec[2][4];  // [S - 1][FMAX / 4 - 1]
+    NormKernel wide[2];    // [VPT / 4 - 1]
+};
 
 template <int FL>
-static SkipNormKernel skip_norm_fl_kernel(int S, int fm, int vpt) {
-    if (vpt) return vpt == 4 ? skip_norm_wide_kernel<4, FL> : skip_norm_wide_kernel<8, FL>;
-    switch (S * 100 + fm) {
-        case 104: return skip_norm_vec_kernel<1, 4, FL>;
-        case 108: return skip_norm_vec_kernel<1, 8, FL>;
-        case 116: return skip_norm_vec_kernel<1, 16, FL>;
-        case 204: return skip_norm_vec_kernel<2, 4, FL>;
-        case 208: return skip_norm_vec_kernel<2, 8, FL>;
-        default: return skip_norm_vec_kernel<2, 16, FL>;
-    }
+static constexpr NormKernels norm_kernels() {
+    return {{{norm_vec_kernel<1, 4, FL>, norm_vec_kernel<1, 8, FL>, norm_vec_kernel<1, 12, FL>, norm_vec_kernel<1, 16, FL>},
+             {norm_vec_kernel<2, 4, FL>, norm_vec_kernel<2, 8, FL>, norm_vec_kernel<2, 12, FL>, norm_vec_kernel<2, 16, FL>}},
+            {norm_wide_kernel<4, FL>, norm_wide_kernel<8, FL>}};
 }
 
-rten_status launch_skip_norm(rten_ctx* ctx, const SkipNormParams& p) {
+rten_status launch_norm(rten_ctx* ctx, const NormParams& p) {
     if (p.rows == 0 || p.n == 0) return RTEN_OK;
     const int n = p.n;
     auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
@@ -646,12 +507,15 @@ rten_status launch_skip_norm(rten_ctx* ctx, const SkipNormParams& p) {
                         al16(p.sum) && p.rows < 0x7fffffffLL;
     const int fl = (p.rms ? NORM_RMS : 0) | (p.skip ? NORM_SKIP : 0) | (p.bias ? NORM_BIAS : 0) | (p.sum ? NORM_SUM : 0);
     const bool flags_ok = p.skip || (!p.bias && !p.sum);  // (no bias or sum output without a skip input)
-    if (vec_ok && flags_ok && n <= 8192) {
-        int S = 0, fm = 0, vpt = 0;
-        unsigned blocks;
-        // as launch_layer_norm: 16 S lanes per row, F = n / (64 S) <= 16 float4s per thread; two segments per row when
-        // that is possible and the rows alone would leave the SMs short of warps.  No S fits widths such as 1600
-        // (n / 64 > 16 and odd): those take the wide kernel.
+    if (vec_ok && flags_ok && n <= 8192 && !getenv("RTEN_B200_NO_VEC_ROWS")) {
+        // [fl]; flags_ok leaves out the sets with a bias or a sum output but no skip (4, 5, 8, 9, 12, 13)
+        static constexpr NormKernels kernels[16] = {
+            norm_kernels<0>(), norm_kernels<1>(), norm_kernels<2>(), norm_kernels<3>(), {}, {}, norm_kernels<6>(),
+            norm_kernels<7>(), {}, {}, norm_kernels<10>(), norm_kernels<11>(), {}, {}, norm_kernels<14>(), norm_kernels<15>()};
+        // 16 S lanes per row, F = n / (64 S) <= 16 float4s per thread; two segments per row when that is possible and
+        // the rows alone would leave the SMs short of warps.  No S fits widths such as 1600 (n / 64 > 16 and odd):
+        // those take the wide kernel.
+        int S = 0;
         for (int c = 1; c <= 2; c *= 2) {
             if (n % (64 * c) != 0 || n / (64 * c) > 16) continue;
             S = c;
@@ -659,31 +523,14 @@ rten_status launch_skip_norm(rten_ctx* ctx, const SkipNormParams& p) {
         }
         if (S) {
             const int F = n / (64 * S);
-            fm = F <= 4 ? 4 : (F <= 8 ? 8 : 16);
+            const int fm = F <= 4 ? 4 : (F <= 8 ? 8 : (F <= 12 ? 12 : 16));
             const long long warps = (p.rows + 2 / S - 1) / (2 / S);
-            blocks = (unsigned)((warps + 3) / 4);
-        } else {
-            vpt = n <= 4 * 4 * WIDE_THREADS ? 4 : 8;  // float4s per thread
-            blocks = (unsigned)p.rows;
+            return launch(ctx, "norm launch", kernels[fl].vec[S - 1][fm / 4 - 1], {(unsigned)((warps + 3) / 4), 128}, p);
         }
-        SkipNormKernel kern;
-        switch (fl) {
-            case NORM_RMS: kern = skip_norm_fl_kernel<NORM_RMS>(S, fm, vpt); break;
-#define RTB_SKIP_NORM_CASE(F) \
-    case F: kern = skip_norm_fl_kernel<F>(S, fm, vpt); break; \
-    case F | NORM_RMS: kern = skip_norm_fl_kernel<F | NORM_RMS>(S, fm, vpt); break;
-            RTB_SKIP_NORM_CASE(NORM_SKIP)
-            RTB_SKIP_NORM_CASE(NORM_SKIP | NORM_BIAS)
-            RTB_SKIP_NORM_CASE(NORM_SKIP | NORM_SUM)
-            RTB_SKIP_NORM_CASE(NORM_SKIP | NORM_BIAS | NORM_SUM)
-#undef RTB_SKIP_NORM_CASE
-            default: return fail(ctx, RTEN_ERR_INVALID_VALUE, "skip_norm: no kernel for these flags");
-        }
-        if (vpt) return launch(ctx, "skip_norm launch", kern, {blocks, WIDE_THREADS, (size_t)n * 4}, p);
-        return launch(ctx, "skip_norm launch", kern, {blocks, 128}, p);
+        const int vpt = n <= 4 * 4 * WIDE_THREADS ? 4 : 8;  // float4s per thread
+        return launch(ctx, "norm launch", kernels[fl].wide[vpt / 4 - 1], {(unsigned)p.rows, WIDE_THREADS, (size_t)n * 4}, p);
     }
-    const long long blocks = (p.rows + 7) / 8;
-    return launch(ctx, "skip_norm launch", skip_norm_kernel, {(unsigned)blocks, 256}, p);
+    return launch(ctx, "norm launch", norm_kernel, {(unsigned)((p.rows + 7) / 8), 256}, p);
 }
 
 // Row sums in the reference's Sum order (GlobalAveragePool = Sum / len, src/ops/pooling.rs:516-521).
@@ -695,23 +542,7 @@ row_mean_kernel(const float* x, float* y, long long rows, int n, long long rows_
     const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (row >= rows) return;
     const float* xr = x + (row / rows_inner) * s_outer + (row % rows_inner) * s_inner;
-    float a0 = 0.0f, a1 = 0.0f;
-    const int nfull = n / 64;
-    for (int c = 0; c < nfull; c++) {
-        a0 = __fadd_rn(a0, xr[(long long)(c * 64 + lane) * kstride]);
-        a1 = __fadd_rn(a1, xr[(long long)(c * 64 + 32 + lane) * kstride]);
-    }
-    const float b = __shfl_down_sync(0xffffffffu, a0, 16);
-    const float d = __shfl_down_sync(0xffffffffu, a1, 16);
-    float acc = __fadd_rn(__fadd_rn(__fadd_rn(a0, b), a1), d);
-    int i = nfull * 64;
-    if (lane < VL) {
-        for (; i + VL <= n; i += VL) acc = __fadd_rn(acc, xr[(long long)(i + lane) * kstride]);
-        if (i + lane < n) acc = __fadd_rn(acc, xr[(long long)(i + lane) * kstride]);
-    }
-    float s = 0.0f;
-#pragma unroll
-    for (int l = 0; l < VL; l++) s = __fadd_rn(s, __shfl_sync(0xffffffffu, acc, l));
+    const float s = simd_fold_unroll4<false>(xr, n, kstride, 0.0f, lane);
     if (lane == 0) y[row] = __fdiv_rn(s, (float)n);
 }
 

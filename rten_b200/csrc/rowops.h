@@ -24,14 +24,12 @@ enum {
 rten_status launch_softmax(rten_ctx* ctx, const float* x, float* y, long long rows, int n, int flush_nan,
                            const float* mask, int nlead, const long long* lead, const long long* mstride,
                            long long mstride_last);
-// gamma_sp / beta_sp: scalar scale / bias resident on the device (then gamma / beta are null and the host scalars unused)
-rten_status launch_layer_norm(rten_ctx* ctx, const float* x, float* y, long long rows, int n, const float* gamma,
-                              float gamma_scalar, const float* beta, float beta_scalar, float eps,
-                              const float* gamma_sp = nullptr, const float* beta_sp = nullptr);
-// RMSNormalization and the skip layer norms over rows of n floats: s = (x + skip) + bias (skip and bias optional),
-// normalised as LayerNormalization (rms = 0) or with the root mean square and no centring (rms = 1).  y and sum are
-// dense [rows, n]; sum (the rounded s) is written when not null.
-struct SkipNormParams {
+// LayerNormalization, RMSNormalization / SimplifiedLayerNormalization and the skip layer norms
+// (SkipLayerNormalization, SkipSimplifiedLayerNormalization) over rows of n floats: s = (x + skip) + bias (skip and bias
+// optional), normalised with mean and variance (rms = 0) or with the root mean square and no centring (rms = 1).  y and
+// sum are dense [rows, n]; sum (the rounded s) is written when not null.  y may be x when there is no skip (in-place
+// LayerNormalization); it never aliases skip, bias or sum.
+struct NormParams {
     const float* x = nullptr;     // row r at x + r * xs (elements contiguous)
     const float* skip = nullptr;  // row r at skip + (r % skip_rows) * ss, or null
     const float* bias = nullptr;  // element i at bias[i * bias_inc] (bias_inc 0: one value for the row), or null
@@ -45,7 +43,7 @@ struct SkipNormParams {
     int n = 0, bias_inc = 1, rms = 0;
     float eps = 1e-5f;
 };
-rten_status launch_skip_norm(rten_ctx* ctx, const SkipNormParams& p);
+rten_status launch_norm(rten_ctx* ctx, const NormParams& p);
 // y[row] = Sum(x_row) / n in the reference's Sum order; row r starts at
 // x + (r / rows_inner) * s_outer + (r % rows_inner) * s_inner, elements kstride apart.
 rten_status launch_row_mean(rten_ctx* ctx, const float* x, float* y, long long rows, int n, long long rows_inner,

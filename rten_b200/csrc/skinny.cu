@@ -85,7 +85,7 @@ __device__ __forceinline__ uint32_t quant4(float4 a, float inv, int zp) {
 
 // One row of x, layer-normalised, as float4s in the vector-LayerNorm mapping (32 lanes per row): thread
 // (c = lane & 15, seg = lane >> 4) holds the float4s f = c + 16 (seg F + k), k < F = K / 128 <= 8.  Same arithmetic
-// as layer_norm_vec_kernel<2, .> (rowops.cu), so the values equal the LayerNormalization operator's bit for bit.
+// as norm_vec_kernel<2, ., 0> (rowops.cu), so the values equal the LayerNormalization operator's bit for bit.
 template <int FLN>
 __device__ __forceinline__ void qlin_ln_row(const QLinearLaunch& L, int r, int lane, float4 (&v)[FLN]) {
     const int c = lane & 15, seg = lane >> 4;
@@ -107,21 +107,10 @@ __device__ __forceinline__ void qlin_ln_row(const QLinearLaunch& L, int r, int l
     const float mean = __fdiv_rn(ln_vec_fold<2, false, FLN>(v, F, 0.0f, c, seg), (float)L.K);
     const float var = __fdiv_rn(ln_vec_fold<2, true, FLN>(v, F, mean, c, seg), (float)L.K);
     const float rstd = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(var, L.ln_eps)));
+    // Normalize's arm 1 (per-element scale, no bias) or arm 2 with beta and the scalar bias 0
 #pragma unroll
-    for (int k = 0; k < FLN; k++) {
-        if (k < F) {
-            const float4 a = v[k];
-            if (!L.ln_beta) {  // (same arm as layer_norm_vec_kernel's mode 1)
-                v[k] = make_float4(__fmul_rn(__fsub_rn(a.x, mean), __fmul_rn(g[k].x, rstd)), __fmul_rn(__fsub_rn(a.y, mean), __fmul_rn(g[k].y, rstd)),
-                                   __fmul_rn(__fsub_rn(a.z, mean), __fmul_rn(g[k].z, rstd)), __fmul_rn(__fsub_rn(a.w, mean), __fmul_rn(g[k].w, rstd)));
-            } else {  // (mode 2: beta + the scalar bias 0.0)
-                v[k] = make_float4(__fmaf_rn(__fsub_rn(a.x, mean), __fmul_rn(g[k].x, rstd), __fadd_rn(bt[k].x, 0.0f)),
-                                   __fmaf_rn(__fsub_rn(a.y, mean), __fmul_rn(g[k].y, rstd), __fadd_rn(bt[k].y, 0.0f)),
-                                   __fmaf_rn(__fsub_rn(a.z, mean), __fmul_rn(g[k].z, rstd), __fadd_rn(bt[k].z, 0.0f)),
-                                   __fmaf_rn(__fsub_rn(a.w, mean), __fmul_rn(g[k].w, rstd), __fadd_rn(bt[k].w, 0.0f)));
-            }
-        }
-    }
+    for (int k = 0; k < FLN; k++)
+        if (k < F) v[k] = norm_arm4(L.ln_beta ? 2 : 1, v[k], mean, rstd, g[k], bt[k], 0.0f);
 }
 
 // The (row m, column offset j) whose complete sum lane `lane` holds after reduce_scatter_warp<NV> (a function of the

@@ -232,8 +232,8 @@ def test_kernel_identity():
     res = subprocess.run([sys.executable, "-s", "-c", code], capture_output=True, text=True, timeout=600)
     assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-4000:]
     names = json.loads(res.stdout.strip().splitlines()[-1])
-    want = {**{str(h): "skip_norm_vec_kernel" for h in VEC}, **{str(h): "skip_norm_wide_kernel" for h in WIDE},
-            **{str(h): "skip_norm_kernel" for h in GENERIC}, "unaligned": "skip_norm_kernel"}
+    want = {**{str(h): "norm_vec_kernel" for h in VEC}, **{str(h): "norm_wide_kernel" for h in WIDE},
+            **{str(h): "norm_kernel" for h in GENERIC}, "unaligned": "norm_kernel"}
     for key, kname in want.items():
         ks = [n for n in names[key] if "_kernel" in n]  # (the session also lists runtime API calls)
         assert ks and all(kname + "(" in n or kname + "<" in n for n in ks), (key, ks)

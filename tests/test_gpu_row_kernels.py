@@ -1,7 +1,8 @@
-"""`pytest -m gpu`: every template instance of the Softmax / AddSoftmax, LayerNormalization, f32 skinny-GEMM and fused
-quantized-linear kernels, each selected by name and checked bit for bit.
+"""`pytest -m gpu`: every template instance of the Softmax / AddSoftmax, row normalization (LayerNormalization,
+RMSNormalization and the skip layer norms), f32 skinny-GEMM and fused quantized-linear kernels, each selected by name and
+checked bit for bit.
 
-The launchers (rowops.cu launch_softmax / launch_layer_norm, skinny.cu launch_skinny_f32 / launch_qlinear) pick an
+The launchers (rowops.cu launch_softmax / launch_norm, skinny.cu launch_skinny_f32 / launch_qlinear) pick an
 instance at run time from the row width, the row count, the SM count and pointer alignment.  The rules are restated
 below (`*_rule`); `VARIANTS` lists every instance the library compiles (tests/test_row_kernel_table_cpu.py keeps it
 equal to the built library's symbols).  The case lists select every instance at least twice, one of them with a
@@ -13,9 +14,10 @@ third.
   * kernel identity: every call the numbers tests make of a case (each skinny epilogue, the generic rerun of each row
     case) runs under CUPTI in a child process; the kernel that ran must be the one the rule names, and every instance
     of `VARIANTS` must have run;
-  * Softmax / AddSoftmax and LayerNormalization: bit-exact against the oracle, and the same bits again with the vector
-    kernels switched off (RTEN_B200_NO_VEC_ROWS), with -inf / +inf / NaN / +-3e38 rows, constant rows, eps = 0, rows far
-    from zero, broadcast masks, misaligned / in-place / strided inputs and outputs; random rows also against float64;
+  * Softmax / AddSoftmax and the row normalizations: bit-exact against the oracle, and the same bits again with the
+    vector kernels switched off (RTEN_B200_NO_VEC_ROWS), with -inf / +inf / NaN / +-3e38 rows, constant rows, eps = 0,
+    rows far from zero, broadcast masks, misaligned / in-place / strided inputs and outputs; random rows also against
+    float64;
   * skinny GEMM: small-integer operands (every partial sum exact in f32, so the result is the exact product bit for bit
     in any summation order) and U[0, 1) floats against a float64 product under 1e-8 + 1e-5 |ref|, with alpha, bias,
     Gemm's beta * C, an activation, a row-strided A and a strided output, in both f32 modes;
@@ -43,12 +45,21 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 F32 = np.float32
 
 # ---- the instances the library compiles, and the launchers' selection rules ------------------------------------------
+# The operators of launch_norm and their flag sets FL: RMS 1, skip 2, bias 4, sum output 8
+NORM_OPS = {"LayerNormalization": 0, "RMSNormalization": 1,
+            "SkipLayerNormalization": 2, "SkipLayerNormalization + bias": 6, "SkipLayerNormalization + sum": 10,
+            "SkipLayerNormalization + bias + sum": 14, "SkipSimplifiedLayerNormalization": 3,
+            "SkipSimplifiedLayerNormalization + bias": 7, "SkipSimplifiedLayerNormalization + sum": 11,
+            "SkipSimplifiedLayerNormalization + bias + sum": 15}
+NORM_FLAGS = sorted(NORM_OPS.values())
 VARIANTS = {
     # <S (threads per row / 4), FMAX (float4s per thread)>
     "softmax_vec_kernel": [(1, 2), (1, 4), (1, 8), (1, 16), (2, 2), (2, 4), (2, 8), (2, 16),
                            (4, 2), (4, 4), (4, 8), (4, 16), (8, 2), (8, 4), (8, 8), (8, 16)],
-    # <S (threads per row / 16), FMAX>
-    "layer_norm_vec_kernel": [(1, 4), (1, 8), (1, 12), (1, 16), (2, 4), (2, 8), (2, 12), (2, 16)],
+    # <S (threads per row / 16), FMAX, FL (the operator's flag set, NORM_FLAGS)>
+    "norm_vec_kernel": [(S, fm, fl) for S in (1, 2) for fm in (4, 8, 12, 16) for fl in NORM_FLAGS],
+    # <VPT (float4s per thread), FL>
+    "norm_wide_kernel": [(vpt, fl) for vpt in (4, 8) for fl in NORM_FLAGS],
     # <MT (rows), CPW (columns per warp)>
     "skinny_f32_kernel": [(8, 1), (8, 2), (16, 1), (16, 2), (32, 1)],
     # <MT, CPW, KI (16-byte chunks per lane / 32), WSIGNED, FLN (float4s per lane of the layer norm), DB (double-buffered)>
@@ -61,8 +72,8 @@ VARIANTS = {
                        (16, 1, 2, 0, 8, 0), (16, 1, 2, 1, 8, 0), (16, 2, 2, 0, 8, 0), (16, 2, 2, 1, 8, 0),
                        (16, 4, 2, 0, 8, 1), (16, 4, 2, 1, 8, 1)],
 }
-GENERIC = ("softmax_kernel", "layer_norm_kernel")
-FAMILY_KERNELS = {"softmax": ("softmax_vec_kernel", "softmax_kernel"), "layer_norm": ("layer_norm_vec_kernel", "layer_norm_kernel"),
+GENERIC = ("softmax_kernel", "norm_kernel")
+FAMILY_KERNELS = {"softmax": ("softmax_vec_kernel", "softmax_kernel"), "norm": ("norm_vec_kernel", "norm_wide_kernel", "norm_kernel"),
                   "skinny": ("skinny_f32_kernel",), "qlinear": ("qlinear_kernel",)}
 
 _NAME = re.compile(r"rtb::(\w+)(?:<([^<>]*)>)?\(")
@@ -97,9 +108,13 @@ def softmax_rule(n, rows, sms, vec_ok=True):
     return "softmax_vec_kernel", (S, 2 if F <= 2 else 4 if F <= 4 else 8 if F <= 8 else 16)
 
 
-def layer_norm_rule(n, rows, sms, aligned=True):
-    """launch_layer_norm: S = 1 (16 threads per row) when n % 64 == 0, n <= 1024 and the rows give every SM 32 warps or
-    no S = 2 fits; S = 2 when n % 128 == 0, n <= 2048; F = n / 64 S float4s per thread rounded up to 4, 8, 12 or 16."""
+def norm_rule(n, rows, sms, fl, aligned=True):
+    """launch_norm, for aligned rows with n % 64 == 0 and n <= 8192: S = 1 (16 threads per row) when n <= 1024 and the
+    rows give every SM 32 warps or no S = 2 fits; S = 2 when n % 128 == 0, n <= 2048; F = n / 64 S float4s per thread
+    rounded up to 4, 8, 12 or 16.  No S fits (n > 2048, or n / 64 > 16 and odd): one CTA per row, 4 float4s per thread
+    up to n = 4096, else 8.  Any other row: the generic warp-per-row kernel."""
+    if n % 64 or n > 8192 or not aligned:
+        return "norm_kernel", ()
     S = 0
     for c in (1, 2):
         if n % (64 * c) or n // (64 * c) > 16:
@@ -107,10 +122,10 @@ def layer_norm_rule(n, rows, sms, aligned=True):
         S = c
         if (rows * 16 * c + 31) // 32 >= 32 * sms:
             break
-    if not S or not aligned:
-        return "layer_norm_kernel", ()
+    if not S:
+        return "norm_wide_kernel", (4 if n <= 4096 else 8, fl)
     F = n // (64 * S)
-    return "layer_norm_vec_kernel", (S, 4 if F <= 4 else 8 if F <= 8 else 12 if F <= 12 else 16)
+    return "norm_vec_kernel", (S, 4 if F <= 4 else 8 if F <= 8 else 12 if F <= 12 else 16, fl)
 
 
 def skinny_rule(M, N):
@@ -278,26 +293,31 @@ def softmax_f64_check(s, inp, got, what):
     gc.assert_reference_rule(got.reshape(-1, x.shape[-1])[inp["first"]:], e / e.sum(1, keepdims=True), what)
 
 
-# ---- LayerNormalization -----------------------------------------------------------------------------------------------
+# ---- row normalization ------------------------------------------------------------------------------------------------
 LN_ARMS = ("scalar scale", "scalar scale + scalar bias", "scale", "scale + bias", "scale + scalar bias", "scale + bias, eps 0")
 
 
-def layer_norm_specs(sms):
+def norm_specs(sms):
     big = 2 * 32 * sms + 1  # rows at which 16 lanes per row give every SM 32 warps (odd: a dead row in the last warp)
-    shapes = [(64, 7), (192, 5), (256, big), (320, 3), (448, 9), (512, big), (576, 5), (704, 3), (768, big),
-              (832, 3), (960, 7), (1024, big), (128, 6), (512, 3), (768, 5), (1024, 4), (1152, 3), (1536, 2),
-              (1664, 3), (2048, 5), (100, 5), (4096, 3), (2112, 3)]
-    return [dict(kind="layer_norm", n=n, rows=rows) for n, rows in shapes] + [
-        dict(kind="misaligned x", n=768, rows=5), dict(kind="misaligned out", n=768, rows=5),
-        dict(kind="strided out", n=768, rows=5), dict(kind="in place", n=1024, rows=3)]
+    # For every operator: per vector instance (S = 1, then S = 2; FMAX 4, 8, 12, 16) a row of fewer float4s per thread
+    # than the instance holds and a full one; the CTA-per-row kernel at 4 and 8 float4s per thread, partial and full;
+    # the generic kernel
+    shapes = [(64, 7), (256, big), (320, 3), (512, big), (576, 5), (768, big), (832, 3), (1024, big),
+              (128, 6), (512, 3), (768, 5), (1024, 4), (1152, 3), (1536, 2), (1664, 3), (2048, 5),
+              (2112, 3), (4096, 3), (5120, 3), (8192, 2), (100, 5)]
+    ln = "LayerNormalization"
+    specs = [dict(kind="rows", op=op, n=n, rows=rows) for op in NORM_OPS for n, rows in shapes]
+    specs += [dict(kind="rows", op=ln, n=n, rows=rows) for n, rows in ((192, 5), (448, 9), (704, 3), (960, 7))]
+    return specs + [dict(kind=k, op=ln, n=n, rows=rows) for k, n, rows in (
+        ("misaligned x", 768, 5), ("misaligned out", 768, 5), ("strided out", 768, 5), ("in place", 1024, 3))]
 
 
-def layer_norm_expected(s, sms):
-    return layer_norm_rule(s["n"], s["rows"], sms, aligned=not s["kind"].startswith("misaligned"))
+def norm_expected(s, sms):
+    return norm_rule(s["n"], s["rows"], sms, NORM_OPS[s["op"]], aligned=not s["kind"].startswith("misaligned"))
 
 
-def layer_norm_prepare(s):
-    r = _rng("layer_norm", sorted(s.items()))
+def norm_prepare(s):
+    r = _rng("norm", sorted(s.items()))
     n, rows = s["n"], s["rows"]
     x = (r.standard_normal((rows, n)) * 2).astype(F32)
     specials = [lambda v: v.fill(0.75), lambda v: v.__setitem__(slice(None), (1e4 + r.standard_normal(n)).astype(F32)),
@@ -307,7 +327,9 @@ def layer_norm_prepare(s):
         specials[i](x[i])
     g = (1 + 0.1 * r.standard_normal(n)).astype(F32)
     b = (0.1 * r.standard_normal(n)).astype(F32)
-    return dict(x=x, g=g, b=b, first=first)
+    k = r.standard_normal((rows, n)).astype(F32)  # skip
+    bi = (0.1 * r.standard_normal(n)).astype(F32)  # the skip norms' bias
+    return dict(x=x, g=g, b=b, k=k, bi=bi, first=first)
 
 
 def _ln_params(inp, arm):
@@ -317,7 +339,7 @@ def _ln_params(inp, arm):
             "scale + bias, eps 0": (inp["g"], inp["b"], 0.0)}[arm]
 
 
-def layer_norm_launch(rt, ctx, s, inp, arm="scale + bias"):
+def _layer_norm_launch(rt, ctx, s, inp, arm):
     x = inp["x"]
     g, b, eps = _ln_params(inp, arm)
     op = rt.LayerNormalization(-1, eps)
@@ -345,9 +367,34 @@ def layer_norm_launch(rt, ctx, s, inp, arm="scale + bias"):
     return op.run(ctx, ctx.to_device(x), gd, bd).numpy()
 
 
-def layer_norm_want(oracle, inp, arm):
-    g, b, eps = _ln_params(inp, arm)
-    return oracle.layer_norm(inp["x"], g, b, -1, eps)
+def norm_launch(rt, ctx, s, inp, arm="scale + bias"):
+    """The operator's output; with the sum output, output and sum stacked"""
+    op = s["op"]
+    if op == "LayerNormalization":
+        return _layer_norm_launch(rt, ctx, s, inp, arm)
+    x, g = ctx.to_device(inp["x"]), ctx.to_device(inp["g"])
+    if op == "RMSNormalization":
+        return rt.RMSNormalization(-1, 1e-5).run(ctx, x, g).numpy()
+    skip, bias, want_sum = ctx.to_device(inp["k"]), ctx.to_device(inp["bi"]) if "bias" in op else None, op.endswith("sum")
+    if op.startswith("SkipSimplified"):
+        res = rt.SkipSimplifiedLayerNormalization(1e-5).run(ctx, x, skip, g, bias, want_sum=want_sum)
+    else:
+        res = rt.SkipLayerNormalization(1e-5).run(ctx, x, skip, g, ctx.to_device(inp["b"]), bias, want_sum=want_sum)
+    return np.stack([t.numpy() for t in res]) if want_sum else res.numpy()
+
+
+def norm_want(oracle, s, inp, arm="scale + bias"):
+    from oracle import norms
+    op = s["op"]
+    if op == "LayerNormalization":
+        g, b, eps = _ln_params(inp, arm)
+        return oracle.layer_norm(inp["x"], g, b, -1, eps)
+    if op == "RMSNormalization":
+        return norms.rms_norm(inp["x"], inp["g"], -1, 1e-5)
+    rms = op.startswith("SkipSimplified")
+    out, sm = norms.skip_layer_norm(inp["x"], inp["k"], inp["g"], None if rms else inp["b"], inp["bi"] if "bias" in op else None,
+                                    1e-5, rms=rms)
+    return np.stack([out, sm]) if op.endswith("sum") else out
 
 
 # ---- skinny f32 GEMM --------------------------------------------------------------------------------------------------
@@ -511,7 +558,7 @@ def qlinear_want(oracle, s, inp):
 
 FAMILIES = {
     "softmax": (softmax_specs, softmax_expected, softmax_prepare, softmax_launch),
-    "layer_norm": (layer_norm_specs, layer_norm_expected, layer_norm_prepare, layer_norm_launch),
+    "norm": (norm_specs, norm_expected, norm_prepare, norm_launch),
     "skinny": (skinny_specs, skinny_expected, skinny_prepare, skinny_launch),
     "qlinear": (qlinear_specs, qlinear_expected, qlinear_prepare, qlinear_launch),
 }
@@ -544,8 +591,8 @@ def probe_runs(fam, s, sms):
     want = FAMILIES[fam][1](s, sms)
     if fam == "skinny":
         return [(f"epi={e}", want, dict(epi=e), False) for e in SKINNY_EPILOGUES]
-    if fam in ("softmax", "layer_norm"):
-        return [("", want, {}, False), ("no vector rows", (FAMILY_KERNELS[fam][1], ()), {}, True)]
+    if fam in ("softmax", "norm"):
+        return [("", want, {}, False), ("no vector rows", (FAMILY_KERNELS[fam][-1], ()), {}, True)]
     return [("", want, {}, False)]
 
 
@@ -658,25 +705,42 @@ def test_softmax_bit_exact(rt, oracle, sms):
 
 def test_layer_norm_bit_exact(rt, oracle, sms):
     ctx = rt.Context(0)
-    for s in layer_norm_specs(sms):
-        inp = layer_norm_prepare(s)
-        sid = spec_id("layer_norm", s)
+    for s in norm_specs(sms):
+        if s["op"] != "LayerNormalization":
+            continue
+        inp = norm_prepare(s)
+        sid = spec_id("norm", s)
         for arm in LN_ARMS:
-            got = layer_norm_launch(rt, ctx, s, inp, arm)
-            _bits(got, layer_norm_want(oracle, inp, arm), f"{sid} {arm}")
+            got = norm_launch(rt, ctx, s, inp, arm)
+            _bits(got, norm_want(oracle, s, inp, arm), f"{sid} {arm}")
             with _NoVecRows():
-                _bits(layer_norm_launch(rt, ctx, s, inp, arm), got, f"{sid} {arm}: generic kernel")
+                _bits(norm_launch(rt, ctx, s, inp, arm), got, f"{sid} {arm}: generic kernel")
             if arm == "scale + bias" and inp["first"] < s["rows"]:
                 x = inp["x"][inp["first"]:].astype(np.float64)
                 d = x - x.mean(1, keepdims=True)
                 ref = d / np.sqrt((d * d).mean(1, keepdims=True) + 1e-5) * inp["g"] + inp["b"]
                 err = float(np.abs(got[inp["first"]:] - ref).max())
                 assert err <= 1e-5 * float(np.abs(ref).max()), f"{sid}: float64 error {err:.3e}"
-        if s["kind"] == "layer_norm" and inp["first"] > 0:
+        if s["kind"] == "rows" and inp["first"] > 0:
             # a constant row: (x - mean) = 0 exactly, so the output row is the bias; with eps = 0 it is NaN (0 * inf)
-            y = layer_norm_launch(rt, ctx, s, inp, "scale + bias")
+            y = norm_launch(rt, ctx, s, inp, "scale + bias")
             _bits(y[0], inp["b"], f"{sid}: constant row")
-            assert np.isnan(layer_norm_launch(rt, ctx, s, inp, "scale + bias, eps 0")[0]).all(), f"{sid}: constant row, eps 0"
+            assert np.isnan(norm_launch(rt, ctx, s, inp, "scale + bias, eps 0")[0]).all(), f"{sid}: constant row, eps 0"
+
+
+def test_rms_and_skip_norms_bit_exact(rt, oracle, sms):
+    """RMSNormalization and the eight forms of the skip layer norms (output, and the sum output where one is asked
+    for): bit-exact against oracle/norms.py, and the same bits again from the generic kernel"""
+    ctx = rt.Context(0)
+    for s in norm_specs(sms):
+        if s["op"] == "LayerNormalization":
+            continue
+        inp = norm_prepare(s)
+        sid = spec_id("norm", s)
+        got = norm_launch(rt, ctx, s, inp)
+        _bits(got, norm_want(oracle, s, inp), sid)
+        with _NoVecRows():
+            _bits(norm_launch(rt, ctx, s, inp), got, f"{sid}: generic kernel")
 
 
 @pytest.mark.parametrize("tf32", [False, True], ids=["3xTF32", "TF32"])

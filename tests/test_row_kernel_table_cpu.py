@@ -1,4 +1,4 @@
-"""CPU-only: the variant table of tests/test_gpu_row_kernels.py is exactly the set of Softmax, LayerNormalization,
+"""CPU-only: the variant table of tests/test_gpu_row_kernels.py is exactly the set of Softmax, row normalization,
 skinny-GEMM and quantized-linear kernel instances compiled into the library (its sm_90a symbols, demangled), and its
 case lists select every instance at least twice.  An instance added without a test, or one removed, fails here before
 any GPU time is spent."""
@@ -42,7 +42,7 @@ def test_variant_table_matches_the_library(lib_path):
             f"in the table but not compiled {sorted(set(args) - found.get(base, set()))}")
     for base in rk.GENERIC:
         assert found.get(base) == {()}, f"{base} is not compiled"
-    assert sum(len(v) for v in rk.VARIANTS.values()) == 57
+    assert sum(len(v) for v in rk.VARIANTS.values()) == 149
 
 
 @pytest.mark.parametrize("sms", [132, 114])
@@ -69,5 +69,6 @@ def test_kernel_key_spellings():
     assert rk.kernel_key("void rtb::qlinear_kernel<16, 4, 2, true, 8, true>(rtb::QLinearParams)") == ("qlinear_kernel", (16, 4, 2, 1, 8, 1))
     assert rk.kernel_key("void rtb::qlinear_kernel<(int)8, (int)1, (int)6, (bool)0, (int)6, (bool)0>(rtb::QLinearParams)") == (
         "qlinear_kernel", (8, 1, 6, 0, 6, 0))
-    assert rk.kernel_key("rtb::layer_norm_kernel(rtb::LayerNormParams)") == ("layer_norm_kernel", ())
-    assert rk.kernel_key("void rtb::skip_norm_vec_kernel<1, 4, 2>(rtb::SkipNormParams)") is None
+    assert rk.kernel_key("rtb::norm_kernel(rtb::NormParams)") == ("norm_kernel", ())
+    assert rk.kernel_key("void rtb::norm_vec_kernel<1, 4, 2>(rtb::NormParams)") == ("norm_vec_kernel", (1, 4, 2))
+    assert rk.kernel_key("void rtb::norm_wide_kernel<(int)8, (int)15>(rtb::NormParams)") == ("norm_wide_kernel", (8, 15))

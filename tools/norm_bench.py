@@ -1,9 +1,10 @@
-"""Time the skip layer norms and RMSNormalization at LLM / encoder shapes:
+"""Time LayerNormalization, the skip layer norms and RMSNormalization at LLM / encoder shapes:
   SkipSimplifiedLayerNormalization with the sum output (the decoder residual) against torch (x + skip + bias, then
   F.rms_norm); SkipLayerNormalization with bias and beta against the composed path a caller has without it
   (rten_b200_add x 2 + rten_b200_layer_norm) and against torch (x + skip + bias, then F.layer_norm); RMSNormalization
-  against F.rms_norm.  Shapes: Llama-3-8B decode (8 x 4096) and prefill (2048 x 4096, 8 x 512 x 4096), Qwen2-7B (3584),
-  70B (8192), Phi-3 (3072), BERT-base SkipLayerNorm (16 x 128 x 768).
+  against F.rms_norm; plain LayerNormalization (scale and bias) against F.layer_norm.  Shapes: Llama-3-8B decode
+  (8 x 4096) and prefill (2048 x 4096, 8 x 512 x 4096), Qwen2-7B (3584), 70B (8192), Phi-3 (3072), BERT-base
+  (16 x 128 x 768).
 Each form is captured once as a CUDA graph after warm-up; forms alternate, the L2 cache is flushed before every timed
 replay, and each of `--repeats` samples averages `--iters` replays timed with CUDA events (tools/depthwise_bench.py).
 The bytes bound counts x, skip and out (and the sum for the skip-simplified form) plus gamma / beta / bias once, at
@@ -78,11 +79,13 @@ def main():
             "skip_layer_norm": lambda: keep.append(slo.run(ctx, x, k, g, be, bi)),
             "composed add+add+layer_norm": lambda: keep.append(ln.run(ctx, add.run(ctx, add.run(ctx, x, k), bi), g, be)),
             "rms_norm": lambda: keep.append(rms.run(ctx, x, g)),
+            "layer_norm": lambda: keep.append(ln.run(ctx, x, g, be)),
         }
         torch_forms = {
             "torch skip+rms_norm": lambda: keep.append(F.rms_norm(xt + kt + bit, (H,), gt, eps)),
             "torch skip+layer_norm": lambda: keep.append(F.layer_norm(xt + kt + bit, (H,), gt, bet, eps)),
             "torch rms_norm": lambda: keep.append(F.rms_norm(xt, (H,), gt, eps)),
+            "torch layer_norm": lambda: keep.append(F.layer_norm(xt, (H,), gt, bet, eps)),
         }
         graphs = {}
         with torch.cuda.stream(stream):
@@ -109,6 +112,7 @@ def main():
             "skip_simplified+sum": 4 * (4 * numel + 2 * H), "torch skip+rms_norm": 4 * (3 * numel + 2 * H),
             "skip_layer_norm": 4 * (3 * numel + 3 * H), "composed add+add+layer_norm": 4 * (3 * numel + 3 * H),
             "torch skip+layer_norm": 4 * (3 * numel + 3 * H), "rms_norm": 4 * (2 * numel + H), "torch rms_norm": 4 * (2 * numel + H),
+            "layer_norm": 4 * (2 * numel + 2 * H), "torch layer_norm": 4 * (2 * numel + 2 * H),
         }
         row = dict(shape=sname, dims=list(shape))
         for fname, ts in times.items():
