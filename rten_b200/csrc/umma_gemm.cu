@@ -832,9 +832,9 @@ rten_status launch_umma_gemm(rten_ctx* ctx, const GemmLaunch& L) {
                 // stride-1 windows: the halo-reuse kernel (umma_halo.cu) over a few unit shapes, same timing
                 int halo_bn = 0, halo_T = 0;
                 if (L.conv && L.kind == 0 && L.g.kh * L.g.kw > 1 && !L.x3_cb && !L.proj.C && !getenv("RTEN_B200_NO_HALO")) {
-                    for (int hbn : {32, 64})  // the halo kernel's unit shapes: one 128-slot tile, bn <= 64
-                        for (int hT : {1}) {
-                            if (hbn > L.N) continue;
+                    for (int hbn : {32, 64, 128})  // the halo kernel's unit shapes: 128 or 256 slots, bn <= 64 at 128
+                        for (int hT : {1, 2}) {
+                            if (hbn > L.N || (hT == 1 && hbn > 64)) continue;
                             auto time_halo = [&](int n) -> double {
                                 if (launch_umma_halo_conv(ctx, L, hbn, hT) != RTEN_OK) return -1.0;
                                 cudaEventRecord(e0, ctx->stream);
