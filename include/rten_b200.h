@@ -23,7 +23,8 @@
  *  - Calls enqueue work on the context stream and return without synchronising unless a host
  *    tensor is involved; asynchronous CUDA errors surface on the next call or rten_b200_sync().
  *  - Errors: status codes mirror `OpError` (src/operator.rs:116-144); rten_b200_last_error()
- *    returns the reference's static message string for that error.
+ *    returns the reference's static message string for that error.  When a call fails, every output it
+ *    allocated (`data == NULL` on entry) is freed and its `data` is NULL again: nothing is left to release.
  *  - No CPU fallback exists: without an H100 + driver every op fails with RTEN_ERR_CUDA.
  */
 #ifndef RTEN_B200_H

@@ -220,16 +220,6 @@ rten_status in_last_contiguous(OpScope& sc, const rten_tensor* t, rten_tensor* v
     return s;
 }
 
-// An output a one-kernel attention branch allocated but cannot write (its layout does not fit the kernel): back to the
-// pool, so that the branches below start from the caller's `out` as it was.
-void give_back_output(rten_ctx* ctx, OpScope& sc, rten_tensor* out, const rten_tensor& ov) {
-    if (out->data == ov.data && sc.allocated.size()) {
-        pool_free(ctx, ov.data);
-        out->data = nullptr;
-        sc.allocated.clear();
-    }
-}
-
 // [first, last) byte range a tensor spans
 void byte_span(const rten_tensor* t, uintptr_t* a, uintptr_t* b) {
     *a = reinterpret_cast<uintptr_t>(t->data);
@@ -356,7 +346,7 @@ extern "C" {
 rten_status rten_b200_attention(rten_ctx* ctx, const rten_tensor* query, const rten_tensor* key, const rten_tensor* value,
                                 const rten_tensor* attn_mask, const rten_tensor* nonpad_kv_seqlen, const rten_attention_params* prm,
                                 const rten_tensor* new_key, const rten_tensor* new_value, rten_tensor* out) {
-    if (!ctx) return RTEN_ERR_INVALID_VALUE;
+    RTB_TRY(check_ctx(ctx));
     if (!query || !key || !value || !prm || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
     if (query->dtype != RTEN_F32 || key->dtype != RTEN_F32 || value->dtype != RTEN_F32)
         return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
@@ -434,15 +424,14 @@ rten_status rten_b200_attention(rten_ctx* ctx, const rten_tensor* query, const r
             OpScope sc(ctx);
             rten_tensor ov;
             const int64_t oshape[4] = {B, qh, 1, dh};
-            rten_status st = sc.out(out, RTEN_F32, 4, oshape, &ov, nullptr);
-            if (st == RTEN_OK && ov.strides[3] != 1) st = fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "output head dimension must be contiguous");
-            if (st == RTEN_OK) {
-                decode_out(L, cache_rows(&ov));
-                st = launch_attn_decode(ctx, L);
-            }
-            return sc.finish(st);
+            RTB_TRY(sc.out(out, RTEN_F32, 4, oshape, &ov, nullptr));
+            if (ov.strides[3] != 1) return fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "output head dimension must be contiguous");
+            decode_out(L, cache_rows(&ov));
+            return sc.finish(launch_attn_decode(ctx, L));
         }
     }
+    // The one-kernel branches below allocate `out` in a scope of their own: a branch whose kernel declines the layout
+    // leaves that scope without finishing it, which returns the output, and the next branch starts from `out` as given.
     // ---- encoder shapes (128 keys, head size 64, value tensor stored transposed): one fused kernel per layer where available
     // (single-pass TF32 products: only when the context opted in to that mode)
     if (resident && ctx->f32_mode == RTEN_F32_TF32 && !new_key && !nonpad_kv_seqlen && !prm->is_causal && qh == kvh && dv == dh &&
@@ -451,27 +440,22 @@ rten_status rten_b200_attention(rten_ctx* ctx, const rten_tensor* query, const r
         OpScope sc(ctx);
         rten_tensor ov;
         const int64_t oshape[4] = {B, qh, qs, dh};
-        rten_status st = sc.out(out, RTEN_F32, 4, oshape, &ov, nullptr);
-        if (st == RTEN_OK) {
-            AttnFusedLaunch L;
-            stream_io(L, B, qh, kvh, qs, total, dh, qr, kr, cache_rows(&ov));
-            L.heads = (int)qh;
-            if (value->strides[3] == 1 && value->strides[2] != 1) {  // natural layout: the kernel transposes the tile itself
-                L.v = vr.p;
-                L.v_b = vr.sb;
-                L.v_h = vr.sh;
-                L.v_s = vr.ss;
-            } else {
-                L.vt = transposed_operand(value);
-            }
-            L.mask = attn_mask ? (const float*)attn_mask->data : nullptr;
-            L.m_b = ms[0];
-            L.scale = scale;
-            if (ov.strides[3] == 1 && attn_fused_supported(L)) return sc.finish(launch_attn_fused(ctx, L));
-            give_back_output(ctx, sc, out, ov);  // compose below
+        RTB_TRY(sc.out(out, RTEN_F32, 4, oshape, &ov, nullptr));
+        AttnFusedLaunch L;
+        stream_io(L, B, qh, kvh, qs, total, dh, qr, kr, cache_rows(&ov));
+        L.heads = (int)qh;
+        if (value->strides[3] == 1 && value->strides[2] != 1) {  // natural layout: the kernel transposes the tile itself
+            L.v = vr.p;
+            L.v_b = vr.sb;
+            L.v_h = vr.sh;
+            L.v_s = vr.ss;
+        } else {
+            L.vt = transposed_operand(value);
         }
-        st = sc.finish(st);
-        if (st != RTEN_OK) return st;
+        L.mask = attn_mask ? (const float*)attn_mask->data : nullptr;
+        L.m_b = ms[0];
+        L.scale = scale;
+        if (ov.strides[3] == 1 && attn_fused_supported(L)) return sc.finish(launch_attn_fused(ctx, L));
     }
     // ---- causal, right-padded (nonpad_kv_seqlen) or grouped-query calls with q_seq > 1: the streaming prefill kernel
     // (head size 64 / 128, f32 products in the context's mode); other layouts keep the errors below
@@ -481,19 +465,14 @@ rten_status rten_b200_attention(rten_ctx* ctx, const rten_tensor* query, const r
         OpScope sc(ctx);
         rten_tensor ov;
         const int64_t oshape[4] = {B, qh, qs, dh};
-        rten_status st = sc.out(out, RTEN_F32, 4, oshape, &ov, nullptr);
-        if (st == RTEN_OK) {
-            AttnPrefillLaunch L = prefill_launch(ctx, B, qh, kvh, qs, total, dh, scale, qr, kr, vr, cache_rows(&ov));
-            L.v_natural = value->strides[3] == 1;
-            if (!L.v_natural) L.v = transposed_operand(value);
-            L.len = nonpad_kv_seqlen ? (const int32_t*)nonpad_kv_seqlen->data : nullptr;
-            L.causal = prm->is_causal ? 1 : 0;
-            set_mask(L, attn_mask, ms);
-            if (ov.strides[3] == 1 && attn_prefill_supported(L)) return sc.finish(launch_attn_prefill(ctx, L));
-            give_back_output(ctx, sc, out, ov);
-        }
-        st = sc.finish(st);
-        if (st != RTEN_OK) return st;
+        RTB_TRY(sc.out(out, RTEN_F32, 4, oshape, &ov, nullptr));
+        AttnPrefillLaunch L = prefill_launch(ctx, B, qh, kvh, qs, total, dh, scale, qr, kr, vr, cache_rows(&ov));
+        L.v_natural = value->strides[3] == 1;
+        if (!L.v_natural) L.v = transposed_operand(value);
+        L.len = nonpad_kv_seqlen ? (const int32_t*)nonpad_kv_seqlen->data : nullptr;
+        L.causal = prm->is_causal ? 1 : 0;
+        set_mask(L, attn_mask, ms);
+        if (ov.strides[3] == 1 && attn_prefill_supported(L)) return sc.finish(launch_attn_prefill(ctx, L));
     }
     // ---- general path: scale * Q K^T (+ mask) -> Softmax (NaNs flushed) -> . V  with this library's operators.
     // Causal masking / externally managed caches with q_seq > 1 need the mask spelled out by the caller.
@@ -506,18 +485,16 @@ rten_status rten_b200_attention(rten_ctx* ctx, const rten_tensor* query, const r
     kt.shape[3] = total;
     kt.strides[2] = key->strides[3];
     kt.strides[3] = key->strides[2];
-    rten_tensor scores = empty_tensor();
-    rten_status st = rten_b200_matmul_ex(ctx, query, &kt, nullptr, nullptr, scale, nullptr, 0, &scores);
-    if (st == RTEN_OK) st = rten_b200_softmax(ctx, &scores, attn_mask, -1, 1, &scores);
-    if (st == RTEN_OK) st = rten_b200_matmul(ctx, &scores, value, nullptr, nullptr, 1.0f, out);
-    free_if(ctx, scores);
-    return st;
+    Intermediate scores(ctx);
+    RTB_TRY(rten_b200_matmul_ex(ctx, query, &kt, nullptr, nullptr, scale, nullptr, 0, &scores));
+    RTB_TRY(rten_b200_softmax(ctx, &scores, attn_mask, -1, 1, &scores));
+    return rten_b200_matmul(ctx, &scores, value, nullptr, nullptr, 1.0f, out);
 }
 
 rten_status rten_b200_rotary_embedding(rten_ctx* ctx, const rten_tensor* input, const rten_tensor* cos, const rten_tensor* sin,
                                        const rten_tensor* position_ids, int interleaved, int num_heads, int rotary_embedding_dim,
                                        rten_tensor* out) {
-    if (!ctx) return RTEN_ERR_INVALID_VALUE;
+    RTB_TRY(check_ctx(ctx));
     if (!input || !cos || !sin || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
     if (input->dtype != RTEN_F32 || cos->dtype != RTEN_F32 || sin->dtype != RTEN_F32 || (position_ids && position_ids->dtype != RTEN_I32))
         return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
@@ -544,36 +521,30 @@ rten_status rten_b200_rotary_embedding(rten_ctx* ctx, const rten_tensor* input, 
     const int64_t half = rd / 2;
     OpScope sc(ctx);
     rten_tensor xv, cv, sv, pv;
-    rten_status st = sc.in(input, &xv);
-    if (st == RTEN_OK) st = sc.in(cos, &cv);
-    if (st == RTEN_OK) st = sc.in(sin, &sv);
-    if (st != RTEN_OK) return sc.finish(st);
+    RTB_TRY(sc.in(input, &xv));
+    RTB_TRY(sc.in(cos, &cv));
+    RTB_TRY(sc.in(sin, &sv));
     RotaryTable tab;
     if (position_ids) {
         // the caches are gathered by position: [max_pos, half] tables, gathered to [pb, ps, half]
-        if (position_ids->ndim != 2) return sc.finish(rank_fail(ctx, 3, 2, position_ids->ndim));
-        if (cos->ndim != 2 || sin->ndim != 2) return sc.finish(fail(ctx, RTEN_ERR_INVALID_VALUE, "cos/sin cache must be a 3D tensor"));
-        st = position_view(ctx, sc, position_ids, cos->shape[0], sin->shape[0], &pv);
-        if (st != RTEN_OK) return sc.finish(st);
+        if (position_ids->ndim != 2) return rank_fail(ctx, 3, 2, position_ids->ndim);
+        if (cos->ndim != 2 || sin->ndim != 2) return fail(ctx, RTEN_ERR_INVALID_VALUE, "cos/sin cache must be a 3D tensor");
+        RTB_TRY(position_view(ctx, sc, position_ids, cos->shape[0], sin->shape[0], &pv));
         const int64_t gc[3] = {position_ids->shape[0], position_ids->shape[1], cos->shape[1]};
         const int64_t gs[3] = {position_ids->shape[0], position_ids->shape[1], sin->shape[1]};
-        st = cache_dims(ctx, 3, gc, B, S, half, COS_LAST);
-        if (st == RTEN_OK) st = cache_dims(ctx, 3, gs, B, S, half, SIN_LAST);
-        if (st == RTEN_OK && (cos->shape[0] < 1 || sin->shape[0] < 1)) st = fail(ctx, RTEN_ERR_INVALID_VALUE, "Entry in `indices` is out of range");
-        if (st != RTEN_OK) return sc.finish(st);
+        RTB_TRY(cache_dims(ctx, 3, gc, B, S, half, COS_LAST));
+        RTB_TRY(cache_dims(ctx, 3, gs, B, S, half, SIN_LAST));
+        if (cos->shape[0] < 1 || sin->shape[0] < 1) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Entry in `indices` is out of range");
         rten_tensor cc, scc;
-        st = sc.contiguous(&cv, &cc);
-        if (st == RTEN_OK) st = sc.contiguous(&sv, &scc);
-        if (st != RTEN_OK) return sc.finish(st);
+        RTB_TRY(sc.contiguous(&cv, &cc));
+        RTB_TRY(sc.contiguous(&sv, &scc));
         tab = position_table(cc, scc, half, interleaved, &pv);
     } else {
-        st = cache_dims(ctx, cos->ndim, cos->shape, B, S, half, COS_LAST);
-        if (st == RTEN_OK) st = cache_dims(ctx, sin->ndim, sin->shape, B, S, half, SIN_LAST);
-        if (st != RTEN_OK) return sc.finish(st);
+        RTB_TRY(cache_dims(ctx, cos->ndim, cos->shape, B, S, half, COS_LAST));
+        RTB_TRY(cache_dims(ctx, sin->ndim, sin->shape, B, S, half, SIN_LAST));
         rten_tensor cc = cv, scc = sv;
-        if (cv.strides[2] != 1 && half > 1) st = sc.contiguous(&cv, &cc);
-        if (st == RTEN_OK && sv.strides[2] != 1 && half > 1) st = sc.contiguous(&sv, &scc);
-        if (st != RTEN_OK) return sc.finish(st);
+        if (cv.strides[2] != 1 && half > 1) RTB_TRY(sc.contiguous(&cv, &cc));
+        if (sv.strides[2] != 1 && half > 1) RTB_TRY(sc.contiguous(&sv, &scc));
         tab.cos = (const float*)cc.data;
         tab.sin = (const float*)scc.data;
         tab.half = (int)half;
@@ -584,8 +555,7 @@ rten_status rten_b200_rotary_embedding(rten_ctx* ctx, const rten_tensor* input, 
         tab.s_s = bstride(&scc, 1);
     }
     rten_tensor ov;
-    st = sc.out(out, RTEN_F32, input->ndim, input->shape, &ov, nullptr);
-    if (st != RTEN_OK) return sc.finish(st);
+    RTB_TRY(sc.out(out, RTEN_F32, input->ndim, input->shape, &ov, nullptr));
     RotaryLaunch L;
     L.B = (int)B;
     L.S = (int)S;
@@ -594,8 +564,7 @@ rten_status rten_b200_rotary_embedding(rten_ctx* ctx, const rten_tensor* input, 
     L.rot = tab;
     L.x = input->ndim == 3 ? rows3(&xv, D, 0) : cache_rows(&xv);
     L.y = input->ndim == 3 ? rows3(&ov, D, 0) : cache_rows(&ov);
-    if (B * S * H * D > 0) st = launch_rotary(ctx, L);
-    return sc.finish(st);
+    return sc.finish(B * S * H * D > 0 ? launch_rotary(ctx, L) : RTEN_OK);
 }
 
 rten_status rten_b200_group_query_attention(rten_ctx* ctx, const rten_tensor* query, const rten_tensor* key, const rten_tensor* value,
@@ -603,7 +572,7 @@ rten_status rten_b200_group_query_attention(rten_ctx* ctx, const rten_tensor* qu
                                             const rten_tensor* total_sequence_length, const rten_tensor* cos, const rten_tensor* sin,
                                             const rten_tensor* position_ids, const rten_tensor* attention_bias, const rten_gqa_params* prm,
                                             rten_tensor* out, rten_tensor* present_key, rten_tensor* present_value) {
-    if (!ctx) return RTEN_ERR_INVALID_VALUE;
+    RTB_TRY(check_ctx(ctx));
     if (!query || !seqlens_k || !total_sequence_length || !prm || !out || !present_key || !present_value)
         return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
     for (const rten_tensor* t : {query, key, value, past_key, past_value, cos, sin, attention_bias})
@@ -702,38 +671,37 @@ rten_status rten_b200_group_query_attention(rten_ctx* ctx, const rten_tensor* qu
     // ---- device views
     OpScope sc(ctx);
     rten_tensor qv, kv, vv, pkv, pvv, slv, cv, snv, posv, biasv;
-    rten_status st = sc.in(query, &qv);
-    if (st == RTEN_OK && key) st = sc.in(key, &kv);
-    if (st == RTEN_OK && value) st = sc.in(value, &vv);
-    if (st == RTEN_OK && past_key) st = sc.in(past_key, &pkv);
-    if (st == RTEN_OK && past_value) st = sc.in(past_value, &pvv);
-    if (st == RTEN_OK) st = sc.in(seqlens_k, &slv);
-    if (st == RTEN_OK && attention_bias) st = in_last_contiguous(sc, attention_bias, &biasv);
+    RTB_TRY(sc.in(query, &qv));
+    if (key) RTB_TRY(sc.in(key, &kv));
+    if (value) RTB_TRY(sc.in(value, &vv));
+    if (past_key) RTB_TRY(sc.in(past_key, &pkv));
+    if (past_value) RTB_TRY(sc.in(past_value, &pvv));
+    RTB_TRY(sc.in(seqlens_k, &slv));
+    if (attention_bias) RTB_TRY(in_last_contiguous(sc, attention_bias, &biasv));
     RotaryTable tab;
-    if (st == RTEN_OK && prm->do_rotary) {
-        st = sc.in(cos, &cv);
-        if (st == RTEN_OK) st = sc.in(sin, &snv);
+    if (prm->do_rotary) {
+        RTB_TRY(sc.in(cos, &cv));
+        RTB_TRY(sc.in(sin, &snv));
         rten_tensor cc, scc;
-        if (st == RTEN_OK) st = sc.contiguous(&cv, &cc);
-        if (st == RTEN_OK) st = sc.contiguous(&snv, &scc);
-        if (st == RTEN_OK && position_ids) st = position_view(ctx, sc, position_ids, cos->shape[0], sin->shape[0], &posv);
-        if (st == RTEN_OK && position_ids) {
+        RTB_TRY(sc.contiguous(&cv, &cc));
+        RTB_TRY(sc.contiguous(&snv, &scc));
+        if (position_ids) {
+            RTB_TRY(position_view(ctx, sc, position_ids, cos->shape[0], sin->shape[0], &posv));
             const int64_t gc[3] = {position_ids->shape[0], position_ids->shape[1], half};
-            st = cache_dims(ctx, 3, gc, B, S, half, COS_LAST);
+            RTB_TRY(cache_dims(ctx, 3, gc, B, S, half, COS_LAST));
         }
-        if (st == RTEN_OK && cos->shape[1] != half) st = fail(ctx, RTEN_ERR_INVALID_VALUE, COS_LAST);
-        if (st == RTEN_OK && sin->shape[1] != half) st = fail(ctx, RTEN_ERR_INVALID_VALUE, SIN_LAST);
-        if (st == RTEN_OK && (cos->shape[0] < 1 || sin->shape[0] < 1)) st = fail(ctx, RTEN_ERR_INVALID_VALUE, "Entry in `indices` is out of range");
-        if (st == RTEN_OK) tab = position_table(cc, scc, half, prm->rotary_interleaved, position_ids ? &posv : nullptr);
+        if (cos->shape[1] != half) return fail(ctx, RTEN_ERR_INVALID_VALUE, COS_LAST);
+        if (sin->shape[1] != half) return fail(ctx, RTEN_ERR_INVALID_VALUE, SIN_LAST);
+        if (cos->shape[0] < 1 || sin->shape[0] < 1) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Entry in `indices` is out of range");
+        tab = position_table(cc, scc, half, prm->rotary_interleaved, position_ids ? &posv : nullptr);
     }
     rten_tensor ov, pk, pv;
     const int64_t oshape[3] = {B, S, H * D}, cshape[4] = {B, Hkv, T, D};
-    if (st == RTEN_OK) st = sc.out(out, RTEN_F32, 3, oshape, &ov, nullptr);
-    if (st == RTEN_OK) st = sc.out(present_key, RTEN_F32, 4, cshape, &pk, nullptr);
-    if (st == RTEN_OK) st = sc.out(present_value, RTEN_F32, 4, cshape, &pv, nullptr);
-    if (st == RTEN_OK && (ov.strides[2] != 1 || pk.strides[3] != 1 || pv.strides[3] != 1))
-        st = fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "GroupQueryAttention: the outputs need a contiguous last dimension");
-    if (st != RTEN_OK) return sc.finish(st);
+    RTB_TRY(sc.out(out, RTEN_F32, 3, oshape, &ov, nullptr));
+    RTB_TRY(sc.out(present_key, RTEN_F32, 4, cshape, &pk, nullptr));
+    RTB_TRY(sc.out(present_value, RTEN_F32, 4, cshape, &pv, nullptr));
+    if (ov.strides[2] != 1 || pk.strides[3] != 1 || pv.strides[3] != 1)
+        return fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "GroupQueryAttention: the outputs need a contiguous last dimension");
     if (B * S == 0 || H * D == 0) return sc.finish(RTEN_OK);
 
     const RotaryRows qr = rows3(&qv, D, 0), orows = rows3(&ov, D, 0);
@@ -779,9 +747,8 @@ rten_status rten_b200_group_query_attention(rten_ctx* ctx, const rten_tensor* qu
         }
         decode_out(L, orows);
         if (qr.sd == 1 && kr.sd == 1 && vr.sd == 1 && attn_decode_supported(L)) {
-            if (build) st = launch_rotary(ctx, Rb);
-            if (st == RTEN_OK) st = launch_attn_decode(ctx, L);
-            return sc.finish(st);
+            if (build) RTB_TRY(launch_rotary(ctx, Rb));
+            return sc.finish(launch_attn_decode(ctx, L));
         }
         // (a layout the single-query kernel cannot read: the prompt path below serves one query as well)
     }
@@ -789,9 +756,8 @@ rten_status rten_b200_group_query_attention(rten_ctx* ctx, const rten_tensor* qu
     // ---- prompt: rotary + append, then the streaming prefill kernel over the present caches
     void* qs = nullptr;
     void* le = nullptr;
-    st = temp_alloc(ctx, (size_t)(B * S * H * D) * 4, &qs);
-    if (st == RTEN_OK) st = temp_alloc(ctx, (size_t)B * 4, &le);
-    if (st != RTEN_OK) return sc.finish(st);
+    RTB_TRY(temp_alloc(ctx, (size_t)(B * S * H * D) * 4, &qs));
+    RTB_TRY(temp_alloc(ctx, (size_t)B * 4, &le));
     cache_prep(R, B, S, H, Hkv, D, T, kr, vr, kc, vc, nullptr, nullptr, false, false);
     R.x = qr;
     R.y = dense_rows(qs, S, H, D, false);
@@ -802,11 +768,10 @@ rten_status rten_b200_group_query_attention(rten_ctx* ctx, const rten_tensor* qu
     A.window = window;
     set_mask(A, attention_bias ? &biasv : nullptr, ms);
     if (!attn_prefill_supported(A))
-        return sc.finish(fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "GroupQueryAttention: the present caches and the output need 16-byte aligned rows"));
-    if (build) st = launch_rotary(ctx, Rb);
-    if (st == RTEN_OK) st = launch_rotary(ctx, R);
-    if (st == RTEN_OK) st = launch_attn_prefill(ctx, A);
-    return sc.finish(st);
+        return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "GroupQueryAttention: the present caches and the output need 16-byte aligned rows");
+    if (build) RTB_TRY(launch_rotary(ctx, Rb));
+    RTB_TRY(launch_rotary(ctx, R));
+    return sc.finish(launch_attn_prefill(ctx, A));
 }
 
 rten_status rten_b200_multi_head_attention(rten_ctx* ctx, const rten_tensor* query, const rten_tensor* key, const rten_tensor* value,
@@ -814,7 +779,7 @@ rten_status rten_b200_multi_head_attention(rten_ctx* ctx, const rten_tensor* que
                                            const rten_tensor* past_key, const rten_tensor* past_value, const rten_tensor* past_sequence_length,
                                            const rten_tensor* cache_indirection, const rten_mha_params* prm, rten_tensor* out,
                                            rten_tensor* present_key, rten_tensor* present_value) {
-    if (!ctx) return RTEN_ERR_INVALID_VALUE;
+    RTB_TRY(check_ctx(ctx));
     if (!query || !prm || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
     for (const rten_tensor* t : {query, key, value, bias, attention_bias, past_key, past_value})
         if (t && t->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
@@ -898,22 +863,21 @@ rten_status rten_b200_multi_head_attention(rten_ctx* ctx, const rten_tensor* que
     // ---- device views (head dimension contiguous)
     OpScope sc(ctx);
     rten_tensor qv, kv, vv, bv, mv, abv, pkv, pvv;
-    rten_status st = in_last_contiguous(sc, query, &qv);
-    if (st == RTEN_OK && key) st = in_last_contiguous(sc, key, &kv);
-    if (st == RTEN_OK && key) st = in_last_contiguous(sc, value, &vv);
-    if (st == RTEN_OK && bias) st = in_last_contiguous(sc, bias, &bv);
-    if (st == RTEN_OK && key_padding_mask) st = in_last_contiguous(sc, key_padding_mask, &mv);
-    if (st == RTEN_OK && attention_bias) st = sc.in(attention_bias, &abv);
-    if (st == RTEN_OK && past_key) st = in_last_contiguous(sc, past_key, &pkv);
-    if (st == RTEN_OK && past_value) st = in_last_contiguous(sc, past_value, &pvv);
+    RTB_TRY(in_last_contiguous(sc, query, &qv));
+    if (key) RTB_TRY(in_last_contiguous(sc, key, &kv));
+    if (key) RTB_TRY(in_last_contiguous(sc, value, &vv));
+    if (bias) RTB_TRY(in_last_contiguous(sc, bias, &bv));
+    if (key_padding_mask) RTB_TRY(in_last_contiguous(sc, key_padding_mask, &mv));
+    if (attention_bias) RTB_TRY(sc.in(attention_bias, &abv));
+    if (past_key) RTB_TRY(in_last_contiguous(sc, past_key, &pkv));
+    if (past_value) RTB_TRY(in_last_contiguous(sc, past_value, &pvv));
     rten_tensor ov, pk, pv;
     const int64_t oshape[3] = {B, S, H * D}, cshape[4] = {B, H, T, D};
-    if (st == RTEN_OK) st = sc.out(out, RTEN_F32, 3, oshape, &ov, nullptr);
-    if (st == RTEN_OK && present_key) st = sc.out(present_key, RTEN_F32, 4, cshape, &pk, nullptr);
-    if (st == RTEN_OK && present_value) st = sc.out(present_value, RTEN_F32, 4, cshape, &pv, nullptr);
-    if (st == RTEN_OK && (ov.strides[2] != 1 || (present_key && pk.strides[3] != 1) || (present_value && pv.strides[3] != 1)))
-        st = fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "MultiHeadAttention: the outputs need a contiguous last dimension");
-    if (st != RTEN_OK) return sc.finish(st);
+    RTB_TRY(sc.out(out, RTEN_F32, 3, oshape, &ov, nullptr));
+    if (present_key) RTB_TRY(sc.out(present_key, RTEN_F32, 4, cshape, &pk, nullptr));
+    if (present_value) RTB_TRY(sc.out(present_value, RTEN_F32, 4, cshape, &pv, nullptr));
+    if (ov.strides[2] != 1 || (present_key && pk.strides[3] != 1) || (present_value && pv.strides[3] != 1))
+        return fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "MultiHeadAttention: the outputs need a contiguous last dimension");
     if (B * S == 0) return sc.finish(RTEN_OK);
 
     // head rows (b, s, h, i) of q and of the new k / v
@@ -933,10 +897,9 @@ rten_status rten_b200_multi_head_attention(rten_ctx* ctx, const rten_tensor* que
         void* ks = nullptr;
         void* vs = nullptr;
         const size_t ncache = (size_t)(B * H * T * D);
-        if (bias) st = scratch((size_t)(B * S * H * D), &qs);
-        if (st == RTEN_OK && !present_key) st = scratch(ncache, &ks);
-        if (st == RTEN_OK && !present_value) st = scratch(ncache, &vs);
-        if (st != RTEN_OK) return sc.finish(st);
+        if (bias) RTB_TRY(scratch((size_t)(B * S * H * D), &qs));
+        if (!present_key) RTB_TRY(scratch(ncache, &ks));
+        if (!present_value) RTB_TRY(scratch(ncache, &vs));
         kc = present_key ? cache_rows(&pk) : dense_rows(ks, T, H, D, true);
         vc = present_value ? cache_rows(&pv) : dense_rows(vs, T, H, D, true);
         if (bias) {
@@ -970,9 +933,8 @@ rten_status rten_b200_multi_head_attention(rten_ctx* ctx, const rten_tensor* que
         A.kpm = kpm_d;
         A.kpm_b = kpm_b;
         if (attn_decode_supported(A)) {
-            if (prep) st = launch_rotary(ctx, R);
-            if (st == RTEN_OK) st = launch_attn_decode(ctx, A);
-            return sc.finish(st);
+            if (prep) RTB_TRY(launch_rotary(ctx, R));
+            return sc.finish(launch_attn_decode(ctx, A));
         }
         // (a cache longer than the single-query kernel takes: the prefill kernel serves one query as well)
     }
@@ -991,11 +953,9 @@ rten_status rten_b200_multi_head_attention(rten_ctx* ctx, const rten_tensor* que
     set_mask(A, attention_bias ? &abv : nullptr, ms);
     A.mha = &M;
     if (qa.sd != 1 || kc.sd != 1 || vc.sd != 1 || !attn_prefill_supported(A))
-        return sc.finish(fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE,
-                              "MultiHeadAttention: query, key, value, the caches and the output need 16-byte aligned rows"));
-    if (prep) st = launch_rotary(ctx, R);
-    if (st == RTEN_OK) st = launch_attn_prefill(ctx, A);
-    return sc.finish(st);
+        return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MultiHeadAttention: query, key, value, the caches and the output need 16-byte aligned rows");
+    if (prep) RTB_TRY(launch_rotary(ctx, R));
+    return sc.finish(launch_attn_prefill(ctx, A));
 }
 
 }  // extern "C"

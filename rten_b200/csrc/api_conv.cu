@@ -525,8 +525,7 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
         }
         L.b = packed_weight(wsm, kb, O, kh);
         epilogue(L.epi, 0);
-        rten_status st = launch_umma_gemm(ctx, L);
-        if (st == RTEN_OK) return RTEN_OK;
+        const rten_status st = launch_umma_gemm(ctx, L);
         if (st != RTEN_ERR_UNSUPPORTED_VALUE) return st;
         // otherwise fall through to the generic explicit path
     }
@@ -571,13 +570,14 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
                 R.epi.s_row = OW;
                 R.epi.s_z1 = 1;
                 R.epi.s_col = B * OH * OW;
-                rten_status st = launch_umma_gemm(ctx, R);
-                if (st != RTEN_OK) return fail(ctx, st, "conv window-sum GEMM could not be launched");
+                if (const rten_status st = launch_umma_gemm(ctx, R)) return fail(ctx, st, "conv window-sum GEMM could not be launched");
                 e.rowsum = rs;
             }
-            rten_status st = launch_umma_gemm(ctx, L);
-            if (st == RTEN_OK) continue;
-            if (st != RTEN_ERR_UNSUPPORTED_VALUE) return st;
+            const rten_status st = launch_umma_gemm(ctx, L);
+            if (st != RTEN_ERR_UNSUPPORTED_VALUE) {
+                RTB_TRY(st);
+                continue;
+            }
             // fall through to the explicit path
         }
         // explicit im2col: A = [B*OH*OW, kpad]
@@ -646,8 +646,7 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
                 e.r_row = res_v.strides[3];
                 e.r_z0 = e.r_z1 = 0;
             }
-            rten_status st = launch_umma_gemm(ctx, L);
-            if (st != RTEN_OK) return fail(ctx, st, "conv GEMM could not be launched");
+            if (const rten_status st = launch_umma_gemm(ctx, L)) return fail(ctx, st, "conv GEMM could not be launched");
         } else {
             // NCHW-style output: GEMM into [pixels, Og] temp (no fusion), then strided copy + residual/act
             void* tmp = nullptr;
@@ -661,8 +660,7 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
             e2.act = A.residual ? 0 : A.act;
             GemmLaunch L2 = L;
             L2.epi = e2;
-            rten_status st = launch_umma_gemm(ctx, L2);
-            if (st != RTEN_OK) return fail(ctx, st, "conv GEMM could not be launched");
+            if (const rten_status st = launch_umma_gemm(ctx, L2)) return fail(ctx, st, "conv GEMM could not be launched");
             long long shape[4] = {B, OH, OW, Og};
             long long ss[4] = {OH * OW * Og, OW * Og, Og, 1};
             long long ds[4] = {ov.strides[0], ov.strides[2], ov.strides[3], ov.strides[1]};
@@ -1181,33 +1179,26 @@ rten_status rten_b200_prepack_conv_weight(rten_ctx* ctx, const rten_tensor* w, i
     if (w->dtype == RTEN_I32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
     OpScope sc(ctx);
     rten_tensor wv;
-    rten_status st = sc.in(w, &wv);
-    rten_packed* p = nullptr;
-    if (st == RTEN_OK) {
-        const int es = dtype_size(w->dtype);
-        p = new rten_packed();
-        p->kind = 1;
-        p->dtype = w->dtype;
-        p->O = wv.shape[0];
-        p->Cg = wv.shape[1];
-        p->kh = wv.shape[2];
-        p->kw = wv.shape[3];
-        p->groups = groups;
-        const int64_t n = std::max<int64_t>(p->O * p->Cg * p->kh * p->kw, 1);
-        st = pool_alloc(ctx, (size_t)n * es, &p->data);
-        if (st == RTEN_OK) st = pack_conv_weight(ctx, &wv, es, p->data);
-        if (st == RTEN_OK && es == 1 && p->O > 0) {
-            st = pool_alloc(ctx, (size_t)p->O * 4, (void**)&p->colsum);
-            const int64_t Kd = p->Cg * p->kh * p->kw;
-            if (st == RTEN_OK) st = launch_rowsum8(ctx, p->data, p->dtype == RTEN_I8, p->O, (int)Kd, Kd, p->colsum);
-        }
+    RTB_TRY(sc.in(w, &wv));
+    const int es = dtype_size(w->dtype);
+    PackedPtr p(new rten_packed(), PackedFree{ctx});
+    p->kind = 1;
+    p->dtype = w->dtype;
+    p->O = wv.shape[0];
+    p->Cg = wv.shape[1];
+    p->kh = wv.shape[2];
+    p->kw = wv.shape[3];
+    p->groups = groups;
+    const int64_t n = std::max<int64_t>(p->O * p->Cg * p->kh * p->kw, 1);
+    RTB_TRY(pool_alloc(ctx, (size_t)n * es, &p->data));
+    RTB_TRY(pack_conv_weight(ctx, &wv, es, p->data));
+    if (es == 1 && p->O > 0) {
+        RTB_TRY(pool_alloc(ctx, (size_t)p->O * 4, (void**)&p->colsum));
+        const int64_t Kd = p->Cg * p->kh * p->kw;
+        RTB_TRY(launch_rowsum8(ctx, p->data, p->dtype == RTEN_I8, p->O, (int)Kd, Kd, p->colsum));
     }
-    st = sc.finish(st);
-    if (st != RTEN_OK) {
-        if (p) rten_b200_packed_free(ctx, p);
-        return st;
-    }
-    *out = p;
+    RTB_TRY(sc.finish(RTEN_OK));
+    *out = p.release();
     return RTEN_OK;
 }
 
@@ -1322,46 +1313,38 @@ rten_status rten_b200_prepack_conv_transpose_weight(rten_ctx* ctx, const rten_te
     OpScope sc(ctx);
     rten_tensor wv;
     ConvTShape S;
-    rten_status st = sc.in(w, &wv);
-    if (st == RTEN_OK) st = conv_transpose_shape(ctx, nullptr, wv, nullptr, params, S);
-    if (st == RTEN_OK && (S.sy > 256 || S.sx > 256))
-        st = fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "ConvTranspose strides above 256 are not supported");
-    rten_packed* p = nullptr;
-    if (st == RTEN_OK) {
-        p = new rten_packed();
-        p->kind = 2;
-        p->O = S.O;
-        p->Cg = S.Cg;
-        p->kh = S.kh;
-        p->kw = S.kw;
-        p->groups = S.groups;
-        p->sy = S.sy;
-        p->sx = S.sx;
-        p->dy = S.dy;
-        p->dx = S.dx;
-        p->phases.assign((size_t)(S.sy * S.sx), nullptr);
-        for (int64_t ry = 0; ry < S.sy && st == RTEN_OK; ry++)
-            for (int64_t rx = 0; rx < S.sx && st == RTEN_OK; rx++) {
-                const AxisTaps ty = axis_taps(S.kh, S.sy, S.dy, ry), tx = axis_taps(S.kw, S.sx, S.dx, rx);
-                if (ty.T == 0 || tx.T == 0) continue;
-                rten_packed* ph = new rten_packed();
-                p->phases[(size_t)(ry * S.sx + rx)] = ph;
-                ph->kind = 1;
-                ph->O = S.O;
-                ph->Cg = S.Cg;
-                ph->kh = ty.T;
-                ph->kw = tx.T;
-                ph->groups = S.groups;
-                st = pool_alloc(ctx, (size_t)std::max<int64_t>(S.O * ty.T * tx.T * S.Cg, 1) * 4, &ph->data);
-                if (st == RTEN_OK) st = pack_transpose_phase(ctx, S, ty, tx, ph->data);
-            }
-    }
-    st = sc.finish(st);
-    if (st != RTEN_OK) {
-        if (p) rten_b200_packed_free(ctx, p);
-        return st;
-    }
-    *out = p;
+    RTB_TRY(sc.in(w, &wv));
+    RTB_TRY(conv_transpose_shape(ctx, nullptr, wv, nullptr, params, S));
+    if (S.sy > 256 || S.sx > 256) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "ConvTranspose strides above 256 are not supported");
+    PackedPtr p(new rten_packed(), PackedFree{ctx});
+    p->kind = 2;
+    p->O = S.O;
+    p->Cg = S.Cg;
+    p->kh = S.kh;
+    p->kw = S.kw;
+    p->groups = S.groups;
+    p->sy = S.sy;
+    p->sx = S.sx;
+    p->dy = S.dy;
+    p->dx = S.dx;
+    p->phases.assign((size_t)(S.sy * S.sx), nullptr);
+    for (int64_t ry = 0; ry < S.sy; ry++)
+        for (int64_t rx = 0; rx < S.sx; rx++) {
+            const AxisTaps ty = axis_taps(S.kh, S.sy, S.dy, ry), tx = axis_taps(S.kw, S.sx, S.dx, rx);
+            if (ty.T == 0 || tx.T == 0) continue;
+            rten_packed* ph = new rten_packed();
+            p->phases[(size_t)(ry * S.sx + rx)] = ph;
+            ph->kind = 1;
+            ph->O = S.O;
+            ph->Cg = S.Cg;
+            ph->kh = ty.T;
+            ph->kw = tx.T;
+            ph->groups = S.groups;
+            RTB_TRY(pool_alloc(ctx, (size_t)std::max<int64_t>(S.O * ty.T * tx.T * S.Cg, 1) * 4, &ph->data));
+            RTB_TRY(pack_transpose_phase(ctx, S, ty, tx, ph->data));
+        }
+    RTB_TRY(sc.finish(RTEN_OK));
+    *out = p.release();
     return RTEN_OK;
 }
 
@@ -1401,6 +1384,7 @@ rten_status rten_b200_conv_integer_ex(rten_ctx* ctx, const rten_tensor* x, const
     if ((bias && bias->dtype != RTEN_F32) || (residual && residual->dtype != RTEN_F32))
         return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
     if (activation < 0 || activation > 1) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "only Relu can follow an integer convolution");
+    if (out_range && !scale) return fail(ctx, RTEN_ERR_INVALID_VALUE, "the output range is defined for float outputs: a scale is required");
     OpScope sc(ctx);
     ConvArgs A{};
     A.kind = 1;
@@ -1416,7 +1400,6 @@ rten_status rten_b200_conv_integer_ex(rten_ctx* ctx, const rten_tensor* x, const
     A.residual = residual;
     A.act = activation;
     A.out_range = out_range;
-    if (out_range && !scale) return fail(ctx, RTEN_ERR_INVALID_VALUE, "the output range is defined for float outputs: a scale is required");
     return sc.finish(conv_core(sc, A, out));
 }
 
@@ -1430,41 +1413,36 @@ static rten_status pool2d(rten_ctx* ctx, const rten_tensor* x, const int32_t ker
     if (x->ndim != 4) return fail(ctx, RTEN_ERR_INVALID_VALUE, "input must have 4 dims (NCHW)");
     OpScope sc(ctx);
     rten_tensor xv, ov;
-    rten_status st = sc.in(x, &xv);
+    RTB_TRY(sc.in(x, &xv));
     int64_t OH = 0, OW = 0, p0, p1;
-    if (st == RTEN_OK) st = axis_out(ctx, xv.shape[2], kernel[0], strides[0], false, pads[0], pads[2], 1, &OH, &p0, &p1);
-    if (st == RTEN_OK) st = axis_out(ctx, xv.shape[3], kernel[1], strides[1], false, pads[1], pads[3], 1, &OW, &p0, &p1);
-    if (st == RTEN_OK) {
-        const int64_t B = xv.shape[0], C = xv.shape[1];
-        st = out_like(sc, out, RTEN_F32, xv, false, B, C, OH, OW, &ov);
-        if (st == RTEN_OK) {
-            PoolParams p;
-            p.B = (int)B;
-            p.C = (int)C;
-            p.H = (int)xv.shape[2];
-            p.W = (int)xv.shape[3];
-            p.OH = (int)OH;
-            p.OW = (int)OW;
-            p.kh = kernel[0];
-            p.kw = kernel[1];
-            p.sy = strides[0];
-            p.sx = strides[1];
-            p.pt = pads[0];
-            p.pl = pads[1];
-            p.xs_b = xv.strides[0];
-            p.xs_c = xv.strides[1];
-            p.xs_h = xv.strides[2];
-            p.xs_w = xv.strides[3];
-            p.ys_b = ov.strides[0];
-            p.ys_c = ov.strides[1];
-            p.ys_h = ov.strides[2];
-            p.ys_w = ov.strides[3];
-            p.channels_fastest = ov.strides[1] == 1;
-            st = average ? launch_avgpool(ctx, (const float*)xv.data, (float*)ov.data, p, count_include_pad)
-                         : launch_maxpool(ctx, (const float*)xv.data, (float*)ov.data, p);
-        }
-    }
-    return sc.finish(st);
+    RTB_TRY(axis_out(ctx, xv.shape[2], kernel[0], strides[0], false, pads[0], pads[2], 1, &OH, &p0, &p1));
+    RTB_TRY(axis_out(ctx, xv.shape[3], kernel[1], strides[1], false, pads[1], pads[3], 1, &OW, &p0, &p1));
+    const int64_t B = xv.shape[0], C = xv.shape[1];
+    RTB_TRY(out_like(sc, out, RTEN_F32, xv, false, B, C, OH, OW, &ov));
+    PoolParams p;
+    p.B = (int)B;
+    p.C = (int)C;
+    p.H = (int)xv.shape[2];
+    p.W = (int)xv.shape[3];
+    p.OH = (int)OH;
+    p.OW = (int)OW;
+    p.kh = kernel[0];
+    p.kw = kernel[1];
+    p.sy = strides[0];
+    p.sx = strides[1];
+    p.pt = pads[0];
+    p.pl = pads[1];
+    p.xs_b = xv.strides[0];
+    p.xs_c = xv.strides[1];
+    p.xs_h = xv.strides[2];
+    p.xs_w = xv.strides[3];
+    p.ys_b = ov.strides[0];
+    p.ys_c = ov.strides[1];
+    p.ys_h = ov.strides[2];
+    p.ys_w = ov.strides[3];
+    p.channels_fastest = ov.strides[1] == 1;
+    return sc.finish(average ? launch_avgpool(ctx, (const float*)xv.data, (float*)ov.data, p, count_include_pad)
+                             : launch_maxpool(ctx, (const float*)xv.data, (float*)ov.data, p));
 }
 
 rten_status rten_b200_max_pool(rten_ctx* ctx, const rten_tensor* x, const int32_t kernel[2], const int32_t pads[4],
@@ -1492,7 +1470,7 @@ rten_status rten_b200_resize(rten_ctx* ctx, const rten_tensor* x, const rten_res
     const int nd = xv.ndim;
     int64_t osz[4] = {0, 0, 0, 0};
     float inv[4] = {1.0f, 1.0f, 1.0f, 1.0f};
-    if (const rten_status st = resize_output_size(ctx, xv, p, osz, inv)) return sc.finish(st);
+    RTB_TRY(resize_output_size(ctx, xv, p, osz, inv));
     // resize_impl (resize.rs:350-407): which input axis plays (n, c, h, w); -1 = an added axis of size 1
     bool same = true;
     for (int i = 0; i < nd; i++) same = same && osz[i] == xv.shape[i];
@@ -1510,20 +1488,13 @@ rten_status rten_b200_resize(rten_ctx* ctx, const rten_tensor* x, const rten_res
     } else if (nd == 1) {
         map[3] = 0;
     } else {
-        return sc.finish(fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Only 1D to 4D inputs are supported with up to two resized dimensions"));
+        return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Only 1D to 4D inputs are supported with up to two resized dimensions");
     }
     // output: a 4-D result follows the input's layout, like MaxPool and the convolutions
     rten_tensor ov;
-    {
-        const rten_status st = nd == 4 ? out_like(sc, out, RTEN_F32, xv, false, osz[0], osz[1], osz[2], osz[3], &ov)
-                                       : sc.out(out, RTEN_F32, nd, osz, &ov, nullptr);
-        if (st != RTEN_OK) return sc.finish(st);
-    }
-    if (same) {
-        long long shape[RTEN_MAX_DIMS], ss[RTEN_MAX_DIMS], ds[RTEN_MAX_DIMS];
-        for (int i = 0; i < nd; i++) shape[i] = xv.shape[i], ss[i] = xv.strides[i], ds[i] = ov.strides[i];
-        return sc.finish(numel(&xv) ? launch_nd_copy(ctx, 4, xv.data, ov.data, nd, shape, ss, ds) : RTEN_OK);
-    }
+    RTB_TRY(nd == 4 ? out_like(sc, out, RTEN_F32, xv, false, osz[0], osz[1], osz[2], osz[3], &ov)
+                    : sc.out(out, RTEN_F32, nd, osz, &ov, nullptr));
+    if (same) return sc.finish(numel(&xv) ? copy_view(ctx, xv, ov) : RTEN_OK);
     ResizeParams r;
     r.mode = p->mode;
     r.coord_mode = p->coord_mode;
@@ -1537,9 +1508,9 @@ rten_status rten_b200_resize(rten_ctx* ctx, const rten_tensor* x, const rten_res
         r.os[i] = a >= 0 ? ov.strides[a] : 0;
     }
     if (out4[0] * out4[1] * out4[2] * out4[3] != 0 && in4[2] * in4[3] == 0)
-        return sc.finish(fail(ctx, RTEN_ERR_INVALID_VALUE, "cannot resize an empty input"));
+        return fail(ctx, RTEN_ERR_INVALID_VALUE, "cannot resize an empty input");
     for (int i = 0; i < 4; i++)
-        if (in4[i] > INT32_MAX || out4[i] > INT32_MAX) return sc.finish(fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "dimension too large"));
+        if (in4[i] > INT32_MAX || out4[i] > INT32_MAX) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "dimension too large");
     r.B = (int)out4[0];
     r.C = (int)out4[1];
     r.H = (int)in4[2];
@@ -1579,18 +1550,12 @@ rten_status rten_b200_concat(rten_ctx* ctx, const rten_tensor* const* inputs, in
     }
     OpScope sc(ctx);
     std::vector<rten_tensor> iv((size_t)n);
-    for (int i = 0; i < n; i++) {
-        rten_status st = sc.in(inputs[i], &iv[(size_t)i]);
-        if (st != RTEN_OK) return sc.finish(st);
-    }
+    for (int i = 0; i < n; i++) RTB_TRY(sc.in(inputs[i], &iv[(size_t)i]));
     rten_tensor ov;
-    {
-        // an allocated 4-D output follows input 0's layout
-        OutLayout l;
-        if (nd == 4) l = layout_like(iv[0], false, oshape[0], oshape[1], oshape[2], oshape[3]);
-        rten_status st = sc.out(out, dt, nd, oshape, &ov, (nd == 4 && !out->data) ? l.strides : nullptr);
-        if (st != RTEN_OK) return sc.finish(st);
-    }
+    // an allocated 4-D output follows input 0's layout
+    OutLayout l;
+    if (nd == 4) l = layout_like(iv[0], false, oshape[0], oshape[1], oshape[2], oshape[3]);
+    RTB_TRY(sc.out(out, dt, nd, oshape, &ov, (nd == 4 && !out->data) ? l.strides : nullptr));
     const int es = dtype_size(dt);
     // dimensions of extent 1 dropped, the rest put in the output's memory order, then adjacent dimensions merged where the
     // output and every copied input allow it (the concat axis merges with the dimensions inside it only)
@@ -1666,8 +1631,7 @@ rten_status rten_b200_concat(rten_ctx* ctx, const rten_tensor* const* inputs, in
         cp.shape[j] = j == k - 1 ? shape[j] / unit : shape[j];
         cp.out_strides[j] = stride_of(j, ost[j]);
     }
-    rten_status st = RTEN_OK;
-    for (size_t base = 0; base < srcs.size() && st == RTEN_OK; base += kConcatMaxSources) {
+    for (size_t base = 0; base < srcs.size(); base += kConcatMaxSources) {
         cp.nsrc = (int)std::min<size_t>(kConcatMaxSources, srcs.size() - base);
         for (int i = 0; i < cp.nsrc; i++) {
             const Src& s = srcs[base + (size_t)i];
@@ -1681,9 +1645,9 @@ rten_status rten_b200_concat(rten_ctx* ctx, const rten_tensor* const* inputs, in
                 c.n *= j == ax ? c.ext : cp.shape[j];
             }
         }
-        st = launch_concat(ctx, cp);
+        RTB_TRY(launch_concat(ctx, cp));
     }
-    return sc.finish(st);
+    return sc.finish(RTEN_OK);
 }
 
 rten_status rten_b200_global_average_pool(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out) {
@@ -1693,23 +1657,16 @@ rten_status rten_b200_global_average_pool(rten_ctx* ctx, const rten_tensor* x, r
     if (x->ndim != 4) return fail(ctx, RTEN_ERR_INVALID_VALUE, "input must have 4 dims (NCHW)");
     OpScope sc(ctx);
     rten_tensor xv, ov;
-    rten_status st = sc.in(x, &xv);
-    if (st == RTEN_OK) {
-        const int64_t B = xv.shape[0], C = xv.shape[1], H = xv.shape[2], W = xv.shape[3];
-        int64_t oshape[4] = {B, C, 1, 1};
-        st = sc.out(out, RTEN_F32, 4, oshape, &ov, nullptr);
-        if (st == RTEN_OK && !is_contiguous(&ov)) st = fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "pooled output must be contiguous");
-        if (st == RTEN_OK && B * C > 0) {
-            rten_tensor src = xv;
-            if (!(xv.strides[2] == W * xv.strides[3])) {  // need a uniform stride over (h, w)
-                st = sc.contiguous(&xv, &src);
-            }
-            if (st == RTEN_OK)
-                st = launch_row_mean(ctx, (const float*)src.data, (float*)ov.data, B * C, (int)(H * W), C, src.strides[0],
-                                     src.strides[1], src.strides[3]);
-        }
-    }
-    return sc.finish(st);
+    RTB_TRY(sc.in(x, &xv));
+    const int64_t B = xv.shape[0], C = xv.shape[1], H = xv.shape[2], W = xv.shape[3];
+    int64_t oshape[4] = {B, C, 1, 1};
+    RTB_TRY(sc.out(out, RTEN_F32, 4, oshape, &ov, nullptr));
+    if (!is_contiguous(&ov)) return fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "pooled output must be contiguous");
+    if (B * C == 0) return sc.finish(RTEN_OK);
+    rten_tensor src = xv;
+    if (!(xv.strides[2] == W * xv.strides[3])) RTB_TRY(sc.contiguous(&xv, &src));  // need a uniform stride over (h, w)
+    return sc.finish(launch_row_mean(ctx, (const float*)src.data, (float*)ov.data, B * C, (int)(H * W), C, src.strides[0],
+                                     src.strides[1], src.strides[3]));
 }
 
 }  // extern "C"

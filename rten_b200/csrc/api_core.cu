@@ -165,25 +165,17 @@ rten_status OpScope::contiguous(const rten_tensor* v, rten_tensor* c) {
     }
     *c = *v;
     set_contiguous(c);
-    void* d = nullptr;
-    const int es = dtype_size(v->dtype);
-    RTB_TRY(temp_alloc(ctx, (size_t)(numel(v) ? numel(v) : 1) * es, &d));
-    c->data = d;
-    long long shape[RTEN_MAX_DIMS], ss[RTEN_MAX_DIMS], ds[RTEN_MAX_DIMS];
-    for (int i = 0; i < v->ndim; i++) {
-        shape[i] = v->shape[i];
-        ss[i] = v->strides[i];
-        ds[i] = c->strides[i];
-    }
-    return launch_nd_copy(ctx, es, v->data, d, v->ndim, shape, ss, ds);
+    RTB_TRY(temp_alloc(ctx, (size_t)(numel(v) ? numel(v) : 1) * dtype_size(v->dtype), &c->data));
+    return copy_view(ctx, *v, *c);
 }
 
-rten_status OpScope::finish(rten_status st) {
-    if (st == RTEN_OK) {
+rten_status OpScope::finish(rten_status result) {
+    finished = true;
+    if (result == RTEN_OK) {
         for (auto& cb : copybacks) {
             if (cb.bytes) {
                 cudaError_t e = cudaMemcpyAsync(cb.host, cb.dev, cb.bytes, cudaMemcpyDeviceToHost, ctx->stream);
-                if (e != cudaSuccess) st = fail_cuda(ctx, e, "cudaMemcpyAsync(D2H)");
+                if (e != cudaSuccess) result = fail_cuda(ctx, e, "cudaMemcpyAsync(D2H)");
             }
         }
     } else {
@@ -196,9 +188,9 @@ rten_status OpScope::finish(rten_status st) {
     release_temps(ctx);
     if (host_involved && !ctx->capturing) {
         cudaError_t e = cudaStreamSynchronize(ctx->stream);
-        if (e != cudaSuccess && st == RTEN_OK) st = fail_cuda(ctx, e, "cudaStreamSynchronize");
+        if (e != cudaSuccess && result == RTEN_OK) result = fail_cuda(ctx, e, "cudaStreamSynchronize");
     }
-    return st;
+    return result;
 }
 
 }  // namespace rtb
@@ -400,26 +392,11 @@ rten_status rten_b200_copy(rten_ctx* ctx, const rten_tensor* src, rten_tensor* d
         return RTEN_OK;
     }
     OpScope sc(ctx);
-    rten_tensor s, d;
-    rten_status st = sc.in(src, &s);
-    if (st == RTEN_OK) {
-        if (dst->device >= 0) {
-            d = *dst;
-        } else {
-            rten_tensor tmp = *dst;  // host dst (must be contiguous) via temp
-            st = sc.out(&tmp, dst->dtype, dst->ndim, dst->shape, &d, nullptr);
-        }
-    }
-    if (st == RTEN_OK) {
-        long long shape[RTEN_MAX_DIMS], ss[RTEN_MAX_DIMS], ds[RTEN_MAX_DIMS];
-        for (int i = 0; i < s.ndim; i++) {
-            shape[i] = s.shape[i];
-            ss[i] = s.strides[i];
-            ds[i] = d.strides[i];
-        }
-        st = launch_nd_copy(ctx, es, s.data, d.data, s.ndim, shape, ss, ds);
-    }
-    return sc.finish(st);
+    rten_tensor s, d = *dst;
+    RTB_TRY(sc.in(src, &s));
+    rten_tensor tmp = *dst;  // host dst (must be contiguous) via temp
+    if (dst->device < 0) RTB_TRY(sc.out(&tmp, dst->dtype, dst->ndim, dst->shape, &d, nullptr));
+    return sc.finish(copy_view(ctx, s, d));
 }
 
 // ---- CUDA graphs --------------------------------------------------------------------------

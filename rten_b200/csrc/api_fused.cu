@@ -16,7 +16,7 @@ rten_status rten_b200_quantized_linear(rten_ctx* ctx, const rten_tensor* x, cons
                                        float ln_epsilon, const rten_tensor* w, const rten_packed* pw, const rten_tensor* w_zp,
                                        const rten_tensor* w_scale, const rten_tensor* bias, const rten_tensor* residual,
                                        int activation, rten_tensor* out) {
-    if (!ctx) return RTEN_ERR_INVALID_VALUE;
+    RTB_TRY(check_ctx(ctx));
     if (!x || !w || !w_scale || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
     if (x->dtype != RTEN_F32 || w_scale->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
     if (w->dtype != RTEN_I8 && w->dtype != RTEN_U8) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
@@ -86,40 +86,31 @@ rten_status rten_b200_quantized_linear(rten_ctx* ctx, const rten_tensor* x, cons
             int64_t oshape[RTEN_MAX_DIMS];
             for (int i = 0; i + 1 < x->ndim; i++) oshape[i] = x->shape[i];
             oshape[x->ndim - 1] = N;
-            rten_status st = sc.out(out, RTEN_F32, x->ndim, oshape, &ov, nullptr);
-            if (st == RTEN_OK && !is_contiguous(&ov)) st = fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "output tensor must be contiguous");
-            if (st == RTEN_OK && w_zp) {
+            RTB_TRY(sc.out(out, RTEN_F32, x->ndim, oshape, &ov, nullptr));
+            if (!is_contiguous(&ov)) return fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "output tensor must be contiguous");
+            if (w_zp) {
                 int32_t* zb = nullptr;
                 const int len = (int)numel(w_zp);
-                st = temp_alloc(ctx, (size_t)len * 4, (void**)&zb);
-                if (st == RTEN_OK) st = launch_zp_to_i32(ctx, w_zp->data, w_zp->dtype == RTEN_I8, len, w_zp->ndim == 0 ? 0 : w_zp->strides[0], zb);
+                RTB_TRY(temp_alloc(ctx, (size_t)len * 4, (void**)&zb));
+                RTB_TRY(launch_zp_to_i32(ctx, w_zp->data, w_zp->dtype == RTEN_I8, len, w_zp->ndim == 0 ? 0 : w_zp->strides[0], zb));
                 L.zb = zb;
                 L.zb_len = len;
             }
-            if (st == RTEN_OK) {
-                L.out = (float*)ov.data;
-                L.os = N;
-                st = launch_qlinear(ctx, L);
-            }
-            return sc.finish(st);
+            L.out = (float*)ov.data;
+            L.os = N;
+            return sc.finish(launch_qlinear(ctx, L));
         }
     }
 
     // ---- general path: the operator chain, through this library's own entry points
-    rten_tensor h = empty_tensor(), q = empty_tensor(), qs = empty_tensor(), qz = empty_tensor();
+    Intermediate h(ctx), q(ctx), qs(ctx), qz(ctx);
     const rten_tensor* cur = x;
-    rten_status st = RTEN_OK;
     if (ln_scale) {
-        st = rten_b200_layer_norm(ctx, x, ln_scale, ln_bias, -1, ln_epsilon, &h);
+        RTB_TRY(rten_b200_layer_norm(ctx, x, ln_scale, ln_bias, -1, ln_epsilon, &h));
         cur = &h;
     }
-    if (st == RTEN_OK) st = rten_b200_dynamic_quantize_linear(ctx, cur, &q, &qs, &qz, nullptr);
-    if (st == RTEN_OK) st = rten_b200_matmul_integer_ex(ctx, &q, w, pw, &qz, w_zp, w_scale, &qs, bias, residual, activation, nullptr, out);
-    free_if(ctx, h);
-    free_if(ctx, q);
-    free_if(ctx, qs);
-    free_if(ctx, qz);
-    return st;
+    RTB_TRY(rten_b200_dynamic_quantize_linear(ctx, cur, &q, &qs, &qz, nullptr));
+    return rten_b200_matmul_integer_ex(ctx, &q, w, pw, &qz, w_zp, w_scale, &qs, bias, residual, activation, nullptr, out);
 }
 
 }  // extern "C"

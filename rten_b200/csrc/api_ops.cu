@@ -398,16 +398,7 @@ rten_status matmul_core(OpScope& sc, MatMulArgs& A, rten_tensor* out) {
         }
     launched:;
     }
-    if (copy_out) {
-        long long shape[RTEN_MAX_DIMS], ss[RTEN_MAX_DIMS], ds[RTEN_MAX_DIMS];
-        for (int i = 0; i < on; i++) {
-            shape[i] = oshape[i];
-            ss[i] = dv.strides[i];
-            ds[i] = ov.strides[i];
-        }
-        RTB_TRY(launch_nd_copy(ctx, 4, dv.data, ov.data, on, shape, ss, ds));
-    }
-    return RTEN_OK;
+    return copy_out ? copy_view(ctx, dv, ov) : RTEN_OK;
 }
 
 // The leading ndim - 1 dims of `t` as one row dimension of uniform stride (*rs; any value when there is one row).
@@ -489,18 +480,11 @@ rten_status matmul_nbits(OpScope& sc, const rten_tensor* a, const rten_tensor* b
         int64_t a_rs;
         const float* ap = (const float*)av.data;
         if (!flat_rows(av, &a_rs) || av.strides[av.ndim - 1] != 1 || (a_rs & 3) || (reinterpret_cast<uintptr_t>(ap) & 15)) {
-            float* t = nullptr;
-            RTB_TRY(temp_alloc(ctx, (size_t)(rows * K) * 4, (void**)&t));
-            long long shape[RTEN_MAX_DIMS], ss[RTEN_MAX_DIMS], ds[RTEN_MAX_DIMS];
             rten_tensor c = av;
             set_contiguous(&c);
-            for (int i = 0; i < av.ndim; i++) {
-                shape[i] = av.shape[i];
-                ss[i] = av.strides[i];
-                ds[i] = c.strides[i];
-            }
-            RTB_TRY(launch_nd_copy(ctx, 4, av.data, t, av.ndim, shape, ss, ds));
-            ap = t;
+            RTB_TRY(temp_alloc(ctx, (size_t)(rows * K) * 4, &c.data));
+            RTB_TRY(copy_view(ctx, av, c));
+            ap = (const float*)c.data;
             a_rs = K;
         }
         // B: rows of K / 2 contiguous bytes at a pitch of a multiple of 16 bytes (K % 32 == 0), else copied to one
@@ -533,16 +517,7 @@ rten_status matmul_nbits(OpScope& sc, const rten_tensor* a, const rten_tensor* b
         L.os = o_rs;
         RTB_TRY(launch_nbits(ctx, L));
     }
-    if (!direct) {
-        long long shape[RTEN_MAX_DIMS], ss[RTEN_MAX_DIMS], ds[RTEN_MAX_DIMS];
-        for (int i = 0; i < ov.ndim; i++) {
-            shape[i] = ov.shape[i];
-            ss[i] = dv.strides[i];
-            ds[i] = ov.strides[i];
-        }
-        RTB_TRY(launch_nd_copy(ctx, 4, dv.data, ov.data, ov.ndim, shape, ss, ds));
-    }
-    return RTEN_OK;
+    return direct ? RTEN_OK : copy_view(ctx, dv, ov);
 }
 
 // src/ops/matmul.rs:513-533 zero_point_to_vec validation
@@ -558,33 +533,24 @@ rten_status rten_b200_prepack_b(rten_ctx* ctx, const rten_tensor* b, rten_packed
     if (b->dtype == RTEN_I32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
     OpScope sc(ctx);
     rten_tensor bv;
-    rten_status st = sc.in(b, &bv);
-    rten_packed* p = nullptr;
-    if (st == RTEN_OK) {
-        const int es = dtype_size(b->dtype);
-        p = new rten_packed();
-        p->kind = 0;
-        p->dtype = b->dtype;
-        p->K = bv.shape[0];
-        p->N = bv.shape[1];
-        p->ld = round_up(std::max<int64_t>(p->K, 1), 16 / es);
-        st = pool_alloc(ctx, (size_t)std::max<int64_t>(p->N * p->ld, 1) * es, &p->data);
-        if (st == RTEN_OK) {
-            RTB_CUDA(ctx, cudaMemsetAsync(p->data, 0, (size_t)std::max<int64_t>(p->N * p->ld, 1) * es, ctx->stream));
-            long long shape[2] = {p->N, p->K}, ss[2] = {bv.strides[1], bv.strides[0]}, ds[2] = {p->ld, 1};
-            st = launch_nd_copy(ctx, es, bv.data, p->data, 2, shape, ss, ds);
-        }
-        if (st == RTEN_OK && es == 1 && p->N > 0) {
-            st = pool_alloc(ctx, (size_t)p->N * 4, (void**)&p->colsum);
-            if (st == RTEN_OK) st = launch_rowsum8(ctx, p->data, p->dtype == RTEN_I8, p->N, (int)p->K, p->ld, p->colsum);
-        }
+    RTB_TRY(sc.in(b, &bv));
+    const int es = dtype_size(b->dtype);
+    PackedPtr p(new rten_packed(), PackedFree{ctx});
+    p->kind = 0;
+    p->dtype = b->dtype;
+    p->K = bv.shape[0];
+    p->N = bv.shape[1];
+    p->ld = round_up(std::max<int64_t>(p->K, 1), 16 / es);
+    RTB_TRY(pool_alloc(ctx, (size_t)std::max<int64_t>(p->N * p->ld, 1) * es, &p->data));
+    RTB_CUDA(ctx, cudaMemsetAsync(p->data, 0, (size_t)std::max<int64_t>(p->N * p->ld, 1) * es, ctx->stream));
+    long long shape[2] = {p->N, p->K}, ss[2] = {bv.strides[1], bv.strides[0]}, ds[2] = {p->ld, 1};
+    RTB_TRY(launch_nd_copy(ctx, es, bv.data, p->data, 2, shape, ss, ds));
+    if (es == 1 && p->N > 0) {
+        RTB_TRY(pool_alloc(ctx, (size_t)p->N * 4, (void**)&p->colsum));
+        RTB_TRY(launch_rowsum8(ctx, p->data, p->dtype == RTEN_I8, p->N, (int)p->K, p->ld, p->colsum));
     }
-    st = sc.finish(st);
-    if (st != RTEN_OK) {
-        if (p) rten_b200_packed_free(ctx, p);
-        return st;
-    }
-    *out = p;
+    RTB_TRY(sc.finish(RTEN_OK));
+    *out = p.release();
     return RTEN_OK;
 }
 
@@ -609,59 +575,46 @@ rten_status rten_b200_gemm(rten_ctx* ctx, const rten_tensor* a, const rten_tenso
     if (a->ndim != 2 || b->ndim != 2) return fail(ctx, RTEN_ERR_INVALID_VALUE, "input must have 2 dims");
     OpScope sc(ctx);
     rten_tensor av, bv, cv;
-    rten_status st = sc.in(a, &av);
-    if (st == RTEN_OK) st = sc.in(b, &bv);
-    if (st == RTEN_OK && c) st = sc.in(c, &cv);
-    if (st == RTEN_OK) {
-        auto transpose = [](rten_tensor& t) {
-            std::swap(t.shape[0], t.shape[1]);
-            std::swap(t.strides[0], t.strides[1]);
-        };
-        if (trans_a) transpose(av);
-        if (trans_b) transpose(bv);
-        if (av.shape[1] != bv.shape[0]) {
-            st = fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Columns of first matrix does not match rows of second matrix");
-        } else {
-            MatMulArgs A{};
-            A.kind = 0;
-            A.a = &av;
-            A.b = &bv;
-            A.pb = nullptr;
-            A.out_dtype = RTEN_F32;
-            A.epi.alpha = alpha;
-            const int64_t M = av.shape[0], N = bv.shape[1];
-            if (c && beta != 0.0f) {
-                // broadcast c to [M, N] (matmul.rs:63-67)
-                int64_t cs[2] = {0, 0};
-                bool ok = cv.ndim <= 2;
-                if (ok) {
-                    for (int i = 0; i < cv.ndim; i++) {
-                        const int od = 2 - cv.ndim + i;
-                        const int64_t want = od == 0 ? M : N;
-                        if (cv.shape[i] == want)
-                            cs[od] = cv.strides[i];
-                        else if (cv.shape[i] == 1)
-                            cs[od] = 0;
-                        else
-                            ok = false;
-                    }
-                }
-                if (!ok) {
-                    st = fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Cannot broadcast c to output shape");
-                } else {
-                    A.epi.r = (const float*)cv.data;
-                    A.epi.r_scale = beta;
-                    A.epi.r_row = cs[0];
-                    A.epi.r_col = cs[1];
-                }
-            }
-            if (st == RTEN_OK) {
-                // matmul_core's residual plumbing is for same-shape tensors; C is already set in epi.
-                st = matmul_core(sc, A, out);
-            }
+    RTB_TRY(sc.in(a, &av));
+    RTB_TRY(sc.in(b, &bv));
+    if (c) RTB_TRY(sc.in(c, &cv));
+    auto transpose = [](rten_tensor& t) {
+        std::swap(t.shape[0], t.shape[1]);
+        std::swap(t.strides[0], t.strides[1]);
+    };
+    if (trans_a) transpose(av);
+    if (trans_b) transpose(bv);
+    if (av.shape[1] != bv.shape[0])
+        return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Columns of first matrix does not match rows of second matrix");
+    MatMulArgs A{};
+    A.kind = 0;
+    A.a = &av;
+    A.b = &bv;
+    A.pb = nullptr;
+    A.out_dtype = RTEN_F32;
+    A.epi.alpha = alpha;
+    const int64_t M = av.shape[0], N = bv.shape[1];
+    if (c && beta != 0.0f) {
+        // broadcast c to [M, N] (matmul.rs:63-67)
+        int64_t cs[2] = {0, 0};
+        if (cv.ndim > 2) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Cannot broadcast c to output shape");
+        for (int i = 0; i < cv.ndim; i++) {
+            const int od = 2 - cv.ndim + i;
+            const int64_t want = od == 0 ? M : N;
+            if (cv.shape[i] == want)
+                cs[od] = cv.strides[i];
+            else if (cv.shape[i] == 1)
+                cs[od] = 0;
+            else
+                return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Cannot broadcast c to output shape");
         }
+        A.epi.r = (const float*)cv.data;
+        A.epi.r_scale = beta;
+        A.epi.r_row = cs[0];
+        A.epi.r_col = cs[1];
     }
-    return sc.finish(st);
+    // matmul_core's residual plumbing is for same-shape tensors; C is already set in epi.
+    return sc.finish(matmul_core(sc, A, out));
 }
 
 // ---- MatMul / FusedMatMul -----------------------------------------------------------------
@@ -674,14 +627,12 @@ rten_status rten_b200_matmul_ex(rten_ctx* ctx, const rten_tensor* a, const rten_
         return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
     OpScope sc(ctx);
     rten_tensor av, bv, biasv, biasc;
-    rten_status st = sc.in(a, &av);
-    if (st == RTEN_OK) {
-        if (pb) {
-            bv = *b;  // only the shape is consulted
-            bv.data = nullptr;
-        } else {
-            st = sc.in(b, &bv);
-        }
+    RTB_TRY(sc.in(a, &av));
+    if (pb) {
+        bv = *b;  // only the shape is consulted
+        bv.data = nullptr;
+    } else {
+        RTB_TRY(sc.in(b, &bv));
     }
     MatMulArgs A{};
     A.kind = 0;
@@ -692,20 +643,16 @@ rten_status rten_b200_matmul_ex(rten_ctx* ctx, const rten_tensor* a, const rten_
     A.epi.alpha = alpha;
     A.epi.act = activation;
     A.residual = residual;
-    if (st == RTEN_OK && bias) {
-        if (bias->dtype != RTEN_F32 || bias->ndim != 1) {
-            st = fail(ctx, RTEN_ERR_CAST_FAILED, "bias must be a float vector");
-        } else {
-            st = sc.in(bias, &biasv);
-            if (st == RTEN_OK) st = sc.contiguous(&biasv, &biasc);
-            const int64_t N = bv.ndim >= 2 ? bv.shape[bv.ndim - 1] : 1;
-            if (st == RTEN_OK && biasc.shape[0] != N) st = fail(ctx, RTEN_ERR_INVALID_VALUE, "WrongBiasSize");
-            A.epi.bias = (const float*)biasc.data;
-            A.epi.bias_kind = 1;
-        }
+    if (bias) {
+        if (bias->dtype != RTEN_F32 || bias->ndim != 1) return fail(ctx, RTEN_ERR_CAST_FAILED, "bias must be a float vector");
+        RTB_TRY(sc.in(bias, &biasv));
+        RTB_TRY(sc.contiguous(&biasv, &biasc));
+        const int64_t N = bv.ndim >= 2 ? bv.shape[bv.ndim - 1] : 1;
+        if (biasc.shape[0] != N) return fail(ctx, RTEN_ERR_INVALID_VALUE, "WrongBiasSize");
+        A.epi.bias = (const float*)biasc.data;
+        A.epi.bias_kind = 1;
     }
-    if (st == RTEN_OK) st = matmul_core(sc, A, out);
-    return sc.finish(st);
+    return sc.finish(matmul_core(sc, A, out));
 }
 
 rten_status rten_b200_matmul(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, const rten_packed* pb,
@@ -748,15 +695,13 @@ rten_status rten_b200_matmul_integer_ex(rten_ctx* ctx, const rten_tensor* a, con
     RTB_TRY(check_zero_point(ctx, b_zp, b_cols, b->dtype));
     OpScope sc(ctx);
     rten_tensor av, bv, sv, svc;
-    rten_status st = sc.in(a, &av);
-    if (st == RTEN_OK) {
-        if (pb && pb->dtype == b->dtype) {
-            bv = *b;
-            bv.data = nullptr;
-        } else {
-            pb = nullptr;
-            st = sc.in(b, &bv);
-        }
+    RTB_TRY(sc.in(a, &av));
+    if (pb && pb->dtype == b->dtype) {
+        bv = *b;
+        bv.data = nullptr;
+    } else {
+        pb = nullptr;
+        RTB_TRY(sc.in(b, &bv));
     }
     MatMulArgs A{};
     A.kind = 1;
@@ -766,52 +711,40 @@ rten_status rten_b200_matmul_integer_ex(rten_ctx* ctx, const rten_tensor* a, con
     A.a_zp = a_zp;
     A.b_zp = b_zp;
     A.out_dtype = scale ? RTEN_F32 : RTEN_I32;
-    if (st == RTEN_OK && scale) {
+    if (scale) {
         // OutputScale::from_view (matmul.rs:712-721)
-        if (scale->dtype != RTEN_F32) {
-            st = fail(ctx, RTEN_ERR_CAST_FAILED, "scale must be float");
-        } else if (scale->ndim > 1) {
-            st = fail(ctx, RTEN_ERR_INVALID_VALUE, "scale should have rank 0 or 1");
-        } else {
-            st = sc.in(scale, &sv);
-            if (st == RTEN_OK) st = sc.contiguous(&sv, &svc);
-            const int64_t len = svc.ndim == 0 ? 1 : svc.shape[0];
-            if (st == RTEN_OK && len != 1 && len != b_cols)
-                st = fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Scale length does not match tensor columns");
-            A.epi.scale = (const float*)svc.data;
-            A.epi.scale_len = (int)len;
-        }
+        if (scale->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_CAST_FAILED, "scale must be float");
+        if (scale->ndim > 1) return fail(ctx, RTEN_ERR_INVALID_VALUE, "scale should have rank 0 or 1");
+        RTB_TRY(sc.in(scale, &sv));
+        RTB_TRY(sc.contiguous(&sv, &svc));
+        const int64_t len = svc.ndim == 0 ? 1 : svc.shape[0];
+        if (len != 1 && len != b_cols) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Scale length does not match tensor columns");
+        A.epi.scale = (const float*)svc.data;
+        A.epi.scale_len = (int)len;
     }
     rten_tensor biasv, biasc, s2v;
-    if (st == RTEN_OK && scale_b) {
-        if (scale_b->dtype != RTEN_F32 || numel(scale_b) != 1) {
-            st = fail(ctx, RTEN_ERR_INVALID_VALUE, "the second scale factor must be a float scalar");
-        } else {
-            st = sc.in(scale_b, &s2v);
-            A.epi.scale2 = (const float*)s2v.data;
-        }
+    if (scale_b) {
+        if (scale_b->dtype != RTEN_F32 || numel(scale_b) != 1)
+            return fail(ctx, RTEN_ERR_INVALID_VALUE, "the second scale factor must be a float scalar");
+        RTB_TRY(sc.in(scale_b, &s2v));
+        A.epi.scale2 = (const float*)s2v.data;
     }
-    if (st == RTEN_OK && bias) {
-        if (bias->dtype != RTEN_F32 || bias->ndim != 1) {
-            st = fail(ctx, RTEN_ERR_CAST_FAILED, "bias must be a float vector");
-        } else {
-            st = sc.in(bias, &biasv);
-            if (st == RTEN_OK) st = sc.contiguous(&biasv, &biasc);
-            if (st == RTEN_OK && biasc.shape[0] != b_cols) st = fail(ctx, RTEN_ERR_INVALID_VALUE, "WrongBiasSize");
-            A.epi.bias = (const float*)biasc.data;
-            A.epi.bias_kind = 1;
-        }
+    if (bias) {
+        if (bias->dtype != RTEN_F32 || bias->ndim != 1) return fail(ctx, RTEN_ERR_CAST_FAILED, "bias must be a float vector");
+        RTB_TRY(sc.in(bias, &biasv));
+        RTB_TRY(sc.contiguous(&biasv, &biasc));
+        if (biasc.shape[0] != b_cols) return fail(ctx, RTEN_ERR_INVALID_VALUE, "WrongBiasSize");
+        A.epi.bias = (const float*)biasc.data;
+        A.epi.bias_kind = 1;
     }
     A.epi.act = activation;
     A.residual = residual;
-    if (st == RTEN_OK && out_range) {
+    if (out_range) {
         if (!scale || out_range->dtype != RTEN_I32 || numel(out_range) != 2 || out_range->device < 0 || !is_contiguous(out_range))
-            st = fail(ctx, RTEN_ERR_INVALID_VALUE, "the output range must be a device-resident i32[2] (float outputs only)");
-        else
-            A.epi.range = (int*)out_range->data;
+            return fail(ctx, RTEN_ERR_INVALID_VALUE, "the output range must be a device-resident i32[2] (float outputs only)");
+        A.epi.range = (int*)out_range->data;
     }
-    if (st == RTEN_OK) st = matmul_core(sc, A, out);
-    return sc.finish(st);
+    return sc.finish(matmul_core(sc, A, out));
 }
 
 }  // extern "C"

@@ -32,97 +32,73 @@ rten_status rten_b200_softmax(rten_ctx* ctx, const rten_tensor* x, const rten_te
     const int ax = axis < 0 ? axis + nd : axis;
     OpScope sc(ctx);
     rten_tensor xv, mv, ov;
-    rten_status st = sc.in(x, &xv);
-    if (st == RTEN_OK && mask) st = sc.in(mask, &mv);
-    if (st == RTEN_OK) st = sc.out(out, RTEN_F32, nd, xv.shape, &ov, nullptr);
-    if (st == RTEN_OK && numel(&xv) > 0) {
-        // view with `ax` moved last
-        int perm[RTEN_MAX_DIMS], k = 0;
-        for (int i = 0; i < nd; i++)
-            if (i != ax) perm[k++] = i;
-        perm[nd - 1] = ax;
-        rten_tensor xp = xv, op = ov;
-        for (int i = 0; i < nd; i++) {
-            xp.shape[i] = xv.shape[perm[i]];
-            xp.strides[i] = xv.strides[perm[i]];
-            op.shape[i] = ov.shape[perm[i]];
-            op.strides[i] = ov.strides[perm[i]];
-        }
-        rten_tensor xc;
-        st = sc.contiguous(&xp, &xc);
-        // run in place on the output when it is lane-contiguous in the permuted view, else via temp
-        rten_tensor yc = op;
-        const bool out_direct = is_contiguous(&op);
-        if (st == RTEN_OK && !out_direct) {
-            set_contiguous(&yc);
-            void* t = nullptr;
-            st = temp_alloc(ctx, (size_t)numel(&xv) * 4, &t);
-            yc.data = t;
-        }
-        if (st == RTEN_OK) {
-            const int n = (int)xp.shape[nd - 1];
-            const long long rows = numel(&xv) / n;
-            const float* mp = nullptr;
-            long long lead[4] = {1, 1, 1, 1}, ms[4] = {0, 0, 0, 0}, ms_last = 0;
-            int nlead = 0;
-            if (mask) {
-                // broadcast mask to x's shape (numpy rules), in the permuted dim order
-                if (mv.ndim > nd) {
-                    st = fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Cannot broadcast inputs");
-                } else {
-                    long long mstr[RTEN_MAX_DIMS];
-                    for (int i = 0; i < nd && st == RTEN_OK; i++) {
-                        const int mi = i - (nd - mv.ndim);
-                        if (mi < 0 || mv.shape[mi] == 1)
-                            mstr[i] = 0;
-                        else if (mv.shape[mi] == xv.shape[i])
-                            mstr[i] = mv.strides[mi];
-                        else
-                            st = fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Cannot broadcast inputs");
-                    }
-                    if (st == RTEN_OK) {
-                        // leading dims in permuted order, collapsed where the mask advances uniformly
-                        std::vector<long long> ls, lst;
-                        for (int i = 0; i < nd - 1; i++) {
-                            const long long s = xp.shape[i], stv = mstr[perm[i]];
-                            if (s == 1) continue;
-                            if (!ls.empty() && lst.back() == stv * s) {
-                                ls.back() *= s;
-                                lst.back() = stv;
-                            } else {
-                                ls.push_back(s);
-                                lst.push_back(stv);
-                            }
-                        }
-                        if (ls.size() > 4) {
-                            st = fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "mask broadcast pattern needs more than 4 strided dims");
-                        } else {
-                            nlead = (int)ls.size();
-                            for (int i = 0; i < nlead; i++) {
-                                lead[i] = ls[i];
-                                ms[i] = lst[i];
-                            }
-                            ms_last = mstr[ax];
-                            mp = (const float*)mv.data;
-                        }
-                    }
-                }
-            }
-            if (st == RTEN_OK)
-                st = launch_softmax(ctx, (const float*)xc.data, (float*)yc.data, rows, n, flush_nans, mp, nlead, lead, ms,
-                                    ms_last);
-            if (st == RTEN_OK && !out_direct) {
-                long long shape[RTEN_MAX_DIMS], ss[RTEN_MAX_DIMS], ds[RTEN_MAX_DIMS];
-                for (int i = 0; i < nd; i++) {
-                    shape[i] = yc.shape[i];
-                    ss[i] = yc.strides[i];
-                    ds[i] = op.strides[i];
-                }
-                st = launch_nd_copy(ctx, 4, yc.data, op.data, nd, shape, ss, ds);
-            }
-        }
+    RTB_TRY(sc.in(x, &xv));
+    if (mask) RTB_TRY(sc.in(mask, &mv));
+    RTB_TRY(sc.out(out, RTEN_F32, nd, xv.shape, &ov, nullptr));
+    if (numel(&xv) == 0) return sc.finish(RTEN_OK);
+    // view with `ax` moved last
+    int perm[RTEN_MAX_DIMS], k = 0;
+    for (int i = 0; i < nd; i++)
+        if (i != ax) perm[k++] = i;
+    perm[nd - 1] = ax;
+    rten_tensor xp = xv, op = ov;
+    for (int i = 0; i < nd; i++) {
+        xp.shape[i] = xv.shape[perm[i]];
+        xp.strides[i] = xv.strides[perm[i]];
+        op.shape[i] = ov.shape[perm[i]];
+        op.strides[i] = ov.strides[perm[i]];
     }
-    return sc.finish(st);
+    rten_tensor xc;
+    RTB_TRY(sc.contiguous(&xp, &xc));
+    // run in place on the output when it is lane-contiguous in the permuted view, else via temp
+    rten_tensor yc = op;
+    const bool out_direct = is_contiguous(&op);
+    if (!out_direct) {
+        set_contiguous(&yc);
+        RTB_TRY(temp_alloc(ctx, (size_t)numel(&xv) * 4, &yc.data));
+    }
+    const int n = (int)xp.shape[nd - 1];
+    const long long rows = numel(&xv) / n;
+    const float* mp = nullptr;
+    long long lead[4] = {1, 1, 1, 1}, ms[4] = {0, 0, 0, 0}, ms_last = 0;
+    int nlead = 0;
+    if (mask) {
+        // broadcast mask to x's shape (numpy rules), in the permuted dim order
+        if (mv.ndim > nd) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Cannot broadcast inputs");
+        long long mstr[RTEN_MAX_DIMS];
+        for (int i = 0; i < nd; i++) {
+            const int mi = i - (nd - mv.ndim);
+            if (mi < 0 || mv.shape[mi] == 1)
+                mstr[i] = 0;
+            else if (mv.shape[mi] == xv.shape[i])
+                mstr[i] = mv.strides[mi];
+            else
+                return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Cannot broadcast inputs");
+        }
+        // leading dims in permuted order, collapsed where the mask advances uniformly
+        std::vector<long long> ls, lst;
+        for (int i = 0; i < nd - 1; i++) {
+            const long long s = xp.shape[i], stv = mstr[perm[i]];
+            if (s == 1) continue;
+            if (!ls.empty() && lst.back() == stv * s) {
+                ls.back() *= s;
+                lst.back() = stv;
+            } else {
+                ls.push_back(s);
+                lst.push_back(stv);
+            }
+        }
+        if (ls.size() > 4) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "mask broadcast pattern needs more than 4 strided dims");
+        nlead = (int)ls.size();
+        for (int i = 0; i < nlead; i++) {
+            lead[i] = ls[i];
+            ms[i] = lst[i];
+        }
+        ms_last = mstr[ax];
+        mp = (const float*)mv.data;
+    }
+    RTB_TRY(launch_softmax(ctx, (const float*)xc.data, (float*)yc.data, rows, n, flush_nans, mp, nlead, lead, ms, ms_last));
+    return sc.finish(out_direct ? RTEN_OK : copy_view(ctx, yc, op));
 }
 
 // ---- LayerNormalization -------------------------------------------------------------------------
@@ -171,46 +147,34 @@ rten_status rten_b200_layer_norm(rten_ctx* ctx, const rten_tensor* x, const rten
     rten_tensor xv, xc, sv, bv, ov;
     NormParams p;
     p.eps = epsilon < 0.0f ? 1e-5f : epsilon;
-    rten_status st = sc.in(x, &xv);
-    if (st == RTEN_OK) st = sc.in(scale, &sv);
-    if (st == RTEN_OK && bias) st = sc.in(bias, &bv);
+    RTB_TRY(sc.in(x, &xv));
+    RTB_TRY(sc.in(scale, &sv));
+    if (bias) RTB_TRY(sc.in(bias, &bv));
     bool g_scalar = false, b_scalar = false;
-    if (st == RTEN_OK) st = norm_param(sc, sv, xv, ax, "`scale` is not broadcastable to normalized axes of input", &p.gamma, &g_scalar);
-    if (st == RTEN_OK && bias) st = norm_param(sc, bv, xv, ax, "`bias` is not broadcastable to normalized axes of input", &p.beta, &b_scalar);
-    if (st == RTEN_OK) st = sc.contiguous(&xv, &xc);
-    if (st == RTEN_OK) st = sc.out(out, RTEN_F32, nd, xv.shape, &ov, nullptr);
-    if (st == RTEN_OK && numel(&xv) > 0) {
-        long long n = 1;
-        for (int i = ax; i < nd; i++) n *= xv.shape[i];
-        // scalar gamma / beta stay on the device and are read by the kernel (the reference's scalar-scale arm computes
-        // rstd = scale / sqrt(var + eps), src/ops/norm.rs:456-529): no host read, no synchronisation, capturable
-        if (g_scalar) std::swap(p.gamma, p.gamma_sp);
-        if (b_scalar) std::swap(p.beta, p.beta_sp);
-        rten_tensor yc = ov;
-        const bool direct = is_contiguous(&ov);
-        if (!direct) {
-            set_contiguous(&yc);
-            void* t = nullptr;
-            st = temp_alloc(ctx, (size_t)numel(&xv) * 4, &t);
-            yc.data = t;
-        }
-        p.x = (const float*)xc.data;
-        p.xs = n;
-        p.y = (float*)yc.data;
-        p.n = (int)n;
-        p.rows = numel(&xv) / n;
-        if (st == RTEN_OK) st = launch_norm(ctx, p);
-        if (st == RTEN_OK && !direct) {
-            long long shape[RTEN_MAX_DIMS], ss[RTEN_MAX_DIMS], ds[RTEN_MAX_DIMS];
-            for (int i = 0; i < nd; i++) {
-                shape[i] = yc.shape[i];
-                ss[i] = yc.strides[i];
-                ds[i] = ov.strides[i];
-            }
-            st = launch_nd_copy(ctx, 4, yc.data, ov.data, nd, shape, ss, ds);
-        }
+    RTB_TRY(norm_param(sc, sv, xv, ax, "`scale` is not broadcastable to normalized axes of input", &p.gamma, &g_scalar));
+    if (bias) RTB_TRY(norm_param(sc, bv, xv, ax, "`bias` is not broadcastable to normalized axes of input", &p.beta, &b_scalar));
+    RTB_TRY(sc.contiguous(&xv, &xc));
+    RTB_TRY(sc.out(out, RTEN_F32, nd, xv.shape, &ov, nullptr));
+    if (numel(&xv) == 0) return sc.finish(RTEN_OK);
+    long long n = 1;
+    for (int i = ax; i < nd; i++) n *= xv.shape[i];
+    // scalar gamma / beta stay on the device and are read by the kernel (the reference's scalar-scale arm computes
+    // rstd = scale / sqrt(var + eps), src/ops/norm.rs:456-529): no host read, no synchronisation, capturable
+    if (g_scalar) std::swap(p.gamma, p.gamma_sp);
+    if (b_scalar) std::swap(p.beta, p.beta_sp);
+    rten_tensor yc = ov;
+    const bool direct = is_contiguous(&ov);
+    if (!direct) {
+        set_contiguous(&yc);
+        RTB_TRY(temp_alloc(ctx, (size_t)numel(&xv) * 4, &yc.data));
     }
-    return sc.finish(st);
+    p.x = (const float*)xc.data;
+    p.xs = n;
+    p.y = (float*)yc.data;
+    p.n = (int)n;
+    p.rows = numel(&xv) / n;
+    RTB_TRY(launch_norm(ctx, p));
+    return sc.finish(direct ? RTEN_OK : copy_view(ctx, yc, ov));
 }
 
 // ---- RMSNormalization and the skip layer norms ------------------------------------------------------
@@ -265,22 +229,20 @@ rten_status rten_b200_rms_norm(rten_ctx* ctx, const rten_tensor* x, const rten_t
     p.eps = epsilon < 0.0f ? 1e-5f : epsilon;
     p.rms = 1;
     bool g_scalar = false;
-    rten_status st = sc.in(x, &xv);
-    if (st == RTEN_OK) st = sc.in(scale, &sv);
-    if (st == RTEN_OK) st = norm_param(sc, sv, xv, ax, "`scale` is not broadcastable to normalized axes of input", &p.gamma, &g_scalar);
-    if (st == RTEN_OK) st = norm_out(sc, out, xv, &ov);
-    if (st == RTEN_OK && numel(&xv) > 0) {
-        st = norm_rows(sc, xv, ax, &xr, &p.xs);
-        if (g_scalar) std::swap(p.gamma, p.gamma_sp);
-        long long n = 1;
-        for (int i = ax; i < nd; i++) n *= xv.shape[i];
-        p.x = (const float*)xr.data;
-        p.y = (float*)ov.data;
-        p.n = (int)n;
-        p.rows = numel(&xv) / n;
-        if (st == RTEN_OK) st = launch_norm(ctx, p);
-    }
-    return sc.finish(st);
+    RTB_TRY(sc.in(x, &xv));
+    RTB_TRY(sc.in(scale, &sv));
+    RTB_TRY(norm_param(sc, sv, xv, ax, "`scale` is not broadcastable to normalized axes of input", &p.gamma, &g_scalar));
+    RTB_TRY(norm_out(sc, out, xv, &ov));
+    if (numel(&xv) == 0) return sc.finish(RTEN_OK);
+    RTB_TRY(norm_rows(sc, xv, ax, &xr, &p.xs));
+    if (g_scalar) std::swap(p.gamma, p.gamma_sp);
+    long long n = 1;
+    for (int i = ax; i < nd; i++) n *= xv.shape[i];
+    p.x = (const float*)xr.data;
+    p.y = (float*)ov.data;
+    p.n = (int)n;
+    p.rows = numel(&xv) / n;
+    return sc.finish(launch_norm(ctx, p));
 }
 
 rten_status rten_b200_skip_layer_norm(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* skip, const rten_tensor* gamma,
@@ -310,35 +272,33 @@ rten_status rten_b200_skip_layer_norm(rten_ctx* ctx, const rten_tensor* x, const
     p.eps = epsilon;
     p.rms = rms ? 1 : 0;
     bool g_scalar = false, b_scalar = false;
-    rten_status st = sc.in(x, &xv);
-    if (st == RTEN_OK) st = sc.in(skip, &kv);
-    if (st == RTEN_OK) st = sc.in(gamma, &gv);
-    if (st == RTEN_OK && beta) st = sc.in(beta, &bev);
-    if (st == RTEN_OK && bias) st = sc.in(bias, &biv);
+    RTB_TRY(sc.in(x, &xv));
+    RTB_TRY(sc.in(skip, &kv));
+    RTB_TRY(sc.in(gamma, &gv));
+    if (beta) RTB_TRY(sc.in(beta, &bev));
+    if (bias) RTB_TRY(sc.in(bias, &biv));
     const int ax = nd - 1;
-    if (st == RTEN_OK) st = norm_param(sc, gv, xv, ax, "`scale` is not broadcastable to normalized axes of input", &p.gamma, &g_scalar);
-    if (st == RTEN_OK && beta) st = norm_param(sc, bev, xv, ax, "`bias` is not broadcastable to normalized axes of input", &p.beta, &b_scalar);
-    if (st == RTEN_OK) st = norm_out(sc, out, xv, &ov);
-    if (st == RTEN_OK && sum_out) st = norm_out(sc, sum_out, xv, &smv);
-    if (st == RTEN_OK && numel(&xv) > 0) {
-        st = norm_rows(sc, xv, ax, &xr, &p.xs);
-        if (st == RTEN_OK) st = norm_rows(sc, kv, sd - 1, &kr, &p.ss);
-        if (g_scalar) std::swap(p.gamma, p.gamma_sp);
-        if (b_scalar) std::swap(p.beta, p.beta_sp);
-        if (bias) {
-            p.bias = (const float*)biv.data;
-            p.bias_inc = biv.shape[0] == 1 ? 0 : (int)biv.strides[0];
-        }
-        p.x = (const float*)xr.data;
-        p.skip = (const float*)kr.data;
-        p.skip_rows = numel(&kv) / H;
-        p.y = (float*)ov.data;
-        p.sum = sum_out ? (float*)smv.data : nullptr;
-        p.n = (int)H;
-        p.rows = numel(&xv) / H;
-        if (st == RTEN_OK) st = launch_norm(ctx, p);
+    RTB_TRY(norm_param(sc, gv, xv, ax, "`scale` is not broadcastable to normalized axes of input", &p.gamma, &g_scalar));
+    if (beta) RTB_TRY(norm_param(sc, bev, xv, ax, "`bias` is not broadcastable to normalized axes of input", &p.beta, &b_scalar));
+    RTB_TRY(norm_out(sc, out, xv, &ov));
+    if (sum_out) RTB_TRY(norm_out(sc, sum_out, xv, &smv));
+    if (numel(&xv) == 0) return sc.finish(RTEN_OK);
+    RTB_TRY(norm_rows(sc, xv, ax, &xr, &p.xs));
+    RTB_TRY(norm_rows(sc, kv, sd - 1, &kr, &p.ss));
+    if (g_scalar) std::swap(p.gamma, p.gamma_sp);
+    if (b_scalar) std::swap(p.beta, p.beta_sp);
+    if (bias) {
+        p.bias = (const float*)biv.data;
+        p.bias_inc = biv.shape[0] == 1 ? 0 : (int)biv.strides[0];
     }
-    return sc.finish(st);
+    p.x = (const float*)xr.data;
+    p.skip = (const float*)kr.data;
+    p.skip_rows = numel(&kv) / H;
+    p.y = (float*)ov.data;
+    p.sum = sum_out ? (float*)smv.data : nullptr;
+    p.n = (int)H;
+    p.rows = numel(&xv) / H;
+    return sc.finish(launch_norm(ctx, p));
 }
 
 // ---- unary elementwise ----------------------------------------------------------------------------
@@ -349,38 +309,21 @@ template <class Flat>
 rten_status elementwise_op(OpScope& sc, const rten_tensor* x, rten_tensor* out, Flat flat) {
     rten_ctx* ctx = sc.ctx;
     rten_tensor xv, ov;
-    rten_status st = sc.in(x, &xv);
-    bool dense = false;
-    if (st == RTEN_OK) dense = span_elems(&xv) == numel(&xv);
-    if (st == RTEN_OK) st = sc.out(out, xv.dtype, xv.ndim, xv.shape, &ov, (out->data == nullptr && dense) ? xv.strides : nullptr);
-    if (st == RTEN_OK && numel(&xv) > 0) {
-        bool same_layout = dense;
-        for (int i = 0; i < xv.ndim && same_layout; i++)
-            if (xv.shape[i] != 1 && xv.strides[i] != ov.strides[i]) same_layout = false;
-        if (same_layout) {
-            st = flat(xv.data, ov.data, numel(&xv));
-        } else {
-            rten_tensor xc;
-            st = sc.contiguous(&xv, &xc);
-            if (st == RTEN_OK && is_contiguous(&ov)) {
-                st = flat(xc.data, ov.data, numel(&xv));
-            } else if (st == RTEN_OK) {
-                void* t = nullptr;
-                st = temp_alloc(ctx, (size_t)numel(&xv) * 4, &t);
-                if (st == RTEN_OK) st = flat(xc.data, t, numel(&xv));
-                if (st == RTEN_OK) {
-                    long long shape[RTEN_MAX_DIMS], ss[RTEN_MAX_DIMS], ds[RTEN_MAX_DIMS];
-                    for (int i = 0; i < xv.ndim; i++) {
-                        shape[i] = xc.shape[i];
-                        ss[i] = xc.strides[i];
-                        ds[i] = ov.strides[i];
-                    }
-                    st = launch_nd_copy(ctx, 4, t, ov.data, xv.ndim, shape, ss, ds);
-                }
-            }
-        }
-    }
-    return st;
+    RTB_TRY(sc.in(x, &xv));
+    const bool dense = span_elems(&xv) == numel(&xv);
+    RTB_TRY(sc.out(out, xv.dtype, xv.ndim, xv.shape, &ov, (out->data == nullptr && dense) ? xv.strides : nullptr));
+    if (numel(&xv) == 0) return RTEN_OK;
+    bool same_layout = dense;
+    for (int i = 0; i < xv.ndim && same_layout; i++)
+        if (xv.shape[i] != 1 && xv.strides[i] != ov.strides[i]) same_layout = false;
+    if (same_layout) return flat(xv.data, ov.data, numel(&xv));
+    rten_tensor xc;
+    RTB_TRY(sc.contiguous(&xv, &xc));
+    if (is_contiguous(&ov)) return flat(xc.data, ov.data, numel(&xv));
+    rten_tensor t = xc;
+    RTB_TRY(temp_alloc(ctx, (size_t)numel(&xv) * 4, &t.data));
+    RTB_TRY(flat(xc.data, t.data, numel(&xv)));
+    return copy_view(ctx, t, ov);
 }
 }  // extern "C++"
 
@@ -404,14 +347,11 @@ rten_status rten_b200_clip(rten_ctx* ctx, const rten_tensor* x, const rten_tenso
             return fail(ctx, RTEN_ERR_INVALID_VALUE, "min and max must be scalars of the input's type");
     OpScope sc(ctx);
     rten_tensor mn, mx;  // (read on the device by the kernel: no host synchronisation)
-    rten_status st = RTEN_OK;
-    if (min) st = sc.in(min, &mn);
-    if (st == RTEN_OK && max) st = sc.in(max, &mx);
-    if (st == RTEN_OK)
-        st = elementwise_op(sc, x, out, [&](const void* a, void* y, long long n) {
-            return launch_clip(ctx, x->dtype == RTEN_I32, a, y, n, min ? mn.data : nullptr, max ? mx.data : nullptr);
-        });
-    return sc.finish(st);
+    if (min) RTB_TRY(sc.in(min, &mn));
+    if (max) RTB_TRY(sc.in(max, &mx));
+    return sc.finish(elementwise_op(sc, x, out, [&](const void* a, void* y, long long n) {
+        return launch_clip(ctx, x->dtype == RTEN_I32, a, y, n, min ? mn.data : nullptr, max ? mx.data : nullptr);
+    }));
 }
 
 rten_status rten_b200_erf(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out) { return unary_op(ctx, UNARY_ERF, x, out); }
@@ -436,40 +376,35 @@ static rten_status binary_f32(rten_ctx* ctx, const rten_tensor* a, const rten_te
     if (a->dtype != RTEN_F32 || b->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
     OpScope sc(ctx);
     rten_tensor av, bv, ov;
-    rten_status st = sc.in(a, &av);
-    if (st == RTEN_OK) st = sc.in(b, &bv);
+    RTB_TRY(sc.in(a, &av));
+    RTB_TRY(sc.in(b, &bv));
     int nd = std::max(a->ndim, b->ndim);
     int64_t shape[RTEN_MAX_DIMS];
     long long sa[RTEN_MAX_DIMS], sb[RTEN_MAX_DIMS];
-    for (int i = 0; i < nd && st == RTEN_OK; i++) {
+    for (int i = 0; i < nd; i++) {
         const int ia = i - (nd - av.ndim), ib = i - (nd - bv.ndim);
         const int64_t da = ia >= 0 ? av.shape[ia] : 1, db = ib >= 0 ? bv.shape[ib] : 1;
-        if (da != db && da != 1 && db != 1) st = fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Cannot broadcast inputs");
+        if (da != db && da != 1 && db != 1) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Cannot broadcast inputs");
         shape[i] = (da == 0 || db == 0) ? 0 : std::max(da, db);
         sa[i] = (ia >= 0 && da != 1) ? av.strides[ia] : 0;
         sb[i] = (ib >= 0 && db != 1) ? bv.strides[ib] : 0;
     }
     // same-shape dense operands: keep a's layout for the output
-    bool same = st == RTEN_OK && av.ndim == bv.ndim && span_elems(&av) == numel(&av);
+    bool same = av.ndim == bv.ndim && span_elems(&av) == numel(&av);
     for (int i = 0; i < nd && same; i++)
         if (av.shape[i] != bv.shape[i] || (av.shape[i] != 1 && av.strides[i] != bv.strides[i])) same = false;
-    if (st == RTEN_OK) st = sc.out(out, RTEN_F32, nd, shape, &ov, (out->data == nullptr && same) ? av.strides : nullptr);
-    if (st == RTEN_OK && numel(&ov) > 0) {
-        bool flat = same;
-        for (int i = 0; i < nd && flat; i++)
-            if (ov.shape[i] != 1 && ov.strides[i] != av.strides[i]) flat = false;
-        if (flat) {
-            st = launch_add_flat(ctx, (const float*)av.data, (const float*)bv.data, (float*)ov.data, numel(&ov), flags);
-        } else {
-            long long shp[RTEN_MAX_DIMS], sd[RTEN_MAX_DIMS];
-            for (int i = 0; i < nd; i++) {
-                shp[i] = shape[i];
-                sd[i] = ov.strides[i];
-            }
-            st = launch_nd_add(ctx, (const float*)av.data, (const float*)bv.data, (float*)ov.data, nd, shp, sa, sb, sd, flags);
-        }
+    RTB_TRY(sc.out(out, RTEN_F32, nd, shape, &ov, (out->data == nullptr && same) ? av.strides : nullptr));
+    if (numel(&ov) == 0) return sc.finish(RTEN_OK);
+    bool flat = same;
+    for (int i = 0; i < nd && flat; i++)
+        if (ov.shape[i] != 1 && ov.strides[i] != av.strides[i]) flat = false;
+    if (flat) return sc.finish(launch_add_flat(ctx, (const float*)av.data, (const float*)bv.data, (float*)ov.data, numel(&ov), flags));
+    long long shp[RTEN_MAX_DIMS], sd[RTEN_MAX_DIMS];
+    for (int i = 0; i < nd; i++) {
+        shp[i] = shape[i];
+        sd[i] = ov.strides[i];
     }
-    return sc.finish(st);
+    return sc.finish(launch_nd_add(ctx, (const float*)av.data, (const float*)bv.data, (float*)ov.data, nd, shp, sa, sb, sd, flags));
 }
 
 rten_status rten_b200_add(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out) {
@@ -504,64 +439,59 @@ rten_status rten_b200_dynamic_quantize_linear_ranged(rten_ctx* ctx, const rten_t
         return fail(ctx, RTEN_ERR_INVALID_VALUE, "the range must be a device-resident i32[2]");
     OpScope sc(ctx);
     rten_tensor xv, xc, yv, sv, zv;
-    rten_status st = sc.in(x, &xv);
+    RTB_TRY(sc.in(x, &xv));
     // The op is elementwise plus an order-independent min / max: a DENSE input in any dim order (e.g. channels-last
     // activations) is processed in memory order and the quantised output keeps the input's strides.
-    bool dense = st == RTEN_OK && span_elems(&xv) == numel(&xv) && y->data == nullptr;
+    bool dense = span_elems(&xv) == numel(&xv) && y->data == nullptr;
     for (int i = 0; i < xv.ndim && dense; i++)
         if (xv.strides[i] <= 0 && xv.shape[i] > 1) dense = false;
-    const bool x_cl_dense = st == RTEN_OK && xv.ndim == 4 && xv.strides[1] == 1 && xv.strides[3] == xv.shape[1] &&
+    const bool x_cl_dense = xv.ndim == 4 && xv.strides[1] == 1 && xv.strides[3] == xv.shape[1] &&
                             xv.strides[2] == xv.shape[3] * xv.shape[1] && xv.strides[0] == xv.shape[2] * xv.shape[3] * xv.shape[1];
-    if (dense || (x_cl_dense && y->data && y->ndim == 4 && y->strides[1] == 1)) {
+    if (dense || (x_cl_dense && y->data && y->ndim == 4 && y->strides[1] == 1))
         xc = xv;
-    } else if (st == RTEN_OK) {
-        st = sc.contiguous(&xv, &xc);
-    }
+    else
+        RTB_TRY(sc.contiguous(&xv, &xc));
     // A caller-provided channels-last output whose rows (b, h) sit at arbitrary pitches -- the interior of a spatially
     // pre-padded buffer, so that the consuming ConvInteger needs no padded copy -- is written row by row.
     bool rows_out = false;
-    if (st == RTEN_OK && y->data && xv.ndim == 4 && y->ndim == 4 && y->device >= 0) {
+    if (y->data && xv.ndim == 4 && y->ndim == 4 && y->device >= 0) {
         const int64_t Cc = xv.shape[1], Hh = xv.shape[2], Ww = xv.shape[3];
         rows_out = xv.strides[1] == 1 && xv.strides[3] == Cc && xv.strides[2] == Ww * Cc && xv.strides[0] == Hh * Ww * Cc &&
                    y->strides[1] == 1 && y->strides[3] == Cc && !is_contiguous(y) &&
                    !(y->strides[2] == Ww * Cc && y->strides[0] == Hh * Ww * Cc);
         if (rows_out) xc = xv;
     }
-    if (st == RTEN_OK) st = sc.out(y, RTEN_U8, xv.ndim, xv.shape, &yv, dense ? xv.strides : nullptr);
-    if (st == RTEN_OK) st = sc.out(scale, RTEN_F32, 0, nullptr, &sv, nullptr);
-    if (st == RTEN_OK) st = sc.out(zero_point, RTEN_U8, 0, nullptr, &zv, nullptr);
-    if (st == RTEN_OK && !dense && !rows_out && !is_contiguous(&yv)) st = fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "quantized output must be contiguous");
-    if (st == RTEN_OK) {
-        const long long n = numel(&xv);
-        if (n == 0) {
-            // quantize.rs:378-386: scale 1, zero point 0
-            const float one = 1.0f;
-            RTB_CUDA(ctx, cudaMemcpyAsync(sv.data, &one, 4, cudaMemcpyHostToDevice, ctx->stream));
-            RTB_CUDA(ctx, cudaMemsetAsync(zv.data, 0, 1, ctx->stream));
-        } else if (!nccl_comm && !range && !rows_out && n <= 16384) {
-            st = launch_dql_small(ctx, (const float*)xc.data, (uint8_t*)yv.data, (int)n, (float*)sv.data, (uint8_t*)zv.data);
-        } else {
-            // `range`: the producer of x already accumulated (min, max) in its epilogue -- no pass over x for it
-            int* mm = range ? (int*)range->data : nullptr;
-            if (!mm) {
-                st = temp_alloc(ctx, 8, (void**)&mm);
-                if (st == RTEN_OK) st = launch_minmax(ctx, (const float*)xc.data, n, mm);
-            }
-            // batch-sharded run: the range is the range of the whole (unsharded) tensor -- exchanged over NVLink peer
-            // mailboxes by the quantise kernel's own prologue, or by two ncclAllReduce calls in front of it
-            RangeExchange xch;
-            const bool fused_xch = nccl_comm && comm_range_exchange(reinterpret_cast<rten_comm*>(nccl_comm), &xch);
-            if (st == RTEN_OK && nccl_comm && !fused_xch) st = comm_allreduce_minmax(ctx, reinterpret_cast<rten_comm*>(nccl_comm), mm);
-            if (st == RTEN_OK && rows_out)
-                st = launch_dql_quantize_rows(ctx, (const float*)xc.data, (uint8_t*)yv.data, xv.shape[0] * xv.shape[2],
-                                              (int)(xv.shape[3] * xv.shape[1]), (int)xv.shape[2], yv.strides[2], yv.strides[0], mm,
-                                              (float*)sv.data, (uint8_t*)zv.data, fused_xch ? &xch : nullptr);
-            else if (st == RTEN_OK)
-                st = launch_dql_quantize(ctx, (const float*)xc.data, (uint8_t*)yv.data, n, mm, (float*)sv.data, (uint8_t*)zv.data,
-                                         fused_xch ? &xch : nullptr);
-        }
+    RTB_TRY(sc.out(y, RTEN_U8, xv.ndim, xv.shape, &yv, dense ? xv.strides : nullptr));
+    RTB_TRY(sc.out(scale, RTEN_F32, 0, nullptr, &sv, nullptr));
+    RTB_TRY(sc.out(zero_point, RTEN_U8, 0, nullptr, &zv, nullptr));
+    if (!dense && !rows_out && !is_contiguous(&yv)) return fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "quantized output must be contiguous");
+    const long long n = numel(&xv);
+    if (n == 0) {
+        // quantize.rs:378-386: scale 1, zero point 0
+        const float one = 1.0f;
+        RTB_CUDA(ctx, cudaMemcpyAsync(sv.data, &one, 4, cudaMemcpyHostToDevice, ctx->stream));
+        RTB_CUDA(ctx, cudaMemsetAsync(zv.data, 0, 1, ctx->stream));
+        return sc.finish(RTEN_OK);
     }
-    return sc.finish(st);
+    if (!nccl_comm && !range && !rows_out && n <= 16384)
+        return sc.finish(launch_dql_small(ctx, (const float*)xc.data, (uint8_t*)yv.data, (int)n, (float*)sv.data, (uint8_t*)zv.data));
+    // `range`: the producer of x already accumulated (min, max) in its epilogue -- no pass over x for it
+    int* mm = range ? (int*)range->data : nullptr;
+    if (!mm) {
+        RTB_TRY(temp_alloc(ctx, 8, (void**)&mm));
+        RTB_TRY(launch_minmax(ctx, (const float*)xc.data, n, mm));
+    }
+    // batch-sharded run: the range is the range of the whole (unsharded) tensor -- exchanged over NVLink peer
+    // mailboxes by the quantise kernel's own prologue, or by two ncclAllReduce calls in front of it
+    RangeExchange xch;
+    const bool fused_xch = nccl_comm && comm_range_exchange(reinterpret_cast<rten_comm*>(nccl_comm), &xch);
+    if (nccl_comm && !fused_xch) RTB_TRY(comm_allreduce_minmax(ctx, reinterpret_cast<rten_comm*>(nccl_comm), mm));
+    if (rows_out)
+        return sc.finish(launch_dql_quantize_rows(ctx, (const float*)xc.data, (uint8_t*)yv.data, xv.shape[0] * xv.shape[2],
+                                                  (int)(xv.shape[3] * xv.shape[1]), (int)xv.shape[2], yv.strides[2], yv.strides[0],
+                                                  mm, (float*)sv.data, (uint8_t*)zv.data, fused_xch ? &xch : nullptr));
+    return sc.finish(launch_dql_quantize(ctx, (const float*)xc.data, (uint8_t*)yv.data, n, mm, (float*)sv.data, (uint8_t*)zv.data,
+                                         fused_xch ? &xch : nullptr));
 }
 
 // ---- gather / scatter ------------------------------------------------------------------------------
@@ -572,21 +502,17 @@ rten_status rten_b200_gather_rows(rten_ctx* ctx, const rten_tensor* table, const
     if (table->ndim != 2) return fail(ctx, RTEN_ERR_INVALID_VALUE, "gather_rows expects a 2-D table");
     OpScope sc(ctx);
     rten_tensor tv, iv, ic, ov;
-    rten_status st = sc.in(table, &tv);
-    if (st == RTEN_OK) st = sc.in(idx, &iv);
-    if (st == RTEN_OK) st = sc.contiguous(&iv, &ic);
-    if (st == RTEN_OK) {
-        int64_t oshape[RTEN_MAX_DIMS];
-        if (iv.ndim + 1 > RTEN_MAX_DIMS) return sc.finish(fail(ctx, RTEN_ERR_INVALID_VALUE, "tensor rank out of range"));
-        for (int i = 0; i < iv.ndim; i++) oshape[i] = iv.shape[i];
-        oshape[iv.ndim] = tv.shape[1];
-        st = sc.out(out, RTEN_F32, iv.ndim + 1, oshape, &ov, nullptr);
-        if (st == RTEN_OK && !is_contiguous(&ov)) st = fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "gather output must be contiguous");
-        if (st == RTEN_OK)
-            st = launch_gather_rows(ctx, (const float*)tv.data, (const int*)ic.data, (float*)ov.data, numel(&iv),
-                                    (int)tv.shape[1], tv.strides[0], tv.strides[1], tv.shape[0]);
-    }
-    return sc.finish(st);
+    RTB_TRY(sc.in(table, &tv));
+    RTB_TRY(sc.in(idx, &iv));
+    RTB_TRY(sc.contiguous(&iv, &ic));
+    int64_t oshape[RTEN_MAX_DIMS];
+    if (iv.ndim + 1 > RTEN_MAX_DIMS) return fail(ctx, RTEN_ERR_INVALID_VALUE, "tensor rank out of range");
+    for (int i = 0; i < iv.ndim; i++) oshape[i] = iv.shape[i];
+    oshape[iv.ndim] = tv.shape[1];
+    RTB_TRY(sc.out(out, RTEN_F32, iv.ndim + 1, oshape, &ov, nullptr));
+    if (!is_contiguous(&ov)) return fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "gather output must be contiguous");
+    return sc.finish(launch_gather_rows(ctx, (const float*)tv.data, (const int*)ic.data, (float*)ov.data, numel(&iv),
+                                        (int)tv.shape[1], tv.strides[0], tv.strides[1], tv.shape[0]));
 }
 
 rten_status rten_b200_scatter_rows(rten_ctx* ctx, rten_tensor* table, const rten_tensor* idx, const rten_tensor* src) {
@@ -600,14 +526,12 @@ rten_status rten_b200_scatter_rows(rten_ctx* ctx, rten_tensor* table, const rten
     if (table->device < 0) return fail(ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, "the table must be device resident (updated in place)");
     OpScope sc(ctx);
     rten_tensor iv, ic, sv;
-    rten_status st = sc.in(idx, &iv);
-    if (st == RTEN_OK) st = sc.contiguous(&iv, &ic);
-    if (st == RTEN_OK) st = sc.in(src, &sv);
-    if (st == RTEN_OK)
-        st = launch_scatter_rows(ctx, (float*)table->data, (const int*)ic.data, (const float*)sv.data, iv.shape[0],
-                                 (int)table->shape[1], table->strides[0], table->strides[1], sv.strides[0], sv.strides[1],
-                                 table->shape[0]);
-    return sc.finish(st);
+    RTB_TRY(sc.in(idx, &iv));
+    RTB_TRY(sc.contiguous(&iv, &ic));
+    RTB_TRY(sc.in(src, &sv));
+    return sc.finish(launch_scatter_rows(ctx, (float*)table->data, (const int*)ic.data, (const float*)sv.data, iv.shape[0],
+                                         (int)table->shape[1], table->strides[0], table->strides[1], sv.strides[0], sv.strides[1],
+                                         table->shape[0]));
 }
 
 }  // extern "C"

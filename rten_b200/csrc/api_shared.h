@@ -26,8 +26,6 @@ struct Mat {
 
 rten_status to_kmajor(rten_ctx* ctx, int esize, const Mat& m, OperandDesc* od);
 
-inline rten_status check_ctx(rten_ctx* ctx) { return ctx ? RTEN_OK : RTEN_ERR_INVALID_VALUE; }
-
 inline rten_status check_zero_point(rten_ctx* ctx, const rten_tensor* zp, int64_t expected, int want_dtype) {
     if (!zp) return RTEN_OK;
     if (zp->dtype != want_dtype) return fail(ctx, RTEN_ERR_CAST_FAILED, "zero point type does not match its tensor");

@@ -1,9 +1,11 @@
 // Per-call scope used by every operator entry point: stages host tensors through HBM, allocates /
 // validates outputs, and at the end copies host outputs back and releases temporaries.
 #pragma once
+#include <memory>
 #include <vector>
 
 #include "common.h"
+#include "rowops.h"
 
 struct rten_packed {
     int kind = 0;   // 0: MatMul B, 1: Conv weight
@@ -24,9 +26,21 @@ struct rten_packed {
 
 namespace rtb {
 
+// a pack under construction, freed unless released to the caller
+struct PackedFree {
+    rten_ctx* ctx;
+    void operator()(rten_packed* p) const { rten_b200_packed_free(ctx, p); }
+};
+using PackedPtr = std::unique_ptr<rten_packed, PackedFree>;
+
+// An entry point opens one scope after its argument checks and returns success only through `return sc.finish(...)`.
+// Any other return from inside the scope is a failure: the destructor then frees the outputs the call allocated (their
+// `data` back to NULL), releases the temporaries and synchronises when a host tensor was staged.  Scopes do not nest
+// (the temporaries live on the context): an entry point calls another only after its own scope has closed.
 struct OpScope {
     rten_ctx* ctx;
     bool host_involved = false;
+    bool finished = false;
     struct Copyback {
         void* host;
         void* dev;
@@ -36,6 +50,12 @@ struct OpScope {
     std::vector<rten_tensor*> allocated;
 
     explicit OpScope(rten_ctx* c) : ctx(c) { cudaSetDevice(c->device); }
+    OpScope(const OpScope&) = delete;
+    OpScope& operator=(const OpScope&) = delete;
+    // (any failing status takes finish's failure path, which leaves the context's error message as it is)
+    ~OpScope() {
+        if (!finished) finish(RTEN_ERR_CUDA);
+    }
 
     // device view of an input (H2D copy of the spanned region for host tensors)
     rten_status in(const rten_tensor* t, rten_tensor* view);
@@ -44,20 +64,33 @@ struct OpScope {
                     const int64_t* preferred_strides);
     // contiguous device copy (no-op when already contiguous)
     rten_status contiguous(const rten_tensor* v, rten_tensor* c);
+    // success: host outputs copied back; failure: allocated outputs freed.  Either way the temporaries are released.
     rten_status finish(rten_status st);
 };
 
-// a tensor with no data, shape or strides, for an entry point to allocate
-inline rten_tensor empty_tensor() {
-    rten_tensor t;
-    memset(&t, 0, sizeof(t));
-    return t;
+// copies the device view `src` into the device view `dst` of the same shape
+inline rten_status copy_view(rten_ctx* ctx, const rten_tensor& src, const rten_tensor& dst) {
+    long long shape[RTEN_MAX_DIMS], ss[RTEN_MAX_DIMS], ds[RTEN_MAX_DIMS];
+    for (int i = 0; i < src.ndim; i++) {
+        shape[i] = src.shape[i];
+        ss[i] = src.strides[i];
+        ds[i] = dst.strides[i];
+    }
+    return launch_nd_copy(ctx, dtype_size(src.dtype), src.data, dst.data, src.ndim, shape, ss, ds);
 }
 
-// releases a temporary an entry point allocated
-inline void free_if(rten_ctx* ctx, rten_tensor& t) {
-    if (t.data) rten_b200_free(ctx, t.data);
-    t.data = nullptr;
-}
+inline rten_status check_ctx(rten_ctx* ctx) { return ctx ? RTEN_OK : RTEN_ERR_INVALID_VALUE; }
+
+// An intermediate of a composed operator: starts with no data, shape or strides for an entry point to allocate, and goes
+// back to the pool when it goes out of scope.
+struct Intermediate : rten_tensor {
+    rten_ctx* ctx;
+    explicit Intermediate(rten_ctx* c) : rten_tensor(), ctx(c) {}
+    Intermediate(const Intermediate&) = delete;
+    Intermediate& operator=(const Intermediate&) = delete;
+    ~Intermediate() {
+        if (data) rten_b200_free(ctx, data);
+    }
+};
 
 }  // namespace rtb
