@@ -4,7 +4,8 @@
 //   warps 0-3 (one warpgroup), wgmma tf32:  S = Q K^T in two 64-column halves -> accumulator tile in shared memory
 //   the same warps, one query row per thread: S row, scale, + mask, the reference's softmax (rten-vecmath/src/softmax.rs:
 //       60-101,176-228: ReducedRangeExp, 16 lane partial sums in index order) -> P written as the A operand (128B-swizzled
-//       K-major tiles) in shared memory
+//       K-major tiles) in shared memory, NaNs flushed to zero as in the reference (src/ops/attention.rs:549-551): a row
+//       whose mask is -inf at every key, or +inf / NaN at one, gives zeros
 //   wgmma tf32:  O = P V -> accumulator tile -> rows staged in shared memory -> global
 // Replaces, for these shapes, FusedMatMul(QK^T) + AddSoftmax + MatMul(PV) (src/ops/attention.rs:30-165, :518-560): three
 // launches and two round trips of the [batch, heads, 128, 128] score tensor through HBM per layer.
@@ -177,6 +178,15 @@ attn_fused_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_consta
             unpack2(part[l], a, b2);
             s = __fadd_rn(s, a);
             s = __fadd_rn(s, b2);
+        }
+        // AddSoftmax in attention flushes NaNs in P to zero (flush_nans_to_zero).  Here that is a whole-row matter: s is
+        // NaN (a NaN or +inf score) or 0 (every key at -inf) exactly when every element of P = e * (1 / s) is NaN; any
+        // other s is >= 1 (the maximum's own exponential) and leaves no NaN.  Such a row stores zeros instead: the same
+        // bits as a select on each element, without one in the rows that need none
+        if (!(s > 0.0f)) {
+#pragma unroll
+            for (int i = 0; i < SK; i++) z[i] = 0.0f;
+            s = 1.0f;
         }
         const f32x2 inv = splat2(__fdiv_rn(1.0f, s));
         // P as the A operand: tile c holds keys [32 c, 32 c + 32); row r = 128 bytes, 16-byte chunks XOR-swizzled by r & 7
