@@ -535,6 +535,28 @@ rten_status rten_b200_rms_norm(rten_ctx* ctx, const rten_tensor* x, const rten_t
 rten_status rten_b200_skip_layer_norm(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* skip, const rten_tensor* gamma,
                                       const rten_tensor* beta_or_null, const rten_tensor* bias_or_null, float epsilon, int rms,
                                       rten_tensor* out, rten_tensor* sum_out_or_null);
+/* InstanceNormalization (src/ops/norm.rs instance_normalization): each (n, c) lane of x [N, C, ...] normalised over its
+ * L elements, mean = Sum / L and var = SumSquareSub(mean) / L in the reference's fold order, then
+ * y = fma(x - mean, scale[c] / sqrt(var + epsilon), bias[c]).  scale and bias are 1-D [C]; epsilon < 0 => default 1e-5.
+ * The reference's statuses and messages: "expected input with >= 2 dims", "scale length should match channel count",
+ * "bias length should match channel count".  NCHW-contiguous and dense channels-last 4-D x are read as they are and the
+ * output keeps x's layout; x in any other strides is copied to contiguous first.  `out` may alias `x` (run_in_place).
+ * Bit-identical to the reference.  One kernel launch for rows up to 51200 elements, else two (three for channels-last). */
+rten_status rten_b200_instance_norm(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* scale, const rten_tensor* bias,
+                                    float epsilon, rten_tensor* out);
+/* GroupNorm as torch exports it, in one normalization pass: exactly the result of
+ *   Reshape(x, [N, groups, -1]) -> InstanceNormalization(inst_scale, inst_bias, epsilon) -> Reshape to x's shape
+ *   -> Mul(gamma [C, 1, ..]) -> Add(beta [C, 1, ..]) -> activation
+ * each step rounded on its own: the InstanceNormalization value of row (n, g) -- the channels g C/groups ..
+ * (g + 1) C/groups - 1 of image n in (c, spatial) order -- then y * gamma[c] (when gamma), + beta[c] (when beta), then
+ * the activation (NULL or RTEN_ACT_NONE: none), computed as the standalone operator computes it.  inst_scale and
+ * inst_bias are 1-D [groups]; gamma and beta have C elements, one per channel.  C % groups != 0 returns
+ * RTEN_ERR_INVALID_VALUE "Input length must be a multiple of specified dimensions", as the Reshape does; gamma or beta
+ * with another length returns RTEN_ERR_INCOMPATIBLE_SHAPES "Cannot broadcast inputs"; otherwise the errors of
+ * rten_b200_instance_norm against [N, groups, L].  Layouts, aliasing and launches as rten_b200_instance_norm. */
+rten_status rten_b200_group_norm(rten_ctx* ctx, const rten_tensor* x, int groups, const rten_tensor* inst_scale,
+                                 const rten_tensor* inst_bias, const rten_tensor* gamma_or_null, const rten_tensor* beta_or_null,
+                                 float epsilon, const rten_activation* act_or_null, rten_tensor* out);
 /* Clip (src/ops/unary_elementwise.rs:249-333), f32 or i32: x.max(min).min(max) with `a > b ? a : b` comparisons, so
  * NaN becomes min and -0.0 clipped at min = 0 becomes +0.0.  min / max are scalar tensors of x's type (NULL: the type's
  * finite minimum / maximum), read on the device: no host synchronisation, capturable in a CUDA graph.  `out` may alias

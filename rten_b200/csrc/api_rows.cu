@@ -12,6 +12,7 @@
 #include "api_shared.h"
 #include "comm_device.cuh"
 #include "api_util.h"
+#include "groupnorm.h"
 #include "rowops.h"
 #include "skinny.h"
 #include "umma_gemm.h"
@@ -299,6 +300,105 @@ rten_status rten_b200_skip_layer_norm(rten_ctx* ctx, const rten_tensor* x, const
     p.n = (int)H;
     p.rows = numel(&xv) / H;
     return sc.finish(launch_norm(ctx, p));
+}
+
+// ---- InstanceNormalization and the GroupNorm chain ------------------------------------------------------
+// The kernels' view of x: 0 for [N, C, P] contiguous, 1 for a dense channels-last 4-D tensor, -1 for anything else
+static int gn_layout(const rten_tensor& t) {
+    if (is_contiguous(&t)) return 0;
+    if (t.ndim != 4) return -1;
+    const int64_t C = t.shape[1], H = t.shape[2], W = t.shape[3];
+    return t.strides[1] == 1 && t.strides[3] == C && (t.strides[2] == W * C || H == 1) && (t.strides[0] == H * W * C || t.shape[0] == 1)
+               ? 1 : -1;
+}
+
+// One [n] vector of an operator as a contiguous device array (checked by the caller)
+static rten_status gn_vector(OpScope& sc, const rten_tensor* t, const float** ptr) {
+    rten_tensor v, c;
+    RTB_TRY(sc.in(t, &v));
+    RTB_TRY(sc.contiguous(&v, &c));
+    *ptr = (const float*)c.data;
+    return RTEN_OK;
+}
+
+// Rows of `groups` per image, checked by the entry points
+static rten_status group_norm_run(rten_ctx* ctx, const rten_tensor* x, int groups, const rten_tensor* inst_scale,
+                                  const rten_tensor* inst_bias, const rten_tensor* gamma, const rten_tensor* beta, float epsilon,
+                                  const rten_activation* act, rten_tensor* out) {
+    OpScope sc(ctx);
+    rten_tensor xv, xc, ov;
+    GroupNormParams p;
+    RTB_TRY(sc.in(x, &xv));
+    int layout = gn_layout(xv);
+    if (layout < 0) {  // any other strides: a contiguous copy, and the [N, C, P] path
+        RTB_TRY(sc.contiguous(&xv, &xc));
+        layout = 0;
+    } else {
+        xc = xv;
+    }
+    RTB_TRY(sc.out(out, RTEN_F32, xv.ndim, xv.shape, &ov, (out->data == nullptr && layout == 1) ? xc.strides : nullptr));
+    if (numel(&xv) == 0) return sc.finish(RTEN_OK);
+    RTB_TRY(gn_vector(sc, inst_scale, &p.inst_scale));
+    RTB_TRY(gn_vector(sc, inst_bias, &p.inst_bias));
+    if (gamma) RTB_TRY(gn_vector(sc, gamma, &p.gamma));
+    if (beta) RTB_TRY(gn_vector(sc, beta, &p.beta));
+    // the output in the layout the kernels write: `out` itself when it has it, else a temporary copied into `out`
+    bool direct = gn_layout(ov) == layout;
+    for (int i = 0; i < ov.ndim && direct; i++)
+        if (ov.shape[i] != 1 && ov.strides[i] != xc.strides[i]) direct = false;
+    rten_tensor yc = xc;
+    if (direct) yc.data = ov.data;
+    else RTB_TRY(temp_alloc(ctx, (size_t)numel(&xv) * 4, &yc.data));
+    p.x = (const float*)xc.data;
+    p.y = (float*)yc.data;
+    p.N = xv.shape[0];
+    p.C = (int)xv.shape[1];
+    p.G = groups;
+    p.P = numel(&xv) / (p.N * p.C);
+    p.channels_last = layout;
+    p.eps = epsilon < 0.0f ? 1e-5f : epsilon;
+    if (act) {
+        p.act = act->kind;
+        p.act_alpha = act->alpha;
+        p.act_beta = act->beta;
+    }
+    RTB_TRY(launch_group_norm(ctx, p));
+    return sc.finish(direct ? RTEN_OK : copy_view(ctx, yc, ov));
+}
+
+rten_status rten_b200_instance_norm(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* scale, const rten_tensor* bias,
+                                    float epsilon, rten_tensor* out) {
+    RTB_TRY(check_ctx(ctx));
+    if (!x || !scale || !bias || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    for (const rten_tensor* t : {x, scale, bias})
+        if (t->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    if (scale->ndim != 1 || bias->ndim != 1) return fail(ctx, RTEN_ERR_CAST_FAILED, "scale and bias must be 1-D tensors");
+    // src/ops/norm.rs instance_normalization_in_place
+    if (x->ndim < 2) return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected input with >= 2 dims");
+    if (scale->shape[0] != x->shape[1]) return fail(ctx, RTEN_ERR_INVALID_VALUE, "scale length should match channel count");
+    if (bias->shape[0] != x->shape[1]) return fail(ctx, RTEN_ERR_INVALID_VALUE, "bias length should match channel count");
+    if (x->shape[1] > INT32_MAX) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "channel count out of range");
+    return group_norm_run(ctx, x, (int)x->shape[1], scale, bias, nullptr, nullptr, epsilon, nullptr, out);
+}
+
+rten_status rten_b200_group_norm(rten_ctx* ctx, const rten_tensor* x, int groups, const rten_tensor* inst_scale,
+                                 const rten_tensor* inst_bias, const rten_tensor* gamma, const rten_tensor* beta, float epsilon,
+                                 const rten_activation* act, rten_tensor* out) {
+    RTB_TRY(check_ctx(ctx));
+    if (!x || !inst_scale || !inst_bias || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    for (const rten_tensor* t : {x, inst_scale, inst_bias, gamma, beta})
+        if (t && t->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    if (inst_scale->ndim != 1 || inst_bias->ndim != 1) return fail(ctx, RTEN_ERR_CAST_FAILED, "scale and bias must be 1-D tensors");
+    if (x->ndim < 2) return fail(ctx, RTEN_ERR_INVALID_VALUE, "expected input with >= 2 dims");
+    if (groups <= 0 || x->shape[1] % groups != 0 || x->shape[1] > INT32_MAX)  // Reshape [N, G, -1]
+        return fail(ctx, RTEN_ERR_INVALID_VALUE, "Input length must be a multiple of specified dimensions");
+    if (inst_scale->shape[0] != groups) return fail(ctx, RTEN_ERR_INVALID_VALUE, "scale length should match channel count");
+    if (inst_bias->shape[0] != groups) return fail(ctx, RTEN_ERR_INVALID_VALUE, "bias length should match channel count");
+    for (const rten_tensor* t : {gamma, beta})  // Mul / Add of a per-channel [C, 1, ..] constant
+        if (t && numel(t) != x->shape[1]) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Cannot broadcast inputs");
+    if (act && (act->kind < RTEN_ACT_NONE || act->kind > RTEN_ACT_HARD_SWISH))
+        return fail(ctx, RTEN_ERR_INVALID_VALUE, "unknown activation kind");
+    return group_norm_run(ctx, x, groups, inst_scale, inst_bias, gamma, beta, epsilon, act, out);
 }
 
 // ---- unary elementwise ----------------------------------------------------------------------------

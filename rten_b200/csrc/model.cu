@@ -696,6 +696,54 @@ rten_status run_skip_norm(Runner& r, OpNode& o, rten_tensor* y) {
     return RTEN_OK;
 }
 
+// The shape a Reshape node with the constant target `target` gives `y`
+rten_status reshape_target(Runner& r, int target, bool allowzero, const rten_tensor& y, std::vector<int64_t>* shape) {
+    std::vector<int64_t> want;
+    RTB_TRY(r.ints_of(target, &want));
+    shape->clear();
+    const int64_t total = numel(&y);
+    int64_t known = 1;
+    int infer = -1;
+    for (size_t i = 0; i < want.size(); i++) {
+        int64_t d = want[i];
+        if (d == 0 && !allowzero) d = (int)i < y.ndim ? y.shape[i] : 0;
+        if (d == -1) {
+            if (infer >= 0) return mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "Multiple dimensions in new shape set to -1");
+            infer = (int)i;
+            d = 1;
+        }
+        shape->push_back(d);
+        known *= d;
+    }
+    if (infer >= 0) {
+        if (known == 0 || total % known) return mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "Input length must be a multiple of specified dimensions");
+        (*shape)[(size_t)infer] = total / known;
+    }
+    return RTEN_OK;
+}
+
+// The GroupNorm chain the load fused (inputs x, inst_scale, inst_bias, gamma, beta, the two Reshape targets; the
+// InstanceNormalization node's attributes).  The Reshapes' shapes are checked as they would resolve for this x, so an
+// input the pattern does not fit fails with the message the node chain gives.
+rten_status run_group_norm(Runner& r, OpNode& o, rten_tensor* y) {
+    const rten_tensor* x = r.T(o, 0);
+    const rten_tensor *gamma = r.T(o, 3), *beta = r.T(o, 4);
+    const int64_t G = r.T(o, 1)->shape[0];
+    std::vector<int64_t> s1, s2;
+    rten_tensor v = *x;
+    RTB_TRY(reshape_target(r, o.in[5], false, v, &s1));
+    if ((int)s1.size() > RTEN_MAX_DIMS) return mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "tensor rank out of range");
+    v.ndim = (int)s1.size();
+    for (int i = 0; i < v.ndim; i++) v.shape[i] = s1[(size_t)i];
+    RTB_TRY(reshape_target(r, o.in[6], false, v, &s2));
+    const bool grouped = x->ndim == 4 && s1.size() == 3 && s1[0] == x->shape[0] && s1[1] == G;
+    if (!grouped || s2 != std::vector<int64_t>(x->shape, x->shape + 4))
+        return mfail(r.ctx, RTEN_ERR_UNSUPPORTED_VALUE, "GroupNorm: the input does not fit the fused Reshape pattern");
+    if (x->shape[1] != numel(gamma) || x->shape[1] != numel(beta))
+        return mfail(r.ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Cannot broadcast inputs");
+    return rten_b200_group_norm(r.ctx, x, (int)G, r.T(o, 1), r.T(o, 2), gamma, beta, o.n.attr_f("epsilon", 1e-5f), &o.activation, y);
+}
+
 constexpr OpDef OPS[] = {
     {"Conv", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
          rten_conv_params p;
@@ -806,26 +854,8 @@ constexpr OpDef OPS[] = {
          return RTEN_OK;
      }},
     {"Reshape", ONNX, VIEW | RESHAPE, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
-         std::vector<int64_t> want, shape;
-         RTB_TRY(r.ints_of(o.in.size() > 1 ? o.in[1] : -1, &want));
-         const int64_t total = numel(y);
-         int64_t known = 1;
-         int infer = -1;
-         for (size_t i = 0; i < want.size(); i++) {
-             int64_t d = want[i];
-             if (d == 0 && !o.n.attr_i("allowzero", 0)) d = (int)i < y->ndim ? y->shape[i] : 0;
-             if (d == -1) {
-                 if (infer >= 0) return mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "Multiple dimensions in new shape set to -1");
-                 infer = (int)i;
-                 d = 1;
-             }
-             shape.push_back(d);
-             known *= d;
-         }
-         if (infer >= 0) {
-             if (known == 0 || total % known) return mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "Input length must be a multiple of specified dimensions");
-             shape[(size_t)infer] = total / known;
-         }
+         std::vector<int64_t> shape;
+         RTB_TRY(reshape_target(r, o.in.size() > 1 ? o.in[1] : -1, o.n.attr_i("allowzero", 0) != 0, *y, &shape));
          return r.reshape(y, shape);
      }},
     {"Flatten", ONNX, VIEW | RESHAPE, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
@@ -899,6 +929,9 @@ constexpr OpDef OPS[] = {
          return rten_b200_layer_norm(r.ctx, r.T(o, 0), r.T(o, 1), r.T(o, 2), (int)o.n.attr_i("axis", -1), o.n.attr_f("epsilon", 1e-5f), y); }},
     {"RMSNormalization", ONNX, 0, 0b11, run_rms_norm, check_rms_norm},
     {"SimplifiedLayerNormalization", ONNX, 0, 0b11, run_rms_norm, check_rms_norm},
+    {"InstanceNormalization", ONNX, IN_PLACE, 0b111, [](Runner& r, OpNode& o, rten_tensor* y) {
+         return rten_b200_instance_norm(r.ctx, r.T(o, 0), r.T(o, 1), r.T(o, 2), o.n.attr_f("epsilon", 1e-5f), y); }},
+    {"GroupNorm", 0, IN_PLACE, 0b1111111, run_group_norm},  // (GroupNormFusion)
     {"SkipLayerNormalization", MS, 0, 0b1, run_skip_norm<false>, check_skip_norm},
     {"SkipSimplifiedLayerNormalization", MS, 0, 0b1, run_skip_norm<true>, check_skip_norm},
     {"Gather", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
@@ -1028,8 +1061,10 @@ constexpr const OpDef* row(std::string_view name) {
 
 // the operators the load-time passes look for
 constexpr const OpDef *CONV = row("Conv"), *CONV_TRANSPOSE = row("ConvTranspose"), *CONCAT = row("Concat"), *SIGMOID = row("Sigmoid"),
-                      *MUL = row("Mul"), *SILU = row("Silu"), *MATMUL = row("MatMul"), *ADD = row("Add");
-static_assert(CONV && CONV_TRANSPOSE && CONCAT && SIGMOID && MUL && SILU && MATMUL && ADD, "a row the load looks for is missing");
+                      *MUL = row("Mul"), *SILU = row("Silu"), *MATMUL = row("MatMul"), *ADD = row("Add"), *RESHAPE_OP = row("Reshape"),
+                      *INSTANCE_NORM = row("InstanceNormalization"), *GROUP_NORM = row("GroupNorm");
+static_assert(CONV && CONV_TRANSPOSE && CONCAT && SIGMOID && MUL && SILU && MATMUL && ADD && RESHAPE_OP && INSTANCE_NORM && GROUP_NORM,
+              "a row the load looks for is missing");
 
 }  // namespace
 
@@ -1160,6 +1195,93 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
         mul.n.attrs.clear();
         mul.in = {x};
         m->nodes.erase(m->nodes.begin() + (long)i);
+    }
+    // the node that reads value `vid` first after node i, when that is its only consumer, else -1
+    auto sole_consumer = [&](size_t i, int vid) -> long {
+        if (vid < 0 || consumers(vid) != 1) return -1;
+        for (size_t j = i + 1; j < m->nodes.size(); j++)
+            if (std::find(m->nodes[j].in.begin(), m->nodes[j].in.end(), vid) != m->nodes[j].in.end()) return (long)j;
+        return -1;
+    };
+    // GroupNormFusion: torch's export of nn.GroupNorm(G, C) -- Reshape(x, [0 | N, G, -1]) -> InstanceNormalization(
+    // scale [G], bias [G]) -> Reshape(to a constant 4-D shape) -> Mul(gamma [C, 1, 1]) -> Add(beta [C, 1, 1]), every
+    // intermediate with one consumer -- and a following Relu / Sigmoid / Silu / HardSigmoid / HardSwish become one
+    // GroupNorm node: one pass over x instead of two copies, the norm and three elementwise launches.  After SiluFusion,
+    // which makes the activation's Silu node.  The Reshape targets stay inputs, resolved for each run's x.
+    // RTEN_B200_NO_GROUP_NORM_FUSION=1 (read at load) keeps the node chain.  Only constant targets match: a target
+    // computed from Shape(x) is not fused.
+    if (!getenv("RTEN_B200_NO_GROUP_NORM_FUSION")) {
+        auto cval = [&](int vid) -> const ValueSlot* {
+            return vid >= 0 && m->values[(size_t)vid].kind == V_CONST ? &m->values[(size_t)vid] : nullptr;
+        };
+        // a per-channel constant of C elements: [C], broadcast over the spatial axes, i.e. shape [.., C, 1, 1]
+        auto per_channel = [&](int vid, int64_t* C) {
+            const ValueSlot* v = cval(vid);
+            if (!v || v->t.dtype != RTEN_F32 || v->t.ndim < 3 || v->t.ndim > 4) return false;
+            const int nd = v->t.ndim;
+            if (v->t.shape[nd - 1] != 1 || v->t.shape[nd - 2] != 1 || (nd == 4 && v->t.shape[0] != 1)) return false;
+            *C = v->t.shape[nd - 3];
+            return true;
+        };
+        for (size_t i = 0; i < m->nodes.size(); i++) {
+            const OpNode& r1 = m->nodes[i];
+            if (r1.def != RESHAPE_OP || r1.in.size() != 2 || r1.out.size() != 1 || r1.n.attr_i("allowzero", 0)) continue;
+            const ValueSlot* t1 = cval(r1.in[1]);
+            if (!t1 || !t1->has_host_ints || t1->host_ints.size() != 3 || t1->host_ints[0] < 0 || t1->host_ints[1] <= 0 ||
+                t1->host_ints[2] != -1)
+                continue;
+            const int64_t G = t1->host_ints[1];
+            const long j_in = sole_consumer(i, r1.out[0]);
+            if (j_in < 0) continue;
+            const OpNode& in = m->nodes[(size_t)j_in];
+            if (in.def != INSTANCE_NORM || in.in.size() != 3 || in.in[0] != r1.out[0] || in.out.size() != 1) continue;
+            const ValueSlot *sc = cval(in.in[1]), *bi = cval(in.in[2]);
+            if (!sc || !bi || sc->t.ndim != 1 || bi->t.ndim != 1 || sc->t.shape[0] != G || bi->t.shape[0] != G) continue;
+            const long j_r2 = sole_consumer((size_t)j_in, in.out[0]);
+            if (j_r2 < 0) continue;
+            const OpNode& r2 = m->nodes[(size_t)j_r2];
+            if (r2.def != RESHAPE_OP || r2.in.size() != 2 || r2.in[0] != in.out[0] || r2.out.size() != 1 || r2.n.attr_i("allowzero", 0))
+                continue;
+            const ValueSlot* t2 = cval(r2.in[1]);
+            if (!t2 || !t2->has_host_ints || t2->host_ints.size() != 4) continue;
+            const long j_mul = sole_consumer((size_t)j_r2, r2.out[0]);
+            if (j_mul < 0) continue;
+            const OpNode& mul = m->nodes[(size_t)j_mul];
+            if (mul.def != MUL || mul.in.size() != 2 || mul.out.size() != 1) continue;
+            const int gamma = mul.in[0] == r2.out[0] ? mul.in[1] : mul.in[0];
+            int64_t C = 0, Cb = 0;
+            if (gamma == r2.out[0] || !per_channel(gamma, &C) || C % G != 0) continue;
+            const long j_add = sole_consumer((size_t)j_mul, mul.out[0]);
+            if (j_add < 0) continue;
+            const OpNode& add = m->nodes[(size_t)j_add];
+            if (add.def != ADD || add.in.size() != 2 || add.out.size() != 1) continue;
+            const int beta = add.in[0] == mul.out[0] ? add.in[1] : add.in[0];
+            if (beta == mul.out[0] || !per_channel(beta, &Cb) || Cb != C) continue;
+            long last = j_add;
+            rten_activation act = {RTEN_ACT_NONE, 0.0f, 0.0f};
+            const long j_act = sole_consumer((size_t)j_add, add.out[0]);
+            if (j_act >= 0) {
+                const OpNode& a = m->nodes[(size_t)j_act];
+                if (a.def->act != RTEN_ACT_NONE && a.in.size() == 1 && a.out.size() == 1) {
+                    const bool hs = a.def->act == RTEN_ACT_HARD_SIGMOID;
+                    act = {(int32_t)a.def->act, hs ? hard_sigmoid_alpha(a.n) : 0.0f, hs ? hard_sigmoid_beta(a.n) : 0.0f};
+                    last = j_act;
+                }
+            }
+            OpNode gn;
+            gn.n = in.n;
+            gn.n.op_type = GROUP_NORM->name;
+            gn.def = GROUP_NORM;
+            gn.in = {r1.in[0], in.in[1], in.in[2], gamma, beta, r1.in[1], r2.in[1]};
+            gn.out = m->nodes[(size_t)last].out;
+            gn.activation = act;
+            // the fused node takes the last node's place (every input exists by then); the others go
+            const long chain[] = {(long)i, j_in, j_r2, j_mul, j_add, j_act >= 0 && last == j_act ? j_act : -1};
+            m->nodes[(size_t)last] = gn;
+            for (long k = (long)m->nodes.size() - 1; k >= 0; k--)
+                if (k != last && std::find(std::begin(chain), std::end(chain), k) != std::end(chain)) m->nodes.erase(m->nodes.begin() + k);
+            i = (size_t)-1;  // (indices moved: look again from the start; every match removes nodes, so this ends)
+        }
     }
     for (size_t i = 0; i + 1 < m->nodes.size(); i++) {
         OpNode& a = m->nodes[i];

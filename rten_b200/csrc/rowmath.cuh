@@ -144,4 +144,54 @@ __device__ __forceinline__ float ln_smem_fold(const float4* s4, int F, float off
     return __shfl_sync(0xffffffffu, s, 3);
 }
 
+// ln_smem_fold for any n, in two steps so that the 64 chains can run over a row that arrives chunk by chunk
+// (groupnorm.cu).  smem_fold_chunks adds F full 64-element chunks (F * 16 float4s at s4) to the running chains `acc`
+// (lane c = lane & 15 owns chains 4c .. 4c + 3); smem_fold_finish then combines the chains and folds the rem < 64
+// elements after the last full chunk -- its full 16-element chunks, then the masked tail -- into acc[0], and sums the
+// 16 lanes in order (simd_fold_unroll4 in rowops.cu, over shared memory).  A whole warp calls both; every lane returns
+// the total.  (ln_smem_fold is the rem = 0 case; it stays as it is so that the kernels using it keep their code.)
+template <bool SQSUB>
+__device__ __forceinline__ void smem_fold_chunks(float4& acc, const float4* s4, int F, float off) {
+    const int c = threadIdx.x & 15;
+#pragma unroll 4
+    for (int k = 0; k < F; k++) {
+        const float4 v = s4[c + 16 * k];
+        acc.x = fold_step<SQSUB>(acc.x, v.x, off);
+        acc.y = fold_step<SQSUB>(acc.y, v.y, off);
+        acc.z = fold_step<SQSUB>(acc.z, v.z, off);
+        acc.w = fold_step<SQSUB>(acc.w, v.w, off);
+    }
+}
+
+template <bool SQSUB>
+__device__ __forceinline__ float smem_fold_finish(float4 acc, const float* t, int rem, float off) {
+    const int c = threadIdx.x & 15;
+    float4 r = acc;  // acc[0][l] = ((acc[0][l] + acc[1][l]) + acc[2][l]) + acc[3][l]: thread c < 4 holds l = 4c .. 4c + 3
+#pragma unroll
+    for (int u = 1; u < 4; u++) {
+        r.x = __fadd_rn(r.x, __shfl_down_sync(0xffffffffu, acc.x, 4 * u));
+        r.y = __fadd_rn(r.y, __shfl_down_sync(0xffffffffu, acc.y, 4 * u));
+        r.z = __fadd_rn(r.z, __shfl_down_sync(0xffffffffu, acc.z, 4 * u));
+        r.w = __fadd_rn(r.w, __shfl_down_sync(0xffffffffu, acc.w, 4 * u));
+    }
+    if (c < 4) {
+        for (int i = 4 * c; i < rem; i += 16) {  // element i of the remainder goes to lane l = i % 16
+            r.x = fold_step<SQSUB>(r.x, t[i], off);
+            if (i + 1 < rem) r.y = fold_step<SQSUB>(r.y, t[i + 1], off);
+            if (i + 2 < rem) r.z = fold_step<SQSUB>(r.z, t[i + 2], off);
+            if (i + 3 < rem) r.w = fold_step<SQSUB>(r.w, t[i + 3], off);
+        }
+    }
+    float s = 0.0f;
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+        const float in = __shfl_up_sync(0xffffffffu, s, 1);
+        if (c == q) {
+            if (q > 0) s = in;
+            s = __fadd_rn(__fadd_rn(__fadd_rn(__fadd_rn(s, r.x), r.y), r.z), r.w);
+        }
+    }
+    return __shfl_sync(0xffffffffu, s, 3);
+}
+
 }  // namespace rtb

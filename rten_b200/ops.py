@@ -846,6 +846,39 @@ class SkipSimplifiedLayerNormalization(SkipLayerNormalization):
         return self._run(ctx, x, skip, gamma, None, bias, want_sum)
 
 
+class InstanceNormalization:
+    """src/ops/norm.rs instance_normalization: each (n, c) lane normalised over its spatial elements, scale / bias [C].
+    `run(..., out=x)` normalises in place."""
+
+    def __init__(self, epsilon: Optional[float] = None):
+        self.epsilon = epsilon
+
+    def run(self, ctx, x, scale, bias, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        ctx.check(ctx.lib.rten_b200_instance_norm(ctx.handle, A.t(x), A.t(scale), A.t(bias),
+                                                  -1.0 if self.epsilon is None else float(self.epsilon), C.byref(o)))
+        return A.wrap(o, out)
+
+
+class GroupNorm:
+    """torch's exported GroupNorm chain in one pass: Reshape [N, groups, -1] -> InstanceNormalization(inst_scale,
+    inst_bias) -> Reshape back -> Mul(gamma) -> Add(beta) -> activation (an ACT_* code or (kind, alpha, beta)), each step
+    rounded as the node chain rounds it (rten_b200_group_norm)."""
+
+    def __init__(self, groups: int, epsilon: Optional[float] = None, activation=ACT_NONE):
+        self.groups, self.epsilon, self.activation = int(groups), epsilon, activation
+
+    def run(self, ctx, x, inst_scale, inst_bias, gamma=None, beta=None, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        act = _activation(self.activation)
+        ctx.check(ctx.lib.rten_b200_group_norm(ctx.handle, A.t(x), self.groups, A.t(inst_scale), A.t(inst_bias), A.t(gamma),
+                                               A.t(beta), -1.0 if self.epsilon is None else float(self.epsilon), C.byref(act),
+                                               C.byref(o)))
+        return A.wrap(o, out)
+
+
 class _Unary:
     fn = ""
 
