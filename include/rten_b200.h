@@ -611,10 +611,17 @@ rten_status rten_b200_dynamic_quantize_linear_ranged(rten_ctx* ctx, const rten_t
 
 /* ---- residency glue (SURVEY.md 8f-1) so whole models stay in HBM ------------------------------ */
 rten_status rten_b200_relu(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
-/* Add with numpy broadcasting (src/ops/binary_elementwise.rs). */
+/* Add, Sub and Mul (src/ops/binary_elementwise.rs) with numpy broadcasting: f32 (each result rounded once) or i32
+ * (wrapping); a and b of the same type. */
 rten_status rten_b200_add(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
-/* Mul (src/ops/binary_elementwise.rs), f32, numpy broadcasting. */
+rten_status rten_b200_sub(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
 rten_status rten_b200_mul(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
+/* ReduceSum (src/ops/reduce.rs), f32 or i32, one launch.  `axes` (n_axes values in [-ndim, ndim - 1], duplicates
+ * allowed) are the reduced axes; n_axes = 0 reduces every axis.  keep_dims != 0 keeps them as size-1 axes.  Each f32
+ * output is the reference's Sum (the 64-chain fold of rten-vecmath/src/sum.rs) of its elements taken in row-major order
+ * of the reduced axes, bit for bit, whatever the input's strides; i32 sums wrap.  An empty reduction gives 0; a 0-D
+ * input (n_axes = 0) gives its value plus 0. */
+rten_status rten_b200_reduce_sum(rten_ctx* ctx, const rten_tensor* x, const int32_t* axes, int n_axes, int keep_dims, rten_tensor* out);
 /* MaxPool 2-D (src/ops/pooling.rs): kernel {kh,kw}; pads/strides as conv; padding never wins. */
 rten_status rten_b200_max_pool(rten_ctx* ctx, const rten_tensor* x, const int32_t kernel[2], const int32_t pads[4],
                                const int32_t strides[2], rten_tensor* out);
@@ -700,21 +707,29 @@ rten_status rten_b200_scatter_rows(rten_ctx* ctx, rten_tensor* table, const rten
  * HardSwish, MaxPool, AveragePool (ceil_mode = 1 fails the load), Resize and Upsample (scales / sizes must be constants;
  * the attribute checks and defaults of the reference's reader: antialias, exclude_outside, extrapolation_value,
  * keep_aspect_ratio_policy and cubic_coeff_a at their defaults, cubic computed as linear), Concat (a missing axis fails
- * the load), GlobalAveragePool, ReduceMean (spatial axes), Gemm, MatMul, MatMulInteger, Add, Mul, Softmax, LayerNormalization,
+ * the load), GlobalAveragePool, ReduceMean (spatial axes), ReduceSum (f32 / i32; axes from the attribute or a host-known
+ * input 1), Gemm, MatMul, MatMulInteger, Add, Sub and Mul (f32, or i32 wrapping), Softmax, LayerNormalization,
  * RMSNormalization and SimplifiedLayerNormalization (stash_type 1), SkipLayerNormalization and
  * SkipSimplifiedLayerNormalization (com.microsoft; outputs 0 and 3: a missing epsilon or a named mean / inv_std_var output
- * fails the load), Gelu, Erf, Gather (rows), Cast (i32 -> f32),
+ * fails the load), Gelu, Erf, Gather (rows of a 2-D table; or, on the host, a host-known vector with host-known indices),
+ * Cast (i32 -> f32; an integer Cast of a host-known value stays on the host), Shape (start / end; a host value),
  * DynamicQuantizeLinear, Attention (4-D), MatMulNBits (com.microsoft, bits 4; constant B / scales used in place),
  * RotaryEmbedding, GroupQueryAttention (com.microsoft; output and present_key / present_value, inputs 12-15 rejected;
- * the executor allocates new present caches, so each decode step also copies the past: two launches, not one),
+ * a present cache is a new buffer, so a decode step also copies the past -- two launches, not one -- unless the past is
+ * a writable input with capacity, see rten_b200_model_run_ex),
  * MultiHeadAttention (com.microsoft; outputs 0-2; a missing num_heads, an explicit scale <= 0, inputs 8 / 9 and the
- * qk output 3 fail the load; the executor allocates new present caches), GRU / LSTM (outputs 0-2; constant W prepacked at
+ * qk output 3 fail the load; present caches as for GroupQueryAttention), GRU / LSTM (outputs 0-2; constant W prepacked at
  * load; activation_alpha / activation_beta, non-default activations, clip != 0, layout != 0, LSTM input_forget != 0, a
  * missing hidden_size and a non-empty peephole input fail the load), Constant and the view operators.  MatMulNBits,
  * GroupQueryAttention, MultiHeadAttention and the two Skip norms are com.microsoft operators, Gelu is both, every other
  * one is of the default domain ("" or "ai.onnx"); any other (domain, operator) pair fails the LOAD with
  * RTEN_ERR_UNSUPPORTED_VALUE ("unsupported operator <name>", "com.microsoft.<name>" in that domain), and any other
- * domain with "unsupported operator domain '<domain>'". */
+ * domain with "unsupported operator domain '<domain>'".
+ * Host values: Shape, a Gather of a host-known vector on axis 0 with host-known indices (scalar or vector, negative
+ * indices from the end), an integer Cast and Reshape / Flatten / Squeeze / Unsqueeze / Identity of a host-known value
+ * are computed on the host -- no launch, no device memory -- and may be a Reshape target or an axes input.  An operator
+ * taking one as a tensor gets a host tensor: GroupQueryAttention reads total_sequence_length from it without a copy back
+ * (onnxruntime-genai's attention-mask subgraph), the others stage it. */
 typedef struct rten_model rten_model;
 rten_status rten_b200_model_load(rten_ctx* ctx, const void* onnx_bytes, size_t len, rten_model** out);
 void rten_b200_model_free(rten_model* model);
@@ -730,6 +745,24 @@ const char* rten_b200_model_summary(const rten_model* model); /* JSON: the decod
  * tensor the caller owns (rten_b200_free). */
 rten_status rten_b200_model_run(rten_model* model, int32_t n_inputs, const char* const* input_names, const rten_tensor* inputs,
                                 int32_t n_outputs, const char* const* output_names, rten_tensor* outputs);
+/* rten_b200_model_run with writable inputs (the reference's owned inputs with spare capacity, run_in_place).
+ * opts_or_null[i] describes inputs[i].  A writable input must be device-resident and have the strides of a dense tensor
+ * whose grow_axis has `capacity` positions (grow_axis -1: dense as it is); anything else fails with
+ * RTEN_ERR_INVALID_VALUE.  The caller keeps the buffer: the run never frees it.
+ * GroupQueryAttention (past inputs 3 / 4) and MultiHeadAttention (6 / 7) write their present cache into the past's
+ * buffer -- only the new positions, nothing beyond P + new -- when the past is a writable input with grow_axis 2, the
+ * node is its last consumer, it is not a requested output and the capacity holds P + S (GQA) or P + L (MHA).  Otherwise
+ * the node builds a new present cache as rten_b200_model_run does.  A requested output that is such a present cache
+ * comes back as the view of the input's buffer (not contiguous: the input's strides), and output_alias_or_null[i] is the
+ * index of that input; every other output is handed over as by rten_b200_model_run, with output_alias -1. */
+typedef struct {
+    int32_t writable;  /* the run may write into this input's buffer and return it as an output */
+    int32_t grow_axis; /* the axis `capacity` extends (-1: none) */
+    int64_t capacity;  /* positions along grow_axis the buffer holds (>= shape[grow_axis]) */
+} rten_model_input_opts;
+rten_status rten_b200_model_run_ex(rten_model* model, int32_t n_inputs, const char* const* input_names, const rten_tensor* inputs,
+                                   const rten_model_input_opts* opts_or_null, int32_t n_outputs, const char* const* output_names,
+                                   rten_tensor* outputs, int32_t* output_alias_or_null);
 /* The reader alone -- no context, no GPU: JSON description (opset, nodes with operator / inputs / outputs / attribute
  * names, initialisers with type and shape, graph inputs / outputs) of an ONNX file.  `needed` receives the size of the
  * full text incl. the terminator. */

@@ -32,6 +32,10 @@ class RtenTensor(C.Structure):
     ]
 
 
+class RtenModelInputOpts(C.Structure):
+    _fields_ = [("writable", C.c_int32), ("grow_axis", C.c_int32), ("capacity", C.c_int64)]
+
+
 class RtenConvParams(C.Structure):
     _fields_ = [
         ("pads", C.c_int32 * 4),
@@ -161,6 +165,8 @@ _SIGNATURES = {
     "rten_b200_clip": (C.c_int, [_vp, _TP, _TP, _TP, _TP]),
     "rten_b200_add": (C.c_int, [_vp, _TP, _TP, _TP]),
     "rten_b200_mul": (C.c_int, [_vp, _TP, _TP, _TP]),
+    "rten_b200_sub": (C.c_int, [_vp, _TP, _TP, _TP]),
+    "rten_b200_reduce_sum": (C.c_int, [_vp, _TP, C.POINTER(C.c_int32), C.c_int, C.c_int, _TP]),
     "rten_b200_conv_integer_ex": (C.c_int, [_vp, _TP, _TP, _vp, _TP, _TP, _TP, _TP, C.POINTER(RtenConvParams), _TP, _TP, C.c_int, _TP, _TP]),
     "rten_b200_range_reset": (C.c_int, [_vp, _TP]),
     "rten_b200_dynamic_quantize_linear_ranged": (C.c_int, [_vp, _TP, _TP, _TP, _TP, _TP, _vp]),
@@ -181,6 +187,8 @@ _SIGNATURES = {
     "rten_b200_model_node_op": (C.c_char_p, [_vp, C.c_int32]),
     "rten_b200_model_summary": (C.c_char_p, [_vp]),
     "rten_b200_model_run": (C.c_int, [_vp, C.c_int32, C.POINTER(C.c_char_p), _TP, C.c_int32, C.POINTER(C.c_char_p), _TP]),
+    "rten_b200_model_run_ex": (C.c_int, [_vp, C.c_int32, C.POINTER(C.c_char_p), _TP, C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), _TP,
+                                         C.POINTER(C.c_int32)]),
     "rten_b200_onnx_summary": (C.c_int, [_vp, C.c_size_t, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]),
 }
 

@@ -13,6 +13,7 @@
 #include "comm_device.cuh"
 #include "api_util.h"
 #include "groupnorm.h"
+#include "reduce.h"
 #include "rowops.h"
 #include "skinny.h"
 #include "umma_gemm.h"
@@ -468,12 +469,16 @@ rten_status rten_b200_hard_swish(rten_ctx* ctx, const rten_tensor* x, rten_tenso
     return unary_op(ctx, UNARY_HARD_SWISH, x, out);
 }
 
-// ---- Add ----------------------------------------------------------------------------------------------
-// Add / Mul with numpy broadcasting (src/ops/binary_elementwise.rs); flags: 0 = Add, 2 = Mul
-static rten_status binary_f32(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out, int flags) {
+// ---- Add / Sub / Mul ----------------------------------------------------------------------------------
+// Add / Sub / Mul with numpy broadcasting (src/ops/binary_elementwise.rs), f32 or i32 (wrapping).  f32 Add and Mul run on
+// launch_add_flat / launch_nd_add (flags 0 = Add, 2 = Mul), everything else on launch_binary.
+static rten_status binary_op(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out, int op) {
     RTB_TRY(check_ctx(ctx));
     if (!a || !b || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
-    if (a->dtype != RTEN_F32 || b->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    if ((a->dtype != RTEN_F32 && a->dtype != RTEN_I32) || b->dtype != a->dtype) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    const int dt = a->dtype;
+    const bool add_kernels = dt == RTEN_F32 && op != BIN_SUB;
+    const int flags = op == BIN_MUL ? 2 : 0;
     OpScope sc(ctx);
     rten_tensor av, bv, ov;
     RTB_TRY(sc.in(a, &av));
@@ -493,25 +498,91 @@ static rten_status binary_f32(rten_ctx* ctx, const rten_tensor* a, const rten_te
     bool same = av.ndim == bv.ndim && span_elems(&av) == numel(&av);
     for (int i = 0; i < nd && same; i++)
         if (av.shape[i] != bv.shape[i] || (av.shape[i] != 1 && av.strides[i] != bv.strides[i])) same = false;
-    RTB_TRY(sc.out(out, RTEN_F32, nd, shape, &ov, (out->data == nullptr && same) ? av.strides : nullptr));
+    RTB_TRY(sc.out(out, dt, nd, shape, &ov, (out->data == nullptr && same) ? av.strides : nullptr));
     if (numel(&ov) == 0) return sc.finish(RTEN_OK);
     bool flat = same;
     for (int i = 0; i < nd && flat; i++)
         if (ov.shape[i] != 1 && ov.strides[i] != av.strides[i]) flat = false;
-    if (flat) return sc.finish(launch_add_flat(ctx, (const float*)av.data, (const float*)bv.data, (float*)ov.data, numel(&ov), flags));
+    if (flat && add_kernels)
+        return sc.finish(launch_add_flat(ctx, (const float*)av.data, (const float*)bv.data, (float*)ov.data, numel(&ov), flags));
     long long shp[RTEN_MAX_DIMS], sd[RTEN_MAX_DIMS];
     for (int i = 0; i < nd; i++) {
         shp[i] = shape[i];
         sd[i] = ov.strides[i];
     }
+    if (!add_kernels) {
+        if (flat) {  // dense operands of one layout: one flat pass over the n elements from the lowest address
+            const long long n = numel(&ov), one = 1;
+            return sc.finish(launch_binary(ctx, dt, op, av.data, bv.data, ov.data, 1, &n, &one, &one, &one, true));
+        }
+        return sc.finish(launch_binary(ctx, dt, op, av.data, bv.data, ov.data, nd, shp, sa, sb, sd, false));
+    }
     return sc.finish(launch_nd_add(ctx, (const float*)av.data, (const float*)bv.data, (float*)ov.data, nd, shp, sa, sb, sd, flags));
 }
 
 rten_status rten_b200_add(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out) {
-    return binary_f32(ctx, a, b, out, 0);
+    return binary_op(ctx, a, b, out, BIN_ADD);
+}
+rten_status rten_b200_sub(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out) {
+    return binary_op(ctx, a, b, out, BIN_SUB);
 }
 rten_status rten_b200_mul(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out) {
-    return binary_f32(ctx, a, b, out, 2);
+    return binary_op(ctx, a, b, out, BIN_MUL);
+}
+
+// ---- ReduceSum ----------------------------------------------------------------------------------------
+// src/ops/reduce.rs reduce_sum: the axes resolved (negative from the end), sorted and de-duplicated; none reduces every
+// axis.  A 0-D input is its own one-element lane.
+rten_status rten_b200_reduce_sum(rten_ctx* ctx, const rten_tensor* x, const int32_t* axes, int n_axes, int keep_dims, rten_tensor* out) {
+    RTB_TRY(check_ctx(ctx));
+    if (!x || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    if (x->dtype != RTEN_F32 && x->dtype != RTEN_I32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    if (n_axes < 0 || (n_axes > 0 && !axes)) return fail(ctx, RTEN_ERR_INVALID_VALUE, "axes must be a list of n_axes values");
+    const int nd = x->ndim;
+    bool red[RTEN_MAX_DIMS] = {};
+    for (int i = 0; i < n_axes; i++) {
+        const int64_t a = axes[i] < 0 ? (int64_t)axes[i] + nd : axes[i];
+        if (a < 0 || a >= nd) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Axis is invalid");
+        red[a] = true;
+    }
+    if (n_axes == 0)
+        for (int i = 0; i < nd; i++) red[i] = true;
+    int ond = 0;
+    int64_t oshape[RTEN_MAX_DIMS];
+    for (int i = 0; i < nd; i++)
+        if (!red[i] || keep_dims) oshape[ond++] = red[i] ? 1 : x->shape[i];
+    OpScope sc(ctx);
+    rten_tensor xv, ov;
+    RTB_TRY(sc.in(x, &xv));
+    RTB_TRY(sc.out(out, x->dtype, ond, oshape, &ov, nullptr));
+    ReduceParams p;
+    p.x = xv.data;
+    p.y = ov.data;
+    p.nout = numel(&ov);
+    p.L = 1;
+    // kept dims of size > 1 (with the output stride of each), reduced dims of size != 1, adjacent dense reduced dims merged
+    for (int i = 0, k = 0; i < nd; i++) {
+        const int oi = (!red[i] || keep_dims) ? k++ : -1;
+        if (!red[i]) {
+            if (xv.shape[i] == 1) continue;
+            p.os[p.no] = xv.shape[i], p.ox[p.no] = xv.strides[i], p.oy[p.no] = ov.strides[oi];
+            p.no++;
+        } else {
+            p.L *= xv.shape[i];
+            if (xv.shape[i] == 1) continue;
+            if (p.nr > 0 && p.rx[p.nr - 1] == xv.strides[i] * xv.shape[i]) {
+                p.rs[p.nr - 1] *= xv.shape[i];
+                p.rx[p.nr - 1] = xv.strides[i];
+            } else {
+                p.rs[p.nr] = xv.shape[i], p.rx[p.nr] = xv.strides[i];
+                p.nr++;
+            }
+        }
+    }
+    bool vec = (p.nr == 0 || (p.nr == 1 && p.rx[0] == 1)) && (reinterpret_cast<uintptr_t>(xv.data) & 15) == 0;
+    for (int k = 0; k < p.no && vec; k++) vec = p.ox[k] % 4 == 0;
+    p.vec = vec;
+    return sc.finish(launch_reduce_sum(ctx, x->dtype, p));
 }
 
 // ---- DynamicQuantizeLinear ---------------------------------------------------------------------------

@@ -9,6 +9,10 @@
 //          returned to the context pool after their last consumer (src/graph.rs:1100-1180); an operator that can run in
 //          place does so when the executor holds the last reference to its input (src/graph.rs:973-1049); shape-only
 //          operators (Reshape, Flatten, Squeeze, Unsqueeze, Transpose, Identity) are views -- no kernel, no copy.
+//          Shape-like values are computed on the host (Runner::set_host): Shape, a Gather of a host-known vector with
+//          host-known indices, an integer Cast and the order-keeping views of such values launch nothing, so a Reshape
+//          target or the total_sequence_length of onnxruntime-genai's attention-mask subgraph is known without a copy
+//          back; an operator that takes one as a tensor gets a host tensor (GroupQueryAttention reads it in place).
 //          A Concat over the channels of NCHW tensors is written in place by its producers where the load found that
 //          possible (plan_concat_elision): the first such producer to run allocates the Concat's buffer and every one of
 //          them gets a strided view of its channel slice as `out`, so the Concat node copies only the other inputs --
@@ -42,8 +46,12 @@ struct ValueSlot {
     std::string name;
     ValueKind kind = V_UNSET;
     rten_tensor t{};
-    bool has_host_ints = false;       // shape-like constant (int64 in the file): usable by Reshape / axes inputs
+    // shape-like value known on the host: usable by Reshape / axes inputs.  A constant (int64 in the file), or a run-time
+    // value computed on the host from shapes (Shape, Gather, Cast and the views of such values), whose tensor is then a
+    // host tensor over host_i32 for the rest of the run.
+    bool has_host_ints = false;
     std::vector<int64_t> host_ints;
+    std::vector<int32_t> host_i32;
     bool has_host_floats = false;     // small f32 constant: usable as the scales of Resize / Upsample
     std::vector<float> host_floats;
     // run state
@@ -52,6 +60,13 @@ struct ValueSlot {
     int views = 0;        // live views of this owner
     bool live = false;
     bool owned = false;   // allocation belongs to the executor (pool)
+    // a graph input the caller made writable (rten_b200_model_run_ex): its buffer holds `capacity` positions along
+    // `grow_axis`; input_index is its index in the call's inputs.  On any value: the writable input whose buffer it is a
+    // view of (an in-place present cache), else -1.
+    bool writable = false;
+    int grow_axis = -1;
+    int64_t capacity = 0;
+    int input_index = -1, alias_of = -1;
 };
 
 struct OpNode;
@@ -397,6 +412,7 @@ struct Runner {
     void consumed(int id) {
         if (id < 0) return;
         ValueSlot& v = V(id);
+        if (v.kind == V_INPUT) v.pending--;  // (only to know a writable input's last consumer)
         if (v.kind != V_TEMP) return;
         v.pending--;
         if (v.pending > 0) return;
@@ -435,6 +451,46 @@ struct Runner {
         } else {
             v.root = -1;  // view of a constant / graph input: nothing to keep alive
         }
+    }
+
+    // output `id` as a run-time host value: `ints` in `shape` (no device memory, no launch)
+    void set_host(int id, const std::vector<int64_t>& ints, int ndim, const int64_t* shape) {
+        ValueSlot& v = V(id);
+        v.has_host_ints = true;
+        v.host_ints = ints;
+        v.host_i32.assign(ints.size() ? ints.size() : 1, 0);
+        for (size_t i = 0; i < ints.size(); i++) v.host_i32[i] = (int32_t)ints[i];
+        rten_tensor t{};
+        t.data = v.host_i32.data();
+        t.dtype = RTEN_I32;
+        t.ndim = ndim;
+        for (int i = 0; i < ndim; i++) t.shape[i] = shape[i];
+        set_contiguous(&t);
+        t.device = RTEN_DEVICE_HOST;
+        v.t = t;
+        v.root = -1;
+        v.live = true;
+        v.owned = false;
+    }
+
+    // The attention cache input `slot` of node o extended in place (the reference's run_in_place, gqa_present_cache):
+    // when it is a writable graph input whose grow axis is 2, this node is its last consumer, it is not a requested
+    // output, the node wants present output `out_k` and the buffer holds grow more positions, `present` becomes the
+    // past's buffer with the grown shape and true is returned.  Otherwise the node builds a new present cache.
+    bool cache_in_place(const OpNode& o, size_t slot, size_t out_k, int64_t grow, rten_tensor* present) {
+        if (slot >= o.in.size() || o.in[slot] < 0 || !wants(o, out_k)) return false;
+        const ValueSlot& v = V(o.in[slot]);
+        if (!v.writable || v.grow_axis != 2 || v.t.ndim != 4 || v.pending != 1 || keep.count(o.in[slot])) return false;
+        if (v.t.shape[2] + grow > v.capacity) return false;
+        *present = v.t;
+        present->shape[2] += grow;
+        return true;
+    }
+    // present output k of node o after the call: a view of the writable input it was written into, or a new buffer
+    void set_present(const OpNode& o, size_t k, size_t slot, bool in_place, const rten_tensor& t) {
+        if (!in_place) return set_output(o, k, t);
+        set_view(o.out[k], t, o.in[slot]);
+        V(o.out[k]).alias_of = V(o.in[slot]).input_index;
     }
 
     static bool contiguous(const rten_tensor& t) { return is_contiguous(&t); }
@@ -566,6 +622,13 @@ struct Runner {
         RTB_TRY(o.def->run(*this, o, &y));
         if (alloc) set_owned(o.out[0], y);
         else set_view(o.out[0], y, o.in[0]);
+        // a view of a host-known value that keeps its element order stays host-known
+        const ValueSlot& x = V(o.in[0]);
+        if (x.has_host_ints && ((o.def->flags & RESHAPE) || std::string_view(o.def->name) == "Identity")) {
+            ValueSlot& v = V(o.out[0]);
+            v.has_host_ints = true;
+            v.host_ints = x.host_ints;
+        }
         return RTEN_OK;
     }
 
@@ -744,6 +807,72 @@ rten_status run_group_norm(Runner& r, OpNode& o, rten_tensor* y) {
     return rten_b200_group_norm(r.ctx, x, (int)G, r.T(o, 1), r.T(o, 2), gamma, beta, o.n.attr_f("epsilon", 1e-5f), &o.activation, y);
 }
 
+// ReduceSum (src/ops/reduce.rs:1116-1163): axes from the attribute (opset < 13) or input 1; none or empty reduces
+// every axis, or, with noop_with_empty_axes, copies the input
+rten_status run_reduce_sum(Runner& r, OpNode& o, rten_tensor* y) {
+    const rten_tensor* x = r.T(o, 0);
+    std::vector<int64_t> axes;
+    RTB_TRY(r.axes_of(o, &axes));
+    if (axes.empty() && o.n.attr_i("noop_with_empty_axes", 0)) {
+        rten_tensor c = *x;
+        set_contiguous(&c);
+        c.device = r.ctx->device;
+        RTB_TRY(pool_alloc(r.ctx, (size_t)std::max<int64_t>(numel(&c), 1) * dtype_size(c.dtype), &c.data));
+        const rten_status st = rten_b200_copy(r.ctx, x, &c);
+        if (st != RTEN_OK) {
+            pool_free(r.ctx, c.data);
+            return st;
+        }
+        *y = c;
+        return RTEN_OK;
+    }
+    std::vector<int32_t> a(axes.begin(), axes.end());
+    return rten_b200_reduce_sum(r.ctx, x, a.data(), (int)a.size(), (int)o.n.attr_i("keepdims", 1), y);
+}
+
+// Shape (src/ops/layout.rs): the input's dims [start, end) -- negative from the end, clamped to [0, ndim], end at least
+// start -- as a host value
+rten_status run_shape(Runner& r, OpNode& o, rten_tensor*) {
+    const rten_tensor* x = r.T(o, 0);
+    const int64_t nd = x->ndim;
+    auto bound = [&](const char* name, int64_t dflt) {
+        if (!o.n.attr(name)) return dflt;
+        const int64_t v = o.n.attr_i(name, 0);
+        return std::min(nd, std::max<int64_t>(0, v < 0 ? v + nd : v));
+    };
+    const int64_t start = bound("start", 0), end = std::max(start, bound("end", nd));
+    const std::vector<int64_t> dims(x->shape + start, x->shape + end);
+    const int64_t n = (int64_t)dims.size();
+    if (Runner::wants(o, 0)) r.set_host(o.out[0], dims, 1, &n);
+    return RTEN_OK;
+}
+
+// Gather (src/ops/gather.rs gather) of a host-known vector on axis 0 with host-known indices (a scalar or a vector): a
+// host value, negative indices from the end.  false: not such a Gather.
+bool host_gather(Runner& r, OpNode& o, rten_status* st) {
+    const ValueSlot& data = r.V(o.in[0]);
+    const ValueSlot* idx = o.in.size() > 1 && o.in[1] >= 0 ? &r.V(o.in[1]) : nullptr;
+    if (!data.has_host_ints || !idx || !idx->has_host_ints || data.t.ndim > 1 || idx->t.ndim > 1) return false;
+    const int64_t axis = o.n.attr_i("axis", 0);
+    if (data.t.ndim == 0 || (axis != 0 && axis != -1)) {
+        *st = mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "Axis is invalid");
+        return true;
+    }
+    const int64_t len = data.t.shape[0];
+    std::vector<int64_t> out;
+    for (int64_t i : idx->host_ints) {
+        const int64_t k = i < 0 ? i + len : i;
+        if (k < 0 || k >= len) {
+            *st = mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "Entry in `indices` is out of range");
+            return true;
+        }
+        out.push_back(data.host_ints[(size_t)k]);
+    }
+    if (Runner::wants(o, 0)) r.set_host(o.out[0], out, idx->t.ndim, idx->t.shape);
+    *st = RTEN_OK;
+    return true;
+}
+
 constexpr OpDef OPS[] = {
     {"Conv", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
          rten_conv_params p;
@@ -836,6 +965,8 @@ constexpr OpDef OPS[] = {
          return n.attr("axis") ? RTEN_OK : mfail(m->ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Concat: missing attribute axis");
      }},
     {"GlobalAveragePool", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_global_average_pool(r.ctx, r.T(o, 0), y); }},
+    {"ReduceSum", ONNX, 0, 0b1, run_reduce_sum},
+    {"Shape", ONNX, 0, 0b1, run_shape},
     {"ReduceMean", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
          const rten_tensor* x = r.T(o, 0);
          std::vector<int64_t> axes;
@@ -924,6 +1055,7 @@ constexpr OpDef OPS[] = {
          return RTEN_OK;
      }},
     {"Add", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_add(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
+    {"Sub", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_sub(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
     {"Mul", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_mul(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
     {"LayerNormalization", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
          return rten_b200_layer_norm(r.ctx, r.T(o, 0), r.T(o, 1), r.T(o, 2), (int)o.n.attr_i("axis", -1), o.n.attr_f("epsilon", 1e-5f), y); }},
@@ -935,6 +1067,8 @@ constexpr OpDef OPS[] = {
     {"SkipLayerNormalization", MS, 0, 0b1, run_skip_norm<false>, check_skip_norm},
     {"SkipSimplifiedLayerNormalization", MS, 0, 0b1, run_skip_norm<true>, check_skip_norm},
     {"Gather", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
+         rten_status st;
+         if (host_gather(r, o, &st)) return st;
          if (o.n.attr_i("axis", 0) != 0 || r.T(o, 0)->ndim != 2)
              return mfail(r.ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Gather: only axis 0 of a 2-D table is supported");
          return rten_b200_gather_rows(r.ctx, r.T(o, 0), r.T(o, 1), y);
@@ -942,14 +1076,35 @@ constexpr OpDef OPS[] = {
     {"Cast", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
          const int64_t to = o.n.attr_i("to", 0);
          const rten_tensor* x = r.T(o, 0);
-         if ((to == onnx::DT_FLOAT && x->dtype == RTEN_F32) || ((to == onnx::DT_INT32 || to == onnx::DT_INT64) && x->dtype == RTEN_I32)) {
+         const bool to_int = to == onnx::DT_INT32 || to == onnx::DT_INT64;
+         if ((to == onnx::DT_FLOAT && x->dtype == RTEN_F32) || (to_int && x->dtype == RTEN_I32)) {
              r.set_view(o.out[0], *x, o.in[0]);
+             if (to_int && r.V(o.in[0]).has_host_ints) {  // (stays host-known)
+                 ValueSlot& v = r.V(o.out[0]);
+                 v.has_host_ints = true;
+                 v.host_ints = r.V(o.in[0]).host_ints;
+                 if (to == onnx::DT_INT32)
+                     for (int64_t& i : v.host_ints) i = (int32_t)i;
+             }
              return RTEN_OK;
          }
          if (to != onnx::DT_FLOAT || x->dtype != RTEN_I32) return mfail(r.ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Cast: only int32 -> float is supported");
          rten_tensor c;
          bool alloc = false;
-         RTB_TRY(r.make_contiguous(*x, &c, &alloc));
+         if (x->device < 0) {  // a host value: uploaded first
+             c = *x;
+             set_contiguous(&c);
+             c.device = r.ctx->device;
+             RTB_TRY(pool_alloc(r.ctx, (size_t)std::max<int64_t>(numel(x), 1) * 4, &c.data));
+             alloc = true;
+             const rten_status st = rten_b200_copy(r.ctx, x, &c);
+             if (st != RTEN_OK) {
+                 pool_free(r.ctx, c.data);
+                 return st;
+             }
+         } else {
+             RTB_TRY(r.make_contiguous(*x, &c, &alloc));
+         }
          *y = c;
          y->dtype = RTEN_F32;
          void* d = nullptr;
@@ -997,10 +1152,12 @@ constexpr OpDef OPS[] = {
          p.local_window_size = (int32_t)o.n.attr_i("local_window_size", -1);
          p.softcap = o.n.attr_f("softcap", 0.0f);
          rten_tensor pk{}, pv{};
+         const int64_t S = r.T(o, 0)->ndim >= 2 ? r.T(o, 0)->shape[1] : 0;
+         const bool ik = r.cache_in_place(o, 3, 1, S, &pk), iv = r.cache_in_place(o, 4, 2, S, &pv);
          RTB_TRY(rten_b200_group_query_attention(r.ctx, r.T(o, 0), r.T(o, 1), r.T(o, 2), r.T(o, 3), r.T(o, 4), r.T(o, 5), r.T(o, 6),
                                                  r.T(o, 7), r.T(o, 8), r.T(o, 9), r.T(o, 10), &p, y, &pk, &pv));
-         r.set_output(o, 1, pk);
-         r.set_output(o, 2, pv);
+         r.set_present(o, 1, 3, ik, pk);
+         r.set_present(o, 2, 4, iv, pv);
          return RTEN_OK;
      }, [](rten_model* m, onnx::Node& n) {  // src/op_registry/onnx_registry.rs:1467-1492, contrib.rs:817-821
          if (!n.attr("num_heads") || !n.attr("kv_num_heads"))
@@ -1017,10 +1174,14 @@ constexpr OpDef OPS[] = {
          p.mask_filter_value = o.n.attr_f("mask_filter_value", -10000.0f);
          p.unidirectional = (int32_t)o.n.attr_i("unidirectional", 0);
          rten_tensor pk{}, pv{};
+         // new positions: key [B, L, H * D]; without key (packed QKV or self-attention on the query) the query's S
+         const rten_tensor *q = r.T(o, 0), *k = r.T(o, 1);
+         const int64_t L = k && k->ndim == 3 ? k->shape[1] : k ? -1 : (q->ndim >= 2 ? q->shape[1] : -1);
+         const bool ik = L >= 0 && r.cache_in_place(o, 6, 1, L, &pk), iv = L >= 0 && r.cache_in_place(o, 7, 2, L, &pv);
          RTB_TRY(rten_b200_multi_head_attention(r.ctx, r.T(o, 0), r.T(o, 1), r.T(o, 2), r.T(o, 3), r.T(o, 4), r.T(o, 5), r.T(o, 6),
                                                 r.T(o, 7), nullptr, nullptr, &p, y, r.wants(o, 1) ? &pk : nullptr, r.wants(o, 2) ? &pv : nullptr));
-         r.set_output(o, 1, pk);
-         r.set_output(o, 2, pv);
+         r.set_present(o, 1, 6, ik, pk);
+         r.set_present(o, 2, 7, iv, pv);
          return RTEN_OK;
      }, [](rten_model* m, onnx::Node& n) {  // src/op_registry/onnx_registry.rs:1495-1505, contrib.rs:302-315
          if (!n.attr("num_heads")) return mfail(m->ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MultiHeadAttention: missing attribute num_heads");
@@ -1409,6 +1570,23 @@ const char* rten_b200_model_summary(const rten_model* m) { return m ? m->summary
 
 rten_status rten_b200_model_run(rten_model* m, int32_t n_inputs, const char* const* input_names, const rten_tensor* inputs,
                                 int32_t n_outputs, const char* const* output_names, rten_tensor* outputs) {
+    return rten_b200_model_run_ex(m, n_inputs, input_names, inputs, nullptr, n_outputs, output_names, outputs, nullptr);
+}
+
+// A writable input's strides are those of a dense tensor whose grow axis has `capacity` positions
+static bool dense_with_capacity(const rten_tensor& t, int grow_axis, int64_t capacity) {
+    int64_t st = 1;
+    for (int i = t.ndim - 1; i >= 0; i--) {
+        const int64_t n = i == grow_axis ? capacity : t.shape[i];
+        if (n != 1 && t.strides[i] != st) return false;
+        st *= n;
+    }
+    return true;
+}
+
+rten_status rten_b200_model_run_ex(rten_model* m, int32_t n_inputs, const char* const* input_names, const rten_tensor* inputs,
+                                   const rten_model_input_opts* opts, int32_t n_outputs, const char* const* output_names,
+                                   rten_tensor* outputs, int32_t* output_alias) {
     if (!m || (n_inputs && (!input_names || !inputs)) || n_outputs < 1 || !output_names || !outputs) return RTEN_ERR_INVALID_VALUE;
     rten_ctx* ctx = m->ctx;
     cudaSetDevice(ctx->device);
@@ -1421,7 +1599,16 @@ rten_status rten_b200_model_run(rten_model* m, int32_t n_inputs, const char* con
             v.root = -1;
             v.views = 0;
             v.pending = 0;
-            if (v.kind == V_TEMP) v.t.data = nullptr;
+            v.writable = false;
+            v.grow_axis = -1;
+            v.capacity = 0;
+            v.input_index = -1;
+            v.alias_of = -1;
+            if (v.kind == V_TEMP) {
+                v.t.data = nullptr;
+                v.has_host_ints = false;
+                v.host_ints.clear();
+            }
         }
     }
     std::vector<void*> staged;  // device copies of host inputs
@@ -1441,6 +1628,20 @@ rten_status rten_b200_model_run(rten_model* m, int32_t n_inputs, const char* con
             return mfail(ctx, RTEN_ERR_INVALID_VALUE, std::string("unknown model input '") + (input_names[i] ? input_names[i] : "") + "'");
         ValueSlot& v = m->values[(size_t)it->second];
         v.t = inputs[i];
+        if (opts && opts[i].writable) {
+            const rten_model_input_opts& op = opts[i];
+            const rten_tensor& t = inputs[i];
+            if (t.device < 0)
+                return cleanup(mfail(ctx, RTEN_ERR_INVALID_VALUE, std::string("writable input '") + input_names[i] + "' must be device-resident"));
+            if (op.grow_axis < -1 || op.grow_axis >= t.ndim || (op.grow_axis >= 0 && op.capacity < t.shape[op.grow_axis]) ||
+                !dense_with_capacity(t, op.grow_axis, op.grow_axis >= 0 ? op.capacity : 0))
+                return cleanup(mfail(ctx, RTEN_ERR_INVALID_VALUE, std::string("writable input '") + input_names[i] +
+                                                                      "': strides must be dense with capacity >= shape on grow_axis"));
+            v.writable = true;
+            v.grow_axis = op.grow_axis;
+            v.capacity = op.grow_axis >= 0 ? op.capacity : 0;
+        }
+        v.input_index = i;
         if (inputs[i].device < 0) {  // host tensor: staged through HBM for the duration of the run
             rten_tensor d = inputs[i];
             set_contiguous(&d);
@@ -1476,10 +1677,17 @@ rten_status rten_b200_model_run(rten_model* m, int32_t n_inputs, const char* con
         if (st != RTEN_OK) return cleanup(st);
         for (int i : o.in) r.consumed(i);
     }
-    // hand the requested outputs over: owned buffers move to the caller; views / constants / inputs are copied
+    // hand the requested outputs over: owned buffers move to the caller; a present cache written into a writable input is
+    // returned as that view (output_alias names the input); other views / constants / inputs are copied
     for (int32_t i = 0; i < n_outputs; i++) {
         ValueSlot& v = m->values[(size_t)want[(size_t)i]];
         if (!v.live && v.kind != V_CONST) return cleanup(mfail(ctx, RTEN_ERR_INVALID_VALUE, "requested output '" + v.name + "' was not computed"));
+        if (output_alias) output_alias[i] = -1;
+        if (v.alias_of >= 0 && output_alias) {
+            outputs[i] = v.t;
+            output_alias[i] = v.alias_of;
+            continue;
+        }
         const bool movable = v.kind == V_TEMP && v.owned && v.root < 0 && v.views == 0 && is_contiguous(&v.t);
         bool dup = false;
         for (int32_t k = 0; k < i; k++) dup = dup || want[(size_t)k] == want[(size_t)i];
@@ -1490,6 +1698,7 @@ rten_status rten_b200_model_run(rten_model* m, int32_t n_inputs, const char* con
         } else {
             rten_tensor c = v.t;
             set_contiguous(&c);
+            c.device = ctx->device;  // (a host value is handed over in HBM like every other output)
             void* p = nullptr;
             rten_status st = pool_alloc(ctx, (size_t)std::max<int64_t>(numel(&c), 1) * dtype_size(c.dtype), &p);
             if (st != RTEN_OK) return cleanup(st);

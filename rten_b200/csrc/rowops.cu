@@ -861,6 +861,73 @@ rten_status launch_add_flat(rten_ctx* ctx, const float* a, const float* b, float
     return launch(ctx, "add launch", add_flat_kernel, {ew_grid(ctx, (n + 3) / 4), 256}, a, b, d, n, relu);
 }
 
+// The binary operations the f32 Add / Mul kernels above do not run, one instance per (type, operation): they are kept
+// apart so that those kernels stay as they are.  i32 arithmetic wraps (src/ops/binary_elementwise.rs on i32).
+template <typename T, int OP>
+__device__ __forceinline__ T binary_apply(T a, T b) {
+    if constexpr (std::is_same<T, float>::value) {
+        static_assert(OP == BIN_SUB, "f32 Add / Mul run on add_flat_kernel / nd_add_kernel");
+        return __fsub_rn(a, b);
+    } else {
+        const unsigned x = (unsigned)a, y = (unsigned)b;
+        return (int)(OP == BIN_ADD ? x + y : OP == BIN_SUB ? x - y : x * y);
+    }
+}
+
+template <typename T, int OP>
+__global__ void __launch_bounds__(256) binary_flat_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d, long long n) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) d[i] = binary_apply<T, OP>(a[i], b[i]);
+}
+
+template <typename T, int OP>
+__global__ void __launch_bounds__(256) binary_nd_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d, const NdParams p) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += stride) {
+        long long rem = i, ao = 0, bo = 0, dof = 0;
+#pragma unroll 1
+        for (int k = p.ndim - 1; k >= 0; k--) {
+            const long long idx = rem % p.shape[k];
+            rem /= p.shape[k];
+            ao += idx * p.sa[k];
+            bo += idx * p.sb[k];
+            dof += idx * p.sd[k];
+        }
+        d[dof] = binary_apply<T, OP>(a[ao], b[bo]);
+    }
+}
+
+template <typename T, int OP>
+static rten_status launch_binary_typed(rten_ctx* ctx, const T* a, const T* b, T* d, const NdParams& p, bool flat) {
+    if (flat) return launch(ctx, "binary launch", binary_flat_kernel<T, OP>, {ew_grid(ctx, p.n), 256}, a, b, d, p.n);
+    return launch(ctx, "binary launch", binary_nd_kernel<T, OP>, {ew_grid(ctx, p.n), 256}, a, b, d, p);
+}
+
+rten_status launch_binary(rten_ctx* ctx, int dtype, int op, const void* a, const void* b, void* d, int ndim, const long long* shape,
+                          const long long* sa, const long long* sb, const long long* sd, bool flat) {
+    NdParams p;
+    memset(&p, 0, sizeof(p));
+    p.ndim = ndim;
+    p.n = 1;
+    for (int i = 0; i < ndim; i++) {
+        p.shape[i] = shape[i];
+        p.sa[i] = sa[i];
+        p.sb[i] = sb[i];
+        p.sd[i] = sd[i];
+        p.n *= shape[i];
+    }
+    if (p.n == 0) return RTEN_OK;
+    const int *ai = (const int*)a, *bi = (const int*)b;
+    int* di = (int*)d;
+    if (dtype == RTEN_F32 && op == BIN_SUB) return launch_binary_typed<float, BIN_SUB>(ctx, (const float*)a, (const float*)b, (float*)d, p, flat);
+    if (dtype != RTEN_I32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    switch (op) {
+        case BIN_ADD: return launch_binary_typed<int, BIN_ADD>(ctx, ai, bi, di, p, flat);
+        case BIN_SUB: return launch_binary_typed<int, BIN_SUB>(ctx, ai, bi, di, p, flat);
+        default: return launch_binary_typed<int, BIN_MUL>(ctx, ai, bi, di, p, flat);
+    }
+}
+
 // =========================================================================================
 // DynamicQuantizeLinear (src/ops/quantize.rs:352-434; rten-vecmath/src/quantize.rs:38-77)
 //   pass 1: min / max  (order independent) -> 2 floats (ordered-int atomics)

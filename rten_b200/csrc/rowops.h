@@ -57,6 +57,11 @@ rten_status launch_nd_copy(rten_ctx* ctx, int esize, const void* src, void* dst,
 rten_status launch_nd_add(rten_ctx* ctx, const float* a, const float* b, float* d, int ndim, const long long* shape,
                           const long long* sa, const long long* sb, const long long* sd, int relu);
 rten_status launch_add_flat(rten_ctx* ctx, const float* a, const float* b, float* d, long long n, int relu);
+// d = a (op) b for the operations launch_nd_add / launch_add_flat do not run: f32 Sub (__fsub_rn) and i32 Add / Sub / Mul,
+// which wrap.  Same operand layouts as launch_nd_add; `flat`: a, b and d dense with the same strides (n elements).
+enum BinaryOp { BIN_ADD = 0, BIN_SUB = 1, BIN_MUL = 2 };
+rten_status launch_binary(rten_ctx* ctx, int dtype, int op, const void* a, const void* b, void* d, int ndim, const long long* shape,
+                          const long long* sa, const long long* sb, const long long* sd, bool flat);
 rten_status launch_minmax(rten_ctx* ctx, const float* x, long long n, int* mm /* 2 ordered ints */);
 // `xch` (batch-sharded runs): the kernel first exchanges the local range in `mm` with the other ranks (comm_device.cuh)
 struct RangeExchange;

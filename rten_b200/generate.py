@@ -119,6 +119,73 @@ class GPT2DecoderModel:
         return {k: res[k] for k in outputs}
 
 
+def grow_capacity(capacity: int, needed: int) -> int:
+    """The capacity a cache of `capacity` positions grows to so that it holds `needed`: doubled until it does
+    (KvCacheData::clone_with_capacity, generator.rs:878-884)"""
+    capacity = max(int(capacity), 1)
+    while capacity < needed:
+        capacity *= 2
+    return capacity
+
+
+class ModelDecoder:
+    """A loaded `Model` (an onnxruntime-genai / Optimum decoder export) behind the contract `Generator` speaks, the one
+    GPT2DecoderModel speaks: `input_names`, `output_names`, `run(inputs, outputs) -> dict`.  The KV caches are
+    KvCacheHandles passed to the model as writable inputs with spare capacity, so the attention nodes append the new
+    positions in place instead of copying the past every step.  The first step gets empty caches
+    [batch, kv_heads, 0, head] (kv_heads and the head size from the file's declared input dims) of capacity
+    `kv_cache_capacity` (or 1).  After each step a cache that cannot take one more position is re-allocated with twice
+    the length and its valid prefix copied (one copy launch per cache), as generator.rs:878-884 does."""
+
+    def __init__(self, model, batch: int, kv_cache_capacity: Optional[int] = None):
+        self.model, self.ctx, self.batch = model, model.ctx, batch
+        self.capacity = max(int(kv_cache_capacity or 1), 1)
+        self.input_names, self.output_names = list(model.input_names), list(model.output_names)
+        dims = {v["name"]: v["dims"] for v in model.summary["inputs"]}
+        self.kv_dims = {}
+        for n in self.input_names:
+            if n.startswith("past_key_values."):
+                d = dims.get(n, [])
+                if len(d) != 4 or d[1] <= 0 or d[3] <= 0:
+                    raise ValueError(f"{n}: the file does not declare [batch, kv_heads, seq, head] with known kv_heads and head")
+                self.kv_dims[n] = (int(d[1]), int(d[3]))
+
+    def _empty(self, name: str) -> KvCacheHandle:
+        h, d = self.kv_dims[name]
+        return KvCacheHandle(self.ctx.empty((self.batch, h, self.capacity, d)), 0, self.capacity)
+
+    def _with_room(self, c) -> KvCacheHandle:
+        """`c` (a handle, or a new present tensor) as a handle that holds one more position"""
+        if not isinstance(c, KvCacheHandle):
+            c = KvCacheHandle(c, c.shape[2], c.shape[2])
+        if c.has_capacity(c.seq_len + 1):
+            return c
+        cap = grow_capacity(c.capacity, c.seq_len + 1)
+        B, H, _, D = c.shape
+        t = self.ctx.empty((B, H, cap, D))
+        if c.seq_len:
+            src = c.tensor.view((B, H, c.seq_len, D), c.tensor.strides)
+            t.view((B, H, c.seq_len, D), t.strides).assign(src)
+        return KvCacheHandle(t, c.seq_len, cap)
+
+    def run(self, inputs: Dict[str, object], outputs: Sequence[str]) -> Dict[str, object]:
+        feeds = {}
+        for n, v in inputs.items():
+            if n not in self.input_names:
+                continue
+            if n in self.kv_dims and v is None:
+                v = self._empty(n)
+            feeds[n] = v
+        got = dict(zip(outputs, self.model.run(feeds, list(outputs))))
+        for n, v in got.items():
+            if n.startswith("present."):
+                got[n] = self._with_room(v)
+        if "logits" in got and got["logits"].ndim == 3:  # the last position's logits [batch, vocab], as Generator samples
+            lg = got["logits"]
+            got["logits"] = lg.view((lg.shape[0], lg.shape[2]), (lg.strides[0], lg.strides[2]), (lg.shape[1] - 1) * lg.strides[1])
+        return got
+
+
 class ArgMaxSampler:
     """rten-generate/src/sampler.rs ArgMax: the greedy choice (ties -> lowest id)."""
 

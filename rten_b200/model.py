@@ -47,20 +47,44 @@ class Model:
     def summary(self) -> dict:
         return json.loads(self.ctx.lib.rten_b200_model_summary(self.handle).decode())
 
-    def run(self, inputs: Dict[str, Union[np.ndarray, DeviceTensor]], outputs: Optional[Sequence[str]] = None) -> List[DeviceTensor]:
+    def run(self, inputs: Dict[str, object], outputs: Optional[Sequence[str]] = None) -> List[object]:
+        """Inputs are numpy arrays, DeviceTensors or KvCacheHandles (generate.py).  A handle is passed as a writable view
+        of its first seq_len positions with its capacity (rten_b200_model_run_ex): an attention node may write its present
+        cache into it, and such an output comes back as a KvCacheHandle over the same buffer with the new length."""
+        from .generate import KvCacheHandle
         outputs = list(outputs) if outputs is not None else self.output_names
         A = _Args(self.ctx)
         names = list(inputs)
         in_names = (C.c_char_p * len(names))(*[n.encode() for n in names])
         in_t = (RtenTensor * max(len(names), 1))()
+        opts = (_lib.RtenModelInputOpts * max(len(names), 1))()
+        handles = {}
         for i, n in enumerate(names):
-            ref = A.t(inputs[n])
+            v = inputs[n]
+            if isinstance(v, KvCacheHandle):
+                if v.transposed:
+                    raise OpError(5, f"{n}: a transposed cache handle cannot be a model input")
+                t = v.tensor
+                v = t.view(t.shape[:2] + (v.seq_len,) + t.shape[3:], t.strides)
+                opts[i].writable, opts[i].grow_axis, opts[i].capacity = 1, 2, inputs[n].capacity
+                handles[i] = inputs[n]
+            ref = A.t(v)
             C.memmove(C.byref(in_t, i * C.sizeof(RtenTensor)), ref, C.sizeof(RtenTensor))
         out_names = (C.c_char_p * len(outputs))(*[n.encode() for n in outputs])
         out_t = (RtenTensor * len(outputs))()
-        self.ctx.check(self.ctx.lib.rten_b200_model_run(self.handle, len(names), in_names, in_t, len(outputs), out_names, out_t))
+        if handles:
+            alias = (C.c_int32 * len(outputs))()
+            self.ctx.check(self.ctx.lib.rten_b200_model_run_ex(self.handle, len(names), in_names, in_t, C.cast(opts, C.c_void_p),
+                                                               len(outputs), out_names, out_t, alias))
+        else:
+            alias = [-1] * len(outputs)
+            self.ctx.check(self.ctx.lib.rten_b200_model_run(self.handle, len(names), in_names, in_t, len(outputs), out_names, out_t))
         res = []
-        for d in out_t:
+        for d, a in zip(out_t, alias):
+            if a >= 0:
+                h = handles[a]
+                res.append(KvCacheHandle(h.tensor, int(d.shape[2]), h.capacity))
+                continue
             shape = tuple(d.shape[i] for i in range(d.ndim))
             strides = tuple(d.strides[i] for i in range(d.ndim))
             res.append(DeviceTensor(self.ctx, d.data, shape, strides, _RT2NP[d.dtype], owner=True))

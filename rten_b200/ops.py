@@ -1027,6 +1027,37 @@ class Mul:
         return A.wrap(o, out)
 
 
+class Sub:
+    """src/ops/binary_elementwise.rs Sub (f32 or wrapping i32, broadcasting)."""
+
+    def run(self, ctx, a, b, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        ctx.check(ctx.lib.rten_b200_sub(ctx.handle, A.t(a), A.t(b), C.byref(o)))
+        return A.wrap(o, out)
+
+
+class ReduceSum:
+    """src/ops/reduce.rs ReduceSum (f32 or wrapping i32): axes None or empty reduces every axis, unless
+    noop_with_empty_axes, which makes it a copy."""
+
+    def __init__(self, axes=None, keep_dims: bool = True, noop_with_empty_axes: bool = False):
+        self.axes = None if axes is None else [int(a) for a in axes]
+        self.keep_dims, self.noop_with_empty_axes = keep_dims, noop_with_empty_axes
+
+    def run(self, ctx, x, out=None):
+        if not self.axes and self.noop_with_empty_axes:
+            src = x if isinstance(x, DeviceTensor) else ctx.to_device(np.asarray(x))
+            y = out if out is not None else ctx.empty(src.shape, src.dtype)
+            y.assign(src)
+            return y
+        A = _Args(ctx)
+        o = A.out(out)
+        ax = (C.c_int32 * max(len(self.axes or []), 1))(*(self.axes or []))
+        ctx.check(ctx.lib.rten_b200_reduce_sum(ctx.handle, A.t(x), ax, len(self.axes or []), int(self.keep_dims), C.byref(o)))
+        return A.wrap(o, out)
+
+
 class MaxPool:
     """src/ops/pooling.rs MaxPool: kernel_size, padding [t,l,b,r], strides."""
 
