@@ -8,6 +8,7 @@
 
 #include "api_util.h"
 #include "rowops.h"
+#include "umma_gemm.h"
 
 namespace rtb {
 
@@ -201,56 +202,6 @@ using namespace rtb;
 extern "C" {
 
 const char* rten_b200_version(void) { return "rten-b200 0.1 (sm_90a)"; }
-
-// Measured launch plans can be kept across processes: RTEN_B200_TUNE_FILE names a text file that is read when a
-// context is created and rewritten when a context that measured new plans is destroyed (one line per problem:
-// key integers, '|', the three plan integers `bn splitk nbuf`).  Lines with any other number of plan integers (files
-// written by older builds) are skipped: those problems are planned afresh.
-static void tune_cache_load(rten_ctx* ctx, const char* path) {
-    FILE* f = fopen(path, "r");
-    if (!f) return;
-    char line[2048];
-    while (fgets(line, sizeof(line), f)) {
-        std::vector<long long> key;
-        std::array<int, 3> plan{};
-        char* p = line;
-        bool in_plan = false;
-        int np = 0;
-        while (*p) {
-            while (*p == ' ') p++;
-            if (*p == '|') {
-                in_plan = true;
-                p++;
-                continue;
-            }
-            if (*p == '\n' || *p == 0) break;
-            char* end = nullptr;
-            const long long v = strtoll(p, &end, 10);
-            if (end == p) break;
-            if (in_plan) {
-                if (np < 3) plan[np] = (int)v;
-                np++;
-            } else {
-                key.push_back(v);
-            }
-            p = end;
-        }
-        if (np == 3 && !key.empty()) ctx->tune_cache[key] = plan;
-    }
-    fclose(f);
-}
-
-static void tune_cache_save(rten_ctx* ctx, const char* path) {
-    FILE* f = fopen(path, "w");
-    if (!f) return;
-    for (const auto& kv : ctx->tune_cache) {
-        for (long long v : kv.first) fprintf(f, "%lld ", v);
-        fprintf(f, "|");
-        for (int v : kv.second) fprintf(f, " %d", v);
-        fprintf(f, "\n");
-    }
-    fclose(f);
-}
 
 rten_status rten_b200_ctx_create(int device, void* cuda_stream_or_null, size_t workspace_bytes, rten_ctx** out) {
     if (!out) return RTEN_ERR_INVALID_VALUE;

@@ -70,7 +70,7 @@ struct rten_ctx {
     void* encode_tiled = nullptr;  // cuTensorMapEncodeTiled (driver entry point)
     void* sk_counters = nullptr;   // split-K arrival counters (zero between launches)
     bool autotune = false;         // time candidate launch plans on first sight of a problem (umma_gemm.cu)
-    // autotuned plans: problem signature -> {bn, splitk, nbuf}, or {-1, bn, T} for the halo-reuse kernel (umma_gemm.cu)
+    // autotuned plans: problem signature -> the plan's three-integer record (umma_gemm.cu: tune_key, plan_record)
     std::map<std::vector<long long>, std::array<int, 3>> tune_cache;
     size_t tune_loaded = 0;        // entries read from RTEN_B200_TUNE_FILE (the file is rewritten when more exist at destroy)
     std::vector<rten_graph*> graphs;  // graphs captured on this context that still exist

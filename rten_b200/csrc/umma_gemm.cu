@@ -135,12 +135,23 @@ static void pick_conv_tile(const ConvGeom& g, int& tw, int& th, int& tb) {
 // ------------------------------------------------------------------------------------------
 // Launch plans
 // ------------------------------------------------------------------------------------------
-// A plan fixes the tile shape and the work decomposition of one launch.  Plans come from (a) the cost model below or
-// (b) the per-context autotune cache: with rten_b200_set_autotune(ctx, 1) the first launch of every distinct problem
-// times the model's best candidates on the device (CUDA events on the context stream) and remembers the winner.
+// A plan fixes the kernel, tile shape and work decomposition of one launch: bn, splitk, nbuf on the implicit-GEMM
+// kernels, or units of bn channels x T 128-slot tiles on the halo-reuse kernel (umma_halo.cu).  Plans come from (a) the
+// cost models or (b) the per-context autotune cache: with rten_b200_set_autotune(ctx, 1) the first launch of every
+// distinct problem times the best candidates on the device (CUDA events on the context stream) and remembers the winner.
 struct Plan {
     int bn = 32, splitk = 1, nbuf = 1;
+    bool halo = false;
+    int T = 0;  // (halo)
 };
+
+static Plan halo_plan(int bn, int T) {
+    Plan pl;
+    pl.halo = true;
+    pl.bn = bn;
+    pl.T = T;
+    return pl;
+}
 
 // Everything about a launch that does not depend on the plan.
 struct Prepared {
@@ -582,12 +593,70 @@ static std::vector<long long> tune_key(const GemmLaunch& L, const Prepared& q) {
     return k;
 }
 
-static Plan plan_from_array(const std::array<int, 3>& a) {
+// A plan as the three integers of its tune_cache entry and plans-file line: `bn splitk nbuf`, or `-1 bn T` for the
+// halo-reuse kernel.
+static std::array<int, 3> plan_record(const Plan& pl) {
+    return pl.halo ? std::array<int, 3>{-1, pl.bn, pl.T} : std::array<int, 3>{pl.bn, pl.splitk, pl.nbuf};
+}
+
+static Plan plan_from_record(const std::array<int, 3>& r) {
+    if (r[0] < 0) return halo_plan(r[1], r[2]);
     Plan pl;
-    pl.bn = a[0];
-    pl.splitk = a[1];
-    pl.nbuf = a[2];
+    pl.bn = r[0];
+    pl.splitk = r[1];
+    pl.nbuf = r[2];
     return pl;
+}
+
+// Measured launch plans can be kept across processes: RTEN_B200_TUNE_FILE names a text file that is read when a
+// context is created and rewritten when a context that measured new plans is destroyed (one line per problem:
+// tune_key's integers, '|', the three integers of plan_record).  Lines with any other number of plan integers (files
+// written by older builds) are skipped: those problems are planned afresh.  A recorded plan that no longer fits its
+// problem is dropped when it is used.
+void tune_cache_load(rten_ctx* ctx, const char* path) {
+    FILE* f = fopen(path, "r");
+    if (!f) return;
+    char line[2048];
+    while (fgets(line, sizeof(line), f)) {
+        std::vector<long long> key;
+        std::array<int, 3> plan{};
+        char* p = line;
+        bool in_plan = false;
+        int np = 0;
+        while (*p) {
+            while (*p == ' ') p++;
+            if (*p == '|') {
+                in_plan = true;
+                p++;
+                continue;
+            }
+            if (*p == '\n' || *p == 0) break;
+            char* end = nullptr;
+            const long long v = strtoll(p, &end, 10);
+            if (end == p) break;
+            if (in_plan) {
+                if (np < 3) plan[np] = (int)v;
+                np++;
+            } else {
+                key.push_back(v);
+            }
+            p = end;
+        }
+        if (np == 3 && !key.empty()) ctx->tune_cache[key] = plan;
+    }
+    fclose(f);
+}
+
+void tune_cache_save(rten_ctx* ctx, const char* path) {
+    FILE* f = fopen(path, "w");
+    if (!f) return;
+    for (const auto& kv : ctx->tune_cache) {
+        for (long long v : kv.first) fprintf(f, "%lld ", v);
+        fprintf(f, "|");
+        for (int v : kv.second) fprintf(f, " %d", v);
+        fprintf(f, "\n");
+    }
+    fclose(f);
 }
 
 // RTEN_F32_TF32X3: run the same kernel over split operands -- K (plain) or C (conv; K order is (ky, kx, c)) tripled:
@@ -688,39 +757,131 @@ static rten_status launch_tf32x3(rten_ctx* ctx, const GemmLaunch& L0) {
     return st;
 }
 
+static rten_status run_plan(rten_ctx* ctx, const GemmLaunch& L, const Prepared& q, const Plan& pl, bool verbose,
+                            void* ws = nullptr) {
+    return pl.halo ? launch_umma_halo_conv(ctx, L, pl.bn, pl.T, verbose) : launch_plan(ctx, L, q, pl, verbose, ws);
+}
+
+// With the stream idle and the launch safe to repeat: times up to 24 of the model's candidates and, where `halo`, the
+// halo kernel's unit shapes, records the fastest and leaves it in `plan`.  Otherwise leaves `plan` as it is.
+static rten_status autotune(rten_ctx* ctx, const GemmLaunch& L, const Prepared& q,
+                            const std::vector<std::pair<double, Plan>>& cands, bool halo, bool verbose, Plan& plan) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    cudaStreamIsCapturing(ctx->stream, &cs);
+    // re-running the launch must be idempotent: the output may not alias the residual
+    if (ctx->capturing || cs != cudaStreamCaptureStatusNone || (L.epi.r && (const void*)L.epi.r == (const void*)L.epi.d))
+        return RTEN_OK;
+    const size_t ncand = std::min<size_t>(cands.size(), 24);
+    // one split-K workspace for every candidate (allocating inside the timed launches would time cudaMalloc)
+    size_t ws_max = 0;
+    for (size_t i = 0; i < ncand; i++) {
+        PlanShape ps;
+        if (plan_shape(q, cands[i].second, ps)) ws_max = std::max(ws_max, splitk_ws_bytes(ps, cands[i].second));
+    }
+    void* ws = nullptr;
+    if (ws_max) {
+        RTB_TRY(ensure_splitk_counters(ctx));
+        RTB_TRY(temp_alloc(ctx, ws_max, &ws));
+        cudaStreamSynchronize(ctx->stream);
+    }
+    cudaEvent_t e0, e1;
+    cudaEventCreate(&e0);
+    cudaEventCreate(&e1);
+    // ms per launch over n launches after a warm-up launch (which also validates the plan); < 0: the plan did not run
+    auto time_plan = [&](const Plan& x, int n) -> double {
+        if (run_plan(ctx, L, q, x, false, ws) != RTEN_OK) return -1.0;
+        cudaEventRecord(e0, ctx->stream);
+        bool ok = true;
+        for (int r = 0; r < n && ok; r++) ok = run_plan(ctx, L, q, x, false, ws) == RTEN_OK;
+        cudaEventRecord(e1, ctx->stream);
+        if (cudaEventSynchronize(e1) != cudaSuccess || !ok) return -1.0;
+        float t = 0.f;
+        cudaEventElapsedTime(&t, e0, e1);
+        return (double)t / n;
+    };
+    double best_ms = 1e30;
+    int reps = 4;  // raised after the first candidate so that every timed window is >= ~150 us (event resolution)
+    std::vector<std::pair<double, size_t>> timed;
+    for (size_t i = 0; i < ncand; i++) {
+        const Plan& x = cands[i].second;
+        double ms = time_plan(x, reps);
+        if (ms < 0) continue;
+        timed.emplace_back(ms, i);
+        if (verbose)
+            fprintf(stderr, "[autotune] bn=%d splitk=%d nbuf=%d model=%.0f -> %.2f us\n", x.bn, x.splitk, x.nbuf,
+                    cands[i].first, ms * 1e3);
+        if (ms < best_ms) {
+            best_ms = ms;
+            plan = x;
+        }
+        reps = std::max(4, std::min(32, (int)(0.15 / std::max(best_ms, 1e-3))));
+    }
+    // second look at the three fastest with longer windows: single measurements of 20-40 us kernels are noisy enough
+    // to flip the choice between near-equal plans from run to run
+    std::sort(timed.begin(), timed.end());
+    best_ms = 1e30;
+    for (size_t k = 0; k < std::min<size_t>(3, timed.size()); k++) {
+        const Plan& x = cands[timed[k].second].second;
+        const double again = time_plan(x, 2 * reps);
+        const double ms = again < 0 ? timed[k].first : again;  // the longer window decides
+        if (ms < best_ms) {
+            best_ms = ms;
+            plan = x;
+        }
+    }
+    for (const auto& s : HALO_SHAPES) {
+        const Plan x = halo_plan(s[0], s[1]);
+        if (!halo || x.bn > L.N) continue;
+        double ms = time_plan(x, reps);
+        if (ms > 0 && ms < best_ms * 1.05) ms = time_plan(x, 2 * reps);  // a second, longer look at contenders
+        if (verbose && ms > 0) fprintf(stderr, "[autotune] halo bn=%d T=%d -> %.2f us\n", x.bn, x.T, ms * 1e3);
+        if (ms > 0 && ms < best_ms * 0.97) {  // must win clearly: the generic kernel is the better-trodden path
+            best_ms = ms;
+            plan = x;
+        }
+    }
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    ctx->tune_cache[tune_key(L, q)] = plan_record(plan);
+    return RTEN_OK;
+}
+
 rten_status launch_umma_gemm(rten_ctx* ctx, const GemmLaunch& L) {
+    const bool verbose = getenv("RTEN_B200_VERBOSE") != nullptr;
+    const char* force_bn = getenv("RTEN_B200_FORCE_BN");
+    const char* force_sk = getenv("RTEN_B200_FORCE_SPLITK");
+    const char* halo_on = getenv("RTEN_B200_HALO");
+    // stride-1 windows (the 3x3 layers) may run on the halo-reuse kernel, which moves the activations into shared
+    // memory once per channel block instead of once per filter tap (umma_halo.cu)
+    const bool halo = L.conv && L.kind == 0 && L.g.kh * L.g.kw > 1 && !L.x3_cb && !L.proj.C && !getenv("RTEN_B200_NO_HALO");
+    Prepared q;
     if (L.chain.N2 > 0) {
         // chained: a fixed plan (128-column passes of one pixel tile), not autotuned; single-pass TF32 only (a 3xTF32
         // chain would not equal the separate launches)
         if (L.kind != 0 || ctx->f32_mode != RTEN_F32_TF32 || L.x3_cb || getenv("RTEN_B200_NO_CHAIN"))
             return RTEN_ERR_UNSUPPORTED_VALUE;
-        Prepared q;
         RTB_TRY(prepare_launch(ctx, L, q));
         Plan pl;
         pl.bn = 128;
         pl.nbuf = 2;
-        return launch_plan(ctx, L, q, pl, getenv("RTEN_B200_VERBOSE") != nullptr);
+        return launch_plan(ctx, L, q, pl, verbose);
     }
     if (L.kind == 0 && ctx->f32_mode == RTEN_F32_TF32X3) return launch_tf32x3(ctx, L);
-    // stride-1 windows (the 3x3 layers): the halo-reuse kernel moves the activations into shared memory once per channel
-    // block instead of once per filter tap (umma_halo.cu); everything it does not cover falls through
-    if (L.conv && L.kind == 0 && L.g.kh * L.g.kw > 1 && !L.x3_cb && !L.proj.C) {
-        const rten_status hs = launch_umma_halo_conv(ctx, L);
+    // RTEN_B200_HALO=1: the halo kernel's model shape without measurements.  Otherwise only a measurement picks the halo
+    // kernel: which of the two kernels is faster depends on the layer.
+    int hbn, hT;
+    if (halo && halo_on && atoi(halo_on) != 0 && halo_model_shape(ctx, L, hbn, hT)) {
+        const rten_status hs = run_plan(ctx, L, q, halo_plan(hbn, hT), verbose);
         if (hs != RTEN_ERR_UNSUPPORTED_VALUE) return hs;
     }
-    Prepared q;
     RTB_TRY(prepare_launch(ctx, L, q));
-    const bool verbose = getenv("RTEN_B200_VERBOSE") != nullptr;
-    const bool forced = getenv("RTEN_B200_FORCE_BN") || getenv("RTEN_B200_FORCE_SPLITK");
+    const bool forced = force_bn || force_sk;
     if (!forced && !ctx->tune_cache.empty()) {  // measured plan on record: no need to enumerate and rank candidates
         auto hit = ctx->tune_cache.find(tune_key(L, q));
         if (hit != ctx->tune_cache.end()) {
+            const Plan pl = plan_from_record(hit->second);
             PlanShape ps;
-            if (hit->second[0] < 0) {  // the halo-reuse kernel measured faster: {-1, bn, T}
-                const rten_status hs = launch_umma_halo_conv(ctx, L, hit->second[1], hit->second[2]);
-                if (hs != RTEN_ERR_UNSUPPORTED_VALUE) return hs;
-            } else
-            if (plan_shape(q, plan_from_array(hit->second), ps)) return launch_plan(ctx, L, q, plan_from_array(hit->second), verbose);
+            if (pl.halo ? halo && halo_shape_fits(L, pl.bn, pl.T) : plan_shape(q, pl, ps)) return run_plan(ctx, L, q, pl, verbose);
             // a stale entry (plans file written by another build / geometry): drop it and plan afresh
             if (verbose) fprintf(stderr, "[umma_gemm] recorded plan no longer valid for this problem: re-planning\n");
             ctx->tune_cache.erase(hit);
@@ -730,16 +891,13 @@ rten_status launch_umma_gemm(rten_ctx* ctx, const GemmLaunch& L) {
     enumerate_plans(q, ctx->num_sms, cands);
     if (cands.empty()) return RTEN_ERR_UNSUPPORTED_VALUE;
     Plan plan = cands[0].second;
-
     if (forced) {
         // debugging / sweeps: the best-ranked candidate that matches every forced field
-        const char* fb = getenv("RTEN_B200_FORCE_BN");
-        const char* fs = getenv("RTEN_B200_FORCE_SPLITK");
         bool found = false;
         for (const auto& c : cands) {
             const Plan& x = c.second;
-            if (fb && x.bn != atoi(fb)) continue;
-            if (fs && x.splitk != atoi(fs)) continue;
+            if (force_bn && x.bn != atoi(force_bn)) continue;
+            if (force_sk && x.splitk != atoi(force_sk)) continue;
             plan = x;
             found = true;
             break;
@@ -754,119 +912,10 @@ rten_status launch_umma_gemm(rten_ctx* ctx, const GemmLaunch& L) {
         } else {
             ctx->forced_hits++;
         }
-    } else if (ctx->autotune || !ctx->tune_cache.empty()) {
-        // measured plans are used whenever they exist; new measurements are only taken while autotuning is on
-        const std::vector<long long> key = tune_key(L, q);
-        auto it = ctx->tune_cache.find(key);
-        PlanShape ps_hit;
-        if (it != ctx->tune_cache.end() && it->second[0] < 0) {
-            const rten_status hs = launch_umma_halo_conv(ctx, L, it->second[1], it->second[2]);
-            if (hs != RTEN_ERR_UNSUPPORTED_VALUE) return hs;
-            ctx->tune_cache.erase(it);
-        } else if (it != ctx->tune_cache.end() && plan_shape(q, plan_from_array(it->second), ps_hit)) {
-            plan = plan_from_array(it->second);
-        } else if (ctx->autotune) {
-            cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-            cudaStreamIsCapturing(ctx->stream, &cs);
-            // re-running the launch must be idempotent: the output may not alias the residual
-            const bool safe = !ctx->capturing && cs == cudaStreamCaptureStatusNone &&
-                              (L.epi.r == nullptr || (const void*)L.epi.r != (const void*)L.epi.d);
-            if (safe) {
-                cudaEvent_t e0, e1;
-                cudaEventCreate(&e0);
-                cudaEventCreate(&e1);
-                const size_t ncand = std::min<size_t>(cands.size(), 24);
-                // one split-K workspace for every candidate (allocating inside the timed launches would time cudaMalloc)
-                size_t ws_max = 0;
-                for (size_t i = 0; i < ncand; i++) {
-                    PlanShape ps;
-                    if (plan_shape(q, cands[i].second, ps)) ws_max = std::max(ws_max, splitk_ws_bytes(ps, cands[i].second));
-                }
-                void* ws = nullptr;
-                if (ws_max) {
-                    RTB_TRY(ensure_splitk_counters(ctx));
-                    RTB_TRY(temp_alloc(ctx, ws_max, &ws));
-                    cudaStreamSynchronize(ctx->stream);
-                }
-                double best_ms = 1e30;
-                int reps = 4;  // raised after the first candidate so that every timed window is >= ~150 us (event resolution)
-                std::vector<std::pair<double, size_t>> timed;
-                auto time_plan = [&](const Plan& x, int n) -> double {
-                    if (launch_plan(ctx, L, q, x, false, ws) != RTEN_OK) return -1.0;  // warm-up (also validates the plan)
-                    cudaEventRecord(e0, ctx->stream);
-                    bool ok = true;
-                    for (int r = 0; r < n && ok; r++) ok = launch_plan(ctx, L, q, x, false, ws) == RTEN_OK;
-                    cudaEventRecord(e1, ctx->stream);
-                    if (cudaEventSynchronize(e1) != cudaSuccess || !ok) return -1.0;
-                    float t = 0.f;
-                    cudaEventElapsedTime(&t, e0, e1);
-                    return (double)t / n;
-                };
-                for (size_t i = 0; i < ncand; i++) {
-                    const Plan& x = cands[i].second;
-                    double ms = time_plan(x, reps);
-                    if (ms < 0) continue;
-                    timed.emplace_back(ms, i);
-                    if (verbose)
-                        fprintf(stderr, "[autotune] bn=%d splitk=%d nbuf=%d model=%.0f -> %.2f us\n", x.bn, x.splitk, x.nbuf,
-                                cands[i].first, ms * 1e3);
-                    if (ms < best_ms) {
-                        best_ms = ms;
-                        plan = x;
-                    }
-                    reps = std::max(4, std::min(32, (int)(0.15 / std::max(best_ms, 1e-3))));
-                }
-                // second look at the three fastest with longer windows: single measurements of 20-40 us kernels are noisy
-                // enough to flip the choice between near-equal plans from run to run
-                std::sort(timed.begin(), timed.end());
-                best_ms = 1e30;
-                for (size_t k = 0; k < std::min<size_t>(3, timed.size()); k++) {
-                    const Plan& x = cands[timed[k].second].second;
-                    const double again = time_plan(x, 2 * reps);
-                    const double ms = again < 0 ? timed[k].first : again;  // the longer window decides
-                    if (ms < best_ms) {
-                        best_ms = ms;
-                        plan = x;
-                    }
-                }
-                // stride-1 windows: the halo-reuse kernel (umma_halo.cu) over a few unit shapes, same timing
-                int halo_bn = 0, halo_T = 0;
-                if (L.conv && L.kind == 0 && L.g.kh * L.g.kw > 1 && !L.x3_cb && !L.proj.C && !getenv("RTEN_B200_NO_HALO")) {
-                    for (int hbn : {32, 64, 128})  // the halo kernel's unit shapes: 128 or 256 slots, bn <= 64 at 128
-                        for (int hT : {1, 2}) {
-                            if (hbn > L.N || (hT == 1 && hbn > 64)) continue;
-                            auto time_halo = [&](int n) -> double {
-                                if (launch_umma_halo_conv(ctx, L, hbn, hT) != RTEN_OK) return -1.0;
-                                cudaEventRecord(e0, ctx->stream);
-                                bool ok = true;
-                                for (int r = 0; r < n && ok; r++) ok = launch_umma_halo_conv(ctx, L, hbn, hT) == RTEN_OK;
-                                cudaEventRecord(e1, ctx->stream);
-                                if (cudaEventSynchronize(e1) != cudaSuccess || !ok) return -1.0;
-                                float t = 0.f;
-                                cudaEventElapsedTime(&t, e0, e1);
-                                return (double)t / n;
-                            };
-                            double ms = time_halo(reps);
-                            if (ms > 0 && ms < best_ms * 1.05) ms = time_halo(2 * reps);  // a second, longer look at contenders
-                            if (verbose && ms > 0) fprintf(stderr, "[autotune] halo bn=%d T=%d -> %.2f us\n", hbn, hT, ms * 1e3);
-                            if (ms > 0 && ms < best_ms * 0.97) {  // must win clearly: the generic kernel is the better-trodden path
-                                best_ms = ms;
-                                halo_bn = hbn;
-                                halo_T = hT;
-                            }
-                        }
-                }
-                cudaEventDestroy(e0);
-                cudaEventDestroy(e1);
-                if (halo_bn) {
-                    ctx->tune_cache[key] = {-1, halo_bn, halo_T};
-                    return launch_umma_halo_conv(ctx, L, halo_bn, halo_T);
-                }
-                ctx->tune_cache[key] = {plan.bn, plan.splitk, plan.nbuf};
-            }
-        }
+    } else if (ctx->autotune) {
+        RTB_TRY(autotune(ctx, L, q, cands, halo, verbose, plan));
     }
-    return launch_plan(ctx, L, q, plan, verbose);
+    return run_plan(ctx, L, q, plan, verbose);
 }
 
 }  // namespace rtb

@@ -122,9 +122,18 @@ bool encode_map(rten_ctx* ctx, CUtensorMap* map, const OperandDesc& od, int esiz
                 const uint32_t estr[4]);
 
 // Stride-1 convolutions with a kh x kw > 1 window on the halo-reuse kernel (umma_halo.cu): one activation patch per
-// channel block in shared memory, every filter tap a shifted window of it.  RTEN_ERR_UNSUPPORTED_VALUE = not applicable
-// (the caller then takes the generic implicit-GEMM kernel).
-rten_status launch_umma_halo_conv(rten_ctx* ctx, const GemmLaunch& L, int force_bn = 0, int force_T = 0);
+// channel block in shared memory, every filter tap a shifted window of it.  Its unit shapes {bn, T}: bn output channels
+// x T tiles of 128 pixel slots (T = 1: one m64 half per consumer warpgroup, bn <= 64; T = 2: two halves).
+constexpr int HALO_SHAPES[5][2] = {{32, 1}, {32, 2}, {64, 1}, {64, 2}, {128, 2}};
+bool halo_shape_fits(const GemmLaunch& L, int bn, int T);  // the halo kernel can run L with unit shape (bn, T)
+// The unit shape the halo kernel's cost model ranks first for L; false if no shape fits.
+bool halo_model_shape(rten_ctx* ctx, const GemmLaunch& L, int& bn, int& T);
+// RTEN_ERR_UNSUPPORTED_VALUE if the shape does not fit L.
+rten_status launch_umma_halo_conv(rten_ctx* ctx, const GemmLaunch& L, int bn, int T, bool verbose);
+
+// The plans file (RTEN_B200_TUNE_FILE, rten_b200_save_plans / rten_b200_load_plans): ctx->tune_cache as text.
+void tune_cache_load(rten_ctx* ctx, const char* path);
+void tune_cache_save(rten_ctx* ctx, const char* path);
 
 // true if `od` can be fed to TMA directly (16-B aligned base and strides, inner stride 1).
 bool tma_compatible(const OperandDesc& od, int esize, int rank);

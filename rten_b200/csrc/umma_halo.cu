@@ -281,26 +281,22 @@ umma_halo_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
 
 }  // namespace
 
-// force_bn / force_T > 0: that unit shape or RTEN_ERR_UNSUPPORTED_VALUE (the autotuner times a few of them against the
-// generic kernel's plans and records the winner); 0: the cost model's choice, and only with RTEN_B200_HALO=1 -- without
-// measurements the generic kernel stays the default (which of the two is faster depends on the layer).
-rten_status launch_umma_halo_conv(rten_ctx* ctx, const GemmLaunch& L, int force_bn, int force_T) {
-    if (getenv("RTEN_B200_NO_HALO")) return RTEN_ERR_UNSUPPORTED_VALUE;
-    if (!force_bn) {
-        const char* on = getenv("RTEN_B200_HALO");
-        if (!on || atoi(on) == 0) return RTEN_ERR_UNSUPPORTED_VALUE;
-    }
-    if (!L.conv || L.kind != 0) return RTEN_ERR_UNSUPPORTED_VALUE;
+// The kernel's parameters for unit shape (bn, T) (one of HALO_SHAPES) of launch L, or false where the kernel cannot
+// take L or that unit does not fit it.  A unit covers whole images (tb >= 1 images of OH + kh - 1 patch rows) when they
+// fit T tiles, else a strip of R rows of one image.
+static bool halo_params(const GemmLaunch& L, int bn, int T, HaloParams& p) {
+    bool listed = false;
+    for (const auto& s : HALO_SHAPES) listed = listed || (s[0] == bn && s[1] == T);
+    if (!listed || !L.conv || L.kind != 0) return false;
     const ConvGeom& g = L.g;
     const EpilogueDesc& e = L.epi;
-    if (g.sy != 1 || g.sx != 1 || g.dy != 1 || g.dx != 1 || g.kh * g.kw < 2 || g.kh * g.kw > 32) return RTEN_ERR_UNSUPPORTED_VALUE;
-    if (g.C % 32 || g.C < 32) return RTEN_ERR_UNSUPPORTED_VALUE;
-    if (L.N % 32 || L.N < 32) return RTEN_ERR_UNSUPPORTED_VALUE;
-    if (e.r || e.range || e.bias_kind == 2 || e.act > 1 || e.s_col != 1 || e.d_is_i32 || e.alpha != 1.0f) return RTEN_ERR_UNSUPPORTED_VALUE;
+    if (g.sy != 1 || g.sx != 1 || g.dy != 1 || g.dx != 1 || g.kh * g.kw < 2 || g.kh * g.kw > 32) return false;
+    if (g.C % 32 || g.C < 32) return false;
+    if (L.N < bn || L.N % bn) return false;
+    if (e.r || e.range || e.bias_kind == 2 || e.act > 1 || e.s_col != 1 || e.d_is_i32 || e.alpha != 1.0f) return false;
     auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-    if (!al16(e.d) || (e.s_z0 & 3) || (e.s_row & 3) || (e.s_z1 & 3) || (e.bias_kind == 1 && !al16(e.bias))) return RTEN_ERR_UNSUPPORTED_VALUE;
-    if (!tma_compatible(L.a, 4, 4) || !tma_compatible(L.b, 4, 4)) return RTEN_ERR_UNSUPPORTED_VALUE;
-    HaloParams p;
+    if (!al16(e.d) || (e.s_z0 & 3) || (e.s_row & 3) || (e.s_z1 & 3) || (e.bias_kind == 1 && !al16(e.bias))) return false;
+    if (!tma_compatible(L.a, 4, 4) || !tma_compatible(L.b, 4, 4)) return false;
     memset(&p, 0, sizeof(p));
     p.B = g.B;
     p.OH = g.OH;
@@ -315,96 +311,89 @@ rten_status launch_umma_halo_conv(rten_ctx* ctx, const GemmLaunch& L, int force_
     p.c_blocks = g.C / 32;
     p.taps = g.kh * g.kw;
     p.epi = e;
-    if (p.P > 256) return RTEN_ERR_UNSUPPORTED_VALUE;
-    // ---- unit shape.  Candidates: output-channel tile bn, 128-slot tiles T per unit (T = 1: one m64 half per consumer,
-    // bn <= 64; T = 2: two halves per consumer), whole images (tb >= 1 images of OH + kh - 1 patch rows) or row strips
-    // (R rows of one image).  Ranked by waves x (clocks of a unit), with the slots that are thrown away counted in.
-    const int num_sms = ctx->num_sms;
-    double best = 1e30;
-    int bbn = 0, bT = 0, bR = 0, btb = 0;
-    const char* fbn = getenv("RTEN_B200_HALO_BN");
-    const char* fT = getenv("RTEN_B200_HALO_T");
-    const int want_bn = force_bn ? force_bn : (fbn ? atoi(fbn) : 0), want_T = force_T ? force_T : (fT ? atoi(fT) : 0);
-    for (int bn = 32; bn <= std::min(L.N, 128); bn *= 2) {
-        if (L.N % bn) continue;
-        if (want_bn && bn != want_bn) continue;
-        for (int T = 1; T <= 2; T++) {
-            if (want_T && T != want_T) continue;
-            if (T == 1 && bn > 64) continue;  // (a 64-slot half per consumer: the wide columns go to T = 2)
-            // whole-image mode when tb >= 1 padded images fit T tiles, else strips of R rows
-            const int img_slots = (g.OH + g.kh - 1) * p.P;
-            int tb = 1, R = 0;
-            if (g.OH * p.P <= T * 128) {
-                R = g.OH;
-                tb = 1 + (T * 128 - g.OH * p.P) / img_slots;
-                tb = std::min(tb, g.B);
-            } else {
-                R = (T * 128) / p.P;
-                if (R < 1) continue;
-            }
-            const int nr = R + g.kh - 1;
-            if (nr > 256 || tb > 256) continue;
-            const long long alloc_slots = (long long)T * 128 + (g.kh - 1) * p.P + g.kw - 1;
-            const long long loaded_slots = (long long)tb * nr * p.P;
-            const long long patch_bytes = (std::max(alloc_slots, loaded_slots) * 128 + 1023) / 1024 * 1024;
-            // a weight stage must be requested ~1500 clk (TMA latency + its own transfer) before its MMAs start: at least
-            // three stages in flight beside the two patches
-            const long long budget = HALO_SMEM_MAX - HALO_FIXED_BYTES - 2 * patch_bytes;
-            if ((long long)bn * 128 * 3 > budget) continue;
-            const long long strips = (g.OH + R - 1) / R;
-            const long long units = strips * ((g.B + tb - 1) / tb) * (L.N / bn);
-            const double waves = std::ceil((double)units / num_sms);
-            // per unit: MMA clocks (c_blocks x taps stages of 2 T m64 instructions x 4 k8 steps, bn / 2 clocks each, plus a
-            // fixed cost per stage) vs the operand bytes entering the SM, then the epilogue (bn columns of 128 T slots
-            // through the staging buffers).  The clock and bandwidth constants are unmeasured estimates that only rank the
-            // candidate shapes.
-            const double mma = (double)p.c_blocks * p.taps * (8.0 * T * std::max(16.0, bn / 2.0) + 60.0);
-            const double bytes = (double)p.c_blocks * (loaded_slots * 128.0 + (double)p.taps * bn * 128.0);
-            const double ingest = bytes / 55.0;
-            const double epi = (double)T * 128 * bn * 4 / 16.0;
-            const double unit = std::max(mma, ingest) + epi + 800.0;
-            const double cost = waves * unit + 4000.0;
-            if (cost < best) {
-                best = cost;
-                bbn = bn;
-                bT = T;
-                bR = R;
-                btb = tb;
-            }
-        }
+    if (p.P > 256) return false;
+    int tb = 1, R = 0;
+    if (g.OH * p.P <= T * 128) {
+        R = g.OH;
+        tb = std::min(1 + (T * 128 - g.OH * p.P) / ((g.OH + g.kh - 1) * p.P), g.B);
+    } else {
+        R = (T * 128) / p.P;
+        if (R < 1) return false;
     }
-    if (!bbn) return RTEN_ERR_UNSUPPORTED_VALUE;
-    p.bn = bbn;
-    p.T = bT;
-    p.R = bR;
-    p.tb = btb;
-    p.nr = p.R + g.kh - 1;
-    p.strips = (g.OH + p.R - 1) / p.R;
-    p.units_n = L.N / p.bn;
-    p.units_total = p.strips * ((g.B + p.tb - 1) / p.tb) * p.units_n;
-    const long long alloc_slots = (long long)p.T * 128 + (g.kh - 1) * p.P + g.kw - 1;
-    const long long loaded_slots = (long long)p.tb * p.nr * p.P;
-    p.patch_bytes = (uint32_t)((std::max(alloc_slots, loaded_slots) * 128 + 1023) / 1024 * 1024);
+    const int nr = R + g.kh - 1;
+    if (nr > 256 || tb > 256) return false;
+    const long long alloc_slots = (long long)T * 128 + (g.kh - 1) * p.P + g.kw - 1;
+    const long long loaded_slots = (long long)tb * nr * p.P;
+    const long long patch_bytes = (std::max(alloc_slots, loaded_slots) * 128 + 1023) / 1024 * 1024;
+    // a weight stage must be requested ~1500 clk (TMA latency + its own transfer) before its MMAs start: at least
+    // three stages in flight beside the two patches
+    const long long budget = HALO_SMEM_MAX - HALO_FIXED_BYTES - 2 * patch_bytes;
+    if ((long long)bn * 128 * 3 > budget) return false;
+    p.bn = bn;
+    p.T = T;
+    p.R = R;
+    p.tb = tb;
+    p.nr = nr;
+    p.strips = (g.OH + R - 1) / R;
+    p.units_n = L.N / bn;
+    p.units_total = p.strips * ((g.B + tb - 1) / tb) * p.units_n;
+    p.patch_bytes = (uint32_t)patch_bytes;
     p.patch_tx = (uint32_t)(loaded_slots * 128);
-    p.b_bytes = (uint32_t)p.bn * 128u;
-    p.b_stages = (int)std::min<long long>(HB_MAX, (HALO_SMEM_MAX - HALO_FIXED_BYTES - 2LL * p.patch_bytes) / p.b_bytes);
+    p.b_bytes = (uint32_t)bn * 128u;
+    p.b_stages = (int)std::min<long long>(HB_MAX, budget / p.b_bytes);
     for (int ky = 0; ky < g.kh; ky++)
         for (int kx = 0; kx < g.kw; kx++) p.tap_off[ky * g.kw + kx] = (uint32_t)((ky * p.P + kx) * 128);
     p.m_img = (uint32_t)(0x100000000ull / (unsigned long long)(p.nr * p.P)) + 1u;
     p.m_P = (uint32_t)(0x100000000ull / (unsigned long long)p.P) + 1u;
+    return true;
+}
 
+bool halo_shape_fits(const GemmLaunch& L, int bn, int T) {
+    HaloParams p;
+    return halo_params(L, bn, T, p);
+}
+
+// Ranked by waves x (clocks of a unit), with the slots that are thrown away counted in.  Per unit: MMA clocks (c_blocks
+// x taps stages of 2 T m64 instructions x 4 k8 steps, bn / 2 clocks each, plus a fixed cost per stage) vs the operand
+// bytes entering the SM, then the epilogue (bn columns of 128 T slots through the staging buffers).  The clock and
+// bandwidth constants are unmeasured estimates that only rank the candidate shapes.
+bool halo_model_shape(rten_ctx* ctx, const GemmLaunch& L, int& bn, int& T) {
+    double best = 1e30;
+    bn = T = 0;
+    for (const auto& s : HALO_SHAPES) {
+        HaloParams p;
+        if (!halo_params(L, s[0], s[1], p)) continue;
+        const double waves = std::ceil((double)p.units_total / ctx->num_sms);
+        const double mma = (double)p.c_blocks * p.taps * (8.0 * p.T * std::max(16.0, p.bn / 2.0) + 60.0);
+        const double bytes = (double)p.c_blocks * ((double)p.patch_tx + (double)p.taps * p.bn * 128.0);
+        const double ingest = bytes / 55.0;
+        const double epi = (double)p.T * 128 * p.bn * 4 / 16.0;
+        const double unit = std::max(mma, ingest) + epi + 800.0;
+        const double cost = waves * unit + 4000.0;
+        if (cost < best) {
+            best = cost;
+            bn = p.bn;
+            T = p.T;
+        }
+    }
+    return bn != 0;
+}
+
+rten_status launch_umma_halo_conv(rten_ctx* ctx, const GemmLaunch& L, int bn, int T, bool verbose) {
+    HaloParams p;
+    if (!halo_params(L, bn, T, p)) return RTEN_ERR_UNSUPPORTED_VALUE;
     uint32_t abox[4] = {32u, (uint32_t)p.P, (uint32_t)p.nr, (uint32_t)p.tb}, ones[4] = {1, 1, 1, 1};
     uint32_t bbox[4] = {32u, (uint32_t)p.bn, 1u, 1u};
     CUtensorMap map_a, map_b;
     if (!encode_map(ctx, &map_a, L.a, 4, true, abox, ones)) return RTEN_ERR_UNSUPPORTED_VALUE;
     if (!encode_map(ctx, &map_b, L.b, 4, true, bbox, ones)) return RTEN_ERR_UNSUPPORTED_VALUE;
-    if (getenv("RTEN_B200_VERBOSE"))
-        fprintf(stderr, "[umma_halo] B=%d %dx%d C=%d N=%d k=%dx%d: bn=%d T=%d R=%d tb=%d P=%d units=%d b_stages=%d patch=%u B\n", g.B,
-                g.OH, g.OW, g.C, L.N, g.kh, g.kw, p.bn, p.T, p.R, p.tb, p.P, p.units_total, p.b_stages, p.patch_bytes);
+    if (verbose)
+        fprintf(stderr, "[umma_halo] B=%d %dx%d C=%d N=%d k=%dx%d: bn=%d T=%d R=%d tb=%d P=%d units=%d b_stages=%d patch=%u B\n", p.B,
+                p.OH, p.OW, p.C, p.N, p.kh, p.kw, p.bn, p.T, p.R, p.tb, p.P, p.units_total, p.b_stages, p.patch_bytes);
     const size_t smem = HALO_FIXED_BYTES + 2 * (size_t)p.patch_bytes + (size_t)p.b_stages * p.b_bytes;
     auto kern = p.T == 1 ? (p.bn == 32 ? umma_halo_kernel<32, 1> : umma_halo_kernel<64, 1>)
                          : (p.bn == 32 ? umma_halo_kernel<32, 2> : p.bn == 64 ? umma_halo_kernel<64, 2> : umma_halo_kernel<128, 2>);
-    return launch(ctx, "umma_halo launch", kern, {std::min(p.units_total, num_sms), HALO_THREADS, smem, HALO_SMEM_MAX, true},
+    return launch(ctx, "umma_halo launch", kern, {std::min(p.units_total, ctx->num_sms), HALO_THREADS, smem, HALO_SMEM_MAX, true},
                   map_a, map_b, p);
 }
 
