@@ -1,10 +1,9 @@
 // Minimal graph executor behind the C ABI (include/rten_b200.h: rten_b200_model_*): what RTen's `Model::load` +
 // `Graph::run_plan` do around the operators of this library (src/model.rs, src/graph.rs:880-1286), restated for the
 // hot-path operator set:
-//   load : ONNX bytes -> nodes + initialisers (onnx_reader.cu; int64 tensors become i32 like rten's loader does) ->
-//          constants uploaded to HBM once -> load-time fusions (Mul(x, Sigmoid(x)) -> Silu, then Conv + activation
-//          and MatMul + Add(bias): the subset of src/optimize.rs the models need) -> weights prepacked once
-//          (`Operator::prepack`, src/graph.rs:488-565).
+//   load : build_graph (ONNX bytes -> nodes + initialisers, onnx_reader.cu; int64 tensors become i32 like rten's loader
+//          does; constants uploaded to HBM once) -> the fusions of src/optimize.rs the models need, in this order:
+//          fuse_silu, fuse_group_norm, fuse_into_producers -> plan_concat_elision -> prepack_weights (src/graph.rs:488-565).
 //   run  : the nodes in topological (file) order, one C-ABI operator call each; temporaries are reference counted and
 //          returned to the context pool after their last consumer (src/graph.rs:1100-1180); an operator that can run in
 //          place does so when the executor holds the last reference to its input (src/graph.rs:973-1049); shape-only
@@ -98,8 +97,8 @@ struct OpNode {
     const OpDef* def = nullptr;
     std::vector<int> in, out;  // value ids (-1 = absent optional input)
     rten_packed* packed = nullptr;
-    rten_activation activation = {RTEN_ACT_NONE, 0.0f, 0.0f};  // fused activation of a Conv
-    int bias_value = -1;       // fused Add(bias) of a MatMul
+    rten_activation activation = {RTEN_ACT_NONE, 0.0f, 0.0f};  // fused activation of a Conv or GroupNorm
+    int bias_value = -1;       // fused Add(bias) of a MatMul (fuse_into_producers)
     // Concat elision (plan_concat_elision).  On a Concat: the channel count of every input and whether its producer
     // writes it in place.  On a producer: the Concat node and the input slot its output is written into.
     std::vector<int64_t> cat_channels;
@@ -149,8 +148,9 @@ int dtype_of(int32_t onnx_dt) {
 }
 
 // initialiser / Constant tensor -> device constant (int64 narrowed to i32, the only integer width of the path)
-rten_status upload_constant(rten_model* m, const onnx::Tensor& t, ValueSlot* v) {
+rten_status upload_constant(rten_model* m, const onnx::Tensor& t) {
     rten_ctx* ctx = m->ctx;
+    ValueSlot* v = &m->values[(size_t)m->value_id(t.name)];
     const int dt = dtype_of(t.data_type);
     if (dt < 0) return mfail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported tensor type in initializer '" + t.name + "'");
     if (t.external) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "external tensor data is not supported ('" + t.name + "')");
@@ -218,8 +218,7 @@ rten_status attr_to_input(rten_model* m, onnx::Node& n, const char* attr, size_t
     if (!scalar) t.dims = {(int64_t)v.size()};
     t.data.resize(v.size() * 4);
     if (!v.empty()) memcpy(t.data.data(), v.data(), t.data.size());
-    const int id = m->value_id(t.name);
-    RTB_TRY(upload_constant(m, t, &m->values[(size_t)id]));
+    RTB_TRY(upload_constant(m, t));
     if (n.inputs.size() <= slot) n.inputs.resize(slot + 1);
     n.inputs[slot] = t.name;
     return RTEN_OK;
@@ -1227,6 +1226,286 @@ constexpr const OpDef *CONV = row("Conv"), *CONV_TRANSPOSE = row("ConvTranspose"
 static_assert(CONV && CONV_TRANSPOSE && CONCAT && SIGMOID && MUL && SILU && MATMUL && ADD && RESHAPE_OP && INSTANCE_NORM && GROUP_NORM,
               "a row the load looks for is missing");
 
+// the decoded file as values and nodes: constants uploaded, every node checked against OPS
+rten_status build_graph(rten_model* m, const onnx::Model& om) {
+    rten_ctx* ctx = m->ctx;
+    m->summary = onnx::summary_json(om);
+    for (const onnx::Tensor& t : om.graph.initializers) RTB_TRY(upload_constant(m, t));
+    {
+        void* d = nullptr;
+        RTB_TRY(pool_alloc(ctx, 16, &d));
+        m->const_allocs.push_back(d);
+        const float one = 1.0f;
+        RTB_CUDA(ctx, cudaMemcpy(d, &one, 4, cudaMemcpyHostToDevice));
+        m->one = (float*)d;
+    }
+    for (const onnx::ValueInfo& vi : om.graph.inputs) {
+        const int id = m->value_id(vi.name);
+        if (m->values[(size_t)id].kind == V_CONST) continue;  // (old exporters list initialisers among the inputs)
+        m->values[(size_t)id].kind = V_INPUT;
+        m->inputs.push_back(id);
+    }
+    // nodes (the file order is topological: onnx.proto3 requires it, like src/model.rs relies on)
+    for (const onnx::Node& n : om.graph.nodes) {
+        if (!n.domain.empty() && n.domain != "ai.onnx" && n.domain != "com.microsoft")
+            return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "unsupported operator domain '" + n.domain + "'");
+        // (domain, op_type) as the reference's registry looks it up (src/op_registry/onnx_registry.rs read_op)
+        const OpDomain domain = n.domain == "com.microsoft" ? MS : ONNX;
+        const OpDef* def = nullptr;
+        for (const OpDef& d : OPS)
+            if (n.op_type == d.name && (d.domains & domain)) def = &d;
+        if (!def)
+            return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "unsupported operator " + std::string(domain == MS ? "com.microsoft." : "") + n.op_type);
+        if (n.op_type == "Constant") {
+            const onnx::Attribute* a = n.attr("value");
+            if (!a || !a->has_t || n.outputs.size() != 1) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Constant without a tensor value");
+            onnx::Tensor t = a->t;
+            t.name = n.outputs[0];
+            RTB_TRY(upload_constant(m, t));
+            continue;
+        }
+        OpNode on;
+        on.n = n;
+        on.def = def;
+        if (def->load) RTB_TRY(def->load(m, on.n));
+        for (const std::string& s : on.n.inputs) {
+            const int id = m->value_id(s);
+            if (id >= 0 && m->values[(size_t)id].kind == V_UNSET)
+                return mfail(ctx, RTEN_ERR_INVALID_VALUE, "node '" + n.name + "' (" + n.op_type + ") reads '" + s + "' before it is produced");
+            on.in.push_back(id);
+        }
+        for (const std::string& s : n.outputs) {
+            const int id = m->value_id(s);
+            if (id >= 0) m->values[(size_t)id].kind = V_TEMP;
+            on.out.push_back(id);
+        }
+        m->nodes.push_back(on);
+    }
+    for (const onnx::ValueInfo& vi : om.graph.outputs) {
+        auto it = m->by_name.find(vi.name);
+        if (it == m->by_name.end() || m->values[(size_t)it->second].kind == V_UNSET)
+            return mfail(ctx, RTEN_ERR_INVALID_VALUE, "graph output '" + vi.name + "' is never produced");
+        m->outputs.push_back(it->second);
+    }
+    return RTEN_OK;
+}
+
+// ---- load-time passes (src/optimize.rs: the patterns the hot-path models contain)
+// Who reads and who writes each value, over the nodes not absorbed: built when a fusion starts and again after each
+// rewrite, never updated in place.
+struct Uses {
+    std::vector<int> uses;                  // the input slots that name the value, plus its places among the graph outputs
+    std::vector<OpNode*> reader, producer;  // a node that reads it (the only one when uses == 1); the first that writes it
+    explicit Uses(rten_model& m) : uses(m.values.size()), reader(m.values.size()), producer(m.values.size()) {
+        for (OpNode& o : m.nodes) {
+            if (!o.def) continue;
+            for (int v : o.in)
+                if (v >= 0) uses[(size_t)v]++, reader[(size_t)v] = &o;
+            for (int v : o.out)
+                if (v >= 0 && !producer[(size_t)v]) producer[(size_t)v] = &o;
+        }
+        for (int v : m.outputs) uses[(size_t)v]++;
+    }
+    // the node that reads `v` when that read is v's only use, else nullptr
+    OpNode* sole_reader(int v) const { return v >= 0 && uses[(size_t)v] == 1 ? reader[(size_t)v] : nullptr; }
+};
+
+// One fusion: `fuse(node, uses)` on each node in order, true when it rewrote the graph.  It absorbs a node by clearing
+// its `def`; absorbed nodes are skipped, and dropped at the end, the others keeping their order.
+template <class Fuse>
+void fuse_each(rten_model* m, Fuse fuse) {
+    Uses u(*m);
+    for (OpNode& o : m->nodes)
+        if (o.def && fuse(o, u)) u = Uses(*m);
+    m->nodes.erase(std::remove_if(m->nodes.begin(), m->nodes.end(), [](const OpNode& o) { return !o.def; }), m->nodes.end());
+}
+
+// what activation node `a` computes, as a fused epilogue takes it
+rten_activation activation_of(const OpNode& a) {
+    const bool hs = a.def->act == RTEN_ACT_HARD_SIGMOID;
+    return {(int32_t)a.def->act, hs ? hard_sigmoid_alpha(a.n) : 0.0f, hs ? hard_sigmoid_beta(a.n) : 0.0f};
+}
+
+// SiluFusion (src/optimize/fusions.rs:567-588): Mul(x, Sigmoid(x)), either operand order, becomes Silu(x) in the Mul's
+// place when the Sigmoid's output has no other use; Silu rounds once where the pair rounds twice, as the reference's
+// Model::run does.  First: the Sigmoid and the Mul are two readers of a Conv's output, and GroupNormFusion takes the Silu.
+void fuse_silu(rten_model* m) {
+    fuse_each(m, [](OpNode& s, const Uses& u) {
+        if (s.def != SIGMOID || s.in.size() != 1 || s.out.size() != 1) return false;
+        OpNode* mul = u.sole_reader(s.out[0]);
+        if (!mul || mul->def != MUL || mul->in.size() != 2 || mul->out.size() != 1) return false;
+        const int x = s.in[0];
+        if (!((mul->in[0] == s.out[0] && mul->in[1] == x) || (mul->in[1] == s.out[0] && mul->in[0] == x))) return false;
+        mul->def = SILU;
+        mul->n.op_type = SILU->name;
+        mul->n.inputs = {s.n.inputs[0]};
+        mul->n.attrs.clear();
+        mul->in = {x};
+        s.def = nullptr;
+        return true;
+    });
+}
+
+// GroupNormFusion: torch's export of nn.GroupNorm(G, C) -- Reshape(x, [0 | N, G, -1]) -> InstanceNormalization(
+// scale [G], bias [G]) -> Reshape(to a constant 4-D shape) -> Mul(gamma [C, 1, 1]) -> Add(beta [C, 1, 1]), every
+// intermediate with one reader -- and a following Relu / Sigmoid / Silu / HardSigmoid / HardSwish become one GroupNorm
+// node in the last node's place: one pass over x instead of two copies, the norm and three elementwise launches.  The
+// Reshape targets stay inputs, resolved for each run's x.  Only constant targets match, not one computed from Shape(x).
+void fuse_group_norm(rten_model* m) {
+    auto cval = [&](int vid) -> const ValueSlot* {
+        return vid >= 0 && m->values[(size_t)vid].kind == V_CONST ? &m->values[(size_t)vid] : nullptr;
+    };
+    // a per-channel constant of C elements: [C], broadcast over the spatial axes, i.e. shape [.., C, 1, 1]
+    auto per_channel = [&](int vid, int64_t* C) {
+        const ValueSlot* v = cval(vid);
+        if (!v || v->t.dtype != RTEN_F32 || v->t.ndim < 3 || v->t.ndim > 4) return false;
+        const int nd = v->t.ndim;
+        if (v->t.shape[nd - 1] != 1 || v->t.shape[nd - 2] != 1 || (nd == 4 && v->t.shape[0] != 1)) return false;
+        *C = v->t.shape[nd - 3];
+        return true;
+    };
+    fuse_each(m, [&](OpNode& r1, const Uses& u) {
+        if (r1.def != RESHAPE_OP || r1.in.size() != 2 || r1.out.size() != 1 || r1.n.attr_i("allowzero", 0)) return false;
+        const ValueSlot* t1 = cval(r1.in[1]);
+        if (!t1 || !t1->has_host_ints || t1->host_ints.size() != 3 || t1->host_ints[0] < 0 || t1->host_ints[1] <= 0 ||
+            t1->host_ints[2] != -1)
+            return false;
+        const int64_t G = t1->host_ints[1];
+        OpNode* in = u.sole_reader(r1.out[0]);
+        if (!in || in->def != INSTANCE_NORM || in->in.size() != 3 || in->in[0] != r1.out[0] || in->out.size() != 1) return false;
+        const ValueSlot *sc = cval(in->in[1]), *bi = cval(in->in[2]);
+        if (!sc || !bi || sc->t.ndim != 1 || bi->t.ndim != 1 || sc->t.shape[0] != G || bi->t.shape[0] != G) return false;
+        OpNode* r2 = u.sole_reader(in->out[0]);
+        if (!r2 || r2->def != RESHAPE_OP || r2->in.size() != 2 || r2->in[0] != in->out[0] || r2->out.size() != 1 ||
+            r2->n.attr_i("allowzero", 0))
+            return false;
+        const ValueSlot* t2 = cval(r2->in[1]);
+        if (!t2 || !t2->has_host_ints || t2->host_ints.size() != 4) return false;
+        OpNode* mul = u.sole_reader(r2->out[0]);
+        if (!mul || mul->def != MUL || mul->in.size() != 2 || mul->out.size() != 1) return false;
+        const int gamma = mul->in[0] == r2->out[0] ? mul->in[1] : mul->in[0];
+        int64_t C = 0, Cb = 0;
+        if (gamma == r2->out[0] || !per_channel(gamma, &C) || C % G != 0) return false;
+        OpNode* add = u.sole_reader(mul->out[0]);
+        if (!add || add->def != ADD || add->in.size() != 2 || add->out.size() != 1) return false;
+        const int beta = add->in[0] == mul->out[0] ? add->in[1] : add->in[0];
+        if (beta == mul->out[0] || !per_channel(beta, &Cb) || Cb != C) return false;
+        OpNode* last = add;
+        OpNode* a = u.sole_reader(add->out[0]);
+        if (a && a->def->act != RTEN_ACT_NONE && a->in.size() == 1 && a->out.size() == 1) last = a;
+        in->def = GROUP_NORM;
+        in->n.op_type = GROUP_NORM->name;
+        in->in = {r1.in[0], in->in[1], in->in[2], gamma, beta, r1.in[1], r2->in[1]};
+        in->out = last->out;
+        if (last != add) in->activation = activation_of(*last);
+        *last = *in;  // (every input exists by then)
+        for (OpNode* o : {&r1, in, r2, mul, add})
+            if (o != last) o->def = nullptr;
+        return true;
+    });
+}
+
+// Conv + activation -> the activation in the convolution epilogue (Clip is not fused); MatMul + Add(constant vector over
+// the last axis) -> FusedMatMul with a row bias (MatMulAddFusion).  The Conv / MatMul takes the absorbed node's output.
+void fuse_into_producers(rten_model* m) {
+    fuse_each(m, [&](OpNode& a, const Uses& u) {
+        OpNode* b = a.out.size() == 1 ? u.sole_reader(a.out[0]) : nullptr;
+        if (b && a.def == CONV && a.activation.kind == RTEN_ACT_NONE && b->def->act != RTEN_ACT_NONE) {
+            a.activation = activation_of(*b);
+        } else if (b && a.def == MATMUL && b->def == ADD && a.bias_value < 0 && b->in.size() == 2) {
+            const int other = b->in[0] == a.out[0] ? b->in[1] : b->in[0];
+            const ValueSlot& bv = m->values[(size_t)other];
+            const ValueSlot& wv = m->values[(size_t)a.in[1]];
+            if (!(bv.kind == V_CONST && bv.t.dtype == RTEN_F32 && bv.t.ndim == 1 && wv.t.ndim >= 2 && wv.kind == V_CONST &&
+                  bv.t.shape[0] == wv.t.shape[wv.t.ndim - 1]))
+                return false;
+            a.bias_value = other;
+        } else {
+            return false;
+        }
+        a.out = b->out;
+        b->def = nullptr;
+        return true;
+    });
+}
+
+// Concat elision, decided once: which inputs of which channel Concat their producers write in place, reported as the
+// summary's "concat_in_place" member.  `inputs`: the file's graph inputs, whose dims give their channel counts.
+void plan_concat_elision(rten_model* m, const std::vector<onnx::ValueInfo>& inputs) {
+    const Uses u(*m);
+    std::map<std::string, std::vector<int64_t>> input_dims;
+    for (const onnx::ValueInfo& vi : inputs) input_dims[vi.name] = vi.dims;
+    // channels of a 4-D value as far as the file tells them, else -1
+    std::function<int64_t(int, int)> channels = [&](int vid, int depth) -> int64_t {
+        if (vid < 0 || depth > 64) return -1;
+        const ValueSlot& v = m->values[(size_t)vid];
+        if (v.kind == V_INPUT) {
+            const std::vector<int64_t>& d = input_dims[v.name];
+            return d.size() == 4 && d[1] > 0 ? d[1] : -1;
+        }
+        if (!u.producer[(size_t)vid]) return -1;
+        const OpNode& p = *u.producer[(size_t)vid];
+        auto weight = [&]() -> const rten_tensor* {
+            if (p.in.size() < 2 || p.in[1] < 0 || m->values[(size_t)p.in[1]].kind != V_CONST) return nullptr;
+            const rten_tensor& w = m->values[(size_t)p.in[1]].t;
+            return w.ndim == 4 ? &w : nullptr;
+        };
+        if (p.def == CONV) return weight() ? weight()->shape[0] : -1;
+        if (p.def == CONV_TRANSPOSE) return weight() ? weight()->shape[1] * p.n.attr_i("group", 1) : -1;
+        // the pools and Resize / Upsample (the other Concat-slice writers) and the elementwise operators
+        if (p.def->shape || (p.def->flags & IN_PLACE)) return channels(p.in[0], depth + 1);
+        if (p.def == CONCAT && p.n.attr_i("axis", 0) == 1) {
+            int64_t sum = 0;
+            for (int i : p.in) {
+                const int64_t c = channels(i, depth + 1);
+                if (c < 0) return -1;
+                sum += c;
+            }
+            return sum;
+        }
+        return -1;
+    };
+    std::string report;
+    for (size_t k = 0; k < m->nodes.size(); k++) {
+        OpNode& c = m->nodes[k];
+        if (c.def != CONCAT || c.n.attr_i("axis", 0) != 1 || c.out.size() != 1 || c.out[0] < 0 || u.uses[(size_t)c.out[0]] < 1) continue;
+        std::vector<int64_t> ch;
+        for (int i : c.in) ch.push_back(channels(i, 0));
+        if (std::find(ch.begin(), ch.end(), (int64_t)-1) != ch.end()) continue;
+        std::vector<char> mark(c.in.size(), 0);
+        std::string names;
+        for (size_t i = 0; i < c.in.size(); i++) {
+            const int vid = c.in[i];
+            if (m->values[(size_t)vid].kind != V_TEMP) continue;
+            if (std::count(c.in.begin(), c.in.end(), vid) != 1) continue;
+            if (std::find(m->outputs.begin(), m->outputs.end(), vid) != m->outputs.end()) continue;  // a graph output is copied
+            OpNode& p = *u.producer[(size_t)vid];
+            if (!p.def->shape || p.out.size() != 1 || p.cat_node >= 0) continue;
+            p.cat_node = (int)k;
+            p.cat_slot = (int)i;
+            mark[i] = 1;
+            names += (names.empty() ? "\"" : ",\"") + m->values[(size_t)vid].name + "\"";
+        }
+        if (names.empty()) continue;
+        c.cat_channels = ch;
+        c.cat_in_place = mark;
+        report += (report.empty() ? "" : ",") + std::string("{\"output\":\"") + m->values[(size_t)c.out[0]].name +
+                  "\",\"copied\":" + std::to_string(std::count(mark.begin(), mark.end(), 0)) + ",\"in_place\":[" + names + "]}";
+    }
+    // (the summary is the decoded file's JSON object: the plan is appended as one more member)
+    const size_t close = m->summary.rfind('}');
+    if (close != std::string::npos) m->summary.insert(close, ",\"concat_in_place\":[" + report + "]");
+}
+
+// constant weights prepacked once (`Operator::prepack`, src/graph.rs:488-565)
+rten_status prepack_weights(rten_model* m) {
+    for (OpNode& o : m->nodes) {
+        const int w = o.in.size() >= 2 ? o.in[1] : -1;
+        if (o.def->prepack && w >= 0 && m->values[(size_t)w].kind == V_CONST) RTB_TRY(o.def->prepack(m->ctx, o, m->values[(size_t)w].t));
+    }
+    return RTEN_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1263,292 +1542,12 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
     if (!om.has_graph) return mfail(ctx, RTEN_ERR_INVALID_VALUE, "ONNX model has no graph");
     std::unique_ptr<rten_model, void (*)(rten_model*)> m(new rten_model(), rten_b200_model_free);
     m->ctx = ctx;
-    m->summary = onnx::summary_json(om);
-    // constants
-    for (const onnx::Tensor& t : om.graph.initializers) {
-        const int id = m->value_id(t.name);
-        RTB_TRY(upload_constant(m.get(), t, &m->values[(size_t)id]));
-    }
-    {
-        void* d = nullptr;
-        RTB_TRY(pool_alloc(ctx, 16, &d));
-        m->const_allocs.push_back(d);
-        const float one = 1.0f;
-        RTB_CUDA(ctx, cudaMemcpy(d, &one, 4, cudaMemcpyHostToDevice));
-        m->one = (float*)d;
-    }
-    for (const onnx::ValueInfo& vi : om.graph.inputs) {
-        const int id = m->value_id(vi.name);
-        if (m->values[(size_t)id].kind == V_CONST) continue;  // (old exporters list initialisers among the inputs)
-        m->values[(size_t)id].kind = V_INPUT;
-        m->inputs.push_back(id);
-    }
-    // nodes (the file order is topological: onnx.proto3 requires it, like src/model.rs relies on)
-    for (const onnx::Node& n : om.graph.nodes) {
-        if (!n.domain.empty() && n.domain != "ai.onnx" && n.domain != "com.microsoft")
-            return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "unsupported operator domain '" + n.domain + "'");
-        // (domain, op_type) as the reference's registry looks it up (src/op_registry/onnx_registry.rs read_op)
-        const OpDomain domain = n.domain == "com.microsoft" ? MS : ONNX;
-        const OpDef* def = nullptr;
-        for (const OpDef& d : OPS)
-            if (n.op_type == d.name && (d.domains & domain)) def = &d;
-        if (!def)
-            return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "unsupported operator " + std::string(domain == MS ? "com.microsoft." : "") + n.op_type);
-        if (n.op_type == "Constant") {
-            const onnx::Attribute* a = n.attr("value");
-            if (!a || !a->has_t || n.outputs.size() != 1) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Constant without a tensor value");
-            onnx::Tensor t = a->t;
-            t.name = n.outputs[0];
-            const int id = m->value_id(t.name);
-            RTB_TRY(upload_constant(m.get(), t, &m->values[(size_t)id]));
-            continue;
-        }
-        OpNode on;
-        on.n = n;
-        on.def = def;
-        if (def->load) RTB_TRY(def->load(m.get(), on.n));
-        for (const std::string& s : on.n.inputs) {
-            const int id = m->value_id(s);
-            if (id >= 0 && m->values[(size_t)id].kind == V_UNSET)
-                return mfail(ctx, RTEN_ERR_INVALID_VALUE, "node '" + n.name + "' (" + n.op_type + ") reads '" + s + "' before it is produced");
-            on.in.push_back(id);
-        }
-        for (const std::string& s : n.outputs) {
-            const int id = m->value_id(s);
-            if (id >= 0) m->values[(size_t)id].kind = V_TEMP;
-            on.out.push_back(id);
-        }
-        m->nodes.push_back(on);
-    }
-    for (const onnx::ValueInfo& vi : om.graph.outputs) {
-        auto it = m->by_name.find(vi.name);
-        if (it == m->by_name.end() || m->values[(size_t)it->second].kind == V_UNSET)
-            return mfail(ctx, RTEN_ERR_INVALID_VALUE, "graph output '" + vi.name + "' is never produced");
-        m->outputs.push_back(it->second);
-    }
-    // ---- load-time fusions (src/optimize.rs: the patterns the hot-path models contain)
-    auto consumers = [&](int vid) {
-        int c = 0;
-        for (const OpNode& o : m->nodes)
-            for (int i : o.in)
-                if (i == vid) c++;
-        for (int o : m->outputs)
-            if (o == vid) c++;
-        return c;
-    };
-    // SiluFusion (src/optimize/fusions.rs:567-588): Mul(x, Sigmoid(x)), either operand order, becomes Silu(x) when the
-    // Sigmoid's output has no other consumer.  Silu rounds once where Mul(x, Sigmoid(x)) rounds twice, so the reference's
-    // Model::run computes Silu.  First, because the Sigmoid and the Mul are two consumers of a Conv's output.
-    for (size_t i = m->nodes.size(); i-- > 0;) {  // (backwards: erasing node i keeps the indices still to visit)
-        OpNode& s = m->nodes[i];
-        if (s.def != SIGMOID || s.in.size() != 1 || s.out.size() != 1 || consumers(s.out[0]) != 1) continue;
-        size_t j = i + 1;
-        for (; j < m->nodes.size(); j++)
-            if (std::find(m->nodes[j].in.begin(), m->nodes[j].in.end(), s.out[0]) != m->nodes[j].in.end()) break;
-        if (j == m->nodes.size()) continue;
-        OpNode& mul = m->nodes[j];
-        if (mul.def != MUL || mul.in.size() != 2 || mul.out.size() != 1) continue;
-        const int x = s.in[0];
-        if (!((mul.in[0] == s.out[0] && mul.in[1] == x) || (mul.in[1] == s.out[0] && mul.in[0] == x))) continue;
-        mul.def = SILU;
-        mul.n.op_type = SILU->name;
-        mul.n.inputs = {s.n.inputs[0]};
-        mul.n.attrs.clear();
-        mul.in = {x};
-        m->nodes.erase(m->nodes.begin() + (long)i);
-    }
-    // the node that reads value `vid` first after node i, when that is its only consumer, else -1
-    auto sole_consumer = [&](size_t i, int vid) -> long {
-        if (vid < 0 || consumers(vid) != 1) return -1;
-        for (size_t j = i + 1; j < m->nodes.size(); j++)
-            if (std::find(m->nodes[j].in.begin(), m->nodes[j].in.end(), vid) != m->nodes[j].in.end()) return (long)j;
-        return -1;
-    };
-    // GroupNormFusion: torch's export of nn.GroupNorm(G, C) -- Reshape(x, [0 | N, G, -1]) -> InstanceNormalization(
-    // scale [G], bias [G]) -> Reshape(to a constant 4-D shape) -> Mul(gamma [C, 1, 1]) -> Add(beta [C, 1, 1]), every
-    // intermediate with one consumer -- and a following Relu / Sigmoid / Silu / HardSigmoid / HardSwish become one
-    // GroupNorm node: one pass over x instead of two copies, the norm and three elementwise launches.  After SiluFusion,
-    // which makes the activation's Silu node.  The Reshape targets stay inputs, resolved for each run's x.
-    // RTEN_B200_NO_GROUP_NORM_FUSION=1 (read at load) keeps the node chain.  Only constant targets match: a target
-    // computed from Shape(x) is not fused.
-    if (!getenv("RTEN_B200_NO_GROUP_NORM_FUSION")) {
-        auto cval = [&](int vid) -> const ValueSlot* {
-            return vid >= 0 && m->values[(size_t)vid].kind == V_CONST ? &m->values[(size_t)vid] : nullptr;
-        };
-        // a per-channel constant of C elements: [C], broadcast over the spatial axes, i.e. shape [.., C, 1, 1]
-        auto per_channel = [&](int vid, int64_t* C) {
-            const ValueSlot* v = cval(vid);
-            if (!v || v->t.dtype != RTEN_F32 || v->t.ndim < 3 || v->t.ndim > 4) return false;
-            const int nd = v->t.ndim;
-            if (v->t.shape[nd - 1] != 1 || v->t.shape[nd - 2] != 1 || (nd == 4 && v->t.shape[0] != 1)) return false;
-            *C = v->t.shape[nd - 3];
-            return true;
-        };
-        for (size_t i = 0; i < m->nodes.size(); i++) {
-            const OpNode& r1 = m->nodes[i];
-            if (r1.def != RESHAPE_OP || r1.in.size() != 2 || r1.out.size() != 1 || r1.n.attr_i("allowzero", 0)) continue;
-            const ValueSlot* t1 = cval(r1.in[1]);
-            if (!t1 || !t1->has_host_ints || t1->host_ints.size() != 3 || t1->host_ints[0] < 0 || t1->host_ints[1] <= 0 ||
-                t1->host_ints[2] != -1)
-                continue;
-            const int64_t G = t1->host_ints[1];
-            const long j_in = sole_consumer(i, r1.out[0]);
-            if (j_in < 0) continue;
-            const OpNode& in = m->nodes[(size_t)j_in];
-            if (in.def != INSTANCE_NORM || in.in.size() != 3 || in.in[0] != r1.out[0] || in.out.size() != 1) continue;
-            const ValueSlot *sc = cval(in.in[1]), *bi = cval(in.in[2]);
-            if (!sc || !bi || sc->t.ndim != 1 || bi->t.ndim != 1 || sc->t.shape[0] != G || bi->t.shape[0] != G) continue;
-            const long j_r2 = sole_consumer((size_t)j_in, in.out[0]);
-            if (j_r2 < 0) continue;
-            const OpNode& r2 = m->nodes[(size_t)j_r2];
-            if (r2.def != RESHAPE_OP || r2.in.size() != 2 || r2.in[0] != in.out[0] || r2.out.size() != 1 || r2.n.attr_i("allowzero", 0))
-                continue;
-            const ValueSlot* t2 = cval(r2.in[1]);
-            if (!t2 || !t2->has_host_ints || t2->host_ints.size() != 4) continue;
-            const long j_mul = sole_consumer((size_t)j_r2, r2.out[0]);
-            if (j_mul < 0) continue;
-            const OpNode& mul = m->nodes[(size_t)j_mul];
-            if (mul.def != MUL || mul.in.size() != 2 || mul.out.size() != 1) continue;
-            const int gamma = mul.in[0] == r2.out[0] ? mul.in[1] : mul.in[0];
-            int64_t C = 0, Cb = 0;
-            if (gamma == r2.out[0] || !per_channel(gamma, &C) || C % G != 0) continue;
-            const long j_add = sole_consumer((size_t)j_mul, mul.out[0]);
-            if (j_add < 0) continue;
-            const OpNode& add = m->nodes[(size_t)j_add];
-            if (add.def != ADD || add.in.size() != 2 || add.out.size() != 1) continue;
-            const int beta = add.in[0] == mul.out[0] ? add.in[1] : add.in[0];
-            if (beta == mul.out[0] || !per_channel(beta, &Cb) || Cb != C) continue;
-            long last = j_add;
-            rten_activation act = {RTEN_ACT_NONE, 0.0f, 0.0f};
-            const long j_act = sole_consumer((size_t)j_add, add.out[0]);
-            if (j_act >= 0) {
-                const OpNode& a = m->nodes[(size_t)j_act];
-                if (a.def->act != RTEN_ACT_NONE && a.in.size() == 1 && a.out.size() == 1) {
-                    const bool hs = a.def->act == RTEN_ACT_HARD_SIGMOID;
-                    act = {(int32_t)a.def->act, hs ? hard_sigmoid_alpha(a.n) : 0.0f, hs ? hard_sigmoid_beta(a.n) : 0.0f};
-                    last = j_act;
-                }
-            }
-            OpNode gn;
-            gn.n = in.n;
-            gn.n.op_type = GROUP_NORM->name;
-            gn.def = GROUP_NORM;
-            gn.in = {r1.in[0], in.in[1], in.in[2], gamma, beta, r1.in[1], r2.in[1]};
-            gn.out = m->nodes[(size_t)last].out;
-            gn.activation = act;
-            // the fused node takes the last node's place (every input exists by then); the others go
-            const long chain[] = {(long)i, j_in, j_r2, j_mul, j_add, j_act >= 0 && last == j_act ? j_act : -1};
-            m->nodes[(size_t)last] = gn;
-            for (long k = (long)m->nodes.size() - 1; k >= 0; k--)
-                if (k != last && std::find(std::begin(chain), std::end(chain), k) != std::end(chain)) m->nodes.erase(m->nodes.begin() + k);
-            i = (size_t)-1;  // (indices moved: look again from the start; every match removes nodes, so this ends)
-        }
-    }
-    for (size_t i = 0; i + 1 < m->nodes.size(); i++) {
-        OpNode& a = m->nodes[i];
-        if (a.out.size() != 1 || consumers(a.out[0]) != 1) continue;
-        // the single consumer
-        size_t j = i + 1;
-        for (; j < m->nodes.size(); j++)
-            if (std::find(m->nodes[j].in.begin(), m->nodes[j].in.end(), a.out[0]) != m->nodes[j].in.end()) break;
-        if (j == m->nodes.size()) continue;
-        OpNode& b = m->nodes[j];
-        if (a.def == CONV && a.activation.kind == RTEN_ACT_NONE && b.def->act != RTEN_ACT_NONE) {  // (Clip is not fused)
-            const bool hs = b.def->act == RTEN_ACT_HARD_SIGMOID;  // the activation in the convolution epilogue
-            a.activation = {(int32_t)b.def->act, hs ? hard_sigmoid_alpha(b.n) : 0.0f, hs ? hard_sigmoid_beta(b.n) : 0.0f};
-            a.out = b.out;
-            m->nodes.erase(m->nodes.begin() + (long)j);
-        } else if (a.def == MATMUL && b.def == ADD && a.bias_value < 0 && b.in.size() == 2) {
-            // MatMul + Add(constant vector over the last axis) -> FusedMatMul with a row bias (MatMulAddFusion)
-            const int other = b.in[0] == a.out[0] ? b.in[1] : b.in[0];
-            const ValueSlot& bv = m->values[(size_t)other];
-            const ValueSlot& wv = m->values[(size_t)a.in[1]];
-            if (bv.kind == V_CONST && bv.t.dtype == RTEN_F32 && bv.t.ndim == 1 && wv.t.ndim >= 2 && wv.kind == V_CONST &&
-                bv.t.shape[0] == wv.t.shape[wv.t.ndim - 1]) {
-                a.bias_value = other;
-                a.out = b.out;
-                m->nodes.erase(m->nodes.begin() + (long)j);
-            }
-        }
-    }
-    // ---- Concat elision, decided once: which inputs of which channel Concat their producers write in place
-    if (!getenv("RTEN_B200_NO_CONCAT_ELISION")) {
-        std::map<std::string, std::vector<int64_t>> input_dims;
-        for (const onnx::ValueInfo& vi : om.graph.inputs) input_dims[vi.name] = vi.dims;
-        auto producer = [&](int vid) {
-            for (size_t i = 0; i < m->nodes.size(); i++)
-                for (int o : m->nodes[i].out)
-                    if (o == vid) return (int)i;
-            return -1;
-        };
-        // channels of a 4-D value as far as the file tells them, else -1
-        std::function<int64_t(int, int)> channels = [&](int vid, int depth) -> int64_t {
-            if (vid < 0 || depth > 64) return -1;
-            const ValueSlot& v = m->values[(size_t)vid];
-            if (v.kind == V_INPUT) {
-                const std::vector<int64_t>& d = input_dims[v.name];
-                return d.size() == 4 && d[1] > 0 ? d[1] : -1;
-            }
-            const int pi = producer(vid);
-            if (pi < 0) return -1;
-            const OpNode& p = m->nodes[(size_t)pi];
-            auto weight = [&]() -> const rten_tensor* {
-                if (p.in.size() < 2 || p.in[1] < 0 || m->values[(size_t)p.in[1]].kind != V_CONST) return nullptr;
-                const rten_tensor& w = m->values[(size_t)p.in[1]].t;
-                return w.ndim == 4 ? &w : nullptr;
-            };
-            if (p.def == CONV) return weight() ? weight()->shape[0] : -1;
-            if (p.def == CONV_TRANSPOSE) return weight() ? weight()->shape[1] * p.n.attr_i("group", 1) : -1;
-            // the pools and Resize / Upsample (the other Concat-slice writers) and the elementwise operators
-            if (p.def->shape || (p.def->flags & IN_PLACE)) return channels(p.in[0], depth + 1);
-            if (p.def == CONCAT && p.n.attr_i("axis", 0) == 1) {
-                int64_t sum = 0;
-                for (int i : p.in) {
-                    const int64_t c = channels(i, depth + 1);
-                    if (c < 0) return -1;
-                    sum += c;
-                }
-                return sum;
-            }
-            return -1;
-        };
-        std::string report;
-        for (size_t k = 0; k < m->nodes.size(); k++) {
-            OpNode& c = m->nodes[k];
-            if (c.def != CONCAT || c.n.attr_i("axis", 0) != 1 || c.out.size() != 1 || consumers(c.out[0]) < 1) continue;
-            std::vector<int64_t> ch;
-            for (int i : c.in) ch.push_back(channels(i, 0));
-            if (std::find(ch.begin(), ch.end(), (int64_t)-1) != ch.end()) continue;
-            std::vector<char> mark(c.in.size(), 0);
-            std::string names;
-            for (size_t i = 0; i < c.in.size(); i++) {
-                const int vid = c.in[i];
-                if (m->values[(size_t)vid].kind != V_TEMP) continue;
-                if (std::count(c.in.begin(), c.in.end(), vid) != 1) continue;
-                if (std::find(m->outputs.begin(), m->outputs.end(), vid) != m->outputs.end()) continue;  // a graph output is copied
-                const int pi = producer(vid);
-                OpNode& p = m->nodes[(size_t)pi];
-                if (!p.def->shape || p.out.size() != 1 || p.cat_node >= 0) continue;
-                p.cat_node = (int)k;
-                p.cat_slot = (int)i;
-                mark[i] = 1;
-                names += (names.empty() ? "\"" : ",\"") + m->values[(size_t)vid].name + "\"";
-            }
-            if (names.empty()) continue;
-            c.cat_channels = ch;
-            c.cat_in_place = mark;
-            report += (report.empty() ? "" : ",") + std::string("{\"output\":\"") + m->values[(size_t)c.out[0]].name +
-                      "\",\"copied\":" + std::to_string(std::count(mark.begin(), mark.end(), 0)) + ",\"in_place\":[" + names + "]}";
-        }
-        // (the summary is the decoded file's JSON object: the plan is appended as one more member)
-        const size_t close = m->summary.rfind('}');
-        if (close != std::string::npos) m->summary.insert(close, ",\"concat_in_place\":[" + report + "]");
-    }
-    // ---- prepack constant weights once
-    for (OpNode& o : m->nodes) {
-        const int w = o.in.size() >= 2 ? o.in[1] : -1;
-        if (o.def->prepack && w >= 0 && m->values[(size_t)w].kind == V_CONST) RTB_TRY(o.def->prepack(ctx, o, m->values[(size_t)w].t));
-    }
+    RTB_TRY(build_graph(m.get(), om));
+    fuse_silu(m.get());
+    if (!getenv("RTEN_B200_NO_GROUP_NORM_FUSION")) fuse_group_norm(m.get());
+    fuse_into_producers(m.get());
+    if (!getenv("RTEN_B200_NO_CONCAT_ELISION")) plan_concat_elision(m.get(), om.graph.inputs);
+    RTB_TRY(prepack_weights(m.get()));
     RTB_TRY(rten_b200_sync(ctx));
     *out = m.release();
     return RTEN_OK;
