@@ -316,17 +316,62 @@ rten_status fill_resize_params(rten_ctx* ctx, const onnx::Node& n, bool upsample
     return RTEN_OK;
 }
 
-// MaxPool / AveragePool attributes (kernel_shape, pads, strides)
+// MaxPool / AveragePool auto_pad (src/op_registry/onnx_registry.rs get_padding): NOTSET and VALID take the pads
+// attribute, SAME_UPPER is `Padding::Same`; SAME_LOWER is refused as Conv refuses it
+rten_status pool_auto_pad(rten_ctx* ctx, const onnx::Node& n, bool* same) {
+    const onnx::Attribute* ap = n.attr("auto_pad");
+    *same = ap && ap->s == "SAME_UPPER";
+    if (ap && ap->s == "SAME_LOWER") return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "auto_pad SAME_LOWER is not supported");
+    if (ap && !ap->s.empty() && ap->s != "NOTSET" && ap->s != "VALID" && ap->s != "SAME_UPPER")
+        return mfail(ctx, RTEN_ERR_INVALID_VALUE, "auto_pad: unsupported value");
+    return RTEN_OK;
+}
+
+// MaxPool / AveragePool attributes (kernel_shape, pads, strides, auto_pad, ceil_mode) for the NCHW input x, as pads under
+// which the floor-rounded output size of the pooling entry points is the reference's (src/ops/pooling.rs
+// output_size_and_padding_for_axis).  SAME_UPPER: the pads axis_out computes.  ceil_mode: the end pad that makes the
+// floor formula give the ceil size, after the reference drops a last window that would start inside the end padding.
+// Only the output size depends on the end pads: both pool kernels skip every tap outside the image, and divide by
+// kh * kw under count_include_pad, as the reference's `average` does.
 struct PoolAttrs {
     int32_t kernel[2], pads[4] = {0, 0, 0, 0}, strides[2] = {1, 1};
 };
-rten_status fill_pool_attrs(rten_ctx* ctx, const onnx::Node& n, PoolAttrs* a) {
+rten_status fill_pool_attrs(rten_ctx* ctx, const onnx::Node& n, const rten_tensor& x, PoolAttrs* a) {
     const std::vector<int64_t> k = n.attr_ints("kernel_shape"), pd = n.attr_ints("pads"), sd = n.attr_ints("strides");
     if (k.size() != 2) return mfail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, n.op_type + ": only 2-D kernels are supported");
+    if (x.ndim != 4) return mfail(ctx, RTEN_ERR_INVALID_VALUE, "input must have 4 dims (NCHW)");
+    bool same = false;
+    RTB_TRY(pool_auto_pad(ctx, n, &same));
+    const bool ceil = n.attr_i("ceil_mode", 0) != 0;
     a->kernel[0] = (int32_t)k[0];
     a->kernel[1] = (int32_t)k[1];
     for (size_t i = 0; i < pd.size() && i < 4; i++) a->pads[i] = (int32_t)pd[i];
     for (size_t i = 0; i < sd.size() && i < 2; i++) a->strides[i] = (int32_t)sd[i];
+    const int64_t in[2] = {x.shape[2], x.shape[3]};
+    for (int i = 0; i < 2; i++) {
+        int64_t out, ps, pe;
+        RTB_TRY(api::axis_out(ctx, in[i], a->kernel[i], a->strides[i], same, a->pads[i], a->pads[2 + i], 1, &out, &ps, &pe));
+        if (ceil && !same) {
+            const int64_t s = a->strides[i], windows = in[i] + ps + pe - a->kernel[i];  // >= 0 past axis_out
+            out = (windows + s - 1) / s + 1;
+            if ((out - 1) * s >= in[i] + ps) out--;
+            // floor((in + ps + pe' - k) / s) + 1 == out; 0 when the unpadded end already gives out windows
+            pe = std::max<int64_t>(0, (out - 1) * s + a->kernel[i] - in[i] - ps);
+        }
+        a->pads[i] = (int32_t)ps;
+        a->pads[2 + i] = (int32_t)pe;
+    }
+    return RTEN_OK;
+}
+
+// load checks of MaxPool / AveragePool: auto_pad, and MaxPool's Indices output, which the reference's MaxPool does not
+// produce (max_outputs = 1)
+template <bool max_pool>
+rten_status check_pool(rten_model* m, onnx::Node& n) {
+    bool same;
+    RTB_TRY(pool_auto_pad(m->ctx, n, &same));
+    if (max_pool && n.outputs.size() > 1 && !n.outputs[1].empty())
+        return mfail(m->ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MaxPool: the Indices output (1) is not supported");
     return RTEN_OK;
 }
 
@@ -705,7 +750,7 @@ rten_status prepack_rnn(rten_ctx* ctx, OpNode& o, const rten_tensor& w0) {
 bool pool_shape(Runner& r, const OpNode& o, const rten_tensor& x, int64_t shape[4]) {
     PoolAttrs a;
     int64_t p0, p1;
-    if (fill_pool_attrs(r.ctx, o.n, &a) != RTEN_OK) return false;
+    if (fill_pool_attrs(r.ctx, o.n, x, &a) != RTEN_OK) return false;
     for (int i = 0; i < 2; i++)
         if (api::axis_out(r.ctx, x.shape[2 + i], a.kernel[i], a.strides[i], false, a.pads[i], a.pads[2 + i], 1, &shape[2 + i], &p0, &p1) != RTEN_OK)
             return false;
@@ -935,16 +980,14 @@ constexpr OpDef OPS[] = {
     {"Softmax", ONNX, IN_PLACE, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_softmax(r.ctx, r.T(o, 0), nullptr, (int)o.n.attr_i("axis", -1), 0, y); }},
     {"MaxPool", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
          PoolAttrs a;
-         RTB_TRY(fill_pool_attrs(r.ctx, o.n, &a));
+         RTB_TRY(fill_pool_attrs(r.ctx, o.n, *r.T(o, 0), &a));
          return rten_b200_max_pool(r.ctx, r.T(o, 0), a.kernel, a.pads, a.strides, y);
-     }, nullptr, nullptr, pool_shape},
+     }, check_pool<true>, nullptr, pool_shape},
     {"AveragePool", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
          PoolAttrs a;
-         RTB_TRY(fill_pool_attrs(r.ctx, o.n, &a));
+         RTB_TRY(fill_pool_attrs(r.ctx, o.n, *r.T(o, 0), &a));
          return rten_b200_average_pool(r.ctx, r.T(o, 0), a.kernel, a.pads, a.strides, (int)o.n.attr_i("count_include_pad", 0), y);
-     }, [](rten_model* m, onnx::Node& n) {
-         return n.attr_i("ceil_mode", 0) == 0 ? RTEN_OK : mfail(m->ctx, RTEN_ERR_UNSUPPORTED_VALUE, "AveragePool: ceil_mode = 1 is not supported");
-     }, nullptr, pool_shape},
+     }, check_pool<false>, nullptr, pool_shape},
     {"Resize", ONNX, 0, 0b1, run_resize<false>, [](rten_model* m, onnx::Node& n) { rten_resize_params p; return fill_resize_params(m->ctx, n, false, &p); },
      nullptr, resize_shape<false>},
     {"Upsample", ONNX, 0, 0b1, run_resize<true>, [](rten_model* m, onnx::Node& n) {

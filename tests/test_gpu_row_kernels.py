@@ -79,15 +79,17 @@ FAMILY_KERNELS = {"softmax": ("softmax_vec_kernel", "softmax_kernel"), "norm": (
 _NAME = re.compile(r"rtb::(\w+)(?:<([^<>]*)>)?\(")
 
 
-def kernel_key(name):
-    """(kernel, template arguments as ints) of a demangled kernel name of the four families, else None.  Accepts both
-    spellings of the arguments: `<1, 2>` / `<.., false, ..>` (CUPTI) and `<(int)1, (int)2>` / `(bool)0` (cu++filt)."""
+def kernel_key(name, kernels=None):
+    """(kernel, template arguments) of a demangled kernel name of `kernels` (default: the four families here), else
+    None.  Accepts both spellings of the arguments: `<1, 2>` / `<.., false, ..>` (CUPTI) and `<(int)1, (int)2>` /
+    `(bool)0` (cu++filt).  Values become ints, type arguments stay names (`float`, `int`)."""
+    kernels = set(VARIANTS) | set(GENERIC) if kernels is None else kernels
     for m in _NAME.finditer(name):
-        if m.group(1) in VARIANTS or m.group(1) in GENERIC:
+        if m.group(1) in kernels:
             args = []
             for a in (m.group(2).split(",") if m.group(2) else []):
                 a = re.sub(r"^\((int|bool)\)", "", a.strip())
-                args.append({"true": 1, "false": 0}[a] if a in ("true", "false") else int(a))
+                args.append({"true": 1, "false": 0}[a] if a in ("true", "false") else int(a) if re.fullmatch(r"-?\d+", a) else a)
             return m.group(1), tuple(args)
     return None
 
@@ -647,24 +649,35 @@ def _kernel_probe():
                 def call():
                     launch(rt, ctx, s, inp, **kw)
                     ctx.sync()
-                # Every call launches kernels.  A capture with no kernel record at all (seen, rarely, before the
-                # window was widened in _capture) is taken again, at most twice, and counted in the output.
-                for attempt in range(3):
-                    with (_NoVecRows() if no_vec else contextlib.nullcontext()):
-                        names = _capture(call)
-                    if any("_kernel" in n for n in names):
-                        break
-                    retaken += 1
+                with (_NoVecRows() if no_vec else contextlib.nullcontext()):
+                    names, again = capture_kernels(call)
+                retaken += again
                 res[spec_id(fam, s) + " " + label] = sorted(names)
     print(json.dumps({"sms": n_sms, "names": res, "retaken": retaken}))
 
 
-def test_kernel_identity():
+def capture_kernels(call):
+    """(names of the kernels `call` launches, captures taken again).  Every call launches kernels.  A capture with no
+    kernel record at all (seen, rarely, before the window was widened in _capture) is taken again, at most twice."""
+    for attempt in range(3):
+        names = _capture(call)
+        if any("_kernel" in n for n in names):
+            break
+    return names, attempt
+
+
+def probe_in_child(module):
+    """`module._kernel_probe()` in a child process, so that no profiler state stays behind in the test session: the JSON
+    line it prints last"""
     code = (f"import sys; sys.path[:0] = [{os.path.dirname(HERE)!r}, {HERE!r}]; "
-            "import test_gpu_row_kernels as t; t._kernel_probe()")
+            f"import {module} as t; t._kernel_probe()")
     res = subprocess.run([sys.executable, "-s", "-c", code], capture_output=True, text=True, timeout=1200)
     assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-4000:]
-    out = json.loads(res.stdout.strip().splitlines()[-1])
+    return json.loads(res.stdout.strip().splitlines()[-1])
+
+
+def test_kernel_identity():
+    out = probe_in_child("test_gpu_row_kernels")
     n_sms, names = out["sms"], out["names"]
     seen, wrong = set(), []
     for fam, (specs, _, _, _) in FAMILIES.items():
