@@ -666,7 +666,7 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
             long long ds[4] = {ov.strides[0], ov.strides[2], ov.strides[3], ov.strides[1]};
             if (A.residual) {
                 long long rs4[4] = {res_v.strides[0], res_v.strides[2], res_v.strides[3], res_v.strides[1]};
-                RTB_TRY(launch_nd_add(ctx, (const float*)tmp, e.r, (float*)e.d, 4, shape, ss, rs4, ds, A.act == 1));
+                RTB_TRY(launch_binary(ctx, RTEN_F32, BIN_ADD, A.act == 1, tmp, e.r, e.d, 4, shape, ss, rs4, ds));
                 if (A.act > 1)
                     return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "an activation other than Relu after a residual needs a pixel-contiguous output");
             } else {

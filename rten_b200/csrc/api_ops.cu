@@ -211,7 +211,7 @@ rten_status matmul_core(OpScope& sc, MatMulArgs& A, rten_tensor* out) {
         RTB_CUDA(ctx, cudaMemsetAsync(dv.data, 0, (size_t)total * 4, ctx->stream));
         if (A.kind == 0 && L.epi.bias) {
             long long shp[2] = {total / N, N}, s0[2] = {N, 1}, sb[2] = {0, 1};
-            RTB_TRY(launch_nd_add(ctx, (const float*)dv.data, L.epi.bias, (float*)dv.data, 2, shp, s0, sb, s0, 0));
+            RTB_TRY(launch_binary(ctx, RTEN_F32, BIN_ADD, 0, dv.data, L.epi.bias, dv.data, 2, shp, s0, sb, s0));
         }
     } else {
         // B operand

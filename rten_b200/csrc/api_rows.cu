@@ -470,15 +470,12 @@ rten_status rten_b200_hard_swish(rten_ctx* ctx, const rten_tensor* x, rten_tenso
 }
 
 // ---- Add / Sub / Mul ----------------------------------------------------------------------------------
-// Add / Sub / Mul with numpy broadcasting (src/ops/binary_elementwise.rs), f32 or i32 (wrapping).  f32 Add and Mul run on
-// launch_add_flat / launch_nd_add (flags 0 = Add, 2 = Mul), everything else on launch_binary.
+// Add / Sub / Mul with numpy broadcasting (src/ops/binary_elementwise.rs), f32 or i32 (wrapping).
 static rten_status binary_op(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out, int op) {
     RTB_TRY(check_ctx(ctx));
     if (!a || !b || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
     if ((a->dtype != RTEN_F32 && a->dtype != RTEN_I32) || b->dtype != a->dtype) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
     const int dt = a->dtype;
-    const bool add_kernels = dt == RTEN_F32 && op != BIN_SUB;
-    const int flags = op == BIN_MUL ? 2 : 0;
     OpScope sc(ctx);
     rten_tensor av, bv, ov;
     RTB_TRY(sc.in(a, &av));
@@ -503,21 +500,16 @@ static rten_status binary_op(rten_ctx* ctx, const rten_tensor* a, const rten_ten
     bool flat = same;
     for (int i = 0; i < nd && flat; i++)
         if (ov.shape[i] != 1 && ov.strides[i] != av.strides[i]) flat = false;
-    if (flat && add_kernels)
-        return sc.finish(launch_add_flat(ctx, (const float*)av.data, (const float*)bv.data, (float*)ov.data, numel(&ov), flags));
+    if (flat) {  // dense operands of one layout: one flat pass over the n elements from the lowest address
+        const long long n = numel(&ov), one = 1;
+        return sc.finish(launch_binary(ctx, dt, op, 0, av.data, bv.data, ov.data, 1, &n, &one, &one, &one));
+    }
     long long shp[RTEN_MAX_DIMS], sd[RTEN_MAX_DIMS];
     for (int i = 0; i < nd; i++) {
         shp[i] = shape[i];
         sd[i] = ov.strides[i];
     }
-    if (!add_kernels) {
-        if (flat) {  // dense operands of one layout: one flat pass over the n elements from the lowest address
-            const long long n = numel(&ov), one = 1;
-            return sc.finish(launch_binary(ctx, dt, op, av.data, bv.data, ov.data, 1, &n, &one, &one, &one, true));
-        }
-        return sc.finish(launch_binary(ctx, dt, op, av.data, bv.data, ov.data, nd, shp, sa, sb, sd, false));
-    }
-    return sc.finish(launch_nd_add(ctx, (const float*)av.data, (const float*)bv.data, (float*)ov.data, nd, shp, sa, sb, sd, flags));
+    return sc.finish(launch_binary(ctx, dt, op, 0, av.data, bv.data, ov.data, nd, shp, sa, sb, sd));
 }
 
 rten_status rten_b200_add(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out) {

@@ -593,8 +593,8 @@ rten_status launch_row_mean(rten_ctx* ctx, const float* x, float* y, long long r
 }
 
 // =========================================================================================
-// Elementwise (contiguous): Erf, Gelu, ApproxGelu, Relu, Sigmoid, Silu, HardSigmoid, HardSwish, and same-shape Add
-// (+ optional Relu).  128-bit loads/stores, grid sized to fill the SMs.
+// Elementwise (contiguous): Erf, Gelu, ApproxGelu, Relu, Sigmoid, Silu, HardSigmoid, HardSwish.  128-bit loads/stores,
+// grid sized to fill the SMs.
 // =========================================================================================
 template <int OP>
 __device__ __forceinline__ float unary_apply(float v, float alpha, float beta) {
@@ -655,8 +655,8 @@ rten_status launch_unary(rten_ctx* ctx, int op, const float* x, float* y, long l
     return launch(ctx, "unary launch", kern, {grid, 256}, x, y, n, vec, alpha, beta);
 }
 
-// General N-d strided kernels (up to 8 dims): copy / broadcast add.  Used for layout changes
-// (NCHW <-> NHWC views, weight prepack), host staging of strided tensors and broadcast Add.
+// General N-d strided kernels (up to 8 dims): copy / broadcast Add, Sub and Mul.  Used for layout changes
+// (NCHW <-> NHWC views, weight prepack), host staging of strided tensors and broadcast arithmetic.
 struct NdParams {
     int ndim;
     long long shape[RTEN_MAX_DIMS];
@@ -665,6 +665,22 @@ struct NdParams {
     long long sd[RTEN_MAX_DIMS];
     long long n;
 };
+
+// sb may be null (a copy has no b); n = the element count
+static NdParams nd_params(int ndim, const long long* shape, const long long* sa, const long long* sb, const long long* sd) {
+    NdParams p;
+    memset(&p, 0, sizeof(p));
+    p.ndim = ndim;
+    p.n = 1;
+    for (int i = 0; i < ndim; i++) {
+        p.shape[i] = shape[i];
+        p.sa[i] = sa[i];
+        p.sb[i] = sb ? sb[i] : 0;
+        p.sd[i] = sd[i];
+        p.n *= shape[i];
+    }
+    return p;
+}
 
 template <typename T>
 __global__ void __launch_bounds__(256) nd_copy_kernel(const T* __restrict__ src, T* __restrict__ dst, const NdParams p) {
@@ -699,63 +715,11 @@ __global__ void __launch_bounds__(256) nd_copy_kernel(const T* __restrict__ src,
     }
 }
 
-__global__ void __launch_bounds__(256)
-nd_add_kernel(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ d, const NdParams p, int relu) {
-    const long long stride = (long long)gridDim.x * blockDim.x;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += stride) {
-        long long rem = i, ao = 0, bo = 0, dof = 0;
-#pragma unroll 1
-        for (int k = p.ndim - 1; k >= 0; k--) {
-            const long long idx = rem % p.shape[k];
-            rem /= p.shape[k];
-            ao += idx * p.sa[k];
-            bo += idx * p.sb[k];
-            dof += idx * p.sd[k];
-        }
-        float v = (relu & 2) ? __fmul_rn(a[ao], b[bo]) : __fadd_rn(a[ao], b[bo]);  // flags: 1 = Relu after, 2 = Mul
-        if (relu & 1) v = v > 0.0f ? v : 0.0f;
-        d[dof] = v;
-    }
-}
-
-__global__ void __launch_bounds__(256)
-add_flat_kernel(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ d, long long n, int relu) {
-    const long long n4 = n >> 2;
-    const long long stride = (long long)gridDim.x * blockDim.x;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
-        const float4 x = reinterpret_cast<const float4*>(a)[i];
-        const float4 y = reinterpret_cast<const float4*>(b)[i];
-        float4 o = (relu & 2) ? make_float4(__fmul_rn(x.x, y.x), __fmul_rn(x.y, y.y), __fmul_rn(x.z, y.z), __fmul_rn(x.w, y.w))
-                              : make_float4(__fadd_rn(x.x, y.x), __fadd_rn(x.y, y.y), __fadd_rn(x.z, y.z), __fadd_rn(x.w, y.w));
-        if (relu & 1) {
-            o.x = o.x > 0.f ? o.x : 0.f;
-            o.y = o.y > 0.f ? o.y : 0.f;
-            o.z = o.z > 0.f ? o.z : 0.f;
-            o.w = o.w > 0.f ? o.w : 0.f;
-        }
-        reinterpret_cast<float4*>(d)[i] = o;
-    }
-    for (long long j = (n4 << 2) + (long long)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride) {
-        float v = (relu & 2) ? __fmul_rn(a[j], b[j]) : __fadd_rn(a[j], b[j]);
-        if (relu & 1) v = v > 0.f ? v : 0.f;
-        d[j] = v;
-    }
-}
-
 // Collapse to the iteration order that makes the DESTINATION contiguous-fastest: dims are visited in
 // the given order; callers pass dims sorted so that the last has the smallest dst stride.
 rten_status launch_nd_copy(rten_ctx* ctx, int esize, const void* src, void* dst, int ndim, const long long* shape,
                            const long long* sstride, const long long* dstride) {
-    NdParams p;
-    memset(&p, 0, sizeof(p));
-    p.ndim = ndim;
-    p.n = 1;
-    for (int i = 0; i < ndim; i++) {
-        p.shape[i] = shape[i];
-        p.sa[i] = sstride[i];
-        p.sd[i] = dstride[i];
-        p.n *= shape[i];
-    }
+    NdParams p = nd_params(ndim, shape, sstride, nullptr, dstride);
     if (p.n == 0) return RTEN_OK;
     if (esize != 4 && esize != 1) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported element size");
     // Wider elements when both sides are contiguous along the innermost visited dim: a padded copy of a channels-last
@@ -789,99 +753,72 @@ rten_status launch_nd_copy(rten_ctx* ctx, int esize, const void* src, void* dst,
     }
 }
 
-// a and d dense, b dense over the TRAILING dims and broadcast over the leading ones (bias rows, position embeddings):
-// d[i] = a[i] (+|*) b[i mod period], 128 bits per thread, 32-bit index arithmetic
-__global__ void __launch_bounds__(256)
-add_periodic_kernel(const float4* __restrict__ a, const float4* __restrict__ b, float4* __restrict__ d, unsigned n4, unsigned period4, int relu) {
-    const unsigned stride = gridDim.x * blockDim.x;
-    for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
-        const float4 x = a[i];
-        const float4 y = b[i % period4];
-        float4 o = (relu & 2) ? make_float4(__fmul_rn(x.x, y.x), __fmul_rn(x.y, y.y), __fmul_rn(x.z, y.z), __fmul_rn(x.w, y.w))
-                              : make_float4(__fadd_rn(x.x, y.x), __fadd_rn(x.y, y.y), __fadd_rn(x.z, y.z), __fadd_rn(x.w, y.w));
-        if (relu & 1) {
-            o.x = o.x > 0.f ? o.x : 0.f;
-            o.y = o.y > 0.f ? o.y : 0.f;
-            o.z = o.z > 0.f ? o.z : 0.f;
-            o.w = o.w > 0.f ? o.w : 0.f;
-        }
-        d[i] = o;
-    }
-}
-
-rten_status launch_nd_add(rten_ctx* ctx, const float* a, const float* b, float* d, int ndim, const long long* shape,
-                          const long long* sa, const long long* sb, const long long* sd, int relu) {
-    {
-        // fast path: a / d dense, b = a dense block of the trailing dims repeated over the leading ones
-        long long dense = 1, period = 0, n = 1;
-        bool ok = ndim >= 1, in_bcast = false;
-        for (int i = ndim - 1; i >= 0 && ok; i--) {
-            if (shape[i] != 1) {
-                ok = sa[i] == dense && sd[i] == dense;
-                if (!in_bcast && sb[i] == dense) {
-                } else if (sb[i] == 0) {
-                    if (!in_bcast) period = dense;
-                    in_bcast = true;
-                } else {
-                    ok = false;
-                }
-            }
-            dense *= shape[i];
-            n *= shape[i];
-        }
-        if (ok && in_bcast && period > 0 && (period & 3) == 0 && n < 0x7fffffffLL && n > 0 &&
-            ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(d)) & 15) == 0)
-            return launch(ctx, "nd_add launch", add_periodic_kernel, {ew_grid(ctx, n / 4), 256}, reinterpret_cast<const float4*>(a),
-                          reinterpret_cast<const float4*>(b), reinterpret_cast<float4*>(d), (unsigned)(n / 4), (unsigned)(period / 4),
-                          relu);
-    }
-    NdParams p;
-    memset(&p, 0, sizeof(p));
-    p.ndim = ndim;
-    p.n = 1;
-    for (int i = 0; i < ndim; i++) {
-        p.shape[i] = shape[i];
-        p.sa[i] = sa[i];
-        p.sb[i] = sb[i];
-        p.sd[i] = sd[i];
-        p.n *= shape[i];
-    }
-    if (p.n == 0) return RTEN_OK;
-    return launch(ctx, "nd_add launch", nd_add_kernel, {ew_grid(ctx, p.n), 256}, a, b, d, p, relu);
-}
-
-rten_status launch_add_flat(rten_ctx* ctx, const float* a, const float* b, float* d, long long n, int relu) {
-    if (n == 0) return RTEN_OK;
-    const bool aligned =
-        ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(d)) & 15) == 0;
-    if (!aligned) {
-        long long shape[1] = {n}, s1[1] = {1};
-        return launch_nd_add(ctx, a, b, d, 1, shape, s1, s1, s1, relu);
-    }
-    return launch(ctx, "add launch", add_flat_kernel, {ew_grid(ctx, (n + 3) / 4), 256}, a, b, d, n, relu);
-}
-
-// The binary operations the f32 Add / Mul kernels above do not run, one instance per (type, operation): they are kept
-// apart so that those kernels stay as they are.  i32 arithmetic wraps (src/ops/binary_elementwise.rs on i32).
-template <typename T, int OP>
-__device__ __forceinline__ T binary_apply(T a, T b) {
+// Add / Sub / Mul: f32 correctly rounded, then Relu when `relu`; i32 in unsigned arithmetic, so it wraps
+// (src/ops/binary_elementwise.rs on i32).  One instance per element type: the operation is a runtime argument.
+template <typename T>
+__device__ __forceinline__ T binary_apply(T a, T b, int op, int relu) {
+    T v;
     if constexpr (std::is_same<T, float>::value) {
-        static_assert(OP == BIN_SUB, "f32 Add / Mul run on add_flat_kernel / nd_add_kernel");
-        return __fsub_rn(a, b);
+        v = op == BIN_MUL ? __fmul_rn(a, b) : __fadd_rn(a, op == BIN_SUB ? -b : b);  // (a - b is a + -b, exactly)
     } else {
         const unsigned x = (unsigned)a, y = (unsigned)b;
-        return (int)(OP == BIN_ADD ? x + y : OP == BIN_SUB ? x - y : x * y);
+        v = (int)(op == BIN_MUL ? x * y : op == BIN_SUB ? x - y : x + y);
     }
+    if (relu) v = v > T(0) ? v : T(0);
+    return v;
 }
 
-template <typename T, int OP>
-__global__ void __launch_bounds__(256) binary_flat_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d, long long n) {
-    const long long stride = (long long)gridDim.x * blockDim.x;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) d[i] = binary_apply<T, OP>(a[i], b[i]);
+// f(op) with op a compile-time constant: the flat and periodic kernels get one loop per operation, with no per-element
+// choice of operation.  (The strided kernel keeps one loop: its index loop compiles shorter that way.)
+template <typename F>
+__device__ __forceinline__ void with_op(int op, F f) {
+    if (op == BIN_MUL) f(std::integral_constant<int, BIN_MUL>());
+    else if (op == BIN_SUB) f(std::integral_constant<int, BIN_SUB>());
+    else f(std::integral_constant<int, BIN_ADD>());
 }
 
-template <typename T, int OP>
-__global__ void __launch_bounds__(256) binary_nd_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d, const NdParams p) {
+template <typename T>
+using Vec4 = typename std::conditional<std::is_same<T, float>::value, float4, int4>::type;  // 16 bytes of T
+
+template <typename T>
+__device__ __forceinline__ Vec4<T> binary_apply4(Vec4<T> x, Vec4<T> y, int op, int relu) {
+    return {binary_apply(x.x, y.x, op, relu), binary_apply(x.y, y.y, op, relu), binary_apply(x.z, y.z, op, relu),
+            binary_apply(x.w, y.w, op, relu)};
+}
+
+// a, b and d dense in one layout: 16 bytes per thread when `vec` (all three bases 16-byte aligned), then a scalar tail
+// (everything when not)
+template <typename T>
+__global__ void __launch_bounds__(256)
+binary_flat_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d, long long n, int vec, int op, int relu) {
+    with_op(op, [&](auto o) {
+        const long long n4 = vec ? (n >> 2) : 0;
+        const long long stride = (long long)gridDim.x * blockDim.x;
+        for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride)
+            reinterpret_cast<Vec4<T>*>(d)[i] =
+                binary_apply4<T>(reinterpret_cast<const Vec4<T>*>(a)[i], reinterpret_cast<const Vec4<T>*>(b)[i], decltype(o)::value, relu);
+        for (long long j = (n4 << 2) + (long long)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride)
+            d[j] = binary_apply(a[j], b[j], decltype(o)::value, relu);
+    });
+}
+
+// a and d dense, b dense over the TRAILING dims and broadcast over the leading ones (bias rows, position embeddings):
+// d[i] = a[i] (op) b[i mod period], 16 bytes per thread, 32-bit index arithmetic
+template <typename T>
+__global__ void __launch_bounds__(256) binary_periodic_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d,
+                                                              unsigned n4, unsigned period4, int op, int relu) {
+    with_op(op, [&](auto o) {
+        const unsigned stride = gridDim.x * blockDim.x;
+        for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride)
+            reinterpret_cast<Vec4<T>*>(d)[i] = binary_apply4<T>(reinterpret_cast<const Vec4<T>*>(a)[i],
+                                                                reinterpret_cast<const Vec4<T>*>(b)[i % period4],
+                                                                decltype(o)::value, relu);
+    });
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256)
+binary_nd_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d, const NdParams p, int op, int relu) {
     const long long stride = (long long)gridDim.x * blockDim.x;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += stride) {
         long long rem = i, ao = 0, bo = 0, dof = 0;
@@ -893,39 +830,50 @@ __global__ void __launch_bounds__(256) binary_nd_kernel(const T* __restrict__ a,
             bo += idx * p.sb[k];
             dof += idx * p.sd[k];
         }
-        d[dof] = binary_apply<T, OP>(a[ao], b[bo]);
+        d[dof] = binary_apply(a[ao], b[bo], op, relu);
     }
 }
 
-template <typename T, int OP>
-static rten_status launch_binary_typed(rten_ctx* ctx, const T* a, const T* b, T* d, const NdParams& p, bool flat) {
-    if (flat) return launch(ctx, "binary launch", binary_flat_kernel<T, OP>, {ew_grid(ctx, p.n), 256}, a, b, d, p.n);
-    return launch(ctx, "binary launch", binary_nd_kernel<T, OP>, {ew_grid(ctx, p.n), 256}, a, b, d, p);
+template <typename T>
+static rten_status launch_binary_typed(rten_ctx* ctx, int op, int relu, const T* a, const T* b, T* d, int ndim,
+                                       const long long* shape, const long long* sa, const long long* sb, const long long* sd) {
+    // Innermost dim first: `dense` while a and d are dense and b is too, or is from the first dim it broadcasts (stride
+    // 0) over, which makes the dims inside it (`period` elements) a block repeated over the rest.
+    long long n = 1, period = 0;
+    bool dense = true, bcast = false;
+    for (int i = ndim - 1; i >= 0; i--) {
+        if (shape[i] != 1) {
+            dense = dense && sa[i] == n && sd[i] == n;
+            if (!bcast && sb[i] == n) {
+            } else if (sb[i] == 0) {
+                if (!bcast) period = n;
+                bcast = true;
+            } else {
+                dense = false;
+            }
+        }
+        n *= shape[i];
+    }
+    if (n == 0) return RTEN_OK;
+    const bool aligned =
+        ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(d)) & 15) == 0;
+    const char* what = "binary launch";
+    if (dense && !bcast)
+        return launch(ctx, what, binary_flat_kernel<T>, {ew_grid(ctx, aligned ? (n + 3) / 4 : n), 256}, a, b, d, n,
+                      aligned ? 1 : 0, op, relu);
+    if (dense && (period & 3) == 0 && n < 0x7fffffffLL && aligned)
+        return launch(ctx, what, binary_periodic_kernel<T>, {ew_grid(ctx, n / 4), 256}, a, b, d, (unsigned)(n / 4),
+                      (unsigned)(period / 4), op, relu);
+    return launch(ctx, what, binary_nd_kernel<T>, {ew_grid(ctx, n), 256}, a, b, d, nd_params(ndim, shape, sa, sb, sd), op, relu);
 }
 
-rten_status launch_binary(rten_ctx* ctx, int dtype, int op, const void* a, const void* b, void* d, int ndim, const long long* shape,
-                          const long long* sa, const long long* sb, const long long* sd, bool flat) {
-    NdParams p;
-    memset(&p, 0, sizeof(p));
-    p.ndim = ndim;
-    p.n = 1;
-    for (int i = 0; i < ndim; i++) {
-        p.shape[i] = shape[i];
-        p.sa[i] = sa[i];
-        p.sb[i] = sb[i];
-        p.sd[i] = sd[i];
-        p.n *= shape[i];
-    }
-    if (p.n == 0) return RTEN_OK;
-    const int *ai = (const int*)a, *bi = (const int*)b;
-    int* di = (int*)d;
-    if (dtype == RTEN_F32 && op == BIN_SUB) return launch_binary_typed<float, BIN_SUB>(ctx, (const float*)a, (const float*)b, (float*)d, p, flat);
-    if (dtype != RTEN_I32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
-    switch (op) {
-        case BIN_ADD: return launch_binary_typed<int, BIN_ADD>(ctx, ai, bi, di, p, flat);
-        case BIN_SUB: return launch_binary_typed<int, BIN_SUB>(ctx, ai, bi, di, p, flat);
-        default: return launch_binary_typed<int, BIN_MUL>(ctx, ai, bi, di, p, flat);
-    }
+rten_status launch_binary(rten_ctx* ctx, int dtype, int op, int relu, const void* a, const void* b, void* d, int ndim,
+                          const long long* shape, const long long* sa, const long long* sb, const long long* sd) {
+    if (dtype == RTEN_F32)
+        return launch_binary_typed(ctx, op, relu, (const float*)a, (const float*)b, (float*)d, ndim, shape, sa, sb, sd);
+    if (dtype == RTEN_I32)
+        return launch_binary_typed(ctx, op, relu, (const int*)a, (const int*)b, (int*)d, ndim, shape, sa, sb, sd);
+    return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
 }
 
 // =========================================================================================

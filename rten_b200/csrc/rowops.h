@@ -54,14 +54,14 @@ rten_status launch_unary(rten_ctx* ctx, int op, const float* x, float* y, long l
 rten_status launch_clip(rten_ctx* ctx, int is_i32, const void* x, void* y, long long n, const void* mn, const void* mx);
 rten_status launch_nd_copy(rten_ctx* ctx, int esize, const void* src, void* dst, int ndim, const long long* shape,
                            const long long* sstride, const long long* dstride);
-rten_status launch_nd_add(rten_ctx* ctx, const float* a, const float* b, float* d, int ndim, const long long* shape,
-                          const long long* sa, const long long* sb, const long long* sd, int relu);
-rten_status launch_add_flat(rten_ctx* ctx, const float* a, const float* b, float* d, long long n, int relu);
-// d = a (op) b for the operations launch_nd_add / launch_add_flat do not run: f32 Sub (__fsub_rn) and i32 Add / Sub / Mul,
-// which wrap.  Same operand layouts as launch_nd_add; `flat`: a, b and d dense with the same strides (n elements).
+// d = a (op) b over the iteration space `shape`, element strides sa / sb / sd (0 where an operand broadcasts): f32
+// (__fadd_rn / __fsub_rn / __fmul_rn, then Relu when `relu`) or i32 (wrapping).  The flat kernel when a, b and d are
+// dense row-major over `shape` (so a dense view of any layout runs flat when passed as [n] with unit strides), the
+// periodic one when a and d are and b is a dense block of the trailing dims repeated over the leading ones (period a
+// multiple of 4, fewer than 2^31 elements, 16-byte aligned bases), else the strided one.
 enum BinaryOp { BIN_ADD = 0, BIN_SUB = 1, BIN_MUL = 2 };
-rten_status launch_binary(rten_ctx* ctx, int dtype, int op, const void* a, const void* b, void* d, int ndim, const long long* shape,
-                          const long long* sa, const long long* sb, const long long* sd, bool flat);
+rten_status launch_binary(rten_ctx* ctx, int dtype, int op, int relu, const void* a, const void* b, void* d, int ndim,
+                          const long long* shape, const long long* sa, const long long* sb, const long long* sd);
 rten_status launch_minmax(rten_ctx* ctx, const float* x, long long n, int* mm /* 2 ordered ints */);
 // `xch` (batch-sharded runs): the kernel first exchanges the local range in `mm` with the other ranks (comm_device.cuh)
 struct RangeExchange;

@@ -2,14 +2,14 @@
 rowops.cu, each selected by name and checked bit for bit; and the executor's MaxPool / AveragePool ceil_mode and
 auto_pad, which load as the reference reads them.
 
-The launchers (launch_maxpool / launch_avgpool, launch_row_mean, launch_add_flat / launch_nd_add, launch_binary,
-launch_gather_rows / launch_scatter_rows, behind the entry points of api_conv.cu and api_rows.cu) pick a kernel at run
+The launchers (launch_maxpool / launch_avgpool, launch_row_mean, launch_binary, launch_gather_rows /
+launch_scatter_rows, behind the entry points of api_conv.cu and api_rows.cu) pick a kernel at run
 time from the operands' strides, the channel count and pointer alignment.  The rules are restated below (`*_rule`);
 `VARIANTS` lists every kernel they pick from (tests/test_glue_kernel_table_cpu.py keeps it equal to the built library's
 symbols).  Some kernels also take a runtime mode the name does not show: the thread mapping of maxpool_kernel /
-avgpool_kernel (`channels_fastest`, from the output's layout) and the Add / Mul flag of the three f32 add kernels.  The
-case lists reach every (kernel, mode) at least twice, one of them with a partial last unit (a block with idle threads
-or rows, or a scalar tail).
+avgpool_kernel (`channels_fastest`, from the output's layout) and the operation (Add, Sub or Mul) of the three
+broadcast-arithmetic kernels.  The case lists reach every (kernel, mode) at least twice, one of them with a partial last
+unit (a block with idle threads or rows, or a scalar tail).
 
   * kernel identity: every case runs once under CUPTI in a child process; the kernel that ran must be the one the rule
     names, and every kernel of `VARIANTS` must have run;
@@ -22,7 +22,7 @@ or rows, or a scalar tail).
     reference's fold, four layouts and row counts that leave idle lanes, with +-inf, inf - inf and NaN rows;
   * Add / Mul / Sub: exactly the correctly rounded f32 result (float64, rounded once), on dense operands with every
     n % 4, a misaligned operand, bias rows, position tables, two-sided broadcasts, channels-last operands, strided and
-    in-place outputs, signed zeros, inf - inf and NaN; i32 wraps mod 2^32 on the flat and the strided kernel;
+    in-place outputs, signed zeros, inf - inf and NaN; f32 Sub and i32 on the same kernels, i32 wrapping mod 2^32;
   * Gather / Scatter: both gather kernels with column-sliced, misaligned and row-padded tables, negative indices,
     3-D and empty index tensors; scatter into a strided table from strided updates.  Indices stay in range: the gather
     kernels do not bounds-check (the reference returns an error), so an out-of-range index is a contract for the
@@ -43,20 +43,20 @@ pytestmark = pytest.mark.gpu
 F32, I32 = np.float32, np.int32
 
 # ---- the kernels, and the launchers' selection rules ------------------------------------------------------------------
-BIN_TYPES = [("float", 1), ("int", 0), ("int", 1), ("int", 2)]  # <T, OP>: OP 0 Add, 1 Sub, 2 Mul (f32 Sub only)
+BIN_TYPES = [("float",), ("int",)]  # <T>: the operation is a runtime argument
 VARIANTS = {
     "maxpool_cl4_kernel": [()], "maxpool_kernel": [()], "avgpool_cl4_kernel": [()], "avgpool_kernel": [()],
     "row_mean_kernel": [()], "row_mean_thread_kernel": [()],
-    "add_flat_kernel": [()], "add_periodic_kernel": [()], "nd_add_kernel": [()],
-    "binary_flat_kernel": BIN_TYPES, "binary_nd_kernel": BIN_TYPES,
+    "binary_flat_kernel": BIN_TYPES, "binary_periodic_kernel": BIN_TYPES, "binary_nd_kernel": BIN_TYPES,
     "gather_rows_kernel": [()], "gather_rows_vec_kernel": [()], "scatter_rows_kernel": [()],
 }
 # the runtime modes a kernel's name does not show: each (kernel, mode) is a unit of coverage
 MODES = {"maxpool_kernel": ("rows fastest", "channels fastest"), "avgpool_kernel": ("rows fastest", "channels fastest"),
-         "add_flat_kernel": ("Add", "Mul"), "add_periodic_kernel": ("Add", "Mul"), "nd_add_kernel": ("Add", "Mul")}
+         "binary_flat_kernel": ("Add", "Sub", "Mul"), "binary_periodic_kernel": ("Add", "Sub", "Mul"),
+         "binary_nd_kernel": ("Add", "Sub", "Mul")}
 FAMILY_KERNELS = {"pool": ("maxpool_cl4_kernel", "maxpool_kernel", "avgpool_cl4_kernel", "avgpool_kernel"),
                   "gap": ("row_mean_kernel", "row_mean_thread_kernel"),
-                  "binary": ("add_flat_kernel", "add_periodic_kernel", "nd_add_kernel", "binary_flat_kernel", "binary_nd_kernel"),
+                  "binary": ("binary_flat_kernel", "binary_periodic_kernel", "binary_nd_kernel"),
                   "gather": ("gather_rows_kernel", "gather_rows_vec_kernel", "scatter_rows_kernel")}
 KERNELS = set(VARIANTS)
 BLOCK = 256  # threads per block of the elementwise launches (ew_grid)
@@ -157,44 +157,44 @@ def binary_layouts(s):
     return a, b, out, same, shape
 
 
-def binary_rule(s):
-    """binary_op: f32 Add / Mul on launch_add_flat when the operands and output are dense in one layout (its float4
-    kernel when all three are 16-byte aligned, else the strided kernel), else launch_nd_add: the periodic kernel when a
-    and the output are dense and b is a dense block of the trailing dims repeated over the leading ones, whose length
-    (the period) is a multiple of 4, with aligned bases; else the strided kernel.  f32 Sub and i32: the flat kernel
-    when dense in one layout, else the strided one."""
-    a, b, out, same, shape = binary_layouts(s)
-    flat = same and all(d == 1 or so == sa for d, so, sa in zip(shape, out[1], a[1]))
-    mode = "Mul" if s["op"] == "Mul" else "Add"
-    if s["dtype"] == "f32" and s["op"] != "Sub":
-        aligned = _aligned(a[2]) and _aligned(b[2]) and _aligned(out[2])
-        if flat:
-            return ("add_flat_kernel" if aligned else "nd_add_kernel", ()), mode
-        nd = len(shape)
+def _binary_aligned(s):
+    a, b, out, _, _ = binary_layouts(s)
+    return _aligned(a[2]) and _aligned(b[2]) and _aligned(out[2])
 
-        def bstrides(v):  # binary_op's broadcast strides: 0 over a missing or size-1 dim
-            return [0] * (nd - len(v[0])) + [st if d != 1 else 0 for d, st in zip(v[0], v[1])]
-        sa, sb = bstrides(a), bstrides(b)
-        dense, period, ok, bcast = 1, 0, nd >= 1, False
-        for i in range(nd - 1, -1, -1):
-            if not ok:
-                break
-            if shape[i] != 1:
-                ok = sa[i] == dense and out[1][i] == dense
-                if not bcast and sb[i] == dense:
-                    pass
-                elif sb[i] == 0:
-                    if not bcast:
-                        period = dense
-                    bcast = True
-                else:
-                    ok = False
-            dense *= shape[i]
-        if ok and bcast and period > 0 and period % 4 == 0 and 0 < dense < 2 ** 31 - 1 and aligned:
-            return ("add_periodic_kernel", ()), mode
-        return ("nd_add_kernel", ()), mode
-    t = ("float", 1) if s["dtype"] == "f32" else ("int", {"Add": 0, "Sub": 1, "Mul": 2}[s["op"]])
-    return ("binary_flat_kernel" if flat else "binary_nd_kernel", t), None
+
+def binary_rule(s):
+    """binary_op hands launch_binary dense operands and output of one layout as one [n] view with unit strides, anything
+    else with its broadcast strides.  For every type and operation, launch_binary runs the flat kernel when a, b and the
+    output are dense row-major over the iteration space; the periodic kernel when a and the output are and b is a dense
+    block of the trailing dims repeated over the leading ones, whose length (the period) is a multiple of 4, with
+    16-byte aligned bases; else the strided kernel."""
+    a, b, out, same, shape = binary_layouts(s)
+    t = ("float",) if s["dtype"] == "f32" else ("int",)
+    if same and all(d == 1 or so == sa for d, so, sa in zip(shape, out[1], a[1])):
+        return ("binary_flat_kernel", t), s["op"]
+    nd = len(shape)
+
+    def bstrides(v):  # binary_op's broadcast strides: 0 over a missing or size-1 dim
+        return [0] * (nd - len(v[0])) + [st if d != 1 else 0 for d, st in zip(v[0], v[1])]
+    sa, sb = bstrides(a), bstrides(b)
+    n, period, dense, bcast = 1, 0, True, False
+    for i in range(nd - 1, -1, -1):
+        if shape[i] != 1:
+            dense = dense and sa[i] == n and out[1][i] == n
+            if not bcast and sb[i] == n:
+                pass
+            elif sb[i] == 0:
+                if not bcast:
+                    period = n
+                bcast = True
+            else:
+                dense = False
+        n *= shape[i]
+    if dense and not bcast:
+        return ("binary_flat_kernel", t), s["op"]
+    if dense and period % 4 == 0 and n < 2 ** 31 - 1 and _binary_aligned(s):
+        return ("binary_periodic_kernel", t), s["op"]
+    return ("binary_nd_kernel", t), s["op"]
 
 
 def gather_rule(s):
@@ -326,12 +326,16 @@ def binary_specs(sms):
     sub = dict(op="Sub", dtype="f32")
     specs += [dict(sub, kind="dense", a=L((1027,)), b=L((1027,))), dict(sub, kind="dense", a=L((4, 64)), b=L((4, 64))),
               dict(sub, kind="bias", a=L((3, 5, 100)), b=L((100,))), dict(sub, kind="position", a=L((2, 9, 64)), b=L((9, 64))),
-              dict(sub, kind="specials", a=L((2, 9)), b=L((2, 9))), dict(sub, kind="specials", a=L((2, 9)), b=L((9,)))]
+              dict(sub, kind="specials", a=L((2, 9)), b=L((2, 9))), dict(sub, kind="specials", a=L((2, 9)), b=L((9,))),
+              dict(sub, kind="misaligned a", a=L((4, 257), off=1), b=L((4, 257))),
+              dict(sub, kind="position", a=L((3, 5, 6)), b=L((5, 6)))]  # period 30: strided
     for op in ("Add", "Sub", "Mul"):
         i = dict(op=op, dtype="i32")
         specs += [dict(i, kind="dense", a=L((1027,)), b=L((1027,))), dict(i, kind="wrap", a=L((2, 8)), b=L((2, 8))),
                   dict(i, kind="bias", a=L((3, 5, 100)), b=L((100,))), dict(i, kind="wrap", a=L((2, 8)), b=L((8,))),
-                  dict(i, kind="strided out", a=L((5, 33)), b=L((5, 33)), out=L((5, 33), (37, 1)))]
+                  dict(i, kind="strided out", a=L((5, 33)), b=L((5, 33)), out=L((5, 33), (37, 1))),
+                  dict(i, kind="misaligned a", a=L((4, 257), off=1), b=L((4, 257))),
+                  dict(i, kind="both broadcast", a=L((2, 1, 12)), b=L((1, 7, 1)))]
     return specs
 
 
@@ -373,9 +377,9 @@ def partial(fam, s):
         return rows % (8 if k == "row_mean_kernel" else 128) != 0
     if fam == "binary":
         n = int(np.prod(binary_layouts(s)[4]))
-        if k == "add_flat_kernel":
+        if k == "binary_flat_kernel" and _binary_aligned(s):
             return n % 4 != 0
-        return (n // 4 if k == "add_periodic_kernel" else n) % BLOCK != 0
+        return (n // 4 if k == "binary_periodic_kernel" else n) % BLOCK != 0
     n = int(np.prod(s["idx"])) * s["table"][1]
     return (n // 4 if k == "gather_rows_vec_kernel" else n) % BLOCK != 0
 
