@@ -622,6 +622,23 @@ rten_status rten_b200_mul(rten_ctx* ctx, const rten_tensor* a, const rten_tensor
  * of the reduced axes, bit for bit, whatever the input's strides; i32 sums wrap.  An empty reduction gives 0; a 0-D
  * input (n_axes = 0) gives its value plus 0. */
 rten_status rten_b200_reduce_sum(rten_ctx* ctx, const rten_tensor* x, const int32_t* axes, int n_axes, int keep_dims, rten_tensor* out);
+/* TopK (src/ops/reduce.rs topk), f32 or i32 x in any strides: the k largest (largest != 0) or smallest elements along
+ * `axis` (in [-ndim, ndim - 1]), values (x's type) and i32 indices, both with x's shape but k along the axis, best first.
+ * Order: NaN is above every number for both directions (so largest = 0 takes NaNs last); -0.0 and +0.0 are equal;
+ * equal values, and several NaNs, come in ascending index order.  Values are copied bit for bit.  `sorted` is accepted
+ * and ignored: the output is always sorted.  k = 0 gives empty outputs.  Errors: a 0-D x or an axis out of range
+ * "Axis is invalid", k < 0 "k must be positive", k > the axis size "k > dimension size" (RTEN_ERR_INVALID_VALUE);
+ * k > 2048 or an axis of 2^31 or more elements RTEN_ERR_UNSUPPORTED_VALUE.  Outputs are the caller's (data set, any
+ * strides) or allocated (data NULL); one or two launches.  k = 1 runs on the ArgMax kernels. */
+rten_status rten_b200_topk(rten_ctx* ctx, const rten_tensor* x, int64_t k, int axis, int largest, int sorted,
+                           rten_tensor* values_out, rten_tensor* indices_out);
+/* ArgMax / ArgMin (src/ops/reduce.rs arg_max / arg_min: Iterator::max_by), f32 or i32 x in any strides, i32 indices,
+ * one launch.  The index of the first NaN of a lane if it holds one, else of the LAST maximum (ArgMax) or minimum
+ * (ArgMin); -0.0 and +0.0 are equal.  keep_dims != 0 keeps the axis with size 1.  Errors: a 0-D x or an axis out of
+ * range "Axis is invalid", an empty lane "Cannot select index from empty sequence" (RTEN_ERR_INVALID_VALUE); an axis
+ * of 2^31 or more elements RTEN_ERR_UNSUPPORTED_VALUE.  Outputs as for rten_b200_reduce_sum. */
+rten_status rten_b200_arg_max(rten_ctx* ctx, const rten_tensor* x, int axis, int keep_dims, rten_tensor* out);
+rten_status rten_b200_arg_min(rten_ctx* ctx, const rten_tensor* x, int axis, int keep_dims, rten_tensor* out);
 /* MaxPool 2-D (src/ops/pooling.rs): kernel {kh,kw}; pads/strides as conv; padding never wins. */
 rten_status rten_b200_max_pool(rten_ctx* ctx, const rten_tensor* x, const int32_t kernel[2], const int32_t pads[4],
                                const int32_t strides[2], rten_tensor* out);

@@ -167,6 +167,9 @@ _SIGNATURES = {
     "rten_b200_mul": (C.c_int, [_vp, _TP, _TP, _TP]),
     "rten_b200_sub": (C.c_int, [_vp, _TP, _TP, _TP]),
     "rten_b200_reduce_sum": (C.c_int, [_vp, _TP, C.POINTER(C.c_int32), C.c_int, C.c_int, _TP]),
+    "rten_b200_topk": (C.c_int, [_vp, _TP, C.c_int64, C.c_int, C.c_int, C.c_int, _TP, _TP]),
+    "rten_b200_arg_max": (C.c_int, [_vp, _TP, C.c_int, C.c_int, _TP]),
+    "rten_b200_arg_min": (C.c_int, [_vp, _TP, C.c_int, C.c_int, _TP]),
     "rten_b200_conv_integer_ex": (C.c_int, [_vp, _TP, _TP, _vp, _TP, _TP, _TP, _TP, C.POINTER(RtenConvParams), _TP, _TP, C.c_int, _TP, _TP]),
     "rten_b200_range_reset": (C.c_int, [_vp, _TP]),
     "rten_b200_dynamic_quantize_linear_ranged": (C.c_int, [_vp, _TP, _TP, _TP, _TP, _TP, _vp]),

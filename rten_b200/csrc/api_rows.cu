@@ -577,6 +577,107 @@ rten_status rten_b200_reduce_sum(rten_ctx* ctx, const rten_tensor* x, const int3
     return sc.finish(launch_reduce_sum(ctx, x->dtype, p));
 }
 
+// ---- TopK, ArgMax, ArgMin --------------------------------------------------------------------------------
+// One lane per output row along axis `a` of x (any strides); ys[i] is the output stride of input dim i != a, and
+// ys[a] the output stride along the axis (TopK).  p.r.y / p.vals are the caller's.
+static void select_lanes(const rten_tensor& xv, int a, const int64_t* ys, SelectParams& p) {
+    p.r.x = xv.data;
+    p.r.L = xv.shape[a];
+    p.r.nr = 1, p.r.rs[0] = xv.shape[a], p.r.rx[0] = xv.strides[a];
+    p.r.nout = 1;
+    for (int i = 0; i < xv.ndim; i++) {
+        if (i == a) continue;
+        p.r.nout *= xv.shape[i];
+        if (xv.shape[i] == 1) continue;
+        p.r.os[p.r.no] = xv.shape[i], p.r.ox[p.r.no] = xv.strides[i], p.r.oy[p.r.no] = ys[i];
+        p.r.no++;
+    }
+    p.ys = ys[a];
+}
+
+static bool same_layout(const rten_tensor& a, const rten_tensor& b) {
+    for (int i = 0; i < a.ndim; i++)
+        if (a.shape[i] != 1 && a.strides[i] != b.strides[i]) return false;
+    return true;
+}
+
+// src/ops/reduce.rs topk (reduce.rs:1236-1306), with the checks in the reference's order
+rten_status rten_b200_topk(rten_ctx* ctx, const rten_tensor* x, int64_t k, int axis, int largest, int sorted,
+                           rten_tensor* values, rten_tensor* indices) {
+    (void)sorted;  // the output is always sorted, which the reference's unspecified unsorted order allows
+    RTB_TRY(check_ctx(ctx));
+    if (!x || !values || !indices) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    if (x->dtype != RTEN_F32 && x->dtype != RTEN_I32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    if (k < 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "k must be positive");
+    const int nd = x->ndim;
+    const int a = axis < 0 ? axis + nd : axis;
+    if (a < 0 || a >= nd) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Axis is invalid");
+    if (k > 0 && k > x->shape[a]) return fail(ctx, RTEN_ERR_INVALID_VALUE, "k > dimension size");
+    if (k > TOPK_MAX_K) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "TopK: k > 2048 is not supported");
+    if (x->shape[a] > INT32_MAX)
+        return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "TopK: an axis of 2^31 or more elements is not supported (i32 indices)");
+    int64_t oshape[RTEN_MAX_DIMS];
+    for (int i = 0; i < nd; i++) oshape[i] = i == a ? k : x->shape[i];
+    OpScope sc(ctx);
+    rten_tensor xv, vv, iv;
+    RTB_TRY(sc.in(x, &xv));
+    RTB_TRY(sc.out(values, x->dtype, nd, oshape, &vv, nullptr));
+    RTB_TRY(sc.out(indices, RTEN_I32, nd, oshape, &iv, vv.strides));
+    if (numel(&vv) == 0) return sc.finish(RTEN_OK);
+    // the kernels write both outputs at the same offsets: indices laid out otherwise go through a copy
+    rten_tensor ik = iv;
+    if (!same_layout(vv, iv)) {
+        ik = vv;
+        ik.dtype = RTEN_I32;
+        RTB_TRY(temp_alloc(ctx, (size_t)span_elems(&vv) * 4, &ik.data));
+    }
+    SelectParams p;
+    select_lanes(xv, a, vv.strides, p);
+    p.r.y = ik.data;
+    p.vals = vv.data;
+    p.k = (int)k;
+    p.mode = largest ? SEL_LARGEST : SEL_SMALLEST;
+    RTB_TRY(launch_topk(ctx, x->dtype, p));
+    if (ik.data != iv.data) RTB_TRY(copy_view(ctx, ik, iv));
+    return sc.finish(RTEN_OK);
+}
+
+// src/ops/reduce.rs select_max_index (reduce.rs:62-177)
+static rten_status arg_select(rten_ctx* ctx, const rten_tensor* x, int axis, int keep_dims, rten_tensor* out, int mode) {
+    RTB_TRY(check_ctx(ctx));
+    if (!x || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    if (x->dtype != RTEN_F32 && x->dtype != RTEN_I32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    const int nd = x->ndim;
+    const int a = axis < 0 ? axis + nd : axis;
+    if (a < 0 || a >= nd) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Axis is invalid");
+    if (x->shape[a] == 0) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Cannot select index from empty sequence");
+    if (x->shape[a] > INT32_MAX)
+        return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "ArgMax / ArgMin: an axis of 2^31 or more elements is not supported (i32 indices)");
+    int ond = 0;
+    int64_t oshape[RTEN_MAX_DIMS];
+    for (int i = 0; i < nd; i++)
+        if (i != a || keep_dims) oshape[ond++] = i == a ? 1 : x->shape[i];
+    OpScope sc(ctx);
+    rten_tensor xv, ov;
+    RTB_TRY(sc.in(x, &xv));
+    RTB_TRY(sc.out(out, RTEN_I32, ond, oshape, &ov, nullptr));
+    if (numel(&ov) == 0) return sc.finish(RTEN_OK);
+    int64_t ys[RTEN_MAX_DIMS];
+    for (int i = 0, o = 0; i < nd; i++) ys[i] = (i != a || keep_dims) ? ov.strides[o++] : 0;
+    SelectParams p;
+    select_lanes(xv, a, ys, p);
+    p.r.y = ov.data;
+    p.mode = mode;
+    return sc.finish(launch_arg_reduce(ctx, x->dtype, p));
+}
+
+rten_status rten_b200_arg_max(rten_ctx* ctx, const rten_tensor* x, int axis, int keep_dims, rten_tensor* out) {
+    return arg_select(ctx, x, axis, keep_dims, out, SEL_ARGMAX);
+}
+rten_status rten_b200_arg_min(rten_ctx* ctx, const rten_tensor* x, int axis, int keep_dims, rten_tensor* out) {
+    return arg_select(ctx, x, axis, keep_dims, out, SEL_ARGMIN);
+}
+
 // ---- DynamicQuantizeLinear ---------------------------------------------------------------------------
 rten_status rten_b200_range_reset(rten_ctx* ctx, rten_tensor* ranges) {
     RTB_TRY(check_ctx(ctx));

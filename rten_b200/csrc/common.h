@@ -148,6 +148,7 @@ struct LaunchShape {
     size_t smem = 0;     // dynamic shared memory, bytes
     int smem_optin = 0;  // > 0: the kernel's MaxDynamicSharedMemorySize is set to this before the launch
     bool pdl = false;    // programmatic dependent launch: the kernel must pdl_wait() (ptx.cuh) before it reads its inputs
+    int cluster = 0;     // > 1: thread-block clusters of this many CTAs along x (> 8 opts in to the non-portable size)
 };
 
 // Launches `kern` on the context stream and counts it.  A failed launch returns RTEN_ERR_CUDA with `what` in the
@@ -160,15 +161,19 @@ rten_status launch(rten_ctx* ctx, const char* what, void (*kern)(P...), const La
     cfg.blockDim = s.block;
     cfg.dynamicSmemBytes = s.smem;
     cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
+    cudaLaunchAttribute attr[2];
+    cfg.attrs = attr;
     if (s.pdl && !getenv("RTEN_B200_NO_PDL")) {
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
+        attr[cfg.numAttrs].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[cfg.numAttrs++].val.programmaticStreamSerializationAllowed = 1;
+    }
+    if (s.cluster > 1) {
+        attr[cfg.numAttrs].id = cudaLaunchAttributeClusterDimension;
+        attr[cfg.numAttrs++].val.clusterDim = {(unsigned)s.cluster, 1, 1};
     }
     cudaError_t e = cudaSuccess;
     if (s.smem_optin > 0) e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, s.smem_optin);
+    if (e == cudaSuccess && s.cluster > 8) e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
     if (e == cudaSuccess) e = cudaLaunchKernelEx(&cfg, kern, std::forward<A>(args)...);
     const cudaError_t last = cudaGetLastError();
     if (e == cudaSuccess) e = last;

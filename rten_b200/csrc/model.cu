@@ -874,6 +874,41 @@ rten_status run_reduce_sum(Runner& r, OpNode& o, rten_tensor* y) {
     return rten_b200_reduce_sum(r.ctx, x, a.data(), (int)a.size(), (int)o.n.attr_i("keepdims", 1), y);
 }
 
+// TopK (src/ops/reduce.rs:1236-1306): K is input 1 (opset >= 10) or the `k` attribute (opset < 10).  A host-known K
+// (a constant, or Shape -> Gather) costs nothing; a device-resident K is copied to the host and waited for, which
+// keeps a step holding this node out of CUDA-graph capture.
+rten_status run_topk(Runner& r, OpNode& o, rten_tensor* y) {
+    int64_t k = 0;
+    if (o.n.attr("k")) {
+        k = o.n.attr_i("k", 0);
+    } else {
+        const rten_tensor* kt = r.T(o, 1);
+        if (!kt) return mfail(r.ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+        if (numel(kt) != 1 || kt->dtype != RTEN_I32) return mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "TopK: K must be one integer");
+        const ValueSlot& kv = r.V(o.in[1]);
+        if (kv.has_host_ints) {
+            k = kv.host_ints[0];
+        } else {
+            int32_t hk = 0;
+            RTB_CUDA(r.ctx, cudaMemcpyAsync(&hk, kt->data, 4, cudaMemcpyDeviceToHost, r.ctx->stream));
+            RTB_CUDA(r.ctx, cudaStreamSynchronize(r.ctx->stream));
+            k = hk;
+        }
+    }
+    rten_tensor idx{};
+    RTB_TRY(rten_b200_topk(r.ctx, r.T(o, 0), k, (int)o.n.attr_i("axis", -1), (int)o.n.attr_i("largest", 1),
+                           (int)o.n.attr_i("sorted", 1), y, &idx));
+    r.set_output(o, 1, idx);
+    return RTEN_OK;
+}
+
+// ArgMax / ArgMin (src/op_registry/onnx_registry.rs get_common_arg_reduce_attrs): select_last_index must be 0
+rten_status load_arg_reduce(rten_model* m, onnx::Node& n) {
+    if (n.attr_i("select_last_index", 0) != 0)
+        return mfail(m->ctx, RTEN_ERR_UNSUPPORTED_VALUE, n.op_type + ": select_last_index = 1 is not supported");
+    return RTEN_OK;
+}
+
 // Shape (src/ops/layout.rs): the input's dims [start, end) -- negative from the end, clamped to [0, ndim], end at least
 // start -- as a host value
 rten_status run_shape(Runner& r, OpNode& o, rten_tensor*) {
@@ -1008,6 +1043,13 @@ constexpr OpDef OPS[] = {
      }},
     {"GlobalAveragePool", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_global_average_pool(r.ctx, r.T(o, 0), y); }},
     {"ReduceSum", ONNX, 0, 0b1, run_reduce_sum},
+    {"TopK", ONNX, 0, 0b1, run_topk},
+    {"ArgMax", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
+         return rten_b200_arg_max(r.ctx, r.T(o, 0), (int)o.n.attr_i("axis", 0), (int)o.n.attr_i("keepdims", 1), y); },
+     load_arg_reduce},
+    {"ArgMin", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
+         return rten_b200_arg_min(r.ctx, r.T(o, 0), (int)o.n.attr_i("axis", 0), (int)o.n.attr_i("keepdims", 1), y); },
+     load_arg_reduce},
     {"Shape", ONNX, 0, 0b1, run_shape},
     {"ReduceMean", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
          const rten_tensor* x = r.T(o, 0);

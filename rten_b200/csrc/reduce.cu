@@ -10,6 +10,12 @@
 //     never straddle two stages.
 // i32 sums wrap, and every order gives the same result: the threads add their own elements and the partial sums are
 // combined in any order, in registers.
+//
+// ArgMax, ArgMin and TopK with k = 1 (arg_reduce_*_kernel) take the largest composite key of each lane (select.cuh), a
+// total order, so partial maxima combine in any order.  Short lanes: one warp per output; long lanes: one CTA per
+// output, or, when the outputs are too few to give every SM one, one thread-block cluster per output whose CTAs take
+// contiguous slices of the lane and combine their maxima through distributed shared memory.
+#include <cooperative_groups.h>
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -36,17 +42,6 @@ __device__ __forceinline__ long long lane_off(const ReduceParams& p, long long j
         j = q;
     }
     return off;
-}
-
-__device__ __forceinline__ void out_offs(const ReduceParams& p, long long o, long long& xo, long long& yo) {
-    xo = 0, yo = 0;
-#pragma unroll 1
-    for (int k = p.no - 1; k >= 0; k--) {
-        const long long s = p.os[k], q = o / s, i = o - q * s;
-        xo += i * p.ox[k];
-        yo += i * p.oy[k];
-        o = q;
-    }
 }
 
 template <typename T>
@@ -157,6 +152,124 @@ __global__ void __launch_bounds__(RC_THREADS) reduce_sum_cta_kernel(const Reduce
     }
 }
 
+// ---- arg-reduce --------------------------------------------------------------------------------------------------------
+constexpr int AC_THREADS = 256, AC_MIN_SLICE = 2048;  // CTA / cluster kernels; a cluster gives each CTA >= AC_MIN_SLICE
+
+// this thread's largest key among the lane elements j = j0 + t, j0 + t + nt, ... < j1
+template <typename T>
+__device__ __forceinline__ uint64_t arg_partial(const SelectParams& a, const T* x, long long j0, long long j1, int t, int nt) {
+    const ReduceParams& p = a.r;
+    const bool contig = p.nr == 0 || p.rx[0] == 1;
+    uint64_t best = 0;  // below or equal to every key
+    auto take = [&](T v, long long j) {
+        const uint64_t k = sel_key(v, (uint32_t)j, a.mode);
+        best = k > best ? k : best;
+    };
+    if (contig && (reinterpret_cast<uintptr_t>(x + j0) & 15) == 0) {  // 16-byte loads: four elements in flight each
+        const long long n4 = (j1 - j0) >> 2;
+        const Vec4<T>* x4 = reinterpret_cast<const Vec4<T>*>(x + j0);
+        for (long long q = t; q < n4; q += nt) {
+            const Vec4<T> v = x4[q];
+            const long long j = j0 + 4 * q;
+            take(v.x, j), take(v.y, j + 1), take(v.z, j + 2), take(v.w, j + 3);
+        }
+        j0 += 4 * n4;
+    }
+    for (long long j = j0 + t; j < j1; j += nt) {
+        const uint64_t k = sel_key(contig ? x[j] : x[lane_off(p, j)], (uint32_t)j, a.mode);
+        best = k > best ? k : best;
+    }
+    return best;
+}
+
+template <typename T>
+__device__ __forceinline__ void arg_store(const SelectParams& a, const T* x, long long yo, uint64_t best) {
+    const uint32_t i = sel_index<T>(best, a.mode);
+    static_cast<int*>(a.r.y)[yo] = (int)i;
+    if (a.vals) static_cast<T*>(a.vals)[yo] = x[lane_off(a.r, i)];
+}
+
+// the CTA's largest key, in every thread
+__device__ __forceinline__ uint64_t block_max_u64(uint64_t v, uint64_t* part) {
+    v = warp_max_u64(v);
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
+    __syncthreads();
+    v = (threadIdx.x & 31) < AC_THREADS / 32 ? part[threadIdx.x & 31] : 0;
+    v = warp_max_u64(v);
+    __syncthreads();  // (part is reused)
+    return v;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(RW_WARPS * 32) arg_reduce_warp_kernel(const SelectParams a) {
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (long long o = (long long)blockIdx.x * RW_WARPS + w; o < a.r.nout; o += (long long)gridDim.x * RW_WARPS) {
+        long long xo, yo;
+        out_offs(a.r, o, xo, yo);
+        const T* x = static_cast<const T*>(a.r.x) + xo;
+        const uint64_t best = warp_max_u64(arg_partial<T>(a, x, 0, a.r.L, lane, 32));
+        if (lane == 0) arg_store<T>(a, x, yo, best);
+    }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(AC_THREADS) arg_reduce_cta_kernel(const SelectParams a) {
+    __shared__ uint64_t part[AC_THREADS / 32];
+    for (long long o = blockIdx.x; o < a.r.nout; o += gridDim.x) {
+        long long xo, yo;
+        out_offs(a.r, o, xo, yo);
+        const T* x = static_cast<const T*>(a.r.x) + xo;
+        const uint64_t best = block_max_u64(arg_partial<T>(a, x, 0, a.r.L, threadIdx.x, AC_THREADS), part);
+        if (threadIdx.x == 0) arg_store<T>(a, x, yo, best);
+    }
+}
+
+// one cluster per output: CTA `rank` takes elements [rank * S, (rank + 1) * S) of the lane, rank 0 combines
+template <typename T>
+__global__ void __launch_bounds__(AC_THREADS) arg_reduce_cluster_kernel(const SelectParams a) {
+    namespace cg = cooperative_groups;
+    cg::cluster_group cl = cg::this_cluster();
+    const int C = (int)cl.num_blocks(), rank = (int)cl.block_rank();
+    __shared__ uint64_t part[AC_THREADS / 32];
+    __shared__ uint64_t cta_best;
+    const long long S = ((a.r.L + C - 1) / C + 3) & ~3LL, j0 = min(a.r.L, rank * S), j1 = min(a.r.L, j0 + S);
+    for (long long o = blockIdx.x / C; o < a.r.nout; o += gridDim.x / C) {
+        long long xo, yo;
+        out_offs(a.r, o, xo, yo);
+        const T* x = static_cast<const T*>(a.r.x) + xo;
+        const uint64_t best = block_max_u64(arg_partial<T>(a, x, j0, j1, threadIdx.x, AC_THREADS), part);
+        if (threadIdx.x == 0) cta_best = best;
+        cl.sync();
+        if (rank == 0 && threadIdx.x < 32) {
+            uint64_t v = threadIdx.x < C ? *cl.map_shared_rank(&cta_best, (int)threadIdx.x) : 0;
+            v = warp_max_u64(v);
+            if (threadIdx.x == 0) arg_store<T>(a, x, yo, v);
+        }
+        cl.sync();  // rank 0 has read every CTA's cta_best
+    }
+}
+
+template <typename T>
+rten_status launch_arg_typed(rten_ctx* ctx, const SelectParams& a) {
+    const ReduceParams& p = a.r;
+    const long long cap = (long long)ctx->num_sms * 8;
+    if (p.L <= RW_MAX) {
+        const LaunchShape s{dim3((unsigned)std::min(cap, (p.nout + RW_WARPS - 1) / RW_WARPS)), dim3(RW_WARPS * 32)};
+        return launch(ctx, "arg_reduce launch", arg_reduce_warp_kernel<T>, s, a);
+    }
+    // a cluster per lane while the lanes leave SMs idle, each CTA with at least AC_MIN_SLICE elements
+    long long C = std::min({16LL, (ctx->num_sms + p.nout - 1) / p.nout, (p.L + AC_MIN_SLICE - 1) / AC_MIN_SLICE});
+    if (C >= 2) {
+        LaunchShape s{dim3(1), dim3(AC_THREADS)};
+        C = cluster_size_fit<arg_reduce_cluster_kernel<T>>((int)C, s);
+        s.grid = dim3((unsigned)(std::min(p.nout, 65535LL) * C));
+        s.cluster = (int)C;
+        return launch(ctx, "arg_reduce launch", arg_reduce_cluster_kernel<T>, s, a);
+    }
+    const LaunchShape s{dim3((unsigned)std::min(cap, p.nout)), dim3(AC_THREADS)};
+    return launch(ctx, "arg_reduce launch", arg_reduce_cta_kernel<T>, s, a);
+}
+
 template <typename T>
 rten_status launch_typed(rten_ctx* ctx, const ReduceParams& p) {
     const long long cap = (long long)ctx->num_sms * 8;
@@ -175,6 +288,11 @@ rten_status launch_typed(rten_ctx* ctx, const ReduceParams& p) {
 rten_status launch_reduce_sum(rten_ctx* ctx, int dtype, const ReduceParams& p) {
     if (p.nout == 0) return RTEN_OK;
     return dtype == RTEN_F32 ? launch_typed<float>(ctx, p) : launch_typed<int>(ctx, p);
+}
+
+rten_status launch_arg_reduce(rten_ctx* ctx, int dtype, const SelectParams& a) {
+    if (a.r.nout == 0) return RTEN_OK;
+    return dtype == RTEN_F32 ? launch_arg_typed<float>(ctx, a) : launch_arg_typed<int>(ctx, a);
 }
 
 }  // namespace rtb

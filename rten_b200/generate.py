@@ -192,6 +192,15 @@ class ArgMaxSampler:
     def sample(self, logits: np.ndarray) -> np.ndarray:
         return logits.argmax(-1).astype(np.int32)
 
+    def can_sample_device(self, logits: O.DeviceTensor) -> bool:
+        return True
+
+    def sample_device(self, logits: O.DeviceTensor) -> np.ndarray:
+        """`sample` of device-resident `[batch, vocab]` logits (any strides): TopK with k = 1 on the GPU -- the first
+        maximum, or the first NaN, as np.argmax -- and B indices copied back."""
+        _, idx = O.TopK(axis=-1).run(logits.ctx, logits, 1)
+        return idx.numpy()[:, 0].astype(np.int32)
+
 
 class TopKSampler:
     """rten-generate/src/sampler.rs TopK: sample from the softmax of the k largest logits / temperature (seeded)."""
@@ -201,7 +210,23 @@ class TopKSampler:
 
     def sample(self, logits: np.ndarray) -> np.ndarray:
         idx = np.argsort(-logits, axis=-1)[:, :self.k]
-        top = np.take_along_axis(logits, idx, -1) / self.temperature
+        return self._draw(np.take_along_axis(logits, idx, -1), idx)
+
+    def can_sample_device(self, logits: O.DeviceTensor) -> bool:
+        """TopK on the device takes k up to TOPK_MAX_K (2048) and at most the vocabulary; any other k samples on the
+        host, as before"""
+        return 0 < self.k <= min(O.TOPK_MAX_K, logits.shape[-1])
+
+    def sample_device(self, logits: O.DeviceTensor) -> np.ndarray:
+        """`sample` of device-resident `[batch, vocab]` logits (any strides): TopK(k) on the GPU, B x k values and
+        indices copied back, then the same temperature, softmax and draws as `sample`.  The tokens and the random stream
+        are those of `sample` wherever its result is determined: no NaN and no ties among the k + 1 largest logits of a
+        row (argsort's order among ties is unspecified; TopK takes the lowest index)."""
+        vals, idx = O.TopK(axis=-1).run(logits.ctx, logits, self.k)
+        return self._draw(vals.numpy(), idx.numpy())
+
+    def _draw(self, vals: np.ndarray, idx: np.ndarray) -> np.ndarray:
+        top = vals / self.temperature
         p = np.exp(top - top.max(-1, keepdims=True))
         p /= p.sum(-1, keepdims=True)
         pick = [self.rng.choice(self.k, p=row) for row in p]
@@ -241,7 +266,17 @@ class Generator:
         self._seq_len = 0
         self.sampler = ArgMaxSampler()
         self.logits_filters: List[Callable[[np.ndarray, np.ndarray], np.ndarray]] = []
-        self.last_logits: Optional[np.ndarray] = None
+        self._last_logits: Optional[np.ndarray] = None
+        self._last_device = None  # the step's device logits, until last_logits copies them
+
+    @property
+    def last_logits(self) -> Optional[np.ndarray]:
+        """The logits the last step sampled from, `[batch, vocab]` on the host (after the logits filters).  Without
+        filters the step samples on the device; the logits are then copied here on first access."""
+        if self._last_logits is None and self._last_device is not None:
+            self._last_logits = self._last_device.numpy()
+            self._last_device = None
+        return self._last_logits
 
     @classmethod
     def from_model(cls, model) -> "Generator":
@@ -296,12 +331,20 @@ class Generator:
         for i, o in self.kv_pairs:  # the present.* of this step is the past_key_values.* of the next (:858-886)
             self.kv_cache[i] = out[o]
         self._seq_len += T
-        logits = out["logits"].numpy()
-        prev = self.prev_tokens()
-        for f in self.logits_filters:
-            logits = f(logits, prev)
-        self.last_logits = logits
-        tok = self.sampler.sample(logits)
+        dev = out["logits"]
+        on_device = (not self.logits_filters and isinstance(dev, O.DeviceTensor) and hasattr(self.sampler, "can_sample_device")
+                     and self.sampler.can_sample_device(dev))
+        if on_device:
+            # sampled on the device: only the picked tokens (and TopK's k candidates) reach the host
+            self._last_logits, self._last_device = None, dev
+            tok = self.sampler.sample_device(dev)
+        else:
+            logits = dev.numpy()
+            prev = self.prev_tokens()
+            for f in self.logits_filters:
+                logits = f(logits, prev)
+            self._last_logits, self._last_device = logits, None
+            tok = self.sampler.sample(logits)
         self._tokens.append(tok)
         self._prompt = tok[:, None]  # next step feeds the sampled token
         return tok

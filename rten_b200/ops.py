@@ -1037,6 +1037,44 @@ class Sub:
         return A.wrap(o, out)
 
 
+TOPK_MAX_K = 2048  # the largest k rten_b200_topk takes (RTEN_ERR_UNSUPPORTED_VALUE above)
+
+
+class TopK:
+    """src/ops/reduce.rs topk (f32 or i32): the k largest (or smallest) elements along `axis` and their i32 indices,
+    best first, ties by ascending index; NaN is above every number in both directions, -0.0 equals +0.0.  The output is
+    always sorted (`sorted` is accepted for the ONNX attribute).  k <= TOPK_MAX_K."""
+
+    def __init__(self, axis: int = -1, largest: bool = True, sorted: bool = True):
+        self.axis, self.largest, self.sorted = int(axis), bool(largest), bool(sorted)
+
+    def run(self, ctx, x, k: int, values_out=None, indices_out=None):
+        A = _Args(ctx)
+        v, i = A.out(values_out), A.out(indices_out)
+        ctx.check(ctx.lib.rten_b200_topk(ctx.handle, A.t(x), int(k), self.axis, int(self.largest), int(self.sorted),
+                                         C.byref(v), C.byref(i)))
+        return A.wrap(v, values_out), A.wrap(i, indices_out)
+
+
+class ArgMax:
+    """src/ops/reduce.rs arg_max (f32 or i32 -> i32): the first NaN's index, else the last maximum's."""
+    _fn = "rten_b200_arg_max"
+
+    def __init__(self, axis: int = 0, keep_dims: bool = True):
+        self.axis, self.keep_dims = int(axis), bool(keep_dims)
+
+    def run(self, ctx, x, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        ctx.check(getattr(ctx.lib, self._fn)(ctx.handle, A.t(x), self.axis, int(self.keep_dims), C.byref(o)))
+        return A.wrap(o, out)
+
+
+class ArgMin(ArgMax):
+    """src/ops/reduce.rs arg_min (f32 or i32 -> i32): the first NaN's index, else the last minimum's."""
+    _fn = "rten_b200_arg_min"
+
+
 class ReduceSum:
     """src/ops/reduce.rs ReduceSum (f32 or wrapping i32): axes None or empty reduces every axis, unless
     noop_with_empty_axes, which makes it a copy."""
