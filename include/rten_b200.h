@@ -580,6 +580,21 @@ rten_status rten_b200_sigmoid(rten_ctx* ctx, const rten_tensor* x, rten_tensor* 
 rten_status rten_b200_silu(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
 rten_status rten_b200_hard_sigmoid(rten_ctx* ctx, const rten_tensor* x, float alpha, float beta, rten_tensor* out);
 rten_status rten_b200_hard_swish(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
+/* Sqrt, Reciprocal, Exp, Tanh, Neg and Abs, f32 only, bit-identical to the reference including +-0, +-inf and NaN:
+ *   Sqrt        IEEE square root (x.sqrt())             src/ops/unary_elementwise.rs:743-745
+ *   Reciprocal  1 / x, IEEE division                    :607-609 (1 / +-0 = +-inf)
+ *   Exp         rten-vecmath's Exp (inf from 104 on, 0 from -104 down)   :391, rten-vecmath/src/exp.rs
+ *   Tanh        rten-vecmath's Tanh                      :758, rten-vecmath/src/tanh.rs
+ *   Neg         -x, the sign bit flipped (-(+0) = -0)    :550-555
+ *   Abs         the sign bit cleared                      :195-220
+ * x in any strides; `out` may alias `x` (run_in_place).  One kernel launch for dense device-resident x, capturable in a
+ * CUDA graph.  None of them is a convolution-epilogue activation. */
+rten_status rten_b200_sqrt(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
+rten_status rten_b200_reciprocal(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
+rten_status rten_b200_exp(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
+rten_status rten_b200_tanh(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
+rten_status rten_b200_neg(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
+rten_status rten_b200_abs(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
 /* Communicator of a batch-sharded run (one process per GPU).  The reference has no counterpart (single process, rayon
  * threads); it exists so that DynamicQuantizeLinear can use the range of the WHOLE tensor when the batch is split over
  * ranks.  NCCL (libnccl.so.2) is resolved with dlopen at the first call; rank 0 creates the 128-byte id, the host
@@ -616,12 +631,35 @@ rten_status rten_b200_relu(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out
 rten_status rten_b200_add(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
 rten_status rten_b200_sub(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
 rten_status rten_b200_mul(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
+/* Div (src/ops/binary_elementwise.rs:600-638) with numpy broadcasting, a and b of the same type:
+ *   f32: a / b, IEEE-rounded; x / 0 is +-inf or NaN.  A b of exactly one element (any rank) is the reference's
+ *        "division as multiplication-by-reciprocal": a * (1 / b), two roundings, and the output takes a's shape, not
+ *        the broadcast one (Div(a[4], b[1, 1]) is [4]).  b is read on the device.
+ *   i32: truncates toward zero.  A zero divisor returns RTEN_ERR_INVALID_VALUE "Divisor contains zero", as the reference
+ *        does, and so does INT_MIN / -1 (an overflow panic in Rust).  An i32 Div SYNCHRONISES with the host: the
+ *        kernel's flag is read back after the launch (so it cannot be captured in a CUDA graph).  On an error the
+ *        outputs the call allocated are freed.  Every element of b is checked, also when the output is empty (the
+ *        reference checks b before broadcasting). */
+rten_status rten_b200_div(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
+/* Pow (src/ops/binary_elementwise.rs:965-1029, FastPow) with numpy broadcasting, base a and exponent b:
+ *   f32 ^ f32: exponent 2 is x * x, 3 is x * x * x (rounded left to right), both bit-identical to the reference; any
+ *              other exponent is CUDA's powf, within its documented 4 ulp of the exact result (the reference's is libm's).
+ *   i32 ^ i32: exponents >= 0 wrap (wrapping_pow); a negative one is computed as f32 powf(x, e) and converted back with
+ *              Rust's saturating `as i32` (NaN -> 0): 1 ^ -n = 1, 0 ^ -n = INT32_MAX, |x| >= 2 gives 0.
+ * A one-element exponent (any rank) maps the base: the output takes a's shape (the reference's map_in).  Mixed types
+ * (the reference's i32 ^ f32) return RTEN_ERR_UNSUPPORTED_TYPE: that case is left out. */
+rten_status rten_b200_pow(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
 /* ReduceSum (src/ops/reduce.rs), f32 or i32, one launch.  `axes` (n_axes values in [-ndim, ndim - 1], duplicates
  * allowed) are the reduced axes; n_axes = 0 reduces every axis.  keep_dims != 0 keeps them as size-1 axes.  Each f32
  * output is the reference's Sum (the 64-chain fold of rten-vecmath/src/sum.rs) of its elements taken in row-major order
  * of the reduced axes, bit for bit, whatever the input's strides; i32 sums wrap.  An empty reduction gives 0; a 0-D
  * input (n_axes = 0) gives its value plus 0. */
 rten_status rten_b200_reduce_sum(rten_ctx* ctx, const rten_tensor* x, const int32_t* axes, int n_axes, int keep_dims, rten_tensor* out);
+/* ReduceMean (src/ops/reduce.rs:524-541), f32 only, one launch: each output is rten_b200_reduce_sum's Sum of its lane
+ * divided by the lane length as f32 (one IEEE division).  An empty lane gives NaN.  Axes, keep_dims, strides and a 0-D
+ * input as rten_b200_reduce_sum. */
+rten_status rten_b200_reduce_mean(rten_ctx* ctx, const rten_tensor* x, const int32_t* axes, int n_axes, int keep_dims,
+                                  rten_tensor* out);
 /* TopK (src/ops/reduce.rs topk), f32 or i32 x in any strides: the k largest (largest != 0) or smallest elements along
  * `axis` (in [-ndim, ndim - 1]), values (x's type) and i32 indices, both with x's shape but k along the axis, best first.
  * Order: NaN is above every number for both directions (so largest = 0 takes NaNs last); -0.0 and +0.0 are equal;

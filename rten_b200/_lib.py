@@ -166,7 +166,16 @@ _SIGNATURES = {
     "rten_b200_add": (C.c_int, [_vp, _TP, _TP, _TP]),
     "rten_b200_mul": (C.c_int, [_vp, _TP, _TP, _TP]),
     "rten_b200_sub": (C.c_int, [_vp, _TP, _TP, _TP]),
+    "rten_b200_div": (C.c_int, [_vp, _TP, _TP, _TP]),
+    "rten_b200_pow": (C.c_int, [_vp, _TP, _TP, _TP]),
+    "rten_b200_sqrt": (C.c_int, [_vp, _TP, _TP]),
+    "rten_b200_reciprocal": (C.c_int, [_vp, _TP, _TP]),
+    "rten_b200_exp": (C.c_int, [_vp, _TP, _TP]),
+    "rten_b200_tanh": (C.c_int, [_vp, _TP, _TP]),
+    "rten_b200_neg": (C.c_int, [_vp, _TP, _TP]),
+    "rten_b200_abs": (C.c_int, [_vp, _TP, _TP]),
     "rten_b200_reduce_sum": (C.c_int, [_vp, _TP, C.POINTER(C.c_int32), C.c_int, C.c_int, _TP]),
+    "rten_b200_reduce_mean": (C.c_int, [_vp, _TP, C.POINTER(C.c_int32), C.c_int, C.c_int, _TP]),
     "rten_b200_topk": (C.c_int, [_vp, _TP, C.c_int64, C.c_int, C.c_int, C.c_int, _TP, _TP]),
     "rten_b200_arg_max": (C.c_int, [_vp, _TP, C.c_int, C.c_int, _TP]),
     "rten_b200_arg_min": (C.c_int, [_vp, _TP, C.c_int, C.c_int, _TP]),

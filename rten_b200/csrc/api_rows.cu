@@ -1,4 +1,5 @@
-// Operator entry points of the C ABI, row / elementwise operators (Softmax, LayerNormalization, Erf / Gelu / Relu, Add / Mul,
+// Operator entry points of the C ABI, row / elementwise operators (Softmax, LayerNormalization, Erf / Gelu / Relu / Sqrt / Exp
+// / Tanh ..., Add / Mul / Div / Pow, ReduceSum / ReduceMean,
 // DynamicQuantizeLinear, Gather / Scatter rows): shape / argument validation with the reference's error strings,
 // operand normalisation (K-major, TMA-addressable), kernel dispatch.  Mirrors, per function, the
 // reference operator named in include/rten_b200.h.
@@ -468,10 +469,21 @@ rten_status rten_b200_hard_sigmoid(rten_ctx* ctx, const rten_tensor* x, float al
 rten_status rten_b200_hard_swish(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out) {
     return unary_op(ctx, UNARY_HARD_SWISH, x, out);
 }
+rten_status rten_b200_sqrt(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out) { return unary_op(ctx, UNARY_SQRT, x, out); }
+rten_status rten_b200_reciprocal(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out) {
+    return unary_op(ctx, UNARY_RECIPROCAL, x, out);
+}
+rten_status rten_b200_exp(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out) { return unary_op(ctx, UNARY_EXP, x, out); }
+rten_status rten_b200_tanh(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out) { return unary_op(ctx, UNARY_TANH, x, out); }
+rten_status rten_b200_neg(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out) { return unary_op(ctx, UNARY_NEG, x, out); }
+rten_status rten_b200_abs(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out) { return unary_op(ctx, UNARY_ABS, x, out); }
 
-// ---- Add / Sub / Mul ----------------------------------------------------------------------------------
-// Add / Sub / Mul with numpy broadcasting (src/ops/binary_elementwise.rs), f32 or i32 (wrapping).
-static rten_status binary_op(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out, int op) {
+// ---- Add / Sub / Mul / Div / Pow ----------------------------------------------------------------------------
+// Add / Sub / Mul / Div / Pow with numpy broadcasting (src/ops/binary_elementwise.rs), f32 or i32.  `scalar_b`: a
+// one-element b is the 0-D scalar the reference maps a with (Div's multiplication by the reciprocal, Pow's map_in), so
+// the output takes a's shape.
+static rten_status binary_op(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out, int op,
+                             bool scalar_b = false) {
     RTB_TRY(check_ctx(ctx));
     if (!a || !b || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
     if ((a->dtype != RTEN_F32 && a->dtype != RTEN_I32) || b->dtype != a->dtype) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
@@ -480,7 +492,10 @@ static rten_status binary_op(rten_ctx* ctx, const rten_tensor* a, const rten_ten
     rten_tensor av, bv, ov;
     RTB_TRY(sc.in(a, &av));
     RTB_TRY(sc.in(b, &bv));
-    int nd = std::max(a->ndim, b->ndim);
+    scalar_b = scalar_b && numel(&bv) == 1;
+    if (scalar_b) bv.ndim = 0;
+    if (scalar_b && dt == RTEN_F32 && op == BIN_DIV) op = BIN_RCP_MUL;
+    int nd = std::max(av.ndim, bv.ndim);
     int64_t shape[RTEN_MAX_DIMS];
     long long sa[RTEN_MAX_DIMS], sb[RTEN_MAX_DIMS];
     for (int i = 0; i < nd; i++) {
@@ -491,25 +506,55 @@ static rten_status binary_op(rten_ctx* ctx, const rten_tensor* a, const rten_ten
         sa[i] = (ia >= 0 && da != 1) ? av.strides[ia] : 0;
         sb[i] = (ib >= 0 && db != 1) ? bv.strides[ib] : 0;
     }
-    // same-shape dense operands: keep a's layout for the output
-    bool same = av.ndim == bv.ndim && span_elems(&av) == numel(&av);
+    // same-shape dense operands, or a dense a and a scalar b: keep a's layout for the output
+    const bool a_dense = span_elems(&av) == numel(&av);
+    bool same = av.ndim == bv.ndim && a_dense;
     for (int i = 0; i < nd && same; i++)
         if (av.shape[i] != bv.shape[i] || (av.shape[i] != 1 && av.strides[i] != bv.strides[i])) same = false;
-    RTB_TRY(sc.out(out, dt, nd, shape, &ov, (out->data == nullptr && same) ? av.strides : nullptr));
-    if (numel(&ov) == 0) return sc.finish(RTEN_OK);
-    bool flat = same;
+    RTB_TRY(sc.out(out, dt, nd, shape, &ov, (out->data == nullptr && (same || (scalar_b && a_dense))) ? av.strides : nullptr));
+    // i32 Div checks every divisor, also when nothing is divided: the reference's check_nonzero runs over all of b
+    // before the broadcast (binary_elementwise.rs:627-629)
+    const bool check_b_only = numel(&ov) == 0 && dt == RTEN_I32 && op == BIN_DIV && numel(&bv) > 0;
+    if (numel(&ov) == 0 && !check_b_only) return sc.finish(RTEN_OK);
+    // i32 Div: the kernels flag a zero divisor or INT_MIN / -1, read back below
+    int* err = nullptr;
+    if (dt == RTEN_I32 && op == BIN_DIV) {
+        RTB_TRY(temp_alloc(ctx, sizeof(int), (void**)&err));
+        RTB_CUDA(ctx, cudaMemsetAsync(err, 0, sizeof(int), ctx->stream));
+    }
+    bool flat = same || (scalar_b && a_dense);
     for (int i = 0; i < nd && flat; i++)
         if (ov.shape[i] != 1 && ov.strides[i] != av.strides[i]) flat = false;
-    if (flat) {  // dense operands of one layout: one flat pass over the n elements from the lowest address
-        const long long n = numel(&ov), one = 1;
-        return sc.finish(launch_binary(ctx, dt, op, 0, av.data, bv.data, ov.data, 1, &n, &one, &one, &one));
+    const long long n = numel(&ov), one = 1, zero = 0;
+    if (check_b_only) {  // b / b over b's own elements flags exactly its zeros
+        long long shp[RTEN_MAX_DIMS], bs[RTEN_MAX_DIMS], sd[RTEN_MAX_DIMS];
+        long long st = 1;
+        for (int i = bv.ndim - 1; i >= 0; i--) {
+            shp[i] = bv.shape[i];
+            bs[i] = bv.strides[i];
+            sd[i] = st;
+            st *= bv.shape[i];
+        }
+        void* tmp = nullptr;
+        RTB_TRY(temp_alloc(ctx, (size_t)numel(&bv) * sizeof(int), &tmp));
+        RTB_TRY(launch_binary(ctx, dt, op, 0, bv.data, bv.data, tmp, bv.ndim, shp, bs, bs, sd, err));
+    } else if (flat) {  // dense operands of one layout: one flat pass over the n elements from the lowest address
+        RTB_TRY(launch_binary(ctx, dt, op, 0, av.data, bv.data, ov.data, 1, &n, &one, same ? &one : &zero, &one, err));
+    } else {
+        long long shp[RTEN_MAX_DIMS], sd[RTEN_MAX_DIMS];
+        for (int i = 0; i < nd; i++) {
+            shp[i] = shape[i];
+            sd[i] = ov.strides[i];
+        }
+        RTB_TRY(launch_binary(ctx, dt, op, 0, av.data, bv.data, ov.data, nd, shp, sa, sb, sd, err));
     }
-    long long shp[RTEN_MAX_DIMS], sd[RTEN_MAX_DIMS];
-    for (int i = 0; i < nd; i++) {
-        shp[i] = shape[i];
-        sd[i] = ov.strides[i];
+    if (err) {
+        int h = 0;
+        RTB_CUDA(ctx, cudaMemcpyAsync(&h, err, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+        RTB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        if (h) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Divisor contains zero");
     }
-    return sc.finish(launch_binary(ctx, dt, op, 0, av.data, bv.data, ov.data, nd, shp, sa, sb, sd));
+    return sc.finish(RTEN_OK);
 }
 
 rten_status rten_b200_add(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out) {
@@ -521,14 +566,21 @@ rten_status rten_b200_sub(rten_ctx* ctx, const rten_tensor* a, const rten_tensor
 rten_status rten_b200_mul(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out) {
     return binary_op(ctx, a, b, out, BIN_MUL);
 }
+rten_status rten_b200_div(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out) {
+    return binary_op(ctx, a, b, out, BIN_DIV, b && b->dtype == RTEN_F32);
+}
+rten_status rten_b200_pow(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out) {
+    return binary_op(ctx, a, b, out, BIN_POW, true);
+}
 
-// ---- ReduceSum ----------------------------------------------------------------------------------------
-// src/ops/reduce.rs reduce_sum: the axes resolved (negative from the end), sorted and de-duplicated; none reduces every
-// axis.  A 0-D input is its own one-element lane.
-rten_status rten_b200_reduce_sum(rten_ctx* ctx, const rten_tensor* x, const int32_t* axes, int n_axes, int keep_dims, rten_tensor* out) {
+// ---- ReduceSum, ReduceMean ----------------------------------------------------------------------------------
+// src/ops/reduce.rs reduce_sum / reduce_mean: the axes resolved (negative from the end), sorted and de-duplicated; none
+// reduces every axis.  A 0-D input is its own one-element lane.  `mean`: f32 only, each sum divided by the lane length.
+static rten_status reduce_run(rten_ctx* ctx, const rten_tensor* x, const int32_t* axes, int n_axes, int keep_dims, rten_tensor* out,
+                              int mean) {
     RTB_TRY(check_ctx(ctx));
     if (!x || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
-    if (x->dtype != RTEN_F32 && x->dtype != RTEN_I32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    if (x->dtype != RTEN_F32 && (mean || x->dtype != RTEN_I32)) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
     if (n_axes < 0 || (n_axes > 0 && !axes)) return fail(ctx, RTEN_ERR_INVALID_VALUE, "axes must be a list of n_axes values");
     const int nd = x->ndim;
     bool red[RTEN_MAX_DIMS] = {};
@@ -574,7 +626,16 @@ rten_status rten_b200_reduce_sum(rten_ctx* ctx, const rten_tensor* x, const int3
     bool vec = (p.nr == 0 || (p.nr == 1 && p.rx[0] == 1)) && (reinterpret_cast<uintptr_t>(xv.data) & 15) == 0;
     for (int k = 0; k < p.no && vec; k++) vec = p.ox[k] % 4 == 0;
     p.vec = vec;
+    p.mean = mean;
     return sc.finish(launch_reduce_sum(ctx, x->dtype, p));
+}
+
+rten_status rten_b200_reduce_sum(rten_ctx* ctx, const rten_tensor* x, const int32_t* axes, int n_axes, int keep_dims, rten_tensor* out) {
+    return reduce_run(ctx, x, axes, n_axes, keep_dims, out, 0);
+}
+rten_status rten_b200_reduce_mean(rten_ctx* ctx, const rten_tensor* x, const int32_t* axes, int n_axes, int keep_dims,
+                                  rten_tensor* out) {
+    return reduce_run(ctx, x, axes, n_axes, keep_dims, out, 1);
 }
 
 // ---- TopK, ArgMax, ArgMin --------------------------------------------------------------------------------

@@ -851,9 +851,10 @@ rten_status run_group_norm(Runner& r, OpNode& o, rten_tensor* y) {
     return rten_b200_group_norm(r.ctx, x, (int)G, r.T(o, 1), r.T(o, 2), gamma, beta, o.n.attr_f("epsilon", 1e-5f), &o.activation, y);
 }
 
-// ReduceSum (src/ops/reduce.rs:1116-1163): axes from the attribute (opset < 13) or input 1; none or empty reduces
-// every axis, or, with noop_with_empty_axes, copies the input
-rten_status run_reduce_sum(Runner& r, OpNode& o, rten_tensor* y) {
+// ReduceSum (src/ops/reduce.rs:1116-1163) and ReduceMean (:543-580): axes from the attribute (opset < 13 / < 18) or
+// input 1; none or empty reduces every axis, or, with noop_with_empty_axes, copies the input
+template <bool MEAN>
+rten_status run_reduce(Runner& r, OpNode& o, rten_tensor* y) {
     const rten_tensor* x = r.T(o, 0);
     std::vector<int64_t> axes;
     RTB_TRY(r.axes_of(o, &axes));
@@ -871,7 +872,7 @@ rten_status run_reduce_sum(Runner& r, OpNode& o, rten_tensor* y) {
         return RTEN_OK;
     }
     std::vector<int32_t> a(axes.begin(), axes.end());
-    return rten_b200_reduce_sum(r.ctx, x, a.data(), (int)a.size(), (int)o.n.attr_i("keepdims", 1), y);
+    return (MEAN ? rten_b200_reduce_mean : rten_b200_reduce_sum)(r.ctx, x, a.data(), (int)a.size(), (int)o.n.attr_i("keepdims", 1), y);
 }
 
 // TopK (src/ops/reduce.rs:1236-1306): K is input 1 (opset >= 10) or the `k` attribute (opset < 10).  A host-known K
@@ -1012,6 +1013,12 @@ constexpr OpDef OPS[] = {
          return rten_b200_gelu(r.ctx, r.T(o, 0), (a && a->s == "tanh") ? 1 : 0, y);
      }},
     {"Erf", ONNX, IN_PLACE, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_erf(r.ctx, r.T(o, 0), y); }},
+    {"Sqrt", ONNX, IN_PLACE, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_sqrt(r.ctx, r.T(o, 0), y); }},
+    {"Reciprocal", ONNX, IN_PLACE, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_reciprocal(r.ctx, r.T(o, 0), y); }},
+    {"Exp", ONNX, IN_PLACE, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_exp(r.ctx, r.T(o, 0), y); }},
+    {"Tanh", ONNX, IN_PLACE, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_tanh(r.ctx, r.T(o, 0), y); }},
+    {"Neg", ONNX, IN_PLACE, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_neg(r.ctx, r.T(o, 0), y); }},
+    {"Abs", ONNX, IN_PLACE, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_abs(r.ctx, r.T(o, 0), y); }},
     {"Softmax", ONNX, IN_PLACE, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_softmax(r.ctx, r.T(o, 0), nullptr, (int)o.n.attr_i("axis", -1), 0, y); }},
     {"MaxPool", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
          PoolAttrs a;
@@ -1042,7 +1049,7 @@ constexpr OpDef OPS[] = {
          return n.attr("axis") ? RTEN_OK : mfail(m->ctx, RTEN_ERR_UNSUPPORTED_VALUE, "Concat: missing attribute axis");
      }},
     {"GlobalAveragePool", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_global_average_pool(r.ctx, r.T(o, 0), y); }},
-    {"ReduceSum", ONNX, 0, 0b1, run_reduce_sum},
+    {"ReduceSum", ONNX, 0, 0b1, run_reduce<false>},
     {"TopK", ONNX, 0, 0b1, run_topk},
     {"ArgMax", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
          return rten_b200_arg_max(r.ctx, r.T(o, 0), (int)o.n.attr_i("axis", 0), (int)o.n.attr_i("keepdims", 1), y); },
@@ -1060,7 +1067,7 @@ constexpr OpDef OPS[] = {
              const int64_t p = a < 0 ? a + x->ndim : a;
              if (p != 2 && p != 3) spatial = false;
          }
-         if (!spatial) return mfail(r.ctx, RTEN_ERR_UNSUPPORTED_VALUE, "ReduceMean: only the spatial axes of an NCHW tensor are supported");
+         if (!spatial) return run_reduce<true>(r, o, y);
          RTB_TRY(rten_b200_global_average_pool(r.ctx, x, y));
          if (o.n.attr_i("keepdims", 1) == 0) {
              y->ndim = 2;
@@ -1141,6 +1148,8 @@ constexpr OpDef OPS[] = {
     {"Add", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_add(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
     {"Sub", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_sub(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
     {"Mul", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_mul(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
+    {"Div", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_div(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
+    {"Pow", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_pow(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
     {"LayerNormalization", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
          return rten_b200_layer_norm(r.ctx, r.T(o, 0), r.T(o, 1), r.T(o, 2), (int)o.n.attr_i("axis", -1), o.n.attr_f("epsilon", 1e-5f), y); }},
     {"RMSNormalization", ONNX, 0, 0b11, run_rms_norm, check_rms_norm},

@@ -1,9 +1,9 @@
-// ReduceSum (src/ops/reduce.rs reduce / reduce_sum).  Every output is one lane: the reduced elements in row-major order of
+// ReduceSum and ReduceMean (src/ops/reduce.rs reduce / reduce_sum / reduce_mean).  Every output is one lane: the reduced elements in row-major order of
 // the reduced axes.  The reference sums each lane with vecmath::Sum, its 64-chain fold (rten-vecmath/src/sum.rs), in
 // every branch of `reduce`: the contiguous inner chunks, the single-axis lanes and the permuted multi-axis slices all
 // present the elements in that order.  So the kernels gather a lane into shared memory in that order -- straight from
 // the strided input, no permuted copy -- and fold it there with smem_fold_chunks / smem_fold_finish (rowmath.cuh), the
-// fold InstanceNormalization uses.
+// fold InstanceNormalization uses.  ReduceMean is the same fold with one division by the lane length at the store.
 //   - lanes of up to RW_MAX elements: one warp per output, the whole lane staged at once (reduce_sum_warp_kernel);
 //   - longer lanes: one CTA per output (reduce_sum_cta_kernel).  Warps 1.. stage the next RC_CHUNK elements of the lane
 //     while warp 0 folds the current ones into its 64 chains; RC_CHUNK is a multiple of 64, so the chunks of the fold
@@ -99,7 +99,7 @@ __global__ void __launch_bounds__(RW_WARPS * 32) reduce_sum_warp_kernel(const Re
             float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
             smem_fold_chunks<false>(acc, reinterpret_cast<const float4*>(buf[w]), F, 0.0f);
             const float s = smem_fold_finish<false>(acc, buf[w] + 64 * F, L - 64 * F, 0.0f);
-            if (lane == 0) static_cast<float*>(p.y)[yo] = s;
+            if (lane == 0) static_cast<float*>(p.y)[yo] = p.mean ? __fdiv_rn(s, (float)p.L) : s;
             __syncwarp();  // (the next output reuses the buffer)
         } else {
             const unsigned s = warp_sum(int_partial<VEC>(p, x, lane, 32));
@@ -137,7 +137,7 @@ __global__ void __launch_bounds__(RC_THREADS) reduce_sum_cta_kernel(const Reduce
                 }
                 __syncthreads();
             }
-            if (threadIdx.x == 0) static_cast<float*>(p.y)[yo] = total;
+            if (threadIdx.x == 0) static_cast<float*>(p.y)[yo] = p.mean ? __fdiv_rn(total, (float)p.L) : total;
         } else {
             const unsigned s = warp_sum(int_partial<VEC>(p, x, threadIdx.x, RC_THREADS));
             if (lane == 0) ring[0][w] = (int)s;

@@ -14,7 +14,8 @@ namespace rtb {
 //   roff(j) = sum_k idx_k(j) rx[k] over the reduced dims (shape rs, row-major, ascending axis order),
 //   yoff(o) = sum_k idx_k(o) oy[k].
 // f32 sums are the reference's Sum (rten-vecmath/src/sum.rs) over the elements in j order, bit for bit; i32 sums wrap.
-// L = 0 gives 0.  vec: nr == 1, rx[0] == 1 and every lane starts 16-byte aligned (16-byte loads).
+// L = 0 gives 0.  vec: nr == 1, rx[0] == 1 and every lane starts 16-byte aligned (16-byte loads).  mean (f32):
+// ReduceMean, each sum divided by (float)L, IEEE (src/ops/reduce.rs reduce_mean; L = 0 gives NaN).
 struct ReduceParams {
     const void* x = nullptr;
     void* y = nullptr;
@@ -22,7 +23,7 @@ struct ReduceParams {
     int no = 0, nr = 0;
     long long os[RTEN_MAX_DIMS], ox[RTEN_MAX_DIMS], oy[RTEN_MAX_DIMS];
     long long rs[RTEN_MAX_DIMS], rx[RTEN_MAX_DIMS];
-    int vec = 0;
+    int vec = 0, mean = 0;
 };
 rten_status launch_reduce_sum(rten_ctx* ctx, int dtype, const ReduceParams& p);
 

@@ -593,11 +593,18 @@ rten_status launch_row_mean(rten_ctx* ctx, const float* x, float* y, long long r
 }
 
 // =========================================================================================
-// Elementwise (contiguous): Erf, Gelu, ApproxGelu, Relu, Sigmoid, Silu, HardSigmoid, HardSwish.  128-bit loads/stores,
-// grid sized to fill the SMs.
+// Elementwise (contiguous): Erf, Gelu, ApproxGelu, Relu, Sigmoid, Silu, HardSigmoid, HardSwish, Sqrt, Reciprocal, Exp,
+// Tanh, Neg, Abs.  128-bit loads/stores, grid sized to fill the SMs.
 // =========================================================================================
 template <int OP>
 __device__ __forceinline__ float unary_apply(float v, float alpha, float beta) {
+    // (src/ops/unary_elementwise.rs: Rust's f32 sqrt, 1.0 / x, -x and abs are the IEEE operations)
+    if (OP == UNARY_SQRT) return __fsqrt_rn(v);
+    if (OP == UNARY_RECIPROCAL) return __fdiv_rn(1.0f, v);
+    if (OP == UNARY_EXP) return exp_ref(v);
+    if (OP == UNARY_TANH) return tanh_ref(v);
+    if (OP == UNARY_NEG) return __uint_as_float(__float_as_uint(v) ^ 0x80000000u);
+    if (OP == UNARY_ABS) return __uint_as_float(__float_as_uint(v) & 0x7fffffffu);
     if (OP == UNARY_ERF) return erf_ref(v);
     if (OP == UNARY_GELU) return gelu_ref(v);
     if (OP == UNARY_APPROX_GELU) return approx_gelu_ref(v);
@@ -650,6 +657,12 @@ rten_status launch_unary(rten_ctx* ctx, int op, const float* x, float* y, long l
         case UNARY_SILU: kern = unary_kernel<UNARY_SILU>; break;
         case UNARY_HARD_SIGMOID: kern = unary_kernel<UNARY_HARD_SIGMOID>; break;
         case UNARY_HARD_SWISH: kern = unary_kernel<UNARY_HARD_SWISH>; break;
+        case UNARY_SQRT: kern = unary_kernel<UNARY_SQRT>; break;
+        case UNARY_RECIPROCAL: kern = unary_kernel<UNARY_RECIPROCAL>; break;
+        case UNARY_EXP: kern = unary_kernel<UNARY_EXP>; break;
+        case UNARY_TANH: kern = unary_kernel<UNARY_TANH>; break;
+        case UNARY_NEG: kern = unary_kernel<UNARY_NEG>; break;
+        case UNARY_ABS: kern = unary_kernel<UNARY_ABS>; break;
         default: return fail(ctx, RTEN_ERR_INVALID_VALUE, "unknown unary op");
     }
     return launch(ctx, "unary launch", kern, {grid, 256}, x, y, n, vec, alpha, beta);
@@ -753,12 +766,48 @@ rten_status launch_nd_copy(rten_ctx* ctx, int esize, const void* src, void* dst,
     }
 }
 
+// FastPow (src/ops/binary_elementwise.rs): exponents 2 and 3 as products rounded left to right, else powf
+__device__ __forceinline__ float pow_ref(float x, float e) {
+    if (e == 2.0f) return __fmul_rn(x, x);
+    if (e == 3.0f) return __fmul_rn(__fmul_rn(x, x), x);
+    return powf(x, e);
+}
+
+// i32 ^ i32: i32::wrapping_pow for a non-negative exponent (any multiplication order gives the product mod 2^32); a
+// negative one through f32, then Rust's saturating `as i32` (NaN -> 0)
+__device__ __forceinline__ int pow_ref(int x, int e) {
+    if (e >= 0) {
+        unsigned r = 1, b = (unsigned)x;
+        for (unsigned n = (unsigned)e; n; n >>= 1, b *= b)
+            if (n & 1) r *= b;
+        return (int)r;
+    }
+    const float v = pow_ref((float)x, (float)e);
+    if (v != v) return 0;
+    if (v >= 2147483648.0f) return 0x7fffffff;
+    if (v <= -2147483648.0f) return (int)0x80000000;
+    return __float2int_rz(v);
+}
+
 // Add / Sub / Mul: f32 correctly rounded, then Relu when `relu`; i32 in unsigned arithmetic, so it wraps
-// (src/ops/binary_elementwise.rs on i32).  One instance per element type: the operation is a runtime argument.
-template <typename T>
-__device__ __forceinline__ T binary_apply(T a, T b, int op, int relu) {
+// (src/ops/binary_elementwise.rs on i32).  MATH (the Div / Pow kernels): f32 Div correctly rounded, a * (1 / b) with two
+// roundings, Pow as pow_ref; i32 Div truncating, flagging in *err the divisions Rust refuses, i32 Pow as pow_ref.  One
+// instance per element type and family: the operation is a runtime argument.
+template <bool MATH, typename T>
+__device__ __forceinline__ T binary_apply(T a, T b, int op, int relu, int* err) {
     T v;
-    if constexpr (std::is_same<T, float>::value) {
+    if constexpr (MATH) {
+        if (op == BIN_POW) {
+            v = pow_ref(a, b);
+        } else if constexpr (std::is_same<T, float>::value) {
+            v = op == BIN_DIV ? __fdiv_rn(a, b) : __fmul_rn(a, __fdiv_rn(1.0f, b));
+        } else if (b == 0 || (b == -1 && a == (int)0x80000000)) {
+            *err = 1;
+            v = 0;
+        } else {
+            v = a / b;
+        }
+    } else if constexpr (std::is_same<T, float>::value) {
         v = op == BIN_MUL ? __fmul_rn(a, b) : __fadd_rn(a, op == BIN_SUB ? -b : b);  // (a - b is a + -b, exactly)
     } else {
         const unsigned x = (unsigned)a, y = (unsigned)b;
@@ -770,55 +819,66 @@ __device__ __forceinline__ T binary_apply(T a, T b, int op, int relu) {
 
 // f(op) with op a compile-time constant: the flat and periodic kernels get one loop per operation, with no per-element
 // choice of operation.  (The strided kernel keeps one loop: its index loop compiles shorter that way.)
-template <typename F>
+template <bool MATH, typename F>
 __device__ __forceinline__ void with_op(int op, F f) {
-    if (op == BIN_MUL) f(std::integral_constant<int, BIN_MUL>());
-    else if (op == BIN_SUB) f(std::integral_constant<int, BIN_SUB>());
-    else f(std::integral_constant<int, BIN_ADD>());
+    if constexpr (MATH) {
+        if (op == BIN_POW) f(std::integral_constant<int, BIN_POW>());
+        else if (op == BIN_RCP_MUL) f(std::integral_constant<int, BIN_RCP_MUL>());
+        else f(std::integral_constant<int, BIN_DIV>());
+    } else {
+        if (op == BIN_MUL) f(std::integral_constant<int, BIN_MUL>());
+        else if (op == BIN_SUB) f(std::integral_constant<int, BIN_SUB>());
+        else f(std::integral_constant<int, BIN_ADD>());
+    }
 }
 
 template <typename T>
 using Vec4 = typename std::conditional<std::is_same<T, float>::value, float4, int4>::type;  // 16 bytes of T
 
-template <typename T>
-__device__ __forceinline__ Vec4<T> binary_apply4(Vec4<T> x, Vec4<T> y, int op, int relu) {
-    return {binary_apply(x.x, y.x, op, relu), binary_apply(x.y, y.y, op, relu), binary_apply(x.z, y.z, op, relu),
-            binary_apply(x.w, y.w, op, relu)};
+template <bool MATH, typename T>
+__device__ __forceinline__ Vec4<T> binary_apply4(Vec4<T> x, Vec4<T> y, int op, int relu, int* err) {
+    return {binary_apply<MATH>(x.x, y.x, op, relu, err), binary_apply<MATH>(x.y, y.y, op, relu, err),
+            binary_apply<MATH>(x.z, y.z, op, relu, err), binary_apply<MATH>(x.w, y.w, op, relu, err)};
 }
 
+// The three layouts' loops, shared by the Add / Sub / Mul kernels and the Div / Pow ones.  Div and Pow have kernels of
+// their own so that their code (powf above all) does not raise the registers, and lower the occupancy, of Add / Sub / Mul.
 // a, b and d dense in one layout: 16 bytes per thread when `vec` (all three bases 16-byte aligned), then a scalar tail
-// (everything when not)
-template <typename T>
-__global__ void __launch_bounds__(256)
-binary_flat_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d, long long n, int vec, int op, int relu) {
-    with_op(op, [&](auto o) {
+// (everything when not).  `bscalar` (the Div / Pow kernels): b is one element, broadcast over a.
+template <bool MATH, typename T>
+__device__ __forceinline__ void binary_flat(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d, long long n,
+                                            int vec, int op, int relu, int* err, bool bscalar = false) {
+    with_op<MATH>(op, [&](auto o) {
         const long long n4 = vec ? (n >> 2) : 0;
         const long long stride = (long long)gridDim.x * blockDim.x;
+        const T b0 = bscalar ? b[0] : T(0);
         for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride)
             reinterpret_cast<Vec4<T>*>(d)[i] =
-                binary_apply4<T>(reinterpret_cast<const Vec4<T>*>(a)[i], reinterpret_cast<const Vec4<T>*>(b)[i], decltype(o)::value, relu);
+                binary_apply4<MATH, T>(reinterpret_cast<const Vec4<T>*>(a)[i],
+                                       bscalar ? Vec4<T>{b0, b0, b0, b0} : reinterpret_cast<const Vec4<T>*>(b)[i], decltype(o)::value,
+                                       relu, err);
         for (long long j = (n4 << 2) + (long long)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride)
-            d[j] = binary_apply(a[j], b[j], decltype(o)::value, relu);
+            d[j] = binary_apply<MATH>(a[j], bscalar ? b0 : b[j], decltype(o)::value, relu, err);
     });
 }
 
 // a and d dense, b dense over the TRAILING dims and broadcast over the leading ones (bias rows, position embeddings):
 // d[i] = a[i] (op) b[i mod period], 16 bytes per thread, 32-bit index arithmetic
-template <typename T>
-__global__ void __launch_bounds__(256) binary_periodic_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d,
-                                                              unsigned n4, unsigned period4, int op, int relu) {
-    with_op(op, [&](auto o) {
+template <bool MATH, typename T>
+__device__ __forceinline__ void binary_periodic(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d, unsigned n4,
+                                                unsigned period4, int op, int relu, int* err) {
+    with_op<MATH>(op, [&](auto o) {
         const unsigned stride = gridDim.x * blockDim.x;
         for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride)
-            reinterpret_cast<Vec4<T>*>(d)[i] = binary_apply4<T>(reinterpret_cast<const Vec4<T>*>(a)[i],
-                                                                reinterpret_cast<const Vec4<T>*>(b)[i % period4],
-                                                                decltype(o)::value, relu);
+            reinterpret_cast<Vec4<T>*>(d)[i] = binary_apply4<MATH, T>(reinterpret_cast<const Vec4<T>*>(a)[i],
+                                                                      reinterpret_cast<const Vec4<T>*>(b)[i % period4],
+                                                                      decltype(o)::value, relu, err);
     });
 }
 
-template <typename T>
-__global__ void __launch_bounds__(256)
-binary_nd_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d, const NdParams p, int op, int relu) {
+template <bool MATH, typename T>
+__device__ __forceinline__ void binary_nd(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d, const NdParams& p,
+                                          int op, int relu, int* err) {
     const long long stride = (long long)gridDim.x * blockDim.x;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += stride) {
         long long rem = i, ao = 0, bo = 0, dof = 0;
@@ -830,13 +890,47 @@ binary_nd_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict
             bo += idx * p.sb[k];
             dof += idx * p.sd[k];
         }
-        d[dof] = binary_apply(a[ao], b[bo], op, relu);
+        d[dof] = binary_apply<MATH>(a[ao], b[bo], op, relu, err);
     }
 }
 
 template <typename T>
+__global__ void __launch_bounds__(256)
+binary_flat_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d, long long n, int vec, int op, int relu) {
+    binary_flat<false>(a, b, d, n, vec, op, relu, nullptr);
+}
+template <typename T>
+__global__ void __launch_bounds__(256) binary_periodic_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d,
+                                                              unsigned n4, unsigned period4, int op, int relu) {
+    binary_periodic<false>(a, b, d, n4, period4, op, relu, nullptr);
+}
+template <typename T>
+__global__ void __launch_bounds__(256)
+binary_nd_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d, const NdParams p, int op, int relu) {
+    binary_nd<false>(a, b, d, p, op, relu, nullptr);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256)
+binary_math_flat_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d, long long n, int vec, int bscalar,
+                        int op, int* err) {
+    binary_flat<true>(a, b, d, n, vec, op, 0, err, bscalar != 0);
+}
+template <typename T>
+__global__ void __launch_bounds__(256) binary_math_periodic_kernel(const T* __restrict__ a, const T* __restrict__ b,
+                                                                   T* __restrict__ d, unsigned n4, unsigned period4, int op, int* err) {
+    binary_periodic<true>(a, b, d, n4, period4, op, 0, err);
+}
+template <typename T>
+__global__ void __launch_bounds__(256)
+binary_math_nd_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ d, const NdParams p, int op, int* err) {
+    binary_nd<true>(a, b, d, p, op, 0, err);
+}
+
+template <typename T>
 static rten_status launch_binary_typed(rten_ctx* ctx, int op, int relu, const T* a, const T* b, T* d, int ndim,
-                                       const long long* shape, const long long* sa, const long long* sb, const long long* sd) {
+                                       const long long* shape, const long long* sa, const long long* sb, const long long* sd,
+                                       int* err) {
     // Innermost dim first: `dense` while a and d are dense and b is too, or is from the first dim it broadcasts (stride
     // 0) over, which makes the dims inside it (`period` elements) a block repeated over the rest.
     long long n = 1, period = 0;
@@ -858,21 +952,34 @@ static rten_status launch_binary_typed(rten_ctx* ctx, int op, int relu, const T*
     const bool aligned =
         ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(d)) & 15) == 0;
     const char* what = "binary launch";
-    if (dense && !bcast)
-        return launch(ctx, what, binary_flat_kernel<T>, {ew_grid(ctx, aligned ? (n + 3) / 4 : n), 256}, a, b, d, n,
-                      aligned ? 1 : 0, op, relu);
-    if (dense && (period & 3) == 0 && n < 0x7fffffffLL && aligned)
-        return launch(ctx, what, binary_periodic_kernel<T>, {ew_grid(ctx, n / 4), 256}, a, b, d, (unsigned)(n / 4),
-                      (unsigned)(period / 4), op, relu);
-    return launch(ctx, what, binary_nd_kernel<T>, {ew_grid(ctx, n), 256}, a, b, d, nd_params(ndim, shape, sa, sb, sd), op, relu);
+    const LaunchShape flat{dim3(ew_grid(ctx, aligned ? (n + 3) / 4 : n)), dim3(256)}, per{dim3(ew_grid(ctx, n / 4)), dim3(256)},
+        nd{dim3(ew_grid(ctx, n)), dim3(256)};
+    const bool periodic = dense && (period & 3) == 0 && n < 0x7fffffffLL && aligned;
+    if (op >= BIN_DIV) {
+        if (dense && !bcast) return launch(ctx, what, binary_math_flat_kernel<T>, flat, a, b, d, n, aligned ? 1 : 0, 0, op, err);
+        // b one element broadcast over dense a and d (period 1): the flat kernel, b read once per thread
+        if (dense && period == 1) {
+            const bool ad_aligned = ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(d)) & 15) == 0;
+            const LaunchShape fs{dim3(ew_grid(ctx, ad_aligned ? (n + 3) / 4 : n)), dim3(256)};
+            return launch(ctx, what, binary_math_flat_kernel<T>, fs, a, b, d, n, ad_aligned ? 1 : 0, 1, op, err);
+        }
+        if (periodic)
+            return launch(ctx, what, binary_math_periodic_kernel<T>, per, a, b, d, (unsigned)(n / 4), (unsigned)(period / 4), op, err);
+        return launch(ctx, what, binary_math_nd_kernel<T>, nd, a, b, d, nd_params(ndim, shape, sa, sb, sd), op, err);
+    }
+    if (dense && !bcast) return launch(ctx, what, binary_flat_kernel<T>, flat, a, b, d, n, aligned ? 1 : 0, op, relu);
+    if (periodic)
+        return launch(ctx, what, binary_periodic_kernel<T>, per, a, b, d, (unsigned)(n / 4), (unsigned)(period / 4), op, relu);
+    return launch(ctx, what, binary_nd_kernel<T>, nd, a, b, d, nd_params(ndim, shape, sa, sb, sd), op, relu);
 }
 
 rten_status launch_binary(rten_ctx* ctx, int dtype, int op, int relu, const void* a, const void* b, void* d, int ndim,
-                          const long long* shape, const long long* sa, const long long* sb, const long long* sd) {
+                          const long long* shape, const long long* sa, const long long* sb, const long long* sd, int* err) {
+    if (op >= BIN_DIV && relu) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Div / Pow take no Relu");
     if (dtype == RTEN_F32)
-        return launch_binary_typed(ctx, op, relu, (const float*)a, (const float*)b, (float*)d, ndim, shape, sa, sb, sd);
+        return launch_binary_typed(ctx, op, relu, (const float*)a, (const float*)b, (float*)d, ndim, shape, sa, sb, sd, err);
     if (dtype == RTEN_I32)
-        return launch_binary_typed(ctx, op, relu, (const int*)a, (const int*)b, (int*)d, ndim, shape, sa, sb, sd);
+        return launch_binary_typed(ctx, op, relu, (const int*)a, (const int*)b, (int*)d, ndim, shape, sa, sb, sd, err);
     return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
 }
 

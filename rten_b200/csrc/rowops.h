@@ -15,7 +15,13 @@ enum {
     UNARY_SIGMOID = 4,
     UNARY_SILU = 5,
     UNARY_HARD_SIGMOID = 6,  // alpha * x + beta, clamped
-    UNARY_HARD_SWISH = 7
+    UNARY_HARD_SWISH = 7,
+    UNARY_SQRT = 8,        // __fsqrt_rn
+    UNARY_RECIPROCAL = 9,  // 1 / x, IEEE
+    UNARY_EXP = 10,        // exp_ref
+    UNARY_TANH = 11,       // tanh_ref
+    UNARY_NEG = 12,        // -x (the sign bit flipped)
+    UNARY_ABS = 13         // the sign bit cleared
 };
 
 // Softmax over the last (contiguous) axis of x viewed as [rows, n]; optional mask broadcast over
@@ -55,13 +61,23 @@ rten_status launch_clip(rten_ctx* ctx, int is_i32, const void* x, void* y, long 
 rten_status launch_nd_copy(rten_ctx* ctx, int esize, const void* src, void* dst, int ndim, const long long* shape,
                            const long long* sstride, const long long* dstride);
 // d = a (op) b over the iteration space `shape`, element strides sa / sb / sd (0 where an operand broadcasts): f32
-// (__fadd_rn / __fsub_rn / __fmul_rn, then Relu when `relu`) or i32 (wrapping).  The flat kernel when a, b and d are
-// dense row-major over `shape` (so a dense view of any layout runs flat when passed as [n] with unit strides), the
-// periodic one when a and d are and b is a dense block of the trailing dims repeated over the leading ones (period a
-// multiple of 4, fewer than 2^31 elements, 16-byte aligned bases), else the strided one.
-enum BinaryOp { BIN_ADD = 0, BIN_SUB = 1, BIN_MUL = 2 };
+// (__fadd_rn / __fsub_rn / __fmul_rn / __fdiv_rn, Pow as FastPow, then Relu when `relu`) or i32 (Add / Sub / Mul / Pow
+// wrapping, Div truncating).  The flat kernel when a, b and d are dense row-major over `shape` (so a dense view of any
+// layout runs flat when passed as [n] with unit strides), the periodic one when a and d are and b is a dense block of
+// the trailing dims repeated over the leading ones (period a multiple of 4, fewer than 2^31 elements, 16-byte aligned
+// bases), else the strided one.  Div, Pow and BIN_RCP_MUL run on kernels of their own (binary_math_*) with the same
+// three layouts, so that Add / Sub / Mul keep their code and registers; a one-element b over dense a and d also runs
+// their flat kernel, which reads b once.
+//   BIN_RCP_MUL (f32): a * (1 / b), two roundings -- the reference's Div by a one-element divisor.
+//   BIN_POW: f32 ^ f32 and i32 ^ i32 (src/ops/binary_elementwise.rs FastPow): exponent 2 is x * x, 3 is x * x * x
+//     (rounded left to right), any other f32 exponent powf; a non-negative i32 exponent wraps, a negative one goes
+//     through f32 and back with Rust's saturating `as i32`.
+//   i32 BIN_DIV: a zero divisor or INT_MIN / -1 sets *err to 1 (err must then be a device int the caller zeroed) and
+//     stores 0 there; err is read by i32 Div only.
+enum BinaryOp { BIN_ADD = 0, BIN_SUB = 1, BIN_MUL = 2, BIN_DIV = 3, BIN_POW = 4, BIN_RCP_MUL = 5 };
 rten_status launch_binary(rten_ctx* ctx, int dtype, int op, int relu, const void* a, const void* b, void* d, int ndim,
-                          const long long* shape, const long long* sa, const long long* sb, const long long* sd);
+                          const long long* shape, const long long* sa, const long long* sb, const long long* sd,
+                          int* err = nullptr);
 rten_status launch_minmax(rten_ctx* ctx, const float* x, long long n, int* mm /* 2 ordered ints */);
 // `xch` (batch-sharded runs): the kernel first exchanges the local range in `mm` with the other ranks (comm_device.cuh)
 struct RangeExchange;

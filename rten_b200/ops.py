@@ -759,9 +759,9 @@ class Softmax:
     def __init__(self, axis=-1, flush_nans_to_zero=False):
         self.axis, self.flush_nans_to_zero = axis, flush_nans_to_zero
 
-    def run(self, ctx, x, in_place=False):
+    def run(self, ctx, x, in_place=False, out=None):
         A = _Args(ctx)
-        into = x if (in_place and isinstance(x, DeviceTensor)) else None
+        into = x if (in_place and isinstance(x, DeviceTensor)) else out
         o = A.out(into)
         ctx.check(ctx.lib.rten_b200_softmax(ctx.handle, A.t(x), None, self.axis, int(self.flush_nans_to_zero), C.byref(o)))
         return A.wrap(o, into)
@@ -882,9 +882,9 @@ class GroupNorm:
 class _Unary:
     fn = ""
 
-    def run(self, ctx, x, in_place=False):
+    def run(self, ctx, x, in_place=False, out=None):
         A = _Args(ctx)
-        into = x if (in_place and isinstance(x, DeviceTensor)) else None
+        into = x if (in_place and isinstance(x, DeviceTensor)) else out
         o = A.out(into)
         ctx.check(self._call(ctx, A.t(x), C.byref(o)))
         return A.wrap(o, into)
@@ -941,6 +941,48 @@ class HardSwish(_Unary):
 
     def _call(self, ctx, x, o):
         return ctx.lib.rten_b200_hard_swish(ctx.handle, x, o)
+
+
+class Sqrt(_Unary):
+    """src/ops/unary_elementwise.rs:743-745: IEEE square root (f32)"""
+
+    def _call(self, ctx, x, o):
+        return ctx.lib.rten_b200_sqrt(ctx.handle, x, o)
+
+
+class Reciprocal(_Unary):
+    """src/ops/unary_elementwise.rs:607-609: 1 / x, IEEE (f32)"""
+
+    def _call(self, ctx, x, o):
+        return ctx.lib.rten_b200_reciprocal(ctx.handle, x, o)
+
+
+class Exp(_Unary):
+    """rten-vecmath/src/exp.rs Exp (f32): inf from 104 on, 0 from -104 down"""
+
+    def _call(self, ctx, x, o):
+        return ctx.lib.rten_b200_exp(ctx.handle, x, o)
+
+
+class Tanh(_Unary):
+    """rten-vecmath/src/tanh.rs Tanh (f32)"""
+
+    def _call(self, ctx, x, o):
+        return ctx.lib.rten_b200_tanh(ctx.handle, x, o)
+
+
+class Neg(_Unary):
+    """src/ops/unary_elementwise.rs:550-555: -x, the sign bit flipped (f32)"""
+
+    def _call(self, ctx, x, o):
+        return ctx.lib.rten_b200_neg(ctx.handle, x, o)
+
+
+class Abs(_Unary):
+    """src/ops/unary_elementwise.rs:195-220: the sign bit cleared (f32)"""
+
+    def _call(self, ctx, x, o):
+        return ctx.lib.rten_b200_abs(ctx.handle, x, o)
 
 
 class Clip:
@@ -1037,6 +1079,28 @@ class Sub:
         return A.wrap(o, out)
 
 
+class Div:
+    """src/ops/binary_elementwise.rs:600-638 Div (f32, or truncating i32 that refuses a zero divisor and INT_MIN / -1,
+    broadcasting).  A one-element f32 divisor is a * (1 / b), with a's shape."""
+
+    def run(self, ctx, a, b, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        ctx.check(ctx.lib.rten_b200_div(ctx.handle, A.t(a), A.t(b), C.byref(o)))
+        return A.wrap(o, out)
+
+
+class Pow:
+    """src/ops/binary_elementwise.rs:965-1029 Pow (FastPow; f32 ^ f32 or i32 ^ i32, broadcasting).  A one-element
+    exponent maps the base (a's shape)."""
+
+    def run(self, ctx, a, b, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        ctx.check(ctx.lib.rten_b200_pow(ctx.handle, A.t(a), A.t(b), C.byref(o)))
+        return A.wrap(o, out)
+
+
 TOPK_MAX_K = 2048  # the largest k rten_b200_topk takes (RTEN_ERR_UNSUPPORTED_VALUE above)
 
 
@@ -1093,6 +1157,19 @@ class ReduceSum:
         o = A.out(out)
         ax = (C.c_int32 * max(len(self.axes or []), 1))(*(self.axes or []))
         ctx.check(ctx.lib.rten_b200_reduce_sum(ctx.handle, A.t(x), ax, len(self.axes or []), int(self.keep_dims), C.byref(o)))
+        return A.wrap(o, out)
+
+
+class ReduceMean(ReduceSum):
+    """src/ops/reduce.rs:524-541 ReduceMean (f32): each lane's ReduceSum divided by its length; an empty lane is NaN"""
+
+    def run(self, ctx, x, out=None):
+        if not self.axes and self.noop_with_empty_axes:
+            return super().run(ctx, x, out)
+        A = _Args(ctx)
+        o = A.out(out)
+        ax = (C.c_int32 * max(len(self.axes or []), 1))(*(self.axes or []))
+        ctx.check(ctx.lib.rten_b200_reduce_mean(ctx.handle, A.t(x), ax, len(self.axes or []), int(self.keep_dims), C.byref(o)))
         return A.wrap(o, out)
 
 
