@@ -468,7 +468,6 @@ rten_status conv_core(OpScope& sc, ConvArgs& A, rten_tensor* out) {
     //      per pixel, one 128-byte K block per filter row holding kw pixels x pitch channels.  The 8-bit copy also holds
     //      the vertical padding (the reference's pad value); f32 leaves vertical padding / stride to the TMA tile addressing.
     const bool smallc_ok = !implicit_ok && groups == 1 && dil[1] == 1 && (int64_t)B * OH * OW > 0 &&
-                           !getenv("RTEN_B200_NO_SMALLC") &&
                            (A.kind == 0 ? Cg <= 4 && kw * 4 <= 32 : Cg <= 16 && kw <= 8 && !zb);
     if (smallc_ok) {
         const bool q8 = A.kind == 1;

@@ -104,7 +104,7 @@ rten_status comm_allreduce_minmax(rten_ctx* ctx, rten_comm* comm, int* mm) {
 // communicator exchanges through NCCL (the caller then takes comm_allreduce_minmax first)
 bool comm_range_exchange(rten_comm* comm, RangeExchange* out) {
     memset(out, 0, sizeof(*out));
-    if (!comm || comm->world <= 1 || !comm->peer_ok || getenv("RTEN_B200_UNFUSED_RANGE_EXCHANGE")) return false;
+    if (!comm || comm->world <= 1 || !comm->peer_ok) return false;
     out->peers = comm->peers;
     out->rank = comm->rank;
     out->world = comm->world;

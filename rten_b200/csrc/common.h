@@ -153,7 +153,6 @@ struct LaunchShape {
 
 // Launches `kern` on the context stream and counts it.  A failed launch returns RTEN_ERR_CUDA with `what` in the
 // message, is not counted, and leaves no pending error behind for the next launch's check.
-// RTEN_B200_NO_PDL turns programmatic dependent launch off for every kernel.
 template <typename... P, typename... A>
 rten_status launch(rten_ctx* ctx, const char* what, void (*kern)(P...), const LaunchShape& s, A&&... args) {
     cudaLaunchConfig_t cfg = {};
@@ -163,7 +162,7 @@ rten_status launch(rten_ctx* ctx, const char* what, void (*kern)(P...), const La
     cfg.stream = ctx->stream;
     cudaLaunchAttribute attr[2];
     cfg.attrs = attr;
-    if (s.pdl && !getenv("RTEN_B200_NO_PDL")) {
+    if (s.pdl) {
         attr[cfg.numAttrs].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         attr[cfg.numAttrs++].val.programmaticStreamSerializationAllowed = 1;
     }

@@ -371,7 +371,6 @@ static void qlinear_shape(const QLinearLaunch& L, int& mt, int& cpw, int& ki) {
 }
 
 bool qlinear_supported(const QLinearLaunch& L) {
-    if (getenv("RTEN_B200_NO_SKINNY")) return false;
     if (L.M < 1 || L.M > 16 || L.N < 1 || L.K < 16 || (L.K & 15)) return false;
     if ((L.K >> 4) > 192) return false;  // weights of a tile live in registers: K <= 3072
     auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
@@ -494,7 +493,6 @@ __global__ void __launch_bounds__(256) skinny_f32_kernel(const SkinnyF32Params p
 }
 
 bool skinny_f32_supported(const SkinnyF32Launch& L) {
-    if (getenv("RTEN_B200_NO_SKINNY")) return false;
     if (L.M < 1 || L.M > 32 || L.N < 1 || L.K < 4 || (L.K & 3)) return false;
     auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
     return al16(L.a) && al16(L.b) && !(L.as & 3) && !(L.bs & 3);
@@ -818,7 +816,6 @@ __global__ void __launch_bounds__(NW * 32, DH == 64 ? (NW == 8 ? 3 : 4) : 1) att
 }
 
 bool attn_decode_supported(const AttnDecodeLaunch& L) {
-    if (getenv("RTEN_B200_NO_SKINNY")) return false;
     if (L.dh != 64 && L.dh != 128) return false;
     if (L.B < 1 || L.q_heads < 1 || L.kv_heads < 1 || L.q_heads % L.kv_heads) return false;
     if (L.kv_cap < 1 || L.kv_cap > ATTN_DECODE_MAX_CACHE) return false;
@@ -851,7 +848,7 @@ rten_status launch_attn_decode(rten_ctx* ctx, const AttnDecodeLaunch& L) {
         return ns;
     };
     int nw = 8, ns = splits_for(ATTN_CHUNK);
-    if (L.dh == 64 && !getenv("RTEN_B200_ATTN_8WARPS")) {  // six-warp CTAs when their grid needs fewer waves (see the kernel's comment)
+    if (L.dh == 64) {  // six-warp CTAs when their grid needs fewer waves (see the kernel's comment)
         const int ns6 = splits_for(96);
         const long long waves8 = ((long long)bh * ns + 3LL * ctx->num_sms - 1) / (3LL * ctx->num_sms);
         const long long waves6 = ((long long)bh * ns6 + 4LL * ctx->num_sms - 1) / (4LL * ctx->num_sms);

@@ -289,7 +289,7 @@ static void enumerate_plans(const Prepared& q, int num_sms, std::vector<std::pai
             PlanShape ps;
             if (is_wide(bn)) {
                 pl.nbuf = 2;  // (the wide kernel has two fixed staging buffers)
-            } else if (pl.nbuf == 2 && !getenv("RTEN_B200_NO_NBUF3")) {
+            } else if (pl.nbuf == 2) {
                 // A third staging buffer per group takes the wait for the previous store's shared-memory read and, with a
                 // residual, the late request of the next residual tile off the chunk's critical path -- as long as the
                 // operand ring keeps three stages (or loses none)
@@ -400,7 +400,6 @@ static rten_status prepare_launch(rten_ctx* ctx, const GemmLaunch& L, Prepared& 
         q.dbox[1] = BM;
     }
     q.tma_store = (e.s_col == 1 && L.N >= 4 && tma_compatible(od, 4, 4)) ? 1 : 0;
-    if (getenv("RTEN_B200_NO_TMA_STORE")) q.tma_store = 0;
     // residual prefetched by TMA: same geometry as the output, own strides (fast-path epilogue only)
     ord = od;
     ord.base = e.r;
@@ -420,7 +419,6 @@ static rten_status prepare_launch(rten_ctx* ctx, const GemmLaunch& L, Prepared& 
     // a broadcast residual (Gemm's C) has zero strides on real dims: keep the register path for it
     for (int i = 1; i < 4; i++)
         if (ord.dims[i] > 1 && ord.strides[i] == 0) q.res_tma = 0;
-    if (getenv("RTEN_B200_NO_RES_TMA")) q.res_tma = 0;
     p.res_tx_bytes = q.a_rows * KBYTES;
     q.step = q.tma_store ? 32 : 16;
     const bool plain = is_plain_f32(pick_epilogue(L, q.tma_store, q.res_tma, 1));
@@ -697,7 +695,7 @@ static rten_status launch_tf32x3(rten_ctx* ctx, const GemmLaunch& L0) {
         d0p = (d0 + 3) / 4 * 4;
         if (b0.dims[0] != d0) return RTEN_ERR_UNSUPPORTED_VALUE;
         // ---- B
-        if (slot && !getenv("RTEN_B200_X3_NO_CACHE")) {
+        if (slot) {
             if (!*slot && !ctx->capturing) {
                 long long n = 3 * d0p;
                 for (int i = 1; i < 4; i++) n *= (b0.strides[i] == 0 ? 1 : b0.dims[i]);
@@ -712,7 +710,7 @@ static rten_status launch_tf32x3(rten_ctx* ctx, const GemmLaunch& L0) {
                 *slot = buf;
             }
         }
-        if (slot && *slot && !getenv("RTEN_B200_X3_NO_CACHE")) {
+        if (slot && *slot) {
             b = b0;
             b.base = *slot;
             b.dims[0] = 3 * d0p;

@@ -18,20 +18,48 @@ FORCE_KEYS = ("RTEN_B200_FORCE_BN", "RTEN_B200_FORCE_SPLITK", "RTEN_B200_FORCE_S
 
 
 @contextlib.contextmanager
+def switches(**env):
+    """The library's RTEN_B200_* environment switches set to `env` inside the block (None unsets one); every switch
+    named gets its previous value back on exit, so a value the caller had set survives."""
+    saved = {k: os.environ.get(k) for k in env}
+
+    def put(values):
+        for k, v in values.items():
+            if v is None:
+                os.environ.pop(k, None)
+            else:
+                os.environ[k] = str(v)
+
+    try:
+        put(env)
+        yield
+    finally:
+        put(saved)
+
+
+def run_verbose(fn):
+    """fn() with RTEN_B200_VERBOSE=1 and file descriptor 2 sent to a temporary file: (its result, the text the library
+    printed to stderr, which holds its plan and launch lines)."""
+    import sys
+    import tempfile
+    sys.stderr.flush()
+    saved = os.dup(2)
+    with tempfile.TemporaryFile() as f:
+        os.dup2(f.fileno(), 2)
+        try:
+            with switches(RTEN_B200_VERBOSE=1):
+                out = fn()
+        finally:
+            os.dup2(saved, 2)
+            os.close(saved)
+        f.seek(0)
+        return out, f.read().decode(errors="replace")
+
+
 def forced(bn, strict=True):
     """Launches inside take the best-ranked plan with `bn`-column tiles and no split-K; under `strict` a launch that no
     such plan can run fails instead of falling back to the model's choice."""
-    for k in FORCE_KEYS:
-        os.environ.pop(k, None)
-    os.environ["RTEN_B200_FORCE_BN"] = str(bn)
-    os.environ["RTEN_B200_FORCE_SPLITK"] = "1"
-    if strict:
-        os.environ["RTEN_B200_FORCE_STRICT"] = "1"
-    try:
-        yield
-    finally:
-        for k in FORCE_KEYS:
-            os.environ.pop(k, None)
+    return switches(RTEN_B200_FORCE_BN=bn, RTEN_B200_FORCE_SPLITK=1, RTEN_B200_FORCE_STRICT=1 if strict else None)
 
 
 @contextlib.contextmanager
@@ -410,10 +438,8 @@ def check_matmul_integer(rt, oracle):
 def check_plans(rt, oracle):
     """Every launch-plan family (32- and 64-column tiles, split-K with the last-arriver reduction) must give the same answers: forced through the debug environment knobs,
     then chosen by the autotuner."""
-    import os
     ctx = new_ctx(rt)
     r = oracle.XorShiftRng(99)
-    keys = ("RTEN_B200_FORCE_BN", "RTEN_B200_FORCE_SPLITK")
     plans = [dict(), dict(BN=32), dict(BN=64), dict(BN=32, SPLITK=2), dict(BN=64, SPLITK=2), dict(BN=64, SPLITK=3),
              dict(BN=32, SPLITK=3), dict(BN=64, SPLITK=4)]
     a8 = r.u8((300, 2048))
@@ -425,12 +451,8 @@ def check_plans(rt, oracle):
     worst = 0.0
     hits_before = 0
     never = []
-    try:
-        for pl in plans:
-            for k in keys:
-                os.environ.pop(k, None)
-            for k, v in pl.items():
-                os.environ["RTEN_B200_FORCE_" + k] = str(v)
+    for pl in plans:
+        with switches(RTEN_B200_FORCE_BN=pl.get("BN"), RTEN_B200_FORCE_SPLITK=pl.get("SPLITK")):
             tag = f"plan {pl}"
             worst = max(worst, _matmul_case(rt, oracle, ctx, (384, 1024), (1024, 512), bias=True, prepack=True, seed=5))
             worst = max(worst, _matmul_case(rt, oracle, ctx, (3, 130, 520), (520, 300), seed=6))
@@ -448,9 +470,6 @@ def check_plans(rt, oracle):
                     f"{tag}: no launch of this sweep ran the forced plan ({miss} fell back to the model's choice)"
                 never.append(str(pl))
             hits_before = hit
-    finally:
-        for k in keys:
-            os.environ.pop(k, None)
     # autotuned plans: first call measures, second call replays the cached plan
     ctx2 = new_ctx(rt)
     ctx2.set_autotune(True)
@@ -815,9 +834,8 @@ def check_tf32x3(rt, oracle):
     finally:
         TF32_REL = saved
     # The two-plane form (A = original tensor for both `hi` segments + a low-part plane; prepacked B split once and
-    # cached) must be BIT-IDENTICAL to the three-segment copies built per call: kind::tf32 ignores the 13 low
+    # cached) must be BIT-IDENTICAL to the three-segment A copies built per call: kind::tf32 ignores the 13 low
     # mantissa bits, so feeding the raw f32 values is the same as feeding their truncations.
-    import os
     r = oracle.XorShiftRng(99)
     n_same = 0
     for (xs, ws, pads, strides) in [((4, 64, 14, 14), (128, 64, 3, 3), (1, 1, 1, 1), (1, 1)), ((3, 256, 9, 9), (64, 256, 1, 1), (0, 0, 0, 0), (1, 1)),
@@ -827,26 +845,16 @@ def check_tf32x3(rt, oracle):
         op = rt.Conv(1, (1, 1), pads, strides, activation=rt.ACT_RELU)
         pk = op.prepack(ctx, 1, wt)
         two = op.run(ctx, x, wt, packed_w=pk).numpy()
-        os.environ["RTEN_B200_X3_THREE_PLANES"] = "1"
-        os.environ["RTEN_B200_X3_NO_CACHE"] = "1"
-        try:
+        with switches(RTEN_B200_X3_THREE_PLANES=1):
             three = op.run(ctx, x, wt, packed_w=pk).numpy()
-        finally:
-            os.environ.pop("RTEN_B200_X3_THREE_PLANES")
-            os.environ.pop("RTEN_B200_X3_NO_CACHE")
         assert_bit_exact(two, three, f"3xTF32 conv {xs}x{ws}: two-plane vs three-segment operands")
         n_same += 1
     a, b = r.f32((300, 768)), r.f32((768, 320))
     db = ctx.to_device(b)
     pk = rt.MatMul().prepack(ctx, 1, db)
     two = rt.MatMul().run(ctx, ctx.to_device(a), db, packed_b=pk).numpy()
-    os.environ["RTEN_B200_X3_THREE_PLANES"] = "1"
-    os.environ["RTEN_B200_X3_NO_CACHE"] = "1"
-    try:
+    with switches(RTEN_B200_X3_THREE_PLANES=1):
         three = rt.MatMul().run(ctx, ctx.to_device(a), db, packed_b=pk).numpy()
-    finally:
-        os.environ.pop("RTEN_B200_X3_THREE_PLANES")
-        os.environ.pop("RTEN_B200_X3_NO_CACHE")
     assert_bit_exact(two, three, "3xTF32 MatMul 300x768x320: two-plane vs three-segment operands")
     assert_reference_rule(two, oracle.matmul(a, b), "3xTF32 MatMul 300x768x320 (two-plane)")
     rng = oracle.XorShiftRng(5678)
@@ -1299,12 +1307,9 @@ def check_gelu_epilogue(rt, oracle):
     the Gelu operator (the reference's scalar recipe, bit-exact against the oracle in check_unary) applied to the same
     product: FusedMatMul(bias, Gelu) vs FusedMatMul(bias) -> Gelu with the launch plan pinned (same accumulation order),
     for erf-Gelu and the tanh form, values spanning the exp cut-off, zeros and large magnitudes."""
-    import os
     ctx = new_ctx(rt, tf32=True)
     r = oracle.XorShiftRng(2718)
-    forced = {"RTEN_B200_FORCE_BN": "64", "RTEN_B200_FORCE_SPLITK": "1"}
-    os.environ.update(forced)
-    try:
+    with switches(RTEN_B200_FORCE_BN=64, RTEN_B200_FORCE_SPLITK=1):
         n = 0
         for (m, k, nn), amp in [((384, 64, 256), 1.0), ((256, 128, 384), 6.0), ((128, 32, 128), 40.0)]:
             a = (r.uniform((m, k), -1, 1) * amp).astype(np.float32)
@@ -1319,9 +1324,6 @@ def check_gelu_epilogue(rt, oracle):
                 two = rt.Gelu(approximate=approx).run(ctx, plain).numpy()
                 assert_bit_exact(fused, two, f"Gelu epilogue (approximate={approx}) {m}x{k}x{nn} amp {amp}")
                 n += 1
-    finally:
-        for kname in forced:
-            os.environ.pop(kname, None)
     return f"{n} fused-vs-operator comparisons bit-identical"
 
 
@@ -1357,26 +1359,6 @@ def _kernels_launched(fn):
     return out, names
 
 
-def _launch_lines(fn):
-    """Run `fn` under RTEN_B200_VERBOSE with file descriptor 2 sent to a temporary file: (its result, the launch lines
-    the library printed)."""
-    import sys
-    import tempfile
-    sys.stderr.flush()
-    saved = os.dup(2)
-    with tempfile.TemporaryFile() as f:
-        os.dup2(f.fileno(), 2)
-        os.environ["RTEN_B200_VERBOSE"] = "1"
-        try:
-            out = fn()
-        finally:
-            os.environ.pop("RTEN_B200_VERBOSE", None)
-            os.dup2(saved, 2)
-            os.close(saved)
-        f.seek(0)
-        return out, f.read().decode(errors="replace")
-
-
 def check_halo_conv(rt, oracle):
     """Stride-1 windows on the halo-reuse kernel (one activation patch per channel block in shared memory, the filter taps
     as shifted matrix descriptors): ResNet-50's 3x3 layer shapes at several batch sizes (row strips, whole images, batch
@@ -1385,16 +1367,11 @@ def check_halo_conv(rt, oracle):
     comes out at one image per unit; tests/test_gpu_plan_space.py pins units of several.)  The same cases in 3xTF32 run
     on the generic kernel, which is asserted too: the split operands carry a second A plane (x3_cb), which the halo
     kernel does not take."""
-    import os
-    os.environ["RTEN_B200_HALO"] = "1"  # the kernel is opt-in (the generic kernel stays the default)
-    try:
+    with switches(RTEN_B200_HALO=1):  # the kernel is opt-in (the generic kernel stays the default)
         return _check_halo_conv(rt, oracle)
-    finally:
-        os.environ.pop("RTEN_B200_HALO", None)
 
 
 def _check_halo_conv(rt, oracle):
-    import os
     worst, n = 0.0, 0
     cases = [((2, 64, 56, 56), (64, 64, 3, 3), (1, 1, 1, 1)), ((3, 128, 28, 28), (128, 128, 3, 3), (1, 1, 1, 1)),
              ((5, 256, 14, 14), (256, 256, 3, 3), (1, 1, 1, 1)), ((7, 512, 7, 7), (512, 512, 3, 3), (1, 1, 1, 1)),
@@ -1409,7 +1386,7 @@ def _check_halo_conv(rt, oracle):
         try:
             for xs, ws, pads in cases:
                 for act in (0, 1):
-                    w, log = _launch_lines(lambda: _conv_case(rt, oracle, ctx, xs, ws, pads=pads, cl=True, prepack=True, act=act))
+                    w, log = run_verbose(lambda: _conv_case(rt, oracle, ctx, xs, ws, pads=pads, cl=True, prepack=True, act=act))
                     kernel = "umma_halo" if tf32 else "umma_gemm"
                     other = "umma_gemm" if tf32 else "umma_halo"
                     assert f"[{kernel}]" in log and f"[{other}]" not in log, \
@@ -1426,12 +1403,9 @@ def _check_halo_conv(rt, oracle):
     op = rt.Conv(1, (1, 1), (1, 1, 1, 1), (1, 1), activation=1)
     halo, names = _kernels_launched(lambda: op.run(ctx, xd, w, b).numpy())
     assert any("umma_halo_kernel" in k for k in names), f"the halo kernel did not run (kernels: {sorted(names)})"
-    os.environ["RTEN_B200_NO_HALO"] = "1"
-    try:
+    with switches(RTEN_B200_NO_HALO=1):
         generic, names = _kernels_launched(lambda: op.run(ctx, xd, w, b).numpy())
         assert not any("umma_halo_kernel" in k for k in names), "RTEN_B200_NO_HALO must select the generic kernel"
-    finally:
-        os.environ.pop("RTEN_B200_NO_HALO", None)
     exact, absum = _conv_exact(x, w, b, (1, 1, 1, 1), 1, (1, 1), (1, 1))
     assert_tf32_close(halo, np.maximum(exact, 0), absum, "halo kernel")
     assert_tf32_close(generic, np.maximum(exact, 0), absum, "generic kernel")

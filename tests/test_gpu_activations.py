@@ -10,7 +10,6 @@ the convolution epilogues.
   * unknown activation kinds, and the new kinds on conv2d_ex and conv_integer_ex, are refused;
   * EfficientNet- and MobileNetV3-style block models through the executor: SiluFusion in both Mul operand orders, a
     Sigmoid with a second consumer left alone, Conv + activation fused, Clip not fused -- equal to the op-by-op calls."""
-import os
 import re
 
 import numpy as np
@@ -180,10 +179,10 @@ def test_residual_then_activation(rt, oracle):
 
 _PLAN_LINE = re.compile(r"\[umma_gemm\] [^\n]*?\bepi=(\w+)")
 _KNOBS = {"default": {}, "no_plain": {"RTEN_B200_NO_PLAIN": "1"}, "no_fast": {"RTEN_B200_NO_FAST": "1"}}
-_ENV_KEYS = ("RTEN_B200_NO_PLAIN", "RTEN_B200_NO_FAST", "RTEN_B200_NO_WIDE", "RTEN_B200_VERBOSE") + gc.FORCE_KEYS
+_ENV_KEYS = ("RTEN_B200_NO_PLAIN", "RTEN_B200_NO_FAST", "RTEN_B200_NO_WIDE") + gc.FORCE_KEYS
 
 
-def test_epilogue_variants_agree(rt, oracle, capfd):
+def test_epilogue_variants_agree(rt, oracle):
     """A 1x1 convolution + bias + each new code on umma_gemm_kernel: PlainF32Gelu, FastGelu and Generic (the variants
     with the out-of-line activation call, and the rolled generic loop) give the same bits."""
     r = oracle.XorShiftRng(11)
@@ -193,16 +192,9 @@ def test_epilogue_variants_agree(rt, oracle, capfd):
     for aname, _, _, act in _ops(rt):
         ref = None
         for (knob, env), want in zip(_KNOBS.items(), ("PlainF32Gelu", "FastGelu", "Generic")):
-            capfd.readouterr()
-            saved = {k: os.environ.pop(k) for k in _ENV_KEYS if k in os.environ}
-            os.environ.update(env, RTEN_B200_VERBOSE="1", RTEN_B200_NO_WIDE="1")
-            try:
-                out = rt.Conv(activation=act).run(ctx, xd, w, b).numpy()
-            finally:
-                for k in _ENV_KEYS:
-                    os.environ.pop(k, None)
-                os.environ.update(saved)
-            epis = _PLAN_LINE.findall(capfd.readouterr().err)
+            with gc.switches(**{**dict.fromkeys(_ENV_KEYS), **env, "RTEN_B200_NO_WIDE": "1"}):
+                out, err = gc.run_verbose(lambda: rt.Conv(activation=act).run(ctx, xd, w, b).numpy())
+            epis = _PLAN_LINE.findall(err)
             assert epis and all(v == want for v in epis), f"{aname} ({knob}): ran {epis}, expected {want}"
             if ref is None:
                 ref = out

@@ -7,7 +7,6 @@ run as ONE launch of the wide kernel's chained mode (GemmLaunch::chain), which c
   * 3xTF32 and pairs that do not qualify run as the separate calls (no `chain=` launch), bit for bit;
   * ResNet50Runner(chain=True) gives the logits of chain=False bit for bit;
   * invalid arguments fail with their status."""
-import os
 import re
 
 import numpy as np
@@ -94,25 +93,20 @@ class _Dev:
         return y.numpy(), z.numpy()
 
 
-def _lines(capfd, fn):
-    capfd.readouterr()
-    os.environ["RTEN_B200_VERBOSE"] = "1"
-    try:
-        out = fn()
-    finally:
-        os.environ.pop("RTEN_B200_VERBOSE", None)
-    return out, _PLAN_LINE.findall(capfd.readouterr().err)
+def _lines(fn):
+    out, err = gc.run_verbose(fn)
+    return out, _PLAN_LINE.findall(err)
 
 
 @pytest.mark.parametrize("name", list(PAIRS))
-def test_chained_pairs_equal_separate_calls(rt, oracle, capfd, name):
+def test_chained_pairs_equal_separate_calls(rt, oracle, name):
     shape = PAIRS[name]
     c = _case(oracle, shape)
     ctx = gc.new_ctx(rt)
     d = _Dev(rt, ctx, c)
     ref_y, ref_z = d.separate()
     for rep in range(3):
-        (y, z), lines = _lines(capfd, d.chained)
+        (y, z), lines = _lines(d.chained)
         assert len(lines) == 1 and f" chain={shape[4]}" in lines[0], f"{name}: not one chained launch ({lines})"
         gc.assert_bit_exact(y, ref_y, f"{name} run {rep}: y")
         gc.assert_bit_exact(z, ref_z, f"{name} run {rep}: z")
@@ -123,29 +117,26 @@ def test_chained_pairs_equal_separate_calls(rt, oracle, capfd, name):
 
 
 @pytest.mark.parametrize("kind", ["tf32x3", "NCHW", "3x3 next", "N2=96", "N=288"])
-def test_fallback_equals_separate_calls(rt, oracle, capfd, kind):
+def test_fallback_equals_separate_calls(rt, oracle, kind):
     shape = {"N2=96": (2, 9, 64, 96, 96, 0), "N=288": (2, 9, 64, 288, 64, 0)}.get(kind, (2, 9, 64, 96, 64, 0))
     c = _case(oracle, shape, seed=11, k_next=3 if kind == "3x3 next" else 1)
     ctx = gc.new_ctx(rt, tf32=kind != "tf32x3")
     d = _Dev(rt, ctx, c, nchw=kind == "NCHW")
-    (y, z), lines = _lines(capfd, d.chained)
+    (y, z), lines = _lines(d.chained)
     assert not any("chain=" in ln for ln in lines), f"{kind}: chained although it must not ({lines})"
     ref_y, ref_z = d.separate()
     gc.assert_bit_exact(y, ref_y, f"{kind}: y")
     gc.assert_bit_exact(z, ref_z, f"{kind}: z")
 
 
-def test_no_chain_switch(rt, oracle, capfd):
+def test_no_chain_switch(rt, oracle):
     c = _case(oracle, PAIRS["B3 9x9 N96 residual"])
     ctx = gc.new_ctx(rt)
     d = _Dev(rt, ctx, c)
-    os.environ["RTEN_B200_NO_CHAIN"] = "1"
-    try:
-        (y, z), lines = _lines(capfd, d.chained)
-    finally:
-        os.environ.pop("RTEN_B200_NO_CHAIN", None)
+    with gc.switches(RTEN_B200_NO_CHAIN=1):
+        (y, z), lines = _lines(d.chained)
     assert not any("chain=" in ln for ln in lines)
-    (y2, z2), lines = _lines(capfd, d.chained)
+    (y2, z2), lines = _lines(d.chained)
     assert any("chain=" in ln for ln in lines)
     gc.assert_bit_exact(y, y2, "RTEN_B200_NO_CHAIN: y")
     gc.assert_bit_exact(z, z2, "RTEN_B200_NO_CHAIN: z")

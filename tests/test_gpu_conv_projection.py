@@ -8,7 +8,6 @@ wgmma kernels' projection source, GemmLaunch::proj); the rest run as two convolu
     launch more work units than the device has SMs;
   * pairs that must not fold equal conv2d_ex(down) followed by conv2d_ex(c3, residual, relu) bit for bit;
   * mismatched output shapes and non-f32 inputs fail with their status."""
-import os
 import re
 
 import numpy as np
@@ -99,24 +98,19 @@ class _Dev:
         return self.op.run(self.ctx, self.t, self.w3, self.b3, packed_w=self.pk3, residual=ident).numpy()
 
 
-def _plan_lines(capfd, fn):
-    capfd.readouterr()
-    os.environ["RTEN_B200_VERBOSE"] = "1"
-    try:
-        out = fn()
-    finally:
-        os.environ.pop("RTEN_B200_VERBOSE", None)
-    return out, [tuple(int(v) for v in m) for m in _PLAN_LINE.findall(capfd.readouterr().err)]
+def _plan_lines(fn):
+    out, err = gc.run_verbose(fn)
+    return out, [tuple(int(v) for v in m) for m in _PLAN_LINE.findall(err)]
 
 
 @pytest.mark.parametrize("tf32", [True, False], ids=["tf32", "tf32x3"])
 @pytest.mark.parametrize("name", list(BLOCKS) + list(RAGGED))
-def test_projection_blocks(rt, oracle, capfd, name, tf32):
+def test_projection_blocks(rt, oracle, name, tf32):
     shape = BLOCKS.get(name) or RAGGED[name]
     c = _case(oracle, shape)
     ctx = gc.new_ctx(rt, tf32=tf32)
     d = _Dev(rt, ctx, c)
-    got, plans = _plan_lines(capfd, d.folded)
+    got, plans = _plan_lines(d.folded)
     assert len(plans) == 1 and plans[0][0] == shape[1] // 32 * (1 if tf32 else 3), f"{name}: not folded into one GEMM ({plans})"
     exact, absum = _exact(name, c)
     with bound(tf32):
@@ -125,7 +119,7 @@ def test_projection_blocks(rt, oracle, capfd, name, tf32):
 
 @pytest.mark.parametrize("tf32", [True, False], ids=["tf32", "tf32x3"])
 @pytest.mark.parametrize("shape", [(8, 64, 56, 64, 256, 1), (8, 256, 56, 128, 512, 2)], ids=["s1", "s2"])
-def test_forced_plans_agree(rt, oracle, capfd, shape, tf32):
+def test_forced_plans_agree(rt, oracle, shape, tf32):
     c = _case(oracle, shape, seed=99)
     ctx = gc.new_ctx(rt, tf32=tf32)
     d = _Dev(rt, ctx, c)
@@ -139,7 +133,7 @@ def test_forced_plans_agree(rt, oracle, capfd, shape, tf32):
     for bn in (64, 128, 256):
         with forced(bn):
             h0, _ = ctx.forced_plan_counts()
-            outs[bn], plans = _plan_lines(capfd, d.folded)
+            outs[bn], plans = _plan_lines(d.folded)
             h1, _ = ctx.forced_plan_counts()
         assert h1 > h0, f"bn={bn}: the forced plan was not taken"
         assert len(plans) == 1 and plans[0][0] > 0 and plans[0][1] == bn, f"bn={bn}: {plans}"
@@ -155,12 +149,12 @@ def test_forced_plans_agree(rt, oracle, capfd, shape, tf32):
 
 @pytest.mark.parametrize("tf32", [True, False], ids=["tf32", "tf32x3"])
 @pytest.mark.parametrize("kind", ["3x3 main", "48-channel projection", "NCHW"])
-def test_fallback_matches_two_calls(rt, oracle, capfd, kind, tf32):
+def test_fallback_matches_two_calls(rt, oracle, kind, tf32):
     shape = (3, 48 if kind == "48-channel projection" else 64, 14, 64, 128, 2)
     c = _case(oracle, shape, seed=7, main_k=3 if kind == "3x3 main" else 1)
     ctx = gc.new_ctx(rt, tf32=tf32)
     d = _Dev(rt, ctx, c, nchw=kind == "NCHW")
-    got, plans = _plan_lines(capfd, d.folded)
+    got, plans = _plan_lines(d.folded)
     assert all(p[0] == 0 for p in plans), f"{kind}: folded although it must not ({plans})"
     gc.assert_bit_exact(got, d.two_calls(), f"{kind}: projected vs two calls")
     exact, absum = _exact(f"fallback {kind}", c)

@@ -4,7 +4,6 @@ RTEN_B200_NO_FAST (everything on Generic).  The variant that ran is read from th
 and so are the work units: every variant runs at least one launch with more units than SMs, so the staging ring and
 the barrier phases carry over from one unit to the next.  f32 outputs, i32 outputs and the *ToFloat output ranges must
 be bit-identical across the three runs."""
-import os
 import re
 
 import numpy as np
@@ -17,7 +16,7 @@ pytestmark = pytest.mark.gpu
 _PLAN_LINE = re.compile(r"\[umma_gemm\] [^\n]*?\bsplitk=(\d+) units=(\d+) [^\n]*?\bepi=(\w+)")
 KNOBS = {"default": {}, "no_plain": {"RTEN_B200_NO_PLAIN": "1"}, "no_fast": {"RTEN_B200_NO_FAST": "1"}}
 VARIANTS = ("Generic", "Fast", "FastGelu", "PlainF32", "PlainF32Gelu", "PlainI8", "PlainI8Gelu")
-_ENV_KEYS = ("RTEN_B200_NO_PLAIN", "RTEN_B200_NO_FAST", "RTEN_B200_NO_WIDE", "RTEN_B200_VERBOSE") + gc.FORCE_KEYS
+_ENV_KEYS = ("RTEN_B200_NO_PLAIN", "RTEN_B200_NO_FAST", "RTEN_B200_NO_WIDE") + gc.FORCE_KEYS
 
 
 @pytest.fixture(scope="module")
@@ -28,19 +27,12 @@ def rt():
     return rten_b200
 
 
-def _under(capfd, env, run):
+def _under(env, run):
     """run() with `env` and RTEN_B200_VERBOSE set, on umma_gemm_kernel only (no wide-tile plans): its outputs and the
     (splitk, units, epi) of every GEMM launch."""
-    capfd.readouterr()
-    saved = {k: os.environ.pop(k) for k in _ENV_KEYS if k in os.environ}
-    os.environ.update(env, RTEN_B200_VERBOSE="1", RTEN_B200_NO_WIDE="1")
-    try:
-        outs = run()
-    finally:
-        for k in _ENV_KEYS:
-            os.environ.pop(k, None)
-        os.environ.update(saved)
-    plans = [(int(s), int(u), v) for s, u, v in _PLAN_LINE.findall(capfd.readouterr().err)]
+    with gc.switches(**{**dict.fromkeys(_ENV_KEYS), **env, "RTEN_B200_NO_WIDE": "1"}):
+        outs, err = gc.run_verbose(run)
+    plans = [(int(s), int(u), v) for s, u, v in _PLAN_LINE.findall(err)]
     return outs, plans
 
 
@@ -119,7 +111,7 @@ def _cases(rt, oracle, ctx):
     return cases
 
 
-def test_epilogue_variants_agree(rt, oracle, capfd):
+def test_epilogue_variants_agree(rt, oracle):
     import torch
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     ctx = gc.new_ctx(rt, tf32=True)
@@ -127,7 +119,7 @@ def test_epilogue_variants_agree(rt, oracle, capfd):
     for name, run, expect in _cases(rt, oracle, ctx):
         ref = None
         for (knob, env), want in zip(KNOBS.items(), expect):
-            outs, plans = _under(capfd, env, run)
+            outs, plans = _under(env, run)
             assert plans, f"{name} ({knob}): no GEMM launch line was printed"
             assert all(v == want for _, _, v in plans), f"{name} ({knob}): ran {plans}, expected epi={want}"
             persistent.update(v for _, u, v in plans if u > sms)
@@ -143,7 +135,7 @@ def test_epilogue_variants_agree(rt, oracle, capfd):
     assert not missing, f"variants never run on more work units than SMs: {missing}"
 
 
-def test_epilogue_variants_splitk(rt, oracle, capfd):
+def test_epilogue_variants_splitk(rt, oracle):
     """Forced split-K (two CTAs per tile, the last to arrive sums in split order and runs the epilogue): the same bits
     from PlainF32, Fast and Generic, and from Fast and Generic for the integer kind (PlainI8 takes no split-K)."""
     ctx = gc.new_ctx(rt, tf32=True)
@@ -167,7 +159,7 @@ def test_epilogue_variants_splitk(rt, oracle, capfd):
     for name, run, expect in cases:
         ref = None
         for (knob, env), want in zip(KNOBS.items(), expect):
-            outs, plans = _under(capfd, {**env, **split}, run)
+            outs, plans = _under({**env, **split}, run)
             assert plans and all(s == 2 and v == want for s, _, v in plans), \
                 f"{name} ({knob}): ran {plans}, expected split-K 2 with epi={want}"
             if ref is None:

@@ -4,8 +4,6 @@ test_gpu_plan_space.py do not reach.  For each accepted shape: the [umma_halo] l
 float64 TF32 bound, bit-identical to the 128-slot plan `-1 32 1` of the same problem, or to its first 256-slot plan where
 no 128-slot unit holds a row (every halo shape accumulates in one order), and two CUDA-graph replays into a NaN-poisoned output give the eager run's bits.  A shape the geometry cannot take
 (a patch that no longer fits in shared memory, bn not dividing N) must be rejected and the launch re-planned."""
-import os
-
 import pytest
 
 import gpu_checks as gc
@@ -42,24 +40,21 @@ def rt():
 
 @pytest.fixture(autouse=True)
 def _clean_env():
-    saved = {k: os.environ.pop(k) for k in ps._ENV if k in os.environ}
-    yield
-    for k in ps._ENV:
-        os.environ.pop(k, None)
-    os.environ.update(saved)
+    with gc.switches(**dict.fromkeys(ps._ENV)):
+        yield
 
 
 @pytest.mark.parametrize("name,kw,t1,want", WIDE_CASES, ids=[c[0] for c in WIDE_CASES])
-def test_halo_256_slot_units(rt, capfd, tmp_path, name, kw, t1, want):
+def test_halo_256_slot_units(rt, tmp_path, name, kw, t1, want):
     import torch
     prob = ps.ConvF32(f"halo-wide {name}", True, **kw)
-    _, key = ps._candidates(rt, capfd, prob, tmp_path)
+    _, key = ps._candidates(rt, prob, tmp_path)
     ctx = gc.new_ctx(rt, tf32=True)
     run = prob.build(rt, ctx)
     exact, absum = prob.exact()
     # the bits every halo shape must give: the 128-slot plan's where the geometry has one, else the first 256-slot plan's
     ref, worst = None, 0.0
-    outs, err = ps._pin(capfd, ctx, run, prob, key, (-1, 32, 1), tmp_path)
+    outs, err = ps._pin(ctx, run, prob, key, (-1, 32, 1), tmp_path)
     if t1:
         assert ps._ran(err, (-1, 32, 1), prob.name)[1] == 1
         ref = (outs[0], "-1 32 1")
@@ -69,7 +64,7 @@ def test_halo_256_slot_units(rt, capfd, tmp_path, name, kw, t1, want):
     ran = []
     for bn, shape in want.items():
         plan = (-1, bn, 2)
-        outs, err = ps._pin(capfd, ctx, run, prob, key, plan, tmp_path)
+        outs, err = ps._pin(ctx, run, prob, key, plan, tmp_path)
         if shape is None:
             assert ps._STALE in err and len(ps._GEMM.findall(err)) == 1 and not ps._HALO.search(err), \
                 f"{prob.name}: `-1 {bn} 2` cannot fit this geometry and must be re-planned; printed: {err.strip()}"

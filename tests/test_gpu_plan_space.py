@@ -20,7 +20,6 @@ Single-pass TF32 problems use non-negative operands (U[0, 1)): one lost or doubl
 by at least 1 / k_blocks of it, more than the 2^-9 bound (test_gpu_bench_gemm.py explains why signed data hides it).
 3xTF32 problems use signed data; their bound is tight enough either way.  The last test asserts that the pinned plans
 covered every split-K count, nbuf and bn the kernels have, and halo units of several images."""
-import os
 import re
 
 import numpy as np
@@ -35,8 +34,8 @@ _CAND_HALO = re.compile(r"\[autotune\] halo bn=(\d+) T=(\d+)")
 _GEMM = re.compile(r"\[umma_gemm\] [^\n]*?\bbn=(\d+) splitk=(\d+) [^\n]*?\bnbuf=(\d+)")
 _HALO = re.compile(r"\[umma_halo\] [^\n]*?: bn=(\d+) T=(\d+) R=(\d+) tb=(\d+) P=(\d+)")
 _STALE = "recorded plan no longer valid"
-_ENV = ("RTEN_B200_VERBOSE", "RTEN_B200_HALO", "RTEN_B200_NO_HALO", "RTEN_B200_NO_WIDE", "RTEN_B200_NO_NBUF3",
-        "RTEN_B200_AUTOTUNE", "RTEN_B200_TUNE_FILE") + gc.FORCE_KEYS
+_ENV = ("RTEN_B200_VERBOSE", "RTEN_B200_HALO", "RTEN_B200_NO_HALO", "RTEN_B200_NO_WIDE", "RTEN_B200_AUTOTUNE",
+        "RTEN_B200_TUNE_FILE") + gc.FORCE_KEYS
 GELU_SLOPE = 1.13  # max |d gelu / dx| = 1.1289...: a pre-activation error bound carries through Gelu scaled by this
 
 # what the pinned plans of the whole module covered (test_coverage)
@@ -53,22 +52,8 @@ def rt():
 
 @pytest.fixture(autouse=True)
 def _clean_env():
-    saved = {k: os.environ.pop(k) for k in _ENV if k in os.environ}
-    yield
-    for k in _ENV:
-        os.environ.pop(k, None)
-    os.environ.update(saved)
-
-
-def _logged(capfd, fn):
-    """fn() under RTEN_B200_VERBOSE: (its result, what the library printed)."""
-    capfd.readouterr()
-    os.environ["RTEN_B200_VERBOSE"] = "1"
-    try:
-        out = fn()
-    finally:
-        os.environ.pop("RTEN_B200_VERBOSE", None)
-    return out, capfd.readouterr().err
+    with gc.switches(**dict.fromkeys(_ENV)):
+        yield
 
 
 # ------------------------------------------------------------------------------------------
@@ -342,12 +327,12 @@ def _collect(prob, run, ctx):
     return [_np(t) for t in ts]
 
 
-def _candidates(rt, capfd, prob, tmp_path):
+def _candidates(rt, prob, tmp_path):
     """Step 1: the plans the autotuner times for `prob` ((bn, splitk, nbuf), halo: (-1, bn, T)) and its plans-file key."""
     ctx = gc.new_ctx(rt, tf32=prob.tf32 is not False)
     ctx.set_autotune(True)
     run = prob.build(rt, ctx)
-    _, err = _logged(capfd, lambda: _collect(prob, run, ctx))
+    _, err = gc.run_verbose(lambda: _collect(prob, run, ctx))
     cands = [tuple(int(v) for v in c) for c in _CAND.findall(err)]
     cands += [(-1, int(b), int(t)) for b, t in _CAND_HALO.findall(err)]
     path = tmp_path / "autotuned.plans"
@@ -359,12 +344,12 @@ def _candidates(rt, capfd, prob, tmp_path):
     return list(dict.fromkeys(cands)), lines[0].split("|")[0].strip()
 
 
-def _pin(capfd, ctx, run, prob, key, plan, tmp_path):
+def _pin(ctx, run, prob, key, plan, tmp_path):
     """Load `<key> | plan` into ctx and run: (outputs, what the library printed)."""
     path = tmp_path / "pinned.plans"
     path.write_text(f"{key} | {plan[0]} {plan[1]} {plan[2]}\n")
     ctx.load_plans(str(path))
-    return _logged(capfd, lambda: _collect(prob, run, ctx))
+    return gc.run_verbose(lambda: _collect(prob, run, ctx))
 
 
 def _ran(err, plan, what):
@@ -386,10 +371,10 @@ def _decode_range(i):
     return float(np.int32(i if i >= 0 else i ^ 0x7FFFFFFF).view(np.float32))
 
 
-def _sweep(rt, oracle, capfd, tmp_path, prob):
+def _sweep(rt, oracle, tmp_path, prob):
     import torch
     what = prob.name
-    pins, key = _candidates(rt, capfd, prob, tmp_path)
+    pins, key = _candidates(rt, prob, tmp_path)
     assert pins, f"{what}: the autotuner timed no plan"
     ctx = gc.new_ctx(rt, tf32=prob.tf32 is not False)
     run = prob.build(rt, ctx)
@@ -404,7 +389,7 @@ def _sweep(rt, oracle, capfd, tmp_path, prob):
             extra = 2.0 ** -20 * np.abs(exact)  # the activation's own f32 evaluation
     reps, worst = {}, 0.0  # K-order class (split-K count, or "halo") -> (first plan, its outputs)
     for plan in pins:
-        outs, err = _pin(capfd, ctx, run, prob, key, plan, tmp_path)
+        outs, err = _pin(ctx, run, prob, key, plan, tmp_path)
         halo = _ran(err, plan, what)
         if halo is None:
             _COVERED["splitk"].add(plan[1])
@@ -429,7 +414,7 @@ def _sweep(rt, oracle, capfd, tmp_path, prob):
     plan = max((p for p in pins if p[0] > 0), key=lambda p: p[1], default=None)
     if plan is not None:
         ref = reps[plan[1]][1]
-        runs = [_pin(capfd, ctx, run, prob, key, plan, tmp_path)[0] for _ in range(2)]
+        runs = [_pin(ctx, run, prob, key, plan, tmp_path)[0] for _ in range(2)]
         ctx.graph_begin()
         run()
         g = ctx.graph_end()
@@ -452,21 +437,21 @@ def _sweep(rt, oracle, capfd, tmp_path, prob):
 
 
 @pytest.mark.parametrize("name,cls,kw", F32_PROBLEMS, ids=[n for n, _, _ in F32_PROBLEMS])
-def test_f32_plans(rt, oracle, capfd, tmp_path, name, cls, kw):
-    _sweep(rt, oracle, capfd, tmp_path, cls(name, **kw))
+def test_f32_plans(rt, oracle, tmp_path, name, cls, kw):
+    _sweep(rt, oracle, tmp_path, cls(name, **kw))
 
 
 @pytest.mark.parametrize("name,cls,kw", INT_PROBLEMS, ids=[n for n, _, _ in INT_PROBLEMS])
-def test_integer_plans(rt, oracle, capfd, tmp_path, name, cls, kw):
-    _sweep(rt, oracle, capfd, tmp_path, cls(name, **kw))
+def test_integer_plans(rt, oracle, tmp_path, name, cls, kw):
+    _sweep(rt, oracle, tmp_path, cls(name, **kw))
 
 
 @pytest.mark.parametrize("name,kw,want", HALO_CASES, ids=[n for n, _, _ in HALO_CASES])
-def test_halo_unit_shapes(rt, capfd, tmp_path, name, kw, want):
+def test_halo_unit_shapes(rt, tmp_path, name, kw, want):
     """Both halo tiles pinned with `{-1, bn, 1}`: the unit shape the [umma_halo] line reports, the float64 bound, and
     the same bits from bn = 32 and 64."""
     prob = ConvF32(f"halo {name}", True, **kw)
-    _, key = _candidates(rt, capfd, prob, tmp_path)
+    _, key = _candidates(rt, prob, tmp_path)
     ctx = gc.new_ctx(rt, tf32=True)
     run = prob.build(rt, ctx)
     exact, absum = prob.exact()
@@ -475,7 +460,7 @@ def test_halo_unit_shapes(rt, capfd, tmp_path, name, kw, want):
         if kw["ws"][0] % bn:
             continue
         plan = (-1, bn, 1)
-        outs, err = _pin(capfd, ctx, run, prob, key, plan, tmp_path)
+        outs, err = _pin(ctx, run, prob, key, plan, tmp_path)
         if want is None:
             assert _STALE in err and len(_GEMM.findall(err)) == 1 and not _HALO.search(err), \
                 f"{prob.name}: the halo kernel cannot take this window; pinned bn={bn} printed: {err.strip()}"
@@ -496,7 +481,7 @@ def test_halo_unit_shapes(rt, capfd, tmp_path, name, kw, want):
     print(f"\n  {prob.name}: {shapes if shapes else 'falls back to the generic kernel'}; worst err/bound {worst:.3f}")
 
 
-def test_bad_recorded_plans(rt, capfd, tmp_path):
+def test_bad_recorded_plans(rt, tmp_path):
     """Plans files are outside input: an entry no kernel can run (split-K 0 or negative, a 96-column tile, a 48-column
     halo tile, a halo tile for a stride-2 window) is dropped with a message and the launch planned afresh, computing
     the bits of an unpinned launch."""
@@ -504,16 +489,16 @@ def test_bad_recorded_plans(rt, capfd, tmp_path):
              (ConvF32("3x3 s2", True, (4, 256, 14, 14), (256, 256, 3, 3), 2, 1, seed=52), ("-1 32 1", "32 0 1"))]
     path = tmp_path / "bad.plans"
     for prob, entries in cases:
-        _, key = _candidates(rt, capfd, prob, tmp_path)
+        _, key = _candidates(rt, prob, tmp_path)
         ctx = gc.new_ctx(rt, tf32=True)
         run = prob.build(rt, ctx)
-        want, err = _logged(capfd, lambda: _collect(prob, run, ctx))  # no plans recorded: the cost model's plan
+        want, err = gc.run_verbose(lambda: _collect(prob, run, ctx))  # no plans recorded: the cost model's plan
         model = _GEMM.findall(err)
         assert len(model) == 1, err
         for entry in entries:
             path.write_text(f"{key} | {entry}\n")
             ctx.load_plans(str(path))
-            got, err = _logged(capfd, lambda: _collect(prob, run, ctx))
+            got, err = gc.run_verbose(lambda: _collect(prob, run, ctx))
             assert _STALE in err, f"{prob.name}: `| {entry}` was not reported as invalid: {err.strip()}"
             assert _GEMM.findall(err) == model and not _HALO.search(err), \
                 f"{prob.name}: `| {entry}` did not re-plan to the unpinned launch {model}: {err.strip()}"

@@ -3,7 +3,6 @@ oracle/resize.py across modes, layouts, ranks and output strides; the decoder mo
 the model API in both f32 modes, with the Concat elision on and off giving identical bits."""
 import itertools
 import json
-import os
 
 import numpy as np
 import pytest
@@ -166,14 +165,9 @@ def test_average_pool_bit_exact(rt, ctx, count_include_pad):
 
 
 def _run_model(rt, data, x, tf32, elide, outputs=None):
-    os.environ.pop("RTEN_B200_NO_CONCAT_ELISION", None)
-    if not elide:
-        os.environ["RTEN_B200_NO_CONCAT_ELISION"] = "1"
-    try:
+    with gpu_checks.switches(RTEN_B200_NO_CONCAT_ELISION=None if elide else 1):
         ctx = gpu_checks.new_ctx(rt, tf32)
         model = rt.model.Model(ctx, data)
-    finally:
-        os.environ.pop("RTEN_B200_NO_CONCAT_ELISION", None)
     xd = ctx.to_device(x, channels_last=True)
     model.run({"x": xd}, outputs)  # (first run: weights split / plans made)
     before = ctx.launches

@@ -11,12 +11,12 @@ import os
 import numpy as np
 import pytest
 
+import gpu_checks as gc
 from oracle import oracle
 from oracle import rnn as orn
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 FLOOR = 3e-5  # absolute, on outputs in [-1, 1]: f32 FMA-chain / 3xTF32 rounding beyond the f32 restatement's own
-NO_CLUSTER = "RTEN_B200_NO_RNN_CLUSTER"
 
 
 @pytest.fixture(scope="module")
@@ -33,18 +33,6 @@ def _ctx(rt, tf32=False):
     return ctx
 
 
-class _Path:
-    def __init__(self, per_step):
-        self.per_step = per_step
-
-    def __enter__(self):
-        if self.per_step:
-            os.environ[NO_CLUSTER] = "1"
-
-    def __exit__(self, *a):
-        os.environ.pop(NO_CLUSTER, None)
-
-
 def _run(rt, ctx, op, ins, direction, per_step=False, outputs=None, packed=False):
     G = 3 if op == "gru" else 4
     H = ins["w"].shape[1] // G
@@ -54,7 +42,7 @@ def _run(rt, ctx, op, ins, direction, per_step=False, outputs=None, packed=False
         kw["outputs"] = outputs
     if packed:
         kw["packed_w"] = o.prepack(ctx, ins["w"])
-    with _Path(per_step):
+    with gc.switches(RTEN_B200_NO_RNN_CLUSTER=1 if per_step else None):
         res = o.run(ctx, ins["x"], ins["w"], ins["r"], **kw)
     return [None if t is None else t.numpy() for t in res]
 
@@ -198,7 +186,7 @@ def test_launch_counts_graph_replay_and_determinism(rt, op):
     assert ctx.launches - n0 == n_gemm + 1, f"cluster path: {ctx.launches - n0} launches, expected {n_gemm + 1}"
     for a, b in zip(eager, again):
         np.testing.assert_array_equal(a, b)
-    with _Path(True):
+    with gc.switches(RTEN_B200_NO_RNN_CLUSTER=1):
         n0 = ctx.launches
         per = [t.numpy() for t in call()]
         assert ctx.launches - n0 == n_gemm + 1 + T * 3, f"per-step path: {ctx.launches - n0} launches"

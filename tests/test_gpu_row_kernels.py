@@ -26,7 +26,6 @@ third.
     kernel's limits;
   * DynamicQuantizeLinear: degenerate ranges on the one-kernel and three-kernel paths, and the ranged form fed by a
     MatMulIntegerToFloat out_range, before and after re-arming it."""
-import contextlib
 import json
 import os
 import re
@@ -152,16 +151,6 @@ def _rng(*key):
 
 def _bits(got, want, what):
     gc.assert_bit_exact(np.asarray(got), np.asarray(want), what)
-
-
-class _NoVecRows:
-    """RTEN_B200_NO_VEC_ROWS inside the block: the row launchers read it per launch and take the generic kernels."""
-
-    def __enter__(self):
-        os.environ["RTEN_B200_NO_VEC_ROWS"] = "1"
-
-    def __exit__(self, *exc):
-        os.environ.pop("RTEN_B200_NO_VEC_ROWS", None)
 
 
 # ---- Softmax / AddSoftmax ---------------------------------------------------------------------------------------------
@@ -649,7 +638,7 @@ def _kernel_probe():
                 def call():
                     launch(rt, ctx, s, inp, **kw)
                     ctx.sync()
-                with (_NoVecRows() if no_vec else contextlib.nullcontext()):
+                with gc.switches(RTEN_B200_NO_VEC_ROWS=1 if no_vec else None):
                     names, again = capture_kernels(call)
                 retaken += again
                 res[spec_id(fam, s) + " " + label] = sorted(names)
@@ -711,7 +700,7 @@ def test_softmax_bit_exact(rt, oracle, sms):
             want = softmax_want(oracle, s, inp, flush)
             got = softmax_launch(rt, ctx, s, inp, flush)
             _bits(got, want, f"{sid} flush={flush}")
-            with _NoVecRows():
+            with gc.switches(RTEN_B200_NO_VEC_ROWS=1):
                 _bits(softmax_launch(rt, ctx, s, inp, flush), got, f"{sid} flush={flush}: generic kernel")
         softmax_f64_check(s, inp, got, f"{sid}: float64")
 
@@ -726,7 +715,7 @@ def test_layer_norm_bit_exact(rt, oracle, sms):
         for arm in LN_ARMS:
             got = norm_launch(rt, ctx, s, inp, arm)
             _bits(got, norm_want(oracle, s, inp, arm), f"{sid} {arm}")
-            with _NoVecRows():
+            with gc.switches(RTEN_B200_NO_VEC_ROWS=1):
                 _bits(norm_launch(rt, ctx, s, inp, arm), got, f"{sid} {arm}: generic kernel")
             if arm == "scale + bias" and inp["first"] < s["rows"]:
                 x = inp["x"][inp["first"]:].astype(np.float64)
@@ -752,7 +741,7 @@ def test_rms_and_skip_norms_bit_exact(rt, oracle, sms):
         sid = spec_id("norm", s)
         got = norm_launch(rt, ctx, s, inp)
         _bits(got, norm_want(oracle, s, inp), sid)
-        with _NoVecRows():
+        with gc.switches(RTEN_B200_NO_VEC_ROWS=1):
             _bits(norm_launch(rt, ctx, s, inp), got, f"{sid}: generic kernel")
 
 

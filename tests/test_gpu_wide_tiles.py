@@ -4,7 +4,6 @@ result must meet the TF32 (or 3xTF32) bound against float64, the wide kernel mus
 CUPTI kernel records where the session has them), and both plans must agree bit for bit (same K order, same epilogue
 roundings).  The persistent-schedule cases launch more work units than the device has SMs, so every CTA carries its
 pipeline state from one unit to the next."""
-import os
 import re
 
 import numpy as np
@@ -27,31 +26,26 @@ def rt():
     return rten_b200
 
 
-def _with_plan_lines(capfd, fn):
+def _with_plan_lines(fn):
     """`fn()` with RTEN_B200_VERBOSE=1, and the (bn, units) of every GEMM launch it printed to stderr."""
-    capfd.readouterr()
-    os.environ["RTEN_B200_VERBOSE"] = "1"
-    try:
-        out = fn()
-    finally:
-        os.environ.pop("RTEN_B200_VERBOSE", None)
-    return out, [(int(b), int(u)) for b, u in _PLAN_LINE.findall(capfd.readouterr().err)]
+    out, err = gc.run_verbose(fn)
+    return out, [(int(b), int(u)) for b, u in _PLAN_LINE.findall(err)]
 
 
-def _wide_vs_narrow(ctx, run, bn, what, seen, capfd=None, repeats=1):
+def _wide_vs_narrow(ctx, run, bn, what, seen, log=False, repeats=1):
     """Output of `run` on a forced wide plan and its largest difference from the forced 64-column plan.  Under
     FORCE_STRICT a forced-plan hit means a bn > 64 plan was launched, and only umma_wide_kernel runs those.  CUPTI must
     agree: no umma_gemm_kernel in the session, and umma_wide_kernel among its umma_ records.  (Inside the whole GPU
     suite a session can miss the records of kernels launched with launch attributes while keeping others; `seen`
-    counts the sessions that did record the wide kernel.)  With `capfd` the (bn, units) of the wide launches are
+    counts the sessions that did record the wide kernel.)  With `log` the (bn, units) of the wide launches are
     returned too.  `repeats` > 1 runs the wide plan that many times in all, and every run must give the same bits."""
     plans = None
     with forced(bn):
         hit0, _ = ctx.forced_plan_counts()
-        if capfd is None:
-            wide, names = gc._kernels_launched(run)
+        if log:
+            (wide, names), plans = _with_plan_lines(lambda: gc._kernels_launched(run))
         else:
-            (wide, names), plans = _with_plan_lines(capfd, lambda: gc._kernels_launched(run))
+            wide, names = gc._kernels_launched(run)
         hit1, _ = ctx.forced_plan_counts()
         again = [run() for _ in range(repeats - 1)]
     assert hit1 > hit0, f"{what}: the forced bn={bn} plan was not taken"
@@ -69,8 +63,8 @@ def _wide_vs_narrow(ctx, run, bn, what, seen, capfd=None, repeats=1):
     return wide, diff, plans
 
 
-def _case(ctx, run, bn, what, exact, absum, seen, capfd=None, repeats=1, extra_abs=0.0):
-    got, diff, plans = _wide_vs_narrow(ctx, run, bn, what, seen, capfd, repeats)
+def _case(ctx, run, bn, what, exact, absum, seen, log=False, repeats=1, extra_abs=0.0):
+    got, diff, plans = _wide_vs_narrow(ctx, run, bn, what, seen, log, repeats)
     worst = gc.assert_tf32_close(got, exact, absum, what, extra_abs=extra_abs)
     return dict(what=what, diff=diff, worst=worst, plans=plans)
 
@@ -197,7 +191,7 @@ def test_wide_tiles(rt, oracle, bn, tf32):
 
 @pytest.mark.parametrize("tf32", [True, False], ids=["tf32", "tf32x3"])
 @pytest.mark.parametrize("bn", [128, 256])
-def test_wide_tiles_persistent(rt, oracle, capfd, bn, tf32):
+def test_wide_tiles_persistent(rt, oracle, bn, tf32):
     """Persistent schedules: every launch has more work units than the device has SMs, so CTAs run several units in
     turn and carry the operand ring's stage and phases, the staging-buffer parity, the residual barrier phases, the
     residual prefetch of the next unit and the shared bias vector from one unit to the next.  The unit counts are read
@@ -206,7 +200,7 @@ def test_wide_tiles_persistent(rt, oracle, capfd, bn, tf32):
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     ctx = gc.new_ctx(rt, tf32=tf32)
     rows, seen = [], []
-    kw = dict(seen=seen, capfd=capfd)
+    kw = dict(seen=seen, log=True)
     with bound(tf32):
         # ragged last M tile; 17 K blocks, which neither ring size (4 or 6 stages) divides, so every unit starts at a
         # different stage and phase; three runs that must agree bit for bit
