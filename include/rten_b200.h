@@ -649,6 +649,51 @@ rten_status rten_b200_div(rten_ctx* ctx, const rten_tensor* a, const rten_tensor
  * A one-element exponent (any rank) maps the base: the output takes a's shape (the reference's map_in).  Mixed types
  * (the reference's i32 ^ f32) return RTEN_ERR_UNSUPPORTED_TYPE: that case is left out. */
 rten_status rten_b200_pow(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
+/* Where (src/ops/binary_elementwise.rs where_op): out = cond != 0 ? x : y, with cond, x and y broadcast together
+ * (numpy rules; RTEN_ERR_INCOMPATIBLE_SHAPES "Cannot broadcast inputs" otherwise).  cond is i32 (ONNX bool maps to
+ * i32), x and y are both f32 or both i32; the elements are copied as bits.  Any layouts: dense operands of the output's
+ * shape (a one-element operand is read once per thread) run one flat pass; strided windows and broadcasts run a pass over
+ * the output's rows.  An allocated output is contiguous; a given `out` may be any strided view (not aliasing an input). */
+rten_status rten_b200_where(rten_ctx* ctx, const rten_tensor* cond, const rten_tensor* x, const rten_tensor* y, rten_tensor* out);
+/* Equal, Less, LessOrEqual, Greater, GreaterOrEqual (binary_elementwise.rs boolean_op): i32 0 / 1 of a (op) b, a and b
+ * both f32 or both i32, broadcast as Where broadcasts.  f32 comparisons are IEEE: NaN compares false, -0 == +0, and
+ * subnormals are not flushed. */
+rten_status rten_b200_equal(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
+rten_status rten_b200_less(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
+rten_status rten_b200_less_or_equal(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
+rten_status rten_b200_greater(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
+rten_status rten_b200_greater_or_equal(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
+/* And, Or, Xor (logical_boolean_op) and Not (unary_elementwise.rs not): i32 inputs, nonzero is true, i32 0 / 1 out;
+ * the binary ones broadcast as Where broadcasts.  Other types: RTEN_ERR_UNSUPPORTED_TYPE. */
+rten_status rten_b200_and(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
+rten_status rten_b200_or(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
+rten_status rten_b200_xor(rten_ctx* ctx, const rten_tensor* a, const rten_tensor* b, rten_tensor* out);
+rten_status rten_b200_not(rten_ctx* ctx, const rten_tensor* x, rten_tensor* out);
+/* Trilu (src/ops/trilu.rs), f32 or i32, over every matrix of the last two dims: element (i, j) is kept when
+ * i + k - j <= 0 (upper != 0) or >= 0 (upper == 0), else 0.  x with fewer than 2 dims: RTEN_ERR_INVALID_VALUE "Input
+ * must have >= 2 dims".  x and out may be any strided views. */
+rten_status rten_b200_trilu(rten_ctx* ctx, const rten_tensor* x, int64_t k, int upper, rten_tensor* out);
+/* Expand (src/ops/layout.rs expand): x (f32 or i32) broadcast with the n-dim target `shape` (bidirectionally, numpy
+ * rules).  A negative target dim: RTEN_ERR_INVALID_VALUE "Target shape contains negative values"; shapes that do not
+ * broadcast: RTEN_ERR_INCOMPATIBLE_SHAPES "Cannot broadcast input with target shape".  A dense x broadcast over one run
+ * of adjacent dims into a dense output, with repeated rows of at least 128 elements (repeat_kv's [b, kv, 1, l, d] ->
+ * [b, kv, n, l, d], or a leading broadcast), runs the repeat kernel, 16 bytes per thread when the rows allow; anything
+ * else is a strided copy. */
+rten_status rten_b200_expand(rten_ctx* ctx, const rten_tensor* x, const int64_t* shape, int n, rten_tensor* out);
+/* Slice (src/ops/slice.rs) of a 4-byte-element x, copied into out: n entries of starts and ends, and of axes and steps
+ * when not NULL (axes default to 0 .. n - 1, steps to 1).  Ranges clamp as the reference's SliceRange::clamp, negative
+ * starts / ends count from the end.  Errors (RTEN_ERR_INVALID_VALUE): "`axes` length must be <= input rank", "`starts`
+ * length must match axis count", "steps must be non-zero", "Axis is invalid".  A negative step is
+ * RTEN_ERR_UNSUPPORTED_VALUE: the library's strides are non-negative. */
+rten_status rten_b200_slice(rten_ctx* ctx, const rten_tensor* x, const int32_t* starts, const int32_t* ends, const int32_t* axes,
+                            const int32_t* steps, int n, rten_tensor* out);
+/* Split (src/ops/split.rs) of a 4-byte-element x along `axis` into copies: by the n_split sizes of `split` when not NULL,
+ * else into num_outputs pieces of ceil(dim / num_outputs) (the last one shorter, and fewer pieces when they run out).
+ * outs has room for n_outs tensors; *n_pieces gets the number written.  Errors (RTEN_ERR_INVALID_VALUE): "Split sizes
+ * must be >= 0", "Split sizes do not sum to dimension size", "num_outputs must be > 0", "num_outputs exceeds dim
+ * size", "Axis is invalid", and more pieces than n_outs.  On an error every output the call allocated is freed. */
+rten_status rten_b200_split(rten_ctx* ctx, const rten_tensor* x, int axis, const int32_t* split, int n_split, int num_outputs,
+                            rten_tensor* outs, int n_outs, int32_t* n_pieces);
 /* ReduceSum (src/ops/reduce.rs), f32 or i32, one launch.  `axes` (n_axes values in [-ndim, ndim - 1], duplicates
  * allowed) are the reduced axes; n_axes = 0 reduces every axis.  keep_dims != 0 keeps them as size-1 axes.  Each f32
  * output is the reference's Sum (the 64-chain fold of rten-vecmath/src/sum.rs) of its elements taken in row-major order

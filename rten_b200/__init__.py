@@ -10,3 +10,6 @@ from .ops import (  # noqa: F401
     LayerNormalization, LSTM, MatMul, MatMulInteger, MatMulIntegerToFloat, MatMulNBits, MaxPool, Mul, MultiHeadAttention, Neg, OpError, Packed, Pow, QuantizedLinear, Reciprocal, ReduceMean, ReduceSum, Relu, Resize, RMSNormalization, RotaryEmbedding, ScatterRows, Sigmoid,
     SimplifiedLayerNormalization, Silu, SkipLayerNormalization, SkipSimplifiedLayerNormalization, Softmax, Sqrt, Sub, Tanh, TopK, Upsample, from_torch,
 )
+from .ops import (  # noqa: F401
+    And, Equal, Expand, Greater, GreaterOrEqual, Less, LessOrEqual, Not, Or, Slice, Split, Trilu, Where, Xor,
+)

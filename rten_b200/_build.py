@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "librten_b200.so")
-SOURCES = ["umma_gemm.cu", "umma_halo.cu", "rowops.cu", "groupnorm.cu", "reduce.cu", "topk.cu", "depthwise.cu", "resize.cu", "skinny.cu", "attn_fused.cu", "attn_prefill.cu", "nbits.cu", "rotary.cu", "rnn.cu", "api_core.cu", "api_ops.cu", "api_conv.cu", "api_rows.cu", "api_fused.cu", "api_attention.cu", "api_rnn.cu", "onnx_reader.cu", "model.cu", "comm.cu"]
+SOURCES = ["umma_gemm.cu", "umma_halo.cu", "rowops.cu", "groupnorm.cu", "reduce.cu", "topk.cu", "depthwise.cu", "resize.cu", "skinny.cu", "attn_fused.cu", "attn_prefill.cu", "nbits.cu", "rotary.cu", "rnn.cu", "masks.cu", "api_core.cu", "api_ops.cu", "api_conv.cu", "api_rows.cu", "api_fused.cu", "api_attention.cu", "api_rnn.cu", "api_masks.cu", "onnx_reader.cu", "model.cu", "comm.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--cudart", "static",

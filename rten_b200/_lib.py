@@ -174,6 +174,21 @@ _SIGNATURES = {
     "rten_b200_tanh": (C.c_int, [_vp, _TP, _TP]),
     "rten_b200_neg": (C.c_int, [_vp, _TP, _TP]),
     "rten_b200_abs": (C.c_int, [_vp, _TP, _TP]),
+    "rten_b200_where": (C.c_int, [_vp, _TP, _TP, _TP, _TP]),
+    "rten_b200_equal": (C.c_int, [_vp, _TP, _TP, _TP]),
+    "rten_b200_less": (C.c_int, [_vp, _TP, _TP, _TP]),
+    "rten_b200_less_or_equal": (C.c_int, [_vp, _TP, _TP, _TP]),
+    "rten_b200_greater": (C.c_int, [_vp, _TP, _TP, _TP]),
+    "rten_b200_greater_or_equal": (C.c_int, [_vp, _TP, _TP, _TP]),
+    "rten_b200_and": (C.c_int, [_vp, _TP, _TP, _TP]),
+    "rten_b200_or": (C.c_int, [_vp, _TP, _TP, _TP]),
+    "rten_b200_xor": (C.c_int, [_vp, _TP, _TP, _TP]),
+    "rten_b200_not": (C.c_int, [_vp, _TP, _TP]),
+    "rten_b200_trilu": (C.c_int, [_vp, _TP, C.c_int64, C.c_int, _TP]),
+    "rten_b200_expand": (C.c_int, [_vp, _TP, C.POINTER(C.c_int64), C.c_int, _TP]),
+    "rten_b200_slice": (C.c_int, [_vp, _TP, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                  C.c_int, _TP]),
+    "rten_b200_split": (C.c_int, [_vp, _TP, C.c_int, C.POINTER(C.c_int32), C.c_int, C.c_int, _TP, C.c_int, C.POINTER(C.c_int32)]),
     "rten_b200_reduce_sum": (C.c_int, [_vp, _TP, C.POINTER(C.c_int32), C.c_int, C.c_int, _TP]),
     "rten_b200_reduce_mean": (C.c_int, [_vp, _TP, C.POINTER(C.c_int32), C.c_int, C.c_int, _TP]),
     "rten_b200_topk": (C.c_int, [_vp, _TP, C.c_int64, C.c_int, C.c_int, C.c_int, _TP, _TP]),

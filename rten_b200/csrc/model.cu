@@ -7,9 +7,11 @@
 //   run  : the nodes in topological (file) order, one C-ABI operator call each; temporaries are reference counted and
 //          returned to the context pool after their last consumer (src/graph.rs:1100-1180); an operator that can run in
 //          place does so when the executor holds the last reference to its input (src/graph.rs:973-1049); shape-only
-//          operators (Reshape, Flatten, Squeeze, Unsqueeze, Transpose, Identity) are views -- no kernel, no copy.
+//          operators (Reshape, Flatten, Squeeze, Unsqueeze, Transpose, Identity) and Slice / Split are views -- no kernel,
+//          no copy.
 //          Shape-like values are computed on the host (Runner::set_host): Shape, a Gather of a host-known vector with
-//          host-known indices, an integer Cast and the order-keeping views of such values launch nothing, so a Reshape
+//          host-known indices, an integer Cast, the order-keeping views of such values, and Add / Sub / Mul / Div, the
+//          comparisons, Where, Concat and Slice of host-known inputs, i32 Range and integer ConstantOfShape launch nothing, so a Reshape
 //          target or the total_sequence_length of onnxruntime-genai's attention-mask subgraph is known without a copy
 //          back; an operator that takes one as a tensor gets a host tensor (GroupQueryAttention reads it in place).
 //          A Concat over the channels of NCHW tensors is written in place by its producers where the load found that
@@ -32,6 +34,7 @@
 
 #include "api_shared.h"
 #include "api_util.h"
+#include "masks.h"
 #include "onnx_reader.h"
 #include "rowops.h"
 
@@ -953,6 +956,355 @@ bool host_gather(Runner& r, OpNode& o, rten_status* st) {
     return true;
 }
 
+// ---- host values: shape arithmetic (the reference's i32 semantics)
+// A host-known value's elements as the reference holds them: i32, an int64 constant saturated as the loader does
+std::vector<int64_t> host_i32(const ValueSlot& v) {
+    std::vector<int64_t> r(v.host_ints.size());
+    for (size_t i = 0; i < r.size(); i++) r[i] = std::max<int64_t>(INT32_MIN, std::min<int64_t>(INT32_MAX, v.host_ints[i]));
+    return r;
+}
+
+bool all_host(Runner& r, const OpNode& o, size_t n) {
+    for (size_t i = 0; i < n; i++)
+        if (i >= o.in.size() || o.in[i] < 0 || !r.V(o.in[i]).has_host_ints) return false;
+    return true;
+}
+
+// The first n inputs of o, all host-known, broadcast together (numpy rules): `shape` and each input's elements at every
+// output position
+rten_status host_broadcast(Runner& r, const OpNode& o, size_t n, std::vector<int64_t>* shape, std::vector<std::vector<int64_t>>* vals) {
+    int nd = 0;
+    for (size_t i = 0; i < n; i++) nd = std::max(nd, r.V(o.in[i]).t.ndim);
+    shape->assign((size_t)nd, 1);
+    for (size_t i = 0; i < n; i++) {
+        const rten_tensor& t = r.V(o.in[i]).t;
+        for (int k = 0; k < t.ndim; k++) {
+            int64_t& d = (*shape)[(size_t)(k + nd - t.ndim)];
+            if (t.shape[k] != 1) {
+                if (d != 1 && d != t.shape[k]) return mfail(r.ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "Cannot broadcast inputs");
+                d = t.shape[k];
+            }
+        }
+    }
+    int64_t total = 1;
+    for (int64_t d : *shape) total *= d;
+    vals->assign(n, std::vector<int64_t>((size_t)total));
+    for (size_t i = 0; i < n; i++) {
+        const ValueSlot& v = r.V(o.in[i]);
+        const std::vector<int64_t> src = host_i32(v);
+        for (int64_t e = 0; e < total; e++) {
+            int64_t rem = e, off = 0, st = 1;
+            for (int k = nd - 1; k >= 0; k--) {
+                const int64_t idx = rem % (*shape)[(size_t)k];
+                rem /= (*shape)[(size_t)k];
+                const int kk = k - (nd - v.t.ndim);
+                if (kk >= 0) {
+                    if (v.t.shape[kk] != 1) off += idx * st;
+                    st *= v.t.shape[kk];
+                }
+            }
+            (*vals)[i][(size_t)e] = src[(size_t)off];
+        }
+    }
+    return RTEN_OK;
+}
+
+// f over the broadcast host inputs of o as its host output.  false: an input is not host-known (the node runs on the
+// device).
+template <size_t N, class F>
+bool host_map(Runner& r, OpNode& o, rten_status* st, F f) {
+    if (!all_host(r, o, N)) return false;
+    std::vector<int64_t> shape;
+    std::vector<std::vector<int64_t>> v;
+    *st = host_broadcast(r, o, N, &shape, &v);
+    if (*st != RTEN_OK) return true;
+    std::vector<int64_t> out(v[0].size());
+    for (size_t e = 0; e < out.size(); e++) {
+        int64_t x[N];
+        for (size_t i = 0; i < N; i++) x[i] = v[i][e];
+        out[e] = f(x);
+    }
+    if (Runner::wants(o, 0)) r.set_host(o.out[0], out, (int)shape.size(), shape.data());
+    *st = RTEN_OK;
+    return true;
+}
+
+// Add / Sub / Mul wrap, Div truncates; a zero divisor (or INT_MIN / -1) fails as the device Div does
+template <int OP>
+bool host_arith(Runner& r, OpNode& o, rten_status* st) {
+    // Div: every divisor is checked before the broadcast, as the reference's check_nonzero does; INT_MIN / -1 where the
+    // two meet fails with the same message, as the device Div does
+    if (OP == BIN_DIV && all_host(r, o, 2)) {
+        bool bad = false;
+        for (int64_t d : host_i32(r.V(o.in[1]))) bad = bad || d == 0;
+        std::vector<int64_t> shape;
+        std::vector<std::vector<int64_t>> v;
+        if (!bad && host_broadcast(r, o, 2, &shape, &v) == RTEN_OK)
+            for (size_t e = 0; e < v[0].size(); e++) bad = bad || (v[0][e] == INT32_MIN && v[1][e] == -1);
+        if (bad) {
+            *st = mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "Divisor contains zero");
+            return true;
+        }
+    }
+    return host_map<2>(r, o, st, [](const int64_t* x) -> int64_t {
+        const uint32_t a = (uint32_t)x[0], b = (uint32_t)x[1];
+        if (OP == BIN_ADD) return (int32_t)(a + b);
+        if (OP == BIN_SUB) return (int32_t)(a - b);
+        if (OP == BIN_MUL) return (int32_t)(a * b);
+        return (int32_t)(x[0] / x[1]);  // (no zero divisor, no INT_MIN / -1: refused above)
+    });
+}
+
+template <int OP>
+bool host_compare(Runner& r, OpNode& o, rten_status* st) {
+    return host_map<2>(r, o, st, [](const int64_t* x) -> int64_t {
+        switch (OP) {
+            case CMP_EQ: return x[0] == x[1];
+            case CMP_LT: return x[0] < x[1];
+            case CMP_LE: return x[0] <= x[1];
+            case CMP_GT: return x[0] > x[1];
+            default: return x[0] >= x[1];
+        }
+    });
+}
+
+template <int OP>
+rten_status run_compare(Runner& r, OpNode& o, rten_tensor* y) {
+    rten_status st;
+    if (host_compare<OP>(r, o, &st)) return st;
+    auto fn = OP == CMP_EQ ? rten_b200_equal : OP == CMP_LT ? rten_b200_less : OP == CMP_LE ? rten_b200_less_or_equal
+            : OP == CMP_GT ? rten_b200_greater : rten_b200_greater_or_equal;
+    return fn(r.ctx, r.T(o, 0), r.T(o, 1), y);
+}
+
+// Concat on axis 0 of 1-D host values: a host value
+bool host_concat(Runner& r, OpNode& o, rten_status* st) {
+    if (o.in.empty() || !all_host(r, o, o.in.size())) return false;
+    for (int i : o.in)
+        if (r.V(i).t.ndim != 1) return false;
+    if (o.n.attr_i("axis", 0) != 0 && o.n.attr_i("axis", 0) != -1) return false;
+    std::vector<int64_t> out;
+    for (int i : o.in) {
+        const std::vector<int64_t> v = host_i32(r.V(i));
+        out.insert(out.end(), v.begin(), v.end());
+    }
+    const int64_t n = (int64_t)out.size();
+    if (Runner::wants(o, 0)) r.set_host(o.out[0], out, 1, &n);
+    *st = RTEN_OK;
+    return true;
+}
+
+// an i32 list input (host-known, saturated) or attribute `attr`; `present` false when neither is given
+rten_status int_list(Runner& r, const OpNode& o, size_t slot, const char* attr, std::vector<int32_t>* v, bool* present) {
+    v->clear();
+    *present = false;
+    if (slot < o.in.size() && o.in[slot] >= 0) {
+        if (!r.V(o.in[slot]).has_host_ints)
+            return mfail(r.ctx, RTEN_ERR_UNSUPPORTED_VALUE, o.n.op_type + ": input " + std::to_string(slot) + " must be known on the host");
+        for (int64_t x : host_i32(r.V(o.in[slot]))) v->push_back((int32_t)x);
+        *present = true;
+    } else if (attr && o.n.attr(attr)) {
+        for (int64_t x : o.n.attr_ints(attr)) v->push_back((int32_t)std::max<int64_t>(INT32_MIN, std::min<int64_t>(INT32_MAX, x)));
+        *present = true;
+    }
+    return RTEN_OK;
+}
+
+// Slice (src/ops/slice.rs): a strided view of x (strides times the steps, an offset), no copy; of a 1-D host value, a
+// host value.  Starts / ends / axes / steps are inputs (opset >= 10) or attributes (earlier), known on the host.
+rten_status run_slice(Runner& r, OpNode& o, rten_tensor*) {
+    const rten_tensor* x = r.T(o, 0);
+    std::vector<int32_t> s, e, a, st;
+    bool hs, he, ha, hst;
+    RTB_TRY(int_list(r, o, 1, "starts", &s, &hs));
+    RTB_TRY(int_list(r, o, 2, "ends", &e, &he));
+    RTB_TRY(int_list(r, o, 3, "axes", &a, &ha));
+    RTB_TRY(int_list(r, o, 4, nullptr, &st, &hst));
+    if (!hs || !he) return mfail(r.ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    int64_t b[RTEN_MAX_DIMS], len[RTEN_MAX_DIMS], step[RTEN_MAX_DIMS];
+    RTB_TRY(slice_ranges(r.ctx, x->ndim, x->shape, s.data(), (int)s.size(), e.data(), (int)e.size(), ha ? a.data() : nullptr, (int)a.size(),
+                         hst ? st.data() : nullptr, (int)st.size(), b, len, step));
+    if (!Runner::wants(o, 0)) return RTEN_OK;
+    const ValueSlot& xv = r.V(o.in[0]);
+    if (xv.has_host_ints && x->ndim == 1) {
+        std::vector<int64_t> out;
+        const std::vector<int64_t> src = host_i32(xv);
+        for (int64_t i = 0; i < len[0]; i++) out.push_back(src[(size_t)(b[0] + i * step[0])]);
+        r.set_host(o.out[0], out, 1, &len[0]);
+        return RTEN_OK;
+    }
+    rten_tensor v = *x;
+    for (int i = 0; i < x->ndim; i++) {
+        if (len[i] > 0) v.data = (char*)v.data + b[i] * x->strides[i] * dtype_size(x->dtype);
+        v.shape[i] = len[i];
+        v.strides[i] = x->strides[i] * step[i];
+    }
+    r.set_view(o.out[0], v, o.in[0]);
+    return RTEN_OK;
+}
+
+// Split (src/ops/split.rs): every output a view of its piece of x, no copy.  The sizes are input 1 (opset >= 13), the
+// `split` attribute (earlier), else num_outputs (opset 18) or the node's output count pieces of ceil(n / k).
+rten_status run_split(Runner& r, OpNode& o, rten_tensor*) {
+    const rten_tensor* x = r.T(o, 0);
+    const int64_t axis0 = o.n.attr_i("axis", 0), axis = axis0 < 0 ? axis0 + x->ndim : axis0;
+    if (axis < 0 || axis >= x->ndim) return mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "Axis is invalid");
+    std::vector<int32_t> sizes;
+    bool given;
+    RTB_TRY(int_list(r, o, 1, "split", &sizes, &given));
+    const int64_t k = o.n.attr("num_outputs") ? o.n.attr_i("num_outputs", 0) : (int64_t)o.out.size();
+    std::vector<int64_t> pieces;
+    RTB_TRY(split_pieces(r.ctx, x->shape[axis], given ? sizes.data() : nullptr, (int)sizes.size(), k, &pieces));
+    // (an output without a piece would be read unset; a piece without an output would be dropped)
+    if (pieces.size() / 2 != o.out.size())
+        return mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "Split: " + std::to_string(pieces.size() / 2) + " pieces for " +
+                                                        std::to_string(o.out.size()) + " outputs");
+    for (size_t i = 0; i < o.out.size(); i++) {
+        if (!Runner::wants(o, i)) continue;
+        rten_tensor v = *x;
+        v.shape[axis] = pieces[2 * i + 1];
+        if (v.shape[axis] > 0) v.data = (char*)v.data + pieces[2 * i] * x->strides[axis] * dtype_size(x->dtype);
+        r.set_view(o.out[i], v, o.in[0]);
+    }
+    return RTEN_OK;
+}
+
+// one element of a Range input: host-known, else read back (a synchronisation)
+rten_status range_scalar(Runner& r, int id, bool as_float, double* out) {
+    const ValueSlot& v = r.V(id);
+    if (numel(&v.t) != 1) return mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "`start` must be a scalar");
+    if (v.has_host_ints) *out = (double)host_i32(v)[0];
+    else if (v.has_host_floats) *out = v.host_floats[0];
+    else {
+        uint32_t bits = 0;
+        RTB_CUDA(r.ctx, cudaMemcpyAsync(&bits, v.t.data, 4, v.t.device < 0 ? cudaMemcpyHostToHost : cudaMemcpyDeviceToHost, r.ctx->stream));
+        RTB_CUDA(r.ctx, cudaStreamSynchronize(r.ctx->stream));
+        float f;
+        int32_t i;
+        memcpy(&f, &bits, 4);
+        memcpy(&i, &bits, 4);
+        *out = as_float ? (double)f : (double)i;
+    }
+    return RTEN_OK;
+}
+
+// Range (src/ops/generate.rs range): i32 gives a host value; f32 is computed on the host by the reference's serial
+// `val = val + delta` in f32 and uploaded once
+rten_status run_range(Runner& r, OpNode& o, rten_tensor* y) {
+    const int dt = r.T(o, 0)->dtype;
+    if (dt != RTEN_F32 && dt != RTEN_I32) return mfail(r.ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    double s, l, d;
+    RTB_TRY(range_scalar(r, o.in[0], dt == RTEN_F32, &s));
+    RTB_TRY(range_scalar(r, o.in[1], dt == RTEN_F32, &l));
+    RTB_TRY(range_scalar(r, o.in[2], dt == RTEN_F32, &d));
+    if (dt == RTEN_I32) {
+        const int32_t limit = (int32_t)l, delta = (int32_t)d;
+        if (delta == 0) return mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "delta must be non-zero");
+        std::vector<int64_t> out;
+        for (int64_t v = (int32_t)s; (delta > 0 && v < limit) || (delta < 0 && v > limit); v += delta) out.push_back(v);
+        const int64_t n = (int64_t)out.size();
+        if (Runner::wants(o, 0)) r.set_host(o.out[0], out, 1, &n);
+        return RTEN_OK;
+    }
+    const float limit = (float)l, delta = (float)d;
+    if (delta == 0.0f) return mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "delta must be non-zero");
+    std::vector<float> out;
+    for (float v = (float)s; (delta > 0.0f && v < limit) || (delta < 0.0f && v > limit); v = v + delta) out.push_back(v);
+    rten_tensor t{};
+    t.dtype = RTEN_F32;
+    t.ndim = 1;
+    t.shape[0] = (int64_t)out.size();
+    set_contiguous(&t);
+    t.device = r.ctx->device;
+    RTB_TRY(pool_alloc(r.ctx, std::max<size_t>(out.size(), 1) * 4, &t.data));
+    if (!out.empty()) {
+        cudaError_t e = cudaMemcpyAsync(t.data, out.data(), out.size() * 4, cudaMemcpyHostToDevice, r.ctx->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(r.ctx->stream);  // (`out` goes away)
+        if (e != cudaSuccess) {
+            pool_free(r.ctx, t.data);
+            return fail_cuda(r.ctx, e, "Range upload");
+        }
+    }
+    *y = t;
+    return RTEN_OK;
+}
+
+// ConstantOfShape (src/ops/generate.rs): the `value` attribute's one element (default f32 0) over the host-known shape;
+// an integer fill is a host value, an f32 one a device fill
+rten_status run_constant_of_shape(Runner& r, OpNode& o, rten_tensor* y) {
+    std::vector<int32_t> dims;
+    bool given;
+    RTB_TRY(int_list(r, o, 0, nullptr, &dims, &given));
+    std::vector<int64_t> shape;
+    int64_t n = 1;
+    for (int32_t d : dims) {
+        if (d < 0) return mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "Invalid shape");
+        shape.push_back(d);
+        n *= d;
+    }
+    if ((int)shape.size() > RTEN_MAX_DIMS) return mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "tensor rank out of range");
+    const onnx::Attribute* a = o.n.attr("value");
+    int32_t type = onnx::DT_FLOAT;
+    uint32_t bits = 0;
+    if (a && a->has_t) {
+        const onnx::Tensor& t = a->t;
+        if (t.numel() != 1) return mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "ConstantOfShape: value must have one element");
+        type = t.data_type;
+        if (type == onnx::DT_INT64) {
+            int64_t v;
+            memcpy(&v, t.data.data(), 8);
+            bits = (uint32_t)(int32_t)std::max<int64_t>(INT32_MIN, std::min<int64_t>(INT32_MAX, v));
+        } else if (type == onnx::DT_INT32 || type == onnx::DT_FLOAT) {
+            memcpy(&bits, t.data.data(), 4);
+        } else if (type == onnx::DT_BOOL) {
+            bits = t.data[0] ? 1 : 0;
+        } else {
+            return mfail(r.ctx, RTEN_ERR_UNSUPPORTED_TYPE, "ConstantOfShape: unsupported value type");
+        }
+    }
+    if (type != onnx::DT_FLOAT) {
+        if (Runner::wants(o, 0)) r.set_host(o.out[0], std::vector<int64_t>((size_t)n, (int64_t)(int32_t)bits), (int)shape.size(), shape.data());
+        return RTEN_OK;
+    }
+    rten_tensor t{};
+    t.dtype = RTEN_F32;
+    t.ndim = (int)shape.size();
+    for (int i = 0; i < t.ndim; i++) t.shape[i] = shape[(size_t)i];
+    set_contiguous(&t);
+    t.device = r.ctx->device;
+    RTB_TRY(pool_alloc(r.ctx, (size_t)std::max<int64_t>(n, 1) * 4, &t.data));
+    const rten_status st = launch_fill(r.ctx, t.data, bits, n);
+    if (st != RTEN_OK) {
+        pool_free(r.ctx, t.data);
+        return st;
+    }
+    *y = t;
+    return RTEN_OK;
+}
+
+// Where: of host-known inputs a host value, else on the device
+rten_status run_where(Runner& r, OpNode& o, rten_tensor* y) {
+    rten_status st;
+    if (host_map<3>(r, o, &st, [](const int64_t* x) { return x[0] != 0 ? x[1] : x[2]; })) return st;
+    return rten_b200_where(r.ctx, r.T(o, 0), r.T(o, 1), r.T(o, 2), y);
+}
+
+rten_status run_expand(Runner& r, OpNode& o, rten_tensor* y) {
+    std::vector<int32_t> dims;
+    bool given;
+    RTB_TRY(int_list(r, o, 1, nullptr, &dims, &given));
+    const std::vector<int64_t> shape(dims.begin(), dims.end());
+    return rten_b200_expand(r.ctx, r.T(o, 0), shape.data(), (int)shape.size(), y);
+}
+
+rten_status run_trilu(Runner& r, OpNode& o, rten_tensor* y) {
+    std::vector<int32_t> k;
+    bool given;
+    RTB_TRY(int_list(r, o, 1, nullptr, &k, &given));
+    if (given && k.size() != 1) return mfail(r.ctx, RTEN_ERR_INVALID_VALUE, "k must be a scalar");
+    return rten_b200_trilu(r.ctx, r.T(o, 0), given ? k[0] : 0, (int)o.n.attr_i("upper", 1), y);
+}
+
 constexpr OpDef OPS[] = {
     {"Conv", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
          rten_conv_params p;
@@ -1038,6 +1390,8 @@ constexpr OpDef OPS[] = {
          return attr_to_input(m, n, "scales", 1, "upsample_scales", false);
      }, nullptr, resize_shape<true>},
     {"Concat", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
+         rten_status st;
+         if (host_concat(r, o, &st)) return st;
          std::vector<const rten_tensor*> ins;
          for (size_t i = 0; i < o.in.size(); i++)
              if (r.T(o, i)) ins.push_back(r.T(o, i));
@@ -1145,10 +1499,26 @@ constexpr OpDef OPS[] = {
          if (!n.attr("block_size")) return mfail(m->ctx, RTEN_ERR_UNSUPPORTED_VALUE, "MatMulNBits: missing attribute block_size");
          return RTEN_OK;
      }},
-    {"Add", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_add(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
-    {"Sub", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_sub(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
-    {"Mul", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_mul(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
-    {"Div", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_div(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
+    {"Add", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) {
+         rten_status st;
+         if (host_arith<BIN_ADD>(r, o, &st)) return st;
+         return rten_b200_add(r.ctx, r.T(o, 0), r.T(o, 1), y);
+     }},
+    {"Sub", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) {
+         rten_status st;
+         if (host_arith<BIN_SUB>(r, o, &st)) return st;
+         return rten_b200_sub(r.ctx, r.T(o, 0), r.T(o, 1), y);
+     }},
+    {"Mul", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) {
+         rten_status st;
+         if (host_arith<BIN_MUL>(r, o, &st)) return st;
+         return rten_b200_mul(r.ctx, r.T(o, 0), r.T(o, 1), y);
+     }},
+    {"Div", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) {
+         rten_status st;
+         if (host_arith<BIN_DIV>(r, o, &st)) return st;
+         return rten_b200_div(r.ctx, r.T(o, 0), r.T(o, 1), y);
+     }},
     {"Pow", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_pow(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
     {"LayerNormalization", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
          return rten_b200_layer_norm(r.ctx, r.T(o, 0), r.T(o, 1), r.T(o, 2), (int)o.n.attr_i("axis", -1), o.n.attr_f("epsilon", 1e-5f), y); }},
@@ -1169,7 +1539,7 @@ constexpr OpDef OPS[] = {
     {"Cast", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
          const int64_t to = o.n.attr_i("to", 0);
          const rten_tensor* x = r.T(o, 0);
-         const bool to_int = to == onnx::DT_INT32 || to == onnx::DT_INT64;
+         const bool to_int = to == onnx::DT_INT32 || to == onnx::DT_INT64 || to == onnx::DT_BOOL;  // (bool is i32)
          if ((to == onnx::DT_FLOAT && x->dtype == RTEN_F32) || (to_int && x->dtype == RTEN_I32)) {
              r.set_view(o.out[0], *x, o.in[0]);
              if (to_int && r.V(o.in[0]).has_host_ints) {  // (stays host-known)
@@ -1304,6 +1674,22 @@ constexpr OpDef OPS[] = {
          r.set_output(o, 2, c);
          return RTEN_OK;
      }, [](rten_model* m, onnx::Node& n) { return check_rnn_attrs(m->ctx, n, false); }, prepack_rnn},
+    {"Where", ONNX, 0, 0b111, run_where},
+    {"Equal", ONNX, 0, 0b11, run_compare<CMP_EQ>},
+    {"Less", ONNX, 0, 0b11, run_compare<CMP_LT>},
+    {"LessOrEqual", ONNX, 0, 0b11, run_compare<CMP_LE>},
+    {"Greater", ONNX, 0, 0b11, run_compare<CMP_GT>},
+    {"GreaterOrEqual", ONNX, 0, 0b11, run_compare<CMP_GE>},
+    {"And", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_and(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
+    {"Or", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_or(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
+    {"Xor", ONNX, 0, 0b11, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_xor(r.ctx, r.T(o, 0), r.T(o, 1), y); }},
+    {"Not", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) { return rten_b200_not(r.ctx, r.T(o, 0), y); }},
+    {"Expand", ONNX, 0, 0b11, run_expand},
+    {"Slice", ONNX, 0, 0b1, run_slice},
+    {"Split", ONNX, 0, 0b1, run_split},
+    {"Range", ONNX, 0, 0b111, run_range},
+    {"ConstantOfShape", ONNX, 0, 0b1, run_constant_of_shape},
+    {"Trilu", ONNX, 0, 0b1, run_trilu},
     {"Constant", ONNX, 0, 0b1, nullptr},  // (becomes a constant value at load, not a node)
 };
 

@@ -1101,6 +1101,127 @@ class Pow:
         return A.wrap(o, out)
 
 
+class Where:
+    """src/ops/binary_elementwise.rs where_op: cond (i32, nonzero is true) ? x : y, the three broadcast together; x and y
+    both f32 or both i32."""
+
+    def run(self, ctx, cond, x, y, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        ctx.check(ctx.lib.rten_b200_where(ctx.handle, A.t(cond), A.t(x), A.t(y), C.byref(o)))
+        return A.wrap(o, out)
+
+
+class _Compare:
+    """binary_elementwise.rs boolean_op / logical_boolean_op: i32 0 / 1 of a (op) b, broadcasting.  The comparisons take
+    f32 or i32 (IEEE: NaN compares false, -0 == +0), the logical operators i32 with nonzero as true."""
+    _fn = ""
+
+    def run(self, ctx, a, b, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        ctx.check(getattr(ctx.lib, self._fn)(ctx.handle, A.t(a), A.t(b), C.byref(o)))
+        return A.wrap(o, out)
+
+
+class Equal(_Compare):
+    _fn = "rten_b200_equal"
+
+
+class Less(_Compare):
+    _fn = "rten_b200_less"
+
+
+class LessOrEqual(_Compare):
+    _fn = "rten_b200_less_or_equal"
+
+
+class Greater(_Compare):
+    _fn = "rten_b200_greater"
+
+
+class GreaterOrEqual(_Compare):
+    _fn = "rten_b200_greater_or_equal"
+
+
+class And(_Compare):
+    _fn = "rten_b200_and"
+
+
+class Or(_Compare):
+    _fn = "rten_b200_or"
+
+
+class Xor(_Compare):
+    _fn = "rten_b200_xor"
+
+
+class Not:
+    """src/ops/unary_elementwise.rs not: i32 1 where x == 0, else 0."""
+
+    def run(self, ctx, x, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        ctx.check(ctx.lib.rten_b200_not(ctx.handle, A.t(x), C.byref(o)))
+        return A.wrap(o, out)
+
+
+class Trilu:
+    """src/ops/trilu.rs: the upper (or lower) triangle of every matrix over the last two dims, shifted by k; f32 or i32."""
+
+    def __init__(self, upper: bool = True):
+        self.upper = bool(upper)
+
+    def run(self, ctx, x, k: int = 0, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        ctx.check(ctx.lib.rten_b200_trilu(ctx.handle, A.t(x), int(k), int(self.upper), C.byref(o)))
+        return A.wrap(o, out)
+
+
+def _ints(ctype, v):
+    return None if v is None else (ctype * max(len(v), 1))(*[int(i) for i in v])
+
+
+class Expand:
+    """src/ops/layout.rs expand: x (f32 or i32) broadcast bidirectionally with the target `shape`."""
+
+    def run(self, ctx, x, shape, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        ctx.check(ctx.lib.rten_b200_expand(ctx.handle, A.t(x), _ints(C.c_int64, shape), len(shape), C.byref(o)))
+        return A.wrap(o, out)
+
+
+class Slice:
+    """src/ops/slice.rs slice, copied: starts / ends (and axes, steps when given) of equal length; positive steps only."""
+
+    def run(self, ctx, x, starts, ends, axes=None, steps=None, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        ctx.check(ctx.lib.rten_b200_slice(ctx.handle, A.t(x), _ints(C.c_int32, starts), _ints(C.c_int32, ends), _ints(C.c_int32, axes),
+                                          _ints(C.c_int32, steps), len(starts), C.byref(o)))
+        return A.wrap(o, out)
+
+
+class Split:
+    """src/ops/split.rs split, copied: by `split` sizes when given, else into num_outputs pieces of ceil(n / k)."""
+
+    def __init__(self, axis: int = 0, num_outputs: Optional[int] = None):
+        self.axis, self.num_outputs = int(axis), num_outputs
+
+    def run(self, ctx, x, split=None, num_outputs: Optional[int] = None):
+        A = _Args(ctx)
+        k = num_outputs if num_outputs is not None else self.num_outputs
+        cap = len(split) if split is not None else int(k or 0)
+        outs = (RtenTensor * max(cap, 1))()
+        A.keep.append(outs)
+        n = C.c_int32(0)
+        ctx.check(ctx.lib.rten_b200_split(ctx.handle, A.t(x), self.axis, _ints(C.c_int32, split), len(split) if split is not None else 0,
+                                          int(k or 0), outs, cap, C.byref(n)))
+        return [A.wrap(outs[i], None) for i in range(n.value)]
+
+
 TOPK_MAX_K = 2048  # the largest k rten_b200_topk takes (RTEN_ERR_UNSUPPORTED_VALUE above)
 
 
