@@ -1348,13 +1348,19 @@ def check_skinny_f32(rt, oracle):
 
 def _kernels_launched(fn):
     """Run `fn` under CUPTI (torch.profiler) and return the names of the CUDA kernels it launched: lets a check insist
-    that a specialised kernel ran instead of a fall-back path that would meet the same tolerances."""
+    that a specialised kernel ran instead of a fall-back path that would meet the same tolerances.  Kineto keeps only
+    the activity records whose timestamps, converted from the GPU clock, fall inside the capture window; the kernels of
+    a short call (an ArgMax over a few hundred rows) can end microseconds before the window closes and be dropped, so
+    the window is held open a few milliseconds on both sides of the call (as test_gpu_row_kernels._capture does)."""
+    import time
     import torch
     from torch.profiler import ProfilerActivity, profile
     torch.cuda.init()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        time.sleep(0.005)
         out = fn()
         torch.cuda.synchronize()
+        time.sleep(0.005)
     names = {e.name for e in prof.events()}
     return out, names
 

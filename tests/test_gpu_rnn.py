@@ -375,3 +375,5 @@ def test_kernel_identity():
     for key in ("gru256", "lstm256"):
         assert has(key, "rnn_cluster_kernel") and not has(key, "rnn_step_gates_kernel"), names[key]
     assert has("lstm1024", "rnn_step_gates_kernel") and not has("lstm1024", "rnn_cluster_kernel"), names["lstm1024"]
+    # the per-step path sets its state buffers from h0 / c0 (or zeros) first
+    assert has("lstm1024", "rnn_state_init_kernel") and not has("lstm256", "rnn_state_init_kernel"), names["lstm1024"]

@@ -18,6 +18,7 @@ def test_sharded_int8_resnet50_bit_exact():
     out = subprocess.run(cmd, cwd=ROOT, capture_output=True, text=True, timeout=600)
     assert out.returncode == 0, out.stdout[-2000:] + out.stderr[-2000:]
     assert "bit-identical to the unsharded oracle: True" in out.stdout
-    # both forms of the exchange are exact: the NVLink peer-mailbox kernel (default) and the NCCL fallback
+    # both forms of the exchange are exact: the NVLink peer-mailbox kernel (peer_minmax_kernel, the default) and the NCCL
+    # fallback
     assert "NCCL fallback bit-identical: True" in out.stdout and "(timeouts 0)" in out.stdout, out.stdout[-1500:]
     print(out.stdout[-600:])

@@ -5,8 +5,8 @@ empty-phase fill), each selected by name and checked bit for bit.
 
 The launchers pick a kernel at run time from shapes, strides, pointer alignment and the f32 mode.  The rules are
 restated below (`*_rule`); `VARIANTS` lists every instance they pick from (tests/test_staging_kernel_table_cpu.py keeps it
-equal to the built library's symbols, and checks that every kernel of rowops.cu is in this table or another by-name
-table).  `MODES` lists the runtime branches a name does not show.  The case lists reach every (kernel, mode) at least
+equal to the built library's symbols; tests/test_kernel_names_cpu.py checks that every kernel of the library is in this
+table or another by-name table).  `MODES` lists the runtime branches a name does not show.  The case lists reach every (kernel, mode) at least
 twice, once with a partial last unit (a block with idle threads, a warp-per-row block with idle rows or lanes, a scalar
 tail after the vector blocks).
 

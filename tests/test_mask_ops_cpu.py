@@ -9,7 +9,7 @@ import pytest
 import mask_ops as mo
 import test_gpu_mask_ops as gm
 from test_row_kernel_table_cpu import compiled_instances, lib_path  # noqa: F401  (lib_path: a fixture)
-from test_staging_kernel_table_cpu import global_kernels
+from test_kernel_names_cpu import library_kernels
 
 MASKS = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "rten_b200", "csrc", "masks.cu")
 
@@ -84,6 +84,6 @@ def test_kernel_table_matches_the_library(lib_path):  # noqa: F811
 
 
 def test_every_masks_kernel_is_in_the_table():
-    names = global_kernels(MASKS)
+    names = set(library_kernels([MASKS]))
     assert len(names) >= 6, sorted(names)
     assert names == set(gm.VARIANTS), (sorted(names - set(gm.VARIANTS)), sorted(set(gm.VARIANTS) - names))

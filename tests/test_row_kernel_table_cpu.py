@@ -21,15 +21,15 @@ def _cuda_tool(name):
     return os.path.join(os.path.dirname(_build._nvcc()), name)
 
 
-def compiled_instances(lib, kernels=None):
-    """{kernel: its compiled template argument tuples} over the kernels `kernel_key` accepts (`kernels`, default the
-    four families of tests/test_gpu_row_kernels.py)"""
+def compiled_instances(lib, kernels=None, key=None):
+    """{kernel: its compiled template argument tuples} over the kernels `key` (default rk.kernel_key) accepts
+    (`kernels`, default the four families of tests/test_gpu_row_kernels.py)"""
     syms = subprocess.run([_cuda_tool("cuobjdump"), "-symbols", lib], capture_output=True, text=True, check=True).stdout
     mangled = [ln.split()[-1] for ln in syms.splitlines() if "STT_FUNC" in ln]
     names = subprocess.run([_cuda_tool("cu++filt")], input="\n".join(mangled), capture_output=True, text=True, check=True).stdout
     found = {}
     for name in names.splitlines():
-        k = rk.kernel_key(name, kernels)
+        k = (key or rk.kernel_key)(name, kernels)
         if k is not None:
             found.setdefault(k[0], set()).add(k[1])
     return found
