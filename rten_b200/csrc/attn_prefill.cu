@@ -13,7 +13,9 @@
 //           reduced_range_exp(old max - new max); P = reduced_range_exp(z - max) -> shared memory as the A operand
 //       wgmma tf32: O += P V (3xTF32 as above) in registers
 //   O / row sum (NaN of a fully masked row flushed to 0) -> global.
-// Key tiles wholly above the causal diagonal or past the valid length are neither loaded nor multiplied; the launch
+// Key tiles wholly above the causal diagonal or past the valid length are neither loaded nor multiplied, and in the tile
+// that holds the last valid key the value rows past it are zeroed, so a NaN or inf left in a padded cache never reaches
+// the output (as in the decode kernel); the launch
 // depends on shapes only (valid lengths are read on the device), so the call can be captured in a CUDA graph.  No
 // atomics and no split over CTAs: every output element is written once, and repeated runs are bit-identical.
 #include <cuda.h>
@@ -216,7 +218,10 @@ __device__ __forceinline__ void attn_prefill_body(const CUtensorMap& tma_q, cons
         const uint8_t* tk = sk + s * C::KT;
         const uint8_t* tv = sv + s * C::VT;
         mbar_wait(&full[s], ((j - jlo) / NS) & 1);
-        if (X3 || p.v_natural) {
+        // keys [nv, BN) of the tile lie at or past the valid length (only in the tile of key lim - 1): their value rows
+        // are zeroed below, as a decode step never reads them -- P = 0 there, but 0 * NaN or 0 * inf would be NaN
+        const int nv = min(lim - j * BN, BN);
+        if (X3 || p.v_natural || nv < BN) {
             // every warp's products of the previous tile have completed before its operands are overwritten
             if (j > jlo) asm volatile("bar.sync 1, 128;" ::: "memory");
             if constexpr (X3) split_lo(sk_lo, tk, C::KT, tid);
@@ -224,7 +229,8 @@ __device__ __forceinline__ void attn_prefill_body(const CUtensorMap& tma_q, cons
                 // V tile (key row, d column) -> V^T tile (d row, key column); 32 lanes write 32 keys of one row of V^T
                 for (int i = tid; i < BN * DH / 4; i += 128) {
                     const int key = i % BN, d = 4 * (i / BN);
-                    const float4 x = *reinterpret_cast<const float4*>(tv + sw_off(key, d, BN));
+                    float4 x = *reinterpret_cast<const float4*>(tv + sw_off(key, d, BN));
+                    if (key >= nv) x = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
                     const float e[4] = {x.x, x.y, x.z, x.w};
 #pragma unroll
                     for (int q = 0; q < 4; q++) {
@@ -233,8 +239,17 @@ __device__ __forceinline__ void attn_prefill_body(const CUtensorMap& tma_q, cons
                     }
                 }
                 tv = svt;
-            } else if constexpr (X3) {
-                split_lo(sv_lo, tv, C::VT, tid);
+            } else {
+                if (nv < BN) {
+                    // the V^T tile's columns of keys past the valid length -> 0 (in the stage buffer: TMA rewrites it
+                    // only after this tile's products, and the proxy fence below orders these stores before them)
+                    for (int i = tid; i < BN * DH; i += 128) {
+                        const int key = i % BN, d = i / BN;
+                        if (key >= nv) *reinterpret_cast<float*>(sv + s * C::VT + sw_off(d, key, DH)) = 0.0f;
+                    }
+                    if constexpr (X3) asm volatile("bar.sync 1, 128;" ::: "memory");
+                }
+                if constexpr (X3) split_lo(sv_lo, tv, C::VT, tid);
             }
         }
         fence_proxy_async();  // the tensor core reads the bytes written above through the async proxy
