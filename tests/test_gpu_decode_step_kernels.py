@@ -659,9 +659,10 @@ def sms():
 
 
 # ---- kernel identity --------------------------------------------------------------------------------------------------
-def _launches(fn):
+def _launches(fn, smem=False):
     """[(name, grid, block)] of the kernels `fn` launches, from Kineto's trace (grid and block: x * y * z, None when the
-    trace does not record them); the capture window is held open around the call as rk._capture does"""
+    trace does not record them); with `smem`, [(name, grid, block, shared memory)], the shared memory Kineto records or
+    None.  The capture window is held open around the call as rk._capture does"""
     import time
     import torch
     from torch.profiler import ProfilerActivity, profile
@@ -682,7 +683,8 @@ def _launches(fn):
             continue
         a = e.get("args", {})
         g, b = a.get("grid"), a.get("block")
-        out.append((e["name"], int(np.prod(g)) if g else None, int(np.prod(b)) if b else None))
+        launch = (e["name"], int(np.prod(g)) if g else None, int(np.prod(b)) if b else None)
+        out.append(launch + (a.get("shared memory"),) if smem else launch)
     return out
 
 

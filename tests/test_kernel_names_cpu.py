@@ -1,12 +1,14 @@
 """CPU-only: every `__global__` kernel defined in rten_b200/csrc (*.cu and *.cuh) is in exactly one by-name table -- the
 row kernels, glue, elementwise math and operand staging of rowops.cu, TopK / arg-reduce, the mask kernels, the
 depthwise / GroupNorm / Resize / Concat / ReduceSum / rotary table, the single-query attention / MatMulNBits table,
-and the prefill attention table.  Each of those tables is kept equal to the compiled instances and checked kernel by
-kernel, bit for bit, by its GPU test.  A kernel added without a by-name test fails here before any GPU time is spent.
+the prefill attention table and the GRU / LSTM table.  Each of those tables is kept equal to the compiled instances and
+checked kernel by kernel, bit for bit, by its GPU test.  A kernel added without a by-name test fails here before any GPU
+time is spent.
 
 A few kernels are named only by their own operator's tests (`AD_HOC`: the wgmma GEMM and halo kernels, the encoder
-attention kernel, the RNN kernels and the multi-GPU range exchange).  For those this file checks only that the test module's source names the kernel -- a weaker guarantee than a table: nothing here proves the module
-asserts that the kernel ran, or covers every instance."""
+attention kernel and the multi-GPU range exchange).  For those this file checks only that the test module's source names
+the kernel -- a weaker guarantee than a table: nothing here proves the module asserts that the kernel ran, or covers
+every instance."""
 import glob
 import os
 import re
@@ -17,6 +19,7 @@ import test_gpu_elementwise_math as em
 import test_gpu_glue_kernels as gk
 import test_gpu_mask_ops as mo
 import test_gpu_prefill_attention_kernels as pk
+import test_gpu_rnn_kernels as nk
 import test_gpu_row_kernels as rk
 import test_gpu_select as sel
 import test_gpu_staging_kernels as sk
@@ -29,7 +32,6 @@ AD_HOC = {
     "umma_gemm_kernel": "test_gpu_epilogue_variants", "umma_wide_kernel": "test_gpu_wide_tiles",
     "umma_halo_kernel": "gpu_checks",
     "attn_fused_kernel": "test_gpu_attention_encoder",
-    "rnn_cluster_kernel": "test_gpu_rnn", "rnn_step_gates_kernel": "test_gpu_rnn", "rnn_state_init_kernel": "test_gpu_rnn",
     "peer_minmax_kernel": "test_gpu_sharded",
 }
 
@@ -38,7 +40,7 @@ def tables():
     return {"row kernels": set(rk.VARIANTS) | set(rk.GENERIC), "glue": set(gk.VARIANTS), "elementwise math": set(em.KERNELS),
             "staging": set(sk.VARIANTS), "select": set(sel.KERNELS), "masks": set(mo.VARIANTS),
             "conv / norm / resize": set(ck.VARIANTS), "decode step": set(dk.VARIANTS),
-            "prefill attention": set(pk.VARIANTS)}
+            "prefill attention": set(pk.VARIANTS), "GRU / LSTM": set(nk.VARIANTS)}
 
 
 _GLOBAL = re.compile(r"\b__global__\b")
