@@ -557,6 +557,19 @@ rten_status rten_b200_instance_norm(rten_ctx* ctx, const rten_tensor* x, const r
 rten_status rten_b200_group_norm(rten_ctx* ctx, const rten_tensor* x, int groups, const rten_tensor* inst_scale,
                                  const rten_tensor* inst_bias, const rten_tensor* gamma_or_null, const rten_tensor* beta_or_null,
                                  float epsilon, const rten_activation* act_or_null, rten_tensor* out);
+/* BatchNormalization in inference mode (src/ops/norm.rs batch_norm_in_place): per channel c,
+ *   s = scale[c] / sqrt(var[c] + epsilon)        (a rounded add, a correctly rounded sqrt and division)
+ *   y = fma(x - mean[c], s, bias[c])             (the subtraction rounded, then one fused multiply-add)
+ * then the activation (NULL or RTEN_ACT_NONE: none), computed as the standalone operator computes it.  The channel is
+ * axis 1 of x when x has rank >= 2; a rank-1 x is one channel.  scale, bias, mean and var are 1-D [C]; epsilon < 0 =>
+ * default 1e-5.  The reference's statuses and messages: rank 0 returns RTEN_ERR_INVALID_VALUE "Input must have at least
+ * 1 dim"; a parameter of another length returns RTEN_ERR_INCOMPATIBLE_SHAPES "scale.size(0) != channels" (bias, mean,
+ * var alike).  NCHW-contiguous x (any rank) and dense channels-last 4-D x are read as they are and the output keeps x's
+ * layout; x in any other strides is copied to contiguous first.  `out` may alias `x` (run_in_place).  Bit-identical to
+ * the reference; one kernel launch for dense device-resident operands, capturable in a CUDA graph. */
+rten_status rten_b200_batch_norm(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* scale, const rten_tensor* bias,
+                                 const rten_tensor* mean, const rten_tensor* var, float epsilon,
+                                 const rten_activation* act_or_null, rten_tensor* out);
 /* Clip (src/ops/unary_elementwise.rs:249-333), f32 or i32: x.max(min).min(max) with `a > b ? a : b` comparisons, so
  * NaN becomes min and -0.0 clipped at min = 0 becomes +0.0.  min / max are scalar tensors of x's type (NULL: the type's
  * finite minimum / maximum), read on the device: no host synchronisation, capturable in a CUDA graph.  `out` may alias

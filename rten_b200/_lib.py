@@ -149,6 +149,7 @@ _SIGNATURES = {
     "rten_b200_skip_layer_norm": (C.c_int, [_vp, _TP, _TP, _TP, _TP, _TP, C.c_float, C.c_int, _TP, _TP]),
     "rten_b200_instance_norm": (C.c_int, [_vp, _TP, _TP, _TP, C.c_float, _TP]),
     "rten_b200_group_norm": (C.c_int, [_vp, _TP, C.c_int, _TP, _TP, _TP, _TP, C.c_float, C.POINTER(RtenActivation), _TP]),
+    "rten_b200_batch_norm": (C.c_int, [_vp, _TP, _TP, _TP, _TP, _TP, C.c_float, C.POINTER(RtenActivation), _TP]),
     "rten_b200_erf": (C.c_int, [_vp, _TP, _TP]),
     "rten_b200_gelu": (C.c_int, [_vp, _TP, C.c_int, _TP]),
     "rten_b200_dynamic_quantize_linear": (C.c_int, [_vp, _TP, _TP, _TP, _TP, _vp]),

@@ -304,7 +304,7 @@ rten_status rten_b200_skip_layer_norm(rten_ctx* ctx, const rten_tensor* x, const
     return sc.finish(launch_norm(ctx, p));
 }
 
-// ---- InstanceNormalization and the GroupNorm chain ------------------------------------------------------
+// ---- InstanceNormalization, the GroupNorm chain and BatchNormalization ------------------------------------
 // The kernels' view of x: 0 for [N, C, P] contiguous, 1 for a dense channels-last 4-D tensor, -1 for anything else
 static int gn_layout(const rten_tensor& t) {
     if (is_contiguous(&t)) return 0;
@@ -323,10 +323,12 @@ static rten_status gn_vector(OpScope& sc, const rten_tensor* t, const float** pt
     return RTEN_OK;
 }
 
-// Rows of `groups` per image, checked by the entry points
+// Rows of `groups` per image, checked by the entry points.  With bn_mean (and bn_var): BatchNormalization, groups = C,
+// inst_scale / inst_bias its scale and bias; a rank-1 x is one channel.
 static rten_status group_norm_run(rten_ctx* ctx, const rten_tensor* x, int groups, const rten_tensor* inst_scale,
                                   const rten_tensor* inst_bias, const rten_tensor* gamma, const rten_tensor* beta, float epsilon,
-                                  const rten_activation* act, rten_tensor* out) {
+                                  const rten_activation* act, rten_tensor* out, const rten_tensor* bn_mean = nullptr,
+                                  const rten_tensor* bn_var = nullptr) {
     OpScope sc(ctx);
     rten_tensor xv, xc, ov;
     GroupNormParams p;
@@ -344,6 +346,9 @@ static rten_status group_norm_run(rten_ctx* ctx, const rten_tensor* x, int group
     RTB_TRY(gn_vector(sc, inst_bias, &p.inst_bias));
     if (gamma) RTB_TRY(gn_vector(sc, gamma, &p.gamma));
     if (beta) RTB_TRY(gn_vector(sc, beta, &p.beta));
+    const float *mean = nullptr, *var = nullptr;
+    if (bn_mean) RTB_TRY(gn_vector(sc, bn_mean, &mean));
+    if (bn_var) RTB_TRY(gn_vector(sc, bn_var, &var));
     // the output in the layout the kernels write: `out` itself when it has it, else a temporary copied into `out`
     bool direct = gn_layout(ov) == layout;
     for (int i = 0; i < ov.ndim && direct; i++)
@@ -354,17 +359,22 @@ static rten_status group_norm_run(rten_ctx* ctx, const rten_tensor* x, int group
     p.x = (const float*)xc.data;
     p.y = (float*)yc.data;
     p.N = xv.shape[0];
-    p.C = (int)xv.shape[1];
+    p.C = xv.ndim >= 2 ? (int)xv.shape[1] : 1;
     p.G = groups;
     p.P = numel(&xv) / (p.N * p.C);
     p.channels_last = layout;
+    if (bn_mean && p.P == 1) {  // [N, C], [N, C, 1, ..] and rank 1: the memory of one channels-last image of N pixels
+        p.P = p.N;
+        p.N = 1;
+        p.channels_last = 1;
+    }
     p.eps = epsilon < 0.0f ? 1e-5f : epsilon;
     if (act) {
         p.act = act->kind;
         p.act_alpha = act->alpha;
         p.act_beta = act->beta;
     }
-    RTB_TRY(launch_group_norm(ctx, p));
+    RTB_TRY(mean ? launch_batch_norm(ctx, p, mean, var) : launch_group_norm(ctx, p));
     return sc.finish(direct ? RTEN_OK : copy_view(ctx, yc, ov));
 }
 
@@ -401,6 +411,28 @@ rten_status rten_b200_group_norm(rten_ctx* ctx, const rten_tensor* x, int groups
     if (act && (act->kind < RTEN_ACT_NONE || act->kind > RTEN_ACT_HARD_SWISH))
         return fail(ctx, RTEN_ERR_INVALID_VALUE, "unknown activation kind");
     return group_norm_run(ctx, x, groups, inst_scale, inst_bias, gamma, beta, epsilon, act, out);
+}
+
+rten_status rten_b200_batch_norm(rten_ctx* ctx, const rten_tensor* x, const rten_tensor* scale, const rten_tensor* bias,
+                                 const rten_tensor* mean, const rten_tensor* var, float epsilon, const rten_activation* act,
+                                 rten_tensor* out) {
+    RTB_TRY(check_ctx(ctx));
+    if (!x || !scale || !bias || !mean || !var || !out) return fail(ctx, RTEN_ERR_MISSING_INPUTS, "missing inputs");
+    for (const rten_tensor* t : {x, scale, bias, mean, var})
+        if (t->dtype != RTEN_F32) return fail(ctx, RTEN_ERR_UNSUPPORTED_TYPE, "unsupported type");
+    if (scale->ndim != 1 || bias->ndim != 1 || mean->ndim != 1 || var->ndim != 1)
+        return fail(ctx, RTEN_ERR_CAST_FAILED, "scale, bias, mean and var must be 1-D tensors");
+    // src/ops/norm.rs batch_norm_in_place
+    if (x->ndim < 1) return fail(ctx, RTEN_ERR_INVALID_VALUE, "Input must have at least 1 dim");
+    const int64_t C = x->ndim >= 2 ? x->shape[1] : 1;
+    if (scale->shape[0] != C) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "scale.size(0) != channels");
+    if (bias->shape[0] != C) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "bias.size(0) != channels");
+    if (mean->shape[0] != C) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "mean.size(0) != channels");
+    if (var->shape[0] != C) return fail(ctx, RTEN_ERR_INCOMPATIBLE_SHAPES, "var.size(0) != channels");
+    if (C > INT32_MAX) return fail(ctx, RTEN_ERR_UNSUPPORTED_VALUE, "channel count out of range");
+    if (act && (act->kind < RTEN_ACT_NONE || act->kind > RTEN_ACT_HARD_SWISH))
+        return fail(ctx, RTEN_ERR_INVALID_VALUE, "unknown activation kind");
+    return group_norm_run(ctx, x, (int)C, scale, bias, nullptr, nullptr, epsilon, act, out, mean, var);
 }
 
 // ---- unary elementwise ----------------------------------------------------------------------------

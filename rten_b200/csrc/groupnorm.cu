@@ -19,6 +19,11 @@
 //                     which a 4 MB row spread over 32 CTAs does not fit.
 // The fold of one row is serial: 2 ceil(L / 64) dependent adds / FMAs per lane, which bounds a long row's time no
 // matter how fast it arrives.
+//
+// BatchNormalization (src/ops/norm.rs batch_norm_in_place: normalize_each_channel with MeanNormalize::Static) is the
+// output pass alone, gn_apply_kernel with G = C and its constants per channel: mean[c], and
+// scale[c] / sqrt(var[c] + epsilon) computed by each thread as the reference computes it, then Normalize's arm 0.
+// The mean and variance are kernel arguments of their own, so GroupNormParams and the other kernels stay as they were.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -172,35 +177,61 @@ __global__ void __launch_bounds__(STATS_THREADS) gn_stats_kernel(const float* __
     }
 }
 
-// The output of the streaming path over all SMs.  NCHW: blockIdx.y walks the (n, c) planes, threads the plane's
-// pixels.  Channels-last: blockIdx.y walks the images; thread i of an image keeps the channel unit i % CU (CU = C / 4
-// float4s with vec, else C floats) and walks the pixels i / CU, i / CU + k, ...  vec: 16-byte accesses.
+// (mean, rstd) of row `row` = (n, g): the statistics pass's, or BatchNormalization's constants of channel g (bn_mean set)
+__device__ __forceinline__ float2 row_stats(const GroupNormParams& p, const float2* __restrict__ stats, const float* __restrict__ bn_mean,
+                                            const float* __restrict__ bn_var, long long row, int g) {
+    if (!bn_mean) return stats[row];
+    return make_float2(__ldg(bn_mean + g), __fdiv_rn(__ldg(p.inst_scale + g), __fsqrt_rn(__fadd_rn(__ldg(bn_var + g), p.eps))));
+}
+
+// The output of the streaming path, and BatchNormalization, over all SMs.  NCHW, k == 0: blockIdx.y walks the (n, c)
+// planes, threads the plane's pixels.  NCHW, k > 0 (planes of at most blockDim.x / k units): each block takes k whole
+// planes at a time, thread t unit t % n4 of plane t / n4, so small planes do not leave most of a block idle.
+// Channels-last: blockIdx.y walks the images; thread i of an image keeps the channel unit i % CU (CU = C / 4 float4s
+// with vec, else C floats) and walks the pixels i / CU, i / CU + k, ...  vec: 16-byte accesses.  bn_mean / bn_var:
+// BatchNormalization's mean and variance (G = C, no `stats`), else null.
 template <bool CL>
 __global__ void __launch_bounds__(APPLY_THREADS) gn_apply_kernel(const GroupNormParams p, const float2* __restrict__ stats, int vec,
-                                                                 int k) {
+                                                                 int k, const float* __restrict__ bn_mean, const float* __restrict__ bn_var) {
     const int cg = p.C / p.G;
     const long long P = p.P;
     if (!CL) {
         const long long n4 = vec ? P / 4 : P;
-        for (long long plane = blockIdx.y; plane < p.N * p.C; plane += gridDim.y) {
-            const int c = (int)(plane % p.C);
-            const long long row = (plane / p.C) * p.G + c / cg;
-            const float2 st = stats[row];
-            const float ib = __ldg(p.inst_bias + c / cg), gm = p.gamma ? __ldg(p.gamma + c) : 1.0f, bt = p.beta ? __ldg(p.beta + c) : 0.0f;
+        // unit f of plane `plane`
+        auto unit = [&](long long plane, long long f, float2 st, float ib, float gm, float bt) {
             const float* xp = p.x + plane * P;
             float* yp = p.y + plane * P;
-            for (long long f = (long long)blockIdx.x * blockDim.x + threadIdx.x; f < n4; f += (long long)gridDim.x * blockDim.x) {
-                if (vec) {
-                    float4 v = reinterpret_cast<const float4*>(xp)[f];
-                    v.x = gn_out(p, v.x, st.x, st.y, ib, gm, bt);
-                    v.y = gn_out(p, v.y, st.x, st.y, ib, gm, bt);
-                    v.z = gn_out(p, v.z, st.x, st.y, ib, gm, bt);
-                    v.w = gn_out(p, v.w, st.x, st.y, ib, gm, bt);
-                    reinterpret_cast<float4*>(yp)[f] = v;
-                } else {
-                    yp[f] = gn_out(p, xp[f], st.x, st.y, ib, gm, bt);
-                }
+            if (vec) {
+                float4 v = reinterpret_cast<const float4*>(xp)[f];
+                v.x = gn_out(p, v.x, st.x, st.y, ib, gm, bt);
+                v.y = gn_out(p, v.y, st.x, st.y, ib, gm, bt);
+                v.z = gn_out(p, v.z, st.x, st.y, ib, gm, bt);
+                v.w = gn_out(p, v.w, st.x, st.y, ib, gm, bt);
+                reinterpret_cast<float4*>(yp)[f] = v;
+            } else {
+                yp[f] = gn_out(p, xp[f], st.x, st.y, ib, gm, bt);
             }
+        };
+        auto plane_consts = [&](long long plane, float2* st, float* ib, float* gm, float* bt) {
+            const int c = (int)(plane % p.C);
+            *st = row_stats(p, stats, bn_mean, bn_var, (plane / p.C) * p.G + c / cg, c / cg);
+            *ib = __ldg(p.inst_bias + c / cg), *gm = p.gamma ? __ldg(p.gamma + c) : 1.0f, *bt = p.beta ? __ldg(p.beta + c) : 0.0f;
+        };
+        float2 st;
+        float ib, gm, bt;
+        if (k > 0) {
+            const int lp = (int)(threadIdx.x / n4), f = (int)(threadIdx.x - lp * n4);
+            if (lp >= k) return;
+            for (long long plane = (long long)blockIdx.x * k + lp; plane < p.N * p.C; plane += (long long)gridDim.x * k) {
+                plane_consts(plane, &st, &ib, &gm, &bt);
+                unit(plane, f, st, ib, gm, bt);
+            }
+            return;
+        }
+        for (long long plane = blockIdx.y; plane < p.N * p.C; plane += gridDim.y) {
+            plane_consts(plane, &st, &ib, &gm, &bt);
+            for (long long f = (long long)blockIdx.x * blockDim.x + threadIdx.x; f < n4; f += (long long)gridDim.x * blockDim.x)
+                unit(plane, f, st, ib, gm, bt);
         }
         return;
     }
@@ -213,7 +244,7 @@ __global__ void __launch_bounds__(APPLY_THREADS) gn_apply_kernel(const GroupNorm
 #pragma unroll
         for (int j = 0; j < 4; j++) {
             const int c = cu * W + (j < W ? j : 0);
-            const float2 st = stats[n * p.G + c / cg];
+            const float2 st = row_stats(p, stats, bn_mean, bn_var, n * p.G + c / cg, c / cg);
             mean[j] = st.x, rstd[j] = st.y;
             ib[j] = __ldg(p.inst_bias + c / cg);
             gm[j] = p.gamma ? __ldg(p.gamma + c) : 1.0f;
@@ -234,6 +265,41 @@ __global__ void __launch_bounds__(APPLY_THREADS) gn_apply_kernel(const GroupNorm
             }
         }
     }
+}
+
+// gn_apply_kernel over the whole tensor: NCHW one (n, c) plane per block row -- or, for BatchNormalization's planes of
+// at most half a block, whole planes packed into each block -- channels-last k pixels per sweep
+static rten_status launch_apply(rten_ctx* ctx, const GroupNormParams& p, const float2* stats, const float* bn_mean = nullptr,
+                                const float* bn_var = nullptr) {
+    auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+    const long long blocks_wanted = 8LL * ctx->num_sms;
+    if (!p.channels_last) {
+        const int vec = p.P % 4 == 0 && al16(p.x) && al16(p.y);
+        const long long n4 = vec ? p.P / 4 : p.P, planes = p.N * p.C;
+        if (bn_mean && n4 <= APPLY_THREADS / 2) {
+            const long long k = APPLY_THREADS / n4, gx = std::min<long long>((planes + k - 1) / k, 4 * blocks_wanted);
+            return launch(ctx, "batch_norm launch", gn_apply_kernel<false>, {dim3((unsigned)gx), dim3(APPLY_THREADS)}, p, stats, vec,
+                          (int)k, bn_mean, bn_var);
+        }
+        const long long gy = std::min<long long>(planes, 65535);
+        const long long gx = std::max<long long>(1, std::min<long long>((n4 + APPLY_THREADS * 4 - 1) / (APPLY_THREADS * 4),
+                                                                        (blocks_wanted + gy - 1) / gy));
+        return launch(ctx, "group_norm apply launch", gn_apply_kernel<false>, {dim3((unsigned)gx, (unsigned)gy), dim3(APPLY_THREADS)}, p,
+                      stats, vec, 0, bn_mean, bn_var);
+    }
+    const int vec = p.C % 4 == 0 && al16(p.x) && al16(p.y);
+    const long long CU = vec ? p.C / 4 : p.C, gy = std::min<long long>(p.N, 65535);
+    // k pixels per sweep: about blocks_wanted CTAs in all, each thread walking at least four pixels
+    long long k = std::max<long long>(1, (blocks_wanted / gy) * APPLY_THREADS / CU);
+    k = std::min<long long>(k, std::max<long long>(1, (p.P + 3) / 4));
+    const long long gx = (CU * k + APPLY_THREADS - 1) / APPLY_THREADS;
+    return launch(ctx, "group_norm apply launch", gn_apply_kernel<true>, {dim3((unsigned)gx, (unsigned)gy), dim3(APPLY_THREADS)}, p,
+                  stats, vec, (int)k, bn_mean, bn_var);
+}
+
+rten_status launch_batch_norm(rten_ctx* ctx, const GroupNormParams& p, const float* mean, const float* var) {
+    if (p.N == 0 || p.C == 0 || p.P == 0) return RTEN_OK;
+    return launch_apply(ctx, p, nullptr, mean, var);
 }
 
 rten_status launch_group_norm(rten_ctx* ctx, const GroupNormParams& p) {
@@ -266,24 +332,7 @@ rten_status launch_group_norm(rten_ctx* ctx, const GroupNormParams& p) {
     const size_t ring = (size_t)RING_STAGES * RING_CHUNK * 4;
     RTB_TRY(launch(ctx, "group_norm stats launch", gn_stats_kernel, {dim3((unsigned)rows), dim3(STATS_THREADS), ring, (int)ring}, xs, p, L,
                    (int)(L % 4 == 0 && al16(xs)), stats));
-    const long long blocks_wanted = 8LL * ctx->num_sms;
-    if (!cl) {
-        const int vec = p.P % 4 == 0 && al16(p.x) && al16(p.y);
-        const long long n4 = vec ? p.P / 4 : p.P, planes = p.N * p.C;
-        const long long gy = std::min<long long>(planes, 65535);
-        const long long gx = std::max<long long>(1, std::min<long long>((n4 + APPLY_THREADS * 4 - 1) / (APPLY_THREADS * 4),
-                                                                        (blocks_wanted + gy - 1) / gy));
-        return launch(ctx, "group_norm apply launch", gn_apply_kernel<false>, {dim3((unsigned)gx, (unsigned)gy), dim3(APPLY_THREADS)}, p,
-                      (const float2*)stats, vec, 0);
-    }
-    const int vec = p.C % 4 == 0 && al16(p.x) && al16(p.y);
-    const long long CU = vec ? p.C / 4 : p.C, gy = std::min<long long>(p.N, 65535);
-    // k pixels per sweep: about blocks_wanted CTAs in all, each thread walking at least four pixels
-    long long k = std::max<long long>(1, (blocks_wanted / gy) * APPLY_THREADS / CU);
-    k = std::min<long long>(k, std::max<long long>(1, (p.P + 3) / 4));
-    const long long gx = (CU * k + APPLY_THREADS - 1) / APPLY_THREADS;
-    return launch(ctx, "group_norm apply launch", gn_apply_kernel<true>, {dim3((unsigned)gx, (unsigned)gy), dim3(APPLY_THREADS)}, p,
-                  (const float2*)stats, vec, (int)k);
+    return launch_apply(ctx, p, stats);
 }
 
 }  // namespace rtb

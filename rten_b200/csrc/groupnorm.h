@@ -1,5 +1,5 @@
-// InstanceNormalization and the GroupNorm chain torch exports (groupnorm.cu).  All pointers are device pointers; all
-// launches go to ctx->stream.
+// InstanceNormalization, the GroupNorm chain torch exports and BatchNormalization (groupnorm.cu).  All pointers are
+// device pointers; all launches go to ctx->stream.
 #pragma once
 #include "common.h"
 
@@ -27,5 +27,9 @@ struct GroupNormParams {
     float act_alpha = 0.0f, act_beta = 0.0f;
 };
 rten_status launch_group_norm(rten_ctx* ctx, const GroupNormParams& p);
+// BatchNormalization: G = C and no statistics pass; channel c's mean is mean[c] ([C]) and its rstd is
+// inst_scale[c] / sqrt(var[c] + eps), each step rounded on its own; inst_bias[c] is the operator's bias.  One launch of
+// the output pass.  Any N, C, P whose channel count fits an int.
+rten_status launch_batch_norm(rten_ctx* ctx, const GroupNormParams& p, const float* mean, const float* var);
 
 }  // namespace rtb

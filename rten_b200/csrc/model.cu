@@ -3,7 +3,12 @@
 // hot-path operator set:
 //   load : build_graph (ONNX bytes -> nodes + initialisers, onnx_reader.cu; int64 tensors become i32 like rten's loader
 //          does; constants uploaded to HBM once) -> the fusions of src/optimize.rs the models need, in this order:
-//          fuse_silu, fuse_group_norm, fuse_into_producers -> plan_concat_elision -> prepack_weights (src/graph.rs:488-565).
+//          fuse_silu, fuse_group_norm, fold_batch_norm, fuse_into_producers -> plan_concat_elision -> prepack_weights
+//          (src/graph.rs:488-565).  fold_batch_norm is this executor's own: a BatchNormalization that is the only reader of
+//          an f32 Conv / ConvTranspose with constant weights goes into those weights and bias, as export tools fold it.
+//          The folded convolution rounds each weight product once more than the reference's Conv then
+//          BatchNormalization, so its output is held to the f32 convolution tolerance, not bit for bit -- depthwise
+//          layers included, whose unfolded kernel is bit-identical to the reference.
 //   run  : the nodes in topological (file) order, one C-ABI operator call each; temporaries are reference counted and
 //          returned to the context pool after their last consumer (src/graph.rs:1100-1180); an operator that can run in
 //          place does so when the executor holds the last reference to its input (src/graph.rs:973-1049); shape-only
@@ -913,6 +918,23 @@ rten_status load_arg_reduce(rten_model* m, onnx::Node& n) {
     return RTEN_OK;
 }
 
+// BatchNormalization (src/op_registry/onnx_registry.rs:830-842): inference mode only; momentum, a training attribute,
+// is read and ignored as the reference does.  Outputs 1-4 are the training statistics (src/ops/norm.rs check_outputs).
+rten_status check_batch_norm(rten_model* m, onnx::Node& n) {
+    for (const char* a : {"training_mode", "spatial"})
+        if (n.attr(a) && n.attr_i(a, 0) != (std::string_view(a) == "spatial" ? 1 : 0))
+            return mfail(m->ctx, RTEN_ERR_UNSUPPORTED_VALUE, "BatchNormalization: error in attribute \"" + std::string(a) + "\": unsupported value");
+    static const char* const stats[] = {"running_mean", "running_var", "saved_mean", "saved_var"};
+    for (size_t i = 1; i < n.outputs.size() && i < 5; i++)
+        if (!n.outputs[i].empty()) return mfail(m->ctx, RTEN_ERR_UNSUPPORTED_OUTPUT, std::string("unsupported output: ") + stats[i - 1]);
+    return RTEN_OK;
+}
+
+rten_status run_batch_norm(Runner& r, OpNode& o, rten_tensor* y) {
+    return rten_b200_batch_norm(r.ctx, r.T(o, 0), r.T(o, 1), r.T(o, 2), r.T(o, 3), r.T(o, 4), o.n.attr_f("epsilon", 1e-5f),
+                                &o.activation, y);
+}
+
 // Shape (src/ops/layout.rs): the input's dims [start, end) -- negative from the end, clamped to [0, ndim], end at least
 // start -- as a host value
 rten_status run_shape(Runner& r, OpNode& o, rten_tensor*) {
@@ -1527,6 +1549,7 @@ constexpr OpDef OPS[] = {
     {"InstanceNormalization", ONNX, IN_PLACE, 0b111, [](Runner& r, OpNode& o, rten_tensor* y) {
          return rten_b200_instance_norm(r.ctx, r.T(o, 0), r.T(o, 1), r.T(o, 2), o.n.attr_f("epsilon", 1e-5f), y); }},
     {"GroupNorm", 0, IN_PLACE, 0b1111111, run_group_norm},  // (GroupNormFusion)
+    {"BatchNormalization", ONNX, IN_PLACE, 0b11111, run_batch_norm, check_batch_norm},
     {"SkipLayerNormalization", MS, 0, 0b1, run_skip_norm<false>, check_skip_norm},
     {"SkipSimplifiedLayerNormalization", MS, 0, 0b1, run_skip_norm<true>, check_skip_norm},
     {"Gather", ONNX, 0, 0b1, [](Runner& r, OpNode& o, rten_tensor* y) {
@@ -1702,8 +1725,9 @@ constexpr const OpDef* row(std::string_view name) {
 // the operators the load-time passes look for
 constexpr const OpDef *CONV = row("Conv"), *CONV_TRANSPOSE = row("ConvTranspose"), *CONCAT = row("Concat"), *SIGMOID = row("Sigmoid"),
                       *MUL = row("Mul"), *SILU = row("Silu"), *MATMUL = row("MatMul"), *ADD = row("Add"), *RESHAPE_OP = row("Reshape"),
-                      *INSTANCE_NORM = row("InstanceNormalization"), *GROUP_NORM = row("GroupNorm");
-static_assert(CONV && CONV_TRANSPOSE && CONCAT && SIGMOID && MUL && SILU && MATMUL && ADD && RESHAPE_OP && INSTANCE_NORM && GROUP_NORM,
+                      *INSTANCE_NORM = row("InstanceNormalization"), *GROUP_NORM = row("GroupNorm"), *BATCH_NORM = row("BatchNormalization");
+static_assert(CONV && CONV_TRANSPOSE && CONCAT && SIGMOID && MUL && SILU && MATMUL && ADD && RESHAPE_OP && INSTANCE_NORM && GROUP_NORM &&
+                  BATCH_NORM,
               "a row the load looks for is missing");
 
 // the decoded file as values and nodes: constants uploaded, every node checked against OPS
@@ -1885,12 +1909,115 @@ void fuse_group_norm(rten_model* m) {
     });
 }
 
-// Conv + activation -> the activation in the convolution epilogue (Clip is not fused); MatMul + Add(constant vector over
-// the last axis) -> FusedMatMul with a row bias (MatMulAddFusion).  The Conv / MatMul takes the absorbed node's output.
+// The f32 elements of the constant `v`, copied back from the device
+rten_status constant_floats(rten_model* m, int v, std::vector<float>* out) {
+    const rten_tensor& t = m->values[(size_t)v].t;
+    out->resize((size_t)numel(&t));
+    if (!out->empty()) RTB_CUDA(m->ctx, cudaMemcpy(out->data(), t.data, out->size() * 4, cudaMemcpyDeviceToHost));
+    return RTEN_OK;
+}
+
+// The constant `v` released: its device memory goes back to the pool and the value no longer exists.  Only for a
+// constant nothing reads any more.
+void release_constant(rten_model* m, int v) {
+    ValueSlot& s = m->values[(size_t)v];
+    m->const_allocs.erase(std::find(m->const_allocs.begin(), m->const_allocs.end(), s.t.data));
+    pool_free(m->ctx, s.t.data);
+    s.t.data = nullptr;
+    s.kind = V_UNSET;
+}
+
+// Input `slot` of node o becomes a new f32 constant `name` of `dims` holding `data`.  The constant it replaces is
+// released when o was its only reader (`uses`: its uses before the replacement).
+rten_status replace_constant(rten_model* m, OpNode& o, size_t slot, int uses, const std::string& name, const std::vector<int64_t>& dims,
+                             const std::vector<float>& data) {
+    onnx::Tensor t;
+    t.name = name;
+    t.data_type = onnx::DT_FLOAT;
+    t.dims = dims;
+    t.data.resize(data.size() * 4);
+    if (!data.empty()) memcpy(t.data.data(), data.data(), t.data.size());
+    RTB_TRY(upload_constant(m, t));
+    const int old = slot < o.in.size() ? o.in[slot] : -1;
+    if (old >= 0 && uses == 1) release_constant(m, old);
+    if (o.in.size() <= slot) o.in.resize(slot + 1, -1), o.n.inputs.resize(slot + 1);
+    o.in[slot] = m->value_id(name);
+    o.n.inputs[slot] = name;
+    return RTEN_OK;
+}
+
+// Conv / ConvTranspose -> BatchNormalization, folded into the convolution at load when the BatchNormalization is the
+// convolution's only reader, the convolution is f32 with a constant weight (and bias, when it has one) and no
+// activation, and the four BatchNormalization parameters are constants of C_out elements.  On the host, in float32:
+//   s[co] = scale[co] / sqrt(var[co] + epsilon)
+//   w'[co, ..] = w[co, ..] * s[co]    (ConvTranspose: weight axis 1, co = g (C_out / G) + j)
+//   b'[co] = fma(bias[co] - mean[co], s[co], beta[co])    (bias 0 without one): the operator applied to the bias
+// The convolution takes the folded weights and the BatchNormalization's output, and the node launches nothing.  The
+// replaced weights and the BatchNormalization's parameters are released where nothing else reads them.
+rten_status fold_batch_norm(rten_model* m) {
+    rten_status st = RTEN_OK;
+    auto cval = [&](int vid, int64_t n) {
+        if (vid < 0) return false;
+        const ValueSlot& v = m->values[(size_t)vid];
+        return v.kind == V_CONST && v.t.dtype == RTEN_F32 && v.t.ndim == 1 && v.t.shape[0] == n;
+    };
+    fuse_each(m, [&](OpNode& bn, const Uses& u) {
+        if (st != RTEN_OK || bn.def != BATCH_NORM || bn.in.size() != 5) return false;
+        for (size_t i = 1; i < bn.out.size(); i++)
+            if (bn.out[i] >= 0) return false;
+        const int x = bn.in[0];
+        OpNode* c = x >= 0 ? u.producer[(size_t)x] : nullptr;
+        if (!c || (c->def != CONV && c->def != CONV_TRANSPOSE) || c->out.size() != 1 || u.sole_reader(x) != &bn ||
+            c->activation.kind != RTEN_ACT_NONE || c->in.size() < 2 || c->in[1] < 0)
+            return false;
+        const ValueSlot& wv = m->values[(size_t)c->in[1]];
+        if (wv.kind != V_CONST || wv.t.dtype != RTEN_F32 || wv.t.ndim < 3) return false;
+        const bool tr = c->def == CONV_TRANSPOSE;
+        const int64_t G = c->n.attr_i("group", 1);
+        if (G <= 0 || (tr && wv.t.shape[0] % G != 0)) return false;
+        const int64_t co_n = tr ? wv.t.shape[1] * G : wv.t.shape[0];
+        const int bias = c->in.size() > 2 ? c->in[2] : -1;
+        if ((bias >= 0 && !cval(bias, co_n)) || !cval(bn.in[1], co_n) || !cval(bn.in[2], co_n) || !cval(bn.in[3], co_n) ||
+            !cval(bn.in[4], co_n))
+            return false;
+        std::vector<float> w, b(co_n, 0.0f), scale, beta, mean, var;
+        if ((st = constant_floats(m, c->in[1], &w)) != RTEN_OK || (bias >= 0 && (st = constant_floats(m, bias, &b)) != RTEN_OK) ||
+            (st = constant_floats(m, bn.in[1], &scale)) != RTEN_OK || (st = constant_floats(m, bn.in[2], &beta)) != RTEN_OK ||
+            (st = constant_floats(m, bn.in[3], &mean)) != RTEN_OK || (st = constant_floats(m, bn.in[4], &var)) != RTEN_OK)
+            return false;
+        const float eps = bn.n.attr_f("epsilon", 1e-5f);
+        std::vector<float> s((size_t)co_n);
+        for (int64_t k = 0; k < co_n; k++) {
+            s[(size_t)k] = scale[(size_t)k] / std::sqrt(var[(size_t)k] + eps);
+            b[(size_t)k] = std::fmaf(b[(size_t)k] - mean[(size_t)k], s[(size_t)k], beta[(size_t)k]);
+        }
+        // elements per output channel of one weight slice: Conv [C_out, C_in / G, k..], ConvTranspose [C_in, C_out / G, k..]
+        const int64_t K = numel(&wv.t) / (wv.t.shape[0] * wv.t.shape[1]), cpg = wv.t.shape[1], cin_g = wv.t.shape[0] / G;
+        for (size_t i = 0; i < w.size(); i++) {
+            const int64_t co = tr ? (int64_t)i / (cpg * K) / cin_g * cpg + (int64_t)i / K % cpg : (int64_t)i / (cpg * K);
+            w[i] = w[i] * s[(size_t)co];
+        }
+        const std::vector<int64_t> wdims(wv.t.shape, wv.t.shape + wv.t.ndim);
+        const std::string tag = "/batch_norm_folded/" + m->values[(size_t)bn.out[0]].name;
+        if ((st = replace_constant(m, *c, 1, u.uses[(size_t)c->in[1]], m->values[(size_t)c->in[1]].name + tag, wdims, w)) != RTEN_OK ||
+            (st = replace_constant(m, *c, 2, bias >= 0 ? u.uses[(size_t)bias] : 0, "bias" + tag, {co_n}, b)) != RTEN_OK)
+            return false;
+        for (size_t i = 1; i < 5; i++)  // the parameters only this node read
+            if (u.uses[(size_t)bn.in[i]] == 1) release_constant(m, bn.in[i]);
+        c->out = bn.out;
+        bn.def = nullptr;
+        return true;
+    });
+    return st;
+}
+
+// Conv or BatchNormalization + activation -> the activation in the convolution epilogue / the normalization pass (Clip is
+// not fused); MatMul + Add(constant vector over the last axis) -> FusedMatMul with a row bias (MatMulAddFusion).  The
+// Conv / BatchNormalization / MatMul takes the absorbed node's output.
 void fuse_into_producers(rten_model* m) {
     fuse_each(m, [&](OpNode& a, const Uses& u) {
         OpNode* b = a.out.size() == 1 ? u.sole_reader(a.out[0]) : nullptr;
-        if (b && a.def == CONV && a.activation.kind == RTEN_ACT_NONE && b->def->act != RTEN_ACT_NONE) {
+        if (b && (a.def == CONV || a.def == BATCH_NORM) && a.activation.kind == RTEN_ACT_NONE && b->def->act != RTEN_ACT_NONE) {
             a.activation = activation_of(*b);
         } else if (b && a.def == MATMUL && b->def == ADD && a.bias_value < 0 && b->in.size() == 2) {
             const int other = b->in[0] == a.out[0] ? b->in[1] : b->in[0];
@@ -2025,6 +2152,7 @@ rten_status rten_b200_model_load(rten_ctx* ctx, const void* bytes, size_t len, r
     RTB_TRY(build_graph(m.get(), om));
     fuse_silu(m.get());
     if (!getenv("RTEN_B200_NO_GROUP_NORM_FUSION")) fuse_group_norm(m.get());
+    RTB_TRY(fold_batch_norm(m.get()));
     fuse_into_producers(m.get());
     if (!getenv("RTEN_B200_NO_CONCAT_ELISION")) plan_concat_elision(m.get(), om.graph.inputs);
     RTB_TRY(prepack_weights(m.get()));

@@ -879,6 +879,24 @@ class GroupNorm:
         return A.wrap(o, out)
 
 
+class BatchNormalization:
+    """src/ops/norm.rs batch_norm: y = fma(x - mean[c], scale[c] / sqrt(var[c] + epsilon), bias[c]) over channel axis 1
+    (a rank-1 x is one channel), then the activation (an ACT_* code or (kind, alpha, beta)); rten_b200_batch_norm.
+    `run(..., out=x)` normalises in place."""
+
+    def __init__(self, epsilon: Optional[float] = None, activation=ACT_NONE):
+        self.epsilon, self.activation = epsilon, activation
+
+    def run(self, ctx, x, scale, bias, mean, var, out=None):
+        A = _Args(ctx)
+        o = A.out(out)
+        act = _activation(self.activation)
+        ctx.check(ctx.lib.rten_b200_batch_norm(ctx.handle, A.t(x), A.t(scale), A.t(bias), A.t(mean), A.t(var),
+                                               -1.0 if self.epsilon is None else float(self.epsilon), C.byref(act),
+                                               C.byref(o)))
+        return A.wrap(o, out)
+
+
 class _Unary:
     fn = ""
 
