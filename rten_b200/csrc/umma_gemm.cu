@@ -399,7 +399,9 @@ static rten_status prepare_launch(rten_ctx* ctx, const GemmLaunch& L, Prepared& 
         od.strides[3] = e.s_z1;
         q.dbox[1] = BM;
     }
-    q.tma_store = (e.s_col == 1 && L.N >= 4 && tma_compatible(od, 4, 4)) ? 1 : 0;
+    // N % 4 == 0: the store writes the row's last 16 bytes whole, so with N % 4 != 0 it would overwrite up to three
+    // floats past N in a row that the output view does not own (a column slice of a wider tensor)
+    q.tma_store = (e.s_col == 1 && L.N % 4 == 0 && tma_compatible(od, 4, 4)) ? 1 : 0;
     // residual prefetched by TMA: same geometry as the output, own strides (fast-path epilogue only)
     ord = od;
     ord.base = e.r;

@@ -1372,7 +1372,9 @@ def check_halo_conv(rt, oracle):
     showing the halo kernel ran, and the generic implicit-GEMM kernel must agree within the same bound.  (Every case here
     comes out at one image per unit; tests/test_gpu_plan_space.py pins units of several.)  The same cases in 3xTF32 run
     on the generic kernel, which is asserted too: the split operands carry a second A plane (x3_cb), which the halo
-    kernel does not take."""
+    kernel does not take.  Every halo unit shape, the windows and the paddings are also held bit for bit against an exact
+    product by tests/test_gpu_wgmma_kernels.py; these cases stay for ResNet-50's layer shapes and the agreement of the
+    two kernels."""
     with switches(RTEN_B200_HALO=1):  # the kernel is opt-in (the generic kernel stays the default)
         return _check_halo_conv(rt, oracle)
 

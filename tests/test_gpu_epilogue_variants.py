@@ -3,7 +3,9 @@ with the default choice, under RTEN_B200_NO_PLAIN (the plain variants give way t
 RTEN_B200_NO_FAST (everything on Generic).  The variant that ran is read from the RTEN_B200_VERBOSE plan line (`epi=`),
 and so are the work units: every variant runs at least one launch with more units than SMs, so the staging ring and
 the barrier phases carry over from one unit to the next.  f32 outputs, i32 outputs and the *ToFloat output ranges must
-be bit-identical across the three runs."""
+be bit-identical across the three runs.  Each variant is also held bit for bit against a float32 model of its
+roundings, on data whose products are exact, by tests/test_gpu_wgmma_kernels.py; the cases here stay for the agreement
+of the variants on full-mantissa data and the benched shapes."""
 import re
 
 import numpy as np

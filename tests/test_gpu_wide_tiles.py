@@ -3,7 +3,9 @@ the plain f32 epilogue).  Each case is forced onto a wide plan and onto a 64-col
 result must meet the TF32 (or 3xTF32) bound against float64, the wide kernel must have run (forced-plan counter, and
 CUPTI kernel records where the session has them), and both plans must agree bit for bit (same K order, same epilogue
 roundings).  The persistent-schedule cases launch more work units than the device has SMs, so every CTA carries its
-pipeline state from one unit to the next."""
+pipeline state from one unit to the next.  Both wide instances and the chained ones are also held bit for bit against
+an exact product, with CUPTI required to show them, by tests/test_gpu_wgmma_kernels.py; the cases here stay for the
+agreement of wide and narrow plans on full-mantissa data and the benched shapes."""
 import re
 
 import numpy as np

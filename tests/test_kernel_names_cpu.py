@@ -1,12 +1,12 @@
 """CPU-only: every `__global__` kernel defined in rten_b200/csrc (*.cu and *.cuh) is in exactly one by-name table -- the
 row kernels, glue, elementwise math and operand staging of rowops.cu, TopK / arg-reduce, the mask kernels, the
 depthwise / GroupNorm / Resize / Concat / ReduceSum / rotary table, the single-query attention / MatMulNBits table,
-the prefill attention table and the GRU / LSTM table.  Each of those tables is kept equal to the compiled instances and
+the prefill attention table, the GRU / LSTM table and the wgmma GEMM / wide-tile / halo table.  Each of those tables is kept equal to the compiled instances and
 checked kernel by kernel, bit for bit, by its GPU test.  A kernel added without a by-name test fails here before any GPU
 time is spent.
 
-A few kernels are named only by their own operator's tests (`AD_HOC`: the wgmma GEMM and halo kernels, the encoder
-attention kernel and the multi-GPU range exchange).  For those this file checks only that the test module's source names
+Two kernels are named only by their own operator's tests (`AD_HOC`: the encoder attention kernel and the multi-GPU range
+exchange).  For those this file checks only that the test module's source names
 the kernel -- a weaker guarantee than a table: nothing here proves the module asserts that the kernel ran, or covers
 every instance."""
 import glob
@@ -23,14 +23,13 @@ import test_gpu_rnn_kernels as nk
 import test_gpu_row_kernels as rk
 import test_gpu_select as sel
 import test_gpu_staging_kernels as sk
+import test_gpu_wgmma_kernels as wk
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(os.path.dirname(HERE), "rten_b200", "csrc")
 
 # kernel -> the test module that names it (and checks, in its own way, that it runs)
 AD_HOC = {
-    "umma_gemm_kernel": "test_gpu_epilogue_variants", "umma_wide_kernel": "test_gpu_wide_tiles",
-    "umma_halo_kernel": "gpu_checks",
     "attn_fused_kernel": "test_gpu_attention_encoder",
     "peer_minmax_kernel": "test_gpu_sharded",
 }
@@ -40,7 +39,8 @@ def tables():
     return {"row kernels": set(rk.VARIANTS) | set(rk.GENERIC), "glue": set(gk.VARIANTS), "elementwise math": set(em.KERNELS),
             "staging": set(sk.VARIANTS), "select": set(sel.KERNELS), "masks": set(mo.VARIANTS),
             "conv / norm / resize": set(ck.VARIANTS), "decode step": set(dk.VARIANTS),
-            "prefill attention": set(pk.VARIANTS), "GRU / LSTM": set(nk.VARIANTS)}
+            "prefill attention": set(pk.VARIANTS), "GRU / LSTM": set(nk.VARIANTS),
+            "wgmma GEMM / halo": set(wk.VARIANTS)}
 
 
 _GLOBAL = re.compile(r"\b__global__\b")
